@@ -22,7 +22,6 @@ SIGNATURES = {
     "delora_sort_by_range": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "delora_normals_fwd": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_int, c_void_p,
                                    c_void_p, c_void_p, c_void_p]),
-    "delora_normals_select_staging": (c_int, [c_int]),
     "delora_scan_blocks": (c_int, [c_int]),
     "delora_lists_from_images": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                          c_void_p, c_void_p, c_void_p, c_void_p]),
@@ -44,7 +43,6 @@ SIGNATURES = {
                                        c_void_p, c_void_p]),
     "delora_conv2d_fprop_bf16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                          c_int, c_int, c_int, c_int, c_int, c_void_p]),
-    "delora_conv_select_kernel": (c_int, [c_int]),
     "delora_conv2d_dgrad_bf16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                          c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "delora_conv2d_wgrad_scratch_floats": (c_i64, [c_int, c_int, c_int, c_int, c_int, c_int]),
@@ -75,7 +73,7 @@ SIGNATURES = {
                                           ctypes.c_longlong, c_float, c_u32, c_int, c_int, c_void_p, c_void_p]),
 }
 
-ABI_VERSION = 1
+ABI_VERSION = 2
 _lib = None
 
 

@@ -313,17 +313,8 @@ static int rows_pick_ns(int Wg) {
     return ns < 16 ? 16 : ns;
 }
 
-// DELORA_CONV_PIXM=0 (or delora_conv_select_kernel(2)) keeps the pixel-on-M form off (Cout = 64 / 128 layers then take
-// the first-generation kernel for the forward pass)
-static int g_rows_pixm = -1;
-bool rows_use_pixm() {
-    if (g_rows_pixm < 0) { const char* e = getenv("DELORA_CONV_PIXM"); g_rows_pixm = (e && e[0] == '0') ? 0 : 1; }
-    return g_rows_pixm == 1;
-}
-void rows_set_pixm(int on) { g_rows_pixm = on ? 1 : 0; }
-
 // pixel-on-M mode: Cout = 64 or 128 and a job grid at least one full 128-pixel segment wide
-static bool rows_pixm(int Cout, int Wg) { return (Cout == 64 || Cout == 128) && Wg >= 128 && rows_use_pixm(); }
+static bool rows_pixm(int Cout, int Wg) { return (Cout == 64 || Cout == 128) && Wg >= 128; }
 
 // Wg = width of the job grid (the output width for a stride-1 convolution, ceil(Wout / stride_w) for a data gradient)
 bool conv_rows_eligible(int Cin, int Cout, int ksize, int Wg) {

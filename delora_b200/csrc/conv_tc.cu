@@ -782,7 +782,6 @@ static const TensorMaps* get_maps(const void* x, const void* w, int B, int Hin, 
 
 namespace delora {
 bool conv_rows_eligible(int Cin, int Cout, int ksize, int Wg);
-void rows_set_pixm(int on);
 bool wgrad2_eligible(int Cin, int Cout, int ksize, int stride_h, int stride_w);
 int64_t wgrad2_scratch_floats(int B, int Hout, int Wout, int Cin, int Cout, int sw);
 int wgrad2_launch(const void* x, const void* dz, float* dw, float* scratch, int B, int Hin, int Win, int Cin, int Cin_true,
@@ -790,22 +789,9 @@ int wgrad2_launch(const void* x, const void* dz, float* dw, float* scratch, int 
 int conv_rows_launch(const void* x, const void* w, const void* residual, const void* saved, void* y, int B, int Hout,
                      int Wout, int Cin, int Cout, int ksize, int up_h, int up_w, int act, cudaStream_t stream,
                      int residual_on_grid);
-// DELORA_CONV_ROWS=0 keeps every convolution on the first-generation kernel (A/B measurements)
-static int g_conv_rows = -1;
-static bool use_conv_rows() {
-    if (g_conv_rows < 0) { const char* e = getenv("DELORA_CONV_ROWS"); g_conv_rows = (e && e[0] == '0') ? 0 : 1; }
-    return g_conv_rows == 1;
-}
 }  // namespace delora
 
 using namespace delora;
-
-extern "C" int delora_conv_select_kernel(int rows_kernel) {
-    const int prev = use_conv_rows() ? 1 : 0;
-    if (rows_kernel == 0 || rows_kernel == 1) { g_conv_rows = rows_kernel; rows_set_pixm(1); }
-    if (rows_kernel == 2) { g_conv_rows = 1; rows_set_pixm(0); }           // row-block kernel, pixel-on-M form off
-    return prev;
-}
 
 extern "C" int delora_conv2d_fprop_bf16(const void* x, const void* w, const void* residual, const void* saved, void* y,
                                         int B, int Hin, int Win, int Cin, int Cout, int ksize, int stride_h,
@@ -817,7 +803,7 @@ extern "C" int delora_conv2d_fprop_bf16(const void* x, const void* w, const void
                      Cin, Cout);
     DELORA_CHECK_ARG((stride_h == 1 || stride_h == 2) && (stride_w == 1 || stride_w == 2) && Hin >= 1 && Win >= 1,
                      "delora_conv2d_fprop_bf16: stride (%d,%d) unsupported", stride_h, stride_w);
-    if (stride_h == 1 && stride_w == 1 && conv_rows_eligible(Cin, Cout, ksize, Win) && use_conv_rows())
+    if (stride_h == 1 && stride_w == 1 && conv_rows_eligible(Cin, Cout, ksize, Win))
         return conv_rows_launch(x, w, residual, saved, y, B, Hin, Win, Cin, Cout, ksize, 1, 1, act, (cudaStream_t)stream, 0);
     ConvParams p;
     p.B = B; p.Cin = Cin; p.Cout = Cout; p.ksize = ksize; p.taps = ksize * ksize;
@@ -896,9 +882,11 @@ static int wgrad_splits(int B, int Hout, int Wout, int Cin, int Cout, int ksize)
     return splits > k_tiles ? (k_tiles > 0 ? k_tiles : 1) : splits;
 }
 
+// The query has no stride argument, so the size covers every kernel a layer of this shape may take: the
+// first-generation kernel (1x1 layers, strided layers with Cout = 64) and the second kernel at stride 1 or 2.
 extern "C" int64_t delora_conv2d_wgrad_scratch_floats(int B, int Hout, int Wout, int Cin, int Cout, int ksize) {
     int64_t n = (int64_t)wgrad_splits(B, Hout, Wout, Cin, Cout, ksize) * ksize * ksize * Cout * Cin;
-    if (wgrad2_eligible(Cin, Cout, ksize, 1, 1)) {           // either kernel may run (delora_conv_select_kernel)
+    if (wgrad2_eligible(Cin, Cout, ksize, 1, 1)) {
         const int64_t n1 = wgrad2_scratch_floats(B, Hout, Wout, Cin, Cout, 1), n2 = wgrad2_scratch_floats(B, Hout, Wout, Cin, Cout, 2);
         n = n > n1 ? n : n1;
         n = n > n2 ? n : n2;
@@ -915,7 +903,7 @@ extern "C" int delora_conv2d_wgrad_bf16(const void* x, const void* dz, float* dw
                      "delora_conv2d_wgrad_bf16: Cin=%d, Cout=%d must be multiples of 64", Cin, Cout);
     DELORA_CHECK_ARG((stride_h == 1 || stride_h == 2) && (stride_w == 1 || stride_w == 2) && Hin >= 1 && Win >= 1,
                      "delora_conv2d_wgrad_bf16: stride (%d,%d) unsupported", stride_h, stride_w);
-    if (use_conv_rows() && wgrad2_eligible(Cin, Cout, ksize, stride_h, stride_w))
+    if (wgrad2_eligible(Cin, Cout, ksize, stride_h, stride_w))
         return wgrad2_launch(x, dz, dw, scratch, B, Hin, Win, Cin, Cin_true, Cout, stride_h, stride_w, (cudaStream_t)stream);
     WgradParams p;
     p.B = B; p.Cin = Cin; p.Cout = Cout; p.ksize = ksize; p.taps = ksize * ksize;

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DELORA_B200_ABI_VERSION 1
+#define DELORA_B200_ABI_VERSION 2
 
 /* float4-packed list element: (x, y, z, tag).  `tag` is an int32 bit pattern or a float flag,
  * as documented per array. */
@@ -105,11 +105,6 @@ int delora_sort_by_range(const float* range, const int32_t* n_points, int B, int
 int delora_normals_fwd(const float* image, int B, int C_img, int H, int W, int nb_h, int nb_w,
                        float epsilon_range, int min_neighbors, float* normals,
                        delora_f4* pts_grid, delora_f4* nrm_grid, void* stream);
-/* How the 7x11 kernel stages its halo tile: 0 (default) coalesced loads + clamp + repack in one pass; 1 one TMA box
- * (cp.async.bulk.tensor.4d, three channel planes) + the same repack from shared memory (needs W % 4 == 0 and a 16-byte
- * aligned image, else mode 0 is used).  Results are bit-identical; mode 1 exists to measure what TMA buys this kernel
- * (DESIGN.md 4.2).  Returns the previous mode. */
-int delora_normals_select_staging(int mode);
 
 /* ---------------------------------------------------------------------------------------
  * Image -> lists (row-major order of the valid pixels), the layout the reference stores and
@@ -248,11 +243,6 @@ int delora_icp_point_grads(const delora_f4* point_dir, const delora_f4* normal_d
 int delora_conv2d_fprop_bf16(const void* x, const void* w, const void* residual, const void* saved, void* y, int B,
                              int Hin, int Win, int Cin, int Cout, int ksize, int stride_h, int stride_w, int act,
                              void* stream);
-/* Measurement switch: 1 (default) lets delora_conv2d_fprop_bf16 use the row-block kernel (csrc/conv_rows.cu) for
- * stride-1 layers with Cout % 128 == 0, 0 keeps every layer on the tap-per-TMA kernel (csrc/conv_tc.cu), 2 keeps the
- * row-block kernel but without its pixel-on-M form for Cout = 64 / 128 (DELORA_CONV_PIXM=0); any other value only
- * queries.  Returns the previous setting.  0 has the same effect as the environment variable DELORA_CONV_ROWS=0. */
-int delora_conv_select_kernel(int rows_kernel);
 /* Data gradient of a 3x3 convolution of stride (stride_h, stride_w) in {1,2}^2 -- autograd's backward of the same
  * nn.Conv2d layers (src/models/resnet_modified.py:126-134) w.r.t. their input -- by PHASE DECOMPOSITION: every
  * output phase (h % stride_h, w % stride_w) is a small convolution of the (un-upsampled) output gradient with the

@@ -167,29 +167,3 @@ def test_stem_kernels_match_torch(b, h, w, cuda_lib):
     dw = ops.stem_wgrad(x16, dzp, h, w, 8)
     assert (dw - wr.grad).abs().max().item() <= 1e-3 * wr.grad.abs().max().item()
     assert F.cosine_similarity(dw.flatten(), wr.grad.flatten(), dim=0).item() > 0.999999
-
-
-@pytest.mark.parametrize("h,w", [(64, 2048), (64, 720), (16, 180), (5, 12), (64, 2250)])
-def test_normals_tma_staging_is_bit_identical(h, w, cuda_lib):
-    """The TMA-staged variant of the 7x11 kernel (one cp.async.bulk.tensor box for the three channel planes, repack from
-    shared memory, delora_normals_select_staging(1)) against the default staging: identical normals and grids, image
-    borders and partial tiles included; W % 4 != 0 (2250) silently keeps the default."""
-    from delora_b200 import ops, synthetic
-    L = ops._lib.lib()
-    vf = (-25.0, 3.0) if h == 64 else (-15.0, 15.0)
-    cfg = synthetic.fov_config(h=h, w=w, vfov_deg=vf, device="cuda")
-    s1, _, _, _ = synthetic.make_pair(3, w_raw=min(w, 1024), rings=h if h in (16, 64) else 16, vfov_deg=vf)
-    pts = s1.unsqueeze(0).cuda().contiguous()
-    n = torch.tensor([s1.shape[1]], dtype=torch.int32, device="cuda")
-    image, _ = ops.project(pts, n, h, w, cfg["horizontal_field_of_view"], cfg["kitti"]["vertical_field_of_view"])
-    image = torch.cat((image, image.flip(3)), dim=0).contiguous()            # two images, the second mirrored
-    ref = ops.normals(image, grids=True)
-    old = L.delora_normals_select_staging(1)
-    try:
-        got = ops.normals(image, grids=True)
-    finally:
-        L.delora_normals_select_staging(old)
-    assert old == 0
-    for a, b_ in zip(ref, got):
-        assert torch.equal(a.view(torch.int32), b_.view(torch.int32))
-    assert int((ref[0] != 0).any(dim=1).sum()) > 0.2 * image.shape[0] * (h if h < 6 else h) * w * 0.5 or h < 6
