@@ -156,32 +156,49 @@ icp_kernel(const float4* __restrict__ src_pts4, const float4* __restrict__ src_n
         write_warp_partials(acc, partial_rows + ((size_t)b * rows_per_pair + warp_row) * DELORA_ICP_PARTIAL);
 }
 
-// Column sums of the per-warp partial rows: one block per (column, pair), fixed-order tree in fp64
-// (deterministic); the last block of a pair to finish turns the 40 sums into the means and the
-// 3x4 gradient and re-arms the pair's counter.
+// Column sums of the per-warp partial rows: one block per (group of 8 columns, pair).  Thread t reads the group's
+// 32 contiguous bytes of rows t, t + 256, ... (every sector fetched once, by one block) and keeps 8 fp64 sums; each
+// column is then reduced by the same fixed-order tree (deterministic).  The last block of a pair to finish turns the
+// 40 sums into the means and the 3x4 gradient and re-arms the pair's counter.
+constexpr int kFinCols = 8, kFinGroups = DELORA_ICP_PARTIAL / kFinCols;
+static_assert(DELORA_ICP_PARTIAL % kFinCols == 0, "partial rows are whole column groups");
+
 __global__ void __launch_bounds__(256)
 icp_finalize_kernel(const float* __restrict__ rows, int rows_per_pair, float* __restrict__ colsum,
                     int* __restrict__ counter, float lambda_po2pl, float* __restrict__ losses,
                     float* __restrict__ grad_T) {
-    __shared__ double red[256];
+    __shared__ double red[kFinCols][256];
     __shared__ float s[DELORA_ICP_PARTIAL];
     __shared__ int is_last;
-    const int c = blockIdx.x, b = blockIdx.y;
-    const float* __restrict__ p = rows + (size_t)b * rows_per_pair * DELORA_ICP_PARTIAL + c;
-    double a = 0.0;
-    for (int r = threadIdx.x; r < rows_per_pair; r += 256) a += (double)p[(size_t)r * DELORA_ICP_PARTIAL];
-    red[threadIdx.x] = a;
+    const int c0 = blockIdx.x * kFinCols, b = blockIdx.y;
+    const float* __restrict__ p = rows + (size_t)b * rows_per_pair * DELORA_ICP_PARTIAL + c0;
+    double a[kFinCols];
+#pragma unroll
+    for (int k = 0; k < kFinCols; ++k) a[k] = 0.0;
+    for (int r = threadIdx.x; r < rows_per_pair; r += 256) {
+        const float* __restrict__ q = p + (size_t)r * DELORA_ICP_PARTIAL;
+#pragma unroll
+        for (int k = 0; k < kFinCols; ++k) a[k] += (double)q[k];
+    }
+#pragma unroll
+    for (int k = 0; k < kFinCols; ++k) red[k][threadIdx.x] = a[k];
     __syncthreads();
 #pragma unroll
     for (int o = 128; o > 0; o >>= 1) {
-        if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+        if (threadIdx.x < o) {
+#pragma unroll
+            for (int k = 0; k < kFinCols; ++k) red[k][threadIdx.x] += red[k][threadIdx.x + o];
+        }
         __syncthreads();
     }
-    if (threadIdx.x == 0) {
-        colsum[(size_t)b * DELORA_ICP_PARTIAL + c] = (float)red[0];
+    if (threadIdx.x < kFinCols) {
+        colsum[(size_t)b * DELORA_ICP_PARTIAL + c0 + threadIdx.x] = (float)red[threadIdx.x][0];
         __threadfence();
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
         const int prev = atomicAdd(counter + b, 1);
-        is_last = (prev == DELORA_ICP_PARTIAL - 1);
+        is_last = (prev == kFinGroups - 1);
     }
     __syncthreads();
     if (!is_last) return;
@@ -218,7 +235,7 @@ int launch_icp_finalize(float* scratch, int B, int rows, float lambda_po2pl, uin
                         float* grad_T, cudaStream_t st) {
     (void)flags;
     const IcpScratch sc = icp_scratch(scratch, B, rows);
-    dim3 grid(DELORA_ICP_PARTIAL, B);
+    dim3 grid(kFinGroups, B);
     icp_finalize_kernel<<<grid, 256, 0, st>>>(sc.rows, rows, sc.colsum, sc.counter, lambda_po2pl, losses, grad_T);
     DELORA_CHECK_LAUNCH("icp_finalize_kernel");
     return 0;
@@ -310,11 +327,13 @@ extern "C" int delora_icp_partial_rows(int src_stride) { return (src_stride + 31
 
 extern "C" int64_t delora_icp_scratch_floats(int B, int src_stride) {
     // partial rows + column sums + counters; then, for the dense path: the 4x16-cell range pyramid (2 floats per
-    // block, at most src_stride/64 + H + W/16 + 1 <= src_stride/16 + 4096 blocks per pair) and the work list of
+    // block, at most src_stride/64 + H + W/16 + 1 <= src_stride/16 + 4096 blocks per pair), the prefix and suffix
+    // range extents of the pixel rows (4 floats per row, H <= src_stride) + one counter per pair, and the work list of
     // its second kernel (4 counters, int4 + done counter per warp, float4 search state + int result per source pixel)
     const int64_t rows = delora_icp_partial_rows(src_stride);
     return (int64_t)B * rows * DELORA_ICP_PARTIAL + (int64_t)B * DELORA_ICP_PARTIAL + B + 2 +
-           (int64_t)B * 2 * (src_stride / 16 + 4096) + 8 + 5 * (int64_t)B * rows + 5 * (int64_t)B * rows * 32;
+           (int64_t)B * 2 * (src_stride / 16 + 4096) + (int64_t)B * 4 * src_stride + B + 8 + 5 * (int64_t)B * rows +
+           5 * (int64_t)B * rows * 32;
 }
 
 extern "C" int delora_icp_fwd_bwd(const delora_f4* src_pts4, const delora_f4* src_nrm4, const int32_t* n_src,

@@ -132,22 +132,31 @@ __device__ __forceinline__ void accumulate_pair(uint32_t flags, const float4 p, 
 // keep the lower half of the live columns and receive the partner's contribution to them (31 shuffles for 32
 // columns instead of 32 x 5 for per-column shuffle trees); after the five rounds lane L holds the total of column L.
 // The (few) columns >= 32 use plain shuffle trees.
+// Every round is its own instantiation so that all indices into v[] are compile-time constants: a `for (o = 16; o > 0;
+// o >>= 1)` loop is not unrolled by nvcc, and its inner loop then indexes v[] at run time, i.e. in local memory.
+template <int O>
+__device__ __forceinline__ void halving_round(float (&v)[32], int lane) {
+    const bool upper = (lane & O) != 0;
+#pragma unroll
+    for (int k = 0; k < O; ++k) {
+        const float lo = v[k], hi = v[k + O];
+        const float send = upper ? lo : hi;
+        const float keep = upper ? hi : lo;
+        v[k] = keep + __shfl_xor_sync(0xffffffffu, send, O);
+    }
+}
+
 template <int N>
 __device__ __forceinline__ void warp_column_sums(const float (&acc)[kIcpAcc], float& keep0, float& keep1) {
     const int lane = threadIdx.x & 31;
     float v[32];
 #pragma unroll
     for (int k = 0; k < 32; ++k) v[k] = (k < N) ? acc[k] : 0.0f;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const bool upper = (lane & o) != 0;
-#pragma unroll
-        for (int k = 0; k < o; ++k) {
-            const float send = upper ? v[k] : v[k + o];
-            const float keep = upper ? v[k + o] : v[k];
-            v[k] = keep + __shfl_xor_sync(0xffffffffu, send, o);
-        }
-    }
+    halving_round<16>(v, lane);
+    halving_round<8>(v, lane);
+    halving_round<4>(v, lane);
+    halving_round<2>(v, lane);
+    halving_round<1>(v, lane);
     keep0 = v[0];
     keep1 = 0.0f;
 #pragma unroll

@@ -12,13 +12,14 @@
 // grows one strip at a time while ANY lane's exactness guard still fails, on the side the first
 // failing lane needs.  Control flow is warp-uniform (no divergence), adjacent lanes read adjacent
 // cells (coalesced, L1-resident), and the guard is the same proof as in icp.cu: all unsearched
-// targets lie beyond a border half-plane (azimuth) or cone (elevation) of the lane's window.
+// targets lie beyond a border half-plane (azimuth) or cone (elevation) of the lane's window.  Row (cone)
+// borders also use the RANGE of the targets beyond them (row_border_bound).
 //
-// Four launches per call (DESIGN.md 4.3): icp_dense_kernel (window search, bounded number of growing steps;
-// lanes still open are appended to a work list), block_range_kernel ([min, max] range per 4 x 16-cell block of the
-// target grids, overlapped with the tail of the first kernel), icp_dense_pending_kernel (one warp per open lane:
-// range-pruned block search, float64 tie re-ranking, accumulation by the warp that completes an item) and
-// icp_finalize_kernel (icp.cu: fixed-order fp64 column sums -> losses and the 3x4 transform gradient).
+// Four launches per call (DESIGN.md 4.3): target_extents_kernel ([min, max] range per 4 x 16-cell block and prefix /
+// suffix range extents per pixel row of the target grids), icp_dense_kernel (its programmatic dependent: window
+// search, bounded number of growing steps; lanes still open are appended to a work list), icp_dense_pending_kernel
+// (one warp per open lane: range-pruned block search, float64 tie re-ranking, accumulation by the warp that completes
+// an item) and icp_finalize_kernel (icp.cu: fixed-order fp64 column sums -> losses and the 3x4 transform gradient).
 #include <stdlib.h>
 #include <algorithm>
 #include "icp_common.cuh"
@@ -93,7 +94,7 @@ __device__ __noinline__ int nn_exact_rescan(const float4* __restrict__ tg, int H
 }
 
 // ---------------------------------------------------------------------------------------------
-// Range pyramid for the far / misaligned case.  The strip search above certifies exactness with a
+// Range pyramid for the far / misaligned case.  The strip search certifies its column borders with a
 // purely ANGULAR bound, so a source point that is d away from the target surface has to scan every
 // cell within the angle asin(d/r) -- thousands of cells when the predicted transform is still poor
 // (d ~ 1 m), although almost all of them are provably farther than d once their RANGE is taken into
@@ -108,34 +109,155 @@ constexpr int kBlkH = 4, kBlkW = 16;
 //  9 max blocks tested by one owner | 10 owners with > 256 blocks | 11 owners without any candidate so far |
 //  16..23 warps by strip count {0, 1-2, 3-5, 6-10, 11-20, 21-40, 41-63, >= limit} | 24..31 cells per lane, same buckets
 __device__ unsigned int g_dbg[32];
-constexpr int kDefaultMaxStrips = 16; // window-growing steps before a lane is handed to the block-search kernel
+constexpr int kDefaultMaxStrips = 32; // window-growing steps before a lane is handed to the block-search kernel
 
-__global__ void __launch_bounds__(256)
-block_range_kernel(const float4* __restrict__ grid, int H, int W, int nbh, int nbw, float2* __restrict__ blk) {
-    const int b = blockIdx.y;
-    const int warp = (blockIdx.x * 256 + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (warp >= nbh * nbw) return;
-    const int br = warp / nbw, bc = warp % nbw;
-    float lo = 3.0e38f, hi = -1.0f;
+// Range extents of the target grids, per pair:
+//   blk[nbh * nbw]       [min, max] of |t| per 4 x 16-cell block (the block search's pyramid)
+//   row_pre[H], row_suf[H]  [min, max] of |t| over the valid cells of the pixel rows <= k / >= k
+// Every extent is widened by a relative 1e-6 so that bounds built on it stay conservative against the fp32 norm
+// rounding; an empty block or row set has max < 0.
+struct TargetExtents {
+    float2* blk;
+    float2* row_pre;
+    float2* row_suf;
+    int* counter;          // per pair: CTAs of the pre-pass that have finished (0 when idle)
+};
+
+constexpr int kExtThreads = 1024, kExtUnroll = 4;
+
+// inclusive min / max scan of a[0..H) in place, forward (prefix) or backward (suffix); one warp.  min and max are
+// exact, so the result does not depend on the order of the combination.
+__device__ __forceinline__ void extent_scan(float2* __restrict__ a, int H, bool backward) {
+    const int lane = threadIdx.x & 31;
+    float2 carry = make_float2(3.0e38f, -3.0e38f);
+    for (int r0 = 0; r0 < H; r0 += 32) {
+        const int k = r0 + lane, r = backward ? H - 1 - k : k;
+        float2 v = (k < H) ? __ldcg(a + r) : make_float2(3.0e38f, -3.0e38f);
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-        const int c = lane + 32 * h;
-        const int row = br * kBlkH + (c >> 4), col = bc * kBlkW + (c & 15);
-        if (row < H && col < W) {
-            const float4 t = __ldg(grid + (size_t)b * H * W + (size_t)row * W + col);
-            if (__float_as_int(t.w) >= 0) {
-                const float rr = sqrtf(fmaf(t.z, t.z, fmaf(t.y, t.y, t.x * t.x)));
-                lo = fminf(lo, rr); hi = fmaxf(hi, rr);
+        for (int o = 1; o < 32; o <<= 1) {
+            const float ux = __shfl_up_sync(0xffffffffu, v.x, o), uy = __shfl_up_sync(0xffffffffu, v.y, o);
+            if (lane >= o) { v.x = fminf(v.x, ux); v.y = fmaxf(v.y, uy); }
+        }
+        v.x = fminf(v.x, carry.x); v.y = fmaxf(v.y, carry.y);
+        if (k < H) a[r] = v;
+        carry.x = __shfl_sync(0xffffffffu, v.x, 31); carry.y = __shfl_sync(0xffffffffu, v.y, 31);
+    }
+}
+
+// Pre-pass over the target grids: one CTA per (block row of kBlkH pixel rows, pair), each of the 32 warps takes every
+// 32nd block of the row, kExtUnroll blocks at a time (8 independent 16-byte loads per lane): at W = 2048 a CTA issues
+// all of its 128 KB at once.  The kernel is latency-bound, so it needs that many loads in flight.  The CTA writes its blocks and its
+// rows' extents; the last CTA of a pair turns the row extents into the prefix / suffix extents and re-arms the counter.
+// The window search is launched as this kernel's programmatic dependent: it may start once every CTA here has begun.
+__global__ void __launch_bounds__(kExtThreads)
+target_extents_kernel(const float4* __restrict__ grid, int H, int W, int nbh, int nbw, TargetExtents ext) {
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    constexpr int kWarps = kExtThreads / 32;
+    __shared__ float s_lo[kWarps][kBlkH], s_hi[kWarps][kBlkH];
+    __shared__ int is_last;
+    const int br = blockIdx.x, b = blockIdx.y;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const float4* __restrict__ tg = grid + (size_t)b * H * W;
+    float2* __restrict__ blk = ext.blk + (size_t)b * nbh * nbw;
+    // lane's cells of a block: (row (lane >> 4) + 2 h, column lane & 15), h = 0, 1
+    float rlo[2] = {3.0e38f, 3.0e38f}, rhi[2] = {-1.0f, -1.0f};
+    for (int bc0 = warp; bc0 < nbw; bc0 += kWarps * kExtUnroll) {
+        // all loads first (unconditional, at a clamped address), so that none waits behind a branch on another
+        float4 t[kExtUnroll][2];
+        bool in[kExtUnroll][2];
+#pragma unroll
+        for (int u = 0; u < kExtUnroll; ++u) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int c = lane + 32 * h;
+                const int row = br * kBlkH + (c >> 4), col = (bc0 + u * kWarps) * kBlkW + (c & 15);
+                in[u][h] = row < H && col < W;
+                t[u][h] = __ldg(tg + (size_t)min(row, H - 1) * W + min(col, W - 1));
             }
+        }
+        float rr[kExtUnroll][2];                                   // |t|, or -1 for an empty / outside cell
+#pragma unroll
+        for (int u = 0; u < kExtUnroll; ++u) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const float4 q = t[u][h];
+                rr[u][h] = (in[u][h] && __float_as_int(q.w) >= 0) ? sqrtf(fmaf(q.z, q.z, fmaf(q.y, q.y, q.x * q.x)))
+                                                                  : -1.0f;
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < kExtUnroll; ++u) {
+            const int bc = bc0 + u * kWarps;
+            float lo = 3.0e38f, hi = -1.0f;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                if (rr[u][h] >= 0.0f) {
+                    lo = fminf(lo, rr[u][h]); hi = fmaxf(hi, rr[u][h]);
+                    rlo[h] = fminf(rlo[h], rr[u][h]); rhi[h] = fmaxf(rhi[h], rr[u][h]);
+                }
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                lo = fminf(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+                hi = fmaxf(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+            }
+            if (lane == 0 && bc < nbw) blk[br * nbw + bc] = make_float2(lo * (1.0f - 1e-6f), hi * (1.0f + 1e-6f));
         }
     }
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        lo = fminf(lo, __shfl_xor_sync(0xffffffffu, lo, o));
-        hi = fmaxf(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int o = 8; o > 0; o >>= 1) {
+            rlo[h] = fminf(rlo[h], __shfl_xor_sync(0xffffffffu, rlo[h], o));
+            rhi[h] = fmaxf(rhi[h], __shfl_xor_sync(0xffffffffu, rhi[h], o));
+        }
+        if ((lane & 15) == 0) { s_lo[warp][(lane >> 4) + 2 * h] = rlo[h]; s_hi[warp][(lane >> 4) + 2 * h] = rhi[h]; }
     }
-    // widen by a relative 1e-6 so that the bound stays conservative against the fp32 norm rounding
-    if (lane == 0) blk[(size_t)b * nbh * nbw + warp] = make_float2(lo * (1.0f - 1e-6f), hi * (1.0f + 1e-6f));
+    __syncthreads();
+    if (threadIdx.x < kBlkH && br * kBlkH + (int)threadIdx.x < H) {
+        float lo = s_lo[0][threadIdx.x], hi = s_hi[0][threadIdx.x];
+#pragma unroll
+        for (int w = 1; w < kWarps; ++w) { lo = fminf(lo, s_lo[w][threadIdx.x]); hi = fmaxf(hi, s_hi[w][threadIdx.x]); }
+        const float2 e = make_float2(lo * (1.0f - 1e-6f), hi * (1.0f + 1e-6f));
+        const size_t r = (size_t)b * H + br * kBlkH + threadIdx.x;
+        ext.row_pre[r] = e;
+        ext.row_suf[r] = e;
+        __threadfence();
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) is_last = (atomicAdd(ext.counter + b, 1) == nbh - 1);
+    __syncthreads();
+    if (!is_last) return;
+    __threadfence();
+    if (warp == 0) extent_scan(ext.row_pre + (size_t)b * H, H, false);
+    if (warp == 1) extent_scan(ext.row_suf + (size_t)b * H, H, true);
+    if (threadIdx.x == 0) ext.counter[b] = 0;
+}
+
+// Lower bound of |s - t|^2 (times 0.999, the fp32 / __sinf margin) over targets t whose range |t| lies in
+// [rho.x, rho.y] and whose direction is at an angle theta from the source direction with sin^2(theta / 2) >= S:
+//     |s - t|^2 = (r - rho)^2 + 4 r rho sin^2(theta / 2)
+// is convex in rho with its minimum at rho = r (1 - 2 S), so the bound is its value there, clamped to the extent.
+// Over all rho >= 0 the minimum is r^2 sin^2(theta): never weaker than the purely angular bound.
+__device__ __forceinline__ float range_lb2(float r, float S, float2 rho) {
+    const float rh = fminf(fmaxf(r * (1.0f - 2.0f * S), rho.x), rho.y);
+    const float dr = r - rh;
+    return fmaf(dr, dr, 4.0f * r * rh * S) * 0.999f;
+}
+
+// Lower bound of the distance from the source point (range r) to every target beyond a ROW border that is `dpx`
+// pixels (of `rad_per_px` radians) of elevation away, when the rows beyond it have the range extent `rho`.
+// Exactness: a target in those rows differs from the source direction by at least the elevation gap, so
+// theta >= gap and sin^2(theta / 2) >= sin^2(gap / 2); the angular bound r sin(gap) is kept as a floor (the two are
+// equal at rho = r, and taking the larger is safe against the rounding of either).  No valid target beyond: no bound.
+// __sinf of the HALF angle: its absolute error (~2^-21.4) changes sin^2 by at most 2^-20.4 / (half angle) relative,
+// which the 0.999 margin on the squared bound covers for half angles >= 7.2e-4 rad.  A row border is at least
+// 1 - 2e-3 rows from the source direction, so this holds for row pitches down to 1.45e-3 rad (0.083 deg).
+__device__ __forceinline__ float row_border_bound(float dpx, float rad_per_px, float r, float2 rho) {
+    if (!(rho.y >= 0.0f)) return 3.0e38f;
+    const float d = fminf(fmaxf(dpx * rad_per_px, 0.0f), kHalfPiF);
+    const float sh = __sinf(0.5f * d);
+    return fmaxf(r * __sinf(d), sqrtf(range_lb2(r, sh * sh, rho)));
 }
 
 // first / last pixel column of the (unwrapped) block column bc; bc in [-nbw, 2 nbw)
@@ -215,11 +337,7 @@ __global__ void __launch_bounds__(kDenseThreads, 8)
 icp_dense_kernel(const float4* __restrict__ src_grid, const float4* __restrict__ src_ngrid,
                  const float* __restrict__ T, const float4* __restrict__ tgt_grid,
                  const float4* __restrict__ tgt_ngrid, int max_strips, GridParams g, uint32_t flags,
-                 float* __restrict__ partial_rows, int rows_per_pair, PendingList pend) {
-    // Programmatic dependent launch: the range-pyramid kernel that follows in the stream reads nothing this kernel
-    // writes, so it may start as soon as every CTA of this grid has been scheduled (it then fills the SMs that the
-    // last, partially filled wave leaves idle).  A no-op unless the next launch opts in.
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+                 float* __restrict__ partial_rows, int rows_per_pair, PendingList pend, TargetExtents ext) {
     const int b = blockIdx.y;
     const int H = g.H, W = g.W, HW = H * W;
     const float4* __restrict__ tg = tgt_grid + (size_t)b * HW;
@@ -232,20 +350,16 @@ icp_dense_kernel(const float4* __restrict__ src_grid, const float4* __restrict__
 
     const SrcLane s = load_src_lane(src_grid, src_ngrid, T, b, i, HW, g);
     const bool active = s.active;
+    const bool any_active = __ballot_sync(0xffffffffu, active) != 0u;
     const float sx = s.sx, sy = s.sy, sz = s.sz;
-    int best_j = -1;
-    if (__ballot_sync(0xffffffffu, active) != 0u) {
-        const float us = s.us, vs = s.vs, r = s.r, rxy = s.rxy;
-        const int rc = s.rc, cc = s.cc;
-        // distance (px) from the source direction to the four borders of its own centre cell
-        const float f_dn = (vs - (float)rc) + 0.5f - kSlack, f_up = ((float)rc - vs) + 0.5f - kSlack;
-        const float f_lf = (us - (float)cc) + 0.5f - kSlack, f_rt = ((float)cc - us) + 0.5f - kSlack;
-
-        NN2 nn;
-        nn.m1 = kInf; nn.m2 = kInf; nn.j1 = -1;
-        // warp-uniform window extents around every lane's own (rc, cc); the 3 x 5 start window is
-        // fully unrolled: 15 independent loads in flight
-        int e_dn = 1, e_up = 1, e_lf = 2, e_rt = 2;
+    const float us = s.us, vs = s.vs, r = s.r, rxy = s.rxy;
+    const int rc = s.rc, cc = s.cc;
+    NN2 nn;
+    nn.m1 = kInf; nn.m2 = kInf; nn.j1 = -1;
+    // warp-uniform window extents around every lane's own (rc, cc); the 3 x 5 start window is
+    // fully unrolled: 15 independent loads in flight
+    int e_dn = 1, e_up = 1, e_lf = 2, e_rt = 2;
+    if (any_active) {
         if (H >= 3 && W >= 5) {
             int col[5];
 #pragma unroll
@@ -263,8 +377,23 @@ icp_dense_kernel(const float4* __restrict__ src_grid, const float4* __restrict__
             e_dn = e_up = e_lf = e_rt = 0;
             nn2_eval(__ldg(tg + rc * W + cc), rc * W + cc, sx, sy, sz, nn, active);
         }
-        float b_dn = (rc - e_dn > 0) ? border_bound(f_dn + (float)e_dn, g.dv_rad, r) : kInf;
-        float b_up = (rc + e_up < H - 1) ? border_bound(f_up + (float)e_up, g.dv_rad, r) : kInf;
+    }
+    // Everything above reads only the source and target grids.  This kernel is the programmatic dependent of the
+    // target-extents pre-pass: wait for that grid (and its writes) before the first bound.  Every thread waits, so
+    // this grid never completes before the pre-pass has.
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    int best_j = -1;
+    if (any_active) {
+        // distance (px) from the source direction to the four borders of its own centre cell
+        const float f_dn = (vs - (float)rc) + 0.5f - kSlack, f_up = ((float)rc - vs) + 0.5f - kSlack;
+        const float f_lf = (us - (float)cc) + 0.5f - kSlack, f_rt = ((float)cc - us) + 0.5f - kSlack;
+        // row borders: angular + range bound over the rows beyond (row_border_bound); column borders: angular
+        const float2* __restrict__ row_pre = ext.row_pre + (size_t)b * H;
+        const float2* __restrict__ row_suf = ext.row_suf + (size_t)b * H;
+        float b_dn = (rc - e_dn > 0) ? row_border_bound(f_dn + (float)e_dn, g.dv_rad, r, __ldg(row_pre + rc - e_dn - 1))
+                                     : kInf;
+        float b_up = (rc + e_up < H - 1) ? row_border_bound(f_up + (float)e_up, g.dv_rad, r, __ldg(row_suf + rc + e_up + 1))
+                                         : kInf;
         // a border at or beyond the +-180 deg seam is seam_px closer than its unwrapped pixel distance
         float b_lf = (e_lf + e_rt + 1 >= W) ? kInf
                    : border_bound(f_lf + (float)e_lf - (cc - e_lf <= 0 ? g.seam_px : 0.0f), g.du_rad, rxy);
@@ -314,8 +443,13 @@ icp_dense_kernel(const float4* __restrict__ src_grid, const float4* __restrict__
                     ++col;
                     col = (col == W) ? 0 : col;
                 }
-                if (side == 0) b_dn = (rc - e_dn > 0) ? border_bound(f_dn + (float)e_dn, g.dv_rad, r) : kInf;
-                else           b_up = (rc + e_up < H - 1) ? border_bound(f_up + (float)e_up, g.dv_rad, r) : kInf;
+                if (side == 0)
+                    b_dn = (rc - e_dn > 0) ? row_border_bound(f_dn + (float)e_dn, g.dv_rad, r, __ldg(row_pre + rc - e_dn - 1))
+                                           : kInf;
+                else
+                    b_up = (rc + e_up < H - 1)
+                               ? row_border_bound(f_up + (float)e_up, g.dv_rad, r, __ldg(row_suf + rc + e_up + 1))
+                               : kInf;
             } else {
                 const int step = min(2, W - (e_lf + e_rt + 1));
                 const int c0 = wrap_col((side == 2) ? cc - e_lf - 1 : cc + e_rt + 1, W);
@@ -417,10 +551,7 @@ __device__ __forceinline__ int block_pass(const float4* __restrict__ tg, const f
                 const float sv = __sinf(fminf(0.5f * gv, kHalfPiF)), su = __sinf(fminf(0.5f * gu, kHalfPiF));
                 const float e_lo = g.vf0 + v_lo * g.dv_rad, e_hi = g.vf0 + v_hi * g.dv_rad;
                 const float c_blk = fmaxf(fminf(__cosf(e_lo), __cosf(e_hi)), 0.0f);
-                const float S = fmaxf(sv * sv, o.cos_es * c_blk * su * su);
-                const float rho = fminf(fmaxf(o.r * (1.0f - 2.0f * S), rg.x), rg.y);
-                const float dr_ = o.r - rho;
-                lb2 = fmaf(dr_, dr_, 4.0f * o.r * rho * S) * 0.999f;
+                lb2 = range_lb2(o.r, fmaxf(sv * sv, o.cos_es * c_blk * su * su), rg);
             } else {
                 ok = false;                                       // empty block
             }
@@ -491,7 +622,7 @@ template <bool PO2PO, bool STATS>
 __global__ void __launch_bounds__(kPendThreads, 4)
 icp_dense_pending_kernel(const float4* __restrict__ src_grid, const float4* __restrict__ src_ngrid,
                          const float* __restrict__ T, const float4* __restrict__ tgt_grid,
-                         const float4* __restrict__ tgt_ngrid, const float2* __restrict__ blk_range, int nbh, int nbw,
+                         const float4* __restrict__ tgt_ngrid, TargetExtents ext, int nbh, int nbw,
                          GridParams g, uint32_t flags, float* __restrict__ partial_rows, int rows_per_pair,
                          PendingList pend) {
     const int H = g.H, W = g.W, HW = H * W;
@@ -508,7 +639,7 @@ icp_dense_pending_kernel(const float4* __restrict__ src_grid, const float4* __re
         const int b = it.x, warp_in_pair = it.y;
         const unsigned pending = (unsigned)it.z;
         const float4* __restrict__ tg = tgt_grid + (size_t)b * HW;
-        const float2* __restrict__ blk = blk_range + (size_t)b * nbh * nbw;
+        const float2* __restrict__ blk = ext.blk + (size_t)b * nbh * nbw;
         // every lane rebuilds the SAME source point (uniform addresses: broadcast loads)
         const SrcLane o = load_src_lane(src_grid, src_ngrid, T, b, warp_in_pair * 32 + owner, HW, g);
         const float osx = o.sx, osy = o.sy, osz = o.sz, orr = o.r, ous = o.us, ovs = o.vs, orxy = o.rxy;
@@ -525,9 +656,13 @@ icp_dense_pending_kernel(const float4* __restrict__ src_grid, const float4* __re
         const float obest0 = obest;
         const float d0 = (obest < kInf) ? sqrtf(obest) * (1.00001f / 0.9995f) : kInf;
         int br_lo = obr, br_hi = obr, bc_lo = obc, bc_hi = obc;            // bc_* unwrapped
-        while (br_lo > 0 && border_bound(ovs - ((float)(br_lo * kBlkH) - 0.5f) - kSlack, g.dv_rad, orr) < d0) --br_lo;
-        while (br_hi < nbh - 1 &&
-               border_bound(((float)min(br_hi * kBlkH + kBlkH - 1, H - 1) + 0.5f) - ovs - kSlack, g.dv_rad, orr) < d0)
+        const float2* __restrict__ row_pre = ext.row_pre + (size_t)b * H;
+        const float2* __restrict__ row_suf = ext.row_suf + (size_t)b * H;
+        while (br_lo > 0 && row_border_bound(ovs - ((float)(br_lo * kBlkH) - 0.5f) - kSlack, g.dv_rad, orr,
+                                             __ldg(row_pre + br_lo * kBlkH - 1)) < d0)
+            --br_lo;
+        while (br_hi < nbh - 1 && row_border_bound(((float)(br_hi * kBlkH + kBlkH - 1) + 0.5f) - ovs - kSlack, g.dv_rad,
+                                                   orr, __ldg(row_suf + br_hi * kBlkH + kBlkH)) < d0)
             ++br_hi;
         // (unwrapped block columns: W need not be a multiple of kBlkW, so the pixel span of block column
         //  bc outside [0, nbw) is that of its wrapped twin shifted by +-W, not bc * kBlkW)
@@ -628,24 +763,6 @@ extern "C" int delora_icp_stats(uint32_t* out32, int reset) {
     return 0;
 }
 
-// The range pyramid of the target grids is independent of the window-search kernel launched just before it:
-// programmatic stream serialization lets it overlap that kernel's tail (icp_dense_kernel issues
-// griddepcontrol.launch_dependents); the block-search kernel after it is a normal launch and waits for both.
-static cudaError_t launch_block_range(cudaStream_t st, const float4* tgt_grid, int B, int H, int W, int nbh, int nbw,
-                                      float2* blk) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((nbh * nbw * 32 + 255) / 256, B);
-    cfg.blockDim = dim3(256);
-    cfg.dynamicSmemBytes = 0;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, block_range_kernel, tgt_grid, H, W, nbh, nbw, blk);
-}
-
 extern "C" int delora_icp_dense_fwd_bwd(const delora_f4* src_grid, const delora_f4* src_ngrid, const float* T,
                                         const delora_f4* tgt_grid, const delora_f4* tgt_ngrid, int B, int H, int W,
                                         double hfov0, double hfov1, double vfov0, double vfov1, float lambda_po2pl,
@@ -665,8 +782,14 @@ extern "C" int delora_icp_dense_fwd_bwd(const delora_f4* src_grid, const delora_
     // work list of the second kernel (see delora_icp_scratch_floats)
     const int nbh = (H + kBlkH - 1) / kBlkH, nbw = (W + kBlkW - 1) / kBlkW;
     size_t off = (size_t)B * rows * DELORA_ICP_PARTIAL + (size_t)B * DELORA_ICP_PARTIAL + (((size_t)B + 1) & ~(size_t)1);
-    float2* blk = reinterpret_cast<float2*>(scratch + off);
+    TargetExtents ext;
+    ext.blk = reinterpret_cast<float2*>(scratch + off);
     off += (size_t)B * 2 * ((size_t)HW / 16 + 4096);
+    ext.row_pre = reinterpret_cast<float2*>(scratch + off);
+    ext.row_suf = ext.row_pre + (size_t)B * H;
+    off += (size_t)B * 4 * H;
+    ext.counter = reinterpret_cast<int*>(scratch + off);
+    off += B;
     off = (off + 3) & ~(size_t)3;                      // 16-byte alignment
     PendingList pend;
     pend.counters = reinterpret_cast<int*>(scratch + off);
@@ -677,15 +800,28 @@ extern "C" int delora_icp_dense_fwd_bwd(const delora_f4* src_grid, const delora_
     // persistent second kernel: enough CTAs for one wave, never more than there can be items
     const int pend_threads = kPendThreads, pend_mult = 4;     // up to 4 CTAs per SM
     const int pend_grid = (int)std::min<long long>(((long long)B * rows * 32 + 7) / 8, (long long)pend_mult * num_sms());
+    // the window search is the programmatic dependent of the pre-pass (see griddepcontrol.wait in the kernel): its
+    // CTAs load their source lanes and start windows while the pre-pass is still running
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = dim3(kDenseThreads);
+    cfg.dynamicSmemBytes = 0;
+    cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    target_extents_kernel<<<dim3(nbh, B), kExtThreads, 0, st>>>((const float4*)tgt_grid, H, W, nbh, nbw, ext);
+    DELORA_CHECK_LAUNCH("target_extents_kernel");
 #define DELORA_LAUNCH_DENSE(PO2PO, STATS)                                                                           \
     do {                                                                                                            \
-        icp_dense_kernel<PO2PO, STATS><<<grid, kDenseThreads, 0, st>>>(                                             \
-            (const float4*)src_grid, (const float4*)src_ngrid, T, (const float4*)tgt_grid, (const float4*)tgt_ngrid, \
-            max_strips, g, flags, sc.rows, rows, pend);                                                             \
-        launch_block_range(st, (const float4*)tgt_grid, B, H, W, nbh, nbw, blk);                                    \
+        cudaLaunchKernelEx(&cfg, icp_dense_kernel<PO2PO, STATS>, (const float4*)src_grid, (const float4*)src_ngrid, \
+                           T, (const float4*)tgt_grid, (const float4*)tgt_ngrid, max_strips, g, flags, sc.rows,     \
+                           rows, pend, ext);                                                                        \
         icp_dense_pending_kernel<PO2PO, STATS><<<pend_grid, pend_threads, 0, st>>>(                                 \
             (const float4*)src_grid, (const float4*)src_ngrid, T, (const float4*)tgt_grid, (const float4*)tgt_ngrid, \
-            blk, nbh, nbw, g, flags, sc.rows, rows, pend);                                                          \
+            ext, nbh, nbw, g, flags, sc.rows, rows, pend);                                                          \
     } while (0)
     const bool po2po = (flags & DELORA_LOSS_PO2PO) != 0u, stats = (flags & DELORA_ICP_STATS) != 0u;
     if (po2po && stats) DELORA_LAUNCH_DENSE(true, true);

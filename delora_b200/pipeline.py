@@ -58,7 +58,7 @@ class ScanPairPipeline:
                     self._subs.append({"b0": b0, "n": b1 - b0, "stream": torch.cuda.Stream(device=dev),
                                        "scratch": ops.icp_scratch(b1 - b0, hw, dev), "done": torch.cuda.Event()})
             self._fork = torch.cuda.Event()
-        # per step: (scatter + resolve) + normals + (block_range + icp_dense + icp_dense_pending + finalize); with
+        # per step: (scatter + resolve) + normals + (target_extents + icp_dense + icp_dense_pending + finalize); with
         # sub-batches the two scans of a pair are separate image ranges -> two projection / normals calls each
         self.launches_per_step = (2 + 1 + 4) if not self._subs else len(self._subs) * (2 * 2 + 2 * 1 + 4)
 

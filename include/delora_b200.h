@@ -196,9 +196,10 @@ int delora_icp_fwd_bwd(const delora_f4* src_pts4, const delora_f4* src_nrm4, con
  * (src/deploy/deployer.py:252-261 keeps exactly one point per pixel of both scans).
  * src_grid/src_ngrid, tgt_grid/tgt_ngrid: [B, H*W] float4;  T: [B, 12];
  * scratch: fp32 [delora_icp_scratch_floats(B, H*W)], zeroed once (see above).
- * Launches block_range_kernel, icp_dense_kernel (window search, at most 16 growing steps per warp; the environment
- * variable DELORA_ICP_MAX_STRIPS overrides the limit for profiling), icp_dense_pending_kernel (range-pruned block
- * search of the lanes still open) and icp_finalize_kernel; results do not depend on the limit. */
+ * Launches target_extents_kernel (range extents of the target grids), icp_dense_kernel (window search, at most 32
+ * growing steps per warp; the environment variable DELORA_ICP_MAX_STRIPS overrides the limit for profiling),
+ * icp_dense_pending_kernel (range-pruned block search of the lanes still open) and icp_finalize_kernel; results do
+ * not depend on the limit. */
 int delora_icp_dense_fwd_bwd(const delora_f4* src_grid, const delora_f4* src_ngrid, const float* T,
                              const delora_f4* tgt_grid, const delora_f4* tgt_ngrid, int B, int H, int W,
                              double hfov0, double hfov1, double vfov0, double vfov1,

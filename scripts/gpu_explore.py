@@ -46,22 +46,43 @@ step = timeit(lambda: pipe.step(), "full step")
 print(f"sum of parts {tot*1e3:.1f} us; step {step*1e3:.1f} us -> {B/(step*1e-3):.0f} pairs/s")
 print("losses", pipe.losses[0].tolist())
 import json
+from torch.profiler import profile, ProfilerActivity
+
 def t_icp_stats():
     _lib.check(L.delora_icp_dense_fwd_bwd(pipe.pts_grid.data_ptr() + B * hw * 16, pipe.nrm_grid.data_ptr() + B * hw * 16, pipe.transform.data_ptr(), pipe.pts_grid.data_ptr(), pipe.nrm_grid.data_ptr(), B, H, W, hf[0], hf[1], vf[0], vf[1], 1.0, 6 | ops.ICP_STATS, pipe.losses.data_ptr(), pipe.grad_T.data_ptr(), pipe.icp_scratch.data_ptr(), st), "i")
 def stats(tag):
     ops.icp_stats(reset=True); t_icp_stats(); torch.cuda.synchronize()
     print(tag, json.dumps(ops.icp_stats(reset=True)))
-stats("stats(predicted T)")
-# misaligned case: identity transform instead of the (nearly correct) predicted one -> NN distances ~0.5 m
+
+def split(tag, reps=10):
+    """Per-kernel split of one ICP call (torch.profiler, a run of its own; L2 flushed before every call)."""
+    t_icp(); torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(reps):
+            flush.zero_(); t_icp()
+        torch.cuda.synchronize()
+    parts = []
+    for e in prof.key_averages():
+        if "icp" in e.key or "extents" in e.key:
+            us = getattr(e, "device_time_total", None) or getattr(e, "cuda_time_total", 0.0)
+            parts.append((e.key.split("(")[0].split("<")[0].replace("void ", "").replace("delora::", ""), us / reps))
+    print(f"split({tag})", "  ".join(f"{n} {t:.1f} us" for n, t in sorted(parts, key=lambda x: -x[1])),
+          f"  sum {sum(t for _, t in parts):.1f} us")
+
+def case(tag, iters=20):
+    timeit(t_icp, "icp_" + tag, iters=iters)
+    split(tag)
+    stats(f"stats({tag})")
+    print(f"losses({tag})", pipe.losses[0].tolist())
+
+case("predictedT")
+# misaligned cases (what an untrained network produces): identity transform instead of the (nearly correct)
+# predicted one -> NN distances ~0.5 m; and a bad transform (2 m, 10 deg)
 import math
 saved_T = pipe.transform.clone()
 pipe.transform.copy_(torch.eye(4, device="cuda")[:3, :].reshape(1, 12).repeat(B, 1))
-timeit(t_icp, "icp_identityT")
-stats("stats(identity T)")
-print("losses(identity T)", pipe.losses[0].tolist())
+case("identityT")
 tb = torch.from_numpy(synthetic.transform_matrix(2.0, 1.0, 0.3, math.radians(10.0), math.radians(2.0), 0.0)).float().cuda()
 pipe.transform.copy_(tb[:3, :].reshape(1, 12).repeat(B, 1))
-timeit(t_icp, "icp_badT", iters=5)
-stats("stats(bad T)")
-print("losses(bad T)", pipe.losses[0].tolist())
+case("badT", iters=5)
 pipe.transform.copy_(saved_T)

@@ -121,7 +121,7 @@ def main():
             # bench.py reads the per-OPERATOR totals (operator = the kernels one C-ABI call launches)
             ops = {"projection": ("project_scatter_kernel", "project_resolve_kernel"),
                    "normals": ("normals_7x11_kernel",),
-                   "icp": ("icp_dense_kernel", "icp_dense_pending_kernel", "icp_finalize_kernel", "block_range_kernel")}
+                   "icp": ("icp_dense_kernel", "icp_dense_pending_kernel", "icp_finalize_kernel", "target_extents_kernel")}
             doc = {}
             for op, names in ops.items():
                 tot = sum(t["dram_bytes"] for k, t in traffic.items() if k.split("<")[0] in names)
