@@ -1,0 +1,31 @@
+#!/usr/bin/env python3
+"""Write a checkpoint's model as a .dlw weight file for the C ABI's `delora_odometry_*` entry points
+(delora_b200/deploy/export.py; byte layout in include/delora_b200.h).  The image size and fields of view come from
+the checkpoint's `parameters` when it has them (they win over config/*.yaml, as in bin/run_testing.py);
+`--n_stride` (max points per scan) and `--max_batch` (max pairs per delora_odometry_pairs call) size the buffers."""
+import os
+import sys
+
+import click
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+from delora_b200.deploy import export as export_module  # noqa: E402
+
+
+@click.command()
+@click.option("--checkpoint", required=True, help="Checkpoint written by the trainer (torch.save).")
+@click.option("--dataset", default="kitti", show_default=True, help="Dataset whose range image the model runs on.")
+@click.option("--out", required=True, help="Output .dlw file.")
+@click.option("--n_stride", default=131072, show_default=True, help="Max points per scan.")
+@click.option("--max_batch", default=1, show_default=True, help="Max pairs per delora_odometry_pairs call.")
+@click.option("--config_dir", default="config", show_default=True, help="YAML files, used when the checkpoint has no "
+              "`parameters`.")
+def main(checkpoint, dataset, out, n_stride, max_batch, config_dir):
+    d = export_module.export(checkpoint, dataset, out, n_stride, max_batch, config_dir)
+    print(f"wrote {out}: {d.H}x{d.W}, layers {list(d.layers)}, act {'relu' if d.act == 1 else 'tanh'}, "
+          f"resnet_outputs {d.resnet_outputs}, single_mlp {d.single_mlp}, n_stride {d.n_stride}, max_batch {d.max_batch}")
+
+
+if __name__ == "__main__":
+    main()

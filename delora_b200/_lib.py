@@ -10,6 +10,16 @@ LIB_PATH = os.path.join(_HERE, "libdelora_b200.so")
 c_int, c_float, c_double, c_void_p = ctypes.c_int, ctypes.c_float, ctypes.c_double, ctypes.c_void_p
 c_u32, c_i64 = ctypes.c_uint32, ctypes.c_int64
 
+
+class OdometryDesc(ctypes.Structure):
+    """delora_odometry_desc (include/delora_b200.h): the model and buffer sizes of the odometry entry points."""
+    _fields_ = [("H", c_int), ("W", c_int), ("hfov0", c_double), ("hfov1", c_double), ("vfov0", c_double),
+                ("vfov1", c_double), ("n_stride", c_int), ("max_batch", c_int), ("act", c_int),
+                ("layers", c_int * 4), ("resnet_outputs", c_int), ("single_mlp", c_int)]
+
+
+c_desc_p = ctypes.POINTER(OdometryDesc)
+
 # name -> (restype, argtypes); every symbol declared in include/delora_b200.h
 SIGNATURES = {
     "delora_abi_version": (c_int, []),
@@ -71,9 +81,15 @@ SIGNATURES = {
     "delora_grad_allreduce_flag_words": (c_int, []),
     "delora_grad_allreduce_f32": (c_int, [c_void_p, c_void_p, ctypes.c_uint64, c_int, c_int, ctypes.c_longlong,
                                           ctypes.c_longlong, c_float, c_u32, c_int, c_int, c_void_p, c_void_p]),
+    "delora_odometry_weight_floats": (c_i64, [c_desc_p]),
+    "delora_odometry_workspace_bytes": (c_i64, [c_desc_p]),
+    "delora_odometry_init": (c_int, [c_desc_p, c_void_p, c_void_p]),
+    "delora_odometry_load_weights": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_pairs": (c_int, [c_desc_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_push": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 _lib = None
 
 

@@ -174,6 +174,22 @@ __device__ __forceinline__ void pixel_coords(const GridParams& g, float x, float
     }
 }
 
+// kornia 0.3.0 quaternion_to_rotation_matrix ((x,y,z,w), L2-normalised with eps 1e-12) and the
+// [R|t; 0 0 0 1] assembly of src/models/model_parts.py:37-44, for one batch element: q[4], t[3] -> o[16].
+__device__ __forceinline__ void quat_to_T_row(float qx, float qy, float qz, float qw, float t0, float t1, float t2,
+                                              float* __restrict__ o) {
+    const float nrm = fmaxf(sqrtf(qx * qx + qy * qy + qz * qz + qw * qw), 1e-12f);
+    const float x = qx / nrm, y = qy / nrm, z = qz / nrm, w = qw / nrm;
+    const float tx = 2.f * x, ty = 2.f * y, tz = 2.f * z;
+    const float twx = tx * w, twy = ty * w, twz = tz * w;
+    const float txx = tx * x, txy = ty * x, txz = tz * x;
+    const float tyy = ty * y, tyz = tz * y, tzz = tz * z;
+    o[0] = 1.f - (tyy + tzz); o[1] = txy - twz;         o[2] = txz + twy;         o[3] = t0;
+    o[4] = txy + twz;         o[5] = 1.f - (txx + tzz); o[6] = tyz - twx;         o[7] = t1;
+    o[8] = txz - twy;         o[9] = tyz + twx;         o[10] = 1.f - (txx + tyy); o[11] = t2;
+    o[12] = 0.f; o[13] = 0.f; o[14] = 0.f; o[15] = 1.f;
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

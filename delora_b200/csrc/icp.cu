@@ -273,24 +273,13 @@ icp_point_grads_kernel(const float4* __restrict__ point_dir, const float4* __res
     gn[0] = hx; gn[src_stride] = hy; gn[2 * (size_t)src_stride] = hz;
 }
 
-// kornia 0.3.0 quaternion_to_rotation_matrix ((x,y,z,w), L2-normalised with eps 1e-12) and the
-// [R|t; 0 0 0 1] assembly of src/models/model_parts.py:37-44; one thread per batch element.
+// quaternion + translation -> 4x4 (quat_to_T_row, common.cuh); one thread per batch element.
 __global__ void quat_to_T_kernel(const float* __restrict__ quat, const float* __restrict__ trans, int B,
                                  float* __restrict__ T) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= B) return;
-    const float qx = quat[b * 4 + 0], qy = quat[b * 4 + 1], qz = quat[b * 4 + 2], qw = quat[b * 4 + 3];
-    const float nrm = fmaxf(sqrtf(qx * qx + qy * qy + qz * qz + qw * qw), 1e-12f);
-    const float x = qx / nrm, y = qy / nrm, z = qz / nrm, w = qw / nrm;
-    const float tx = 2.f * x, ty = 2.f * y, tz = 2.f * z;
-    const float twx = tx * w, twy = ty * w, twz = tz * w;
-    const float txx = tx * x, txy = ty * x, txz = tz * x;
-    const float tyy = ty * y, tyz = tz * y, tzz = tz * z;
-    float* __restrict__ o = T + (size_t)b * 16;
-    o[0] = 1.f - (tyy + tzz); o[1] = txy - twz;         o[2] = txz + twy;         o[3] = trans[b * 3 + 0];
-    o[4] = txy + twz;         o[5] = 1.f - (txx + tzz); o[6] = tyz - twx;         o[7] = trans[b * 3 + 1];
-    o[8] = txz - twy;         o[9] = tyz + twx;         o[10] = 1.f - (txx + tyy); o[11] = trans[b * 3 + 2];
-    o[12] = 0.f; o[13] = 0.f; o[14] = 0.f; o[15] = 1.f;
+    quat_to_T_row(quat[b * 4 + 0], quat[b * 4 + 1], quat[b * 4 + 2], quat[b * 4 + 3], trans[b * 3 + 0],
+                  trans[b * 3 + 1], trans[b * 3 + 2], T + (size_t)b * 16);
 }
 
 __global__ void quat_to_T_bwd_kernel(const float* __restrict__ quat, const float* __restrict__ gT, int B,

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DELORA_B200_ABI_VERSION 2
+#define DELORA_B200_ABI_VERSION 3
 
 /* float4-packed list element: (x, y, z, tag).  `tag` is an int32 bit pattern or a float flag,
  * as documented per array. */
@@ -331,6 +331,79 @@ int delora_nhwc_to_nchw_f32(const void* x, int B, int H, int W, int C, float* y,
 int delora_quat_to_T(const float* quaternion, const float* translation, int B, float* T, void* stream);
 int delora_quat_to_T_bwd(const float* quaternion, const float* grad_T, int B,
                          float* grad_quaternion, float* grad_translation, void* stream);
+
+/* ---------------------------------------------------------------------------------------
+ * Odometry inference: raw scans -> relative transforms, the whole model behind one call.
+ * Replaces, for inference, deploy.tester.Tester.test_dataset's per-frame path
+ *   (src/deploy/tester.py:38-107 -> src/deploy/deployer.py:237-281): the projection of both scans,
+ *   models.model.OdometryModel.forward (src/models/model.py:96-116: encoder trunk, resnet.fc, the two MLP
+ *   heads or the single MLP, quaternion / norm of the whole [B,4] block) and GeometryHandler's quaternion -> T.
+ *
+ * The trunk runs the kernels above in the order the Python encoder runs them (the projected images are
+ * bit-identical to delora_project_fwd's, the pooled features to the Python trunk's); the fully connected tail is one
+ * fp32 launch per layer (odometry_linear_kernel) plus one launch for the last layer, the norm and quaternion -> T
+ * (odometry_out_kernel), with a fixed summation order.  Not representable: pre_feature_extraction,
+ * factor_fewer_resnet_channels != 1; dropout is the identity at inference.
+ *
+ * Workspace: one caller-owned device buffer of delora_odometry_workspace_bytes(d) bytes holds every activation,
+ * the bf16 filters, the fp32 tail weights and the stream's cached range image.  Its layout is a function of the
+ * descriptor only.  Use: _init once, _load_weights, then any number of _pairs / _push calls.  One workspace serves
+ * one stream of calls at a time.
+ */
+typedef struct {
+    int H, W;                            /* range image of the model (vertical_cells, horizontal_cells);
+                                            (W - 1) / 2 + 1 must be even (the stem's max-pool halves it) */
+    double hfov0, hfov1, vfov0, vfov1;   /* radians, as the bin scripts pass them */
+    int n_stride;                        /* max points per scan: the point stride of `points` */
+    int max_batch;                       /* max pairs per delora_odometry_pairs call (1 .. 1024) */
+    int act;                             /* 1 relu, 2 tanh */
+    int layers[4];                       /* BasicBlocks per stage, e.g. {2,2,2,2} (1 .. 16 each) */
+    int resnet_outputs;                  /* fc width, 1000 in the shipped config */
+    int single_mlp;                      /* use_single_mlp_at_output (0 / 1) */
+} delora_odometry_desc;
+
+/* Weight file (.dlw, written by delora_b200/deploy/export.py), little-endian, readable with fread alone:
+ *   bytes   0..127  delora_odometry_file_header below (explicit offsets: magic 0, abi_version 8, header_bytes 12,
+ *                   desc 16: H 16, W 20, hfov0 24, hfov1 32, vfov0 40, vfov1 48, n_stride 56, max_batch 60, act 64,
+ *                   layers 68..83, resnet_outputs 84, single_mlp 88, 4 pad bytes; blob_floats 96; zero 104..127)
+ *   bytes 128..     float32[blob_floats]: the tensors of OdometryModel.state_dict() concatenated in state_dict order,
+ *                   each tensor row-major (the blob delora_odometry_load_weights takes). */
+#define DELORA_ODOMETRY_FILE_MAGIC "DELORAW"     /* 7 characters + NUL = the 8 magic bytes */
+typedef struct {
+    char magic[8];
+    int32_t abi_version;                 /* DELORA_B200_ABI_VERSION of the exporter */
+    int32_t header_bytes;                /* 128 */
+    delora_odometry_desc desc;
+    int64_t blob_floats;                 /* == delora_odometry_weight_floats(&desc) */
+    uint8_t reserved[24];
+} delora_odometry_file_header;
+
+/* Host only (no GPU needed): validate the descriptor (non-zero + delora_last_error() if it is invalid; the size
+ * functions then return -1) and size the weight blob / the workspace. */
+int64_t delora_odometry_weight_floats(const delora_odometry_desc* d);
+int64_t delora_odometry_workspace_bytes(const delora_odometry_desc* d);
+/* Zero the workspace (every activation buffer's zero halo rows) and set the projection key buffer to all ones.
+ * Once after allocation; later calls never write those regions except as the kernels above do. */
+int delora_odometry_init(const delora_odometry_desc* d, void* workspace, void* stream);
+/* weights: DEVICE fp32[delora_odometry_weight_floats(d)], the .dlw blob.  Converts the convolution filters to the bf16
+ * layouts (delora_conv_weight_prep_multi) and copies the fc / head tensors into the workspace; every weight region is
+ * rewritten, so loading a second blob replaces the first completely.  `weights` must stay valid until the stream has
+ * run the call.  The prep table is copied from host memory (the call may wait for the stream to reach it). */
+int delora_odometry_load_weights(const delora_odometry_desc* d, const float* weights, void* workspace, void* stream);
+/* B pairs (1 <= B <= max_batch): points [2B, 3, n_stride] fp32 (scan_1 of pair 0..B-1, then scan_2 of pair 0..B-1),
+ * n_points [2B] int32 (device).  T [B, 16] out (row-major 4x4: scan_2 -> scan_1 frame); pooled [B, 512] fp32 out
+ * (the average-pooled encoder features) or NULL.  The quaternion is divided by the norm of the whole [B, 4] block
+ * (src/models/model.py:114), so a row's T can differ in the last bits with the batch it was computed in.
+ * Device counts above n_stride are clamped to n_stride on the device (a host-side check would need a synchronise).
+ * Only launches: no allocation, no synchronisation, no host decision on device data. */
+int delora_odometry_pairs(const delora_odometry_desc* d, const float* points, const int32_t* n_points, int B,
+                          void* workspace, float* T, float* pooled, void* stream);
+/* Streaming, batch 1: project the frame points [1, 3, n_stride] (n_points [1], device), run the model on (cached
+ * previous image, this image), write T [16], then cache this image.  T == NULL: only project and cache (the first
+ * frame of a stream).  Bit-identical to delora_odometry_pairs with B = 1 on (previous scan, this scan).  With T
+ * non-NULL the launch sequence is fixed, so one call can be captured into a CUDA graph and replayed per frame. */
+int delora_odometry_push(const delora_odometry_desc* d, const float* points, const int32_t* n_points,
+                         void* workspace, float* T, void* stream);
 
 /* ---- Data-parallel training step: average of the weight gradients over the ranks (SURVEY.md 8(e); the reference
  * steps one optimizer on one device, src/deploy/trainer.py:23-24, on `loss / batch_size`, src/deploy/deployer.py:329-342
