@@ -32,6 +32,9 @@ SIGNATURES = {
     "delora_sort_by_range": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "delora_normals_fwd": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_int, c_void_p,
                                    c_void_p, c_void_p, c_void_p]),
+    "delora_project_normals_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_double, c_double,
+                                           c_double, c_double, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                           c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "delora_scan_blocks": (c_int, [c_int]),
     "delora_lists_from_images": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                          c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -6,20 +6,23 @@
 // the CPU) and scatters the survivors (:98-103).  "First in range order" == "minimum range",
 // so here every point does one 64-bit atomicMin of (range_bits << 32 | point_index) on its
 // pixel (equal ranges: lowest index wins == a stable sort); a second pass resolves the winners
-// into the image and the pixel -> point index map and re-arms the key buffer.
+// into the image and the pixel -> point index map and re-arms the key buffer.  delora_project_normals_fwd
+// (normals.cu) runs the same scatter and resolves the keys inside its 7x11 normals kernel instead.
 //
 // HBM/L2 traffic per scan: read 12 N (xyz) [+ 8 HW key RMW in L2] ; write 4 (C+1) HW + 4 HW.
-#include "common.cuh"
+#include "projection.cuh"
 
 namespace delora {
 
 constexpr int kScatterThreads = 256;
 constexpr int kScatterPPT = 4;       // points per thread (independent loads in flight)
-constexpr unsigned long long kEmptyKey = 0xFFFFFFFFFFFFFFFFull;
 
 __global__ void __launch_bounds__(kScatterThreads)
 project_scatter_kernel(const float* __restrict__ points, const int32_t* __restrict__ n_points,
                        int C, int n_stride, GridParams g, unsigned long long* __restrict__ keys) {
+    // A programmatic dependent (project_normals_7x11_kernel) may start its key-independent prologue on SMs this grid
+    // frees; it waits for this whole grid before it reads a key.
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     const int b = blockIdx.y;
     const int n = n_points[b];
     const int base = blockIdx.x * (kScatterThreads * kScatterPPT) + threadIdx.x;
@@ -149,6 +152,13 @@ project_uv_kernel(const float* __restrict__ points, const int32_t* __restrict__ 
     if (r_out) r_out[(size_t)b * n_stride + idx] = range3(x, y, z);
 }
 
+void launch_project_scatter(const float* points, const int32_t* n_points, int B, int C, int n_stride,
+                            const GridParams& g, unsigned long long* keys, cudaStream_t st) {
+    const int per_block = kScatterThreads * kScatterPPT;
+    dim3 grid((n_stride + per_block - 1) / per_block, B);
+    project_scatter_kernel<<<grid, kScatterThreads, 0, st>>>(points, n_points, C, n_stride, g, keys);
+}
+
 }  // namespace delora
 
 using namespace delora;
@@ -163,10 +173,7 @@ extern "C" int delora_project_fwd(const float* points, const int32_t* n_points, 
     DELORA_CHECK_ARG((long long)H * W < (1ll << 31) && B <= 65535, "delora_project_fwd: image or batch too large");
     cudaStream_t st = (cudaStream_t)stream;
     const GridParams g = make_grid(H, W, hfov0, hfov1, vfov0, vfov1, div_mode);
-    const int per_block = kScatterThreads * kScatterPPT;
-    dim3 grid1((n_stride + per_block - 1) / per_block, B);
-    project_scatter_kernel<<<grid1, kScatterThreads, 0, st>>>(points, n_points, C, n_stride, g,
-                                                              (unsigned long long*)keys);
+    launch_project_scatter(points, n_points, B, C, n_stride, g, (unsigned long long*)keys, st);
     DELORA_CHECK_LAUNCH("project_scatter_kernel");
     const int HW = H * W;
     dim3 grid2((HW + 1023) / 1024, B);

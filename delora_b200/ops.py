@@ -60,7 +60,7 @@ def _req(t, dtype, name):
 
 
 def _keys(device, b, hw):
-    """All-ones uint64 key scratch; delora_project_fwd leaves it all-ones again."""
+    """All-ones uint64 key scratch; delora_project_fwd / delora_project_normals_fwd leave it all-ones again."""
     k = (device.index, b, hw)
     buf = _keys_cache.get(k)
     if buf is None:
@@ -82,6 +82,28 @@ def project(points, n_points, h, w, hfov, vfov, div_mode=0):
                                     int(div_mode), keys.data_ptr(), image.data_ptr(), index_map.data_ptr(),
                                     _stream()), "delora_project_fwd")
     return image, index_map
+
+
+def project_normals(points, n_points, h, w, hfov, vfov, neighborhood=(7, 11), epsilon_range=0.5, min_neighbors=10,
+                    div_mode=0):
+    """project() followed by normals(image, ..., grids=True) in one call, bit-identical to the two:
+    -> image [B,C+1,H,W], index_map [B,H,W] int32, pts_grid [B,HW,4], nrm_grid [B,HW,4]."""
+    b, c, n = points.shape
+    dev = points.device
+    image = torch.empty((b, c + 1, h, w), dtype=torch.float32, device=dev)
+    index_map = torch.empty((b, h, w), dtype=torch.int32, device=dev)
+    pg = torch.empty((b, h * w, 4), dtype=torch.float32, device=dev)
+    ng = torch.empty((b, h * w, 4), dtype=torch.float32, device=dev)
+    keys = _keys(dev, b, h * w)
+    L = _lib.lib()
+    _lib.check(L.delora_project_normals_fwd(_req(points, torch.float32, "points"),
+                                            _req(n_points, torch.int32, "n_points"), b, c, n, h, w, float(hfov[0]),
+                                            float(hfov[1]), float(vfov[0]), float(vfov[1]), int(div_mode),
+                                            keys.data_ptr(), image.data_ptr(), index_map.data_ptr(),
+                                            int(neighborhood[0]), int(neighborhood[1]), float(epsilon_range),
+                                            int(min_neighbors), pg.data_ptr(), ng.data_ptr(), None, _stream()),
+               "delora_project_normals_fwd")
+    return image, index_map, pg, ng
 
 
 def project_uv(points, n_points, h, w, hfov, vfov, div_mode=0):

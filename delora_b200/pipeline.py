@@ -40,12 +40,12 @@ class ScanPairPipeline:
         self.losses = torch.empty((self.B, ops.LOSS_ROW), dtype=f32, device=dev)
         self.grad_T = torch.empty((self.B, 12), dtype=f32, device=dev)
         self.icp_scratch = ops.icp_scratch(self.B, hw, dev)       # zeroed once; the kernels keep it armed
-        # `concurrency` sub-batches of pairs, each on its own stream (forked from / joined into the caller's stream inside
-        # step()): the latency-bound kernels of one sub-batch (projection scatter / resolve, block search, finalize) run
-        # beside the FP32-bound normals and window search of the other and fill the tails of their waves.  Measured on one
-        # H100 80GB HBM3 SXM (400 W power limit) at 8 pairs of 64 x 2048, L2 flushed (scripts/gpu_two_streams.py,
-        # medians): 466 -> 443 us per step with 2 sub-batches, 451 with 4;
-        # bit-identical results (every pair is independent).  Default: 2 from 4 pairs up.
+        # `concurrency` sub-batches of pairs for the ICP operator, each on its own stream (forked from / joined into the
+        # caller's stream inside step()); bit-identical results (every pair is independent).  Default: 2 from 4 pairs up.
+        # Projection + normals always run as ONE call for the whole batch on the caller's stream: its normals kernel
+        # resolves the projection itself and fills the GPU on its own, so per-sub-batch calls only add launches, wave
+        # tails and key re-arms (H100 80GB HBM3 at a 400 W power limit, 8 pairs of 64 x 2048, 4 rotating input sets:
+        # ~379 us per step against ~389 us with projection + normals per sub-batch).
         if concurrency is None:
             concurrency = 2 if self.B >= 4 else 1
         self.concurrency = max(1, min(int(concurrency), self.B))
@@ -58,9 +58,9 @@ class ScanPairPipeline:
                     self._subs.append({"b0": b0, "n": b1 - b0, "stream": torch.cuda.Stream(device=dev),
                                        "scratch": ops.icp_scratch(b1 - b0, hw, dev), "done": torch.cuda.Event()})
             self._fork = torch.cuda.Event()
-        # per step: (scatter + resolve) + normals + (target_extents + icp_dense + icp_dense_pending + finalize); with
-        # sub-batches the two scans of a pair are separate image ranges -> two projection / normals calls each
-        self.launches_per_step = (2 + 1 + 4) if not self._subs else len(self._subs) * (2 * 2 + 2 * 1 + 4)
+        # per step: (scatter + fused resolve / normals + key re-arm memset) + (target_extents + icp_dense +
+        # icp_dense_pending + finalize) per ICP sub-batch
+        self.launches_per_step = 3 + 4 * max(1, len(self._subs))
 
     @staticmethod
     def staging_layout(batch, channels, n_max):
@@ -96,7 +96,8 @@ class ScanPairPipeline:
     def step(self, events=None):
         """Enqueue the whole hot path on the current stream; returns (losses [B,8], grad_T [B,12]).
         `events`: optional list of 4 torch.cuda.Event (timing enabled) recorded before the first and
-        after each of the three operators, for per-kernel timing inside a measured region."""
+        after each of the three operators, for per-kernel timing inside a measured region.  Projection and normals
+        are one call whose normals kernel also resolves the projection: "projection" ends after its scatter pass."""
         if ops.NVTX:
             torch.cuda.nvtx.range_push("scan-pair step")
             try:
@@ -109,18 +110,18 @@ class ScanPairPipeline:
         if self._subs and events is None:
             return self._step_concurrent()
         L, st = self.L, torch.cuda.current_stream().cuda_stream
+        split = None
         if events is not None:
             events[0].record()
+            events[1].record()         # creates the event; the call below records it again after the scatter pass
+            split = events[1].cuda_event
         b2, B, H, W, hw = 2 * self.B, self.B, self.H, self.W, self.H * self.W
         hf, vf = self.hfov, self.vfov
-        _lib.check(L.delora_project_fwd(self.points.data_ptr(), self.n_points.data_ptr(), b2, self.C, self.N, H, W,
-                                        hf[0], hf[1], vf[0], vf[1], self.div_mode, self.keys.data_ptr(),
-                                        self.image.data_ptr(), self.index_map.data_ptr(), st), "delora_project_fwd")
-        if events is not None:
-            events[1].record()
-        _lib.check(L.delora_normals_fwd(self.image.data_ptr(), b2, self.C + 1, H, W, self.nb[0], self.nb[1],
-                                        self.eps, self.min_nb, None, self.pts_grid.data_ptr(),
-                                        self.nrm_grid.data_ptr(), st), "delora_normals_fwd")
+        _lib.check(L.delora_project_normals_fwd(self.points.data_ptr(), self.n_points.data_ptr(), b2, self.C, self.N,
+                                                H, W, hf[0], hf[1], vf[0], vf[1], self.div_mode, self.keys.data_ptr(),
+                                                self.image.data_ptr(), self.index_map.data_ptr(), self.nb[0],
+                                                self.nb[1], self.eps, self.min_nb, self.pts_grid.data_ptr(),
+                                                self.nrm_grid.data_ptr(), split, st), "delora_project_normals_fwd")
         if events is not None:
             events[2].record()
         # source = scan_2 (second half), target = scan_1 (first half): deployer.py:294-307
@@ -136,27 +137,22 @@ class ScanPairPipeline:
         return self.losses, self.grad_T
 
     def _step_concurrent(self):
-        """The same work as step(), as `concurrency` independent sub-batches of pairs on their own streams."""
+        """The same work as step(): projection + normals for the whole batch on the caller's stream, then the ICP as
+        `concurrency` independent sub-batches of pairs on their own streams."""
         L, B, H, W, C, N = self.L, self.B, self.H, self.W, self.C, self.N
         hw, hf, vf = H * W, self.hfov, self.vfov
         cur = torch.cuda.current_stream(self.device)
-        self._fork.record(cur)
         pts, npt, keys = self.points.data_ptr(), self.n_points.data_ptr(), self.keys.data_ptr()
         img, imap = self.image.data_ptr(), self.index_map.data_ptr()
         pg, ng = self.pts_grid.data_ptr(), self.nrm_grid.data_ptr()
+        _lib.check(L.delora_project_normals_fwd(pts, npt, 2 * B, C, N, H, W, hf[0], hf[1], vf[0], vf[1], self.div_mode,
+                                                keys, img, imap, self.nb[0], self.nb[1], self.eps, self.min_nb, pg, ng,
+                                                None, cur.cuda_stream), "delora_project_normals_fwd")
+        self._fork.record(cur)
         for sub in self._subs:
             s, b0, n = sub["stream"], sub["b0"], sub["n"]
             s.wait_event(self._fork)
             st = s.cuda_stream
-            for first in (b0, B + b0):                            # the sub-batch's scan_1 images, then its scan_2 images
-                _lib.check(L.delora_project_fwd(pts + first * C * N * 4, npt + first * 4, n, C, N, H, W, hf[0], hf[1],
-                                                vf[0], vf[1], self.div_mode, keys + first * hw * 8,
-                                                img + first * (C + 1) * hw * 4, imap + first * hw * 4, st),
-                           "delora_project_fwd")
-            for first in (b0, B + b0):
-                _lib.check(L.delora_normals_fwd(img + first * (C + 1) * hw * 4, n, C + 1, H, W, self.nb[0], self.nb[1],
-                                                self.eps, self.min_nb, None, pg + first * hw * 16, ng + first * hw * 16,
-                                                st), "delora_normals_fwd")
             _lib.check(L.delora_icp_dense_fwd_bwd(pg + (B + b0) * hw * 16, ng + (B + b0) * hw * 16,
                                                   self.transform.data_ptr() + b0 * 48, pg + b0 * hw * 16,
                                                   ng + b0 * hw * 16, n, H, W, hf[0], hf[1], vf[0], vf[1], self.lam,

@@ -106,6 +106,21 @@ int delora_normals_fwd(const float* image, int B, int C_img, int H, int W, int n
                        float epsilon_range, int min_neighbors, float* normals,
                        delora_f4* pts_grid, delora_f4* nrm_grid, void* stream);
 
+/* Projection followed by the normals' dense grids, in one call: the same arguments and outputs as delora_project_fwd
+ * (keys all-ones on entry and on exit) followed by delora_normals_fwd(image, B, C+1, H, W, nb_h, nb_w, epsilon_range,
+ * min_neighbors, NULL, pts_grid, nrm_grid), bit-identical to those two calls.  For C = 3 or 4 and the 7x11
+ * neighbourhood the normals kernel resolves the projection's depth keys itself (no separate resolve pass, the image
+ * is written but not read back); other C or neighbourhoods run the two calls.
+ * pts_grid, nrm_grid  [B, H*W] float4 out, as delora_normals_fwd writes them (both required)
+ * split_event         cudaEvent_t or NULL: recorded on `stream` after the projection's scatter pass (or after the whole
+ *                     projection on the two-call path) and before the normals kernel, for per-kernel timing.
+ */
+int delora_project_normals_fwd(const float* points, const int32_t* n_points, int B, int C, int n_stride,
+                               int H, int W, double hfov0, double hfov1, double vfov0, double vfov1,
+                               int div_mode, uint64_t* keys, float* image, int32_t* index_map, int nb_h, int nb_w,
+                               float epsilon_range, int min_neighbors, delora_f4* pts_grid, delora_f4* nrm_grid,
+                               void* split_event, void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * Image -> lists (row-major order of the valid pixels), the layout the reference stores and
  * trains on (src/preprocessing/normal_computation.py:30-41, :84-87;
