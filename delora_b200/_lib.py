@@ -18,7 +18,15 @@ class OdometryDesc(ctypes.Structure):
                 ("layers", c_int * 4), ("resnet_outputs", c_int), ("single_mlp", c_int)]
 
 
+class OdometryTrainParams(ctypes.Structure):
+    """delora_odometry_train_params (include/delora_b200.h): Adam, the loss and the normals' settings of a step."""
+    _fields_ = [("lr", c_float), ("beta1", c_float), ("beta2", c_float), ("eps", c_float), ("lambda_po2pl", c_float),
+                ("loss_flags", c_u32), ("nb_h", c_int), ("nb_w", c_int), ("epsilon_range", c_float),
+                ("min_neighbors", c_int)]
+
+
 c_desc_p = ctypes.POINTER(OdometryDesc)
+c_train_p = ctypes.POINTER(OdometryTrainParams)
 
 # name -> (restype, argtypes); every symbol declared in include/delora_b200.h
 SIGNATURES = {
@@ -90,6 +98,11 @@ SIGNATURES = {
     "delora_odometry_load_weights": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_pairs": (c_int, [c_desc_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_push": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_train_workspace_bytes": (c_i64, [c_desc_p]),
+    "delora_odometry_train_init": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_train_step": (c_int, [c_desc_p, c_train_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_train_weights": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),
 }
 
 ABI_VERSION = 3

@@ -190,6 +190,30 @@ __device__ __forceinline__ void quat_to_T_row(float qx, float qy, float qz, floa
     o[12] = 0.f; o[13] = 0.f; o[14] = 0.f; o[15] = 1.f;
 }
 
+// Backward of quat_to_T_row for one batch element: g = dL/dT in the row-major layout of its first 12 entries (a 4x4 or
+// a 3x4 row: the indices coincide) -> dL/dq (q as passed in, before the per-row normalisation) and dL/dt.
+__device__ __forceinline__ void quat_to_T_bwd_row(float qx, float qy, float qz, float qw, const float* __restrict__ g,
+                                                  float* __restrict__ gq, float* __restrict__ gt) {
+    const float nrm_raw = sqrtf(qx * qx + qy * qy + qz * qz + qw * qw);
+    const float nrm = fmaxf(nrm_raw, 1e-12f);
+    const float x = qx / nrm, y = qy / nrm, z = qz / nrm, w = qw / nrm;
+    const float g00 = g[0], g01 = g[1], g02 = g[2], g10 = g[4], g11 = g[5], g12 = g[6], g20 = g[8], g21 = g[9],
+                g22 = g[10];
+    // dL/d(unit quaternion): R = I + 2*[[-(yy+zz), xy-wz, xz+wy],[xy+wz, -(xx+zz), yz-wx],[xz-wy, yz+wx, -(xx+yy)]]
+    const float dx = 2.f * (y * (g01 + g10) + z * (g02 + g20) - 2.f * x * (g11 + g22) + w * (g21 - g12));
+    const float dy = 2.f * (x * (g01 + g10) + z * (g12 + g21) - 2.f * y * (g00 + g22) + w * (g02 - g20));
+    const float dz = 2.f * (x * (g02 + g20) + y * (g12 + g21) - 2.f * z * (g00 + g11) + w * (g10 - g01));
+    const float dw = 2.f * (x * (g21 - g12) + y * (g02 - g20) + z * (g10 - g01));
+    // back through q / max(|q|, eps)
+    float ox = dx / nrm, oy = dy / nrm, oz = dz / nrm, ow = dw / nrm;
+    if (nrm_raw > 1e-12f) {
+        const float dot = (dx * x + dy * y + dz * z + dw * w) / nrm;
+        ox -= dot * x; oy -= dot * y; oz -= dot * z; ow -= dot * w;
+    }
+    gq[0] = ox; gq[1] = oy; gq[2] = oz; gq[3] = ow;
+    gt[0] = g[3]; gt[1] = g[7]; gt[2] = g[11];
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -286,26 +286,8 @@ __global__ void quat_to_T_bwd_kernel(const float* __restrict__ quat, const float
                                      float* __restrict__ gq, float* __restrict__ gt) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= B) return;
-    const float qx = quat[b * 4 + 0], qy = quat[b * 4 + 1], qz = quat[b * 4 + 2], qw = quat[b * 4 + 3];
-    const float nrm_raw = sqrtf(qx * qx + qy * qy + qz * qz + qw * qw);
-    const float nrm = fmaxf(nrm_raw, 1e-12f);
-    const float x = qx / nrm, y = qy / nrm, z = qz / nrm, w = qw / nrm;
-    const float* __restrict__ g = gT + (size_t)b * 16;
-    const float g00 = g[0], g01 = g[1], g02 = g[2], g10 = g[4], g11 = g[5], g12 = g[6], g20 = g[8], g21 = g[9],
-                g22 = g[10];
-    // dL/d(unit quaternion): R = I + 2*[[-(yy+zz), xy-wz, xz+wy],[xy+wz, -(xx+zz), yz-wx],[xz-wy, yz+wx, -(xx+yy)]]
-    const float dx = 2.f * (y * (g01 + g10) + z * (g02 + g20) - 2.f * x * (g11 + g22) + w * (g21 - g12));
-    const float dy = 2.f * (x * (g01 + g10) + z * (g12 + g21) - 2.f * y * (g00 + g22) + w * (g02 - g20));
-    const float dz = 2.f * (x * (g02 + g20) + y * (g12 + g21) - 2.f * z * (g00 + g11) + w * (g10 - g01));
-    const float dw = 2.f * (x * (g21 - g12) + y * (g02 - g20) + z * (g10 - g01));
-    // back through q / max(|q|, eps)
-    float ox = dx / nrm, oy = dy / nrm, oz = dz / nrm, ow = dw / nrm;
-    if (nrm_raw > 1e-12f) {
-        const float dot = (dx * x + dy * y + dz * z + dw * w) / nrm;
-        ox -= dot * x; oy -= dot * y; oz -= dot * z; ow -= dot * w;
-    }
-    gq[b * 4 + 0] = ox; gq[b * 4 + 1] = oy; gq[b * 4 + 2] = oz; gq[b * 4 + 3] = ow;
-    gt[b * 3 + 0] = g[3]; gt[b * 3 + 1] = g[7]; gt[b * 3 + 2] = g[11];
+    quat_to_T_bwd_row(quat[b * 4 + 0], quat[b * 4 + 1], quat[b * 4 + 2], quat[b * 4 + 3], gT + (size_t)b * 16,
+                      gq + b * 4, gt + b * 3);
 }
 
 }  // namespace delora

@@ -99,8 +99,9 @@ odometry_linear_kernel(TailLinear p0, TailLinear p1, int B, int act_out, int vec
 }
 
 // Last layer of the heads (rot: 4 outputs, trans: 3), quaternion / ||quaternion block||_F, quaternion -> T.
+// raw [B, 7] or NULL: the head outputs before the normalisation (quaternion, translation), which training keeps.
 __global__ void __launch_bounds__(kTailWarps * 32)
-odometry_out_kernel(TailLinear rot, TailLinear trans, int B, int vec, float* __restrict__ T) {
+odometry_out_kernel(TailLinear rot, TailLinear trans, int B, int vec, float* __restrict__ T, float* __restrict__ raw) {
     extern __shared__ float s_out[];                        // [B, 7]: quaternion (x, y, z, w), translation
     __shared__ float s_norm;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -113,6 +114,8 @@ odometry_out_kernel(TailLinear rot, TailLinear trans, int B, int vec, float* __r
         if (lane == 0) s_out[i] = acc[0] + __ldg(p.bias + n);
     }
     __syncthreads();
+    if (raw)
+        for (int i = threadIdx.x; i < B * 7; i += blockDim.x) raw[i] = s_out[i];
     if (threadIdx.x == 0) {                                 // torch.norm of the [B, 4] block: one ordered sum
         float ss = 0.0f;
         for (int b = 0; b < B; ++b)
@@ -309,17 +312,40 @@ static int run_trunk(const Plan& p, char* ws, int act, const float* img1, const 
     return delora_avgpool_nhwc_bf16(cur, B, p.stage_h[3], p.stage_w[3], 512, pooled, st);
 }
 
-static TailLinear tail_args(const Plan& p, char* ws, const Linear& l, const float* x, int ldx, float* y, int ldy) {
+// Where the tail reads its weights and writes its activations.  Inference: the workspace copies of the weights and two
+// hidden buffers the layers alternate between; training: the fp32 master blob and one buffer per layer (the backward
+// reads every activation).
+struct TailIO {
+    const float* fc_w;
+    const float* fc_b;
+    const float* w[kMaxLinear];
+    const float* b[kMaxLinear];
+    float* fc_out;                     // [B, nout]: act(resnet.fc(pooled))
+    float* hid[kMaxLinear];            // output of lin[i], i < n_lin - 1; two heads: hid[0] = [rot1 | trans1], ld 200
+    float* raw;                        // [B, 7] head outputs before the normalisation, or NULL
+};
+
+static TailLinear tail_args(const Linear& l, const float* w, const float* bias, const float* x, int ldx, float* y, int ldy) {
     TailLinear t;
-    t.w = reinterpret_cast<const float*>(ws + l.ws_w);
-    t.bias = reinterpret_cast<const float*>(ws + l.ws_b);
+    t.w = w;
+    t.bias = bias;
     t.x = x; t.y = y; t.K = l.K; t.N = l.N; t.ldx = ldx; t.ldy = ldy;
     return t;
 }
 
-static int run_tail(const Plan& p, char* ws, int act, const float* pooled, int B, float* T, cudaStream_t st) {
-    float* fc_out = reinterpret_cast<float*>(ws + p.fc_out);
-    float* hid[2] = {reinterpret_cast<float*>(ws + p.hid[0]), reinterpret_cast<float*>(ws + p.hid[1])};
+static TailIO inference_tail_io(const Plan& p, char* ws) {
+    TailIO io;
+    memset(&io, 0, sizeof(io));
+    auto f = [&](size_t off) { return reinterpret_cast<float*>(ws + off); };
+    io.fc_w = f(p.fc.ws_w); io.fc_b = f(p.fc.ws_b);
+    for (int i = 0; i < p.n_lin; ++i) { io.w[i] = f(p.lin[i].ws_w); io.b[i] = f(p.lin[i].ws_b); }
+    io.fc_out = f(p.fc_out);
+    for (int i = 0; i < kMaxLinear; ++i) io.hid[i] = f(p.hid[i & 1]);
+    return io;
+}
+
+static int run_tail(const Plan& p, const TailIO& io, int act, const float* pooled, int B, float* T, cudaStream_t st) {
+    float* fc_out = io.fc_out;
     TailLinear none;
     memset(&none, 0, sizeof(none));
     auto linear = [&](const TailLinear& a, const TailLinear& b) {
@@ -331,26 +357,28 @@ static int run_tail(const Plan& p, char* ws, int act, const float* pooled, int B
     };
     int rc;
     const int nout = p.fc.N;
-    if ((rc = linear(tail_args(p, ws, p.fc, pooled, 512, fc_out, nout), none))) return rc;     // act(resnet.fc(x))
+    if ((rc = linear(tail_args(p.fc, io.fc_w, io.fc_b, pooled, 512, fc_out, nout), none))) return rc;   // act(resnet.fc(x))
     TailLinear rot, trans;
     if (p.n_lin == 4) {
         // hidden layers of both heads in one launch: hid[0] = [act(rot1 h) | act(trans1 h)], row stride 200
         const int ld = 2 * kHeadHidden;
-        if ((rc = linear(tail_args(p, ws, p.lin[0], fc_out, nout, hid[0], ld),
-                         tail_args(p, ws, p.lin[2], fc_out, nout, hid[0] + kHeadHidden, ld)))) return rc;
-        rot = tail_args(p, ws, p.lin[1], hid[0], ld, nullptr, 0);
-        trans = tail_args(p, ws, p.lin[3], hid[0] + kHeadHidden, ld, nullptr, 0);
+        float* hid = io.hid[0];
+        if ((rc = linear(tail_args(p.lin[0], io.w[0], io.b[0], fc_out, nout, hid, ld),
+                         tail_args(p.lin[2], io.w[2], io.b[2], fc_out, nout, hid + kHeadHidden, ld)))) return rc;
+        rot = tail_args(p.lin[1], io.w[1], io.b[1], hid, ld, nullptr, 0);
+        trans = tail_args(p.lin[3], io.w[3], io.b[3], hid + kHeadHidden, ld, nullptr, 0);
     } else {
         const float* x = fc_out;
         int ldx = nout;
         for (int i = 0; i < p.n_lin - 1; ++i) {
-            float* y = hid[i & 1];
-            if ((rc = linear(tail_args(p, ws, p.lin[i], x, ldx, y, p.lin[i].N), none))) return rc;
+            float* y = io.hid[i];
+            if ((rc = linear(tail_args(p.lin[i], io.w[i], io.b[i], x, ldx, y, p.lin[i].N), none))) return rc;
             x = y; ldx = p.lin[i].N;
         }
         // fully_connected_rot_trans's last layer: rows 0..3 -> rotation, rows 4..6 -> translation
-        const Linear& l = p.lin[p.n_lin - 1];
-        rot = tail_args(p, ws, l, x, ldx, nullptr, 0);
+        const int last = p.n_lin - 1;
+        const Linear& l = p.lin[last];
+        rot = tail_args(l, io.w[last], io.b[last], x, ldx, nullptr, 0);
         rot.N = 4;
         trans = rot;
         trans.w = rot.w + 4 * (size_t)l.K;
@@ -358,7 +386,7 @@ static int run_tail(const Plan& p, char* ws, int act, const float* pooled, int B
         trans.N = 3;
     }
     const int vec = (rot.K % 4 == 0 && rot.ldx % 4 == 0) ? 1 : 0;
-    odometry_out_kernel<<<1, kTailWarps * 32, (size_t)B * 7 * sizeof(float), st>>>(rot, trans, B, vec, T);
+    odometry_out_kernel<<<1, kTailWarps * 32, (size_t)B * 7 * sizeof(float), st>>>(rot, trans, B, vec, T, io.raw);
     DELORA_CHECK_LAUNCH("odometry_out_kernel");
     return 0;
 }
@@ -458,7 +486,7 @@ extern "C" int delora_odometry_pairs(const delora_odometry_desc* d, const float*
     int rc;
     if ((rc = project(p, d, ws, points, n_points, 2 * B, images, st))) return rc;
     if ((rc = run_trunk(p, ws, d->act, images, images + (size_t)B * img, B, pooled_ws, st))) return rc;
-    if ((rc = run_tail(p, ws, d->act, pooled_ws, B, T, st))) return rc;
+    if ((rc = run_tail(p, inference_tail_io(p, ws), d->act, pooled_ws, B, T, st))) return rc;
     if (pooled) {
         const cudaError_t e = cudaMemcpyAsync(pooled, pooled_ws, (size_t)B * 512 * sizeof(float), cudaMemcpyDeviceToDevice, st);
         DELORA_CHECK_ARG(e == cudaSuccess, "delora_odometry_pairs: %s", cudaGetErrorString(e));
@@ -481,9 +509,664 @@ extern "C" int delora_odometry_push(const delora_odometry_desc* d, const float* 
     if (T) {
         float* pooled_ws = reinterpret_cast<float*>(ws + p.pooled);
         if ((rc = run_trunk(p, ws, d->act, prev, image, 1, pooled_ws, st))) return rc;
-        if ((rc = run_tail(p, ws, d->act, pooled_ws, 1, T, st))) return rc;
+        if ((rc = run_tail(p, inference_tail_io(p, ws), d->act, pooled_ws, 1, T, st))) return rc;
     }
     const cudaError_t e = cudaMemcpyAsync(prev, image, (size_t)4 * d->H * d->W * sizeof(float), cudaMemcpyDeviceToDevice, st);
     DELORA_CHECK_ARG(e == cudaSuccess, "delora_odometry_push: %s", cudaGetErrorString(e));
+    return 0;
+}
+
+// ================================================================================================ training
+// delora_odometry_train_step: projection + normals of the 2B scans, the trunk forward keeping its activations (the
+// kernel sequence of TensorCoreEncoder._forward_saving), the tail forward keeping its activations, the dense ICP
+// losses with dL/dT, the tail backward (below), the trunk backward (TensorCoreEncoder._backward), one Adam update of
+// the fp32 master blob and one re-prep of the bf16 filters from it.  Weight gradients land in a gradient blob with
+// the layout of the weight blob: the wgrad kernels write each filter at its blob offset ([Cout, Cin, k, k] is both
+// the state_dict layout and theirs), the tail kernels each fc / head tensor at its own.
+//
+// New kernels (fp32, fixed summation order, no atomics: bit-identical from run to run):
+//   odometry_out_bwd_kernel (one CTA): grad_T / B -> quaternion -> T backward (quat_to_T_bwd_row, shared with
+//     quat_to_T_bwd_kernel) -> backward of the division by the norm of the whole [B, 4] block (all rows coupled) ->
+//     d(head outputs) [B, 7]; the last Linear of each head (dW, db) and d(hidden) * act'.
+//   odometry_linear_bwd_kernel: y = act(W x + b) backward for up to two layers that read the same x (the heads'
+//     hidden layers: their contributions to dx are summed in a fixed order), dW / db and dx * act'(x) in one launch.
+//   odometry_adam_kernel: torch's Adam (fused formula, no weight decay) over the whole blob, float4 per thread; the
+//     step count is read from the workspace, so the bias corrections need no host value.
+//   odometry_icp_rearm_kernel: zeroes the ICP scratch when B differs from the batch size of the previous step (the
+//     scratch layout depends on B); otherwise every CTA exits at once.
+namespace delora {
+
+constexpr int kBwdThreads = 256;
+constexpr int kDgradCols = 32;         // dx tile: 32 columns (one per lane) x 4 batch rows; the 8 warps split the outputs
+constexpr int kDgradRows = 4;
+constexpr int kMaxBlocks = 4 * kMaxBlocksPerStage;
+
+// torch's activation backward from the stored output y: tanh' = 1 - y^2, relu' = [y > 0] (threshold_backward)
+__device__ __forceinline__ float tail_act_bwd(float g, float y, int act) {
+    if (act == 2) return g * (1.0f - y * y);
+    if (act == 1) return y <= 0.0f ? 0.0f : g;
+    return g;
+}
+
+struct TailGrad {
+    const float* w;        // [N, K] row-major
+    const float* x;        // [B, ldx]: the layer's input
+    const float* dz;       // [B, ldz]: gradient w.r.t. the layer's output before its activation
+    float* gw;             // [N, K]
+    float* gb;             // [N]
+    int K, N, ldx, ldz;
+};
+
+// blocks [0, p0.N + p1.N): one weight row n each, dW[n, k] = sum_b dz[b, n] x[b, k] and db[n] = sum_b dz[b, n], b in
+// order.  The other blocks: dx tiles, dx[b, k] = sum over the concatenated outputs of p0 then p1 of W[n, k] dz[b, n]
+// (warp w adds the w-th chunk of n in order, the chunks are added in warp order), times act_in'(x[b, k]) (0: none).
+__global__ void __launch_bounds__(kBwdThreads)
+odometry_linear_bwd_kernel(TailGrad p0, TailGrad p1, int B, int act_in, float* __restrict__ dx, int lddx) {
+    const int nrows = p0.N + p1.N;
+    if ((int)blockIdx.x < nrows) {
+        int n = blockIdx.x;
+        const bool second = n >= p0.N;
+        const TailGrad p = second ? p1 : p0;
+        if (second) n -= p0.N;
+        for (int k = threadIdx.x; k < p.K; k += blockDim.x) {
+            float acc = 0.0f;
+            for (int b = 0; b < B; ++b) acc = fmaf(__ldg(p.dz + (size_t)b * p.ldz + n), __ldg(p.x + (size_t)b * p.ldx + k), acc);
+            p.gw[(size_t)n * p.K + k] = acc;
+        }
+        if (threadIdx.x == 0) {
+            float s = 0.0f;
+            for (int b = 0; b < B; ++b) s += __ldg(p.dz + (size_t)b * p.ldz + n);
+            p.gb[n] = s;
+        }
+        return;
+    }
+    __shared__ float s_part[kTailWarps][kDgradRows][kDgradCols];
+    const int tile = blockIdx.x - nrows;
+    const int tiles_k = (p0.K + kDgradCols - 1) / kDgradCols;
+    const int k0 = (tile % tiles_k) * kDgradCols, b0 = (tile / tiles_k) * kDgradRows;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int k = k0 + lane;
+    const int chunk = (nrows + kTailWarps - 1) / kTailWarps;
+    const int n_lo = warp * chunk, n_hi = min(nrows, n_lo + chunk);
+    float acc[kDgradRows] = {0.0f, 0.0f, 0.0f, 0.0f};
+    if (k < p0.K) {
+        for (int n = n_lo; n < n_hi; ++n) {
+            const bool second = n >= p0.N;
+            const int nn = second ? n - p0.N : n;
+            const float* __restrict__ w = second ? p1.w : p0.w;
+            const float* __restrict__ dz = second ? p1.dz : p0.dz;
+            const int ldz = second ? p1.ldz : p0.ldz;
+            const float wv = __ldg(w + (size_t)nn * p0.K + k);
+#pragma unroll
+            for (int j = 0; j < kDgradRows; ++j)
+                if (b0 + j < B) acc[j] = fmaf(__ldg(dz + (size_t)(b0 + j) * ldz + nn), wv, acc[j]);
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < kDgradRows; ++j) s_part[warp][j][lane] = acc[j];
+    __syncthreads();
+    if (threadIdx.x < kDgradRows * kDgradCols) {
+        const int j = threadIdx.x / kDgradCols, c = threadIdx.x % kDgradCols;
+        const int b = b0 + j, kk = k0 + c;
+        if (b < B && kk < p0.K) {
+            float s = 0.0f;
+#pragma unroll
+            for (int w = 0; w < kTailWarps; ++w) s += s_part[w][j][c];
+            dx[(size_t)b * lddx + kk] = tail_act_bwd(s, act_in ? p0.x[(size_t)b * p0.ldx + kk] : 0.0f, act_in);
+        }
+    }
+}
+
+struct OutBwd {
+    const float* raw;                  // [B, 7] head outputs (odometry_out_kernel's raw)
+    const float* grad_T;               // [B, 12] the ICP kernel's dL/dT of each pair
+    const float* w_rot;                // [4, K] last layer of the rotation head (single MLP: rows 0..3)
+    const float* w_trans;              // [3, K]
+    const float* x_rot;                // [B, ldx] the hidden input of w_rot
+    const float* x_trans;              // [B, ldx]
+    float *gw_rot, *gb_rot, *gw_trans, *gb_trans;
+    float* dz;                         // [B, ldz] out: gradient w.r.t. the hidden layer's pre-activation
+    long long* ctr;                    // [0] Adam's step count, [1] the batch size of the ICP scratch
+    int K, ldx, ldz, single;
+};
+
+__global__ void __launch_bounds__(kBwdThreads)
+odometry_out_bwd_kernel(OutBwd a, int B, float inv_B, int act) {
+    extern __shared__ float s_d[];                          // [B, 7]: d(quaternion), d(translation)
+    __shared__ float s_red[2];
+    const float* __restrict__ raw = a.raw;
+    if (threadIdx.x == 0) {                                 // the forward's ordered sum
+        float ss = 0.0f;
+        for (int b = 0; b < B; ++b)
+            for (int j = 0; j < 4; ++j) ss = fmaf(raw[b * 7 + j], raw[b * 7 + j], ss);
+        s_red[0] = sqrtf(ss);
+    }
+    __syncthreads();
+    const float nrm = s_red[0];
+    for (int b = threadIdx.x; b < B; b += blockDim.x) {
+        const float* q = raw + b * 7;
+        float g[12];
+#pragma unroll
+        for (int i = 0; i < 12; ++i) g[i] = a.grad_T[(size_t)b * 12 + i] * inv_B;    // d(mean over pairs)
+        quat_to_T_bwd_row(q[0] / nrm, q[1] / nrm, q[2] / nrm, q[3] / nrm, g, s_d + b * 7, s_d + b * 7 + 4);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {                                 // q / n: d n = -sum(g * q) / n^2 over the whole block
+        float s = 0.0f;
+        for (int b = 0; b < B; ++b)
+            for (int j = 0; j < 4; ++j) s = fmaf(s_d[b * 7 + j], raw[b * 7 + j], s);
+        s_red[1] = -s / (nrm * nrm);
+        a.ctr[0] += 1;
+        a.ctr[1] = B;
+    }
+    __syncthreads();
+    const float gn = s_red[1];
+    for (int i = threadIdx.x; i < B * 4; i += blockDim.x) {  // div backward + norm backward (q * dn / n)
+        const int b = i >> 2, j = i & 3;
+        s_d[b * 7 + j] = s_d[b * 7 + j] / nrm + raw[b * 7 + j] * (gn / nrm);
+    }
+    __syncthreads();
+    const int K = a.K;
+    for (int i = threadIdx.x; i < 7 * (K + 1); i += blockDim.x) {
+        const int o = i / (K + 1), k = i - o * (K + 1);
+        const float* __restrict__ x = o < 4 ? a.x_rot : a.x_trans;
+        float acc = 0.0f;
+        if (k < K) {
+            for (int b = 0; b < B; ++b) acc = fmaf(s_d[b * 7 + o], x[(size_t)b * a.ldx + k], acc);
+            (o < 4 ? a.gw_rot + (size_t)o * K : a.gw_trans + (size_t)(o - 4) * K)[k] = acc;
+        } else {
+            for (int b = 0; b < B; ++b) acc += s_d[b * 7 + o];
+            (o < 4 ? a.gb_rot + o : a.gb_trans + (o - 4))[0] = acc;
+        }
+    }
+    // hidden gradient: single MLP -> all 7 outputs read the same K inputs; two heads -> [rot hidden | trans hidden]
+    const int ncol = a.single ? K : 2 * K;
+    for (int i = threadIdx.x; i < B * ncol; i += blockDim.x) {
+        const int b = i / ncol, c = i - b * ncol;
+        const float* d = s_d + b * 7;
+        float s = 0.0f, y;
+        if (a.single) {
+            for (int o = 0; o < 4; ++o) s = fmaf(a.w_rot[(size_t)o * K + c], d[o], s);
+            for (int o = 0; o < 3; ++o) s = fmaf(a.w_trans[(size_t)o * K + c], d[4 + o], s);
+            y = a.x_rot[(size_t)b * a.ldx + c];
+        } else if (c < K) {
+            for (int o = 0; o < 4; ++o) s = fmaf(a.w_rot[(size_t)o * K + c], d[o], s);
+            y = a.x_rot[(size_t)b * a.ldx + c];
+        } else {
+            const int cc = c - K;
+            for (int o = 0; o < 3; ++o) s = fmaf(a.w_trans[(size_t)o * K + cc], d[4 + o], s);
+            y = a.x_trans[(size_t)b * a.ldx + cc];
+        }
+        a.dz[(size_t)b * a.ldz + c] = tail_act_bwd(s, y, act);
+    }
+}
+
+// torch.optim.Adam (the fused implementation's formula; no weight decay, no amsgrad) on n floats
+__global__ void __launch_bounds__(256)
+odometry_adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
+                     long long n, const long long* __restrict__ ctr, float lr, float beta1, float beta2, float eps) {
+    const float t = (float)ctr[0];
+    const float bc1 = 1.0f - powf(beta1, t);
+    const float step_size = lr / bc1;
+    const float bc2_sqrt = sqrtf(1.0f - powf(beta2, t));
+    auto upd = [&](float& pp, float gg, float& mm, float& vv) {
+        mm = beta1 * mm + (1.0f - beta1) * gg;
+        vv = beta2 * vv + (1.0f - beta2) * gg * gg;
+        const float denom = sqrtf(vv) / bc2_sqrt + eps;
+        pp -= step_size * mm / denom;
+    };
+    const long long n4 = n >> 2;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += stride) {
+        float4 pp = reinterpret_cast<float4*>(p)[i];
+        const float4 gg = __ldg(reinterpret_cast<const float4*>(g) + i);
+        float4 mm = reinterpret_cast<float4*>(m)[i];
+        float4 vv = reinterpret_cast<float4*>(v)[i];
+        upd(pp.x, gg.x, mm.x, vv.x); upd(pp.y, gg.y, mm.y, vv.y);
+        upd(pp.z, gg.z, mm.z, vv.z); upd(pp.w, gg.w, mm.w, vv.w);
+        reinterpret_cast<float4*>(p)[i] = pp;
+        reinterpret_cast<float4*>(m)[i] = mm;
+        reinterpret_cast<float4*>(v)[i] = vv;
+    }
+    if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
+        const long long i = n4 * 4 + threadIdx.x;
+        upd(p[i], g[i], m[i], v[i]);
+    }
+}
+
+__global__ void odometry_icp_rearm_kernel(float4* __restrict__ s, long long n4, int B, const long long* __restrict__ ctr) {
+    if (ctr[1] == B) return;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += stride)
+        s[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+}
+
+// ---------------------------------------------------------------- training plan: workspace layout
+struct TrainPlan {
+    Plan p;
+    size_t master, grad, m, v, ctr, table;
+    size_t w_fwd[kMaxConv], w_flip[kMaxConv];
+    size_t keys, index_map, counts, images, pts_grid, nrm_grid;
+    size_t icp, losses, grad_T, T16, T12;
+    // trunk activations kept by the forward: 16- or 64-channel input, stem pre-activation, pool output + argmax,
+    // per block conv1 output and block output, per stage the downsample output
+    size_t x_in, y0, p0, idx, t1[kMaxBlocks], out[kMaxBlocks], ds[4];
+    // trunk backward: per stage two alternating data-gradient buffers + the conv1 gradient; strided blocks: the
+    // downsample's gradient at the output size and (zero-upsample path) the upsampled conv1 gradient
+    size_t g[4][3], gds[4], gu1[4], g_stem;
+    int phase_dgrad[kMaxBlocks];
+    // tail activations and gradients
+    size_t pooled, fc_out, hid[kMaxLinear], raw, dz_hid[kMaxLinear], dz_fc, g_pooled;
+    size_t wg_scratch;
+    int64_t icp_floats, wg_floats;
+    size_t total;
+};
+
+// ops.conv2d_dgrad_eligible: the phase-decomposed data gradient of delora_conv2d_dgrad_bf16 takes the layer
+static bool dgrad_eligible(int cin, int cout, int win, int sw) {
+    const int wg = (win + sw - 1) / sw;
+    return cout % 64 == 0 && (cin % 128 == 0 || (cin == 64 && wg >= 128)) && (sw == 1 || win % 2 == 0);
+}
+
+static void make_train_plan(const delora_odometry_desc* d, TrainPlan* tp) {
+    memset(tp, 0, sizeof(TrainPlan));
+    make_plan(d, &tp->p);
+    const Plan& p = tp->p;
+    const int MB = d->max_batch, H = d->H, W = d->W, HW = H * W, nout = d->resnet_outputs;
+    size_t off = 0;
+    auto take = [&](size_t bytes) { const size_t o = off; off += align256(bytes); return o; };
+    const size_t blob = (size_t)p.blob_floats * 4;
+    tp->master = take(blob); tp->grad = take(blob); tp->m = take(blob); tp->v = take(blob);
+    tp->ctr = take(2 * sizeof(long long));
+    tp->table = take((size_t)p.n_conv * 8 * 8);
+    for (int i = 0; i < p.n_conv; ++i) {
+        const ConvLayer& c = p.conv[i];
+        if (i == 0) {
+            tp->w_fwd[0] = take(p.stem_fast ? (size_t)3 * 64 * 64 * 2 : (size_t)64 * 9 * 64 * 2);
+        } else {
+            tp->w_fwd[i] = take((size_t)c.cout * c.k * c.k * c.cin * 2);
+            tp->w_flip[i] = take((size_t)c.cin * c.k * c.k * c.cout * 2);
+        }
+    }
+    tp->keys = take((size_t)2 * MB * HW * 8);
+    tp->index_map = take((size_t)2 * MB * HW * 4);
+    tp->counts = take((size_t)2 * MB * 4);
+    tp->images = take((size_t)2 * MB * 4 * HW * 4);
+    tp->pts_grid = take((size_t)2 * MB * HW * 16);
+    tp->nrm_grid = take((size_t)2 * MB * HW * 16);
+    tp->icp_floats = delora_icp_scratch_floats(MB, HW);
+    tp->icp = take((size_t)tp->icp_floats * 4);
+    tp->losses = take((size_t)MB * DELORA_LOSS_ROW * 4);
+    tp->grad_T = take((size_t)MB * 12 * 4);
+    tp->T16 = take((size_t)MB * 16 * 4);
+    tp->T12 = take((size_t)MB * 12 * 4);
+    tp->x_in = take(nhwc_bytes(MB, H, W, p.stem_fast ? 16 : 64));
+    tp->y0 = take(nhwc_bytes(MB, H, p.w2, 64));
+    tp->p0 = take(nhwc_bytes(MB, H, p.w4, 64));
+    tp->idx = take((size_t)MB * H * p.w4 * 64);
+    for (int i = 0; i < p.n_block; ++i) {
+        const Block& b = p.block[i];
+        tp->t1[i] = take(nhwc_bytes(MB, b.hout, b.wout, b.cout));
+        tp->out[i] = take(nhwc_bytes(MB, b.hout, b.wout, b.cout));
+        if (b.ds >= 0) tp->ds[b.stage] = take(nhwc_bytes(MB, b.hout, b.wout, b.cout));
+    }
+    for (int s = 0; s < 4; ++s)
+        for (int j = 0; j < 3; ++j) tp->g[s][j] = take(nhwc_bytes(MB, p.stage_h[s], p.stage_w[s], p.stage_c[s]));
+    for (int i = 0; i < p.n_block; ++i) {
+        const Block& b = p.block[i];
+        tp->phase_dgrad[i] = b.ds >= 0 && i > 0 && dgrad_eligible(b.cin, b.cout, b.win, b.sw);
+        if (b.ds < 0) continue;
+        tp->gds[b.stage] = take(nhwc_bytes(MB, b.hout, b.wout, b.cin));
+        if (!tp->phase_dgrad[i]) tp->gu1[b.stage] = take(nhwc_bytes(MB, b.hin, b.win, b.cout));
+    }
+    tp->g_stem = take(nhwc_bytes(MB, H, p.w2, 64));
+    tp->pooled = take((size_t)MB * 512 * 4);
+    tp->g_pooled = take((size_t)MB * 512 * 4);
+    tp->fc_out = take((size_t)MB * nout * 4);
+    tp->dz_fc = take((size_t)MB * nout * 4);
+    tp->raw = take((size_t)MB * 7 * 4);
+    if (p.n_lin == 4) {
+        tp->hid[0] = take((size_t)MB * 2 * kHeadHidden * 4);
+        tp->dz_hid[0] = take((size_t)MB * 2 * kHeadHidden * 4);
+    } else {
+        for (int i = 0; i < p.n_lin - 1; ++i) {
+            tp->hid[i] = take((size_t)MB * p.lin[i].N * 4);
+            tp->dz_hid[i] = take((size_t)MB * p.lin[i].N * 4);
+        }
+    }
+    // one split-K scratch for every wgrad launch: the largest need at max_batch (the need grows with B)
+    int64_t wg = p.stem_fast ? delora_stem_wgrad_scratch_floats(MB, H, W)
+                             : delora_conv2d_wgrad_scratch_floats(MB, H, p.w2, 64, 64, 3);
+    for (int i = 0; i < p.n_block; ++i) {
+        const Block& b = p.block[i];
+        int64_t n = delora_conv2d_wgrad_scratch_floats(MB, b.hout, b.wout, b.cin, b.cout, 3);
+        wg = n > wg ? n : wg;
+        n = delora_conv2d_wgrad_scratch_floats(MB, b.hout, b.wout, b.cout, b.cout, 3);
+        wg = n > wg ? n : wg;
+        if (b.ds >= 0) {
+            n = delora_conv2d_wgrad_scratch_floats(MB, b.hout, b.wout, b.cin, b.cout, 1);
+            wg = n > wg ? n : wg;
+        }
+    }
+    tp->wg_floats = wg;
+    tp->wg_scratch = take((size_t)wg * 4);
+    tp->total = off;
+}
+
+static int check_train_params(const delora_odometry_train_params* hp, const char* who) {
+    DELORA_CHECK_ARG(hp != nullptr, "%s: null hyperparameters", who);
+    DELORA_CHECK_ARG(isfinite(hp->lr) && hp->lr >= 0.0f, "%s: lr=%g must be finite and >= 0", who, (double)hp->lr);
+    DELORA_CHECK_ARG(hp->beta1 >= 0.0f && hp->beta1 < 1.0f, "%s: beta1=%g must be in [0, 1)", who, (double)hp->beta1);
+    DELORA_CHECK_ARG(hp->beta2 >= 0.0f && hp->beta2 < 1.0f, "%s: beta2=%g must be in [0, 1)", who, (double)hp->beta2);
+    DELORA_CHECK_ARG(isfinite(hp->eps) && hp->eps > 0.0f, "%s: eps=%g must be > 0", who, (double)hp->eps);
+    DELORA_CHECK_ARG(isfinite(hp->lambda_po2pl), "%s: lambda_po2pl=%g must be finite", who, (double)hp->lambda_po2pl);
+    DELORA_CHECK_ARG((hp->loss_flags & (DELORA_LOSS_PO2PO | DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL)) != 0,
+                     "%s: loss_flags=0x%x sets no loss bit", who, hp->loss_flags);
+    DELORA_CHECK_ARG(hp->nb_h >= 1 && hp->nb_h % 2 == 1, "%s: nb_h=%d must be odd and positive", who, hp->nb_h);
+    DELORA_CHECK_ARG(hp->nb_w >= 1 && hp->nb_w % 2 == 1, "%s: nb_w=%d must be odd and positive", who, hp->nb_w);
+    DELORA_CHECK_ARG(isfinite(hp->epsilon_range) && hp->epsilon_range >= 0.0f, "%s: epsilon_range=%g must be >= 0", who,
+                     (double)hp->epsilon_range);
+    DELORA_CHECK_ARG(hp->min_neighbors >= 0, "%s: min_neighbors=%d must be >= 0", who, hp->min_neighbors);
+    return 0;
+}
+
+static int train_trunk_forward(const TrainPlan& tp, char* ws, int act, const float* img1, const float* img2, int B,
+                               cudaStream_t st) {
+    const Plan& p = tp.p;
+    int rc;
+    const int H = p.H, W = p.W;
+    // the stem keeps its PRE-activation (fp16 on the 16-channel path); the max-pool applies the activation
+    if (p.stem_fast) {
+        if ((rc = delora_images_to_nhwc16_bf16(img1, img2, B, H, W, ws + tp.x_in, st))) return rc;
+        if ((rc = delora_stem_fprop_bf16(ws + tp.x_in, ws + tp.w_fwd[0], ws + tp.y0, B, H, W, 0, 1, st))) return rc;
+    } else {
+        if ((rc = delora_images_to_nhwc_bf16(img1, img2, B, H, W, 64, ws + tp.x_in, st))) return rc;
+        if ((rc = delora_conv2d_fprop_bf16(ws + tp.x_in, ws + tp.w_fwd[0], nullptr, nullptr, ws + tp.y0, B, H, W, 64, 64, 3,
+                                           1, 2, 0, st))) return rc;
+    }
+    if ((rc = delora_maxpool_w_idx_nhwc_bf16(ws + tp.y0, B, H, p.w2, 64, ws + tp.p0, ws + tp.idx, act, p.stem_fast, st)))
+        return rc;
+    const char* cur = ws + tp.p0;
+    for (int i = 0; i < p.n_block; ++i) {
+        const Block& b = p.block[i];
+        char* t1 = ws + tp.t1[i];
+        const char* ident = cur;
+        if ((rc = delora_conv2d_fprop_bf16(cur, ws + tp.w_fwd[b.c1], nullptr, nullptr, t1, B, b.hin, b.win, b.cin, b.cout,
+                                           3, b.sh, b.sw, act, st))) return rc;
+        if (b.ds >= 0) {
+            ident = ws + tp.ds[b.stage];
+            if ((rc = delora_conv2d_fprop_bf16(cur, ws + tp.w_fwd[b.ds], nullptr, nullptr, ws + tp.ds[b.stage], B, b.hin,
+                                               b.win, b.cin, b.cout, 1, b.sh, b.sw, 0, st))) return rc;
+        }
+        if ((rc = delora_conv2d_fprop_bf16(t1, ws + tp.w_fwd[b.c2], ident, nullptr, ws + tp.out[i], B, b.hout, b.wout,
+                                           b.cout, b.cout, 3, 1, 1, act, st))) return rc;
+        cur = ws + tp.out[i];
+    }
+    return delora_avgpool_nhwc_bf16(cur, B, p.stage_h[3], p.stage_w[3], 512, reinterpret_cast<float*>(ws + tp.pooled), st);
+}
+
+static int train_trunk_backward(const TrainPlan& tp, char* ws, int act, int B, cudaStream_t st) {
+    const Plan& p = tp.p;
+    int rc;
+    const int act_bwd = act == 1 ? 4 : 3;                 // ACT_RELU_BWD / ACT_TANH_BWD: multiply by act'(saved)
+    float* grad = reinterpret_cast<float*>(ws + tp.grad);
+    float* scratch = reinterpret_cast<float*>(ws + tp.wg_scratch);
+    const int L = p.n_block - 1;
+    char* dz2 = ws + tp.g[3][0];
+    if ((rc = delora_avgpool_bwd_nhwc_bf16(reinterpret_cast<const float*>(ws + tp.g_pooled), ws + tp.out[L], B,
+                                           p.stage_h[3], p.stage_w[3], 512, act, dz2, st))) return rc;
+    for (int i = L; i >= 0; --i) {
+        const Block& b = p.block[i];
+        const int s = b.stage;
+        const char* x = i == 0 ? ws + tp.p0 : ws + tp.out[i - 1];
+        char* dz1 = ws + tp.g[s][2];
+        // the data gradient of the block input: the other buffer of this stage, or a buffer of the previous stage
+        char* next;
+        if (i > 0 && p.block[i - 1].stage != s) next = ws + tp.g[p.block[i - 1].stage][0];
+        else next = (dz2 == ws + tp.g[s][0]) ? ws + tp.g[s][1] : ws + tp.g[s][0];
+        if ((rc = delora_conv2d_wgrad_bf16(ws + tp.t1[i], dz2, grad + p.conv[b.c2].blob, scratch, B, b.hout, b.wout, b.cout,
+                                           b.cout, b.cout, 3, 1, 1, st))) return rc;
+        if ((rc = delora_conv2d_fprop_bf16(dz2, ws + tp.w_flip[b.c2], nullptr, ws + tp.t1[i], dz1, B, b.hout, b.wout, b.cout,
+                                           b.cout, 3, 1, 1, act_bwd, st))) return rc;
+        if ((rc = delora_conv2d_wgrad_bf16(x, dz1, grad + p.conv[b.c1].blob, scratch, B, b.hin, b.win, b.cin, b.cin, b.cout,
+                                           3, b.sh, b.sw, st))) return rc;
+        const char* resid = dz2;
+        const char* src = dz1;
+        if (b.ds >= 0) {
+            if ((rc = delora_conv2d_wgrad_bf16(x, dz2, grad + p.conv[b.ds].blob, scratch, B, b.hin, b.win, b.cin, b.cin,
+                                               b.cout, 1, b.sh, b.sw, st))) return rc;
+            // the 1x1 strided downsample's data gradient: 1x1 convolution of the small dz, scattered afterwards
+            char* small = ws + tp.gds[s];
+            if ((rc = delora_conv2d_fprop_bf16(dz2, ws + tp.w_flip[b.ds], nullptr, nullptr, small, B, b.hout, b.wout, b.cout,
+                                               b.cin, 1, 1, 1, 0, st))) return rc;
+            if (tp.phase_dgrad[i]) {
+                if ((rc = delora_conv2d_dgrad_bf16(dz1, ws + tp.w_flip[b.c1], small, x, next, B, b.hin, b.win, b.cin, b.cout,
+                                                   b.sh, b.sw, act_bwd, 1, st))) return rc;
+                dz2 = next;
+                continue;
+            }
+            char* up_resid = ws + tp.g[p.block[i - 1].stage][1];
+            char* up_src = ws + tp.gu1[s];
+            if ((rc = delora_zero_upsample_nhwc_bf16(small, B, b.hout, b.wout, b.cin, b.sh, b.sw, b.hin, b.win, up_resid, st)))
+                return rc;
+            if ((rc = delora_zero_upsample_nhwc_bf16(dz1, B, b.hout, b.wout, b.cout, b.sh, b.sw, b.hin, b.win, up_src, st)))
+                return rc;
+            resid = up_resid;
+            src = up_src;
+        }
+        // i > 0: the block input is the previous block's activation output, act' folds into the epilogue; the first
+        // block reads the max-pool output (ACT_NONE: the pool's backward applies the stem's act')
+        if ((rc = delora_conv2d_fprop_bf16(src, ws + tp.w_flip[b.c1], resid, i > 0 ? x : nullptr, next, B, b.hin, b.win,
+                                           b.cout, b.cin, 3, 1, 1, i > 0 ? act_bwd : 0, st))) return rc;
+        dz2 = next;
+    }
+    if ((rc = delora_maxpool_w_bwd_nhwc_bf16(dz2, ws + tp.idx, ws + tp.y0, B, p.H, p.w2, 64, 4 + act, ws + tp.g_stem,
+                                             p.stem_fast, st))) return rc;
+    if (p.stem_fast)
+        return delora_stem_wgrad_bf16(ws + tp.x_in, ws + tp.g_stem, grad, scratch, B, p.H, p.W, 8, st);
+    return delora_conv2d_wgrad_bf16(ws + tp.x_in, ws + tp.g_stem, grad, scratch, B, p.H, p.W, 64, 8, 64, 3, 1, 2, st);
+}
+
+static TailIO train_tail_io(const TrainPlan& tp, char* ws) {
+    const Plan& p = tp.p;
+    TailIO io;
+    memset(&io, 0, sizeof(io));
+    const float* master = reinterpret_cast<const float*>(ws + tp.master);
+    io.fc_w = master + p.fc.blob_w; io.fc_b = master + p.fc.blob_b;
+    for (int i = 0; i < p.n_lin; ++i) { io.w[i] = master + p.lin[i].blob_w; io.b[i] = master + p.lin[i].blob_b; }
+    io.fc_out = reinterpret_cast<float*>(ws + tp.fc_out);
+    for (int i = 0; i < p.n_lin - 1; ++i) io.hid[i] = reinterpret_cast<float*>(ws + tp.hid[p.n_lin == 4 ? 0 : i]);
+    io.raw = reinterpret_cast<float*>(ws + tp.raw);
+    return io;
+}
+
+static int linear_bwd(const TailGrad& p0, const TailGrad& p1, int B, int act_in, float* dx, int lddx, cudaStream_t st) {
+    const int tiles = ((p0.K + kDgradCols - 1) / kDgradCols) * ((B + kDgradRows - 1) / kDgradRows);
+    odometry_linear_bwd_kernel<<<p0.N + p1.N + tiles, kBwdThreads, 0, st>>>(p0, p1, B, act_in, dx, lddx);
+    DELORA_CHECK_LAUNCH("odometry_linear_bwd_kernel");
+    return 0;
+}
+
+static int train_tail_backward(const TrainPlan& tp, char* ws, int act, int B, cudaStream_t st) {
+    const Plan& p = tp.p;
+    auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
+    const float* master = f(tp.master);
+    float* grad = f(tp.grad);
+    const int nout = p.fc.N;
+    OutBwd a;
+    memset(&a, 0, sizeof(a));
+    a.raw = f(tp.raw); a.grad_T = f(tp.grad_T); a.ctr = reinterpret_cast<long long*>(ws + tp.ctr);
+    if (p.n_lin == 4) {
+        a.K = kHeadHidden; a.ldx = a.ldz = 2 * kHeadHidden; a.single = 0;
+        a.w_rot = master + p.lin[1].blob_w; a.w_trans = master + p.lin[3].blob_w;
+        a.x_rot = f(tp.hid[0]); a.x_trans = f(tp.hid[0]) + kHeadHidden;
+        a.gw_rot = grad + p.lin[1].blob_w; a.gb_rot = grad + p.lin[1].blob_b;
+        a.gw_trans = grad + p.lin[3].blob_w; a.gb_trans = grad + p.lin[3].blob_b;
+        a.dz = f(tp.dz_hid[0]);
+    } else {
+        const int last = p.n_lin - 1;
+        const Linear& l = p.lin[last];
+        a.K = l.K; a.ldx = a.ldz = l.K; a.single = 1;
+        a.w_rot = master + l.blob_w; a.w_trans = a.w_rot + 4 * (size_t)l.K;
+        a.x_rot = a.x_trans = f(tp.hid[last - 1]);
+        a.gw_rot = grad + l.blob_w; a.gw_trans = a.gw_rot + 4 * (size_t)l.K;
+        a.gb_rot = grad + l.blob_b; a.gb_trans = a.gb_rot + 4;
+        a.dz = f(tp.dz_hid[last - 1]);
+    }
+    odometry_out_bwd_kernel<<<1, kBwdThreads, (size_t)B * 7 * sizeof(float), st>>>(a, B, 1.0f / (float)B, act);
+    DELORA_CHECK_LAUNCH("odometry_out_bwd_kernel");
+    auto tg = [&](const Linear& l, const float* x, int ldx, const float* dz, int ldz) {
+        TailGrad t;
+        t.w = master + l.blob_w; t.x = x; t.dz = dz; t.gw = grad + l.blob_w; t.gb = grad + l.blob_b;
+        t.K = l.K; t.N = l.N; t.ldx = ldx; t.ldz = ldz;
+        return t;
+    };
+    TailGrad none;
+    memset(&none, 0, sizeof(none));
+    int rc;
+    float* fc_out = f(tp.fc_out);
+    float* dz_fc = f(tp.dz_fc);
+    if (p.n_lin == 4) {
+        // the heads' hidden layers read the same fc output: dx = rot1^T dz_rot + trans1^T dz_trans, then act'(fc_out)
+        const int ld = 2 * kHeadHidden;
+        if ((rc = linear_bwd(tg(p.lin[0], fc_out, nout, f(tp.dz_hid[0]), ld),
+                             tg(p.lin[2], fc_out, nout, f(tp.dz_hid[0]) + kHeadHidden, ld), B, act, dz_fc, nout, st)))
+            return rc;
+    } else {
+        for (int i = p.n_lin - 2; i >= 0; --i) {
+            const float* x = i == 0 ? fc_out : f(tp.hid[i - 1]);
+            const int ldx = i == 0 ? nout : p.lin[i - 1].N;
+            float* dx = i == 0 ? dz_fc : f(tp.dz_hid[i - 1]);
+            if ((rc = linear_bwd(tg(p.lin[i], x, ldx, f(tp.dz_hid[i]), p.lin[i].N), none, B, act, dx, ldx, st))) return rc;
+        }
+    }
+    // resnet.fc: its input is the pooled trunk output; the last block's act' is applied by the average pool's backward
+    return linear_bwd(tg(p.fc, f(tp.pooled), 512, dz_fc, nout), none, B, 0, f(tp.g_pooled), 512, st);
+}
+
+static int write_prep_table(const TrainPlan& tp, char* ws, cudaStream_t st, const char* who) {
+    const Plan& p = tp.p;
+    long long table[kMaxConv * 8];
+    const float* master = reinterpret_cast<const float*>(ws + tp.master);
+    for (int i = 0; i < p.n_conv; ++i) {
+        const ConvLayer& c = p.conv[i];
+        long long* r = table + (size_t)i * 8;
+        r[0] = (long long)(uintptr_t)(master + c.blob);
+        r[1] = (long long)(uintptr_t)(ws + tp.w_fwd[i]);
+        r[2] = i == 0 ? 0 : (long long)(uintptr_t)(ws + tp.w_flip[i]);
+        r[3] = c.cout; r[4] = c.cin; r[5] = c.k;
+        r[6] = (i == 0) ? (p.stem_fast ? 16 : 64) : c.cin;
+        r[7] = (i == 0 && p.stem_fast) ? 1 : 0;
+    }
+    const cudaError_t e = cudaMemcpyAsync(ws + tp.table, table, (size_t)p.n_conv * 8 * sizeof(long long),
+                                          cudaMemcpyHostToDevice, st);
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+    return 0;
+}
+
+}  // namespace delora
+
+extern "C" int64_t delora_odometry_train_workspace_bytes(const delora_odometry_desc* d) {
+    if (check_desc(d, "delora_odometry_train_workspace_bytes")) return -1;
+    TrainPlan tp;
+    make_train_plan(d, &tp);
+    return (int64_t)tp.total;
+}
+
+extern "C" int delora_odometry_train_init(const delora_odometry_desc* d, const float* weights, void* workspace,
+                                          void* stream) {
+    const char* who = "delora_odometry_train_init";
+    if (check_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(weights && workspace, "%s: null pointer", who);
+    TrainPlan tp;
+    make_train_plan(d, &tp);
+    cudaStream_t st = (cudaStream_t)stream;
+    char* ws = (char*)workspace;
+    cudaError_t e = cudaMemsetAsync(ws, 0, tp.total, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(ws + tp.keys, 0xFF, (size_t)2 * d->max_batch * d->H * d->W * 8, st);
+    if (e == cudaSuccess)
+        e = cudaMemcpyAsync(ws + tp.master, weights, (size_t)tp.p.blob_floats * 4, cudaMemcpyDeviceToDevice, st);
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+    int rc = write_prep_table(tp, ws, st, who);
+    if (rc) return rc;
+    return delora_conv_weight_prep_multi(ws + tp.table, tp.p.n_conv, st);
+}
+
+extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
+                                          const float* points, const int32_t* n_points, int B, void* workspace,
+                                          float* losses, float* T, float* pooled, float* grads, void* stream) {
+    const char* who = "delora_odometry_train_step";
+    if (check_desc(d, who)) return 1;
+    if (check_train_params(hp, who)) return 1;
+    DELORA_CHECK_ARG(points && n_points && workspace, "%s: null pointer", who);
+    DELORA_CHECK_ARG(B >= 1 && B <= d->max_batch, "%s: B=%d outside [1, max_batch=%d]", who, B, d->max_batch);
+    TrainPlan tp;
+    make_train_plan(d, &tp);
+    const Plan& p = tp.p;
+    cudaStream_t st = (cudaStream_t)stream;
+    char* ws = (char*)workspace;
+    auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
+    const int H = d->H, W = d->W, HW = H * W;
+    long long* ctr = reinterpret_cast<long long*>(ws + tp.ctr);
+    int rc;
+    cudaError_t e = cudaSuccess;
+
+    // 1. projection + normals of the 2B scans (scan_1 x B, then scan_2 x B)
+    int32_t* counts = reinterpret_cast<int32_t*>(ws + tp.counts);
+    odometry_counts_kernel<<<(2 * B + 255) / 256, 256, 0, st>>>(n_points, 2 * B, d->n_stride, counts);
+    DELORA_CHECK_LAUNCH("odometry_counts_kernel");
+    delora_f4* pts_grid = reinterpret_cast<delora_f4*>(ws + tp.pts_grid);
+    delora_f4* nrm_grid = reinterpret_cast<delora_f4*>(ws + tp.nrm_grid);
+    float* images = f(tp.images);
+    if ((rc = delora_project_normals_fwd(points, counts, 2 * B, 3, d->n_stride, H, W, d->hfov0, d->hfov1, d->vfov0,
+                                         d->vfov1, 0, reinterpret_cast<uint64_t*>(ws + tp.keys), images,
+                                         reinterpret_cast<int32_t*>(ws + tp.index_map), hp->nb_h, hp->nb_w,
+                                         hp->epsilon_range, hp->min_neighbors, pts_grid, nrm_grid, nullptr, st)))
+        return rc;
+    // 2. forward, keeping the activations
+    if ((rc = train_trunk_forward(tp, ws, d->act, images, images + (size_t)B * 4 * HW, B, st))) return rc;
+    if ((rc = run_tail(p, train_tail_io(tp, ws), d->act, f(tp.pooled), B, f(tp.T16), st))) return rc;
+    // 3. ICP losses and dL/dT: source = scan_2 moved by T, target = scan_1
+    e = cudaMemcpy2DAsync(f(tp.T12), 12 * sizeof(float), f(tp.T16), 16 * sizeof(float), 12 * sizeof(float), B,
+                          cudaMemcpyDeviceToDevice, st);
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+    const long long icp_n4 = (delora_icp_scratch_floats(B, HW) + 3) / 4;
+    odometry_icp_rearm_kernel<<<2 * num_sms(), 256, 0, st>>>(reinterpret_cast<float4*>(ws + tp.icp), icp_n4, B, ctr);
+    DELORA_CHECK_LAUNCH("odometry_icp_rearm_kernel");
+    if ((rc = delora_icp_dense_fwd_bwd(pts_grid + (size_t)B * HW, nrm_grid + (size_t)B * HW, f(tp.T12), pts_grid, nrm_grid,
+                                       B, H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, hp->lambda_po2pl, hp->loss_flags,
+                                       f(tp.losses), f(tp.grad_T), f(tp.icp), st))) return rc;
+    // 4. backward: tail, average pool, trunk
+    if ((rc = train_tail_backward(tp, ws, d->act, B, st))) return rc;
+    if ((rc = train_trunk_backward(tp, ws, d->act, B, st))) return rc;
+    // outputs (T: the weights before the update)
+    auto out = [&](float* dst, size_t src, size_t n) {
+        if (dst && e == cudaSuccess) e = cudaMemcpyAsync(dst, ws + src, n * sizeof(float), cudaMemcpyDeviceToDevice, st);
+    };
+    out(losses, tp.losses, (size_t)B * DELORA_LOSS_ROW);
+    out(T, tp.T16, (size_t)B * 16);
+    out(pooled, tp.pooled, (size_t)B * 512);
+    out(grads, tp.grad, (size_t)p.blob_floats);
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+    // 5. Adam on the master blob, then the bf16 filters from the updated weights
+    const long long n = p.blob_floats;
+    const long long blocks = (n / 4 + 255) / 256;
+    const int grid = (int)(blocks < 8ll * num_sms() ? (blocks > 0 ? blocks : 1) : 8ll * num_sms());
+    odometry_adam_kernel<<<grid, 256, 0, st>>>(f(tp.master), f(tp.grad), f(tp.m), f(tp.v), n, ctr, hp->lr, hp->beta1,
+                                               hp->beta2, hp->eps);
+    DELORA_CHECK_LAUNCH("odometry_adam_kernel");
+    return delora_conv_weight_prep_multi(ws + tp.table, p.n_conv, st);
+}
+
+extern "C" int delora_odometry_train_weights(const delora_odometry_desc* d, const void* workspace, float* weights,
+                                             void* stream) {
+    const char* who = "delora_odometry_train_weights";
+    if (check_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(workspace && weights, "%s: null pointer", who);
+    TrainPlan tp;
+    make_train_plan(d, &tp);
+    const cudaError_t e = cudaMemcpyAsync(weights, (const char*)workspace + tp.master, (size_t)tp.p.blob_floats * 4,
+                                          cudaMemcpyDeviceToDevice, (cudaStream_t)stream);
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
     return 0;
 }

@@ -7,6 +7,7 @@ alone and hands the blob to `delora_odometry_load_weights`.  The network configu
 `config/*.yaml` (angles there are in degrees).  Checkpoints of models the C ABI cannot express are refused:
 `pre_feature_extraction: True` and `factor_fewer_resnet_channels != 1`; dropout is the identity at inference.
 """
+import collections
 import os
 import struct
 
@@ -96,6 +97,23 @@ def pack_state_dict(state_dict, config):
             raise ValueError(f"{key}: shape {tuple(t.shape)}, the configuration needs {shape}")
         parts.append(t.detach().to("cpu", torch.float32).contiguous().reshape(-1).numpy())
     return np.concatenate(parts).astype(np.float32, copy=False)
+
+
+def unpack_blob(blob, config):
+    """The inverse of pack_state_dict: a weight blob (e.g. read from a fine-tuned .dlw) -> an OdometryModel state dict
+    of fp32 CPU tensors, loadable with `model.load_state_dict`."""
+    check_supported(config)
+    flat = torch.as_tensor(np.ascontiguousarray(blob, dtype=np.float32)).reshape(-1)
+    order = state_dict_order(config)
+    want = sum(int(np.prod(shape, dtype=np.int64)) for _, shape in order)
+    if flat.numel() != want:
+        raise ValueError(f"blob has {flat.numel()} floats, the configuration needs {want}")
+    state, off = collections.OrderedDict(), 0
+    for key, shape in order:
+        n = int(np.prod(shape, dtype=np.int64))
+        state[key] = flat[off:off + n].reshape(shape).clone()
+        off += n
+    return state
 
 
 def write_dlw(path, desc, blob):

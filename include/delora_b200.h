@@ -420,6 +420,51 @@ int delora_odometry_pairs(const delora_odometry_desc* d, const float* points, co
 int delora_odometry_push(const delora_odometry_desc* d, const float* points, const int32_t* n_points,
                          void* workspace, float* T, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * Odometry training: raw scan pairs -> updated weights, one call per step.
+ * Replaces, for the self-supervised step, deploy.deployer.Deployer.step + Trainer's Adam
+ *   (src/deploy/deployer.py:237-342, src/deploy/trainer.py:23-24) as delora_b200/train_step.py's SyntheticTrainStep
+ *   runs it: projection and normals of both scans, OdometryModel.forward, the dense ICP losses (source = scan_2 moved
+ *   by the predicted T, target = scan_1), objective = mean over the pairs of po2po + lambda_po2pl * po2pl + pl2pl,
+ *   the backward through the heads, resnet.fc and the encoder trunk (the kernels and order of the Python training
+ *   encoder), one Adam update (no weight decay) of the fp32 master weights and one re-prep of the bf16 filters.
+ * Same descriptor and .dlw blob as inference; the same models are not representable.
+ *
+ * Workspace: one caller-owned device buffer of delora_odometry_train_workspace_bytes(d) bytes holds the fp32 master
+ * weights, their gradient, Adam's m, v and step count, the bf16 filters, every saved activation and backward buffer
+ * for max_batch pairs and the ICP scratch.  Its layout is a function of the descriptor (the split-K scratch of the
+ * weight gradients is sized for the current device's SM count; 132, an H100 SXM, without a device).  It holds device
+ * pointers into itself: do not move or copy it to another address.  Use: _train_init once, then any number of
+ * _train_step calls, _train_weights to read the weights out.  Every step is launches only (no allocation, no
+ * synchronisation, no host decision on device data), so a step can be captured into a CUDA graph and replayed;
+ * B may change from one step to the next.  Results are bit-identical from run to run. */
+typedef struct {
+    float lr, beta1, beta2, eps;         /* Adam (torch defaults 0.9, 0.999, 1e-8); lr >= 0, betas in [0, 1), eps > 0 */
+    float lambda_po2pl;                  /* config lambda_po2pl */
+    uint32_t loss_flags;                 /* DELORA_LOSS_* / DELORA_NORMAL_LINEAR bits, at least one loss bit */
+    int nb_h, nb_w;                      /* neighborhood_side_length (7, 11): odd and positive */
+    float epsilon_range;                 /* 0.5 */
+    int min_neighbors;                   /* min_num_points_in_neighborhood_to_determine_point_class, 10 */
+} delora_odometry_train_params;
+
+/* Host only (no GPU needed): -1 (and delora_last_error()) for an invalid descriptor. */
+int64_t delora_odometry_train_workspace_bytes(const delora_odometry_desc* d);
+/* Zero the workspace, set the projection key buffer to all ones, copy `weights` (DEVICE fp32, the .dlw blob) into the
+ * master weights, zero Adam's m, v and step count and prep the bf16 filters (fprop and flipped layouts).  The prep
+ * table is copied from host memory (the call may wait for the stream to reach it). */
+int delora_odometry_train_init(const delora_odometry_desc* d, const float* weights, void* workspace, void* stream);
+/* One training step on B pairs (1 <= B <= max_batch): points [2B, 3, n_stride] and n_points [2B] as for
+ * delora_odometry_pairs.  Outputs, each DEVICE and each may be NULL: losses [B, DELORA_LOSS_ROW] as the ICP operator
+ * writes them; T [B, 16] of the weights BEFORE the update; pooled [B, 512]; grads [weight_floats] the gradient of the
+ * objective in blob order.  Refused before any launch: an invalid descriptor or hyperparameter (the message names the
+ * field), null points / n_points / workspace, B outside [1, max_batch]. */
+int delora_odometry_train_step(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
+                               const float* points, const int32_t* n_points, int B, void* workspace,
+                               float* losses, float* T, float* pooled, float* grads, void* stream);
+/* Copy the current fp32 master weights to `weights` (DEVICE fp32[weight_floats]): a .dlw blob, loadable by
+ * delora_odometry_load_weights and delora_odometry_train_init. */
+int delora_odometry_train_weights(const delora_odometry_desc* d, const void* workspace, float* weights, void* stream);
+
 /* ---- Data-parallel training step: average of the weight gradients over the ranks (SURVEY.md 8(e); the reference
  * steps one optimizer on one device, src/deploy/trainer.py:23-24, on `loss / batch_size`, src/deploy/deployer.py:329-342
  * -- equal per-rank batches + the mean over ranks reproduce it over the global batch).
