@@ -98,6 +98,12 @@ SIGNATURES = {
     "delora_odometry_load_weights": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_pairs": (c_int, [c_desc_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_push": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_streams_workspace_bytes": (c_i64, [c_desc_p]),
+    "delora_odometry_streams_init": (c_int, [c_desc_p, c_void_p, c_void_p]),
+    "delora_odometry_streams_load_weights": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_streams_push": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                             c_void_p]),
+    "delora_odometry_streams_reset": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_train_workspace_bytes": (c_i64, [c_desc_p]),
     "delora_odometry_train_init": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_train_step": (c_int, [c_desc_p, c_train_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,

@@ -14,6 +14,7 @@
 //     of the WHOLE [B, 4] block (a quirk of the reference, :114) and quaternion -> T, in one CTA.
 // Every sum has a fixed order (lane partials in k order, then an xor butterfly; the norm is one thread's loop), there
 // are no atomics, so results are bit-identical from run to run and do not depend on B except through the norm.
+#include <cuda_bf16.h>
 #include <math.h>
 #include <string.h>
 
@@ -160,12 +161,13 @@ struct Plan {
     Linear fc;
     int64_t blob_floats;
     int stage_h[4], stage_w[4], stage_c[4];
-    // byte offsets
-    size_t keys, index_map, counts, images, prev_image, x_in, stem, pool, act[4][3], table, pooled, fc_out, hid[2];
-    size_t w_stem, total;
+    // byte offsets (has_prev: the streams layout only)
+    size_t keys, index_map, counts, images, prev_image, has_prev, x_in, stem, pool, act[4][3], table, pooled, fc_out, hid[2];
+    size_t w_stem, keys_bytes, total;
 };
 
 static size_t align256(size_t n) { return (n + 255) & ~(size_t)255; }
+static size_t take(size_t& off, size_t bytes) { const size_t o = off; off += align256(bytes); return o; }
 static int out_size(int n, int s) { return (n - 1) / s + 1; }
 static size_t nhwc_bytes(int b, int h, int w, int c) { return (size_t)b * (h + 2) * (w + 2) * c * 2; }
 
@@ -190,9 +192,9 @@ static int check_desc(const delora_odometry_desc* d, const char* who) {
     return 0;
 }
 
-// Walks the model in state_dict order (src/models/resnet_modified.py:49-66 + model.py:58-84) and lays out the
-// workspace.  A pure function of the descriptor.
-static void make_plan(const delora_odometry_desc* d, Plan* p) {
+// Walks the model in state_dict order (src/models/resnet_modified.py:49-66 + model.py:58-84).  A pure function of the
+// descriptor.
+static void plan_model(const delora_odometry_desc* d, Plan* p) {
     memset(p, 0, sizeof(Plan));
     p->H = d->H; p->W = d->W; p->MB = d->max_batch;
     p->w2 = out_size(d->W, 2); p->w4 = p->w2 / 2;
@@ -238,54 +240,78 @@ static void make_plan(const delora_odometry_desc* d, Plan* p) {
         p->n_lin = 4;
     }
     p->blob_floats = blob;
+}
 
-    // workspace
-    const int MB = d->max_batch, HW = d->H * d->W;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { const size_t o = off; off += align256(bytes); return o; };
-    p->keys = take((size_t)2 * MB * HW * 8);
-    p->index_map = take((size_t)2 * MB * HW * 4);
-    p->counts = take((size_t)2 * MB * 4);
-    p->images = take((size_t)2 * MB * 4 * HW * 4);
-    p->prev_image = take((size_t)4 * HW * 4);
-    p->x_in = take(nhwc_bytes(MB, d->H, d->W, p->stem_fast ? 16 : 64));
-    p->stem = take(nhwc_bytes(MB, d->H, p->w2, 64));
+// The part of a workspace after its frame buffers, common to the pairs / push and the streams layouts: the trunk's
+// activations for max_batch images, the tail's, the prep table and the weights.
+static void plan_trunk_tail(const delora_odometry_desc* d, Plan* p, size_t off) {
+    const int MB = d->max_batch, nout = d->resnet_outputs;
+    p->x_in = take(off, nhwc_bytes(MB, d->H, d->W, p->stem_fast ? 16 : 64));
+    p->stem = take(off, nhwc_bytes(MB, d->H, p->w2, 64));
     // stage s buffers: [0] the pool output (stage 0) / the downsample output, [1] conv1 output, [2] block output;
     // later blocks of the stage alternate their output between [0] and [2]
     for (int s = 0; s < 4; ++s)
-        for (int j = 0; j < 3; ++j) p->act[s][j] = take(nhwc_bytes(MB, p->stage_h[s], p->stage_w[s], p->stage_c[s]));
+        for (int j = 0; j < 3; ++j) p->act[s][j] = take(off, nhwc_bytes(MB, p->stage_h[s], p->stage_w[s], p->stage_c[s]));
     p->pool = p->act[0][0];
-    p->pooled = take((size_t)MB * 512 * 4);
-    p->fc_out = take((size_t)MB * nout * 4);
-    p->hid[0] = take((size_t)MB * 512 * 4);
-    p->hid[1] = take((size_t)MB * 512 * 4);
-    p->table = take((size_t)(kMaxConv + 1) * 8 * 8);
-    p->w_stem = take(p->stem_fast ? (size_t)3 * 64 * 64 * 2 : (size_t)64 * 9 * 64 * 2);
+    p->pooled = take(off, (size_t)MB * 512 * 4);
+    p->fc_out = take(off, (size_t)MB * nout * 4);
+    p->hid[0] = take(off, (size_t)MB * 512 * 4);
+    p->hid[1] = take(off, (size_t)MB * 512 * 4);
+    p->table = take(off, (size_t)(kMaxConv + 1) * 8 * 8);
+    p->w_stem = take(off, p->stem_fast ? (size_t)3 * 64 * 64 * 2 : (size_t)64 * 9 * 64 * 2);
     for (int i = 1; i < p->n_conv; ++i) {
         ConvLayer& c = p->conv[i];
-        c.ws = take((size_t)c.cout * c.k * c.k * c.cin * 2);
+        c.ws = take(off, (size_t)c.cout * c.k * c.k * c.cin * 2);
     }
     p->conv[0].ws = p->w_stem;
-    p->fc.ws_w = take((size_t)p->fc.K * p->fc.N * 4);
-    p->fc.ws_b = take((size_t)p->fc.N * 4);
+    p->fc.ws_w = take(off, (size_t)p->fc.K * p->fc.N * 4);
+    p->fc.ws_b = take(off, (size_t)p->fc.N * 4);
     for (int i = 0; i < p->n_lin; ++i) {
-        p->lin[i].ws_w = take((size_t)p->lin[i].K * p->lin[i].N * 4);
-        p->lin[i].ws_b = take((size_t)p->lin[i].N * 4);
+        p->lin[i].ws_w = take(off, (size_t)p->lin[i].K * p->lin[i].N * 4);
+        p->lin[i].ws_b = take(off, (size_t)p->lin[i].N * 4);
     }
     p->total = off;
 }
 
-static int run_trunk(const Plan& p, char* ws, int act, const float* img1, const float* img2, int B, float* pooled,
-                     cudaStream_t st) {
+// The pairs / push workspace: frame buffers for 2 * max_batch scans and the one cached previous image of _push.
+static void make_plan(const delora_odometry_desc* d, Plan* p) {
+    plan_model(d, p);
+    const int MB = d->max_batch, HW = d->H * d->W;
+    size_t off = 0;
+    p->keys_bytes = (size_t)2 * MB * HW * 8;
+    p->keys = take(off, p->keys_bytes);
+    p->index_map = take(off, (size_t)2 * MB * HW * 4);
+    p->counts = take(off, (size_t)2 * MB * 4);
+    p->images = take(off, (size_t)2 * MB * 4 * HW * 4);
+    p->prev_image = take(off, (size_t)4 * HW * 4);
+    plan_trunk_tail(d, p, off);
+}
+
+// The streams workspace (S = max_batch streams): this tick's S frames, each stream's previous frame and whether it has
+// one; the trunk and tail then run at B = S.
+static void make_streams_plan(const delora_odometry_desc* d, Plan* p) {
+    plan_model(d, p);
+    const int S = d->max_batch, HW = d->H * d->W;
+    size_t off = 0;
+    p->keys_bytes = (size_t)S * HW * 8;
+    p->keys = take(off, p->keys_bytes);
+    p->index_map = take(off, (size_t)S * HW * 4);
+    p->counts = take(off, (size_t)S * 4);
+    p->images = take(off, (size_t)S * 4 * HW * 4);
+    p->prev_image = take(off, (size_t)S * 4 * HW * 4);
+    p->has_prev = take(off, (size_t)S * 4);
+    plan_trunk_tail(d, p, off);
+}
+
+// The trunk from its bf16 NHWC input (x_in, 16 channels when W is even, 64 otherwise) to the pooled features.
+static int run_trunk_from_input(const Plan& p, char* ws, int act, int B, float* pooled, cudaStream_t st) {
     int rc;
     const int H = p.H, W = p.W;
     void* x_in = ws + p.x_in;
     void* stem = ws + p.stem;
     if (p.stem_fast) {
-        if ((rc = delora_images_to_nhwc16_bf16(img1, img2, B, H, W, x_in, st))) return rc;
         if ((rc = delora_stem_fprop_bf16(x_in, ws + p.w_stem, stem, B, H, W, act, 0, st))) return rc;
     } else {
-        if ((rc = delora_images_to_nhwc_bf16(img1, img2, B, H, W, 64, x_in, st))) return rc;
         if ((rc = delora_conv2d_fprop_bf16(x_in, ws + p.w_stem, nullptr, nullptr, stem, B, H, W, 64, 64, 3, 1, 2, act, st)))
             return rc;
     }
@@ -310,6 +336,14 @@ static int run_trunk(const Plan& p, char* ws, int act, const float* img1, const 
         cur = out;
     }
     return delora_avgpool_nhwc_bf16(cur, B, p.stage_h[3], p.stage_w[3], 512, pooled, st);
+}
+
+static int run_trunk(const Plan& p, char* ws, int act, const float* img1, const float* img2, int B, float* pooled,
+                     cudaStream_t st) {
+    const int rc = p.stem_fast ? delora_images_to_nhwc16_bf16(img1, img2, B, p.H, p.W, ws + p.x_in, st)
+                               : delora_images_to_nhwc_bf16(img1, img2, B, p.H, p.W, 64, ws + p.x_in, st);
+    if (rc) return rc;
+    return run_trunk_from_input(p, ws, act, B, pooled, st);
 }
 
 // Where the tail reads its weights and writes its activations.  Inference: the workspace copies of the weights and two
@@ -344,7 +378,9 @@ static TailIO inference_tail_io(const Plan& p, char* ws) {
     return io;
 }
 
-static int run_tail(const Plan& p, const TailIO& io, int act, const float* pooled, int B, float* T, cudaStream_t st) {
+// resnet.fc and the heads' hidden layers for B rows; rot / trans: the heads' last layers, for the output kernel
+static int run_tail_hidden(const Plan& p, const TailIO& io, int act, const float* pooled, int B, TailLinear* rot_out,
+                           TailLinear* trans_out, cudaStream_t st) {
     float* fc_out = io.fc_out;
     TailLinear none;
     memset(&none, 0, sizeof(none));
@@ -385,6 +421,15 @@ static int run_tail(const Plan& p, const TailIO& io, int act, const float* poole
         trans.bias = rot.bias + 4;
         trans.N = 3;
     }
+    *rot_out = rot;
+    *trans_out = trans;
+    return 0;
+}
+
+static int run_tail(const Plan& p, const TailIO& io, int act, const float* pooled, int B, float* T, cudaStream_t st) {
+    TailLinear rot, trans;
+    const int rc = run_tail_hidden(p, io, act, pooled, B, &rot, &trans, st);
+    if (rc) return rc;
     const int vec = (rot.K % 4 == 0 && rot.ldx % 4 == 0) ? 1 : 0;
     odometry_out_kernel<<<1, kTailWarps * 32, (size_t)B * 7 * sizeof(float), st>>>(rot, trans, B, vec, T, io.raw);
     DELORA_CHECK_LAUNCH("odometry_out_kernel");
@@ -419,26 +464,17 @@ extern "C" int64_t delora_odometry_workspace_bytes(const delora_odometry_desc* d
     return (int64_t)p.total;
 }
 
-extern "C" int delora_odometry_init(const delora_odometry_desc* d, void* workspace, void* stream) {
-    if (check_desc(d, "delora_odometry_init")) return 1;
-    DELORA_CHECK_ARG(workspace, "delora_odometry_init: null workspace");
-    Plan p;
-    make_plan(d, &p);
-    cudaStream_t st = (cudaStream_t)stream;
+namespace delora {
+
+static int init_workspace(const Plan& p, void* workspace, cudaStream_t st, const char* who) {
     char* ws = (char*)workspace;
     cudaError_t e = cudaMemsetAsync(ws, 0, p.total, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(ws + p.keys, 0xFF, (size_t)2 * p.MB * p.H * p.W * 8, st);
-    DELORA_CHECK_ARG(e == cudaSuccess, "delora_odometry_init: %s", cudaGetErrorString(e));
+    if (e == cudaSuccess) e = cudaMemsetAsync(ws + p.keys, 0xFF, p.keys_bytes, st);
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
     return 0;
 }
 
-extern "C" int delora_odometry_load_weights(const delora_odometry_desc* d, const float* weights, void* workspace,
-                                            void* stream) {
-    if (check_desc(d, "delora_odometry_load_weights")) return 1;
-    DELORA_CHECK_ARG(weights && workspace, "delora_odometry_load_weights: null pointer");
-    Plan p;
-    make_plan(d, &p);
-    cudaStream_t st = (cudaStream_t)stream;
+static int load_weights(const Plan& p, const float* weights, void* workspace, cudaStream_t st, const char* who) {
     char* ws = (char*)workspace;
     // one delora_conv_weight_prep_multi row per filter: {fp32 src, w_fwd, w_flip, Cout, Cin, k, Cin_pad, kind};
     // the stem in the 16-channel layout (kind 1) when W is even, channel-padded to 64 otherwise
@@ -454,7 +490,7 @@ extern "C" int delora_odometry_load_weights(const delora_odometry_desc* d, const
         r[7] = (i == 0 && p.stem_fast) ? 1 : 0;
     }
     cudaError_t e = cudaMemcpyAsync(ws + p.table, table, (size_t)p.n_conv * 8 * sizeof(long long), cudaMemcpyHostToDevice, st);
-    DELORA_CHECK_ARG(e == cudaSuccess, "delora_odometry_load_weights: %s", cudaGetErrorString(e));
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
     int rc = delora_conv_weight_prep_multi(ws + p.table, p.n_conv, st);
     if (rc) return rc;
     auto copy = [&](size_t dst, int64_t src, int64_t n) {
@@ -466,8 +502,27 @@ extern "C" int delora_odometry_load_weights(const delora_odometry_desc* d, const
         e = copy(p.lin[i].ws_w, p.lin[i].blob_w, (int64_t)p.lin[i].K * p.lin[i].N);
         if (e == cudaSuccess) e = copy(p.lin[i].ws_b, p.lin[i].blob_b, p.lin[i].N);
     }
-    DELORA_CHECK_ARG(e == cudaSuccess, "delora_odometry_load_weights: %s", cudaGetErrorString(e));
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
     return 0;
+}
+
+}  // namespace delora
+
+extern "C" int delora_odometry_init(const delora_odometry_desc* d, void* workspace, void* stream) {
+    if (check_desc(d, "delora_odometry_init")) return 1;
+    DELORA_CHECK_ARG(workspace, "delora_odometry_init: null workspace");
+    Plan p;
+    make_plan(d, &p);
+    return init_workspace(p, workspace, (cudaStream_t)stream, "delora_odometry_init");
+}
+
+extern "C" int delora_odometry_load_weights(const delora_odometry_desc* d, const float* weights, void* workspace,
+                                            void* stream) {
+    if (check_desc(d, "delora_odometry_load_weights")) return 1;
+    DELORA_CHECK_ARG(weights && workspace, "delora_odometry_load_weights: null pointer");
+    Plan p;
+    make_plan(d, &p);
+    return load_weights(p, weights, workspace, (cudaStream_t)stream, "delora_odometry_load_weights");
 }
 
 extern "C" int delora_odometry_pairs(const delora_odometry_desc* d, const float* points, const int32_t* n_points, int B,
@@ -513,6 +568,210 @@ extern "C" int delora_odometry_push(const delora_odometry_desc* d, const float* 
     }
     const cudaError_t e = cudaMemcpyAsync(prev, image, (size_t)4 * d->H * d->W * sizeof(float), cudaMemcpyDeviceToDevice, st);
     DELORA_CHECK_ARG(e == cudaSuccess, "delora_odometry_push: %s", cudaGetErrorString(e));
+    return 0;
+}
+
+// ================================================================================================ streams
+// delora_odometry_streams_push: S = max_batch independent streams in one workspace.  Per tick: the masked count clamp,
+// the projection of the S new frames (inactive streams project 0 points), the fused input conversion + cache update,
+// the trunk and the fc / hidden layers at B = S (the launches of _pairs), and the per-row output kernel.  A stream's row
+// goes through the same instructions as _push's batch-1 call: the trunk's kernels and the tail's row_dot4 sum a row
+// in an order that does not depend on B, and the output kernel divides each quaternion by its own norm, which at B = 1
+// is the block norm of odometry_out_kernel.  Every launch is unconditional; activity and per-stream state are read on
+// the device only.
+namespace delora {
+
+__device__ __forceinline__ bool stream_active(const int32_t* __restrict__ active, int s) {
+    return active == nullptr || active[s] != 0;
+}
+
+// counts[s] = active ? clamp(n_points[s], 0, n_stride) : 0
+__global__ void odometry_streams_counts_kernel(const int32_t* __restrict__ n_in, const int32_t* __restrict__ active,
+                                               int S, int n_stride, int32_t* __restrict__ n_out) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s < S) n_out[s] = stream_active(active, s) ? min(max(n_in[s], 0), n_stride) : 0;
+}
+
+// (prev [S,4,H,W], cur [S,4,H,W]) fp32 -> the trunk input [S, H+2, W+2, C] bf16 with the bits of images_to_nhwc16_kernel
+// (C = 16) / images_to_nhwc_kernel (C = 64, Cpad 64), and cur -> prev for every active stream.
+// One thread per (stream, padded row, image column w, 8-channel group; C = 16 has one group of 16).  The thread of
+// column w writes padded column w + 1, and also the circular halo column 0 when w = W - 1 and column W + 1 when w = 0.
+// So every prev pixel has exactly one reader, the thread that then overwrites it: no pixel is overwritten before it is
+// read, without a barrier.  prev is read with plain loads (it is written in this kernel).
+template <int C>
+__global__ void __launch_bounds__(256)
+odometry_streams_input_kernel(const float* __restrict__ cur, float* prev, const int32_t* __restrict__ active, int S,
+                              int H, int W, __nv_bfloat16* __restrict__ x) {
+    constexpr int G = C == 16 ? 1 : C / 8;
+    const int Hp = H + 2, Wp = W + 2;
+    const size_t total = (size_t)S * Hp * W * G;
+    const size_t i = (size_t)blockIdx.x * 256 + threadIdx.x;
+    if (i >= total) return;
+    const int grp = (int)(i % G);
+    const size_t pix = i / G;
+    const int w = (int)(pix % W), hp = (int)((pix / W) % Hp), s = (int)(pix / ((size_t)W * Hp));
+    uint4 v0 = make_uint4(0u, 0u, 0u, 0u), v1 = make_uint4(0u, 0u, 0u, 0u);
+    const bool interior = hp != 0 && hp != Hp - 1;
+    if (grp == 0 && interior) {
+        const size_t plane = (size_t)H * W, base = (size_t)s * 4 * plane + (size_t)(hp - 1) * W + w;
+        float f[8];
+#pragma unroll
+        for (int c = 0; c < 4; ++c) { f[c] = prev[base + c * plane]; f[4 + c] = __ldg(cur + base + c * plane); }
+        if (C == 16) {
+            __nv_bfloat16 hv[8], lv[8];
+#pragma unroll
+            for (int c = 0; c < 8; ++c) {
+                hv[c] = __float2bfloat16_rn(f[c]);
+                lv[c] = __float2bfloat16_rn(f[c] - __bfloat162float(hv[c]));
+            }
+            v0 = *reinterpret_cast<uint4*>(hv);
+            v1 = *reinterpret_cast<uint4*>(lv);
+        } else {
+            __nv_bfloat162 v[4];
+#pragma unroll
+            for (int c = 0; c < 4; ++c) v[c] = __floats2bfloat162_rn(f[2 * c], f[2 * c + 1]);
+            v0 = *reinterpret_cast<uint4*>(v);
+        }
+        if (stream_active(active, s)) {
+#pragma unroll
+            for (int c = 0; c < 4; ++c) prev[base + c * plane] = f[4 + c];
+        }
+    }
+    auto store = [&](int wp) {
+        __nv_bfloat16* dst = x + (((size_t)s * Hp + hp) * Wp + wp) * C + grp * 8;
+        reinterpret_cast<uint4*>(dst)[0] = v0;
+        if (C == 16) reinterpret_cast<uint4*>(dst)[1] = v1;
+    };
+    store(w + 1);
+    if (w == W - 1) store(0);
+    if (w == 0) store(W + 1);
+}
+
+// The last layer of the heads and quaternion -> T for every stream with an active frame and a previous one; each
+// quaternion is divided by the norm of its own row, with the instructions odometry_out_kernel runs at B = 1 (row_dot4
+// with nb = 1, fmaf over the 4 components in order, sqrtf, the four divisions, quat_to_T_row).  valid[s] = 1 for those
+// streams, 0 for the others (whose T row is not written); then every active stream has a previous frame.
+__global__ void __launch_bounds__(kTailWarps * 32)
+odometry_streams_out_kernel(TailLinear rot, TailLinear trans, int S, int vec, const int32_t* __restrict__ active,
+                            int32_t* __restrict__ has_prev, float* __restrict__ T, int32_t* __restrict__ valid) {
+    extern __shared__ float s_out[];                        // [S, 7]: quaternion (x, y, z, w), translation
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int i = warp; i < S * 7; i += kTailWarps) {
+        const int b = i / 7, o = i - b * 7;
+        if (!stream_active(active, b) || has_prev[b] == 0) continue;    // warp-uniform
+        const TailLinear p = o < 4 ? rot : trans;
+        const int n = o < 4 ? o : o - 4;
+        float acc[4];
+        row_dot4(p.w + (size_t)n * p.K, p.x + (size_t)b * p.ldx, p.ldx, p.K, 1, lane, vec, acc);
+        if (lane == 0) s_out[i] = acc[0] + __ldg(p.bias + n);
+    }
+    __syncthreads();
+    for (int b = threadIdx.x; b < S; b += blockDim.x) {
+        const bool act = stream_active(active, b);
+        const bool ok = act && has_prev[b] != 0;
+        if (ok) {
+            const float* q = s_out + b * 7;
+            float ss = 0.0f;
+            for (int j = 0; j < 4; ++j) ss = fmaf(q[j], q[j], ss);
+            const float nrm = sqrtf(ss);
+            quat_to_T_row(q[0] / nrm, q[1] / nrm, q[2] / nrm, q[3] / nrm, q[4], q[5], q[6], T + (size_t)b * 16);
+        }
+        valid[b] = ok ? 1 : 0;
+        if (act) has_prev[b] = 1;
+    }
+}
+
+__global__ void odometry_streams_reset_kernel(const int32_t* __restrict__ mask, int S, int32_t* __restrict__ has_prev) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s < S && mask[s] != 0) has_prev[s] = 0;
+}
+
+}  // namespace delora
+
+extern "C" int64_t delora_odometry_streams_workspace_bytes(const delora_odometry_desc* d) {
+    if (check_desc(d, "delora_odometry_streams_workspace_bytes")) return -1;
+    Plan p;
+    make_streams_plan(d, &p);
+    return (int64_t)p.total;
+}
+
+extern "C" int delora_odometry_streams_init(const delora_odometry_desc* d, void* workspace, void* stream) {
+    const char* who = "delora_odometry_streams_init";
+    if (check_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    Plan p;
+    make_streams_plan(d, &p);
+    return init_workspace(p, workspace, (cudaStream_t)stream, who);
+}
+
+extern "C" int delora_odometry_streams_load_weights(const delora_odometry_desc* d, const float* weights, void* workspace,
+                                                    void* stream) {
+    const char* who = "delora_odometry_streams_load_weights";
+    if (check_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(weights, "%s: null weights", who);
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    Plan p;
+    make_streams_plan(d, &p);
+    return load_weights(p, weights, workspace, (cudaStream_t)stream, who);
+}
+
+extern "C" int delora_odometry_streams_push(const delora_odometry_desc* d, const float* points, const int32_t* n_points,
+                                            const int32_t* active, void* workspace, float* T, int32_t* valid,
+                                            void* stream) {
+    const char* who = "delora_odometry_streams_push";
+    if (check_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(points, "%s: null points", who);
+    DELORA_CHECK_ARG(n_points, "%s: null n_points", who);
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    DELORA_CHECK_ARG(T, "%s: null T", who);
+    DELORA_CHECK_ARG(valid, "%s: null valid", who);
+    Plan p;
+    make_streams_plan(d, &p);
+    cudaStream_t st = (cudaStream_t)stream;
+    char* ws = (char*)workspace;
+    const int S = d->max_batch, H = d->H, W = d->W;
+    float* cur = reinterpret_cast<float*>(ws + p.images);
+    float* prev = reinterpret_cast<float*>(ws + p.prev_image);
+    int32_t* counts = reinterpret_cast<int32_t*>(ws + p.counts);
+    int32_t* has_prev = reinterpret_cast<int32_t*>(ws + p.has_prev);
+    odometry_streams_counts_kernel<<<(S + 255) / 256, 256, 0, st>>>(n_points, active, S, d->n_stride, counts);
+    DELORA_CHECK_LAUNCH("odometry_streams_counts_kernel");
+    int rc;
+    if ((rc = delora_project_fwd(points, counts, S, 3, d->n_stride, H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, 0,
+                                 reinterpret_cast<uint64_t*>(ws + p.keys), cur,
+                                 reinterpret_cast<int32_t*>(ws + p.index_map), st))) return rc;
+    __nv_bfloat16* x_in = reinterpret_cast<__nv_bfloat16*>(ws + p.x_in);
+    if (p.stem_fast) {
+        const size_t n = (size_t)S * (H + 2) * W;
+        odometry_streams_input_kernel<16><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(cur, prev, active, S, H, W, x_in);
+    } else {
+        const size_t n = (size_t)S * (H + 2) * W * 8;
+        odometry_streams_input_kernel<64><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(cur, prev, active, S, H, W, x_in);
+    }
+    DELORA_CHECK_LAUNCH("odometry_streams_input_kernel");
+    float* pooled = reinterpret_cast<float*>(ws + p.pooled);
+    if ((rc = run_trunk_from_input(p, ws, d->act, S, pooled, st))) return rc;
+    TailLinear rot, trans;
+    if ((rc = run_tail_hidden(p, inference_tail_io(p, ws), d->act, pooled, S, &rot, &trans, st))) return rc;
+    const int vec = (rot.K % 4 == 0 && rot.ldx % 4 == 0) ? 1 : 0;
+    odometry_streams_out_kernel<<<1, kTailWarps * 32, (size_t)S * 7 * sizeof(float), st>>>(rot, trans, S, vec, active,
+                                                                                          has_prev, T, valid);
+    DELORA_CHECK_LAUNCH("odometry_streams_out_kernel");
+    return 0;
+}
+
+extern "C" int delora_odometry_streams_reset(const delora_odometry_desc* d, const int32_t* mask, void* workspace,
+                                             void* stream) {
+    const char* who = "delora_odometry_streams_reset";
+    if (check_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(mask, "%s: null mask", who);
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    Plan p;
+    make_streams_plan(d, &p);
+    const int S = d->max_batch;
+    odometry_streams_reset_kernel<<<(S + 255) / 256, 256, 0, (cudaStream_t)stream>>>(
+        mask, S, reinterpret_cast<int32_t*>((char*)workspace + p.has_prev));
+    DELORA_CHECK_LAUNCH("odometry_streams_reset_kernel");
     return 0;
 }
 

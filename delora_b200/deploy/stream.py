@@ -7,7 +7,11 @@ runs the encoder through cuDNN and synchronises with the host three times.  Here
 (the previous frame's range image is kept on the device), the encoder forward on the wgmma kernels and the
 quaternion -> T kernel, captured once in a CUDA graph (25 launches replayed as one) between a pinned-memory
 H2D of the raw scan and a 64-byte D2H of the relative transform.  BASELINE config #5.
+
+OdometryStreams serves several streams of one sensor geometry and model from one C-ABI workspace, batched.
 """
+import ctypes
+
 import numpy as np
 import torch
 
@@ -111,3 +115,133 @@ class OdometryStream:
     def reset(self):
         self.frames = 0
         self.relative = []
+
+
+class OdometryStreams:
+    """Several LiDAR streams (sensors of one robot, or vehicles served by one process) through one streams workspace of
+    the C ABI (`delora_odometry_streams_*`): all streams share the image geometry and the model, and one tick runs the
+    model once at batch `n_streams`.  Each stream's transforms are bit-identical to a `delora_odometry_push` workspace
+    fed only that stream's frames (each quaternion is divided by its own row's norm, as at batch 1).
+
+    Per tick: the scans are copied into one pinned staging buffer (points, counts, activity flags), one H2D copy, one
+    graph replay (or the eager call), one D2H copy of T and valid, one synchronise."""
+
+    def __init__(self, model, config, dataset, n_streams, n_max, use_cuda_graph=True):
+        from .. import _lib
+        from . import export
+        self.config = config
+        self.dataset = dataset
+        self.device = torch.device(config["device"])
+        if self.device.type != "cuda":
+            raise RuntimeError("OdometryStreams runs on CUDA devices only (no CPU fallback)")
+        self.n_streams, self.n_max = int(n_streams), int(n_max)
+        self._L = _lib.lib()
+        self._check = _lib.check
+        self.desc = export.desc_from_config(config, dataset, self.n_max, self.n_streams)
+        self._dp = ctypes.byref(self.desc)
+        nbytes = int(self._L.delora_odometry_streams_workspace_bytes(self._dp))
+        if nbytes < 0:
+            raise ValueError(self._L.delora_last_error().decode())
+        S, n = self.n_streams, self.n_max
+        with torch.cuda.device(self.device):
+            self.workspace = torch.empty((nbytes,), dtype=torch.uint8, device=self.device)
+            self.blob = torch.from_numpy(export.pack_state_dict(model.state_dict(), config)).to(self.device)
+            self._check(self._L.delora_odometry_streams_init(self._dp, self.workspace.data_ptr(), self._stream()),
+                        "delora_odometry_streams_init")
+            self._check(self._L.delora_odometry_streams_load_weights(self._dp, self.blob.data_ptr(),
+                                                                     self.workspace.data_ptr(), self._stream()),
+                        "delora_odometry_streams_load_weights")
+            # staging: points [S, 3, n_max] fp32, then counts [S] and active [S] int32, one buffer each way
+            in_bytes = S * 3 * n * 4 + 2 * S * 4
+            self.host_in = torch.zeros((in_bytes,), dtype=torch.uint8).pin_memory()
+            self.dev_in = torch.zeros((in_bytes,), dtype=torch.uint8, device=self.device)
+            out_bytes = S * 16 * 4 + S * 4                       # T [S, 16] fp32, valid [S] int32
+            self.host_out = torch.zeros((out_bytes,), dtype=torch.uint8).pin_memory()
+            self.dev_out = torch.zeros((out_bytes,), dtype=torch.uint8, device=self.device)
+            self.dev_mask = torch.zeros((S,), dtype=torch.int32, device=self.device)
+        raw = self.host_in.numpy()
+        self._host_points = raw[:S * 3 * n * 4].view(np.float32).reshape(S, 3, n)
+        self._host_counts = raw[S * 3 * n * 4:S * 3 * n * 4 + S * 4].view(np.int32)
+        self._host_active = raw[S * 3 * n * 4 + S * 4:].view(np.int32)
+        out = self.host_out.numpy()
+        self._host_T = out[:S * 64].view(np.float32).reshape(S, 4, 4)
+        self._host_valid = out[S * 64:].view(np.int32)
+        base_in, base_out = self.dev_in.data_ptr(), self.dev_out.data_ptr()
+        self._ptrs = (base_in, base_in + S * 3 * n * 4, base_in + S * 3 * n * 4 + S * 4, base_out, base_out + S * 64)
+        self.relative = [[] for _ in range(S)]
+        self.use_cuda_graph = bool(use_cuda_graph)
+        self.graph = None
+
+    @staticmethod
+    def _stream():
+        return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+    def _tick(self):
+        points, counts, active, T, valid = self._ptrs
+        self._check(self._L.delora_odometry_streams_push(self._dp, points, counts, active, self.workspace.data_ptr(), T,
+                                                         valid, self._stream()), "delora_odometry_streams_push")
+
+    def _capture(self):
+        # a tick with every stream inactive changes no stream's state: it warms the launchers' host-side caches, then
+        # the call is captured (capturing runs nothing)
+        active = self._ptrs[2]
+        torch.cuda.current_stream().synchronize()
+        self.dev_in[active - self._ptrs[0]:].zero_()
+        self._tick()
+        torch.cuda.current_stream().synchronize()
+        self.graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.graph):
+            self._tick()
+
+    def push(self, scans):
+        """scans: a list of n_streams entries, each a [3, N] (or [1, 3, N]) float32 host tensor with N <= n_max, or
+        None for a stream without a frame this tick.  Returns a list of n_streams entries: the relative transform
+        T_{k-1,k} of the stream as a [1, 4, 4] numpy array, or None (no frame, or the stream's first frame)."""
+        if len(scans) != self.n_streams:
+            raise ValueError(f"push takes {self.n_streams} entries (one per stream, None = inactive), got {len(scans)}")
+        with torch.cuda.device(self.device):
+            if self.use_cuda_graph and self.graph is None:
+                self._capture()
+            for s, scan in enumerate(scans):
+                if scan is None:
+                    self._host_active[s] = 0
+                    self._host_counts[s] = 0
+                    continue
+                scan = scan[0] if scan.dim() == 3 else scan
+                n = int(scan.shape[1])
+                if n > self.n_max:
+                    raise Exception(f"stream {s}: scan has more points than the streams were sized for")
+                np.copyto(self._host_points[s, :, :n], scan[:3].numpy())
+                self._host_counts[s] = n
+                self._host_active[s] = 1
+            self.dev_in.copy_(self.host_in, non_blocking=True)
+            if self.graph is not None:
+                self.graph.replay()
+            else:
+                self._tick()
+            self.host_out.copy_(self.dev_out, non_blocking=True)
+            torch.cuda.current_stream().synchronize()
+        out = []
+        for s in range(self.n_streams):
+            if self._host_valid[s]:
+                t = self._host_T[s][None].copy()
+                self.relative[s].append(t)
+                out.append(t)
+            else:
+                out.append(None)
+        return out
+
+    def poses(self, s):
+        """World-frame KITTI poses of stream s so far (src/utility/poses.py:11-58)."""
+        return poses_module.compute_poses(self.relative[s])
+
+    def reset(self, s):
+        """Forget stream s's previous frame and its transforms: its next frame starts it again."""
+        with torch.cuda.device(self.device):
+            self.dev_mask.zero_()
+            self.dev_mask[s] = 1
+            self._check(self._L.delora_odometry_streams_reset(self._dp, self.dev_mask.data_ptr(),
+                                                              self.workspace.data_ptr(), self._stream()),
+                        "delora_odometry_streams_reset")
+            torch.cuda.current_stream().synchronize()
+        self.relative[s] = []

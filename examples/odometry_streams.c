@@ -1,0 +1,191 @@
+/*
+ * Several LiDAR streams from a C host, batched in one workspace: no Python, no torch.  Links libdelora_b200.so and
+ * cudart only.
+ *
+ *   odometry_streams model.dlw stream0_dir stream1_dir ...
+ *
+ * model.dlw is written by bin/export_odometry_weights.py (layout: include/delora_b200.h); every directory holds one
+ * stream's KITTI velodyne .bin files ([N, 4] float32 rows: x, y, z, reflectance), taken in name order.  All streams
+ * share the model and the sensor geometry of model.dlw; the number of directories is the number of streams.  Streams
+ * of different lengths go inactive once they run out of scans.  Per tick, for every stream with a transform, it prints
+ * one line: the stream index, the frame index k, and T_{k-1,k} as 12 floats (the top three rows of the 4x4, row-major).
+ *
+ * Build:  cc odometry_streams.c -I include -I $CUDA_HOME/include -L delora_b200 -ldelora_b200 \
+ *            -L $CUDA_HOME/lib64 -lcudart -Wl,-rpath,$PWD/delora_b200 -o odometry_streams
+ */
+#include <dirent.h>
+#include <stdio.h>
+#include <stdlib.h>
+#include <string.h>
+
+#include <cuda_runtime.h>
+
+#include "delora_b200.h"
+
+static int fail(const char* what) {
+    fprintf(stderr, "odometry_streams: %s\n", what);
+    return 1;
+}
+
+#define CUDA_OK(call)                                                                  \
+    do {                                                                               \
+        cudaError_t e_ = (call);                                                       \
+        if (e_ != cudaSuccess) return fail(cudaGetErrorString(e_));                     \
+    } while (0)
+
+#define DELORA_OK(call)                                                                \
+    do {                                                                               \
+        if ((call) != 0) return fail(delora_last_error());                             \
+    } while (0)
+
+typedef struct {
+    char** paths;
+    int n;
+} scan_list;
+
+static int by_name(const void* a, const void* b) { return strcmp(*(char* const*)a, *(char* const*)b); }
+
+/* the .bin files of one directory, sorted by name; 0 on success */
+static int list_scans(const char* dir, scan_list* out) {
+    DIR* d = opendir(dir);
+    if (!d) return 1;
+    int cap = 16;
+    out->n = 0;
+    out->paths = (char**)malloc(sizeof(char*) * (size_t)cap);
+    if (!out->paths) { closedir(d); return 1; }
+    const struct dirent* e;
+    while ((e = readdir(d)) != NULL) {
+        const size_t len = strlen(e->d_name);
+        if (len < 5 || strcmp(e->d_name + len - 4, ".bin") != 0) continue;
+        if (out->n == cap) {
+            cap *= 2;
+            char** grown = (char**)realloc(out->paths, sizeof(char*) * (size_t)cap);
+            if (!grown) { closedir(d); return 1; }
+            out->paths = grown;
+        }
+        char* p = (char*)malloc(strlen(dir) + len + 2);
+        if (!p) { closedir(d); return 1; }
+        sprintf(p, "%s/%s", dir, e->d_name);
+        out->paths[out->n++] = p;
+    }
+    closedir(d);
+    qsort(out->paths, (size_t)out->n, sizeof(char*), by_name);
+    return 0;
+}
+
+/* one KITTI .bin -> channels-first x, y, z rows of stride n_stride; the point count, or -1 */
+static int32_t read_scan(const char* path, float* dst, int n_stride) {
+    FILE* s = fopen(path, "rb");
+    if (!s) return -1;
+    fseek(s, 0, SEEK_END);
+    const long bytes = ftell(s);
+    fseek(s, 0, SEEK_SET);
+    const int32_t n = (int32_t)(bytes / (4 * sizeof(float)));
+    if (n > n_stride) { fclose(s); return -1; }
+    float* rows = (float*)malloc((size_t)n * 4 * sizeof(float) + 1);
+    if (!rows || fread(rows, 4 * sizeof(float), (size_t)n, s) != (size_t)n) { free(rows); fclose(s); return -1; }
+    fclose(s);
+    memset(dst, 0, (size_t)3 * n_stride * sizeof(float));
+    for (int32_t i = 0; i < n; ++i)
+        for (int c = 0; c < 3; ++c) dst[(size_t)c * n_stride + i] = rows[(size_t)i * 4 + c];
+    free(rows);
+    return n;
+}
+
+int main(int argc, char** argv) {
+    if (argc < 3) return fail("usage: odometry_streams model.dlw stream_dir [stream_dir ...]");
+    const int S = argc - 2;
+
+    /* weight file: fixed header, then the fp32 blob; the workspace serves S streams (max_batch = S) */
+    FILE* f = fopen(argv[1], "rb");
+    if (!f) return fail("cannot open the weight file");
+    delora_odometry_file_header hdr;
+    if (fread(&hdr, sizeof hdr, 1, f) != 1) return fail("truncated header");
+    if (memcmp(hdr.magic, DELORA_ODOMETRY_FILE_MAGIC, 8) != 0) return fail("not a .dlw file");
+    if (hdr.abi_version != delora_abi_version()) return fail("weight file and library ABI versions differ");
+    delora_odometry_desc desc = hdr.desc;
+    desc.max_batch = S;
+    const delora_odometry_desc* d = &desc;
+    const int64_t n_weights = delora_odometry_weight_floats(d);
+    if (n_weights < 0) return fail(delora_last_error());
+    if (n_weights != hdr.blob_floats) return fail("blob length does not match the descriptor");
+    float* h_blob = (float*)malloc((size_t)n_weights * sizeof(float));
+    if (!h_blob || fread(h_blob, sizeof(float), (size_t)n_weights, f) != (size_t)n_weights) return fail("truncated blob");
+    fclose(f);
+
+    scan_list* lists = (scan_list*)calloc((size_t)S, sizeof(scan_list));
+    if (!lists) return fail("out of host memory");
+    int ticks = 0;
+    for (int s = 0; s < S; ++s) {
+        if (list_scans(argv[2 + s], &lists[s])) return fail("cannot list a stream directory");
+        if (lists[s].n > ticks) ticks = lists[s].n;
+    }
+
+    cudaStream_t stream;
+    CUDA_OK(cudaStreamCreate(&stream));
+    const size_t pts_floats = (size_t)S * 3 * d->n_stride;
+    float *weights, *points, *T;
+    int32_t *count, *active, *valid;
+    void* workspace;
+    const int64_t ws_bytes = delora_odometry_streams_workspace_bytes(d);
+    if (ws_bytes < 0) return fail(delora_last_error());
+    CUDA_OK(cudaMalloc((void**)&weights, (size_t)n_weights * sizeof(float)));
+    CUDA_OK(cudaMalloc(&workspace, (size_t)ws_bytes));
+    CUDA_OK(cudaMalloc((void**)&points, pts_floats * sizeof(float)));
+    CUDA_OK(cudaMalloc((void**)&count, (size_t)S * sizeof(int32_t)));
+    CUDA_OK(cudaMalloc((void**)&active, (size_t)S * sizeof(int32_t)));
+    CUDA_OK(cudaMalloc((void**)&valid, (size_t)S * sizeof(int32_t)));
+    CUDA_OK(cudaMalloc((void**)&T, (size_t)S * 16 * sizeof(float)));
+    CUDA_OK(cudaMemcpy(weights, h_blob, (size_t)n_weights * sizeof(float), cudaMemcpyHostToDevice));
+    DELORA_OK(delora_odometry_streams_init(d, workspace, stream));
+    DELORA_OK(delora_odometry_streams_load_weights(d, weights, workspace, stream));
+
+    float* h_points = (float*)malloc(pts_floats * sizeof(float));
+    int32_t* h_count = (int32_t*)malloc((size_t)S * sizeof(int32_t));
+    int32_t* h_active = (int32_t*)malloc((size_t)S * sizeof(int32_t));
+    int32_t* h_valid = (int32_t*)malloc((size_t)S * sizeof(int32_t));
+    float* h_T = (float*)malloc((size_t)S * 16 * sizeof(float));
+    if (!h_points || !h_count || !h_active || !h_valid || !h_T) return fail("out of host memory");
+    for (int k = 0; k < ticks; ++k) {
+        for (int s = 0; s < S; ++s) {
+            h_active[s] = k < lists[s].n;
+            h_count[s] = 0;
+            if (!h_active[s]) continue;
+            h_count[s] = read_scan(lists[s].paths[k], h_points + (size_t)s * 3 * d->n_stride, d->n_stride);
+            if (h_count[s] < 0) return fail("cannot read a scan (missing, truncated or more points than n_stride)");
+        }
+        CUDA_OK(cudaMemcpyAsync(points, h_points, pts_floats * sizeof(float), cudaMemcpyHostToDevice, stream));
+        CUDA_OK(cudaMemcpyAsync(count, h_count, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+        CUDA_OK(cudaMemcpyAsync(active, h_active, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+        DELORA_OK(delora_odometry_streams_push(d, points, count, active, workspace, T, valid, stream));
+        CUDA_OK(cudaMemcpyAsync(h_T, T, (size_t)S * 16 * sizeof(float), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaMemcpyAsync(h_valid, valid, (size_t)S * sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+        for (int s = 0; s < S; ++s) {
+            if (!h_valid[s]) continue;
+            printf("%d %d", s, k);
+            for (int i = 0; i < 12; ++i) printf(" %.9g", h_T[(size_t)s * 16 + i]);
+            printf("\n");
+        }
+    }
+    for (int s = 0; s < S; ++s) {
+        for (int i = 0; i < lists[s].n; ++i) free(lists[s].paths[i]);
+        free(lists[s].paths);
+    }
+    free(lists);
+    free(h_T);
+    free(h_valid);
+    free(h_active);
+    free(h_count);
+    free(h_points);
+    free(h_blob);
+    cudaFree(T);
+    cudaFree(valid);
+    cudaFree(active);
+    cudaFree(count);
+    cudaFree(points);
+    cudaFree(workspace);
+    cudaFree(weights);
+    cudaStreamDestroy(stream);
+    return 0;
+}

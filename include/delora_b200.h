@@ -420,6 +420,32 @@ int delora_odometry_pairs(const delora_odometry_desc* d, const float* points, co
 int delora_odometry_push(const delora_odometry_desc* d, const float* points, const int32_t* n_points,
                          void* workspace, float* T, void* stream);
 
+/* Several streams in one workspace: S = d->max_batch independent sensors (or vehicles) that share the descriptor, i.e.
+ * the image geometry and the model.  One call per tick projects the S new frames and runs the model once at batch S.
+ * Each quaternion is divided by the norm of its own row, so row s of T is bit-identical to what a delora_odometry_push
+ * workspace returns when fed only stream s's active frames (after a reset: as if that stream had just started).
+ * The workspace (its own layout, delora_odometry_streams_workspace_bytes) holds each stream's previous frame and whether
+ * it has one; both live on the device.  _streams_push only enqueues work (no allocation, no synchronisation, no host
+ * decision on device data) and its launch sequence depends on neither `active` nor the stream state, so one captured
+ * call can be replayed every tick whatever the activity pattern.  Refused before any launch, with the field or pointer
+ * named: an invalid descriptor, and null points / n_points / workspace / T / valid. */
+int64_t delora_odometry_streams_workspace_bytes(const delora_odometry_desc* d);     /* host only, -1 if invalid */
+/* Zero the workspace (no stream has a previous frame) and arm the projection keys.  Once after allocation. */
+int delora_odometry_streams_init(const delora_odometry_desc* d, void* workspace, void* stream);
+/* The .dlw blob of delora_odometry_load_weights (DEVICE fp32[weight_floats]), same conversion and same rules. */
+int delora_odometry_streams_load_weights(const delora_odometry_desc* d, const float* weights, void* workspace,
+                                         void* stream);
+/* points [S, 3, n_stride], n_points [S] (device, clamped to [0, n_stride] on the device), active [S] int32 (device;
+ * NULL = all active).  For every active stream: project its frame; if the stream has a previous frame, write T[s]
+ * (row-major 4x4, this frame -> previous frame, as _push) and valid[s] = 1; then this frame becomes the stream's
+ * previous frame.  Inactive streams: T row untouched, valid[s] = 0, cached frame untouched.  T [S, 16] fp32 and
+ * valid [S] int32 are device outputs; valid[s] is written for every stream. */
+int delora_odometry_streams_push(const delora_odometry_desc* d, const float* points, const int32_t* n_points,
+                                 const int32_t* active, void* workspace, float* T, int32_t* valid, void* stream);
+/* Forget the previous frame of every stream with mask[s] != 0 (device int32 [S]); the next push of such a stream only
+ * caches its frame.  Refused: an invalid descriptor, null mask / workspace. */
+int delora_odometry_streams_reset(const delora_odometry_desc* d, const int32_t* mask, void* workspace, void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * Odometry training: raw scan pairs -> updated weights, one call per step.
  * Replaces, for the self-supervised step, deploy.deployer.Deployer.step + Trainer's Adam
