@@ -24,6 +24,7 @@ namespace delora {
 
 constexpr int kTailWarps = 8;
 constexpr int kMaxBlocksPerStage = 16;
+constexpr int kMaxBlocks = 4 * kMaxBlocksPerStage;
 constexpr int kMaxConv = 1 + 4 * (2 * kMaxBlocksPerStage) + 3;
 constexpr int kMaxLinear = 5;
 constexpr int kMaxBatch = 1024;
@@ -99,21 +100,30 @@ odometry_linear_kernel(TailLinear p0, TailLinear p1, int B, int act_out, int vec
     }
 }
 
-// Last layer of the heads (rot: 4 outputs, trans: 3), quaternion / ||quaternion block||_F, quaternion -> T.
-// raw [B, 7] or NULL: the head outputs before the normalisation (quaternion, translation), which training keeps.
-__global__ void __launch_bounds__(kTailWarps * 32)
-odometry_out_kernel(TailLinear rot, TailLinear trans, int B, int vec, float* __restrict__ T, float* __restrict__ raw) {
-    extern __shared__ float s_out[];                        // [B, 7]: quaternion (x, y, z, w), translation
-    __shared__ float s_norm;
+// The last layer of the heads (rot: 4 outputs, trans: 3) for every row b < B with want(b) (warp-uniform):
+// s_out[b * 7 + o] = the quaternion (x, y, z, w), then the translation.  One warp per output, row_dot4 with nb = 1.
+template <class Want>
+__device__ __forceinline__ void head_outputs(const TailLinear& rot, const TailLinear& trans, int B, int vec, Want want,
+                                             float* s_out) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int i = warp; i < B * 7; i += kTailWarps) {
         const int b = i / 7, o = i - b * 7;
+        if (!want(b)) continue;
         const TailLinear p = o < 4 ? rot : trans;
         const int n = o < 4 ? o : o - 4;
         float acc[4];
         row_dot4(p.w + (size_t)n * p.K, p.x + (size_t)b * p.ldx, p.ldx, p.K, 1, lane, vec, acc);
         if (lane == 0) s_out[i] = acc[0] + __ldg(p.bias + n);
     }
+}
+
+// Last layer of the heads, quaternion / ||quaternion block||_F, quaternion -> T.
+// raw [B, 7] or NULL: the head outputs before the normalisation (quaternion, translation), which training keeps.
+__global__ void __launch_bounds__(kTailWarps * 32)
+odometry_out_kernel(TailLinear rot, TailLinear trans, int B, int vec, float* __restrict__ T, float* __restrict__ raw) {
+    extern __shared__ float s_out[];                        // [B, 7]: quaternion (x, y, z, w), translation
+    __shared__ float s_norm;
+    head_outputs(rot, trans, B, vec, [](int) { return true; }, s_out);
     __syncthreads();
     if (raw)
         for (int i = threadIdx.x; i < B * 7; i += blockDim.x) raw[i] = s_out[i];
@@ -131,17 +141,22 @@ odometry_out_kernel(TailLinear rot, TailLinear trans, int B, int vec, float* __r
     }
 }
 
-// counts[i] = clamp(n_points[i], 0, n_stride): the projection never reads past a scan's stride
-__global__ void odometry_counts_kernel(const int32_t* __restrict__ n_in, int n, int n_stride, int32_t* __restrict__ n_out) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) n_out[i] = min(max(n_in[i], 0), n_stride);
+__device__ __forceinline__ bool stream_active(const int32_t* __restrict__ active, int s) {
+    return active == nullptr || active[s] != 0;
 }
 
-// ---------------------------------------------------------------- the plan: layer sequence + workspace layout
+// counts[i] = active ? clamp(n_points[i], 0, n_stride) : 0 (active NULL: every scan is): the projection never reads
+// past a scan's stride, and an inactive stream's scatter does no work
+__global__ void odometry_counts_kernel(const int32_t* __restrict__ n_in, const int32_t* __restrict__ active, int n,
+                                       int n_stride, int32_t* __restrict__ n_out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) n_out[i] = stream_active(active, i) ? min(max(n_in[i], 0), n_stride) : 0;
+}
+
+// ---------------------------------------------------------------- the model: layer sequence + weight-blob offsets
 struct ConvLayer {
     int cout, cin, k;
     int64_t blob;          // offset in floats of the fp32 filter in the weight blob
-    size_t ws;             // byte offset of the bf16 w_fwd [cout, k*k, cin_pad] in the workspace
 };
 struct Block {
     int stage, sh, sw, c1, c2, ds;     // conv indices (ds = -1: identity shortcut)
@@ -150,20 +165,16 @@ struct Block {
 struct Linear {
     int K, N;
     int64_t blob_w, blob_b;
-    size_t ws_w, ws_b;
 };
-struct Plan {
-    int H, W, w2, w4, stem_fast, MB;
+struct Model {
+    int H, W, w2, w4, stem_fast;
     int n_conv, n_block, n_lin;
     ConvLayer conv[kMaxConv];
-    Block block[4 * kMaxBlocksPerStage];
+    Block block[kMaxBlocks];
     Linear lin[kMaxLinear];            // two heads: rot1, rot2, trans1, trans2; single MLP: 5 layers
     Linear fc;
     int64_t blob_floats;
     int stage_h[4], stage_w[4], stage_c[4];
-    // byte offsets (has_prev: the streams layout only)
-    size_t keys, index_map, counts, images, prev_image, has_prev, x_in, stem, pool, act[4][3], table, pooled, fc_out, hid[2];
-    size_t w_stem, keys_bytes, total;
 };
 
 static size_t align256(size_t n) { return (n + 255) & ~(size_t)255; }
@@ -194,25 +205,25 @@ static int check_desc(const delora_odometry_desc* d, const char* who) {
 
 // Walks the model in state_dict order (src/models/resnet_modified.py:49-66 + model.py:58-84).  A pure function of the
 // descriptor.
-static void plan_model(const delora_odometry_desc* d, Plan* p) {
-    memset(p, 0, sizeof(Plan));
-    p->H = d->H; p->W = d->W; p->MB = d->max_batch;
-    p->w2 = out_size(d->W, 2); p->w4 = p->w2 / 2;
-    p->stem_fast = d->W % 2 == 0;
+static void plan_model(const delora_odometry_desc* d, Model* m) {
+    memset(m, 0, sizeof(Model));
+    m->H = d->H; m->W = d->W;
+    m->w2 = out_size(d->W, 2); m->w4 = m->w2 / 2;
+    m->stem_fast = d->W % 2 == 0;
     int64_t blob = 0;
     auto add_conv = [&](int cout, int cin, int k) {
-        ConvLayer& c = p->conv[p->n_conv];
+        ConvLayer& c = m->conv[m->n_conv];
         c.cout = cout; c.cin = cin; c.k = k; c.blob = blob;
         blob += (int64_t)cout * cin * k * k;
-        return p->n_conv++;
+        return m->n_conv++;
     };
     add_conv(64, 8, 3);                                     // resnet.conv1
     static const int widths[4] = {64, 128, 256, 512};
     static const int strides_h[4] = {1, 1, 1, 2}, strides_w[4] = {1, 2, 2, 2};
-    int inplanes = 64, h = d->H, w = p->w4;
+    int inplanes = 64, h = d->H, w = m->w4;
     for (int s = 0; s < 4; ++s) {
         for (int bi = 0; bi < d->layers[s]; ++bi) {
-            Block& b = p->block[p->n_block++];
+            Block& b = m->block[m->n_block++];
             b.stage = s;
             b.sh = bi == 0 ? strides_h[s] : 1; b.sw = bi == 0 ? strides_w[s] : 1;
             b.hin = h; b.win = w; b.hout = out_size(h, b.sh); b.wout = out_size(w, b.sw);
@@ -223,127 +234,199 @@ static void plan_model(const delora_odometry_desc* d, Plan* p) {
             b.ds = (bi == 0 && (strided || inplanes != widths[s])) ? add_conv(b.cout, b.cin, 1) : -1;
             inplanes = b.cout; h = b.hout; w = b.wout;
         }
-        p->stage_h[s] = h; p->stage_w[s] = w; p->stage_c[s] = widths[s];
+        m->stage_h[s] = h; m->stage_w[s] = w; m->stage_c[s] = widths[s];
     }
     auto add_lin = [&](Linear& l, int K, int N) {
         l.K = K; l.N = N; l.blob_w = blob; blob += (int64_t)K * N; l.blob_b = blob; blob += N;
     };
     const int nout = d->resnet_outputs;
-    add_lin(p->fc, 512, nout);
+    add_lin(m->fc, 512, nout);
     if (d->single_mlp) {
         static const int dims[6] = {0, 512, 512, 256, 64, 7};
         int k = nout;
-        for (int i = 1; i < 6; ++i) { add_lin(p->lin[p->n_lin++], k, dims[i]); k = dims[i]; }
+        for (int i = 1; i < 6; ++i) { add_lin(m->lin[m->n_lin++], k, dims[i]); k = dims[i]; }
     } else {
-        add_lin(p->lin[0], nout, kHeadHidden); add_lin(p->lin[1], kHeadHidden, 4);     // fully_connected_rotation
-        add_lin(p->lin[2], nout, kHeadHidden); add_lin(p->lin[3], kHeadHidden, 3);     // fully_connected_translation
-        p->n_lin = 4;
+        add_lin(m->lin[0], nout, kHeadHidden); add_lin(m->lin[1], kHeadHidden, 4);     // fully_connected_rotation
+        add_lin(m->lin[2], nout, kHeadHidden); add_lin(m->lin[3], kHeadHidden, 3);     // fully_connected_translation
+        m->n_lin = 4;
     }
-    p->blob_floats = blob;
+    m->blob_floats = blob;
 }
 
-// The part of a workspace after its frame buffers, common to the pairs / push and the streams layouts: the trunk's
-// activations for max_batch images, the tail's, the prep table and the weights.
-static void plan_trunk_tail(const delora_odometry_desc* d, Plan* p, size_t off) {
+// ---------------------------------------------------------------- workspace sections
+// Each workspace kind (pairs / push, streams, training) has a plan: the Model plus the byte offsets of its own
+// layout, built from the sections below.  Every buffer starts on a 256-byte boundary.
+
+// The frame section: n_scans projected scans (depth keys, index map, clamped counts, fp32 images), n_cached cached
+// previous images and, with has_prev, one "has a previous frame" flag per cached image.
+struct Frames {
+    size_t keys, keys_bytes, index_map, counts, images;
+    size_t prev_image;                 // n_cached > 0 only
+    size_t has_prev;                   // with has_prev only
+};
+
+static Frames plan_frames(const delora_odometry_desc* d, int n_scans, int n_cached, bool has_prev, size_t& off) {
+    const size_t HW = (size_t)d->H * d->W;
+    Frames f;
+    memset(&f, 0, sizeof(f));
+    f.keys_bytes = (size_t)n_scans * HW * 8;
+    f.keys = take(off, f.keys_bytes);
+    f.index_map = take(off, (size_t)n_scans * HW * 4);
+    f.counts = take(off, (size_t)n_scans * 4);
+    f.images = take(off, (size_t)n_scans * 4 * HW * 4);
+    if (n_cached > 0) f.prev_image = take(off, (size_t)n_cached * 4 * HW * 4);
+    if (has_prev) f.has_prev = take(off, (size_t)n_cached * 4);
+    return f;
+}
+
+// The weight section: the delora_conv_weight_prep_multi table (one row per filter), each filter's bf16 forward copy
+// w_fwd [cout, k*k, cin_pad] and, when the workspace trains (flip), its flipped copy w_flip for the data gradient
+// (every filter but the stem's).
+struct Weights {
+    bool flip;
+    size_t table, w_fwd[kMaxConv], w_flip[kMaxConv];
+};
+
+static Weights plan_weights(const Model& m, bool flip, size_t& off) {
+    Weights w;
+    memset(&w, 0, sizeof(w));
+    w.flip = flip;
+    w.table = take(off, (size_t)m.n_conv * 8 * 8);
+    for (int i = 0; i < m.n_conv; ++i) {
+        const ConvLayer& c = m.conv[i];
+        if (i == 0) {
+            w.w_fwd[0] = take(off, m.stem_fast ? (size_t)3 * 64 * 64 * 2 : (size_t)64 * 9 * 64 * 2);
+        } else {
+            w.w_fwd[i] = take(off, (size_t)c.cout * c.k * c.k * c.cin * 2);
+            if (flip) w.w_flip[i] = take(off, (size_t)c.cin * c.k * c.k * c.cout * 2);
+        }
+    }
+    return w;
+}
+
+// The bf16 filters of the section from the fp32 blob src: the table rows {fp32 src, w_fwd, w_flip or 0, Cout, Cin, k,
+// Cin_pad, kind}, the stem in the 16-channel layout (kind 1) when W is even, channel-padded to 64 otherwise; then
+// one delora_conv_weight_prep_multi launch.
+static int prep_weights(const Model& m, const Weights& w, char* ws, const float* src, cudaStream_t st, const char* who) {
+    long long table[kMaxConv * 8];
+    for (int i = 0; i < m.n_conv; ++i) {
+        const ConvLayer& c = m.conv[i];
+        long long* r = table + (size_t)i * 8;
+        r[0] = (long long)(uintptr_t)(src + c.blob);
+        r[1] = (long long)(uintptr_t)(ws + w.w_fwd[i]);
+        r[2] = (w.flip && i > 0) ? (long long)(uintptr_t)(ws + w.w_flip[i]) : 0;
+        r[3] = c.cout; r[4] = c.cin; r[5] = c.k;
+        r[6] = (i == 0) ? (m.stem_fast ? 16 : 64) : c.cin;
+        r[7] = (i == 0 && m.stem_fast) ? 1 : 0;
+    }
+    const cudaError_t e = cudaMemcpyAsync(ws + w.table, table, (size_t)m.n_conv * 8 * sizeof(long long),
+                                          cudaMemcpyHostToDevice, st);
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+    return delora_conv_weight_prep_multi(ws + w.table, m.n_conv, st);
+}
+
+// Where the trunk forward reads and writes: its bf16 NHWC input (16 channels when W is even, 64 otherwise), the stem
+// output, the max-pool output (and its argmax when the forward saves its activations), and for every block i its
+// conv1 output t1[i], its downsample output ds[i] (blocks with a downsample) and its output out[i].
+struct Trunk {
+    size_t x_in, stem, pool, idx, t1[kMaxBlocks], ds[kMaxBlocks], out[kMaxBlocks];
+};
+
+// The pairs / push and the streams workspaces.  Inference keeps no activations: each stage owns three buffers, [0]
+// the pool output (stage 0) / the downsample output, [1] conv1 output, [2] block output; later blocks of the stage
+// alternate their output between [0] and [2].  The tail reads fp32 copies of its weights (256-byte aligned).
+struct InferPlan {
+    Model m;
+    Frames f;
+    Trunk t;
+    size_t pooled, fc_out, hid[2];
+    Weights w;
+    size_t fc_w, fc_b, lin_w[kMaxLinear], lin_b[kMaxLinear];
+    size_t total;
+};
+
+// streams: S = max_batch streams, this tick's S frames, each stream's previous frame and whether it has one; the
+// trunk and tail then run at B = S.  Otherwise (pairs / push): 2 * max_batch scans and the one cached image of _push.
+static void make_infer_plan(const delora_odometry_desc* d, bool streams, InferPlan* p) {
+    memset(p, 0, sizeof(InferPlan));
+    plan_model(d, &p->m);
+    const Model& m = p->m;
     const int MB = d->max_batch, nout = d->resnet_outputs;
-    p->x_in = take(off, nhwc_bytes(MB, d->H, d->W, p->stem_fast ? 16 : 64));
-    p->stem = take(off, nhwc_bytes(MB, d->H, p->w2, 64));
-    // stage s buffers: [0] the pool output (stage 0) / the downsample output, [1] conv1 output, [2] block output;
-    // later blocks of the stage alternate their output between [0] and [2]
+    size_t off = 0;
+    p->f = streams ? plan_frames(d, MB, MB, true, off) : plan_frames(d, 2 * MB, 1, false, off);
+    p->t.x_in = take(off, nhwc_bytes(MB, d->H, d->W, m.stem_fast ? 16 : 64));
+    p->t.stem = take(off, nhwc_bytes(MB, d->H, m.w2, 64));
+    size_t act[4][3];
     for (int s = 0; s < 4; ++s)
-        for (int j = 0; j < 3; ++j) p->act[s][j] = take(off, nhwc_bytes(MB, p->stage_h[s], p->stage_w[s], p->stage_c[s]));
-    p->pool = p->act[0][0];
+        for (int j = 0; j < 3; ++j) act[s][j] = take(off, nhwc_bytes(MB, m.stage_h[s], m.stage_w[s], m.stage_c[s]));
+    p->t.pool = act[0][0];
+    size_t cur = p->t.pool;
+    for (int i = 0; i < m.n_block; ++i) {
+        const Block& b = m.block[i];
+        const size_t* r = act[b.stage];
+        p->t.t1[i] = r[1];
+        if (b.ds >= 0) {
+            p->t.ds[i] = r[0];
+            p->t.out[i] = r[2];
+        } else {
+            p->t.out[i] = cur == r[2] ? r[0] : r[2];
+        }
+        cur = p->t.out[i];
+    }
     p->pooled = take(off, (size_t)MB * 512 * 4);
     p->fc_out = take(off, (size_t)MB * nout * 4);
     p->hid[0] = take(off, (size_t)MB * 512 * 4);
     p->hid[1] = take(off, (size_t)MB * 512 * 4);
-    p->table = take(off, (size_t)(kMaxConv + 1) * 8 * 8);
-    p->w_stem = take(off, p->stem_fast ? (size_t)3 * 64 * 64 * 2 : (size_t)64 * 9 * 64 * 2);
-    for (int i = 1; i < p->n_conv; ++i) {
-        ConvLayer& c = p->conv[i];
-        c.ws = take(off, (size_t)c.cout * c.k * c.k * c.cin * 2);
-    }
-    p->conv[0].ws = p->w_stem;
-    p->fc.ws_w = take(off, (size_t)p->fc.K * p->fc.N * 4);
-    p->fc.ws_b = take(off, (size_t)p->fc.N * 4);
-    for (int i = 0; i < p->n_lin; ++i) {
-        p->lin[i].ws_w = take(off, (size_t)p->lin[i].K * p->lin[i].N * 4);
-        p->lin[i].ws_b = take(off, (size_t)p->lin[i].N * 4);
+    p->w = plan_weights(m, false, off);
+    p->fc_w = take(off, (size_t)m.fc.K * m.fc.N * 4);
+    p->fc_b = take(off, (size_t)m.fc.N * 4);
+    for (int i = 0; i < m.n_lin; ++i) {
+        p->lin_w[i] = take(off, (size_t)m.lin[i].K * m.lin[i].N * 4);
+        p->lin_b[i] = take(off, (size_t)m.lin[i].N * 4);
     }
     p->total = off;
 }
 
-// The pairs / push workspace: frame buffers for 2 * max_batch scans and the one cached previous image of _push.
-static void make_plan(const delora_odometry_desc* d, Plan* p) {
-    plan_model(d, p);
-    const int MB = d->max_batch, HW = d->H * d->W;
-    size_t off = 0;
-    p->keys_bytes = (size_t)2 * MB * HW * 8;
-    p->keys = take(off, p->keys_bytes);
-    p->index_map = take(off, (size_t)2 * MB * HW * 4);
-    p->counts = take(off, (size_t)2 * MB * 4);
-    p->images = take(off, (size_t)2 * MB * 4 * HW * 4);
-    p->prev_image = take(off, (size_t)4 * HW * 4);
-    plan_trunk_tail(d, p, off);
+// (img1, img2) fp32 [B, 4, H, W] each -> the trunk input
+static int trunk_input(const Model& m, const Trunk& t, char* ws, const float* img1, const float* img2, int B,
+                       cudaStream_t st) {
+    return m.stem_fast ? delora_images_to_nhwc16_bf16(img1, img2, B, m.H, m.W, ws + t.x_in, st)
+                       : delora_images_to_nhwc_bf16(img1, img2, B, m.H, m.W, 64, ws + t.x_in, st);
 }
 
-// The streams workspace (S = max_batch streams): this tick's S frames, each stream's previous frame and whether it has
-// one; the trunk and tail then run at B = S.
-static void make_streams_plan(const delora_odometry_desc* d, Plan* p) {
-    plan_model(d, p);
-    const int S = d->max_batch, HW = d->H * d->W;
-    size_t off = 0;
-    p->keys_bytes = (size_t)S * HW * 8;
-    p->keys = take(off, p->keys_bytes);
-    p->index_map = take(off, (size_t)S * HW * 4);
-    p->counts = take(off, (size_t)S * 4);
-    p->images = take(off, (size_t)S * 4 * HW * 4);
-    p->prev_image = take(off, (size_t)S * 4 * HW * 4);
-    p->has_prev = take(off, (size_t)S * 4);
-    plan_trunk_tail(d, p, off);
-}
-
-// The trunk from its bf16 NHWC input (x_in, 16 channels when W is even, 64 otherwise) to the pooled features.
-static int run_trunk_from_input(const Plan& p, char* ws, int act, int B, float* pooled, cudaStream_t st) {
+// The trunk from its input to the pooled features.  saving (training): the stem keeps its PRE-activation (fp16 on the
+// 16-channel path) and the max-pool applies the activation and records its argmax; otherwise the stem applies it.
+static int trunk_forward(const Model& m, const Trunk& t, const Weights& w, bool saving, char* ws, int act, int B,
+                         float* pooled, cudaStream_t st) {
     int rc;
-    const int H = p.H, W = p.W;
-    void* x_in = ws + p.x_in;
-    void* stem = ws + p.stem;
-    if (p.stem_fast) {
-        if ((rc = delora_stem_fprop_bf16(x_in, ws + p.w_stem, stem, B, H, W, act, 0, st))) return rc;
-    } else {
-        if ((rc = delora_conv2d_fprop_bf16(x_in, ws + p.w_stem, nullptr, nullptr, stem, B, H, W, 64, 64, 3, 1, 2, act, st)))
-            return rc;
-    }
-    if ((rc = delora_maxpool_w_nhwc_bf16(stem, B, H, p.w2, 64, ws + p.pool, st))) return rc;
-    char* cur = ws + p.pool;
-    for (int i = 0; i < p.n_block; ++i) {
-        const Block& b = p.block[i];
-        char* r[3] = {ws + p.act[b.stage][0], ws + p.act[b.stage][1], ws + p.act[b.stage][2]};
-        char* t1 = r[1];
-        char* ident = cur;
-        char* out = (cur == r[2]) ? r[0] : r[2];
-        if ((rc = delora_conv2d_fprop_bf16(cur, ws + p.conv[b.c1].ws, nullptr, nullptr, t1, B, b.hin, b.win, b.cin, b.cout,
+    const int H = m.H, W = m.W, stem_act = saving ? 0 : act;
+    char* stem = ws + t.stem;
+    if (m.stem_fast)
+        rc = delora_stem_fprop_bf16(ws + t.x_in, ws + w.w_fwd[0], stem, B, H, W, stem_act, saving ? 1 : 0, st);
+    else
+        rc = delora_conv2d_fprop_bf16(ws + t.x_in, ws + w.w_fwd[0], nullptr, nullptr, stem, B, H, W, 64, 64, 3, 1, 2,
+                                      stem_act, st);
+    if (rc) return rc;
+    if (saving) rc = delora_maxpool_w_idx_nhwc_bf16(stem, B, H, m.w2, 64, ws + t.pool, ws + t.idx, act, m.stem_fast, st);
+    else rc = delora_maxpool_w_nhwc_bf16(stem, B, H, m.w2, 64, ws + t.pool, st);
+    if (rc) return rc;
+    const char* cur = ws + t.pool;
+    for (int i = 0; i < m.n_block; ++i) {
+        const Block& b = m.block[i];
+        char* t1 = ws + t.t1[i];
+        const char* ident = cur;
+        if ((rc = delora_conv2d_fprop_bf16(cur, ws + w.w_fwd[b.c1], nullptr, nullptr, t1, B, b.hin, b.win, b.cin, b.cout,
                                            3, b.sh, b.sw, act, st))) return rc;
         if (b.ds >= 0) {
-            ident = r[0];
-            out = r[2];
-            if ((rc = delora_conv2d_fprop_bf16(cur, ws + p.conv[b.ds].ws, nullptr, nullptr, ident, B, b.hin, b.win, b.cin,
-                                               b.cout, 1, b.sh, b.sw, 0, st))) return rc;
+            ident = ws + t.ds[i];
+            if ((rc = delora_conv2d_fprop_bf16(cur, ws + w.w_fwd[b.ds], nullptr, nullptr, ws + t.ds[i], B, b.hin, b.win,
+                                               b.cin, b.cout, 1, b.sh, b.sw, 0, st))) return rc;
         }
-        if ((rc = delora_conv2d_fprop_bf16(t1, ws + p.conv[b.c2].ws, ident, nullptr, out, B, b.hout, b.wout, b.cout, b.cout,
-                                           3, 1, 1, act, st))) return rc;
-        cur = out;
+        if ((rc = delora_conv2d_fprop_bf16(t1, ws + w.w_fwd[b.c2], ident, nullptr, ws + t.out[i], B, b.hout, b.wout,
+                                           b.cout, b.cout, 3, 1, 1, act, st))) return rc;
+        cur = ws + t.out[i];
     }
-    return delora_avgpool_nhwc_bf16(cur, B, p.stage_h[3], p.stage_w[3], 512, pooled, st);
-}
-
-static int run_trunk(const Plan& p, char* ws, int act, const float* img1, const float* img2, int B, float* pooled,
-                     cudaStream_t st) {
-    const int rc = p.stem_fast ? delora_images_to_nhwc16_bf16(img1, img2, B, p.H, p.W, ws + p.x_in, st)
-                               : delora_images_to_nhwc_bf16(img1, img2, B, p.H, p.W, 64, ws + p.x_in, st);
-    if (rc) return rc;
-    return run_trunk_from_input(p, ws, act, B, pooled, st);
+    return delora_avgpool_nhwc_bf16(cur, B, m.stage_h[3], m.stage_w[3], 512, pooled, st);
 }
 
 // Where the tail reads its weights and writes its activations.  Inference: the workspace copies of the weights and two
@@ -367,53 +450,60 @@ static TailLinear tail_args(const Linear& l, const float* w, const float* bias, 
     return t;
 }
 
-static TailIO inference_tail_io(const Plan& p, char* ws) {
+static TailIO inference_tail_io(const InferPlan& p, char* ws) {
     TailIO io;
     memset(&io, 0, sizeof(io));
     auto f = [&](size_t off) { return reinterpret_cast<float*>(ws + off); };
-    io.fc_w = f(p.fc.ws_w); io.fc_b = f(p.fc.ws_b);
-    for (int i = 0; i < p.n_lin; ++i) { io.w[i] = f(p.lin[i].ws_w); io.b[i] = f(p.lin[i].ws_b); }
+    io.fc_w = f(p.fc_w); io.fc_b = f(p.fc_b);
+    for (int i = 0; i < p.m.n_lin; ++i) { io.w[i] = f(p.lin_w[i]); io.b[i] = f(p.lin_b[i]); }
     io.fc_out = f(p.fc_out);
     for (int i = 0; i < kMaxLinear; ++i) io.hid[i] = f(p.hid[i & 1]);
     return io;
 }
 
+// Whether row_dot4 may read t with float4 loads: K and ldx multiples of 4, w and x 16-byte aligned.  The workspace
+// copies of inference are; the master blob of training puts a layer's weights at a float offset that is a multiple of
+// 4 only when resnet_outputs is.
+static int tail_vec(const TailLinear& t) {
+    return t.K % 4 == 0 && t.ldx % 4 == 0 && (uintptr_t)t.w % 16 == 0 && (uintptr_t)t.x % 16 == 0;
+}
+
 // resnet.fc and the heads' hidden layers for B rows; rot / trans: the heads' last layers, for the output kernel
-static int run_tail_hidden(const Plan& p, const TailIO& io, int act, const float* pooled, int B, TailLinear* rot_out,
+static int run_tail_hidden(const Model& m, const TailIO& io, int act, const float* pooled, int B, TailLinear* rot_out,
                            TailLinear* trans_out, cudaStream_t st) {
     float* fc_out = io.fc_out;
     TailLinear none;
     memset(&none, 0, sizeof(none));
     auto linear = [&](const TailLinear& a, const TailLinear& b) {
-        const int vec = (a.K % 4 == 0 && a.ldx % 4 == 0 && (b.N == 0 || (b.K % 4 == 0 && b.ldx % 4 == 0))) ? 1 : 0;
+        const int vec = tail_vec(a) && (b.N == 0 || tail_vec(b));
         const int warps = a.N + b.N;
         odometry_linear_kernel<<<(warps + kTailWarps - 1) / kTailWarps, kTailWarps * 32, 0, st>>>(a, b, B, act, vec);
         DELORA_CHECK_LAUNCH("odometry_linear_kernel");
         return 0;
     };
     int rc;
-    const int nout = p.fc.N;
-    if ((rc = linear(tail_args(p.fc, io.fc_w, io.fc_b, pooled, 512, fc_out, nout), none))) return rc;   // act(resnet.fc(x))
+    const int nout = m.fc.N;
+    if ((rc = linear(tail_args(m.fc, io.fc_w, io.fc_b, pooled, 512, fc_out, nout), none))) return rc;   // act(resnet.fc(x))
     TailLinear rot, trans;
-    if (p.n_lin == 4) {
+    if (m.n_lin == 4) {
         // hidden layers of both heads in one launch: hid[0] = [act(rot1 h) | act(trans1 h)], row stride 200
         const int ld = 2 * kHeadHidden;
         float* hid = io.hid[0];
-        if ((rc = linear(tail_args(p.lin[0], io.w[0], io.b[0], fc_out, nout, hid, ld),
-                         tail_args(p.lin[2], io.w[2], io.b[2], fc_out, nout, hid + kHeadHidden, ld)))) return rc;
-        rot = tail_args(p.lin[1], io.w[1], io.b[1], hid, ld, nullptr, 0);
-        trans = tail_args(p.lin[3], io.w[3], io.b[3], hid + kHeadHidden, ld, nullptr, 0);
+        if ((rc = linear(tail_args(m.lin[0], io.w[0], io.b[0], fc_out, nout, hid, ld),
+                         tail_args(m.lin[2], io.w[2], io.b[2], fc_out, nout, hid + kHeadHidden, ld)))) return rc;
+        rot = tail_args(m.lin[1], io.w[1], io.b[1], hid, ld, nullptr, 0);
+        trans = tail_args(m.lin[3], io.w[3], io.b[3], hid + kHeadHidden, ld, nullptr, 0);
     } else {
         const float* x = fc_out;
         int ldx = nout;
-        for (int i = 0; i < p.n_lin - 1; ++i) {
+        for (int i = 0; i < m.n_lin - 1; ++i) {
             float* y = io.hid[i];
-            if ((rc = linear(tail_args(p.lin[i], io.w[i], io.b[i], x, ldx, y, p.lin[i].N), none))) return rc;
-            x = y; ldx = p.lin[i].N;
+            if ((rc = linear(tail_args(m.lin[i], io.w[i], io.b[i], x, ldx, y, m.lin[i].N), none))) return rc;
+            x = y; ldx = m.lin[i].N;
         }
         // fully_connected_rot_trans's last layer: rows 0..3 -> rotation, rows 4..6 -> translation
-        const int last = p.n_lin - 1;
-        const Linear& l = p.lin[last];
+        const int last = m.n_lin - 1;
+        const Linear& l = m.lin[last];
         rot = tail_args(l, io.w[last], io.b[last], x, ldx, nullptr, 0);
         rot.N = 4;
         trans = rot;
@@ -426,24 +516,59 @@ static int run_tail_hidden(const Plan& p, const TailIO& io, int act, const float
     return 0;
 }
 
-static int run_tail(const Plan& p, const TailIO& io, int act, const float* pooled, int B, float* T, cudaStream_t st) {
+static int run_tail(const Model& m, const TailIO& io, int act, const float* pooled, int B, float* T, cudaStream_t st) {
     TailLinear rot, trans;
-    const int rc = run_tail_hidden(p, io, act, pooled, B, &rot, &trans, st);
+    const int rc = run_tail_hidden(m, io, act, pooled, B, &rot, &trans, st);
     if (rc) return rc;
-    const int vec = (rot.K % 4 == 0 && rot.ldx % 4 == 0) ? 1 : 0;
+    const int vec = tail_vec(rot) && tail_vec(trans);
     odometry_out_kernel<<<1, kTailWarps * 32, (size_t)B * 7 * sizeof(float), st>>>(rot, trans, B, vec, T, io.raw);
     DELORA_CHECK_LAUNCH("odometry_out_kernel");
     return 0;
 }
 
-static int project(const Plan& p, const delora_odometry_desc* d, char* ws, const float* points, const int32_t* n_points,
-                   int n_scans, float* images, cudaStream_t st) {
-    int32_t* counts = reinterpret_cast<int32_t*>(ws + p.counts);
-    odometry_counts_kernel<<<(n_scans + 255) / 256, 256, 0, st>>>(n_points, n_scans, d->n_stride, counts);
+// counts = the clamped n_points of n scans (active: see odometry_counts_kernel)
+static int clamp_counts(const Frames& f, char* ws, const int32_t* n_points, const int32_t* active, int n, int n_stride,
+                        cudaStream_t st) {
+    odometry_counts_kernel<<<(n + 255) / 256, 256, 0, st>>>(n_points, active, n, n_stride,
+                                                            reinterpret_cast<int32_t*>(ws + f.counts));
     DELORA_CHECK_LAUNCH("odometry_counts_kernel");
-    return delora_project_fwd(points, counts, n_scans, 3, d->n_stride, d->H, d->W, d->hfov0, d->hfov1, d->vfov0, d->vfov1,
-                              0, reinterpret_cast<uint64_t*>(ws + p.keys), images,
-                              reinterpret_cast<int32_t*>(ws + p.index_map), st);
+    return 0;
+}
+
+static int project(const Frames& f, const delora_odometry_desc* d, char* ws, const float* points, const int32_t* n_points,
+                   const int32_t* active, int n_scans, cudaStream_t st) {
+    const int rc = clamp_counts(f, ws, n_points, active, n_scans, d->n_stride, st);
+    if (rc) return rc;
+    return delora_project_fwd(points, reinterpret_cast<int32_t*>(ws + f.counts), n_scans, 3, d->n_stride, d->H, d->W,
+                              d->hfov0, d->hfov1, d->vfov0, d->vfov1, 0, reinterpret_cast<uint64_t*>(ws + f.keys),
+                              reinterpret_cast<float*>(ws + f.images), reinterpret_cast<int32_t*>(ws + f.index_map), st);
+}
+
+// Every workspace starts zeroed, with its depth keys at all ones (the projection's empty key)
+static int init_workspace(const Frames& f, size_t total, void* workspace, cudaStream_t st, const char* who) {
+    char* ws = (char*)workspace;
+    cudaError_t e = cudaMemsetAsync(ws, 0, total, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(ws + f.keys, 0xFF, f.keys_bytes, st);
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+    return 0;
+}
+
+static int load_weights(const InferPlan& p, const float* weights, void* workspace, cudaStream_t st, const char* who) {
+    char* ws = (char*)workspace;
+    const Model& m = p.m;
+    int rc = prep_weights(m, p.w, ws, weights, st, who);
+    if (rc) return rc;
+    auto copy = [&](size_t dst, int64_t src, int64_t n) {
+        return cudaMemcpyAsync(ws + dst, weights + src, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, st);
+    };
+    cudaError_t e = copy(p.fc_w, m.fc.blob_w, (int64_t)m.fc.K * m.fc.N);
+    if (e == cudaSuccess) e = copy(p.fc_b, m.fc.blob_b, m.fc.N);
+    for (int i = 0; i < m.n_lin && e == cudaSuccess; ++i) {
+        e = copy(p.lin_w[i], m.lin[i].blob_w, (int64_t)m.lin[i].K * m.lin[i].N);
+        if (e == cudaSuccess) e = copy(p.lin_b[i], m.lin[i].blob_b, m.lin[i].N);
+    }
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+    return 0;
 }
 
 }  // namespace delora
@@ -452,76 +577,32 @@ using namespace delora;
 
 extern "C" int64_t delora_odometry_weight_floats(const delora_odometry_desc* d) {
     if (check_desc(d, "delora_odometry_weight_floats")) return -1;
-    Plan p;
-    make_plan(d, &p);
-    return p.blob_floats;
+    Model m;
+    plan_model(d, &m);
+    return m.blob_floats;
 }
 
 extern "C" int64_t delora_odometry_workspace_bytes(const delora_odometry_desc* d) {
     if (check_desc(d, "delora_odometry_workspace_bytes")) return -1;
-    Plan p;
-    make_plan(d, &p);
+    InferPlan p;
+    make_infer_plan(d, false, &p);
     return (int64_t)p.total;
 }
-
-namespace delora {
-
-static int init_workspace(const Plan& p, void* workspace, cudaStream_t st, const char* who) {
-    char* ws = (char*)workspace;
-    cudaError_t e = cudaMemsetAsync(ws, 0, p.total, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(ws + p.keys, 0xFF, p.keys_bytes, st);
-    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
-    return 0;
-}
-
-static int load_weights(const Plan& p, const float* weights, void* workspace, cudaStream_t st, const char* who) {
-    char* ws = (char*)workspace;
-    // one delora_conv_weight_prep_multi row per filter: {fp32 src, w_fwd, w_flip, Cout, Cin, k, Cin_pad, kind};
-    // the stem in the 16-channel layout (kind 1) when W is even, channel-padded to 64 otherwise
-    long long table[kMaxConv * 8];
-    for (int i = 0; i < p.n_conv; ++i) {
-        const ConvLayer& c = p.conv[i];
-        long long* r = table + (size_t)i * 8;
-        r[0] = (long long)(uintptr_t)(weights + c.blob);
-        r[1] = (long long)(uintptr_t)(ws + c.ws);
-        r[2] = 0;
-        r[3] = c.cout; r[4] = c.cin; r[5] = c.k;
-        r[6] = (i == 0) ? (p.stem_fast ? 16 : 64) : c.cin;
-        r[7] = (i == 0 && p.stem_fast) ? 1 : 0;
-    }
-    cudaError_t e = cudaMemcpyAsync(ws + p.table, table, (size_t)p.n_conv * 8 * sizeof(long long), cudaMemcpyHostToDevice, st);
-    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
-    int rc = delora_conv_weight_prep_multi(ws + p.table, p.n_conv, st);
-    if (rc) return rc;
-    auto copy = [&](size_t dst, int64_t src, int64_t n) {
-        return cudaMemcpyAsync(ws + dst, weights + src, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, st);
-    };
-    e = copy(p.fc.ws_w, p.fc.blob_w, (int64_t)p.fc.K * p.fc.N);
-    if (e == cudaSuccess) e = copy(p.fc.ws_b, p.fc.blob_b, p.fc.N);
-    for (int i = 0; i < p.n_lin && e == cudaSuccess; ++i) {
-        e = copy(p.lin[i].ws_w, p.lin[i].blob_w, (int64_t)p.lin[i].K * p.lin[i].N);
-        if (e == cudaSuccess) e = copy(p.lin[i].ws_b, p.lin[i].blob_b, p.lin[i].N);
-    }
-    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
-    return 0;
-}
-
-}  // namespace delora
 
 extern "C" int delora_odometry_init(const delora_odometry_desc* d, void* workspace, void* stream) {
     if (check_desc(d, "delora_odometry_init")) return 1;
     DELORA_CHECK_ARG(workspace, "delora_odometry_init: null workspace");
-    Plan p;
-    make_plan(d, &p);
-    return init_workspace(p, workspace, (cudaStream_t)stream, "delora_odometry_init");
+    InferPlan p;
+    make_infer_plan(d, false, &p);
+    return init_workspace(p.f, p.total, workspace, (cudaStream_t)stream, "delora_odometry_init");
 }
 
 extern "C" int delora_odometry_load_weights(const delora_odometry_desc* d, const float* weights, void* workspace,
                                             void* stream) {
     if (check_desc(d, "delora_odometry_load_weights")) return 1;
     DELORA_CHECK_ARG(weights && workspace, "delora_odometry_load_weights: null pointer");
-    Plan p;
-    make_plan(d, &p);
+    InferPlan p;
+    make_infer_plan(d, false, &p);
     return load_weights(p, weights, workspace, (cudaStream_t)stream, "delora_odometry_load_weights");
 }
 
@@ -531,17 +612,18 @@ extern "C" int delora_odometry_pairs(const delora_odometry_desc* d, const float*
     DELORA_CHECK_ARG(points && n_points && workspace && T, "delora_odometry_pairs: null pointer");
     DELORA_CHECK_ARG(B >= 1 && B <= d->max_batch, "delora_odometry_pairs: B=%d outside [1, max_batch=%d]", B,
                      d->max_batch);
-    Plan p;
-    make_plan(d, &p);
+    InferPlan p;
+    make_infer_plan(d, false, &p);
     cudaStream_t st = (cudaStream_t)stream;
     char* ws = (char*)workspace;
-    float* images = reinterpret_cast<float*>(ws + p.images);
+    float* images = reinterpret_cast<float*>(ws + p.f.images);
     const size_t img = (size_t)4 * d->H * d->W;
     float* pooled_ws = reinterpret_cast<float*>(ws + p.pooled);
     int rc;
-    if ((rc = project(p, d, ws, points, n_points, 2 * B, images, st))) return rc;
-    if ((rc = run_trunk(p, ws, d->act, images, images + (size_t)B * img, B, pooled_ws, st))) return rc;
-    if ((rc = run_tail(p, inference_tail_io(p, ws), d->act, pooled_ws, B, T, st))) return rc;
+    if ((rc = project(p.f, d, ws, points, n_points, nullptr, 2 * B, st))) return rc;
+    if ((rc = trunk_input(p.m, p.t, ws, images, images + (size_t)B * img, B, st))) return rc;
+    if ((rc = trunk_forward(p.m, p.t, p.w, false, ws, d->act, B, pooled_ws, st))) return rc;
+    if ((rc = run_tail(p.m, inference_tail_io(p, ws), d->act, pooled_ws, B, T, st))) return rc;
     if (pooled) {
         const cudaError_t e = cudaMemcpyAsync(pooled, pooled_ws, (size_t)B * 512 * sizeof(float), cudaMemcpyDeviceToDevice, st);
         DELORA_CHECK_ARG(e == cudaSuccess, "delora_odometry_pairs: %s", cudaGetErrorString(e));
@@ -553,18 +635,19 @@ extern "C" int delora_odometry_push(const delora_odometry_desc* d, const float* 
                                     void* workspace, float* T, void* stream) {
     if (check_desc(d, "delora_odometry_push")) return 1;
     DELORA_CHECK_ARG(points && n_points && workspace, "delora_odometry_push: null pointer");
-    Plan p;
-    make_plan(d, &p);
+    InferPlan p;
+    make_infer_plan(d, false, &p);
     cudaStream_t st = (cudaStream_t)stream;
     char* ws = (char*)workspace;
-    float* image = reinterpret_cast<float*>(ws + p.images);
-    float* prev = reinterpret_cast<float*>(ws + p.prev_image);
+    float* image = reinterpret_cast<float*>(ws + p.f.images);
+    float* prev = reinterpret_cast<float*>(ws + p.f.prev_image);
     int rc;
-    if ((rc = project(p, d, ws, points, n_points, 1, image, st))) return rc;
+    if ((rc = project(p.f, d, ws, points, n_points, nullptr, 1, st))) return rc;
     if (T) {
         float* pooled_ws = reinterpret_cast<float*>(ws + p.pooled);
-        if ((rc = run_trunk(p, ws, d->act, prev, image, 1, pooled_ws, st))) return rc;
-        if ((rc = run_tail(p, inference_tail_io(p, ws), d->act, pooled_ws, 1, T, st))) return rc;
+        if ((rc = trunk_input(p.m, p.t, ws, prev, image, 1, st))) return rc;
+        if ((rc = trunk_forward(p.m, p.t, p.w, false, ws, d->act, 1, pooled_ws, st))) return rc;
+        if ((rc = run_tail(p.m, inference_tail_io(p, ws), d->act, pooled_ws, 1, T, st))) return rc;
     }
     const cudaError_t e = cudaMemcpyAsync(prev, image, (size_t)4 * d->H * d->W * sizeof(float), cudaMemcpyDeviceToDevice, st);
     DELORA_CHECK_ARG(e == cudaSuccess, "delora_odometry_push: %s", cudaGetErrorString(e));
@@ -580,17 +663,6 @@ extern "C" int delora_odometry_push(const delora_odometry_desc* d, const float* 
 // is the block norm of odometry_out_kernel.  Every launch is unconditional; activity and per-stream state are read on
 // the device only.
 namespace delora {
-
-__device__ __forceinline__ bool stream_active(const int32_t* __restrict__ active, int s) {
-    return active == nullptr || active[s] != 0;
-}
-
-// counts[s] = active ? clamp(n_points[s], 0, n_stride) : 0
-__global__ void odometry_streams_counts_kernel(const int32_t* __restrict__ n_in, const int32_t* __restrict__ active,
-                                               int S, int n_stride, int32_t* __restrict__ n_out) {
-    const int s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s < S) n_out[s] = stream_active(active, s) ? min(max(n_in[s], 0), n_stride) : 0;
-}
 
 // (prev [S,4,H,W], cur [S,4,H,W]) fp32 -> the trunk input [S, H+2, W+2, C] bf16 with the bits of images_to_nhwc16_kernel
 // (C = 16) / images_to_nhwc_kernel (C = 64, Cpad 64), and cur -> prev for every active stream.
@@ -655,16 +727,7 @@ __global__ void __launch_bounds__(kTailWarps * 32)
 odometry_streams_out_kernel(TailLinear rot, TailLinear trans, int S, int vec, const int32_t* __restrict__ active,
                             int32_t* __restrict__ has_prev, float* __restrict__ T, int32_t* __restrict__ valid) {
     extern __shared__ float s_out[];                        // [S, 7]: quaternion (x, y, z, w), translation
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    for (int i = warp; i < S * 7; i += kTailWarps) {
-        const int b = i / 7, o = i - b * 7;
-        if (!stream_active(active, b) || has_prev[b] == 0) continue;    // warp-uniform
-        const TailLinear p = o < 4 ? rot : trans;
-        const int n = o < 4 ? o : o - 4;
-        float acc[4];
-        row_dot4(p.w + (size_t)n * p.K, p.x + (size_t)b * p.ldx, p.ldx, p.K, 1, lane, vec, acc);
-        if (lane == 0) s_out[i] = acc[0] + __ldg(p.bias + n);
-    }
+    head_outputs(rot, trans, S, vec, [&](int b) { return stream_active(active, b) && has_prev[b] != 0; }, s_out);
     __syncthreads();
     for (int b = threadIdx.x; b < S; b += blockDim.x) {
         const bool act = stream_active(active, b);
@@ -690,8 +753,8 @@ __global__ void odometry_streams_reset_kernel(const int32_t* __restrict__ mask, 
 
 extern "C" int64_t delora_odometry_streams_workspace_bytes(const delora_odometry_desc* d) {
     if (check_desc(d, "delora_odometry_streams_workspace_bytes")) return -1;
-    Plan p;
-    make_streams_plan(d, &p);
+    InferPlan p;
+    make_infer_plan(d, true, &p);
     return (int64_t)p.total;
 }
 
@@ -699,9 +762,9 @@ extern "C" int delora_odometry_streams_init(const delora_odometry_desc* d, void*
     const char* who = "delora_odometry_streams_init";
     if (check_desc(d, who)) return 1;
     DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
-    Plan p;
-    make_streams_plan(d, &p);
-    return init_workspace(p, workspace, (cudaStream_t)stream, who);
+    InferPlan p;
+    make_infer_plan(d, true, &p);
+    return init_workspace(p.f, p.total, workspace, (cudaStream_t)stream, who);
 }
 
 extern "C" int delora_odometry_streams_load_weights(const delora_odometry_desc* d, const float* weights, void* workspace,
@@ -710,8 +773,8 @@ extern "C" int delora_odometry_streams_load_weights(const delora_odometry_desc* 
     if (check_desc(d, who)) return 1;
     DELORA_CHECK_ARG(weights, "%s: null weights", who);
     DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
-    Plan p;
-    make_streams_plan(d, &p);
+    InferPlan p;
+    make_infer_plan(d, true, &p);
     return load_weights(p, weights, workspace, (cudaStream_t)stream, who);
 }
 
@@ -725,23 +788,18 @@ extern "C" int delora_odometry_streams_push(const delora_odometry_desc* d, const
     DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
     DELORA_CHECK_ARG(T, "%s: null T", who);
     DELORA_CHECK_ARG(valid, "%s: null valid", who);
-    Plan p;
-    make_streams_plan(d, &p);
+    InferPlan p;
+    make_infer_plan(d, true, &p);
     cudaStream_t st = (cudaStream_t)stream;
     char* ws = (char*)workspace;
     const int S = d->max_batch, H = d->H, W = d->W;
-    float* cur = reinterpret_cast<float*>(ws + p.images);
-    float* prev = reinterpret_cast<float*>(ws + p.prev_image);
-    int32_t* counts = reinterpret_cast<int32_t*>(ws + p.counts);
-    int32_t* has_prev = reinterpret_cast<int32_t*>(ws + p.has_prev);
-    odometry_streams_counts_kernel<<<(S + 255) / 256, 256, 0, st>>>(n_points, active, S, d->n_stride, counts);
-    DELORA_CHECK_LAUNCH("odometry_streams_counts_kernel");
+    float* cur = reinterpret_cast<float*>(ws + p.f.images);
+    float* prev = reinterpret_cast<float*>(ws + p.f.prev_image);
+    int32_t* has_prev = reinterpret_cast<int32_t*>(ws + p.f.has_prev);
     int rc;
-    if ((rc = delora_project_fwd(points, counts, S, 3, d->n_stride, H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, 0,
-                                 reinterpret_cast<uint64_t*>(ws + p.keys), cur,
-                                 reinterpret_cast<int32_t*>(ws + p.index_map), st))) return rc;
-    __nv_bfloat16* x_in = reinterpret_cast<__nv_bfloat16*>(ws + p.x_in);
-    if (p.stem_fast) {
+    if ((rc = project(p.f, d, ws, points, n_points, active, S, st))) return rc;
+    __nv_bfloat16* x_in = reinterpret_cast<__nv_bfloat16*>(ws + p.t.x_in);
+    if (p.m.stem_fast) {
         const size_t n = (size_t)S * (H + 2) * W;
         odometry_streams_input_kernel<16><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(cur, prev, active, S, H, W, x_in);
     } else {
@@ -750,10 +808,10 @@ extern "C" int delora_odometry_streams_push(const delora_odometry_desc* d, const
     }
     DELORA_CHECK_LAUNCH("odometry_streams_input_kernel");
     float* pooled = reinterpret_cast<float*>(ws + p.pooled);
-    if ((rc = run_trunk_from_input(p, ws, d->act, S, pooled, st))) return rc;
+    if ((rc = trunk_forward(p.m, p.t, p.w, false, ws, d->act, S, pooled, st))) return rc;
     TailLinear rot, trans;
-    if ((rc = run_tail_hidden(p, inference_tail_io(p, ws), d->act, pooled, S, &rot, &trans, st))) return rc;
-    const int vec = (rot.K % 4 == 0 && rot.ldx % 4 == 0) ? 1 : 0;
+    if ((rc = run_tail_hidden(p.m, inference_tail_io(p, ws), d->act, pooled, S, &rot, &trans, st))) return rc;
+    const int vec = tail_vec(rot) && tail_vec(trans);
     odometry_streams_out_kernel<<<1, kTailWarps * 32, (size_t)S * 7 * sizeof(float), st>>>(rot, trans, S, vec, active,
                                                                                           has_prev, T, valid);
     DELORA_CHECK_LAUNCH("odometry_streams_out_kernel");
@@ -766,11 +824,11 @@ extern "C" int delora_odometry_streams_reset(const delora_odometry_desc* d, cons
     if (check_desc(d, who)) return 1;
     DELORA_CHECK_ARG(mask, "%s: null mask", who);
     DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
-    Plan p;
-    make_streams_plan(d, &p);
+    InferPlan p;
+    make_infer_plan(d, true, &p);
     const int S = d->max_batch;
     odometry_streams_reset_kernel<<<(S + 255) / 256, 256, 0, (cudaStream_t)stream>>>(
-        mask, S, reinterpret_cast<int32_t*>((char*)workspace + p.has_prev));
+        mask, S, reinterpret_cast<int32_t*>((char*)workspace + p.f.has_prev));
     DELORA_CHECK_LAUNCH("odometry_streams_reset_kernel");
     return 0;
 }
@@ -798,7 +856,6 @@ namespace delora {
 constexpr int kBwdThreads = 256;
 constexpr int kDgradCols = 32;         // dx tile: 32 columns (one per lane) x 4 batch rows; the 8 warps split the outputs
 constexpr int kDgradRows = 4;
-constexpr int kMaxBlocks = 4 * kMaxBlocksPerStage;
 
 // torch's activation backward from the stored output y: tanh' = 1 - y^2, relu' = [y > 0] (threshold_backward)
 __device__ __forceinline__ float tail_act_bwd(float g, float y, int act) {
@@ -1002,14 +1059,14 @@ __global__ void odometry_icp_rearm_kernel(float4* __restrict__ s, long long n4, 
 
 // ---------------------------------------------------------------- training plan: workspace layout
 struct TrainPlan {
-    Plan p;
-    size_t master, grad, m, v, ctr, table;
-    size_t w_fwd[kMaxConv], w_flip[kMaxConv];
-    size_t keys, index_map, counts, images, pts_grid, nrm_grid;
-    size_t icp, losses, grad_T, T16, T12;
+    Model m;
+    size_t master, grad, adam_m, adam_v, ctr;
+    Weights w;
+    Frames f;                          // 2 * max_batch scans, no cached image
+    size_t pts_grid, nrm_grid, icp, losses, grad_T, T16, T12;
     // trunk activations kept by the forward: 16- or 64-channel input, stem pre-activation, pool output + argmax,
-    // per block conv1 output and block output, per stage the downsample output
-    size_t x_in, y0, p0, idx, t1[kMaxBlocks], out[kMaxBlocks], ds[4];
+    // per block conv1 output and block output, per downsampling block the downsample output
+    Trunk t;
     // trunk backward: per stage two alternating data-gradient buffers + the conv1 gradient; strided blocks: the
     // downsample's gradient at the output size and (zero-upsample path) the upsampled conv1 gradient
     size_t g[4][3], gds[4], gu1[4], g_stem;
@@ -1017,7 +1074,6 @@ struct TrainPlan {
     // tail activations and gradients
     size_t pooled, fc_out, hid[kMaxLinear], raw, dz_hid[kMaxLinear], dz_fc, g_pooled;
     size_t wg_scratch;
-    int64_t icp_floats, wg_floats;
     size_t total;
 };
 
@@ -1029,75 +1085,61 @@ static bool dgrad_eligible(int cin, int cout, int win, int sw) {
 
 static void make_train_plan(const delora_odometry_desc* d, TrainPlan* tp) {
     memset(tp, 0, sizeof(TrainPlan));
-    make_plan(d, &tp->p);
-    const Plan& p = tp->p;
+    plan_model(d, &tp->m);
+    const Model& m = tp->m;
     const int MB = d->max_batch, H = d->H, W = d->W, HW = H * W, nout = d->resnet_outputs;
     size_t off = 0;
-    auto take = [&](size_t bytes) { const size_t o = off; off += align256(bytes); return o; };
-    const size_t blob = (size_t)p.blob_floats * 4;
-    tp->master = take(blob); tp->grad = take(blob); tp->m = take(blob); tp->v = take(blob);
-    tp->ctr = take(2 * sizeof(long long));
-    tp->table = take((size_t)p.n_conv * 8 * 8);
-    for (int i = 0; i < p.n_conv; ++i) {
-        const ConvLayer& c = p.conv[i];
-        if (i == 0) {
-            tp->w_fwd[0] = take(p.stem_fast ? (size_t)3 * 64 * 64 * 2 : (size_t)64 * 9 * 64 * 2);
-        } else {
-            tp->w_fwd[i] = take((size_t)c.cout * c.k * c.k * c.cin * 2);
-            tp->w_flip[i] = take((size_t)c.cin * c.k * c.k * c.cout * 2);
-        }
-    }
-    tp->keys = take((size_t)2 * MB * HW * 8);
-    tp->index_map = take((size_t)2 * MB * HW * 4);
-    tp->counts = take((size_t)2 * MB * 4);
-    tp->images = take((size_t)2 * MB * 4 * HW * 4);
-    tp->pts_grid = take((size_t)2 * MB * HW * 16);
-    tp->nrm_grid = take((size_t)2 * MB * HW * 16);
-    tp->icp_floats = delora_icp_scratch_floats(MB, HW);
-    tp->icp = take((size_t)tp->icp_floats * 4);
-    tp->losses = take((size_t)MB * DELORA_LOSS_ROW * 4);
-    tp->grad_T = take((size_t)MB * 12 * 4);
-    tp->T16 = take((size_t)MB * 16 * 4);
-    tp->T12 = take((size_t)MB * 12 * 4);
-    tp->x_in = take(nhwc_bytes(MB, H, W, p.stem_fast ? 16 : 64));
-    tp->y0 = take(nhwc_bytes(MB, H, p.w2, 64));
-    tp->p0 = take(nhwc_bytes(MB, H, p.w4, 64));
-    tp->idx = take((size_t)MB * H * p.w4 * 64);
-    for (int i = 0; i < p.n_block; ++i) {
-        const Block& b = p.block[i];
-        tp->t1[i] = take(nhwc_bytes(MB, b.hout, b.wout, b.cout));
-        tp->out[i] = take(nhwc_bytes(MB, b.hout, b.wout, b.cout));
-        if (b.ds >= 0) tp->ds[b.stage] = take(nhwc_bytes(MB, b.hout, b.wout, b.cout));
+    const size_t blob = (size_t)m.blob_floats * 4;
+    tp->master = take(off, blob); tp->grad = take(off, blob); tp->adam_m = take(off, blob); tp->adam_v = take(off, blob);
+    tp->ctr = take(off, 2 * sizeof(long long));
+    tp->w = plan_weights(m, true, off);
+    tp->f = plan_frames(d, 2 * MB, 0, false, off);
+    tp->pts_grid = take(off, (size_t)2 * MB * HW * 16);
+    tp->nrm_grid = take(off, (size_t)2 * MB * HW * 16);
+    tp->icp = take(off, (size_t)delora_icp_scratch_floats(MB, HW) * 4);
+    tp->losses = take(off, (size_t)MB * DELORA_LOSS_ROW * 4);
+    tp->grad_T = take(off, (size_t)MB * 12 * 4);
+    tp->T16 = take(off, (size_t)MB * 16 * 4);
+    tp->T12 = take(off, (size_t)MB * 12 * 4);
+    tp->t.x_in = take(off, nhwc_bytes(MB, H, W, m.stem_fast ? 16 : 64));
+    tp->t.stem = take(off, nhwc_bytes(MB, H, m.w2, 64));
+    tp->t.pool = take(off, nhwc_bytes(MB, H, m.w4, 64));
+    tp->t.idx = take(off, (size_t)MB * H * m.w4 * 64);
+    for (int i = 0; i < m.n_block; ++i) {
+        const Block& b = m.block[i];
+        tp->t.t1[i] = take(off, nhwc_bytes(MB, b.hout, b.wout, b.cout));
+        tp->t.out[i] = take(off, nhwc_bytes(MB, b.hout, b.wout, b.cout));
+        if (b.ds >= 0) tp->t.ds[i] = take(off, nhwc_bytes(MB, b.hout, b.wout, b.cout));
     }
     for (int s = 0; s < 4; ++s)
-        for (int j = 0; j < 3; ++j) tp->g[s][j] = take(nhwc_bytes(MB, p.stage_h[s], p.stage_w[s], p.stage_c[s]));
-    for (int i = 0; i < p.n_block; ++i) {
-        const Block& b = p.block[i];
+        for (int j = 0; j < 3; ++j) tp->g[s][j] = take(off, nhwc_bytes(MB, m.stage_h[s], m.stage_w[s], m.stage_c[s]));
+    for (int i = 0; i < m.n_block; ++i) {
+        const Block& b = m.block[i];
         tp->phase_dgrad[i] = b.ds >= 0 && i > 0 && dgrad_eligible(b.cin, b.cout, b.win, b.sw);
         if (b.ds < 0) continue;
-        tp->gds[b.stage] = take(nhwc_bytes(MB, b.hout, b.wout, b.cin));
-        if (!tp->phase_dgrad[i]) tp->gu1[b.stage] = take(nhwc_bytes(MB, b.hin, b.win, b.cout));
+        tp->gds[b.stage] = take(off, nhwc_bytes(MB, b.hout, b.wout, b.cin));
+        if (!tp->phase_dgrad[i]) tp->gu1[b.stage] = take(off, nhwc_bytes(MB, b.hin, b.win, b.cout));
     }
-    tp->g_stem = take(nhwc_bytes(MB, H, p.w2, 64));
-    tp->pooled = take((size_t)MB * 512 * 4);
-    tp->g_pooled = take((size_t)MB * 512 * 4);
-    tp->fc_out = take((size_t)MB * nout * 4);
-    tp->dz_fc = take((size_t)MB * nout * 4);
-    tp->raw = take((size_t)MB * 7 * 4);
-    if (p.n_lin == 4) {
-        tp->hid[0] = take((size_t)MB * 2 * kHeadHidden * 4);
-        tp->dz_hid[0] = take((size_t)MB * 2 * kHeadHidden * 4);
+    tp->g_stem = take(off, nhwc_bytes(MB, H, m.w2, 64));
+    tp->pooled = take(off, (size_t)MB * 512 * 4);
+    tp->g_pooled = take(off, (size_t)MB * 512 * 4);
+    tp->fc_out = take(off, (size_t)MB * nout * 4);
+    tp->dz_fc = take(off, (size_t)MB * nout * 4);
+    tp->raw = take(off, (size_t)MB * 7 * 4);
+    if (m.n_lin == 4) {
+        tp->hid[0] = take(off, (size_t)MB * 2 * kHeadHidden * 4);
+        tp->dz_hid[0] = take(off, (size_t)MB * 2 * kHeadHidden * 4);
     } else {
-        for (int i = 0; i < p.n_lin - 1; ++i) {
-            tp->hid[i] = take((size_t)MB * p.lin[i].N * 4);
-            tp->dz_hid[i] = take((size_t)MB * p.lin[i].N * 4);
+        for (int i = 0; i < m.n_lin - 1; ++i) {
+            tp->hid[i] = take(off, (size_t)MB * m.lin[i].N * 4);
+            tp->dz_hid[i] = take(off, (size_t)MB * m.lin[i].N * 4);
         }
     }
     // one split-K scratch for every wgrad launch: the largest need at max_batch (the need grows with B)
-    int64_t wg = p.stem_fast ? delora_stem_wgrad_scratch_floats(MB, H, W)
-                             : delora_conv2d_wgrad_scratch_floats(MB, H, p.w2, 64, 64, 3);
-    for (int i = 0; i < p.n_block; ++i) {
-        const Block& b = p.block[i];
+    int64_t wg = m.stem_fast ? delora_stem_wgrad_scratch_floats(MB, H, W)
+                             : delora_conv2d_wgrad_scratch_floats(MB, H, m.w2, 64, 64, 3);
+    for (int i = 0; i < m.n_block; ++i) {
+        const Block& b = m.block[i];
         int64_t n = delora_conv2d_wgrad_scratch_floats(MB, b.hout, b.wout, b.cin, b.cout, 3);
         wg = n > wg ? n : wg;
         n = delora_conv2d_wgrad_scratch_floats(MB, b.hout, b.wout, b.cout, b.cout, 3);
@@ -1107,8 +1149,7 @@ static void make_train_plan(const delora_odometry_desc* d, TrainPlan* tp) {
             wg = n > wg ? n : wg;
         }
     }
-    tp->wg_floats = wg;
-    tp->wg_scratch = take((size_t)wg * 4);
+    tp->wg_scratch = take(off, (size_t)wg * 4);
     tp->total = off;
 }
 
@@ -1129,82 +1170,47 @@ static int check_train_params(const delora_odometry_train_params* hp, const char
     return 0;
 }
 
-static int train_trunk_forward(const TrainPlan& tp, char* ws, int act, const float* img1, const float* img2, int B,
-                               cudaStream_t st) {
-    const Plan& p = tp.p;
-    int rc;
-    const int H = p.H, W = p.W;
-    // the stem keeps its PRE-activation (fp16 on the 16-channel path); the max-pool applies the activation
-    if (p.stem_fast) {
-        if ((rc = delora_images_to_nhwc16_bf16(img1, img2, B, H, W, ws + tp.x_in, st))) return rc;
-        if ((rc = delora_stem_fprop_bf16(ws + tp.x_in, ws + tp.w_fwd[0], ws + tp.y0, B, H, W, 0, 1, st))) return rc;
-    } else {
-        if ((rc = delora_images_to_nhwc_bf16(img1, img2, B, H, W, 64, ws + tp.x_in, st))) return rc;
-        if ((rc = delora_conv2d_fprop_bf16(ws + tp.x_in, ws + tp.w_fwd[0], nullptr, nullptr, ws + tp.y0, B, H, W, 64, 64, 3,
-                                           1, 2, 0, st))) return rc;
-    }
-    if ((rc = delora_maxpool_w_idx_nhwc_bf16(ws + tp.y0, B, H, p.w2, 64, ws + tp.p0, ws + tp.idx, act, p.stem_fast, st)))
-        return rc;
-    const char* cur = ws + tp.p0;
-    for (int i = 0; i < p.n_block; ++i) {
-        const Block& b = p.block[i];
-        char* t1 = ws + tp.t1[i];
-        const char* ident = cur;
-        if ((rc = delora_conv2d_fprop_bf16(cur, ws + tp.w_fwd[b.c1], nullptr, nullptr, t1, B, b.hin, b.win, b.cin, b.cout,
-                                           3, b.sh, b.sw, act, st))) return rc;
-        if (b.ds >= 0) {
-            ident = ws + tp.ds[b.stage];
-            if ((rc = delora_conv2d_fprop_bf16(cur, ws + tp.w_fwd[b.ds], nullptr, nullptr, ws + tp.ds[b.stage], B, b.hin,
-                                               b.win, b.cin, b.cout, 1, b.sh, b.sw, 0, st))) return rc;
-        }
-        if ((rc = delora_conv2d_fprop_bf16(t1, ws + tp.w_fwd[b.c2], ident, nullptr, ws + tp.out[i], B, b.hout, b.wout,
-                                           b.cout, b.cout, 3, 1, 1, act, st))) return rc;
-        cur = ws + tp.out[i];
-    }
-    return delora_avgpool_nhwc_bf16(cur, B, p.stage_h[3], p.stage_w[3], 512, reinterpret_cast<float*>(ws + tp.pooled), st);
-}
-
 static int train_trunk_backward(const TrainPlan& tp, char* ws, int act, int B, cudaStream_t st) {
-    const Plan& p = tp.p;
+    const Model& m = tp.m;
     int rc;
     const int act_bwd = act == 1 ? 4 : 3;                 // ACT_RELU_BWD / ACT_TANH_BWD: multiply by act'(saved)
     float* grad = reinterpret_cast<float*>(ws + tp.grad);
     float* scratch = reinterpret_cast<float*>(ws + tp.wg_scratch);
-    const int L = p.n_block - 1;
+    const int L = m.n_block - 1;
     char* dz2 = ws + tp.g[3][0];
-    if ((rc = delora_avgpool_bwd_nhwc_bf16(reinterpret_cast<const float*>(ws + tp.g_pooled), ws + tp.out[L], B,
-                                           p.stage_h[3], p.stage_w[3], 512, act, dz2, st))) return rc;
+    if ((rc = delora_avgpool_bwd_nhwc_bf16(reinterpret_cast<const float*>(ws + tp.g_pooled), ws + tp.t.out[L], B,
+                                           m.stage_h[3], m.stage_w[3], 512, act, dz2, st))) return rc;
     for (int i = L; i >= 0; --i) {
-        const Block& b = p.block[i];
+        const Block& b = m.block[i];
         const int s = b.stage;
-        const char* x = i == 0 ? ws + tp.p0 : ws + tp.out[i - 1];
+        const char* x = i == 0 ? ws + tp.t.pool : ws + tp.t.out[i - 1];
         char* dz1 = ws + tp.g[s][2];
         // the data gradient of the block input: the other buffer of this stage, or a buffer of the previous stage
         char* next;
-        if (i > 0 && p.block[i - 1].stage != s) next = ws + tp.g[p.block[i - 1].stage][0];
+        if (i > 0 && m.block[i - 1].stage != s) next = ws + tp.g[m.block[i - 1].stage][0];
         else next = (dz2 == ws + tp.g[s][0]) ? ws + tp.g[s][1] : ws + tp.g[s][0];
-        if ((rc = delora_conv2d_wgrad_bf16(ws + tp.t1[i], dz2, grad + p.conv[b.c2].blob, scratch, B, b.hout, b.wout, b.cout,
+        if ((rc = delora_conv2d_wgrad_bf16(ws + tp.t.t1[i], dz2, grad + m.conv[b.c2].blob, scratch, B, b.hout, b.wout, b.cout,
                                            b.cout, b.cout, 3, 1, 1, st))) return rc;
-        if ((rc = delora_conv2d_fprop_bf16(dz2, ws + tp.w_flip[b.c2], nullptr, ws + tp.t1[i], dz1, B, b.hout, b.wout, b.cout,
+        if ((rc = delora_conv2d_fprop_bf16(dz2, ws + tp.w.w_flip[b.c2], nullptr, ws + tp.t.t1[i], dz1, B, b.hout, b.wout, b.cout,
                                            b.cout, 3, 1, 1, act_bwd, st))) return rc;
-        if ((rc = delora_conv2d_wgrad_bf16(x, dz1, grad + p.conv[b.c1].blob, scratch, B, b.hin, b.win, b.cin, b.cin, b.cout,
+        if ((rc = delora_conv2d_wgrad_bf16(x, dz1, grad + m.conv[b.c1].blob, scratch, B, b.hin, b.win, b.cin, b.cin, b.cout,
                                            3, b.sh, b.sw, st))) return rc;
         const char* resid = dz2;
         const char* src = dz1;
         if (b.ds >= 0) {
-            if ((rc = delora_conv2d_wgrad_bf16(x, dz2, grad + p.conv[b.ds].blob, scratch, B, b.hin, b.win, b.cin, b.cin,
+            if ((rc = delora_conv2d_wgrad_bf16(x, dz2, grad + m.conv[b.ds].blob, scratch, B, b.hin, b.win, b.cin, b.cin,
                                                b.cout, 1, b.sh, b.sw, st))) return rc;
             // the 1x1 strided downsample's data gradient: 1x1 convolution of the small dz, scattered afterwards
             char* small = ws + tp.gds[s];
-            if ((rc = delora_conv2d_fprop_bf16(dz2, ws + tp.w_flip[b.ds], nullptr, nullptr, small, B, b.hout, b.wout, b.cout,
+            if ((rc = delora_conv2d_fprop_bf16(dz2, ws + tp.w.w_flip[b.ds], nullptr, nullptr, small, B, b.hout, b.wout, b.cout,
                                                b.cin, 1, 1, 1, 0, st))) return rc;
             if (tp.phase_dgrad[i]) {
-                if ((rc = delora_conv2d_dgrad_bf16(dz1, ws + tp.w_flip[b.c1], small, x, next, B, b.hin, b.win, b.cin, b.cout,
+                if ((rc = delora_conv2d_dgrad_bf16(dz1, ws + tp.w.w_flip[b.c1], small, x, next, B, b.hin, b.win, b.cin, b.cout,
                                                    b.sh, b.sw, act_bwd, 1, st))) return rc;
                 dz2 = next;
                 continue;
             }
-            char* up_resid = ws + tp.g[p.block[i - 1].stage][1];
+            char* up_resid = ws + tp.g[m.block[i - 1].stage][1];
             char* up_src = ws + tp.gu1[s];
             if ((rc = delora_zero_upsample_nhwc_bf16(small, B, b.hout, b.wout, b.cin, b.sh, b.sw, b.hin, b.win, up_resid, st)))
                 return rc;
@@ -1215,26 +1221,26 @@ static int train_trunk_backward(const TrainPlan& tp, char* ws, int act, int B, c
         }
         // i > 0: the block input is the previous block's activation output, act' folds into the epilogue; the first
         // block reads the max-pool output (ACT_NONE: the pool's backward applies the stem's act')
-        if ((rc = delora_conv2d_fprop_bf16(src, ws + tp.w_flip[b.c1], resid, i > 0 ? x : nullptr, next, B, b.hin, b.win,
+        if ((rc = delora_conv2d_fprop_bf16(src, ws + tp.w.w_flip[b.c1], resid, i > 0 ? x : nullptr, next, B, b.hin, b.win,
                                            b.cout, b.cin, 3, 1, 1, i > 0 ? act_bwd : 0, st))) return rc;
         dz2 = next;
     }
-    if ((rc = delora_maxpool_w_bwd_nhwc_bf16(dz2, ws + tp.idx, ws + tp.y0, B, p.H, p.w2, 64, 4 + act, ws + tp.g_stem,
-                                             p.stem_fast, st))) return rc;
-    if (p.stem_fast)
-        return delora_stem_wgrad_bf16(ws + tp.x_in, ws + tp.g_stem, grad, scratch, B, p.H, p.W, 8, st);
-    return delora_conv2d_wgrad_bf16(ws + tp.x_in, ws + tp.g_stem, grad, scratch, B, p.H, p.W, 64, 8, 64, 3, 1, 2, st);
+    if ((rc = delora_maxpool_w_bwd_nhwc_bf16(dz2, ws + tp.t.idx, ws + tp.t.stem, B, m.H, m.w2, 64, 4 + act, ws + tp.g_stem,
+                                             m.stem_fast, st))) return rc;
+    if (m.stem_fast)
+        return delora_stem_wgrad_bf16(ws + tp.t.x_in, ws + tp.g_stem, grad, scratch, B, m.H, m.W, 8, st);
+    return delora_conv2d_wgrad_bf16(ws + tp.t.x_in, ws + tp.g_stem, grad, scratch, B, m.H, m.W, 64, 8, 64, 3, 1, 2, st);
 }
 
 static TailIO train_tail_io(const TrainPlan& tp, char* ws) {
-    const Plan& p = tp.p;
+    const Model& m = tp.m;
     TailIO io;
     memset(&io, 0, sizeof(io));
     const float* master = reinterpret_cast<const float*>(ws + tp.master);
-    io.fc_w = master + p.fc.blob_w; io.fc_b = master + p.fc.blob_b;
-    for (int i = 0; i < p.n_lin; ++i) { io.w[i] = master + p.lin[i].blob_w; io.b[i] = master + p.lin[i].blob_b; }
+    io.fc_w = master + m.fc.blob_w; io.fc_b = master + m.fc.blob_b;
+    for (int i = 0; i < m.n_lin; ++i) { io.w[i] = master + m.lin[i].blob_w; io.b[i] = master + m.lin[i].blob_b; }
     io.fc_out = reinterpret_cast<float*>(ws + tp.fc_out);
-    for (int i = 0; i < p.n_lin - 1; ++i) io.hid[i] = reinterpret_cast<float*>(ws + tp.hid[p.n_lin == 4 ? 0 : i]);
+    for (int i = 0; i < m.n_lin - 1; ++i) io.hid[i] = reinterpret_cast<float*>(ws + tp.hid[m.n_lin == 4 ? 0 : i]);
     io.raw = reinterpret_cast<float*>(ws + tp.raw);
     return io;
 }
@@ -1247,24 +1253,24 @@ static int linear_bwd(const TailGrad& p0, const TailGrad& p1, int B, int act_in,
 }
 
 static int train_tail_backward(const TrainPlan& tp, char* ws, int act, int B, cudaStream_t st) {
-    const Plan& p = tp.p;
+    const Model& m = tp.m;
     auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
     const float* master = f(tp.master);
     float* grad = f(tp.grad);
-    const int nout = p.fc.N;
+    const int nout = m.fc.N;
     OutBwd a;
     memset(&a, 0, sizeof(a));
     a.raw = f(tp.raw); a.grad_T = f(tp.grad_T); a.ctr = reinterpret_cast<long long*>(ws + tp.ctr);
-    if (p.n_lin == 4) {
+    if (m.n_lin == 4) {
         a.K = kHeadHidden; a.ldx = a.ldz = 2 * kHeadHidden; a.single = 0;
-        a.w_rot = master + p.lin[1].blob_w; a.w_trans = master + p.lin[3].blob_w;
+        a.w_rot = master + m.lin[1].blob_w; a.w_trans = master + m.lin[3].blob_w;
         a.x_rot = f(tp.hid[0]); a.x_trans = f(tp.hid[0]) + kHeadHidden;
-        a.gw_rot = grad + p.lin[1].blob_w; a.gb_rot = grad + p.lin[1].blob_b;
-        a.gw_trans = grad + p.lin[3].blob_w; a.gb_trans = grad + p.lin[3].blob_b;
+        a.gw_rot = grad + m.lin[1].blob_w; a.gb_rot = grad + m.lin[1].blob_b;
+        a.gw_trans = grad + m.lin[3].blob_w; a.gb_trans = grad + m.lin[3].blob_b;
         a.dz = f(tp.dz_hid[0]);
     } else {
-        const int last = p.n_lin - 1;
-        const Linear& l = p.lin[last];
+        const int last = m.n_lin - 1;
+        const Linear& l = m.lin[last];
         a.K = l.K; a.ldx = a.ldz = l.K; a.single = 1;
         a.w_rot = master + l.blob_w; a.w_trans = a.w_rot + 4 * (size_t)l.K;
         a.x_rot = a.x_trans = f(tp.hid[last - 1]);
@@ -1285,42 +1291,22 @@ static int train_tail_backward(const TrainPlan& tp, char* ws, int act, int B, cu
     int rc;
     float* fc_out = f(tp.fc_out);
     float* dz_fc = f(tp.dz_fc);
-    if (p.n_lin == 4) {
+    if (m.n_lin == 4) {
         // the heads' hidden layers read the same fc output: dx = rot1^T dz_rot + trans1^T dz_trans, then act'(fc_out)
         const int ld = 2 * kHeadHidden;
-        if ((rc = linear_bwd(tg(p.lin[0], fc_out, nout, f(tp.dz_hid[0]), ld),
-                             tg(p.lin[2], fc_out, nout, f(tp.dz_hid[0]) + kHeadHidden, ld), B, act, dz_fc, nout, st)))
+        if ((rc = linear_bwd(tg(m.lin[0], fc_out, nout, f(tp.dz_hid[0]), ld),
+                             tg(m.lin[2], fc_out, nout, f(tp.dz_hid[0]) + kHeadHidden, ld), B, act, dz_fc, nout, st)))
             return rc;
     } else {
-        for (int i = p.n_lin - 2; i >= 0; --i) {
+        for (int i = m.n_lin - 2; i >= 0; --i) {
             const float* x = i == 0 ? fc_out : f(tp.hid[i - 1]);
-            const int ldx = i == 0 ? nout : p.lin[i - 1].N;
+            const int ldx = i == 0 ? nout : m.lin[i - 1].N;
             float* dx = i == 0 ? dz_fc : f(tp.dz_hid[i - 1]);
-            if ((rc = linear_bwd(tg(p.lin[i], x, ldx, f(tp.dz_hid[i]), p.lin[i].N), none, B, act, dx, ldx, st))) return rc;
+            if ((rc = linear_bwd(tg(m.lin[i], x, ldx, f(tp.dz_hid[i]), m.lin[i].N), none, B, act, dx, ldx, st))) return rc;
         }
     }
     // resnet.fc: its input is the pooled trunk output; the last block's act' is applied by the average pool's backward
-    return linear_bwd(tg(p.fc, f(tp.pooled), 512, dz_fc, nout), none, B, 0, f(tp.g_pooled), 512, st);
-}
-
-static int write_prep_table(const TrainPlan& tp, char* ws, cudaStream_t st, const char* who) {
-    const Plan& p = tp.p;
-    long long table[kMaxConv * 8];
-    const float* master = reinterpret_cast<const float*>(ws + tp.master);
-    for (int i = 0; i < p.n_conv; ++i) {
-        const ConvLayer& c = p.conv[i];
-        long long* r = table + (size_t)i * 8;
-        r[0] = (long long)(uintptr_t)(master + c.blob);
-        r[1] = (long long)(uintptr_t)(ws + tp.w_fwd[i]);
-        r[2] = i == 0 ? 0 : (long long)(uintptr_t)(ws + tp.w_flip[i]);
-        r[3] = c.cout; r[4] = c.cin; r[5] = c.k;
-        r[6] = (i == 0) ? (p.stem_fast ? 16 : 64) : c.cin;
-        r[7] = (i == 0 && p.stem_fast) ? 1 : 0;
-    }
-    const cudaError_t e = cudaMemcpyAsync(ws + tp.table, table, (size_t)p.n_conv * 8 * sizeof(long long),
-                                          cudaMemcpyHostToDevice, st);
-    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
-    return 0;
+    return linear_bwd(tg(m.fc, f(tp.pooled), 512, dz_fc, nout), none, B, 0, f(tp.g_pooled), 512, st);
 }
 
 }  // namespace delora
@@ -1341,14 +1327,12 @@ extern "C" int delora_odometry_train_init(const delora_odometry_desc* d, const f
     make_train_plan(d, &tp);
     cudaStream_t st = (cudaStream_t)stream;
     char* ws = (char*)workspace;
-    cudaError_t e = cudaMemsetAsync(ws, 0, tp.total, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(ws + tp.keys, 0xFF, (size_t)2 * d->max_batch * d->H * d->W * 8, st);
-    if (e == cudaSuccess)
-        e = cudaMemcpyAsync(ws + tp.master, weights, (size_t)tp.p.blob_floats * 4, cudaMemcpyDeviceToDevice, st);
-    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
-    int rc = write_prep_table(tp, ws, st, who);
+    int rc = init_workspace(tp.f, tp.total, ws, st, who);
     if (rc) return rc;
-    return delora_conv_weight_prep_multi(ws + tp.table, tp.p.n_conv, st);
+    const cudaError_t e = cudaMemcpyAsync(ws + tp.master, weights, (size_t)tp.m.blob_floats * 4, cudaMemcpyDeviceToDevice,
+                                          st);
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+    return prep_weights(tp.m, tp.w, ws, reinterpret_cast<const float*>(ws + tp.master), st, who);
 }
 
 extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
@@ -1361,7 +1345,7 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
     DELORA_CHECK_ARG(B >= 1 && B <= d->max_batch, "%s: B=%d outside [1, max_batch=%d]", who, B, d->max_batch);
     TrainPlan tp;
     make_train_plan(d, &tp);
-    const Plan& p = tp.p;
+    const Model& m = tp.m;
     cudaStream_t st = (cudaStream_t)stream;
     char* ws = (char*)workspace;
     auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
@@ -1371,20 +1355,20 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
     cudaError_t e = cudaSuccess;
 
     // 1. projection + normals of the 2B scans (scan_1 x B, then scan_2 x B)
-    int32_t* counts = reinterpret_cast<int32_t*>(ws + tp.counts);
-    odometry_counts_kernel<<<(2 * B + 255) / 256, 256, 0, st>>>(n_points, 2 * B, d->n_stride, counts);
-    DELORA_CHECK_LAUNCH("odometry_counts_kernel");
+    if ((rc = clamp_counts(tp.f, ws, n_points, nullptr, 2 * B, d->n_stride, st))) return rc;
+    int32_t* counts = reinterpret_cast<int32_t*>(ws + tp.f.counts);
     delora_f4* pts_grid = reinterpret_cast<delora_f4*>(ws + tp.pts_grid);
     delora_f4* nrm_grid = reinterpret_cast<delora_f4*>(ws + tp.nrm_grid);
-    float* images = f(tp.images);
+    float* images = f(tp.f.images);
     if ((rc = delora_project_normals_fwd(points, counts, 2 * B, 3, d->n_stride, H, W, d->hfov0, d->hfov1, d->vfov0,
-                                         d->vfov1, 0, reinterpret_cast<uint64_t*>(ws + tp.keys), images,
-                                         reinterpret_cast<int32_t*>(ws + tp.index_map), hp->nb_h, hp->nb_w,
+                                         d->vfov1, 0, reinterpret_cast<uint64_t*>(ws + tp.f.keys), images,
+                                         reinterpret_cast<int32_t*>(ws + tp.f.index_map), hp->nb_h, hp->nb_w,
                                          hp->epsilon_range, hp->min_neighbors, pts_grid, nrm_grid, nullptr, st)))
         return rc;
     // 2. forward, keeping the activations
-    if ((rc = train_trunk_forward(tp, ws, d->act, images, images + (size_t)B * 4 * HW, B, st))) return rc;
-    if ((rc = run_tail(p, train_tail_io(tp, ws), d->act, f(tp.pooled), B, f(tp.T16), st))) return rc;
+    if ((rc = trunk_input(m, tp.t, ws, images, images + (size_t)B * 4 * HW, B, st))) return rc;
+    if ((rc = trunk_forward(m, tp.t, tp.w, true, ws, d->act, B, f(tp.pooled), st))) return rc;
+    if ((rc = run_tail(m, train_tail_io(tp, ws), d->act, f(tp.pooled), B, f(tp.T16), st))) return rc;
     // 3. ICP losses and dL/dT: source = scan_2 moved by T, target = scan_1
     e = cudaMemcpy2DAsync(f(tp.T12), 12 * sizeof(float), f(tp.T16), 16 * sizeof(float), 12 * sizeof(float), B,
                           cudaMemcpyDeviceToDevice, st);
@@ -1405,16 +1389,16 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
     out(losses, tp.losses, (size_t)B * DELORA_LOSS_ROW);
     out(T, tp.T16, (size_t)B * 16);
     out(pooled, tp.pooled, (size_t)B * 512);
-    out(grads, tp.grad, (size_t)p.blob_floats);
+    out(grads, tp.grad, (size_t)m.blob_floats);
     DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
     // 5. Adam on the master blob, then the bf16 filters from the updated weights
-    const long long n = p.blob_floats;
+    const long long n = m.blob_floats;
     const long long blocks = (n / 4 + 255) / 256;
     const int grid = (int)(blocks < 8ll * num_sms() ? (blocks > 0 ? blocks : 1) : 8ll * num_sms());
-    odometry_adam_kernel<<<grid, 256, 0, st>>>(f(tp.master), f(tp.grad), f(tp.m), f(tp.v), n, ctr, hp->lr, hp->beta1,
+    odometry_adam_kernel<<<grid, 256, 0, st>>>(f(tp.master), f(tp.grad), f(tp.adam_m), f(tp.adam_v), n, ctr, hp->lr, hp->beta1,
                                                hp->beta2, hp->eps);
     DELORA_CHECK_LAUNCH("odometry_adam_kernel");
-    return delora_conv_weight_prep_multi(ws + tp.table, p.n_conv, st);
+    return delora_conv_weight_prep_multi(ws + tp.w.table, m.n_conv, st);
 }
 
 extern "C" int delora_odometry_train_weights(const delora_odometry_desc* d, const void* workspace, float* weights,
@@ -1424,7 +1408,7 @@ extern "C" int delora_odometry_train_weights(const delora_odometry_desc* d, cons
     DELORA_CHECK_ARG(workspace && weights, "%s: null pointer", who);
     TrainPlan tp;
     make_train_plan(d, &tp);
-    const cudaError_t e = cudaMemcpyAsync(weights, (const char*)workspace + tp.master, (size_t)tp.p.blob_floats * 4,
+    const cudaError_t e = cudaMemcpyAsync(weights, (const char*)workspace + tp.master, (size_t)tp.m.blob_floats * 4,
                                           cudaMemcpyDeviceToDevice, (cudaStream_t)stream);
     DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
     return 0;

@@ -118,12 +118,16 @@ def _close(t, ref, tol=1e-5):
 
 
 SIZES = [(64, 2048, 2048), (64, 720, 1024), (64, 512, 1024), (16, 720, 1024)]   # H, W, w_raw
+VARIANTS = [("tanh", False), ("relu", False), ("tanh", True), ("relu", True)]
+# resnet_outputs = 1002: the heads' first layers have K = 1002, which the tail reads without float4 loads
+PAIRS_CASES = ([pytest.param(act, single, *size, 1000, id="-".join(map(str, (act, single) + size)))
+                for act, single in VARIANTS for size in SIZES] +
+               [pytest.param("tanh", False, 16, 720, 1024, 1002, id="tanh-False-16-720-1024-nout1002")])
 
 
-@pytest.mark.parametrize("h,w,w_raw", SIZES)
-@pytest.mark.parametrize("act,single", [("tanh", False), ("relu", False), ("tanh", True), ("relu", True)])
-def test_pairs_match_the_python_path(cuda_lib, h, w, w_raw, act, single):
-    cfg = _config(h, w, act, single)
+@pytest.mark.parametrize("act,single,h,w,w_raw,nout", PAIRS_CASES)
+def test_pairs_match_the_python_path(cuda_lib, h, w, w_raw, act, single, nout):
+    cfg = _config(h, w, act, single, nout=nout)
     model = _model(cfg)
     frames = _frames(h, w_raw, 8)
     n_stride = max(s.shape[1] for s in frames)

@@ -177,12 +177,17 @@ def _rel(a, b):
 
 SIZES = [(64, 2048, 2048, 4), (64, 720, 1024, 2), (16, 720, 1024, 2), (16, 259, 512, 2)]     # H, W, w_raw, B
 VARIANTS = [("tanh", False), ("relu", False), ("tanh", True), ("relu", True)]
+# resnet_outputs = 1002: every head layer starts at a float offset = 2 (mod 4) in the master blob the tail reads, so
+# the tail must not read it with float4 loads
+STEP_CASES = ([pytest.param(act, single, *size, 1000, id="-".join(map(str, (act, single) + size)))
+               for act, single in VARIANTS for size in SIZES] +
+              [pytest.param("tanh", single, 16, 259, 512, 2, 1002, id=f"tanh-{single}-16-259-512-2-nout1002")
+               for single in (False, True)])
 
 
-@pytest.mark.parametrize("h,w,w_raw,b", SIZES)
-@pytest.mark.parametrize("act,single", VARIANTS)
-def test_step_matches_the_python_training_step(cuda_lib, h, w, w_raw, b, act, single):
-    cfg = _config(h, w, act, single)
+@pytest.mark.parametrize("act,single,h,w,w_raw,b,nout", STEP_CASES)
+def test_step_matches_the_python_training_step(cuda_lib, h, w, w_raw, b, act, single, nout):
+    cfg = _config(h, w, act, single, nout=nout)
     model = _model(cfg)
     pairs = _pairs(h, w_raw, b)
     n_stride = _n_stride(pairs)
@@ -197,7 +202,7 @@ def test_step_matches_the_python_training_step(cuda_lib, h, w, w_raw, b, act, si
     l_err = _rel(losses[:, :3], py_losses[:, :3])
     assert l_err <= 1e-5, f"losses differ by {l_err:.3e} (relative)"
     tail, trunk = _grad_spread(_grad_dict(grads, cfg), py_grads)
-    print(f"\n[{h}x{w} B={b} {act} single={single}] T {t_err:.2e}  losses {l_err:.2e}  grads: tail {tail:.2e}, "
+    print(f"\n[{h}x{w} B={b} {act} single={single} nout={nout}] T {t_err:.2e}  losses {l_err:.2e}  grads: tail {tail:.2e}, "
           f"trunk {trunk:.2e}")
     assert tail <= TAIL_TOL, f"fc / head gradients differ by {tail:.3e} of their max-abs"
     assert trunk <= TRUNK_TOL, f"trunk gradients differ by {trunk:.3e} of their max-abs"
