@@ -64,6 +64,7 @@ SIGNATURES = {
                                        c_void_p, c_void_p]),
     "delora_conv2d_fprop_bf16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                          c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "delora_conv2d_dgrad_eligible": (c_int, [c_int, c_int, c_int, c_int, c_int]),
     "delora_conv2d_dgrad_bf16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                          c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "delora_conv2d_wgrad_scratch_floats": (c_i64, [c_int, c_int, c_int, c_int, c_int, c_int]),

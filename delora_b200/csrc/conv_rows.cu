@@ -24,7 +24,7 @@
 // Warp roles: 0..7 MMA + epilogue (two warpgroups), 8 halo-tile producer, 9 filter producer.
 #include <string.h>
 #include <stdlib.h>
-#include "tc_common.cuh"
+#include "conv_internal.cuh"
 
 namespace delora {
 
@@ -253,59 +253,6 @@ conv_rows_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
 }
 
 // ---------------------------------------------------------------- host side
-static int rows_encode_maps(CUtensorMap* mx, CUtensorMap* mw, const void* x, const void* w, int B, int Hin, int Win,
-                            int Cin, int Cout, int wtaps, int NS, int R, int w_rows) {
-    PFN_cuTensorMapEncodeTiled_v12000 encode = get_tensor_map_encoder();
-    if (!encode) return 1;
-    const int Hp = Hin + 2, Wp = Win + 2;
-    {
-        cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)Wp, (cuuint64_t)Hp, (cuuint64_t)B};
-        cuuint64_t strides[3] = {(cuuint64_t)Cin * 2, (cuuint64_t)Wp * Cin * 2, (cuuint64_t)Hp * Wp * Cin * 2};
-        cuuint32_t box[4] = {64, (cuuint32_t)(NS + 2), (cuuint32_t)(R + 2), 1};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        if (encode(mx, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return 2;
-    }
-    {
-        cuuint64_t dims[2] = {(cuuint64_t)wtaps * Cin, (cuuint64_t)Cout};
-        cuuint64_t strides[1] = {(cuuint64_t)wtaps * Cin * 2};
-        cuuint32_t box[2] = {64, (cuuint32_t)w_rows};
-        cuuint32_t estr[2] = {1, 1};
-        if (encode(mw, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(w), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return 3;
-    }
-    return 0;
-}
-
-// Tensor maps depend only on (pointers, shapes); the encoder's activations, filters and gradients live in
-// persistent buffers, so a small per-thread cache removes the encode cost from the 40 launches of a step.
-struct RowsMapKey { const void* x; const void* w; int B, Hin, Win, Cin, Cout, wtaps, NS, R, w_rows; };
-struct RowsMapEntry { RowsMapKey k; CUtensorMap mx, mw; };
-
-static const RowsMapEntry* rows_get_maps(const RowsMapKey& key) {
-    static thread_local RowsMapEntry cache[128];
-    static thread_local int used = 0, next = 0;
-    for (int i = 0; i < used; ++i) {
-        const RowsMapKey& c = cache[i].k;
-        if (c.x == key.x && c.w == key.w && c.B == key.B && c.Hin == key.Hin && c.Win == key.Win && c.Cin == key.Cin &&
-            c.Cout == key.Cout && c.wtaps == key.wtaps && c.NS == key.NS && c.R == key.R && c.w_rows == key.w_rows)
-            return &cache[i];
-    }
-    RowsMapEntry& e = cache[next];
-    if (rows_encode_maps(&e.mx, &e.mw, key.x, key.w, key.B, key.Hin, key.Win, key.Cin, key.Cout, key.wtaps, key.NS,
-                         key.R, key.w_rows) != 0)
-        return nullptr;
-    e.k = key;
-    const RowsMapEntry* out = &e;
-    next = (next + 1) % 128;
-    if (used < 128) ++used;
-    return out;
-}
-
 // segment width for a job grid Hg x Wg: NS = multiple of 16 covering the row in equal segments of at most 128 pixels
 static int rows_pick_ns(int Wg) {
     const int segs = (Wg + 127) / 128;
@@ -399,28 +346,21 @@ int conv_rows_launch(const void* x, const void* w, const void* residual, const v
     if (ws > 8) ws = 8;
     DELORA_CHECK_ARG(ws >= 2, "conv_rows: tile %dx%d leaves no room for the filter ring", p.NS, p.R);
     p.w_stages = ws;
-    const RowsMapKey key = {x, w, B, Hin, Win, Cin, Cout, ksize * ksize, p.NS, p.R, p.w_tile_bytes / 128};
-    const RowsMapEntry* maps = rows_get_maps(key);
-    DELORA_CHECK_ARG(maps != nullptr, "conv_rows: cuTensorMapEncodeTiled failed or is unavailable");
+    CUtensorMap mx, mw;
+    int rc = tma_nhwc(&mx, x, B, Hin, Win, Cin, p.NS + 2, p.R + 2, 1, 1, false);
+    if (rc == 0) rc = tma_filter(&mw, w, ksize * ksize * Cin, Cout, p.w_tile_bytes / 128, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+    DELORA_CHECK_ARG(rc == 0, "conv_rows: cuTensorMapEncodeTiled failed or is unavailable: %d", rc);
     const size_t smem = (size_t)fixed + (size_t)ws * p.w_tile_bytes;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    static bool attr_set[64] = {};
-    if (dev < 64 && !attr_set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(conv_rows_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e == cudaSuccess)
-            e = cudaFuncSetAttribute(conv_rows_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        DELORA_CHECK_ARG(e == cudaSuccess, "conv_rows: shared-memory opt-in failed: %s", cudaGetErrorString(e));
-        attr_set[dev] = true;
-    }
+    const cudaError_t e = pixm ? smem_opt_in<conv_rows_tc_kernel<true>>() : smem_opt_in<conv_rows_tc_kernel<false>>();
+    DELORA_CHECK_ARG(e == cudaSuccess, "conv_rows: shared-memory opt-in failed: %s", cudaGetErrorString(e));
     const int grid = p.n_jobs < num_sms() ? p.n_jobs : num_sms();
     const __nv_bfloat16* res_p = (const __nv_bfloat16*)residual;
     const __nv_bfloat16* sav_p = (const __nv_bfloat16*)saved;
     __nv_bfloat16* y_p = (__nv_bfloat16*)y;
     if (pixm)
-        conv_rows_tc_kernel<true><<<grid, kRowsThreads, smem, stream>>>(maps->mx, maps->mw, res_p, sav_p, y_p, p);
+        conv_rows_tc_kernel<true><<<grid, kRowsThreads, smem, stream>>>(mx, mw, res_p, sav_p, y_p, p);
     else
-        conv_rows_tc_kernel<false><<<grid, kRowsThreads, smem, stream>>>(maps->mx, maps->mw, res_p, sav_p, y_p, p);
+        conv_rows_tc_kernel<false><<<grid, kRowsThreads, smem, stream>>>(mx, mw, res_p, sav_p, y_p, p);
     cudaError_t le = cudaGetLastError();
     DELORA_CHECK_ARG(le == cudaSuccess, "conv_rows: launch failed: %s", cudaGetErrorString(le));
     DELORA_CHECK_LAUNCH("conv_rows_tc_kernel");
@@ -431,18 +371,21 @@ int conv_rows_launch(const void* x, const void* w, const void* residual, const v
 
 using namespace delora;
 
+extern "C" int delora_conv2d_dgrad_eligible(int Cin, int Cout, int Win, int stride_h, int stride_w) {
+    if (!(stride_h == 1 || stride_h == 2) || !(stride_w == 1 || stride_w == 2) || Win < 1) return 0;
+    if (stride_w == 2 && Win % 2 != 0) return 0;     // an odd circular width mixes the phases at the seam
+    return conv_rows_eligible(Cout, Cin, 3, (Win + stride_w - 1) / stride_w) ? 1 : 0;
+}
+
 extern "C" int delora_conv2d_dgrad_bf16(const void* dz, const void* w_flip, const void* residual, const void* saved,
                                         void* dx, int B, int Hin, int Win, int Cin, int Cout, int stride_h, int stride_w,
                                         int act, int residual_strided, void* stream) {
     // Cin / Cout are those of the FORWARD convolution: dz has Cout channels, dx has Cin channels
     DELORA_CHECK_ARG(dz && w_flip && dx, "delora_conv2d_dgrad_bf16: null pointer");
     DELORA_CHECK_ARG(act >= 0 && act <= 4 && (act < 3 || saved), "delora_conv2d_dgrad_bf16: act=%d (3/4 need `saved`)", act);
-    DELORA_CHECK_ARG((stride_h == 1 || stride_h == 2) && (stride_w == 1 || stride_w == 2) && Hin >= 1 && Win >= 1,
-                     "delora_conv2d_dgrad_bf16: stride (%d,%d) unsupported", stride_h, stride_w);
-    DELORA_CHECK_ARG(stride_w == 1 || Win % 2 == 0, "delora_conv2d_dgrad_bf16: stride_w = 2 needs an even Win (got %d)", Win);
-    DELORA_CHECK_ARG(conv_rows_eligible(Cout, Cin, 3, (Win + stride_w - 1) / stride_w),
-                     "delora_conv2d_dgrad_bf16: needs Cout %% 64 == 0 and Cin %% 128 == 0 (or Cin = 64 / 128 with at least "
-                     "128 columns per phase); got Cin=%d, Cout=%d, Win=%d", Cin, Cout, Win);
+    DELORA_CHECK_ARG(Hin >= 1 && delora_conv2d_dgrad_eligible(Cin, Cout, Win, stride_h, stride_w),
+                     "delora_conv2d_dgrad_bf16: layer not supported (see delora_conv2d_dgrad_eligible): Cin=%d, Cout=%d, "
+                     "Hin=%d, Win=%d, stride (%d,%d)", Cin, Cout, Hin, Win, stride_h, stride_w);
     return conv_rows_launch(dz, w_flip, residual, saved, dx, B, Hin, Win, Cout, Cin, 3, stride_h, stride_w, act,
                             (cudaStream_t)stream, residual_strided);
 }

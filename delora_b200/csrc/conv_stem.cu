@@ -18,7 +18,7 @@
 //   wgrad:  the plan-driven kernel of conv_wgrad.cu (mode 2) on the same tensor map.
 #include <string.h>
 #include <cuda_fp16.h>
-#include "tc_common.cuh"
+#include "conv_internal.cuh"
 
 namespace delora {
 
@@ -249,22 +249,14 @@ weight_prep_multi_kernel(const long long* __restrict__ table) {
 }
 
 // the overlapping-stride view of the 16-channel input: (k, wo, hp, b) -> x16[b][hp][2 wo + k / 16][k % 16]
-int stem_encode_x_map(CUtensorMap* m, const void* x16, int B, int H, int W, int box_w) {
-    PFN_cuTensorMapEncodeTiled_v12000 encode = get_tensor_map_encoder();
-    if (!encode) return 1;
+static int stem_encode_x_map(CUtensorMap* m, const void* x16, int B, int H, int W) {
     const int Hp = H + 2, Wp = W + 2, Wout = W / 2;
-    cuuint64_t dims[4] = {64, (cuuint64_t)Wout, (cuuint64_t)Hp, (cuuint64_t)B};
-    cuuint64_t strides[3] = {64, (cuuint64_t)Wp * 32, (cuuint64_t)Hp * Wp * 32};
-    cuuint32_t box[4] = {64, (cuuint32_t)box_w, 1, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    return encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x16), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS ? 0 : 2;
+    const cuuint64_t dims[4] = {64, (cuuint64_t)Wout, (cuuint64_t)Hp, (cuuint64_t)B};
+    const cuuint64_t strides[3] = {64, (cuuint64_t)Wp * 32, (cuuint64_t)Hp * Wp * 32};
+    const cuuint32_t box[4] = {64, 128, 1, 1};
+    const cuuint32_t estr[4] = {1, 1, 1, 1};
+    return tma_encode(m, x16, 4, dims, strides, box, estr, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
-
-int wgrad2_launch_stem(const CUtensorMap& map_x, const void* dz, float* dw, float* scratch, int B, int H, int Wout,
-                       int Cin_true, cudaStream_t st);
-int64_t wgrad2_stem_scratch_floats(int B, int H, int Wout);
 
 }  // namespace delora
 
@@ -303,27 +295,13 @@ extern "C" int delora_stem_fprop_bf16(const void* x16, const void* w_stem, void*
     p.B = B; p.H = H; p.Wout = W / 2; p.segs = (p.Wout + 127) / 128; p.n_jobs = B * H * p.segs; p.act = act;
     p.out_f16 = out_f16 ? 1 : 0;
     CUtensorMap mx, mw;
-    DELORA_CHECK_ARG(stem_encode_x_map(&mx, x16, B, H, W, 128) == 0, "delora_stem_fprop_bf16: tensor map (x) failed");
-    {
-        PFN_cuTensorMapEncodeTiled_v12000 encode = get_tensor_map_encoder();
-        cuuint64_t dims[2] = {64, 192};
-        cuuint64_t strides[1] = {128};
-        cuuint32_t box[2] = {64, 64};
-        cuuint32_t estr[2] = {1, 1};
-        CUresult rc = encode(&mw, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(w_stem), dims, strides, box, estr,
-                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        DELORA_CHECK_ARG(rc == CUDA_SUCCESS, "delora_stem_fprop_bf16: tensor map (w) failed: %d", (int)rc);
-    }
+    int rc = stem_encode_x_map(&mx, x16, B, H, W);
+    DELORA_CHECK_ARG(rc == 0, "delora_stem_fprop_bf16: tensor map (x) failed: %d", rc);
+    rc = tma_filter(&mw, w_stem, 64, 192, 64, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);     // [3 rows x 64 co][64 k]
+    DELORA_CHECK_ARG(rc == 0, "delora_stem_fprop_bf16: tensor map (w) failed: %d", rc);
     const size_t smem = 3 * 8192 + (size_t)kStemStages * 3 * kStemTile + 2 * kAccTileBytes + 256 + 1024;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    static bool attr_set[64] = {};
-    if (dev < 64 && !attr_set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(stem_fprop_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        DELORA_CHECK_ARG(e == cudaSuccess, "delora_stem_fprop_bf16: shared-memory opt-in failed: %s", cudaGetErrorString(e));
-        attr_set[dev] = true;
-    }
+    const cudaError_t e = smem_opt_in<stem_fprop_tc_kernel>();
+    DELORA_CHECK_ARG(e == cudaSuccess, "delora_stem_fprop_bf16: shared-memory opt-in failed: %s", cudaGetErrorString(e));
     const int grid = p.n_jobs < num_sms() ? p.n_jobs : num_sms();
     stem_fprop_tc_kernel<<<grid, kStemThreads, smem, (cudaStream_t)stream>>>(mx, mw, (__nv_bfloat16*)y, p);
     DELORA_CHECK_LAUNCH("stem_fprop_tc_kernel");
@@ -337,6 +315,7 @@ extern "C" int delora_stem_wgrad_bf16(const void* x16, const void* dz, float* dw
     DELORA_CHECK_ARG(x16 && dz && dw && scratch, "delora_stem_wgrad_bf16: null pointer");
     DELORA_CHECK_ARG(W % 2 == 0 && W >= 2 && Cin_true >= 1 && Cin_true <= 8, "delora_stem_wgrad_bf16: bad shape");
     CUtensorMap mx;
-    DELORA_CHECK_ARG(stem_encode_x_map(&mx, x16, B, H, W, 128) == 0, "delora_stem_wgrad_bf16: tensor map (x) failed");
+    const int rc = stem_encode_x_map(&mx, x16, B, H, W);
+    DELORA_CHECK_ARG(rc == 0, "delora_stem_wgrad_bf16: tensor map (x) failed: %d", rc);
     return wgrad2_launch_stem(mx, dz, dw, scratch, B, H, W / 2, Cin_true, (cudaStream_t)stream);
 }

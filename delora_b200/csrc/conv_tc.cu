@@ -21,7 +21,7 @@
 // columns).  Warp roles: 0..7 = MMA + epilogue, 8 = TMA producer.
 #include <stdlib.h>
 #include <cuda_fp16.h>
-#include "tc_common.cuh"
+#include "conv_internal.cuh"
 
 namespace delora {
 
@@ -711,12 +711,6 @@ weight_prep_kernel(const float* __restrict__ w, int Cout, int Cin, int k, int Ci
 }
 
 // ---------------------------------------------------------------- host side
-static PFN_cuTensorMapEncodeTiled_v12000 get_encode() { return get_tensor_map_encoder(); }
-
-struct TensorMaps {
-    CUtensorMap x, w;
-};
-
 // Output tile of `pixels` (128 fprop / 64 wgrad) = TW x TH with TW a power of two >= 4: the shape that wastes
 // the fewest pixels on a Hout x Wout image (ragged tiles are zero-filled by TMA on the way in and masked
 // on the way out), the widest one on ties.  64x2048 images tile exactly; KITTI's 64x720 (widths 360, 180,
@@ -731,64 +725,6 @@ static void pick_tile(int Hout, int Wout, int pixels, int* TW, int* TH) {
     }
 }
 
-// Tensor maps depend only on (pointers, shapes); encoding them costs a few microseconds of host time
-// per call, which matters when 20 convolutions are launched back to back.  Small per-thread cache.
-static const TensorMaps* get_maps(const void* x, const void* w, int B, int Hin, int Win, int Cin, int Cout,
-                                  const ConvParams& p) {
-    struct Key { const void* x; const void* w; int B, Hin, Win, Cin, Cout, ks, sh, sw; };
-    struct Entry { Key k; TensorMaps m; };
-    static thread_local Entry cache[64];
-    static thread_local int used = 0, next = 0;
-    const Key key = {x, w, B, Hin, Win, Cin, Cout, p.ksize, p.stride_h, p.stride_w};
-    for (int i = 0; i < used; ++i) {
-        const Key& c = cache[i].k;
-        if (c.x == key.x && c.w == key.w && c.B == key.B && c.Hin == key.Hin && c.Win == key.Win && c.Cin == key.Cin &&
-            c.Cout == key.Cout && c.ks == key.ks && c.sh == key.sh && c.sw == key.sw)
-            return &cache[i].m;
-    }
-    PFN_cuTensorMapEncodeTiled_v12000 encode = get_encode();
-    if (!encode) return nullptr;
-    Entry& e = cache[next];
-    const int Hp = Hin + 2, Wp = Win + 2;
-    {
-        cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)Wp, (cuuint64_t)Hp, (cuuint64_t)B};
-        cuuint64_t strides[3] = {(cuuint64_t)Cin * 2, (cuuint64_t)Wp * Cin * 2, (cuuint64_t)Hp * Wp * Cin * 2};
-        // with a traversal stride the box spans TW*stride_w (TH*stride_h) elements and loads every stride-th one
-        cuuint32_t box[4] = {(cuuint32_t)kBlockK, (cuuint32_t)(p.TW * p.stride_w), (cuuint32_t)(p.TH * p.stride_h), 1};
-        cuuint32_t estr[4] = {1, (cuuint32_t)p.stride_w, (cuuint32_t)p.stride_h, 1};
-        if (encode(&e.m.x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return nullptr;
-    }
-    {
-        cuuint64_t dims[2] = {(cuuint64_t)p.taps * Cin, (cuuint64_t)Cout};
-        cuuint64_t strides[1] = {(cuuint64_t)p.taps * Cin * 2};
-        cuuint32_t box[2] = {(cuuint32_t)kBlockK, (cuuint32_t)p.BN};
-        cuuint32_t estr[2] = {1, 1};
-        if (encode(&e.m.w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(w), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-            return nullptr;
-    }
-    e.k = key;
-    const TensorMaps* out = &e.m;
-    next = (next + 1) % 64;
-    if (used < 64) ++used;
-    return out;
-}
-
-}  // namespace delora
-
-namespace delora {
-bool conv_rows_eligible(int Cin, int Cout, int ksize, int Wg);
-bool wgrad2_eligible(int Cin, int Cout, int ksize, int stride_h, int stride_w);
-int64_t wgrad2_scratch_floats(int B, int Hout, int Wout, int Cin, int Cout, int sw);
-int wgrad2_launch(const void* x, const void* dz, float* dw, float* scratch, int B, int Hin, int Win, int Cin, int Cin_true,
-                  int Cout, int stride_h, int stride_w, cudaStream_t st);
-int conv_rows_launch(const void* x, const void* w, const void* residual, const void* saved, void* y, int B, int Hout,
-                     int Wout, int Cin, int Cout, int ksize, int up_h, int up_w, int act, cudaStream_t stream,
-                     int residual_on_grid);
 }  // namespace delora
 
 using namespace delora;
@@ -815,21 +751,18 @@ extern "C" int delora_conv2d_fprop_bf16(const void* x, const void* w, const void
     p.tiles_h = (p.Hout + p.TH - 1) / p.TH;
     p.BN = (Cout % 128 == 0) ? 128 : 64;
     p.stages = kMaxStages;                               // ring of 4 x 32 KB (BN = 128) or 4 x 24 KB (BN = 64)
-    const TensorMaps* maps = get_maps(x, w, B, Hin, Win, Cin, Cout, p);
-    DELORA_CHECK_ARG(maps != nullptr, "delora_conv2d_fprop_bf16: cuTensorMapEncodeTiled failed or is unavailable");
+    // with a traversal stride the box spans TW*stride_w (TH*stride_h) elements and loads every stride-th one
+    CUtensorMap mx, mw;
+    int rc = tma_nhwc(&mx, x, B, Hin, Win, Cin, p.TW * stride_w, p.TH * stride_h, stride_w, stride_h, false);
+    if (rc == 0) rc = tma_filter(&mw, w, p.taps * Cin, Cout, p.BN, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+    DELORA_CHECK_ARG(rc == 0, "delora_conv2d_fprop_bf16: cuTensorMapEncodeTiled failed or is unavailable: %d", rc);
     const size_t smem = (size_t)p.stages * (kBlockM * kBlockK * 2 + p.BN * kBlockK * 2) + 2 * kAccTileBytes +
                         2 * kMaxStages * 8 + 1024;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    static bool attr_set[64] = {};                       // the opt-in is per device (one process may drive several)
-    if (dev < 64 && !attr_set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(conv_fprop_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        DELORA_CHECK_ARG(e == cudaSuccess, "delora_conv2d_fprop_bf16: smem opt-in failed: %s", cudaGetErrorString(e));
-        attr_set[dev] = true;
-    }
+    const cudaError_t e = smem_opt_in<conv_fprop_tc_kernel>();
+    DELORA_CHECK_ARG(e == cudaSuccess, "delora_conv2d_fprop_bf16: smem opt-in failed: %s", cudaGetErrorString(e));
     dim3 grid(B * p.tiles_h * p.tiles_w, Cout / p.BN);
     conv_fprop_tc_kernel<<<grid, kConvThreads, smem, (cudaStream_t)stream>>>(
-        maps->x, maps->w, (const __nv_bfloat16*)residual, (const __nv_bfloat16*)saved, (__nv_bfloat16*)y, p);
+        mx, mw, (const __nv_bfloat16*)residual, (const __nv_bfloat16*)saved, (__nv_bfloat16*)y, p);
     DELORA_CHECK_LAUNCH("conv_fprop_tc_kernel");
     return 0;
 }
@@ -921,42 +854,14 @@ extern "C" int delora_conv2d_wgrad_bf16(const void* x, const void* dz, float* dw
     p.tg = wgrad_tap_group(Cin, ksize);
     p.groups_per_row = (ksize + p.tg - 1) / p.tg;
     p.stages = (p.nb * p.tg == 4) ? 3 : 4;
-    PFN_cuTensorMapEncodeTiled_v12000 encode = get_encode();
-    DELORA_CHECK_ARG(encode != nullptr, "delora_conv2d_wgrad_bf16: cuTensorMapEncodeTiled not available");
     CUtensorMap map_dz, map_x;
-    {
-        const int Hp = p.Hout + 2, Wp = p.Wout + 2;
-        // extents stop at the last REAL pixel (padded index Wout / Hout): a ragged K tile then reads zeros from
-        // TMA's out-of-bounds fill instead of the circular halo column, so it adds nothing to the sum
-        cuuint64_t dims[4] = {(cuuint64_t)Cout, (cuuint64_t)(Wp - 1), (cuuint64_t)(Hp - 1), (cuuint64_t)B};
-        cuuint64_t strides[3] = {(cuuint64_t)Cout * 2, (cuuint64_t)Wp * Cout * 2, (cuuint64_t)Hp * Wp * Cout * 2};
-        cuuint32_t box[4] = {64, (cuuint32_t)p.TW, (cuuint32_t)p.TH, 1};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        CUresult rc = encode(&map_dz, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(dz), dims, strides, box, estr,
-                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        DELORA_CHECK_ARG(rc == CUDA_SUCCESS, "delora_conv2d_wgrad_bf16: tensor map (dz) failed: %d", (int)rc);
-    }
-    {
-        const int Hp = Hin + 2, Wp = Win + 2;
-        cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)Wp, (cuuint64_t)Hp, (cuuint64_t)B};
-        cuuint64_t strides[3] = {(cuuint64_t)Cin * 2, (cuuint64_t)Wp * Cin * 2, (cuuint64_t)Hp * Wp * Cin * 2};
-        cuuint32_t box[4] = {64, (cuuint32_t)(p.TW * stride_w), (cuuint32_t)(p.TH * stride_h), 1};
-        cuuint32_t estr[4] = {1, (cuuint32_t)stride_w, (cuuint32_t)stride_h, 1};
-        CUresult rc = encode(&map_x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x), dims, strides, box, estr,
-                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        DELORA_CHECK_ARG(rc == CUDA_SUCCESS, "delora_conv2d_wgrad_bf16: tensor map (x) failed: %d", (int)rc);
-    }
+    int rc = tma_nhwc(&map_dz, dz, B, p.Hout, p.Wout, Cout, p.TW, p.TH, 1, 1, true);
+    DELORA_CHECK_ARG(rc == 0, "delora_conv2d_wgrad_bf16: tensor map (dz) failed: %d", rc);
+    rc = tma_nhwc(&map_x, x, B, Hin, Win, Cin, p.TW * stride_w, p.TH * stride_h, stride_w, stride_h, false);
+    DELORA_CHECK_ARG(rc == 0, "delora_conv2d_wgrad_bf16: tensor map (x) failed: %d", rc);
     const size_t smem = (size_t)p.stages * (2 + p.nb * p.tg) * 8192 + 2 * kAccTileBytes + 2 * kMaxStages * 8 + 1024;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    static bool attr_set[64] = {};
-    if (dev < 64 && !attr_set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(conv_wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        DELORA_CHECK_ARG(e == cudaSuccess, "delora_conv2d_wgrad_bf16: smem opt-in failed: %s", cudaGetErrorString(e));
-        attr_set[dev] = true;
-    }
+    const cudaError_t e = smem_opt_in<conv_wgrad_tc_kernel>();
+    DELORA_CHECK_ARG(e == cudaSuccess, "delora_conv2d_wgrad_bf16: smem opt-in failed: %s", cudaGetErrorString(e));
     cudaStream_t st = (cudaStream_t)stream;
     dim3 grid(p.ksize * p.groups_per_row, co_tiles * p.ci_tiles, p.splits);
     conv_wgrad_tc_kernel<<<grid, kConvThreads, smem, st>>>(map_dz, map_x, scratch, p);

@@ -17,7 +17,7 @@
 // rows: grid = tiles x splits <= #SMs, fp32 partials, a coalesced fixed-order reduction (deterministic) into the torch
 // layout.  Warp roles: 0..11 MMA + epilogue (three warpgroups), 12 TMA producer.
 #include <string.h>
-#include "tc_common.cuh"
+#include "conv_internal.cuh"
 
 namespace delora {
 
@@ -295,42 +295,14 @@ int wgrad2_launch(const void* x, const void* dz, float* dw, float* scratch, int 
     DELORA_CHECK_ARG(stages >= 2, "conv_wgrad2: stage of %d bytes does not fit twice", p.stage_bytes);
     p.stages = stages;
 
-    PFN_cuTensorMapEncodeTiled_v12000 encode = get_tensor_map_encoder();
-    DELORA_CHECK_ARG(encode != nullptr, "conv_wgrad2: cuTensorMapEncodeTiled not available");
     CUtensorMap map_dz, map_x;
-    {
-        const int Hp = p.Hout + 2, Wp = p.Wout + 2;
-        // extents stop at the last REAL pixel: a ragged K row reads zeros from the out-of-bounds fill, not the halo
-        cuuint64_t dims[4] = {(cuuint64_t)Cout, (cuuint64_t)(Wp - 1), (cuuint64_t)(Hp - 1), (cuuint64_t)B};
-        cuuint64_t strides[3] = {(cuuint64_t)Cout * 2, (cuuint64_t)Wp * Cout * 2, (cuuint64_t)Hp * Wp * Cout * 2};
-        cuuint32_t box[4] = {64, (cuuint32_t)NS, 1, 1};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        CUresult rc = encode(&map_dz, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(dz), dims, strides, box, estr,
-                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        DELORA_CHECK_ARG(rc == CUDA_SUCCESS, "conv_wgrad2: tensor map (dz) failed: %d", (int)rc);
-    }
-    {
-        const int Hp = Hin + 2, Wp = Win + 2;
-        cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)Wp, (cuuint64_t)Hp, (cuuint64_t)B};
-        cuuint64_t strides[3] = {(cuuint64_t)Cin * 2, (cuuint64_t)Wp * Cin * 2, (cuuint64_t)Hp * Wp * Cin * 2};
-        // with a traversal stride the box spans xpix * stride_w elements and loads every stride_w-th one
-        cuuint32_t box[4] = {64, (cuuint32_t)(xpix * stride_w), 1, 1};
-        cuuint32_t estr[4] = {1, (cuuint32_t)stride_w, 1, 1};
-        CUresult rc = encode(&map_x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(x), dims, strides, box, estr,
-                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        DELORA_CHECK_ARG(rc == CUDA_SUCCESS, "conv_wgrad2: tensor map (x) failed: %d", (int)rc);
-    }
+    int rc = tma_nhwc(&map_dz, dz, B, p.Hout, p.Wout, Cout, NS, 1, 1, 1, true);
+    DELORA_CHECK_ARG(rc == 0, "conv_wgrad2: tensor map (dz) failed: %d", rc);
+    rc = tma_nhwc(&map_x, x, B, Hin, Win, Cin, xpix * stride_w, 1, stride_w, 1, false);
+    DELORA_CHECK_ARG(rc == 0, "conv_wgrad2: tensor map (x) failed: %d", rc);
     const size_t smem = (size_t)p.stages * p.stage_bytes + kWgConsumers * kAccTileBytes + 2 * kWgMaxStages * 8 + 1024;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    static bool attr_set[64] = {};
-    if (dev < 64 && !attr_set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(conv_wgrad2_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        DELORA_CHECK_ARG(e == cudaSuccess, "conv_wgrad2: shared-memory opt-in failed: %s", cudaGetErrorString(e));
-        attr_set[dev] = true;
-    }
+    const cudaError_t e = smem_opt_in<conv_wgrad2_tc_kernel>();
+    DELORA_CHECK_ARG(e == cudaSuccess, "conv_wgrad2: shared-memory opt-in failed: %s", cudaGetErrorString(e));
     conv_wgrad2_tc_kernel<<<p.n_tiles * p.splits, kWgThreads, smem, st>>>(map_dz, map_x, scratch, p);
     DELORA_CHECK_LAUNCH("conv_wgrad2_tc_kernel");
     const size_t total4 = (size_t)9 * Cout * Cin / 4;
@@ -366,29 +338,12 @@ int wgrad2_launch_stem(const CUtensorMap& map_x, const void* dz, float* dw, floa
     for (int rr = 0; rr < 3; ++rr) p.units[rr] = WgUnit{T + rr * T, 0, rr, 0, 0};     // filter row rr
     p.n_loads = 4; p.n_units = 3; p.stage_bytes = 4 * T; p.stage_tx = 4 * T;
     p.stages = (kWgSmemBudget - kWgConsumers * kAccTileBytes) / p.stage_bytes;
-    PFN_cuTensorMapEncodeTiled_v12000 encode = get_tensor_map_encoder();
-    DELORA_CHECK_ARG(encode != nullptr, "stem wgrad: cuTensorMapEncodeTiled not available");
     CUtensorMap map_dz;
-    {
-        const int Hp = H + 2, Wp = Wout + 2;
-        cuuint64_t dims[4] = {64, (cuuint64_t)(Wp - 1), (cuuint64_t)(Hp - 1), (cuuint64_t)B};
-        cuuint64_t strides[3] = {128, (cuuint64_t)Wp * 128, (cuuint64_t)Hp * Wp * 128};
-        cuuint32_t box[4] = {64, 128, 1, 1};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        CUresult rc = encode(&map_dz, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(dz), dims, strides, box, estr,
-                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        DELORA_CHECK_ARG(rc == CUDA_SUCCESS, "stem wgrad: tensor map (dz) failed: %d", (int)rc);
-    }
+    const int rc = tma_nhwc(&map_dz, dz, B, H, Wout, 64, 128, 1, 1, 1, true);
+    DELORA_CHECK_ARG(rc == 0, "stem wgrad: tensor map (dz) failed: %d", rc);
     const size_t smem = (size_t)p.stages * p.stage_bytes + kWgConsumers * kAccTileBytes + 2 * kWgMaxStages * 8 + 1024;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    static bool attr_set[64] = {};
-    if (dev < 64 && !attr_set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(conv_wgrad2_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        DELORA_CHECK_ARG(e == cudaSuccess, "stem wgrad: shared-memory opt-in failed: %s", cudaGetErrorString(e));
-        attr_set[dev] = true;
-    }
+    const cudaError_t e = smem_opt_in<conv_wgrad2_tc_kernel>();
+    DELORA_CHECK_ARG(e == cudaSuccess, "stem wgrad: shared-memory opt-in failed: %s", cudaGetErrorString(e));
     conv_wgrad2_tc_kernel<<<p.n_tiles * p.splits, kWgThreads, smem, st>>>(map_dz, map_x, scratch, p);
     DELORA_CHECK_LAUNCH("conv_wgrad2_tc_kernel (stem)");
     stem_reduce_kernel<<<(9 * 64 * 8 + 255) / 256, 256, 0, st>>>(scratch, p.splits, Cin_true, dw);

@@ -1077,12 +1077,6 @@ struct TrainPlan {
     size_t total;
 };
 
-// ops.conv2d_dgrad_eligible: the phase-decomposed data gradient of delora_conv2d_dgrad_bf16 takes the layer
-static bool dgrad_eligible(int cin, int cout, int win, int sw) {
-    const int wg = (win + sw - 1) / sw;
-    return cout % 64 == 0 && (cin % 128 == 0 || (cin == 64 && wg >= 128)) && (sw == 1 || win % 2 == 0);
-}
-
 static void make_train_plan(const delora_odometry_desc* d, TrainPlan* tp) {
     memset(tp, 0, sizeof(TrainPlan));
     plan_model(d, &tp->m);
@@ -1115,7 +1109,7 @@ static void make_train_plan(const delora_odometry_desc* d, TrainPlan* tp) {
         for (int j = 0; j < 3; ++j) tp->g[s][j] = take(off, nhwc_bytes(MB, m.stage_h[s], m.stage_w[s], m.stage_c[s]));
     for (int i = 0; i < m.n_block; ++i) {
         const Block& b = m.block[i];
-        tp->phase_dgrad[i] = b.ds >= 0 && i > 0 && dgrad_eligible(b.cin, b.cout, b.win, b.sw);
+        tp->phase_dgrad[i] = b.ds >= 0 && i > 0 && delora_conv2d_dgrad_eligible(b.cin, b.cout, b.win, b.sh, b.sw);
         if (b.ds < 0) continue;
         tp->gds[b.stage] = take(off, nhwc_bytes(MB, b.hout, b.wout, b.cin));
         if (!tp->phase_dgrad[i]) tp->gu1[b.stage] = take(off, nhwc_bytes(MB, b.hin, b.win, b.cout));

@@ -1,10 +1,12 @@
 // PTX wrappers shared by the wgmma convolution kernels (conv_tc.cu, conv_rows.cu, conv_wgrad.cu, conv_stem.cu):
-// mbarrier, TMA (cp.async.bulk.tensor), wgmma, shared-memory matrix descriptors, the accumulator hand-off.
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma, shared-memory matrix descriptors, the accumulator hand-off; and the host
+// side of their launchers: the tensor-map encoder with its cache, the shared-memory opt-in.
 //
 // With SWIZZLE_128B the swizzle phase of a row follows from its ABSOLUTE shared-memory address (TMA writes and the
 // tensor core reads alike), so an operand may start at any multiple of 128 B inside a 1024-byte-aligned TMA-written
 // tile with the descriptor's base offset left at 0.  This is what lets one halo tile serve all filter taps.
 #pragma once
+#include <string.h>
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cudaTypedefs.h>
@@ -135,17 +137,95 @@ __device__ __forceinline__ float apply_act(float v, int act) {
     return v;
 }
 
-// host: cuTensorMapEncodeTiled through the runtime's driver entry point (no -lcuda link dependency)
-inline PFN_cuTensorMapEncodeTiled_v12000 get_tensor_map_encoder() {
-    static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
-    if (!fn) {
+// ---- host: TMA tensor maps.  Every map of the convolution kernels is bf16 with the 128-byte swizzle the smem
+// descriptors above assume, no interleave and zero out-of-bounds fill; what differs is the request below.
+struct TmaRequest {
+    const void* ptr;
+    cuuint64_t dims[4], strides[3];               // strides in bytes, of dims 1 .. rank - 1
+    cuuint32_t box[4], estr[4];
+    int rank;
+    CUtensorMapL2promotion promo;
+};
+static_assert(sizeof(TmaRequest) == 104, "TmaRequest is compared with memcmp: it must have no padding");
+
+// Encodes a map (cuTensorMapEncodeTiled through the runtime's driver entry point: no -lcuda link dependency) behind a
+// per-thread cache keyed on the complete request.  Activations, filters and gradients live in persistent buffers, so
+// the cache takes the encode cost (microseconds of host time per map) out of the convolution launches; it holds 512
+// maps: the 384 of the two caches it replaced, plus room for the weight-gradient and stem maps.
+// Returns 0, the encoder's CUresult, or CUDA_ERROR_NOT_FOUND when the driver has no encoder.
+inline int tma_encode(CUtensorMap* map, const void* ptr, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
+                      const cuuint32_t* box, const cuuint32_t* estr, CUtensorMapL2promotion promo) {
+    constexpr int kCap = 512;
+    struct Cache { TmaRequest keys[kCap]; CUtensorMap maps[kCap]; int used, next; };
+    static thread_local Cache cache;
+    TmaRequest req;
+    memset(&req, 0, sizeof(req));
+    req.ptr = ptr; req.rank = rank; req.promo = promo;
+    for (int i = 0; i < rank; ++i) {
+        req.dims[i] = dims[i]; req.box[i] = box[i]; req.estr[i] = estr[i];
+        if (i > 0) req.strides[i - 1] = strides[i - 1];
+    }
+    for (int i = 0; i < cache.used; ++i)          // the pointer first: most entries differ there
+        if (cache.keys[i].ptr == ptr && memcmp(&cache.keys[i], &req, sizeof(req)) == 0) {
+            *map = cache.maps[i];
+            return 0;
+        }
+    static PFN_cuTensorMapEncodeTiled_v12000 encode = nullptr;
+    if (!encode) {
         void* p = nullptr;
         cudaDriverEntryPointQueryResult q;
         if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
             q == cudaDriverEntryPointSuccess)
-            fn = (PFN_cuTensorMapEncodeTiled_v12000)p;
+            encode = (PFN_cuTensorMapEncodeTiled_v12000)p;
     }
-    return fn;
+    if (!encode) return CUDA_ERROR_NOT_FOUND;
+    const CUresult rc = encode(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(ptr), req.dims,
+                               req.strides, req.box, req.estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                               promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (rc != CUDA_SUCCESS) return (int)rc;
+    cache.keys[cache.next] = req;
+    cache.maps[cache.next] = *map;
+    cache.next = (cache.next + 1) % kCap;
+    if (cache.used < kCap) ++cache.used;
+    return 0;
+}
+
+// Padded NHWC activation [B, H+2, W+2, C] as the map (channel, column, row, image), box (64, box_w, box_h, 1).
+// sw / sh: traversal strides -- the box spans box_w (box_h) elements and loads every sw-th (sh-th) one.
+// clip: the extents stop at the last REAL pixel (padded index W / H), so a ragged tile reads zeros from the
+// out-of-bounds fill instead of the circular halo column (output-gradient maps of the weight gradients: the halo
+// would add to the sum).
+inline int tma_nhwc(CUtensorMap* map, const void* x, int B, int H, int W, int C, int box_w, int box_h, int sw, int sh,
+                    bool clip) {
+    const cuuint64_t Hp = (cuuint64_t)H + 2, Wp = (cuuint64_t)W + 2, pixel = (cuuint64_t)C * 2;
+    const cuuint64_t dims[4] = {(cuuint64_t)C, clip ? Wp - 1 : Wp, clip ? Hp - 1 : Hp, (cuuint64_t)B};
+    const cuuint64_t strides[3] = {pixel, Wp * pixel, Hp * Wp * pixel};
+    const cuuint32_t box[4] = {64, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
+    const cuuint32_t estr[4] = {1, (cuuint32_t)sw, (cuuint32_t)sh, 1};
+    return tma_encode(map, x, 4, dims, strides, box, estr, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+}
+
+// Row-major bf16 filter matrix [rows][cols] as the map (column, row), box (64, box_rows).
+inline int tma_filter(CUtensorMap* map, const void* w, int cols, int rows, int box_rows, CUtensorMapL2promotion promo) {
+    const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+    const cuuint64_t strides[1] = {(cuuint64_t)cols * 2};
+    const cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
+    const cuuint32_t estr[2] = {1, 1};
+    return tma_encode(map, w, 2, dims, strides, box, estr, promo);
+}
+
+// Lets `kernel` use the full 227 KB of dynamic shared memory a CTA may have on sm_90, once per (kernel, device).  The
+// flags are per template instance, i.e. per kernel ADDRESS: two instances of one kernel template share a function
+// type but not their flags.
+template <auto kernel>
+inline cudaError_t smem_opt_in() {
+    static bool done[64] = {};
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev < 64 && done[dev]) return cudaSuccess;
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (e == cudaSuccess && dev < 64) done[dev] = true;
+    return e;
 }
 
 // Epilogue of one output pixel's 32 consecutive channels (fp32 accumulators in v[32]): residual add, activation or

@@ -354,9 +354,7 @@ def conv2d_fprop(x, weight, hin, win, ksize, stride, act=ACT_NONE, residual=None
 
 def conv2d_dgrad_eligible(cin, cout, win, stride):
     """Can delora_conv2d_dgrad_bf16 (phase-decomposed data gradient) take this layer?"""
-    wg = (win + stride[1] - 1) // stride[1]
-    return (cout % 64 == 0 and (cin % 128 == 0 or (cin == 64 and wg >= 128))
-            and (stride[1] == 1 or win % 2 == 0))
+    return _lib.lib().delora_conv2d_dgrad_eligible(cin, cout, win, stride[0], stride[1]) == 1
 
 
 def conv2d_dgrad(dz, w_flip, hin, win, stride, act=ACT_NONE, residual=None, out=None, saved=None,

@@ -268,11 +268,16 @@ int delora_conv2d_fprop_bf16(const void* x, const void* w, const void* residual,
  * residual_strided = 1: `residual` is [B,Hout+2,Wout+2,Cin] instead and is added at the input pixels
  * (stride_h * h, stride_w * w) only -- the data gradient of the block's 1x1 strided downsample (:134), which never
  * reaches the other pixels (replaces a zero-upsampled copy of it).
- * Needs Cout % 64 == 0, Cin % 128 == 0 (or Cin = 64 with >= 128 columns per phase) and, for stride_w = 2, an even Win (an odd circular width mixes the phases at
- * the seam: use delora_zero_upsample_nhwc_bf16 + delora_conv2d_fprop_bf16 there). */
+ * Takes the layers delora_conv2d_dgrad_eligible accepts; for the others use delora_zero_upsample_nhwc_bf16 +
+ * delora_conv2d_fprop_bf16. */
 int delora_conv2d_dgrad_bf16(const void* dz, const void* w_flip, const void* residual, const void* saved, void* dx,
                              int B, int Hin, int Win, int Cin, int Cout, int stride_h, int stride_w, int act,
                              int residual_strided, void* stream);
+/* 1 if delora_conv2d_dgrad_bf16 takes the data gradient of this 3x3 layer (Cin, Cout of the FORWARD convolution, Win its
+ * input width), 0 if not: strides in {1,2}, Cout % 64 == 0, Cin % 128 == 0 or Cin = 64 with >= 128 columns per phase
+ * (ceil(Win / stride_w)), and an even Win for stride_w = 2 (an odd circular width mixes the phases at the seam).
+ * Host only: needs no device and launches nothing. */
+int delora_conv2d_dgrad_eligible(int Cin, int Cout, int Win, int stride_h, int stride_w);
 /* Weight gradient of the same convolution on wgmma (split-K over pixels, deterministic reduction):
  * x [B,Hin+2,Win+2,Cin] padded NHWC bf16 (the layer input), dz [B,Hout+2,Wout+2,Cout] padded NHWC bf16
  * (gradient w.r.t. the pre-activation output) -> dw [Cout, Cin_true, k, k] fp32 (torch layout; Cin_true <= Cin
