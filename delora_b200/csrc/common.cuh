@@ -17,14 +17,38 @@ void set_error(const char* fmt, ...);
         }                                                  \
     } while (0)
 
-#define DELORA_CHECK_LAUNCH(name)                                                   \
+// `err`: the result of a launch call that returns it (launch_pdl).  A failed launch is also the runtime's last error,
+// which is cleared here so that it is not reported again by a later check.
+#define DELORA_CHECK_LAUNCH_RESULT(err, name)                                       \
     do {                                                                            \
-        cudaError_t e__ = cudaGetLastError();                                       \
+        const cudaError_t e__ = (err);                                              \
         if (e__ != cudaSuccess) {                                                   \
+            cudaGetLastError();                                                     \
             ::delora::set_error("%s: launch failed: %s", name, cudaGetErrorString(e__)); \
             return 2;                                                               \
         }                                                                           \
     } while (0)
+
+// after a <<<...>>> launch
+#define DELORA_CHECK_LAUNCH(name) DELORA_CHECK_LAUNCH_RESULT(cudaGetLastError(), name)
+
+// Launches `kernel` as the programmatic dependent of the kernel before it on `st`: its CTAs may start once every CTA of
+// that kernel has executed griddepcontrol.launch_dependents (or exited), and must execute griddepcontrol.wait before
+// they read what that kernel writes.  Returns the launch error.
+template <typename... Params, typename... Args>
+inline cudaError_t launch_pdl(void (*kernel)(Params...), dim3 grid, dim3 block, cudaStream_t st, Args... args) {
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = 0;
+    cfg.stream = st;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, kernel, args...);
+}
 
 // SMs of the current device: persistent grids and split-K factors are sized to it (132 on an H100 SXM, 114 on an
 // H100 PCIe).  Cached per device; 132 when no device answers (host-side size queries without a GPU).

@@ -121,9 +121,9 @@ icp_kernel(const float4* __restrict__ src_pts4, const float4* __restrict__ src_n
     const float4* __restrict__ tn = tgt_nrm4 + (size_t)b * tgt_stride;
     const int32_t* __restrict__ cs = cell_start + (size_t)b * ((size_t)g.H * g.W + 1);
 
-    float4 p = make_float4(0.f, 0.f, 0.f, 0.f), m = p, tq = p, tnq = p;
+    float4 p = make_float4(0.f, 0.f, 0.f, 0.f), m = p;
     float sx = 0.f, sy = 0.f, sz = 0.f, nsx = 0.f, nsy = 0.f, nsz = 0.f;
-    bool paired = false;
+    int pos = -1;
     if (active) {
         p = __ldg(src_pts4 + (size_t)b * src_stride + i);
         m = __ldg(src_nrm4 + (size_t)b * src_stride + i);
@@ -135,25 +135,14 @@ icp_kernel(const float4* __restrict__ src_pts4, const float4* __restrict__ src_n
         }
         const NNBest best = nn_search(g, tp, cs, sx, sy, sz);
         if (nn_index) nn_index[(size_t)b * src_stride + i] = best.pos >= 0 ? best.tag : -1;
-        if (best.pos >= 0) {
-            paired = true;
-            tq = __ldg(tp + best.pos);
-            tnq = __ldg(tn + best.pos);
-        }
+        pos = best.pos;
     }
     // the accumulators only come alive after the search (keeps the search loop's register set small)
-    float acc[kIcpAcc];
-#pragma unroll
-    for (int k = 0; k < kIcpAcc; ++k) acc[k] = 0.0f;
-    if (active) {
-        float4 pd = make_float4(0.f, 0.f, 0.f, 0.f), nd = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (paired) accumulate_pair(flags, p, m, sx, sy, sz, nsx, nsy, nsz, tq, tnq, acc, pd, nd);
-        if (point_dir) point_dir[(size_t)b * src_stride + i] = pd;
-        if (normal_dir) normal_dir[(size_t)b * src_stride + i] = nd;
-    }
-    const int warp_row = (blockIdx.x * kIcpThreads + threadIdx.x) >> 5;
-    if (warp_row < rows_per_pair)
-        write_warp_partials(acc, partial_rows + ((size_t)b * rows_per_pair + warp_row) * DELORA_ICP_PARTIAL);
+    const size_t k = (size_t)b * src_stride + i;
+    accumulate_warp_row<kIcpAcc, false>(pos >= 0, flags, p, m, sx, sy, sz, nsx, nsy, nsz, tp, tn, pos,
+                                        active && point_dir ? point_dir + k : nullptr,
+                                        active && normal_dir ? normal_dir + k : nullptr,
+                                        partial_rows, b, rows_per_pair, (blockIdx.x * kIcpThreads + threadIdx.x) >> 5);
 }
 
 // Column sums of the per-warp partial rows: one block per (group of 8 columns, pair).  Thread t reads the group's
@@ -206,35 +195,34 @@ icp_finalize_kernel(const float* __restrict__ rows, int rows_per_pair, float* __
     if (threadIdx.x < DELORA_ICP_PARTIAL) s[threadIdx.x] = __ldcg(colsum + (size_t)b * DELORA_ICP_PARTIAL + threadIdx.x);
     if (threadIdx.x == 0) counter[b] = 0;
     __syncthreads();
-    const float M = s[2], Mp = s[25];
+    const float M = s[kColM], Mp = s[kColMp];
     const float inv_m = M > 0.0f ? 1.0f / M : 0.0f;              // torch's mean over an empty set is NaN; we return 0
     const float inv_mp = Mp > 0.0f ? 1.0f / (3.0f * Mp) : 0.0f;  // MSE over 3*M' coordinates (icp_losses.py:169)
     if (threadIdx.x == 0) {
         float* __restrict__ o = losses + (size_t)b * DELORA_LOSS_ROW;
-        o[0] = s[24] * inv_mp;
-        o[1] = s[0] * inv_m;
-        o[2] = s[1] * inv_m;
-        o[3] = M;
-        o[4] = Mp;
-        o[5] = 0.f; o[6] = 0.f; o[7] = 0.f;
+        o[kLossPo2po] = s[kColD2] * inv_mp;
+        o[kLossPo2pl] = s[kColR2] * inv_m;
+        o[kLossPl2pl] = s[kColPl2pl] * inv_m;
+        o[kLossM] = M;
+        o[kLossMp] = Mp;
+        for (int k = kLossMp + 1; k < DELORA_LOSS_ROW; ++k) o[k] = 0.f;
     }
     if (threadIdx.x < 12) {
         const int row = threadIdx.x / 4, col = threadIdx.x % 4;
         float gval;
         const float k_pl = 2.0f * lambda_po2pl * inv_m, k_nn = 2.0f * inv_m, k_pp = 2.0f * inv_mp;
         if (col < 3) {
-            gval = k_pl * s[6 + row * 3 + col] + k_nn * s[15 + row * 3 + col] + k_pp * s[29 + row * 3 + col];
+            gval = k_pl * s[kColRnP + row * 3 + col] + k_nn * s[kColGnM + row * 3 + col] +
+                   k_pp * s[kColDP + row * 3 + col];
         } else {
-            gval = k_pl * s[3 + row] + k_pp * s[26 + row];
+            gval = k_pl * s[kColRn + row] + k_pp * s[kColD + row];
         }
         grad_T[(size_t)b * 12 + threadIdx.x] = gval;
     }
 }
 
-int launch_icp_finalize(float* scratch, int B, int rows, float lambda_po2pl, uint32_t flags, float* losses,
-                        float* grad_T, cudaStream_t st) {
-    (void)flags;
-    const IcpScratch sc = icp_scratch(scratch, B, rows);
+int launch_icp_finalize(const IcpScratch& sc, int B, int rows, float lambda_po2pl, float* losses, float* grad_T,
+                        cudaStream_t st) {
     dim3 grid(kFinGroups, B);
     icp_finalize_kernel<<<grid, 256, 0, st>>>(sc.rows, rows, sc.colsum, sc.counter, lambda_po2pl, losses, grad_T);
     DELORA_CHECK_LAUNCH("icp_finalize_kernel");
@@ -253,7 +241,7 @@ icp_point_grads_kernel(const float4* __restrict__ point_dir, const float4* __res
     if (i >= src_stride) return;
     float gx = 0.f, gy = 0.f, gz = 0.f, hx = 0.f, hy = 0.f, hz = 0.f;
     if (i < n_src[b]) {
-        const float M = losses[(size_t)b * DELORA_LOSS_ROW + 3], Mp = losses[(size_t)b * DELORA_LOSS_ROW + 4];
+        const float M = losses[(size_t)b * DELORA_LOSS_ROW + kLossM], Mp = losses[(size_t)b * DELORA_LOSS_ROW + kLossMp];
         const float g_po2po = upstream[b * 3 + 0], g_po2pl = upstream[b * 3 + 1], g_pl2pl = upstream[b * 3 + 2];
         const float4 pd = point_dir[(size_t)b * src_stride + i];
         const float4 nd = normal_dir[(size_t)b * src_stride + i];
@@ -294,18 +282,9 @@ __global__ void quat_to_T_bwd_kernel(const float* __restrict__ quat, const float
 
 using namespace delora;
 
-extern "C" int delora_icp_partial_rows(int src_stride) { return (src_stride + 31) / 32; }
+extern "C" int delora_icp_partial_rows(int src_stride) { return icp_layout(1, src_stride).rows; }
 
-extern "C" int64_t delora_icp_scratch_floats(int B, int src_stride) {
-    // partial rows + column sums + counters; then, for the dense path: the 4x16-cell range pyramid (2 floats per
-    // block, at most src_stride/64 + H + W/16 + 1 <= src_stride/16 + 4096 blocks per pair), the prefix and suffix
-    // range extents of the pixel rows (4 floats per row, H <= src_stride) + one counter per pair, and the work list of
-    // its second kernel (4 counters, int4 + done counter per warp, float4 search state + int result per source pixel)
-    const int64_t rows = delora_icp_partial_rows(src_stride);
-    return (int64_t)B * rows * DELORA_ICP_PARTIAL + (int64_t)B * DELORA_ICP_PARTIAL + B + 2 +
-           (int64_t)B * 2 * (src_stride / 16 + 4096) + (int64_t)B * 4 * src_stride + B + 8 + 5 * (int64_t)B * rows +
-           5 * (int64_t)B * rows * 32;
-}
+extern "C" int64_t delora_icp_scratch_floats(int B, int src_stride) { return icp_layout(B, src_stride).total; }
 
 extern "C" int delora_icp_fwd_bwd(const delora_f4* src_pts4, const delora_f4* src_nrm4, const int32_t* n_src,
                                   int src_stride, const float* T, const delora_f4* tgt_pts4,
@@ -319,8 +298,9 @@ extern "C" int delora_icp_fwd_bwd(const delora_f4* src_pts4, const delora_f4* sr
     DELORA_CHECK_ARG(B > 0 && B <= 65535 && src_stride > 0 && tgt_stride > 0 && H > 0 && W > 0,
                      "delora_icp_fwd_bwd: bad shape");
     const GridParams g = make_grid(H, W, hfov0, hfov1, vfov0, vfov1, 1);
-    const int rows = delora_icp_partial_rows(src_stride);
-    const IcpScratch sc = icp_scratch(partials, B, rows);
+    const IcpLayout L = icp_layout(B, src_stride);
+    const int rows = L.rows;
+    const IcpScratch sc = icp_scratch(partials, L);
     dim3 grid((src_stride + kIcpThreads - 1) / kIcpThreads, B);
     cudaStream_t st = (cudaStream_t)stream;
     if (T) {
@@ -335,7 +315,7 @@ extern "C" int delora_icp_fwd_bwd(const delora_f4* src_pts4, const delora_f4* sr
             (float4*)normal_dir, sc.rows, rows);
     }
     DELORA_CHECK_LAUNCH("icp_kernel");
-    return launch_icp_finalize(partials, B, rows, lambda_po2pl, flags, losses, grad_T, st);
+    return launch_icp_finalize(sc, B, rows, lambda_po2pl, losses, grad_T, st);
 }
 
 extern "C" int delora_icp_point_grads(const delora_f4* point_dir, const delora_f4* normal_dir,

@@ -5,7 +5,27 @@
 namespace delora {
 
 constexpr float kHalfPiF = 1.57079632679489661923f;
-constexpr int kIcpAcc = 38;
+
+// Columns of a partial row (DELORA_ICP_PARTIAL floats: sums over the pairs of one warp).  p, m: source point /
+// normal before the transform; r = (s - t).n_t; g_n = d(pl2pl term)/d(n_s) / 2; 3 x 3 blocks are row-major.
+constexpr int kColR2 = 0;       // sum r^2
+constexpr int kColPl2pl = 1;    // sum of the pl2pl term
+constexpr int kColM = 2;        // M: pairs with a normal on both sides
+constexpr int kColRn = 3;       // 3: sum r n_t
+constexpr int kColRnP = 6;      // 9: sum (r n_t) p^T
+constexpr int kColGnM = 15;     // 9: sum g_n m^T
+constexpr int kColPo2po = 24;   // the po2po block, last: a kernel without po2po reduces only the columns before it
+constexpr int kColD2 = 24;      // sum |s - t|^2
+constexpr int kColMp = 25;      // M': pairs with a normal on neither side
+constexpr int kColD = 26;       // 3: sum (s - t)
+constexpr int kColDP = 29;      // 9: sum (s - t) p^T
+constexpr int kIcpAcc = 38;     // accumulated columns; the rest of the row is padding
+static_assert(kColGnM + 9 == kColPo2po && kColDP + 9 == kIcpAcc, "the po2po block is the last one");
+static_assert(kIcpAcc <= DELORA_ICP_PARTIAL, "the accumulators fit a partial row");
+
+// Columns of a `losses` row (DELORA_LOSS_ROW floats)
+constexpr int kLossPo2po = 0, kLossPo2pl = 1, kLossPl2pl = 2, kLossM = 3, kLossMp = 4;
+static_assert(kLossMp < DELORA_LOSS_ROW, "the loss columns fit a losses row");
 
 // Running nearest neighbour.  Ranking is EXACT in float64 (what cKDTree measures), but float64 is
 // only touched when two candidates are closer than 1e-5 relative in fp32 (the fp32 squared
@@ -75,13 +95,15 @@ __device__ __forceinline__ void apply_rigid(const Rigid& r, const float4 p, cons
     nsz = fmaf(r.r22, m.z, fmaf(r.r21, m.y, r.r20 * m.x));
 }
 
-// Per-pair accumulators (DELORA_ICP_PARTIAL = 40 floats per partial row):
-//  0 sum r^2            1 sum pl2pl term      2 M
-//  3..5   sum r*n_t                 6..14  sum (r*n_t) p^T
-//  15..23 sum g_n m^T               24 sum |s-t|^2 (po2po)   25 M'
-//  26..28 sum (s-t)                 29..37 sum (s-t) p^T      38,39 pad
-// p, m: source point / normal before the transform; (sx..), (nsx..): after; t, q: matched target
-// point and (normal, has-normal flag).  Masks: src/losses/icp_losses.py:48-52, :110-121, :83-99.
+// acc[c + 3 i + j] = a_i v_j: the outer product (ax, ay, az) v^T into a 3 x 3 block of columns
+__device__ __forceinline__ void acc_outer(float (&acc)[kIcpAcc], int c, float ax, float ay, float az, const float4 v) {
+    acc[c + 0] = ax * v.x; acc[c + 1] = ax * v.y; acc[c + 2] = ax * v.z;
+    acc[c + 3] = ay * v.x; acc[c + 4] = ay * v.y; acc[c + 5] = ay * v.z;
+    acc[c + 6] = az * v.x; acc[c + 7] = az * v.y; acc[c + 8] = az * v.z;
+}
+
+// The columns of one (source, target) pair.  (sx..), (nsx..): source point / normal after the transform; t, q: matched
+// target point and (normal, has-normal flag).  Masks: src/losses/icp_losses.py:48-52, :110-121, :83-99.
 __device__ __forceinline__ void accumulate_pair(uint32_t flags, const float4 p, const float4 m, float sx, float sy,
                                                 float sz, float nsx, float nsy, float nsz, const float4 t,
                                                 const float4 q, float (&acc)[kIcpAcc], float4& pd, float4& nd) {
@@ -89,40 +111,34 @@ __device__ __forceinline__ void accumulate_pair(uint32_t flags, const float4 p, 
     const bool tgt_has = q.w != 0.0f;
     const float dx = sx - t.x, dy = sy - t.y, dz = sz - t.z;
     if (src_has && tgt_has) {
-        acc[2] = 1.0f;
+        acc[kColM] = 1.0f;
         if (flags & DELORA_LOSS_PO2PL) {
             const float r = fmaf(dz, q.z, fmaf(dy, q.y, dx * q.x));                      // icp_losses.py:197-199
-            acc[0] = r * r;
+            acc[kColR2] = r * r;
             const float gx = r * q.x, gy = r * q.y, gz = r * q.z;
-            acc[3] = gx; acc[4] = gy; acc[5] = gz;
-            acc[6] = gx * p.x; acc[7] = gx * p.y; acc[8] = gx * p.z;
-            acc[9] = gy * p.x; acc[10] = gy * p.y; acc[11] = gy * p.z;
-            acc[12] = gz * p.x; acc[13] = gz * p.y; acc[14] = gz * p.z;
+            acc[kColRn + 0] = gx; acc[kColRn + 1] = gy; acc[kColRn + 2] = gz;
+            acc_outer(acc, kColRnP, gx, gy, gz, p);
             pd = make_float4(gx, gy, gz, 1.0f);
         }
         if (flags & DELORA_LOSS_PL2PL) {
             float hx, hy, hz;
             if (flags & DELORA_NORMAL_LINEAR) {                                          // :226-231
                 const float om = 1.0f - fmaf(nsz, q.z, fmaf(nsy, q.y, nsx * q.x));
-                acc[1] = om * om;
+                acc[kColPl2pl] = om * om;
                 hx = -om * q.x; hy = -om * q.y; hz = -om * q.z;
             } else {                                                                     // :232-238
                 hx = nsx - q.x; hy = nsy - q.y; hz = nsz - q.z;
-                acc[1] = fmaf(hz, hz, fmaf(hy, hy, hx * hx));
+                acc[kColPl2pl] = fmaf(hz, hz, fmaf(hy, hy, hx * hx));
             }
-            acc[15] = hx * m.x; acc[16] = hx * m.y; acc[17] = hx * m.z;
-            acc[18] = hy * m.x; acc[19] = hy * m.y; acc[20] = hy * m.z;
-            acc[21] = hz * m.x; acc[22] = hz * m.y; acc[23] = hz * m.z;
+            acc_outer(acc, kColGnM, hx, hy, hz, m);
             nd = make_float4(hx, hy, hz, 1.0f);
             pd.w = 1.0f;
         }
     } else if ((flags & DELORA_LOSS_PO2PO) && !src_has && !tgt_has) {                    // :168-179
-        acc[24] = fmaf(dz, dz, fmaf(dy, dy, dx * dx));
-        acc[25] = 1.0f;
-        acc[26] = dx; acc[27] = dy; acc[28] = dz;
-        acc[29] = dx * p.x; acc[30] = dx * p.y; acc[31] = dx * p.z;
-        acc[32] = dy * p.x; acc[33] = dy * p.y; acc[34] = dy * p.z;
-        acc[35] = dz * p.x; acc[36] = dz * p.y; acc[37] = dz * p.z;
+        acc[kColD2] = fmaf(dz, dz, fmaf(dy, dy, dx * dx));
+        acc[kColMp] = 1.0f;
+        acc[kColD + 0] = dx; acc[kColD + 1] = dy; acc[kColD + 2] = dz;
+        acc_outer(acc, kColDP, dx, dy, dz, p);
         pd = make_float4(dx, dy, dz, 2.0f);
     }
 }
@@ -166,41 +182,136 @@ __device__ __forceinline__ void warp_column_sums(const float (&acc)[kIcpAcc], fl
     }
 }
 
-// one partial row per warp, lane k writes column k (and k+32)
-template <int N = kIcpAcc>   // columns >= N are known to be zero (e.g. the po2po block when it is off)
-__device__ __forceinline__ void write_warp_partials(const float (&acc)[kIcpAcc], float* __restrict__ row) {
+// The end of every ICP kernel.  The lane's pair (when `paired`: target tg[j], tn[j]) is accumulated, and the warp's
+// column sums are written to (ADD = false) or added to (ADD = true, the dense path's block search adding to the row
+// the window search wrote) partial row `warp_row` of pair b; lane k keeps column k and 32 + k.  N: the live
+// columns, kIcpAcc or kColPo2po; below kIcpAcc the po2po flag is masked off, so the columns from N on stay zero.
+template <int N, bool ADD>
+__device__ __forceinline__ void accumulate_warp_row(bool paired, uint32_t flags, const float4 p, const float4 m,
+                                                    float sx, float sy, float sz, float nsx, float nsy, float nsz,
+                                                    const float4* __restrict__ tg, const float4* __restrict__ tn,
+                                                    int j, float4* __restrict__ point_dir, float4* __restrict__ normal_dir, float* __restrict__ partial_rows,
+                                                    int b, int rows_per_pair, int warp_row) {
+    static_assert(N == kIcpAcc || N == kColPo2po, "all columns, or all but the po2po block");
+    float acc[kIcpAcc];
+#pragma unroll
+    for (int k = 0; k < kIcpAcc; ++k) acc[k] = 0.0f;
+    float4 pd = make_float4(0.f, 0.f, 0.f, 0.f), nd = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (paired)
+        accumulate_pair(N == kIcpAcc ? flags : (flags & ~DELORA_LOSS_PO2PO), p, m, sx, sy, sz, nsx, nsy, nsz,
+                        __ldg(tg + j), __ldg(tn + j), acc, pd, nd);
+    if (point_dir) *point_dir = pd;
+    if (normal_dir) *normal_dir = nd;
+    if (warp_row >= rows_per_pair) return;
+    float* __restrict__ row = partial_rows + ((size_t)b * rows_per_pair + warp_row) * DELORA_ICP_PARTIAL;
     const int lane = threadIdx.x & 31;
     float keep0, keep1;
     warp_column_sums<N>(acc, keep0, keep1);
-    row[lane] = keep0;
-    if (lane < DELORA_ICP_PARTIAL - 32) row[32 + lane] = keep1;
+    if (ADD) {
+        row[lane] += keep0;
+        if (lane < DELORA_ICP_PARTIAL - 32) row[32 + lane] += keep1;
+    } else {
+        row[lane] = keep0;
+        if (lane < DELORA_ICP_PARTIAL - 32) row[32 + lane] = keep1;
+    }
 }
 
-// same reduction, ADDED to a row that already holds the sums of the other lanes (second kernel of the dense path)
-template <int N = kIcpAcc>
-__device__ __forceinline__ void add_warp_partials(const float (&acc)[kIcpAcc], float* __restrict__ row) {
-    const int lane = threadIdx.x & 31;
-    float keep0, keep1;
-    warp_column_sums<N>(acc, keep0, keep1);
-    row[lane] += keep0;
-    if (lane < DELORA_ICP_PARTIAL - 32) row[32 + lane] += keep1;
+// Range extents of the dense path's target grids, per pair (target_extents_kernel):
+//   blk[nbh * nbw]       [min, max] of |t| per 4 x 16-cell block (the block search's pyramid)
+//   row_pre[H], row_suf[H]  [min, max] of |t| over the valid cells of the pixel rows <= k / >= k
+// Every extent is widened by a relative 1e-6 so that bounds built on it stay conservative against the fp32 norm
+// rounding; an empty block or row set has max < 0.
+struct TargetExtents {
+    float2* blk;
+    float2* row_pre;
+    float2* row_suf;
+    int* counter;          // per pair: CTAs of the pre-pass that have finished (0 when idle)
+};
+
+// Work list of the dense path's block search (icp_dense_pending_kernel).  An ITEM is a warp of icp_dense_kernel that
+// gave up on some of its lanes after `max_strips` window-growing steps; an ENTRY is one such lane.
+struct PendingList {
+    int* counters;          // [0] items, [1] CTAs of the second kernel that have finished, [2] entries; 0 when idle
+    int4* items;            // (pair, warp in pair, mask of unfinished lanes, first entry)
+    int* item_done;         // entries of the item already searched (0 when idle)
+    float4* entries;        // (m1, m2, bits(j1), bits(item * 32 + lane)) of the window search so far
+    int* result;            // per entry: pixel id of the nearest neighbour
+};
+
+// The scratch buffer of both ICP paths (delora_icp_scratch_floats floats), as element offsets in floats.  Every
+// capacity follows from (B, src_stride) alone; the dense path uses src_stride = H * W.  Sections are ordered by the
+// alignment they need (16-byte int4 / float4, then 8-byte float2, then 4-byte) and every size is a multiple of the
+// next section's alignment, so no section needs padding.  The buffer is zeroed once; the kernels leave every counter
+// at zero again.
+struct IcpLayout {
+    int rows;                  // partial rows per pair: one per warp of 32 source points
+    int64_t blk_per_pair;      // range-pyramid blocks per pair
+    int64_t partials;          // [B, rows, DELORA_ICP_PARTIAL] per-warp partial rows
+    int64_t colsum;            // [B, DELORA_ICP_PARTIAL] column sums
+    int64_t items;             // int4 [B * rows]: work-list items (at most one per warp)
+    int64_t entries;           // float4 [B * rows * 32]: work-list entries (at most one per source point)
+    int64_t blk;               // float2 [B, blk_per_pair]: range pyramid
+    int64_t row_pre, row_suf;  // float2 [B, src_stride] each: row prefix / suffix extents (H <= src_stride)
+    int64_t result;            // int [B * rows * 32]: per entry
+    int64_t item_done;         // int [B * rows]: per item
+    int64_t counter;           // int [B + 2]: finalize counters, one per pair
+    int64_t ext_counter;       // int [B]: extents counters, one per pair
+    int64_t pend_counters;     // int [8]: work-list counters
+    int64_t total;
+};
+static_assert(sizeof(int4) == 16 && sizeof(float4) == 16 && sizeof(float2) == 8, "element sizes the layout assumes");
+static_assert(DELORA_ICP_PARTIAL % 4 == 0, "the partial rows and column sums keep the int4 / float4 sections 16-byte aligned");
+
+inline IcpLayout icp_layout(int B, int src_stride) {
+    IcpLayout L;
+    const int64_t b = B, s = src_stride;
+    L.rows = (int)((s + 31) / 32);
+    L.blk_per_pair = s / 16 + 4096;
+    int64_t off = 0;
+    auto take = [&off](int64_t n) { const int64_t o = off; off += n; return o; };
+    L.partials = take(b * L.rows * DELORA_ICP_PARTIAL);
+    L.colsum = take(b * DELORA_ICP_PARTIAL);
+    L.items = take(4 * b * L.rows);
+    L.entries = take(4 * b * L.rows * 32);
+    L.blk = take(2 * b * L.blk_per_pair);
+    L.row_pre = take(2 * b * s);
+    L.row_suf = take(2 * b * s);
+    L.result = take(b * L.rows * 32);
+    L.item_done = take(b * L.rows);
+    L.counter = take(b + 2);
+    L.ext_counter = take(b);
+    L.pend_counters = take(8);
+    L.total = off;
+    return L;
 }
 
-// scratch layout (floats): [B * rows * 40 partial rows][B * 40 column sums][B int32 counters]
+// device views of a scratch buffer laid out by icp_layout
 struct IcpScratch {
     float* rows;
     float* colsum;
     int* counter;
+    TargetExtents ext;
+    PendingList pend;
 };
-inline IcpScratch icp_scratch(float* base, int B, int rows) {
+
+inline IcpScratch icp_scratch(float* base, const IcpLayout& L) {
     IcpScratch s;
-    s.rows = base;
-    s.colsum = base + (size_t)B * rows * DELORA_ICP_PARTIAL;
-    s.counter = reinterpret_cast<int*>(s.colsum + (size_t)B * DELORA_ICP_PARTIAL);
+    s.rows = base + L.partials;
+    s.colsum = base + L.colsum;
+    s.counter = reinterpret_cast<int*>(base + L.counter);
+    s.ext.blk = reinterpret_cast<float2*>(base + L.blk);
+    s.ext.row_pre = reinterpret_cast<float2*>(base + L.row_pre);
+    s.ext.row_suf = reinterpret_cast<float2*>(base + L.row_suf);
+    s.ext.counter = reinterpret_cast<int*>(base + L.ext_counter);
+    s.pend.counters = reinterpret_cast<int*>(base + L.pend_counters);
+    s.pend.items = reinterpret_cast<int4*>(base + L.items);
+    s.pend.item_done = reinterpret_cast<int*>(base + L.item_done);
+    s.pend.entries = reinterpret_cast<float4*>(base + L.entries);
+    s.pend.result = reinterpret_cast<int*>(base + L.result);
     return s;
 }
 
-int launch_icp_finalize(float* scratch, int B, int rows, float lambda_po2pl, uint32_t flags, float* losses,
-                        float* grad_T, cudaStream_t st);
+int launch_icp_finalize(const IcpScratch& sc, int B, int rows, float lambda_po2pl, float* losses, float* grad_T,
+                        cudaStream_t st);
 
 }  // namespace delora

@@ -27,6 +27,8 @@
 namespace delora {
 
 constexpr int kDenseThreads = 128;
+constexpr float kInf = 3.0e38f;     // "no bound": the border does not exist, or nothing valid lies beyond it
+constexpr float kSlack = 2e-3f;     // px subtracted from every border distance; covers the fp32 error of the cell binning
 
 __device__ __forceinline__ int wrap_col(int c, int W) {
     c += (c < 0) ? W : 0;
@@ -110,18 +112,6 @@ constexpr int kBlkH = 4, kBlkW = 16;
 //  16..23 warps by strip count {0, 1-2, 3-5, 6-10, 11-20, 21-40, 41-63, >= limit} | 24..31 cells per lane, same buckets
 __device__ unsigned int g_dbg[32];
 constexpr int kDefaultMaxStrips = 32; // window-growing steps before a lane is handed to the block-search kernel
-
-// Range extents of the target grids, per pair:
-//   blk[nbh * nbw]       [min, max] of |t| per 4 x 16-cell block (the block search's pyramid)
-//   row_pre[H], row_suf[H]  [min, max] of |t| over the valid cells of the pixel rows <= k / >= k
-// Every extent is widened by a relative 1e-6 so that bounds built on it stay conservative against the fp32 norm
-// rounding; an empty block or row set has max < 0.
-struct TargetExtents {
-    float2* blk;
-    float2* row_pre;
-    float2* row_suf;
-    int* counter;          // per pair: CTAs of the pre-pass that have finished (0 when idle)
-};
 
 constexpr int kExtThreads = 1024, kExtUnroll = 4;
 
@@ -254,7 +244,7 @@ __device__ __forceinline__ float range_lb2(float r, float S, float2 rho) {
 // which the 0.999 margin on the squared bound covers for half angles >= 7.2e-4 rad.  A row border is at least
 // 1 - 2e-3 rows from the source direction, so this holds for row pitches down to 1.45e-3 rad (0.083 deg).
 __device__ __forceinline__ float row_border_bound(float dpx, float rad_per_px, float r, float2 rho) {
-    if (!(rho.y >= 0.0f)) return 3.0e38f;
+    if (!(rho.y >= 0.0f)) return kInf;
     const float d = fminf(fmaxf(dpx * rad_per_px, 0.0f), kHalfPiF);
     const float sh = __sinf(0.5f * d);
     return fmaxf(r * __sinf(d), sqrtf(range_lb2(r, sh * sh, rho)));
@@ -274,7 +264,7 @@ __device__ __forceinline__ void nn2_merge(NN2& a, float bm1, float bm2, int bj) 
     if (bj >= 0 && bj == a.j1) { a.m2 = fminf(a.m2, bm2); return; }     // the same cell seen twice is not a tie
     const bool take = (bm1 < a.m1) || (bm1 == a.m1 && bj >= 0 && (a.j1 < 0 || bj < a.j1));
     const float lose = take ? a.m1 : bm1;                   // the larger of the two minima
-    a.m2 = fminf(fminf(a.m2, bm2), (bj >= 0 && a.j1 >= 0) ? lose : 3.0e38f);
+    a.m2 = fminf(fminf(a.m2, bm2), (bj >= 0 && a.j1 >= 0) ? lose : kInf);
     if (take) { a.m1 = bm1; a.j1 = bj; }
 }
 
@@ -315,15 +305,27 @@ __device__ __forceinline__ SrcLane load_src_lane(const float4* __restrict__ src_
     return s;
 }
 
-// Work list of the second kernel (in `scratch`).  An ITEM is a warp of icp_dense_kernel that gave up on some
-// of its lanes after `max_strips` window-growing steps; an ENTRY is one such lane.
-struct PendingList {
-    int* counters;          // [0] items, [1] CTAs of the second kernel that have finished, [2] entries; 0 when idle
-    int4* items;            // (pair, warp in pair, mask of unfinished lanes, first entry)
-    int* item_done;         // entries of the item already searched (0 when idle)
-    float4* entries;        // (m1, m2, bits(j1), bits(item * 32 + lane)) of the window search so far
-    int* result;            // per entry: pixel id of the nearest neighbour
-};
+// Exactness bound of the window's lower (DOWN) or upper row border, `e` rows from the lane's centre row rc; `f` is the
+// distance (px) from the source direction to that border of the centre cell.  Angular + range bound over the rows
+// beyond (row_border_bound; prefix extents below, suffix extents above); no row beyond: no bound.
+template <bool DOWN>
+__device__ __forceinline__ float window_row_bound(int e, int rc, int H, float f, float dv_rad, float r,
+                                                  const float2* __restrict__ row_pre,
+                                                  const float2* __restrict__ row_suf) {
+    const bool open = DOWN ? rc - e > 0 : rc + e < H - 1;
+    return open ? row_border_bound(f + (float)e, dv_rad, r, __ldg(DOWN ? row_pre + rc - e - 1 : row_suf + rc + e + 1))
+                : kInf;
+}
+
+// Exactness bounds of the window's left and right column borders, e_lf / e_rt columns from the lane's centre column
+// cc (f_lf, f_rt as for window_row_bound); angular only.  A window as wide as the grid has no column border, and a
+// border at or beyond the +-180 deg seam is seam_px closer than its unwrapped pixel distance.
+__device__ __forceinline__ void window_col_bounds(int e_lf, int e_rt, int cc, int W, float f_lf, float f_rt, float rxy,
+                                                  const GridParams& g, float& b_lf, float& b_rt) {
+    const bool full_w = e_lf + e_rt + 1 >= W;
+    b_lf = full_w ? kInf : border_bound(f_lf + (float)e_lf - (cc - e_lf <= 0 ? g.seam_px : 0.0f), g.du_rad, rxy);
+    b_rt = full_w ? kInf : border_bound(f_rt + (float)e_rt - (cc + e_rt >= W - 1 ? g.seam_px : 0.0f), g.du_rad, rxy);
+}
 
 // ---------------------------------------------------------------------------------------------
 // Kernel 1: window search for everybody; the (few) lanes whose exactness guard still fails after
@@ -345,8 +347,6 @@ icp_dense_kernel(const float4* __restrict__ src_grid, const float4* __restrict__
     const int i = blockIdx.x * kDenseThreads + threadIdx.x;
     const int warp_in_pair = i >> 5;
     const int lane = threadIdx.x & 31;
-    constexpr float kInf = 3.0e38f;
-    constexpr float kSlack = 2e-3f;     // px; covers the fp32 error of the cell binning
 
     const SrcLane s = load_src_lane(src_grid, src_ngrid, T, b, i, HW, g);
     const bool active = s.active;
@@ -387,18 +387,12 @@ icp_dense_kernel(const float4* __restrict__ src_grid, const float4* __restrict__
         // distance (px) from the source direction to the four borders of its own centre cell
         const float f_dn = (vs - (float)rc) + 0.5f - kSlack, f_up = ((float)rc - vs) + 0.5f - kSlack;
         const float f_lf = (us - (float)cc) + 0.5f - kSlack, f_rt = ((float)cc - us) + 0.5f - kSlack;
-        // row borders: angular + range bound over the rows beyond (row_border_bound); column borders: angular
         const float2* __restrict__ row_pre = ext.row_pre + (size_t)b * H;
         const float2* __restrict__ row_suf = ext.row_suf + (size_t)b * H;
-        float b_dn = (rc - e_dn > 0) ? row_border_bound(f_dn + (float)e_dn, g.dv_rad, r, __ldg(row_pre + rc - e_dn - 1))
-                                     : kInf;
-        float b_up = (rc + e_up < H - 1) ? row_border_bound(f_up + (float)e_up, g.dv_rad, r, __ldg(row_suf + rc + e_up + 1))
-                                         : kInf;
-        // a border at or beyond the +-180 deg seam is seam_px closer than its unwrapped pixel distance
-        float b_lf = (e_lf + e_rt + 1 >= W) ? kInf
-                   : border_bound(f_lf + (float)e_lf - (cc - e_lf <= 0 ? g.seam_px : 0.0f), g.du_rad, rxy);
-        float b_rt = (e_lf + e_rt + 1 >= W) ? kInf
-                   : border_bound(f_rt + (float)e_rt - (cc + e_rt >= W - 1 ? g.seam_px : 0.0f), g.du_rad, rxy);
+        float b_dn = window_row_bound<true>(e_dn, rc, H, f_dn, g.dv_rad, r, row_pre, row_suf);
+        float b_up = window_row_bound<false>(e_up, rc, H, f_up, g.dv_rad, r, row_pre, row_suf);
+        float b_lf, b_rt;
+        window_col_bounds(e_lf, e_rt, cc, W, f_lf, f_rt, rxy, g, b_lf, b_rt);
         unsigned pending = 0u;                                   // lanes that still fail after max_strips steps
         int n_strips = 0, n_cells = 15;
         for (int strip = 0;; ++strip) {
@@ -444,12 +438,9 @@ icp_dense_kernel(const float4* __restrict__ src_grid, const float4* __restrict__
                     col = (col == W) ? 0 : col;
                 }
                 if (side == 0)
-                    b_dn = (rc - e_dn > 0) ? row_border_bound(f_dn + (float)e_dn, g.dv_rad, r, __ldg(row_pre + rc - e_dn - 1))
-                                           : kInf;
+                    b_dn = window_row_bound<true>(e_dn, rc, H, f_dn, g.dv_rad, r, row_pre, row_suf);
                 else
-                    b_up = (rc + e_up < H - 1)
-                               ? row_border_bound(f_up + (float)e_up, g.dv_rad, r, __ldg(row_suf + rc + e_up + 1))
-                               : kInf;
+                    b_up = window_row_bound<false>(e_up, rc, H, f_up, g.dv_rad, r, row_pre, row_suf);
             } else {
                 const int step = min(2, W - (e_lf + e_rt + 1));
                 const int c0 = wrap_col((side == 2) ? cc - e_lf - 1 : cc + e_rt + 1, W);
@@ -466,9 +457,7 @@ icp_dense_kernel(const float4* __restrict__ src_grid, const float4* __restrict__
                     nn2_eval(__ldg(tg + (unsigned)(rbase + c1)), rbase + c1, sx, sy, sz, nn, rok && two);
                 }
                 if (side == 2) e_lf += step; else e_rt += step;
-                const bool full_w = (e_lf + e_rt + 1 >= W);
-                b_lf = full_w ? kInf : border_bound(f_lf + (float)e_lf - (cc - e_lf <= 0 ? g.seam_px : 0.0f), g.du_rad, rxy);
-                b_rt = full_w ? kInf : border_bound(f_rt + (float)e_rt - (cc + e_rt >= W - 1 ? g.seam_px : 0.0f), g.du_rad, rxy);
+                window_col_bounds(e_lf, e_rt, cc, W, f_lf, f_rt, rxy, g, b_lf, b_rt);
             }
         }
         if (STATS && lane == 0) {
@@ -499,17 +488,9 @@ icp_dense_kernel(const float4* __restrict__ src_grid, const float4* __restrict__
             best_j = nn_exact_rescan(tg, H, W, rc, cc, e_dn, e_up, e_lf, e_rt, sx, sy, sz, nn.m1 * (1.0f + kNNBand));
         }
     }
-    float acc[kIcpAcc];
-#pragma unroll
-    for (int k = 0; k < kIcpAcc; ++k) acc[k] = 0.0f;
-    if (active && best_j >= 0) {
-        float4 pd, nd;
-        accumulate_pair(PO2PO ? flags : (flags & ~DELORA_LOSS_PO2PO), s.p, s.m, sx, sy, sz, s.nsx, s.nsy, s.nsz,
-                        __ldg(tg + best_j), __ldg(tn + best_j), acc, pd, nd);
-    }
-    if (warp_in_pair < rows_per_pair)
-        write_warp_partials<(PO2PO ? kIcpAcc : 24)>(
-            acc, partial_rows + ((size_t)b * rows_per_pair + warp_in_pair) * DELORA_ICP_PARTIAL);
+    accumulate_warp_row<(PO2PO ? kIcpAcc : kColPo2po), false>(active && best_j >= 0, flags, s.p, s.m, sx, sy, sz, s.nsx,
+                                                              s.nsy, s.nsz, tg, tn, best_j, nullptr, nullptr,
+                                                              partial_rows, b, rows_per_pair, warp_in_pair);
 }
 
 struct OwnerGeom { float sx, sy, sz, us, vs, r, cos_es; };
@@ -524,8 +505,6 @@ template <bool EXACT>
 __device__ __forceinline__ int block_pass(const float4* __restrict__ tg, const float2* __restrict__ blk,
                                           const GridParams& g, int nbw, const OwnerGeom& o, const BlockRect& rect,
                                           float& bound, NN2& loc, double& ebest, int& ej) {
-    constexpr float kInf = 3.0e38f;
-    constexpr float kSlack = 2e-3f;
     const int H = g.H, W = g.W;
     const int lane = threadIdx.x & 31;
     int scanned = 0;
@@ -598,7 +577,7 @@ __device__ __noinline__ int exact_rerank_warp(const float4* __restrict__ tg, con
     double ebest = 1.0e300;
     int ej = 0x7fffffff;
     NN2 unused;
-    unused.m1 = unused.m2 = 3.0e38f; unused.j1 = -1;
+    unused.m1 = unused.m2 = kInf; unused.j1 = -1;
     block_pass<true>(tg, blk, g, nbw, o, rect, thresh, unused, ebest, ej);
 #pragma unroll
     for (int s = 16; s > 0; s >>= 1) {
@@ -629,8 +608,6 @@ icp_dense_pending_kernel(const float4* __restrict__ src_grid, const float4* __re
     const int lane = threadIdx.x & 31;
     const int warps_per_cta = (int)blockDim.x >> 5;
     const int gwarp = blockIdx.x * warps_per_cta + ((int)threadIdx.x >> 5), n_warps = gridDim.x * warps_per_cta;
-    constexpr float kInf = 3.0e38f;
-    constexpr float kSlack = 2e-3f;
     const int n_entries = *reinterpret_cast<volatile int*>(pend.counters + 2);
     for (int e = gwarp; e < n_entries; e += n_warps) {
         const float4 ent = __ldg(pend.entries + e);
@@ -719,17 +696,10 @@ icp_dense_pending_kernel(const float4* __restrict__ src_grid, const float4* __re
             const SrcLane s = load_src_lane(src_grid, src_ngrid, T, b, warp_in_pair * 32 + lane, HW, g);
             const bool mine = ((pending >> lane) & 1u) != 0u && s.active;
             const int best_j = mine ? __ldcg(pend.result + it.w + __popc(pending & ((1u << lane) - 1u))) : -1;
-            float acc[kIcpAcc];
-#pragma unroll
-            for (int k = 0; k < kIcpAcc; ++k) acc[k] = 0.0f;
-            if (mine && best_j >= 0) {
-                float4 pd, nd;
-                accumulate_pair(PO2PO ? flags : (flags & ~DELORA_LOSS_PO2PO), s.p, s.m, s.sx, s.sy, s.sz, s.nsx, s.nsy,
-                                s.nsz, __ldg(tg + best_j), __ldg(tn + best_j), acc, pd, nd);
-            }
-            if (warp_in_pair < rows_per_pair)
-                add_warp_partials<(PO2PO ? kIcpAcc : 24)>(
-                    acc, partial_rows + ((size_t)b * rows_per_pair + warp_in_pair) * DELORA_ICP_PARTIAL);
+            accumulate_warp_row<(PO2PO ? kIcpAcc : kColPo2po), true>(mine && best_j >= 0, flags, s.p, s.m, s.sx, s.sy,
+                                                                     s.sz, s.nsx, s.nsy, s.nsz, tg, tn, best_j, nullptr,
+                                                                     nullptr, partial_rows, b, rows_per_pair,
+                                                                     warp_in_pair);
             if (lane == 0) pend.item_done[item] = 0;                    // re-arm
         }
     }
@@ -744,6 +714,25 @@ icp_dense_pending_kernel(const float4* __restrict__ src_grid, const float4* __re
             __threadfence();
         }
     }
+}
+
+// The window search of one (PO2PO, STATS) instantiation, as the programmatic dependent of target_extents_kernel (see
+// griddepcontrol.wait in the kernel: its CTAs load their source lanes and start windows while the pre-pass is still
+// running), then the block search of the lanes it hands over.
+template <bool PO2PO, bool STATS>
+int launch_dense_search(const float4* src_grid, const float4* src_ngrid, const float* T, const float4* tgt_grid,
+                        const float4* tgt_ngrid, int B, int rows, int nbh, int nbw, int max_strips, const GridParams& g,
+                        uint32_t flags, const IcpScratch& sc, cudaStream_t st) {
+    const dim3 grid((g.H * g.W + kDenseThreads - 1) / kDenseThreads, B);
+    const cudaError_t e = launch_pdl(icp_dense_kernel<PO2PO, STATS>, grid, dim3(kDenseThreads), st, src_grid, src_ngrid,
+                                     T, tgt_grid, tgt_ngrid, max_strips, g, flags, sc.rows, rows, sc.pend, sc.ext);
+    DELORA_CHECK_LAUNCH_RESULT(e, "icp_dense_kernel");
+    // persistent block search: enough CTAs for one wave (up to 4 per SM), never more than there can be items
+    const int pend_grid = (int)std::min<long long>(((long long)B * rows * 32 + 7) / 8, 4ll * num_sms());
+    icp_dense_pending_kernel<PO2PO, STATS><<<pend_grid, kPendThreads, 0, st>>>(
+        src_grid, src_ngrid, T, tgt_grid, tgt_ngrid, sc.ext, nbh, nbw, g, flags, sc.rows, rows, sc.pend);
+    DELORA_CHECK_LAUNCH("icp_dense_pending_kernel");
+    return 0;
 }
 
 }  // namespace delora
@@ -769,66 +758,26 @@ extern "C" int delora_icp_dense_fwd_bwd(const delora_f4* src_grid, const delora_
                                         uint32_t flags, float* losses, float* grad_T, float* scratch, void* stream) {
     DELORA_CHECK_ARG(src_grid && src_ngrid && T && tgt_grid && tgt_ngrid && losses && grad_T && scratch,
                      "delora_icp_dense_fwd_bwd: null pointer");
-    DELORA_CHECK_ARG(B > 0 && B <= 65535 && H > 0 && W > 0, "delora_icp_dense_fwd_bwd: bad shape");
+    DELORA_CHECK_ARG(B > 0 && B <= 65535 && H > 0 && W > 0 && (long long)H * W < (1ll << 31),
+                     "delora_icp_dense_fwd_bwd: bad shape");
+    const IcpLayout L = icp_layout(B, H * W);
+    const int nbh = (H + kBlkH - 1) / kBlkH, nbw = (W + kBlkW - 1) / kBlkW;
+    DELORA_CHECK_ARG((int64_t)nbh * nbw <= L.blk_per_pair,
+                     "delora_icp_dense_fwd_bwd: H=%d W=%d needs %lld range-pyramid blocks per pair, the scratch holds %lld",
+                     H, W, (long long)nbh * nbw, (long long)L.blk_per_pair);
     const GridParams g = make_grid(H, W, hfov0, hfov1, vfov0, vfov1, 1);
-    const int HW = H * W;
-    const int rows = (HW + 31) / 32;                  // one partial row per warp of 32 source pixels
-    const IcpScratch sc = icp_scratch(scratch, B, rows);
-    dim3 grid((HW + kDenseThreads - 1) / kDenseThreads, B);
+    const IcpScratch sc = icp_scratch(scratch, L);
     cudaStream_t st = (cudaStream_t)stream;
     int max_strips = kDefaultMaxStrips;
     if (const char* e = getenv("DELORA_ICP_MAX_STRIPS")) max_strips = atoi(e);      // tuning knob (tests / profiling)
-    // scratch behind the partial rows / column sums / counters: the range pyramid of the TARGET grids, then the
-    // work list of the second kernel (see delora_icp_scratch_floats)
-    const int nbh = (H + kBlkH - 1) / kBlkH, nbw = (W + kBlkW - 1) / kBlkW;
-    size_t off = (size_t)B * rows * DELORA_ICP_PARTIAL + (size_t)B * DELORA_ICP_PARTIAL + (((size_t)B + 1) & ~(size_t)1);
-    TargetExtents ext;
-    ext.blk = reinterpret_cast<float2*>(scratch + off);
-    off += (size_t)B * 2 * ((size_t)HW / 16 + 4096);
-    ext.row_pre = reinterpret_cast<float2*>(scratch + off);
-    ext.row_suf = ext.row_pre + (size_t)B * H;
-    off += (size_t)B * 4 * H;
-    ext.counter = reinterpret_cast<int*>(scratch + off);
-    off += B;
-    off = (off + 3) & ~(size_t)3;                      // 16-byte alignment
-    PendingList pend;
-    pend.counters = reinterpret_cast<int*>(scratch + off);
-    pend.items = reinterpret_cast<int4*>(scratch + off + 4);
-    pend.entries = reinterpret_cast<float4*>(scratch + off + 4 + (size_t)4 * B * rows);
-    pend.item_done = reinterpret_cast<int*>(scratch + off + 4 + (size_t)4 * B * rows + (size_t)4 * B * rows * 32);
-    pend.result = pend.item_done + (size_t)B * rows;
-    // persistent second kernel: enough CTAs for one wave, never more than there can be items
-    const int pend_threads = kPendThreads, pend_mult = 4;     // up to 4 CTAs per SM
-    const int pend_grid = (int)std::min<long long>(((long long)B * rows * 32 + 7) / 8, (long long)pend_mult * num_sms());
-    // the window search is the programmatic dependent of the pre-pass (see griddepcontrol.wait in the kernel): its
-    // CTAs load their source lanes and start windows while the pre-pass is still running
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid;
-    cfg.blockDim = dim3(kDenseThreads);
-    cfg.dynamicSmemBytes = 0;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    target_extents_kernel<<<dim3(nbh, B), kExtThreads, 0, st>>>((const float4*)tgt_grid, H, W, nbh, nbw, ext);
+    target_extents_kernel<<<dim3(nbh, B), kExtThreads, 0, st>>>((const float4*)tgt_grid, H, W, nbh, nbw, sc.ext);
     DELORA_CHECK_LAUNCH("target_extents_kernel");
-#define DELORA_LAUNCH_DENSE(PO2PO, STATS)                                                                           \
-    do {                                                                                                            \
-        cudaLaunchKernelEx(&cfg, icp_dense_kernel<PO2PO, STATS>, (const float4*)src_grid, (const float4*)src_ngrid, \
-                           T, (const float4*)tgt_grid, (const float4*)tgt_ngrid, max_strips, g, flags, sc.rows,     \
-                           rows, pend, ext);                                                                        \
-        icp_dense_pending_kernel<PO2PO, STATS><<<pend_grid, pend_threads, 0, st>>>(                                 \
-            (const float4*)src_grid, (const float4*)src_ngrid, T, (const float4*)tgt_grid, (const float4*)tgt_ngrid, \
-            ext, nbh, nbw, g, flags, sc.rows, rows, pend);                                                          \
-    } while (0)
-    const bool po2po = (flags & DELORA_LOSS_PO2PO) != 0u, stats = (flags & DELORA_ICP_STATS) != 0u;
-    if (po2po && stats) DELORA_LAUNCH_DENSE(true, true);
-    else if (po2po) DELORA_LAUNCH_DENSE(true, false);
-    else if (stats) DELORA_LAUNCH_DENSE(false, true);
-    else DELORA_LAUNCH_DENSE(false, false);
-#undef DELORA_LAUNCH_DENSE
-    DELORA_CHECK_LAUNCH("icp_dense_kernel / icp_dense_pending_kernel");
-    return launch_icp_finalize(scratch, B, rows, lambda_po2pl, flags, losses, grad_T, st);
+    using DenseSearch = decltype(&launch_dense_search<false, false>);
+    constexpr DenseSearch kSearch[2][2] = {{launch_dense_search<false, false>, launch_dense_search<false, true>},
+                                           {launch_dense_search<true, false>, launch_dense_search<true, true>}};
+    const int rc = kSearch[(flags & DELORA_LOSS_PO2PO) != 0u][(flags & DELORA_ICP_STATS) != 0u](
+        (const float4*)src_grid, (const float4*)src_ngrid, T, (const float4*)tgt_grid, (const float4*)tgt_ngrid, B,
+        L.rows, nbh, nbw, max_strips, g, flags, sc, st);
+    if (rc != 0) return rc;
+    return launch_icp_finalize(sc, B, L.rows, lambda_po2pl, losses, grad_T, st);
 }

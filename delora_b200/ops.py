@@ -32,7 +32,9 @@ class nvtx_range:
         return False
 
 
+# include/delora_b200.h's DELORA_* constants (tests/test_icp_layout_cpu.py checks that they agree)
 LOSS_PO2PO, LOSS_PO2PL, LOSS_PL2PL, NORMAL_LINEAR = 1, 2, 4, 8
+ICP_STATS = 256      # DELORA_ICP_STATS flag bit
 LOSS_ROW, ICP_PARTIAL = 8, 40
 
 _keys_cache = {}
@@ -267,9 +269,6 @@ def icp_dense_fwd_bwd(src_grid, src_ngrid, transform, tgt_grid, tgt_ngrid, h, w,
         float(vfov[1]), float(lambda_po2pl), int(flags), losses.data_ptr(), grad_t.data_ptr(),
         scratch.data_ptr(), _stream()), "delora_icp_dense_fwd_bwd")
     return losses, grad_t
-
-
-ICP_STATS = 256      # DELORA_ICP_STATS flag bit
 
 
 def icp_stats(reset=True):

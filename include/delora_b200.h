@@ -187,10 +187,12 @@ int delora_pack_lists(const float* pts, const float* nrm, const int32_t* n, int 
  *                   kept (normal, normal) pair; (s - t) with w = 2 for a po2po pair; w = 0 otherwise
  * normal_dir        [B, src_stride] float4 out or NULL: unscaled d(pl2pl)/d(source normal)
  *                   (delora_icp_point_grads turns the two into the reference-shaped gradients)
- * scratch           fp32 [delora_icp_scratch_floats(B, src_stride)]: per-warp partial rows, column sums and
- *                   B int32 completion counters (+ the dense path's range pyramid and work list).  Zero it ONCE after
- *                   allocation; every call leaves the counters at zero again.  The layout depends on (B, src_stride):
- *                   a buffer that is reused with a different batch size or image size must be zeroed again first.
+ * scratch           fp32 [delora_icp_scratch_floats(B, src_stride)]: per-warp partial rows and their column sums, the
+ *                   dense path's work list (an int4 item per warp, a float4 entry and an int32 result per source point,
+ *                   an int32 count per warp) and range extents (float2 per 4 x 16-cell block and per pixel row), and
+ *                   int32 counters.  Zero it ONCE after allocation; every call leaves the counters at zero again.  The
+ *                   place and size of every section follow from (B, src_stride) alone: a buffer that is reused with a
+ *                   different batch size or image size must be zeroed again first.
  * The NN is the exact float64 Euclidean nearest neighbour (lowest tag on exact ties).
  */
 int     delora_icp_partial_rows(int src_stride);
@@ -210,7 +212,9 @@ int delora_icp_fwd_bwd(const delora_f4* src_pts4, const delora_f4* src_nrm4, con
  * list compaction nor a CSR index is needed.  This is the training-step fast path
  * (src/deploy/deployer.py:252-261 keeps exactly one point per pixel of both scans).
  * src_grid/src_ngrid, tgt_grid/tgt_ngrid: [B, H*W] float4;  T: [B, 12];
- * scratch: fp32 [delora_icp_scratch_floats(B, H*W)], zeroed once (see above).
+ * scratch: fp32 [delora_icp_scratch_floats(B, H*W)], zeroed once (see above).  Its range-pyramid section holds
+ * H*W/16 + 4096 blocks per pair; a grid that needs more, ceil(H/4) * ceil(W/16) (very tall and narrow grids such as
+ * W = 1 with H > 21844), is refused before any launch.
  * Launches target_extents_kernel (range extents of the target grids), icp_dense_kernel (window search, at most 32
  * growing steps per warp; the environment variable DELORA_ICP_MAX_STRIPS overrides the limit for profiling),
  * icp_dense_pending_kernel (range-pruned block search of the lanes still open) and icp_finalize_kernel; results do
