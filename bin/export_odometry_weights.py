@@ -21,10 +21,15 @@ from delora_b200.deploy import export as export_module  # noqa: E402
 @click.option("--max_batch", default=1, show_default=True, help="Max pairs per delora_odometry_pairs call.")
 @click.option("--config_dir", default="config", show_default=True, help="YAML files, used when the checkpoint has no "
               "`parameters`.")
-def main(checkpoint, dataset, out, n_stride, max_batch, config_dir):
-    d = export_module.export(checkpoint, dataset, out, n_stride, max_batch, config_dir)
+@click.option("--preprocessing-normals", "preprocessing_normals", is_flag=True, default=False,
+              help="Training through the C ABI estimates the normals at horizontal_cells_preprocessing and projects "
+                   "the points at the model width, as the reference's preprocessing + training does (w_pre in the "
+                   "header).  Off: normals at the model width.  Inference ignores it.")
+def main(checkpoint, dataset, out, n_stride, max_batch, config_dir, preprocessing_normals):
+    d = export_module.export(checkpoint, dataset, out, n_stride, max_batch, config_dir, preprocessing_normals)
     print(f"wrote {out}: {d.H}x{d.W}, layers {list(d.layers)}, act {'relu' if d.act == 1 else 'tanh'}, "
-          f"resnet_outputs {d.resnet_outputs}, single_mlp {d.single_mlp}, n_stride {d.n_stride}, max_batch {d.max_batch}")
+          f"resnet_outputs {d.resnet_outputs}, single_mlp {d.single_mlp}, n_stride {d.n_stride}, max_batch {d.max_batch}"
+          + (f", training normals at {d.H}x{d.w_pre}" if d.w_pre else ""))
 
 
 if __name__ == "__main__":

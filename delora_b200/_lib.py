@@ -15,7 +15,7 @@ class OdometryDesc(ctypes.Structure):
     """delora_odometry_desc (include/delora_b200.h): the model and buffer sizes of the odometry entry points."""
     _fields_ = [("H", c_int), ("W", c_int), ("hfov0", c_double), ("hfov1", c_double), ("vfov0", c_double),
                 ("vfov1", c_double), ("n_stride", c_int), ("max_batch", c_int), ("act", c_int),
-                ("layers", c_int * 4), ("resnet_outputs", c_int), ("single_mlp", c_int)]
+                ("layers", c_int * 4), ("resnet_outputs", c_int), ("single_mlp", c_int), ("w_pre", c_int)]
 
 
 class OdometryTrainParams(ctypes.Structure):
@@ -50,6 +50,8 @@ SIGNATURES = {
                                   c_double, c_double, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "delora_grids_from_projection": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                              c_void_p, c_void_p, c_void_p]),
+    "delora_project_grids_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_double, c_double, c_double,
+                                         c_double, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "delora_pack_lists": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "delora_icp_partial_rows": (c_int, [c_int]),
     "delora_icp_scratch_floats": (c_i64, [c_int, c_int]),

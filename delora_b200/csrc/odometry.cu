@@ -258,18 +258,20 @@ static void plan_model(const delora_odometry_desc* d, Model* m) {
 // layout, built from the sections below.  Every buffer starts on a 256-byte boundary.
 
 // The frame section: n_scans projected scans (depth keys, index map, clamped counts, fp32 images), n_cached cached
-// previous images and, with has_prev, one "has a previous frame" flag per cached image.
+// previous images and, with has_prev, one "has a previous frame" flag per cached image.  The depth keys are sized for
+// images key_w wide (>= W): the training step projects at the preprocessing width in them as well.
 struct Frames {
     size_t keys, keys_bytes, index_map, counts, images;
     size_t prev_image;                 // n_cached > 0 only
     size_t has_prev;                   // with has_prev only
 };
 
-static Frames plan_frames(const delora_odometry_desc* d, int n_scans, int n_cached, bool has_prev, size_t& off) {
+static Frames plan_frames(const delora_odometry_desc* d, int n_scans, int n_cached, bool has_prev, int key_w,
+                          size_t& off) {
     const size_t HW = (size_t)d->H * d->W;
     Frames f;
     memset(&f, 0, sizeof(f));
-    f.keys_bytes = (size_t)n_scans * HW * 8;
+    f.keys_bytes = (size_t)n_scans * d->H * key_w * 8;
     f.keys = take(off, f.keys_bytes);
     f.index_map = take(off, (size_t)n_scans * HW * 4);
     f.counts = take(off, (size_t)n_scans * 4);
@@ -353,7 +355,7 @@ static void make_infer_plan(const delora_odometry_desc* d, bool streams, InferPl
     const Model& m = p->m;
     const int MB = d->max_batch, nout = d->resnet_outputs;
     size_t off = 0;
-    p->f = streams ? plan_frames(d, MB, MB, true, off) : plan_frames(d, 2 * MB, 1, false, off);
+    p->f = streams ? plan_frames(d, MB, MB, true, d->W, off) : plan_frames(d, 2 * MB, 1, false, d->W, off);
     p->t.x_in = take(off, nhwc_bytes(MB, d->H, d->W, m.stem_fast ? 16 : 64));
     p->t.stem = take(off, nhwc_bytes(MB, d->H, m.w2, 64));
     size_t act[4][3];
@@ -834,7 +836,8 @@ extern "C" int delora_odometry_streams_reset(const delora_odometry_desc* d, cons
 }
 
 // ================================================================================================ training
-// delora_odometry_train_step: projection + normals of the 2B scans, the trunk forward keeping its activations (the
+// delora_odometry_train_step: projection + normals of the 2B scans (with w_pre > 0: at H x w_pre, then re-projected at
+// H x W by delora_project_grids_fwd), the trunk forward keeping its activations (the
 // kernel sequence of TensorCoreEncoder._forward_saving), the tail forward keeping its activations, the dense ICP
 // losses with dL/dT, the tail backward (below), the trunk backward (TensorCoreEncoder._backward), one Adam update of
 // the fp32 master blob and one re-prep of the bf16 filters from it.  Weight gradients land in a gradient blob with
@@ -1067,6 +1070,9 @@ struct TrainPlan {
     // trunk activations kept by the forward: 16- or 64-channel input, stem pre-activation, pool output + argmax,
     // per block conv1 output and block output, per downsampling block the downsample output
     Trunk t;
+    // w_pre > 0 only: the preprocessing projection of the 2 * max_batch scans at H x w_pre (image, index map and the
+    // dense grids with their normals), placed after every other buffer
+    size_t pre_image, pre_index_map, pre_pts_grid, pre_nrm_grid;
     // trunk backward: per stage two alternating data-gradient buffers + the conv1 gradient; strided blocks: the
     // downsample's gradient at the output size and (zero-upsample path) the upsampled conv1 gradient
     size_t g[4][3], gds[4], gu1[4], g_stem;
@@ -1087,7 +1093,8 @@ static void make_train_plan(const delora_odometry_desc* d, TrainPlan* tp) {
     tp->master = take(off, blob); tp->grad = take(off, blob); tp->adam_m = take(off, blob); tp->adam_v = take(off, blob);
     tp->ctr = take(off, 2 * sizeof(long long));
     tp->w = plan_weights(m, true, off);
-    tp->f = plan_frames(d, 2 * MB, 0, false, off);
+    // one key buffer serves both projections of a step, one after the other
+    tp->f = plan_frames(d, 2 * MB, 0, false, d->w_pre > W ? d->w_pre : W, off);
     tp->pts_grid = take(off, (size_t)2 * MB * HW * 16);
     tp->nrm_grid = take(off, (size_t)2 * MB * HW * 16);
     tp->icp = take(off, (size_t)delora_icp_scratch_floats(MB, HW) * 4);
@@ -1144,7 +1151,22 @@ static void make_train_plan(const delora_odometry_desc* d, TrainPlan* tp) {
         }
     }
     tp->wg_scratch = take(off, (size_t)wg * 4);
+    if (d->w_pre > 0) {
+        const size_t HWp = (size_t)H * d->w_pre;
+        tp->pre_image = take(off, (size_t)2 * MB * 4 * HWp * 4);
+        tp->pre_index_map = take(off, (size_t)2 * MB * HWp * 4);
+        tp->pre_pts_grid = take(off, (size_t)2 * MB * HWp * 16);
+        tp->pre_nrm_grid = take(off, (size_t)2 * MB * HWp * 16);
+    }
     tp->total = off;
+}
+
+// check_desc plus the field only training reads
+static int check_train_desc(const delora_odometry_desc* d, const char* who) {
+    if (check_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(d->w_pre == 0 || (d->w_pre >= 2 && (long long)d->H * d->w_pre < (1ll << 27)),
+                     "%s: w_pre=%d must be 0 or >= 2 with H * w_pre < 2^27 (H=%d)", who, d->w_pre, d->H);
+    return 0;
 }
 
 static int check_train_params(const delora_odometry_train_params* hp, const char* who) {
@@ -1306,7 +1328,7 @@ static int train_tail_backward(const TrainPlan& tp, char* ws, int act, int B, cu
 }  // namespace delora
 
 extern "C" int64_t delora_odometry_train_workspace_bytes(const delora_odometry_desc* d) {
-    if (check_desc(d, "delora_odometry_train_workspace_bytes")) return -1;
+    if (check_train_desc(d, "delora_odometry_train_workspace_bytes")) return -1;
     TrainPlan tp;
     make_train_plan(d, &tp);
     return (int64_t)tp.total;
@@ -1315,7 +1337,7 @@ extern "C" int64_t delora_odometry_train_workspace_bytes(const delora_odometry_d
 extern "C" int delora_odometry_train_init(const delora_odometry_desc* d, const float* weights, void* workspace,
                                           void* stream) {
     const char* who = "delora_odometry_train_init";
-    if (check_desc(d, who)) return 1;
+    if (check_train_desc(d, who)) return 1;
     DELORA_CHECK_ARG(weights && workspace, "%s: null pointer", who);
     TrainPlan tp;
     make_train_plan(d, &tp);
@@ -1333,7 +1355,7 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
                                           const float* points, const int32_t* n_points, int B, void* workspace,
                                           float* losses, float* T, float* pooled, float* grads, void* stream) {
     const char* who = "delora_odometry_train_step";
-    if (check_desc(d, who)) return 1;
+    if (check_train_desc(d, who)) return 1;
     if (check_train_params(hp, who)) return 1;
     DELORA_CHECK_ARG(points && n_points && workspace, "%s: null pointer", who);
     DELORA_CHECK_ARG(B >= 1 && B <= d->max_batch, "%s: B=%d outside [1, max_batch=%d]", who, B, d->max_batch);
@@ -1348,17 +1370,33 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
     int rc;
     cudaError_t e = cudaSuccess;
 
-    // 1. projection + normals of the 2B scans (scan_1 x B, then scan_2 x B)
+    // 1. projection + normals of the 2B scans (scan_1 x B, then scan_2 x B).  w_pre > 0: the reference's two stages,
+    // projection + normals at H x w_pre (its offline preprocessing), then those grids projected at H x W (Deployer.step)
     if ((rc = clamp_counts(tp.f, ws, n_points, nullptr, 2 * B, d->n_stride, st))) return rc;
     int32_t* counts = reinterpret_cast<int32_t*>(ws + tp.f.counts);
     delora_f4* pts_grid = reinterpret_cast<delora_f4*>(ws + tp.pts_grid);
     delora_f4* nrm_grid = reinterpret_cast<delora_f4*>(ws + tp.nrm_grid);
     float* images = f(tp.f.images);
-    if ((rc = delora_project_normals_fwd(points, counts, 2 * B, 3, d->n_stride, H, W, d->hfov0, d->hfov1, d->vfov0,
-                                         d->vfov1, 0, reinterpret_cast<uint64_t*>(ws + tp.f.keys), images,
-                                         reinterpret_cast<int32_t*>(ws + tp.f.index_map), hp->nb_h, hp->nb_w,
-                                         hp->epsilon_range, hp->min_neighbors, pts_grid, nrm_grid, nullptr, st)))
+    uint64_t* keys = reinterpret_cast<uint64_t*>(ws + tp.f.keys);
+    if (d->w_pre > 0) {
+        delora_f4* pre_pts = reinterpret_cast<delora_f4*>(ws + tp.pre_pts_grid);
+        delora_f4* pre_nrm = reinterpret_cast<delora_f4*>(ws + tp.pre_nrm_grid);
+        if ((rc = delora_project_normals_fwd(points, counts, 2 * B, 3, d->n_stride, H, d->w_pre, d->hfov0, d->hfov1,
+                                             d->vfov0, d->vfov1, 0, keys, f(tp.pre_image),
+                                             reinterpret_cast<int32_t*>(ws + tp.pre_index_map), hp->nb_h, hp->nb_w,
+                                             hp->epsilon_range, hp->min_neighbors, pre_pts, pre_nrm, nullptr, st)))
+            return rc;
+        if ((rc = delora_project_grids_fwd(pre_pts, pre_nrm, 2 * B, H, d->w_pre, W, d->hfov0, d->hfov1, d->vfov0,
+                                           d->vfov1, 0, keys, images, reinterpret_cast<int32_t*>(ws + tp.f.index_map),
+                                           pts_grid, nrm_grid, st)))
+            return rc;
+    } else if ((rc = delora_project_normals_fwd(points, counts, 2 * B, 3, d->n_stride, H, W, d->hfov0, d->hfov1,
+                                                d->vfov0, d->vfov1, 0, keys, images,
+                                                reinterpret_cast<int32_t*>(ws + tp.f.index_map), hp->nb_h, hp->nb_w,
+                                                hp->epsilon_range, hp->min_neighbors, pts_grid, nrm_grid, nullptr,
+                                                st))) {
         return rc;
+    }
     // 2. forward, keeping the activations
     if ((rc = trunk_input(m, tp.t, ws, images, images + (size_t)B * 4 * HW, B, st))) return rc;
     if ((rc = trunk_forward(m, tp.t, tp.w, true, ws, d->act, B, f(tp.pooled), st))) return rc;
@@ -1398,7 +1436,7 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
 extern "C" int delora_odometry_train_weights(const delora_odometry_desc* d, const void* workspace, float* weights,
                                              void* stream) {
     const char* who = "delora_odometry_train_weights";
-    if (check_desc(d, who)) return 1;
+    if (check_train_desc(d, who)) return 1;
     DELORA_CHECK_ARG(workspace && weights, "%s: null pointer", who);
     TrainPlan tp;
     make_train_plan(d, &tp);

@@ -8,6 +8,8 @@
 // pixel (equal ranges: lowest index wins == a stable sort); a second pass resolves the winners
 // into the image and the pixel -> point index map and re-arms the key buffer.  delora_project_normals_fwd
 // (normals.cu) runs the same scatter and resolves the keys inside its 7x11 normals kernel instead.
+// delora_project_grids_fwd re-projects the dense grids of such a projection at another width with the same per-point
+// arithmetic (project_pixel, depth_key in projection.cuh) and the same two passes.
 //
 // HBM/L2 traffic per scan: read 12 N (xyz) [+ 8 HW key RMW in L2] ; write 4 (C+1) HW + 4 HW.
 #include "projection.cuh"
@@ -44,17 +46,13 @@ project_scatter_kernel(const float* __restrict__ points, const int32_t* __restri
 #pragma unroll
     for (int i = 0; i < kScatterPPT; ++i) {
         const int idx = base + i * kScatterThreads;
-        float u, v;
-        pixel_coords(g, x[i], y[i], z[i], u, v);
-        const float ru = rintf(u), rv = rintf(v);            // torch.round: half to even (:74-77)
-        const bool inside = (idx < n) && (ru <= g.wm1) && (ru >= 0.0f) && (rv <= g.hm1) && (rv >= 0.0f);
-        if (inside) {
-            const unsigned rbits = __float_as_uint(range3(x[i], y[i], z[i]));
+        const int pix = project_pixel(g, x[i], y[i], z[i]);
+        if (idx < n && pix >= 0) {
             // One 64-bit atomicMin (a fire-and-forget RED at L2) per in-FOV point.  A match.any /
             // redux.min warp aggregation does not pay here: redux with per-group masks serialises
             // once per distinct pixel (~28 groups per warp at W = 2048), while 2 M atomics per step
             // are far below the L2 atomic rate.
-            atomicMin(kb + (int)rv * g.W + (int)ru, ((unsigned long long)rbits << 32) | (unsigned)idx);
+            atomicMin(kb + pix, depth_key(x[i], y[i], z[i], (unsigned)idx));
         }
     }
 }
@@ -159,6 +157,65 @@ void launch_project_scatter(const float* points, const int32_t* n_points, int B,
     project_scatter_kernel<<<grid, kScatterThreads, 0, st>>>(points, n_points, C, n_stride, g, keys);
 }
 
+// ---- delora_project_grids_fwd: the dense grids of a projection at one width, re-projected at another.
+// The preprocessing-resolution grids hold one point per pixel, and a valid cell's pixel id grows with its row-major
+// position, which is the point's index in the list delora_lists_from_images would make of them.  So the cell id serves
+// as the depth key's tie-break id, and the result is the list path's (lists -> delora_project_fwd ->
+// delora_grids_from_projection) without building the list.
+// Scatter: one atomicMin per valid cell, kScatterPPT independent 16-byte loads in flight per thread.
+__global__ void __launch_bounds__(kScatterThreads)
+grids_scatter_kernel(const float4* __restrict__ pts_pre, int HWp, GridParams g, unsigned long long* __restrict__ keys) {
+    const int b = blockIdx.y;
+    const int base = blockIdx.x * (kScatterThreads * kScatterPPT) + threadIdx.x;
+    const float4* __restrict__ pb = pts_pre + (size_t)b * HWp;
+    unsigned long long* __restrict__ kb = keys + (size_t)b * g.H * g.W;
+    float4 p[kScatterPPT];
+#pragma unroll
+    for (int i = 0; i < kScatterPPT; ++i) {
+        const int cell = base + i * kScatterThreads;
+        p[i] = cell < HWp ? __ldg(pb + cell) : make_float4(0.0f, 0.0f, 0.0f, __int_as_float(-1));
+    }
+#pragma unroll
+    for (int i = 0; i < kScatterPPT; ++i) {
+        if (__float_as_int(p[i].w) < 0) continue;                          // empty cell: (+inf, +inf, +inf, -1)
+        const int pix = project_pixel(g, p[i].x, p[i].y, p[i].z);
+        if (pix >= 0) atomicMin(kb + pix, depth_key(p[i].x, p[i].y, p[i].z, (unsigned)(base + i * kScatterThreads)));
+    }
+}
+
+// Resolve: one model pixel per thread.  The values and empty conventions of project_resolve_kernel<3> (image) and
+// grids_from_projection_kernel (grids); the index map holds the preprocessing cell of the kept point.
+__global__ void __launch_bounds__(256)
+grids_resolve_kernel(const float4* __restrict__ pts_pre, const float4* __restrict__ nrm_pre, int HWp, int HW,
+                     unsigned long long* __restrict__ keys, float* __restrict__ image, int32_t* __restrict__ index_map,
+                     float4* __restrict__ pts_grid, float4* __restrict__ nrm_grid) {
+    const int b = blockIdx.y, pix = blockIdx.x * 256 + threadIdx.x;
+    if (pix >= HW) return;
+    const size_t o = (size_t)b * HW + pix;
+    const unsigned long long k = keys[o];
+    keys[o] = kEmptyKey;                                                   // re-arm for the next call
+    const float inf = __int_as_float(0x7f800000);
+    float4 c = make_float4(0.0f, 0.0f, 0.0f, 0.0f), q = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    float rng = 0.0f;
+    int cell = -1;
+    if (k != kEmptyKey) {
+        cell = (int)(unsigned)(k & 0xffffffffull);
+        c = __ldg(pts_pre + (size_t)b * HWp + cell);
+        const float4 n = __ldg(nrm_pre + (size_t)b * HWp + cell);
+        const bool has = (n.x != 0.0f) | (n.y != 0.0f) | (n.z != 0.0f);    // icp_losses.py:48-52
+        q = make_float4(n.x, n.y, n.z, has ? 1.0f : 0.0f);
+        rng = __uint_as_float((unsigned)(k >> 32));
+    }
+    float* __restrict__ ib = image + (size_t)b * 4 * HW;
+    ib[pix] = c.x;
+    ib[HW + pix] = c.y;
+    ib[2 * (size_t)HW + pix] = c.z;
+    ib[3 * (size_t)HW + pix] = rng;
+    if (index_map) index_map[o] = cell;
+    pts_grid[o] = cell >= 0 ? make_float4(c.x, c.y, c.z, __int_as_float(pix)) : make_float4(inf, inf, inf, __int_as_float(-1));
+    nrm_grid[o] = q;
+}
+
 }  // namespace delora
 
 using namespace delora;
@@ -184,6 +241,30 @@ extern "C" int delora_project_fwd(const float* points, const int32_t* n_points, 
     else
         project_resolve_kernel<0><<<grid2, 256, 0, st>>>(points, C, n_stride, HW, (unsigned long long*)keys, image, index_map);
     DELORA_CHECK_LAUNCH("project_resolve_kernel");
+    return 0;
+}
+
+extern "C" int delora_project_grids_fwd(const delora_f4* pts_grid_pre, const delora_f4* nrm_grid_pre, int S, int H,
+                                        int Wp, int W, double hfov0, double hfov1, double vfov0, double vfov1,
+                                        int div_mode, uint64_t* keys, float* image, int32_t* index_map,
+                                        delora_f4* pts_grid, delora_f4* nrm_grid, void* stream) {
+    DELORA_CHECK_ARG(pts_grid_pre && nrm_grid_pre && keys && image && pts_grid && nrm_grid,
+                     "delora_project_grids_fwd: null pointer");
+    DELORA_CHECK_ARG(S > 0 && S <= 65535 && H > 0 && Wp > 0 && W > 0,
+                     "delora_project_grids_fwd: bad shape S=%d H=%d Wp=%d W=%d", S, H, Wp, W);
+    DELORA_CHECK_ARG((long long)H * Wp < (1ll << 31) && (long long)H * W < (1ll << 31),
+                     "delora_project_grids_fwd: image too large");
+    cudaStream_t st = (cudaStream_t)stream;
+    const GridParams g = make_grid(H, W, hfov0, hfov1, vfov0, vfov1, div_mode);
+    const int HWp = H * Wp, HW = H * W;
+    const int per_block = kScatterThreads * kScatterPPT;
+    grids_scatter_kernel<<<dim3((HWp + per_block - 1) / per_block, S), kScatterThreads, 0, st>>>(
+        (const float4*)pts_grid_pre, HWp, g, (unsigned long long*)keys);
+    DELORA_CHECK_LAUNCH("grids_scatter_kernel");
+    grids_resolve_kernel<<<dim3((HW + 255) / 256, S), 256, 0, st>>>(
+        (const float4*)pts_grid_pre, (const float4*)nrm_grid_pre, HWp, HW, (unsigned long long*)keys, image, index_map,
+        (float4*)pts_grid, (float4*)nrm_grid);
+    DELORA_CHECK_LAUNCH("grids_resolve_kernel");
     return 0;
 }
 

@@ -19,8 +19,9 @@ from .. import _lib
 MAGIC = b"DELORAW\x00"
 HEADER_BYTES = 128
 # magic, abi_version, header_bytes | H, W, hfov0, hfov1, vfov0, vfov1 | n_stride, max_batch, act, layers[4],
-# resnet_outputs, single_mlp, 4 pad bytes | blob_floats | 24 reserved bytes
-_HEADER = struct.Struct("<8sii" + "ii4d" + "iii4iii4x" + "q" + "24x")
+# resnet_outputs, single_mlp, w_pre (byte 92; files written before the field have zeros there) | blob_floats |
+# 24 reserved bytes
+_HEADER = struct.Struct("<8sii" + "ii4d" + "iii4iiii" + "q" + "24x")
 assert _HEADER.size == HEADER_BYTES
 
 
@@ -51,8 +52,10 @@ def check_supported(config):
         raise ValueError(f"activation_fct: {config.get('activation_fct')!r} must be 'relu' or 'tanh'")
 
 
-def desc_from_config(config, dataset, n_stride, max_batch=1):
-    """-> _lib.OdometryDesc for the model of `config` on `dataset`'s range image."""
+def desc_from_config(config, dataset, n_stride, max_batch=1, preprocessing_normals=False):
+    """-> _lib.OdometryDesc for the model of `config` on `dataset`'s range image.
+    preprocessing_normals: train through the C ABI on the reference's recipe, normals estimated at
+    `horizontal_cells_preprocessing` (w_pre); otherwise at the model width (w_pre = 0)."""
     check_supported(config)
     ds = config[dataset]
     layers = [int(v) for v in config["layers"]]
@@ -67,6 +70,10 @@ def desc_from_config(config, dataset, n_stride, max_batch=1):
     d.layers[:] = layers
     d.resnet_outputs = int(config["resnet_outputs"])
     d.single_mlp = 1 if config["use_single_mlp_at_output"] else 0
+    if preprocessing_normals:
+        if "horizontal_cells_preprocessing" not in ds:
+            raise ValueError(f"{dataset}: horizontal_cells_preprocessing is needed for preprocessing_normals")
+        d.w_pre = int(ds["horizontal_cells_preprocessing"])
     return d
 
 
@@ -120,7 +127,7 @@ def write_dlw(path, desc, blob):
     blob = np.ascontiguousarray(blob, dtype=np.float32)
     header = _HEADER.pack(MAGIC, _lib.ABI_VERSION, HEADER_BYTES, desc.H, desc.W, desc.hfov0, desc.hfov1, desc.vfov0,
                           desc.vfov1, desc.n_stride, desc.max_batch, desc.act, *list(desc.layers), desc.resnet_outputs,
-                          desc.single_mlp, blob.size)
+                          desc.single_mlp, desc.w_pre, blob.size)
     with open(path, "wb") as f:
         f.write(header)
         f.write(blob.tobytes())
@@ -137,24 +144,24 @@ def read_dlw(path):
             raise ValueError(f"{path}: not an odometry weight file (magic {v[0]!r})")
         blob = np.fromfile(f, dtype=np.float32)
     names = ("magic", "abi_version", "header_bytes", "H", "W", "hfov0", "hfov1", "vfov0", "vfov1", "n_stride",
-             "max_batch", "act", "l0", "l1", "l2", "l3", "resnet_outputs", "single_mlp", "blob_floats")
+             "max_batch", "act", "l0", "l1", "l2", "l3", "resnet_outputs", "single_mlp", "w_pre", "blob_floats")
     h = dict(zip(names, v))
     h["layers"] = [h.pop("l0"), h.pop("l1"), h.pop("l2"), h.pop("l3")]
     if blob.size != h["blob_floats"]:
         raise ValueError(f"{path}: blob has {blob.size} floats, the header says {h['blob_floats']}")
     d = _lib.OdometryDesc()
     for k in ("H", "W", "hfov0", "hfov1", "vfov0", "vfov1", "n_stride", "max_batch", "act", "resnet_outputs",
-              "single_mlp"):
+              "single_mlp", "w_pre"):
         setattr(d, k, h[k])
     d.layers[:] = h["layers"]
     return h, d, blob
 
 
-def export(checkpoint_path, dataset, out_path, n_stride, max_batch=1, config_dir="config"):
+def export(checkpoint_path, dataset, out_path, n_stride, max_batch=1, config_dir="config", preprocessing_normals=False):
     """Checkpoint (torch.save of the trainer's dict, or a bare state dict with `config_dir` YAMLs) -> .dlw file."""
     ckpt = torch.load(checkpoint_path, map_location="cpu", weights_only=False)
     config = model_config(ckpt, config_dir)
     state = ckpt["model_state_dict"] if isinstance(ckpt, dict) and "model_state_dict" in ckpt else ckpt
-    desc = desc_from_config(config, dataset, n_stride, max_batch)
+    desc = desc_from_config(config, dataset, n_stride, max_batch, preprocessing_normals)
     write_dlw(out_path, desc, pack_state_dict(state, config))
     return desc

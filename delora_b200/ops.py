@@ -204,6 +204,30 @@ def grids_from_projection(points, normal_lists, index_map):
     return pg, ng
 
 
+def project_grids(pts_grid_pre, nrm_grid_pre, h, w_pre, w, hfov, vfov, div_mode=0, index_map=True):
+    """Dense grids [S,H*w_pre,4] of a projection at H x w_pre (from project_normals / normals(grids=True)) re-projected
+    at H x w: -> image [S,4,H,W], index_map [S,H,W] int32 (the H x w_pre cell of the kept point; None with
+    index_map=False), pts_grid, nrm_grid [S,HW,4].  Bit-identical to lists_from_images -> project ->
+    grids_from_projection on the same scans."""
+    s = pts_grid_pre.shape[0]
+    if tuple(pts_grid_pre.shape) != (s, h * w_pre, 4) or tuple(nrm_grid_pre.shape) != (s, h * w_pre, 4):
+        raise ValueError(f"project_grids: grids must be [S, {h}*{w_pre}, 4], got {tuple(pts_grid_pre.shape)} and "
+                         f"{tuple(nrm_grid_pre.shape)}")
+    dev = pts_grid_pre.device
+    image = torch.empty((s, 4, h, w), dtype=torch.float32, device=dev)
+    imap = torch.empty((s, h, w), dtype=torch.int32, device=dev) if index_map else None
+    pg = torch.empty((s, h * w, 4), dtype=torch.float32, device=dev)
+    ng = torch.empty((s, h * w, 4), dtype=torch.float32, device=dev)
+    keys = _keys(dev, s, h * w)
+    L = _lib.lib()
+    _lib.check(L.delora_project_grids_fwd(_req(pts_grid_pre, torch.float32, "pts_grid_pre"),
+                                          _req(nrm_grid_pre, torch.float32, "nrm_grid_pre"), s, h, w_pre, w,
+                                          float(hfov[0]), float(hfov[1]), float(vfov[0]), float(vfov[1]), int(div_mode),
+                                          keys.data_ptr(), image.data_ptr(), imap.data_ptr() if index_map else None,
+                                          pg.data_ptr(), ng.data_ptr(), _stream()), "delora_project_grids_fwd")
+    return image, imap, pg, ng
+
+
 def pack_lists(pts, nrm, n):
     b, _, ns = pts.shape
     pts4 = torch.empty((b, ns, 4), dtype=torch.float32, device=pts.device)

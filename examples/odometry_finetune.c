@@ -8,6 +8,8 @@
  * consecutive pairs (scan k, scan k+1), min(max_batch, pairs) pairs per step, cycling through the list, and writes the
  * updated weights to out.dlw (same header).  Prints the objective (mean over the step's pairs of
  * po2po + lambda * po2pl + pl2pl, before that step's update) once per step.  No ground truth is needed.
+ * The normals the losses use are estimated at the resolution the header's w_pre names (export with
+ * --preprocessing-normals for the reference's recipe); the program says which on stderr.
  *
  * Build:  cc odometry_finetune.c -I include -I $CUDA_HOME/include -L delora_b200 -ldelora_b200 \
  *            -L $CUDA_HOME/lib64 -lcudart -Wl,-rpath,$PWD/delora_b200 -o odometry_finetune
@@ -89,6 +91,13 @@ int main(int argc, char** argv) {
             return fail("cannot read a scan (missing, truncated, or more points than n_stride)");
     const int n_pairs = n_scans - 1;
     const int B = n_pairs < d->max_batch ? n_pairs : d->max_batch;
+    /* the header's w_pre chooses the objective: 0 = normals at the model's H x W, as the projection the model sees;
+     * > 0 = the reference's recipe (normals at H x w_pre, the points then projected at H x W) */
+    if (d->w_pre > 0)
+        fprintf(stderr, "odometry_finetune: normals at the preprocessing resolution %dx%d, images at %dx%d\n", d->H,
+                d->w_pre, d->H, d->W);
+    else
+        fprintf(stderr, "odometry_finetune: normals at the model resolution %dx%d\n", d->H, d->W);
 
     delora_odometry_train_params hp;
     hp.lr = lr; hp.beta1 = 0.9f; hp.beta2 = 0.999f; hp.eps = 1e-8f;

@@ -160,6 +160,26 @@ int delora_grids_from_projection(const float* points, const float* normal_lists,
                                  int B, int C, int n_stride, int H, int W,
                                  delora_f4* pts_grid, delora_f4* nrm_grid, void* stream);
 
+/* The reference's two-resolution training data in one call: the dense grids of S scans projected at H x Wp, as
+ * delora_normals_fwd / delora_project_normals_fwd write them, re-projected at H x W.  This is the preprocessing stage
+ * (src/preprocessing/preprocesser.py: projection and normals at horizontal_cells_preprocessing, the valid pixels stored
+ * in row-major order) followed by the training stage's projection of those stored points at the model width
+ * (src/deploy/deployer.py:252-261).  The result is bit-identical to
+ *   delora_lists_from_images -> channels-first lists -> delora_project_fwd at H x W with C = 3 ->
+ *   delora_grids_from_projection,
+ * without building the lists: a valid cell's pixel id grows with its list index, so equal ranges in one model pixel
+ * go to the same point ("lowest point index wins").
+ * pts_grid_pre, nrm_grid_pre  [S, H*Wp] float4: valid cells (x, y, z, bits(pixel id)), empty (+inf, +inf, +inf, -1)
+ * keys       [S, H*W] uint64 scratch, all-ones on entry and on exit (as for delora_project_fwd)
+ * image      [S, 4, H, W] fp32 out: x, y, z of the kept point and its range; empty pixels are 0
+ * index_map  [S, H, W] int32 out or NULL: the H x Wp cell of the kept point, -1 if empty
+ * pts_grid, nrm_grid  [S, H*W] float4 out, as delora_grids_from_projection writes them: w = bits(model pixel id),
+ *            has-normal = normal non-zero
+ * hfov/vfov, div_mode as for delora_project_fwd. */
+int delora_project_grids_fwd(const delora_f4* pts_grid_pre, const delora_f4* nrm_grid_pre, int S, int H, int Wp, int W,
+                             double hfov0, double hfov1, double vfov0, double vfov1, int div_mode, uint64_t* keys,
+                             float* image, int32_t* index_map, delora_f4* pts_grid, delora_f4* nrm_grid, void* stream);
+
 /* Pack channels-first lists to float4 (no sorting): pts4.w = bits(list index), nrm4.w = has_normal. */
 int delora_pack_lists(const float* pts, const float* nrm, const int32_t* n, int B, int n_stride,
                       delora_f4* pts4, delora_f4* nrm4, void* stream);
@@ -384,12 +404,18 @@ typedef struct {
     int layers[4];                       /* BasicBlocks per stage, e.g. {2,2,2,2} (1 .. 16 each) */
     int resnet_outputs;                  /* fc width, 1000 in the shipped config */
     int single_mlp;                      /* use_single_mlp_at_output (0 / 1) */
+    int w_pre;                           /* training only: horizontal_cells_preprocessing, the width the normals are
+                                            estimated at (0: at W).  Read and validated by the delora_odometry_train_*
+                                            entry points alone: 0, or >= 2 with H * w_pre < 2^27.  Training callers
+                                            must zero it (or copy the descriptor from a .dlw header); inference and
+                                            streams callers may leave it uninitialised. */
 } delora_odometry_desc;
 
 /* Weight file (.dlw, written by delora_b200/deploy/export.py), little-endian, readable with fread alone:
  *   bytes   0..127  delora_odometry_file_header below (explicit offsets: magic 0, abi_version 8, header_bytes 12,
  *                   desc 16: H 16, W 20, hfov0 24, hfov1 32, vfov0 40, vfov1 48, n_stride 56, max_batch 60, act 64,
- *                   layers 68..83, resnet_outputs 84, single_mlp 88, 4 pad bytes; blob_floats 96; zero 104..127)
+ *                   layers 68..83, resnet_outputs 84, single_mlp 88, w_pre 92; blob_floats 96; zero 104..127;
+ *                   exporters before w_pre wrote zeros at 92, i.e. w_pre = 0)
  *   bytes 128..     float32[blob_floats]: the tensors of OdometryModel.state_dict() concatenated in state_dict order,
  *                   each tensor row-major (the blob delora_odometry_load_weights takes). */
 #define DELORA_ODOMETRY_FILE_MAGIC "DELORAW"     /* 7 characters + NUL = the 8 magic bytes */
@@ -465,6 +491,18 @@ int delora_odometry_streams_reset(const delora_odometry_desc* d, const int32_t* 
  *   encoder), one Adam update (no weight decay) of the fp32 master weights and one re-prep of the bf16 filters.
  * Same descriptor and .dlw blob as inference; the same models are not representable.
  *
+ * Normals (d->w_pre).  0: the normals are estimated on the model's H x W image (SyntheticTrainStep's shortcut).
+ * > 0: the reference's recipe -- its offline stage (src/preprocessing/preprocesser.py) projects each scan at
+ * horizontal_cells_preprocessing and estimates the normals there, its training stage (src/deploy/deployer.py:252-261)
+ * projects the stored points at the model width.  Each step runs delora_project_normals_fwd of the 2B scans at
+ * H x w_pre (nb_h, nb_w, epsilon_range, min_neighbors of the step), then delora_project_grids_fwd to H x W; the trunk
+ * onward is unchanged.  The workspace gains, after every other section, the image, index map and both grids at
+ * H x w_pre for 2 * max_batch scans (2 * max_batch * H * w_pre * 52 bytes, each buffer 256-byte aligned), and its
+ * one depth-key buffer grows to max(W, w_pre) columns; nothing moves at w_pre = 0.  At 64 x 720, n_stride 131072,
+ * w_pre 0 -> 2250: 325.2 -> 341.0 MiB (max_batch 1), 521.3 -> 584.4 MiB (4), 1305.9 -> 1558.3 MiB (16).  Measured
+ * step cost on one H100 80GB HBM3 at a 700 W power limit (graph-replayed steps, paired differences): within the
+ * noise (< 0.02 ms) at B = 1, +0.10 ms at B = 4, +0.38 ms at B = 16 (14.35 -> 14.70 ms).
+ *
  * Workspace: one caller-owned device buffer of delora_odometry_train_workspace_bytes(d) bytes holds the fp32 master
  * weights, their gradient, Adam's m, v and step count, the bf16 filters, every saved activation and backward buffer
  * for max_batch pairs and the ICP scratch.  Its layout is a function of the descriptor (the split-K scratch of the
@@ -482,7 +520,8 @@ typedef struct {
     int min_neighbors;                   /* min_num_points_in_neighborhood_to_determine_point_class, 10 */
 } delora_odometry_train_params;
 
-/* Host only (no GPU needed): -1 (and delora_last_error()) for an invalid descriptor. */
+/* Host only (no GPU needed): -1 (and delora_last_error()) for an invalid descriptor, w_pre included.  The four
+ * training entry points refuse a w_pre other than 0 or >= 2 with H * w_pre < 2^27, naming the field. */
 int64_t delora_odometry_train_workspace_bytes(const delora_odometry_desc* d);
 /* Zero the workspace, set the projection key buffer to all ones, copy `weights` (DEVICE fp32, the .dlw blob) into the
  * master weights, zero Adam's m, v and step count and prep the bf16 filters (fprop and flipped layouts).  The prep

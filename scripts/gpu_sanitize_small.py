@@ -31,6 +31,9 @@ p4, n4, cs, cnt = ops.lists_from_images(image, nrm)
 T = t_pred[:3, :].reshape(1, 12).contiguous().cuda()
 ops.icp_fwd_bwd(p4[1:2].contiguous(), n4[1:2].contiguous(), cnt[1:2].contiguous(), T, p4[0:1].contiguous(),
                 n4[0:1].contiguous(), cs[0:1].contiguous(), h, w, hf, vfr, pointwise=True)
+# grids at 16 x 200 re-projected at 16 x 180 (delora_project_grids_fwd: scatter + resolve)
+_, _, pg200, ng200 = ops.project_normals(pts, n, h, 200, hf, vfr)
+ops.project_grids(pg200, ng200, h, 200, w, hf, vfr)
 q = torch.randn(4, 4, device="cuda")
 ops.quat_to_T_bwd(q, torch.randn(4, 16, device="cuda"))
 torch.cuda.synchronize()
