@@ -847,7 +847,9 @@ extern "C" int delora_odometry_streams_reset(const delora_odometry_desc* d, cons
 // New kernels (fp32, fixed summation order, no atomics: bit-identical from run to run):
 //   odometry_out_bwd_kernel (one CTA): grad_T / B -> quaternion -> T backward (quat_to_T_bwd_row, shared with
 //     quat_to_T_bwd_kernel) -> backward of the division by the norm of the whole [B, 4] block (all rows coupled) ->
-//     d(head outputs) [B, 7]; the last Linear of each head (dW, db) and d(hidden) * act'.
+//     d(head outputs) [B, 7]; the last Linear of each head (dW, db) and d(hidden) * act'.  With
+//     DELORA_LOSS_IDENTITY_FIT its dL/dT is the identity fit's, 2 (T - I) / (16 B) on the last row, taken from the
+//     forward's T, and thread 0 writes that objective (an ordered sum over the 16 entries) to losses[B-1][5].
 //   odometry_linear_bwd_kernel: y = act(W x + b) backward for up to two layers that read the same x (the heads'
 //     hidden layers: their contributions to dx are summed in a fixed order), dW / db and dx * act'(x) in one launch.
 //   odometry_adam_kernel: torch's Adam (fused formula, no weight decay) over the whole blob, float4 per thread; the
@@ -946,7 +948,10 @@ struct OutBwd {
     float *gw_rot, *gb_rot, *gw_trans, *gb_trans;
     float* dz;                         // [B, ldz] out: gradient w.r.t. the hidden layer's pre-activation
     long long* ctr;                    // [0] Adam's step count, [1] the batch size of the ICP scratch
+    const float* T16;                  // [B, 16] the forward's T (read in the identity fit only)
+    float* losses;                     // [B, DELORA_LOSS_ROW]: the identity fit writes its objective to [B-1][5]
     int K, ldx, ldz, single;
+    int identity;                      // DELORA_LOSS_IDENTITY_FIT: objective MSELoss(T_{B-1}, I) / B, not the ICP mean
 };
 
 __global__ void __launch_bounds__(kBwdThreads)
@@ -959,14 +964,31 @@ odometry_out_bwd_kernel(OutBwd a, int B, float inv_B, int act) {
         for (int b = 0; b < B; ++b)
             for (int j = 0; j < 4; ++j) ss = fmaf(raw[b * 7 + j], raw[b * 7 + j], ss);
         s_red[0] = sqrtf(ss);
+        if (a.identity) {                                   // mean over the 16 entries of the last pair's T - I
+            const float* t = a.T16 + (size_t)(B - 1) * 16;
+            float se = 0.0f;
+            for (int i = 0; i < 16; ++i) {
+                const float e = t[i] - (i % 5 == 0 ? 1.0f : 0.0f);
+                se = fmaf(e, e, se);
+            }
+            a.losses[(size_t)(B - 1) * DELORA_LOSS_ROW + 5] = se * (1.0f / 16.0f) * inv_B;
+        }
     }
     __syncthreads();
     const float nrm = s_red[0];
     for (int b = threadIdx.x; b < B; b += blockDim.x) {
         const float* q = raw + b * 7;
         float g[12];
+        if (a.identity) {
+            // d(MSELoss(T_{B-1}, I) / B) = 2 (T - I) / 16 / B on the 3x4 part of the last row (the reference overwrites
+            // its loss inside the pair loop, so only the last pair counts), zero elsewhere
 #pragma unroll
-        for (int i = 0; i < 12; ++i) g[i] = a.grad_T[(size_t)b * 12 + i] * inv_B;    // d(mean over pairs)
+            for (int i = 0; i < 12; ++i)
+                g[i] = b == B - 1 ? 0.125f * (a.T16[(size_t)b * 16 + i] - (i % 5 == 0 ? 1.0f : 0.0f)) * inv_B : 0.0f;
+        } else {
+#pragma unroll
+            for (int i = 0; i < 12; ++i) g[i] = a.grad_T[(size_t)b * 12 + i] * inv_B;    // d(mean over pairs)
+        }
         quat_to_T_bwd_row(q[0] / nrm, q[1] / nrm, q[2] / nrm, q[3] / nrm, g, s_d + b * 7, s_d + b * 7 + 4);
     }
     __syncthreads();
@@ -1268,7 +1290,7 @@ static int linear_bwd(const TailGrad& p0, const TailGrad& p1, int B, int act_in,
     return 0;
 }
 
-static int train_tail_backward(const TrainPlan& tp, char* ws, int act, int B, cudaStream_t st) {
+static int train_tail_backward(const TrainPlan& tp, char* ws, int act, int B, bool identity, cudaStream_t st) {
     const Model& m = tp.m;
     auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
     const float* master = f(tp.master);
@@ -1277,6 +1299,7 @@ static int train_tail_backward(const TrainPlan& tp, char* ws, int act, int B, cu
     OutBwd a;
     memset(&a, 0, sizeof(a));
     a.raw = f(tp.raw); a.grad_T = f(tp.grad_T); a.ctr = reinterpret_cast<long long*>(ws + tp.ctr);
+    a.T16 = f(tp.T16); a.losses = f(tp.losses); a.identity = identity ? 1 : 0;
     if (m.n_lin == 4) {
         a.K = kHeadHidden; a.ldx = a.ldz = 2 * kHeadHidden; a.single = 0;
         a.w_rot = master + m.lin[1].blob_w; a.w_trans = master + m.lin[3].blob_w;
@@ -1401,7 +1424,9 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
     if ((rc = trunk_input(m, tp.t, ws, images, images + (size_t)B * 4 * HW, B, st))) return rc;
     if ((rc = trunk_forward(m, tp.t, tp.w, true, ws, d->act, B, f(tp.pooled), st))) return rc;
     if ((rc = run_tail(m, train_tail_io(tp, ws), d->act, f(tp.pooled), B, f(tp.T16), st))) return rc;
-    // 3. ICP losses and dL/dT: source = scan_2 moved by T, target = scan_1
+    // 3. ICP losses and dL/dT: source = scan_2 moved by T, target = scan_1.  The identity fit still runs them: the
+    // reference logs the ICP losses in that phase too
+    const bool identity = (hp->loss_flags & DELORA_LOSS_IDENTITY_FIT) != 0u;
     e = cudaMemcpy2DAsync(f(tp.T12), 12 * sizeof(float), f(tp.T16), 16 * sizeof(float), 12 * sizeof(float), B,
                           cudaMemcpyDeviceToDevice, st);
     DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
@@ -1409,10 +1434,11 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
     odometry_icp_rearm_kernel<<<2 * num_sms(), 256, 0, st>>>(reinterpret_cast<float4*>(ws + tp.icp), icp_n4, B, ctr);
     DELORA_CHECK_LAUNCH("odometry_icp_rearm_kernel");
     if ((rc = delora_icp_dense_fwd_bwd(pts_grid + (size_t)B * HW, nrm_grid + (size_t)B * HW, f(tp.T12), pts_grid, nrm_grid,
-                                       B, H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, hp->lambda_po2pl, hp->loss_flags,
-                                       f(tp.losses), f(tp.grad_T), f(tp.icp), st))) return rc;
-    // 4. backward: tail, average pool, trunk
-    if ((rc = train_tail_backward(tp, ws, d->act, B, st))) return rc;
+                                       B, H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, hp->lambda_po2pl,
+                                       hp->loss_flags & ~DELORA_LOSS_IDENTITY_FIT, f(tp.losses), f(tp.grad_T), f(tp.icp),
+                                       st))) return rc;
+    // 4. backward: tail (dL/dT of the ICP mean or of the identity fit), average pool, trunk
+    if ((rc = train_tail_backward(tp, ws, d->act, B, identity, st))) return rc;
     if ((rc = train_trunk_backward(tp, ws, d->act, B, st))) return rc;
     // outputs (T: the weights before the update)
     auto out = [&](float* dst, size_t src, size_t n) {
@@ -1444,4 +1470,53 @@ extern "C" int delora_odometry_train_weights(const delora_odometry_desc* d, cons
                                           cudaMemcpyDeviceToDevice, (cudaStream_t)stream);
     DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
     return 0;
+}
+
+extern "C" int delora_odometry_train_get_state(const delora_odometry_desc* d, const void* workspace, float* weights,
+                                               float* exp_avg, float* exp_avg_sq, int64_t* step, void* stream) {
+    const char* who = "delora_odometry_train_get_state";
+    if (check_train_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    TrainPlan tp;
+    make_train_plan(d, &tp);
+    const char* ws = (const char*)workspace;
+    const size_t blob = (size_t)tp.m.blob_floats * 4;
+    cudaError_t e = cudaSuccess;
+    auto out = [&](void* dst, size_t src, size_t bytes) {
+        if (dst && e == cudaSuccess) e = cudaMemcpyAsync(dst, ws + src, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream);
+    };
+    out(weights, tp.master, blob);
+    out(exp_avg, tp.adam_m, blob);
+    out(exp_avg_sq, tp.adam_v, blob);
+    out(step, tp.ctr, sizeof(long long));
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+    return 0;
+}
+
+extern "C" int delora_odometry_train_set_state(const delora_odometry_desc* d, const float* weights, const float* exp_avg,
+                                               const float* exp_avg_sq, const int64_t* step, void* workspace,
+                                               void* stream) {
+    const char* who = "delora_odometry_train_set_state";
+    if (check_train_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(weights, "%s: null weights", who);
+    DELORA_CHECK_ARG(exp_avg, "%s: null exp_avg", who);
+    DELORA_CHECK_ARG(exp_avg_sq, "%s: null exp_avg_sq", who);
+    DELORA_CHECK_ARG(step, "%s: null step", who);
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    TrainPlan tp;
+    make_train_plan(d, &tp);
+    char* ws = (char*)workspace;
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t blob = (size_t)tp.m.blob_floats * 4;
+    cudaError_t e = cudaSuccess;
+    auto in = [&](size_t dst, const void* src, size_t bytes) {
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ws + dst, src, bytes, cudaMemcpyDeviceToDevice, st);
+    };
+    in(tp.master, weights, blob);
+    in(tp.adam_m, exp_avg, blob);
+    in(tp.adam_v, exp_avg_sq, blob);
+    in(tp.ctr, step, sizeof(long long));            // ctr[0] only: ctr[1], the ICP scratch's batch size, stays
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+    // the bf16 filters from the new master weights, through the table _train_init wrote
+    return delora_conv_weight_prep_multi(ws + tp.w.table, tp.m.n_conv, st);
 }

@@ -6,8 +6,13 @@ alone and hands the blob to `delora_odometry_load_weights`.  The network configu
 `parameters` dict when it carries one (it wins over the YAML files, as in bin/run_testing.py), otherwise from
 `config/*.yaml` (angles there are in degrees).  Checkpoints of models the C ABI cannot express are refused:
 `pre_feature_extraction: True` and `factor_fewer_resnet_channels != 1`; dropout is the identity at inference.
+
+A .dlt file is a training checkpoint for `delora_odometry_train_set_state`: a 256-byte header (the .dlw header with
+its own magic, then Adam's step count, the epoch, the phase, Adam's hyperparameters and the last epoch loss) followed
+by the weights, Adam's exp_avg and exp_avg_sq.  It converts both ways to the reference Trainer's checkpoint dict.
 """
 import collections
+import dataclasses
 import os
 import struct
 
@@ -123,45 +128,238 @@ def unpack_blob(blob, config):
     return state
 
 
+def _pack_header(magic, header_bytes, desc, blob_floats):
+    return _HEADER.pack(magic, _lib.ABI_VERSION, header_bytes, desc.H, desc.W, desc.hfov0, desc.hfov1, desc.vfov0,
+                        desc.vfov1, desc.n_stride, desc.max_batch, desc.act, *list(desc.layers), desc.resnet_outputs,
+                        desc.single_mlp, desc.w_pre, blob_floats)
+
+
+def _unpack_header(raw, path, magic, what):
+    """The first 128 bytes of a .dlw / .dlt file -> (header dict, desc)."""
+    if len(raw) != HEADER_BYTES:
+        raise ValueError(f"{path}: truncated header")
+    v = _HEADER.unpack(raw)
+    if v[0] != magic:
+        raise ValueError(f"{path}: not an odometry {what} file (magic {v[0]!r})")
+    names = ("magic", "abi_version", "header_bytes", "H", "W", "hfov0", "hfov1", "vfov0", "vfov1", "n_stride",
+             "max_batch", "act", "l0", "l1", "l2", "l3", "resnet_outputs", "single_mlp", "w_pre", "blob_floats")
+    h = dict(zip(names, v))
+    h["layers"] = [h.pop("l0"), h.pop("l1"), h.pop("l2"), h.pop("l3")]
+    d = _lib.OdometryDesc()
+    for k in ("H", "W", "hfov0", "hfov1", "vfov0", "vfov1", "n_stride", "max_batch", "act", "resnet_outputs",
+              "single_mlp", "w_pre"):
+        setattr(d, k, h[k])
+    d.layers[:] = h["layers"]
+    return h, d
+
+
 def write_dlw(path, desc, blob):
     blob = np.ascontiguousarray(blob, dtype=np.float32)
-    header = _HEADER.pack(MAGIC, _lib.ABI_VERSION, HEADER_BYTES, desc.H, desc.W, desc.hfov0, desc.hfov1, desc.vfov0,
-                          desc.vfov1, desc.n_stride, desc.max_batch, desc.act, *list(desc.layers), desc.resnet_outputs,
-                          desc.single_mlp, desc.w_pre, blob.size)
     with open(path, "wb") as f:
-        f.write(header)
+        f.write(_pack_header(MAGIC, HEADER_BYTES, desc, blob.size))
         f.write(blob.tobytes())
 
 
 def read_dlw(path):
     """-> (header dict, desc, blob float32 array)."""
     with open(path, "rb") as f:
-        raw = f.read(HEADER_BYTES)
-        if len(raw) != HEADER_BYTES:
-            raise ValueError(f"{path}: truncated header")
-        v = _HEADER.unpack(raw)
-        if v[0] != MAGIC:
-            raise ValueError(f"{path}: not an odometry weight file (magic {v[0]!r})")
+        h, d = _unpack_header(f.read(HEADER_BYTES), path, MAGIC, "weight")
         blob = np.fromfile(f, dtype=np.float32)
-    names = ("magic", "abi_version", "header_bytes", "H", "W", "hfov0", "hfov1", "vfov0", "vfov1", "n_stride",
-             "max_batch", "act", "l0", "l1", "l2", "l3", "resnet_outputs", "single_mlp", "w_pre", "blob_floats")
-    h = dict(zip(names, v))
-    h["layers"] = [h.pop("l0"), h.pop("l1"), h.pop("l2"), h.pop("l3")]
     if blob.size != h["blob_floats"]:
         raise ValueError(f"{path}: blob has {blob.size} floats, the header says {h['blob_floats']}")
-    d = _lib.OdometryDesc()
-    for k in ("H", "W", "hfov0", "hfov1", "vfov0", "vfov1", "n_stride", "max_batch", "act", "resnet_outputs",
-              "single_mlp", "w_pre"):
-        setattr(d, k, h[k])
-    d.layers[:] = h["layers"]
     return h, d, blob
 
 
-def export(checkpoint_path, dataset, out_path, n_stride, max_batch=1, config_dir="config", preprocessing_normals=False):
-    """Checkpoint (torch.save of the trainer's dict, or a bare state dict with `config_dir` YAMLs) -> .dlw file."""
-    ckpt = torch.load(checkpoint_path, map_location="cpu", weights_only=False)
-    config = model_config(ckpt, config_dir)
-    state = ckpt["model_state_dict"] if isinstance(ckpt, dict) and "model_state_dict" in ckpt else ckpt
+# ---- training checkpoints (.dlt): the .dlw header and blob plus Adam's state, byte layout in include/delora_b200.h
+TRAIN_MAGIC = b"DELORAT\x00"
+TRAIN_HEADER_BYTES = 256
+# step | epoch, unsupervised | lr, beta1, beta2, eps, loss | 92 zero bytes, after the 128-byte .dlw header
+_TRAIN_TAIL = struct.Struct("<q" + "ii" + "5f" + "92x")
+assert HEADER_BYTES + _TRAIN_TAIL.size == TRAIN_HEADER_BYTES
+
+
+@dataclasses.dataclass
+class TrainingState:
+    """What a .dlt file holds besides the descriptor: the fp32 weight blob, Adam's m (exp_avg) and v (exp_avg_sq) in
+    blob order, the number of Adam updates, the epochs completed, the phase (unsupervised = 0: identity pre-training),
+    Adam's hyperparameters and the last epoch's mean objective."""
+    weights: np.ndarray
+    exp_avg: np.ndarray
+    exp_avg_sq: np.ndarray
+    step: int = 0
+    epoch: int = 0
+    unsupervised: int = 0
+    lr: float = 1e-5
+    beta1: float = 0.9
+    beta2: float = 0.999
+    eps: float = 1e-8
+    loss: float = 0.0
+
+
+def write_dlt(path, desc, state):
+    arrays = [np.ascontiguousarray(a, dtype=np.float32).reshape(-1)
+              for a in (state.weights, state.exp_avg, state.exp_avg_sq)]
+    n = arrays[0].size
+    if any(a.size != n for a in arrays):
+        raise ValueError(f"weights, exp_avg and exp_avg_sq must have the same length ({[a.size for a in arrays]})")
+    with open(path, "wb") as f:
+        f.write(_pack_header(TRAIN_MAGIC, TRAIN_HEADER_BYTES, desc, n))
+        f.write(_TRAIN_TAIL.pack(int(state.step), int(state.epoch), int(state.unsupervised), state.lr, state.beta1,
+                                 state.beta2, state.eps, state.loss))
+        for a in arrays:
+            f.write(a.tobytes())
+
+
+def read_dlt(path):
+    """-> (header dict, desc, TrainingState)."""
+    with open(path, "rb") as f:
+        h, d = _unpack_header(f.read(HEADER_BYTES), path, TRAIN_MAGIC, "training")
+        raw = f.read(_TRAIN_TAIL.size)
+        if len(raw) != _TRAIN_TAIL.size:
+            raise ValueError(f"{path}: truncated header")
+        data = np.fromfile(f, dtype=np.float32)
+    n = h["blob_floats"]
+    if data.size != 3 * n:
+        raise ValueError(f"{path}: {data.size} floats after the header, the header says 3 x {n}")
+    step, epoch, unsupervised, lr, beta1, beta2, eps, loss = _TRAIN_TAIL.unpack(raw)
+    state = TrainingState(data[:n], data[n:2 * n], data[2 * n:], step, epoch, unsupervised, lr, beta1, beta2, eps, loss)
+    return h, d, state
+
+
+def _parameter_order(config):
+    """state_dict_order, asserting that it is also the parameter order: optimizer state index i belongs to the i-th
+    parameter, and OdometryModel has no BatchNorm and no other buffers."""
+    from ..models.model import OdometryModel
+    cfg = dict(config)
+    cfg.update({"device": "cpu", "use_dropout": False})
+    with torch.device("meta"):
+        model = OdometryModel(cfg)
+    params = [(k, tuple(v.shape)) for k, v in model.named_parameters()]
+    assert not list(model.buffers()) and params == [(k, tuple(v.shape)) for k, v in model.state_dict().items()], \
+        "OdometryModel has buffers: optimizer state indices no longer follow the state_dict"
+    return params
+
+
+def training_state_from_checkpoint(checkpoint, config):
+    """The reference Trainer's checkpoint dict (src/deploy/trainer.py:155-173: model_state_dict + optimizer_state_dict
+    of torch.optim.Adam) -> TrainingState.  Without optimizer state: zero moments, step 0.  A checkpoint continues with
+    the ICP objective (unsupervised = 1), as the reference's Trainer does with one (:35-36).  Refused, naming the key:
+    Adam settings the C step does not run (weight_decay, amsgrad, maximize), more than one parameter group,
+    per-parameter steps that differ or are not integers, and tensors whose shapes do not match the model."""
+    order = _parameter_order(config)
+    weights = pack_state_dict(checkpoint["model_state_dict"], config)
+    opt = checkpoint.get("optimizer_state_dict") or {}
+    groups = opt.get("param_groups", [])
+    if len(groups) > 1:
+        raise ValueError(f"optimizer_state_dict.param_groups: {len(groups)} groups, the C step runs one")
+    g = groups[0] if groups else {}
+    for key, default in (("weight_decay", 0), ("amsgrad", False), ("maximize", False)):
+        if g.get(key, default) != default:
+            raise ValueError(f"optimizer_state_dict.param_groups[0].{key}: {g[key]!r} is not supported (the C step runs "
+                             f"Adam with {key} = {default!r})")
+    betas = g.get("betas", (0.9, 0.999))
+    state = TrainingState(weights, np.zeros_like(weights), np.zeros_like(weights), 0,
+                          int(checkpoint.get("epoch", -1)) + 1, 1, float(g.get("lr", config.get("learning_rate", 1e-5))),
+                          float(betas[0]), float(betas[1]), float(g.get("eps", 1e-8)),
+                          float(checkpoint.get("loss", 0.0)))
+    per_param = opt.get("state") or {}
+    if not per_param:
+        return state
+    ids = list(g["params"])
+    if len(ids) != len(order):
+        raise ValueError(f"optimizer_state_dict.param_groups[0].params: {len(ids)} parameters, the model has "
+                         f"{len(order)}")
+    m_parts, v_parts, steps = [], [], set()
+    for pid, (key, shape) in zip(ids, order):
+        s = per_param.get(pid)
+        if s is None:
+            raise ValueError(f"optimizer_state_dict.state[{pid}] ({key}): no state for this parameter")
+        for name, parts in (("exp_avg", m_parts), ("exp_avg_sq", v_parts)):
+            t = s[name]
+            if tuple(t.shape) != shape:
+                raise ValueError(f"optimizer_state_dict.state[{pid}].{name} ({key}): shape {tuple(t.shape)}, the "
+                                 f"model needs {shape}")
+            parts.append(t.detach().to("cpu", torch.float32).contiguous().reshape(-1).numpy())
+        step = float(s["step"])
+        if step != int(step) or step < 0:
+            raise ValueError(f"optimizer_state_dict.state[{pid}].step ({key}): {step} is not a non-negative integer")
+        steps.add(int(step))
+    if len(steps) != 1:
+        raise ValueError(f"optimizer_state_dict.state[*].step: the parameters' steps differ ({sorted(steps)[:4]}); "
+                         "the C step keeps one step count")
+    state.exp_avg = np.concatenate(m_parts).astype(np.float32, copy=False)
+    state.exp_avg_sq = np.concatenate(v_parts).astype(np.float32, copy=False)
+    state.step = steps.pop()
+    return state
+
+
+def checkpoint_from_training_state(state, config):
+    """TrainingState -> the reference Trainer's checkpoint dict (`epoch`, `model_state_dict`, `optimizer_state_dict`,
+    `loss`, `parameters`), which torch.optim.Adam.load_state_dict and both Trainers' config["checkpoint"] accept."""
+    model_sd = unpack_blob(state.weights, config)
+    m, v = unpack_blob(state.exp_avg, config), unpack_blob(state.exp_avg_sq, config)
+    group = {k: val for k, val in torch.optim.Adam([torch.zeros(1)]).param_groups[0].items() if k != "params"}
+    group.update({"lr": float(state.lr), "betas": (float(state.beta1), float(state.beta2)), "eps": float(state.eps),
+                  "weight_decay": 0, "amsgrad": False, "maximize": False, "params": list(range(len(model_sd)))})
+    per_param = {i: {"step": torch.tensor(float(state.step), dtype=torch.float32), "exp_avg": m[k], "exp_avg_sq": v[k]}
+                 for i, k in enumerate(model_sd)}
+    return {"epoch": int(state.epoch) - 1, "model_state_dict": model_sd,
+            "optimizer_state_dict": {"state": per_param, "param_groups": [group]}, "loss": float(state.loss),
+            "parameters": config}
+
+
+def initial_training_state(config, seed):
+    """A freshly initialised OdometryModel (torch's default initialisation, seeded) with a fresh Adam: the from-scratch
+    start of the reference's Trainer, in the identity pre-training phase unless config["unsupervised_at_start"]."""
+    from ..models.model import OdometryModel
+    check_supported(config)
+    cfg = dict(config)
+    cfg.update({"device": "cpu", "use_dropout": False})
+    with torch.random.fork_rng(devices=[]):
+        torch.manual_seed(int(seed))
+        model = OdometryModel(cfg)
+    weights = pack_state_dict(model.state_dict(), config)
+    return TrainingState(weights, np.zeros_like(weights), np.zeros_like(weights), 0, 0,
+                         1 if config.get("unsupervised_at_start", False) else 0,
+                         float(config.get("learning_rate", 1e-5)))
+
+
+def config_from_desc(desc, base=None, dataset="kitti"):
+    """`base` (e.g. the YAML configuration) with the network and range-image keys set from a .dlw / .dlt descriptor,
+    so that the configuration describes the weights of the file."""
+    cfg = dict(base or {})
+    ds = dict(cfg.get(dataset, {}))
+    ds.update({"vertical_cells": int(desc.H), "horizontal_cells": int(desc.W),
+               "vertical_field_of_view": [float(desc.vfov0), float(desc.vfov1)]})
+    if desc.w_pre:
+        ds["horizontal_cells_preprocessing"] = int(desc.w_pre)
+    cfg[dataset] = ds
+    cfg.update({"horizontal_field_of_view": [float(desc.hfov0), float(desc.hfov1)],
+                "activation_fct": "relu" if desc.act == 1 else "tanh", "layers": [int(v) for v in desc.layers],
+                "resnet_outputs": int(desc.resnet_outputs), "use_single_mlp_at_output": bool(desc.single_mlp),
+                "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1})
+    cfg.setdefault("use_dropout", False)
+    cfg.setdefault("datasets", [dataset])
+    return cfg
+
+
+def export(checkpoint_path, dataset, out_path, n_stride, max_batch=1, config_dir="config", preprocessing_normals=False,
+           training_state=False, init_seed=None):
+    """Checkpoint (torch.save of the trainer's dict, or a bare state dict with `config_dir` YAMLs) -> .dlw file.
+    training_state: write a .dlt instead (the checkpoint's optimizer state too).  init_seed (checkpoint_path None): the
+    weights of a freshly initialised model of the `config_dir` YAMLs instead of a checkpoint's."""
+    if init_seed is not None:
+        config = model_config(None, config_dir)
+        state = initial_training_state(config, init_seed)
+    else:
+        ckpt = torch.load(checkpoint_path, map_location="cpu", weights_only=False)
+        config = model_config(ckpt, config_dir)
+        if not (isinstance(ckpt, dict) and "model_state_dict" in ckpt):
+            ckpt = {"model_state_dict": ckpt}
+        state = training_state_from_checkpoint(ckpt, config) if training_state else None
     desc = desc_from_config(config, dataset, n_stride, max_batch, preprocessing_normals)
-    write_dlw(out_path, desc, pack_state_dict(state, config))
+    if training_state:
+        write_dlt(out_path, desc, state)
+    else:
+        write_dlw(out_path, desc, state.weights if state else pack_state_dict(ckpt["model_state_dict"], config))
     return desc

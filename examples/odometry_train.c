@@ -1,0 +1,245 @@
+/*
+ * The reference's training loop (src/deploy/trainer.py, Trainer.train) from a C host: no Python, no torch.  Links
+ * libdelora_b200.so and cudart only.
+ *
+ *   odometry_train [--lr LR] [--switch-below L] in.dlt|in.dlw out.dlt epochs B scan_000.bin scan_001.bin ...
+ *
+ * Reads a training checkpoint (.dlt: weights, Adam's state, epoch and phase; layout in include/delora_b200.h) or a
+ * weight file (.dlw: a fresh Adam with learning rate --lr, default 1e-5, the reference's learning_rate) and a list of
+ * consecutive KITTI velodyne .bin scans ([N, 4] float32 rows: x, y, z, reflectance), then runs `epochs` epochs.  An
+ * epoch walks the consecutive pairs (scan k, scan k+1) in order, B pairs per step (the last step takes the rest), and
+ * its objective is the mean of the steps' objectives:
+ *   - identity pre-training (the .dlt's unsupervised = 0): DELORA_LOSS_IDENTITY_FIT, MSELoss(T_{B-1}, I) / B;
+ *   - afterwards: the mean over the step's pairs of po2po + lambda * po2pl + pl2pl.
+ * Once an epoch's objective drops below --switch-below (default 1e-2, trainer.py:184-186) the next epoch is
+ * unsupervised.  A .dlw, or a .dlt made from a checkpoint, starts unsupervised, as the reference does with a
+ * checkpoint.  After every epoch the state goes to out.dlt (written to out.dlt.tmp, then renamed), so a run that
+ * stops can resume from it: N epochs in one run and N1 + N2 = N epochs in two give the same bytes.
+ * Losses as odometry_finetune.c: po2pl + pl2pl, lambda_po2pl 1, normals at the resolution the header's w_pre names.
+ *
+ * Build:  cc odometry_train.c -I include -I $CUDA_HOME/include -L delora_b200 -ldelora_b200 \
+ *            -L $CUDA_HOME/lib64 -lcudart -Wl,-rpath,$PWD/delora_b200 -o odometry_train
+ */
+#include <stdio.h>
+#include <stdlib.h>
+#include <string.h>
+
+#include <cuda_runtime.h>
+
+#include "delora_b200.h"
+
+static int fail(const char* what) {
+    fprintf(stderr, "odometry_train: %s\n", what);
+    return 1;
+}
+
+#define CUDA_OK(call)                                                                  \
+    do {                                                                               \
+        cudaError_t e_ = (call);                                                       \
+        if (e_ != cudaSuccess) return fail(cudaGetErrorString(e_));                     \
+    } while (0)
+
+#define DELORA_OK(call)                                                                \
+    do {                                                                               \
+        if ((call) != 0) return fail(delora_last_error());                             \
+    } while (0)
+
+/* one scan as [3, n_stride] channels-first (x, y, z), zero-padded; returns the point count or -1 */
+static int32_t read_scan(const char* path, int n_stride, float* out) {
+    FILE* s = fopen(path, "rb");
+    if (!s) return -1;
+    fseek(s, 0, SEEK_END);
+    const long bytes = ftell(s);
+    fseek(s, 0, SEEK_SET);
+    const int32_t n = (int32_t)(bytes / (4 * sizeof(float)));
+    float* rows = (float*)malloc((size_t)n * 4 * sizeof(float) + 1);
+    if (n > n_stride || !rows || fread(rows, 4 * sizeof(float), (size_t)n, s) != (size_t)n) {
+        free(rows);
+        fclose(s);
+        return -1;
+    }
+    fclose(s);
+    memset(out, 0, (size_t)3 * n_stride * sizeof(float));
+    for (int32_t i = 0; i < n; ++i)
+        for (int c = 0; c < 3; ++c) out[(size_t)c * n_stride + i] = rows[(size_t)i * 4 + c];
+    free(rows);
+    return n;
+}
+
+/* the header and the three host arrays (weights, exp_avg, exp_avg_sq) to path, through path.tmp and a rename */
+static int write_dlt(const char* path, const delora_odometry_train_file_header* hdr, float* const* h_state, size_t n) {
+    char tmp[4096];
+    if (snprintf(tmp, sizeof tmp, "%s.tmp", path) >= (int)sizeof tmp) return fail("output path too long");
+    FILE* o = fopen(tmp, "wb");
+    if (!o) return fail("cannot create the output file");
+    int ok = fwrite(hdr, sizeof *hdr, 1, o) == 1;
+    for (int i = 0; i < 3 && ok; ++i) ok = fwrite(h_state[i], sizeof(float), n, o) == n;
+    ok = (fclose(o) == 0) && ok;
+    if (!ok || rename(tmp, path) != 0) return fail("cannot write the output file");
+    return 0;
+}
+
+int main(int argc, char** argv) {
+    float lr = 1e-5f;
+    double switch_below = 1e-2;
+    int a = 1;
+    for (; a + 1 < argc && strncmp(argv[a], "--", 2) == 0; a += 2) {
+        if (strcmp(argv[a], "--lr") == 0) lr = (float)atof(argv[a + 1]);
+        else if (strcmp(argv[a], "--switch-below") == 0) switch_below = atof(argv[a + 1]);
+        else return fail("unknown option");
+    }
+    if (argc - a < 6)
+        return fail("usage: odometry_train [--lr LR] [--switch-below L] in.dlt|in.dlw out.dlt epochs B scan.bin "
+                    "scan.bin [scan.bin ...]");
+    const char* in_path = argv[a];
+    const char* out_path = argv[a + 1];
+    const int epochs = atoi(argv[a + 2]);
+    const int B_max = atoi(argv[a + 3]);
+    const int n_scans = argc - a - 4;
+    char** scan_paths = argv + a + 4;
+
+    /* the .dlw header is the first 128 bytes of both formats; a .dlt adds Adam's state after it */
+    delora_odometry_train_file_header hdr;
+    memset(&hdr, 0, sizeof hdr);
+    FILE* f = fopen(in_path, "rb");
+    if (!f) return fail("cannot open the input file");
+    if (fread(&hdr.base, sizeof hdr.base, 1, f) != 1) return fail("truncated header");
+    const int is_dlt = memcmp(hdr.base.magic, DELORA_TRAINING_FILE_MAGIC, 8) == 0;
+    if (!is_dlt && memcmp(hdr.base.magic, DELORA_ODOMETRY_FILE_MAGIC, 8) != 0) return fail("not a .dlw or .dlt file");
+    if (hdr.base.abi_version != delora_abi_version()) return fail("input file and library ABI versions differ");
+    if (is_dlt && fread((char*)&hdr + sizeof hdr.base, sizeof hdr - sizeof hdr.base, 1, f) != 1)
+        return fail("truncated header");
+    const delora_odometry_desc* d = &hdr.base.desc;
+    const int64_t n_weights = delora_odometry_weight_floats(d);
+    if (n_weights < 0) return fail(delora_last_error());
+    if (n_weights != hdr.base.blob_floats) return fail("blob length does not match the descriptor");
+    const size_t n = (size_t)n_weights;
+    float* h_state[3];
+    for (int i = 0; i < 3; ++i) {
+        h_state[i] = (float*)calloc(n, sizeof(float));
+        if (!h_state[i]) return fail("out of host memory");
+    }
+    for (int i = 0; i < (is_dlt ? 3 : 1); ++i)
+        if (fread(h_state[i], sizeof(float), n, f) != n) return fail("truncated blob");
+    fclose(f);
+    if (!is_dlt) {            /* weights only: a fresh Adam, the ICP objective */
+        hdr.step = 0; hdr.epoch = 0; hdr.unsupervised = 1;
+        hdr.lr = lr; hdr.beta1 = 0.9f; hdr.beta2 = 0.999f; hdr.eps = 1e-8f; hdr.loss = 0.0f;
+    }
+    memcpy(hdr.base.magic, DELORA_TRAINING_FILE_MAGIC, 8);
+    hdr.base.abi_version = delora_abi_version();
+    hdr.base.header_bytes = (int32_t)sizeof hdr;
+    memset(hdr.base.reserved, 0, sizeof hdr.base.reserved);
+    memset(hdr.reserved, 0, sizeof hdr.reserved);
+
+    const int n_pairs = n_scans - 1;
+    if (B_max < 1 || B_max > d->max_batch) return fail("B must be in [1, the header's max_batch]");
+    if (epochs < 0) return fail("epochs must be >= 0");
+    const size_t scan_floats = (size_t)3 * d->n_stride;
+    float* h_scans = (float*)malloc((size_t)n_scans * scan_floats * sizeof(float));
+    int32_t* h_counts = (int32_t*)malloc((size_t)n_scans * sizeof(int32_t));
+    if (!h_scans || !h_counts) return fail("out of host memory");
+    for (int k = 0; k < n_scans; ++k)
+        if ((h_counts[k] = read_scan(scan_paths[k], d->n_stride, h_scans + (size_t)k * scan_floats)) < 0)
+            return fail("cannot read a scan (missing, truncated, or more points than n_stride)");
+
+    delora_odometry_train_params hp;
+    hp.lr = hdr.lr; hp.beta1 = hdr.beta1; hp.beta2 = hdr.beta2; hp.eps = hdr.eps;
+    hp.lambda_po2pl = 1.0f;
+    hp.nb_h = 7; hp.nb_w = 11;
+    hp.epsilon_range = 0.5f;
+    hp.min_neighbors = 10;
+
+    cudaStream_t stream;
+    CUDA_OK(cudaStreamCreate(&stream));
+    float *d_state[3], *points, *losses;
+    int64_t* d_step;
+    int32_t* counts;
+    void* workspace;
+    const int64_t ws_bytes = delora_odometry_train_workspace_bytes(d);
+    if (ws_bytes < 0) return fail(delora_last_error());
+    for (int i = 0; i < 3; ++i) {
+        CUDA_OK(cudaMalloc((void**)&d_state[i], n * sizeof(float)));
+        CUDA_OK(cudaMemcpy(d_state[i], h_state[i], n * sizeof(float), cudaMemcpyHostToDevice));
+    }
+    CUDA_OK(cudaMalloc((void**)&d_step, sizeof(int64_t)));
+    CUDA_OK(cudaMemcpy(d_step, &hdr.step, sizeof(int64_t), cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMalloc(&workspace, (size_t)ws_bytes));
+    CUDA_OK(cudaMalloc((void**)&points, (size_t)2 * B_max * scan_floats * sizeof(float)));
+    CUDA_OK(cudaMalloc((void**)&counts, (size_t)2 * B_max * sizeof(int32_t)));
+    CUDA_OK(cudaMalloc((void**)&losses, (size_t)B_max * DELORA_LOSS_ROW * sizeof(float)));
+    DELORA_OK(delora_odometry_train_init(d, d_state[0], workspace, stream));
+    DELORA_OK(delora_odometry_train_set_state(d, d_state[0], d_state[1], d_state[2], d_step, workspace, stream));
+    fprintf(stderr, "odometry_train: epoch %d, Adam step %lld, %s, %d pairs\n", hdr.epoch, (long long)hdr.step,
+            hdr.unsupervised ? "unsupervised" : "identity pre-training", n_pairs);
+
+    float* h_losses = (float*)malloc((size_t)B_max * DELORA_LOSS_ROW * sizeof(float));
+    int32_t* h_step_counts = (int32_t*)malloc((size_t)2 * B_max * sizeof(int32_t));
+    if (!h_losses || !h_step_counts) return fail("out of host memory");
+    for (int e = 0; e < epochs; ++e) {
+        hp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | (hdr.unsupervised ? 0u : DELORA_LOSS_IDENTITY_FIT);
+        double sum = 0.0;
+        int steps = 0;
+        for (int k0 = 0; k0 < n_pairs; k0 += B_max, ++steps) {
+            const int B = n_pairs - k0 < B_max ? n_pairs - k0 : B_max;
+            /* points of a step: scan_1 of pairs 0..B-1, then scan_2 of pairs 0..B-1 */
+            for (int b = 0; b < B; ++b) {
+                const int k = k0 + b;
+                CUDA_OK(cudaMemcpyAsync(points + (size_t)b * scan_floats, h_scans + (size_t)k * scan_floats,
+                                        scan_floats * sizeof(float), cudaMemcpyHostToDevice, stream));
+                CUDA_OK(cudaMemcpyAsync(points + (size_t)(B + b) * scan_floats, h_scans + (size_t)(k + 1) * scan_floats,
+                                        scan_floats * sizeof(float), cudaMemcpyHostToDevice, stream));
+                h_step_counts[b] = h_counts[k];
+                h_step_counts[B + b] = h_counts[k + 1];
+            }
+            CUDA_OK(cudaMemcpyAsync(counts, h_step_counts, (size_t)2 * B * sizeof(int32_t), cudaMemcpyHostToDevice,
+                                    stream));
+            DELORA_OK(delora_odometry_train_step(d, &hp, points, counts, B, workspace, losses, NULL, NULL, NULL, stream));
+            CUDA_OK(cudaMemcpyAsync(h_losses, losses, (size_t)B * DELORA_LOSS_ROW * sizeof(float),
+                                    cudaMemcpyDeviceToHost, stream));
+            CUDA_OK(cudaStreamSynchronize(stream));
+            if (!hdr.unsupervised) {
+                sum += (double)h_losses[(size_t)(B - 1) * DELORA_LOSS_ROW + 5];
+            } else {
+                double objective = 0.0;
+                for (int b = 0; b < B; ++b) {
+                    const float* l = h_losses + (size_t)b * DELORA_LOSS_ROW;
+                    objective += (double)l[0] + (double)hp.lambda_po2pl * l[1] + (double)l[2];
+                }
+                sum += objective / B;
+            }
+        }
+        const double mean = steps > 0 ? sum / steps : 0.0;
+        printf("epoch %d objective %.9g unsupervised %d\n", hdr.epoch, mean, hdr.unsupervised);
+        hdr.epoch += 1;
+        hdr.loss = (float)mean;
+        if (!hdr.unsupervised && mean < switch_below) {
+            hdr.unsupervised = 1;
+            fprintf(stderr, "odometry_train: objective below %g, switching to the unsupervised objective\n",
+                    switch_below);
+        }
+        /* the state after the epoch, in the phase the next epoch runs */
+        DELORA_OK(delora_odometry_train_get_state(d, workspace, d_state[0], d_state[1], d_state[2], d_step, stream));
+        for (int i = 0; i < 3; ++i)
+            CUDA_OK(cudaMemcpyAsync(h_state[i], d_state[i], n * sizeof(float), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaMemcpyAsync(&hdr.step, d_step, sizeof(int64_t), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+        if (write_dlt(out_path, &hdr, h_state, n)) return 1;
+    }
+
+    free(h_step_counts);
+    free(h_losses);
+    free(h_counts);
+    free(h_scans);
+    for (int i = 0; i < 3; ++i) {
+        free(h_state[i]);
+        cudaFree(d_state[i]);
+    }
+    cudaFree(d_step);
+    cudaFree(losses);
+    cudaFree(counts);
+    cudaFree(points);
+    cudaFree(workspace);
+    cudaStreamDestroy(stream);
+    return 0;
+}

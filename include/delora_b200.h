@@ -40,6 +40,8 @@ typedef struct { float x, y, z, w; } delora_f4;
 #define DELORA_LOSS_PL2PL        4u   /* plane_to_plane_loss                 */
 #define DELORA_NORMAL_LINEAR     8u   /* normal_loss: "linear" (default "squared") */
 #define DELORA_ICP_STATS       256u  /* diagnostic: count the work of the NN search (delora_icp_stats) */
+#define DELORA_LOSS_IDENTITY_FIT 512u /* delora_odometry_train_step only: the identity pre-training objective
+                                         (unsupervised_at_start: False, src/deploy/deployer.py:324-327) */
 
 /* number of floats in one row of the `losses` output of delora_icp_fwd_bwd */
 #define DELORA_LOSS_ROW 8   /* [po2po, po2pl, pl2pl, M_pairs, M_po2po, 0, 0, 0] */
@@ -514,7 +516,8 @@ int delora_odometry_streams_reset(const delora_odometry_desc* d, const int32_t* 
 typedef struct {
     float lr, beta1, beta2, eps;         /* Adam (torch defaults 0.9, 0.999, 1e-8); lr >= 0, betas in [0, 1), eps > 0 */
     float lambda_po2pl;                  /* config lambda_po2pl */
-    uint32_t loss_flags;                 /* DELORA_LOSS_* / DELORA_NORMAL_LINEAR bits, at least one loss bit */
+    uint32_t loss_flags;                 /* DELORA_LOSS_* / DELORA_NORMAL_LINEAR bits, at least one ICP loss bit
+                                            (PO2PO, PO2PL, PL2PL), plus DELORA_LOSS_IDENTITY_FIT (see _train_step) */
     int nb_h, nb_w;                      /* neighborhood_side_length (7, 11): odd and positive */
     float epsilon_range;                 /* 0.5 */
     int min_neighbors;                   /* min_num_points_in_neighborhood_to_determine_point_class, 10 */
@@ -531,13 +534,57 @@ int delora_odometry_train_init(const delora_odometry_desc* d, const float* weigh
  * delora_odometry_pairs.  Outputs, each DEVICE and each may be NULL: losses [B, DELORA_LOSS_ROW] as the ICP operator
  * writes them; T [B, 16] of the weights BEFORE the update; pooled [B, 512]; grads [weight_floats] the gradient of the
  * objective in blob order.  Refused before any launch: an invalid descriptor or hyperparameter (the message names the
- * field), null points / n_points / workspace, B outside [1, max_batch]. */
+ * field), null points / n_points / workspace, B outside [1, max_batch].
+ * Identity pre-training: with DELORA_LOSS_IDENTITY_FIT in hp->loss_flags the objective is the reference's first phase
+ * (unsupervised_at_start: False; src/deploy/deployer.py:324-327, :334-336), MSELoss(T_{B-1}, I) / B: only the LAST
+ * pair's 4x4 transform counts (the reference overwrites its loss inside the pair loop), the mean runs over its 16
+ * entries.  dL/dT is 2 (T - I) / (16 B) on the 3x4 part of row B-1 and zero elsewhere; the backward from there on is
+ * the ICP objective's (the norm of the whole [B, 4] quaternion block still gives every pair's head outputs a
+ * gradient).  The ICP losses are still computed and written to `losses` (the reference logs them in this phase); the
+ * identity objective goes to losses[B-1][5] (column 5 is 0 in the other rows and in steps without the bit).  At least
+ * one ICP loss bit is still required. */
 int delora_odometry_train_step(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
                                const float* points, const int32_t* n_points, int B, void* workspace,
                                float* losses, float* T, float* pooled, float* grads, void* stream);
 /* Copy the current fp32 master weights to `weights` (DEVICE fp32[weight_floats]): a .dlw blob, loadable by
  * delora_odometry_load_weights and delora_odometry_train_init. */
 int delora_odometry_train_weights(const delora_odometry_desc* d, const void* workspace, float* weights, void* stream);
+/* The optimizer state, for checkpoints that resume a run exactly (src/deploy/trainer.py:26-36 loads, :153-173 saves
+ * model_state_dict + optimizer_state_dict).  weights, exp_avg (Adam's m), exp_avg_sq (v): DEVICE fp32[weight_floats]
+ * each, in blob order; step: DEVICE int64, the number of Adam updates so far (torch's state["step"]).
+ * _get_state copies them out of a training workspace; every output may be NULL (skipped).  Launches copies only, no
+ * synchronisation: capturable into a CUDA graph.
+ * _set_state, after _train_init: overwrites the master weights, m, v and the step count and re-preps the bf16 filters
+ * (fprop and flipped layouts) from the new weights; the next step continues as the workspace the state came from
+ * would have (bit-identical), whatever batch size that one last ran.  All four inputs are required (a fresh Adam is
+ * _train_init's).  Both refuse before any launch, naming the argument: an invalid descriptor, a null input, a null
+ * workspace. */
+int delora_odometry_train_get_state(const delora_odometry_desc* d, const void* workspace, float* weights, float* exp_avg,
+                                    float* exp_avg_sq, int64_t* step, void* stream);
+int delora_odometry_train_set_state(const delora_odometry_desc* d, const float* weights, const float* exp_avg,
+                                    const float* exp_avg_sq, const int64_t* step, void* workspace, void* stream);
+
+/* Training checkpoint (.dlt, written by delora_b200/deploy/export.py and examples/odometry_train.c), little-endian,
+ * readable with fread alone:
+ *   bytes   0..127  a delora_odometry_file_header (the .dlw layout above) with magic "DELORAT" and header_bytes 256
+ *   bytes 128..135  step (int64): Adam updates so far
+ *   bytes 136..139  epoch (int32): epochs completed (the reference checkpoint's `epoch` + 1)
+ *   bytes 140..143  unsupervised (int32): 0 = still in the identity pre-training phase, 1 = ICP objective
+ *   bytes 144..159  lr, beta1, beta2, eps (float32 each): Adam's hyperparameters
+ *   bytes 160..163  loss (float32): the mean objective of the last epoch
+ *   bytes 164..255  zero
+ *   bytes 256..     float32[blob_floats] weights, then float32[blob_floats] exp_avg, then float32[blob_floats]
+ *                   exp_avg_sq, each in blob order (the three arrays of delora_odometry_train_set_state). */
+#define DELORA_TRAINING_FILE_MAGIC "DELORAT"     /* 7 characters + NUL = the 8 magic bytes */
+typedef struct {
+    delora_odometry_file_header base;    /* magic DELORA_TRAINING_FILE_MAGIC, header_bytes 256 */
+    int64_t step;
+    int32_t epoch;
+    int32_t unsupervised;
+    float lr, beta1, beta2, eps;
+    float loss;
+    uint8_t reserved[92];
+} delora_odometry_train_file_header;
 
 /* ---- Data-parallel training step: average of the weight gradients over the ranks (SURVEY.md 8(e); the reference
  * steps one optimizer on one device, src/deploy/trainer.py:23-24, on `loss / batch_size`, src/deploy/deployer.py:329-342
