@@ -116,9 +116,6 @@ SIGNATURES = {
     "delora_odometry_train_set_state": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
-# delora_odometry_train_params.loss_flags bit of the identity pre-training objective (include/delora_b200.h)
-LOSS_IDENTITY_FIT = 512
-
 ABI_VERSION = 3
 _lib = None
 

@@ -10,8 +10,6 @@ H2D of the raw scan and a 64-byte D2H of the relative transform.  BASELINE confi
 
 OdometryStreams serves several streams of one sensor geometry and model from one C-ABI workspace, batched.
 """
-import ctypes
-
 import numpy as np
 import torch
 
@@ -127,30 +125,18 @@ class OdometryStreams:
     graph replay (or the eager call), one D2H copy of T and valid, one synchronise."""
 
     def __init__(self, model, config, dataset, n_streams, n_max, use_cuda_graph=True):
-        from .. import _lib
-        from . import export
+        from . import capi, export
         self.config = config
         self.dataset = dataset
         self.device = torch.device(config["device"])
         if self.device.type != "cuda":
             raise RuntimeError("OdometryStreams runs on CUDA devices only (no CPU fallback)")
         self.n_streams, self.n_max = int(n_streams), int(n_max)
-        self._L = _lib.lib()
-        self._check = _lib.check
         self.desc = export.desc_from_config(config, dataset, self.n_max, self.n_streams)
-        self._dp = ctypes.byref(self.desc)
-        nbytes = int(self._L.delora_odometry_streams_workspace_bytes(self._dp))
-        if nbytes < 0:
-            raise ValueError(self._L.delora_last_error().decode())
         S, n = self.n_streams, self.n_max
         with torch.cuda.device(self.device):
-            self.workspace = torch.empty((nbytes,), dtype=torch.uint8, device=self.device)
             self.blob = torch.from_numpy(export.pack_state_dict(model.state_dict(), config)).to(self.device)
-            self._check(self._L.delora_odometry_streams_init(self._dp, self.workspace.data_ptr(), self._stream()),
-                        "delora_odometry_streams_init")
-            self._check(self._L.delora_odometry_streams_load_weights(self._dp, self.blob.data_ptr(),
-                                                                     self.workspace.data_ptr(), self._stream()),
-                        "delora_odometry_streams_load_weights")
+            self.workspace = capi.StreamsWorkspace(self.desc, self.blob)
             # staging: points [S, 3, n_max] fp32, then counts [S] and active [S] int32, one buffer each way
             in_bytes = S * 3 * n * 4 + 2 * S * 4
             self.host_in = torch.zeros((in_bytes,), dtype=torch.uint8).pin_memory()
@@ -166,32 +152,24 @@ class OdometryStreams:
         out = self.host_out.numpy()
         self._host_T = out[:S * 64].view(np.float32).reshape(S, 4, 4)
         self._host_valid = out[S * 64:].view(np.int32)
-        base_in, base_out = self.dev_in.data_ptr(), self.dev_out.data_ptr()
-        self._ptrs = (base_in, base_in + S * 3 * n * 4, base_in + S * 3 * n * 4 + S * 4, base_out, base_out + S * 64)
+        # the push arguments of a tick: points, counts, active, T, valid in the device staging buffers
+        self._dev_active = self.dev_in[S * 3 * n * 4 + S * 4:]
+        self._tick = (self.dev_in[:S * 3 * n * 4], self.dev_in[S * 3 * n * 4:S * 3 * n * 4 + S * 4], self._dev_active,
+                      self.dev_out[:S * 64], self.dev_out[S * 64:])
         self.relative = [[] for _ in range(S)]
         self.use_cuda_graph = bool(use_cuda_graph)
         self.graph = None
 
-    @staticmethod
-    def _stream():
-        return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-    def _tick(self):
-        points, counts, active, T, valid = self._ptrs
-        self._check(self._L.delora_odometry_streams_push(self._dp, points, counts, active, self.workspace.data_ptr(), T,
-                                                         valid, self._stream()), "delora_odometry_streams_push")
-
     def _capture(self):
         # a tick with every stream inactive changes no stream's state: it warms the launchers' host-side caches, then
         # the call is captured (capturing runs nothing)
-        active = self._ptrs[2]
         torch.cuda.current_stream().synchronize()
-        self.dev_in[active - self._ptrs[0]:].zero_()
-        self._tick()
+        self._dev_active.zero_()
+        self.workspace.push(*self._tick)
         torch.cuda.current_stream().synchronize()
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
-            self._tick()
+            self.workspace.push(*self._tick)
 
     def push(self, scans):
         """scans: a list of n_streams entries, each a [3, N] (or [1, 3, N]) float32 host tensor with N <= n_max, or
@@ -218,7 +196,7 @@ class OdometryStreams:
             if self.graph is not None:
                 self.graph.replay()
             else:
-                self._tick()
+                self.workspace.push(*self._tick)
             self.host_out.copy_(self.dev_out, non_blocking=True)
             torch.cuda.current_stream().synchronize()
         out = []
@@ -240,8 +218,6 @@ class OdometryStreams:
         with torch.cuda.device(self.device):
             self.dev_mask.zero_()
             self.dev_mask[s] = 1
-            self._check(self._L.delora_odometry_streams_reset(self._dp, self.dev_mask.data_ptr(),
-                                                              self.workspace.data_ptr(), self._stream()),
-                        "delora_odometry_streams_reset")
+            self.workspace.reset(self.dev_mask)
             torch.cuda.current_stream().synchronize()
         self.relative[s] = []

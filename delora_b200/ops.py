@@ -35,6 +35,7 @@ class nvtx_range:
 # include/delora_b200.h's DELORA_* constants (tests/test_icp_layout_cpu.py checks that they agree)
 LOSS_PO2PO, LOSS_PO2PL, LOSS_PL2PL, NORMAL_LINEAR = 1, 2, 4, 8
 ICP_STATS = 256      # DELORA_ICP_STATS flag bit
+LOSS_IDENTITY_FIT = 512      # delora_odometry_train_step's identity pre-training objective
 LOSS_ROW, ICP_PARTIAL = 8, 40
 
 _keys_cache = {}

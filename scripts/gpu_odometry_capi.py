@@ -9,7 +9,6 @@ The card's name, power limit and SM clock are read in the same run.
     python scripts/gpu_odometry_capi.py [--frames 300] [--json out.json]
 """
 import argparse
-import ctypes
 import json
 import os
 import subprocess
@@ -21,8 +20,9 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
-from delora_b200 import _lib, synthetic  # noqa: E402
+from delora_b200 import synthetic  # noqa: E402
 from delora_b200.deploy import export  # noqa: E402
+from delora_b200.deploy.capi import InferenceWorkspace  # noqa: E402
 from delora_b200.deploy.stream import OdometryStream  # noqa: E402
 from delora_b200.models.model import OdometryModel  # noqa: E402
 
@@ -60,19 +60,13 @@ def main():
     n_stride = max(s.shape[1] for s in scans)
     info_before = gpu_info()
 
-    L = _lib.lib()
     res = {"gpu_before": info_before, "H": h, "W": w, "n_stride": n_stride}
     for mb in (1, 16):
         dd = export.desc_from_config(cfg, "kitti", n_stride, mb)
-        res[f"workspace_bytes_max_batch_{mb}"] = int(L.delora_odometry_workspace_bytes(ctypes.byref(dd)))
-    d = export.desc_from_config(cfg, "kitti", n_stride, 1)
-    dp = ctypes.byref(d)
+        res[f"workspace_bytes_max_batch_{mb}"] = InferenceWorkspace.workspace_bytes(dd)
     st = torch.cuda.current_stream()
-    sp = ctypes.c_void_p(st.cuda_stream)
-    ws = torch.empty((int(L.delora_odometry_workspace_bytes(dp)),), dtype=torch.uint8, device=dev)
-    _lib.check(L.delora_odometry_init(dp, ws.data_ptr(), sp), "init")
     blob = torch.from_numpy(export.pack_state_dict(model.state_dict(), cfg)).to(dev)
-    _lib.check(L.delora_odometry_load_weights(dp, blob.data_ptr(), ws.data_ptr(), sp), "load")
+    ws = InferenceWorkspace(export.desc_from_config(cfg, "kitti", n_stride, 1), blob)
 
     host_pts = torch.zeros((len(scans), 3, n_stride), dtype=torch.float32).pin_memory()
     host_cnt = torch.zeros((len(scans),), dtype=torch.int32).pin_memory()
@@ -90,8 +84,7 @@ def main():
 
     def push(k, first=False):
         upload(k)
-        _lib.check(L.delora_odometry_push(dp, pts.data_ptr(), cnt.data_ptr(), ws.data_ptr(),
-                                          None if first else t_dev.data_ptr(), sp), "push")
+        ws.push(pts, cnt, None if first else t_dev)
 
     def timed(step, n):
         ts = []
@@ -111,8 +104,7 @@ def main():
 
     graph = torch.cuda.CUDAGraph()
     with torch.cuda.graph(graph):
-        _lib.check(L.delora_odometry_push(dp, pts.data_ptr(), cnt.data_ptr(), ws.data_ptr(), t_dev.data_ptr(),
-                                          ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), "push (capture)")
+        ws.push(pts, cnt, t_dev)
 
     def replay(k):
         upload(k)

@@ -10,7 +10,6 @@ torch.profiler splits one eager tick (streams, and the S pushes) into kernels at
     python scripts/gpu_odometry_streams.py [--seconds 1.0] [--profile] [--out DIR]
 """
 import argparse
-import ctypes
 import json
 import math
 import os
@@ -21,8 +20,9 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 import torch  # noqa: E402
 
-from delora_b200 import _lib, synthetic  # noqa: E402
+from delora_b200 import synthetic  # noqa: E402
 from delora_b200.deploy import export  # noqa: E402
+from delora_b200.deploy.capi import InferenceWorkspace, StreamsWorkspace  # noqa: E402
 from delora_b200.models.model import OdometryModel  # noqa: E402
 
 DEV = "cuda:0"
@@ -34,10 +34,6 @@ def gpu_info():
     q = "name,power.limit,clocks.sm,clocks.max.sm"
     r = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True)
     return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "unavailable"
-
-
-def sp():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def frames(h, n):
@@ -84,14 +80,9 @@ def staged(scans, n_stride):
 
 
 class StreamsRun:
-    def __init__(self, L, cfg, blob, scans, n_stride):
+    def __init__(self, cfg, blob, scans, n_stride):
         S = len(scans)
-        self.L = L
-        self.d = export.desc_from_config(cfg, "kitti", n_stride, S)
-        self.dp = ctypes.byref(self.d)
-        self.ws = torch.empty((int(L.delora_odometry_streams_workspace_bytes(self.dp)),), dtype=torch.uint8, device=DEV)
-        _lib.check(L.delora_odometry_streams_init(self.dp, self.ws.data_ptr(), sp()), "streams_init")
-        _lib.check(L.delora_odometry_streams_load_weights(self.dp, blob.data_ptr(), self.ws.data_ptr(), sp()), "load")
+        self.ws = StreamsWorkspace(export.desc_from_config(cfg, "kitti", n_stride, S), blob)
         self.pts, self.counts = staged(scans, n_stride)
         self.active = torch.ones((S,), dtype=torch.int32, device=DEV)
         self.T = torch.zeros((S, 16), dtype=torch.float32, device=DEV)
@@ -103,22 +94,14 @@ class StreamsRun:
             self.push()
 
     def push(self):
-        _lib.check(self.L.delora_odometry_streams_push(self.dp, self.pts.data_ptr(), self.counts.data_ptr(),
-                                                       self.active.data_ptr(), self.ws.data_ptr(), self.T.data_ptr(),
-                                                       self.valid.data_ptr(), sp()), "streams_push")
+        self.ws.push(self.pts, self.counts, self.active, self.T, self.valid)
 
 
 class PushRun:
-    def __init__(self, L, cfg, blob, scans, n_stride):
-        self.L = L
-        self.d = export.desc_from_config(cfg, "kitti", n_stride, 1)
-        self.dp = ctypes.byref(self.d)
-        nbytes = int(L.delora_odometry_workspace_bytes(self.dp))
+    def __init__(self, cfg, blob, scans, n_stride):
         self.ws, self.pts, self.counts, self.T, self.graphs = [], [], [], [], []
         for s in scans:
-            ws = torch.empty((nbytes,), dtype=torch.uint8, device=DEV)
-            _lib.check(L.delora_odometry_init(self.dp, ws.data_ptr(), sp()), "init")
-            _lib.check(L.delora_odometry_load_weights(self.dp, blob.data_ptr(), ws.data_ptr(), sp()), "load")
+            ws = InferenceWorkspace(export.desc_from_config(cfg, "kitti", n_stride, 1), blob)
             p, c = staged([s], n_stride)
             self.ws.append(ws), self.pts.append(p), self.counts.append(c)
             self.T.append(torch.zeros((16,), dtype=torch.float32, device=DEV))
@@ -133,9 +116,7 @@ class PushRun:
             self.graphs.append(g)
 
     def push(self, i, first=False):
-        _lib.check(self.L.delora_odometry_push(self.dp, self.pts[i].data_ptr(), self.counts[i].data_ptr(),
-                                               self.ws[i].data_ptr(), None if first else self.T[i].data_ptr(), sp()),
-                   "push")
+        self.ws[i].push(self.pts[i], self.counts[i], None if first else self.T[i])
 
     def replay(self):
         for g in self.graphs:
@@ -165,7 +146,6 @@ def main():
     ap.add_argument("--out", default="")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs a GPU"
-    L = _lib.lib()
     res = {"gpu_before": gpu_info(), "seconds_per_point": args.seconds, "sizes": {}}
     for h, w in SIZES:
         cfg = synthetic.fov_config(h=h, w=w, device=DEV)
@@ -181,8 +161,8 @@ def main():
         rows = {}
         for S in STREAMS:
             scans = scans_all[:S]
-            st = StreamsRun(L, cfg, blob, scans, n_stride)
-            pu = PushRun(L, cfg, blob, scans, n_stride)
+            st = StreamsRun(cfg, blob, scans, n_stride)
+            pu = PushRun(cfg, blob, scans, n_stride)
             # alternate the two so drift of the card's clock hits both alike
             ms_s1, n_s = time_replays(st.graph.replay, args.seconds / 2)
             ms_p1, n_p = time_replays(pu.replay, args.seconds / 2)
@@ -195,8 +175,8 @@ def main():
                        "pushes_ms_per_tick": ms_p, "pushes_frames_per_s": S * 1e3 / ms_p,
                        "speedup": ms_p / ms_s, "streams_ms_runs": [ms_s1, ms_s2], "pushes_ms_runs": [ms_p1, ms_p2],
                        "replays": [n_s, n_p], "T_bit_identical": same,
-                       "streams_workspace_MiB": st.ws.numel() / 2**20,
-                       "pushes_workspace_MiB": sum(x.numel() for x in pu.ws) / 2**20}
+                       "streams_workspace_MiB": st.ws.workspace.numel() / 2**20,
+                       "pushes_workspace_MiB": sum(x.workspace.numel() for x in pu.ws) / 2**20}
             if args.profile and key in args.profile_sizes.split(",") and S in (1, 16):
                 rows[S]["profile_streams"] = kernel_split(st.push)
                 rows[S]["profile_pushes"] = kernel_split(lambda: [pu.push(i) for i in range(S)])

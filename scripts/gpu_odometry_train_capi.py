@@ -11,7 +11,6 @@ kernels this path adds (the tail backward, Adam, the ICP scratch re-arm) against
 Prints the result as JSON; with --out it is also written to DIR/odometry_train_capi.json.
 """
 import argparse
-import ctypes
 import json
 import os
 import statistics
@@ -45,7 +44,7 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("no CUDA device: this script measures the GPU")
     from delora_b200 import _lib, synthetic
-    from delora_b200.deploy import export
+    from delora_b200.deploy import capi, export
     from delora_b200.train_step import SyntheticTrainStep
     dev = torch.device("cuda:0")
     b = a.batch
@@ -66,23 +65,14 @@ def main():
     py = SyntheticTrainStep(cfg, b, n_max)
     py.load(pts, counts)
     cfg = py.cfg
-    L = _lib.lib()
-    d = export.desc_from_config(cfg, "kitti", n_max, b)
-    dp = ctypes.byref(d)
-    nb = cfg["kitti"]["neighborhood_side_length"]
-    hp = _lib.OdometryTrainParams(lr=py.optimizer.param_groups[0]["lr"], beta1=0.9, beta2=0.999, eps=1e-8,
-                                  lambda_po2pl=cfg["lambda_po2pl"], loss_flags=2 | 4, nb_h=nb[0], nb_w=nb[1],
-                                  epsilon_range=cfg["epsilon_range"],
-                                  min_neighbors=cfg["min_num_points_in_neighborhood_to_determine_point_class"])
     blob = torch.from_numpy(export.pack_state_dict(py.model.state_dict(), cfg)).to(dev)
-    ws_bytes = int(L.delora_odometry_train_workspace_bytes(dp))
-    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
-    st = lambda: ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    _lib.check(L.delora_odometry_train_init(dp, blob.data_ptr(), ws.data_ptr(), st()), "train_init")
+    tr = capi.TrainingWorkspace(export.desc_from_config(cfg, "kitti", n_max, b), blob,
+                                capi.train_params(cfg, py.optimizer.param_groups[0]["lr"]))
+    ws_bytes = tr.workspace.numel()
 
     def c_step(bsz=b):
-        _lib.check(L.delora_odometry_train_step(dp, ctypes.byref(hp), pts.data_ptr(), counts.data_ptr(), bsz,
-                                                ws.data_ptr(), None, None, None, None, st()), "train_step")
+        # B = rows // 2: at bsz < b the step reads the buffer's first 2 * bsz rows (they serve the timing only)
+        tr.step(pts[:2 * bsz], counts[:2 * bsz], outputs=False)
 
     def timed(fn):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -126,9 +116,8 @@ def main():
             kernels["odometry_icp_rearm_kernel (B alternating)"] = {"us_per_call": ev.device_time_total / max(ev.count, 1)}
     c_step(b)
     torch.cuda.synchronize()
-    n = int(L.delora_odometry_weight_floats(dp))
-    floors = {"odometry_adam_kernel": n * 28, "odometry_icp_rearm_kernel (B alternating)":
-              int(L.delora_icp_scratch_floats(b, a.h * a.w)) * 4}
+    floors = {"odometry_adam_kernel": tr.n * 28, "odometry_icp_rearm_kernel (B alternating)":
+              int(_lib.lib().delora_icp_scratch_floats(b, a.h * a.w)) * 4}
     for k, v in kernels.items():
         if k in floors:
             v["bytes"] = floors[k]

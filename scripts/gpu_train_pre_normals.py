@@ -62,7 +62,7 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("no CUDA device: this script measures the GPU")
     from delora_b200 import _lib, ops, synthetic
-    from delora_b200.deploy import export
+    from delora_b200.deploy import capi, export
     from delora_b200.models.model import OdometryModel
     dev = torch.device("cuda:0")
     L = _lib.lib()
@@ -78,10 +78,7 @@ def main():
                 "use_dropout": False, "lambda_po2pl": 1.0})
     torch.manual_seed(0)
     blob = torch.from_numpy(export.pack_state_dict(OdometryModel(cfg).state_dict(), cfg)).to(dev)
-    nb = cfg["kitti"]["neighborhood_side_length"]
-    hp = _lib.OdometryTrainParams(lr=1e-6, beta1=0.9, beta2=0.999, eps=1e-8, lambda_po2pl=1.0, loss_flags=2 | 4,
-                                  nb_h=nb[0], nb_w=nb[1], epsilon_range=cfg["epsilon_range"],
-                                  min_neighbors=cfg["min_num_points_in_neighborhood_to_determine_point_class"])
+    hp = capi.train_params(cfg, 1e-6)
     res = {"card": card(), "H": H, "W": W, "w_pre": W_PRE, "scan_columns": W_RAW, "steps": {}}
 
     for b in batches:
@@ -95,15 +92,10 @@ def main():
         for w_pre in (0, W_PRE):
             d = export.desc_from_config(cfg, "kitti", n_max, b)
             d.w_pre = w_pre
-            ws = torch.empty((int(L.delora_odometry_train_workspace_bytes(ctypes.byref(d))),), dtype=torch.uint8,
-                             device=dev)
-            _lib.check(L.delora_odometry_train_init(ctypes.byref(d), blob.data_ptr(), ws.data_ptr(), st()), "init")
-            runs[w_pre] = (d, ws)
+            runs[w_pre] = capi.TrainingWorkspace(d, blob, hp)
 
         def step(w_pre):
-            d, ws = runs[w_pre]
-            _lib.check(L.delora_odometry_train_step(ctypes.byref(d), ctypes.byref(hp), pts.data_ptr(), counts.data_ptr(),
-                                                    b, ws.data_ptr(), None, None, None, None, st()), "train_step")
+            runs[w_pre].step(pts, counts, outputs=False)
 
         for _ in range(a.warmup):
             step(0)
@@ -123,7 +115,7 @@ def main():
             for w_pre in (0, W_PRE):
                 t[w_pre].append(timed(graphs[w_pre].replay, a.replays))
         deltas = [y - x for x, y in zip(t[0], t[W_PRE])]
-        res["steps"][b] = {"workspace_bytes": {str(k): int(v[1].numel()) for k, v in runs.items()},
+        res["steps"][b] = {"workspace_bytes": {str(k): int(v.workspace.numel()) for k, v in runs.items()},
                            "samples": a.rounds, "replays_per_sample": a.replays,
                            "step_ms_w_pre_0": summary(t[0]), f"step_ms_w_pre_{W_PRE}": summary(t[W_PRE]),
                            "added_ms_paired": summary(deltas)}

@@ -1,0 +1,213 @@
+"""Shared inputs and Python reference steps of the odometry C-ABI tests (test infrastructure, imported like helpers).
+
+Every input is seeded: the scans by their pair index, the models by `seed`.  The scan tuples are cached and shared by
+every module that asks for the same ones, so no caller may modify them in place."""
+import collections
+import copy
+import functools
+import os
+import subprocess
+
+import torch
+
+from delora_b200 import ops
+from helpers import ROOT
+
+DEV = "cuda:0"
+VFOV = (-24.5, 2.0)
+FLAGS = ops.LOSS_PO2PL | ops.LOSS_PL2PL          # SyntheticTrainStep's losses
+# Gradient bounds of the C training step against the Python step, relative to each tensor's max-abs (the reasoning is
+# in test_gpu_odometry_train_capi.py's docstring): the fc / head tensors, and the trunk's
+TAIL_TOL = 5e-6
+TRUNK_TOL = 1e-2
+
+
+def config(h, w, act="tanh", single=False, layers=(2, 2, 2, 2), nout=1000, vfov=VFOV, device=DEV):
+    from delora_b200 import synthetic
+    cfg = synthetic.fov_config(h=h, w=w, vfov_deg=vfov, device=device)
+    cfg.update({"activation_fct": act, "use_single_mlp_at_output": single, "layers": list(layers), "resnet_outputs": nout,
+                "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1, "use_dropout": False})
+    return cfg
+
+
+def model(cfg, seed=0, near_identity=False):
+    """OdometryModel on DEV with torch's initialisation (train mode) after torch.manual_seed(seed).  near_identity:
+    small last layers and the identity quaternion as bias, so T is near I (as after the reference's identity
+    pre-training) and every layer gets a gradient."""
+    from delora_b200.models.model import OdometryModel
+    torch.manual_seed(seed)
+    m = OdometryModel(cfg).to(DEV)
+    if not near_identity:
+        return m
+    with torch.no_grad():
+        if cfg["use_single_mlp_at_output"]:
+            last = m.fully_connected_rot_trans[-1]
+            last.weight.mul_(0.01)
+            last.bias.copy_(torch.tensor([0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0]))
+        else:
+            for head, bias in ((m.fully_connected_rotation, [0.0, 0.0, 0.0, 1.0]),
+                               (m.fully_connected_translation, [0.0, 0.0, 0.0])):
+                head[3].weight.mul_(0.01)
+                head[3].bias.copy_(torch.tensor(bias))
+    return m
+
+
+@functools.lru_cache(maxsize=None)
+def pairs(rings, w_raw, count):
+    """(scan_1, scan_2) of synthetic pairs 0 .. count-1."""
+    from delora_b200 import synthetic
+    return tuple(synthetic.make_pair(i, w_raw=w_raw, rings=rings, vfov_deg=VFOV)[:2] for i in range(count))
+
+
+def frames(rings, w_raw, count):
+    """Consecutive synthetic frames: scan_1, scan_2 of pair 0, scan_1, scan_2 of pair 1, ..."""
+    return tuple(s for p in pairs(rings, w_raw, (count + 1) // 2) for s in p)[:count]
+
+
+def n_stride(pair_list):
+    return max(max(a.shape[1], b.shape[1]) for a, b in pair_list)
+
+
+def stack(scans, stride):
+    """Scans -> points [len, 3, n_stride] (zero padded) and counts [len] on DEV."""
+    pts = torch.zeros((len(scans), 3, stride), dtype=torch.float32)
+    for i, s in enumerate(scans):
+        pts[i, :, :s.shape[1]] = s
+    counts = torch.tensor([s.shape[1] for s in scans], dtype=torch.int32)
+    return pts.to(DEV), counts.to(DEV)
+
+
+def stack_pairs(pair_list, stride):
+    """The rows of a step on these pairs: scan_1 x B, then scan_2 x B."""
+    return stack([p[0] for p in pair_list] + [p[1] for p in pair_list], stride)
+
+
+def blob(m, cfg):
+    from delora_b200.deploy import export
+    return torch.from_numpy(export.pack_state_dict(m.state_dict(), cfg)).to(DEV)
+
+
+def desc(cfg, stride, max_batch, w_pre=0):
+    from delora_b200.deploy import export
+    d = export.desc_from_config(cfg, "kitti", stride, max_batch)
+    d.w_pre = w_pre
+    return d
+
+
+def trainer(cfg, stride, max_batch, weights, lr=1e-5, w_pre=0, flags=FLAGS):
+    from delora_b200.deploy import capi
+    return capi.TrainingWorkspace(desc(cfg, stride, max_batch, w_pre), weights,
+                                  capi.train_params(cfg, lr, loss_flags=flags))
+
+
+def _preprocessed_lists(cfg, pts, counts, w_pre):
+    """The offline stage (Preprocesser.preprocess_scans at horizontal_cells_preprocessing = w_pre) of every scan ->
+    padded channels-first point and normal lists [2B, 3, P] and their lengths [2B]."""
+    from delora_b200.preprocessing.normal_computation import NormalsComputer
+    from delora_b200.preprocessing.preprocesser import Preprocesser
+    pcfg = copy.deepcopy(cfg)
+    pcfg["dataset"] = "kitti"
+    pcfg["kitti"]["horizontal_cells"] = w_pre
+    pre = Preprocesser(config=pcfg)
+    pre.normals_computer = NormalsComputer(config=pcfg, dataset_name="kitti")
+    n_host = counts.cpu().tolist()
+    out = pre.preprocess_scans([pts[i, :, :n].cpu() for i, n in enumerate(n_host)])
+    p_max = max(max(p.shape[0] for _, p in out), 1)
+    plist = torch.zeros((len(out), 3, p_max), dtype=torch.float32)
+    nlist = torch.zeros_like(plist)
+    for i, (nrm, p) in enumerate(out):
+        plist[i, :, :p.shape[0]] = torch.from_numpy(p).t()
+        nlist[i, :, :nrm.shape[0]] = torch.from_numpy(nrm).t()
+    lens = torch.tensor([p.shape[0] for _, p in out], dtype=torch.int32)
+    return plist.to(DEV), nlist.to(DEV), lens.to(DEV)
+
+
+Step = collections.namedtuple("Step", "losses T pooled grads objective")
+
+
+def python_step(m, cfg, pts, counts, w_pre=0, identity=False):
+    """SyntheticTrainStep.step without the optimizer -> Step(losses [B,8], T [B,4,4], pooled [B,512], {name: grad},
+    objective).
+
+    w_pre > 0: the reference's two-resolution recipe through the mirror -- Preprocesser.preprocess_scans in memory (the
+    offline stage's row-major point and normal lists), ops.project at W and ops.grids_from_projection
+    (Deployer.step); otherwise ops.project + ops.normals at W.  Then OdometryModel's training forward (TensorCoreEncoder
+    with autograd, torch heads), GeometryHandler's quaternion -> T and the fused ICP losses.  The objective is their
+    mean over the pairs, or with identity that of unsupervised_at_start: False (delora_b200/deploy/deployer.py:206-210),
+    MSELoss(T_{B-1}, I) / B."""
+    from delora_b200.deploy.deployer import _FusedIcp
+    from delora_b200.models.model_parts import GeometryHandler
+    ds = cfg["kitti"]
+    h, w = ds["vertical_cells"], ds["horizontal_cells"]
+    hf, vf = tuple(cfg["horizontal_field_of_view"]), tuple(ds["vertical_field_of_view"])
+    b = pts.shape[0] // 2
+    if w_pre > 0:
+        plist, nlist, lens = _preprocessed_lists(cfg, pts, counts, w_pre)
+        image, imap = ops.project(plist, lens, h, w, hf, vf)
+        pg, ng = ops.grids_from_projection(plist, nlist, imap)
+    else:
+        image, _ = ops.project(pts, counts, h, w, hf, vf)
+        _, pg, ng = ops.normals(image, ds["neighborhood_side_length"], cfg["epsilon_range"],
+                                cfg["min_num_points_in_neighborhood_to_determine_point_class"], grids=True)
+    img1, img2 = image[:b].contiguous(), image[b:].contiguous()
+    with torch.no_grad():
+        pooled = m._tensor_core_path().pooled_features(img1, img2)
+    m.zero_grad(set_to_none=True)
+    trans, quat = m(image_1=img1, image_2=img2)
+    T = GeometryHandler.get_transformation_matrix_quaternion(trans.float(), quat.float(), DEV)
+    total, parts = _FusedIcp.apply(T, pg[b:].contiguous(), ng[b:].contiguous(), pg[:b].contiguous(),
+                                   ng[:b].contiguous(), (h, w, hf, vf), float(cfg["lambda_po2pl"]), FLAGS,
+                                   ops.icp_scratch(b, h * w, pts.device))
+    if identity:
+        eye = torch.eye(4, device=DEV).view(1, 4, 4)
+        loss = torch.nn.MSELoss()(T[-1:], eye) / b
+    else:
+        loss = total.mean()
+    loss.backward()
+    grads = {k: p.grad.detach().clone() for k, p in m.named_parameters()}
+    return Step(parts.detach(), T.detach(), pooled, grads, loss.item())
+
+
+def grad_dict(flat, cfg):
+    from delora_b200.deploy import export
+    return export.unpack_blob(flat.cpu().numpy(), cfg)
+
+
+def _is_tail(name):
+    return name.startswith("resnet.fc") or name.startswith("fully_connected")
+
+
+def grad_spread(c_grads, py_grads):
+    """-> (worst relative error of the tail tensors, of the trunk tensors), relative to each tensor's max-abs."""
+    worst = {True: 0.0, False: 0.0}
+    for k, ref in py_grads.items():
+        ref = ref.cpu()
+        scale = ref.abs().max().item()
+        assert scale > 0, f"{k}: zero gradient in the Python step"
+        err = (c_grads[k] - ref).abs().max().item() / scale
+        worst[_is_tail(k)] = max(worst[_is_tail(k)], err)
+    return worst[True], worst[False]
+
+
+def rel(a, b):
+    return ((a - b).abs().max() / b.abs().max().clamp_min(1e-30)).item()
+
+
+def build_example(name, out_dir, link):
+    """nvcc examples/<name>.c against include/delora_b200.h: link=False compiles it with -Wall -Werror to an object,
+    link=True links an executable against the built libdelora_b200.so.  -> the output path."""
+    from delora_b200 import build
+    nvcc = build._nvcc()
+    cuda_inc = os.path.join(os.path.dirname(os.path.dirname(os.path.realpath(nvcc))), "include")
+    cmd = [nvcc] + ([] if link else ["-c"]) + [os.path.join(ROOT, "examples", f"{name}.c"), "-I",
+                                               os.path.join(ROOT, "include"), "-I", cuda_inc]
+    if link:
+        libdir = os.path.dirname(build.LIB)
+        out = os.path.join(out_dir, name)
+        cmd += ["-L", libdir, "-ldelora_b200", "-lcudart", "-Xlinker", "-rpath=" + libdir]
+    else:
+        out = os.path.join(out_dir, f"{name}.o")
+        cmd += ["-Xcompiler", "-Wall,-Werror"]
+    r = subprocess.run(cmd + ["-o", out], capture_output=True, text=True)
+    assert r.returncode == 0, r.stdout + r.stderr
+    return out

@@ -4,8 +4,6 @@ Every stream's T row is byte-equal to a delora_odometry_push workspace fed only 
 seeded activity pattern with idle ticks, all-active ticks, a late start, a reset, an empty frame and a count above
 n_stride.  Inactive streams are staged with another stream's points and a non-zero count, so the mask is what keeps
 them out."""
-import ctypes
-import functools
 import math
 import os
 import subprocess
@@ -14,37 +12,13 @@ import numpy as np
 import pytest
 import torch
 
+import odometry_harness as H
+from delora_b200.deploy.capi import InferenceWorkspace, StreamsWorkspace
 from helpers import ROOT
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-VFOV = (-24.5, 2.0)
+DEV = H.DEV
 TICKS = 8
-
-
-def _config(h, w, act="tanh", single=False, vfov=VFOV, layers=(2, 2, 2, 2)):
-    from delora_b200 import synthetic
-    cfg = synthetic.fov_config(h=h, w=w, vfov_deg=vfov, device=DEV)
-    cfg.update({"activation_fct": act, "use_single_mlp_at_output": single, "layers": list(layers),
-                "resnet_outputs": 1000, "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1,
-                "use_dropout": False})
-    return cfg
-
-
-def _model(cfg, seed=0):
-    from delora_b200.models.model import OdometryModel
-    torch.manual_seed(seed)
-    return OdometryModel(cfg).to(DEV).eval()
-
-
-@functools.lru_cache(maxsize=None)
-def _pool(rings, w_raw):
-    from delora_b200 import synthetic
-    out = []
-    for i in range(3):
-        s1, s2, _, _ = synthetic.make_pair(i, w_raw=w_raw, rings=rings, vfov_deg=VFOV)
-        out += [s1, s2]
-    return tuple(out)
 
 
 def _frame(pool, s, k):
@@ -69,45 +43,6 @@ def _pattern(S, seed):
     return act, override, {4: [0]}
 
 
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _blob(model, cfg):
-    from delora_b200.deploy import export
-    return torch.from_numpy(export.pack_state_dict(model.state_dict(), cfg)).to(DEV)
-
-
-class _Streams:
-    def __init__(self, cfg, n_stride, S, blob, extra=0):
-        from delora_b200 import _lib
-        from delora_b200.deploy import export
-        self.L, self.S = _lib.lib(), S
-        self.d = export.desc_from_config(cfg, "kitti", n_stride, S)
-        self.dp = ctypes.byref(self.d)
-        self.nbytes = int(self.L.delora_odometry_streams_workspace_bytes(self.dp))
-        self.ws = torch.empty((self.nbytes + extra,), dtype=torch.uint8, device=DEV)
-        if extra:
-            self.ws[self.nbytes:] = torch.arange(extra, device=DEV).to(torch.uint8) ^ 0xA5
-        _lib.check(self.L.delora_odometry_streams_init(self.dp, self.ws.data_ptr(), _stream()), "streams_init")
-        _lib.check(self.L.delora_odometry_streams_load_weights(self.dp, blob.data_ptr(), self.ws.data_ptr(), _stream()),
-                   "streams_load_weights")
-
-    def push(self, pts, counts, active, T, valid):
-        from delora_b200 import _lib
-        _lib.check(self.L.delora_odometry_streams_push(self.dp, pts.data_ptr(), counts.data_ptr(),
-                                                       active.data_ptr() if active is not None else None,
-                                                       self.ws.data_ptr(), T.data_ptr(), valid.data_ptr(), _stream()),
-                   "streams_push")
-
-    def reset(self, streams):
-        from delora_b200 import _lib
-        mask = torch.zeros((self.S,), dtype=torch.int32, device=DEV)
-        mask[list(streams)] = 1
-        _lib.check(self.L.delora_odometry_streams_reset(self.dp, mask.data_ptr(), self.ws.data_ptr(), _stream()),
-                   "streams_reset")
-
-
 def _ticks(pool, S, n_stride, act, override):
     """Host staging of every tick: points [S, 3, n_stride], counts [S], active [S]."""
     out = []
@@ -126,18 +61,11 @@ def _ticks(pool, S, n_stride, act, override):
 
 def _push_reference(cfg, n_stride, blob, ticks, act, resets):
     """Per stream, one delora_odometry_push workspace fed only that stream's active frames -> {(k, s): T bytes}."""
-    from delora_b200 import _lib
-    from delora_b200.deploy import export
-    L = _lib.lib()
-    d = export.desc_from_config(cfg, "kitti", n_stride, 1)
-    dp = ctypes.byref(d)
-    ws = torch.empty((int(L.delora_odometry_workspace_bytes(dp)),), dtype=torch.uint8, device=DEV)
     t = torch.empty((16,), dtype=torch.float32, device=DEV)
     want = {}
     S = act.shape[1]
     for s in range(S):
-        _lib.check(L.delora_odometry_init(dp, ws.data_ptr(), _stream()), "init")
-        _lib.check(L.delora_odometry_load_weights(dp, blob.data_ptr(), ws.data_ptr(), _stream()), "load")
+        ws = InferenceWorkspace(H.desc(cfg, n_stride, 1), blob)
         has = False
         for k, (pts, counts, _) in enumerate(ticks):
             if s in resets.get(k, []):
@@ -146,8 +74,7 @@ def _push_reference(cfg, n_stride, blob, ticks, act, resets):
                 continue
             p = pts[s:s + 1].to(DEV)
             c = counts[s:s + 1].to(DEV)
-            _lib.check(L.delora_odometry_push(dp, p.data_ptr(), c.data_ptr(), ws.data_ptr(),
-                                              t.data_ptr() if has else None, _stream()), "push")
+            ws.push(p, c, t if has else None)
             if has:
                 want[(k, s)] = t.clone()
             has = True
@@ -160,7 +87,7 @@ SENTINEL = 1234.5
 
 def _run_streams(st, ticks, resets, graph=False):
     """All ticks through one streams workspace -> list of (T [S, 16] cpu, valid [S] cpu) after each tick."""
-    S = st.S
+    S = st.desc.max_batch
     n_stride = ticks[0][0].shape[2]
     pts = torch.zeros((S, 3, n_stride), dtype=torch.float32, device=DEV)
     counts = torch.zeros((S,), dtype=torch.int32, device=DEV)
@@ -178,7 +105,9 @@ def _run_streams(st, ticks, resets, graph=False):
     out = []
     for k, (p, c, a) in enumerate(ticks):
         if k in resets:
-            st.reset(resets[k])
+            mask = torch.zeros((S,), dtype=torch.int32, device=DEV)
+            mask[list(resets[k])] = 1
+            st.reset(mask)
         pts.copy_(p)
         counts.copy_(c)
         active.copy_(a)
@@ -222,34 +151,34 @@ SIZES = [(64, 2048, 2048), (64, 720, 1024), (64, 2047, 2048)]     # H, W, w_raw;
 @pytest.mark.parametrize("act_fn", ["tanh", "relu"])
 @pytest.mark.parametrize("h,w,w_raw", SIZES)
 def test_rows_are_bit_identical_to_push(cuda_lib, h, w, w_raw, act_fn, S):
-    cfg = _config(h, w, act_fn)
-    blob = _blob(_model(cfg), cfg)
-    pool = _pool(h, w_raw)
+    cfg = H.config(h, w, act_fn)
+    blob = H.blob(H.model(cfg).eval(), cfg)
+    pool = H.frames(h, w_raw, 6)
     n_stride = max(s.shape[1] for s in pool) + 64
     act, override, resets = _pattern(S, seed=S * 31 + w)
     ticks = _ticks(pool, S, n_stride, act, override)
     want = _push_reference(cfg, n_stride, blob, ticks, act, resets)
-    out = _run_streams(_Streams(cfg, n_stride, S, blob), ticks, resets)
+    out = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, S), blob), ticks, resets)
     assert _check_against_push(out, want, act, resets) == len(want) > 0
 
 
 @pytest.mark.parametrize("act_fn", ["tanh", "relu"])
 def test_single_mlp_head_rows_are_bit_identical_to_push(cuda_lib, act_fn):
-    cfg = _config(64, 720, act_fn, single=True)
-    blob = _blob(_model(cfg, 2), cfg)
-    pool = _pool(64, 1024)
+    cfg = H.config(64, 720, act_fn, single=True)
+    blob = H.blob(H.model(cfg, 2).eval(), cfg)
+    pool = H.frames(64, 1024, 6)
     n_stride = max(s.shape[1] for s in pool) + 64
     act, override, resets = _pattern(3, seed=5)
     ticks = _ticks(pool, 3, n_stride, act, override)
     want = _push_reference(cfg, n_stride, blob, ticks, act, resets)
-    out = _run_streams(_Streams(cfg, n_stride, 3, blob), ticks, resets)
+    out = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 3), blob), ticks, resets)
     assert _check_against_push(out, want, act, resets) == len(want) > 0
 
 
 def _small_setup(S=4, w=720, seed=9):
-    cfg = _config(64, w)
-    blob = _blob(_model(cfg, 1), cfg)
-    pool = _pool(64, 1024)
+    cfg = H.config(64, w)
+    blob = H.blob(H.model(cfg, 1).eval(), cfg)
+    pool = H.frames(64, 1024, 6)
     n_stride = max(s.shape[1] for s in pool) + 64
     act, override, resets = _pattern(S, seed=seed)
     return cfg, blob, n_stride, _ticks(pool, S, n_stride, act, override), act, resets
@@ -257,8 +186,8 @@ def _small_setup(S=4, w=720, seed=9):
 
 def test_graph_replay_matches_eager(cuda_lib):
     cfg, blob, n_stride, ticks, act, resets = _small_setup()
-    eager = _run_streams(_Streams(cfg, n_stride, 4, blob), ticks, resets)
-    graphed = _run_streams(_Streams(cfg, n_stride, 4, blob), ticks, resets, graph=True)
+    eager = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 4), blob), ticks, resets)
+    graphed = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 4), blob), ticks, resets, graph=True)
     for k, ((te, ve), (tg, vg)) in enumerate(zip(eager, graphed)):
         assert torch.equal(ve, vg), f"tick {k}: valid differs"
         assert torch.equal(_bits(te), _bits(tg)), f"tick {k}: graph replay differs from the eager call"
@@ -266,8 +195,8 @@ def test_graph_replay_matches_eager(cuda_lib):
 
 def test_deterministic(cuda_lib):
     cfg, blob, n_stride, ticks, act, resets = _small_setup(S=3, seed=4)
-    a = _run_streams(_Streams(cfg, n_stride, 3, blob), ticks, resets)
-    b = _run_streams(_Streams(cfg, n_stride, 3, blob), ticks, resets)
+    a = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 3), blob), ticks, resets)
+    b = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 3), blob), ticks, resets)
     for (ta, va), (tb, vb) in zip(a, b):
         assert torch.equal(va, vb) and torch.equal(_bits(ta), _bits(tb))
 
@@ -275,8 +204,8 @@ def test_deterministic(cuda_lib):
 def test_null_active_means_all_active(cuda_lib):
     cfg, blob, n_stride, ticks, _, _ = _small_setup(S=3, seed=6)
     all_on = [(p, c, torch.ones_like(a)) for p, c, a in ticks[:3]]
-    a = _run_streams(_Streams(cfg, n_stride, 3, blob), all_on, {})
-    st = _Streams(cfg, n_stride, 3, blob)
+    a = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 3), blob), all_on, {})
+    st = StreamsWorkspace(H.desc(cfg, n_stride, 3), blob)
     T = torch.full((3, 16), SENTINEL, device=DEV)
     valid = torch.zeros((3,), dtype=torch.int32, device=DEV)
     for k, (p, c, _) in enumerate(all_on):
@@ -287,14 +216,14 @@ def test_null_active_means_all_active(cuda_lib):
 
 def test_inactive_stream_keeps_its_cached_frame(cuda_lib):
     """Stream 1 sits out ticks 1..3 while the others run; at tick 4 it continues from its tick-0 frame."""
-    cfg = _config(64, 720)
-    blob = _blob(_model(cfg, 3), cfg)
-    pool = _pool(64, 1024)
+    cfg = H.config(64, 720)
+    blob = H.blob(H.model(cfg, 3).eval(), cfg)
+    pool = H.frames(64, 1024, 6)
     n_stride = max(s.shape[1] for s in pool) + 64
     act = np.ones((5, 3), dtype=bool)
     act[1:4, 1] = False
     ticks = _ticks(pool, 3, n_stride, act, {})
-    out = _run_streams(_Streams(cfg, n_stride, 3, blob), ticks, {})
+    out = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 3), blob), ticks, {})
     assert [int(v[1]) for _, v in out] == [0, 0, 0, 0, 1]
     want = _push_reference(cfg, n_stride, blob, [ticks[0], ticks[4]], act[[0, 4]], {})
     assert torch.equal(_bits(out[4][0][1]), _bits(want[(1, 1)]))
@@ -304,20 +233,24 @@ def test_inactive_stream_keeps_its_cached_frame(cuda_lib):
 @pytest.mark.parametrize("w", [720, 2047])
 def test_workspace_bounds(cuda_lib, w):
     cfg, blob, n_stride, ticks, act, resets = _small_setup(S=3, w=w, seed=8)
-    st = _Streams(cfg, n_stride, 3, blob, extra=4096)
-    canary = st.ws[st.nbytes:].clone()
+    d = H.desc(cfg, n_stride, 3)
+    nbytes, extra = StreamsWorkspace.workspace_bytes(d), 4096
+    ws = torch.empty((nbytes + extra,), dtype=torch.uint8, device=DEV)
+    ws[nbytes:] = torch.arange(extra, device=DEV).to(torch.uint8) ^ 0xA5
+    st = StreamsWorkspace(d, blob, workspace=ws)
+    canary = ws[nbytes:].clone()
     _run_streams(st, ticks, resets)
     torch.cuda.synchronize()
-    assert torch.equal(st.ws[st.nbytes:], canary), "a streams call wrote past delora_odometry_streams_workspace_bytes"
+    assert torch.equal(ws[nbytes:], canary), "a streams call wrote past delora_odometry_streams_workspace_bytes"
 
 
 @pytest.mark.parametrize("use_graph", [True, False])
 def test_python_class_matches_push_and_the_torch_stream(cuda_lib, use_graph):
     from delora_b200.deploy.stream import OdometryStream, OdometryStreams
-    cfg = _config(64, 720)
-    model = _model(cfg, 4)
-    blob = _blob(model, cfg)
-    pool = _pool(64, 1024)
+    cfg = H.config(64, 720)
+    model = H.model(cfg, 4).eval()
+    blob = H.blob(model, cfg)
+    pool = H.frames(64, 1024, 6)
     n_max = max(s.shape[1] for s in pool) + 64
     S = 3
     act = np.ones((6, S), dtype=bool)
@@ -343,16 +276,9 @@ def test_python_class_matches_push_and_the_torch_stream(cuda_lib, use_graph):
                 assert res[s].shape == (1, 4, 4)
         got.append(res)
     # bit for bit against per-stream _push workspaces
-    from delora_b200 import _lib
-    from delora_b200.deploy import export
-    L = _lib.lib()
-    d = export.desc_from_config(cfg, "kitti", n_max, 1)
-    dp = ctypes.byref(d)
-    ws = torch.empty((int(L.delora_odometry_workspace_bytes(dp)),), dtype=torch.uint8, device=DEV)
     t = torch.empty((16,), dtype=torch.float32, device=DEV)
     for s in range(S):
-        _lib.check(L.delora_odometry_init(dp, ws.data_ptr(), _stream()), "init")
-        _lib.check(L.delora_odometry_load_weights(dp, blob.data_ptr(), ws.data_ptr(), _stream()), "load")
+        ws = InferenceWorkspace(H.desc(cfg, n_max, 1), blob)
         has = False
         for k in range(act.shape[0]):
             if s in resets.get(k, []):
@@ -360,13 +286,8 @@ def test_python_class_matches_push_and_the_torch_stream(cuda_lib, use_graph):
             if not act[k, s]:
                 assert got[k][s] is None
                 continue
-            f = _frame(pool, s, k)
-            p = torch.zeros((1, 3, n_max), dtype=torch.float32)
-            p[0, :, :f.shape[1]] = f
-            c = torch.tensor([f.shape[1]], dtype=torch.int32)
-            p, c = p.to(DEV), c.to(DEV)
-            _lib.check(L.delora_odometry_push(dp, p.data_ptr(), c.data_ptr(), ws.data_ptr(),
-                                              t.data_ptr() if has else None, _stream()), "push")
+            p, c = H.stack([_frame(pool, s, k)], n_max)
+            ws.push(p, c, t if has else None)
             torch.cuda.synchronize()
             if has:
                 assert got[k][s] is not None and got[k][s].tobytes() == t.cpu().numpy().tobytes(), (k, s)
@@ -380,11 +301,11 @@ def test_python_class_matches_push_and_the_torch_stream(cuda_lib, use_graph):
 def test_example_program(cuda_lib, tmp_path):
     """examples/odometry_streams.c on two stream directories of 3 and 2 KITTI .bin scans prints what _lib computes."""
     import sys
-    from delora_b200 import build, synthetic
+    from delora_b200 import synthetic
     from delora_b200.deploy import export
     vfov = (-15.0, 15.0)
-    cfg = _config(16, 720, vfov=vfov, layers=(1, 1, 1, 1))
-    model = _model(cfg, 5)
+    cfg = H.config(16, 720, vfov=vfov, layers=(1, 1, 1, 1))
+    model = H.model(cfg, 5).eval()
     ckpt = os.path.join(tmp_path, "ckpt.pth")
     torch.save({"model_state_dict": model.state_dict(), "parameters": dict(cfg, device="cpu")}, ckpt)
     dlw = os.path.join(tmp_path, "model.dlw")
@@ -403,14 +324,7 @@ def test_example_program(cuda_lib, tmp_path):
             synthetic.kitti_bin_scan(10 * s + i, vfov_deg=vfov).tofile(path)
             mine.append(torch.from_numpy(np.fromfile(path, dtype=np.float32).reshape(-1, 4)[:, :3].T.copy()))
         scans.append(mine)
-    nvcc = build._nvcc()
-    cuda_home = os.path.dirname(os.path.dirname(os.path.realpath(nvcc)))
-    libdir = os.path.dirname(build.LIB)
-    exe = os.path.join(tmp_path, "odometry_streams")
-    r = subprocess.run([nvcc, os.path.join(ROOT, "examples", "odometry_streams.c"), "-I", os.path.join(ROOT, "include"),
-                        "-I", os.path.join(cuda_home, "include"), "-L", libdir, "-ldelora_b200", "-lcudart",
-                        "-Xlinker", "-rpath=" + libdir, "-o", exe], capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
+    exe = H.build_example("odometry_streams", tmp_path, link=True)
     r = subprocess.run([exe, dlw] + dirs, capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, r.stderr
     lines = [line.split() for line in r.stdout.strip().splitlines()]
@@ -420,7 +334,7 @@ def test_example_program(cuda_lib, tmp_path):
     _, d, blob = export.read_dlw(dlw)
     blob_dev = torch.from_numpy(blob).to(DEV)
     S = len(lengths)
-    st = _Streams(cfg, d.n_stride, S, blob_dev)
+    st = StreamsWorkspace(H.desc(cfg, d.n_stride, S), blob_dev)
     T = torch.zeros((S, 16), dtype=torch.float32, device=DEV)
     valid = torch.zeros((S,), dtype=torch.int32, device=DEV)
     want = []

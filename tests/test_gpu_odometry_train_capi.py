@@ -13,166 +13,18 @@ Measured on an H100 over the 16 size x variant cases: tail <= 4.8e-7, trunk <= 6
 relu cases are often bit-identical: relu' does not depend on the bits of the activation).  The bounds leave a 10x
 (tail) and 1.7x (trunk) margin.
 """
-import ctypes
-import functools
+import os
+import subprocess
 
 import numpy as np
 import pytest
 import torch
 
+import odometry_harness as H
+from delora_b200.deploy.capi import InferenceWorkspace
+
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-VFOV = (-24.5, 2.0)
-FLAGS = 2 | 4                      # DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL, SyntheticTrainStep's losses
-TAIL_TOL = 5e-6
-TRUNK_TOL = 1e-2
-
-
-def _config(h, w, act="tanh", single=False, layers=(2, 2, 2, 2), nout=1000):
-    from delora_b200 import synthetic
-    cfg = synthetic.fov_config(h=h, w=w, vfov_deg=VFOV, device=DEV)
-    cfg.update({"activation_fct": act, "use_single_mlp_at_output": single, "layers": list(layers), "resnet_outputs": nout,
-                "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1, "use_dropout": False})
-    return cfg
-
-
-def _model(cfg, seed=0):
-    """Random weights with small last layers and the identity quaternion as bias: T near I (as after the reference's
-    identity pre-training), and every layer gets a gradient."""
-    from delora_b200.models.model import OdometryModel
-    torch.manual_seed(seed)
-    m = OdometryModel(cfg).to(DEV)
-    with torch.no_grad():
-        if cfg["use_single_mlp_at_output"]:
-            last = m.fully_connected_rot_trans[-1]
-            last.weight.mul_(0.01)
-            last.bias.copy_(torch.tensor([0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0]))
-        else:
-            for head, bias in ((m.fully_connected_rotation, [0.0, 0.0, 0.0, 1.0]),
-                               (m.fully_connected_translation, [0.0, 0.0, 0.0])):
-                head[3].weight.mul_(0.01)
-                head[3].bias.copy_(torch.tensor(bias))
-    return m
-
-
-@functools.lru_cache(maxsize=None)
-def _pairs(rings, w_raw, count):
-    from delora_b200 import synthetic
-    return tuple(synthetic.make_pair(i, w_raw=w_raw, rings=rings, vfov_deg=VFOV)[:2] for i in range(count))
-
-
-def _stack(pairs, n_stride):
-    scans = [p[0] for p in pairs] + [p[1] for p in pairs]              # scan_1 x B, then scan_2 x B
-    pts = torch.zeros((len(scans), 3, n_stride), dtype=torch.float32)
-    for i, s in enumerate(scans):
-        pts[i, :, :s.shape[1]] = s
-    counts = torch.tensor([s.shape[1] for s in scans], dtype=torch.int32)
-    return pts.to(DEV), counts.to(DEV)
-
-
-def _n_stride(pairs):
-    return max(max(a.shape[1], b.shape[1]) for a, b in pairs)
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _blob(model, cfg):
-    from delora_b200.deploy import export
-    return torch.from_numpy(export.pack_state_dict(model.state_dict(), cfg)).to(DEV)
-
-
-class _Trainer:
-    """Test-side holder of one descriptor + training workspace (device memory from torch)."""
-
-    def __init__(self, cfg, n_stride, max_batch, blob, lr=1e-5):
-        from delora_b200 import _lib
-        from delora_b200.deploy import export
-        self.L, self.cfg = _lib.lib(), cfg
-        self.d = export.desc_from_config(cfg, "kitti", n_stride, max_batch)
-        self.dp = ctypes.byref(self.d)
-        self.n = int(self.L.delora_odometry_weight_floats(self.dp))
-        nb = cfg["kitti"]["neighborhood_side_length"]
-        self.hp = _lib.OdometryTrainParams(
-            lr=lr, beta1=0.9, beta2=0.999, eps=1e-8, lambda_po2pl=cfg["lambda_po2pl"], loss_flags=FLAGS, nb_h=nb[0],
-            nb_w=nb[1], epsilon_range=cfg["epsilon_range"],
-            min_neighbors=cfg["min_num_points_in_neighborhood_to_determine_point_class"])
-        self.ws = torch.empty((int(self.L.delora_odometry_train_workspace_bytes(self.dp)),), dtype=torch.uint8,
-                              device=DEV)
-        _lib.check(self.L.delora_odometry_train_init(self.dp, blob.data_ptr(), self.ws.data_ptr(), _stream()),
-                   "delora_odometry_train_init")
-
-    def step(self, pts, counts, outputs=True):
-        from delora_b200 import _lib
-        b = pts.shape[0] // 2
-        out = None
-        if outputs:
-            out = (torch.empty((b, 8), device=DEV), torch.empty((b, 4, 4), device=DEV), torch.empty((b, 512), device=DEV),
-                   torch.empty((self.n,), device=DEV))
-        ptr = (lambda i: out[i].data_ptr()) if outputs else (lambda i: None)
-        _lib.check(self.L.delora_odometry_train_step(self.dp, ctypes.byref(self.hp), pts.data_ptr(), counts.data_ptr(), b,
-                                                     self.ws.data_ptr(), ptr(0), ptr(1), ptr(2), ptr(3), _stream()),
-                   "delora_odometry_train_step")
-        return out
-
-    def weights(self):
-        from delora_b200 import _lib
-        w = torch.empty((self.n,), device=DEV)
-        _lib.check(self.L.delora_odometry_train_weights(self.dp, self.ws.data_ptr(), w.data_ptr(), _stream()),
-                   "delora_odometry_train_weights")
-        return w
-
-
-def _python_step(model, cfg, pts, counts):
-    """SyntheticTrainStep.step without the optimizer: -> (losses [B,8], T [B,4,4], pooled [B,512], {name: grad})."""
-    from delora_b200 import ops
-    from delora_b200.deploy.deployer import _FusedIcp
-    from delora_b200.models.model_parts import GeometryHandler
-    ds = cfg["kitti"]
-    h, w = ds["vertical_cells"], ds["horizontal_cells"]
-    hf, vf = tuple(cfg["horizontal_field_of_view"]), tuple(ds["vertical_field_of_view"])
-    b = pts.shape[0] // 2
-    image, _ = ops.project(pts, counts, h, w, hf, vf)
-    _, pg, ng = ops.normals(image, ds["neighborhood_side_length"], cfg["epsilon_range"],
-                            cfg["min_num_points_in_neighborhood_to_determine_point_class"], grids=True)
-    img1, img2 = image[:b].contiguous(), image[b:].contiguous()
-    with torch.no_grad():
-        pooled = model._tensor_core_path().pooled_features(img1, img2)
-    model.zero_grad(set_to_none=True)
-    trans, quat = model(image_1=img1, image_2=img2)
-    T = GeometryHandler.get_transformation_matrix_quaternion(trans.float(), quat.float(), DEV)
-    total, parts = _FusedIcp.apply(T, pg[b:].contiguous(), ng[b:].contiguous(), pg[:b].contiguous(),
-                                   ng[:b].contiguous(), (h, w, hf, vf), float(cfg["lambda_po2pl"]), FLAGS,
-                                   ops.icp_scratch(b, h * w, pts.device))
-    total.mean().backward()
-    grads = {k: p.grad.detach().clone() for k, p in model.named_parameters()}
-    return parts.detach(), T.detach(), pooled, grads
-
-
-def _grad_dict(flat, cfg):
-    from delora_b200.deploy import export
-    return export.unpack_blob(flat.cpu().numpy(), cfg)
-
-
-def _is_tail(name):
-    return name.startswith("resnet.fc") or name.startswith("fully_connected")
-
-
-def _grad_spread(c_grads, py_grads):
-    """-> (worst relative error of the tail tensors, of the trunk tensors), relative to each tensor's max-abs."""
-    worst = {True: 0.0, False: 0.0}
-    for k, ref in py_grads.items():
-        ref = ref.cpu()
-        scale = ref.abs().max().item()
-        assert scale > 0, f"{k}: zero gradient in the Python step"
-        err = (c_grads[k] - ref).abs().max().item() / scale
-        worst[_is_tail(k)] = max(worst[_is_tail(k)], err)
-    return worst[True], worst[False]
-
-
-def _rel(a, b):
-    return ((a - b).abs().max() / b.abs().max().clamp_min(1e-30)).item()
+DEV = H.DEV
 
 
 SIZES = [(64, 2048, 2048, 4), (64, 720, 1024, 2), (16, 720, 1024, 2), (16, 259, 512, 2)]     # H, W, w_raw, B
@@ -187,25 +39,25 @@ STEP_CASES = ([pytest.param(act, single, *size, 1000, id="-".join(map(str, (act,
 
 @pytest.mark.parametrize("act,single,h,w,w_raw,b,nout", STEP_CASES)
 def test_step_matches_the_python_training_step(cuda_lib, h, w, w_raw, b, act, single, nout):
-    cfg = _config(h, w, act, single, nout=nout)
-    model = _model(cfg)
-    pairs = _pairs(h, w_raw, b)
-    n_stride = _n_stride(pairs)
-    pts, counts = _stack(pairs, n_stride)
-    tr = _Trainer(cfg, n_stride, b, _blob(model, cfg))
+    cfg = H.config(h, w, act, single, nout=nout)
+    model = H.model(cfg, near_identity=True)
+    pairs = H.pairs(h, w_raw, b)
+    n_stride = H.n_stride(pairs)
+    pts, counts = H.stack_pairs(pairs, n_stride)
+    tr = H.trainer(cfg, n_stride, b, H.blob(model, cfg))
     losses, T, pooled, grads = tr.step(pts, counts)
-    py_losses, py_T, py_pooled, py_grads = _python_step(model, cfg, pts, counts)
+    py = H.python_step(model, cfg, pts, counts)
     torch.cuda.synchronize()
-    assert torch.equal(pooled, py_pooled), "pooled features differ from TensorCoreEncoder.pooled_features"
-    t_err = (T - py_T).abs().max().item()
+    assert torch.equal(pooled, py.pooled), "pooled features differ from TensorCoreEncoder.pooled_features"
+    t_err = (T - py.T).abs().max().item()
     assert t_err <= 1e-5, f"max |T - T_py| = {t_err:.3e}"
-    l_err = _rel(losses[:, :3], py_losses[:, :3])
+    l_err = H.rel(losses[:, :3], py.losses[:, :3])
     assert l_err <= 1e-5, f"losses differ by {l_err:.3e} (relative)"
-    tail, trunk = _grad_spread(_grad_dict(grads, cfg), py_grads)
+    tail, trunk = H.grad_spread(H.grad_dict(grads, cfg), py.grads)
     print(f"\n[{h}x{w} B={b} {act} single={single} nout={nout}] T {t_err:.2e}  losses {l_err:.2e}  grads: tail {tail:.2e}, "
           f"trunk {trunk:.2e}")
-    assert tail <= TAIL_TOL, f"fc / head gradients differ by {tail:.3e} of their max-abs"
-    assert trunk <= TRUNK_TOL, f"trunk gradients differ by {trunk:.3e} of their max-abs"
+    assert tail <= H.TAIL_TOL, f"fc / head gradients differ by {tail:.3e} of their max-abs"
+    assert trunk <= H.TRUNK_TOL, f"trunk gradients differ by {trunk:.3e} of their max-abs"
 
 
 def _adam_reference(blob, grads_seq, cfg, lr):
@@ -216,7 +68,7 @@ def _adam_reference(blob, grads_seq, cfg, lr):
     opt = torch.optim.Adam(m.parameters(), lr=lr, fused=True)
     params = dict(m.named_parameters())
     for g in grads_seq:
-        gd = _grad_dict(g, cfg)
+        gd = H.grad_dict(g, cfg)
         for k, p in params.items():
             p.grad = gd[k].to(DEV)
         opt.step()
@@ -226,48 +78,41 @@ def _adam_reference(blob, grads_seq, cfg, lr):
 @pytest.mark.parametrize("act,single", [("tanh", False), ("relu", True)])
 def test_adam_matches_torch(cuda_lib, act, single):
     lr = 1e-3
-    cfg = _config(16, 720, act, single)
-    model = _model(cfg, 1)
-    pairs = _pairs(16, 1024, 2)
-    n_stride = _n_stride(pairs)
-    pts, counts = _stack(pairs, n_stride)
-    blob0 = _blob(model, cfg)
-    tr = _Trainer(cfg, n_stride, 2, blob0, lr=lr)
+    cfg = H.config(16, 720, act, single)
+    model = H.model(cfg, 1, near_identity=True)
+    pairs = H.pairs(16, 1024, 2)
+    n_stride = H.n_stride(pairs)
+    pts, counts = H.stack_pairs(pairs, n_stride)
+    blob0 = H.blob(model, cfg)
+    tr = H.trainer(cfg, n_stride, 2, blob0, lr=lr)
     seq = []
     for k in range(3):
         seq.append(tr.step(pts, counts)[3])
         if k in (0, 2):
             want = _adam_reference(blob0, seq, cfg, lr)
-            got = _grad_dict(tr.weights(), cfg)
-            worst = max(_rel(got[n].to(DEV), want[n]) for n in want)
+            got = H.grad_dict(tr.weights(), cfg)
+            worst = max(H.rel(got[n].to(DEV), want[n]) for n in want)
             print(f"\n[Adam, {k + 1} step(s)] worst relative difference {worst:.2e}")
             assert worst <= 1e-6, f"after {k + 1} step(s) the master weights differ from torch's Adam by {worst:.3e}"
 
 
 def test_round_trip_to_inference_and_torch(cuda_lib):
-    from delora_b200 import _lib
     from delora_b200.deploy import export
     from delora_b200.models import model_parts
     from delora_b200.models.model import OdometryModel
-    cfg = _config(64, 720, "tanh", False)
-    model = _model(cfg, 2)
-    pairs = _pairs(64, 1024, 2)
-    n_stride = _n_stride(pairs)
-    pts, counts = _stack(pairs, n_stride)
-    tr = _Trainer(cfg, n_stride, 2, _blob(model, cfg), lr=1e-4)
+    cfg = H.config(64, 720, "tanh", False)
+    model = H.model(cfg, 2, near_identity=True)
+    pairs = H.pairs(64, 1024, 2)
+    n_stride = H.n_stride(pairs)
+    pts, counts = H.stack_pairs(pairs, n_stride)
+    tr = H.trainer(cfg, n_stride, 2, H.blob(model, cfg), lr=1e-4)
     for _ in range(2):
         tr.step(pts, counts, outputs=False)
     tuned = tr.weights()
-    L = tr.L
-    ws = torch.empty((int(L.delora_odometry_workspace_bytes(tr.dp)),), dtype=torch.uint8, device=DEV)
-    _lib.check(L.delora_odometry_init(tr.dp, ws.data_ptr(), _stream()), "init")
-    _lib.check(L.delora_odometry_load_weights(tr.dp, tuned.data_ptr(), ws.data_ptr(), _stream()), "load")
-    T = torch.empty((2, 4, 4), device=DEV)
-    _lib.check(L.delora_odometry_pairs(tr.dp, pts.data_ptr(), counts.data_ptr(), 2, ws.data_ptr(), T.data_ptr(), None,
-                                       _stream()), "pairs")
+    T, _ = InferenceWorkspace(tr.desc, tuned).pairs(pts, counts)
     m2 = OdometryModel(cfg).to(DEV).eval()
     m2.load_state_dict(export.unpack_blob(tuned.cpu().numpy(), cfg))
-    assert not torch.equal(tuned, _blob(model, cfg)), "the steps did not change the weights"
+    assert not torch.equal(tuned, H.blob(model, cfg)), "the steps did not change the weights"
     from delora_b200 import ops
     img, _ = ops.project(pts, counts, 64, 720, cfg["horizontal_field_of_view"], cfg["kitti"]["vertical_field_of_view"])
     with torch.no_grad():
@@ -278,20 +123,20 @@ def test_round_trip_to_inference_and_torch(cuda_lib):
 
 
 def test_deterministic_and_graph_replay(cuda_lib):
-    cfg = _config(64, 720, "relu", False)
-    model = _model(cfg, 3)
-    pairs = _pairs(64, 1024, 2)
-    n_stride = _n_stride(pairs)
-    pts, counts = _stack(pairs, n_stride)
-    blob = _blob(model, cfg)
-    a, b = _Trainer(cfg, n_stride, 2, blob, 1e-4), _Trainer(cfg, n_stride, 2, blob, 1e-4)
+    cfg = H.config(64, 720, "relu", False)
+    model = H.model(cfg, 3, near_identity=True)
+    pairs = H.pairs(64, 1024, 2)
+    n_stride = H.n_stride(pairs)
+    pts, counts = H.stack_pairs(pairs, n_stride)
+    blob = H.blob(model, cfg)
+    a, b = H.trainer(cfg, n_stride, 2, blob, 1e-4), H.trainer(cfg, n_stride, 2, blob, 1e-4)
     for _ in range(5):
         a.step(pts, counts, outputs=False)
         b.step(pts, counts, outputs=False)
     torch.cuda.synchronize()
     assert torch.equal(a.weights(), b.weights()), "two workspaces with the same steps differ"
 
-    eager, graphed = _Trainer(cfg, n_stride, 2, blob, 1e-4), _Trainer(cfg, n_stride, 2, blob, 1e-4)
+    eager, graphed = H.trainer(cfg, n_stride, 2, blob, 1e-4), H.trainer(cfg, n_stride, 2, blob, 1e-4)
     for _ in range(3):
         eager.step(pts, counts, outputs=False)
     graphed.step(pts, counts, outputs=False)        # eager first: sets up the launchers' host-side state
@@ -306,16 +151,16 @@ def test_deterministic_and_graph_replay(cuda_lib):
 
 
 def test_batch_size_may_change_between_steps(cuda_lib):
-    cfg = _config(64, 720, "tanh", True)
-    model = _model(cfg, 4)
-    pairs = _pairs(64, 1024, 4)
-    n_stride = _n_stride(pairs)
-    tr = _Trainer(cfg, n_stride, 4, _blob(model, cfg), 1e-4)
+    cfg = H.config(64, 720, "tanh", True)
+    model = H.model(cfg, 4, near_identity=True)
+    pairs = H.pairs(64, 1024, 4)
+    n_stride = H.n_stride(pairs)
+    tr = H.trainer(cfg, n_stride, 4, H.blob(model, cfg), 1e-4)
     for bsz in (4, 2, 4):
-        pts, counts = _stack(pairs[:bsz], n_stride)
+        pts, counts = H.stack_pairs(pairs[:bsz], n_stride)
         before = tr.weights()
         got = tr.step(pts, counts)
-        fresh = _Trainer(cfg, n_stride, 4, before, 1e-4).step(pts, counts)
+        fresh = H.trainer(cfg, n_stride, 4, before, 1e-4).step(pts, counts)
         torch.cuda.synchronize()
         for x, y, name in zip(got, fresh, ("losses", "T", "pooled", "grads")):
             assert torch.equal(x, y), f"B={bsz}: {name} differ from a fresh workspace"
@@ -323,15 +168,12 @@ def test_batch_size_may_change_between_steps(cuda_lib):
 
 def test_finetune_example_program(cuda_lib, tmp_path):
     """examples/odometry_finetune.c on a .dlw and four KITTI .bin scans: its weights are the C step's on those pairs."""
-    import os
-    import subprocess
-    from delora_b200 import build, synthetic
+    from delora_b200 import synthetic
     from delora_b200.deploy import export
-    from helpers import ROOT
     vfov = (-15.0, 15.0)
-    cfg = _config(16, 720, "tanh", False)
+    cfg = H.config(16, 720, "tanh", False)
     cfg["kitti"]["vertical_field_of_view"] = [v * np.pi / 180.0 for v in vfov]
-    model = _model(cfg, 5)
+    model = H.model(cfg, 5, near_identity=True)
     dlw, out = os.path.join(tmp_path, "in.dlw"), os.path.join(tmp_path, "out.dlw")
     desc = export.desc_from_config(cfg, "kitti", 4096, 2)
     export.write_dlw(dlw, desc, export.pack_state_dict(model.state_dict(), cfg))
@@ -340,14 +182,7 @@ def test_finetune_example_program(cuda_lib, tmp_path):
         path = os.path.join(tmp_path, f"{i:06d}.bin")
         synthetic.kitti_bin_scan(i, vfov_deg=vfov).tofile(path)
         bins.append(path)
-    nvcc = build._nvcc()
-    cuda_home = os.path.dirname(os.path.dirname(os.path.realpath(nvcc)))
-    libdir = os.path.dirname(build.LIB)
-    exe = os.path.join(tmp_path, "odometry_finetune")
-    r = subprocess.run([nvcc, os.path.join(ROOT, "examples", "odometry_finetune.c"), "-I", os.path.join(ROOT, "include"),
-                        "-I", os.path.join(cuda_home, "include"), "-L", libdir, "-ldelora_b200", "-lcudart",
-                        "-Xlinker", "-rpath=" + libdir, "-o", exe], capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
+    exe = H.build_example("odometry_finetune", tmp_path, link=True)
     r = subprocess.run([exe, dlw, out, "3", "1e-4"] + bins, capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, r.stderr
     assert len(r.stdout.strip().splitlines()) == 3
@@ -355,29 +190,27 @@ def test_finetune_example_program(cuda_lib, tmp_path):
     assert (d.H, d.W, d.max_batch) == (16, 720, 2)
     # the program's three steps (two pairs each, cycling): (0,1) (1,2); (2,3) (0,1); (1,2) (2,3)
     scans = [torch.from_numpy(np.fromfile(p, dtype=np.float32).reshape(-1, 4)[:, :3].T.copy()) for p in bins]
-    tr = _Trainer(cfg, 4096, 2, _blob(model, cfg), lr=1e-4)
+    tr = H.trainer(cfg, 4096, 2, H.blob(model, cfg), lr=1e-4)
     for ks in ((0, 1), (2, 0)):
-        pts, counts = _stack([(scans[k], scans[k + 1]) for k in ks], 4096)
+        pts, counts = H.stack_pairs([(scans[k], scans[k + 1]) for k in ks], 4096)
         tr.step(pts, counts, outputs=False)
-    pts, counts = _stack([(scans[1], scans[2]), (scans[2], scans[3])], 4096)
+    pts, counts = H.stack_pairs([(scans[1], scans[2]), (scans[2], scans[3])], 4096)
     tr.step(pts, counts, outputs=False)
     torch.cuda.synchronize()
     assert np.array_equal(tr.weights().cpu().numpy(), blob)
 
 
 def test_training_lowers_the_objective_next_to_synthetic_train_step(cuda_lib):
-    from delora_b200.deploy import export
     from delora_b200.train_step import SyntheticTrainStep
     lr, steps, b = 1e-4, 20, 4
-    pairs = _pairs(64, 2048, b)
-    n_stride = _n_stride(pairs)
-    pts, counts = _stack(pairs, n_stride)
+    pairs = H.pairs(64, 2048, b)
+    n_stride = H.n_stride(pairs)
+    pts, counts = H.stack_pairs(pairs, n_stride)
     torch.manual_seed(0)
-    ref = SyntheticTrainStep(_config(64, 2048), b, n_stride, lr=lr)
+    ref = SyntheticTrainStep(H.config(64, 2048), b, n_stride, lr=lr)
     ref.load(pts, counts)
     cfg = ref.cfg
-    blob = torch.from_numpy(export.pack_state_dict(ref.model.state_dict(), cfg)).to(DEV)
-    tr = _Trainer(cfg, n_stride, b, blob, lr)
+    tr = H.trainer(cfg, n_stride, b, H.blob(ref.model, cfg), lr)
     lam = float(cfg["lambda_po2pl"])
     c_curve, py_curve = [], []
     for _ in range(steps):

@@ -45,5 +45,6 @@ def test_ops_constants_match_the_header():
     from delora_b200 import ops
     text = open(os.path.join(ROOT, "include", "delora_b200.h")).read()
     defines = {k: int(v) for k, v in re.findall(r"#define DELORA_(\w+)\s+(\d+)u?\b", text)}
-    for name in ("LOSS_PO2PO", "LOSS_PO2PL", "LOSS_PL2PL", "NORMAL_LINEAR", "ICP_STATS", "LOSS_ROW", "ICP_PARTIAL"):
+    for name in ("LOSS_PO2PO", "LOSS_PO2PL", "LOSS_PL2PL", "NORMAL_LINEAR", "ICP_STATS", "LOSS_IDENTITY_FIT", "LOSS_ROW",
+                 "ICP_PARTIAL"):
         assert getattr(ops, name) == defines[name], name

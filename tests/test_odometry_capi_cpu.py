@@ -10,24 +10,11 @@ import numpy as np
 import pytest
 import torch
 
+import odometry_harness as H
 from helpers import ROOT
 
 ODOMETRY_SYMBOLS = ("delora_odometry_weight_floats", "delora_odometry_workspace_bytes", "delora_odometry_init",
                     "delora_odometry_load_weights", "delora_odometry_pairs", "delora_odometry_push")
-
-
-def _config(act="tanh", single=False, layers=(2, 2, 2, 2), nout=1000, h=64, w=720, **extra):
-    from delora_b200 import synthetic
-    cfg = synthetic.fov_config(h=h, w=w)
-    cfg.update({"activation_fct": act, "use_single_mlp_at_output": single, "layers": list(layers), "resnet_outputs": nout,
-                "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1, "use_dropout": False})
-    cfg.update(extra)
-    return cfg
-
-
-def _desc(cfg, n_stride=1000, max_batch=1):
-    from delora_b200.deploy import export
-    return export.desc_from_config(cfg, "kitti", n_stride, max_batch)
 
 
 def test_symbols_exported_and_abi_version():
@@ -45,11 +32,11 @@ def test_symbols_exported_and_abi_version():
 def test_weight_floats_match_the_state_dict(act, single, layers, nout):
     from delora_b200 import _lib
     from delora_b200.models.model import OdometryModel
-    cfg = _config(act, single, layers, nout)
+    cfg = H.config(64, 720, act, single, layers, nout, device="cpu")
     with torch.device("meta"):
         model = OdometryModel(dict(cfg, device="cpu"))
     want = sum(t.numel() for t in model.state_dict().values())
-    d = _desc(cfg)
+    d = H.desc(cfg, 1000, 1)
     assert _lib.lib().delora_odometry_weight_floats(ctypes.byref(d)) == want
     assert _lib.lib().delora_odometry_workspace_bytes(ctypes.byref(d)) > 0
 
@@ -57,9 +44,9 @@ def test_weight_floats_match_the_state_dict(act, single, layers, nout):
 def test_workspace_grows_with_max_batch():
     from delora_b200 import _lib
     L = _lib.lib()
-    cfg = _config(h=64, w=2048)
-    one = L.delora_odometry_workspace_bytes(ctypes.byref(_desc(cfg, 131072, 1)))
-    sixteen = L.delora_odometry_workspace_bytes(ctypes.byref(_desc(cfg, 131072, 16)))
+    cfg = H.config(64, 2048, device="cpu")
+    one = L.delora_odometry_workspace_bytes(ctypes.byref(H.desc(cfg, 131072, 1)))
+    sixteen = L.delora_odometry_workspace_bytes(ctypes.byref(H.desc(cfg, 131072, 16)))
     assert 0 < one < sixteen
     assert one % 256 == 0 and sixteen % 256 == 0
 
@@ -72,7 +59,7 @@ def test_workspace_grows_with_max_batch():
 def test_invalid_descriptors_are_reported_without_a_gpu(field, value, message):
     from delora_b200 import _lib
     L = _lib.lib()
-    d = _desc(_config())
+    d = H.desc(H.config(64, 720, device="cpu"), 1000, 1)
     if field == "layers":
         d.layers[2] = value
     else:
@@ -90,7 +77,7 @@ def test_null_arguments_are_reported_without_a_gpu():
     L = _lib.lib()
     assert L.delora_odometry_weight_floats(None) == -1
     assert b"null descriptor" in L.delora_last_error()
-    d = _desc(_config())
+    d = H.desc(H.config(64, 720, device="cpu"), 1000, 1)
     assert L.delora_odometry_pairs(ctypes.byref(d), None, None, 1, None, None, None, None) != 0
     assert b"null pointer" in L.delora_last_error()
     assert L.delora_odometry_push(ctypes.byref(d), None, None, None, None, None) != 0
@@ -112,7 +99,7 @@ def _checkpoint(tmp_path, cfg, seed=0):
 def test_exporter_round_trip(tmp_path, act, single):
     from delora_b200 import _lib
     from delora_b200.deploy import export
-    cfg = _config(act, single, (1, 2, 1, 2), 500, h=16, w=720)
+    cfg = H.config(16, 720, act, single, (1, 2, 1, 2), 500, device="cpu")
     path, model = _checkpoint(tmp_path, cfg)
     out = os.path.join(tmp_path, "model.dlw")
     export.export(path, "kitti", out, n_stride=4096, max_batch=3)
@@ -131,7 +118,7 @@ def test_exporter_round_trip(tmp_path, act, single):
 
 def test_exporter_cli(tmp_path):
     from delora_b200.deploy import export
-    cfg = _config("tanh", False, (1, 1, 1, 1), 100, h=16, w=256)
+    cfg = H.config(16, 256, "tanh", False, (1, 1, 1, 1), 100, device="cpu")
     path, model = _checkpoint(tmp_path, cfg, seed=3)
     out = os.path.join(tmp_path, "cli.dlw")
     r = subprocess.run([sys.executable, os.path.join(ROOT, "bin", "export_odometry_weights.py"), "--checkpoint", path,
@@ -146,7 +133,7 @@ def test_exporter_cli(tmp_path):
 @pytest.mark.parametrize("key,value", [("pre_feature_extraction", True), ("factor_fewer_resnet_channels", 2)])
 def test_exporter_refuses_unsupported_models(tmp_path, key, value):
     from delora_b200.deploy import export
-    cfg = _config("tanh", False, (1, 1, 1, 1), 100, h=16, w=256, **{key: value})
+    cfg = dict(H.config(16, 256, "tanh", False, (1, 1, 1, 1), 100, device="cpu"), **{key: value})
     path, _ = _checkpoint(tmp_path, cfg)
     with pytest.raises(ValueError, match=key):
         export.export(path, "kitti", os.path.join(tmp_path, "x.dlw"), n_stride=100)
@@ -154,10 +141,4 @@ def test_exporter_refuses_unsupported_models(tmp_path, key, value):
 
 
 def test_example_compiles_against_the_header(tmp_path):
-    from delora_b200 import build
-    nvcc = build._nvcc()
-    cuda_inc = os.path.join(os.path.dirname(os.path.dirname(os.path.realpath(nvcc))), "include")
-    r = subprocess.run([nvcc, "-c", os.path.join(ROOT, "examples", "odometry_stream.c"), "-I", os.path.join(ROOT, "include"),
-                        "-I", cuda_inc, "-Xcompiler", "-Wall,-Werror", "-o", os.path.join(tmp_path, "odometry_stream.o")],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
+    H.build_example("odometry_stream", tmp_path, link=False)

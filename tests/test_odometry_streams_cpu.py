@@ -1,30 +1,14 @@
 """-m "not gpu": the streams entry points of the C ABI (delora_odometry_streams_*) without a device -- exported symbols,
 descriptor validation, workspace sizes, every refusal, and that examples/odometry_streams.c compiles."""
 import ctypes
-import os
-import subprocess
 
 import pytest
 
-from helpers import ROOT
+import odometry_harness as H
 
 STREAMS_SYMBOLS = ("delora_odometry_streams_workspace_bytes", "delora_odometry_streams_init",
                    "delora_odometry_streams_load_weights", "delora_odometry_streams_push",
                    "delora_odometry_streams_reset")
-
-
-def _config(h=64, w=720):
-    from delora_b200 import synthetic
-    cfg = synthetic.fov_config(h=h, w=w)
-    cfg.update({"activation_fct": "tanh", "use_single_mlp_at_output": False, "layers": [2, 2, 2, 2],
-                "resnet_outputs": 1000, "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1,
-                "use_dropout": False})
-    return cfg
-
-
-def _desc(cfg, n_stride=1000, streams=1):
-    from delora_b200.deploy import export
-    return export.desc_from_config(cfg, "kitti", n_stride, streams)
 
 
 def test_symbols_exported():
@@ -40,12 +24,12 @@ def test_symbols_exported():
 def test_workspace_grows_with_the_stream_count(h, w):
     from delora_b200 import _lib
     L = _lib.lib()
-    cfg = _config(h, w)
-    sizes = [L.delora_odometry_streams_workspace_bytes(ctypes.byref(_desc(cfg, 131072, s))) for s in (1, 4, 16)]
+    cfg = H.config(h, w, device="cpu")
+    sizes = [L.delora_odometry_streams_workspace_bytes(ctypes.byref(H.desc(cfg, 131072, s))) for s in (1, 4, 16)]
     assert 0 < sizes[0] < sizes[1] < sizes[2]
     assert all(s % 256 == 0 for s in sizes)
     # one stream keeps one cached frame where _push keeps one, but projects one scan where _pairs sizes two
-    push = L.delora_odometry_workspace_bytes(ctypes.byref(_desc(cfg, 131072, 1)))
+    push = L.delora_odometry_workspace_bytes(ctypes.byref(H.desc(cfg, 131072, 1)))
     assert sizes[0] < push
 
 
@@ -56,7 +40,7 @@ def test_workspace_grows_with_the_stream_count(h, w):
 def test_invalid_descriptors_are_refused(field, value, message):
     from delora_b200 import _lib
     L = _lib.lib()
-    d = _desc(_config())
+    d = H.desc(H.config(64, 720, device="cpu"), 1000, 1)
     if field == "layers":
         d.layers[2] = value
     else:
@@ -82,7 +66,7 @@ def test_push_refuses_null_pointers_by_name(missing):
     """Non-null dummies elsewhere: the call is refused before it could launch anything."""
     from delora_b200 import _lib
     L = _lib.lib()
-    d = _desc(_config(), 1000, 3)
+    d = H.desc(H.config(64, 720, device="cpu"), 1000, 3)
     args = {"points": 16, "n_points": 32, "workspace": 48, "T": 64, "valid": 80}
     args[missing] = None
     rc = L.delora_odometry_streams_push(ctypes.byref(d), args["points"], args["n_points"], None, args["workspace"],
@@ -94,7 +78,7 @@ def test_push_refuses_null_pointers_by_name(missing):
 def test_other_entry_points_refuse_null_pointers():
     from delora_b200 import _lib
     L = _lib.lib()
-    dp = ctypes.byref(_desc(_config(), 1000, 2))
+    dp = ctypes.byref(H.desc(H.config(64, 720, device="cpu"), 1000, 2))
     assert L.delora_odometry_streams_init(dp, None, None) != 0
     assert b"delora_odometry_streams_init: null workspace" in L.delora_last_error()
     assert L.delora_odometry_streams_load_weights(dp, None, 16, None) != 0
@@ -108,10 +92,4 @@ def test_other_entry_points_refuse_null_pointers():
 
 
 def test_example_compiles_against_the_header(tmp_path):
-    from delora_b200 import build
-    nvcc = build._nvcc()
-    cuda_inc = os.path.join(os.path.dirname(os.path.dirname(os.path.realpath(nvcc))), "include")
-    r = subprocess.run([nvcc, "-c", os.path.join(ROOT, "examples", "odometry_streams.c"), "-I",
-                        os.path.join(ROOT, "include"), "-I", cuda_inc, "-Xcompiler", "-Wall,-Werror", "-o",
-                        os.path.join(tmp_path, "odometry_streams.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
+    H.build_example("odometry_streams", tmp_path, link=False)

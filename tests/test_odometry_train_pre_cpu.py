@@ -6,13 +6,11 @@ import struct
 
 import pytest
 
+import odometry_harness as H
+
 
 def _cfg(h=64, w=720, w_pre=2250):
-    from delora_b200 import synthetic
-    cfg = synthetic.fov_config(h=h, w=w)
-    cfg.update({"activation_fct": "tanh", "use_single_mlp_at_output": False, "layers": [2, 2, 2, 2],
-                "resnet_outputs": 1000, "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1,
-                "use_dropout": False})
+    cfg = H.config(h, w, device="cpu")
     cfg["kitti"]["horizontal_cells_preprocessing"] = w_pre
     return cfg
 
@@ -73,10 +71,8 @@ def test_default_export_is_unchanged_and_reads_back_as_zero(tmp_path):
 @pytest.mark.parametrize("w_pre", [1, -1, -2250, (1 << 27) // 64])
 def test_bad_w_pre_is_refused_by_name(w_pre):
     from delora_b200 import _lib
-    from delora_b200.deploy import export
     L = _lib.lib()
-    d = export.desc_from_config(_cfg(), "kitti", 131072, 1)
-    d.w_pre = w_pre
+    d = H.desc(_cfg(), 131072, 1, w_pre)
     assert L.delora_odometry_train_workspace_bytes(ctypes.byref(d)) == -1
     assert b"w_pre" in L.delora_last_error()
 
@@ -84,9 +80,8 @@ def test_bad_w_pre_is_refused_by_name(w_pre):
 @pytest.mark.parametrize("w_pre", [1, -7, 2250, 1 << 30])
 def test_inference_and_streams_ignore_w_pre(w_pre):
     from delora_b200 import _lib
-    from delora_b200.deploy import export
     L = _lib.lib()
-    d = export.desc_from_config(_cfg(), "kitti", 131072, 4)
+    d = H.desc(_cfg(), 131072, 4)
     want = (L.delora_odometry_workspace_bytes(ctypes.byref(d)), L.delora_odometry_streams_workspace_bytes(ctypes.byref(d)),
             L.delora_odometry_weight_floats(ctypes.byref(d)))
     d.w_pre = w_pre
@@ -103,9 +98,8 @@ DOCUMENTED = {1: (340982528, 357525248), 4: (546658048, 612828928), 16: (1369363
                                                  (16, 259, 512, 2), (64, 2048, 2048, 1), (64, 2048, 1024, 4)])
 def test_training_workspace_grows_by_the_documented_section(h, w, w_pre, max_batch):
     from delora_b200 import _lib
-    from delora_b200.deploy import export
     L = _lib.lib()
-    d = export.desc_from_config(_cfg(h, w, w_pre), "kitti", 131072, max_batch)
+    d = H.desc(_cfg(h, w, w_pre), 131072, max_batch)
     base = L.delora_odometry_train_workspace_bytes(ctypes.byref(d))
     d.w_pre = w_pre
     grown = L.delora_odometry_train_workspace_bytes(ctypes.byref(d))

@@ -13,20 +13,11 @@ import numpy as np
 import pytest
 import torch
 
+import odometry_harness as H
 from helpers import ROOT
 
 
-def _config(act="tanh", single=False):
-    from delora_b200 import synthetic
-    cfg = synthetic.fov_config(h=16, w=720)
-    cfg.update({"activation_fct": act, "use_single_mlp_at_output": single, "layers": [1, 1, 1, 1], "resnet_outputs": 64,
-                "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1, "use_dropout": False})
-    return cfg
-
-
-def _desc(cfg, n_stride=1000, max_batch=2):
-    from delora_b200.deploy import export
-    return export.desc_from_config(cfg, "kitti", n_stride, max_batch)
+SMALL = {"h": 16, "w": 720, "layers": (1, 1, 1, 1), "nout": 64, "device": "cpu"}
 
 
 def _trained(cfg, steps=3, lr=2.0 ** -10, betas=(0.875, 0.9921875), eps=2.0 ** -24, **adam):
@@ -46,8 +37,8 @@ def _trained(cfg, steps=3, lr=2.0 ** -10, betas=(0.875, 0.9921875), eps=2.0 ** -
 def test_dlt_header_offsets(tmp_path):
     from delora_b200 import _lib
     from delora_b200.deploy import export
-    cfg = _config()
-    d = _desc(cfg)
+    cfg = H.config(**SMALL)
+    d = H.desc(cfg, 1000, 2)
     n = 12
     st = export.TrainingState(np.arange(n, dtype=np.float32), np.full(n, 2.0, np.float32), np.full(n, 3.0, np.float32),
                               step=123456789012, epoch=7, unsupervised=1, lr=0.25, beta1=0.5, beta2=0.75, eps=0.125,
@@ -85,12 +76,12 @@ def test_dlt_header_offsets(tmp_path):
 def test_torch_adam_state_survives_the_dlt(tmp_path, act, single):
     from delora_b200.deploy import export
     from delora_b200.models.model import OdometryModel
-    cfg = _config(act, single)
+    cfg = H.config(act=act, single=single, **SMALL)
     model, opt = _trained(cfg)
     ckpt = {"epoch": 4, "model_state_dict": model.state_dict(), "optimizer_state_dict": opt.state_dict(), "loss": 0.5,
             "parameters": cfg}
     path = os.path.join(tmp_path, "s.dlt")
-    export.write_dlt(path, _desc(cfg), export.training_state_from_checkpoint(ckpt, cfg))
+    export.write_dlt(path, H.desc(cfg, 1000, 2), export.training_state_from_checkpoint(ckpt, cfg))
     _, _, state = export.read_dlt(path)
     assert (state.step, state.epoch, state.unsupervised) == (3, 5, 1)
     back = export.checkpoint_from_training_state(state, cfg)
@@ -128,7 +119,7 @@ def _refusal(cfg, ckpt, match):
 
 
 def test_refusals_name_the_key():
-    cfg = _config()
+    cfg = H.config(**SMALL)
     for adam, key in (({"weight_decay": 1e-4}, "weight_decay"), ({"amsgrad": True}, "amsgrad"),
                       ({"maximize": True}, "maximize")):
         model, opt = _trained(cfg, steps=1, **adam)
@@ -153,7 +144,7 @@ def test_refusals_name_the_key():
 
 def test_checkpoint_without_optimizer_state_gives_zero_moments():
     from delora_b200.deploy import export
-    cfg = dict(_config(), learning_rate=3e-4)
+    cfg = dict(H.config(**SMALL), learning_rate=3e-4)
     model, _ = _trained(cfg, steps=0)
     for ckpt in ({"model_state_dict": model.state_dict()},
                  {"model_state_dict": model.state_dict(), "optimizer_state_dict": torch.optim.Adam(
@@ -216,7 +207,7 @@ def test_init_seed_is_deterministic(tmp_path):
 def test_state_entry_points_refuse_without_a_gpu():
     from delora_b200 import _lib
     L = _lib.lib()
-    d = _desc(_config())
+    d = H.desc(H.config(**SMALL), 1000, 2)
     dp = ctypes.byref(d)
     dummy = ctypes.c_void_p(16)             # never dereferenced: the call is refused before any launch
     assert L.delora_odometry_train_get_state(dp, None, dummy, dummy, dummy, dummy, None) != 0
@@ -226,7 +217,7 @@ def test_state_entry_points_refuse_without_a_gpu():
         args[i] = None
         assert L.delora_odometry_train_set_state(dp, *args, None) != 0
         assert b"null " + name in L.delora_last_error(), name
-    bad = _desc(_config())
+    bad = H.desc(H.config(**SMALL), 1000, 2)
     bad.act = 0
     assert L.delora_odometry_train_set_state(ctypes.byref(bad), dummy, dummy, dummy, dummy, dummy, None) != 0
     assert b"act=0" in L.delora_last_error()
@@ -235,12 +226,11 @@ def test_state_entry_points_refuse_without_a_gpu():
 
 
 def test_identity_bit_alone_is_refused():
-    from delora_b200 import _lib
+    from delora_b200 import _lib, ops
+    from delora_b200.deploy import capi
     L = _lib.lib()
-    d = _desc(_config())
-    hp = _lib.OdometryTrainParams(lr=1e-5, beta1=0.9, beta2=0.999, eps=1e-8, lambda_po2pl=1.0,
-                                  loss_flags=_lib.LOSS_IDENTITY_FIT, nb_h=7, nb_w=11, epsilon_range=0.5,
-                                  min_neighbors=10)
+    d = H.desc(H.config(**SMALL), 1000, 2)
+    hp = capi.train_params(H.config(**SMALL), 1e-5, loss_flags=ops.LOSS_IDENTITY_FIT)
     dummy = ctypes.c_void_p(16)
     rc = L.delora_odometry_train_step(ctypes.byref(d), ctypes.byref(hp), dummy, dummy, 1, dummy, None, None, None, None,
                                       None)
@@ -249,10 +239,4 @@ def test_identity_bit_alone_is_refused():
 
 
 def test_train_example_compiles_against_the_header(tmp_path):
-    from delora_b200 import build
-    nvcc = build._nvcc()
-    cuda_inc = os.path.join(os.path.dirname(os.path.dirname(os.path.realpath(nvcc))), "include")
-    r = subprocess.run([nvcc, "-c", os.path.join(ROOT, "examples", "odometry_train.c"), "-I",
-                        os.path.join(ROOT, "include"), "-I", cuda_inc, "-Xcompiler", "-Wall,-Werror", "-o",
-                        os.path.join(tmp_path, "odometry_train.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
+    H.build_example("odometry_train", tmp_path, link=False)
