@@ -11,30 +11,30 @@ channels): one bf16 output rounding plus a worst-case bound on the fp32 accumula
 or misplaced tap exceeds it by more than an order of magnitude.  Every case prints its worst err / bound (`pytest -s`);
 round-to-nearest bf16 alone may use 2^-8 / (1 + 2^-8) = 0.996 of the first term, so worst ratios of 0.9 .. 0.99 are
 the output rounding, and the fp32 accumulation lives in the second term's slack.
+
+The weight gradients (delora_conv2d_wgrad_bf16: conv_wgrad.cu's wgrad2 modes 0 / 1 and conv_tc.cu's first-generation
+kernel; delora_stem_wgrad_bf16: wgrad2 mode 2) are called through the C ABI, every kernel path and both reduce kernels:
+- Integer operands in [-r, r] with n r^2 < 2^23 (n = products per dW element, asserted): every product is exact in
+  bf16 x bf16 and every partial sum is an integer below 2^23, so any order of fp32 adds -- the wgmma accumulator even
+  with a truncating adder, the split-K slices and the reduce -- gives the true sum.  The fp32 dW has no output
+  rounding, so it must equal float64 autograd bit for bit: one missing, doubled or misplaced product fails at any K.
+- Gaussian bf16 operands: |got - ref| <= (n + 3) 2^-23 ref_abs (2^-23, not 2^-24: the tensor-core adder need not
+  round to nearest), and two calls bit-identical (the split-K reduction has a fixed order and no atomics).
+- The scratch is exactly the size query's floats, NaN-filled, with a NaN guard behind it; dW is a slice of a NaN
+  buffer; the output gradient's halo holds junk.  A finite dW shows every split-K slot the reduce read was written in
+  that call, the untouched guards that the query covers the launch and that nothing lands outside dW, and the exact
+  result that the halo is not read.  Input channels >= Cin_true hold nonzero values the reduce must drop.
 """
+import math
+
 import pytest
 import torch
 import torch.nn.functional as F
 
+from helpers import (DEV, FPROP_BWD_SHAPES, check_bound, check_exact, check_layout, conv3, conv_ref, generator,
+                     interior, rand_bf16, rand_int, run_twice, sentinel_out, to_padded_nhwc)
+
 pytestmark = pytest.mark.gpu
-DEV = "cuda"
-HALO_ROW = 7.0          # the halo rows of an output are never written: they must still hold this after the call
-
-
-def to_padded_nhwc(x):
-    """[B,C,H,W] -> [B,H+2,W+2,C] bf16 with the circular W halo and the zero H halo of the encoder's layout."""
-    xp = F.pad(F.pad(x, (1, 1, 0, 0), mode="circular"), (0, 0, 1, 1))
-    return xp.permute(0, 2, 3, 1).contiguous().to(torch.bfloat16)
-
-
-def interior(y, h, w):
-    """padded NHWC -> [B,C,H,W] float64"""
-    return y[:, 1:h + 1, 1:w + 1].permute(0, 3, 1, 2).double()
-
-
-def rand_bf16(g, shape, scale=1.0):
-    """float64 tensor holding bf16 values: the exact operand the kernel reads."""
-    return (torch.randn(shape, generator=g, device=DEV, dtype=torch.float64) * scale).to(torch.bfloat16).double()
 
 
 def saved_values(g, shape, act):
@@ -53,11 +53,6 @@ def act_prime(s, act):
     return 1.0 - s * s if act == 3 else (s > 0).double()
 
 
-def conv3(x, w, stride):
-    """The encoder's 3x3 convolution: circular padding in W, zero padding in H (src/models/resnet_modified.py)."""
-    return F.conv2d(F.pad(x, (1, 1, 0, 0), mode="circular"), w, stride=stride, padding=(1, 0))
-
-
 def dgrad_ref(dz, w, hin, win, stride):
     """x.grad of conv3 at an Hin x Win input after backward(dz), float64 autograd."""
     x = torch.zeros((dz.shape[0], w.shape[1], hin, win), dtype=torch.float64, device=DEV, requires_grad=True)
@@ -71,49 +66,6 @@ def epilogue_ref(conv, res, res_stride, d):
     if res is not None:
         out[..., ::res_stride[0], ::res_stride[1]] += res
     return out if d is None else out * d
-
-
-def check_bound(got, ref, ref_abs, n, label):
-    assert bool(torch.isfinite(got).all()), f"{label}: non-finite output"
-    bound = 2.0 ** -8 * ref.abs() + (n + 3) * 2.0 ** -24 * ref_abs
-    err = (got - ref).abs()
-    ratio = torch.where(err == 0, torch.zeros_like(err), err / bound)
-    worst = ratio.max().item()
-    print(f"{label}: worst err/bound {worst:.4f}", flush=True)
-    if worst > 1.0:
-        b, c, h, w = (int(i) for i in torch.unravel_index(ratio.argmax(), ratio.shape))
-        bad = ratio > 1.0
-        raise AssertionError(
-            f"{label}: err/bound {worst:.3g} at (b, c, h, w) = ({b}, {c}, {h}, {w}): got {got[b, c, h, w].item():.6g}, "
-            f"ref {ref[b, c, h, w].item():.6g}; {int(bad.sum())} elements over the bar, rows "
-            f"{sorted(set(bad.nonzero()[:, 2].tolist()))[:16]}, columns {sorted(set(bad.nonzero()[:, 3].tolist()))[:16]}")
-
-
-def sentinel_out(b, h, w, c):
-    """Padded NHWC output: bf16 NaN in rows 1..H (interior and halo columns), HALO_ROW in rows 0 and H+1."""
-    out = torch.full((b, h + 2, w + 2, c), float("nan"), dtype=torch.bfloat16, device=DEV)
-    out[:, 0] = HALO_ROW
-    out[:, h + 1] = HALO_ROW
-    return out
-
-
-def check_layout(out, h, w, label):
-    """Every pixel of rows 1..H written, columns 0 / W+1 the circular copies of columns W / 1, halo rows untouched."""
-    rows = out[:, 1:h + 1]
-    nan = torch.isnan(rows)
-    assert not bool(nan.any()), f"{label}: {int(nan.sum())} elements not written, first (b, h-1, w, c) = " \
-                                f"{tuple(nan.nonzero()[0].tolist())}"
-    bits = rows.view(torch.int16)
-    assert torch.equal(bits[:, :, 0], bits[:, :, w]), f"{label}: halo column 0 differs from column W"
-    assert torch.equal(bits[:, :, w + 1], bits[:, :, 1]), f"{label}: halo column W+1 differs from column 1"
-    assert bool((out[:, 0] == HALO_ROW).all()) and bool((out[:, h + 1] == HALO_ROW).all()), f"{label}: halo row written"
-
-
-def run_twice(fn, label):
-    """Two calls into fresh sentinel outputs: both pass the layout checks and agree bit for bit."""
-    a, b = fn(), fn()
-    assert torch.equal(a.view(torch.int16), b.view(torch.int16)), f"{label}: two calls differ"
-    return a
 
 
 # ------------------------------------------------------------------------------------------------ data gradient
@@ -214,12 +166,7 @@ def test_dgrad_fallback_matches_float64_autograd(case, cuda_lib):
 
 
 # ------------------------------------------------------------------------------------------------ stride-1 fprop
-FPROP_BWD_SHAPES = [   # B, Cin, Cout, H, W at stride 1 (the backward's dz1 = conv(dz2) * act'(t1) and its residual form)
-    (2, 512, 512, 4, 64),      # conv_rows, 128 output channels on M
-    (2, 64, 64, 5, 180),       # conv_rows pixel-on-M, ragged second segment
-    (2, 128, 128, 4, 256),     # conv_rows pixel-on-M
-    (2, 64, 64, 5, 45),        # conv_tc (64 output channels on a row narrower than a segment)
-]
+# FPROP_BWD_SHAPES (helpers.py) are shared with the forward epilogue tests of test_gpu_encoder_forward.py
 FPROP_BWD_CASES = [(s, a, r) for s in FPROP_BWD_SHAPES for a in (3, 4) for r in (False, True)]
 ONE_BY_ONE_SHAPES = [          # B, Cin, Cout, H, W: the 1x1 stride-1 convolution forming the downsample's gradient
     (2, 512, 256, 4, 64),      # conv_rows, 128 output channels on M
@@ -264,6 +211,198 @@ def test_fprop_act_prime_epilogue(shape, act, use_res, cuda_lib):
 def test_fprop_1x1_stride1(shape, cuda_lib):
     b, cin, cout, h, w = shape
     _fprop_check(b, cin, cout, h, w, 1, 0, False, f"fprop 1x1 {cin}x{cout} {h}x{w}")
+
+
+# ------------------------------------------------------------------------------------------------ weight gradient
+# Forward layer (B, Cin, Cout, Hin, Win, k, stride), input channels kept (Cin_true; None = Cin), and the kernel path
+# delora_conv2d_wgrad_bf16 takes for it (conv_wgrad.cu: wgrad2 mode 0 for Cout % 128 == 0, mode 1 for Cout = 64 at
+# stride 1; conv_tc.cu: conv_wgrad_tc_kernel for 1x1 and for strided layers with Cout = 64)
+WGRAD_CASES = [
+    ("mode1", (2, 64, 64, 8, 512, 3, (1, 1)), None),        # four 128-pixel segments
+    ("mode1", (1, 64, 64, 6, 180, 3, (1, 1)), None),        # ragged second segment
+    ("mode1", (2, 64, 64, 3, 129, 3, (1, 1)), None),        # 1-pixel second segment
+    ("mode1", (1, 128, 64, 1, 7, 3, (1, 1)), None),         # Hout = 1, NS = 16, two ci tiles, one K row: one split
+    ("mode1", (1, 64, 64, 6, 180, 3, (1, 1)), 37),          # Cin_true < Cin through wgrad2_reduce_kernel
+    ("mode0", (2, 128, 128, 8, 256, 3, (1, 1)), None),
+    ("mode0", (2, 512, 512, 4, 64, 3, (1, 1)), None),
+    ("mode0", (1, 512, 512, 5, 23, 3, (1, 1)), None),       # NS = 32, one ragged segment
+    ("mode0", (2, 64, 128, 8, 512, 3, (1, 2)), None),       # strided: even / odd column tiles
+    ("mode0", (1, 128, 256, 6, 90, 3, (1, 2)), None),       # NS = 48
+    ("mode0", (2, 256, 512, 9, 128, 3, (2, 2)), None),      # odd Hin
+    ("mode0", (1, 256, 512, 5, 45, 3, (2, 2)), None),       # odd Win, Wout = 23
+    ("mode0", (2, 64, 128, 4, 130, 3, (1, 2)), None),       # 1-pixel second segment at the stride-2 cap of 64
+    ("mode0", (1, 128, 256, 6, 90, 3, (1, 2)), 70),         # Cin_true < Cin, strided
+    ("gen1", (2, 64, 128, 8, 512, 1, (1, 2)), None),        # 1x1 downsamples: nb = 1
+    ("gen1", (1, 128, 256, 6, 90, 1, (1, 2)), None),        # nb = 2
+    ("gen1", (2, 256, 512, 9, 45, 1, (2, 2)), None),        # nb = 4
+    ("gen1", (2, 64, 64, 6, 90, 3, (1, 2)), None),          # 3x3, Cout 64, strided: tap group tg = 3
+    ("gen1", (2, 128, 64, 5, 64, 3, (1, 2)), None),         # tg = 2: groups of taps (0, 1) and (2)
+    ("gen1", (1, 256, 64, 7, 46, 3, (2, 2)), None),         # tg = 1
+    ("gen1", (2, 64, 64, 5, 181, 3, (1, 2)), 8),            # the odd-width stem: 8 real channels padded to 64
+]
+# the stem kernel (conv_stem.cu, wgrad2 mode 2): B, H, W of the image, Cin_true
+STEM_WGRAD_CASES = [
+    (2, 64, 2048, 8),       # the bench shape: 8 segments per row, 132 splits
+    (1, 16, 180, 8),        # one ragged segment
+    (1, 1, 10, 4),          # Cin_true = 4, one K row
+    (3, 5, 258, 8),         # 1-pixel second segment
+]
+# the Gaussian tier: a subset covering every kernel and both reduce kernels
+WGRAD_GAUSS_CASES = [WGRAD_CASES[i] for i in (1, 4, 6, 10, 12, 13, 15, 18, 20)]
+STEM_WGRAD_GAUSS_CASES = [STEM_WGRAD_CASES[i] for i in (0, 2, 3)]
+GUARD = 4096            # fp32 NaN guard floats behind the scratch and on both sides of dW
+
+
+def _wgrad_id(case):
+    path, (b, cin, cout, h, w, k, st), ct = case
+    return f"{path}-{cin}x{cout}-k{k}-{h}x{w}-s{st[0]}{st[1]}-b{b}" + (f"-cin{ct}" if ct else "")
+
+
+def _stem_id(case):
+    b, h, w, ct = case
+    return f"stem-{h}x{w}-b{b}-cin{ct}"
+
+
+def wgrad_ref(x, dz, k, stride):
+    """w.grad of the layer's convolution (conv_ref) after backward(dz), float64 autograd."""
+    w = torch.zeros((dz.shape[1], x.shape[1], k, k), dtype=torch.float64, device=DEV, requires_grad=True)
+    conv_ref(x, w, stride).backward(dz)
+    return w.grad
+
+
+def int_range(n):
+    """Largest r <= 8 with n r^2 < 2^23: every partial sum of n products of integers in [-r, r] is then an integer
+    below 2^23, so fp32 adds it exactly in any order and with any rounding mode."""
+    return max(1, min(8, math.isqrt((2 ** 23 - 1) // n)))
+
+
+def assert_exact_premise(n, dz, x, label):
+    bound = n * dz.abs().max().item() * x.abs().max().item()
+    assert bound < 2 ** 23, f"{label}: n max|dz| max|x| = {bound} does not keep the partial sums exact"
+
+
+def padded_grad(dz, junk):
+    """The output gradient in the padded layout with `junk` in all of its halo: the weight gradients never read it
+    (their dz maps stop at the last real pixel), so a halo read changes the result."""
+    p = to_padded_nhwc(dz)
+    p[:, 0] = junk
+    p[:, -1] = junk
+    p[:, :, 0] = junk
+    p[:, :, -1] = junk
+    return p
+
+
+def guarded_wgrad(launch, n_scratch, out_shape, label):
+    """launch(dw_ptr, scratch_ptr) with exactly n_scratch scratch floats (the size query's answer) pre-filled with NaN
+    and followed by a NaN guard, and dW a slice in the middle of a NaN buffer.  Finite dW: every element written, and
+    every split-K slot the reduce read written by this call (the scratch is reused across layers).  Unchanged guards:
+    the query covers every kernel of the launch, and nothing lands outside dW."""
+    numel = math.prod(out_shape)
+    scratch = torch.full((n_scratch + GUARD,), float("nan"), dtype=torch.float32, device=DEV)
+    buf = torch.full((GUARD + numel + GUARD,), float("nan"), dtype=torch.float32, device=DEV)
+    launch(buf[GUARD:GUARD + numel].data_ptr(), scratch.data_ptr())
+    nan_bits = torch.full((GUARD,), float("nan"), dtype=torch.float32, device=DEV).view(torch.int32)
+    assert torch.equal(scratch[n_scratch:].view(torch.int32), nan_bits), \
+        f"{label}: written past the {n_scratch} scratch floats of the size query"
+    assert torch.equal(buf[:GUARD].view(torch.int32), nan_bits) and \
+        torch.equal(buf[GUARD + numel:].view(torch.int32), nan_bits), f"{label}: written outside the dW slice"
+    dw = buf[GUARD:GUARD + numel].view(out_shape)
+    bad = ~torch.isfinite(dw)
+    assert not bool(bad.any()), f"{label}: {int(bad.sum())} non-finite dW elements (unwritten, or built from a split-K " \
+                                f"slot not written this call), first (co, ci, r, q) = {tuple(bad.nonzero()[0].tolist())}"
+    return dw
+
+
+def wgrad_problem(case, exact):
+    """Operands of a delora_conv2d_wgrad_bf16 case in the kernels' layouts, the float64 reference and the launcher."""
+    from delora_b200 import ops
+    L = ops._lib.lib()
+    _, (b, cin, cout, hin, win, k, stride), cin_true = case
+    ct = cin if cin_true is None else cin_true
+    hout, wout = ops.conv_out_size(hin, stride[0]), ops.conv_out_size(win, stride[1])
+    n = b * hout * wout                                     # products per dW element
+    g = generator("wgrad", case, exact)
+    if exact:
+        r = int_range(n)
+        x, dz = rand_int(g, (b, cin, hin, win), r), rand_int(g, (b, cout, hout, wout), r)
+        assert_exact_premise(n, dz, x, _wgrad_id(case))
+    else:
+        x, dz = rand_bf16(g, (b, cin, hin, win)), rand_bf16(g, (b, cout, hout, wout))
+    # channels ct .. Cin of x hold nonzero values: the reduce must drop them
+    ref = wgrad_ref(x[:, :ct], dz, k, stride)
+    ref_abs = None if exact else wgrad_ref(x[:, :ct].abs(), dz.abs(), k, stride)
+    xp, dzp = to_padded_nhwc(x), padded_grad(dz, 3.0 if exact else 1.0)
+    n_scratch = int(L.delora_conv2d_wgrad_scratch_floats(b, hout, wout, cin, cout, k))
+
+    def launch(dw_ptr, scratch_ptr):
+        ops._lib.check(L.delora_conv2d_wgrad_bf16(ops._req(xp, torch.bfloat16, "x"), ops._req(dzp, torch.bfloat16, "dz"),
+                                                  dw_ptr, scratch_ptr, b, hin, win, cin, ct, cout, k, stride[0], stride[1],
+                                                  ops._stream()), "delora_conv2d_wgrad_bf16")
+    return launch, n_scratch, (cout, ct, k, k), ref, ref_abs, n
+
+
+def stem_wgrad_problem(case, exact):
+    """Operands of a delora_stem_wgrad_bf16 case: the 16-channel input whose channels c and c + 8 (bf16(x) and its
+    rounding residual) get independent values and share one weight, so dW = sum dz (x[c] + x[c + 8])."""
+    from delora_b200 import ops
+    L = ops._lib.lib()
+    b, h, w, ct = case
+    wout = w // 2
+    n = 2 * b * h * wout
+    g = generator("stem wgrad", case, exact)
+    if exact:
+        r = int_range(n)
+        x, dz = rand_int(g, (b, 16, h, w), r), rand_int(g, (b, 64, h, wout), r)
+        assert_exact_premise(n, dz, x, _stem_id(case))
+    else:
+        x = torch.cat([rand_bf16(g, (b, 8, h, w)), rand_bf16(g, (b, 8, h, w), 2.0 ** -8)], dim=1)
+        dz = rand_bf16(g, (b, 64, h, wout))
+    # channels ct .. 7 and 8 + ct .. 15 hold nonzero values: the reduce must drop them
+    ref = wgrad_ref(x[:, :ct] + x[:, 8:8 + ct], dz, 3, (1, 2))
+    ref_abs = None if exact else wgrad_ref(x[:, :ct].abs() + x[:, 8:8 + ct].abs(), dz.abs(), 3, (1, 2))
+    xp, dzp = to_padded_nhwc(x), padded_grad(dz, 3.0 if exact else 1.0)
+    n_scratch = int(L.delora_stem_wgrad_scratch_floats(b, h, w))
+
+    def launch(dw_ptr, scratch_ptr):
+        ops._lib.check(L.delora_stem_wgrad_bf16(ops._req(xp, torch.bfloat16, "x16"), ops._req(dzp, torch.bfloat16, "dz"),
+                                                dw_ptr, scratch_ptr, b, h, w, ct, ops._stream()), "delora_stem_wgrad_bf16")
+    return launch, n_scratch, (64, ct, 3, 3), ref, ref_abs, n
+
+
+def _wgrad_exact(problem, label):
+    launch, n_scratch, out_shape, ref, _, _ = problem
+    check_exact(guarded_wgrad(launch, n_scratch, out_shape, label).double(), ref, label)
+
+
+def _wgrad_gauss(problem, label):
+    launch, n_scratch, out_shape, ref, ref_abs, n = problem
+    a = guarded_wgrad(launch, n_scratch, out_shape, label)
+    b = guarded_wgrad(launch, n_scratch, out_shape, label)
+    assert torch.equal(a.view(torch.int32), b.view(torch.int32)), f"{label}: two calls differ"
+    check_bound(a.double(), ref, ref_abs, n, label, out_unit=0.0, acc_unit=2.0 ** -23)
+
+
+@pytest.mark.parametrize("case", WGRAD_CASES, ids=_wgrad_id)
+def test_wgrad_exact_on_integers(case, cuda_lib):
+    """delora_conv2d_wgrad_bf16 on integer operands equals float64 autograd bit for bit."""
+    _wgrad_exact(wgrad_problem(case, True), "wgrad exact " + _wgrad_id(case))
+
+
+@pytest.mark.parametrize("case", STEM_WGRAD_CASES, ids=_stem_id)
+def test_stem_wgrad_exact_on_integers(case, cuda_lib):
+    """delora_stem_wgrad_bf16 on integer operands equals float64 autograd bit for bit."""
+    _wgrad_exact(stem_wgrad_problem(case, True), "wgrad exact " + _stem_id(case))
+
+
+@pytest.mark.parametrize("case", WGRAD_GAUSS_CASES, ids=_wgrad_id)
+def test_wgrad_gaussian(case, cuda_lib):
+    """Gaussian bf16 operands: deterministic (two calls bit-identical) and within the fp32 accumulation bound."""
+    _wgrad_gauss(wgrad_problem(case, False), "wgrad gauss " + _wgrad_id(case))
+
+
+@pytest.mark.parametrize("case", STEM_WGRAD_GAUSS_CASES, ids=_stem_id)
+def test_stem_wgrad_gaussian(case, cuda_lib):
+    _wgrad_gauss(stem_wgrad_problem(case, False), "wgrad gauss " + _stem_id(case))
 
 
 # ------------------------------------------------------------------------------------------------ pools
