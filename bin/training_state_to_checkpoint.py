@@ -3,7 +3,7 @@
 --training-state) back into the reference Trainer's checkpoint (.pth: `epoch`, `model_state_dict`,
 `optimizer_state_dict`, `loss`, `parameters`), loadable by its `--checkpoint` option and by torch.optim.Adam.
 `parameters` is the YAML configuration of `--config_dir` (when it exists) with the network and range-image keys of
-the file's header."""
+the file's header, and `normalization_scaling` from its model_flags."""
 import os
 import sys
 
@@ -21,9 +21,9 @@ from delora_b200.deploy import export as export_module  # noqa: E402
 @click.option("--dataset", default="kitti", show_default=True, help="Dataset whose range image the header describes.")
 @click.option("--config_dir", default="config", show_default=True, help="YAML files for `parameters` (optional).")
 def main(dlt_path, out, dataset, config_dir):
-    _, desc, state = export_module.read_dlt(dlt_path)
+    header, desc, state = export_module.read_dlt(dlt_path)
     base = export_module.model_config(None, config_dir) if os.path.isdir(config_dir) else None
-    config = export_module.config_from_desc(desc, base, dataset)
+    config = export_module.config_from_desc(desc, base, dataset, header["model_flags"])
     torch.save(export_module.checkpoint_from_training_state(state, config), out)
     print(f"wrote {out}: epoch {state.epoch - 1}, Adam step {state.step}, loss {state.loss:.9g}, "
           f"{'unsupervised' if state.unsupervised else 'identity pre-training'}")

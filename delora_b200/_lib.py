@@ -101,6 +101,9 @@ SIGNATURES = {
     "delora_odometry_load_weights": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_pairs": (c_int, [c_desc_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_push": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "delora_normalization_factors": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "delora_odometry_pairs_normalized": (c_int, [c_desc_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                                 c_void_p, c_void_p]),
     "delora_odometry_streams_workspace_bytes": (c_i64, [c_desc_p]),
     "delora_odometry_streams_init": (c_int, [c_desc_p, c_void_p, c_void_p]),
     "delora_odometry_streams_load_weights": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),
@@ -117,6 +120,8 @@ SIGNATURES = {
 }
 
 ABI_VERSION = 3
+# model_flags bits of the .dlw / .dlt header (DELORA_MODEL_* in include/delora_b200.h)
+MODEL_NORMALIZATION_SCALING = 1
 _lib = None
 
 

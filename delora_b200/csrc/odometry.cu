@@ -19,6 +19,7 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "projection.cuh"
 
 namespace delora {
 
@@ -119,8 +120,11 @@ __device__ __forceinline__ void head_outputs(const TailLinear& rot, const TailLi
 
 // Last layer of the heads, quaternion / ||quaternion block||_F, quaternion -> T.
 // raw [B, 7] or NULL: the head outputs before the normalisation (quaternion, translation), which training keeps.
+// kRescale (normalised models, src/deploy/deployer.py:344-346): T[:3, 3] of row b is then multiplied by factor[b].
+template <bool kRescale>
 __global__ void __launch_bounds__(kTailWarps * 32)
-odometry_out_kernel(TailLinear rot, TailLinear trans, int B, int vec, float* __restrict__ T, float* __restrict__ raw) {
+odometry_out_kernel(TailLinear rot, TailLinear trans, int B, int vec, float* __restrict__ T, float* __restrict__ raw,
+                    const float* __restrict__ factor) {
     extern __shared__ float s_out[];                        // [B, 7]: quaternion (x, y, z, w), translation
     __shared__ float s_norm;
     head_outputs(rot, trans, B, vec, [](int) { return true; }, s_out);
@@ -137,7 +141,12 @@ odometry_out_kernel(TailLinear rot, TailLinear trans, int B, int vec, float* __r
     const float nrm = s_norm;
     for (int b = threadIdx.x; b < B; b += blockDim.x) {
         const float* q = s_out + b * 7;
-        quat_to_T_row(q[0] / nrm, q[1] / nrm, q[2] / nrm, q[3] / nrm, q[4], q[5], q[6], T + (size_t)b * 16);
+        float* t = T + (size_t)b * 16;
+        quat_to_T_row(q[0] / nrm, q[1] / nrm, q[2] / nrm, q[3] / nrm, q[4], q[5], q[6], t);
+        if (kRescale) {
+            const float f = factor[b];
+            t[3] = __fmul_rn(t[3], f); t[7] = __fmul_rn(t[7], f); t[11] = __fmul_rn(t[11], f);
+        }
     }
 }
 
@@ -518,12 +527,18 @@ static int run_tail_hidden(const Model& m, const TailIO& io, int act, const floa
     return 0;
 }
 
-static int run_tail(const Model& m, const TailIO& io, int act, const float* pooled, int B, float* T, cudaStream_t st) {
+// factor [B] or NULL: multiply each row's translation by its pair's normalisation factor
+static int run_tail(const Model& m, const TailIO& io, int act, const float* pooled, int B, float* T, cudaStream_t st,
+                    const float* factor = nullptr) {
     TailLinear rot, trans;
     const int rc = run_tail_hidden(m, io, act, pooled, B, &rot, &trans, st);
     if (rc) return rc;
     const int vec = tail_vec(rot) && tail_vec(trans);
-    odometry_out_kernel<<<1, kTailWarps * 32, (size_t)B * 7 * sizeof(float), st>>>(rot, trans, B, vec, T, io.raw);
+    const size_t smem = (size_t)B * 7 * sizeof(float);
+    if (factor)
+        odometry_out_kernel<true><<<1, kTailWarps * 32, smem, st>>>(rot, trans, B, vec, T, io.raw, factor);
+    else
+        odometry_out_kernel<false><<<1, kTailWarps * 32, smem, st>>>(rot, trans, B, vec, T, io.raw, nullptr);
     DELORA_CHECK_LAUNCH("odometry_out_kernel");
     return 0;
 }
@@ -544,6 +559,20 @@ static int project(const Frames& f, const delora_odometry_desc* d, char* ws, con
     return delora_project_fwd(points, reinterpret_cast<int32_t*>(ws + f.counts), n_scans, 3, d->n_stride, d->H, d->W,
                               d->hfov0, d->hfov1, d->vfov0, d->vfov1, 0, reinterpret_cast<uint64_t*>(ws + f.keys),
                               reinterpret_cast<float*>(ws + f.images), reinterpret_cast<int32_t*>(ws + f.index_map), st);
+}
+
+// The 2B scans of B pairs divided by their pair's normalisation factor, then projected: the clamped counts, the factor
+// of every pair into factor [B], and the scaled instantiations of the projection's two passes.
+static int project_normalized(const Frames& f, const delora_odometry_desc* d, char* ws, const float* points,
+                              const int32_t* n_points, int B, float* factor, cudaStream_t st) {
+    int rc = clamp_counts(f, ws, n_points, nullptr, 2 * B, d->n_stride, st);
+    if (rc) return rc;
+    const int32_t* counts = reinterpret_cast<const int32_t*>(ws + f.counts);
+    if ((rc = launch_normalization_factors(points, counts, B, d->n_stride, factor, st))) return rc;
+    const GridParams g = make_grid(d->H, d->W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, 0);
+    return project_fwd(points, counts, 2 * B, 3, d->n_stride, g, reinterpret_cast<uint64_t*>(ws + f.keys),
+                       reinterpret_cast<float*>(ws + f.images), reinterpret_cast<int32_t*>(ws + f.index_map), factor, B,
+                       st);
 }
 
 // Every workspace starts zeroed, with its depth keys at all ones (the projection's empty key)
@@ -608,29 +637,50 @@ extern "C" int delora_odometry_load_weights(const delora_odometry_desc* d, const
     return load_weights(p, weights, workspace, (cudaStream_t)stream, "delora_odometry_load_weights");
 }
 
+// delora_odometry_pairs and, with factor non-NULL, delora_odometry_pairs_normalized (arguments checked by the caller)
+static int run_pairs(const delora_odometry_desc* d, const float* points, const int32_t* n_points, int B, void* workspace,
+                     float* T, float* pooled, float* factor, cudaStream_t st, const char* who) {
+    InferPlan p;
+    make_infer_plan(d, false, &p);
+    char* ws = (char*)workspace;
+    float* images = reinterpret_cast<float*>(ws + p.f.images);
+    const size_t img = (size_t)4 * d->H * d->W;
+    float* pooled_ws = reinterpret_cast<float*>(ws + p.pooled);
+    int rc;
+    if (factor) rc = project_normalized(p.f, d, ws, points, n_points, B, factor, st);
+    else rc = project(p.f, d, ws, points, n_points, nullptr, 2 * B, st);
+    if (rc) return rc;
+    if ((rc = trunk_input(p.m, p.t, ws, images, images + (size_t)B * img, B, st))) return rc;
+    if ((rc = trunk_forward(p.m, p.t, p.w, false, ws, d->act, B, pooled_ws, st))) return rc;
+    if ((rc = run_tail(p.m, inference_tail_io(p, ws), d->act, pooled_ws, B, T, st, factor))) return rc;
+    if (pooled) {
+        const cudaError_t e = cudaMemcpyAsync(pooled, pooled_ws, (size_t)B * 512 * sizeof(float), cudaMemcpyDeviceToDevice, st);
+        DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+    }
+    return 0;
+}
+
 extern "C" int delora_odometry_pairs(const delora_odometry_desc* d, const float* points, const int32_t* n_points, int B,
                                      void* workspace, float* T, float* pooled, void* stream) {
     if (check_desc(d, "delora_odometry_pairs")) return 1;
     DELORA_CHECK_ARG(points && n_points && workspace && T, "delora_odometry_pairs: null pointer");
     DELORA_CHECK_ARG(B >= 1 && B <= d->max_batch, "delora_odometry_pairs: B=%d outside [1, max_batch=%d]", B,
                      d->max_batch);
-    InferPlan p;
-    make_infer_plan(d, false, &p);
-    cudaStream_t st = (cudaStream_t)stream;
-    char* ws = (char*)workspace;
-    float* images = reinterpret_cast<float*>(ws + p.f.images);
-    const size_t img = (size_t)4 * d->H * d->W;
-    float* pooled_ws = reinterpret_cast<float*>(ws + p.pooled);
-    int rc;
-    if ((rc = project(p.f, d, ws, points, n_points, nullptr, 2 * B, st))) return rc;
-    if ((rc = trunk_input(p.m, p.t, ws, images, images + (size_t)B * img, B, st))) return rc;
-    if ((rc = trunk_forward(p.m, p.t, p.w, false, ws, d->act, B, pooled_ws, st))) return rc;
-    if ((rc = run_tail(p.m, inference_tail_io(p, ws), d->act, pooled_ws, B, T, st))) return rc;
-    if (pooled) {
-        const cudaError_t e = cudaMemcpyAsync(pooled, pooled_ws, (size_t)B * 512 * sizeof(float), cudaMemcpyDeviceToDevice, st);
-        DELORA_CHECK_ARG(e == cudaSuccess, "delora_odometry_pairs: %s", cudaGetErrorString(e));
-    }
-    return 0;
+    return run_pairs(d, points, n_points, B, workspace, T, pooled, nullptr, (cudaStream_t)stream, "delora_odometry_pairs");
+}
+
+extern "C" int delora_odometry_pairs_normalized(const delora_odometry_desc* d, const float* points,
+                                                const int32_t* n_points, int B, void* workspace, float* T,
+                                                float* pooled, float* factor, void* stream) {
+    const char* who = "delora_odometry_pairs_normalized";
+    if (check_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(points, "%s: null points", who);
+    DELORA_CHECK_ARG(n_points, "%s: null n_points", who);
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    DELORA_CHECK_ARG(T, "%s: null T", who);
+    DELORA_CHECK_ARG(factor, "%s: null factor", who);
+    DELORA_CHECK_ARG(B >= 1 && B <= d->max_batch, "%s: B=%d outside [1, max_batch=%d]", who, B, d->max_batch);
+    return run_pairs(d, points, n_points, B, workspace, T, pooled, factor, (cudaStream_t)stream, who);
 }
 
 extern "C" int delora_odometry_push(const delora_odometry_desc* d, const float* points, const int32_t* n_points,
@@ -854,6 +904,8 @@ extern "C" int delora_odometry_streams_reset(const delora_odometry_desc* d, cons
 //     hidden layers: their contributions to dx are summed in a fixed order), dW / db and dx * act'(x) in one launch.
 //   odometry_adam_kernel: torch's Adam (fused formula, no weight decay) over the whole blob, float4 per thread; the
 //     step count is read from the workspace, so the bias corrections need no host value.
+//   odometry_train_normalized_out_kernel (DELORA_TRAIN_NORMALIZATION_SCALING): T with its translation rescaled to the
+//     caller's output, the factor to losses[b][6].
 //   odometry_icp_rearm_kernel: zeroes the ICP scratch when B differs from the batch size of the previous step (the
 //     scratch layout depends on B); otherwise every CTA exits at once.
 namespace delora {
@@ -1073,6 +1125,18 @@ odometry_adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* 
         const long long i = n4 * 4 + threadIdx.x;
         upd(p[i], g[i], m[i], v[i]);
     }
+}
+
+// The training step of a normalised model (DELORA_TRAIN_NORMALIZATION_SCALING), after the ICP finalize: T_out [B, 16] =
+// the forward's T with T[:3, 3] multiplied by the pair's factor (or no copy when T_out is NULL), losses[b][6] = factor[b].
+__global__ void odometry_train_normalized_out_kernel(const float* __restrict__ T16, const float* __restrict__ factor,
+                                                     int B, float* __restrict__ T_out, float* __restrict__ losses) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= B * 16) return;
+    const int b = i >> 4, e = i & 15;
+    const float f = factor[b];
+    if (T_out) T_out[i] = (e == 3 || e == 7 || e == 11) ? __fmul_rn(T16[i], f) : T16[i];
+    if (e == 0) losses[(size_t)b * DELORA_LOSS_ROW + 6] = f;
 }
 
 __global__ void odometry_icp_rearm_kernel(float4* __restrict__ s, long long n4, int B, const long long* __restrict__ ctr) {
@@ -1382,6 +1446,10 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
     if (check_train_params(hp, who)) return 1;
     DELORA_CHECK_ARG(points && n_points && workspace, "%s: null pointer", who);
     DELORA_CHECK_ARG(B >= 1 && B <= d->max_batch, "%s: B=%d outside [1, max_batch=%d]", who, B, d->max_batch);
+    const bool normalized = (hp->loss_flags & DELORA_TRAIN_NORMALIZATION_SCALING) != 0u;
+    DELORA_CHECK_ARG(!normalized || d->w_pre > 0,
+                     "%s: DELORA_TRAIN_NORMALIZATION_SCALING needs w_pre > 0 (the reference's recipe: normals from the "
+                     "unscaled points at H x w_pre), got w_pre=%d", who, d->w_pre);
     TrainPlan tp;
     make_train_plan(d, &tp);
     const Model& m = tp.m;
@@ -1409,9 +1477,14 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
                                              reinterpret_cast<int32_t*>(ws + tp.pre_index_map), hp->nb_h, hp->nb_w,
                                              hp->epsilon_range, hp->min_neighbors, pre_pts, pre_nrm, nullptr, st)))
             return rc;
-        if ((rc = delora_project_grids_fwd(pre_pts, pre_nrm, 2 * B, H, d->w_pre, W, d->hfov0, d->hfov1, d->vfov0,
-                                           d->vfov1, 0, keys, images, reinterpret_cast<int32_t*>(ws + tp.f.index_map),
-                                           pts_grid, nrm_grid, st)))
+        // normalised: the factor of each pair from its stored points (the valid H x w_pre cells), kept in the H x w_pre
+        // image, which nothing reads after delora_project_normals_fwd; the stored points are divided by it before the
+        // H x W projection, the normals are not
+        float* factor = normalized ? f(tp.pre_image) : nullptr;
+        if (normalized && (rc = launch_grid_normalization_factors(pre_pts, B, H * d->w_pre, factor, st))) return rc;
+        const GridParams g = make_grid(H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, 0);
+        if ((rc = project_grids_fwd(pre_pts, pre_nrm, 2 * B, d->w_pre, g, keys, images,
+                                    reinterpret_cast<int32_t*>(ws + tp.f.index_map), pts_grid, nrm_grid, factor, B, st)))
             return rc;
     } else if ((rc = delora_project_normals_fwd(points, counts, 2 * B, 3, d->n_stride, H, W, d->hfov0, d->hfov1,
                                                 d->vfov0, d->vfov1, 0, keys, images,
@@ -1435,8 +1508,13 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
     DELORA_CHECK_LAUNCH("odometry_icp_rearm_kernel");
     if ((rc = delora_icp_dense_fwd_bwd(pts_grid + (size_t)B * HW, nrm_grid + (size_t)B * HW, f(tp.T12), pts_grid, nrm_grid,
                                        B, H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, hp->lambda_po2pl,
-                                       hp->loss_flags & ~DELORA_LOSS_IDENTITY_FIT, f(tp.losses), f(tp.grad_T), f(tp.icp),
-                                       st))) return rc;
+                                       hp->loss_flags & ~(DELORA_LOSS_IDENTITY_FIT | DELORA_TRAIN_NORMALIZATION_SCALING),
+                                       f(tp.losses), f(tp.grad_T), f(tp.icp), st))) return rc;
+    if (normalized) {               // T in metres for the caller, the factor in losses[b][6]
+        odometry_train_normalized_out_kernel<<<(B * 16 + 255) / 256, 256, 0, st>>>(f(tp.T16), f(tp.pre_image), B, T,
+                                                                                      f(tp.losses));
+        DELORA_CHECK_LAUNCH("odometry_train_normalized_out_kernel");
+    }
     // 4. backward: tail (dL/dT of the ICP mean or of the identity fit), average pool, trunk
     if ((rc = train_tail_backward(tp, ws, d->act, B, identity, st))) return rc;
     if ((rc = train_trunk_backward(tp, ws, d->act, B, st))) return rc;
@@ -1445,7 +1523,7 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
         if (dst && e == cudaSuccess) e = cudaMemcpyAsync(dst, ws + src, n * sizeof(float), cudaMemcpyDeviceToDevice, st);
     };
     out(losses, tp.losses, (size_t)B * DELORA_LOSS_ROW);
-    out(T, tp.T16, (size_t)B * 16);
+    if (!normalized) out(T, tp.T16, (size_t)B * 16);
     out(pooled, tp.pooled, (size_t)B * 512);
     out(grads, tp.grad, (size_t)m.blob_floats);
     DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));

@@ -26,10 +26,38 @@ __device__ __forceinline__ unsigned long long depth_key(float x, float y, float 
     return ((unsigned long long)__float_as_uint(range3(x, y, z)) << 32) | id;
 }
 
+// A coordinate of a scaled projection: v / f correctly rounded (torch's tensor-by-tensor division), the value itself
+// when the projection is not scaled or the channel is not a coordinate.
+template <bool kScaled>
+__device__ __forceinline__ float scaled(float v, float f, bool coordinate = true) {
+    return (kScaled && coordinate) ? __fdiv_rn(v, f) : v;
+}
+
 // Enqueue project_scatter_kernel: one 64-bit atomicMin of (range_bits << 32 | point_index) per in-FOV point into
 // `keys` ([B, H*W], all-ones on entry).  The kernel lets its programmatic dependent launch as soon as all of its CTAs
-// have started.  Check the launch with DELORA_CHECK_LAUNCH.
+// have started.  Check the launch with DELORA_CHECK_LAUNCH.  factor [fB] or NULL: scan b's coordinates are divided by
+// factor[b % fB] first (a separate instantiation; NULL runs the unscaled kernel).
 void launch_project_scatter(const float* points, const int32_t* n_points, int B, int C, int n_stride,
-                            const GridParams& g, unsigned long long* keys, cudaStream_t st);
+                            const GridParams& g, unsigned long long* keys, cudaStream_t st,
+                            const float* factor = nullptr, int fB = 0);
+
+// delora_normalization_factors' kernel on points [2B, 3, n_stride], counts [2B] (clamped to [0, n_stride] on the device)
+// -> factor [B].  Arguments are not checked.
+int launch_normalization_factors(const float* points, const int32_t* n_points, int B, int n_stride, float* factor,
+                                 cudaStream_t st);
+
+// The same factor of B pairs from the valid cells of the dense grids [2B, n_cells] float4 (delora_normals_fwd's layout:
+// w = pixel-id bits >= 0 for a valid cell), the points the reference's preprocessing stored.  Arguments are not checked.
+int launch_grid_normalization_factors(const delora_f4* grid, int B, int n_cells, float* factor, cudaStream_t st);
+
+// delora_project_grids_fwd's two passes (g: the model's H x W grid), optionally with scan s's cell coordinates divided
+// by factor[s % fB] (factor NULL: the unscaled kernels).  Arguments are not checked.
+int project_grids_fwd(const delora_f4* pts_grid_pre, const delora_f4* nrm_grid_pre, int S, int Wp, const GridParams& g,
+                      uint64_t* keys, float* image, int32_t* index_map, delora_f4* pts_grid, delora_f4* nrm_grid,
+                      const float* factor, int fB, cudaStream_t st);
+
+// delora_project_fwd's scatter and resolve passes, optionally scaled as above.  Arguments are not checked.
+int project_fwd(const float* points, const int32_t* n_points, int B, int C, int n_stride, const GridParams& g,
+                uint64_t* keys, float* image, int32_t* index_map, const float* factor, int fB, cudaStream_t st);
 
 }  // namespace delora

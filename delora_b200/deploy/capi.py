@@ -1,5 +1,5 @@
 """ctypes binding of the odometry workspaces of the C ABI (include/delora_b200.h): inference (`delora_odometry_pairs` /
-`_push`), streams (`delora_odometry_streams_*`) and training (`delora_odometry_train_*`).
+`_pairs_normalized` / `_push`), streams (`delora_odometry_streams_*`) and training (`delora_odometry_train_*`).
 
 Each class holds one descriptor and one workspace, a torch uint8 tensor on the current device.  Every call runs on
 torch's current stream at call time, checks its status with `_lib.check` and does not synchronise (except
@@ -21,8 +21,12 @@ def _ptr(t):
 
 
 def train_params(config, lr, loss_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL, beta1=0.9, beta2=0.999, eps=1e-8):
-    """delora_odometry_train_params: Adam's settings and the loss and normals' settings of a reference-style config."""
+    """delora_odometry_train_params: Adam's settings and the loss and normals' settings of a reference-style config.
+    normalization_scaling: True adds DELORA_TRAIN_NORMALIZATION_SCALING (the step then needs a descriptor with
+    w_pre > 0, and refuses w_pre = 0)."""
     nb = config["kitti"]["neighborhood_side_length"]
+    if config.get("normalization_scaling", False):
+        loss_flags |= ops.TRAIN_NORMALIZATION_SCALING
     return _lib.OdometryTrainParams(
         lr=lr, beta1=beta1, beta2=beta2, eps=eps, lambda_po2pl=config["lambda_po2pl"], loss_flags=loss_flags,
         nb_h=nb[0], nb_w=nb[1], epsilon_range=config["epsilon_range"],
@@ -58,7 +62,7 @@ class _Workspace:
 
 
 class InferenceWorkspace(_Workspace):
-    """delora_odometry_workspace_bytes / _init / _load_weights / _pairs / _push."""
+    """delora_odometry_workspace_bytes / _init / _load_weights / _pairs / _pairs_normalized / _push."""
     SIZE_QUERY = "delora_odometry_workspace_bytes"
 
     def __init__(self, desc, weights, workspace=None):
@@ -77,6 +81,18 @@ class InferenceWorkspace(_Workspace):
         self._call("delora_odometry_pairs", points.data_ptr(), counts.data_ptr(), b, self.workspace.data_ptr(),
                    t.data_ptr(), pooled.data_ptr())
         return t, pooled
+
+    def pairs_normalized(self, points, counts):
+        """A model trained with normalization_scaling: points [2B, 3, n_stride], counts [2B] -> (T [B, 4, 4] with the
+        translation in metres, pooled [B, 512], factor [B])."""
+        b = points.shape[0] // 2
+        dev = self.workspace.device
+        t = torch.empty((b, 4, 4), dtype=torch.float32, device=dev)
+        pooled = torch.empty((b, 512), dtype=torch.float32, device=dev)
+        factor = torch.empty((b,), dtype=torch.float32, device=dev)
+        self._call("delora_odometry_pairs_normalized", points.data_ptr(), counts.data_ptr(), b,
+                   self.workspace.data_ptr(), t.data_ptr(), pooled.data_ptr(), factor.data_ptr())
+        return t, pooled, factor
 
     def push(self, points, count, T):
         """One frame [1, 3, n_stride]; T [16] out, or None for a stream's first frame (project and cache only)."""
@@ -117,7 +133,7 @@ class TrainingWorkspace(_Workspace):
 
     def step(self, points, counts, outputs=True):
         """One step on B = rows // 2 pairs -> (losses [B, 8], T [B, 4, 4], pooled [B, 512], grads [n]), or None
-        without outputs."""
+        without outputs.  Normalised models: losses[:, 6] is each pair's factor and T's translation is in metres."""
         b = points.shape[0] // 2
         out, ptrs = None, (None,) * 4
         if outputs:

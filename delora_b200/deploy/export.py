@@ -6,6 +6,8 @@ alone and hands the blob to `delora_odometry_load_weights`.  The network configu
 `parameters` dict when it carries one (it wins over the YAML files, as in bin/run_testing.py), otherwise from
 `config/*.yaml` (angles there are in degrees).  Checkpoints of models the C ABI cannot express are refused:
 `pre_feature_extraction: True` and `factor_fewer_resnet_channels != 1`; dropout is the identity at inference.
+`normalization_scaling: True` is recorded in the header's `model_flags` (DELORA_MODEL_NORMALIZATION_SCALING): such a
+model runs through `delora_odometry_pairs_normalized`, and reading the file back restores the key.
 
 A .dlt file is a training checkpoint for `delora_odometry_train_set_state`: a 256-byte header (the .dlw header with
 its own magic, then Adam's step count, the epoch, the phase, Adam's hyperparameters and the last epoch loss) followed
@@ -25,8 +27,8 @@ MAGIC = b"DELORAW\x00"
 HEADER_BYTES = 128
 # magic, abi_version, header_bytes | H, W, hfov0, hfov1, vfov0, vfov1 | n_stride, max_batch, act, layers[4],
 # resnet_outputs, single_mlp, w_pre (byte 92; files written before the field have zeros there) | blob_floats |
-# 24 reserved bytes
-_HEADER = struct.Struct("<8sii" + "ii4d" + "iii4iiii" + "q" + "24x")
+# model_flags (byte 104; zeros in files written before the field: no flag) | 20 reserved bytes
+_HEADER = struct.Struct("<8sii" + "ii4d" + "iii4iiii" + "q" + "I20x")
 assert _HEADER.size == HEADER_BYTES
 
 
@@ -55,6 +57,11 @@ def check_supported(config):
                          "the odometry C ABI (only the full-width encoder, 1)")
     if config.get("activation_fct") not in ("relu", "tanh"):
         raise ValueError(f"activation_fct: {config.get('activation_fct')!r} must be 'relu' or 'tanh'")
+
+
+def model_flags_from_config(config):
+    """The header's model_flags of a configuration: DELORA_MODEL_NORMALIZATION_SCALING for normalization_scaling."""
+    return _lib.MODEL_NORMALIZATION_SCALING if config.get("normalization_scaling", False) else 0
 
 
 def desc_from_config(config, dataset, n_stride, max_batch=1, preprocessing_normals=False):
@@ -128,10 +135,10 @@ def unpack_blob(blob, config):
     return state
 
 
-def _pack_header(magic, header_bytes, desc, blob_floats):
+def _pack_header(magic, header_bytes, desc, blob_floats, model_flags):
     return _HEADER.pack(magic, _lib.ABI_VERSION, header_bytes, desc.H, desc.W, desc.hfov0, desc.hfov1, desc.vfov0,
                         desc.vfov1, desc.n_stride, desc.max_batch, desc.act, *list(desc.layers), desc.resnet_outputs,
-                        desc.single_mlp, desc.w_pre, blob_floats)
+                        desc.single_mlp, desc.w_pre, blob_floats, int(model_flags))
 
 
 def _unpack_header(raw, path, magic, what):
@@ -142,7 +149,8 @@ def _unpack_header(raw, path, magic, what):
     if v[0] != magic:
         raise ValueError(f"{path}: not an odometry {what} file (magic {v[0]!r})")
     names = ("magic", "abi_version", "header_bytes", "H", "W", "hfov0", "hfov1", "vfov0", "vfov1", "n_stride",
-             "max_batch", "act", "l0", "l1", "l2", "l3", "resnet_outputs", "single_mlp", "w_pre", "blob_floats")
+             "max_batch", "act", "l0", "l1", "l2", "l3", "resnet_outputs", "single_mlp", "w_pre", "blob_floats",
+             "model_flags")
     h = dict(zip(names, v))
     h["layers"] = [h.pop("l0"), h.pop("l1"), h.pop("l2"), h.pop("l3")]
     d = _lib.OdometryDesc()
@@ -153,15 +161,16 @@ def _unpack_header(raw, path, magic, what):
     return h, d
 
 
-def write_dlw(path, desc, blob):
+def write_dlw(path, desc, blob, model_flags=0):
+    """model_flags: DELORA_MODEL_* bits (model_flags_from_config)."""
     blob = np.ascontiguousarray(blob, dtype=np.float32)
     with open(path, "wb") as f:
-        f.write(_pack_header(MAGIC, HEADER_BYTES, desc, blob.size))
+        f.write(_pack_header(MAGIC, HEADER_BYTES, desc, blob.size, model_flags))
         f.write(blob.tobytes())
 
 
 def read_dlw(path):
-    """-> (header dict, desc, blob float32 array)."""
+    """-> (header dict, desc, blob float32 array); the header dict has `model_flags`."""
     with open(path, "rb") as f:
         h, d = _unpack_header(f.read(HEADER_BYTES), path, MAGIC, "weight")
         blob = np.fromfile(f, dtype=np.float32)
@@ -196,14 +205,14 @@ class TrainingState:
     loss: float = 0.0
 
 
-def write_dlt(path, desc, state):
+def write_dlt(path, desc, state, model_flags=0):
     arrays = [np.ascontiguousarray(a, dtype=np.float32).reshape(-1)
               for a in (state.weights, state.exp_avg, state.exp_avg_sq)]
     n = arrays[0].size
     if any(a.size != n for a in arrays):
         raise ValueError(f"weights, exp_avg and exp_avg_sq must have the same length ({[a.size for a in arrays]})")
     with open(path, "wb") as f:
-        f.write(_pack_header(TRAIN_MAGIC, TRAIN_HEADER_BYTES, desc, n))
+        f.write(_pack_header(TRAIN_MAGIC, TRAIN_HEADER_BYTES, desc, n, model_flags))
         f.write(_TRAIN_TAIL.pack(int(state.step), int(state.epoch), int(state.unsupervised), state.lr, state.beta1,
                                  state.beta2, state.eps, state.loss))
         for a in arrays:
@@ -324,9 +333,10 @@ def initial_training_state(config, seed):
                          float(config.get("learning_rate", 1e-5)))
 
 
-def config_from_desc(desc, base=None, dataset="kitti"):
+def config_from_desc(desc, base=None, dataset="kitti", model_flags=None):
     """`base` (e.g. the YAML configuration) with the network and range-image keys set from a .dlw / .dlt descriptor,
-    so that the configuration describes the weights of the file."""
+    so that the configuration describes the weights of the file.  model_flags (the header's, or None to keep `base`'s
+    value): sets normalization_scaling."""
     cfg = dict(base or {})
     ds = dict(cfg.get(dataset, {}))
     ds.update({"vertical_cells": int(desc.H), "horizontal_cells": int(desc.W),
@@ -338,6 +348,8 @@ def config_from_desc(desc, base=None, dataset="kitti"):
                 "activation_fct": "relu" if desc.act == 1 else "tanh", "layers": [int(v) for v in desc.layers],
                 "resnet_outputs": int(desc.resnet_outputs), "use_single_mlp_at_output": bool(desc.single_mlp),
                 "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1})
+    if model_flags is not None:
+        cfg["normalization_scaling"] = bool(int(model_flags) & _lib.MODEL_NORMALIZATION_SCALING)
     cfg.setdefault("use_dropout", False)
     cfg.setdefault("datasets", [dataset])
     return cfg
@@ -358,8 +370,9 @@ def export(checkpoint_path, dataset, out_path, n_stride, max_batch=1, config_dir
             ckpt = {"model_state_dict": ckpt}
         state = training_state_from_checkpoint(ckpt, config) if training_state else None
     desc = desc_from_config(config, dataset, n_stride, max_batch, preprocessing_normals)
+    flags = model_flags_from_config(config)
     if training_state:
-        write_dlt(out_path, desc, state)
+        write_dlt(out_path, desc, state, flags)
     else:
-        write_dlw(out_path, desc, state.weights if state else pack_state_dict(ckpt["model_state_dict"], config))
+        write_dlw(out_path, desc, state.weights if state else pack_state_dict(ckpt["model_state_dict"], config), flags)
     return desc

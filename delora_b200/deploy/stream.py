@@ -8,7 +8,14 @@ runs the encoder through cuDNN and synchronises with the host three times.  Here
 quaternion -> T kernel, captured once in a CUDA graph (25 launches replayed as one) between a pinned-memory
 H2D of the raw scan and a 64-byte D2H of the relative transform.  BASELINE config #5.
 
-OdometryStreams serves several streams of one sensor geometry and model from one C-ABI workspace, batched.
+A model trained with normalization_scaling (the ROS node's normalisation, odometry_publisher.py:102-111, :155, :176;
+the factor here is the Deployer's, `ops.normalization_factors`) cannot reuse the previous frame's image: it depends on
+the factor of the pair.  Such a stream keeps the previous SCAN on the device instead and per frame computes the factor,
+divides both scans by it, projects both, runs the model and multiplies the translation back by the factor, again in
+one captured graph.
+
+OdometryStreams serves several streams of one sensor geometry and model from one C-ABI workspace, batched; it refuses
+normalised models.
 """
 import numpy as np
 import torch
@@ -34,8 +41,16 @@ class OdometryStream:
         self.host_count = torch.zeros((1,), dtype=torch.int32).pin_memory()
         self.host_T = torch.zeros((1, 4, 4), dtype=torch.float32).pin_memory()
         self._host_scan_np, self._host_count_np = self.host_scan.numpy(), self.host_count.numpy()
-        self.points = torch.zeros((1, 3, self.n_max), dtype=torch.float32, device=self.device)
-        self.count = torch.zeros((1,), dtype=torch.int32, device=self.device)
+        self.normalized = bool(config.get("normalization_scaling", False))
+        if self.normalized:
+            # rows: the previous scan, this scan; a frame's upload goes to row 1, and row 1 moves to row 0 after it
+            self.pair_points = torch.zeros((2, 3, self.n_max), dtype=torch.float32, device=self.device)
+            self.pair_counts = torch.zeros((2,), dtype=torch.int32, device=self.device)
+            self.points, self.count = self.pair_points[1:], self.pair_counts[1:]
+            self.factor = torch.zeros((1,), dtype=torch.float32, device=self.device)
+        else:
+            self.points = torch.zeros((1, 3, self.n_max), dtype=torch.float32, device=self.device)
+            self.count = torch.zeros((1,), dtype=torch.int32, device=self.device)
         self.prev_image = torch.zeros((1, 4, self.h, self.w), dtype=torch.float32, device=self.device)
         self.T = torch.zeros((1, 4, 4), dtype=torch.float32, device=self.device)
         self.frames = 0
@@ -47,6 +62,8 @@ class OdometryStream:
 
     # everything of a frame that runs on the device; static shapes and buffers (graph-capturable)
     def _frame(self):
+        if self.normalized:
+            return self._frame_normalized()
         image, _ = ops.project(self.points, self.count, self.h, self.w, self.hf, self.vf)     # closest point per pixel
         with torch.no_grad():
             translation, quaternion = self.model(image_1=self.prev_image, image_2=image)
@@ -55,7 +72,28 @@ class OdometryStream:
         self.T.copy_(t)
         self.prev_image.copy_(image)
 
+    def _frame_normalized(self):
+        factor = ops.normalization_factors(self.pair_points, self.pair_counts)                # [1]
+        scaled = self.pair_points / factor.view(1, 1, 1)
+        image, _ = ops.project(scaled, self.pair_counts, self.h, self.w, self.hf, self.vf)
+        self.pair_image = image                  # [previous, this] as the model saw them (the graph's output under replay)
+        with torch.no_grad():
+            translation, quaternion = self.model(image_1=image[0:1], image_2=image[1:2])
+            t = model_parts.GeometryHandler.get_transformation_matrix_quaternion(
+                translation=translation, quaternion=quaternion, device=self.device)
+        t[:, :3, 3] *= factor.view(1, 1)
+        self.T.copy_(t)
+        self.factor.copy_(factor)
+        self._advance()
+
+    def _advance(self):
+        """Normalised route: this scan becomes the previous one."""
+        self.pair_points[0].copy_(self.pair_points[1])
+        self.pair_counts[0].copy_(self.pair_counts[1])
+
     def _capture(self):
+        if self.normalized:
+            return self._capture_normalized()
         side = torch.cuda.Stream(device=self.device)
         saved = self.prev_image.clone()          # taken BEFORE the side stream is released: the warm-up frames write prev_image
         side.wait_stream(torch.cuda.current_stream())
@@ -68,6 +106,22 @@ class OdometryStream:
         with torch.cuda.graph(self.graph):
             self._frame()
         self.prev_image.copy_(saved)
+
+    def _capture_normalized(self):
+        # the warm-up frames overwrite the previous scan with this one: restore it before the first replay
+        saved = (self.pair_points[0].clone(), self.pair_counts[0].clone())
+        side = torch.cuda.Stream(device=self.device)
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            for _ in range(3):
+                self._frame()
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+        self.graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.graph):
+            self._frame()
+        self.pair_points[0].copy_(saved[0])
+        self.pair_counts[0].copy_(saved[1])
 
     def push(self, scan):
         """scan: [3,N] or [1,3,N] float32 host tensor (N <= n_max).  Returns the relative transform
@@ -84,9 +138,12 @@ class OdometryStream:
         self.count.copy_(self.host_count, non_blocking=True)
         first = self.frames == 0
         if first:
-            # no previous frame yet: project only
-            image, _ = ops.project(self.points, self.count, self.h, self.w, self.hf, self.vf)
-            self.prev_image.copy_(image)
+            # no previous frame yet: project only (normalised route: keep the scan)
+            if self.normalized:
+                self._advance()
+            else:
+                image, _ = ops.project(self.points, self.count, self.h, self.w, self.hf, self.vf)
+                self.prev_image.copy_(image)
             torch.cuda.current_stream().synchronize()
             self.frames += 1
             return None
@@ -126,6 +183,10 @@ class OdometryStreams:
 
     def __init__(self, model, config, dataset, n_streams, n_max, use_cuda_graph=True):
         from . import capi, export
+        if config.get("normalization_scaling", False):
+            raise ValueError("normalization_scaling: True is not supported by OdometryStreams (its workspace caches "
+                             "each stream's projected image, which a normalised model cannot reuse); run one "
+                             "OdometryStream per sensor")
         self.config = config
         self.dataset = dataset
         self.device = torch.device(config["device"])

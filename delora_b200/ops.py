@@ -36,6 +36,7 @@ class nvtx_range:
 LOSS_PO2PO, LOSS_PO2PL, LOSS_PL2PL, NORMAL_LINEAR = 1, 2, 4, 8
 ICP_STATS = 256      # DELORA_ICP_STATS flag bit
 LOSS_IDENTITY_FIT = 512      # delora_odometry_train_step's identity pre-training objective
+TRAIN_NORMALIZATION_SCALING = 1024   # delora_odometry_train_step: the model uses normalization_scaling (needs w_pre > 0)
 LOSS_ROW, ICP_PARTIAL = 8, 40
 
 _keys_cache = {}
@@ -85,6 +86,21 @@ def project(points, n_points, h, w, hfov, vfov, div_mode=0):
                                     int(div_mode), keys.data_ptr(), image.data_ptr(), index_map.data_ptr(),
                                     _stream()), "delora_project_fwd")
     return image, index_map
+
+
+def normalization_factors(points, n_points):
+    """Deployer.normalize_input's factor of B pairs (src/deploy/deployer.py:222-235), deterministic: points [2B,3,N]
+    fp32 (scan_1 x B, then scan_2 x B), n_points [2B] int32 -> factor [B], the fp32 mean of the two scans' mean
+    ranges (each mean summed in float64 in a fixed order)."""
+    rows, _, n = points.shape
+    if rows % 2:
+        raise ValueError(f"points has {rows} rows: a batch of pairs has an even number of scans")
+    b = rows // 2
+    factor = torch.empty((b,), dtype=torch.float32, device=points.device)
+    _lib.check(_lib.lib().delora_normalization_factors(_req(points, torch.float32, "points"),
+                                                       _req(n_points, torch.int32, "n_points"), b, n,
+                                                       factor.data_ptr(), _stream()), "delora_normalization_factors")
+    return factor
 
 
 def project_normals(points, n_points, h, w, hfov, vfov, neighborhood=(7, 11), epsilon_range=0.5, min_neighbors=10,

@@ -73,6 +73,10 @@ int main(int argc, char** argv) {
     if (fread(&hdr, sizeof hdr, 1, f) != 1) return fail("truncated header");
     if (memcmp(hdr.magic, DELORA_ODOMETRY_FILE_MAGIC, 8) != 0) return fail("not a .dlw file");
     if (hdr.abi_version != delora_abi_version()) return fail("weight file and library ABI versions differ");
+    const int normalized = (hdr.model_flags & DELORA_MODEL_NORMALIZATION_SCALING) != 0;
+    if (normalized && hdr.desc.w_pre == 0)
+        return fail("the model was trained with normalization_scaling, which trains on the reference's recipe only: "
+                    "export it with preprocessing normals (w_pre > 0)");
     const delora_odometry_desc* d = &hdr.desc;
     const int64_t n_weights = delora_odometry_weight_floats(d);
     if (n_weights < 0) return fail(delora_last_error());
@@ -102,7 +106,7 @@ int main(int argc, char** argv) {
     delora_odometry_train_params hp;
     hp.lr = lr; hp.beta1 = 0.9f; hp.beta2 = 0.999f; hp.eps = 1e-8f;
     hp.lambda_po2pl = 1.0f;
-    hp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL;
+    hp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | (normalized ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u);
     hp.nb_h = 7; hp.nb_w = 11;
     hp.epsilon_range = 0.5f;
     hp.min_neighbors = 10;

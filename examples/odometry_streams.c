@@ -103,6 +103,9 @@ int main(int argc, char** argv) {
     if (fread(&hdr, sizeof hdr, 1, f) != 1) return fail("truncated header");
     if (memcmp(hdr.magic, DELORA_ODOMETRY_FILE_MAGIC, 8) != 0) return fail("not a .dlw file");
     if (hdr.abi_version != delora_abi_version()) return fail("weight file and library ABI versions differ");
+    if (hdr.model_flags & DELORA_MODEL_NORMALIZATION_SCALING)
+        return fail("the model was trained with normalization_scaling: a streams workspace caches projected images, "
+                    "which such a model cannot reuse (run odometry_stream per sensor)");
     delora_odometry_desc desc = hdr.desc;
     desc.max_batch = S;
     const delora_odometry_desc* d = &desc;

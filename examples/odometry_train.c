@@ -107,6 +107,10 @@ int main(int argc, char** argv) {
     const int is_dlt = memcmp(hdr.base.magic, DELORA_TRAINING_FILE_MAGIC, 8) == 0;
     if (!is_dlt && memcmp(hdr.base.magic, DELORA_ODOMETRY_FILE_MAGIC, 8) != 0) return fail("not a .dlw or .dlt file");
     if (hdr.base.abi_version != delora_abi_version()) return fail("input file and library ABI versions differ");
+    const int normalized = (hdr.base.model_flags & DELORA_MODEL_NORMALIZATION_SCALING) != 0;
+    if (normalized && hdr.base.desc.w_pre == 0)
+        return fail("the model was trained with normalization_scaling, which trains on the reference's recipe only: "
+                    "export it with preprocessing normals (w_pre > 0)");
     if (is_dlt && fread((char*)&hdr + sizeof hdr.base, sizeof hdr - sizeof hdr.base, 1, f) != 1)
         return fail("truncated header");
     const delora_odometry_desc* d = &hdr.base.desc;
@@ -177,7 +181,8 @@ int main(int argc, char** argv) {
     int32_t* h_step_counts = (int32_t*)malloc((size_t)2 * B_max * sizeof(int32_t));
     if (!h_losses || !h_step_counts) return fail("out of host memory");
     for (int e = 0; e < epochs; ++e) {
-        hp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | (hdr.unsupervised ? 0u : DELORA_LOSS_IDENTITY_FIT);
+        hp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | (hdr.unsupervised ? 0u : DELORA_LOSS_IDENTITY_FIT) |
+                        (normalized ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u);
         double sum = 0.0;
         int steps = 0;
         for (int k0 = 0; k0 < n_pairs; k0 += B_max, ++steps) {

@@ -42,6 +42,8 @@ typedef struct { float x, y, z, w; } delora_f4;
 #define DELORA_ICP_STATS       256u  /* diagnostic: count the work of the NN search (delora_icp_stats) */
 #define DELORA_LOSS_IDENTITY_FIT 512u /* delora_odometry_train_step only: the identity pre-training objective
                                          (unsupervised_at_start: False, src/deploy/deployer.py:324-327) */
+#define DELORA_TRAIN_NORMALIZATION_SCALING 1024u /* delora_odometry_train_step only: the model is trained with
+                                                    normalization_scaling (see _train_step; needs w_pre > 0) */
 
 /* number of floats in one row of the `losses` output of delora_icp_fwd_bwd */
 #define DELORA_LOSS_ROW 8   /* [po2po, po2pl, pl2pl, M_pairs, M_po2po, 0, 0, 0] */
@@ -391,6 +393,8 @@ int delora_quat_to_T_bwd(const float* quaternion, const float* grad_T, int B,
  * (odometry_out_kernel), with a fixed summation order.  Not representable: pre_feature_extraction,
  * factor_fewer_resnet_channels != 1; dropout is the identity at inference.
  *
+ * Models trained with normalization_scaling run through delora_odometry_pairs_normalized (below), not _pairs / _push.
+ *
  * Workspace: one caller-owned device buffer of delora_odometry_workspace_bytes(d) bytes holds every activation,
  * the bf16 filters, the fp32 tail weights and the stream's cached range image.  Its layout is a function of the
  * descriptor only.  Use: _init once, _load_weights, then any number of _pairs / _push calls.  One workspace serves
@@ -416,18 +420,23 @@ typedef struct {
 /* Weight file (.dlw, written by delora_b200/deploy/export.py), little-endian, readable with fread alone:
  *   bytes   0..127  delora_odometry_file_header below (explicit offsets: magic 0, abi_version 8, header_bytes 12,
  *                   desc 16: H 16, W 20, hfov0 24, hfov1 32, vfov0 40, vfov1 48, n_stride 56, max_batch 60, act 64,
- *                   layers 68..83, resnet_outputs 84, single_mlp 88, w_pre 92; blob_floats 96; zero 104..127;
- *                   exporters before w_pre wrote zeros at 92, i.e. w_pre = 0)
+ *                   layers 68..83, resnet_outputs 84, single_mlp 88, w_pre 92; blob_floats 96; model_flags 104;
+ *                   zero 108..127; exporters before w_pre wrote zeros at 92, i.e. w_pre = 0, and exporters before
+ *                   model_flags wrote zeros at 104, i.e. no flag)
  *   bytes 128..     float32[blob_floats]: the tensors of OdometryModel.state_dict() concatenated in state_dict order,
  *                   each tensor row-major (the blob delora_odometry_load_weights takes). */
 #define DELORA_ODOMETRY_FILE_MAGIC "DELORAW"     /* 7 characters + NUL = the 8 magic bytes */
+/* model_flags bits: how the model expects its input, beyond the descriptor */
+#define DELORA_MODEL_NORMALIZATION_SCALING 1u    /* trained with normalization_scaling: run it through
+                                                    delora_odometry_pairs_normalized */
 typedef struct {
     char magic[8];
     int32_t abi_version;                 /* DELORA_B200_ABI_VERSION of the exporter */
     int32_t header_bytes;                /* 128 */
     delora_odometry_desc desc;
     int64_t blob_floats;                 /* == delora_odometry_weight_floats(&desc) */
-    uint8_t reserved[24];
+    uint32_t model_flags;                /* DELORA_MODEL_* bits (byte 104) */
+    uint8_t reserved[20];
 } delora_odometry_file_header;
 
 /* Host only (no GPU needed): validate the descriptor (non-zero + delora_last_error() if it is invalid; the size
@@ -450,6 +459,41 @@ int delora_odometry_load_weights(const delora_odometry_desc* d, const float* wei
  * Only launches: no allocation, no synchronisation, no host decision on device data. */
 int delora_odometry_pairs(const delora_odometry_desc* d, const float* points, const int32_t* n_points, int B,
                           void* workspace, float* T, float* pooled, void* stream);
+
+/* Models trained with normalization_scaling (config/hyperparameters.yaml:23; the file's model_flags has
+ * DELORA_MODEL_NORMALIZATION_SCALING).  Such a model saw each pair divided by a factor and predicts its translation in
+ * those units: Deployer.normalize_input (src/deploy/deployer.py:222-235) and the rescale at :344-346 / :371-373.
+ *
+ * delora_normalization_factors: the factor of B pairs, the operator that replaces normalize_input's mean.
+ *   points [2B, 3, n_stride] fp32 (scan_1 of pair 0..B-1, then scan_2 of pair 0..B-1), n_points [2B] int32 (device,
+ *   clamped to [0, n_stride] on the device) -> factor [B] fp32 out (device).  Per scan, m = the mean of its points'
+ *   ranges: each range is sqrt((x*x + y*y) + z*z) of the fp32 coordinates, correctly rounded (the projection's range
+ *   channel), the ranges are summed in float64 in a fixed order that depends on neither B nor the launch, divided by
+ *   the count and rounded to fp32.  factor = (m_1 + m_2) / 2 in fp32.  Bit-identical from run to run; within a few
+ *   ulp of torch's mean, whose CUDA reduction order is not reproducible.  A scan without points is outside the
+ *   contract: its mean is NaN (0 / 0), as torch.mean of an empty tensor in the reference.  The reference's ROS node
+ *   (src/ros_utils/odometry_publisher.py:102-111) pools the ranges of both scans into one mean instead; that variant
+ *   is not provided.  Refused before any launch, naming the argument: null points / n_points / factor, B outside
+ *   [1, 65535], n_stride < 1.
+ *
+ * delora_odometry_pairs_normalized: delora_odometry_pairs with the factor applied, as the Tester runs such a model.
+ *   Both scans of pair b are divided by factor[b] (x / f correctly rounded, before any other use), projected and run
+ *   through the model; then T[:3, 3] of row b is multiplied by factor[b] in fp32.  The images and pooled features are
+ *   bit-identical to delora_odometry_pairs on a copy of the points divided by the factor.  Same workspace and arguments
+ *   as delora_odometry_pairs, plus factor [B] fp32, a required caller-owned device output that also carries the factor
+ *   between the kernels.  Only launches, so one call can be captured into a CUDA graph.  Refused before any launch,
+ *   naming the argument: an invalid descriptor, null points / n_points / workspace / T / factor, B outside
+ *   [1, max_batch].
+ *
+ * Streaming a normalised model: the _push and _streams_* workspaces cache the previous frame's projected image, which
+ * depends on the factor of the NEXT pair, so they cannot serve normalised models.  Stream one through
+ * delora_odometry_pairs_normalized with B = 1 on (previous scan, this scan), as the reference's ROS node does
+ * (examples/odometry_stream.c does so for flagged files).  Train one with DELORA_TRAIN_NORMALIZATION_SCALING in
+ * delora_odometry_train_params.loss_flags (see delora_odometry_train_step). */
+int delora_normalization_factors(const float* points, const int32_t* n_points, int B, int n_stride, float* factor,
+                                 void* stream);
+int delora_odometry_pairs_normalized(const delora_odometry_desc* d, const float* points, const int32_t* n_points, int B,
+                                     void* workspace, float* T, float* pooled, float* factor, void* stream);
 /* Streaming, batch 1: project the frame points [1, 3, n_stride] (n_points [1], device), run the model on (cached
  * previous image, this image), write T [16], then cache this image.  T == NULL: only project and cache (the first
  * frame of a stream).  Bit-identical to delora_odometry_pairs with B = 1 on (previous scan, this scan).  With T
@@ -517,7 +561,8 @@ typedef struct {
     float lr, beta1, beta2, eps;         /* Adam (torch defaults 0.9, 0.999, 1e-8); lr >= 0, betas in [0, 1), eps > 0 */
     float lambda_po2pl;                  /* config lambda_po2pl */
     uint32_t loss_flags;                 /* DELORA_LOSS_* / DELORA_NORMAL_LINEAR bits, at least one ICP loss bit
-                                            (PO2PO, PO2PL, PL2PL), plus DELORA_LOSS_IDENTITY_FIT (see _train_step) */
+                                            (PO2PO, PO2PL, PL2PL), plus DELORA_LOSS_IDENTITY_FIT and
+                                            DELORA_TRAIN_NORMALIZATION_SCALING (see _train_step) */
     int nb_h, nb_w;                      /* neighborhood_side_length (7, 11): odd and positive */
     float epsilon_range;                 /* 0.5 */
     int min_neighbors;                   /* min_num_points_in_neighborhood_to_determine_point_class, 10 */
@@ -542,7 +587,16 @@ int delora_odometry_train_init(const delora_odometry_desc* d, const float* weigh
  * the ICP objective's (the norm of the whole [B, 4] quaternion block still gives every pair's head outputs a
  * gradient).  The ICP losses are still computed and written to `losses` (the reference logs them in this phase); the
  * identity objective goes to losses[B-1][5] (column 5 is 0 in the other rows and in steps without the bit).  At least
- * one ICP loss bit is still required. */
+ * one ICP loss bit is still required.
+ * Normalised models: with DELORA_TRAIN_NORMALIZATION_SCALING in hp->loss_flags the step trains a model that uses
+ * normalization_scaling as the reference's Deployer.step does (src/deploy/deployer.py:222-235, :252-261, :344-346).  It
+ * needs the reference's recipe, d->w_pre > 0 (refused before any launch otherwise, the message names w_pre): the normals
+ * come from the unscaled points at H x w_pre; the factor of each pair is the mean of its two scans' mean ranges over
+ * the valid H x w_pre cells (the points the preprocessing stored; the definition of delora_normalization_factors, the
+ * same float64 order), and those points are divided by it (correctly rounded) before the H x W projection.  The ICP
+ * losses are in normalised units, as in the reference; the identity fit uses the unscaled T; the T output is rescaled
+ * (T[:3, 3] *= factor in fp32); losses[b][6] is the factor (0 in steps without the bit).  No workspace size changes:
+ * the factor is kept in the H x w_pre image, which nothing reads after the preprocessing projection. */
 int delora_odometry_train_step(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
                                const float* points, const int32_t* n_points, int B, void* workspace,
                                float* losses, float* T, float* pooled, float* grads, void* stream);
