@@ -3,7 +3,7 @@
 --training-state) back into the reference Trainer's checkpoint (.pth: `epoch`, `model_state_dict`,
 `optimizer_state_dict`, `loss`, `parameters`), loadable by its `--checkpoint` option and by torch.optim.Adam.
 `parameters` is the YAML configuration of `--config_dir` (when it exists) with the network and range-image keys of
-the file's header, and `normalization_scaling` from its model_flags."""
+the file's header, and `normalization_scaling` and `use_dropout` from its model_flags."""
 import os
 import sys
 

@@ -117,11 +117,14 @@ SIGNATURES = {
     "delora_odometry_train_weights": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_train_get_state": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_train_set_state": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_train_set_dropout_seed": (c_int, [c_desc_p, ctypes.c_uint64, c_void_p, c_void_p]),
+    "delora_dropout_keep_mask": (c_int, [ctypes.c_uint64, c_i64, c_int, c_i64, c_void_p, c_void_p]),
 }
 
 ABI_VERSION = 3
 # model_flags bits of the .dlw / .dlt header (DELORA_MODEL_* in include/delora_b200.h)
 MODEL_NORMALIZATION_SCALING = 1
+MODEL_DROPOUT = 2
 _lib = None
 
 

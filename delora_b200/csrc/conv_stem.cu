@@ -19,6 +19,7 @@
 #include <string.h>
 #include <cuda_fp16.h>
 #include "conv_internal.cuh"
+#include "dropout.cuh"
 
 namespace delora {
 
@@ -139,9 +140,12 @@ stem_fprop_tc_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_con
 
 // two [B,4,H,W] fp32 range images -> [B, H+2, W+2, 16] bf16: channels 0..7 = bf16(cat(image_1, image_2))
 // (src/models/model.py:98), 8..15 = bf16 of the rounding residual; circular halo columns, zero halo rows.
-__global__ void __launch_bounds__(256)
-images_to_nhwc16_kernel(const float* __restrict__ img1, const float* __restrict__ img2, int B, int H, int W,
-                        __nv_bfloat16* __restrict__ x) {
+// kDrop (the training step's input dropout): element (b, c, h, w) is first multiplied by keep * 1.25f in fp32, so the
+// split sees the bits of images that were multiplied beforehand.
+template <bool kDrop>
+__device__ __forceinline__ void images_to_nhwc16_body(const float* __restrict__ img1, const float* __restrict__ img2,
+                                                      int B, int H, int W, __nv_bfloat16* __restrict__ x,
+                                                      const DropoutCtr& drop) {
     const int Wp = W + 2, Hp = H + 2;
     const size_t total = (size_t)B * Hp * Wp;
     const size_t i = (size_t)blockIdx.x * 256 + threadIdx.x;
@@ -157,6 +161,14 @@ images_to_nhwc16_kernel(const float* __restrict__ img1, const float* __restrict_
         float f[8];
 #pragma unroll
         for (int c = 0; c < 4; ++c) { f[c] = __ldg(img1 + base + c * plane); f[4 + c] = __ldg(img2 + base + c * plane); }
+        if (kDrop) {
+            uint64_t seed, step;
+            dropout_seed_step(drop, seed, step);
+            const size_t e0 = ((size_t)b * 8 * H + h) * W + w;         // element (b, 0, h, w); channel c adds c * plane
+#pragma unroll
+            for (int c = 0; c < 8; ++c)
+                f[c] = dropout_keep(seed, step, kDropInput, e0 + c * plane) ? f[c] * kDropScale : 0.0f;
+        }
         __nv_bfloat16 hv[8], lv[8];
 #pragma unroll
         for (int c = 0; c < 8; ++c) {
@@ -169,6 +181,18 @@ images_to_nhwc16_kernel(const float* __restrict__ img1, const float* __restrict_
     uint4* dst = reinterpret_cast<uint4*>(x + i * 16);
     dst[0] = lo;
     dst[1] = hi_part;
+}
+
+__global__ void __launch_bounds__(256)
+images_to_nhwc16_kernel(const float* __restrict__ img1, const float* __restrict__ img2, int B, int H, int W,
+                        __nv_bfloat16* __restrict__ x) {
+    images_to_nhwc16_body<false>(img1, img2, B, H, W, x, DropoutCtr{nullptr, 0});
+}
+
+__global__ void __launch_bounds__(256)
+images_to_nhwc16_dropout_kernel(const float* __restrict__ img1, const float* __restrict__ img2, int B, int H, int W,
+                                __nv_bfloat16* __restrict__ x, DropoutCtr drop) {
+    images_to_nhwc16_body<true>(img1, img2, B, H, W, x, drop);
 }
 
 // fp32 stem filter [64, 8, 3, 3] -> bf16 [3 rows][64 co][64 k], k = q * 16 + c (q < 3, c < 8), zero elsewhere
@@ -269,6 +293,15 @@ extern "C" int delora_images_to_nhwc16_bf16(const float* image_1, const float* i
     images_to_nhwc16_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(image_1, image_2, B, H, W,
                                                                                                (__nv_bfloat16*)x16);
     DELORA_CHECK_LAUNCH("images_to_nhwc16_kernel");
+    return 0;
+}
+
+int delora::launch_images_to_nhwc16_dropout(const float* img1, const float* img2, int B, int H, int W, void* x16,
+                                            DropoutCtr drop, cudaStream_t st) {
+    const size_t total = (size_t)B * (H + 2) * (W + 2);
+    images_to_nhwc16_dropout_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(img1, img2, B, H, W,
+                                                                                   (__nv_bfloat16*)x16, drop);
+    DELORA_CHECK_LAUNCH("images_to_nhwc16_dropout_kernel");
     return 0;
 }
 

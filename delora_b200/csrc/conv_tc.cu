@@ -22,6 +22,7 @@
 #include <stdlib.h>
 #include <cuda_fp16.h>
 #include "conv_internal.cuh"
+#include "dropout.cuh"
 
 namespace delora {
 
@@ -287,9 +288,11 @@ wgrad_reduce_kernel(const float* __restrict__ partial, int splits, int taps, int
 // ---------------------------------------------------------------- layout helpers (bandwidth kernels)
 // two [B,4,H,W] fp32 range images -> [B, H+2, W+2, Cpad] bf16, channels 0..7 = cat(image_1, image_2)
 // (src/models/model.py:98), the rest zero; circular halo columns, zero halo rows.
-__global__ void __launch_bounds__(256)
-images_to_nhwc_kernel(const float* __restrict__ img1, const float* __restrict__ img2, int B, int H, int W, int Cpad,
-                      __nv_bfloat16* __restrict__ x) {
+// kDrop (the training step's input dropout): element (b, c, h, w) is first multiplied by keep * 1.25f in fp32.
+template <bool kDrop>
+__device__ __forceinline__ void images_to_nhwc_body(const float* __restrict__ img1, const float* __restrict__ img2,
+                                                    int B, int H, int W, int Cpad, __nv_bfloat16* __restrict__ x,
+                                                    const DropoutCtr& drop) {
     // one thread per (padded pixel, group of 8 channels): 16-byte stores, a pixel's Cpad channels are
     // written by Cpad/8 adjacent threads (coalesced); only group 0 carries data (8 real channels)
     const int Wp = W + 2, Hp = H + 2, groups = Cpad / 8;
@@ -306,15 +309,35 @@ images_to_nhwc_kernel(const float* __restrict__ img1, const float* __restrict__ 
         if (w >= W) w = 0;
         const int h = hp - 1;
         __nv_bfloat162 v[4];
+        uint64_t seed = 0, step = 0;
+        if (kDrop) dropout_seed_step(drop, seed, step);
+        const size_t plane = (size_t)H * W, e0 = ((size_t)b * 8 * H + h) * W + w;     // element (b, 0, h, w)
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
             const float* src = (c < 2) ? img1 : img2;
             const size_t base = (((size_t)b * 4 + (2 * c & 3)) * H + h) * W + w;
-            v[c] = __floats2bfloat162_rn(__ldg(src + base), __ldg(src + base + (size_t)H * W));
+            float lo = __ldg(src + base), hi = __ldg(src + base + plane);
+            if (kDrop) {                                                // concatenated channels 2c, 2c + 1
+                lo = dropout_keep(seed, step, kDropInput, e0 + (size_t)(2 * c) * plane) ? lo * kDropScale : 0.0f;
+                hi = dropout_keep(seed, step, kDropInput, e0 + (size_t)(2 * c + 1) * plane) ? hi * kDropScale : 0.0f;
+            }
+            v[c] = __floats2bfloat162_rn(lo, hi);
         }
         out = *reinterpret_cast<uint4*>(v);
     }
     *reinterpret_cast<uint4*>(x + pixel * Cpad + grp * 8) = out;
+}
+
+__global__ void __launch_bounds__(256)
+images_to_nhwc_kernel(const float* __restrict__ img1, const float* __restrict__ img2, int B, int H, int W, int Cpad,
+                      __nv_bfloat16* __restrict__ x) {
+    images_to_nhwc_body<false>(img1, img2, B, H, W, Cpad, x, DropoutCtr{nullptr, 0});
+}
+
+__global__ void __launch_bounds__(256)
+images_to_nhwc_dropout_kernel(const float* __restrict__ img1, const float* __restrict__ img2, int B, int H, int W,
+                              int Cpad, __nv_bfloat16* __restrict__ x, DropoutCtr drop) {
+    images_to_nhwc_body<true>(img1, img2, B, H, W, Cpad, x, drop);
 }
 
 // MaxPool2d(3, stride (1,2), padding (1,0)) after circular W padding (src/models/resnet_modified.py:46,:100-101),
@@ -785,6 +808,15 @@ extern "C" int delora_images_to_nhwc_bf16(const float* image_1, const float* ima
     images_to_nhwc_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
         image_1, image_2, B, H, W, Cpad, (__nv_bfloat16*)x);
     DELORA_CHECK_LAUNCH("images_to_nhwc_kernel");
+    return 0;
+}
+
+int delora::launch_images_to_nhwc_dropout(const float* img1, const float* img2, int B, int H, int W, int Cpad, void* x,
+                                          DropoutCtr drop, cudaStream_t st) {
+    const size_t total = (size_t)B * (H + 2) * (W + 2) * (Cpad / 8);
+    images_to_nhwc_dropout_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(img1, img2, B, H, W, Cpad,
+                                                                                 (__nv_bfloat16*)x, drop);
+    DELORA_CHECK_LAUNCH("images_to_nhwc_dropout_kernel");
     return 0;
 }
 

@@ -19,6 +19,7 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "dropout.cuh"
 #include "projection.cuh"
 
 namespace delora {
@@ -81,9 +82,11 @@ __device__ __forceinline__ void row_dot4(const float* __restrict__ w, const floa
 }
 
 // y = act(W x + b) for two independent problems in one launch (the hidden layers of the two heads share one):
-// warps [0, p0.N) compute p0's outputs, the next p1.N warps p1's.
-__global__ void __launch_bounds__(kTailWarps * 32)
-odometry_linear_kernel(TailLinear p0, TailLinear p1, int B, int act_out, int vec) {
+// warps [0, p0.N) compute p0's outputs, the next p1.N warps p1's.  kDrop (resnet.fc in a dropout training step, p1
+// empty): y = act(keep * 1.25f * (W x + b)), element b * N + n of the fc mask.
+template <bool kDrop>
+__device__ __forceinline__ void linear_body(const TailLinear& p0, const TailLinear& p1, int B, int act_out, int vec,
+                                            const DropoutCtr& drop) {
     const int lane = threadIdx.x & 31;
     int n = blockIdx.x * kTailWarps + (threadIdx.x >> 5);
     const bool second = n >= p0.N;
@@ -97,8 +100,26 @@ odometry_linear_kernel(TailLinear p0, TailLinear p1, int B, int act_out, int vec
         float acc[4];
         row_dot4(w, p.x + (size_t)b0 * p.ldx, p.ldx, p.K, nb, lane, vec, acc);
         const float v = lane == 0 ? acc[0] : lane == 1 ? acc[1] : lane == 2 ? acc[2] : acc[3];
-        if (lane < nb) p.y[(size_t)(b0 + lane) * p.ldy + n] = tail_act(v + bn, act_out);
+        if (lane < nb) {
+            float z = v + bn;
+            if (kDrop) {
+                uint64_t seed, step;
+                dropout_seed_step(drop, seed, step);
+                z = dropout_keep(seed, step, kDropFc, (uint64_t)(b0 + lane) * p.N + n) ? z * kDropScale : 0.0f;
+            }
+            p.y[(size_t)(b0 + lane) * p.ldy + n] = tail_act(z, act_out);
+        }
     }
+}
+
+__global__ void __launch_bounds__(kTailWarps * 32)
+odometry_linear_kernel(TailLinear p0, TailLinear p1, int B, int act_out, int vec) {
+    linear_body<false>(p0, p1, B, act_out, vec, DropoutCtr{nullptr, 0});
+}
+
+__global__ void __launch_bounds__(kTailWarps * 32)
+odometry_linear_dropout_kernel(TailLinear p0, TailLinear p1, int B, int act_out, int vec, DropoutCtr drop) {
+    linear_body<true>(p0, p1, B, act_out, vec, drop);
 }
 
 // The last layer of the heads (rot: 4 outputs, trans: 3) for every row b < B with want(b) (warp-uniform):
@@ -398,17 +419,65 @@ static void make_infer_plan(const delora_odometry_desc* d, bool streams, InferPl
     p->total = off;
 }
 
-// (img1, img2) fp32 [B, 4, H, W] each -> the trunk input
+// (img1, img2) fp32 [B, 4, H, W] each -> the trunk input; drop.ctr non-NULL: with the input dropout applied
 static int trunk_input(const Model& m, const Trunk& t, char* ws, const float* img1, const float* img2, int B,
-                       cudaStream_t st) {
+                       cudaStream_t st, DropoutCtr drop = DropoutCtr{nullptr, 0}) {
+    if (drop.ctr)
+        return m.stem_fast ? launch_images_to_nhwc16_dropout(img1, img2, B, m.H, m.W, ws + t.x_in, drop, st)
+                           : launch_images_to_nhwc_dropout(img1, img2, B, m.H, m.W, 64, ws + t.x_in, drop, st);
     return m.stem_fast ? delora_images_to_nhwc16_bf16(img1, img2, B, m.H, m.W, ws + t.x_in, st)
                        : delora_images_to_nhwc_bf16(img1, img2, B, m.H, m.W, 64, ws + t.x_in, st);
 }
 
+// The stage-3 channel dropout, Dropout2d on layer3's output: x, y [B, Hp, Wp, C] bf16, the padded NHWC layout with its
+// halos (pix = Hp * Wp per pair).  y = bf16_rn(float(x) * 1.25f) where (pair b, channel c) is kept (element b * C + c
+// of the stage-3 mask), 0 where it is dropped.  One thread per 8 channels (two Philox words); y may be x.  The forward
+// writes x3d from layer3's output with it; the backward multiplies the data gradient of layer3's output in place.
+__global__ void __launch_bounds__(256)
+odometry_channel_dropout_kernel(const __nv_bfloat16* x, __nv_bfloat16* y, int B, int pix, int C, DropoutCtr drop) {
+    const int groups = C / 8;
+    const size_t total = (size_t)B * pix * groups;
+    const size_t i = (size_t)blockIdx.x * 256 + threadIdx.x;
+    if (i >= total) return;
+    const int c0 = (int)(i % groups) * 8;
+    const int b = (int)(i / ((size_t)groups * pix));
+    uint64_t seed, step;
+    dropout_seed_step(drop, seed, step);
+    const uint64_t e0 = (uint64_t)b * C + c0;              // a multiple of 8: two whole Philox blocks
+    const Philox4 r0 = dropout_words(seed, step, kDropStage3, e0 >> 2);
+    const Philox4 r1 = dropout_words(seed, step, kDropStage3, (e0 >> 2) + 1);
+    const uint32_t words[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
+    uint4 v = reinterpret_cast<const uint4*>(x)[i];
+    __nv_bfloat16* h = reinterpret_cast<__nv_bfloat16*>(&v);
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+        h[k] = dropout_word_keeps(words[k]) ? __float2bfloat16_rn(__bfloat162float(h[k]) * kDropScale)
+                                            : __float2bfloat16_rn(0.0f);
+    reinterpret_cast<uint4*>(y)[i] = v;
+}
+
+static int channel_dropout(const Model& m, const char* x, char* y, int B, DropoutCtr drop, cudaStream_t st) {
+    const int C = m.stage_c[2], pix = (m.stage_h[2] + 2) * (m.stage_w[2] + 2);
+    const size_t total = (size_t)B * pix * (C / 8);
+    odometry_channel_dropout_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(
+        reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<__nv_bfloat16*>(y), B, pix, C, drop);
+    DELORA_CHECK_LAUNCH("odometry_channel_dropout_kernel");
+    return 0;
+}
+
+// The block whose output is layer3's (x3): the last block of stage 2
+static int last_stage3_block(const Model& m) {
+    int i = 0;
+    while (i + 1 < m.n_block && m.block[i + 1].stage <= 2) ++i;
+    return i;
+}
+
 // The trunk from its input to the pooled features.  saving (training): the stem keeps its PRE-activation (fp16 on the
 // 16-channel path) and the max-pool applies the activation and records its argmax; otherwise the stem applies it.
+// drop.ctr non-NULL (a dropout training step): layer3's output x3 stays as it is (the backward's act' reads it), the
+// channel-dropped x3d is written to x3d (a buffer of x3's size) and layer4's first block reads it.
 static int trunk_forward(const Model& m, const Trunk& t, const Weights& w, bool saving, char* ws, int act, int B,
-                         float* pooled, cudaStream_t st) {
+                         float* pooled, cudaStream_t st, DropoutCtr drop = DropoutCtr{nullptr, 0}, size_t x3d = 0) {
     int rc;
     const int H = m.H, W = m.W, stem_act = saving ? 0 : act;
     char* stem = ws + t.stem;
@@ -436,6 +505,10 @@ static int trunk_forward(const Model& m, const Trunk& t, const Weights& w, bool 
         if ((rc = delora_conv2d_fprop_bf16(t1, ws + w.w_fwd[b.c2], ident, nullptr, ws + t.out[i], B, b.hout, b.wout,
                                            b.cout, b.cout, 3, 1, 1, act, st))) return rc;
         cur = ws + t.out[i];
+        if (drop.ctr && i == last_stage3_block(m)) {
+            if ((rc = channel_dropout(m, cur, ws + x3d, B, drop, st))) return rc;
+            cur = ws + x3d;
+        }
     }
     return delora_avgpool_nhwc_bf16(cur, B, m.stage_h[3], m.stage_w[3], 512, pooled, st);
 }
@@ -480,8 +553,9 @@ static int tail_vec(const TailLinear& t) {
 }
 
 // resnet.fc and the heads' hidden layers for B rows; rot / trans: the heads' last layers, for the output kernel
+// drop.ctr non-NULL: resnet.fc's output goes through the fc dropout before the activation
 static int run_tail_hidden(const Model& m, const TailIO& io, int act, const float* pooled, int B, TailLinear* rot_out,
-                           TailLinear* trans_out, cudaStream_t st) {
+                           TailLinear* trans_out, cudaStream_t st, DropoutCtr drop = DropoutCtr{nullptr, 0}) {
     float* fc_out = io.fc_out;
     TailLinear none;
     memset(&none, 0, sizeof(none));
@@ -494,7 +568,14 @@ static int run_tail_hidden(const Model& m, const TailIO& io, int act, const floa
     };
     int rc;
     const int nout = m.fc.N;
-    if ((rc = linear(tail_args(m.fc, io.fc_w, io.fc_b, pooled, 512, fc_out, nout), none))) return rc;   // act(resnet.fc(x))
+    if (drop.ctr) {                                         // act(dropout(resnet.fc(x)))
+        const TailLinear fc = tail_args(m.fc, io.fc_w, io.fc_b, pooled, 512, fc_out, nout);
+        odometry_linear_dropout_kernel<<<(fc.N + kTailWarps - 1) / kTailWarps, kTailWarps * 32, 0, st>>>(
+            fc, none, B, act, tail_vec(fc), drop);
+        DELORA_CHECK_LAUNCH("odometry_linear_dropout_kernel");
+    } else if ((rc = linear(tail_args(m.fc, io.fc_w, io.fc_b, pooled, 512, fc_out, nout), none))) {   // act(resnet.fc(x))
+        return rc;
+    }
     TailLinear rot, trans;
     if (m.n_lin == 4) {
         // hidden layers of both heads in one launch: hid[0] = [act(rot1 h) | act(trans1 h)], row stride 200
@@ -529,9 +610,9 @@ static int run_tail_hidden(const Model& m, const TailIO& io, int act, const floa
 
 // factor [B] or NULL: multiply each row's translation by its pair's normalisation factor
 static int run_tail(const Model& m, const TailIO& io, int act, const float* pooled, int B, float* T, cudaStream_t st,
-                    const float* factor = nullptr) {
+                    const float* factor = nullptr, DropoutCtr drop = DropoutCtr{nullptr, 0}) {
     TailLinear rot, trans;
-    const int rc = run_tail_hidden(m, io, act, pooled, B, &rot, &trans, st);
+    const int rc = run_tail_hidden(m, io, act, pooled, B, &rot, &trans, st, drop);
     if (rc) return rc;
     const int vec = tail_vec(rot) && tail_vec(trans);
     const size_t smem = (size_t)B * 7 * sizeof(float);
@@ -908,6 +989,9 @@ extern "C" int delora_odometry_streams_reset(const delora_odometry_desc* d, cons
 //     caller's output, the factor to losses[b][6].
 //   odometry_icp_rearm_kernel: zeroes the ICP scratch when B differs from the batch size of the previous step (the
 //     scratch layout depends on B); otherwise every CTA exits at once.
+//   DELORA_TRAIN_DROPOUT (masks from dropout.cuh, regenerated in the backward): the dropout variants of the trunk-input
+//     conversion, of odometry_linear_kernel (the fc launch) and of odometry_linear_bwd_kernel (into dz_fc), and
+//     odometry_channel_dropout_kernel (x3d in the forward, the data gradient of x3 in the backward).
 namespace delora {
 
 constexpr int kBwdThreads = 256;
@@ -933,8 +1017,10 @@ struct TailGrad {
 // blocks [0, p0.N + p1.N): one weight row n each, dW[n, k] = sum_b dz[b, n] x[b, k] and db[n] = sum_b dz[b, n], b in
 // order.  The other blocks: dx tiles, dx[b, k] = sum over the concatenated outputs of p0 then p1 of W[n, k] dz[b, n]
 // (warp w adds the w-th chunk of n in order, the chunks are added in warp order), times act_in'(x[b, k]) (0: none).
-__global__ void __launch_bounds__(kBwdThreads)
-odometry_linear_bwd_kernel(TailGrad p0, TailGrad p1, int B, int act_in, float* __restrict__ dx, int lddx) {
+// kDrop (dx = dz_fc in a dropout training step): then times keep * 1.25f, element b * K + k of the fc mask.
+template <bool kDrop>
+__device__ __forceinline__ void linear_bwd_body(const TailGrad& p0, const TailGrad& p1, int B, int act_in,
+                                                float* __restrict__ dx, int lddx, const DropoutCtr& drop) {
     const int nrows = p0.N + p1.N;
     if ((int)blockIdx.x < nrows) {
         int n = blockIdx.x;
@@ -985,9 +1071,26 @@ odometry_linear_bwd_kernel(TailGrad p0, TailGrad p1, int B, int act_in, float* _
             float s = 0.0f;
 #pragma unroll
             for (int w = 0; w < kTailWarps; ++w) s += s_part[w][j][c];
-            dx[(size_t)b * lddx + kk] = tail_act_bwd(s, act_in ? p0.x[(size_t)b * p0.ldx + kk] : 0.0f, act_in);
+            float g = tail_act_bwd(s, act_in ? p0.x[(size_t)b * p0.ldx + kk] : 0.0f, act_in);
+            if (kDrop) {
+                uint64_t seed, step;
+                dropout_seed_step(drop, seed, step);
+                g = dropout_keep(seed, step, kDropFc, (uint64_t)b * p0.K + kk) ? g * kDropScale : 0.0f;
+            }
+            dx[(size_t)b * lddx + kk] = g;
         }
     }
+}
+
+__global__ void __launch_bounds__(kBwdThreads)
+odometry_linear_bwd_kernel(TailGrad p0, TailGrad p1, int B, int act_in, float* __restrict__ dx, int lddx) {
+    linear_bwd_body<false>(p0, p1, B, act_in, dx, lddx, DropoutCtr{nullptr, 0});
+}
+
+__global__ void __launch_bounds__(kBwdThreads)
+odometry_linear_bwd_dropout_kernel(TailGrad p0, TailGrad p1, int B, int act_in, float* __restrict__ dx, int lddx,
+                                   DropoutCtr drop) {
+    linear_bwd_body<true>(p0, p1, B, act_in, dx, lddx, drop);
 }
 
 struct OutBwd {
@@ -1177,7 +1280,8 @@ static void make_train_plan(const delora_odometry_desc* d, TrainPlan* tp) {
     size_t off = 0;
     const size_t blob = (size_t)m.blob_floats * 4;
     tp->master = take(off, blob); tp->grad = take(off, blob); tp->adam_m = take(off, blob); tp->adam_v = take(off, blob);
-    tp->ctr = take(off, 2 * sizeof(long long));
+    // [0] Adam's step count, [1] the ICP scratch's batch size, [2] the dropout seed (the slot has 256 bytes)
+    tp->ctr = take(off, 3 * sizeof(long long));
     tp->w = plan_weights(m, true, off);
     // one key buffer serves both projections of a step, one after the other
     tp->f = plan_frames(d, 2 * MB, 0, false, d->w_pre > W ? d->w_pre : W, off);
@@ -1272,8 +1376,13 @@ static int check_train_params(const delora_odometry_train_params* hp, const char
     return 0;
 }
 
-static int train_trunk_backward(const TrainPlan& tp, char* ws, int act, int B, cudaStream_t st) {
+// drop.ctr non-NULL (a dropout training step): layer4's first block read x3d (in g[2][2], see the step), so its two
+// weight gradients read it too, while its act' epilogue reads x3; the data gradient of x3 is then multiplied by
+// keep * 1.25 in place (one more bf16 rounding).  g[2][2] is first written by layer3's own backward, after that.
+static int train_trunk_backward(const TrainPlan& tp, char* ws, int act, int B, cudaStream_t st,
+                                DropoutCtr drop = DropoutCtr{nullptr, 0}) {
     const Model& m = tp.m;
+    const int x3_block = last_stage3_block(m);
     int rc;
     const int act_bwd = act == 1 ? 4 : 3;                 // ACT_RELU_BWD / ACT_TANH_BWD: multiply by act'(saved)
     float* grad = reinterpret_cast<float*>(ws + tp.grad);
@@ -1286,6 +1395,9 @@ static int train_trunk_backward(const TrainPlan& tp, char* ws, int act, int B, c
         const Block& b = m.block[i];
         const int s = b.stage;
         const char* x = i == 0 ? ws + tp.t.pool : ws + tp.t.out[i - 1];
+        // the input the forward's convolutions read: x3d for layer4's first block in a dropout step
+        const bool reads_x3d = drop.ctr && i == x3_block + 1;
+        const char* xin = reads_x3d ? ws + tp.g[2][2] : x;
         char* dz1 = ws + tp.g[s][2];
         // the data gradient of the block input: the other buffer of this stage, or a buffer of the previous stage
         char* next;
@@ -1295,12 +1407,12 @@ static int train_trunk_backward(const TrainPlan& tp, char* ws, int act, int B, c
                                            b.cout, b.cout, 3, 1, 1, st))) return rc;
         if ((rc = delora_conv2d_fprop_bf16(dz2, ws + tp.w.w_flip[b.c2], nullptr, ws + tp.t.t1[i], dz1, B, b.hout, b.wout, b.cout,
                                            b.cout, 3, 1, 1, act_bwd, st))) return rc;
-        if ((rc = delora_conv2d_wgrad_bf16(x, dz1, grad + m.conv[b.c1].blob, scratch, B, b.hin, b.win, b.cin, b.cin, b.cout,
+        if ((rc = delora_conv2d_wgrad_bf16(xin, dz1, grad + m.conv[b.c1].blob, scratch, B, b.hin, b.win, b.cin, b.cin, b.cout,
                                            3, b.sh, b.sw, st))) return rc;
         const char* resid = dz2;
         const char* src = dz1;
         if (b.ds >= 0) {
-            if ((rc = delora_conv2d_wgrad_bf16(x, dz2, grad + m.conv[b.ds].blob, scratch, B, b.hin, b.win, b.cin, b.cin,
+            if ((rc = delora_conv2d_wgrad_bf16(xin, dz2, grad + m.conv[b.ds].blob, scratch, B, b.hin, b.win, b.cin, b.cin,
                                                b.cout, 1, b.sh, b.sw, st))) return rc;
             // the 1x1 strided downsample's data gradient: 1x1 convolution of the small dz, scattered afterwards
             char* small = ws + tp.gds[s];
@@ -1309,6 +1421,7 @@ static int train_trunk_backward(const TrainPlan& tp, char* ws, int act, int B, c
             if (tp.phase_dgrad[i]) {
                 if ((rc = delora_conv2d_dgrad_bf16(dz1, ws + tp.w.w_flip[b.c1], small, x, next, B, b.hin, b.win, b.cin, b.cout,
                                                    b.sh, b.sw, act_bwd, 1, st))) return rc;
+                if (reads_x3d && (rc = channel_dropout(m, next, next, B, drop, st))) return rc;
                 dz2 = next;
                 continue;
             }
@@ -1325,6 +1438,7 @@ static int train_trunk_backward(const TrainPlan& tp, char* ws, int act, int B, c
         // block reads the max-pool output (ACT_NONE: the pool's backward applies the stem's act')
         if ((rc = delora_conv2d_fprop_bf16(src, ws + tp.w.w_flip[b.c1], resid, i > 0 ? x : nullptr, next, B, b.hin, b.win,
                                            b.cout, b.cin, 3, 1, 1, i > 0 ? act_bwd : 0, st))) return rc;
+        if (reads_x3d && (rc = channel_dropout(m, next, next, B, drop, st))) return rc;
         dz2 = next;
     }
     if ((rc = delora_maxpool_w_bwd_nhwc_bf16(dz2, ws + tp.t.idx, ws + tp.t.stem, B, m.H, m.w2, 64, 4 + act, ws + tp.g_stem,
@@ -1347,14 +1461,23 @@ static TailIO train_tail_io(const TrainPlan& tp, char* ws) {
     return io;
 }
 
-static int linear_bwd(const TailGrad& p0, const TailGrad& p1, int B, int act_in, float* dx, int lddx, cudaStream_t st) {
+// drop.ctr non-NULL: dx is the gradient of resnet.fc's output, multiplied by the fc mask
+static int linear_bwd(const TailGrad& p0, const TailGrad& p1, int B, int act_in, float* dx, int lddx, cudaStream_t st,
+                      DropoutCtr drop = DropoutCtr{nullptr, 0}) {
     const int tiles = ((p0.K + kDgradCols - 1) / kDgradCols) * ((B + kDgradRows - 1) / kDgradRows);
+    if (drop.ctr) {
+        odometry_linear_bwd_dropout_kernel<<<p0.N + p1.N + tiles, kBwdThreads, 0, st>>>(p0, p1, B, act_in, dx, lddx, drop);
+        DELORA_CHECK_LAUNCH("odometry_linear_bwd_dropout_kernel");
+        return 0;
+    }
     odometry_linear_bwd_kernel<<<p0.N + p1.N + tiles, kBwdThreads, 0, st>>>(p0, p1, B, act_in, dx, lddx);
     DELORA_CHECK_LAUNCH("odometry_linear_bwd_kernel");
     return 0;
 }
 
-static int train_tail_backward(const TrainPlan& tp, char* ws, int act, int B, bool identity, cudaStream_t st) {
+// drop.ctr non-NULL: the gradient of resnet.fc's output (dz_fc) is multiplied by keep * 1.25 after act'
+static int train_tail_backward(const TrainPlan& tp, char* ws, int act, int B, bool identity, cudaStream_t st,
+                               DropoutCtr drop = DropoutCtr{nullptr, 0}) {
     const Model& m = tp.m;
     auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
     const float* master = f(tp.master);
@@ -1398,14 +1521,15 @@ static int train_tail_backward(const TrainPlan& tp, char* ws, int act, int B, bo
         // the heads' hidden layers read the same fc output: dx = rot1^T dz_rot + trans1^T dz_trans, then act'(fc_out)
         const int ld = 2 * kHeadHidden;
         if ((rc = linear_bwd(tg(m.lin[0], fc_out, nout, f(tp.dz_hid[0]), ld),
-                             tg(m.lin[2], fc_out, nout, f(tp.dz_hid[0]) + kHeadHidden, ld), B, act, dz_fc, nout, st)))
+                             tg(m.lin[2], fc_out, nout, f(tp.dz_hid[0]) + kHeadHidden, ld), B, act, dz_fc, nout, st, drop)))
             return rc;
     } else {
         for (int i = m.n_lin - 2; i >= 0; --i) {
             const float* x = i == 0 ? fc_out : f(tp.hid[i - 1]);
             const int ldx = i == 0 ? nout : m.lin[i - 1].N;
             float* dx = i == 0 ? dz_fc : f(tp.dz_hid[i - 1]);
-            if ((rc = linear_bwd(tg(m.lin[i], x, ldx, f(tp.dz_hid[i]), m.lin[i].N), none, B, act, dx, ldx, st))) return rc;
+            if ((rc = linear_bwd(tg(m.lin[i], x, ldx, f(tp.dz_hid[i]), m.lin[i].N), none, B, act, dx, ldx, st,
+                                 i == 0 ? drop : DropoutCtr{nullptr, 0}))) return rc;
         }
     }
     // resnet.fc: its input is the pooled trunk output; the last block's act' is applied by the average pool's backward
@@ -1447,6 +1571,7 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
     DELORA_CHECK_ARG(points && n_points && workspace, "%s: null pointer", who);
     DELORA_CHECK_ARG(B >= 1 && B <= d->max_batch, "%s: B=%d outside [1, max_batch=%d]", who, B, d->max_batch);
     const bool normalized = (hp->loss_flags & DELORA_TRAIN_NORMALIZATION_SCALING) != 0u;
+    const bool dropout = (hp->loss_flags & DELORA_TRAIN_DROPOUT) != 0u;
     DELORA_CHECK_ARG(!normalized || d->w_pre > 0,
                      "%s: DELORA_TRAIN_NORMALIZATION_SCALING needs w_pre > 0 (the reference's recipe: normals from the "
                      "unscaled points at H x w_pre), got w_pre=%d", who, d->w_pre);
@@ -1458,6 +1583,9 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
     auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
     const int H = d->H, W = d->W, HW = H * W;
     long long* ctr = reinterpret_cast<long long*>(ws + tp.ctr);
+    // the masks of this step: the forward reads the step count before odometry_out_bwd_kernel advances it, the
+    // backward after
+    const DropoutCtr drop_fwd{dropout ? ctr : nullptr, 0}, drop_bwd{dropout ? ctr : nullptr, 1};
     int rc;
     cudaError_t e = cudaSuccess;
 
@@ -1493,10 +1621,11 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
                                                 st))) {
         return rc;
     }
-    // 2. forward, keeping the activations
-    if ((rc = trunk_input(m, tp.t, ws, images, images + (size_t)B * 4 * HW, B, st))) return rc;
-    if ((rc = trunk_forward(m, tp.t, tp.w, true, ws, d->act, B, f(tp.pooled), st))) return rc;
-    if ((rc = run_tail(m, train_tail_io(tp, ws), d->act, f(tp.pooled), B, f(tp.T16), st))) return rc;
+    // 2. forward, keeping the activations.  Dropout: x3d goes to the stage-3 backward buffer g[2][2], which nothing
+    // writes before layer3's own backward
+    if ((rc = trunk_input(m, tp.t, ws, images, images + (size_t)B * 4 * HW, B, st, drop_fwd))) return rc;
+    if ((rc = trunk_forward(m, tp.t, tp.w, true, ws, d->act, B, f(tp.pooled), st, drop_fwd, tp.g[2][2]))) return rc;
+    if ((rc = run_tail(m, train_tail_io(tp, ws), d->act, f(tp.pooled), B, f(tp.T16), st, nullptr, drop_fwd))) return rc;
     // 3. ICP losses and dL/dT: source = scan_2 moved by T, target = scan_1.  The identity fit still runs them: the
     // reference logs the ICP losses in that phase too
     const bool identity = (hp->loss_flags & DELORA_LOSS_IDENTITY_FIT) != 0u;
@@ -1508,7 +1637,8 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
     DELORA_CHECK_LAUNCH("odometry_icp_rearm_kernel");
     if ((rc = delora_icp_dense_fwd_bwd(pts_grid + (size_t)B * HW, nrm_grid + (size_t)B * HW, f(tp.T12), pts_grid, nrm_grid,
                                        B, H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, hp->lambda_po2pl,
-                                       hp->loss_flags & ~(DELORA_LOSS_IDENTITY_FIT | DELORA_TRAIN_NORMALIZATION_SCALING),
+                                       hp->loss_flags & ~(DELORA_LOSS_IDENTITY_FIT | DELORA_TRAIN_NORMALIZATION_SCALING |
+                                                          DELORA_TRAIN_DROPOUT),
                                        f(tp.losses), f(tp.grad_T), f(tp.icp), st))) return rc;
     if (normalized) {               // T in metres for the caller, the factor in losses[b][6]
         odometry_train_normalized_out_kernel<<<(B * 16 + 255) / 256, 256, 0, st>>>(f(tp.T16), f(tp.pre_image), B, T,
@@ -1516,8 +1646,8 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
         DELORA_CHECK_LAUNCH("odometry_train_normalized_out_kernel");
     }
     // 4. backward: tail (dL/dT of the ICP mean or of the identity fit), average pool, trunk
-    if ((rc = train_tail_backward(tp, ws, d->act, B, identity, st))) return rc;
-    if ((rc = train_trunk_backward(tp, ws, d->act, B, st))) return rc;
+    if ((rc = train_tail_backward(tp, ws, d->act, B, identity, st, drop_bwd))) return rc;
+    if ((rc = train_trunk_backward(tp, ws, d->act, B, st, drop_bwd))) return rc;
     // outputs (T: the weights before the update)
     auto out = [&](float* dst, size_t src, size_t n) {
         if (dst && e == cudaSuccess) e = cudaMemcpyAsync(dst, ws + src, n * sizeof(float), cudaMemcpyDeviceToDevice, st);
@@ -1597,4 +1727,51 @@ extern "C" int delora_odometry_train_set_state(const delora_odometry_desc* d, co
     DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
     // the bf16 filters from the new master weights, through the table _train_init wrote
     return delora_conv_weight_prep_multi(ws + tp.w.table, tp.m.n_conv, st);
+}
+
+// ================================================================================================ dropout
+namespace delora {
+
+__global__ void odometry_set_seed_kernel(long long* __restrict__ ctr, unsigned long long seed) {
+    ctr[2] = (long long)seed;
+}
+
+// keep[i] = 1 if element i of tensor t is kept at (seed, step), else 0; one thread per 4 elements (one Philox block)
+__global__ void __launch_bounds__(256)
+dropout_keep_mask_kernel(unsigned long long seed, unsigned long long step, int t, long long n, uint8_t* __restrict__ keep) {
+    const long long q = (long long)blockIdx.x * 256 + threadIdx.x;
+    if (q * 4 >= n) return;
+    const Philox4 r = dropout_words(seed, step, t, (uint64_t)q);
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+        if (q * 4 + k < n) keep[q * 4 + k] = dropout_word_keeps(philox_word(r, k)) ? 1 : 0;
+}
+
+}  // namespace delora
+
+extern "C" int delora_odometry_train_set_dropout_seed(const delora_odometry_desc* d, uint64_t seed, void* workspace,
+                                                      void* stream) {
+    const char* who = "delora_odometry_train_set_dropout_seed";
+    if (check_train_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    TrainPlan tp;
+    make_train_plan(d, &tp);
+    odometry_set_seed_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(reinterpret_cast<long long*>((char*)workspace + tp.ctr),
+                                                                (unsigned long long)seed);
+    DELORA_CHECK_LAUNCH("odometry_set_seed_kernel");
+    return 0;
+}
+
+extern "C" int delora_dropout_keep_mask(uint64_t seed, int64_t step, int tensor, int64_t n, uint8_t* keep, void* stream) {
+    const char* who = "delora_dropout_keep_mask";
+    DELORA_CHECK_ARG(keep, "%s: null keep", who);
+    DELORA_CHECK_ARG(n >= 0, "%s: n=%lld must be >= 0", who, (long long)n);
+    DELORA_CHECK_ARG(tensor >= 0 && tensor <= 2, "%s: tensor=%d must be 0 (input), 1 (stage-3 channels) or 2 (fc output)",
+                     who, tensor);
+    if (n == 0) return 0;
+    const long long blocks = ((n + 3) / 4 + 255) / 256;
+    dropout_keep_mask_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(seed, (unsigned long long)step, tensor, n,
+                                                                                keep);
+    DELORA_CHECK_LAUNCH("dropout_keep_mask_kernel");
+    return 0;
 }

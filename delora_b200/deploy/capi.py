@@ -23,10 +23,12 @@ def _ptr(t):
 def train_params(config, lr, loss_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL, beta1=0.9, beta2=0.999, eps=1e-8):
     """delora_odometry_train_params: Adam's settings and the loss and normals' settings of a reference-style config.
     normalization_scaling: True adds DELORA_TRAIN_NORMALIZATION_SCALING (the step then needs a descriptor with
-    w_pre > 0, and refuses w_pre = 0)."""
+    w_pre > 0, and refuses w_pre = 0); use_dropout: True adds DELORA_TRAIN_DROPOUT."""
     nb = config["kitti"]["neighborhood_side_length"]
     if config.get("normalization_scaling", False):
         loss_flags |= ops.TRAIN_NORMALIZATION_SCALING
+    if config.get("use_dropout", False):
+        loss_flags |= ops.TRAIN_DROPOUT
     return _lib.OdometryTrainParams(
         lr=lr, beta1=beta1, beta2=beta2, eps=eps, lambda_po2pl=config["lambda_po2pl"], loss_flags=loss_flags,
         nb_h=nb[0], nb_w=nb[1], epsilon_range=config["epsilon_range"],
@@ -157,6 +159,10 @@ class TrainingWorkspace(_Workspace):
               torch.empty((1,), dtype=torch.int64, device=self.workspace.device))
         self._call("delora_odometry_train_get_state", self.workspace.data_ptr(), *(t.data_ptr() for t in st))
         return st
+
+    def set_dropout_seed(self, seed):
+        """The seed of the dropout masks (DELORA_TRAIN_DROPOUT steps); 0 after construction.  Only launches."""
+        self._call("delora_odometry_train_set_dropout_seed", int(seed) & 0xFFFFFFFFFFFFFFFF, self.workspace.data_ptr())
 
     def set_state(self, weights, exp_avg, exp_avg_sq, step):
         """Array-likes of weight_floats floats each and the Adam step count; synchronises, as its inputs are copies."""

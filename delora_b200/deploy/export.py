@@ -7,10 +7,13 @@ alone and hands the blob to `delora_odometry_load_weights`.  The network configu
 `config/*.yaml` (angles there are in degrees).  Checkpoints of models the C ABI cannot express are refused:
 `pre_feature_extraction: True` and `factor_fewer_resnet_channels != 1`; dropout is the identity at inference.
 `normalization_scaling: True` is recorded in the header's `model_flags` (DELORA_MODEL_NORMALIZATION_SCALING): such a
-model runs through `delora_odometry_pairs_normalized`, and reading the file back restores the key.
+model runs through `delora_odometry_pairs_normalized`, and reading the file back restores the key.  `use_dropout: True`
+is recorded as DELORA_MODEL_DROPOUT: training steps then apply the encoder's dropouts (DELORA_TRAIN_DROPOUT), inference
+ignores the bit, and reading the file back restores the key.
 
 A .dlt file is a training checkpoint for `delora_odometry_train_set_state`: a 256-byte header (the .dlw header with
-its own magic, then Adam's step count, the epoch, the phase, Adam's hyperparameters and the last epoch loss) followed
+its own magic, then Adam's step count, the epoch, the phase, Adam's hyperparameters, the last epoch loss and the
+dropout seed) followed
 by the weights, Adam's exp_avg and exp_avg_sq.  It converts both ways to the reference Trainer's checkpoint dict.
 """
 import collections
@@ -60,8 +63,10 @@ def check_supported(config):
 
 
 def model_flags_from_config(config):
-    """The header's model_flags of a configuration: DELORA_MODEL_NORMALIZATION_SCALING for normalization_scaling."""
-    return _lib.MODEL_NORMALIZATION_SCALING if config.get("normalization_scaling", False) else 0
+    """The header's model_flags of a configuration: DELORA_MODEL_NORMALIZATION_SCALING for normalization_scaling,
+    DELORA_MODEL_DROPOUT for use_dropout."""
+    flags = _lib.MODEL_NORMALIZATION_SCALING if config.get("normalization_scaling", False) else 0
+    return flags | (_lib.MODEL_DROPOUT if config.get("use_dropout", False) else 0)
 
 
 def desc_from_config(config, dataset, n_stride, max_batch=1, preprocessing_normals=False):
@@ -182,8 +187,9 @@ def read_dlw(path):
 # ---- training checkpoints (.dlt): the .dlw header and blob plus Adam's state, byte layout in include/delora_b200.h
 TRAIN_MAGIC = b"DELORAT\x00"
 TRAIN_HEADER_BYTES = 256
-# step | epoch, unsupervised | lr, beta1, beta2, eps, loss | 92 zero bytes, after the 128-byte .dlw header
-_TRAIN_TAIL = struct.Struct("<q" + "ii" + "5f" + "92x")
+# step | epoch, unsupervised | lr, beta1, beta2, eps, loss | dropout_seed (byte 164; zeros in files written before
+# the field: seed 0) | 84 zero bytes, after the 128-byte .dlw header
+_TRAIN_TAIL = struct.Struct("<q" + "ii" + "5f" + "Q" + "84x")
 assert HEADER_BYTES + _TRAIN_TAIL.size == TRAIN_HEADER_BYTES
 
 
@@ -191,7 +197,7 @@ assert HEADER_BYTES + _TRAIN_TAIL.size == TRAIN_HEADER_BYTES
 class TrainingState:
     """What a .dlt file holds besides the descriptor: the fp32 weight blob, Adam's m (exp_avg) and v (exp_avg_sq) in
     blob order, the number of Adam updates, the epochs completed, the phase (unsupervised = 0: identity pre-training),
-    Adam's hyperparameters and the last epoch's mean objective."""
+    Adam's hyperparameters, the last epoch's mean objective and the seed of the dropout masks."""
     weights: np.ndarray
     exp_avg: np.ndarray
     exp_avg_sq: np.ndarray
@@ -203,6 +209,7 @@ class TrainingState:
     beta2: float = 0.999
     eps: float = 1e-8
     loss: float = 0.0
+    dropout_seed: int = 0
 
 
 def write_dlt(path, desc, state, model_flags=0):
@@ -214,7 +221,7 @@ def write_dlt(path, desc, state, model_flags=0):
     with open(path, "wb") as f:
         f.write(_pack_header(TRAIN_MAGIC, TRAIN_HEADER_BYTES, desc, n, model_flags))
         f.write(_TRAIN_TAIL.pack(int(state.step), int(state.epoch), int(state.unsupervised), state.lr, state.beta1,
-                                 state.beta2, state.eps, state.loss))
+                                 state.beta2, state.eps, state.loss, int(state.dropout_seed) & 0xFFFFFFFFFFFFFFFF))
         for a in arrays:
             f.write(a.tobytes())
 
@@ -230,8 +237,9 @@ def read_dlt(path):
     n = h["blob_floats"]
     if data.size != 3 * n:
         raise ValueError(f"{path}: {data.size} floats after the header, the header says 3 x {n}")
-    step, epoch, unsupervised, lr, beta1, beta2, eps, loss = _TRAIN_TAIL.unpack(raw)
-    state = TrainingState(data[:n], data[n:2 * n], data[2 * n:], step, epoch, unsupervised, lr, beta1, beta2, eps, loss)
+    step, epoch, unsupervised, lr, beta1, beta2, eps, loss, seed = _TRAIN_TAIL.unpack(raw)
+    state = TrainingState(data[:n], data[n:2 * n], data[2 * n:], step, epoch, unsupervised, lr, beta1, beta2, eps, loss,
+                          seed)
     return h, d, state
 
 
@@ -336,7 +344,7 @@ def initial_training_state(config, seed):
 def config_from_desc(desc, base=None, dataset="kitti", model_flags=None):
     """`base` (e.g. the YAML configuration) with the network and range-image keys set from a .dlw / .dlt descriptor,
     so that the configuration describes the weights of the file.  model_flags (the header's, or None to keep `base`'s
-    value): sets normalization_scaling."""
+    values): sets normalization_scaling and use_dropout (a file without a bit means False)."""
     cfg = dict(base or {})
     ds = dict(cfg.get(dataset, {}))
     ds.update({"vertical_cells": int(desc.H), "horizontal_cells": int(desc.W),
@@ -350,6 +358,7 @@ def config_from_desc(desc, base=None, dataset="kitti", model_flags=None):
                 "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1})
     if model_flags is not None:
         cfg["normalization_scaling"] = bool(int(model_flags) & _lib.MODEL_NORMALIZATION_SCALING)
+        cfg["use_dropout"] = bool(int(model_flags) & _lib.MODEL_DROPOUT)
     cfg.setdefault("use_dropout", False)
     cfg.setdefault("datasets", [dataset])
     return cfg

@@ -37,6 +37,9 @@ LOSS_PO2PO, LOSS_PO2PL, LOSS_PL2PL, NORMAL_LINEAR = 1, 2, 4, 8
 ICP_STATS = 256      # DELORA_ICP_STATS flag bit
 LOSS_IDENTITY_FIT = 512      # delora_odometry_train_step's identity pre-training objective
 TRAIN_NORMALIZATION_SCALING = 1024   # delora_odometry_train_step: the model uses normalization_scaling (needs w_pre > 0)
+TRAIN_DROPOUT = 2048    # delora_odometry_train_step: the model uses use_dropout (the three dropouts, p = 0.2)
+# tensor ids of the training step's dropout masks (delora_dropout_keep_mask)
+DROPOUT_INPUT, DROPOUT_STAGE3, DROPOUT_FC = 0, 1, 2
 LOSS_ROW, ICP_PARTIAL = 8, 40
 
 _keys_cache = {}
@@ -86,6 +89,17 @@ def project(points, n_points, h, w, hfov, vfov, div_mode=0):
                                     int(div_mode), keys.data_ptr(), image.data_ptr(), index_map.data_ptr(),
                                     _stream()), "delora_project_fwd")
     return image, index_map
+
+
+def dropout_keep_mask(seed, step, tensor, n, device="cuda"):
+    """-> keep [n] uint8: 1 where element i < n of dropout tensor `tensor` (DROPOUT_INPUT, DROPOUT_STAGE3, DROPOUT_FC) is
+    kept at (seed, step) in a DELORA_TRAIN_DROPOUT step, else 0 (the contract is in include/delora_b200.h)."""
+    keep = torch.empty((max(int(n), 0),), dtype=torch.uint8, device=device)
+    if int(n) == 0:
+        return keep
+    _lib.check(_lib.lib().delora_dropout_keep_mask(int(seed) & 0xFFFFFFFFFFFFFFFF, int(step), int(tensor), int(n),
+                                                   keep.data_ptr(), _stream()), "delora_dropout_keep_mask")
+    return keep
 
 
 def normalization_factors(points, n_points):

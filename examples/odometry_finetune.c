@@ -1,7 +1,7 @@
 /*
  * Self-supervised fine-tuning from a C host: no Python, no torch.  Links libdelora_b200.so and cudart only.
  *
- *   odometry_finetune in.dlw out.dlw steps lr scan_000.bin scan_001.bin ...
+ *   odometry_finetune [--dropout-seed S] in.dlw out.dlw steps lr scan_000.bin scan_001.bin ...
  *
  * Reads the weights of in.dlw (written by bin/export_odometry_weights.py, layout: include/delora_b200.h) and a list of
  * consecutive KITTI velodyne .bin scans ([N, 4] float32 rows: x, y, z, reflectance), runs `steps` training steps on the
@@ -10,6 +10,9 @@
  * po2po + lambda * po2pl + pl2pl, before that step's update) once per step.  No ground truth is needed.
  * The normals the losses use are estimated at the resolution the header's w_pre names (export with
  * --preprocessing-normals for the reference's recipe); the program says which on stderr.
+ * A model configured with use_dropout (model_flags has DELORA_MODEL_DROPOUT) trains with its dropouts
+ * (DELORA_TRAIN_DROPOUT); the seed of the masks is --dropout-seed, else the DELORA_DROPOUT_SEED environment variable,
+ * else 0.
  *
  * Build:  cc odometry_finetune.c -I include -I $CUDA_HOME/include -L delora_b200 -ldelora_b200 \
  *            -L $CUDA_HOME/lib64 -lcudart -Wl,-rpath,$PWD/delora_b200 -o odometry_finetune
@@ -61,7 +64,16 @@ static int32_t read_scan(const char* path, int n_stride, float* out) {
 }
 
 int main(int argc, char** argv) {
-    if (argc < 7) return fail("usage: odometry_finetune in.dlw out.dlw steps lr scan.bin scan.bin [scan.bin ...]");
+    unsigned long long dropout_seed = 0;
+    const char* seed_env = getenv("DELORA_DROPOUT_SEED");
+    if (seed_env) dropout_seed = strtoull(seed_env, NULL, 0);
+    if (argc > 2 && strcmp(argv[1], "--dropout-seed") == 0) {
+        dropout_seed = strtoull(argv[2], NULL, 0);
+        argc -= 2;
+        argv += 2;
+    }
+    if (argc < 7)
+        return fail("usage: odometry_finetune [--dropout-seed S] in.dlw out.dlw steps lr scan.bin scan.bin [scan.bin ...]");
     const int steps = atoi(argv[3]);
     const float lr = (float)atof(argv[4]);
     const int n_scans = argc - 5;
@@ -106,7 +118,9 @@ int main(int argc, char** argv) {
     delora_odometry_train_params hp;
     hp.lr = lr; hp.beta1 = 0.9f; hp.beta2 = 0.999f; hp.eps = 1e-8f;
     hp.lambda_po2pl = 1.0f;
-    hp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | (normalized ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u);
+    const int dropout = (hdr.model_flags & DELORA_MODEL_DROPOUT) != 0;
+    hp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | (normalized ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u) |
+                    (dropout ? DELORA_TRAIN_DROPOUT : 0u);
     hp.nb_h = 7; hp.nb_w = 11;
     hp.epsilon_range = 0.5f;
     hp.min_neighbors = 10;
@@ -125,6 +139,8 @@ int main(int argc, char** argv) {
     CUDA_OK(cudaMalloc((void**)&losses, (size_t)B * DELORA_LOSS_ROW * sizeof(float)));
     CUDA_OK(cudaMemcpy(weights, h_blob, (size_t)n_weights * sizeof(float), cudaMemcpyHostToDevice));
     DELORA_OK(delora_odometry_train_init(d, weights, workspace, stream));
+    DELORA_OK(delora_odometry_train_set_dropout_seed(d, dropout_seed, workspace, stream));
+    if (dropout) fprintf(stderr, "odometry_finetune: dropout on, seed %llu\n", dropout_seed);
 
     float* h_losses = (float*)malloc((size_t)B * DELORA_LOSS_ROW * sizeof(float));
     int32_t* h_step_counts = (int32_t*)malloc((size_t)2 * B * sizeof(int32_t));

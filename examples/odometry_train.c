@@ -2,7 +2,7 @@
  * The reference's training loop (src/deploy/trainer.py, Trainer.train) from a C host: no Python, no torch.  Links
  * libdelora_b200.so and cudart only.
  *
- *   odometry_train [--lr LR] [--switch-below L] in.dlt|in.dlw out.dlt epochs B scan_000.bin scan_001.bin ...
+ *   odometry_train [--lr LR] [--switch-below L] [--dropout-seed S] in.dlt|in.dlw out.dlt epochs B scan_000.bin ...
  *
  * Reads a training checkpoint (.dlt: weights, Adam's state, epoch and phase; layout in include/delora_b200.h) or a
  * weight file (.dlw: a fresh Adam with learning rate --lr, default 1e-5, the reference's learning_rate) and a list of
@@ -16,6 +16,10 @@
  * checkpoint.  After every epoch the state goes to out.dlt (written to out.dlt.tmp, then renamed), so a run that
  * stops can resume from it: N epochs in one run and N1 + N2 = N epochs in two give the same bytes.
  * Losses as odometry_finetune.c: po2pl + pl2pl, lambda_po2pl 1, normals at the resolution the header's w_pre names.
+ * A model configured with use_dropout (model_flags has DELORA_MODEL_DROPOUT) trains with its dropouts
+ * (DELORA_TRAIN_DROPOUT).  The seed of the masks is --dropout-seed, else the DELORA_DROPOUT_SEED environment variable,
+ * else the .dlt's (0 for a .dlw); it is written into every out.dlt, so a resumed run draws the masks of an
+ * uninterrupted one.
  *
  * Build:  cc odometry_train.c -I include -I $CUDA_HOME/include -L delora_b200 -ldelora_b200 \
  *            -L $CUDA_HOME/lib64 -lcudart -Wl,-rpath,$PWD/delora_b200 -o odometry_train
@@ -82,15 +86,17 @@ static int write_dlt(const char* path, const delora_odometry_train_file_header* 
 int main(int argc, char** argv) {
     float lr = 1e-5f;
     double switch_below = 1e-2;
+    const char* seed_arg = getenv("DELORA_DROPOUT_SEED");
     int a = 1;
     for (; a + 1 < argc && strncmp(argv[a], "--", 2) == 0; a += 2) {
         if (strcmp(argv[a], "--lr") == 0) lr = (float)atof(argv[a + 1]);
         else if (strcmp(argv[a], "--switch-below") == 0) switch_below = atof(argv[a + 1]);
+        else if (strcmp(argv[a], "--dropout-seed") == 0) seed_arg = argv[a + 1];
         else return fail("unknown option");
     }
     if (argc - a < 6)
-        return fail("usage: odometry_train [--lr LR] [--switch-below L] in.dlt|in.dlw out.dlt epochs B scan.bin "
-                    "scan.bin [scan.bin ...]");
+        return fail("usage: odometry_train [--lr LR] [--switch-below L] [--dropout-seed S] in.dlt|in.dlw out.dlt epochs "
+                    "B scan.bin scan.bin [scan.bin ...]");
     const char* in_path = argv[a];
     const char* out_path = argv[a + 1];
     const int epochs = atoi(argv[a + 2]);
@@ -135,6 +141,13 @@ int main(int argc, char** argv) {
     hdr.base.header_bytes = (int32_t)sizeof hdr;
     memset(hdr.base.reserved, 0, sizeof hdr.base.reserved);
     memset(hdr.reserved, 0, sizeof hdr.reserved);
+    if (seed_arg) {
+        const unsigned long long s = strtoull(seed_arg, NULL, 0);
+        hdr.dropout_seed[0] = (uint32_t)s;
+        hdr.dropout_seed[1] = (uint32_t)(s >> 32);
+    }
+    const uint64_t dropout_seed = (uint64_t)hdr.dropout_seed[0] | ((uint64_t)hdr.dropout_seed[1] << 32);
+    const int dropout = (hdr.base.model_flags & DELORA_MODEL_DROPOUT) != 0;
 
     const int n_pairs = n_scans - 1;
     if (B_max < 1 || B_max > d->max_batch) return fail("B must be in [1, the header's max_batch]");
@@ -174,6 +187,8 @@ int main(int argc, char** argv) {
     CUDA_OK(cudaMalloc((void**)&losses, (size_t)B_max * DELORA_LOSS_ROW * sizeof(float)));
     DELORA_OK(delora_odometry_train_init(d, d_state[0], workspace, stream));
     DELORA_OK(delora_odometry_train_set_state(d, d_state[0], d_state[1], d_state[2], d_step, workspace, stream));
+    DELORA_OK(delora_odometry_train_set_dropout_seed(d, dropout_seed, workspace, stream));
+    if (dropout) fprintf(stderr, "odometry_train: dropout on, seed %llu\n", (unsigned long long)dropout_seed);
     fprintf(stderr, "odometry_train: epoch %d, Adam step %lld, %s, %d pairs\n", hdr.epoch, (long long)hdr.step,
             hdr.unsupervised ? "unsupervised" : "identity pre-training", n_pairs);
 
@@ -182,7 +197,7 @@ int main(int argc, char** argv) {
     if (!h_losses || !h_step_counts) return fail("out of host memory");
     for (int e = 0; e < epochs; ++e) {
         hp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | (hdr.unsupervised ? 0u : DELORA_LOSS_IDENTITY_FIT) |
-                        (normalized ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u);
+                        (normalized ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u) | (dropout ? DELORA_TRAIN_DROPOUT : 0u);
         double sum = 0.0;
         int steps = 0;
         for (int k0 = 0; k0 < n_pairs; k0 += B_max, ++steps) {

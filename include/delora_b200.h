@@ -44,6 +44,8 @@ typedef struct { float x, y, z, w; } delora_f4;
                                          (unsupervised_at_start: False, src/deploy/deployer.py:324-327) */
 #define DELORA_TRAIN_NORMALIZATION_SCALING 1024u /* delora_odometry_train_step only: the model is trained with
                                                     normalization_scaling (see _train_step; needs w_pre > 0) */
+#define DELORA_TRAIN_DROPOUT 2048u /* delora_odometry_train_step only: the model is trained with use_dropout (the
+                                      three dropouts of the reference's encoder; see _train_step) */
 
 /* number of floats in one row of the `losses` output of delora_icp_fwd_bwd */
 #define DELORA_LOSS_ROW 8   /* [po2po, po2pl, pl2pl, M_pairs, M_po2po, 0, 0, 0] */
@@ -429,6 +431,8 @@ typedef struct {
 /* model_flags bits: how the model expects its input, beyond the descriptor */
 #define DELORA_MODEL_NORMALIZATION_SCALING 1u    /* trained with normalization_scaling: run it through
                                                     delora_odometry_pairs_normalized */
+#define DELORA_MODEL_DROPOUT 2u                  /* configured with use_dropout: train it with DELORA_TRAIN_DROPOUT;
+                                                    inference and streams ignore the bit (dropout is the identity) */
 typedef struct {
     char magic[8];
     int32_t abi_version;                 /* DELORA_B200_ABI_VERSION of the exporter */
@@ -561,8 +565,9 @@ typedef struct {
     float lr, beta1, beta2, eps;         /* Adam (torch defaults 0.9, 0.999, 1e-8); lr >= 0, betas in [0, 1), eps > 0 */
     float lambda_po2pl;                  /* config lambda_po2pl */
     uint32_t loss_flags;                 /* DELORA_LOSS_* / DELORA_NORMAL_LINEAR bits, at least one ICP loss bit
-                                            (PO2PO, PO2PL, PL2PL), plus DELORA_LOSS_IDENTITY_FIT and
-                                            DELORA_TRAIN_NORMALIZATION_SCALING (see _train_step) */
+                                            (PO2PO, PO2PL, PL2PL), plus DELORA_LOSS_IDENTITY_FIT,
+                                            DELORA_TRAIN_NORMALIZATION_SCALING and DELORA_TRAIN_DROPOUT (see
+                                            _train_step) */
     int nb_h, nb_w;                      /* neighborhood_side_length (7, 11): odd and positive */
     float epsilon_range;                 /* 0.5 */
     int min_neighbors;                   /* min_num_points_in_neighborhood_to_determine_point_class, 10 */
@@ -596,7 +601,26 @@ int delora_odometry_train_init(const delora_odometry_desc* d, const float* weigh
  * same float64 order), and those points are divided by it (correctly rounded) before the H x W projection.  The ICP
  * losses are in normalised units, as in the reference; the identity fit uses the unscaled T; the T output is rescaled
  * (T[:3, 3] *= factor in fp32); losses[b][6] is the factor (0 in steps without the bit).  No workspace size changes:
- * the factor is kept in the H x w_pre image, which nothing reads after the preprocessing projection. */
+ * the factor is kept in the H x w_pre image, which nothing reads after the preprocessing projection.
+ * Dropout: with DELORA_TRAIN_DROPOUT in hp->loss_flags the step applies the three dropouts (p = 0.2) of a model
+ * configured with use_dropout (src/models/resnet_modified.py:33-38, :96, :110, :117; the reference's Trainer never
+ * calls model.eval(), so they are active in every training step, the identity fit included).  It combines with
+ * DELORA_LOSS_IDENTITY_FIT and DELORA_TRAIN_NORMALIZATION_SCALING.  The masks follow the contract below, with s = the
+ * workspace's Adam step count at the start of the step (the int64 of _train_get_state) and the workspace's seed
+ * (delora_odometry_train_set_dropout_seed, 0 after _train_init); they are drawn on the device, so a graph replay draws
+ * fresh masks every step and a run resumed through _train_set_state + _train_set_dropout_seed draws the masks the
+ * uninterrupted run would have.  The masks are regenerated in the backward; nothing is stored but x3d below, and no
+ * workspace size changes.
+ *   - input (tensor 0): every element of cat(image_1, image_2) is multiplied by keep * 1.25f in fp32 inside the trunk
+ *     input conversion, before the bf16 (+ bf16 residual) rounding: the stem sees the bits of pre-multiplied images.
+ *   - stage-3 channels (tensor 1, Dropout2d): layer4's first block (its conv1, its downsample and both weight
+ *     gradients) reads x3d = bf16_rn(float(x3) * 1.25f) for kept (pair, channel) and 0 for dropped ones, x3 = layer3's
+ *     output, which stays as it was for the act' epilogues.  The backward multiplies the data gradient of x3, after
+ *     act'(x3), by keep * 1.25 and rounds it to bf16 once more.  x3d lives in a stage-3 backward buffer that nothing
+ *     writes before layer3's own backward.
+ *   - fc output (tensor 2): fc_out = act(keep * 1.25f * (W pooled + b)) in fp32; the heads' backward multiplies the
+ *     gradient of fc_out by keep * 1.25 after act'.
+ * Without the bit every launch is the one of a step without dropout; inference and streams never apply dropout. */
 int delora_odometry_train_step(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
                                const float* points, const int32_t* n_points, int B, void* workspace,
                                float* losses, float* T, float* pooled, float* grads, void* stream);
@@ -618,6 +642,24 @@ int delora_odometry_train_get_state(const delora_odometry_desc* d, const void* w
 int delora_odometry_train_set_state(const delora_odometry_desc* d, const float* weights, const float* exp_avg,
                                     const float* exp_avg_sq, const int64_t* step, void* workspace, void* stream);
 
+/* ---- Dropout masks of the training step (DELORA_TRAIN_DROPOUT), exactly enough to re-implement them elsewhere:
+ * Philox4x32-10 (multipliers 0xD2511F53, 0xCD9E8D57; Weyl constants 0x9E3779B9, 0xBB67AE85; curand's philox4x32_10),
+ *   key = (low 32 bits of seed, high 32 bits of seed).  Element i of tensor t at step s: counter = (low 32 bits of
+ *   i >> 2, t, low 32 bits of s, high 32 bits of s), the word is output word i & 3.  The element is kept iff
+ *   (word >> 8) < 13421773, i.e. u < 0.8f with u = (word >> 8) * 2^-24 (0.8f is exactly 13421773 * 2^-24); a kept
+ *   value is multiplied by 1.25f (1 / (1 - p), exact in fp32), a dropped one becomes 0.
+ * Tensor ids and element indices, per pair b (independent of B and max_batch):
+ *   t = 0  input:               ((b * 8 + c) * H + h) * W + w over cat(image_1, image_2) (channels 0..3 image_1)
+ *   t = 1  stage-3 channels:    b * C3 + c, C3 = layer3's channel count (256)
+ *   t = 2  fc output:           b * resnet_outputs + j
+ * delora_odometry_train_set_dropout_seed: store `seed` in the training workspace (launches one kernel, capturable).
+ *   Refused before any launch, naming the argument: an invalid descriptor, a null workspace.
+ * delora_dropout_keep_mask: keep [n] uint8 (device) = 1 for the kept elements 0 .. n-1 of tensor `tensor` at
+ *   (seed, step), else 0, with the device function the step runs.  Refused before any launch, naming the argument:
+ *   null keep, n < 0, tensor outside 0..2. */
+int delora_odometry_train_set_dropout_seed(const delora_odometry_desc* d, uint64_t seed, void* workspace, void* stream);
+int delora_dropout_keep_mask(uint64_t seed, int64_t step, int tensor, int64_t n, uint8_t* keep, void* stream);
+
 /* Training checkpoint (.dlt, written by delora_b200/deploy/export.py and examples/odometry_train.c), little-endian,
  * readable with fread alone:
  *   bytes   0..127  a delora_odometry_file_header (the .dlw layout above) with magic "DELORAT" and header_bytes 256
@@ -626,7 +668,9 @@ int delora_odometry_train_set_state(const delora_odometry_desc* d, const float* 
  *   bytes 140..143  unsupervised (int32): 0 = still in the identity pre-training phase, 1 = ICP objective
  *   bytes 144..159  lr, beta1, beta2, eps (float32 each): Adam's hyperparameters
  *   bytes 160..163  loss (float32): the mean objective of the last epoch
- *   bytes 164..255  zero
+ *   bytes 164..171  dropout_seed (uint64): the seed of delora_odometry_train_set_dropout_seed (files written before the
+ *                   field have zeros there, i.e. seed 0)
+ *   bytes 172..255  zero
  *   bytes 256..     float32[blob_floats] weights, then float32[blob_floats] exp_avg, then float32[blob_floats]
  *                   exp_avg_sq, each in blob order (the three arrays of delora_odometry_train_set_state). */
 #define DELORA_TRAINING_FILE_MAGIC "DELORAT"     /* 7 characters + NUL = the 8 magic bytes */
@@ -637,7 +681,9 @@ typedef struct {
     int32_t unsupervised;
     float lr, beta1, beta2, eps;
     float loss;
-    uint8_t reserved[92];
+    uint32_t dropout_seed[2];            /* bytes 164..171: the uint64 seed as (low word, high word), which keeps the
+                                            struct's layout (a uint64_t member would be aligned to byte 168) */
+    uint8_t reserved[84];
 } delora_odometry_train_file_header;
 
 /* ---- Data-parallel training step: average of the weight gradients over the ranks (SURVEY.md 8(e); the reference
