@@ -125,10 +125,11 @@ def _preprocessed_lists(cfg, pts, counts, w_pre):
 Step = collections.namedtuple("Step", "losses T pooled grads objective")
 
 
-def python_step(m, cfg, pts, counts, w_pre=0, identity=False):
+def python_step(m, cfg, pts, counts, w_pre=0, identity=False, flags=FLAGS):
     """SyntheticTrainStep.step without the optimizer -> Step(losses [B,8], T [B,4,4], pooled [B,512], {name: grad},
     objective).
 
+    flags: the ICP loss bits (DELORA_LOSS_* / DELORA_NORMAL_LINEAR) the step's losses use; lambda_po2pl is cfg's.
     w_pre > 0: the reference's two-resolution recipe through the mirror -- Preprocesser.preprocess_scans in memory (the
     offline stage's row-major point and normal lists), ops.project at W and ops.grids_from_projection
     (Deployer.step); otherwise ops.project + ops.normals at W.  Then OdometryModel's training forward (TensorCoreEncoder
@@ -156,7 +157,7 @@ def python_step(m, cfg, pts, counts, w_pre=0, identity=False):
     trans, quat = m(image_1=img1, image_2=img2)
     T = GeometryHandler.get_transformation_matrix_quaternion(trans.float(), quat.float(), DEV)
     total, parts = _FusedIcp.apply(T, pg[b:].contiguous(), ng[b:].contiguous(), pg[:b].contiguous(),
-                                   ng[:b].contiguous(), (h, w, hf, vf), float(cfg["lambda_po2pl"]), FLAGS,
+                                   ng[:b].contiguous(), (h, w, hf, vf), float(cfg["lambda_po2pl"]), flags,
                                    ops.icp_scratch(b, h * w, pts.device))
     if identity:
         eye = torch.eye(4, device=DEV).view(1, 4, 4)
