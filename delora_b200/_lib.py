@@ -95,6 +95,13 @@ SIGNATURES = {
     "delora_grad_allreduce_flag_words": (c_int, []),
     "delora_grad_allreduce_f32": (c_int, [c_void_p, c_void_p, ctypes.c_uint64, c_int, c_int, ctypes.c_longlong,
                                           ctypes.c_longlong, c_float, c_u32, c_int, c_int, c_void_p, c_void_p]),
+    "delora_trunk_weight_bytes": (c_i64, [c_void_p, c_int]),
+    "delora_trunk_prep_weights": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "delora_trunk_activation_bytes": (c_i64, [c_void_p, c_int, c_int, c_int, c_int]),
+    "delora_trunk_forward": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                     c_void_p, c_void_p, c_void_p]),
+    "delora_trunk_backward": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
+                                      c_int, c_void_p]),
     "delora_odometry_weight_floats": (c_i64, [c_desc_p]),
     "delora_odometry_workspace_bytes": (c_i64, [c_desc_p]),
     "delora_odometry_init": (c_int, [c_desc_p, c_void_p, c_void_p]),

@@ -1,10 +1,6 @@
 // Odometry inference through the C ABI (sm_90a): raw scans -> relative transforms in one call.
 //
-// The trunk is the layer chain of the Python encoder (models/tc_encoder.py, TensorCoreEncoder.features + avgpool),
-// written once here and run through the same entry points in the same order: projection, stem (16-channel layout
-// when W is even, channel-padded conv2d_fprop otherwise), max-pool, the BasicBlocks with their 1x1 downsamples and
-// fused residual + activation, average pool.  Inference keeps no activations, so each stage owns three buffers that
-// its blocks rotate through.
+// Projection, then the encoder trunk of trunk.cuh (the one the Python encoder runs too), then the tail.
 //
 // New here: the fully connected tail (reference: src/models/model.py:58-84, :103-116) in fp32.
 //   odometry_linear_kernel: y = act(W x + b) for all B rows; one warp per output neuron, a float4 per lane per step.
@@ -21,13 +17,11 @@
 #include "common.cuh"
 #include "dropout.cuh"
 #include "projection.cuh"
+#include "trunk.cuh"
 
 namespace delora {
 
 constexpr int kTailWarps = 8;
-constexpr int kMaxBlocksPerStage = 16;
-constexpr int kMaxBlocks = 4 * kMaxBlocksPerStage;
-constexpr int kMaxConv = 1 + 4 * (2 * kMaxBlocksPerStage) + 3;
 constexpr int kMaxLinear = 5;
 constexpr int kMaxBatch = 1024;
 constexpr int kHeadHidden = 100;
@@ -184,47 +178,26 @@ __global__ void odometry_counts_kernel(const int32_t* __restrict__ n_in, const i
 }
 
 // ---------------------------------------------------------------- the model: layer sequence + weight-blob offsets
-struct ConvLayer {
-    int cout, cin, k;
-    int64_t blob;          // offset in floats of the fp32 filter in the weight blob
-};
-struct Block {
-    int stage, sh, sw, c1, c2, ds;     // conv indices (ds = -1: identity shortcut)
-    int hin, win, hout, wout, cin, cout;
-};
 struct Linear {
     int K, N;
     int64_t blob_w, blob_b;
 };
 struct Model {
-    int H, W, w2, w4, stem_fast;
-    int n_conv, n_block, n_lin;
-    ConvLayer conv[kMaxConv];
-    Block block[kMaxBlocks];
+    TrunkPlan t;                       // the trunk's filters open the blob
+    int n_lin;
     Linear lin[kMaxLinear];            // two heads: rot1, rot2, trans1, trans2; single MLP: 5 layers
     Linear fc;
     int64_t blob_floats;
-    int stage_h[4], stage_w[4], stage_c[4];
 };
-
-static size_t align256(size_t n) { return (n + 255) & ~(size_t)255; }
-static size_t take(size_t& off, size_t bytes) { const size_t o = off; off += align256(bytes); return o; }
-static int out_size(int n, int s) { return (n - 1) / s + 1; }
-static size_t nhwc_bytes(int b, int h, int w, int c) { return (size_t)b * (h + 2) * (w + 2) * c * 2; }
 
 static int check_desc(const delora_odometry_desc* d, const char* who) {
     DELORA_CHECK_ARG(d != nullptr, "%s: null descriptor", who);
-    DELORA_CHECK_ARG(d->H >= 1 && d->W >= 2 && (long long)d->H * d->W < (1ll << 27),
-                     "%s: bad image size H=%d W=%d", who, d->H, d->W);
-    DELORA_CHECK_ARG(out_size(d->W, 2) % 2 == 0,
-                     "%s: W=%d: the stem output width (W-1)/2+1 must be even for the max-pool", who, d->W);
+    DELORA_CHECK_ARG((long long)d->H * d->W < (1ll << 27), "%s: bad image size H=%d W=%d", who, d->H, d->W);
+    if (check_trunk(d->layers, d->H, d->W, who)) return 1;
     DELORA_CHECK_ARG(d->n_stride >= 1, "%s: n_stride=%d must be >= 1", who, d->n_stride);
     DELORA_CHECK_ARG(d->max_batch >= 1 && d->max_batch <= kMaxBatch, "%s: max_batch=%d must be in [1, %d]", who,
                      d->max_batch, kMaxBatch);
     DELORA_CHECK_ARG(d->act == 1 || d->act == 2, "%s: act=%d must be 1 (relu) or 2 (tanh)", who, d->act);
-    for (int s = 0; s < 4; ++s)
-        DELORA_CHECK_ARG(d->layers[s] >= 1 && d->layers[s] <= kMaxBlocksPerStage, "%s: layers[%d]=%d must be in [1, %d]",
-                         who, s, d->layers[s], kMaxBlocksPerStage);
     DELORA_CHECK_ARG(d->resnet_outputs >= 1 && d->resnet_outputs <= 65536, "%s: resnet_outputs=%d must be in [1, 65536]",
                      who, d->resnet_outputs);
     DELORA_CHECK_ARG(d->single_mlp == 0 || d->single_mlp == 1, "%s: single_mlp=%d must be 0 or 1", who, d->single_mlp);
@@ -237,35 +210,8 @@ static int check_desc(const delora_odometry_desc* d, const char* who) {
 // descriptor.
 static void plan_model(const delora_odometry_desc* d, Model* m) {
     memset(m, 0, sizeof(Model));
-    m->H = d->H; m->W = d->W;
-    m->w2 = out_size(d->W, 2); m->w4 = m->w2 / 2;
-    m->stem_fast = d->W % 2 == 0;
-    int64_t blob = 0;
-    auto add_conv = [&](int cout, int cin, int k) {
-        ConvLayer& c = m->conv[m->n_conv];
-        c.cout = cout; c.cin = cin; c.k = k; c.blob = blob;
-        blob += (int64_t)cout * cin * k * k;
-        return m->n_conv++;
-    };
-    add_conv(64, 8, 3);                                     // resnet.conv1
-    static const int widths[4] = {64, 128, 256, 512};
-    static const int strides_h[4] = {1, 1, 1, 2}, strides_w[4] = {1, 2, 2, 2};
-    int inplanes = 64, h = d->H, w = m->w4;
-    for (int s = 0; s < 4; ++s) {
-        for (int bi = 0; bi < d->layers[s]; ++bi) {
-            Block& b = m->block[m->n_block++];
-            b.stage = s;
-            b.sh = bi == 0 ? strides_h[s] : 1; b.sw = bi == 0 ? strides_w[s] : 1;
-            b.hin = h; b.win = w; b.hout = out_size(h, b.sh); b.wout = out_size(w, b.sw);
-            b.cin = inplanes; b.cout = widths[s];
-            b.c1 = add_conv(b.cout, b.cin, 3);
-            b.c2 = add_conv(b.cout, b.cout, 3);
-            const bool strided = b.sh != 1 || b.sw != 1;
-            b.ds = (bi == 0 && (strided || inplanes != widths[s])) ? add_conv(b.cout, b.cin, 1) : -1;
-            inplanes = b.cout; h = b.hout; w = b.wout;
-        }
-        m->stage_h[s] = h; m->stage_w[s] = w; m->stage_c[s] = widths[s];
-    }
+    plan_trunk(d->layers, d->H, d->W, &m->t);
+    int64_t blob = m->t.conv_floats;
     auto add_lin = [&](Linear& l, int K, int N) {
         l.K = K; l.N = N; l.blob_w = blob; blob += (int64_t)K * N; l.blob_b = blob; blob += N;
     };
@@ -311,68 +257,14 @@ static Frames plan_frames(const delora_odometry_desc* d, int n_scans, int n_cach
     return f;
 }
 
-// The weight section: the delora_conv_weight_prep_multi table (one row per filter), each filter's bf16 forward copy
-// w_fwd [cout, k*k, cin_pad] and, when the workspace trains (flip), its flipped copy w_flip for the data gradient
-// (every filter but the stem's).
-struct Weights {
-    bool flip;
-    size_t table, w_fwd[kMaxConv], w_flip[kMaxConv];
-};
-
-static Weights plan_weights(const Model& m, bool flip, size_t& off) {
-    Weights w;
-    memset(&w, 0, sizeof(w));
-    w.flip = flip;
-    w.table = take(off, (size_t)m.n_conv * 8 * 8);
-    for (int i = 0; i < m.n_conv; ++i) {
-        const ConvLayer& c = m.conv[i];
-        if (i == 0) {
-            w.w_fwd[0] = take(off, m.stem_fast ? (size_t)3 * 64 * 64 * 2 : (size_t)64 * 9 * 64 * 2);
-        } else {
-            w.w_fwd[i] = take(off, (size_t)c.cout * c.k * c.k * c.cin * 2);
-            if (flip) w.w_flip[i] = take(off, (size_t)c.cin * c.k * c.k * c.cout * 2);
-        }
-    }
-    return w;
-}
-
-// The bf16 filters of the section from the fp32 blob src: the table rows {fp32 src, w_fwd, w_flip or 0, Cout, Cin, k,
-// Cin_pad, kind}, the stem in the 16-channel layout (kind 1) when W is even, channel-padded to 64 otherwise; then
-// one delora_conv_weight_prep_multi launch.
-static int prep_weights(const Model& m, const Weights& w, char* ws, const float* src, cudaStream_t st, const char* who) {
-    long long table[kMaxConv * 8];
-    for (int i = 0; i < m.n_conv; ++i) {
-        const ConvLayer& c = m.conv[i];
-        long long* r = table + (size_t)i * 8;
-        r[0] = (long long)(uintptr_t)(src + c.blob);
-        r[1] = (long long)(uintptr_t)(ws + w.w_fwd[i]);
-        r[2] = (w.flip && i > 0) ? (long long)(uintptr_t)(ws + w.w_flip[i]) : 0;
-        r[3] = c.cout; r[4] = c.cin; r[5] = c.k;
-        r[6] = (i == 0) ? (m.stem_fast ? 16 : 64) : c.cin;
-        r[7] = (i == 0 && m.stem_fast) ? 1 : 0;
-    }
-    const cudaError_t e = cudaMemcpyAsync(ws + w.table, table, (size_t)m.n_conv * 8 * sizeof(long long),
-                                          cudaMemcpyHostToDevice, st);
-    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
-    return delora_conv_weight_prep_multi(ws + w.table, m.n_conv, st);
-}
-
-// Where the trunk forward reads and writes: its bf16 NHWC input (16 channels when W is even, 64 otherwise), the stem
-// output, the max-pool output (and its argmax when the forward saves its activations), and for every block i its
-// conv1 output t1[i], its downsample output ds[i] (blocks with a downsample) and its output out[i].
-struct Trunk {
-    size_t x_in, stem, pool, idx, t1[kMaxBlocks], ds[kMaxBlocks], out[kMaxBlocks];
-};
-
-// The pairs / push and the streams workspaces.  Inference keeps no activations: each stage owns three buffers, [0]
-// the pool output (stage 0) / the downsample output, [1] conv1 output, [2] block output; later blocks of the stage
-// alternate their output between [0] and [2].  The tail reads fp32 copies of its weights (256-byte aligned).
+// The pairs / push and the streams workspaces: the trunk's inference buffers and its weight section without the
+// flipped filters.  The tail reads fp32 copies of its weights (256-byte aligned).
 struct InferPlan {
     Model m;
     Frames f;
-    Trunk t;
+    TrunkActs t;
     size_t pooled, fc_out, hid[2];
-    Weights w;
+    TrunkWeights w;
     size_t fc_w, fc_b, lin_w[kMaxLinear], lin_b[kMaxLinear];
     size_t total;
 };
@@ -386,30 +278,12 @@ static void make_infer_plan(const delora_odometry_desc* d, bool streams, InferPl
     const int MB = d->max_batch, nout = d->resnet_outputs;
     size_t off = 0;
     p->f = streams ? plan_frames(d, MB, MB, true, d->W, off) : plan_frames(d, 2 * MB, 1, false, d->W, off);
-    p->t.x_in = take(off, nhwc_bytes(MB, d->H, d->W, m.stem_fast ? 16 : 64));
-    p->t.stem = take(off, nhwc_bytes(MB, d->H, m.w2, 64));
-    size_t act[4][3];
-    for (int s = 0; s < 4; ++s)
-        for (int j = 0; j < 3; ++j) act[s][j] = take(off, nhwc_bytes(MB, m.stage_h[s], m.stage_w[s], m.stage_c[s]));
-    p->t.pool = act[0][0];
-    size_t cur = p->t.pool;
-    for (int i = 0; i < m.n_block; ++i) {
-        const Block& b = m.block[i];
-        const size_t* r = act[b.stage];
-        p->t.t1[i] = r[1];
-        if (b.ds >= 0) {
-            p->t.ds[i] = r[0];
-            p->t.out[i] = r[2];
-        } else {
-            p->t.out[i] = cur == r[2] ? r[0] : r[2];
-        }
-        cur = p->t.out[i];
-    }
+    p->t = plan_trunk_acts(m.t, MB, false, off);
     p->pooled = take(off, (size_t)MB * 512 * 4);
     p->fc_out = take(off, (size_t)MB * nout * 4);
     p->hid[0] = take(off, (size_t)MB * 512 * 4);
     p->hid[1] = take(off, (size_t)MB * 512 * 4);
-    p->w = plan_weights(m, false, off);
+    p->w = plan_trunk_weights(m.t, false, off);
     p->fc_w = take(off, (size_t)m.fc.K * m.fc.N * 4);
     p->fc_b = take(off, (size_t)m.fc.N * 4);
     for (int i = 0; i < m.n_lin; ++i) {
@@ -417,100 +291,6 @@ static void make_infer_plan(const delora_odometry_desc* d, bool streams, InferPl
         p->lin_b[i] = take(off, (size_t)m.lin[i].N * 4);
     }
     p->total = off;
-}
-
-// (img1, img2) fp32 [B, 4, H, W] each -> the trunk input; drop.ctr non-NULL: with the input dropout applied
-static int trunk_input(const Model& m, const Trunk& t, char* ws, const float* img1, const float* img2, int B,
-                       cudaStream_t st, DropoutCtr drop = DropoutCtr{nullptr, 0}) {
-    if (drop.ctr)
-        return m.stem_fast ? launch_images_to_nhwc16_dropout(img1, img2, B, m.H, m.W, ws + t.x_in, drop, st)
-                           : launch_images_to_nhwc_dropout(img1, img2, B, m.H, m.W, 64, ws + t.x_in, drop, st);
-    return m.stem_fast ? delora_images_to_nhwc16_bf16(img1, img2, B, m.H, m.W, ws + t.x_in, st)
-                       : delora_images_to_nhwc_bf16(img1, img2, B, m.H, m.W, 64, ws + t.x_in, st);
-}
-
-// The stage-3 channel dropout, Dropout2d on layer3's output: x, y [B, Hp, Wp, C] bf16, the padded NHWC layout with its
-// halos (pix = Hp * Wp per pair).  y = bf16_rn(float(x) * 1.25f) where (pair b, channel c) is kept (element b * C + c
-// of the stage-3 mask), 0 where it is dropped.  One thread per 8 channels (two Philox words); y may be x.  The forward
-// writes x3d from layer3's output with it; the backward multiplies the data gradient of layer3's output in place.
-__global__ void __launch_bounds__(256)
-odometry_channel_dropout_kernel(const __nv_bfloat16* x, __nv_bfloat16* y, int B, int pix, int C, DropoutCtr drop) {
-    const int groups = C / 8;
-    const size_t total = (size_t)B * pix * groups;
-    const size_t i = (size_t)blockIdx.x * 256 + threadIdx.x;
-    if (i >= total) return;
-    const int c0 = (int)(i % groups) * 8;
-    const int b = (int)(i / ((size_t)groups * pix));
-    uint64_t seed, step;
-    dropout_seed_step(drop, seed, step);
-    const uint64_t e0 = (uint64_t)b * C + c0;              // a multiple of 8: two whole Philox blocks
-    const Philox4 r0 = dropout_words(seed, step, kDropStage3, e0 >> 2);
-    const Philox4 r1 = dropout_words(seed, step, kDropStage3, (e0 >> 2) + 1);
-    const uint32_t words[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-    uint4 v = reinterpret_cast<const uint4*>(x)[i];
-    __nv_bfloat16* h = reinterpret_cast<__nv_bfloat16*>(&v);
-#pragma unroll
-    for (int k = 0; k < 8; ++k)
-        h[k] = dropout_word_keeps(words[k]) ? __float2bfloat16_rn(__bfloat162float(h[k]) * kDropScale)
-                                            : __float2bfloat16_rn(0.0f);
-    reinterpret_cast<uint4*>(y)[i] = v;
-}
-
-static int channel_dropout(const Model& m, const char* x, char* y, int B, DropoutCtr drop, cudaStream_t st) {
-    const int C = m.stage_c[2], pix = (m.stage_h[2] + 2) * (m.stage_w[2] + 2);
-    const size_t total = (size_t)B * pix * (C / 8);
-    odometry_channel_dropout_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(
-        reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<__nv_bfloat16*>(y), B, pix, C, drop);
-    DELORA_CHECK_LAUNCH("odometry_channel_dropout_kernel");
-    return 0;
-}
-
-// The block whose output is layer3's (x3): the last block of stage 2
-static int last_stage3_block(const Model& m) {
-    int i = 0;
-    while (i + 1 < m.n_block && m.block[i + 1].stage <= 2) ++i;
-    return i;
-}
-
-// The trunk from its input to the pooled features.  saving (training): the stem keeps its PRE-activation (fp16 on the
-// 16-channel path) and the max-pool applies the activation and records its argmax; otherwise the stem applies it.
-// drop.ctr non-NULL (a dropout training step): layer3's output x3 stays as it is (the backward's act' reads it), the
-// channel-dropped x3d is written to x3d (a buffer of x3's size) and layer4's first block reads it.
-static int trunk_forward(const Model& m, const Trunk& t, const Weights& w, bool saving, char* ws, int act, int B,
-                         float* pooled, cudaStream_t st, DropoutCtr drop = DropoutCtr{nullptr, 0}, size_t x3d = 0) {
-    int rc;
-    const int H = m.H, W = m.W, stem_act = saving ? 0 : act;
-    char* stem = ws + t.stem;
-    if (m.stem_fast)
-        rc = delora_stem_fprop_bf16(ws + t.x_in, ws + w.w_fwd[0], stem, B, H, W, stem_act, saving ? 1 : 0, st);
-    else
-        rc = delora_conv2d_fprop_bf16(ws + t.x_in, ws + w.w_fwd[0], nullptr, nullptr, stem, B, H, W, 64, 64, 3, 1, 2,
-                                      stem_act, st);
-    if (rc) return rc;
-    if (saving) rc = delora_maxpool_w_idx_nhwc_bf16(stem, B, H, m.w2, 64, ws + t.pool, ws + t.idx, act, m.stem_fast, st);
-    else rc = delora_maxpool_w_nhwc_bf16(stem, B, H, m.w2, 64, ws + t.pool, st);
-    if (rc) return rc;
-    const char* cur = ws + t.pool;
-    for (int i = 0; i < m.n_block; ++i) {
-        const Block& b = m.block[i];
-        char* t1 = ws + t.t1[i];
-        const char* ident = cur;
-        if ((rc = delora_conv2d_fprop_bf16(cur, ws + w.w_fwd[b.c1], nullptr, nullptr, t1, B, b.hin, b.win, b.cin, b.cout,
-                                           3, b.sh, b.sw, act, st))) return rc;
-        if (b.ds >= 0) {
-            ident = ws + t.ds[i];
-            if ((rc = delora_conv2d_fprop_bf16(cur, ws + w.w_fwd[b.ds], nullptr, nullptr, ws + t.ds[i], B, b.hin, b.win,
-                                               b.cin, b.cout, 1, b.sh, b.sw, 0, st))) return rc;
-        }
-        if ((rc = delora_conv2d_fprop_bf16(t1, ws + w.w_fwd[b.c2], ident, nullptr, ws + t.out[i], B, b.hout, b.wout,
-                                           b.cout, b.cout, 3, 1, 1, act, st))) return rc;
-        cur = ws + t.out[i];
-        if (drop.ctr && i == last_stage3_block(m)) {
-            if ((rc = channel_dropout(m, cur, ws + x3d, B, drop, st))) return rc;
-            cur = ws + x3d;
-        }
-    }
-    return delora_avgpool_nhwc_bf16(cur, B, m.stage_h[3], m.stage_w[3], 512, pooled, st);
 }
 
 // Where the tail reads its weights and writes its activations.  Inference: the workspace copies of the weights and two
@@ -665,10 +445,18 @@ static int init_workspace(const Frames& f, size_t total, void* workspace, cudaSt
     return 0;
 }
 
+// The bf16 filters of the weight section w from the fp32 weight blob
+static int prep_blob_weights(const Model& m, const TrunkWeights& w, char* ws, const float* blob, cudaStream_t st,
+                             const char* who) {
+    const float* src[kMaxConv];
+    for (int i = 0; i < m.t.n_conv; ++i) src[i] = blob + m.t.conv[i].blob;
+    return prep_trunk_weights(m.t, w, ws, src, st, who);
+}
+
 static int load_weights(const InferPlan& p, const float* weights, void* workspace, cudaStream_t st, const char* who) {
     char* ws = (char*)workspace;
     const Model& m = p.m;
-    int rc = prep_weights(m, p.w, ws, weights, st, who);
+    int rc = prep_blob_weights(m, p.w, ws, weights, st, who);
     if (rc) return rc;
     auto copy = [&](size_t dst, int64_t src, int64_t n) {
         return cudaMemcpyAsync(ws + dst, weights + src, (size_t)n * sizeof(float), cudaMemcpyDeviceToDevice, st);
@@ -731,8 +519,8 @@ static int run_pairs(const delora_odometry_desc* d, const float* points, const i
     if (factor) rc = project_normalized(p.f, d, ws, points, n_points, B, factor, st);
     else rc = project(p.f, d, ws, points, n_points, nullptr, 2 * B, st);
     if (rc) return rc;
-    if ((rc = trunk_input(p.m, p.t, ws, images, images + (size_t)B * img, B, st))) return rc;
-    if ((rc = trunk_forward(p.m, p.t, p.w, false, ws, d->act, B, pooled_ws, st))) return rc;
+    if ((rc = trunk_input(p.m.t, p.t, ws, images, images + (size_t)B * img, B, st))) return rc;
+    if ((rc = trunk_forward(p.m.t, p.t, ws, p.w, ws, d->act, B, pooled_ws, nullptr, st))) return rc;
     if ((rc = run_tail(p.m, inference_tail_io(p, ws), d->act, pooled_ws, B, T, st, factor))) return rc;
     if (pooled) {
         const cudaError_t e = cudaMemcpyAsync(pooled, pooled_ws, (size_t)B * 512 * sizeof(float), cudaMemcpyDeviceToDevice, st);
@@ -778,8 +566,8 @@ extern "C" int delora_odometry_push(const delora_odometry_desc* d, const float* 
     if ((rc = project(p.f, d, ws, points, n_points, nullptr, 1, st))) return rc;
     if (T) {
         float* pooled_ws = reinterpret_cast<float*>(ws + p.pooled);
-        if ((rc = trunk_input(p.m, p.t, ws, prev, image, 1, st))) return rc;
-        if ((rc = trunk_forward(p.m, p.t, p.w, false, ws, d->act, 1, pooled_ws, st))) return rc;
+        if ((rc = trunk_input(p.m.t, p.t, ws, prev, image, 1, st))) return rc;
+        if ((rc = trunk_forward(p.m.t, p.t, ws, p.w, ws, d->act, 1, pooled_ws, nullptr, st))) return rc;
         if ((rc = run_tail(p.m, inference_tail_io(p, ws), d->act, pooled_ws, 1, T, st))) return rc;
     }
     const cudaError_t e = cudaMemcpyAsync(prev, image, (size_t)4 * d->H * d->W * sizeof(float), cudaMemcpyDeviceToDevice, st);
@@ -932,7 +720,7 @@ extern "C" int delora_odometry_streams_push(const delora_odometry_desc* d, const
     int rc;
     if ((rc = project(p.f, d, ws, points, n_points, active, S, st))) return rc;
     __nv_bfloat16* x_in = reinterpret_cast<__nv_bfloat16*>(ws + p.t.x_in);
-    if (p.m.stem_fast) {
+    if (p.m.t.stem_fast) {
         const size_t n = (size_t)S * (H + 2) * W;
         odometry_streams_input_kernel<16><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(cur, prev, active, S, H, W, x_in);
     } else {
@@ -941,7 +729,7 @@ extern "C" int delora_odometry_streams_push(const delora_odometry_desc* d, const
     }
     DELORA_CHECK_LAUNCH("odometry_streams_input_kernel");
     float* pooled = reinterpret_cast<float*>(ws + p.pooled);
-    if ((rc = trunk_forward(p.m, p.t, p.w, false, ws, d->act, S, pooled, st))) return rc;
+    if ((rc = trunk_forward(p.m.t, p.t, ws, p.w, ws, d->act, S, pooled, nullptr, st))) return rc;
     TailLinear rot, trans;
     if ((rc = run_tail_hidden(p.m, inference_tail_io(p, ws), d->act, pooled, S, &rot, &trans, st))) return rc;
     const int vec = tail_vec(rot) && tail_vec(trans);
@@ -968,9 +756,8 @@ extern "C" int delora_odometry_streams_reset(const delora_odometry_desc* d, cons
 
 // ================================================================================================ training
 // delora_odometry_train_step: projection + normals of the 2B scans (with w_pre > 0: at H x w_pre, then re-projected at
-// H x W by delora_project_grids_fwd), the trunk forward keeping its activations (the
-// kernel sequence of TensorCoreEncoder._forward_saving), the tail forward keeping its activations, the dense ICP
-// losses with dL/dT, the tail backward (below), the trunk backward (TensorCoreEncoder._backward), one Adam update of
+// H x W by delora_project_grids_fwd), the trunk forward keeping its activations (trunk.cuh), the tail forward keeping
+// its activations, the dense ICP losses with dL/dT, the tail backward (below), the trunk backward, one Adam update of
 // the fp32 master blob and one re-prep of the bf16 filters from it.  Weight gradients land in a gradient blob with
 // the layout of the weight blob: the wgrad kernels write each filter at its blob offset ([Cout, Cin, k, k] is both
 // the state_dict layout and theirs), the tail kernels each fc / head tensor at its own.
@@ -1253,22 +1040,15 @@ __global__ void odometry_icp_rearm_kernel(float4* __restrict__ s, long long n4, 
 struct TrainPlan {
     Model m;
     size_t master, grad, adam_m, adam_v, ctr;
-    Weights w;
+    TrunkWeights w;
     Frames f;                          // 2 * max_batch scans, no cached image
     size_t pts_grid, nrm_grid, icp, losses, grad_T, T16, T12;
-    // trunk activations kept by the forward: 16- or 64-channel input, stem pre-activation, pool output + argmax,
-    // per block conv1 output and block output, per downsampling block the downsample output
-    Trunk t;
+    TrunkActs t;                       // the trunk's saving buffers
     // w_pre > 0 only: the preprocessing projection of the 2 * max_batch scans at H x w_pre (image, index map and the
     // dense grids with their normals), placed after every other buffer
     size_t pre_image, pre_index_map, pre_pts_grid, pre_nrm_grid;
-    // trunk backward: per stage two alternating data-gradient buffers + the conv1 gradient; strided blocks: the
-    // downsample's gradient at the output size and (zero-upsample path) the upsampled conv1 gradient
-    size_t g[4][3], gds[4], gu1[4], g_stem;
-    int phase_dgrad[kMaxBlocks];
     // tail activations and gradients
     size_t pooled, fc_out, hid[kMaxLinear], raw, dz_hid[kMaxLinear], dz_fc, g_pooled;
-    size_t wg_scratch;
     size_t total;
 };
 
@@ -1282,7 +1062,7 @@ static void make_train_plan(const delora_odometry_desc* d, TrainPlan* tp) {
     tp->master = take(off, blob); tp->grad = take(off, blob); tp->adam_m = take(off, blob); tp->adam_v = take(off, blob);
     // [0] Adam's step count, [1] the ICP scratch's batch size, [2] the dropout seed (the slot has 256 bytes)
     tp->ctr = take(off, 3 * sizeof(long long));
-    tp->w = plan_weights(m, true, off);
+    tp->w = plan_trunk_weights(m.t, true, off);
     // one key buffer serves both projections of a step, one after the other
     tp->f = plan_frames(d, 2 * MB, 0, false, d->w_pre > W ? d->w_pre : W, off);
     tp->pts_grid = take(off, (size_t)2 * MB * HW * 16);
@@ -1292,26 +1072,7 @@ static void make_train_plan(const delora_odometry_desc* d, TrainPlan* tp) {
     tp->grad_T = take(off, (size_t)MB * 12 * 4);
     tp->T16 = take(off, (size_t)MB * 16 * 4);
     tp->T12 = take(off, (size_t)MB * 12 * 4);
-    tp->t.x_in = take(off, nhwc_bytes(MB, H, W, m.stem_fast ? 16 : 64));
-    tp->t.stem = take(off, nhwc_bytes(MB, H, m.w2, 64));
-    tp->t.pool = take(off, nhwc_bytes(MB, H, m.w4, 64));
-    tp->t.idx = take(off, (size_t)MB * H * m.w4 * 64);
-    for (int i = 0; i < m.n_block; ++i) {
-        const Block& b = m.block[i];
-        tp->t.t1[i] = take(off, nhwc_bytes(MB, b.hout, b.wout, b.cout));
-        tp->t.out[i] = take(off, nhwc_bytes(MB, b.hout, b.wout, b.cout));
-        if (b.ds >= 0) tp->t.ds[i] = take(off, nhwc_bytes(MB, b.hout, b.wout, b.cout));
-    }
-    for (int s = 0; s < 4; ++s)
-        for (int j = 0; j < 3; ++j) tp->g[s][j] = take(off, nhwc_bytes(MB, m.stage_h[s], m.stage_w[s], m.stage_c[s]));
-    for (int i = 0; i < m.n_block; ++i) {
-        const Block& b = m.block[i];
-        tp->phase_dgrad[i] = b.ds >= 0 && i > 0 && delora_conv2d_dgrad_eligible(b.cin, b.cout, b.win, b.sh, b.sw);
-        if (b.ds < 0) continue;
-        tp->gds[b.stage] = take(off, nhwc_bytes(MB, b.hout, b.wout, b.cin));
-        if (!tp->phase_dgrad[i]) tp->gu1[b.stage] = take(off, nhwc_bytes(MB, b.hin, b.win, b.cout));
-    }
-    tp->g_stem = take(off, nhwc_bytes(MB, H, m.w2, 64));
+    tp->t = plan_trunk_acts(m.t, MB, true, off);
     tp->pooled = take(off, (size_t)MB * 512 * 4);
     tp->g_pooled = take(off, (size_t)MB * 512 * 4);
     tp->fc_out = take(off, (size_t)MB * nout * 4);
@@ -1326,21 +1087,6 @@ static void make_train_plan(const delora_odometry_desc* d, TrainPlan* tp) {
             tp->dz_hid[i] = take(off, (size_t)MB * m.lin[i].N * 4);
         }
     }
-    // one split-K scratch for every wgrad launch: the largest need at max_batch (the need grows with B)
-    int64_t wg = m.stem_fast ? delora_stem_wgrad_scratch_floats(MB, H, W)
-                             : delora_conv2d_wgrad_scratch_floats(MB, H, m.w2, 64, 64, 3);
-    for (int i = 0; i < m.n_block; ++i) {
-        const Block& b = m.block[i];
-        int64_t n = delora_conv2d_wgrad_scratch_floats(MB, b.hout, b.wout, b.cin, b.cout, 3);
-        wg = n > wg ? n : wg;
-        n = delora_conv2d_wgrad_scratch_floats(MB, b.hout, b.wout, b.cout, b.cout, 3);
-        wg = n > wg ? n : wg;
-        if (b.ds >= 0) {
-            n = delora_conv2d_wgrad_scratch_floats(MB, b.hout, b.wout, b.cin, b.cout, 1);
-            wg = n > wg ? n : wg;
-        }
-    }
-    tp->wg_scratch = take(off, (size_t)wg * 4);
     if (d->w_pre > 0) {
         const size_t HWp = (size_t)H * d->w_pre;
         tp->pre_image = take(off, (size_t)2 * MB * 4 * HWp * 4);
@@ -1374,78 +1120,6 @@ static int check_train_params(const delora_odometry_train_params* hp, const char
                      (double)hp->epsilon_range);
     DELORA_CHECK_ARG(hp->min_neighbors >= 0, "%s: min_neighbors=%d must be >= 0", who, hp->min_neighbors);
     return 0;
-}
-
-// drop.ctr non-NULL (a dropout training step): layer4's first block read x3d (in g[2][2], see the step), so its two
-// weight gradients read it too, while its act' epilogue reads x3; the data gradient of x3 is then multiplied by
-// keep * 1.25 in place (one more bf16 rounding).  g[2][2] is first written by layer3's own backward, after that.
-static int train_trunk_backward(const TrainPlan& tp, char* ws, int act, int B, cudaStream_t st,
-                                DropoutCtr drop = DropoutCtr{nullptr, 0}) {
-    const Model& m = tp.m;
-    const int x3_block = last_stage3_block(m);
-    int rc;
-    const int act_bwd = act == 1 ? 4 : 3;                 // ACT_RELU_BWD / ACT_TANH_BWD: multiply by act'(saved)
-    float* grad = reinterpret_cast<float*>(ws + tp.grad);
-    float* scratch = reinterpret_cast<float*>(ws + tp.wg_scratch);
-    const int L = m.n_block - 1;
-    char* dz2 = ws + tp.g[3][0];
-    if ((rc = delora_avgpool_bwd_nhwc_bf16(reinterpret_cast<const float*>(ws + tp.g_pooled), ws + tp.t.out[L], B,
-                                           m.stage_h[3], m.stage_w[3], 512, act, dz2, st))) return rc;
-    for (int i = L; i >= 0; --i) {
-        const Block& b = m.block[i];
-        const int s = b.stage;
-        const char* x = i == 0 ? ws + tp.t.pool : ws + tp.t.out[i - 1];
-        // the input the forward's convolutions read: x3d for layer4's first block in a dropout step
-        const bool reads_x3d = drop.ctr && i == x3_block + 1;
-        const char* xin = reads_x3d ? ws + tp.g[2][2] : x;
-        char* dz1 = ws + tp.g[s][2];
-        // the data gradient of the block input: the other buffer of this stage, or a buffer of the previous stage
-        char* next;
-        if (i > 0 && m.block[i - 1].stage != s) next = ws + tp.g[m.block[i - 1].stage][0];
-        else next = (dz2 == ws + tp.g[s][0]) ? ws + tp.g[s][1] : ws + tp.g[s][0];
-        if ((rc = delora_conv2d_wgrad_bf16(ws + tp.t.t1[i], dz2, grad + m.conv[b.c2].blob, scratch, B, b.hout, b.wout, b.cout,
-                                           b.cout, b.cout, 3, 1, 1, st))) return rc;
-        if ((rc = delora_conv2d_fprop_bf16(dz2, ws + tp.w.w_flip[b.c2], nullptr, ws + tp.t.t1[i], dz1, B, b.hout, b.wout, b.cout,
-                                           b.cout, 3, 1, 1, act_bwd, st))) return rc;
-        if ((rc = delora_conv2d_wgrad_bf16(xin, dz1, grad + m.conv[b.c1].blob, scratch, B, b.hin, b.win, b.cin, b.cin, b.cout,
-                                           3, b.sh, b.sw, st))) return rc;
-        const char* resid = dz2;
-        const char* src = dz1;
-        if (b.ds >= 0) {
-            if ((rc = delora_conv2d_wgrad_bf16(xin, dz2, grad + m.conv[b.ds].blob, scratch, B, b.hin, b.win, b.cin, b.cin,
-                                               b.cout, 1, b.sh, b.sw, st))) return rc;
-            // the 1x1 strided downsample's data gradient: 1x1 convolution of the small dz, scattered afterwards
-            char* small = ws + tp.gds[s];
-            if ((rc = delora_conv2d_fprop_bf16(dz2, ws + tp.w.w_flip[b.ds], nullptr, nullptr, small, B, b.hout, b.wout, b.cout,
-                                               b.cin, 1, 1, 1, 0, st))) return rc;
-            if (tp.phase_dgrad[i]) {
-                if ((rc = delora_conv2d_dgrad_bf16(dz1, ws + tp.w.w_flip[b.c1], small, x, next, B, b.hin, b.win, b.cin, b.cout,
-                                                   b.sh, b.sw, act_bwd, 1, st))) return rc;
-                if (reads_x3d && (rc = channel_dropout(m, next, next, B, drop, st))) return rc;
-                dz2 = next;
-                continue;
-            }
-            char* up_resid = ws + tp.g[m.block[i - 1].stage][1];
-            char* up_src = ws + tp.gu1[s];
-            if ((rc = delora_zero_upsample_nhwc_bf16(small, B, b.hout, b.wout, b.cin, b.sh, b.sw, b.hin, b.win, up_resid, st)))
-                return rc;
-            if ((rc = delora_zero_upsample_nhwc_bf16(dz1, B, b.hout, b.wout, b.cout, b.sh, b.sw, b.hin, b.win, up_src, st)))
-                return rc;
-            resid = up_resid;
-            src = up_src;
-        }
-        // i > 0: the block input is the previous block's activation output, act' folds into the epilogue; the first
-        // block reads the max-pool output (ACT_NONE: the pool's backward applies the stem's act')
-        if ((rc = delora_conv2d_fprop_bf16(src, ws + tp.w.w_flip[b.c1], resid, i > 0 ? x : nullptr, next, B, b.hin, b.win,
-                                           b.cout, b.cin, 3, 1, 1, i > 0 ? act_bwd : 0, st))) return rc;
-        if (reads_x3d && (rc = channel_dropout(m, next, next, B, drop, st))) return rc;
-        dz2 = next;
-    }
-    if ((rc = delora_maxpool_w_bwd_nhwc_bf16(dz2, ws + tp.t.idx, ws + tp.t.stem, B, m.H, m.w2, 64, 4 + act, ws + tp.g_stem,
-                                             m.stem_fast, st))) return rc;
-    if (m.stem_fast)
-        return delora_stem_wgrad_bf16(ws + tp.t.x_in, ws + tp.g_stem, grad, scratch, B, m.H, m.W, 8, st);
-    return delora_conv2d_wgrad_bf16(ws + tp.t.x_in, ws + tp.g_stem, grad, scratch, B, m.H, m.W, 64, 8, 64, 3, 1, 2, st);
 }
 
 static TailIO train_tail_io(const TrainPlan& tp, char* ws) {
@@ -1559,7 +1233,7 @@ extern "C" int delora_odometry_train_init(const delora_odometry_desc* d, const f
     const cudaError_t e = cudaMemcpyAsync(ws + tp.master, weights, (size_t)tp.m.blob_floats * 4, cudaMemcpyDeviceToDevice,
                                           st);
     DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
-    return prep_weights(tp.m, tp.w, ws, reinterpret_cast<const float*>(ws + tp.master), st, who);
+    return prep_blob_weights(tp.m, tp.w, ws, reinterpret_cast<const float*>(ws + tp.master), st, who);
 }
 
 extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
@@ -1621,10 +1295,9 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
                                                 st))) {
         return rc;
     }
-    // 2. forward, keeping the activations.  Dropout: x3d goes to the stage-3 backward buffer g[2][2], which nothing
-    // writes before layer3's own backward
-    if ((rc = trunk_input(m, tp.t, ws, images, images + (size_t)B * 4 * HW, B, st, drop_fwd))) return rc;
-    if ((rc = trunk_forward(m, tp.t, tp.w, true, ws, d->act, B, f(tp.pooled), st, drop_fwd, tp.g[2][2]))) return rc;
+    // 2. forward, keeping the activations
+    if ((rc = trunk_input(m.t, tp.t, ws, images, images + (size_t)B * 4 * HW, B, st, drop_fwd))) return rc;
+    if ((rc = trunk_forward(m.t, tp.t, ws, tp.w, ws, d->act, B, f(tp.pooled), nullptr, st, drop_fwd))) return rc;
     if ((rc = run_tail(m, train_tail_io(tp, ws), d->act, f(tp.pooled), B, f(tp.T16), st, nullptr, drop_fwd))) return rc;
     // 3. ICP losses and dL/dT: source = scan_2 moved by T, target = scan_1.  The identity fit still runs them: the
     // reference logs the ICP losses in that phase too
@@ -1647,7 +1320,10 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
     }
     // 4. backward: tail (dL/dT of the ICP mean or of the identity fit), average pool, trunk
     if ((rc = train_tail_backward(tp, ws, d->act, B, identity, st, drop_bwd))) return rc;
-    if ((rc = train_trunk_backward(tp, ws, d->act, B, st, drop_bwd))) return rc;
+    float* conv_dw[kMaxConv];
+    for (int i = 0; i < m.t.n_conv; ++i) conv_dw[i] = f(tp.grad) + m.t.conv[i].blob;
+    for (int s = 3; s >= 0; --s)
+        if ((rc = trunk_backward(m.t, tp.t, ws, tp.w, ws, d->act, B, f(tp.g_pooled), conv_dw, s, st, drop_bwd))) return rc;
     // outputs (T: the weights before the update)
     auto out = [&](float* dst, size_t src, size_t n) {
         if (dst && e == cudaSuccess) e = cudaMemcpyAsync(dst, ws + src, n * sizeof(float), cudaMemcpyDeviceToDevice, st);
@@ -1664,7 +1340,7 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
     odometry_adam_kernel<<<grid, 256, 0, st>>>(f(tp.master), f(tp.grad), f(tp.adam_m), f(tp.adam_v), n, ctr, hp->lr, hp->beta1,
                                                hp->beta2, hp->eps);
     DELORA_CHECK_LAUNCH("odometry_adam_kernel");
-    return delora_conv_weight_prep_multi(ws + tp.w.table, m.n_conv, st);
+    return delora_conv_weight_prep_multi(ws + tp.w.table, m.t.n_conv, st);
 }
 
 extern "C" int delora_odometry_train_weights(const delora_odometry_desc* d, const void* workspace, float* weights,
@@ -1726,7 +1402,7 @@ extern "C" int delora_odometry_train_set_state(const delora_odometry_desc* d, co
     in(tp.ctr, step, sizeof(long long));            // ctr[0] only: ctr[1], the ICP scratch's batch size, stays
     DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
     // the bf16 filters from the new master weights, through the table _train_init wrote
-    return delora_conv_weight_prep_multi(ws + tp.w.table, tp.m.n_conv, st);
+    return delora_conv_weight_prep_multi(ws + tp.w.table, tp.m.t.n_conv, st);
 }
 
 // ================================================================================================ dropout

@@ -1,34 +1,34 @@
 """Encoder forward and backward on the wgmma convolution kernels.
 
-Takes the weights of an `OdometryModel` (reference parameter names) and runs
-`ResNetModified._forward_impl` (reference: src/models/resnet_modified.py:95-120, BasicBlock :159-177)
-as a chain of `delora_conv2d_fprop_bf16` launches on NHWC bf16 activations with materialised
-circular-W / zero-H padding: stem 3x3 s(1,2) + tanh, 3x3/(1,2) max-pool, 4 stages x 2 BasicBlocks
-(second conv fuses residual add + activation, 1x1 strided downsample convs), then average pool,
-`fc` and the two MLP heads (tiny GEMMs, left to torch as SURVEY.md §7.6 allows).
+Takes the weights of an `OdometryModel` (reference parameter names) and runs `ResNetModified._forward_impl`
+(reference: src/models/resnet_modified.py:95-120, BasicBlock :159-177) through the trunk entry points of the C ABI:
+`delora_trunk_forward` runs stem, max-pool, the BasicBlocks and the average pool in the launch sequence of
+csrc/trunk.cu, the one the odometry entry points run as well.  `fc` and the two MLP heads (tiny GEMMs) are left to
+torch, as SURVEY.md §7.6 allows.
 
-Training (`pooled_features`, an autograd Function) keeps the activations and runs the backward as
-dgrad (the same fprop kernel on the output gradient with flipped filters, act' fused in the epilogue)
-and wgrad (split-K over pixels) launches.  Any image size works (ragged tiles are zero-filled /
-masked): 64x2048 tiles exactly, KITTI's 64x720 runs 360 -> 180 -> 90 -> 45 -> 23 wide.
+Training (`pooled_features`, an autograd Function) keeps the activations and runs the backward as one
+`delora_trunk_backward` call per stage.  Any image size the trunk takes works (ragged tiles are zero-filled / masked):
+64x2048 tiles exactly, KITTI's 64x720 runs 360 -> 180 -> 90 -> 45 -> 23 wide.
 """
+import ctypes
+
 import torch
 
-from .. import ops
+from .. import _lib, ops
+
+_STAGE_CHANNELS = (64, 128, 256, 512)
+_STAGE_STRIDES = ((1, 1), (1, 2), (1, 2), (2, 2))
 
 
 class _EncoderTrainFn(torch.autograd.Function):
-    """Differentiable encoder trunk on the wgmma kernels: images -> pooled [B, C4] features.
-    forward = TensorCoreEncoder chain with the activations kept; backward = per BasicBlock (reverse order)
-    wgrad(conv2), dgrad(conv2) * act'(t1), wgrad(conv1), [wgrad + dgrad of the 1x1 downsample],
-    dgrad(conv1) + identity path, * act'(block input); then max-pool and stem.  The gradients w.r.t. the
+    """Differentiable encoder trunk on the wgmma kernels: images -> pooled [B, C4] features.  The gradients w.r.t. the
     images are not needed (the range images are data)."""
 
     @staticmethod
     def forward(ctx, enc, image_1, image_2, *weights):
         ctx.enc = enc
-        ctx.state = enc._forward_saving(image_1, image_2, weights)
-        return ctx.state["pooled"]
+        ctx.state, pooled = enc._forward_saving(image_1, image_2)
+        return pooled
 
     @staticmethod
     def backward(ctx, g_pooled):
@@ -36,7 +36,7 @@ class _EncoderTrainFn(torch.autograd.Function):
             raise RuntimeError("tensor-core encoder: backward called twice on the same forward (saved activations "
                                "were released); run the forward again")
         grads = ctx.enc._backward(ctx.state, g_pooled.float().contiguous())
-        ctx.state["slot"].release()
+        ctx.state[0].release()
         ctx.state = None
         if ctx.enc.grad_views is not None:
             # the kernels wrote the weight gradients into the synchroniser's flat buffer and announced them
@@ -47,13 +47,14 @@ class _EncoderTrainFn(torch.autograd.Function):
 
 
 class _Slot:
-    """One set of saved-activation buffers.  A grad-enabled forward takes the lowest free slot and keeps it until its
-    backward has run (or its graph is dropped), so a second forward before the first backward -- gradient
-    accumulation, two model calls in one step, a loss pass interleaved with training -- never overwrites tensors an
-    earlier graph still needs."""
+    """One set of saved-activation workspaces (one per (device, B, H, W)).  A grad-enabled forward takes the lowest free
+    slot and keeps it until its backward has run (or its graph is dropped), so a second forward before the first
+    backward -- gradient accumulation, two model calls in one step, a loss pass interleaved with training -- never
+    overwrites tensors an earlier graph still needs."""
 
     def __init__(self, index):
         self.index, self.busy = index, False
+        self.acts = {}
 
 
 class _SlotLease:
@@ -82,91 +83,68 @@ class TensorCoreEncoder:
         if r.conv1.weight.shape[0] % 64 != 0:
             raise Exception("tensor-core encoder needs channel counts that are multiples of 64 "
                             "(factor_fewer_resnet_channels = 1)")
-        self.blocks = []
-        for li in range(1, 5):
-            for blk in getattr(r, f"layer{li}"):
-                stride = blk.stride if isinstance(blk.stride, tuple) else (blk.stride, blk.stride)
-                self.blocks.append({"has_wd": blk.downsample is not None, "stride": stride,
-                                    "cout": blk.conv1.weight.shape[0]})
-        # persistent bf16 copies of the filters in the two layouts the kernels read (fprop / dgrad); rewritten by one
-        # small kernel per layer whenever the fp32 parameters change (every training step; after load_state_dict)
-        self._wbufs = None
-        self._wversion = None
-        self._wtable = None
-        self._buf = {}
+        stages = [getattr(r, f"layer{li}") for li in range(1, 5)]
+        self.layers = (ctypes.c_int * 4)(*[len(s) for s in stages])
+        # trunk_parameters() indices of each stage's filters in the order its backward finishes them (last block
+        # first); the stem's gradient comes with stage 0's
+        self._stage_params, idx = [], 1
+        for s in stages:
+            per_block = []
+            for blk in s:
+                n = 3 if blk.downsample is not None else 2
+                per_block.append(list(range(idx, idx + n)))
+                idx += n
+            self._stage_params.append([i for blk in reversed(per_block) for i in blk])
+        self._stage_params[0].append(0)
+        # bf16 weight sections, one per stem layout met (W % 2): [section, W, (versions, pointers) it was prepped from];
+        # rewritten by one small kernel whenever the fp32 parameters change (every training step; after load_state_dict)
+        self._weights = {}
+        self._acts = {}          # inference activation workspaces by (device, B, H, W)
         self._slots = []
         # data-parallel hook (parallel_grad.BucketedGradAllReduce): weight gradients are written into these views
-        # (trunk_parameters() order) and every finished group is announced through grad_ready(list of indices)
+        # (trunk_parameters() order) and every finished stage is announced through grad_ready(list of indices)
         self.grad_views = None
         self.grad_ready = None
-        idx, self._block_param_idx = 1, []
-        for blk in self.blocks:
-            n = 3 if blk["has_wd"] else 2
-            self._block_param_idx.append(list(range(idx, idx + n)))
-            idx += n
 
-    def _weight_buffers(self):
+    def _prep(self, entry, force):
         params = self.trunk_parameters()
-        if self._wbufs is None or self._wbufs[0][0].device != params[0].device:
-            bufs = []
-            for i, p_ in enumerate(params):
-                cout, cin, k, _ = p_.shape
-                cin_pad = 64 if i == 0 else cin
-                fwd = torch.empty((cout, k * k, cin_pad), dtype=torch.bfloat16, device=p_.device)
-                flip = None if i == 0 else torch.empty((cin, k * k, cout), dtype=torch.bfloat16, device=p_.device)
-                bufs.append((fwd, flip, cin_pad))
-            # stem in the 16-channel layout of csrc/conv_stem.cu (used when the image width is even)
-            self._wstem = torch.empty((3, 64, 64), dtype=torch.bfloat16, device=params[0].device)
-            self._wbufs, self._wversion, self._wtable = bufs, None, None
-        return params, self._wbufs
-
-    def _stem_fast(self, w):
-        p0 = self.model.resnet.conv1.weight
-        return w % 2 == 0 and p0.shape[0] == 64 and p0.shape[1] <= 16
-
-    def _refresh_weights(self, force=False):
-        """-> list of (w_fwd, w_flip) per trunk parameter, up to date with the fp32 parameters: ONE launch rewrites
-        every bf16 filter copy (delora_conv_weight_prep_multi; the pointer table is rebuilt only if a parameter moved)."""
-        params, bufs = self._weight_buffers()
-        ptrs = tuple(p_.data_ptr() for p_ in params)
-        version = tuple(p_._version for p_ in params) + ptrs
-        if force or version != self._wversion:
-            if self._wtable is None or self._wtable[1] != ptrs:
-                rows = []
-                for p_, (fwd, flip, cin_pad) in zip(params, bufs):
-                    cout, cin, k, _ = p_.shape
-                    rows.append([p_.data_ptr(), fwd.data_ptr(), flip.data_ptr() if flip is not None else 0, cout, cin, k,
-                                 cin_pad, 0])
-                p0 = params[0]
-                if p0.shape[0] == 64 and p0.shape[1] <= 16:
-                    rows.append([p0.data_ptr(), self._wstem.data_ptr(), 0, 64, p0.shape[1], 3, 16, 1])
-                table = torch.tensor(rows, dtype=torch.int64).to(params[0].device)
-                self._wtable = (table, ptrs, len(rows))
+        version = tuple(p_._version for p_ in params) + tuple(p_.data_ptr() for p_ in params)
+        if force or version != entry[2]:
             for p_ in params:
                 if p_.dtype != torch.float32 or not p_.is_contiguous():
                     raise Exception("tensor-core encoder: convolution weights must be contiguous fp32")
-            ops.conv_weight_prep_multi(self._wtable[0], self._wtable[2])
-            self._wversion = version
-        return bufs
+            filters = (ctypes.c_void_p * len(params))(*[p_.data_ptr() for p_ in params])
+            _lib.check(_lib.lib().delora_trunk_prep_weights(self.layers, entry[1], filters,
+                                                            ops._req(entry[0], torch.uint8, "weights"), ops._stream()),
+                       "delora_trunk_prep_weights")
+            entry[2] = version
+        return entry[0]
 
-    def _block_weights(self, bufs):
-        """Regroup the flat per-parameter list into (stem, [per block dict])."""
-        it = iter(bufs)
-        stem = next(it)
-        out = []
-        for blk in self.blocks:
-            w1, w2 = next(it), next(it)
-            wd = next(it) if blk["has_wd"] else None
-            out.append({"w1": w1, "w2": w2, "wd": wd})
-        return stem, out
+    def _prepped_weights(self, w, force=False):
+        """-> the weight section for images w wide, up to date with the fp32 parameters."""
+        dev = self.model.resnet.conv1.weight.device
+        entry = self._weights.get(w % 2)
+        if entry is None or entry[0].device != dev:
+            n = int(_lib.lib().delora_trunk_weight_bytes(self.layers, w))
+            _lib.check(int(n < 0), "delora_trunk_weight_bytes")
+            entry = [torch.empty((n,), dtype=torch.uint8, device=dev), w, None]
+            self._weights[w % 2] = entry
+        return self._prep(entry, force)
 
-    def _buffer(self, tag, b, h, w, c, device, slot=0):
-        key = (str(device), slot, tag, b, h, w, c)
-        t = self._buf.get(key)
-        if t is None:
-            t = ops.padded_nhwc_zeros(b, h, w, c, device)      # halo rows stay zero forever
-            self._buf[key] = t
-        return t
+    def _refresh_weights(self):
+        """Bring every weight section up to date with the fp32 parameters (one launch each, none when unchanged)."""
+        for entry in self._weights.values():
+            self._prep(entry, False)
+
+    def _workspace(self, cache, b, h, w, saving, device):
+        key = (device, b, h, w)
+        acts = cache.get(key)
+        if acts is None:
+            n = int(_lib.lib().delora_trunk_activation_bytes(self.layers, b, h, w, saving))
+            _lib.check(int(n < 0), "delora_trunk_activation_bytes")
+            acts = torch.zeros((n,), dtype=torch.uint8, device=device)      # halo rows stay zero forever
+            cache[key] = acts
+        return acts
 
     def _take_slot(self):
         for sl in self._slots:
@@ -176,50 +154,41 @@ class TensorCoreEncoder:
         self._slots.append(sl)
         return _SlotLease(sl)
 
+    def _trunk_forward(self, image_1, image_2, weights, acts, saving, stage_out=None):
+        b, _, h, w = image_1.shape
+        pooled = torch.empty((b, _STAGE_CHANNELS[-1]), dtype=torch.float32, device=image_1.device)
+        _lib.check(_lib.lib().delora_trunk_forward(
+            self.layers, b, h, w, self.act, saving, ops._req(image_1, torch.float32, "image_1"),
+            ops._req(image_2, torch.float32, "image_2"), weights.data_ptr(), acts.data_ptr(), pooled.data_ptr(),
+            stage_out, ops._stream()), "delora_trunk_forward")
+        return pooled
+
     @torch.no_grad()
+    def _infer(self, image_1, image_2):
+        """-> ([x1, x2, x3, x4] as (padded NHWC bf16 view into the inference workspace, H, W), pooled [B, 512])."""
+        image_1, image_2 = image_1.float().contiguous(), image_2.float().contiguous()
+        b, _, h, w = image_1.shape
+        weights = self._prepped_weights(w)
+        acts = self._workspace(self._acts, b, h, w, 0, image_1.device)
+        out = (ctypes.c_void_p * 4)()
+        pooled = self._trunk_forward(image_1, image_2, weights, acts, 0, out)
+        feats = []
+        sh, sw = h, ops.conv_out_size(w, 2) // 2
+        for s, (c, (st_h, st_w)) in enumerate(zip(_STAGE_CHANNELS, _STAGE_STRIDES)):
+            sh, sw = ops.conv_out_size(sh, st_h), ops.conv_out_size(sw, st_w)
+            off = out[s] - acts.data_ptr()
+            n = b * (sh + 2) * (sw + 2) * c * 2
+            feats.append((acts[off:off + n].view(torch.bfloat16).view(b, sh + 2, sw + 2, c), sh, sw))
+        return feats, pooled
+
     def features(self, image_1, image_2):
         """-> [x1, x2, x3, x4] as padded NHWC bf16 + their (H, W)."""
-        b, _, h, w = image_1.shape
-        dev = image_1.device
-        stem_w, blk_w = self._block_weights(self._refresh_weights())
-        w2 = ops.conv_out_size(w, 2)
-        if self._stem_fast(w):
-            x = ops.images_to_nhwc16(image_1.float().contiguous(), image_2.float().contiguous())
-            y = ops.stem_fprop(x, self._wstem, h, w, self.act, self._buffer("stem", b, h, w2, 64, dev))
-        else:
-            x = ops.images_to_nhwc(image_1.float().contiguous(), image_2.float().contiguous(), 64)
-            y = ops.conv2d_fprop(x, stem_w[0], h, w, 3, (1, 2), self.act, None, self._buffer("stem", b, h, w2, 64, dev))
-        w4 = w2 // 2
-        cur = self._buffer("pool", b, h, w4, 64, dev)
-        L = ops._lib.lib()
-        ops._lib.check(L.delora_maxpool_w_nhwc_bf16(y.data_ptr(), b, h, w2, 64, cur.data_ptr(), ops._stream()),
-                       "delora_maxpool_w_nhwc_bf16")
-        ch, cw = h, w4
-        feats = []
-        for i, blk in enumerate(self.blocks):
-            sh, sw = blk["stride"]
-            oh, ow, co = ops.conv_out_size(ch, sh), ops.conv_out_size(cw, sw), blk["cout"]
-            bw = blk_w[i]
-            t1 = ops.conv2d_fprop(cur, bw["w1"][0], ch, cw, 3, (sh, sw), self.act, None,
-                                  self._buffer(f"b{i}a", b, oh, ow, co, dev))
-            if bw["wd"] is not None:
-                ident = ops.conv2d_fprop(cur, bw["wd"][0], ch, cw, 1, (sh, sw), ops.ACT_NONE, None,
-                                         self._buffer(f"b{i}d", b, oh, ow, co, dev))
-            else:
-                ident = cur
-            cur = ops.conv2d_fprop(t1, bw["w2"][0], oh, ow, 3, (1, 1), self.act, ident,
-                                   self._buffer(f"b{i}o", b, oh, ow, co, dev))
-            ch, cw = oh, ow
-            if i % 2 == 1:
-                feats.append((cur, ch, cw))
-        return feats
+        return self._infer(image_1, image_2)[0]
 
     @torch.no_grad()
     def forward(self, image_1, image_2):
         """(translation [B,3], quaternion [B,4]) like OdometryModel.forward (src/models/model.py:103-116)."""
-        feats = self.features(image_1, image_2)
-        x4, h4, w4 = feats[-1]
-        pooled = ops.avgpool(x4, h4, w4)                                          # AdaptiveAvgPool2d((1,1))
+        pooled = self._infer(image_1, image_2)[1]                                # AdaptiveAvgPool2d((1,1))
         m = self.model
         out = m.resnet.fc(pooled)
         if m.config["use_single_mlp_at_output"]:
@@ -232,7 +201,7 @@ class TensorCoreEncoder:
     # ------------------------------------------------------------------------------------------
     # training path (forward keeps activations, backward runs dgrad / wgrad on the tensor cores)
     def trunk_parameters(self):
-        """Conv weights in the fixed order used by the autograd function."""
+        """Conv weights in the fixed order used by the autograd function (the trunk ABI's filter order)."""
         r = self.model.resnet
         params = [r.conv1.weight]
         for li in range(1, 5):
@@ -245,148 +214,37 @@ class TensorCoreEncoder:
     def trunk_parameter_groups(self):
         """Trunk parameter indices grouped in the order the backward finishes them: layer4, layer3, layer2,
         layer1 + stem (the last, exposed bucket is the smallest: 0.15 M parameters)."""
-        nb = len(self.blocks)
-        per_layer = nb // 4 if nb % 4 == 0 and nb >= 4 else None
-        if per_layer is None:
-            return [[i for blk in reversed(self._block_param_idx) for i in blk] + [0]]
-        def blocks(lo, hi):
-            return [i for b in range(hi - 1, lo - 1, -1) for i in self._block_param_idx[b]]
-        return [blocks(3 * per_layer, nb), blocks(2 * per_layer, 3 * per_layer), blocks(per_layer, 2 * per_layer),
-                blocks(0, per_layer) + [0]]
-
-    def _gout(self, index):
-        return self.grad_views[index] if self.grad_views is not None else None
-
-    def _announce(self, indices):
-        if self.grad_ready is not None:
-            self.grad_ready(indices)
+        return [list(self._stage_params[s]) for s in (3, 2, 1, 0)]
 
     def pooled_features(self, image_1, image_2):
         """[B, C4] average-pooled encoder features with autograd through the wgmma kernels."""
         return _EncoderTrainFn.apply(self, image_1.float().contiguous(), image_2.float().contiguous(),
                                      *self.trunk_parameters())
 
-    def _forward_saving(self, image_1, image_2, weights):
+    def _forward_saving(self, image_1, image_2):
         b, _, h, w = image_1.shape
-        dev = image_1.device
-        L = ops._lib.lib()
-        it = iter(weights)
-        slot = self._take_slot()
-        sid = slot.index
-        st = {"B": b, "H": h, "W": w, "blocks": [], "slot": slot}
-        w_stem = next(it)
-        stem_w, blk_w = self._block_weights(self._refresh_weights(force=True))    # bf16 filters of THIS step's weights
-        w2 = ops.conv_out_size(w, 2)
-        st["stem_fast"] = self._stem_fast(w)
-        # the stem stores its PRE-activation z; the pool applies the activation to the maximum (tanh / relu are
-        # monotonic) and the backward evaluates act'(z) from z (exact for saturated units, see maxpool_bwd_act_kernel)
-        if st["stem_fast"]:
-            st["x_in"] = ops.images_to_nhwc16(image_1, image_2)
-            st["y0"] = ops.stem_fprop(st["x_in"], self._wstem, h, w, ops.ACT_NONE, self._buffer("t_stem", b, h, w2, 64, dev, sid),
-                                      out_f16=True)       # fp16 pre-activation: only the two pool kernels read it
-        else:
-            st["x_in"] = ops.images_to_nhwc(image_1, image_2, 64)
-            st["y0"] = ops.conv2d_fprop(st["x_in"], stem_w[0], h, w, 3, (1, 2), ops.ACT_NONE, None,
-                                        self._buffer("t_stem", b, h, w2, 64, dev, sid))
-        w4 = w2 // 2
-        st["p0"] = self._buffer("t_pool", b, h, w4, 64, dev, sid)
-        st["idx"] = torch.empty((b, h, w4, 64), dtype=torch.uint8, device=dev)
-        ops._lib.check(L.delora_maxpool_w_idx_nhwc_bf16(st["y0"].data_ptr(), b, h, w2, 64, st["p0"].data_ptr(),
-                                                        st["idx"].data_ptr(), 1 if self.act == ops.ACT_RELU else 2,
-                                                        1 if st["stem_fast"] else 0, ops._stream()),
-                       "delora_maxpool_w_idx_nhwc_bf16")
-        cur, ch, cw = st["p0"], h, w4
-        for i, blk in enumerate(self.blocks):
-            w1, wc2 = next(it), next(it)
-            wd = next(it) if blk["has_wd"] else None
-            bw = blk_w[i]
-            sh, sw = blk["stride"]
-            oh, ow, co = ops.conv_out_size(ch, sh), ops.conv_out_size(cw, sw), blk["cout"]
-            t1 = ops.conv2d_fprop(cur, bw["w1"][0], ch, cw, 3, (sh, sw), self.act, None,
-                                  self._buffer(f"t{i}a", b, oh, ow, co, dev, sid))
-            if wd is not None:
-                ident = ops.conv2d_fprop(cur, bw["wd"][0], ch, cw, 1, (sh, sw), ops.ACT_NONE, None,
-                                         self._buffer(f"t{i}d", b, oh, ow, co, dev, sid))
-            else:
-                ident = cur
-            out = ops.conv2d_fprop(t1, bw["w2"][0], oh, ow, 3, (1, 1), self.act, ident,
-                                   self._buffer(f"t{i}o", b, oh, ow, co, dev, sid))
-            st["blocks"].append({"x": cur, "t1": t1, "out": out, "w1": w1, "w2": wc2, "wd": wd, "stride": (sh, sw),
-                                 "f1": bw["w1"][1], "f2": bw["w2"][1], "fd": bw["wd"][1] if bw["wd"] is not None else None,
-                                 "in_hw": (ch, cw), "out_hw": (oh, ow)})
-            cur, ch, cw = out, oh, ow
-        st["w_stem"] = w_stem
-        st["pooled"] = ops.avgpool(cur, ch, cw)
-        return st
+        weights = self._prepped_weights(w, force=True)          # bf16 filters of THIS step's weights
+        lease = self._take_slot()
+        acts = self._workspace(lease.slot.acts, b, h, w, 1, image_1.device)
+        pooled = self._trunk_forward(image_1, image_2, weights, acts, 1)
+        return (lease, weights, acts, (b, h, w)), pooled
 
-    def _backward(self, st, g_pooled):
-        b = st["B"]
-        dev = g_pooled.device
-        L = ops._lib.lib()
-        act_id = 1 if self.act == ops.ACT_RELU else 2
-        act_bwd = ops.ACT_RELU_BWD if self.act == ops.ACT_RELU else ops.ACT_TANH_BWD
-        blocks = st["blocks"]
-        last = blocks[-1]
-        oh, ow = last["out_hw"]
-        c_last = last["out"].shape[3]
-        dz2 = self._buffer("g_last", b, oh, ow, c_last, dev)
-        ops._lib.check(L.delora_avgpool_bwd_nhwc_bf16(g_pooled.data_ptr(), last["out"].data_ptr(), b, oh, ow, c_last,
-                                                      act_id, dz2.data_ptr(), ops._stream()),
-                       "delora_avgpool_bwd_nhwc_bf16")
-        grads_rev = []
-        d_pool = None
-        for i in range(len(blocks) - 1, -1, -1):
-            blk = blocks[i]
-            (ch, cw), (oh, ow), (sh, sw) = blk["in_hw"], blk["out_hw"], blk["stride"]
-            cin, cout = blk["x"].shape[3], blk["out"].shape[3]
-            pidx = self._block_param_idx[i]
-            g_w2 = ops.conv2d_wgrad(blk["t1"], dz2, oh, ow, 3, (1, 1), out=self._gout(pidx[1]))
-            dz1 = ops.conv2d_fprop(dz2, blk["f2"], oh, ow, 3, (1, 1), act_bwd, None,
-                                   self._buffer(f"g{i}a", b, oh, ow, cout, dev), saved=blk["t1"])
-            g_w1 = ops.conv2d_wgrad(blk["x"], dz1, ch, cw, 3, (sh, sw), out=self._gout(pidx[0]))
-            g_wd = None
-            if blk["wd"] is not None:
-                g_wd = ops.conv2d_wgrad(blk["x"], dz2, ch, cw, 1, (sh, sw), out=self._gout(pidx[2]))
-            self._announce(pidx)       # this block's weight gradients are enqueued: its bucket may start reducing
-            if blk["wd"] is not None:
-                # 1x1 strided downsample: its data gradient is the 1x1 convolution of the SMALL dz, scattered to the
-                # strided positions afterwards (2-4x fewer MMAs than convolving the zero-upsampled gradient)
-                small = ops.conv2d_fprop(dz2, blk["fd"], oh, ow, 1, (1, 1), ops.ACT_NONE, None,
-                                         self._buffer(f"g{i}ds", b, oh, ow, cin, dev))
-                if i > 0 and ops.conv2d_dgrad_eligible(cin, cout, cw, (sh, sw)):
-                    # phase-decomposed data gradient of the strided conv1: no zero-upsampled tensors, the downsample's
-                    # gradient enters as a residual on the (sh*h, sw*w) pixels, act' of the block input in the epilogue
-                    dz2 = ops.conv2d_dgrad(dz1, blk["f1"], ch, cw, (sh, sw), act_bwd, small,
-                                           self._buffer(f"g{i}x", b, ch, cw, cin, dev), saved=blk["x"],
-                                           residual_strided=True)
-                    grads_rev.append((g_w1, g_w2, g_wd))
-                    continue
-                resid = ops.zero_upsample(small, oh, ow, (sh, sw), self._buffer(f"g{i}d", b, ch, cw, cin, dev), (ch, cw))
-                src = ops.zero_upsample(dz1, oh, ow, (sh, sw), self._buffer(f"g{i}u1", b, ch, cw, cout, dev), (ch, cw))
-            else:
-                resid, src = dz2, dz1
-            if i > 0:     # the block input is the previous block's activation output: fold act' into the epilogue
-                dz2 = ops.conv2d_fprop(src, blk["f1"], ch, cw, 3, (1, 1), act_bwd, resid,
-                                       self._buffer(f"g{i}x", b, ch, cw, cin, dev), saved=blk["x"])
-            else:         # the first block reads the max-pool output
-                d_pool = ops.conv2d_fprop(src, blk["f1"], ch, cw, 3, (1, 1), ops.ACT_NONE, resid,
-                                          self._buffer("g_pool", b, ch, cw, cin, dev))
-            grads_rev.append((g_w1, g_w2, g_wd))
-        h, w = st["H"], st["W"]
-        w2 = ops.conv_out_size(w, 2)
-        dz0 = self._buffer("g_stem", b, h, w2, 64, dev)
-        ops._lib.check(L.delora_maxpool_w_bwd_nhwc_bf16(d_pool.data_ptr(), st["idx"].data_ptr(), st["y0"].data_ptr(), b, h,
-                                                        w2, 64, 4 + act_id, dz0.data_ptr(), 1 if st["stem_fast"] else 0,
-                                                        ops._stream()),
-                       "delora_maxpool_w_bwd_nhwc_bf16")
-        if st["stem_fast"]:
-            g_stem = ops.stem_wgrad(st["x_in"], dz0, h, w, st["w_stem"].shape[1], out=self._gout(0))
+    def _backward(self, state, g_pooled):
+        _, weights, acts, (b, h, w) = state
+        params = self.trunk_parameters()
+        if self.grad_views is not None:
+            grads = self.grad_views
+            for g, p_ in zip(grads, params):
+                if g.shape != p_.shape or g.dtype != torch.float32 or not g.is_contiguous():
+                    raise ValueError(f"gradient output must be a contiguous fp32 tensor of shape {tuple(p_.shape)}")
         else:
-            g_stem = ops.conv2d_wgrad(st["x_in"], dz0, h, w, 3, (1, 2), cin_true=st["w_stem"].shape[1], out=self._gout(0))
-        self._announce([0])
-        grads = [g_stem]
-        for g_w1, g_w2, g_wd in reversed(grads_rev):
-            grads += [g_w1, g_w2]
-            if g_wd is not None:
-                grads.append(g_wd)
+            grads = [torch.empty_like(p_, memory_format=torch.contiguous_format) for p_ in params]
+        conv_dw = (ctypes.c_void_p * len(grads))(*[g.data_ptr() for g in grads])
+        L = _lib.lib()
+        for stage in (3, 2, 1, 0):
+            _lib.check(L.delora_trunk_backward(self.layers, b, h, w, self.act, weights.data_ptr(), acts.data_ptr(),
+                                               ops._req(g_pooled, torch.float32, "g_pooled"), conv_dw, stage,
+                                               ops._stream()), "delora_trunk_backward")
+            if self.grad_ready is not None:
+                self.grad_ready(self._stage_params[stage])    # this stage's weight gradients are enqueued
         return grads

@@ -383,14 +383,45 @@ int delora_quat_to_T_bwd(const float* quaternion, const float* grad_T, int B,
                          float* grad_quaternion, float* grad_translation, void* stream);
 
 /* ---------------------------------------------------------------------------------------
+ * Encoder trunk: ResNetModified (src/models/resnet_modified.py:95-120) from the two range images to the average-pooled
+ * features, the kernels above in one fixed sequence -- the sequence the odometry entry points below run as well.
+ * layers[4]: BasicBlocks per stage (1 .. 64 each).  H >= 1, W >= 2 with (W - 1) / 2 + 1 even (the max-pool halves it).
+ * act: 1 relu, 2 tanh.  The stem takes the 16-channel layout when W is even, the channel-padded one otherwise, so the
+ * weight section depends on W's parity.
+ *
+ * Weight section: delora_trunk_weight_bytes(layers, W) device bytes, written by delora_trunk_prep_weights from the
+ * fp32 filters: filters is a HOST array of device pointers, one per convolution in state_dict order (resnet.conv1,
+ * then per block conv1, conv2 and the downsample's conv if it has one).  The bf16 forward and flipped filters; prep
+ * copies its table from host memory and launches one kernel.
+ * Activation workspace: delora_trunk_activation_bytes(layers, B, H, W, saving) device bytes for batches of exactly B
+ * pairs, zeroed once after allocation (the zero halo rows).  saving = 0: rotating inference buffers; saving = 1: every
+ * activation the backward reads, its gradient buffers and the split-K scratch.  A size query returns -1 on bad
+ * arguments.
+ * forward: img1, img2 [B, 4, H, W] fp32 -> pooled [B, 512] fp32.  stage_out NULL or void*[4]: receives the addresses
+ * (in acts) of x1..x4, [B, h+2, w+2, C] padded NHWC bf16 with C = 64, 128, 256, 512.
+ * backward (after a saving forward of the same arguments, weights unchanged): call it for stage = 3, 2, 1, 0 in that
+ * order.  Stage 3 starts from g_pooled [B, 512] fp32 (read by stage 3 only); stage 0 ends with the max-pool and the
+ * stem.  Each call writes the weight gradient of every convolution of its stage (stage 0: and the stem) to
+ * conv_dw[c] (fp32 [Cout, Cin, k, k], c in the order of `filters`; a HOST array of device pointers), so that the
+ * gradients of a stage can be used once its call is enqueued. */
+int64_t delora_trunk_weight_bytes(const int* layers, int W);
+int delora_trunk_prep_weights(const int* layers, int W, const float* const* filters, void* weights, void* stream);
+int64_t delora_trunk_activation_bytes(const int* layers, int B, int H, int W, int saving);
+int delora_trunk_forward(const int* layers, int B, int H, int W, int act, int saving, const float* img1,
+                         const float* img2, const void* weights, void* acts, float* pooled, void** stage_out,
+                         void* stream);
+int delora_trunk_backward(const int* layers, int B, int H, int W, int act, const void* weights, void* acts,
+                          const float* g_pooled, float* const* conv_dw, int stage, void* stream);
+
+/* ---------------------------------------------------------------------------------------
  * Odometry inference: raw scans -> relative transforms, the whole model behind one call.
  * Replaces, for inference, deploy.tester.Tester.test_dataset's per-frame path
  *   (src/deploy/tester.py:38-107 -> src/deploy/deployer.py:237-281): the projection of both scans,
  *   models.model.OdometryModel.forward (src/models/model.py:96-116: encoder trunk, resnet.fc, the two MLP
  *   heads or the single MLP, quaternion / norm of the whole [B,4] block) and GeometryHandler's quaternion -> T.
  *
- * The trunk runs the kernels above in the order the Python encoder runs them (the projected images are
- * bit-identical to delora_project_fwd's, the pooled features to the Python trunk's); the fully connected tail is one
+ * The trunk is the one of delora_trunk_forward (the projected images are bit-identical to delora_project_fwd's, the
+ * pooled features to the Python trunk's, which runs delora_trunk_forward); the fully connected tail is one
  * fp32 launch per layer (odometry_linear_kernel) plus one launch for the last layer, the norm and quaternion -> T
  * (odometry_out_kernel), with a fixed summation order.  Not representable: pre_feature_extraction,
  * factor_fewer_resnet_channels != 1; dropout is the identity at inference.
@@ -409,7 +440,7 @@ typedef struct {
     int n_stride;                        /* max points per scan: the point stride of `points` */
     int max_batch;                       /* max pairs per delora_odometry_pairs call (1 .. 1024) */
     int act;                             /* 1 relu, 2 tanh */
-    int layers[4];                       /* BasicBlocks per stage, e.g. {2,2,2,2} (1 .. 16 each) */
+    int layers[4];                       /* BasicBlocks per stage, e.g. {2,2,2,2} (1 .. 64 each) */
     int resnet_outputs;                  /* fc width, 1000 in the shipped config */
     int single_mlp;                      /* use_single_mlp_at_output (0 / 1) */
     int w_pre;                           /* training only: horizontal_cells_preprocessing, the width the normals are
