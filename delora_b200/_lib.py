@@ -25,8 +25,16 @@ class OdometryTrainParams(ctypes.Structure):
                 ("min_neighbors", c_int)]
 
 
+class OdometryResidualParams(ctypes.Structure):
+    """delora_odometry_residual_params (include/delora_b200.h): the loss and the normals' settings of the per-frame ICP
+    residual of delora_odometry_streams_push_residual."""
+    _fields_ = [("lambda_po2pl", c_float), ("loss_flags", c_u32), ("nb_h", c_int), ("nb_w", c_int),
+                ("epsilon_range", c_float), ("min_neighbors", c_int)]
+
+
 c_desc_p = ctypes.POINTER(OdometryDesc)
 c_train_p = ctypes.POINTER(OdometryTrainParams)
+c_residual_p = ctypes.POINTER(OdometryResidualParams)
 
 # name -> (restype, argtypes); every symbol declared in include/delora_b200.h
 SIGNATURES = {
@@ -117,10 +125,16 @@ SIGNATURES = {
     "delora_odometry_streams_push": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                              c_void_p]),
     "delora_odometry_streams_reset": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_streams_residual_workspace_bytes": (c_i64, [c_desc_p]),
+    "delora_odometry_streams_residual_init": (c_int, [c_desc_p, c_void_p, c_void_p]),
+    "delora_odometry_streams_push_residual": (c_int, [c_desc_p, c_residual_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                      c_void_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_train_workspace_bytes": (c_i64, [c_desc_p]),
     "delora_odometry_train_init": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_train_step": (c_int, [c_desc_p, c_train_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_train_eval": (c_int, [c_desc_p, c_train_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_void_p]),
     "delora_odometry_train_weights": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_train_get_state": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_train_set_state": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),

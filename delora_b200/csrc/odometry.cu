@@ -266,12 +266,16 @@ struct InferPlan {
     size_t pooled, fc_out, hid[2];
     TrunkWeights w;
     size_t fc_w, fc_b, lin_w[kMaxLinear], lin_b[kMaxLinear];
+    // residual only (delora_odometry_streams_push_residual), after every other section: the dense grids of the S new
+    // frames and of each stream's previous frame, the 3x4 transforms the ICP reads, its outputs and its scratch
+    size_t pts_grid, nrm_grid, prev_pts_grid, prev_nrm_grid, T12, losses, grad_T, icp;
     size_t total;
 };
 
 // streams: S = max_batch streams, this tick's S frames, each stream's previous frame and whether it has one; the
 // trunk and tail then run at B = S.  Otherwise (pairs / push): 2 * max_batch scans and the one cached image of _push.
-static void make_infer_plan(const delora_odometry_desc* d, bool streams, InferPlan* p) {
+// residual (streams only): the sections of the per-frame ICP residual are appended; no other offset moves.
+static void make_infer_plan(const delora_odometry_desc* d, bool streams, bool residual, InferPlan* p) {
     memset(p, 0, sizeof(InferPlan));
     plan_model(d, &p->m);
     const Model& m = p->m;
@@ -289,6 +293,17 @@ static void make_infer_plan(const delora_odometry_desc* d, bool streams, InferPl
     for (int i = 0; i < m.n_lin; ++i) {
         p->lin_w[i] = take(off, (size_t)m.lin[i].K * m.lin[i].N * 4);
         p->lin_b[i] = take(off, (size_t)m.lin[i].N * 4);
+    }
+    if (residual) {
+        const size_t HW = (size_t)d->H * d->W;
+        p->pts_grid = take(off, (size_t)MB * HW * 16);
+        p->nrm_grid = take(off, (size_t)MB * HW * 16);
+        p->prev_pts_grid = take(off, (size_t)MB * HW * 16);
+        p->prev_nrm_grid = take(off, (size_t)MB * HW * 16);
+        p->T12 = take(off, (size_t)MB * 12 * 4);
+        p->losses = take(off, (size_t)MB * DELORA_LOSS_ROW * 4);
+        p->grad_T = take(off, (size_t)MB * 12 * 4);
+        p->icp = take(off, (size_t)delora_icp_scratch_floats(MB, (int)HW) * 4);
     }
     p->total = off;
 }
@@ -436,6 +451,20 @@ static int project_normalized(const Frames& f, const delora_odometry_desc* d, ch
                        st);
 }
 
+// The loss and normals' settings of delora_odometry_train_params and delora_odometry_residual_params
+static int check_icp_params(float lambda_po2pl, uint32_t loss_flags, int nb_h, int nb_w, float epsilon_range,
+                            int min_neighbors, const char* who) {
+    DELORA_CHECK_ARG(isfinite(lambda_po2pl), "%s: lambda_po2pl=%g must be finite", who, (double)lambda_po2pl);
+    DELORA_CHECK_ARG((loss_flags & (DELORA_LOSS_PO2PO | DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL)) != 0,
+                     "%s: loss_flags=0x%x sets no loss bit", who, loss_flags);
+    DELORA_CHECK_ARG(nb_h >= 1 && nb_h % 2 == 1, "%s: nb_h=%d must be odd and positive", who, nb_h);
+    DELORA_CHECK_ARG(nb_w >= 1 && nb_w % 2 == 1, "%s: nb_w=%d must be odd and positive", who, nb_w);
+    DELORA_CHECK_ARG(isfinite(epsilon_range) && epsilon_range >= 0.0f, "%s: epsilon_range=%g must be >= 0", who,
+                     (double)epsilon_range);
+    DELORA_CHECK_ARG(min_neighbors >= 0, "%s: min_neighbors=%d must be >= 0", who, min_neighbors);
+    return 0;
+}
+
 // Every workspace starts zeroed, with its depth keys at all ones (the projection's empty key)
 static int init_workspace(const Frames& f, size_t total, void* workspace, cudaStream_t st, const char* who) {
     char* ws = (char*)workspace;
@@ -485,7 +514,7 @@ extern "C" int64_t delora_odometry_weight_floats(const delora_odometry_desc* d) 
 extern "C" int64_t delora_odometry_workspace_bytes(const delora_odometry_desc* d) {
     if (check_desc(d, "delora_odometry_workspace_bytes")) return -1;
     InferPlan p;
-    make_infer_plan(d, false, &p);
+    make_infer_plan(d, false, false, &p);
     return (int64_t)p.total;
 }
 
@@ -493,7 +522,7 @@ extern "C" int delora_odometry_init(const delora_odometry_desc* d, void* workspa
     if (check_desc(d, "delora_odometry_init")) return 1;
     DELORA_CHECK_ARG(workspace, "delora_odometry_init: null workspace");
     InferPlan p;
-    make_infer_plan(d, false, &p);
+    make_infer_plan(d, false, false, &p);
     return init_workspace(p.f, p.total, workspace, (cudaStream_t)stream, "delora_odometry_init");
 }
 
@@ -502,7 +531,7 @@ extern "C" int delora_odometry_load_weights(const delora_odometry_desc* d, const
     if (check_desc(d, "delora_odometry_load_weights")) return 1;
     DELORA_CHECK_ARG(weights && workspace, "delora_odometry_load_weights: null pointer");
     InferPlan p;
-    make_infer_plan(d, false, &p);
+    make_infer_plan(d, false, false, &p);
     return load_weights(p, weights, workspace, (cudaStream_t)stream, "delora_odometry_load_weights");
 }
 
@@ -510,7 +539,7 @@ extern "C" int delora_odometry_load_weights(const delora_odometry_desc* d, const
 static int run_pairs(const delora_odometry_desc* d, const float* points, const int32_t* n_points, int B, void* workspace,
                      float* T, float* pooled, float* factor, cudaStream_t st, const char* who) {
     InferPlan p;
-    make_infer_plan(d, false, &p);
+    make_infer_plan(d, false, false, &p);
     char* ws = (char*)workspace;
     float* images = reinterpret_cast<float*>(ws + p.f.images);
     const size_t img = (size_t)4 * d->H * d->W;
@@ -557,7 +586,7 @@ extern "C" int delora_odometry_push(const delora_odometry_desc* d, const float* 
     if (check_desc(d, "delora_odometry_push")) return 1;
     DELORA_CHECK_ARG(points && n_points && workspace, "delora_odometry_push: null pointer");
     InferPlan p;
-    make_infer_plan(d, false, &p);
+    make_infer_plan(d, false, false, &p);
     cudaStream_t st = (cudaStream_t)stream;
     char* ws = (char*)workspace;
     float* image = reinterpret_cast<float*>(ws + p.f.images);
@@ -670,12 +699,62 @@ __global__ void odometry_streams_reset_kernel(const int32_t* __restrict__ mask, 
     if (s < S && mask[s] != 0) has_prev[s] = 0;
 }
 
+// ---- the per-frame ICP residual (delora_odometry_streams_push_residual)
+__device__ __forceinline__ float4 empty_grid_cell() {       // what the normals kernel writes for a pixel without a point
+    return make_float4(__int_as_float(0x7f800000), __int_as_float(0x7f800000), __int_as_float(0x7f800000),
+                       __int_as_float(-1));
+}
+
+// every cached grid starts empty: the target of a stream that has not had a frame yet
+__global__ void __launch_bounds__(256)
+odometry_streams_grid_clear_kernel(float4* __restrict__ pts, float4* __restrict__ nrm, size_t n) {
+    const size_t i = (size_t)blockIdx.x * 256 + threadIdx.x;
+    if (i >= n) return;
+    pts[i] = empty_grid_cell();
+    nrm[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+}
+
+// The grids of the S new frames (cur) and of each stream's previous frame (prev) around the ICP, which runs at B = S
+// with source = cur, target = prev.  One thread per cell, a float4 of the point grid and one of the normal grid.
+// kPhase 0, before the ICP: a stream that is active without a transform this tick (its first frame since the start
+//   or a reset) caches its grids now and its cur grids become empty, so the ICP finds no source pixel for it and never
+//   searches its stale target; streams without a frame have empty cur grids from the projection already.  Also
+//   T12 [S, 12] = the 3x4 part of T of the valid streams, the identity for the others (whose T row is not written).
+// kPhase 1, after the ICP has read the targets: the valid streams cache their grids; losses [S, DELORA_LOSS_ROW] =
+//   the ICP's row of the valid streams, zeros for the others.
+// Every stream's grids are copied at most once per tick, and only if it has a frame.
+template <int kPhase>
+__global__ void __launch_bounds__(256)
+odometry_streams_grids_kernel(float4* __restrict__ cur_pts, float4* __restrict__ cur_nrm, float4* __restrict__ prev_pts,
+                              float4* __restrict__ prev_nrm, const int32_t* __restrict__ active,
+                              const int32_t* __restrict__ valid, int S, int HW, const float* __restrict__ T16,
+                              float* __restrict__ T12, const float* __restrict__ icp_losses,
+                              float* __restrict__ losses) {
+    const size_t i = (size_t)blockIdx.x * 256 + threadIdx.x;
+    if (kPhase == 0 && i < (size_t)S * 12) {
+        const int s = (int)i / 12, e = (int)i % 12;
+        T12[i] = valid[s] != 0 ? T16[s * 16 + e] : (e % 5 == 0 ? 1.0f : 0.0f);
+    }
+    if (kPhase == 1 && i < (size_t)S * DELORA_LOSS_ROW)
+        losses[i] = valid[i / DELORA_LOSS_ROW] != 0 ? icp_losses[i] : 0.0f;
+    if (i >= (size_t)S * HW) return;
+    const int s = (int)(i / HW);
+    const bool ok = valid[s] != 0;
+    if (kPhase == 0 ? (ok || !stream_active(active, s)) : !ok) return;
+    prev_pts[i] = cur_pts[i];
+    prev_nrm[i] = cur_nrm[i];
+    if (kPhase == 0) {
+        cur_pts[i] = empty_grid_cell();
+        cur_nrm[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    }
+}
+
 }  // namespace delora
 
 extern "C" int64_t delora_odometry_streams_workspace_bytes(const delora_odometry_desc* d) {
     if (check_desc(d, "delora_odometry_streams_workspace_bytes")) return -1;
     InferPlan p;
-    make_infer_plan(d, true, &p);
+    make_infer_plan(d, true, false, &p);
     return (int64_t)p.total;
 }
 
@@ -684,7 +763,7 @@ extern "C" int delora_odometry_streams_init(const delora_odometry_desc* d, void*
     if (check_desc(d, who)) return 1;
     DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
     InferPlan p;
-    make_infer_plan(d, true, &p);
+    make_infer_plan(d, true, false, &p);
     return init_workspace(p.f, p.total, workspace, (cudaStream_t)stream, who);
 }
 
@@ -695,30 +774,37 @@ extern "C" int delora_odometry_streams_load_weights(const delora_odometry_desc* 
     DELORA_CHECK_ARG(weights, "%s: null weights", who);
     DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
     InferPlan p;
-    make_infer_plan(d, true, &p);
+    make_infer_plan(d, true, false, &p);
     return load_weights(p, weights, workspace, (cudaStream_t)stream, who);
 }
 
-extern "C" int delora_odometry_streams_push(const delora_odometry_desc* d, const float* points, const int32_t* n_points,
-                                            const int32_t* active, void* workspace, float* T, int32_t* valid,
-                                            void* stream) {
-    const char* who = "delora_odometry_streams_push";
-    if (check_desc(d, who)) return 1;
-    DELORA_CHECK_ARG(points, "%s: null points", who);
-    DELORA_CHECK_ARG(n_points, "%s: null n_points", who);
-    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
-    DELORA_CHECK_ARG(T, "%s: null T", who);
-    DELORA_CHECK_ARG(valid, "%s: null valid", who);
+// delora_odometry_streams_push (rp NULL) and delora_odometry_streams_push_residual (arguments checked by the callers)
+static int run_streams_push(const delora_odometry_desc* d, const delora_odometry_residual_params* rp, const float* points,
+                            const int32_t* n_points, const int32_t* active, void* workspace, float* T, int32_t* valid,
+                            float* losses, cudaStream_t st) {
     InferPlan p;
-    make_infer_plan(d, true, &p);
-    cudaStream_t st = (cudaStream_t)stream;
+    make_infer_plan(d, true, rp != nullptr, &p);
     char* ws = (char*)workspace;
     const int S = d->max_batch, H = d->H, W = d->W;
     float* cur = reinterpret_cast<float*>(ws + p.f.images);
     float* prev = reinterpret_cast<float*>(ws + p.f.prev_image);
     int32_t* has_prev = reinterpret_cast<int32_t*>(ws + p.f.has_prev);
+    float4* pts_grid = reinterpret_cast<float4*>(ws + p.pts_grid);
+    float4* nrm_grid = reinterpret_cast<float4*>(ws + p.nrm_grid);
     int rc;
-    if ((rc = project(p.f, d, ws, points, n_points, active, S, st))) return rc;
+    if (rp) {
+        // the image of delora_project_fwd, bit for bit, plus the grids of the S frames with their normals
+        if ((rc = clamp_counts(p.f, ws, n_points, active, S, d->n_stride, st))) return rc;
+        if ((rc = delora_project_normals_fwd(points, reinterpret_cast<int32_t*>(ws + p.f.counts), S, 3, d->n_stride, H, W,
+                                             d->hfov0, d->hfov1, d->vfov0, d->vfov1, 0,
+                                             reinterpret_cast<uint64_t*>(ws + p.f.keys), cur,
+                                             reinterpret_cast<int32_t*>(ws + p.f.index_map), rp->nb_h, rp->nb_w,
+                                             rp->epsilon_range, rp->min_neighbors,
+                                             reinterpret_cast<delora_f4*>(pts_grid), reinterpret_cast<delora_f4*>(nrm_grid),
+                                             nullptr, st))) return rc;
+    } else if ((rc = project(p.f, d, ws, points, n_points, active, S, st))) {
+        return rc;
+    }
     __nv_bfloat16* x_in = reinterpret_cast<__nv_bfloat16*>(ws + p.t.x_in);
     if (p.m.t.stem_fast) {
         const size_t n = (size_t)S * (H + 2) * W;
@@ -736,7 +822,87 @@ extern "C" int delora_odometry_streams_push(const delora_odometry_desc* d, const
     odometry_streams_out_kernel<<<1, kTailWarps * 32, (size_t)S * 7 * sizeof(float), st>>>(rot, trans, S, vec, active,
                                                                                           has_prev, T, valid);
     DELORA_CHECK_LAUNCH("odometry_streams_out_kernel");
+    if (!rp) return 0;
+    // the residual: this frame moved by T against the stream's previous frame (the training step's orientation,
+    // scan_2 -> scan_1), for all S streams in one ICP call whose sources are empty where there is no T
+    const int HW = H * W;
+    float4* prev_pts = reinterpret_cast<float4*>(ws + p.prev_pts_grid);
+    float4* prev_nrm = reinterpret_cast<float4*>(ws + p.prev_nrm_grid);
+    float* T12 = reinterpret_cast<float*>(ws + p.T12);
+    float* icp_losses = reinterpret_cast<float*>(ws + p.losses);
+    const size_t cells = (size_t)S * HW > (size_t)S * 12 ? (size_t)S * HW : (size_t)S * 12;
+    const unsigned blocks = (unsigned)((cells + 255) / 256);
+    odometry_streams_grids_kernel<0><<<blocks, 256, 0, st>>>(pts_grid, nrm_grid, prev_pts, prev_nrm, active, valid, S, HW,
+                                                             T, T12, icp_losses, losses);
+    DELORA_CHECK_LAUNCH("odometry_streams_grids_kernel<0>");
+    if ((rc = delora_icp_dense_fwd_bwd(reinterpret_cast<delora_f4*>(pts_grid), reinterpret_cast<delora_f4*>(nrm_grid), T12,
+                                       reinterpret_cast<delora_f4*>(prev_pts), reinterpret_cast<delora_f4*>(prev_nrm), S,
+                                       H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, rp->lambda_po2pl, rp->loss_flags,
+                                       icp_losses, reinterpret_cast<float*>(ws + p.grad_T),
+                                       reinterpret_cast<float*>(ws + p.icp), st))) return rc;
+    odometry_streams_grids_kernel<1><<<blocks, 256, 0, st>>>(pts_grid, nrm_grid, prev_pts, prev_nrm, active, valid, S, HW,
+                                                             T, T12, icp_losses, losses);
+    DELORA_CHECK_LAUNCH("odometry_streams_grids_kernel<1>");
     return 0;
+}
+
+extern "C" int delora_odometry_streams_push(const delora_odometry_desc* d, const float* points, const int32_t* n_points,
+                                            const int32_t* active, void* workspace, float* T, int32_t* valid,
+                                            void* stream) {
+    const char* who = "delora_odometry_streams_push";
+    if (check_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(points, "%s: null points", who);
+    DELORA_CHECK_ARG(n_points, "%s: null n_points", who);
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    DELORA_CHECK_ARG(T, "%s: null T", who);
+    DELORA_CHECK_ARG(valid, "%s: null valid", who);
+    return run_streams_push(d, nullptr, points, n_points, active, workspace, T, valid, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int64_t delora_odometry_streams_residual_workspace_bytes(const delora_odometry_desc* d) {
+    if (check_desc(d, "delora_odometry_streams_residual_workspace_bytes")) return -1;
+    InferPlan p;
+    make_infer_plan(d, true, true, &p);
+    return (int64_t)p.total;
+}
+
+extern "C" int delora_odometry_streams_residual_init(const delora_odometry_desc* d, void* workspace, void* stream) {
+    const char* who = "delora_odometry_streams_residual_init";
+    if (check_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    InferPlan p;
+    make_infer_plan(d, true, true, &p);
+    cudaStream_t st = (cudaStream_t)stream;
+    const int rc = init_workspace(p.f, p.total, workspace, st, who);    // the ICP scratch is zeroed here, once
+    if (rc) return rc;
+    const size_t n = (size_t)d->max_batch * d->H * d->W;
+    odometry_streams_grid_clear_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
+        reinterpret_cast<float4*>((char*)workspace + p.prev_pts_grid),
+        reinterpret_cast<float4*>((char*)workspace + p.prev_nrm_grid), n);
+    DELORA_CHECK_LAUNCH("odometry_streams_grid_clear_kernel");
+    return 0;
+}
+
+extern "C" int delora_odometry_streams_push_residual(const delora_odometry_desc* d,
+                                                     const delora_odometry_residual_params* rp, const float* points,
+                                                     const int32_t* n_points, const int32_t* active, void* workspace,
+                                                     float* T, int32_t* valid, float* losses, void* stream) {
+    const char* who = "delora_odometry_streams_push_residual";
+    if (check_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(rp, "%s: null residual_params", who);
+    if (check_icp_params(rp->lambda_po2pl, rp->loss_flags, rp->nb_h, rp->nb_w, rp->epsilon_range, rp->min_neighbors, who))
+        return 1;
+    const uint32_t icp_bits = DELORA_LOSS_PO2PO | DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | DELORA_NORMAL_LINEAR;
+    DELORA_CHECK_ARG((rp->loss_flags & ~icp_bits) == 0u,
+                     "%s: loss_flags=0x%x has a bit other than the ICP losses and DELORA_NORMAL_LINEAR", who,
+                     rp->loss_flags);
+    DELORA_CHECK_ARG(points, "%s: null points", who);
+    DELORA_CHECK_ARG(n_points, "%s: null n_points", who);
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    DELORA_CHECK_ARG(T, "%s: null T", who);
+    DELORA_CHECK_ARG(valid, "%s: null valid", who);
+    DELORA_CHECK_ARG(losses, "%s: null losses", who);
+    return run_streams_push(d, rp, points, n_points, active, workspace, T, valid, losses, (cudaStream_t)stream);
 }
 
 extern "C" int delora_odometry_streams_reset(const delora_odometry_desc* d, const int32_t* mask, void* workspace,
@@ -746,7 +912,7 @@ extern "C" int delora_odometry_streams_reset(const delora_odometry_desc* d, cons
     DELORA_CHECK_ARG(mask, "%s: null mask", who);
     DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
     InferPlan p;
-    make_infer_plan(d, true, &p);
+    make_infer_plan(d, true, false, &p);
     const int S = d->max_batch;
     odometry_streams_reset_kernel<<<(S + 255) / 256, 256, 0, (cudaStream_t)stream>>>(
         mask, S, reinterpret_cast<int32_t*>((char*)workspace + p.f.has_prev));
@@ -1111,15 +1277,8 @@ static int check_train_params(const delora_odometry_train_params* hp, const char
     DELORA_CHECK_ARG(hp->beta1 >= 0.0f && hp->beta1 < 1.0f, "%s: beta1=%g must be in [0, 1)", who, (double)hp->beta1);
     DELORA_CHECK_ARG(hp->beta2 >= 0.0f && hp->beta2 < 1.0f, "%s: beta2=%g must be in [0, 1)", who, (double)hp->beta2);
     DELORA_CHECK_ARG(isfinite(hp->eps) && hp->eps > 0.0f, "%s: eps=%g must be > 0", who, (double)hp->eps);
-    DELORA_CHECK_ARG(isfinite(hp->lambda_po2pl), "%s: lambda_po2pl=%g must be finite", who, (double)hp->lambda_po2pl);
-    DELORA_CHECK_ARG((hp->loss_flags & (DELORA_LOSS_PO2PO | DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL)) != 0,
-                     "%s: loss_flags=0x%x sets no loss bit", who, hp->loss_flags);
-    DELORA_CHECK_ARG(hp->nb_h >= 1 && hp->nb_h % 2 == 1, "%s: nb_h=%d must be odd and positive", who, hp->nb_h);
-    DELORA_CHECK_ARG(hp->nb_w >= 1 && hp->nb_w % 2 == 1, "%s: nb_w=%d must be odd and positive", who, hp->nb_w);
-    DELORA_CHECK_ARG(isfinite(hp->epsilon_range) && hp->epsilon_range >= 0.0f, "%s: epsilon_range=%g must be >= 0", who,
-                     (double)hp->epsilon_range);
-    DELORA_CHECK_ARG(hp->min_neighbors >= 0, "%s: min_neighbors=%d must be >= 0", who, hp->min_neighbors);
-    return 0;
+    return check_icp_params(hp->lambda_po2pl, hp->loss_flags, hp->nb_h, hp->nb_w, hp->epsilon_range, hp->min_neighbors,
+                            who);
 }
 
 static TailIO train_tail_io(const TrainPlan& tp, char* ws) {
@@ -1236,32 +1395,24 @@ extern "C" int delora_odometry_train_init(const delora_odometry_desc* d, const f
     return prep_blob_weights(tp.m, tp.w, ws, reinterpret_cast<const float*>(ws + tp.master), st, who);
 }
 
-extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
-                                          const float* points, const int32_t* n_points, int B, void* workspace,
-                                          float* losses, float* T, float* pooled, float* grads, void* stream) {
-    const char* who = "delora_odometry_train_step";
-    if (check_train_desc(d, who)) return 1;
-    if (check_train_params(hp, who)) return 1;
-    DELORA_CHECK_ARG(points && n_points && workspace, "%s: null pointer", who);
-    DELORA_CHECK_ARG(B >= 1 && B <= d->max_batch, "%s: B=%d outside [1, max_batch=%d]", who, B, d->max_batch);
-    const bool normalized = (hp->loss_flags & DELORA_TRAIN_NORMALIZATION_SCALING) != 0u;
-    const bool dropout = (hp->loss_flags & DELORA_TRAIN_DROPOUT) != 0u;
-    DELORA_CHECK_ARG(!normalized || d->w_pre > 0,
-                     "%s: DELORA_TRAIN_NORMALIZATION_SCALING needs w_pre > 0 (the reference's recipe: normals from the "
-                     "unscaled points at H x w_pre), got w_pre=%d", who, d->w_pre);
-    TrainPlan tp;
-    make_train_plan(d, &tp);
+namespace delora {
+
+__global__ void odometry_icp_batch_kernel(long long* __restrict__ ctr, int B) { ctr[1] = B; }
+
+// Stages 1-3 of delora_odometry_train_step and all of delora_odometry_train_eval: the projection + normals of the 2B
+// scans, the forward keeping its activations and the ICP losses with dL/dT, into the workspace (losses, grad_T, T16,
+// pooled).  dropout: the forward draws this step's masks.  Normalised models: T_out [B, 16] or NULL gets T in metres.
+static int train_forward_losses(const delora_odometry_desc* d, const delora_odometry_train_params* hp, const TrainPlan& tp,
+                                char* ws, const float* points, const int32_t* n_points, int B, bool dropout, float* T_out,
+                                cudaStream_t st, const char* who) {
     const Model& m = tp.m;
-    cudaStream_t st = (cudaStream_t)stream;
-    char* ws = (char*)workspace;
     auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
     const int H = d->H, W = d->W, HW = H * W;
+    const bool normalized = (hp->loss_flags & DELORA_TRAIN_NORMALIZATION_SCALING) != 0u;
     long long* ctr = reinterpret_cast<long long*>(ws + tp.ctr);
-    // the masks of this step: the forward reads the step count before odometry_out_bwd_kernel advances it, the
-    // backward after
-    const DropoutCtr drop_fwd{dropout ? ctr : nullptr, 0}, drop_bwd{dropout ? ctr : nullptr, 1};
+    // the forward reads the step count before odometry_out_bwd_kernel advances it
+    const DropoutCtr drop_fwd{dropout ? ctr : nullptr, 0};
     int rc;
-    cudaError_t e = cudaSuccess;
 
     // 1. projection + normals of the 2B scans (scan_1 x B, then scan_2 x B).  w_pre > 0: the reference's two stages,
     // projection + normals at H x w_pre (its offline preprocessing), then those grids projected at H x W (Deployer.step)
@@ -1301,9 +1452,8 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
     if ((rc = run_tail(m, train_tail_io(tp, ws), d->act, f(tp.pooled), B, f(tp.T16), st, nullptr, drop_fwd))) return rc;
     // 3. ICP losses and dL/dT: source = scan_2 moved by T, target = scan_1.  The identity fit still runs them: the
     // reference logs the ICP losses in that phase too
-    const bool identity = (hp->loss_flags & DELORA_LOSS_IDENTITY_FIT) != 0u;
-    e = cudaMemcpy2DAsync(f(tp.T12), 12 * sizeof(float), f(tp.T16), 16 * sizeof(float), 12 * sizeof(float), B,
-                          cudaMemcpyDeviceToDevice, st);
+    const cudaError_t e = cudaMemcpy2DAsync(f(tp.T12), 12 * sizeof(float), f(tp.T16), 16 * sizeof(float),
+                                            12 * sizeof(float), B, cudaMemcpyDeviceToDevice, st);
     DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
     const long long icp_n4 = (delora_icp_scratch_floats(B, HW) + 3) / 4;
     odometry_icp_rearm_kernel<<<2 * num_sms(), 256, 0, st>>>(reinterpret_cast<float4*>(ws + tp.icp), icp_n4, B, ctr);
@@ -1314,10 +1464,62 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
                                                           DELORA_TRAIN_DROPOUT),
                                        f(tp.losses), f(tp.grad_T), f(tp.icp), st))) return rc;
     if (normalized) {               // T in metres for the caller, the factor in losses[b][6]
-        odometry_train_normalized_out_kernel<<<(B * 16 + 255) / 256, 256, 0, st>>>(f(tp.T16), f(tp.pre_image), B, T,
+        odometry_train_normalized_out_kernel<<<(B * 16 + 255) / 256, 256, 0, st>>>(f(tp.T16), f(tp.pre_image), B, T_out,
                                                                                       f(tp.losses));
         DELORA_CHECK_LAUNCH("odometry_train_normalized_out_kernel");
     }
+    return 0;
+}
+
+// losses, T (not for normalised models: train_forward_losses wrote it) and pooled of B pairs to the caller's buffers
+static int train_outputs(const TrainPlan& tp, const char* ws, int B, bool normalized, float* losses, float* T,
+                         float* pooled, cudaStream_t st, const char* who) {
+    cudaError_t e = cudaSuccess;
+    auto out = [&](float* dst, size_t src, size_t n) {
+        if (dst && e == cudaSuccess) e = cudaMemcpyAsync(dst, ws + src, n * sizeof(float), cudaMemcpyDeviceToDevice, st);
+    };
+    out(losses, tp.losses, (size_t)B * DELORA_LOSS_ROW);
+    if (!normalized) out(T, tp.T16, (size_t)B * 16);
+    out(pooled, tp.pooled, (size_t)B * 512);
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+    return 0;
+}
+
+// what _train_step and _train_eval refuse alike
+static int check_train_call(const delora_odometry_desc* d, const delora_odometry_train_params* hp, const float* points,
+                            const int32_t* n_points, int B, const void* workspace, const char* who) {
+    if (check_train_desc(d, who)) return 1;
+    if (check_train_params(hp, who)) return 1;
+    DELORA_CHECK_ARG(points && n_points && workspace, "%s: null pointer", who);
+    DELORA_CHECK_ARG(B >= 1 && B <= d->max_batch, "%s: B=%d outside [1, max_batch=%d]", who, B, d->max_batch);
+    DELORA_CHECK_ARG((hp->loss_flags & DELORA_TRAIN_NORMALIZATION_SCALING) == 0u || d->w_pre > 0,
+                     "%s: DELORA_TRAIN_NORMALIZATION_SCALING needs w_pre > 0 (the reference's recipe: normals from the "
+                     "unscaled points at H x w_pre), got w_pre=%d", who, d->w_pre);
+    return 0;
+}
+
+}  // namespace delora
+
+extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
+                                          const float* points, const int32_t* n_points, int B, void* workspace,
+                                          float* losses, float* T, float* pooled, float* grads, void* stream) {
+    const char* who = "delora_odometry_train_step";
+    if (check_train_call(d, hp, points, n_points, B, workspace, who)) return 1;
+    const bool normalized = (hp->loss_flags & DELORA_TRAIN_NORMALIZATION_SCALING) != 0u;
+    const bool dropout = (hp->loss_flags & DELORA_TRAIN_DROPOUT) != 0u;
+    const bool identity = (hp->loss_flags & DELORA_LOSS_IDENTITY_FIT) != 0u;
+    TrainPlan tp;
+    make_train_plan(d, &tp);
+    const Model& m = tp.m;
+    cudaStream_t st = (cudaStream_t)stream;
+    char* ws = (char*)workspace;
+    auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
+    long long* ctr = reinterpret_cast<long long*>(ws + tp.ctr);
+    // the masks of this step, regenerated after odometry_out_bwd_kernel has advanced the step count
+    const DropoutCtr drop_bwd{dropout ? ctr : nullptr, 1};
+    int rc;
+    // 1-3. projection + normals, forward, ICP losses and dL/dT
+    if ((rc = train_forward_losses(d, hp, tp, ws, points, n_points, B, dropout, T, st, who))) return rc;
     // 4. backward: tail (dL/dT of the ICP mean or of the identity fit), average pool, trunk
     if ((rc = train_tail_backward(tp, ws, d->act, B, identity, st, drop_bwd))) return rc;
     float* conv_dw[kMaxConv];
@@ -1325,14 +1527,12 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
     for (int s = 3; s >= 0; --s)
         if ((rc = trunk_backward(m.t, tp.t, ws, tp.w, ws, d->act, B, f(tp.g_pooled), conv_dw, s, st, drop_bwd))) return rc;
     // outputs (T: the weights before the update)
-    auto out = [&](float* dst, size_t src, size_t n) {
-        if (dst && e == cudaSuccess) e = cudaMemcpyAsync(dst, ws + src, n * sizeof(float), cudaMemcpyDeviceToDevice, st);
-    };
-    out(losses, tp.losses, (size_t)B * DELORA_LOSS_ROW);
-    if (!normalized) out(T, tp.T16, (size_t)B * 16);
-    out(pooled, tp.pooled, (size_t)B * 512);
-    out(grads, tp.grad, (size_t)m.blob_floats);
-    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+    if ((rc = train_outputs(tp, ws, B, normalized, losses, T, pooled, st, who))) return rc;
+    if (grads) {
+        const cudaError_t e = cudaMemcpyAsync(grads, ws + tp.grad, (size_t)m.blob_floats * sizeof(float),
+                                              cudaMemcpyDeviceToDevice, st);
+        DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+    }
     // 5. Adam on the master blob, then the bf16 filters from the updated weights
     const long long n = m.blob_floats;
     const long long blocks = (n / 4 + 255) / 256;
@@ -1341,6 +1541,25 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
                                                hp->beta2, hp->eps);
     DELORA_CHECK_LAUNCH("odometry_adam_kernel");
     return delora_conv_weight_prep_multi(ws + tp.w.table, m.t.n_conv, st);
+}
+
+extern "C" int delora_odometry_train_eval(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
+                                          const float* points, const int32_t* n_points, int B, void* workspace,
+                                          float* losses, float* T, float* pooled, void* stream) {
+    const char* who = "delora_odometry_train_eval";
+    if (check_train_call(d, hp, points, n_points, B, workspace, who)) return 1;
+    TrainPlan tp;
+    make_train_plan(d, &tp);
+    cudaStream_t st = (cudaStream_t)stream;
+    char* ws = (char*)workspace;
+    int rc;
+    // dropout is the identity, as at inference; the identity fit's objective belongs to the step's backward
+    if ((rc = train_forward_losses(d, hp, tp, ws, points, n_points, B, false, T, st, who))) return rc;
+    // the ICP scratch now has the layout of B pairs: the next step or eval re-arms it if its batch size differs
+    odometry_icp_batch_kernel<<<1, 1, 0, st>>>(reinterpret_cast<long long*>(ws + tp.ctr), B);
+    DELORA_CHECK_LAUNCH("odometry_icp_batch_kernel");
+    return train_outputs(tp, ws, B, (hp->loss_flags & DELORA_TRAIN_NORMALIZATION_SCALING) != 0u, losses, T, pooled, st,
+                         who);
 }
 
 extern "C" int delora_odometry_train_weights(const delora_odometry_desc* d, const void* workspace, float* weights,

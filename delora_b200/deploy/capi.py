@@ -1,5 +1,6 @@
 """ctypes binding of the odometry workspaces of the C ABI (include/delora_b200.h): inference (`delora_odometry_pairs` /
-`_pairs_normalized` / `_push`), streams (`delora_odometry_streams_*`) and training (`delora_odometry_train_*`).
+`_pairs_normalized` / `_push`), streams (`delora_odometry_streams_*`, with the per-frame ICP residual
+`delora_odometry_streams_residual_*` / `_push_residual`) and training (`delora_odometry_train_*`).
 
 Each class holds one descriptor and one workspace, a torch uint8 tensor on the current device.  Every call runs on
 torch's current stream at call time, checks its status with `_lib.check` and does not synchronise (except
@@ -32,6 +33,15 @@ def train_params(config, lr, loss_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL, beta1=0
     return _lib.OdometryTrainParams(
         lr=lr, beta1=beta1, beta2=beta2, eps=eps, lambda_po2pl=config["lambda_po2pl"], loss_flags=loss_flags,
         nb_h=nb[0], nb_w=nb[1], epsilon_range=config["epsilon_range"],
+        min_neighbors=config["min_num_points_in_neighborhood_to_determine_point_class"])
+
+
+def residual_params(config, loss_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL):
+    """delora_odometry_residual_params: the loss and normals' settings of a reference-style config."""
+    nb = config["kitti"]["neighborhood_side_length"]
+    return _lib.OdometryResidualParams(
+        lambda_po2pl=config["lambda_po2pl"], loss_flags=loss_flags, nb_h=nb[0], nb_w=nb[1],
+        epsilon_range=config["epsilon_range"],
         min_neighbors=config["min_num_points_in_neighborhood_to_determine_point_class"])
 
 
@@ -104,10 +114,11 @@ class InferenceWorkspace(_Workspace):
 class StreamsWorkspace(_Workspace):
     """delora_odometry_streams_*: S = desc.max_batch streams in one workspace."""
     SIZE_QUERY = "delora_odometry_streams_workspace_bytes"
+    INIT = "delora_odometry_streams_init"
 
     def __init__(self, desc, weights, workspace=None):
         super().__init__(desc, workspace)
-        self._call("delora_odometry_streams_init", self.workspace.data_ptr())
+        self._call(self.INIT, self.workspace.data_ptr())
         self._call("delora_odometry_streams_load_weights", weights.data_ptr(), self.workspace.data_ptr())
 
     def push(self, points, counts, active, T, valid):
@@ -118,6 +129,22 @@ class StreamsWorkspace(_Workspace):
     def reset(self, mask):
         """Forget the previous frame of every stream with mask[s] != 0 (device int32 [S])."""
         self._call("delora_odometry_streams_reset", mask.data_ptr(), self.workspace.data_ptr())
+
+
+class ResidualStreamsWorkspace(StreamsWorkspace):
+    """delora_odometry_streams_residual_* on the streams layout with the residual's sections appended: `push` also
+    writes each stream's ICP loss row; `params` from residual_params.  load_weights / reset are the streams calls."""
+    SIZE_QUERY = "delora_odometry_streams_residual_workspace_bytes"
+    INIT = "delora_odometry_streams_residual_init"
+
+    def __init__(self, desc, weights, params, workspace=None):
+        super().__init__(desc, weights, workspace)
+        self._params = ctypes.byref(params)
+
+    def push(self, points, counts, active, T, valid, losses):
+        """StreamsWorkspace.push plus losses [S, LOSS_ROW] out: the ICP row of every valid stream, zeros elsewhere."""
+        self._call("delora_odometry_streams_push_residual", self._params, points.data_ptr(), counts.data_ptr(),
+                   _ptr(active), self.workspace.data_ptr(), T.data_ptr(), valid.data_ptr(), losses.data_ptr())
 
 
 class TrainingWorkspace(_Workspace):
@@ -146,6 +173,18 @@ class TrainingWorkspace(_Workspace):
             ptrs = tuple(t.data_ptr() for t in out)
         self._call("delora_odometry_train_step", self._params, points.data_ptr(), counts.data_ptr(), b,
                    self.workspace.data_ptr(), *ptrs)
+        return out
+
+    def eval(self, points, counts):
+        """delora_odometry_train_eval on B = rows // 2 pairs -> (losses [B, 8], T [B, 4, 4], pooled [B, 512]): the ICP
+        losses of the current weights, nothing updated; dropout is the identity."""
+        b = points.shape[0] // 2
+        dev = self.workspace.device
+        out = (torch.empty((b, ops.LOSS_ROW), dtype=torch.float32, device=dev),
+               torch.empty((b, 4, 4), dtype=torch.float32, device=dev),
+               torch.empty((b, 512), dtype=torch.float32, device=dev))
+        self._call("delora_odometry_train_eval", self._params, points.data_ptr(), counts.data_ptr(), b,
+                   self.workspace.data_ptr(), *(t.data_ptr() for t in out))
         return out
 
     def weights(self):

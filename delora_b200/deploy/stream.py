@@ -179,9 +179,16 @@ class OdometryStreams:
     fed only that stream's frames (each quaternion is divided by its own row's norm, as at batch 1).
 
     Per tick: the scans are copied into one pinned staging buffer (points, counts, activity flags), one H2D copy, one
-    graph replay (or the eager call), one D2H copy of T and valid, one synchronise."""
+    graph replay (or the eager call), one D2H copy of T and valid, one synchronise.
 
-    def __init__(self, model, config, dataset, n_streams, n_max, use_cuda_graph=True):
+    residual=True serves the streams from the residual workspace (`delora_odometry_streams_push_residual`): `push` then
+    returns, beside each transform, the stream's ICP loss row [LOSS_ROW] (po2po, po2pl, pl2pl, matched pairs, matched
+    po2po pairs, ...) of this frame moved by T against the previous frame, with the normals estimated on the model's
+    H x W image and the config's neighbourhood; `residual_flags` selects the losses.  The transforms are the same bits
+    either way."""
+
+    def __init__(self, model, config, dataset, n_streams, n_max, use_cuda_graph=True, residual=False,
+                 residual_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL):
         from . import capi, export
         if config.get("normalization_scaling", False):
             raise ValueError("normalization_scaling: True is not supported by OdometryStreams (its workspace caches "
@@ -197,12 +204,18 @@ class OdometryStreams:
         S, n = self.n_streams, self.n_max
         with torch.cuda.device(self.device):
             self.blob = torch.from_numpy(export.pack_state_dict(model.state_dict(), config)).to(self.device)
-            self.workspace = capi.StreamsWorkspace(self.desc, self.blob)
+            self.residual = bool(residual)
+            if self.residual:
+                self.workspace = capi.ResidualStreamsWorkspace(self.desc, self.blob,
+                                                               capi.residual_params(config, residual_flags))
+            else:
+                self.workspace = capi.StreamsWorkspace(self.desc, self.blob)
             # staging: points [S, 3, n_max] fp32, then counts [S] and active [S] int32, one buffer each way
             in_bytes = S * 3 * n * 4 + 2 * S * 4
             self.host_in = torch.zeros((in_bytes,), dtype=torch.uint8).pin_memory()
             self.dev_in = torch.zeros((in_bytes,), dtype=torch.uint8, device=self.device)
-            out_bytes = S * 16 * 4 + S * 4                       # T [S, 16] fp32, valid [S] int32
+            # T [S, 16] fp32, valid [S] int32, then with residual losses [S, LOSS_ROW] fp32
+            out_bytes = S * 16 * 4 + S * 4 + (S * ops.LOSS_ROW * 4 if self.residual else 0)
             self.host_out = torch.zeros((out_bytes,), dtype=torch.uint8).pin_memory()
             self.dev_out = torch.zeros((out_bytes,), dtype=torch.uint8, device=self.device)
             self.dev_mask = torch.zeros((S,), dtype=torch.int32, device=self.device)
@@ -212,11 +225,14 @@ class OdometryStreams:
         self._host_active = raw[S * 3 * n * 4 + S * 4:].view(np.int32)
         out = self.host_out.numpy()
         self._host_T = out[:S * 64].view(np.float32).reshape(S, 4, 4)
-        self._host_valid = out[S * 64:].view(np.int32)
+        self._host_valid = out[S * 64:S * 68].view(np.int32)
+        self._host_losses = out[S * 68:].view(np.float32).reshape(S, -1)
         # the push arguments of a tick: points, counts, active, T, valid in the device staging buffers
         self._dev_active = self.dev_in[S * 3 * n * 4 + S * 4:]
         self._tick = (self.dev_in[:S * 3 * n * 4], self.dev_in[S * 3 * n * 4:S * 3 * n * 4 + S * 4], self._dev_active,
-                      self.dev_out[:S * 64], self.dev_out[S * 64:])
+                      self.dev_out[:S * 64], self.dev_out[S * 64:S * 68])
+        if self.residual:
+            self._tick += (self.dev_out[S * 68:],)
         self.relative = [[] for _ in range(S)]
         self.use_cuda_graph = bool(use_cuda_graph)
         self.graph = None
@@ -235,7 +251,8 @@ class OdometryStreams:
     def push(self, scans):
         """scans: a list of n_streams entries, each a [3, N] (or [1, 3, N]) float32 host tensor with N <= n_max, or
         None for a stream without a frame this tick.  Returns a list of n_streams entries: the relative transform
-        T_{k-1,k} of the stream as a [1, 4, 4] numpy array, or None (no frame, or the stream's first frame)."""
+        T_{k-1,k} of the stream as a [1, 4, 4] numpy array, or None (no frame, or the stream's first frame).  With
+        residual=True an entry with a transform is the tuple (T, losses [LOSS_ROW] numpy array)."""
         if len(scans) != self.n_streams:
             raise ValueError(f"push takes {self.n_streams} entries (one per stream, None = inactive), got {len(scans)}")
         with torch.cuda.device(self.device):
@@ -265,7 +282,7 @@ class OdometryStreams:
             if self._host_valid[s]:
                 t = self._host_T[s][None].copy()
                 self.relative[s].append(t)
-                out.append(t)
+                out.append((t, self._host_losses[s].copy()) if self.residual else t)
             else:
                 out.append(None)
         return out

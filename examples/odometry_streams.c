@@ -2,13 +2,16 @@
  * Several LiDAR streams from a C host, batched in one workspace: no Python, no torch.  Links libdelora_b200.so and
  * cudart only.
  *
- *   odometry_streams model.dlw stream0_dir stream1_dir ...
+ *   odometry_streams [--residual] model.dlw stream0_dir stream1_dir ...
  *
  * model.dlw is written by bin/export_odometry_weights.py (layout: include/delora_b200.h); every directory holds one
  * stream's KITTI velodyne .bin files ([N, 4] float32 rows: x, y, z, reflectance), taken in name order.  All streams
  * share the model and the sensor geometry of model.dlw; the number of directories is the number of streams.  Streams
  * of different lengths go inactive once they run out of scans.  Per tick, for every stream with a transform, it prints
  * one line: the stream index, the frame index k, and T_{k-1,k} as 12 floats (the top three rows of the 4x4, row-major).
+ * --residual serves the streams through delora_odometry_streams_push_residual and appends to each line the frame's ICP
+ * residual against the stream's previous frame: the point-to-plane loss, the plane-to-plane loss and the matched pairs
+ * (normals on the model's image, 7 x 11 neighbourhood, the reference's defaults).  The transforms are the same bits.
  *
  * Build:  cc odometry_streams.c -I include -I $CUDA_HOME/include -L delora_b200 -ldelora_b200 \
  *            -L $CUDA_HOME/lib64 -lcudart -Wl,-rpath,$PWD/delora_b200 -o odometry_streams
@@ -93,7 +96,9 @@ static int32_t read_scan(const char* path, float* dst, int n_stride) {
 }
 
 int main(int argc, char** argv) {
-    if (argc < 3) return fail("usage: odometry_streams model.dlw stream_dir [stream_dir ...]");
+    const int residual = argc > 1 && strcmp(argv[1], "--residual") == 0;
+    if (residual) { --argc; ++argv; }
+    if (argc < 3) return fail("usage: odometry_streams [--residual] model.dlw stream_dir [stream_dir ...]");
     const int S = argc - 2;
 
     /* weight file: fixed header, then the fp32 blob; the workspace serves S streams (max_batch = S) */
@@ -127,10 +132,17 @@ int main(int argc, char** argv) {
     cudaStream_t stream;
     CUDA_OK(cudaStreamCreate(&stream));
     const size_t pts_floats = (size_t)S * 3 * d->n_stride;
-    float *weights, *points, *T;
+    float *weights, *points, *T, *losses;
+    delora_odometry_residual_params rp;
+    rp.lambda_po2pl = 1.0f;
+    rp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL;
+    rp.nb_h = 7; rp.nb_w = 11;
+    rp.epsilon_range = 0.5f;
+    rp.min_neighbors = 10;
     int32_t *count, *active, *valid;
     void* workspace;
-    const int64_t ws_bytes = delora_odometry_streams_workspace_bytes(d);
+    const int64_t ws_bytes = residual ? delora_odometry_streams_residual_workspace_bytes(d)
+                                      : delora_odometry_streams_workspace_bytes(d);
     if (ws_bytes < 0) return fail(delora_last_error());
     CUDA_OK(cudaMalloc((void**)&weights, (size_t)n_weights * sizeof(float)));
     CUDA_OK(cudaMalloc(&workspace, (size_t)ws_bytes));
@@ -139,8 +151,10 @@ int main(int argc, char** argv) {
     CUDA_OK(cudaMalloc((void**)&active, (size_t)S * sizeof(int32_t)));
     CUDA_OK(cudaMalloc((void**)&valid, (size_t)S * sizeof(int32_t)));
     CUDA_OK(cudaMalloc((void**)&T, (size_t)S * 16 * sizeof(float)));
+    CUDA_OK(cudaMalloc((void**)&losses, (size_t)S * DELORA_LOSS_ROW * sizeof(float)));
     CUDA_OK(cudaMemcpy(weights, h_blob, (size_t)n_weights * sizeof(float), cudaMemcpyHostToDevice));
-    DELORA_OK(delora_odometry_streams_init(d, workspace, stream));
+    if (residual) DELORA_OK(delora_odometry_streams_residual_init(d, workspace, stream));
+    else DELORA_OK(delora_odometry_streams_init(d, workspace, stream));
     DELORA_OK(delora_odometry_streams_load_weights(d, weights, workspace, stream));
 
     float* h_points = (float*)malloc(pts_floats * sizeof(float));
@@ -148,7 +162,8 @@ int main(int argc, char** argv) {
     int32_t* h_active = (int32_t*)malloc((size_t)S * sizeof(int32_t));
     int32_t* h_valid = (int32_t*)malloc((size_t)S * sizeof(int32_t));
     float* h_T = (float*)malloc((size_t)S * 16 * sizeof(float));
-    if (!h_points || !h_count || !h_active || !h_valid || !h_T) return fail("out of host memory");
+    float* h_losses = (float*)calloc((size_t)S * DELORA_LOSS_ROW, sizeof(float));
+    if (!h_points || !h_count || !h_active || !h_valid || !h_T || !h_losses) return fail("out of host memory");
     for (int k = 0; k < ticks; ++k) {
         for (int s = 0; s < S; ++s) {
             h_active[s] = k < lists[s].n;
@@ -160,7 +175,14 @@ int main(int argc, char** argv) {
         CUDA_OK(cudaMemcpyAsync(points, h_points, pts_floats * sizeof(float), cudaMemcpyHostToDevice, stream));
         CUDA_OK(cudaMemcpyAsync(count, h_count, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
         CUDA_OK(cudaMemcpyAsync(active, h_active, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
-        DELORA_OK(delora_odometry_streams_push(d, points, count, active, workspace, T, valid, stream));
+        if (residual) {
+            DELORA_OK(delora_odometry_streams_push_residual(d, &rp, points, count, active, workspace, T, valid, losses,
+                                                            stream));
+            CUDA_OK(cudaMemcpyAsync(h_losses, losses, (size_t)S * DELORA_LOSS_ROW * sizeof(float), cudaMemcpyDeviceToHost,
+                                    stream));
+        } else {
+            DELORA_OK(delora_odometry_streams_push(d, points, count, active, workspace, T, valid, stream));
+        }
         CUDA_OK(cudaMemcpyAsync(h_T, T, (size_t)S * 16 * sizeof(float), cudaMemcpyDeviceToHost, stream));
         CUDA_OK(cudaMemcpyAsync(h_valid, valid, (size_t)S * sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
         CUDA_OK(cudaStreamSynchronize(stream));
@@ -168,6 +190,10 @@ int main(int argc, char** argv) {
             if (!h_valid[s]) continue;
             printf("%d %d", s, k);
             for (int i = 0; i < 12; ++i) printf(" %.9g", h_T[(size_t)s * 16 + i]);
+            if (residual) {
+                const float* l = h_losses + (size_t)s * DELORA_LOSS_ROW;
+                printf(" %.9g %.9g %.0f", l[1], l[2], l[3]);
+            }
             printf("\n");
         }
     }
@@ -176,12 +202,14 @@ int main(int argc, char** argv) {
         free(lists[s].paths);
     }
     free(lists);
+    free(h_losses);
     free(h_T);
     free(h_valid);
     free(h_active);
     free(h_count);
     free(h_points);
     free(h_blob);
+    cudaFree(losses);
     cudaFree(T);
     cudaFree(valid);
     cudaFree(active);

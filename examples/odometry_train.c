@@ -2,7 +2,8 @@
  * The reference's training loop (src/deploy/trainer.py, Trainer.train) from a C host: no Python, no torch.  Links
  * libdelora_b200.so and cudart only.
  *
- *   odometry_train [--lr LR] [--switch-below L] [--dropout-seed S] in.dlt|in.dlw out.dlt epochs B scan_000.bin ...
+ *   odometry_train [--lr LR] [--switch-below L] [--dropout-seed S] [--eval-dir DIR] in.dlt|in.dlw out.dlt epochs B
+ *                  scan_000.bin ...
  *
  * Reads a training checkpoint (.dlt: weights, Adam's state, epoch and phase; layout in include/delora_b200.h) or a
  * weight file (.dlw: a fresh Adam with learning rate --lr, default 1e-5, the reference's learning_rate) and a list of
@@ -20,10 +21,15 @@
  * (DELORA_TRAIN_DROPOUT).  The seed of the masks is --dropout-seed, else the DELORA_DROPOUT_SEED environment variable,
  * else the .dlt's (0 for a .dlw); it is written into every out.dlt, so a resumed run draws the masks of an
  * uninterrupted one.
+ * --eval-dir DIR: a held-out sequence (the reference's testing_identifiers), the .bin scans of DIR in name order.  After
+ * every epoch the mean ICP objective (po2po + lambda * po2pl + pl2pl per pair) over its consecutive pairs, through
+ * delora_odometry_train_eval on the training workspace, is appended to the epoch's line as "held-out <mean>".  The
+ * evaluation updates nothing: out.dlt has the bytes of a run without the option.
  *
  * Build:  cc odometry_train.c -I include -I $CUDA_HOME/include -L delora_b200 -ldelora_b200 \
  *            -L $CUDA_HOME/lib64 -lcudart -Wl,-rpath,$PWD/delora_b200 -o odometry_train
  */
+#include <dirent.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -35,6 +41,35 @@
 static int fail(const char* what) {
     fprintf(stderr, "odometry_train: %s\n", what);
     return 1;
+}
+
+static int by_name(const void* a, const void* b) { return strcmp(*(char* const*)a, *(char* const*)b); }
+
+/* the .bin files of a directory, sorted by name -> *paths (malloc'ed); the count, or -1 */
+static int list_scans(const char* dir, char*** paths) {
+    DIR* d = opendir(dir);
+    if (!d) return -1;
+    int cap = 16, n = 0;
+    char** out = (char**)malloc(sizeof(char*) * (size_t)cap);
+    const struct dirent* e;
+    while (out && (e = readdir(d)) != NULL) {
+        const size_t len = strlen(e->d_name);
+        if (len < 5 || strcmp(e->d_name + len - 4, ".bin") != 0) continue;
+        if (n == cap) {
+            cap *= 2;
+            char** grown = (char**)realloc(out, sizeof(char*) * (size_t)cap);
+            if (!grown) { closedir(d); return -1; }
+            out = grown;
+        }
+        out[n] = (char*)malloc(strlen(dir) + len + 2);
+        if (!out[n]) { closedir(d); return -1; }
+        sprintf(out[n++], "%s/%s", dir, e->d_name);
+    }
+    closedir(d);
+    if (!out) return -1;
+    qsort(out, (size_t)n, sizeof(char*), by_name);
+    *paths = out;
+    return n;
 }
 
 #define CUDA_OK(call)                                                                  \
@@ -70,6 +105,44 @@ static int32_t read_scan(const char* path, int n_stride, float* out) {
     return n;
 }
 
+/* n scans -> [n, 3, n_stride] host floats and their counts (both malloc'ed); 0 on success */
+static int load_scans(char** paths, int n, int n_stride, float** scans, int32_t** counts) {
+    const size_t scan_floats = (size_t)3 * n_stride;
+    *scans = (float*)malloc((size_t)(n > 0 ? n : 1) * scan_floats * sizeof(float));
+    *counts = (int32_t*)malloc((size_t)(n > 0 ? n : 1) * sizeof(int32_t));
+    if (!*scans || !*counts) return fail("out of host memory");
+    for (int k = 0; k < n; ++k)
+        if (((*counts)[k] = read_scan(paths[k], n_stride, *scans + (size_t)k * scan_floats)) < 0)
+            return fail("cannot read a scan (missing, truncated, or more points than n_stride)");
+    return 0;
+}
+
+/* the points of a step or an evaluation on pairs (k0 + b, k0 + b + 1), b < B: scan_1 of pairs 0..B-1, then scan_2 */
+static int stage_pairs(const float* h_scans, const int32_t* h_counts, int k0, int B, size_t scan_floats, float* points,
+                       int32_t* counts, int32_t* h_step_counts, cudaStream_t stream) {
+    for (int b = 0; b < B; ++b) {
+        const int k = k0 + b;
+        CUDA_OK(cudaMemcpyAsync(points + (size_t)b * scan_floats, h_scans + (size_t)k * scan_floats,
+                                scan_floats * sizeof(float), cudaMemcpyHostToDevice, stream));
+        CUDA_OK(cudaMemcpyAsync(points + (size_t)(B + b) * scan_floats, h_scans + (size_t)(k + 1) * scan_floats,
+                                scan_floats * sizeof(float), cudaMemcpyHostToDevice, stream));
+        h_step_counts[b] = h_counts[k];
+        h_step_counts[B + b] = h_counts[k + 1];
+    }
+    CUDA_OK(cudaMemcpyAsync(counts, h_step_counts, (size_t)2 * B * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+    return 0;
+}
+
+/* mean over the B rows of po2po + lambda * po2pl + pl2pl */
+static double icp_objective(const float* h_losses, int B, float lambda_po2pl) {
+    double objective = 0.0;
+    for (int b = 0; b < B; ++b) {
+        const float* l = h_losses + (size_t)b * DELORA_LOSS_ROW;
+        objective += (double)l[0] + (double)lambda_po2pl * l[1] + (double)l[2];
+    }
+    return objective / B;
+}
+
 /* the header and the three host arrays (weights, exp_avg, exp_avg_sq) to path, through path.tmp and a rename */
 static int write_dlt(const char* path, const delora_odometry_train_file_header* hdr, float* const* h_state, size_t n) {
     char tmp[4096];
@@ -87,16 +160,18 @@ int main(int argc, char** argv) {
     float lr = 1e-5f;
     double switch_below = 1e-2;
     const char* seed_arg = getenv("DELORA_DROPOUT_SEED");
+    const char* eval_dir = NULL;
     int a = 1;
     for (; a + 1 < argc && strncmp(argv[a], "--", 2) == 0; a += 2) {
         if (strcmp(argv[a], "--lr") == 0) lr = (float)atof(argv[a + 1]);
         else if (strcmp(argv[a], "--switch-below") == 0) switch_below = atof(argv[a + 1]);
         else if (strcmp(argv[a], "--dropout-seed") == 0) seed_arg = argv[a + 1];
+        else if (strcmp(argv[a], "--eval-dir") == 0) eval_dir = argv[a + 1];
         else return fail("unknown option");
     }
     if (argc - a < 6)
-        return fail("usage: odometry_train [--lr LR] [--switch-below L] [--dropout-seed S] in.dlt|in.dlw out.dlt epochs "
-                    "B scan.bin scan.bin [scan.bin ...]");
+        return fail("usage: odometry_train [--lr LR] [--switch-below L] [--dropout-seed S] [--eval-dir DIR] in.dlt|in.dlw "
+                    "out.dlt epochs B scan.bin scan.bin [scan.bin ...]");
     const char* in_path = argv[a];
     const char* out_path = argv[a + 1];
     const int epochs = atoi(argv[a + 2]);
@@ -153,12 +228,19 @@ int main(int argc, char** argv) {
     if (B_max < 1 || B_max > d->max_batch) return fail("B must be in [1, the header's max_batch]");
     if (epochs < 0) return fail("epochs must be >= 0");
     const size_t scan_floats = (size_t)3 * d->n_stride;
-    float* h_scans = (float*)malloc((size_t)n_scans * scan_floats * sizeof(float));
-    int32_t* h_counts = (int32_t*)malloc((size_t)n_scans * sizeof(int32_t));
-    if (!h_scans || !h_counts) return fail("out of host memory");
-    for (int k = 0; k < n_scans; ++k)
-        if ((h_counts[k] = read_scan(scan_paths[k], d->n_stride, h_scans + (size_t)k * scan_floats)) < 0)
-            return fail("cannot read a scan (missing, truncated, or more points than n_stride)");
+    float *h_scans, *h_eval_scans = NULL;
+    int32_t *h_counts, *h_eval_counts = NULL;
+    if (load_scans(scan_paths, n_scans, d->n_stride, &h_scans, &h_counts)) return 1;
+    int n_eval_pairs = 0;
+    if (eval_dir) {
+        char** eval_paths;
+        const int n_eval = list_scans(eval_dir, &eval_paths);
+        if (n_eval < 2) return fail("--eval-dir needs a directory with at least two .bin scans");
+        if (load_scans(eval_paths, n_eval, d->n_stride, &h_eval_scans, &h_eval_counts)) return 1;
+        for (int k = 0; k < n_eval; ++k) free(eval_paths[k]);
+        free(eval_paths);
+        n_eval_pairs = n_eval - 1;
+    }
 
     delora_odometry_train_params hp;
     hp.lr = hdr.lr; hp.beta1 = hdr.beta1; hp.beta2 = hdr.beta2; hp.eps = hdr.eps;
@@ -202,18 +284,7 @@ int main(int argc, char** argv) {
         int steps = 0;
         for (int k0 = 0; k0 < n_pairs; k0 += B_max, ++steps) {
             const int B = n_pairs - k0 < B_max ? n_pairs - k0 : B_max;
-            /* points of a step: scan_1 of pairs 0..B-1, then scan_2 of pairs 0..B-1 */
-            for (int b = 0; b < B; ++b) {
-                const int k = k0 + b;
-                CUDA_OK(cudaMemcpyAsync(points + (size_t)b * scan_floats, h_scans + (size_t)k * scan_floats,
-                                        scan_floats * sizeof(float), cudaMemcpyHostToDevice, stream));
-                CUDA_OK(cudaMemcpyAsync(points + (size_t)(B + b) * scan_floats, h_scans + (size_t)(k + 1) * scan_floats,
-                                        scan_floats * sizeof(float), cudaMemcpyHostToDevice, stream));
-                h_step_counts[b] = h_counts[k];
-                h_step_counts[B + b] = h_counts[k + 1];
-            }
-            CUDA_OK(cudaMemcpyAsync(counts, h_step_counts, (size_t)2 * B * sizeof(int32_t), cudaMemcpyHostToDevice,
-                                    stream));
+            if (stage_pairs(h_scans, h_counts, k0, B, scan_floats, points, counts, h_step_counts, stream)) return 1;
             DELORA_OK(delora_odometry_train_step(d, &hp, points, counts, B, workspace, losses, NULL, NULL, NULL, stream));
             CUDA_OK(cudaMemcpyAsync(h_losses, losses, (size_t)B * DELORA_LOSS_ROW * sizeof(float),
                                     cudaMemcpyDeviceToHost, stream));
@@ -221,16 +292,26 @@ int main(int argc, char** argv) {
             if (!hdr.unsupervised) {
                 sum += (double)h_losses[(size_t)(B - 1) * DELORA_LOSS_ROW + 5];
             } else {
-                double objective = 0.0;
-                for (int b = 0; b < B; ++b) {
-                    const float* l = h_losses + (size_t)b * DELORA_LOSS_ROW;
-                    objective += (double)l[0] + (double)hp.lambda_po2pl * l[1] + (double)l[2];
-                }
-                sum += objective / B;
+                sum += icp_objective(h_losses, B, hp.lambda_po2pl);
             }
         }
         const double mean = steps > 0 ? sum / steps : 0.0;
-        printf("epoch %d objective %.9g unsupervised %d\n", hdr.epoch, mean, hdr.unsupervised);
+        printf("epoch %d objective %.9g unsupervised %d", hdr.epoch, mean, hdr.unsupervised);
+        if (eval_dir) {         /* the held-out pairs with the weights after the epoch; no update, no dropout */
+            double held = 0.0;
+            for (int k0 = 0; k0 < n_eval_pairs; k0 += B_max) {
+                const int B = n_eval_pairs - k0 < B_max ? n_eval_pairs - k0 : B_max;
+                if (stage_pairs(h_eval_scans, h_eval_counts, k0, B, scan_floats, points, counts, h_step_counts, stream))
+                    return 1;
+                DELORA_OK(delora_odometry_train_eval(d, &hp, points, counts, B, workspace, losses, NULL, NULL, stream));
+                CUDA_OK(cudaMemcpyAsync(h_losses, losses, (size_t)B * DELORA_LOSS_ROW * sizeof(float),
+                                        cudaMemcpyDeviceToHost, stream));
+                CUDA_OK(cudaStreamSynchronize(stream));
+                held += icp_objective(h_losses, B, hp.lambda_po2pl) * B;
+            }
+            printf(" held-out %.9g", held / n_eval_pairs);
+        }
+        printf("\n");
         hdr.epoch += 1;
         hdr.loss = (float)mean;
         if (!hdr.unsupervised && mean < switch_below) {
@@ -249,6 +330,8 @@ int main(int argc, char** argv) {
 
     free(h_step_counts);
     free(h_losses);
+    free(h_eval_counts);
+    free(h_eval_scans);
     free(h_counts);
     free(h_scans);
     for (int i = 0; i < 3; ++i) {

@@ -562,6 +562,61 @@ int delora_odometry_streams_push(const delora_odometry_desc* d, const float* poi
  * caches its frame.  Refused: an invalid descriptor, null mask / workspace. */
 int delora_odometry_streams_reset(const delora_odometry_desc* d, const int32_t* mask, void* workspace, void* stream);
 
+/* A per-frame ICP residual beside every streamed transform: the model's own training objective (the point-to-plane /
+ * plane-to-plane / point-to-point residual of this frame moved by T against the stream's previous frame, with the
+ * matched-pair counts) as a quality signal that needs no ground truth.  Replaces, per streamed frame, the loss branch
+ * of the reference's Tester (inference_only: False; src/deploy/tester.py:61-65 -> src/deploy/deployer.py:280-369)
+ * without its visible_pixels and log images.  The call reports numbers only; what is a good frame is the host's policy.
+ *
+ * The residual workspace is the streams workspace with sections appended: no offset of the streams layout moves, so
+ * delora_odometry_streams_load_weights and delora_odometry_streams_reset work on it unchanged (_residual_init replaces
+ * _streams_init).  Appended, each 256-byte aligned, for S = max_batch streams of H x W cells: the point and normal grids
+ * (float4 per cell) of the S new frames and of the S previous frames (64 bytes per cell and stream), the S x 12
+ * transforms the ICP reads, its losses and dL/dT (computed, not returned) and its scratch for B = S
+ * (delora_icp_scratch_floats(S, H * W)); the index map of the new frames is the one the streams layout already has.
+ * Sizes from the host-only query (layers {2,2,2,2}, resnet_outputs 1000, two heads, n_stride 131072), streams ->
+ * residual workspace: 64 x 2048: S = 1 86.0 -> 99.3 MiB, S = 4 271.8 -> 325.0 MiB, S = 16 1015.1 -> 1227.9 MiB;
+ * 64 x 720: S = 1 46.2 -> 50.9 MiB, S = 4 112.8 -> 131.6 MiB, S = 16 379.1 -> 454.3 MiB.
+ *
+ * delora_odometry_streams_push_residual: T [S, 16] and valid [S] are what delora_odometry_streams_push writes for the
+ * same history, byte for byte: the new frames go through delora_project_normals_fwd, whose image is bit-identical to
+ * delora_project_fwd's, so the trunk input does not change.  The normals are estimated at the model's H x W on the raw
+ * frame with rp's neighbourhood: a serving-time signal on the images the model sees, not the training recipe's w_pre
+ * normals.  losses [S, DELORA_LOSS_ROW] (device, required): for every stream with valid[s] = 1 the row
+ * delora_icp_dense_fwd_bwd writes for source = this frame's grids moved by T[s], target = the previous frame's grids
+ * (the training step's orientation, scan_2 -> scan_1), bit-identical to that operator run alone at B = 1 on the two
+ * frames; rows with valid[s] = 0 are zeros.  The 3x4 part of T reaches the ICP on the device.
+ * The launch sequence depends on neither `active` nor the stream state (one captured call serves every tick), so the
+ * ICP runs at B = S every tick.  Streams without a transform cost it no search: a stream without a frame has empty
+ * grids from the projection, and a stream on its first frame since the start or a reset has its grids cached and then
+ * emptied before the ICP (odometry_streams_grids_kernel<0>), so no source pixel ever searches a stale or empty target;
+ * the valid streams' grids are cached after the ICP (<1>).  Each stream's grids are thus copied once per tick (64 bytes
+ * per cell read and written) and only when it has a frame; a separate staging grid for the ICP's sources would have
+ * copied every stream's grids twice and cost another 32 bytes per cell and stream.
+ * Measured on one H100 80GB HBM3 at a 700 W power limit (max SM clock 1980 MHz), graph-replayed ticks, all streams
+ * active, near-identity heads on consecutive synthetic frames, medians of alternating samples, _streams_push ->
+ * _streams_push_residual per tick: 64 x 2048: S = 1 1.20 -> 1.28 ms, S = 4 2.15 -> 2.30 ms,
+ * S = 16 8.22 -> 8.70 ms; 64 x 720: S = 1 1.13 -> 1.18 ms, S = 4 1.33 -> 1.40 ms, S = 16 4.97 -> 5.12 ms
+ * (scripts/gpu_odometry_eval.py, profiles/odometry_eval_h100_700w.json).
+ * Refused before any launch, naming the field or pointer: an invalid descriptor; null residual_params; a loss_flags
+ * without an ICP loss bit or with any bit other than DELORA_LOSS_PO2PO / _PO2PL / _PL2PL / DELORA_NORMAL_LINEAR; nb_h or
+ * nb_w not odd and positive; epsilon_range < 0; min_neighbors < 0; null points / n_points / workspace / T / valid /
+ * losses.  Models flagged DELORA_MODEL_NORMALIZATION_SCALING cannot be streamed here either. */
+typedef struct {
+    float lambda_po2pl;                  /* weight of po2pl in dL/dT only; the loss rows are unweighted */
+    uint32_t loss_flags;                 /* DELORA_LOSS_PO2PO / _PO2PL / _PL2PL (at least one), DELORA_NORMAL_LINEAR */
+    int nb_h, nb_w;                      /* neighborhood_side_length (7, 11): odd and positive */
+    float epsilon_range;                 /* 0.5 */
+    int min_neighbors;                   /* min_num_points_in_neighborhood_to_determine_point_class, 10 */
+} delora_odometry_residual_params;
+int64_t delora_odometry_streams_residual_workspace_bytes(const delora_odometry_desc* d);   /* host only, -1 if invalid */
+/* Zero the workspace (no stream has a previous frame, the ICP scratch is armed for B = S), arm the projection keys and
+ * empty the cached grids.  Once after allocation, instead of delora_odometry_streams_init. */
+int delora_odometry_streams_residual_init(const delora_odometry_desc* d, void* workspace, void* stream);
+int delora_odometry_streams_push_residual(const delora_odometry_desc* d, const delora_odometry_residual_params* rp,
+                                          const float* points, const int32_t* n_points, const int32_t* active,
+                                          void* workspace, float* T, int32_t* valid, float* losses, void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * Odometry training: raw scan pairs -> updated weights, one call per step.
  * Replaces, for the self-supervised step, deploy.deployer.Deployer.step + Trainer's Adam
@@ -655,6 +710,26 @@ int delora_odometry_train_init(const delora_odometry_desc* d, const float* weigh
 int delora_odometry_train_step(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
                                const float* points, const int32_t* n_points, int B, void* workspace,
                                float* losses, float* T, float* pooled, float* grads, void* stream);
+/* Evaluation on a training workspace: the ICP losses of the current weights on B pairs, nothing updated.  Replaces the
+ * loss branch of the reference's Tester (inference_only: False; src/deploy/tester.py:61-65 ->
+ * src/deploy/deployer.py:280-369) for a host that trains through delora_odometry_train_step and scores held-out
+ * sequences (training_identifiers / testing_identifiers) on the same workspace.  Same descriptor, hyperparameters,
+ * inputs and losses / T / pooled outputs as the step; it runs the step's projection + normals (at w_pre when set),
+ * forward and ICP losses (one function serves both) and stops: from the same workspace state and inputs its outputs are
+ * bit-identical to the step's (T of the weights before the update), and the master weights, the gradient, Adam's m, v
+ * and step count, the dropout seed and the bf16 filters are byte-for-byte unchanged.  Steps interleaved with evals of
+ * any B end in the state the steps alone reach, bit for bit (the eval records its batch size for the ICP scratch's
+ * re-arm).  Dropout is the identity, as at inference: DELORA_TRAIN_DROPOUT is accepted and ignored, so a host can pass
+ * the parameters it trains with, and the outputs are those of a step without the bit.  DELORA_LOSS_IDENTITY_FIT is
+ * accepted and ignored too: the identity objective belongs to the step's backward, column 5 of `losses` stays 0.
+ * DELORA_TRAIN_NORMALIZATION_SCALING acts as in the step (T in metres, the factor in column 6).  lr, betas and eps are
+ * validated and not used.  Launches only, capturable into a CUDA graph; the step's refusals, naming the argument.
+ * Measured on the H100 above (w_pre 0, lr 0, graph-replayed, medians of alternating samples), _train_step ->
+ * _train_eval: 64 x 720: B = 1 3.53 -> 1.19 ms, B = 4 4.43 -> 1.40 ms, B = 16 14.32 -> 5.20 ms; 64 x 2048: B = 1
+ * 3.73 -> 1.28 ms, B = 4 6.68 -> 2.34 ms, B = 16 22.97 -> 8.83 ms. */
+int delora_odometry_train_eval(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
+                               const float* points, const int32_t* n_points, int B, void* workspace,
+                               float* losses, float* T, float* pooled, void* stream);
 /* Copy the current fp32 master weights to `weights` (DEVICE fp32[weight_floats]): a .dlw blob, loadable by
  * delora_odometry_load_weights and delora_odometry_train_init. */
 int delora_odometry_train_weights(const delora_odometry_desc* d, const void* workspace, float* weights, void* stream);
