@@ -32,9 +32,23 @@ class OdometryResidualParams(ctypes.Structure):
                 ("epsilon_range", c_float), ("min_neighbors", c_int)]
 
 
+GRAD_ALLREDUCE_MAX_WORLD = 16       # DELORA_GRAD_ALLREDUCE_MAX_WORLD
+TRAIN_GROUP_BUCKETS = 5             # DELORA_TRAIN_GROUP_BUCKETS
+
+
+class OdometryTrainGroup(ctypes.Structure):
+    """delora_odometry_train_group (include/delora_b200.h): one rank's view of a data-parallel training group."""
+    _fields_ = [("rank", ctypes.c_int32), ("world", ctypes.c_int32),
+                ("peer_ws", ctypes.c_uint64 * GRAD_ALLREDUCE_MAX_WORLD),
+                ("peer_flags", ctypes.c_uint64 * GRAD_ALLREDUCE_MAX_WORLD), ("multicast", ctypes.c_uint64),
+                ("n_ctas", ctypes.c_int32), ("n_threads", ctypes.c_int32), ("status", c_void_p),
+                ("side_stream", c_void_p), ("fork_events", c_void_p * TRAIN_GROUP_BUCKETS), ("join_event", c_void_p)]
+
+
 c_desc_p = ctypes.POINTER(OdometryDesc)
 c_train_p = ctypes.POINTER(OdometryTrainParams)
 c_residual_p = ctypes.POINTER(OdometryResidualParams)
+c_group_p = ctypes.POINTER(OdometryTrainGroup)
 
 # name -> (restype, argtypes); every symbol declared in include/delora_b200.h
 SIGNATURES = {
@@ -133,6 +147,10 @@ SIGNATURES = {
     "delora_odometry_train_init": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_train_step": (c_int, [c_desc_p, c_train_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_train_step_group": (c_int, [c_desc_p, c_train_p, c_group_p, c_void_p, c_void_p, c_int, c_void_p,
+                                                 c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_train_grad_offset": (c_i64, [c_desc_p]),
+    "delora_odometry_train_group_buckets": (c_int, [c_desc_p, c_void_p, c_void_p]),
     "delora_odometry_train_eval": (c_int, [c_desc_p, c_train_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_void_p]),
     "delora_odometry_train_weights": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),

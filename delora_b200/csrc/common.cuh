@@ -238,6 +238,16 @@ __device__ __forceinline__ void quat_to_T_bwd_row(float qx, float qy, float qz, 
     gt[0] = g[3]; gt[1] = g[7]; gt[2] = g[11];
 }
 
+// The peer-memory gradient all-reduce (grad_allreduce.cu): its limits, and its launcher for the entry points that
+// validated their arguments.  seq_step non-NULL: the device-seq variant, seq = *seq_step * seq_stride + seq.
+constexpr int kArMaxThreads = 128;
+constexpr int kArMaxWorld = 16;
+constexpr int kArMaxCtas = 160;
+int grad_allreduce_launch(const uint64_t* peer_bufs, const uint64_t* peer_flags, uint64_t multicast_ptr, int rank,
+                          int world, long long offset, long long count, float scale, unsigned seq,
+                          const long long* seq_step, unsigned seq_stride, int n_ctas, int n_threads, int32_t* status,
+                          cudaStream_t st);
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

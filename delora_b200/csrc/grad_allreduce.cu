@@ -23,13 +23,16 @@
 // (start: all gradients of the bucket are written; end: all slices are stored), monotonically increasing
 // sequence numbers, no reset.  A wait that exceeds kArTimeoutNs sets *status and carries on: a lost peer shows
 // up as an error on the host, never as a hung GPU.
+//
+// Sequence numbers: delora_grad_allreduce_f32 takes `seq` from the host.  The group training step
+// (delora_odometry_train_step_group) launches the device-seq variant instead, which reads a step counter in device
+// memory at the start of the kernel, seq = step * seq_stride + seq_add: a CUDA graph that captured it replays a new
+// number every step, where a captured host value would repeat and every wait after the first replay would pass at once.
 #include "common.cuh"
 
 namespace delora {
 
-constexpr int kArMaxThreads = 128;
-constexpr int kArMaxWorld = 16;
-constexpr int kArMaxCtas = 160;
+static_assert(kArMaxWorld == DELORA_GRAD_ALLREDUCE_MAX_WORLD, "the header's world limit is the kernel's");
 constexpr unsigned long long kArTimeoutNs = 20ull * 1000ull * 1000ull * 1000ull;
 
 struct ArParams {
@@ -39,7 +42,9 @@ struct ArParams {
     int rank, world;
     long long off, count;                         // bucket = elements [off, off + count) of the flat buffer
     float scale;
-    unsigned seq;
+    unsigned seq;                                 // the host's sequence number, or seq_add of the device-seq variant
+    const long long* seq_step;                    // device-seq variant: seq = *seq_step * seq_stride + seq
+    unsigned seq_stride;
     int* status;
 };
 
@@ -83,14 +88,14 @@ __device__ __forceinline__ int ar_flag_index(int phase, int cta, int src) {
 }
 
 // All ranks' CTA `cta` meet: thread q tells rank q "rank `rank` reached `seq`", then waits for rank q's word here.
-__device__ __forceinline__ void ar_meet(const ArParams& p, int phase, int cta) {
+__device__ __forceinline__ void ar_meet(const ArParams& p, unsigned seq, int phase, int cta) {
     const int q = threadIdx.x;
     if (q < p.world) {
         unsigned* theirs = reinterpret_cast<unsigned*>(p.peer_flag[q]) + ar_flag_index(phase, cta, p.rank);
-        st_release_sys(theirs, p.seq);
+        st_release_sys(theirs, seq);
         const unsigned* mine = reinterpret_cast<const unsigned*>(p.peer_flag[p.rank]) + ar_flag_index(phase, cta, q);
         const unsigned long long t0 = global_timer_ns();
-        while ((int)(ld_acquire_sys(mine) - p.seq) < 0) {
+        while ((int)(ld_acquire_sys(mine) - seq) < 0) {
             if (global_timer_ns() - t0 > kArTimeoutNs) { atomicExch(p.status, 1 + q); break; }
             __nanosleep(64);
         }
@@ -98,11 +103,12 @@ __device__ __forceinline__ void ar_meet(const ArParams& p, int phase, int cta) {
     __syncthreads();
 }
 
-template <bool MC>
+template <bool MC, bool kDevSeq>
 __global__ void __launch_bounds__(kArMaxThreads)
 grad_allreduce_kernel(ArParams p) {
     const int cta = blockIdx.x;
-    ar_meet(p, 0, cta);                                             // every rank's bucket is complete
+    const unsigned seq = kDevSeq ? (unsigned)*p.seq_step * p.seq_stride + p.seq : p.seq;
+    ar_meet(p, seq, 0, cta);                                        // every rank's bucket is complete
 
     const long long n4 = p.count >> 2;
     const long long per = (n4 + p.world - 1) / p.world;
@@ -145,7 +151,34 @@ grad_allreduce_kernel(ArParams p) {
     }
     __threadfence_system();                                         // this thread's stores before the CTA's flag
     __syncthreads();
-    ar_meet(p, 1, cta);                                             // every rank's slice has landed everywhere
+    ar_meet(p, seq, 1, cta);                                        // every rank's slice has landed everywhere
+}
+
+// Both entry points validate their arguments before they get here; count > 0.
+int grad_allreduce_launch(const uint64_t* peer_bufs, const uint64_t* peer_flags, uint64_t multicast_ptr, int rank,
+                          int world, long long offset, long long count, float scale, unsigned seq,
+                          const long long* seq_step, unsigned seq_stride, int n_ctas, int n_threads, int32_t* status,
+                          cudaStream_t st) {
+    ArParams p;
+    for (int q = 0; q < kArMaxWorld; ++q) {
+        p.peer_buf[q] = q < world ? peer_bufs[q] : 0ull;
+        p.peer_flag[q] = q < world ? peer_flags[q] : 0ull;
+    }
+    p.mc = reinterpret_cast<float*>(multicast_ptr);
+    p.rank = rank; p.world = world; p.off = offset; p.count = count; p.scale = scale; p.seq = seq;
+    p.seq_step = seq_step; p.seq_stride = seq_stride; p.status = status;
+    if (seq_step) {
+        if (p.mc)
+            grad_allreduce_kernel<true, true><<<n_ctas, n_threads, 0, st>>>(p);
+        else
+            grad_allreduce_kernel<false, true><<<n_ctas, n_threads, 0, st>>>(p);
+    } else if (p.mc) {
+        grad_allreduce_kernel<true, false><<<n_ctas, n_threads, 0, st>>>(p);
+    } else {
+        grad_allreduce_kernel<false, false><<<n_ctas, n_threads, 0, st>>>(p);
+    }
+    DELORA_CHECK_LAUNCH("grad_allreduce_kernel");
+    return 0;
 }
 
 }  // namespace delora
@@ -167,21 +200,10 @@ extern "C" int delora_grad_allreduce_f32(const uint64_t* peer_bufs, const uint64
     DELORA_CHECK_ARG(n_threads >= 32 && n_threads <= kArMaxThreads && n_threads % 32 == 0,
                      "delora_grad_allreduce_f32: n_threads %d must be 32, 64, 96 or 128", n_threads);
     if (count == 0) return 0;
-    ArParams p;
-    for (int q = 0; q < kArMaxWorld; ++q) {
-        p.peer_buf[q] = q < world ? peer_bufs[q] : 0ull;
-        p.peer_flag[q] = q < world ? peer_flags[q] : 0ull;
-        DELORA_CHECK_ARG(q >= world || (p.peer_buf[q] && p.peer_flag[q] && (p.peer_buf[q] & 15) == 0),
+    for (int q = 0; q < world; ++q)
+        DELORA_CHECK_ARG(peer_bufs[q] && peer_flags[q] && (peer_bufs[q] & 15) == 0,
                          "delora_grad_allreduce_f32: peer %d has a null or unaligned mapping", q);
-    }
     DELORA_CHECK_ARG((multicast_ptr & 15) == 0, "delora_grad_allreduce_f32: unaligned multicast address");
-    p.mc = reinterpret_cast<float*>(multicast_ptr);
-    p.rank = rank; p.world = world; p.off = offset; p.count = count; p.scale = scale; p.seq = seq; p.status = status;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (p.mc)
-        grad_allreduce_kernel<true><<<n_ctas, n_threads, 0, st>>>(p);
-    else
-        grad_allreduce_kernel<false><<<n_ctas, n_threads, 0, st>>>(p);
-    DELORA_CHECK_LAUNCH("grad_allreduce_kernel");
-    return 0;
+    return grad_allreduce_launch(peer_bufs, peer_flags, multicast_ptr, rank, world, offset, count, scale, seq, nullptr, 0,
+                                 n_ctas, n_threads, status, (cudaStream_t)stream);
 }

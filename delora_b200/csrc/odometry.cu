@@ -1500,11 +1500,64 @@ static int check_train_call(const delora_odometry_desc* d, const delora_odometry
 
 }  // namespace delora
 
-extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
-                                          const float* points, const int32_t* n_points, int B, void* workspace,
-                                          float* losses, float* T, float* pooled, float* grads, void* stream) {
-    const char* who = "delora_odometry_train_step";
-    if (check_train_call(d, hp, points, n_points, B, workspace, who)) return 1;
+namespace delora {
+
+// The group step's all-reduce schedule (delora_odometry_train_group_buckets): bucket k of kGroupBuckets in launch
+// order, i.e. the backward's production order: heads + fc, layer4, layer3, layer2, stem + layer1.  Each boundary is a
+// stage boundary rounded up to 4 floats, so a bucket may take up to 3 floats of the section after it in the blob (which
+// the backward produced before it) and never one of the section before it (not produced yet).  The last bucket ends
+// at most 3 floats past blob_floats, in the gradient section's 256-byte padding, which nothing reads.
+constexpr int kGroupBuckets = DELORA_TRAIN_GROUP_BUCKETS;
+static void plan_buckets(const Model& m, long long off[kGroupBuckets], long long cnt[kGroupBuckets]) {
+    auto up4 = [](long long x) { return (x + 3) & ~3ll; };
+    long long edge[kGroupBuckets + 1];            // stage starts in blob order: stem, layer2, layer3, layer4, fc, end
+    edge[0] = 0;
+    for (int s = 1; s < 4; ++s) {
+        int i = 0;
+        while (m.t.block[i].stage < s) ++i;
+        edge[s] = up4(m.t.conv[m.t.block[i].c1].blob);
+    }
+    edge[4] = up4(m.fc.blob_w);
+    edge[5] = up4(m.blob_floats);
+    for (int k = 0; k < kGroupBuckets; ++k) {
+        off[k] = edge[4 - k];
+        cnt[k] = edge[5 - k] - edge[4 - k];
+    }
+}
+
+static int check_group(const delora_odometry_train_group* g, const void* workspace, const char* who) {
+    DELORA_CHECK_ARG(g != nullptr, "%s: null group", who);
+    DELORA_CHECK_ARG(g->world >= 1 && g->world <= kArMaxWorld, "%s: world=%d must be in [1, %d]", who, g->world,
+                     kArMaxWorld);
+    DELORA_CHECK_ARG(g->rank >= 0 && g->rank < g->world, "%s: rank=%d outside [0, world=%d)", who, g->rank, g->world);
+    for (int q = 0; q < g->world; ++q) {
+        DELORA_CHECK_ARG(g->peer_ws[q] != 0 && (g->peer_ws[q] & 15) == 0, "%s: peer_ws[%d] is null or not 16-byte aligned",
+                         who, q);
+        DELORA_CHECK_ARG(g->peer_flags[q] != 0 && (g->peer_flags[q] & 3) == 0,
+                         "%s: peer_flags[%d] is null or not 4-byte aligned", who, q);
+    }
+    DELORA_CHECK_ARG(g->peer_ws[g->rank] == (uint64_t)(uintptr_t)workspace, "%s: peer_ws[rank=%d] is not the workspace",
+                     who, g->rank);
+    DELORA_CHECK_ARG((g->multicast & 15) == 0, "%s: multicast is not 16-byte aligned", who);
+    DELORA_CHECK_ARG(g->status != nullptr, "%s: null status", who);
+    DELORA_CHECK_ARG(g->n_ctas >= 1 && g->n_ctas <= kArMaxCtas, "%s: n_ctas=%d outside [1, %d]", who, g->n_ctas,
+                     kArMaxCtas);
+    DELORA_CHECK_ARG(g->n_threads >= 32 && g->n_threads <= kArMaxThreads && g->n_threads % 32 == 0,
+                     "%s: n_threads=%d must be 32, 64, 96 or 128", who, g->n_threads);
+    if (g->world > 1) {
+        for (int k = 0; k < kGroupBuckets; ++k)
+            DELORA_CHECK_ARG(g->fork_events[k] != nullptr, "%s: null fork_events[%d]", who, k);
+        DELORA_CHECK_ARG(g->join_event != nullptr, "%s: null join_event", who);
+    }
+    return 0;
+}
+
+// delora_odometry_train_step, and with g (world > 1) its group form: bucket k is all-reduced on g->side_stream once
+// the backward has produced it, and `stream` joins g->side_stream before the gradient is read.
+static int train_step(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
+                      const delora_odometry_train_group* g, const float* points, const int32_t* n_points, int B,
+                      void* workspace, float* losses, float* T, float* pooled, float* grads, void* stream,
+                      const char* who) {
     const bool normalized = (hp->loss_flags & DELORA_TRAIN_NORMALIZATION_SCALING) != 0u;
     const bool dropout = (hp->loss_flags & DELORA_TRAIN_DROPOUT) != 0u;
     const bool identity = (hp->loss_flags & DELORA_LOSS_IDENTITY_FIT) != 0u;
@@ -1517,15 +1570,40 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
     long long* ctr = reinterpret_cast<long long*>(ws + tp.ctr);
     // the masks of this step, regenerated after odometry_out_bwd_kernel has advanced the step count
     const DropoutCtr drop_bwd{dropout ? ctr : nullptr, 1};
+    long long b_off[kGroupBuckets], b_cnt[kGroupBuckets];
+    uint64_t peer_grad[kArMaxWorld];
+    if (g) {
+        plan_buckets(m, b_off, b_cnt);
+        for (int q = 0; q < g->world; ++q) peer_grad[q] = g->peer_ws[q] + tp.grad;
+    }
+    cudaStream_t side = g ? (cudaStream_t)g->side_stream : nullptr;
+    // bucket k is complete on `st`: all-reduce it on the side stream; seq = the step count (advanced by
+    // odometry_out_bwd_kernel before bucket 0) * kGroupBuckets + k
+    auto all_reduce = [&](int k) -> int {
+        cudaError_t e = cudaEventRecord((cudaEvent_t)g->fork_events[k], st);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(side, (cudaEvent_t)g->fork_events[k], 0);
+        DELORA_CHECK_ARG(e == cudaSuccess, "%s: fork_events[%d]: %s", who, k, cudaGetErrorString(e));
+        return grad_allreduce_launch(peer_grad, g->peer_flags, g->multicast ? g->multicast + tp.grad : 0ull, g->rank,
+                                     g->world, b_off[k], b_cnt[k], 1.0f / (float)g->world, (unsigned)k, ctr,
+                                     (unsigned)kGroupBuckets, g->n_ctas, g->n_threads, g->status, side);
+    };
     int rc;
     // 1-3. projection + normals, forward, ICP losses and dL/dT
     if ((rc = train_forward_losses(d, hp, tp, ws, points, n_points, B, dropout, T, st, who))) return rc;
     // 4. backward: tail (dL/dT of the ICP mean or of the identity fit), average pool, trunk
     if ((rc = train_tail_backward(tp, ws, d->act, B, identity, st, drop_bwd))) return rc;
+    if (g && (rc = all_reduce(0))) return rc;
     float* conv_dw[kMaxConv];
     for (int i = 0; i < m.t.n_conv; ++i) conv_dw[i] = f(tp.grad) + m.t.conv[i].blob;
-    for (int s = 3; s >= 0; --s)
+    for (int s = 3; s >= 0; --s) {
         if ((rc = trunk_backward(m.t, tp.t, ws, tp.w, ws, d->act, B, f(tp.g_pooled), conv_dw, s, st, drop_bwd))) return rc;
+        if (g && (rc = all_reduce(4 - s))) return rc;
+    }
+    if (g) {
+        cudaError_t e = cudaEventRecord((cudaEvent_t)g->join_event, side);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(st, (cudaEvent_t)g->join_event, 0);
+        DELORA_CHECK_ARG(e == cudaSuccess, "%s: join_event: %s", who, cudaGetErrorString(e));
+    }
     // outputs (T: the weights before the update)
     if ((rc = train_outputs(tp, ws, B, normalized, losses, T, pooled, st, who))) return rc;
     if (grads) {
@@ -1541,6 +1619,46 @@ extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const d
                                                hp->beta2, hp->eps);
     DELORA_CHECK_LAUNCH("odometry_adam_kernel");
     return delora_conv_weight_prep_multi(ws + tp.w.table, m.t.n_conv, st);
+}
+
+}  // namespace delora
+
+extern "C" int delora_odometry_train_step(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
+                                          const float* points, const int32_t* n_points, int B, void* workspace,
+                                          float* losses, float* T, float* pooled, float* grads, void* stream) {
+    const char* who = "delora_odometry_train_step";
+    if (check_train_call(d, hp, points, n_points, B, workspace, who)) return 1;
+    return train_step(d, hp, nullptr, points, n_points, B, workspace, losses, T, pooled, grads, stream, who);
+}
+
+extern "C" int delora_odometry_train_step_group(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
+                                                const delora_odometry_train_group* g, const float* points,
+                                                const int32_t* n_points, int B, void* workspace, float* losses,
+                                                float* T, float* pooled, float* grads, void* stream) {
+    const char* who = "delora_odometry_train_step_group";
+    if (check_train_call(d, hp, points, n_points, B, workspace, who)) return 1;
+    if (check_group(g, workspace, who)) return 1;
+    return train_step(d, hp, g->world > 1 ? g : nullptr, points, n_points, B, workspace, losses, T, pooled, grads,
+                      stream, who);
+}
+
+extern "C" int64_t delora_odometry_train_grad_offset(const delora_odometry_desc* d) {
+    if (check_train_desc(d, "delora_odometry_train_grad_offset")) return -1;
+    TrainPlan tp;
+    make_train_plan(d, &tp);
+    return (int64_t)tp.grad;
+}
+
+extern "C" int delora_odometry_train_group_buckets(const delora_odometry_desc* d, int64_t* offsets, int64_t* counts) {
+    const char* who = "delora_odometry_train_group_buckets";
+    if (check_train_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(offsets && counts, "%s: null pointer", who);
+    Model m;
+    plan_model(d, &m);
+    long long off[kGroupBuckets], cnt[kGroupBuckets];
+    plan_buckets(m, off, cnt);
+    for (int k = 0; k < kGroupBuckets; ++k) { offsets[k] = off[k]; counts[k] = cnt[k]; }
+    return 0;
 }
 
 extern "C" int delora_odometry_train_eval(const delora_odometry_desc* d, const delora_odometry_train_params* hp,

@@ -1,6 +1,7 @@
 """ctypes binding of the odometry workspaces of the C ABI (include/delora_b200.h): inference (`delora_odometry_pairs` /
 `_pairs_normalized` / `_push`), streams (`delora_odometry_streams_*`, with the per-frame ICP residual
-`delora_odometry_streams_residual_*` / `_push_residual`) and training (`delora_odometry_train_*`).
+`delora_odometry_streams_residual_*` / `_push_residual`) and training (`delora_odometry_train_*`, and
+`delora_odometry_train_step_group` for several workspaces stepped as one data-parallel group).
 
 Each class holds one descriptor and one workspace, a torch uint8 tensor on the current device.  Every call runs on
 torch's current stream at call time, checks its status with `_lib.check` and does not synchronise (except
@@ -160,19 +161,31 @@ class TrainingWorkspace(_Workspace):
     def _floats(self):
         return torch.empty((self.n,), dtype=torch.float32, device=self.workspace.device)
 
+    def _step_outputs(self, b, outputs):
+        if not outputs:
+            return None, (None,) * 4
+        dev = self.workspace.device
+        out = (torch.empty((b, ops.LOSS_ROW), dtype=torch.float32, device=dev),
+               torch.empty((b, 4, 4), dtype=torch.float32, device=dev),
+               torch.empty((b, 512), dtype=torch.float32, device=dev), self._floats())
+        return out, tuple(t.data_ptr() for t in out)
+
     def step(self, points, counts, outputs=True):
         """One step on B = rows // 2 pairs -> (losses [B, 8], T [B, 4, 4], pooled [B, 512], grads [n]), or None
         without outputs.  Normalised models: losses[:, 6] is each pair's factor and T's translation is in metres."""
         b = points.shape[0] // 2
-        out, ptrs = None, (None,) * 4
-        if outputs:
-            dev = self.workspace.device
-            out = (torch.empty((b, ops.LOSS_ROW), dtype=torch.float32, device=dev),
-                   torch.empty((b, 4, 4), dtype=torch.float32, device=dev),
-                   torch.empty((b, 512), dtype=torch.float32, device=dev), self._floats())
-            ptrs = tuple(t.data_ptr() for t in out)
+        out, ptrs = self._step_outputs(b, outputs)
         self._call("delora_odometry_train_step", self._params, points.data_ptr(), counts.data_ptr(), b,
                    self.workspace.data_ptr(), *ptrs)
+        return out
+
+    def step_group(self, group, points, counts, outputs=True):
+        """delora_odometry_train_step_group with `group` (a _lib.OdometryTrainGroup whose rank is this workspace):
+        step's outputs, grads being the gradient averaged over the group."""
+        b = points.shape[0] // 2
+        out, ptrs = self._step_outputs(b, outputs)
+        self._call("delora_odometry_train_step_group", self._params, ctypes.byref(group), points.data_ptr(),
+                   counts.data_ptr(), b, self.workspace.data_ptr(), *ptrs)
         return out
 
     def eval(self, points, counts):
@@ -211,3 +224,47 @@ class TrainingWorkspace(_Workspace):
         self._call("delora_odometry_train_set_state", *(a.data_ptr() for a in args), step_t.data_ptr(),
                    self.workspace.data_ptr())
         torch.cuda.synchronize()
+
+
+class TrainingGroup:
+    """The delora_odometry_train_group of each of N TrainingWorkspaces (same descriptor and state), on N devices with
+    peer access enabled between them or all on one device: the flag words and status word of every rank (on its
+    workspace's device, zeroed), a side stream and the six events per rank, unicast path.  `groups[r]` is rank r's
+    descriptor; `step(r, ...)` runs rank r's group step on the current stream of its device."""
+
+    def __init__(self, workspaces, n_ctas=8, n_threads=128):
+        L = _lib.lib()
+        world = len(workspaces)
+        self.workspaces = workspaces
+        self.flags = [torch.zeros(L.delora_grad_allreduce_flag_words(), dtype=torch.int32, device=w.workspace.device)
+                      for w in workspaces]
+        self.status = [torch.zeros(1, dtype=torch.int32, device=w.workspace.device) for w in workspaces]
+        self.side_streams, self.events, self.groups = [], [], []
+        for r, w in enumerate(workspaces):
+            dev = w.workspace.device
+            side = torch.cuda.Stream(device=dev)
+            events = [torch.cuda.Event() for _ in range(_lib.TRAIN_GROUP_BUCKETS + 1)]
+            with torch.cuda.device(dev):
+                for e in events:                    # torch creates the CUDA event at its first record
+                    e.record(side)
+            g = _lib.OdometryTrainGroup(rank=r, world=world, multicast=0, n_ctas=n_ctas, n_threads=n_threads,
+                                        status=self.status[r].data_ptr(), side_stream=side.cuda_stream,
+                                        join_event=events[-1].cuda_event)
+            for q in range(world):
+                g.peer_ws[q] = workspaces[q].workspace.data_ptr()
+                g.peer_flags[q] = self.flags[q].data_ptr()
+            for k in range(_lib.TRAIN_GROUP_BUCKETS):
+                g.fork_events[k] = events[k].cuda_event
+            self.side_streams.append(side)
+            self.events.append(events)
+            self.groups.append(g)
+        for w in workspaces:
+            torch.cuda.synchronize(w.workspace.device)
+
+    def step(self, rank, points, counts, outputs=True):
+        return self.workspaces[rank].step_group(self.groups[rank], points, counts, outputs)
+
+    def reset_flags(self):
+        """Zero every rank's flag words (after a set_state that moved the step count; no step in flight)."""
+        for f in self.flags:
+            f.zero_()

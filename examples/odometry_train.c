@@ -2,8 +2,8 @@
  * The reference's training loop (src/deploy/trainer.py, Trainer.train) from a C host: no Python, no torch.  Links
  * libdelora_b200.so and cudart only.
  *
- *   odometry_train [--lr LR] [--switch-below L] [--dropout-seed S] [--eval-dir DIR] in.dlt|in.dlw out.dlt epochs B
- *                  scan_000.bin ...
+ *   odometry_train [--lr LR] [--switch-below L] [--dropout-seed S] [--eval-dir DIR] [--gpus N] in.dlt|in.dlw out.dlt
+ *                  epochs B scan_000.bin ...
  *
  * Reads a training checkpoint (.dlt: weights, Adam's state, epoch and phase; layout in include/delora_b200.h) or a
  * weight file (.dlw: a fresh Adam with learning rate --lr, default 1e-5, the reference's learning_rate) and a list of
@@ -25,11 +25,19 @@
  * every epoch the mean ICP objective (po2po + lambda * po2pl + pl2pl per pair) over its consecutive pairs, through
  * delora_odometry_train_eval on the training workspace, is appended to the epoch's line as "held-out <mean>".  The
  * evaluation updates nothing: out.dlt has the bytes of a run without the option.
+ * --gpus N (N > 1): data-parallel training on GPUs 0 .. N-1 of this process, one host thread per GPU, peer access
+ * enabled both ways, delora_odometry_train_step_group on the unicast path (the gradient of every step is the mean over
+ * the GPUs).  The pairs are split into N contiguous shards of n_pairs / N pairs (as parallel_grad.shard_pairs does; the
+ * remainder is left out so that every GPU steps the same batch sizes), each GPU walks its shard B pairs per step, and
+ * the epoch's objective is the mean over the GPUs of their mean objectives.  GPU r draws its dropout masks with seed
+ * + r; the .dlt keeps the seed.  GPU 0 writes out.dlt and runs --eval-dir.  Without the option, or with --gpus 1, the
+ * program runs on the current GPU through delora_odometry_train_step.
  *
  * Build:  cc odometry_train.c -I include -I $CUDA_HOME/include -L delora_b200 -ldelora_b200 \
- *            -L $CUDA_HOME/lib64 -lcudart -Wl,-rpath,$PWD/delora_b200 -o odometry_train
+ *            -L $CUDA_HOME/lib64 -lcudart -lpthread -Wl,-rpath,$PWD/delora_b200 -o odometry_train
  */
 #include <dirent.h>
+#include <pthread.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -156,22 +164,154 @@ static int write_dlt(const char* path, const delora_odometry_train_file_header* 
     return 0;
 }
 
+/* the mean ICP objective of the held-out pairs with the workspace's weights (delora_odometry_train_eval); -1 on error */
+static int held_out(const delora_odometry_desc* d, const delora_odometry_train_params* hp, const float* h_eval_scans,
+                    const int32_t* h_eval_counts, int n_eval_pairs, int B_max, size_t scan_floats, void* workspace,
+                    float* points, int32_t* counts, float* losses, float* h_losses, int32_t* h_step_counts,
+                    cudaStream_t stream, double* mean) {
+    double held = 0.0;
+    for (int k0 = 0; k0 < n_eval_pairs; k0 += B_max) {
+        const int B = n_eval_pairs - k0 < B_max ? n_eval_pairs - k0 : B_max;
+        if (stage_pairs(h_eval_scans, h_eval_counts, k0, B, scan_floats, points, counts, h_step_counts, stream))
+            return 1;
+        DELORA_OK(delora_odometry_train_eval(d, hp, points, counts, B, workspace, losses, NULL, NULL, stream));
+        CUDA_OK(cudaMemcpyAsync(h_losses, losses, (size_t)B * DELORA_LOSS_ROW * sizeof(float), cudaMemcpyDeviceToHost,
+                                stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+        held += icp_objective(h_losses, B, hp->lambda_po2pl) * B;
+    }
+    *mean = held / n_eval_pairs;
+    return 0;
+}
+
+/* --gpus N: one GPU of the group, and the epoch its thread runs */
+typedef struct {
+    int rank;
+    const delora_odometry_desc* d;
+    delora_odometry_train_params hp;
+    delora_odometry_train_group g;
+    const float* h_scans;
+    const int32_t* h_counts;
+    int first, n_pairs, B_max, identity;      /* its shard: pairs first .. first + n_pairs - 1 */
+    size_t scan_floats;
+    cudaStream_t stream, side;
+    cudaEvent_t events[DELORA_TRAIN_GROUP_BUCKETS + 1];
+    void* workspace;
+    float *points, *losses, *h_losses;
+    int32_t *counts, *h_step_counts, *flags, *status;
+    double mean;                              /* the epoch's mean objective on this GPU */
+    int rc;
+} rank_state;
+
+static int rank_epoch(rank_state* r) {
+    CUDA_OK(cudaSetDevice(r->rank));
+    double sum = 0.0;
+    int steps = 0;
+    for (int k0 = 0; k0 < r->n_pairs; k0 += r->B_max, ++steps) {
+        const int B = r->n_pairs - k0 < r->B_max ? r->n_pairs - k0 : r->B_max;
+        if (stage_pairs(r->h_scans, r->h_counts, r->first + k0, B, r->scan_floats, r->points, r->counts,
+                        r->h_step_counts, r->stream))
+            return 1;
+        DELORA_OK(delora_odometry_train_step_group(r->d, &r->hp, &r->g, r->points, r->counts, B, r->workspace,
+                                                   r->losses, NULL, NULL, NULL, r->stream));
+        CUDA_OK(cudaMemcpyAsync(r->h_losses, r->losses, (size_t)B * DELORA_LOSS_ROW * sizeof(float),
+                                cudaMemcpyDeviceToHost, r->stream));
+        CUDA_OK(cudaStreamSynchronize(r->stream));
+        sum += r->identity ? (double)r->h_losses[(size_t)(B - 1) * DELORA_LOSS_ROW + 5]
+                           : icp_objective(r->h_losses, B, r->hp.lambda_po2pl);
+    }
+    int32_t status = 0;
+    CUDA_OK(cudaMemcpy(&status, r->status, sizeof status, cudaMemcpyDeviceToHost));
+    if (status != 0) return fail("a GPU of the group did not reach the gradient all-reduce in time");
+    r->mean = steps > 0 ? sum / steps : 0.0;
+    return 0;
+}
+
+static void* rank_thread(void* arg) {
+    rank_state* r = (rank_state*)arg;
+    r->rc = rank_epoch(r);
+    return NULL;
+}
+
+/* one GPU's workspace, buffers, streams and events, its state from the host arrays; 0 on success */
+static int rank_setup(rank_state* r, int world, float* const* h_state, size_t n, int64_t step, uint64_t dropout_seed,
+                      int64_t ws_bytes) {
+    CUDA_OK(cudaSetDevice(r->rank));
+    for (int q = 0; q < world; ++q) {
+        int can = 0;
+        if (q == r->rank) continue;
+        CUDA_OK(cudaDeviceCanAccessPeer(&can, r->rank, q));
+        if (!can) return fail("--gpus: a pair of GPUs has no peer access");
+        const cudaError_t e = cudaDeviceEnablePeerAccess(q, 0);
+        if (e == cudaErrorPeerAccessAlreadyEnabled) cudaGetLastError();
+        else CUDA_OK(e);
+    }
+    CUDA_OK(cudaStreamCreate(&r->stream));
+    CUDA_OK(cudaStreamCreate(&r->side));
+    for (int k = 0; k <= DELORA_TRAIN_GROUP_BUCKETS; ++k)
+        CUDA_OK(cudaEventCreateWithFlags(&r->events[k], cudaEventDisableTiming));
+    float* d_state[3];
+    int64_t* d_step;
+    for (int i = 0; i < 3; ++i) {
+        CUDA_OK(cudaMalloc((void**)&d_state[i], n * sizeof(float)));
+        CUDA_OK(cudaMemcpy(d_state[i], h_state[i], n * sizeof(float), cudaMemcpyHostToDevice));
+    }
+    CUDA_OK(cudaMalloc((void**)&d_step, sizeof(int64_t)));
+    CUDA_OK(cudaMemcpy(d_step, &step, sizeof(int64_t), cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMalloc(&r->workspace, (size_t)ws_bytes));
+    CUDA_OK(cudaMalloc((void**)&r->points, (size_t)2 * r->B_max * r->scan_floats * sizeof(float)));
+    CUDA_OK(cudaMalloc((void**)&r->counts, (size_t)2 * r->B_max * sizeof(int32_t)));
+    CUDA_OK(cudaMalloc((void**)&r->losses, (size_t)r->B_max * DELORA_LOSS_ROW * sizeof(float)));
+    CUDA_OK(cudaMalloc((void**)&r->flags, (size_t)delora_grad_allreduce_flag_words() * sizeof(uint32_t)));
+    CUDA_OK(cudaMemset(r->flags, 0, (size_t)delora_grad_allreduce_flag_words() * sizeof(uint32_t)));
+    CUDA_OK(cudaMalloc((void**)&r->status, sizeof(int32_t)));
+    CUDA_OK(cudaMemset(r->status, 0, sizeof(int32_t)));
+    r->h_losses = (float*)malloc((size_t)r->B_max * DELORA_LOSS_ROW * sizeof(float));
+    r->h_step_counts = (int32_t*)malloc((size_t)2 * r->B_max * sizeof(int32_t));
+    if (!r->h_losses || !r->h_step_counts) return fail("out of host memory");
+    DELORA_OK(delora_odometry_train_init(r->d, d_state[0], r->workspace, r->stream));
+    DELORA_OK(delora_odometry_train_set_state(r->d, d_state[0], d_state[1], d_state[2], d_step, r->workspace,
+                                              r->stream));
+    DELORA_OK(delora_odometry_train_set_dropout_seed(r->d, dropout_seed + (uint64_t)r->rank, r->workspace, r->stream));
+    CUDA_OK(cudaStreamSynchronize(r->stream));
+    for (int i = 0; i < 3; ++i) cudaFree(d_state[i]);
+    cudaFree(d_step);
+    return 0;
+}
+
+static void rank_release(rank_state* r) {
+    cudaSetDevice(r->rank);
+    free(r->h_step_counts);
+    free(r->h_losses);
+    cudaFree(r->status);
+    cudaFree(r->flags);
+    cudaFree(r->losses);
+    cudaFree(r->counts);
+    cudaFree(r->points);
+    cudaFree(r->workspace);
+    for (int k = 0; k <= DELORA_TRAIN_GROUP_BUCKETS; ++k) cudaEventDestroy(r->events[k]);
+    cudaStreamDestroy(r->side);
+    cudaStreamDestroy(r->stream);
+}
+
 int main(int argc, char** argv) {
     float lr = 1e-5f;
     double switch_below = 1e-2;
     const char* seed_arg = getenv("DELORA_DROPOUT_SEED");
     const char* eval_dir = NULL;
+    int gpus = 1;
     int a = 1;
     for (; a + 1 < argc && strncmp(argv[a], "--", 2) == 0; a += 2) {
         if (strcmp(argv[a], "--lr") == 0) lr = (float)atof(argv[a + 1]);
         else if (strcmp(argv[a], "--switch-below") == 0) switch_below = atof(argv[a + 1]);
         else if (strcmp(argv[a], "--dropout-seed") == 0) seed_arg = argv[a + 1];
         else if (strcmp(argv[a], "--eval-dir") == 0) eval_dir = argv[a + 1];
+        else if (strcmp(argv[a], "--gpus") == 0) gpus = atoi(argv[a + 1]);
         else return fail("unknown option");
     }
     if (argc - a < 6)
-        return fail("usage: odometry_train [--lr LR] [--switch-below L] [--dropout-seed S] [--eval-dir DIR] in.dlt|in.dlw "
-                    "out.dlt epochs B scan.bin scan.bin [scan.bin ...]");
+        return fail("usage: odometry_train [--lr LR] [--switch-below L] [--dropout-seed S] [--eval-dir DIR] [--gpus N] "
+                    "in.dlt|in.dlw out.dlt epochs B scan.bin scan.bin [scan.bin ...]");
     const char* in_path = argv[a];
     const char* out_path = argv[a + 1];
     const int epochs = atoi(argv[a + 2]);
@@ -249,6 +389,107 @@ int main(int argc, char** argv) {
     hp.epsilon_range = 0.5f;
     hp.min_neighbors = 10;
 
+    if (gpus < 1 || gpus > DELORA_GRAD_ALLREDUCE_MAX_WORLD) return fail("--gpus must be in [1, 16]");
+    if (gpus > 1) {
+        int n_dev = 0;
+        CUDA_OK(cudaGetDeviceCount(&n_dev));
+        if (gpus > n_dev) return fail("--gpus: more GPUs than the machine has");
+        const int per = n_pairs / gpus;
+        if (per < 1) return fail("--gpus: fewer pairs than GPUs");
+        if (per * gpus < n_pairs)
+            fprintf(stderr, "odometry_train: %d GPUs x %d pairs, the last %d pair(s) left out\n", gpus, per,
+                    n_pairs - per * gpus);
+        const int64_t ws_bytes = delora_odometry_train_workspace_bytes(d);
+        if (ws_bytes < 0) return fail(delora_last_error());
+        rank_state* ranks = (rank_state*)calloc((size_t)gpus, sizeof *ranks);
+        pthread_t* threads = (pthread_t*)calloc((size_t)gpus, sizeof *threads);
+        if (!ranks || !threads) return fail("out of host memory");
+        for (int r = 0; r < gpus; ++r) {
+            rank_state* R = &ranks[r];
+            R->rank = r; R->d = d; R->h_scans = h_scans; R->h_counts = h_counts;
+            R->first = r * per; R->n_pairs = per; R->B_max = B_max; R->scan_floats = scan_floats;
+            if (rank_setup(R, gpus, h_state, n, hdr.step, dropout_seed, ws_bytes)) return 1;
+        }
+        for (int r = 0; r < gpus; ++r) {
+            delora_odometry_train_group* g = &ranks[r].g;
+            memset(g, 0, sizeof *g);
+            g->rank = r; g->world = gpus;
+            for (int q = 0; q < gpus; ++q) {
+                g->peer_ws[q] = (uint64_t)(uintptr_t)ranks[q].workspace;
+                g->peer_flags[q] = (uint64_t)(uintptr_t)ranks[q].flags;
+            }
+            g->multicast = 0;
+            g->n_ctas = 16; g->n_threads = 128;
+            g->status = ranks[r].status;
+            g->side_stream = ranks[r].side;
+            for (int k = 0; k < DELORA_TRAIN_GROUP_BUCKETS; ++k) g->fork_events[k] = ranks[r].events[k];
+            g->join_event = ranks[r].events[DELORA_TRAIN_GROUP_BUCKETS];
+        }
+        CUDA_OK(cudaSetDevice(0));
+        float* d_state[3];
+        int64_t* d_step;
+        for (int i = 0; i < 3; ++i) CUDA_OK(cudaMalloc((void**)&d_state[i], n * sizeof(float)));
+        CUDA_OK(cudaMalloc((void**)&d_step, sizeof(int64_t)));
+        if (dropout) fprintf(stderr, "odometry_train: dropout on, seed %llu + GPU\n", (unsigned long long)dropout_seed);
+        fprintf(stderr, "odometry_train: epoch %d, Adam step %lld, %s, %d pairs on %d GPUs\n", hdr.epoch,
+                (long long)hdr.step, hdr.unsupervised ? "unsupervised" : "identity pre-training", per * gpus, gpus);
+        rank_state* R0 = &ranks[0];
+        for (int e = 0; e < epochs; ++e) {
+            hp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | (hdr.unsupervised ? 0u : DELORA_LOSS_IDENTITY_FIT) |
+                            (normalized ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u) | (dropout ? DELORA_TRAIN_DROPOUT : 0u);
+            for (int r = 0; r < gpus; ++r) {
+                ranks[r].hp = hp;
+                ranks[r].identity = !hdr.unsupervised;
+                if (pthread_create(&threads[r], NULL, rank_thread, &ranks[r]) != 0) return fail("cannot start a thread");
+            }
+            double mean = 0.0;
+            int failed = 0;
+            for (int r = 0; r < gpus; ++r) {
+                pthread_join(threads[r], NULL);
+                failed |= ranks[r].rc;
+                mean += ranks[r].mean;
+            }
+            if (failed) return 1;
+            mean /= gpus;
+            printf("epoch %d objective %.9g unsupervised %d", hdr.epoch, mean, hdr.unsupervised);
+            CUDA_OK(cudaSetDevice(0));
+            if (eval_dir) {
+                double held;
+                if (held_out(d, &hp, h_eval_scans, h_eval_counts, n_eval_pairs, B_max, scan_floats, R0->workspace,
+                             R0->points, R0->counts, R0->losses, R0->h_losses, R0->h_step_counts, R0->stream, &held))
+                    return 1;
+                printf(" held-out %.9g", held);
+            }
+            printf("\n");
+            hdr.epoch += 1;
+            hdr.loss = (float)mean;
+            if (!hdr.unsupervised && mean < switch_below) {
+                hdr.unsupervised = 1;
+                fprintf(stderr, "odometry_train: objective below %g, switching to the unsupervised objective\n",
+                        switch_below);
+            }
+            /* every GPU holds the same state: GPU 0's goes to the file */
+            DELORA_OK(delora_odometry_train_get_state(d, R0->workspace, d_state[0], d_state[1], d_state[2], d_step,
+                                                      R0->stream));
+            for (int i = 0; i < 3; ++i)
+                CUDA_OK(cudaMemcpyAsync(h_state[i], d_state[i], n * sizeof(float), cudaMemcpyDeviceToHost, R0->stream));
+            CUDA_OK(cudaMemcpyAsync(&hdr.step, d_step, sizeof(int64_t), cudaMemcpyDeviceToHost, R0->stream));
+            CUDA_OK(cudaStreamSynchronize(R0->stream));
+            if (write_dlt(out_path, &hdr, h_state, n)) return 1;
+        }
+        for (int i = 0; i < 3; ++i) cudaFree(d_state[i]);
+        cudaFree(d_step);
+        for (int r = 0; r < gpus; ++r) rank_release(&ranks[r]);
+        free(threads);
+        free(ranks);
+        for (int i = 0; i < 3; ++i) free(h_state[i]);
+        free(h_eval_counts);
+        free(h_eval_scans);
+        free(h_counts);
+        free(h_scans);
+        return 0;
+    }
+
     cudaStream_t stream;
     CUDA_OK(cudaStreamCreate(&stream));
     float *d_state[3], *points, *losses;
@@ -298,18 +539,11 @@ int main(int argc, char** argv) {
         const double mean = steps > 0 ? sum / steps : 0.0;
         printf("epoch %d objective %.9g unsupervised %d", hdr.epoch, mean, hdr.unsupervised);
         if (eval_dir) {         /* the held-out pairs with the weights after the epoch; no update, no dropout */
-            double held = 0.0;
-            for (int k0 = 0; k0 < n_eval_pairs; k0 += B_max) {
-                const int B = n_eval_pairs - k0 < B_max ? n_eval_pairs - k0 : B_max;
-                if (stage_pairs(h_eval_scans, h_eval_counts, k0, B, scan_floats, points, counts, h_step_counts, stream))
-                    return 1;
-                DELORA_OK(delora_odometry_train_eval(d, &hp, points, counts, B, workspace, losses, NULL, NULL, stream));
-                CUDA_OK(cudaMemcpyAsync(h_losses, losses, (size_t)B * DELORA_LOSS_ROW * sizeof(float),
-                                        cudaMemcpyDeviceToHost, stream));
-                CUDA_OK(cudaStreamSynchronize(stream));
-                held += icp_objective(h_losses, B, hp.lambda_po2pl) * B;
-            }
-            printf(" held-out %.9g", held / n_eval_pairs);
+            double held;
+            if (held_out(d, &hp, h_eval_scans, h_eval_counts, n_eval_pairs, B_max, scan_floats, workspace, points, counts,
+                         losses, h_losses, h_step_counts, stream, &held))
+                return 1;
+            printf(" held-out %.9g", held);
         }
         printf("\n");
         hdr.epoch += 1;

@@ -812,6 +812,79 @@ int delora_grad_allreduce_f32(const uint64_t* peer_bufs, const uint64_t* peer_fl
                               int world, long long offset, long long count, float scale, uint32_t seq, int n_ctas,
                               int n_threads, int32_t* status, void* stream);
 
+/* ---- Data-parallel training through the C ABI: delora_odometry_train_step on several GPUs, the gradient averaged
+ * over the ranks inside the step (the C route of the Python Trainer's bucketed all-reduce, parallel_grad.py).
+ *
+ * Every rank owns one training workspace (same descriptor, same weights, same Adam state and step count) and calls
+ * delora_odometry_train_step_group once per step on its own B pairs.  The step is _train_step with one change: Adam
+ * consumes the MEAN over the ranks of the gradient (scale 1 / world on the sum over ranks q = 0 .. world-1 in that
+ * order, as BucketedGradAllReduce; every rank ends with bit-identical weights, m and v).  Each rank's objective is its
+ * own mean over its B pairs (its quaternion block normalised over its own B), so with equal B on every rank the
+ * average reproduces the reference's `loss / batch_size` over the global batch (src/deploy/deployer.py:329-342);
+ * unequal B gives an unweighted mean of the ranks' means.  losses, T and pooled stay local to the rank; grads, if
+ * non-NULL, receives the averaged gradient.
+ *
+ * Overlap: the gradient is produced in DELORA_TRAIN_GROUP_BUCKETS buckets, in the backward's order over the blob (the
+ * blob is in state_dict order: stem, layer1 .. layer4, fc, heads): [0] heads + fc after the tail backward, [1] layer4
+ * after stage 3, [2] layer3, [3] layer2, [4] stem + layer1 after stage 0.  Each bucket is all-reduced
+ * (delora_grad_allreduce_f32's kernel, in place in every rank's gradient section) on side_stream as soon as its stage
+ * is done, while the next stage's backward runs on `stream`; `stream` joins side_stream before Adam.  Bucket
+ * boundaries are stage boundaries rounded UP to a multiple of 4 floats (the kernel moves float4s), so a bucket holds
+ * at most 3 floats of the section after it, which the backward produced earlier, and never one it has not produced
+ * yet; the last bucket ends at most 3 floats past the blob, inside the gradient section's padding.
+ * delora_odometry_train_group_buckets gives the table, delora_odometry_train_grad_offset where the gradient section
+ * starts, so a host that brings its own collective (NCCL, MPI) can reproduce the schedule.
+ *
+ * Sequence numbers come from the device: bucket k of the step that takes the Adam step count to s uses
+ * seq = s * DELORA_TRAIN_GROUP_BUCKETS + k, read from the workspace by the kernel, so one captured step replays
+ * correctly.  The flag words must be zeroed on every rank before the first group step, must serve no other all-reduce,
+ * and must be zeroed again on every rank (with no step in flight) whenever delora_odometry_train_set_state changes the
+ * step count, which all ranks must always share.
+ *
+ * Memory: peer_ws[q] is where rank q's training workspace is mapped in this process (peer_ws[rank] = `workspace`).
+ * In one process: device pointers with cudaDeviceEnablePeerAccess both ways (examples/odometry_train.c --gpus N).  In
+ * several processes: allocate each workspace with cuMemCreate (a shareable handle type), export and exchange the
+ * handles, and cuMemMap + cuMemSetAccess every peer's into each process; a multicast object bound to all workspaces
+ * (cuMulticastCreate / cuMulticastBindMem) gives `multicast`, the address of the workspace's multicast mapping.
+ * The step allocates nothing and creates no stream or event: side_stream, fork_events and join_event are the
+ * caller's (with world == 1 they are not used and may be NULL).  Only launches and event records / waits, so one
+ * rank's step can be captured into a CUDA graph on `stream` (side_stream joins the capture through fork_events).
+ * With world == 1 the call launches exactly what delora_odometry_train_step launches: the same bits, no collective.
+ * Refused before any launch, naming the field: everything _train_step refuses; a null group; world outside
+ * [1, DELORA_GRAD_ALLREDUCE_MAX_WORLD], rank outside [0, world); a null or unaligned (16 bytes) peer_ws[q], peer_ws[rank]
+ * other than `workspace`, a null or unaligned (4 bytes) peer_flags[q]; an unaligned multicast; a null status; n_ctas
+ * outside [1, 160]; n_threads not 32, 64, 96 or 128; with world > 1, a null fork_events[k] or join_event.
+ * status: set non-zero by the kernel when a peer did not arrive within 20 s (see delora_grad_allreduce_f32).
+ * Measured on one H100 80GB HBM3 at a 700 W power limit (max SM clock 1980 MHz), B = 16, graph-replayed steps,
+ * medians of paired differences, world = 1 group step - _train_step: 64 x 720 -0.019 ms (14.26 ms), 64 x 2048
+ * -0.000 ms (22.97 ms), i.e. within the noise (scripts/gpu_train_group.py, profiles/train_group_h100_700w.json).
+ * Multi-GPU scaling and the all-reduce time left exposed on an 8-GPU NVLink node are not measured yet
+ * (scripts/gpu_train_group.py --gpus N measures them). */
+#define DELORA_GRAD_ALLREDUCE_MAX_WORLD 16
+#define DELORA_TRAIN_GROUP_BUCKETS 5
+typedef struct {
+    int32_t rank, world;
+    uint64_t peer_ws[DELORA_GRAD_ALLREDUCE_MAX_WORLD];     /* rank q's training workspace, mapped in this process */
+    uint64_t peer_flags[DELORA_GRAD_ALLREDUCE_MAX_WORLD];  /* rank q's delora_grad_allreduce_flag_words() uint32 */
+    uint64_t multicast;                  /* multicast address of the workspaces, or 0 (unicast, rank by rank) */
+    int32_t n_ctas, n_threads;           /* the all-reduce kernel's grid: 1 .. 160 CTAs of 32 .. 128 threads */
+    int32_t* status;                     /* device int32, 0 while every peer arrives */
+    void* side_stream;                   /* cudaStream_t the buckets are all-reduced on */
+    void* fork_events[DELORA_TRAIN_GROUP_BUCKETS];  /* cudaEvent_t, recorded on `stream` when bucket k is complete */
+    void* join_event;                    /* cudaEvent_t, recorded on side_stream after the last bucket */
+} delora_odometry_train_group;
+int delora_odometry_train_step_group(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
+                                     const delora_odometry_train_group* g, const float* points, const int32_t* n_points,
+                                     int B, void* workspace, float* losses, float* T, float* pooled, float* grads,
+                                     void* stream);
+/* Host only (no GPU needed): the byte offset of the gradient section (fp32[weight_floats], blob order) in a training
+ * workspace; -1 (and delora_last_error()) for an invalid descriptor. */
+int64_t delora_odometry_train_grad_offset(const delora_odometry_desc* d);
+/* Host only: the all-reduce schedule of the group step, DELORA_TRAIN_GROUP_BUCKETS entries each, in launch order:
+ * bucket k covers gradient floats [offsets[k], offsets[k] + counts[k]) (multiples of 4).  Non-zero for an invalid
+ * descriptor or a null output. */
+int delora_odometry_train_group_buckets(const delora_odometry_desc* d, int64_t* offsets, int64_t* counts);
+
 #ifdef __cplusplus
 }
 #endif
