@@ -269,6 +269,10 @@ struct InferPlan {
     // residual only (delora_odometry_streams_push_residual), after every other section: the dense grids of the S new
     // frames and of each stream's previous frame, the 3x4 transforms the ICP reads, its outputs and its scratch
     size_t pts_grid, nrm_grid, prev_pts_grid, prev_nrm_grid, T12, losses, grad_T, icp;
+    // normalised streams only (delora_odometry_streams_push_normalized), after every streams section: the point rows
+    // [2S, 3, n_stride] (each stream's previous frame, then its last frame), their counts [2S] followed by the count
+    // of each stream's last frame [S], and the factor of each pair [S]
+    size_t stage, stage_counts, factor;
     size_t total;
 };
 
@@ -305,6 +309,19 @@ static void make_infer_plan(const delora_odometry_desc* d, bool streams, bool re
         p->grad_T = take(off, (size_t)MB * 12 * 4);
         p->icp = take(off, (size_t)delora_icp_scratch_floats(MB, (int)HW) * 4);
     }
+    p->total = off;
+}
+
+// The normalised streams workspace: the streams layout unchanged (so _streams_load_weights and _streams_reset work on
+// it), then the sections of delora_odometry_streams_push_normalized.  Its prev_image section holds this tick's
+// projection of each previous frame; nothing reads it across ticks.
+static void make_normalized_streams_plan(const delora_odometry_desc* d, InferPlan* p) {
+    make_infer_plan(d, true, false, p);
+    const size_t S = (size_t)d->max_batch;
+    size_t off = p->total;
+    p->stage = take(off, 2 * S * 3 * (size_t)d->n_stride * 4);
+    p->stage_counts = take(off, 3 * S * 4);
+    p->factor = take(off, S * 4);
     p->total = off;
 }
 
@@ -673,9 +690,15 @@ odometry_streams_input_kernel(const float* __restrict__ cur, float* prev, const 
 // quaternion is divided by the norm of its own row, with the instructions odometry_out_kernel runs at B = 1 (row_dot4
 // with nb = 1, fmaf over the 4 components in order, sqrtf, the four divisions, quat_to_T_row).  valid[s] = 1 for those
 // streams, 0 for the others (whose T row is not written); then every active stream has a previous frame.
+// kRescale (delora_odometry_streams_push_normalized): T[:3, 3] of a valid row is then multiplied by factor[s] with the
+// instructions of odometry_out_kernel<true>; factor_out[s] = factor[s] where valid, 0 elsewhere; and the count of this
+// tick's frame, counts[S + s], becomes the count of each active stream's last frame, counts[2S + s].
+template <bool kRescale>
 __global__ void __launch_bounds__(kTailWarps * 32)
 odometry_streams_out_kernel(TailLinear rot, TailLinear trans, int S, int vec, const int32_t* __restrict__ active,
-                            int32_t* __restrict__ has_prev, float* __restrict__ T, int32_t* __restrict__ valid) {
+                            int32_t* __restrict__ has_prev, float* __restrict__ T, int32_t* __restrict__ valid,
+                            const float* __restrict__ factor, float* __restrict__ factor_out,
+                            int32_t* __restrict__ counts) {
     extern __shared__ float s_out[];                        // [S, 7]: quaternion (x, y, z, w), translation
     head_outputs(rot, trans, S, vec, [&](int b) { return stream_active(active, b) && has_prev[b] != 0; }, s_out);
     __syncthreads();
@@ -687,10 +710,58 @@ odometry_streams_out_kernel(TailLinear rot, TailLinear trans, int S, int vec, co
             float ss = 0.0f;
             for (int j = 0; j < 4; ++j) ss = fmaf(q[j], q[j], ss);
             const float nrm = sqrtf(ss);
-            quat_to_T_row(q[0] / nrm, q[1] / nrm, q[2] / nrm, q[3] / nrm, q[4], q[5], q[6], T + (size_t)b * 16);
+            float* t = T + (size_t)b * 16;
+            quat_to_T_row(q[0] / nrm, q[1] / nrm, q[2] / nrm, q[3] / nrm, q[4], q[5], q[6], t);
+            if (kRescale) {
+                const float f = factor[b];
+                t[3] = __fmul_rn(t[3], f); t[7] = __fmul_rn(t[7], f); t[11] = __fmul_rn(t[11], f);
+            }
         }
         valid[b] = ok ? 1 : 0;
+        if (kRescale) {
+            factor_out[b] = ok ? factor[b] : 0.0f;
+            if (act) counts[2 * S + b] = counts[S + b];
+        }
         if (act) has_prev[b] = 1;
+    }
+}
+
+// delora_odometry_streams_push_normalized's masked count clamp fused with the staging of the point rows.
+// stage [2S, 3, n_stride]: row s holds stream s's previous frame, row S + s its last frame; counts [3S]: this tick's
+// counts of the 2S rows, then the count of each stream's last frame.  For every active stream: row S + s moves to row s
+// (the counts[2S + s] points of its last frame, if it has a previous frame; none otherwise), then the caller's frame
+// (its clamped count of points) goes to row S + s.  This tick's counts: row s = the moved count, row S + s = the
+// clamped count for an active stream, 0 for an inactive one, whose rows are not touched.  One thread per (point index, stream)
+// moves and copies the three coordinates of its point: the thread that reads an old value of row S + s is the one that
+// then overwrites it, so no value is overwritten before it is read, without a barrier.  counts[2S + s], which every
+// CTA of the stream reads here, is updated by the output kernel.
+__global__ void __launch_bounds__(256)
+odometry_streams_stage_kernel(const float* __restrict__ points, const int32_t* __restrict__ n_points,
+                              const int32_t* __restrict__ active, const int32_t* __restrict__ has_prev, int S,
+                              int n_stride, float* stage, int32_t* counts) {
+    const int s = blockIdx.y;
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    const bool act = stream_active(active, s);
+    const int n_prev = act && has_prev[s] != 0 ? counts[2 * S + s] : 0;
+    const int n_cur = act ? min(max(n_points[s], 0), n_stride) : 0;
+    if (i == 0) {
+        counts[s] = n_prev;
+        counts[S + s] = n_cur;
+    }
+    if (i >= max(n_prev, n_cur)) return;
+    float* prev = stage + (size_t)s * 3 * n_stride;
+    float* last = stage + (size_t)(S + s) * 3 * n_stride;
+    const float* src = points + (size_t)s * 3 * n_stride;
+    float old[3], cur[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        old[c] = i < n_prev ? last[(size_t)c * n_stride + i] : 0.0f;       // plain loads: row S + s is written here
+        cur[c] = i < n_cur ? __ldg(src + (size_t)c * n_stride + i) : 0.0f;
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        if (i < n_prev) prev[(size_t)c * n_stride + i] = old[c];
+        if (i < n_cur) last[(size_t)c * n_stride + i] = cur[c];
     }
 }
 
@@ -819,8 +890,8 @@ static int run_streams_push(const delora_odometry_desc* d, const delora_odometry
     TailLinear rot, trans;
     if ((rc = run_tail_hidden(p.m, inference_tail_io(p, ws), d->act, pooled, S, &rot, &trans, st))) return rc;
     const int vec = tail_vec(rot) && tail_vec(trans);
-    odometry_streams_out_kernel<<<1, kTailWarps * 32, (size_t)S * 7 * sizeof(float), st>>>(rot, trans, S, vec, active,
-                                                                                          has_prev, T, valid);
+    odometry_streams_out_kernel<false><<<1, kTailWarps * 32, (size_t)S * 7 * sizeof(float), st>>>(
+        rot, trans, S, vec, active, has_prev, T, valid, nullptr, nullptr, nullptr);
     DELORA_CHECK_LAUNCH("odometry_streams_out_kernel");
     if (!rp) return 0;
     // the residual: this frame moved by T against the stream's previous frame (the training step's orientation,
@@ -903,6 +974,77 @@ extern "C" int delora_odometry_streams_push_residual(const delora_odometry_desc*
     DELORA_CHECK_ARG(valid, "%s: null valid", who);
     DELORA_CHECK_ARG(losses, "%s: null losses", who);
     return run_streams_push(d, rp, points, n_points, active, workspace, T, valid, losses, (cudaStream_t)stream);
+}
+
+extern "C" int64_t delora_odometry_streams_normalized_workspace_bytes(const delora_odometry_desc* d) {
+    if (check_desc(d, "delora_odometry_streams_normalized_workspace_bytes")) return -1;
+    InferPlan p;
+    make_normalized_streams_plan(d, &p);
+    return (int64_t)p.total;
+}
+
+extern "C" int delora_odometry_streams_normalized_init(const delora_odometry_desc* d, void* workspace, void* stream) {
+    const char* who = "delora_odometry_streams_normalized_init";
+    if (check_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    InferPlan p;
+    make_normalized_streams_plan(d, &p);
+    return init_workspace(p.f, p.total, workspace, (cudaStream_t)stream, who);
+}
+
+// One tick of a normalised model: the staging of the point rows, the factor of the S pairs (side 0 = rows 0..S-1, the
+// previous frames; side 1 = rows S..2S-1, this tick's), the scaled projection of each half (the previous frames into
+// prev_image, this tick's into images; each resolve re-arms the shared keys), the pairs' trunk-input conversion, the
+// trunk and the tail at B = S, and the rescaling output kernel.  A stream without a pair this tick has a row-s count of
+// 0, so its factor is 0 / 0 = NaN and its scaled coordinates project to no pixel; its outputs are not written.
+static int run_streams_push_normalized(const delora_odometry_desc* d, const float* points, const int32_t* n_points,
+                                       const int32_t* active, void* workspace, float* T, int32_t* valid,
+                                       float* factor_out, cudaStream_t st) {
+    InferPlan p;
+    make_normalized_streams_plan(d, &p);
+    char* ws = (char*)workspace;
+    const int S = d->max_batch, ns = d->n_stride;
+    float* stage = reinterpret_cast<float*>(ws + p.stage);
+    int32_t* counts = reinterpret_cast<int32_t*>(ws + p.stage_counts);
+    float* factor = reinterpret_cast<float*>(ws + p.factor);
+    int32_t* has_prev = reinterpret_cast<int32_t*>(ws + p.f.has_prev);
+    float* prev = reinterpret_cast<float*>(ws + p.f.prev_image);
+    float* cur = reinterpret_cast<float*>(ws + p.f.images);
+    uint64_t* keys = reinterpret_cast<uint64_t*>(ws + p.f.keys);
+    int32_t* index_map = reinterpret_cast<int32_t*>(ws + p.f.index_map);
+    odometry_streams_stage_kernel<<<dim3((unsigned)((ns + 255) / 256), (unsigned)S), 256, 0, st>>>(
+        points, n_points, active, has_prev, S, ns, stage, counts);
+    DELORA_CHECK_LAUNCH("odometry_streams_stage_kernel");
+    int rc;
+    if ((rc = launch_normalization_factors(stage, counts, S, ns, factor, st))) return rc;
+    const GridParams g = make_grid(d->H, d->W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, 0);
+    if ((rc = project_fwd(stage, counts, S, 3, ns, g, keys, prev, index_map, factor, S, st))) return rc;
+    if ((rc = project_fwd(stage + (size_t)S * 3 * ns, counts + S, S, 3, ns, g, keys, cur, index_map, factor, S, st)))
+        return rc;
+    if ((rc = trunk_input(p.m.t, p.t, ws, prev, cur, S, st))) return rc;
+    float* pooled = reinterpret_cast<float*>(ws + p.pooled);
+    if ((rc = trunk_forward(p.m.t, p.t, ws, p.w, ws, d->act, S, pooled, nullptr, st))) return rc;
+    TailLinear rot, trans;
+    if ((rc = run_tail_hidden(p.m, inference_tail_io(p, ws), d->act, pooled, S, &rot, &trans, st))) return rc;
+    const int vec = tail_vec(rot) && tail_vec(trans);
+    odometry_streams_out_kernel<true><<<1, kTailWarps * 32, (size_t)S * 7 * sizeof(float), st>>>(
+        rot, trans, S, vec, active, has_prev, T, valid, factor, factor_out, counts);
+    DELORA_CHECK_LAUNCH("odometry_streams_out_kernel<true>");
+    return 0;
+}
+
+extern "C" int delora_odometry_streams_push_normalized(const delora_odometry_desc* d, const float* points,
+                                                       const int32_t* n_points, const int32_t* active, void* workspace,
+                                                       float* T, int32_t* valid, float* factor, void* stream) {
+    const char* who = "delora_odometry_streams_push_normalized";
+    if (check_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(points, "%s: null points", who);
+    DELORA_CHECK_ARG(n_points, "%s: null n_points", who);
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    DELORA_CHECK_ARG(T, "%s: null T", who);
+    DELORA_CHECK_ARG(valid, "%s: null valid", who);
+    DELORA_CHECK_ARG(factor, "%s: null factor", who);
+    return run_streams_push_normalized(d, points, n_points, active, workspace, T, valid, factor, (cudaStream_t)stream);
 }
 
 extern "C" int delora_odometry_streams_reset(const delora_odometry_desc* d, const int32_t* mask, void* workspace,

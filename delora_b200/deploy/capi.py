@@ -1,6 +1,7 @@
 """ctypes binding of the odometry workspaces of the C ABI (include/delora_b200.h): inference (`delora_odometry_pairs` /
 `_pairs_normalized` / `_push`), streams (`delora_odometry_streams_*`, with the per-frame ICP residual
-`delora_odometry_streams_residual_*` / `_push_residual`) and training (`delora_odometry_train_*`, and
+`delora_odometry_streams_residual_*` / `_push_residual`, and for normalised models
+`delora_odometry_streams_normalized_*` / `_push_normalized`) and training (`delora_odometry_train_*`, and
 `delora_odometry_train_step_group` for several workspaces stepped as one data-parallel group).
 
 Each class holds one descriptor and one workspace, a torch uint8 tensor on the current device.  Every call runs on
@@ -120,7 +121,11 @@ class StreamsWorkspace(_Workspace):
     def __init__(self, desc, weights, workspace=None):
         super().__init__(desc, workspace)
         self._call(self.INIT, self.workspace.data_ptr())
-        self._call("delora_odometry_streams_load_weights", weights.data_ptr(), self.workspace.data_ptr())
+        self.load_weights(weights)
+
+    def load_weights(self, blob):
+        """delora_odometry_streams_load_weights: replace the weights; every stream keeps its previous frame."""
+        self._call("delora_odometry_streams_load_weights", blob.data_ptr(), self.workspace.data_ptr())
 
     def push(self, points, counts, active, T, valid):
         """points [S, 3, n_stride], counts [S], active [S] int32 or None (all active); T [S, 16] and valid [S] out."""
@@ -146,6 +151,20 @@ class ResidualStreamsWorkspace(StreamsWorkspace):
         """StreamsWorkspace.push plus losses [S, LOSS_ROW] out: the ICP row of every valid stream, zeros elsewhere."""
         self._call("delora_odometry_streams_push_residual", self._params, points.data_ptr(), counts.data_ptr(),
                    _ptr(active), self.workspace.data_ptr(), T.data_ptr(), valid.data_ptr(), losses.data_ptr())
+
+
+class NormalizedStreamsWorkspace(StreamsWorkspace):
+    """delora_odometry_streams_normalized_* for a model trained with normalization_scaling, on the streams layout with
+    the normalised sections appended: `push` also writes each pair's factor.  load_weights / reset are the streams
+    calls."""
+    SIZE_QUERY = "delora_odometry_streams_normalized_workspace_bytes"
+    INIT = "delora_odometry_streams_normalized_init"
+
+    def push(self, points, counts, active, T, valid, factor):
+        """StreamsWorkspace.push plus factor [S] out: the factor of every valid stream's pair, 0 elsewhere; T's
+        translation is in the points' units."""
+        self._call("delora_odometry_streams_push_normalized", points.data_ptr(), counts.data_ptr(), _ptr(active),
+                   self.workspace.data_ptr(), T.data_ptr(), valid.data_ptr(), factor.data_ptr())
 
 
 class TrainingWorkspace(_Workspace):

@@ -15,7 +15,7 @@ divides both scans by it, projects both, runs the model and multiplies the trans
 one captured graph.
 
 OdometryStreams serves several streams of one sensor geometry and model from one C-ABI workspace, batched; it refuses
-normalised models.
+normalised models, which NormalizedOdometryStreams serves the same way from the normalised streams workspace.
 """
 import numpy as np
 import torch
@@ -189,11 +189,14 @@ class OdometryStreams:
 
     def __init__(self, model, config, dataset, n_streams, n_max, use_cuda_graph=True, residual=False,
                  residual_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL):
-        from . import capi, export
         if config.get("normalization_scaling", False):
             raise ValueError("normalization_scaling: True is not supported by OdometryStreams (its workspace caches "
-                             "each stream's projected image, which a normalised model cannot reuse); run one "
-                             "OdometryStream per sensor")
+                             "each stream's projected image, which a normalised model cannot reuse); serve such a "
+                             "model with NormalizedOdometryStreams")
+        self._setup(model, config, dataset, n_streams, n_max, use_cuda_graph, residual, residual_flags, False)
+
+    def _setup(self, model, config, dataset, n_streams, n_max, use_cuda_graph, residual, residual_flags, normalized):
+        from . import capi, export
         self.config = config
         self.dataset = dataset
         self.device = torch.device(config["device"])
@@ -208,14 +211,17 @@ class OdometryStreams:
             if self.residual:
                 self.workspace = capi.ResidualStreamsWorkspace(self.desc, self.blob,
                                                                capi.residual_params(config, residual_flags))
+            elif normalized:
+                self.workspace = capi.NormalizedStreamsWorkspace(self.desc, self.blob)
             else:
                 self.workspace = capi.StreamsWorkspace(self.desc, self.blob)
             # staging: points [S, 3, n_max] fp32, then counts [S] and active [S] int32, one buffer each way
             in_bytes = S * 3 * n * 4 + 2 * S * 4
             self.host_in = torch.zeros((in_bytes,), dtype=torch.uint8).pin_memory()
             self.dev_in = torch.zeros((in_bytes,), dtype=torch.uint8, device=self.device)
-            # T [S, 16] fp32, valid [S] int32, then with residual losses [S, LOSS_ROW] fp32
-            out_bytes = S * 16 * 4 + S * 4 + (S * ops.LOSS_ROW * 4 if self.residual else 0)
+            # T [S, 16] fp32, valid [S] int32, then with residual losses [S, LOSS_ROW] fp32, normalised factor [S] fp32
+            out_bytes = (S * 16 * 4 + S * 4 + (S * ops.LOSS_ROW * 4 if self.residual else 0)
+                         + (S * 4 if normalized else 0))
             self.host_out = torch.zeros((out_bytes,), dtype=torch.uint8).pin_memory()
             self.dev_out = torch.zeros((out_bytes,), dtype=torch.uint8, device=self.device)
             self.dev_mask = torch.zeros((S,), dtype=torch.int32, device=self.device)
@@ -231,7 +237,7 @@ class OdometryStreams:
         self._dev_active = self.dev_in[S * 3 * n * 4 + S * 4:]
         self._tick = (self.dev_in[:S * 3 * n * 4], self.dev_in[S * 3 * n * 4:S * 3 * n * 4 + S * 4], self._dev_active,
                       self.dev_out[:S * 64], self.dev_out[S * 64:S * 68])
-        if self.residual:
+        if self.residual or normalized:
             self._tick += (self.dev_out[S * 68:],)
         self.relative = [[] for _ in range(S)]
         self.use_cuda_graph = bool(use_cuda_graph)
@@ -299,3 +305,18 @@ class OdometryStreams:
             self.workspace.reset(self.dev_mask)
             torch.cuda.current_stream().synchronize()
         self.relative[s] = []
+
+
+class NormalizedOdometryStreams(OdometryStreams):
+    """OdometryStreams for a model trained with normalization_scaling, through the normalised streams workspace
+    (`delora_odometry_streams_push_normalized`): the workspace keeps each stream's previous scan, and one tick divides
+    both scans of every pair by that pair's factor, projects them, runs the model once at batch `n_streams` and
+    multiplies each translation back by its factor.  Each stream's transforms are bit-identical to
+    `delora_odometry_pairs_normalized` at batch 1 on (its previous frame, this frame).  Same constructor (without the
+    residual), `push`, `poses` and `reset` as OdometryStreams."""
+
+    def __init__(self, model, config, dataset, n_streams, n_max, use_cuda_graph=True):
+        if not config.get("normalization_scaling", False):
+            raise ValueError("NormalizedOdometryStreams serves models trained with normalization_scaling: True; this "
+                             "config has normalization_scaling off, so serve it with OdometryStreams")
+        self._setup(model, config, dataset, n_streams, n_max, use_cuda_graph, False, None, True)

@@ -12,6 +12,8 @@
  * --residual serves the streams through delora_odometry_streams_push_residual and appends to each line the frame's ICP
  * residual against the stream's previous frame: the point-to-plane loss, the plane-to-plane loss and the matched pairs
  * (normals on the model's image, 7 x 11 neighbourhood, the reference's defaults).  The transforms are the same bits.
+ * A model trained with normalization_scaling (model_flags has DELORA_MODEL_NORMALIZATION_SCALING) is served through
+ * delora_odometry_streams_push_normalized, with the same output; --residual is refused for such a model.
  *
  * Build:  cc odometry_streams.c -I include -I $CUDA_HOME/include -L delora_b200 -ldelora_b200 \
  *            -L $CUDA_HOME/lib64 -lcudart -Wl,-rpath,$PWD/delora_b200 -o odometry_streams
@@ -108,9 +110,10 @@ int main(int argc, char** argv) {
     if (fread(&hdr, sizeof hdr, 1, f) != 1) return fail("truncated header");
     if (memcmp(hdr.magic, DELORA_ODOMETRY_FILE_MAGIC, 8) != 0) return fail("not a .dlw file");
     if (hdr.abi_version != delora_abi_version()) return fail("weight file and library ABI versions differ");
-    if (hdr.model_flags & DELORA_MODEL_NORMALIZATION_SCALING)
-        return fail("the model was trained with normalization_scaling: a streams workspace caches projected images, "
-                    "which such a model cannot reuse (run odometry_stream per sensor)");
+    const int normalized = (hdr.model_flags & DELORA_MODEL_NORMALIZATION_SCALING) != 0;
+    if (normalized && residual)
+        return fail("--residual is not provided for models trained with normalization_scaling (serve the file "
+                    "without it)");
     delora_odometry_desc desc = hdr.desc;
     desc.max_batch = S;
     const delora_odometry_desc* d = &desc;
@@ -132,7 +135,7 @@ int main(int argc, char** argv) {
     cudaStream_t stream;
     CUDA_OK(cudaStreamCreate(&stream));
     const size_t pts_floats = (size_t)S * 3 * d->n_stride;
-    float *weights, *points, *T, *losses;
+    float *weights, *points, *T, *losses, *factor;
     delora_odometry_residual_params rp;
     rp.lambda_po2pl = 1.0f;
     rp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL;
@@ -141,8 +144,9 @@ int main(int argc, char** argv) {
     rp.min_neighbors = 10;
     int32_t *count, *active, *valid;
     void* workspace;
-    const int64_t ws_bytes = residual ? delora_odometry_streams_residual_workspace_bytes(d)
-                                      : delora_odometry_streams_workspace_bytes(d);
+    const int64_t ws_bytes = residual     ? delora_odometry_streams_residual_workspace_bytes(d)
+                             : normalized ? delora_odometry_streams_normalized_workspace_bytes(d)
+                                          : delora_odometry_streams_workspace_bytes(d);
     if (ws_bytes < 0) return fail(delora_last_error());
     CUDA_OK(cudaMalloc((void**)&weights, (size_t)n_weights * sizeof(float)));
     CUDA_OK(cudaMalloc(&workspace, (size_t)ws_bytes));
@@ -152,8 +156,10 @@ int main(int argc, char** argv) {
     CUDA_OK(cudaMalloc((void**)&valid, (size_t)S * sizeof(int32_t)));
     CUDA_OK(cudaMalloc((void**)&T, (size_t)S * 16 * sizeof(float)));
     CUDA_OK(cudaMalloc((void**)&losses, (size_t)S * DELORA_LOSS_ROW * sizeof(float)));
+    CUDA_OK(cudaMalloc((void**)&factor, (size_t)S * sizeof(float)));
     CUDA_OK(cudaMemcpy(weights, h_blob, (size_t)n_weights * sizeof(float), cudaMemcpyHostToDevice));
     if (residual) DELORA_OK(delora_odometry_streams_residual_init(d, workspace, stream));
+    else if (normalized) DELORA_OK(delora_odometry_streams_normalized_init(d, workspace, stream));
     else DELORA_OK(delora_odometry_streams_init(d, workspace, stream));
     DELORA_OK(delora_odometry_streams_load_weights(d, weights, workspace, stream));
 
@@ -180,6 +186,9 @@ int main(int argc, char** argv) {
                                                             stream));
             CUDA_OK(cudaMemcpyAsync(h_losses, losses, (size_t)S * DELORA_LOSS_ROW * sizeof(float), cudaMemcpyDeviceToHost,
                                     stream));
+        } else if (normalized) {
+            DELORA_OK(delora_odometry_streams_push_normalized(d, points, count, active, workspace, T, valid, factor,
+                                                              stream));
         } else {
             DELORA_OK(delora_odometry_streams_push(d, points, count, active, workspace, T, valid, stream));
         }
@@ -209,6 +218,7 @@ int main(int argc, char** argv) {
     free(h_count);
     free(h_points);
     free(h_blob);
+    cudaFree(factor);
     cudaFree(losses);
     cudaFree(T);
     cudaFree(valid);

@@ -520,10 +520,11 @@ int delora_odometry_pairs(const delora_odometry_desc* d, const float* points, co
  *   naming the argument: an invalid descriptor, null points / n_points / workspace / T / factor, B outside
  *   [1, max_batch].
  *
- * Streaming a normalised model: the _push and _streams_* workspaces cache the previous frame's projected image, which
- * depends on the factor of the NEXT pair, so they cannot serve normalised models.  Stream one through
+ * Streaming a normalised model: the _push and _streams_push workspaces cache the previous frame's projected image,
+ * which depends on the factor of the NEXT pair, so they cannot serve normalised models.  Stream one sensor through
  * delora_odometry_pairs_normalized with B = 1 on (previous scan, this scan), as the reference's ROS node does
- * (examples/odometry_stream.c does so for flagged files).  Train one with DELORA_TRAIN_NORMALIZATION_SCALING in
+ * (examples/odometry_stream.c does so for flagged files); serve several through delora_odometry_streams_push_normalized
+ * (below), which keeps each stream's previous SCAN instead.  Train one with DELORA_TRAIN_NORMALIZATION_SCALING in
  * delora_odometry_train_params.loss_flags (see delora_odometry_train_step). */
 int delora_normalization_factors(const float* points, const int32_t* n_points, int B, int n_stride, float* factor,
                                  void* stream);
@@ -601,7 +602,8 @@ int delora_odometry_streams_reset(const delora_odometry_desc* d, const int32_t* 
  * Refused before any launch, naming the field or pointer: an invalid descriptor; null residual_params; a loss_flags
  * without an ICP loss bit or with any bit other than DELORA_LOSS_PO2PO / _PO2PL / _PL2PL / DELORA_NORMAL_LINEAR; nb_h or
  * nb_w not odd and positive; epsilon_range < 0; min_neighbors < 0; null points / n_points / workspace / T / valid /
- * losses.  Models flagged DELORA_MODEL_NORMALIZATION_SCALING cannot be streamed here either. */
+ * losses.  Models flagged DELORA_MODEL_NORMALIZATION_SCALING cannot be streamed here: the residual's grids would need a
+ * definition of their units and of the projection they come from. */
 typedef struct {
     float lambda_po2pl;                  /* weight of po2pl in dL/dT only; the loss rows are unweighted */
     uint32_t loss_flags;                 /* DELORA_LOSS_PO2PO / _PO2PL / _PL2PL (at least one), DELORA_NORMAL_LINEAR */
@@ -616,6 +618,51 @@ int delora_odometry_streams_residual_init(const delora_odometry_desc* d, void* w
 int delora_odometry_streams_push_residual(const delora_odometry_desc* d, const delora_odometry_residual_params* rp,
                                           const float* points, const int32_t* n_points, const int32_t* active,
                                           void* workspace, float* T, int32_t* valid, float* losses, void* stream);
+
+/* Several streams of a model flagged DELORA_MODEL_NORMALIZATION_SCALING in one workspace.  Such a model sees each pair
+ * divided by the factor of that pair, so a stream's previous frame is projected anew every tick: the workspace keeps
+ * each stream's previous SCAN, and one call per tick computes the S factors, projects both scans of every pair, runs
+ * the model once at batch S and multiplies each translation back by its factor.
+ *
+ * The normalised streams workspace is the streams workspace with sections appended: no offset of the streams layout
+ * moves, so delora_odometry_streams_load_weights and delora_odometry_streams_reset work on it unchanged
+ * (_streams_normalized_init replaces _streams_init).  The streams layout's cached images become this tick's projection
+ * of each previous frame, rewritten every tick; its S key buffers serve both projections.  Appended, each 256-byte
+ * aligned, for S = max_batch streams: the point rows [2S, 3, n_stride] fp32 (each stream's previous frame, then its
+ * last frame), their counts [2S] and the count of each stream's last frame [S] int32, and the factors [S] fp32.
+ * Sizes from the host-only query (layers {2,2,2,2}, resnet_outputs 1000, two heads, n_stride 131072), streams ->
+ * normalised streams workspace: 64 x 2048: S = 1 86.0 -> 89.0 MiB, S = 4 271.8 -> 283.8 MiB,
+ * S = 16 1015.1 -> 1063.1 MiB; 64 x 720: S = 1 46.2 -> 49.2 MiB, S = 4 112.8 -> 124.8 MiB, S = 16 379.1 -> 427.1 MiB.
+ *
+ * delora_odometry_streams_push_normalized: the arguments of delora_odometry_streams_push, plus factor [S] fp32, a
+ * required device output.  For every stream with valid[s] = 1, row s of T (its translation multiplied by the factor)
+ * and factor[s] are bit-identical to delora_odometry_pairs_normalized with B = 1 on (that stream's previous active
+ * frame, this frame), in an inference workspace with the same weights.  valid[s] follows _streams_push: 1 for an active
+ * stream that has a previous frame.  factor[s] = 0 where valid[s] = 0.  Inactive streams leave their T row and their
+ * cached frame untouched.  An empty active frame gives NaN for the pairs it belongs to (this one and, after it, the
+ * next), as in delora_odometry_pairs_normalized; no other stream is affected.  Per tick: the masked count clamp fused
+ * with the staging of the frames (odometry_streams_stage_kernel), delora_normalization_factors' kernel at B = S (each
+ * factor is the B = 1 factor bit for bit: its per-scan float64 order does not depend on B), two scaled projections,
+ * the pairs' trunk-input conversion, the trunk and the tail at B = S, and odometry_streams_out_kernel's rescaling
+ * variant.
+ * Measured on one H100 80GB HBM3 at a 700 W power limit (SM clock 1980 MHz), graph-replayed ticks, all streams active,
+ * near-identity heads on consecutive synthetic frames, medians of alternating samples, ms per tick: _streams_push on
+ * the same weights / _streams_push_normalized / S captured _pairs_normalized calls at B = 1:
+ * 64 x 2048: S = 1 1.21 / 1.24 / 1.23, S = 4 2.18 / 2.22 / 5.00, S = 16 8.34 / 8.48 / 19.82;
+ * 64 x 720: S = 1 1.14 / 1.17 / 1.17, S = 4 1.35 / 1.39 / 4.69, S = 16 5.02 / 5.09 / 18.91
+ * (scripts/gpu_odometry_streams_normalized.py, profiles/odometry_streams_normalized_h100_700w.json).  At S = 16 a
+ * stream costs 0.53 ms (64 x 2048) and 0.32 ms (64 x 720) instead of 1.24 and 1.18 ms; at S = 1 the staging costs what
+ * the one pairs call does, within 0.01 ms.
+ * Only launches, with a sequence that depends on neither `active` nor the stream state, so one captured call serves
+ * every tick.  Counts above n_stride are clamped on the device.  Refused before any launch, naming the field or
+ * pointer: an invalid descriptor, null points / n_points / workspace / T / valid / factor. */
+int64_t delora_odometry_streams_normalized_workspace_bytes(const delora_odometry_desc* d); /* host only, -1 if invalid */
+/* Zero the workspace (no stream has a previous frame) and arm the projection keys.  Once after allocation, instead of
+ * delora_odometry_streams_init. */
+int delora_odometry_streams_normalized_init(const delora_odometry_desc* d, void* workspace, void* stream);
+int delora_odometry_streams_push_normalized(const delora_odometry_desc* d, const float* points, const int32_t* n_points,
+                                            const int32_t* active, void* workspace, float* T, int32_t* valid,
+                                            float* factor, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Odometry training: raw scan pairs -> updated weights, one call per step.
