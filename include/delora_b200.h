@@ -103,7 +103,10 @@ int delora_sort_by_range(const float* range, const int32_t* n_points, int B, int
  * image      [B, C_img, H, W] fp32 (first three channels are x, y, z)
  * nb_h, nb_w neighbourhood side lengths (7, 11); patch = (2*(nb_h/2)+1) x (2*(nb_w/2)+1), edge-clamped
  * normals    [B, 3, H, W] fp32 out (may be NULL); 0 where the pixel is not valid (x!=0 & y!=0 & z!=0)
- *            or has fewer than `min_neighbors` range-gated neighbours.
+ *            or has fewer than max(`min_neighbors`, 2) range-gated neighbours (the pixel itself included): a set of
+ *            one point has no covariance, so min_neighbors 0 and 1 act as 2 (the reference's eigen-solve raises there).
+ * epsilon_range  the range gate |(|q| - |c|)| <= epsilon_range; NaN, infinite or negative is refused (the same rule as
+ *            delora_odometry_train_params and delora_odometry_residual_params).
  * pts_grid   [B, H*W] float4 out or NULL: (x, y, z, bits(pixel id)) of valid pixels, (+inf,+inf,+inf,-1) else
  * nrm_grid   [B, H*W] float4 out or NULL: (nx, ny, nz, has_normal ? 1 : 0)   (both or neither)
  *            -- the dense layout delora_icp_dense_fwd_bwd consumes (one point per spherical cell).
@@ -117,7 +120,8 @@ int delora_normals_fwd(const float* image, int B, int C_img, int H, int W, int n
  * min_neighbors, NULL, pts_grid, nrm_grid), bit-identical to those two calls.  For C = 3 or 4 and the 7x11
  * neighbourhood the normals kernel resolves the projection's depth keys itself (no separate resolve pass, the image
  * is written but not read back); other C or neighbourhoods run the two calls.
- * pts_grid, nrm_grid  [B, H*W] float4 out, as delora_normals_fwd writes them (both required)
+ * pts_grid, nrm_grid  [B, H*W] float4 out, as delora_normals_fwd writes them (both required); epsilon_range and
+ *                     min_neighbors as there (a NaN, infinite or negative epsilon_range refused, fewer than 2 neighbours: no normal)
  * split_event         cudaEvent_t or NULL: recorded on `stream` after the projection's scatter pass (or after the whole
  *                     projection on the two-call path) and before the normals kernel, for per-kernel timing.
  */
