@@ -155,6 +155,9 @@ SIGNATURES = {
                                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_train_grad_offset": (c_i64, [c_desc_p]),
     "delora_odometry_train_group_buckets": (c_int, [c_desc_p, c_void_p, c_void_p]),
+    "delora_odometry_train_geometries_workspace_bytes": (c_i64, [c_desc_p, c_int]),
+    "delora_odometry_train_geometries_init": (c_int, [c_desc_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_train_use_geometry": (c_int, [c_desc_p, c_int, c_int, c_void_p, c_void_p]),
     "delora_odometry_train_eval": (c_int, [c_desc_p, c_train_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                                            c_void_p, c_void_p]),
     "delora_odometry_train_weights": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),

@@ -12,6 +12,7 @@
 // are no atomics, so results are bit-identical from run to run and do not depend on B except through the norm.
 #include <cuda_bf16.h>
 #include <math.h>
+#include <stdio.h>
 #include <string.h>
 
 #include "common.cuh"
@@ -482,10 +483,12 @@ static int check_icp_params(float lambda_po2pl, uint32_t loss_flags, int nb_h, i
     return 0;
 }
 
-// Every workspace starts zeroed, with its depth keys at all ones (the projection's empty key)
-static int init_workspace(const Frames& f, size_t total, void* workspace, cudaStream_t st, const char* who) {
+// Every workspace starts zeroed, with its depth keys at all ones (the projection's empty key).  from > 0: only bytes
+// [from, total) are zeroed (a training workspace's geometry section, delora_odometry_train_use_geometry).
+static int init_workspace(const Frames& f, size_t total, void* workspace, cudaStream_t st, const char* who,
+                          size_t from = 0) {
     char* ws = (char*)workspace;
-    cudaError_t e = cudaMemsetAsync(ws, 0, total, st);
+    cudaError_t e = cudaMemsetAsync(ws + from, 0, total - from, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(ws + f.keys, 0xFF, f.keys_bytes, st);
     DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
     return 0;
@@ -1360,6 +1363,10 @@ struct TrainPlan {
     size_t total;
 };
 
+// Two sections.  The model section (master weights, gradient, Adam's m and v, the counters, the bf16 filters) comes
+// first and depends only on act, layers, resnet_outputs, single_mlp and the parity of W (the stem's filter layout).
+// The geometry section (frames, grids, ICP scratch, activations, tail buffers, the w_pre buffers) starts at f.keys.
+// delora_odometry_train_geometries_* rely on this split: one model section serves several geometry sections.
 static void make_train_plan(const delora_odometry_desc* d, TrainPlan* tp) {
     memset(tp, 0, sizeof(TrainPlan));
     plan_model(d, &tp->m);
@@ -1520,21 +1527,97 @@ extern "C" int64_t delora_odometry_train_workspace_bytes(const delora_odometry_d
     return (int64_t)tp.total;
 }
 
-extern "C" int delora_odometry_train_init(const delora_odometry_desc* d, const float* weights, void* workspace,
-                                          void* stream) {
-    const char* who = "delora_odometry_train_init";
-    if (check_train_desc(d, who)) return 1;
+namespace delora {
+
+// _train_init on a workspace of `total` bytes (>= d's size), armed for d
+static int train_init(const delora_odometry_desc* d, size_t total, const float* weights, void* workspace,
+                      cudaStream_t st, const char* who) {
     DELORA_CHECK_ARG(weights && workspace, "%s: null pointer", who);
     TrainPlan tp;
     make_train_plan(d, &tp);
-    cudaStream_t st = (cudaStream_t)stream;
     char* ws = (char*)workspace;
-    int rc = init_workspace(tp.f, tp.total, ws, st, who);
+    int rc = init_workspace(tp.f, total, ws, st, who);
     if (rc) return rc;
     const cudaError_t e = cudaMemcpyAsync(ws + tp.master, weights, (size_t)tp.m.blob_floats * 4, cudaMemcpyDeviceToDevice,
                                           st);
     DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
     return prep_blob_weights(tp.m, tp.w, ws, reinterpret_cast<const float*>(ws + tp.master), st, who);
+}
+
+// The descriptors of one shared training workspace: each valid for training, with d[0]'s model fields and W parity,
+// so that all of them plan the same model section
+static int check_geometries(const delora_odometry_desc* d, int n, const char* who) {
+    DELORA_CHECK_ARG(d != nullptr, "%s: null descriptor array", who);
+    DELORA_CHECK_ARG(n >= 1, "%s: n=%d must be >= 1", who, n);
+    for (int g = 0; g < n; ++g) {
+        char w[192];
+        snprintf(w, sizeof w, "%s: d[%d]", who, g);
+        if (check_train_desc(&d[g], w)) return 1;
+        const delora_odometry_desc &a = d[0], &b = d[g];
+        DELORA_CHECK_ARG(b.act == a.act, "%s: d[%d].act=%d differs from d[0].act=%d", who, g, b.act, a.act);
+        for (int s = 0; s < 4; ++s)
+            DELORA_CHECK_ARG(b.layers[s] == a.layers[s], "%s: d[%d].layers[%d]=%d differs from d[0].layers[%d]=%d", who,
+                             g, s, b.layers[s], s, a.layers[s]);
+        DELORA_CHECK_ARG(b.resnet_outputs == a.resnet_outputs, "%s: d[%d].resnet_outputs=%d differs from "
+                         "d[0].resnet_outputs=%d", who, g, b.resnet_outputs, a.resnet_outputs);
+        DELORA_CHECK_ARG(b.single_mlp == a.single_mlp, "%s: d[%d].single_mlp=%d differs from d[0].single_mlp=%d", who,
+                         g, b.single_mlp, a.single_mlp);
+        DELORA_CHECK_ARG(b.W % 2 == a.W % 2, "%s: d[%d].W=%d and d[0].W=%d differ in parity: the stem's filter layout, "
+                         "and with it the model section, would differ", who, g, b.W, a.W);
+    }
+    return 0;
+}
+
+// The shared workspace: the model section and the largest geometry section, i.e. the largest single-geometry size
+static size_t geometries_bytes(const delora_odometry_desc* d, int n) {
+    size_t total = 0;
+    for (int g = 0; g < n; ++g) {
+        TrainPlan tp;
+        make_train_plan(&d[g], &tp);
+        total = tp.total > total ? tp.total : total;
+    }
+    return total;
+}
+
+}  // namespace delora
+
+extern "C" int delora_odometry_train_init(const delora_odometry_desc* d, const float* weights, void* workspace,
+                                          void* stream) {
+    const char* who = "delora_odometry_train_init";
+    if (check_train_desc(d, who)) return 1;
+    TrainPlan tp;
+    make_train_plan(d, &tp);
+    return train_init(d, tp.total, weights, workspace, (cudaStream_t)stream, who);
+}
+
+extern "C" int64_t delora_odometry_train_geometries_workspace_bytes(const delora_odometry_desc* d, int n) {
+    if (check_geometries(d, n, "delora_odometry_train_geometries_workspace_bytes")) return -1;
+    return (int64_t)geometries_bytes(d, n);
+}
+
+extern "C" int delora_odometry_train_geometries_init(const delora_odometry_desc* d, int n, const float* weights,
+                                                     void* workspace, void* stream) {
+    const char* who = "delora_odometry_train_geometries_init";
+    if (check_geometries(d, n, who)) return 1;
+    return train_init(d, geometries_bytes(d, n), weights, workspace, (cudaStream_t)stream, who);
+}
+
+extern "C" int delora_odometry_train_use_geometry(const delora_odometry_desc* d, int n, int g, void* workspace,
+                                                  void* stream) {
+    const char* who = "delora_odometry_train_use_geometry";
+    if (check_geometries(d, n, who)) return 1;
+    DELORA_CHECK_ARG(g >= 0 && g < n, "%s: g=%d outside [0, n=%d)", who, g, n);
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    TrainPlan tp;
+    make_train_plan(&d[g], &tp);
+    cudaStream_t st = (cudaStream_t)stream;
+    char* ws = (char*)workspace;
+    // the geometry section as _train_init leaves it, then the ICP scratch's batch marker ctr[1] as _train_init's zero
+    int rc = init_workspace(tp.f, tp.total, ws, st, who, tp.f.keys);
+    if (rc) return rc;
+    const cudaError_t e = cudaMemsetAsync(ws + tp.ctr + sizeof(long long), 0, sizeof(long long), st);
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+    return 0;
 }
 
 namespace delora {

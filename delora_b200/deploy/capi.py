@@ -2,7 +2,8 @@
 `_pairs_normalized` / `_push`), streams (`delora_odometry_streams_*`, with the per-frame ICP residual
 `delora_odometry_streams_residual_*` / `_push_residual`, and for normalised models
 `delora_odometry_streams_normalized_*` / `_push_normalized`) and training (`delora_odometry_train_*`, and
-`delora_odometry_train_step_group` for several workspaces stepped as one data-parallel group).
+`delora_odometry_train_step_group` for several workspaces stepped as one data-parallel group,
+`delora_odometry_train_geometries_*` / `_use_geometry` for one workspace shared by several sensor geometries).
 
 Each class holds one descriptor and one workspace, a torch uint8 tensor on the current device.  Every call runs on
 torch's current stream at call time, checks its status with `_lib.check` and does not synchronise (except
@@ -175,6 +176,9 @@ class TrainingWorkspace(_Workspace):
         super().__init__(desc, workspace)
         self._params = ctypes.byref(params)
         self.n = int(self._L.delora_odometry_weight_floats(self._dp))
+        self._init(weights)
+
+    def _init(self, weights):
         self._call("delora_odometry_train_init", weights.data_ptr(), self.workspace.data_ptr())
 
     def _floats(self):
@@ -243,6 +247,46 @@ class TrainingWorkspace(_Workspace):
         self._call("delora_odometry_train_set_state", *(a.data_ptr() for a in args), step_t.data_ptr(),
                    self.workspace.data_ptr())
         torch.cuda.synchronize()
+
+
+class GeometriesTrainingWorkspace(TrainingWorkspace):
+    """delora_odometry_train_geometries_*: one training workspace shared by several sensor geometries (descriptors with
+    the same model fields and W parity).  `use(g)` re-arms it for descs[g]; every TrainingWorkspace call after it runs
+    with descs[g].  Armed for descs[0] after construction."""
+
+    @staticmethod
+    def shared_bytes(descs):
+        """delora_odometry_train_geometries_workspace_bytes; ValueError with the C side's message when it refuses."""
+        L = _lib.lib()
+        arr = (_lib.OdometryDesc * len(descs))(*descs)
+        nbytes = int(L.delora_odometry_train_geometries_workspace_bytes(arr, len(arr)))
+        if nbytes < 0:
+            raise ValueError(L.delora_last_error().decode())
+        return nbytes
+
+    def __init__(self, descs, weights, params, workspace=None):
+        self.descs = (_lib.OdometryDesc * len(descs))(*descs)
+        nbytes = self.shared_bytes(self.descs)
+        if workspace is None:
+            workspace = torch.empty((nbytes,), dtype=torch.uint8, device="cuda")
+        elif workspace.numel() < nbytes:
+            raise ValueError(f"the workspace has {workspace.numel()} bytes, the geometries need {nbytes}")
+        self.geometry = 0
+        super().__init__(self.descs[0], weights, params, workspace)
+
+    def _init(self, weights):
+        name = "delora_odometry_train_geometries_init"
+        _lib.check(getattr(self._L, name)(self.descs, len(self.descs), weights.data_ptr(), self.workspace.data_ptr(),
+                                          _stream()), name)
+
+    def use(self, g):
+        """delora_odometry_train_use_geometry: re-arm the geometry section for descs[g] (only launches)."""
+        name = "delora_odometry_train_use_geometry"
+        _lib.check(getattr(self._L, name)(self.descs, len(self.descs), int(g), self.workspace.data_ptr(), _stream()),
+                   name)
+        self.geometry = int(g)
+        self.desc = self.descs[self.geometry]
+        self._dp = ctypes.byref(self.desc)
 
 
 class TrainingGroup:

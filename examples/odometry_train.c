@@ -2,8 +2,8 @@
  * The reference's training loop (src/deploy/trainer.py, Trainer.train) from a C host: no Python, no torch.  Links
  * libdelora_b200.so and cudart only.
  *
- *   odometry_train [--lr LR] [--switch-below L] [--dropout-seed S] [--eval-dir DIR] [--gpus N] in.dlt|in.dlw out.dlt
- *                  epochs B scan_000.bin ...
+ *   odometry_train [--lr LR] [--switch-below L] [--dropout-seed S] [--eval-dir DIR] [--gpus N]
+ *                  [--geometry DIR,H,W,VFOV0,VFOV1[,W_PRE]]... in.dlt|in.dlw out.dlt epochs B scan_000.bin ...
  *
  * Reads a training checkpoint (.dlt: weights, Adam's state, epoch and phase; layout in include/delora_b200.h) or a
  * weight file (.dlw: a fresh Adam with learning rate --lr, default 1e-5, the reference's learning_rate) and a list of
@@ -32,6 +32,16 @@
  * the epoch's objective is the mean over the GPUs of their mean objectives.  GPU r draws its dropout masks with seed
  * + r; the .dlt keeps the seed.  GPU 0 writes out.dlt and runs --eval-dir.  Without the option, or with --gpus 1, the
  * program runs on the current GPU through delora_odometry_train_step.
+ * --geometry DIR,H,W,VFOV0,VFOV1[,W_PRE] (repeatable, one GPU): one more dataset recorded by another sensor, the
+ * reference's `datasets` list.  Its scans are the .bin files of DIR in name order; its descriptor is the header's with
+ * H, W, the vertical field of view (degrees) and w_pre (default 0) replaced.  All datasets train one model in one
+ * workspace (delora_odometry_train_geometries_*).  Each epoch runs the batches of every dataset (its consecutive pairs,
+ * B per step, the last step the rest) in one shuffled order, as the reference's DataLoader shuffles the concatenated
+ * datasets; a batch is always from one dataset, and delora_odometry_train_use_geometry re-arms the workspace when the
+ * dataset changes.  The order is drawn from the epoch number, so a run resumed from out.dlt steps as an uninterrupted
+ * one.  out.dlt keeps the header's descriptor: pass the same --geometry options when resuming.  --eval-dir scores the
+ * header's geometry.  Every geometry takes the header's max_batch, and each switch zeroes the workspace's buffers for
+ * that many pairs: export with max_batch = B (include/delora_b200.h gives the cost).
  *
  * Build:  cc odometry_train.c -I include -I $CUDA_HOME/include -L delora_b200 -ldelora_b200 \
  *            -L $CUDA_HOME/lib64 -lcudart -lpthread -Wl,-rpath,$PWD/delora_b200 -o odometry_train
@@ -184,6 +194,61 @@ static int held_out(const delora_odometry_desc* d, const delora_odometry_train_p
     return 0;
 }
 
+#define MAX_GEOMETRIES 16
+#define DEG_TO_RAD (3.14159265358979323846 / 180.0)
+
+/* one ",value" field at *p: an integer in [0, 1e9] (integral) or a finite number; advances *p; 0 on success */
+static int next_field(const char** p, int integral, double* out) {
+    if (**p != ',') return 1;
+    const char* s = *p + 1;
+    char* end;
+    if (integral) {
+        const long v = strtol(s, &end, 10);
+        if (end == s || v < 0 || v > 1000000000L) return 1;
+        *out = (double)v;
+    } else {
+        const double v = strtod(s, &end);
+        if (end == s || !(v >= -1e300 && v <= 1e300)) return 1;     /* also refuses nan and inf */
+        *out = v;
+    }
+    if (*end != ',' && *end != '\0') return 1;
+    *p = end;
+    return 0;
+}
+
+/* "DIR,H,W,VFOV0,VFOV1[,W_PRE]" (fields of view in degrees) -> *dir (a copy) and *g: base with H, W, vfov and w_pre
+ * replaced; 0 on success.  The library validates the descriptor itself. */
+static int parse_geometry(const char* arg, const delora_odometry_desc* base, char** dir, delora_odometry_desc* g) {
+    const char* comma = strchr(arg, ',');
+    if (!comma || comma == arg) return 1;
+    double v[5] = {0, 0, 0, 0, 0};
+    const int integral[5] = {1, 1, 0, 0, 1};
+    const char* p = comma;
+    for (int i = 0; i < 5; ++i) {
+        if (i == 4 && *p == '\0') break;                              /* W_PRE is optional */
+        if (next_field(&p, integral[i], &v[i])) return 1;
+    }
+    if (*p != '\0' || v[0] < 1 || v[1] < 2 || !(v[3] > v[2])) return 1;
+    *g = *base;
+    g->H = (int)v[0];
+    g->W = (int)v[1];
+    g->vfov0 = v[2] * DEG_TO_RAD;
+    g->vfov1 = v[3] * DEG_TO_RAD;
+    g->w_pre = (int)v[4];
+    *dir = (char*)malloc((size_t)(comma - arg) + 1);
+    if (!*dir) return 1;
+    memcpy(*dir, arg, (size_t)(comma - arg));
+    (*dir)[comma - arg] = '\0';
+    return 0;
+}
+
+static uint64_t splitmix64(uint64_t* state) {
+    uint64_t z = (*state += 0x9E3779B97F4A7C15ull);
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
 /* --gpus N: one GPU of the group, and the epoch its thread runs */
 typedef struct {
     int rank;
@@ -300,6 +365,8 @@ int main(int argc, char** argv) {
     const char* seed_arg = getenv("DELORA_DROPOUT_SEED");
     const char* eval_dir = NULL;
     int gpus = 1;
+    int n_geom = 0;                           /* --geometry datasets, after the header's (dataset 0) */
+    const char* geom_args[MAX_GEOMETRIES];
     int a = 1;
     for (; a + 1 < argc && strncmp(argv[a], "--", 2) == 0; a += 2) {
         if (strcmp(argv[a], "--lr") == 0) lr = (float)atof(argv[a + 1]);
@@ -307,11 +374,27 @@ int main(int argc, char** argv) {
         else if (strcmp(argv[a], "--dropout-seed") == 0) seed_arg = argv[a + 1];
         else if (strcmp(argv[a], "--eval-dir") == 0) eval_dir = argv[a + 1];
         else if (strcmp(argv[a], "--gpus") == 0) gpus = atoi(argv[a + 1]);
+        else if (strcmp(argv[a], "--geometry") == 0) {
+            if (n_geom == MAX_GEOMETRIES - 1) return fail("too many --geometry options");
+            geom_args[n_geom++] = argv[a + 1];
+        }
         else return fail("unknown option");
     }
+    /* checked before anything is read, against a dummy descriptor; parsed again below against the header's */
+    for (int g = 0; g < n_geom; ++g) {
+        delora_odometry_desc probe;
+        char* dir;
+        memset(&probe, 0, sizeof probe);
+        if (parse_geometry(geom_args[g], &probe, &dir, &probe))
+            return fail("--geometry wants DIR,H,W,VFOV0,VFOV1[,W_PRE]: a directory, integers H >= 1, W >= 2 and "
+                        "W_PRE >= 0, and the vertical field of view in degrees with VFOV0 < VFOV1");
+        free(dir);
+    }
+    if (n_geom > 0 && gpus != 1) return fail("--geometry trains on one GPU: it does not combine with --gpus");
     if (argc - a < 6)
         return fail("usage: odometry_train [--lr LR] [--switch-below L] [--dropout-seed S] [--eval-dir DIR] [--gpus N] "
-                    "in.dlt|in.dlw out.dlt epochs B scan.bin scan.bin [scan.bin ...]");
+                    "[--geometry DIR,H,W,VFOV0,VFOV1[,W_PRE]]... in.dlt|in.dlw out.dlt epochs B scan.bin scan.bin "
+                    "[scan.bin ...]");
     const char* in_path = argv[a];
     const char* out_path = argv[a + 1];
     const int epochs = atoi(argv[a + 2]);
@@ -490,13 +573,39 @@ int main(int argc, char** argv) {
         return 0;
     }
 
+    /* dataset 0: the header's geometry and the listed scans; 1 .. n_geom: the --geometry ones */
+    const int n_sets = 1 + n_geom;
+    delora_odometry_desc descs[MAX_GEOMETRIES];
+    float* set_scans[MAX_GEOMETRIES];
+    int32_t* set_counts[MAX_GEOMETRIES];
+    int set_pairs[MAX_GEOMETRIES];
+    descs[0] = *d; set_scans[0] = h_scans; set_counts[0] = h_counts; set_pairs[0] = n_pairs;
+    for (int g = 1; g < n_sets; ++g) {
+        char *dir, **paths;
+        if (parse_geometry(geom_args[g - 1], d, &dir, &descs[g])) return fail("bad --geometry");
+        if (normalized && descs[g].w_pre == 0)
+            return fail("--geometry: a model trained with normalization_scaling needs W_PRE > 0 on every geometry");
+        const int n_set = list_scans(dir, &paths);
+        if (n_set < 2) return fail("--geometry needs a directory with at least two .bin scans");
+        if (load_scans(paths, n_set, d->n_stride, &set_scans[g], &set_counts[g])) return 1;
+        for (int k = 0; k < n_set; ++k) free(paths[k]);
+        free(paths);
+        free(dir);
+        set_pairs[g] = n_set - 1;
+    }
+    /* the epoch's batches (dataset, first pair, size), each dataset's in order */
+    int n_batches = 0;
+    for (int g = 0; g < n_sets; ++g) n_batches += (set_pairs[g] + B_max - 1) / B_max;
+    int (*batches)[3] = (int (*)[3])malloc(sizeof(int[3]) * (size_t)(n_batches > 0 ? n_batches : 1));
+    if (!batches) return fail("out of host memory");
+
     cudaStream_t stream;
     CUDA_OK(cudaStreamCreate(&stream));
     float *d_state[3], *points, *losses;
     int64_t* d_step;
     int32_t* counts;
     void* workspace;
-    const int64_t ws_bytes = delora_odometry_train_workspace_bytes(d);
+    const int64_t ws_bytes = delora_odometry_train_geometries_workspace_bytes(descs, n_sets);
     if (ws_bytes < 0) return fail(delora_last_error());
     for (int i = 0; i < 3; ++i) {
         CUDA_OK(cudaMalloc((void**)&d_state[i], n * sizeof(float)));
@@ -508,12 +617,16 @@ int main(int argc, char** argv) {
     CUDA_OK(cudaMalloc((void**)&points, (size_t)2 * B_max * scan_floats * sizeof(float)));
     CUDA_OK(cudaMalloc((void**)&counts, (size_t)2 * B_max * sizeof(int32_t)));
     CUDA_OK(cudaMalloc((void**)&losses, (size_t)B_max * DELORA_LOSS_ROW * sizeof(float)));
-    DELORA_OK(delora_odometry_train_init(d, d_state[0], workspace, stream));
+    DELORA_OK(delora_odometry_train_geometries_init(descs, n_sets, d_state[0], workspace, stream));
     DELORA_OK(delora_odometry_train_set_state(d, d_state[0], d_state[1], d_state[2], d_step, workspace, stream));
     DELORA_OK(delora_odometry_train_set_dropout_seed(d, dropout_seed, workspace, stream));
+    int armed = 0;                            /* the dataset whose geometry the workspace is armed for */
     if (dropout) fprintf(stderr, "odometry_train: dropout on, seed %llu\n", (unsigned long long)dropout_seed);
     fprintf(stderr, "odometry_train: epoch %d, Adam step %lld, %s, %d pairs\n", hdr.epoch, (long long)hdr.step,
             hdr.unsupervised ? "unsupervised" : "identity pre-training", n_pairs);
+    for (int g = 1; g < n_sets; ++g)
+        fprintf(stderr, "odometry_train: dataset %d: %d x %d, w_pre %d, %d pairs\n", g, descs[g].H, descs[g].W,
+                descs[g].w_pre, set_pairs[g]);
 
     float* h_losses = (float*)malloc((size_t)B_max * DELORA_LOSS_ROW * sizeof(float));
     int32_t* h_step_counts = (int32_t*)malloc((size_t)2 * B_max * sizeof(int32_t));
@@ -521,12 +634,35 @@ int main(int argc, char** argv) {
     for (int e = 0; e < epochs; ++e) {
         hp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | (hdr.unsupervised ? 0u : DELORA_LOSS_IDENTITY_FIT) |
                         (normalized ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u) | (dropout ? DELORA_TRAIN_DROPOUT : 0u);
+        int nb = 0;
+        for (int g = 0; g < n_sets; ++g)
+            for (int k0 = 0; k0 < set_pairs[g]; k0 += B_max, ++nb) {
+                batches[nb][0] = g;
+                batches[nb][1] = k0;
+                batches[nb][2] = set_pairs[g] - k0 < B_max ? set_pairs[g] - k0 : B_max;
+            }
+        if (n_sets > 1) {         /* Fisher-Yates, drawn from the epoch number so that a resumed run repeats it */
+            uint64_t rng = (uint64_t)hdr.epoch;
+            for (int j = n_batches - 1; j > 0; --j) {
+                const int i = (int)(splitmix64(&rng) % (uint64_t)(j + 1));
+                int t[3];
+                memcpy(t, batches[i], sizeof t);
+                memcpy(batches[i], batches[j], sizeof t);
+                memcpy(batches[j], t, sizeof t);
+            }
+        }
         double sum = 0.0;
         int steps = 0;
-        for (int k0 = 0; k0 < n_pairs; k0 += B_max, ++steps) {
-            const int B = n_pairs - k0 < B_max ? n_pairs - k0 : B_max;
-            if (stage_pairs(h_scans, h_counts, k0, B, scan_floats, points, counts, h_step_counts, stream)) return 1;
-            DELORA_OK(delora_odometry_train_step(d, &hp, points, counts, B, workspace, losses, NULL, NULL, NULL, stream));
+        for (; steps < n_batches; ++steps) {
+            const int g = batches[steps][0], k0 = batches[steps][1], B = batches[steps][2];
+            if (g != armed) {
+                DELORA_OK(delora_odometry_train_use_geometry(descs, n_sets, g, workspace, stream));
+                armed = g;
+            }
+            if (stage_pairs(set_scans[g], set_counts[g], k0, B, scan_floats, points, counts, h_step_counts, stream))
+                return 1;
+            DELORA_OK(delora_odometry_train_step(&descs[g], &hp, points, counts, B, workspace, losses, NULL, NULL, NULL,
+                                                 stream));
             CUDA_OK(cudaMemcpyAsync(h_losses, losses, (size_t)B * DELORA_LOSS_ROW * sizeof(float),
                                     cudaMemcpyDeviceToHost, stream));
             CUDA_OK(cudaStreamSynchronize(stream));
@@ -540,6 +676,10 @@ int main(int argc, char** argv) {
         printf("epoch %d objective %.9g unsupervised %d", hdr.epoch, mean, hdr.unsupervised);
         if (eval_dir) {         /* the held-out pairs with the weights after the epoch; no update, no dropout */
             double held;
+            if (armed != 0) {
+                DELORA_OK(delora_odometry_train_use_geometry(descs, n_sets, 0, workspace, stream));
+                armed = 0;
+            }
             if (held_out(d, &hp, h_eval_scans, h_eval_counts, n_eval_pairs, B_max, scan_floats, workspace, points, counts,
                          losses, h_losses, h_step_counts, stream, &held))
                 return 1;
@@ -566,8 +706,11 @@ int main(int argc, char** argv) {
     free(h_losses);
     free(h_eval_counts);
     free(h_eval_scans);
-    free(h_counts);
-    free(h_scans);
+    free(batches);
+    for (int g = 0; g < n_sets; ++g) {
+        free(set_counts[g]);
+        free(set_scans[g]);
+    }
     for (int i = 0; i < 3; ++i) {
         free(h_state[i]);
         cudaFree(d_state[i]);

@@ -936,6 +936,48 @@ int64_t delora_odometry_train_grad_offset(const delora_odometry_desc* d);
  * descriptor or a null output. */
 int delora_odometry_train_group_buckets(const delora_odometry_desc* d, int64_t* offsets, int64_t* counts);
 
+/* ---- Training on several sensor geometries from one workspace (the reference's `datasets` list,
+ * config/deployment_options.yaml:3: its Trainer shuffles over the concatenated datasets, src/deploy/trainer.py:95-101,
+ * and each step projects at the geometry of its batch's dataset, src/deploy/deployer.py:240-255).
+ *
+ * A training workspace has two sections.  The MODEL section comes first: master weights, gradient, Adam's m and v,
+ * the counters (Adam's step count, the ICP scratch's batch marker, the dropout seed) and the bf16 filters.  Its layout
+ * depends only on act, layers, resnet_outputs, single_mlp and the parity of W (which selects the stem's filter
+ * layout).  The GEOMETRY section follows it: frames, grids, ICP scratch, trunk activations, tail buffers and the w_pre
+ * buffers.  So descriptors d[0 .. n-1] that agree in those model fields and in W's parity share one model section,
+ * and one workspace of the model section plus the largest geometry section serves all of them.  H, W, the fields of
+ * view, n_stride, max_batch and w_pre may differ between them.
+ *
+ * delora_odometry_train_geometries_workspace_bytes: host only; that size, which is the largest
+ *   delora_odometry_train_workspace_bytes(&d[g]).  -1 (and delora_last_error()) when the set is refused.
+ * delora_odometry_train_geometries_init: _train_init on the shared size, armed for d[0].
+ * delora_odometry_train_use_geometry: re-arm the geometry section for d[g] exactly as _train_init arms it (zeros, the
+ *   all-ones depth keys, the zeroed ICP scratch with its batch marker).  The model section keeps its weights,
+ *   gradient, m, v, step count, dropout seed and bf16 filters.  Launches only (memsets), capturable into a CUDA graph.
+ *   Afterwards every training entry point called with &d[g] on the workspace (_train_step, _train_eval,
+ *   _train_weights, _train_get_state, _train_set_state, _train_set_dropout_seed, _train_step_group,
+ *   _train_grad_offset) acts exactly as on a single-geometry workspace of d[g] holding the same state: the same bits.
+ *   Call it whenever the next call's geometry differs from the last one's; the host keeps track of which is armed.
+ * Refused before any launch, naming the index and the field: a null d, n < 1, a descriptor _train_workspace_bytes
+ * refuses, a model field (act, layers, resnet_outputs, single_mlp) other than d[0]'s, a W of another parity than
+ * d[0]'s (a different model-section layout); _use_geometry also refuses g outside [0, n) and a null workspace.
+ * Not covered: one step that mixes geometries (the reference cannot either, config/hyperparameters.yaml:3); mixing W
+ * parities; inference and streams.  A model trained this way is served per sensor by the inference and streams
+ * workspaces from the same .dlw blob, one descriptor per sensor.
+ * Memory, n_stride 131072, max_batch 16: 64 x 2048 with 64 x 720 (w_pre 2250) share 2911 MiB where two
+ * single-geometry workspaces take 2911 + 1558 MiB.
+ * Cost: the re-arm zeroes d[g]'s whole geometry section, which max_batch sizes, whatever B the next step takes.  So
+ * set max_batch to the B you train at.  Measured on one H100 80GB HBM3 at a 700 W power limit, graph-replayed, median
+ * paired difference of a step right after a switch against a steady step:
+ *   max_batch = B = 1:    64 x 2048 +0.075 ms (3.69 ms step), 64 x 720 (w_pre 2250) +0.044 ms (3.49 ms);
+ *   max_batch = B = 16:   64 x 2048 +0.91 ms (23.00 ms), 64 x 720 (w_pre 2250) +0.48 ms (14.53 ms);
+ *   max_batch 16, B = 1:  64 x 2048 +0.88 ms (3.71 ms, 24 %), 64 x 720 (w_pre 2250) +0.44 ms (3.51 ms, 13 %).
+ * (scripts/gpu_train_geometries.py, profiles/train_geometries_h100_700w.json) */
+int64_t delora_odometry_train_geometries_workspace_bytes(const delora_odometry_desc* d, int n);
+int delora_odometry_train_geometries_init(const delora_odometry_desc* d, int n, const float* weights, void* workspace,
+                                          void* stream);
+int delora_odometry_train_use_geometry(const delora_odometry_desc* d, int n, int g, void* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
