@@ -147,6 +147,10 @@ SIGNATURES = {
     "delora_odometry_streams_normalized_init": (c_int, [c_desc_p, c_void_p, c_void_p]),
     "delora_odometry_streams_push_normalized": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                                         c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_streams_pre_workspace_bytes": (c_i64, [c_desc_p]),
+    "delora_odometry_streams_pre_init": (c_int, [c_desc_p, c_void_p, c_void_p]),
+    "delora_odometry_streams_push_pre": (c_int, [c_desc_p, c_residual_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                 c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_train_workspace_bytes": (c_i64, [c_desc_p]),
     "delora_odometry_train_init": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_train_step": (c_int, [c_desc_p, c_train_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,

@@ -274,6 +274,10 @@ struct InferPlan {
     // [2S, 3, n_stride] (each stream's previous frame, then its last frame), their counts [2S] followed by the count
     // of each stream's last frame [S], and the factor of each pair [S]
     size_t stage, stage_counts, factor;
+    // recipe streams only (delora_odometry_streams_push_pre), after every residual section: the H x w_pre stage of the
+    // S new frames (depth keys, image, index map), the H x w_pre grids [2S] (each stream's previous frame, then this
+    // tick's frames), the model's T in the units it saw [S, 16]; factor (above) holds the pair factors
+    size_t pre_keys, pre_image, pre_index_map, pre_pts, pre_nrm, T16;
     size_t total;
 };
 
@@ -322,6 +326,23 @@ static void make_normalized_streams_plan(const delora_odometry_desc* d, InferPla
     size_t off = p->total;
     p->stage = take(off, 2 * S * 3 * (size_t)d->n_stride * 4);
     p->stage_counts = take(off, 3 * S * 4);
+    p->factor = take(off, S * 4);
+    p->total = off;
+}
+
+// The recipe streams workspace: the residual layout unchanged (so _streams_load_weights and _streams_reset work on it;
+// its H x W grids and ICP sections serve the recipe's ICP), then the H x w_pre sections.  The streams layout's key
+// buffers serve both H x W projections of a tick, its images hold this tick's projection of both frames of each pair.
+static void make_pre_streams_plan(const delora_odometry_desc* d, InferPlan* p) {
+    make_infer_plan(d, true, true, p);
+    const size_t S = (size_t)d->max_batch, HWp = (size_t)d->H * d->w_pre;
+    size_t off = p->total;
+    p->pre_keys = take(off, S * HWp * 8);
+    p->pre_image = take(off, S * 4 * HWp * 4);
+    p->pre_index_map = take(off, S * HWp * 4);
+    p->pre_pts = take(off, 2 * S * HWp * 16);
+    p->pre_nrm = take(off, 2 * S * HWp * 16);
+    p->T16 = take(off, S * 16 * 4);
     p->factor = take(off, S * 4);
     p->total = off;
 }
@@ -823,6 +844,49 @@ odometry_streams_grids_kernel(float4* __restrict__ cur_pts, float4* __restrict__
     }
 }
 
+// ---- the recipe streams (delora_odometry_streams_push_pre)
+// Between the output kernel (which wrote T16 and valid) and the ICP; one thread per element of the largest of T16
+// [S, 16], the H x W grids [S, HW] and the H x w_pre grids [S, HWp].
+//   T16: for a valid stream T[s] = T16[s] (factor non-NULL: T[:3, 3] multiplied by factor[s] with the instructions of
+//     odometry_out_kernel<true>) and factor_out[s] = factor[s]; factor_out[s] = 0 for the others, whose T row is not
+//     written.  T12 = the 3x4 of T16 (the model's units, the ICP's) for valid streams, the identity for the others.
+//   H x W: a stream without a transform has its source grids (cur) emptied, so the ICP finds no source pixel for it
+//     (a stream without a frame has empty grids already; one on its first frame has points).
+//   H x w_pre: every active stream's new grids become its cached previous frame; inactive streams' slots stay.  The
+//     cached grids were last read by this tick's factor and projection, which precede this kernel.
+__global__ void __launch_bounds__(256)
+odometry_streams_pre_kernel(const float* __restrict__ T16, const float* __restrict__ factor,
+                            const int32_t* __restrict__ active, const int32_t* __restrict__ valid, int S, int HW,
+                            int HWp, float* __restrict__ T, float* __restrict__ T12, float* __restrict__ factor_out,
+                            float4* __restrict__ cur_pts, float4* __restrict__ cur_nrm,
+                            const float4* __restrict__ pre_cur_pts, const float4* __restrict__ pre_cur_nrm,
+                            float4* __restrict__ pre_prev_pts, float4* __restrict__ pre_prev_nrm) {
+    const size_t i = (size_t)blockIdx.x * 256 + threadIdx.x;
+    if (i < (size_t)S * 16) {
+        const int s = (int)i / 16, e = (int)i % 16;
+        const bool ok = valid[s] != 0;
+        const float t = T16[i];
+        if (ok) T[i] = (factor && (e == 3 || e == 7 || e == 11)) ? __fmul_rn(t, factor[s]) : t;
+        if (e < 12) T12[s * 12 + e] = ok ? t : (e % 5 == 0 ? 1.0f : 0.0f);
+        if (e == 0 && factor_out) factor_out[s] = ok ? factor[s] : 0.0f;
+    }
+    if (i < (size_t)S * HW && valid[i / HW] == 0) {
+        cur_pts[i] = empty_grid_cell();
+        cur_nrm[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    }
+    if (i < (size_t)S * HWp && stream_active(active, (int)(i / HWp))) {
+        pre_prev_pts[i] = pre_cur_pts[i];
+        pre_prev_nrm[i] = pre_cur_nrm[i];
+    }
+}
+
+// After the ICP: losses [S, DELORA_LOSS_ROW] = the ICP's row of the valid streams, zeros for the others
+__global__ void odometry_streams_losses_kernel(const int32_t* __restrict__ valid, int S,
+                                               const float* __restrict__ icp_losses, float* __restrict__ losses) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < S * DELORA_LOSS_ROW) losses[i] = valid[i / DELORA_LOSS_ROW] != 0 ? icp_losses[i] : 0.0f;
+}
+
 }  // namespace delora
 
 extern "C" int64_t delora_odometry_streams_workspace_bytes(const delora_odometry_desc* d) {
@@ -1048,6 +1112,133 @@ extern "C" int delora_odometry_streams_push_normalized(const delora_odometry_des
     DELORA_CHECK_ARG(valid, "%s: null valid", who);
     DELORA_CHECK_ARG(factor, "%s: null factor", who);
     return run_streams_push_normalized(d, points, n_points, active, workspace, T, valid, factor, (cudaStream_t)stream);
+}
+
+// check_desc plus the preprocessing width the recipe streams read (the training rule, but w_pre = 0 is refused)
+static int check_pre_desc(const delora_odometry_desc* d, const char* who) {
+    if (check_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(d->w_pre >= 2 && (long long)d->H * d->w_pre < (1ll << 27),
+                     "%s: w_pre=%d must be >= 2 with H * w_pre < 2^27 (H=%d): the recipe streams estimate the normals "
+                     "at H x w_pre", who, d->w_pre, d->H);
+    return 0;
+}
+
+extern "C" int64_t delora_odometry_streams_pre_workspace_bytes(const delora_odometry_desc* d) {
+    if (check_pre_desc(d, "delora_odometry_streams_pre_workspace_bytes")) return -1;
+    InferPlan p;
+    make_pre_streams_plan(d, &p);
+    return (int64_t)p.total;
+}
+
+extern "C" int delora_odometry_streams_pre_init(const delora_odometry_desc* d, void* workspace, void* stream) {
+    const char* who = "delora_odometry_streams_pre_init";
+    if (check_pre_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    InferPlan p;
+    make_pre_streams_plan(d, &p);
+    cudaStream_t st = (cudaStream_t)stream;
+    char* ws = (char*)workspace;
+    const int rc = init_workspace(p.f, p.total, workspace, st, who);     // the ICP scratch is zeroed here, once
+    if (rc) return rc;
+    const size_t n = (size_t)d->max_batch * d->H * d->w_pre;
+    const cudaError_t e = cudaMemsetAsync(ws + p.pre_keys, 0xFF, n * 8, st);
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+    odometry_streams_grid_clear_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
+        reinterpret_cast<float4*>(ws + p.pre_pts), reinterpret_cast<float4*>(ws + p.pre_nrm), n);
+    DELORA_CHECK_LAUNCH("odometry_streams_grid_clear_kernel");
+    return 0;
+}
+
+// One tick of the recipe (the training step's stages 1-3 at B = S, each pair's first frame from the cache): the masked
+// count clamp, projection + normals of the S new frames at H x w_pre, the pair factors over the valid H x w_pre cells
+// (flagged models; cached frames are side 0, new ones side 1), both frames of every pair projected to H x W (scaled by
+// the pair's factor when flagged), the trunk input, trunk and tail at B = S, the output kernel into T16, the
+// bookkeeping kernel (T, T12, factor, emptied sources, cache write), the ICP at B = S and the masked loss rows.
+static int run_streams_push_pre(const delora_odometry_desc* d, const delora_odometry_residual_params* rp,
+                                const float* points, const int32_t* n_points, const int32_t* active, void* workspace,
+                                float* T, int32_t* valid, float* losses, float* factor_out, cudaStream_t st) {
+    InferPlan p;
+    make_pre_streams_plan(d, &p);
+    char* ws = (char*)workspace;
+    const int S = d->max_batch, H = d->H, W = d->W, Wp = d->w_pre, HW = H * W, HWp = H * Wp;
+    auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
+    auto f4 = [&](size_t o) { return reinterpret_cast<delora_f4*>(ws + o); };
+    delora_f4* pre_prev_pts = f4(p.pre_pts);
+    delora_f4* pre_prev_nrm = f4(p.pre_nrm);
+    delora_f4* pre_cur_pts = pre_prev_pts + (size_t)S * HWp;
+    delora_f4* pre_cur_nrm = pre_prev_nrm + (size_t)S * HWp;
+    float* prev = f(p.f.prev_image);
+    float* cur = f(p.f.images);
+    uint64_t* keys = reinterpret_cast<uint64_t*>(ws + p.f.keys);
+    int rc;
+    if ((rc = clamp_counts(p.f, ws, n_points, active, S, d->n_stride, st))) return rc;
+    if ((rc = delora_project_normals_fwd(points, reinterpret_cast<int32_t*>(ws + p.f.counts), S, 3, d->n_stride, H, Wp,
+                                         d->hfov0, d->hfov1, d->vfov0, d->vfov1, 0,
+                                         reinterpret_cast<uint64_t*>(ws + p.pre_keys), f(p.pre_image),
+                                         reinterpret_cast<int32_t*>(ws + p.pre_index_map), rp->nb_h, rp->nb_w,
+                                         rp->epsilon_range, rp->min_neighbors, pre_cur_pts, pre_cur_nrm, nullptr, st)))
+        return rc;
+    float* factor = factor_out ? f(p.factor) : nullptr;
+    if (factor && (rc = launch_grid_normalization_factors(pre_prev_pts, S, HWp, factor, st))) return rc;
+    const GridParams g = make_grid(H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, 0);
+    if ((rc = project_grids_fwd(pre_prev_pts, pre_prev_nrm, S, Wp, g, keys, prev, nullptr, f4(p.prev_pts_grid),
+                                f4(p.prev_nrm_grid), factor, S, st))) return rc;
+    if ((rc = project_grids_fwd(pre_cur_pts, pre_cur_nrm, S, Wp, g, keys, cur, nullptr, f4(p.pts_grid), f4(p.nrm_grid),
+                                factor, S, st))) return rc;
+    if ((rc = trunk_input(p.m.t, p.t, ws, prev, cur, S, st))) return rc;
+    float* pooled = f(p.pooled);
+    if ((rc = trunk_forward(p.m.t, p.t, ws, p.w, ws, d->act, S, pooled, nullptr, st))) return rc;
+    TailLinear rot, trans;
+    if ((rc = run_tail_hidden(p.m, inference_tail_io(p, ws), d->act, pooled, S, &rot, &trans, st))) return rc;
+    const int vec = tail_vec(rot) && tail_vec(trans);
+    int32_t* has_prev = reinterpret_cast<int32_t*>(ws + p.f.has_prev);
+    odometry_streams_out_kernel<false><<<1, kTailWarps * 32, (size_t)S * 7 * sizeof(float), st>>>(
+        rot, trans, S, vec, active, has_prev, f(p.T16), valid, nullptr, nullptr, nullptr);
+    DELORA_CHECK_LAUNCH("odometry_streams_out_kernel");
+    int per_stream = HWp > HW ? HWp : HW;
+    if (per_stream < 16) per_stream = 16;
+    const size_t cells = (size_t)S * per_stream;
+    odometry_streams_pre_kernel<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(
+        f(p.T16), factor, active, valid, S, HW, HWp, T, f(p.T12), factor_out, reinterpret_cast<float4*>(ws + p.pts_grid),
+        reinterpret_cast<float4*>(ws + p.nrm_grid), reinterpret_cast<const float4*>(pre_cur_pts),
+        reinterpret_cast<const float4*>(pre_cur_nrm), reinterpret_cast<float4*>(pre_prev_pts),
+        reinterpret_cast<float4*>(pre_prev_nrm));
+    DELORA_CHECK_LAUNCH("odometry_streams_pre_kernel");
+    if ((rc = delora_icp_dense_fwd_bwd(f4(p.pts_grid), f4(p.nrm_grid), f(p.T12), f4(p.prev_pts_grid), f4(p.prev_nrm_grid),
+                                       S, H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, rp->lambda_po2pl,
+                                       rp->loss_flags & ~DELORA_TRAIN_NORMALIZATION_SCALING, f(p.losses), f(p.grad_T),
+                                       f(p.icp), st))) return rc;
+    odometry_streams_losses_kernel<<<(S * DELORA_LOSS_ROW + 255) / 256, 256, 0, st>>>(valid, S, f(p.losses), losses);
+    DELORA_CHECK_LAUNCH("odometry_streams_losses_kernel");
+    return 0;
+}
+
+extern "C" int delora_odometry_streams_push_pre(const delora_odometry_desc* d, const delora_odometry_residual_params* rp,
+                                                const float* points, const int32_t* n_points, const int32_t* active,
+                                                void* workspace, float* T, int32_t* valid, float* losses, float* factor,
+                                                void* stream) {
+    const char* who = "delora_odometry_streams_push_pre";
+    if (check_pre_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(rp, "%s: null residual_params", who);
+    if (check_icp_params(rp->lambda_po2pl, rp->loss_flags, rp->nb_h, rp->nb_w, rp->epsilon_range, rp->min_neighbors, who))
+        return 1;
+    const uint32_t bits = DELORA_LOSS_PO2PO | DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | DELORA_NORMAL_LINEAR |
+                          DELORA_TRAIN_NORMALIZATION_SCALING;
+    DELORA_CHECK_ARG((rp->loss_flags & ~bits) == 0u,
+                     "%s: loss_flags=0x%x has a bit other than the ICP losses, DELORA_NORMAL_LINEAR and "
+                     "DELORA_TRAIN_NORMALIZATION_SCALING", who, rp->loss_flags);
+    DELORA_CHECK_ARG(points, "%s: null points", who);
+    DELORA_CHECK_ARG(n_points, "%s: null n_points", who);
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    DELORA_CHECK_ARG(T, "%s: null T", who);
+    DELORA_CHECK_ARG(valid, "%s: null valid", who);
+    DELORA_CHECK_ARG(losses, "%s: null losses", who);
+    const bool normalized = (rp->loss_flags & DELORA_TRAIN_NORMALIZATION_SCALING) != 0u;
+    DELORA_CHECK_ARG(!normalized || factor, "%s: null factor with DELORA_TRAIN_NORMALIZATION_SCALING in loss_flags", who);
+    DELORA_CHECK_ARG(normalized || !factor, "%s: factor must be NULL without DELORA_TRAIN_NORMALIZATION_SCALING in "
+                     "loss_flags", who);
+    return run_streams_push_pre(d, rp, points, n_points, active, workspace, T, valid, losses, factor,
+                                (cudaStream_t)stream);
 }
 
 extern "C" int delora_odometry_streams_reset(const delora_odometry_desc* d, const int32_t* mask, void* workspace,

@@ -1,7 +1,8 @@
 """ctypes binding of the odometry workspaces of the C ABI (include/delora_b200.h): inference (`delora_odometry_pairs` /
 `_pairs_normalized` / `_push`), streams (`delora_odometry_streams_*`, with the per-frame ICP residual
-`delora_odometry_streams_residual_*` / `_push_residual`, and for normalised models
-`delora_odometry_streams_normalized_*` / `_push_normalized`) and training (`delora_odometry_train_*`, and
+`delora_odometry_streams_residual_*` / `_push_residual`, for normalised models
+`delora_odometry_streams_normalized_*` / `_push_normalized`, and on the reference's two-resolution recipe
+`delora_odometry_streams_pre_*` / `_push_pre`) and training (`delora_odometry_train_*`, and
 `delora_odometry_train_step_group` for several workspaces stepped as one data-parallel group,
 `delora_odometry_train_geometries_*` / `_use_geometry` for one workspace shared by several sensor geometries).
 
@@ -166,6 +167,24 @@ class NormalizedStreamsWorkspace(StreamsWorkspace):
         translation is in the points' units."""
         self._call("delora_odometry_streams_push_normalized", points.data_ptr(), counts.data_ptr(), _ptr(active),
                    self.workspace.data_ptr(), T.data_ptr(), valid.data_ptr(), factor.data_ptr())
+
+
+class PreStreamsWorkspace(StreamsWorkspace):
+    """delora_odometry_streams_pre_* (the descriptor needs w_pre > 0): the streams served on the reference's
+    two-resolution recipe, with the training step's ICP residual; `params` from residual_params, with
+    TRAIN_NORMALIZATION_SCALING in its loss_flags for a normalised model.  load_weights / reset are the streams calls."""
+    SIZE_QUERY = "delora_odometry_streams_pre_workspace_bytes"
+    INIT = "delora_odometry_streams_pre_init"
+
+    def __init__(self, desc, weights, params, workspace=None):
+        super().__init__(desc, weights, workspace)
+        self._params = ctypes.byref(params)
+
+    def push(self, points, counts, active, T, valid, losses, factor=None):
+        """StreamsWorkspace.push plus losses [S, LOSS_ROW] out (the ICP row of every valid stream, zeros elsewhere) and,
+        for a normalised model only, factor [S] out (the pair's factor where valid, 0 elsewhere)."""
+        self._call("delora_odometry_streams_push_pre", self._params, points.data_ptr(), counts.data_ptr(), _ptr(active),
+                   self.workspace.data_ptr(), T.data_ptr(), valid.data_ptr(), losses.data_ptr(), _ptr(factor))
 
 
 class TrainingWorkspace(_Workspace):

@@ -15,7 +15,9 @@ divides both scans by it, projects both, runs the model and multiplies the trans
 one captured graph.
 
 OdometryStreams serves several streams of one sensor geometry and model from one C-ABI workspace, batched; it refuses
-normalised models, which NormalizedOdometryStreams serves the same way from the normalised streams workspace.
+normalised models, which NormalizedOdometryStreams serves the same way from the normalised streams workspace.  Both feed
+the model raw scans projected at its width (the ROS node's input); PreprocessedOdometryStreams feeds it the images of
+the reference's two-resolution recipe (the Tester's and training's input), with an ICP residual per frame.
 """
 import numpy as np
 import torch
@@ -195,7 +197,8 @@ class OdometryStreams:
                              "model with NormalizedOdometryStreams")
         self._setup(model, config, dataset, n_streams, n_max, use_cuda_graph, residual, residual_flags, False)
 
-    def _setup(self, model, config, dataset, n_streams, n_max, use_cuda_graph, residual, residual_flags, normalized):
+    def _setup(self, model, config, dataset, n_streams, n_max, use_cuda_graph, residual, residual_flags, normalized,
+               pre=False):
         from . import capi, export
         self.config = config
         self.dataset = dataset
@@ -203,12 +206,16 @@ class OdometryStreams:
         if self.device.type != "cuda":
             raise RuntimeError("OdometryStreams runs on CUDA devices only (no CPU fallback)")
         self.n_streams, self.n_max = int(n_streams), int(n_max)
-        self.desc = export.desc_from_config(config, dataset, self.n_max, self.n_streams)
+        self.desc = export.desc_from_config(config, dataset, self.n_max, self.n_streams, preprocessing_normals=pre)
         S, n = self.n_streams, self.n_max
         with torch.cuda.device(self.device):
             self.blob = torch.from_numpy(export.pack_state_dict(model.state_dict(), config)).to(self.device)
-            self.residual = bool(residual)
-            if self.residual:
+            self.residual = bool(residual) or pre
+            self.normalized = bool(normalized)
+            if pre:
+                flags = residual_flags | (ops.TRAIN_NORMALIZATION_SCALING if normalized else 0)
+                self.workspace = capi.PreStreamsWorkspace(self.desc, self.blob, capi.residual_params(config, flags))
+            elif self.residual:
                 self.workspace = capi.ResidualStreamsWorkspace(self.desc, self.blob,
                                                                capi.residual_params(config, residual_flags))
             elif normalized:
@@ -232,12 +239,16 @@ class OdometryStreams:
         out = self.host_out.numpy()
         self._host_T = out[:S * 64].view(np.float32).reshape(S, 4, 4)
         self._host_valid = out[S * 64:S * 68].view(np.int32)
-        self._host_losses = out[S * 68:].view(np.float32).reshape(S, -1)
+        self._host_losses = out[S * 68:S * 68 + S * ops.LOSS_ROW * 4 if pre else None].view(np.float32).reshape(S, -1)
+        self._host_factor = out[S * 68 + S * ops.LOSS_ROW * 4:].view(np.float32) if pre and normalized else None
         # the push arguments of a tick: points, counts, active, T, valid in the device staging buffers
         self._dev_active = self.dev_in[S * 3 * n * 4 + S * 4:]
         self._tick = (self.dev_in[:S * 3 * n * 4], self.dev_in[S * 3 * n * 4:S * 3 * n * 4 + S * 4], self._dev_active,
                       self.dev_out[:S * 64], self.dev_out[S * 64:S * 68])
-        if self.residual or normalized:
+        if pre:
+            self._tick += (self.dev_out[S * 68:S * 68 + S * ops.LOSS_ROW * 4],
+                           self.dev_out[S * 68 + S * ops.LOSS_ROW * 4:] if normalized else None)
+        elif self.residual or normalized:
             self._tick += (self.dev_out[S * 68:],)
         self.relative = [[] for _ in range(S)]
         self.use_cuda_graph = bool(use_cuda_graph)
@@ -288,7 +299,10 @@ class OdometryStreams:
             if self._host_valid[s]:
                 t = self._host_T[s][None].copy()
                 self.relative[s].append(t)
-                out.append((t, self._host_losses[s].copy()) if self.residual else t)
+                if self._host_factor is not None:
+                    out.append((t, self._host_losses[s].copy(), float(self._host_factor[s])))
+                else:
+                    out.append((t, self._host_losses[s].copy()) if self.residual else t)
             else:
                 out.append(None)
         return out
@@ -320,3 +334,21 @@ class NormalizedOdometryStreams(OdometryStreams):
             raise ValueError("NormalizedOdometryStreams serves models trained with normalization_scaling: True; this "
                              "config has normalization_scaling off, so serve it with OdometryStreams")
         self._setup(model, config, dataset, n_streams, n_max, use_cuda_graph, False, None, True)
+
+
+class PreprocessedOdometryStreams(OdometryStreams):
+    """OdometryStreams on the reference's two-resolution recipe, through the recipe streams workspace
+    (`delora_odometry_streams_push_pre`): each frame is projected with its normals at `horizontal_cells_preprocessing`
+    (w_pre) and those points are projected again at the model's width, the images a model trained with
+    `--preprocessing-normals` saw in training and the reference's Tester feeds it.  Serves plain and
+    normalization_scaling configs alike.  `push` returns, per stream with a transform, (T [1, 4, 4], losses [LOSS_ROW])
+    -- the training step's ICP residual of the pair, in the model's units -- plus the pair's factor for a normalised
+    config: (T, losses, factor).  `residual_flags` selects the losses; `poses` and `reset` are OdometryStreams'."""
+
+    def __init__(self, model, config, dataset, n_streams, n_max, use_cuda_graph=True,
+                 residual_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL):
+        if "horizontal_cells_preprocessing" not in config[dataset]:
+            raise ValueError(f"{dataset}: horizontal_cells_preprocessing is missing; PreprocessedOdometryStreams "
+                             "serves the recipe's normals at that width (serve raw scans with OdometryStreams)")
+        self._setup(model, config, dataset, n_streams, n_max, use_cuda_graph, True, residual_flags,
+                    bool(config.get("normalization_scaling", False)), pre=True)

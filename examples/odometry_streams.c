@@ -2,7 +2,7 @@
  * Several LiDAR streams from a C host, batched in one workspace: no Python, no torch.  Links libdelora_b200.so and
  * cudart only.
  *
- *   odometry_streams [--residual] model.dlw stream0_dir stream1_dir ...
+ *   odometry_streams [--residual | --preprocessing] model.dlw stream0_dir stream1_dir ...
  *
  * model.dlw is written by bin/export_odometry_weights.py (layout: include/delora_b200.h); every directory holds one
  * stream's KITTI velodyne .bin files ([N, 4] float32 rows: x, y, z, reflectance), taken in name order.  All streams
@@ -14,6 +14,15 @@
  * (normals on the model's image, 7 x 11 neighbourhood, the reference's defaults).  The transforms are the same bits.
  * A model trained with normalization_scaling (model_flags has DELORA_MODEL_NORMALIZATION_SCALING) is served through
  * delora_odometry_streams_push_normalized, with the same output; --residual is refused for such a model.
+ * --preprocessing serves the streams on the reference's two-resolution recipe through delora_odometry_streams_push_pre:
+ * each frame's normals at the header's w_pre, its points projected again at the model's width (the images the model
+ * trained on with --preprocessing-normals, and the reference's Tester's input), and appends the same three residual
+ * columns, the training step's ICP in the model's units, for plain and normalization_scaling files alike.  It refuses
+ * a file with w_pre = 0 (export it with bin/export_odometry_weights.py --preprocessing-normals).  The recipe adds a
+ * projection + normals at H x w_pre per frame, a second H x W projection per pair, the ICP and the cache write to the
+ * raw-scan tick: on one H100 80GB HBM3 at 700 W, w_pre 2250, graph-replayed, ms per tick --residual / --preprocessing
+ * at 64 x 720: 1.20 / 1.21 (1 stream), 1.41 / 1.47 (4), 5.14 / 5.44 (16); at 64 x 2048: 1.29 / 1.31, 2.31 / 2.38,
+ * 8.73 / 8.98 (scripts/gpu_odometry_streams_pre.py, profiles/odometry_streams_pre_h100_700w.json).
  *
  * Build:  cc odometry_streams.c -I include -I $CUDA_HOME/include -L delora_b200 -ldelora_b200 \
  *            -L $CUDA_HOME/lib64 -lcudart -Wl,-rpath,$PWD/delora_b200 -o odometry_streams
@@ -99,8 +108,10 @@ static int32_t read_scan(const char* path, float* dst, int n_stride) {
 
 int main(int argc, char** argv) {
     const int residual = argc > 1 && strcmp(argv[1], "--residual") == 0;
-    if (residual) { --argc; ++argv; }
-    if (argc < 3) return fail("usage: odometry_streams [--residual] model.dlw stream_dir [stream_dir ...]");
+    const int pre = argc > 1 && strcmp(argv[1], "--preprocessing") == 0;
+    if (residual || pre) { --argc; ++argv; }
+    if (argc < 3)
+        return fail("usage: odometry_streams [--residual | --preprocessing] model.dlw stream_dir [stream_dir ...]");
     const int S = argc - 2;
 
     /* weight file: fixed header, then the fp32 blob; the workspace serves S streams (max_batch = S) */
@@ -114,6 +125,9 @@ int main(int argc, char** argv) {
     if (normalized && residual)
         return fail("--residual is not provided for models trained with normalization_scaling (serve the file "
                     "without it)");
+    if (pre && hdr.desc.w_pre == 0)
+        return fail("--preprocessing needs a file with w_pre > 0: export it with bin/export_odometry_weights.py "
+                    "--preprocessing-normals");
     delora_odometry_desc desc = hdr.desc;
     desc.max_batch = S;
     const delora_odometry_desc* d = &desc;
@@ -139,12 +153,14 @@ int main(int argc, char** argv) {
     delora_odometry_residual_params rp;
     rp.lambda_po2pl = 1.0f;
     rp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL;
+    if (pre && normalized) rp.loss_flags |= DELORA_TRAIN_NORMALIZATION_SCALING;
     rp.nb_h = 7; rp.nb_w = 11;
     rp.epsilon_range = 0.5f;
     rp.min_neighbors = 10;
     int32_t *count, *active, *valid;
     void* workspace;
-    const int64_t ws_bytes = residual     ? delora_odometry_streams_residual_workspace_bytes(d)
+    const int64_t ws_bytes = pre          ? delora_odometry_streams_pre_workspace_bytes(d)
+                             : residual   ? delora_odometry_streams_residual_workspace_bytes(d)
                              : normalized ? delora_odometry_streams_normalized_workspace_bytes(d)
                                           : delora_odometry_streams_workspace_bytes(d);
     if (ws_bytes < 0) return fail(delora_last_error());
@@ -158,7 +174,8 @@ int main(int argc, char** argv) {
     CUDA_OK(cudaMalloc((void**)&losses, (size_t)S * DELORA_LOSS_ROW * sizeof(float)));
     CUDA_OK(cudaMalloc((void**)&factor, (size_t)S * sizeof(float)));
     CUDA_OK(cudaMemcpy(weights, h_blob, (size_t)n_weights * sizeof(float), cudaMemcpyHostToDevice));
-    if (residual) DELORA_OK(delora_odometry_streams_residual_init(d, workspace, stream));
+    if (pre) DELORA_OK(delora_odometry_streams_pre_init(d, workspace, stream));
+    else if (residual) DELORA_OK(delora_odometry_streams_residual_init(d, workspace, stream));
     else if (normalized) DELORA_OK(delora_odometry_streams_normalized_init(d, workspace, stream));
     else DELORA_OK(delora_odometry_streams_init(d, workspace, stream));
     DELORA_OK(delora_odometry_streams_load_weights(d, weights, workspace, stream));
@@ -181,9 +198,13 @@ int main(int argc, char** argv) {
         CUDA_OK(cudaMemcpyAsync(points, h_points, pts_floats * sizeof(float), cudaMemcpyHostToDevice, stream));
         CUDA_OK(cudaMemcpyAsync(count, h_count, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
         CUDA_OK(cudaMemcpyAsync(active, h_active, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
-        if (residual) {
-            DELORA_OK(delora_odometry_streams_push_residual(d, &rp, points, count, active, workspace, T, valid, losses,
-                                                            stream));
+        if (pre || residual) {
+            if (pre)
+                DELORA_OK(delora_odometry_streams_push_pre(d, &rp, points, count, active, workspace, T, valid, losses,
+                                                           normalized ? factor : NULL, stream));
+            else
+                DELORA_OK(delora_odometry_streams_push_residual(d, &rp, points, count, active, workspace, T, valid,
+                                                                losses, stream));
             CUDA_OK(cudaMemcpyAsync(h_losses, losses, (size_t)S * DELORA_LOSS_ROW * sizeof(float), cudaMemcpyDeviceToHost,
                                     stream));
         } else if (normalized) {
@@ -199,7 +220,7 @@ int main(int argc, char** argv) {
             if (!h_valid[s]) continue;
             printf("%d %d", s, k);
             for (int i = 0; i < 12; ++i) printf(" %.9g", h_T[(size_t)s * 16 + i]);
-            if (residual) {
+            if (pre || residual) {
                 const float* l = h_losses + (size_t)s * DELORA_LOSS_ROW;
                 printf(" %.9g %.9g %.0f", l[1], l[2], l[3]);
             }

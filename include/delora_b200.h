@@ -447,11 +447,12 @@ typedef struct {
     int layers[4];                       /* BasicBlocks per stage, e.g. {2,2,2,2} (1 .. 64 each) */
     int resnet_outputs;                  /* fc width, 1000 in the shipped config */
     int single_mlp;                      /* use_single_mlp_at_output (0 / 1) */
-    int w_pre;                           /* training only: horizontal_cells_preprocessing, the width the normals are
-                                            estimated at (0: at W).  Read and validated by the delora_odometry_train_*
-                                            entry points alone: 0, or >= 2 with H * w_pre < 2^27.  Training callers
-                                            must zero it (or copy the descriptor from a .dlw header); inference and
-                                            streams callers may leave it uninitialised. */
+    int w_pre;                           /* horizontal_cells_preprocessing, the width the normals are estimated at.
+                                            Read and validated by the delora_odometry_train_* entry points (0: at W;
+                                            else >= 2 with H * w_pre < 2^27) and by delora_odometry_streams_pre_* and
+                                            _streams_push_pre (>= 2 with H * w_pre < 2^27; 0 is refused) alone.
+                                            Training callers must zero it (or copy the descriptor from a .dlw header);
+                                            other inference and streams callers may leave it uninitialised. */
 } delora_odometry_desc;
 
 /* Weight file (.dlw, written by delora_b200/deploy/export.py), little-endian, readable with fread alone:
@@ -667,6 +668,71 @@ int delora_odometry_streams_normalized_init(const delora_odometry_desc* d, void*
 int delora_odometry_streams_push_normalized(const delora_odometry_desc* d, const float* points, const int32_t* n_points,
                                             const int32_t* active, void* workspace, float* T, int32_t* valid,
                                             float* factor, void* stream);
+
+/* Several streams served on the reference's two-resolution recipe: the images a model trained with w_pre > 0 saw in
+ * training, and the reference's Tester feeds it (its dataset loads the preprocessed point lists, src/data/
+ * dataset.py:115-122, and Deployer.step projects them at the model width, src/deploy/deployer.py:252-255), with the
+ * training step's ICP residual beside every transform, for plain and normalization_scaling models alike.  The raw-scan
+ * streams above feed the model the ROS node's input instead (each frame projected straight to H x W); the two images
+ * differ wherever a w_pre pixel straddles two W pixels.  Per tick, for S = max_batch streams: the training step's stages
+ * 1-3 at B = S (delora_odometry_train_step, w_pre > 0), each pair's first frame coming from the workspace: projection +
+ * normals of the S new frames at H x w_pre (rp's neighbourhood); with DELORA_TRAIN_NORMALIZATION_SCALING in
+ * rp->loss_flags the factor of each pair (cached frame, new frame) over their valid H x w_pre cells; both frames of
+ * every pair projected again to H x W (delora_project_grids_fwd; divided by the pair's factor when flagged, normals
+ * not); the trunk and tail at B = S, each quaternion divided by its own row's norm; the dense ICP at B = S, source =
+ * this frame's H x W grids moved by the model's T, target = the previous frame's (the training orientation), in the
+ * model's units (flagged models: normalised, as training); then each active stream's new H x w_pre grids become its
+ * cached previous frame.  A cached frame is projected again every tick, so one layout serves both kinds of model.
+ *
+ * The recipe streams workspace is the residual workspace with sections appended: no offset of the streams layout
+ * moves, so delora_odometry_streams_load_weights and delora_odometry_streams_reset work on it unchanged
+ * (_streams_pre_init replaces _streams_init).  The residual sections hold this tick's H x W grids of both frames and
+ * the ICP's inputs, outputs and scratch.  Appended, each 256-byte aligned, for S streams: the depth keys, image and
+ * index map of the new frames at H x w_pre (S * H * w_pre * 28 bytes), the H x w_pre point and normal grids of each
+ * stream's cached frame and of the new frames (S * H * w_pre * 64 bytes), T in the model's units [S, 16] and the pair
+ * factors [S].  Sizes from the host-only query (layers {2,2,2,2}, resnet_outputs 1000, two heads, n_stride 131072,
+ * w_pre 2250), streams -> residual -> recipe streams workspace:
+ *   64 x 720:  S = 1 46.2 -> 50.9 -> 63.6 MiB, S = 4 112.8 -> 131.6 -> 182.1 MiB, S = 16 379.1 -> 454.3 -> 656.4 MiB;
+ *   64 x 2048: S = 1 86.0 -> 99.3 -> 111.9 MiB, S = 4 271.8 -> 325.0 -> 375.5 MiB, S = 16 1015.1 -> 1227.9 -> 1430.0 MiB.
+ *
+ * delora_odometry_streams_push_pre: the arguments of delora_odometry_streams_push_residual, plus factor [S] fp32.
+ * T [S, 16] and valid [S] follow _streams_push's rules (valid[s] = 1 for an active stream with a previous frame; T rows
+ * of the others are not written).  For a plain model row s of T is bit-identical to delora_odometry_pairs at B = 1 on
+ * (previous frame, this frame) given as their preprocessed point lists (the valid H x w_pre cells in row-major order,
+ * what Preprocesser.preprocess_scans stores); for a flagged one T's translation is multiplied back by the factor, as
+ * delora_odometry_pairs_normalized does.  losses [S, DELORA_LOSS_ROW] (device, required): the ICP row where valid[s] = 1,
+ * bit-identical to delora_icp_dense_fwd_bwd at B = 1 on the two frames' grids and T's 3x4 in the model's units; zeros
+ * elsewhere.  It is the number delora_odometry_train_eval reports for the pair, up to the trunk's rounding (the
+ * training forward keeps the stem's pre-activation in fp16).  factor [S] (device): required with
+ * DELORA_TRAIN_NORMALIZATION_SCALING in rp->loss_flags and NULL without it; factor[s] = the pair's factor where
+ * valid[s] = 1 (eval's losses[b][6]), 0 elsewhere.  An empty active frame gives what delora_odometry_pairs_normalized
+ * gives (NaN) for flagged models and what _streams_push gives otherwise; no other stream is affected.  A stream
+ * without a transform this tick costs the ICP no search: its source grids are emptied first.  Inactive streams leave
+ * their T row and cached frame untouched.
+ * Cost per tick: the raw-scan path's projection, trunk and tail, plus the projection + normals at H x w_pre, a second
+ * H x W projection per pair, the ICP at B = S and the cache write (64 bytes per H x w_pre cell of each active stream).
+ * Measured on one H100 80GB HBM3 at a 700 W power limit (max SM clock 1980 MHz), graph-replayed ticks, all streams
+ * active, near-identity heads on consecutive synthetic frames, w_pre 2250, medians of alternating samples, ms per tick
+ * _streams_push / _streams_push_residual / _streams_push_pre on the same weights:
+ * 64 x 720: S = 1 1.15 / 1.20 / 1.21, S = 4 1.34 / 1.41 / 1.47, S = 16 4.99 / 5.14 / 5.44;
+ * 64 x 2048: S = 1 1.21 / 1.29 / 1.31, S = 4 2.17 / 2.31 / 2.38, S = 16 8.30 / 8.73 / 8.98
+ * (scripts/gpu_odometry_streams_pre.py, profiles/odometry_streams_pre_h100_700w.json).  The recipe costs 0.02-0.30 ms
+ * per tick over the raw-scan residual, which already pays for normals and the ICP; the re-projection of the cached
+ * frames, the part a second layout caching plain models' images could save, is a share of that, so there is one
+ * layout.  On those synthetic 64-ring scans, 2.2 % (64 x 720) and 7.3 % (64 x 2048) of the H x W pixels differ between
+ * the raw-scan and the recipe image.
+ * Only launches, with a sequence that depends on neither `active` nor the stream state, so one captured call serves
+ * every tick.  Refused before any launch, naming the field or pointer: everything _streams_push_residual refuses,
+ * w_pre < 2 (0 included) or H * w_pre >= 2^27, a loss_flags bit other than the ICP loss bits, DELORA_NORMAL_LINEAR and
+ * DELORA_TRAIN_NORMALIZATION_SCALING, a null losses, and a factor that does not match the flag. */
+int64_t delora_odometry_streams_pre_workspace_bytes(const delora_odometry_desc* d);   /* host only, -1 if invalid */
+/* Zero the workspace (no stream has a previous frame, the ICP scratch is armed for B = S), arm the projection keys and
+ * empty the cached grids.  Once after allocation, instead of delora_odometry_streams_init. */
+int delora_odometry_streams_pre_init(const delora_odometry_desc* d, void* workspace, void* stream);
+int delora_odometry_streams_push_pre(const delora_odometry_desc* d, const delora_odometry_residual_params* rp,
+                                     const float* points, const int32_t* n_points, const int32_t* active,
+                                     void* workspace, float* T, int32_t* valid, float* losses, float* factor,
+                                     void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Odometry training: raw scan pairs -> updated weights, one call per step.
