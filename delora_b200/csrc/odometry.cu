@@ -717,12 +717,15 @@ odometry_streams_input_kernel(const float* __restrict__ cur, float* prev, const 
 // kRescale (delora_odometry_streams_push_normalized): T[:3, 3] of a valid row is then multiplied by factor[s] with the
 // instructions of odometry_out_kernel<true>; factor_out[s] = factor[s] where valid, 0 elsewhere; and the count of this
 // tick's frame, counts[S + s], becomes the count of each active stream's last frame, counts[2S + s].
+// raw [S, 7] or NULL (delora_odometry_streams_push_adapt): the head outputs of the valid rows, which the backward reads;
+// n_valid or NULL: the number of valid streams.
 template <bool kRescale>
 __global__ void __launch_bounds__(kTailWarps * 32)
 odometry_streams_out_kernel(TailLinear rot, TailLinear trans, int S, int vec, const int32_t* __restrict__ active,
                             int32_t* __restrict__ has_prev, float* __restrict__ T, int32_t* __restrict__ valid,
                             const float* __restrict__ factor, float* __restrict__ factor_out,
-                            int32_t* __restrict__ counts) {
+                            int32_t* __restrict__ counts, float* __restrict__ raw = nullptr,
+                            int32_t* __restrict__ n_valid = nullptr) {
     extern __shared__ float s_out[];                        // [S, 7]: quaternion (x, y, z, w), translation
     head_outputs(rot, trans, S, vec, [&](int b) { return stream_active(active, b) && has_prev[b] != 0; }, s_out);
     __syncthreads();
@@ -740,6 +743,8 @@ odometry_streams_out_kernel(TailLinear rot, TailLinear trans, int S, int vec, co
                 const float f = factor[b];
                 t[3] = __fmul_rn(t[3], f); t[7] = __fmul_rn(t[7], f); t[11] = __fmul_rn(t[11], f);
             }
+            if (raw)
+                for (int j = 0; j < 7; ++j) raw[b * 7 + j] = q[j];
         }
         valid[b] = ok ? 1 : 0;
         if (kRescale) {
@@ -747,6 +752,14 @@ odometry_streams_out_kernel(TailLinear rot, TailLinear trans, int S, int vec, co
             if (act) counts[2 * S + b] = counts[S + b];
         }
         if (act) has_prev[b] = 1;
+    }
+    if (n_valid) {
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            int n = 0;
+            for (int b = 0; b < S; ++b) n += valid[b];
+            *n_valid = n;
+        }
     }
 }
 
@@ -844,23 +857,27 @@ odometry_streams_grids_kernel(float4* __restrict__ cur_pts, float4* __restrict__
     }
 }
 
-// ---- the recipe streams (delora_odometry_streams_push_pre)
+// ---- the recipe streams (delora_odometry_streams_push_pre) and the adapting streams (_streams_push_adapt)
 // Between the output kernel (which wrote T16 and valid) and the ICP; one thread per element of the largest of T16
-// [S, 16], the H x W grids [S, HW] and the H x w_pre grids [S, HWp].
+// [S, 16], the H x W grids [S, HW] and the cached grids [S, HWp].
 //   T16: for a valid stream T[s] = T16[s] (factor non-NULL: T[:3, 3] multiplied by factor[s] with the instructions of
-//     odometry_out_kernel<true>) and factor_out[s] = factor[s]; factor_out[s] = 0 for the others, whose T row is not
-//     written.  T12 = the 3x4 of T16 (the model's units, the ICP's) for valid streams, the identity for the others.
-//   H x W: a stream without a transform has its source grids (cur) emptied, so the ICP finds no source pixel for it
-//     (a stream without a frame has empty grids already; one on its first frame has points).
-//   H x w_pre: every active stream's new grids become its cached previous frame; inactive streams' slots stay.  The
-//     cached grids were last read by this tick's factor and projection, which precede this kernel.
+//     odometry_out_kernel<true>) and factor_out[s] = factor[s] (factor_out non-NULL); factor_out[s] = 0 for the others,
+//     whose T row is not written.  T12 = the 3x4 of T16 (the model's units, the ICP's) for valid streams, the identity
+//     for the others.
+//   The masked cache write: every active stream's new grids (pre_cur, HWp cells each) become its cached previous frame
+//     (pre_prev); inactive streams' slots stay.  cur_image non-NULL: so does its image, [S, 4, H, W] read as HW float4
+//     per stream (HWp = HW then).  The cache was last read by stages that precede this kernel.
+//   H x W: then a stream without a transform has its source grids (cur) emptied, so the ICP finds no source pixel for
+//     it (a stream without a frame has empty grids already; one on its first frame has points).  pre_cur may be cur
+//     (the adapting streams at w_pre = 0 cache their H x W grids): the thread that caches a cell is the one that then
+//     empties it.
 __global__ void __launch_bounds__(256)
 odometry_streams_pre_kernel(const float* __restrict__ T16, const float* __restrict__ factor,
                             const int32_t* __restrict__ active, const int32_t* __restrict__ valid, int S, int HW,
                             int HWp, float* __restrict__ T, float* __restrict__ T12, float* __restrict__ factor_out,
-                            float4* __restrict__ cur_pts, float4* __restrict__ cur_nrm,
-                            const float4* __restrict__ pre_cur_pts, const float4* __restrict__ pre_cur_nrm,
-                            float4* __restrict__ pre_prev_pts, float4* __restrict__ pre_prev_nrm) {
+                            float4* cur_pts, float4* cur_nrm, const float4* pre_cur_pts, const float4* pre_cur_nrm,
+                            float4* __restrict__ pre_prev_pts, float4* __restrict__ pre_prev_nrm,
+                            const float4* __restrict__ cur_image = nullptr, float4* __restrict__ cache_image = nullptr) {
     const size_t i = (size_t)blockIdx.x * 256 + threadIdx.x;
     if (i < (size_t)S * 16) {
         const int s = (int)i / 16, e = (int)i % 16;
@@ -870,13 +887,14 @@ odometry_streams_pre_kernel(const float* __restrict__ T16, const float* __restri
         if (e < 12) T12[s * 12 + e] = ok ? t : (e % 5 == 0 ? 1.0f : 0.0f);
         if (e == 0 && factor_out) factor_out[s] = ok ? factor[s] : 0.0f;
     }
-    if (i < (size_t)S * HW && valid[i / HW] == 0) {
-        cur_pts[i] = empty_grid_cell();
-        cur_nrm[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-    }
     if (i < (size_t)S * HWp && stream_active(active, (int)(i / HWp))) {
         pre_prev_pts[i] = pre_cur_pts[i];
         pre_prev_nrm[i] = pre_cur_nrm[i];
+        if (cur_image) cache_image[i] = cur_image[i];
+    }
+    if (i < (size_t)S * HW && valid[i / HW] == 0) {
+        cur_pts[i] = empty_grid_cell();
+        cur_nrm[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
     }
 }
 
@@ -1396,14 +1414,30 @@ struct OutBwd {
     float* losses;                     // [B, DELORA_LOSS_ROW]: the identity fit writes its objective to [B-1][5]
     int K, ldx, ldz, single;
     int identity;                      // DELORA_LOSS_IDENTITY_FIT: objective MSELoss(T_{B-1}, I) / B, not the ICP mean
+    // delora_odometry_streams_push_adapt (NULL otherwise): the objective is the mean over the rows with valid[b] != 0,
+    // *n_valid of them; each row's quaternion was divided by its own norm; the other rows get dL/dT = 0 and d = 0;
+    // with *n_valid = 0 the step count does not advance
+    const int32_t* valid;
+    const int32_t* n_valid;
 };
 
 __global__ void __launch_bounds__(kBwdThreads)
 odometry_out_bwd_kernel(OutBwd a, int B, float inv_B, int act) {
-    extern __shared__ float s_d[];                          // [B, 7]: d(quaternion), d(translation)
-    __shared__ float s_red[2];
+    extern __shared__ float s_d[];                          // [B, 7]: d(quaternion), d(translation); then [B] norms
+    __shared__ float s_red[2];                              // and [B] d(norm) of the per-row form
+    float* s_nrm = s_d + (size_t)B * 7;
+    float* s_gn = s_nrm + B;
     const float* __restrict__ raw = a.raw;
-    if (threadIdx.x == 0) {                                 // the forward's ordered sum
+    const bool rows = a.valid != nullptr;
+    auto row_ok = [&](int b) { return !rows || a.valid[b] != 0; };
+    if (rows) {                                             // each valid row's norm, the forward's ordered sum
+        for (int b = threadIdx.x; b < B; b += blockDim.x) {
+            if (!row_ok(b)) continue;
+            float ss = 0.0f;
+            for (int j = 0; j < 4; ++j) ss = fmaf(raw[b * 7 + j], raw[b * 7 + j], ss);
+            s_nrm[b] = sqrtf(ss);
+        }
+    } else if (threadIdx.x == 0) {                          // the forward's ordered sum
         float ss = 0.0f;
         for (int b = 0; b < B; ++b)
             for (int j = 0; j < 4; ++j) ss = fmaf(raw[b * 7 + j], raw[b * 7 + j], ss);
@@ -1419,8 +1453,14 @@ odometry_out_bwd_kernel(OutBwd a, int B, float inv_B, int act) {
         }
     }
     __syncthreads();
-    const float nrm = s_red[0];
+    // d(mean over pairs): 1 / B, or 1 / n_valid over the valid rows (read only when a row is valid, so n_valid > 0)
+    const float scale = rows ? 1.0f / (float)*a.n_valid : inv_B;
     for (int b = threadIdx.x; b < B; b += blockDim.x) {
+        if (!row_ok(b)) {
+            for (int o = 0; o < 7; ++o) s_d[b * 7 + o] = 0.0f;
+            continue;
+        }
+        const float nrm = rows ? s_nrm[b] : s_red[0];
         const float* q = raw + b * 7;
         float g[12];
         if (a.identity) {
@@ -1431,23 +1471,34 @@ odometry_out_bwd_kernel(OutBwd a, int B, float inv_B, int act) {
                 g[i] = b == B - 1 ? 0.125f * (a.T16[(size_t)b * 16 + i] - (i % 5 == 0 ? 1.0f : 0.0f)) * inv_B : 0.0f;
         } else {
 #pragma unroll
-            for (int i = 0; i < 12; ++i) g[i] = a.grad_T[(size_t)b * 12 + i] * inv_B;    // d(mean over pairs)
+            for (int i = 0; i < 12; ++i) g[i] = a.grad_T[(size_t)b * 12 + i] * scale;
         }
         quat_to_T_bwd_row(q[0] / nrm, q[1] / nrm, q[2] / nrm, q[3] / nrm, g, s_d + b * 7, s_d + b * 7 + 4);
     }
     __syncthreads();
-    if (threadIdx.x == 0) {                                 // q / n: d n = -sum(g * q) / n^2 over the whole block
-        float s = 0.0f;
-        for (int b = 0; b < B; ++b)
+    if (rows) {                                             // q / n of each row: d n = -sum(g * q) / n^2 over the row
+        for (int b = threadIdx.x; b < B; b += blockDim.x) {
+            if (!row_ok(b)) continue;
+            float s = 0.0f;
             for (int j = 0; j < 4; ++j) s = fmaf(s_d[b * 7 + j], raw[b * 7 + j], s);
-        s_red[1] = -s / (nrm * nrm);
-        a.ctr[0] += 1;
+            s_gn[b] = -s / (s_nrm[b] * s_nrm[b]);
+        }
+    }
+    if (threadIdx.x == 0) {                                 // q / n: d n = -sum(g * q) / n^2 over the whole block
+        if (!rows) {
+            float s = 0.0f;
+            for (int b = 0; b < B; ++b)
+                for (int j = 0; j < 4; ++j) s = fmaf(s_d[b * 7 + j], raw[b * 7 + j], s);
+            s_red[1] = -s / (s_red[0] * s_red[0]);
+        }
+        if (!rows || *a.n_valid > 0) a.ctr[0] += 1;
         a.ctr[1] = B;
     }
     __syncthreads();
-    const float gn = s_red[1];
     for (int i = threadIdx.x; i < B * 4; i += blockDim.x) {  // div backward + norm backward (q * dn / n)
         const int b = i >> 2, j = i & 3;
+        if (!row_ok(b)) continue;
+        const float nrm = rows ? s_nrm[b] : s_red[0], gn = rows ? s_gn[b] : s_red[1];
         s_d[b * 7 + j] = s_d[b * 7 + j] / nrm + raw[b * 7 + j] * (gn / nrm);
     }
     __syncthreads();
@@ -1486,10 +1537,13 @@ odometry_out_bwd_kernel(OutBwd a, int B, float inv_B, int act) {
     }
 }
 
-// torch.optim.Adam (the fused implementation's formula; no weight decay, no amsgrad) on n floats
+// torch.optim.Adam (the fused implementation's formula; no weight decay, no amsgrad) on n floats.  run (device, or
+// NULL for always): the update runs only where *run != 0 (the adapting streams' count of valid pairs).
 __global__ void __launch_bounds__(256)
 odometry_adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-                     long long n, const long long* __restrict__ ctr, float lr, float beta1, float beta2, float eps) {
+                     long long n, const long long* __restrict__ ctr, float lr, float beta1, float beta2, float eps,
+                     const int32_t* __restrict__ run) {
+    if (run && *run == 0) return;                           // run non-NULL: update only when *run != 0
     const float t = (float)ctr[0];
     const float bc1 = 1.0f - powf(beta1, t);
     const float step_size = lr / bc1;
@@ -1649,8 +1703,10 @@ static int linear_bwd(const TailGrad& p0, const TailGrad& p1, int B, int act_in,
 }
 
 // drop.ctr non-NULL: the gradient of resnet.fc's output (dz_fc) is multiplied by keep * 1.25 after act'
+// valid / n_valid (delora_odometry_streams_push_adapt): see OutBwd
 static int train_tail_backward(const TrainPlan& tp, char* ws, int act, int B, bool identity, cudaStream_t st,
-                               DropoutCtr drop = DropoutCtr{nullptr, 0}) {
+                               DropoutCtr drop = DropoutCtr{nullptr, 0}, const int32_t* valid = nullptr,
+                               const int32_t* n_valid = nullptr) {
     const Model& m = tp.m;
     auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
     const float* master = f(tp.master);
@@ -1660,6 +1716,7 @@ static int train_tail_backward(const TrainPlan& tp, char* ws, int act, int B, bo
     memset(&a, 0, sizeof(a));
     a.raw = f(tp.raw); a.grad_T = f(tp.grad_T); a.ctr = reinterpret_cast<long long*>(ws + tp.ctr);
     a.T16 = f(tp.T16); a.losses = f(tp.losses); a.identity = identity ? 1 : 0;
+    a.valid = valid; a.n_valid = n_valid;
     if (m.n_lin == 4) {
         a.K = kHeadHidden; a.ldx = a.ldz = 2 * kHeadHidden; a.single = 0;
         a.w_rot = master + m.lin[1].blob_w; a.w_trans = master + m.lin[3].blob_w;
@@ -1677,7 +1734,7 @@ static int train_tail_backward(const TrainPlan& tp, char* ws, int act, int B, bo
         a.gb_rot = grad + l.blob_b; a.gb_trans = a.gb_rot + 4;
         a.dz = f(tp.dz_hid[last - 1]);
     }
-    odometry_out_bwd_kernel<<<1, kBwdThreads, (size_t)B * 7 * sizeof(float), st>>>(a, B, 1.0f / (float)B, act);
+    odometry_out_bwd_kernel<<<1, kBwdThreads, (size_t)B * 9 * sizeof(float), st>>>(a, B, 1.0f / (float)B, act);
     DELORA_CHECK_LAUNCH("odometry_out_bwd_kernel");
     auto tg = [&](const Linear& l, const float* x, int ldx, const float* dz, int ldz) {
         TailGrad t;
@@ -1815,12 +1872,29 @@ namespace delora {
 
 __global__ void odometry_icp_batch_kernel(long long* __restrict__ ctr, int B) { ctr[1] = B; }
 
+// One tick of delora_odometry_streams_push_adapt, as train_forward_losses sees it: the caller's arguments and the
+// stream section of the workspace.
+struct AdaptTick {
+    const int32_t* active;             // [S] or NULL (every stream is)
+    float* T;                          // [S, 16] the caller's T
+    int32_t* valid;                    // [S] the caller's valid
+    int32_t* has_prev;                 // [S]
+    int32_t* n_valid;                  // [1] the number of valid streams this tick
+    float* cache_image;                // [S, 4, H, W] w_pre = 0 only: each stream's previous image
+    delora_f4* cache_pts;              // [S, H, W] (w_pre = 0) or [S, H, w_pre]: its previous stage-1 grids
+    delora_f4* cache_nrm;
+};
+
 // Stages 1-3 of delora_odometry_train_step and all of delora_odometry_train_eval: the projection + normals of the 2B
 // scans, the forward keeping its activations and the ICP losses with dL/dT, into the workspace (losses, grad_T, T16,
 // pooled).  dropout: the forward draws this step's masks.  Normalised models: T_out [B, 16] or NULL gets T in metres.
+// at (delora_odometry_streams_push_adapt, B = S): stage 1 projects only the B scans of this tick (scan_2 of each pair,
+// inactive streams' counts masked to 0) and takes its first half, scan_1's, from the cache; the output kernel divides
+// each quaternion by its own row's norm, writes raw for the valid rows only, valid, has_prev and n_valid; then the
+// bookkeeping kernel writes at->T, T12, the masked cache write and empties the sources of the rows without a pair.
 static int train_forward_losses(const delora_odometry_desc* d, const delora_odometry_train_params* hp, const TrainPlan& tp,
                                 char* ws, const float* points, const int32_t* n_points, int B, bool dropout, float* T_out,
-                                cudaStream_t st, const char* who) {
+                                cudaStream_t st, const char* who, const AdaptTick* at = nullptr) {
     const Model& m = tp.m;
     auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
     const int H = d->H, W = d->W, HW = H * W;
@@ -1832,20 +1906,32 @@ static int train_forward_losses(const delora_odometry_desc* d, const delora_odom
 
     // 1. projection + normals of the 2B scans (scan_1 x B, then scan_2 x B).  w_pre > 0: the reference's two stages,
     // projection + normals at H x w_pre (its offline preprocessing), then those grids projected at H x W (Deployer.step)
-    if ((rc = clamp_counts(tp.f, ws, n_points, nullptr, 2 * B, d->n_stride, st))) return rc;
+    // at: only the B scan_2's are projected (from scan index `first` on), and scan_1's stage-1 output is the cache's
+    const int n_proj = at ? B : 2 * B;
+    const size_t first = at ? (size_t)B : 0;
+    if ((rc = clamp_counts(tp.f, ws, n_points, at ? at->active : nullptr, n_proj, d->n_stride, st))) return rc;
     int32_t* counts = reinterpret_cast<int32_t*>(ws + tp.f.counts);
     delora_f4* pts_grid = reinterpret_cast<delora_f4*>(ws + tp.pts_grid);
     delora_f4* nrm_grid = reinterpret_cast<delora_f4*>(ws + tp.nrm_grid);
     float* images = f(tp.f.images);
     uint64_t* keys = reinterpret_cast<uint64_t*>(ws + tp.f.keys);
+    const size_t HWc = (size_t)H * (d->w_pre > 0 ? d->w_pre : W);         // cells of a stage-1 grid
+    auto from_cache = [&](void* dst, const void* src, size_t bytes) {
+        const cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st);
+        DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+        return 0;
+    };
     if (d->w_pre > 0) {
         delora_f4* pre_pts = reinterpret_cast<delora_f4*>(ws + tp.pre_pts_grid);
         delora_f4* pre_nrm = reinterpret_cast<delora_f4*>(ws + tp.pre_nrm_grid);
-        if ((rc = delora_project_normals_fwd(points, counts, 2 * B, 3, d->n_stride, H, d->w_pre, d->hfov0, d->hfov1,
-                                             d->vfov0, d->vfov1, 0, keys, f(tp.pre_image),
-                                             reinterpret_cast<int32_t*>(ws + tp.pre_index_map), hp->nb_h, hp->nb_w,
-                                             hp->epsilon_range, hp->min_neighbors, pre_pts, pre_nrm, nullptr, st)))
+        if ((rc = delora_project_normals_fwd(points, counts, n_proj, 3, d->n_stride, H, d->w_pre, d->hfov0, d->hfov1,
+                                             d->vfov0, d->vfov1, 0, keys, f(tp.pre_image) + first * 4 * HWc,
+                                             reinterpret_cast<int32_t*>(ws + tp.pre_index_map) + first * HWc, hp->nb_h,
+                                             hp->nb_w, hp->epsilon_range, hp->min_neighbors, pre_pts + first * HWc,
+                                             pre_nrm + first * HWc, nullptr, st)))
             return rc;
+        if (at && ((rc = from_cache(pre_pts, at->cache_pts, (size_t)B * HWc * 16)) ||
+                   (rc = from_cache(pre_nrm, at->cache_nrm, (size_t)B * HWc * 16)))) return rc;
         // normalised: the factor of each pair from its stored points (the valid H x w_pre cells), kept in the H x w_pre
         // image, which nothing reads after delora_project_normals_fwd; the stored points are divided by it before the
         // H x W projection, the normals are not
@@ -1855,22 +1941,53 @@ static int train_forward_losses(const delora_odometry_desc* d, const delora_odom
         if ((rc = project_grids_fwd(pre_pts, pre_nrm, 2 * B, d->w_pre, g, keys, images,
                                     reinterpret_cast<int32_t*>(ws + tp.f.index_map), pts_grid, nrm_grid, factor, B, st)))
             return rc;
-    } else if ((rc = delora_project_normals_fwd(points, counts, 2 * B, 3, d->n_stride, H, W, d->hfov0, d->hfov1,
-                                                d->vfov0, d->vfov1, 0, keys, images,
-                                                reinterpret_cast<int32_t*>(ws + tp.f.index_map), hp->nb_h, hp->nb_w,
-                                                hp->epsilon_range, hp->min_neighbors, pts_grid, nrm_grid, nullptr,
-                                                st))) {
-        return rc;
+    } else {
+        if ((rc = delora_project_normals_fwd(points, counts, n_proj, 3, d->n_stride, H, W, d->hfov0, d->hfov1, d->vfov0,
+                                             d->vfov1, 0, keys, images + first * 4 * HW,
+                                             reinterpret_cast<int32_t*>(ws + tp.f.index_map) + first * HW, hp->nb_h,
+                                             hp->nb_w, hp->epsilon_range, hp->min_neighbors, pts_grid + first * HW,
+                                             nrm_grid + first * HW, nullptr, st)))
+            return rc;
+        if (at && ((rc = from_cache(images, at->cache_image, (size_t)B * 4 * HW * 4)) ||
+                   (rc = from_cache(pts_grid, at->cache_pts, (size_t)B * HW * 16)) ||
+                   (rc = from_cache(nrm_grid, at->cache_nrm, (size_t)B * HW * 16)))) return rc;
     }
     // 2. forward, keeping the activations
     if ((rc = trunk_input(m.t, tp.t, ws, images, images + (size_t)B * 4 * HW, B, st, drop_fwd))) return rc;
     if ((rc = trunk_forward(m.t, tp.t, ws, tp.w, ws, d->act, B, f(tp.pooled), nullptr, st, drop_fwd))) return rc;
-    if ((rc = run_tail(m, train_tail_io(tp, ws), d->act, f(tp.pooled), B, f(tp.T16), st, nullptr, drop_fwd))) return rc;
+    if (at) {
+        const TailIO io = train_tail_io(tp, ws);
+        TailLinear rot, trans;
+        if ((rc = run_tail_hidden(m, io, d->act, f(tp.pooled), B, &rot, &trans, st))) return rc;
+        odometry_streams_out_kernel<false><<<1, kTailWarps * 32, (size_t)B * 7 * sizeof(float), st>>>(
+            rot, trans, B, tail_vec(rot) && tail_vec(trans), at->active, at->has_prev, f(tp.T16), at->valid, nullptr,
+            nullptr, nullptr, io.raw, at->n_valid);
+        DELORA_CHECK_LAUNCH("odometry_streams_out_kernel");
+        // T (normalised: the factor of the H x w_pre grids, kept in pre_image as below), T12, the cache, the sources
+        size_t cells = HWc > (size_t)HW ? HWc : (size_t)HW;
+        if (cells < 16) cells = 16;
+        cells *= (size_t)B;
+        float4* cur_pts = reinterpret_cast<float4*>(pts_grid + (size_t)B * HW);
+        float4* cur_nrm = reinterpret_cast<float4*>(nrm_grid + (size_t)B * HW);
+        const bool pre = d->w_pre > 0;
+        odometry_streams_pre_kernel<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(
+            f(tp.T16), normalized ? f(tp.pre_image) : nullptr, at->active, at->valid, B, HW, (int)HWc, at->T, f(tp.T12),
+            nullptr, cur_pts, cur_nrm,
+            pre ? reinterpret_cast<const float4*>(ws + tp.pre_pts_grid) + (size_t)B * HWc : cur_pts,
+            pre ? reinterpret_cast<const float4*>(ws + tp.pre_nrm_grid) + (size_t)B * HWc : cur_nrm,
+            reinterpret_cast<float4*>(at->cache_pts), reinterpret_cast<float4*>(at->cache_nrm),
+            pre ? nullptr : reinterpret_cast<const float4*>(images + (size_t)B * 4 * HW),
+            reinterpret_cast<float4*>(at->cache_image));
+        DELORA_CHECK_LAUNCH("odometry_streams_pre_kernel");
+    } else {
+        if ((rc = run_tail(m, train_tail_io(tp, ws), d->act, f(tp.pooled), B, f(tp.T16), st, nullptr, drop_fwd)))
+            return rc;
+        const cudaError_t e = cudaMemcpy2DAsync(f(tp.T12), 12 * sizeof(float), f(tp.T16), 16 * sizeof(float),
+                                                12 * sizeof(float), B, cudaMemcpyDeviceToDevice, st);
+        DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+    }
     // 3. ICP losses and dL/dT: source = scan_2 moved by T, target = scan_1.  The identity fit still runs them: the
     // reference logs the ICP losses in that phase too
-    const cudaError_t e = cudaMemcpy2DAsync(f(tp.T12), 12 * sizeof(float), f(tp.T16), 16 * sizeof(float),
-                                            12 * sizeof(float), B, cudaMemcpyDeviceToDevice, st);
-    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
     const long long icp_n4 = (delora_icp_scratch_floats(B, HW) + 3) / 4;
     odometry_icp_rearm_kernel<<<2 * num_sms(), 256, 0, st>>>(reinterpret_cast<float4*>(ws + tp.icp), icp_n4, B, ctr);
     DELORA_CHECK_LAUNCH("odometry_icp_rearm_kernel");
@@ -1968,6 +2085,21 @@ static int check_group(const delora_odometry_train_group* g, const void* workspa
     return 0;
 }
 
+// Stage 5 of the step: Adam on the master blob (only where *run != 0, run non-NULL), then the bf16 filters from the
+// master weights
+static int adam_update(const TrainPlan& tp, char* ws, const delora_odometry_train_params* hp, const int32_t* run,
+                       cudaStream_t st) {
+    auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
+    const long long n = tp.m.blob_floats;
+    const long long blocks = (n / 4 + 255) / 256;
+    const int grid = (int)(blocks < 8ll * num_sms() ? (blocks > 0 ? blocks : 1) : 8ll * num_sms());
+    odometry_adam_kernel<<<grid, 256, 0, st>>>(f(tp.master), f(tp.grad), f(tp.adam_m), f(tp.adam_v), n,
+                                               reinterpret_cast<const long long*>(ws + tp.ctr), hp->lr, hp->beta1,
+                                               hp->beta2, hp->eps, run);
+    DELORA_CHECK_LAUNCH("odometry_adam_kernel");
+    return delora_conv_weight_prep_multi(ws + tp.w.table, tp.m.t.n_conv, st);
+}
+
 // delora_odometry_train_step, and with g (world > 1) its group form: bucket k is all-reduced on g->side_stream once
 // the backward has produced it, and `stream` joins g->side_stream before the gradient is read.
 static int train_step(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
@@ -2028,13 +2160,7 @@ static int train_step(const delora_odometry_desc* d, const delora_odometry_train
         DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
     }
     // 5. Adam on the master blob, then the bf16 filters from the updated weights
-    const long long n = m.blob_floats;
-    const long long blocks = (n / 4 + 255) / 256;
-    const int grid = (int)(blocks < 8ll * num_sms() ? (blocks > 0 ? blocks : 1) : 8ll * num_sms());
-    odometry_adam_kernel<<<grid, 256, 0, st>>>(f(tp.master), f(tp.grad), f(tp.adam_m), f(tp.adam_v), n, ctr, hp->lr, hp->beta1,
-                                               hp->beta2, hp->eps);
-    DELORA_CHECK_LAUNCH("odometry_adam_kernel");
-    return delora_conv_weight_prep_multi(ws + tp.w.table, m.t.n_conv, st);
+    return adam_update(tp, ws, hp, nullptr, st);
 }
 
 }  // namespace delora
@@ -2156,6 +2282,136 @@ extern "C" int delora_odometry_train_set_state(const delora_odometry_desc* d, co
     DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
     // the bf16 filters from the new master weights, through the table _train_init wrote
     return delora_conv_weight_prep_multi(ws + tp.w.table, tp.m.t.n_conv, st);
+}
+
+// ================================================================================================ adapting streams
+// delora_odometry_streams_push_adapt: S = max_batch streams served from a training workspace, which takes the training
+// step on the pairs it has just served.  The workspace is the training layout of d (max_batch = S) followed by the
+// stream section; no training offset moves, so every delora_odometry_train_* entry point works on it unchanged.
+namespace delora {
+
+struct AdaptPlan {
+    size_t cache_image;                // w_pre = 0 only: [S, 4, H, W]
+    size_t cache_pts, cache_nrm;       // [S, H, W] (w_pre = 0) or [S, H, w_pre]
+    size_t has_prev, n_valid;          // [S], [1]
+    size_t cache_cells;                // cells of one stream's cached grid
+    size_t total;
+};
+
+static void make_adapt_plan(const delora_odometry_desc* d, TrainPlan* tp, AdaptPlan* ap) {
+    make_train_plan(d, tp);
+    memset(ap, 0, sizeof(AdaptPlan));
+    const size_t S = (size_t)d->max_batch, HW = (size_t)d->H * d->W;
+    size_t off = tp->total;
+    ap->cache_cells = d->w_pre > 0 ? (size_t)d->H * d->w_pre : HW;
+    if (d->w_pre == 0) ap->cache_image = take(off, S * 4 * HW * 4);
+    ap->cache_pts = take(off, S * ap->cache_cells * 16);
+    ap->cache_nrm = take(off, S * ap->cache_cells * 16);
+    ap->has_prev = take(off, S * 4);
+    ap->n_valid = take(off, 4);
+    ap->total = off;
+}
+
+}  // namespace delora
+
+extern "C" int64_t delora_odometry_streams_adapt_workspace_bytes(const delora_odometry_desc* d) {
+    if (check_train_desc(d, "delora_odometry_streams_adapt_workspace_bytes")) return -1;
+    TrainPlan tp;
+    AdaptPlan ap;
+    make_adapt_plan(d, &tp, &ap);
+    return (int64_t)ap.total;
+}
+
+extern "C" int delora_odometry_streams_adapt_init(const delora_odometry_desc* d, const float* weights, void* workspace,
+                                                  void* stream) {
+    const char* who = "delora_odometry_streams_adapt_init";
+    if (check_train_desc(d, who)) return 1;
+    TrainPlan tp;
+    AdaptPlan ap;
+    make_adapt_plan(d, &tp, &ap);
+    cudaStream_t st = (cudaStream_t)stream;
+    // _train_init over the whole workspace zeroes the stream section too; the cached grids then start empty
+    const int rc = train_init(d, ap.total, weights, workspace, st, who);
+    if (rc) return rc;
+    const size_t n = (size_t)d->max_batch * ap.cache_cells;
+    odometry_streams_grid_clear_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
+        reinterpret_cast<float4*>((char*)workspace + ap.cache_pts), reinterpret_cast<float4*>((char*)workspace + ap.cache_nrm),
+        n);
+    DELORA_CHECK_LAUNCH("odometry_streams_grid_clear_kernel");
+    return 0;
+}
+
+extern "C" int delora_odometry_streams_push_adapt(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
+                                                  int update, const float* points, const int32_t* n_points,
+                                                  const int32_t* active, void* workspace, float* T, int32_t* valid,
+                                                  float* losses, void* stream) {
+    const char* who = "delora_odometry_streams_push_adapt";
+    if (check_train_desc(d, who)) return 1;
+    if (check_train_params(hp, who)) return 1;
+    DELORA_CHECK_ARG(update == 0 || update == 1, "%s: update=%d must be 0 or 1", who, update);
+    DELORA_CHECK_ARG((hp->loss_flags & DELORA_LOSS_IDENTITY_FIT) == 0u,
+                     "%s: loss_flags=0x%x has DELORA_LOSS_IDENTITY_FIT, a pre-training phase, not adaptation", who,
+                     hp->loss_flags);
+    DELORA_CHECK_ARG((hp->loss_flags & DELORA_TRAIN_DROPOUT) == 0u,
+                     "%s: loss_flags=0x%x has DELORA_TRAIN_DROPOUT: the served T is dropout-free, and one forward "
+                     "cannot be both", who, hp->loss_flags);
+    DELORA_CHECK_ARG(points, "%s: null points", who);
+    DELORA_CHECK_ARG(n_points, "%s: null n_points", who);
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    DELORA_CHECK_ARG(T, "%s: null T", who);
+    DELORA_CHECK_ARG(valid, "%s: null valid", who);
+    DELORA_CHECK_ARG(losses, "%s: null losses", who);
+    const int S = d->max_batch;
+    if (check_train_call(d, hp, points, n_points, S, workspace, who)) return 1;
+    TrainPlan tp;
+    AdaptPlan ap;
+    make_adapt_plan(d, &tp, &ap);
+    cudaStream_t st = (cudaStream_t)stream;
+    char* ws = (char*)workspace;
+    auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
+    AdaptTick at;
+    at.active = active;
+    at.T = T;
+    at.valid = valid;
+    at.has_prev = reinterpret_cast<int32_t*>(ws + ap.has_prev);
+    at.n_valid = reinterpret_cast<int32_t*>(ws + ap.n_valid);
+    at.cache_image = d->w_pre == 0 ? f(ap.cache_image) : nullptr;
+    at.cache_pts = reinterpret_cast<delora_f4*>(ws + ap.cache_pts);
+    at.cache_nrm = reinterpret_cast<delora_f4*>(ws + ap.cache_nrm);
+    int rc;
+    // 1-3 at B = S, the first frame of every pair from the cache; T, valid, the cache and the emptied sources
+    if ((rc = train_forward_losses(d, hp, tp, ws, points, n_points, S, false, nullptr, st, who, &at))) return rc;
+    odometry_streams_losses_kernel<<<(S * DELORA_LOSS_ROW + 255) / 256, 256, 0, st>>>(valid, S, f(tp.losses), losses);
+    DELORA_CHECK_LAUNCH("odometry_streams_losses_kernel");
+    long long* ctr = reinterpret_cast<long long*>(ws + tp.ctr);
+    if (!update) {          // the ICP scratch now has the layout of S pairs, as after _train_eval
+        odometry_icp_batch_kernel<<<1, 1, 0, st>>>(ctr, S);
+        DELORA_CHECK_LAUNCH("odometry_icp_batch_kernel");
+        return 0;
+    }
+    // 4. the backward of the mean over the valid pairs (invalid rows: dL/dT = 0), then Adam where n_valid > 0
+    if ((rc = train_tail_backward(tp, ws, d->act, S, false, st, DropoutCtr{nullptr, 0}, valid, at.n_valid))) return rc;
+    float* conv_dw[kMaxConv];
+    for (int i = 0; i < tp.m.t.n_conv; ++i) conv_dw[i] = f(tp.grad) + tp.m.t.conv[i].blob;
+    for (int s = 3; s >= 0; --s)
+        if ((rc = trunk_backward(tp.m.t, tp.t, ws, tp.w, ws, d->act, S, f(tp.g_pooled), conv_dw, s, st))) return rc;
+    return adam_update(tp, ws, hp, at.n_valid, st);
+}
+
+extern "C" int delora_odometry_streams_adapt_reset(const delora_odometry_desc* d, const int32_t* mask, void* workspace,
+                                                   void* stream) {
+    const char* who = "delora_odometry_streams_adapt_reset";
+    if (check_train_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(mask, "%s: null mask", who);
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    TrainPlan tp;
+    AdaptPlan ap;
+    make_adapt_plan(d, &tp, &ap);
+    const int S = d->max_batch;
+    odometry_streams_reset_kernel<<<(S + 255) / 256, 256, 0, (cudaStream_t)stream>>>(
+        mask, S, reinterpret_cast<int32_t*>((char*)workspace + ap.has_prev));
+    DELORA_CHECK_LAUNCH("odometry_streams_reset_kernel");
+    return 0;
 }
 
 // ================================================================================================ dropout

@@ -4,7 +4,8 @@
 `delora_odometry_streams_normalized_*` / `_push_normalized`, and on the reference's two-resolution recipe
 `delora_odometry_streams_pre_*` / `_push_pre`) and training (`delora_odometry_train_*`, and
 `delora_odometry_train_step_group` for several workspaces stepped as one data-parallel group,
-`delora_odometry_train_geometries_*` / `_use_geometry` for one workspace shared by several sensor geometries).
+`delora_odometry_train_geometries_*` / `_use_geometry` for one workspace shared by several sensor geometries), and
+streams that adapt the model while serving it (`delora_odometry_streams_adapt_*` / `_push_adapt`).
 
 Each class holds one descriptor and one workspace, a torch uint8 tensor on the current device.  Every call runs on
 torch's current stream at call time, checks its status with `_lib.check` and does not synchronise (except
@@ -266,6 +267,28 @@ class TrainingWorkspace(_Workspace):
         self._call("delora_odometry_train_set_state", *(a.data_ptr() for a in args), step_t.data_ptr(),
                    self.workspace.data_ptr())
         torch.cuda.synchronize()
+
+
+class AdaptiveStreamsWorkspace(TrainingWorkspace):
+    """delora_odometry_streams_adapt_*: S = desc.max_batch streams served from a training workspace that takes the
+    training step on the pairs it has just served.  Every TrainingWorkspace call works on it (weights, get_state /
+    set_state, eval) and leaves the stream section alone; `params` from train_params (without use_dropout)."""
+    SIZE_QUERY = "delora_odometry_streams_adapt_workspace_bytes"
+
+    def _init(self, weights):
+        self._call("delora_odometry_streams_adapt_init", weights.data_ptr(), self.workspace.data_ptr())
+
+    def push(self, points, counts, active, T, valid, losses, update=True):
+        """points [S, 3, n_stride], counts [S], active [S] int32 or None (all active); T [S, 16], valid [S] and losses
+        [S, LOSS_ROW] out, as for PreStreamsWorkspace.push (T of the weights before this tick's update).  update: then
+        one Adam step on the mean objective of the valid pairs (none without a valid pair)."""
+        self._call("delora_odometry_streams_push_adapt", self._params, 1 if update else 0, points.data_ptr(),
+                   counts.data_ptr(), _ptr(active), self.workspace.data_ptr(), T.data_ptr(), valid.data_ptr(),
+                   losses.data_ptr())
+
+    def reset(self, mask):
+        """Forget the previous frame of every stream with mask[s] != 0 (device int32 [S])."""
+        self._call("delora_odometry_streams_adapt_reset", mask.data_ptr(), self.workspace.data_ptr())
 
 
 class GeometriesTrainingWorkspace(TrainingWorkspace):

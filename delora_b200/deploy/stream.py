@@ -18,6 +18,8 @@ OdometryStreams serves several streams of one sensor geometry and model from one
 normalised models, which NormalizedOdometryStreams serves the same way from the normalised streams workspace.  Both feed
 the model raw scans projected at its width (the ROS node's input); PreprocessedOdometryStreams feeds it the images of
 the reference's two-resolution recipe (the Tester's and training's input), with an ICP residual per frame.
+AdaptiveOdometryStreams serves streams from a training workspace and takes the self-supervised training step on the
+pairs it has just served, so the model adapts while it serves.
 """
 import numpy as np
 import torch
@@ -352,3 +354,97 @@ class PreprocessedOdometryStreams(OdometryStreams):
                              "serves the recipe's normals at that width (serve raw scans with OdometryStreams)")
         self._setup(model, config, dataset, n_streams, n_max, use_cuda_graph, True, residual_flags,
                     bool(config.get("normalization_scaling", False)), pre=True)
+
+
+class AdaptiveOdometryStreams:
+    """Several streams served while the model adapts to them (`delora_odometry_streams_push_adapt`): one tick runs the
+    training step's forward at batch `n_streams`, each pair's first frame taken from the workspace, returns each
+    stream's T and ICP loss row, and with update=True takes one Adam step (learning rate `lr`, torch's default betas)
+    on the mean objective of the pairs it served.  T is always that of the weights before the tick's update; the next
+    tick serves the updated model.  Normals at the model's width, or with preprocessing_normals=True at
+    `horizontal_cells_preprocessing` (the reference's recipe, which normalization_scaling needs).  `state_dict()` is the
+    adapted model.  Dropout configs are refused: the served T must be dropout-free."""
+
+    def __init__(self, model, config, dataset, n_streams, n_max, lr, preprocessing_normals=False,
+                 loss_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL):
+        from . import capi, export
+        if config.get("use_dropout", False):
+            raise ValueError("use_dropout: True is not supported by AdaptiveOdometryStreams: the served transforms "
+                             "are dropout-free, and one forward cannot be both")
+        if config.get("normalization_scaling", False) and not preprocessing_normals:
+            raise ValueError("normalization_scaling: True needs preprocessing_normals=True (the reference's recipe: "
+                             "normals from the unscaled points at horizontal_cells_preprocessing)")
+        self.config = config
+        self.device = torch.device(config["device"])
+        if self.device.type != "cuda":
+            raise RuntimeError("AdaptiveOdometryStreams runs on CUDA devices only (no CPU fallback)")
+        self.n_streams, self.n_max = int(n_streams), int(n_max)
+        self.desc = export.desc_from_config(config, dataset, self.n_max, self.n_streams,
+                                            preprocessing_normals=preprocessing_normals)
+        S, n = self.n_streams, self.n_max
+        with torch.cuda.device(self.device):
+            blob = torch.from_numpy(export.pack_state_dict(model.state_dict(), config)).to(self.device)
+            self.workspace = capi.AdaptiveStreamsWorkspace(self.desc, blob,
+                                                           capi.train_params(config, lr, loss_flags=loss_flags))
+            self.points = torch.zeros((S, 3, n), dtype=torch.float32, device=self.device)
+            self.counts = torch.zeros((S,), dtype=torch.int32, device=self.device)
+            self.active = torch.zeros((S,), dtype=torch.int32, device=self.device)
+            self.T = torch.zeros((S, 16), dtype=torch.float32, device=self.device)
+            self.valid = torch.zeros((S,), dtype=torch.int32, device=self.device)
+            self.losses = torch.zeros((S, ops.LOSS_ROW), dtype=torch.float32, device=self.device)
+            self.mask = torch.zeros((S,), dtype=torch.int32, device=self.device)
+        self.relative = [[] for _ in range(S)]
+
+    def push(self, scans, update=True):
+        """scans: n_streams entries, each a [3, N] (or [1, 3, N]) float32 host tensor with N <= n_max, or None.  Returns
+        n_streams entries: (T [1, 4, 4], losses [LOSS_ROW]) numpy arrays for a stream with a pair this tick, else None."""
+        if len(scans) != self.n_streams:
+            raise ValueError(f"push takes {self.n_streams} entries (one per stream, None = inactive), got {len(scans)}")
+        pts = torch.zeros((self.n_streams, 3, self.n_max), dtype=torch.float32)
+        counts = torch.zeros((self.n_streams,), dtype=torch.int32)
+        active = torch.zeros((self.n_streams,), dtype=torch.int32)
+        for s, scan in enumerate(scans):
+            if scan is None:
+                continue
+            scan = scan[0] if scan.dim() == 3 else scan
+            n = int(scan.shape[1])
+            if n > self.n_max:
+                raise ValueError(f"stream {s}: scan has more points than the streams were sized for")
+            pts[s, :, :n] = scan[:3]
+            counts[s] = n
+            active[s] = 1
+        with torch.cuda.device(self.device):
+            self.points.copy_(pts)
+            self.counts.copy_(counts)
+            self.active.copy_(active)
+            self.workspace.push(self.points, self.counts, self.active, self.T, self.valid, self.losses, update)
+            T, valid, losses = self.T.cpu().numpy(), self.valid.cpu().numpy(), self.losses.cpu().numpy()
+        out = []
+        for s in range(self.n_streams):
+            if valid[s]:
+                t = T[s].reshape(1, 4, 4).copy()
+                self.relative[s].append(t)
+                out.append((t, losses[s].copy()))
+            else:
+                out.append(None)
+        return out
+
+    def poses(self, s):
+        """World-frame KITTI poses of stream s so far (src/utility/poses.py:11-58)."""
+        return poses_module.compute_poses(self.relative[s])
+
+    def reset(self, s):
+        """Forget stream s's previous frame and its transforms: its next frame starts it again."""
+        with torch.cuda.device(self.device):
+            self.mask.zero_()
+            self.mask[s] = 1
+            self.workspace.reset(self.mask)
+            torch.cuda.current_stream().synchronize()
+        self.relative[s] = []
+
+    def state_dict(self):
+        """The adapted weights as an OdometryModel state dict (fp32 CPU tensors)."""
+        from . import export
+        with torch.cuda.device(self.device):
+            w = self.workspace.weights().cpu().numpy()
+        return export.unpack_blob(w, self.config)

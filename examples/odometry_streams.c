@@ -3,6 +3,7 @@
  * cudart only.
  *
  *   odometry_streams [--residual | --preprocessing] model.dlw stream0_dir stream1_dir ...
+ *   odometry_streams --adapt LR --adapt-out adapted.dlw model.dlw stream0_dir stream1_dir ...
  *
  * model.dlw is written by bin/export_odometry_weights.py (layout: include/delora_b200.h); every directory holds one
  * stream's KITTI velodyne .bin files ([N, 4] float32 rows: x, y, z, reflectance), taken in name order.  All streams
@@ -23,6 +24,14 @@
  * raw-scan tick: on one H100 80GB HBM3 at 700 W, w_pre 2250, graph-replayed, ms per tick --residual / --preprocessing
  * at 64 x 720: 1.20 / 1.21 (1 stream), 1.41 / 1.47 (4), 5.14 / 5.44 (16); at 64 x 2048: 1.29 / 1.31, 2.31 / 2.38,
  * 8.73 / 8.98 (scripts/gpu_odometry_streams_pre.py, profiles/odometry_streams_pre_h100_700w.json).
+ * --adapt LR --adapt-out FILE.dlw serves the streams while the model adapts to them, through
+ * delora_odometry_streams_push_adapt with update = 1: every tick serves the streams with the current weights, prints
+ * the same three residual columns (the training step's ICP), then takes one Adam step (learning rate LR, betas 0.9 /
+ * 0.999) on the mean objective of the pairs it served.  Normals at the header's w_pre when it is > 0, else on the
+ * model's image; a normalization_scaling file needs w_pre > 0, and a use_dropout file is refused.  At the end the
+ * adapted weights are written to FILE.dlw with the input file's header.  A tick costs one training step at B = S
+ * (64 x 720: 3.51 ms for 1 stream, 14.20 ms for 16, on one H100 80GB HBM3 at 700 W; scripts/
+ * gpu_odometry_streams_adapt.py, profiles/odometry_streams_adapt_h100_700w.json).
  *
  * Build:  cc odometry_streams.c -I include -I $CUDA_HOME/include -L delora_b200 -ldelora_b200 \
  *            -L $CUDA_HOME/lib64 -lcudart -Wl,-rpath,$PWD/delora_b200 -o odometry_streams
@@ -106,10 +115,38 @@ static int32_t read_scan(const char* path, float* dst, int n_stride) {
     return n;
 }
 
+/* the learning rate of --adapt: a finite number >= 0, the whole argument */
+static int parse_lr(const char* arg, float* lr) {
+    char* end;
+    const double v = strtod(arg, &end);
+    if (end == arg || *end != '\0' || !(v >= 0.0) || v > 3.0e38) return 1;
+    *lr = (float)v;
+    return 0;
+}
+
 int main(int argc, char** argv) {
+    const char* adapt_lr = NULL;
+    const char* adapt_out = NULL;
+    while (argc > 2 && (strcmp(argv[1], "--adapt") == 0 || strcmp(argv[1], "--adapt-out") == 0)) {
+        if (strcmp(argv[1], "--adapt") == 0) adapt_lr = argv[2];
+        else adapt_out = argv[2];
+        argc -= 2;
+        argv += 2;
+    }
+    const int adapt = adapt_lr != NULL || adapt_out != NULL;
+    float lr = 0.0f;
+    if (adapt) {
+        if (!adapt_lr || !adapt_out) return fail("--adapt LR and --adapt-out FILE.dlw go together");
+        if (parse_lr(adapt_lr, &lr)) {
+            char msg[256];
+            snprintf(msg, sizeof msg, "--adapt: LR must be a finite number >= 0, got '%s'", adapt_lr);
+            return fail(msg);
+        }
+    }
     const int residual = argc > 1 && strcmp(argv[1], "--residual") == 0;
     const int pre = argc > 1 && strcmp(argv[1], "--preprocessing") == 0;
     if (residual || pre) { --argc; ++argv; }
+    if (adapt && (residual || pre)) return fail("--adapt serves its own residual: drop --residual / --preprocessing");
     if (argc < 3)
         return fail("usage: odometry_streams [--residual | --preprocessing] model.dlw stream_dir [stream_dir ...]");
     const int S = argc - 2;
@@ -125,6 +162,8 @@ int main(int argc, char** argv) {
     if (normalized && residual)
         return fail("--residual is not provided for models trained with normalization_scaling (serve the file "
                     "without it)");
+    if (adapt && (hdr.model_flags & DELORA_MODEL_DROPOUT))
+        return fail("--adapt does not train with dropout: the served transforms are dropout-free");
     if (pre && hdr.desc.w_pre == 0)
         return fail("--preprocessing needs a file with w_pre > 0: export it with bin/export_odometry_weights.py "
                     "--preprocessing-normals");
@@ -157,9 +196,17 @@ int main(int argc, char** argv) {
     rp.nb_h = 7; rp.nb_w = 11;
     rp.epsilon_range = 0.5f;
     rp.min_neighbors = 10;
+    delora_odometry_train_params hp;                       /* --adapt: Adam, and rp's losses and neighbourhood */
+    hp.lr = lr; hp.beta1 = 0.9f; hp.beta2 = 0.999f; hp.eps = 1e-8f;
+    hp.lambda_po2pl = rp.lambda_po2pl;
+    hp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | (normalized ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u);
+    hp.nb_h = rp.nb_h; hp.nb_w = rp.nb_w;
+    hp.epsilon_range = rp.epsilon_range;
+    hp.min_neighbors = rp.min_neighbors;
     int32_t *count, *active, *valid;
     void* workspace;
-    const int64_t ws_bytes = pre          ? delora_odometry_streams_pre_workspace_bytes(d)
+    const int64_t ws_bytes = adapt        ? delora_odometry_streams_adapt_workspace_bytes(d)
+                             : pre        ? delora_odometry_streams_pre_workspace_bytes(d)
                              : residual   ? delora_odometry_streams_residual_workspace_bytes(d)
                              : normalized ? delora_odometry_streams_normalized_workspace_bytes(d)
                                           : delora_odometry_streams_workspace_bytes(d);
@@ -174,11 +221,15 @@ int main(int argc, char** argv) {
     CUDA_OK(cudaMalloc((void**)&losses, (size_t)S * DELORA_LOSS_ROW * sizeof(float)));
     CUDA_OK(cudaMalloc((void**)&factor, (size_t)S * sizeof(float)));
     CUDA_OK(cudaMemcpy(weights, h_blob, (size_t)n_weights * sizeof(float), cudaMemcpyHostToDevice));
-    if (pre) DELORA_OK(delora_odometry_streams_pre_init(d, workspace, stream));
-    else if (residual) DELORA_OK(delora_odometry_streams_residual_init(d, workspace, stream));
-    else if (normalized) DELORA_OK(delora_odometry_streams_normalized_init(d, workspace, stream));
-    else DELORA_OK(delora_odometry_streams_init(d, workspace, stream));
-    DELORA_OK(delora_odometry_streams_load_weights(d, weights, workspace, stream));
+    if (adapt) {
+        DELORA_OK(delora_odometry_streams_adapt_init(d, weights, workspace, stream));
+    } else {
+        if (pre) DELORA_OK(delora_odometry_streams_pre_init(d, workspace, stream));
+        else if (residual) DELORA_OK(delora_odometry_streams_residual_init(d, workspace, stream));
+        else if (normalized) DELORA_OK(delora_odometry_streams_normalized_init(d, workspace, stream));
+        else DELORA_OK(delora_odometry_streams_init(d, workspace, stream));
+        DELORA_OK(delora_odometry_streams_load_weights(d, weights, workspace, stream));
+    }
 
     float* h_points = (float*)malloc(pts_floats * sizeof(float));
     int32_t* h_count = (int32_t*)malloc((size_t)S * sizeof(int32_t));
@@ -198,8 +249,11 @@ int main(int argc, char** argv) {
         CUDA_OK(cudaMemcpyAsync(points, h_points, pts_floats * sizeof(float), cudaMemcpyHostToDevice, stream));
         CUDA_OK(cudaMemcpyAsync(count, h_count, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
         CUDA_OK(cudaMemcpyAsync(active, h_active, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
-        if (pre || residual) {
-            if (pre)
+        if (adapt || pre || residual) {
+            if (adapt)
+                DELORA_OK(delora_odometry_streams_push_adapt(d, &hp, 1, points, count, active, workspace, T, valid,
+                                                             losses, stream));
+            else if (pre)
                 DELORA_OK(delora_odometry_streams_push_pre(d, &rp, points, count, active, workspace, T, valid, losses,
                                                            normalized ? factor : NULL, stream));
             else
@@ -220,12 +274,22 @@ int main(int argc, char** argv) {
             if (!h_valid[s]) continue;
             printf("%d %d", s, k);
             for (int i = 0; i < 12; ++i) printf(" %.9g", h_T[(size_t)s * 16 + i]);
-            if (pre || residual) {
+            if (adapt || pre || residual) {
                 const float* l = h_losses + (size_t)s * DELORA_LOSS_ROW;
                 printf(" %.9g %.9g %.0f", l[1], l[2], l[3]);
             }
             printf("\n");
         }
+    }
+    if (adapt) {            /* the adapted weights, behind the input file's header */
+        DELORA_OK(delora_odometry_train_weights(d, workspace, weights, stream));
+        CUDA_OK(cudaMemcpyAsync(h_blob, weights, (size_t)n_weights * sizeof(float), cudaMemcpyDeviceToHost, stream));
+        CUDA_OK(cudaStreamSynchronize(stream));
+        FILE* o = fopen(adapt_out, "wb");
+        if (!o) return fail("cannot open the --adapt-out file");
+        const int ok = fwrite(&hdr, sizeof hdr, 1, o) == 1 &&
+                       fwrite(h_blob, sizeof(float), (size_t)n_weights, o) == (size_t)n_weights;
+        if (fclose(o) != 0 || !ok) return fail("cannot write the --adapt-out file");
     }
     for (int s = 0; s < S; ++s) {
         for (int i = 0; i < lists[s].n; ++i) free(lists[s].paths[i]);

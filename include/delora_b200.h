@@ -865,6 +865,74 @@ int delora_odometry_train_get_state(const delora_odometry_desc* d, const void* w
 int delora_odometry_train_set_state(const delora_odometry_desc* d, const float* weights, const float* exp_avg,
                                     const float* exp_avg_sq, const int64_t* step, void* workspace, void* stream);
 
+/* ---- Adapting streams: serve S = max_batch streams and take the training step on the pairs just served, one call per
+ * tick.  The model keeps learning on the frames it serves (a new environment, a new sensor mount, a model trained on
+ * another dataset) without a second workspace, a host copy of each stream's previous scan, a second projection and
+ * forward of every pair, or a weight hand-off (_train_weights -> _streams_load_weights) after every update.
+ *
+ * Workspace: the training workspace of d (max_batch = S; delora_odometry_train_workspace_bytes(d) bytes, its layout
+ * unchanged) followed by the stream section, each buffer 256-byte aligned:
+ *   w_pre = 0: each stream's cached previous frame as its H x W image (S * H * W * 16 bytes) and its H x W point and
+ *              normal grids (2 * S * H * W * 16 bytes);
+ *   w_pre > 0: each stream's cached H x w_pre point and normal grids (2 * S * H * w_pre * 16 bytes);
+ *   then has_prev [S] int32 and the device count of valid pairs (one int32).
+ * So every delora_odometry_train_* entry point called with d works on it unchanged and leaves the stream section alone:
+ * _train_weights, _train_get_state / _set_state (the .dlt checkpoint), _train_set_dropout_seed, _train_eval.  Sizes from
+ * the host-only query (layers {2,2,2,2}, resnet_outputs 1000, two heads, n_stride 131072), training -> adapting streams
+ * workspace:
+ *   64 x 720, w_pre 0:    S = 1 325.2 -> 327.3 MiB, S = 4 521.3 -> 529.8 MiB, S = 16 1305.9 -> 1339.7 MiB;
+ *   64 x 720, w_pre 2250: S = 1 341.0 -> 345.4 MiB, S = 4 584.4 -> 602.0 MiB, S = 16 1558.3 -> 1628.7 MiB;
+ *   64 x 2048, w_pre 0:   S = 1 425.5 -> 431.5 MiB, S = 4 922.5 -> 946.5 MiB, S = 16 2910.6 -> 3006.6 MiB.
+ *
+ * delora_odometry_streams_adapt_init: _train_init on the whole workspace (the stream section zeroed: no stream has a
+ * previous frame), then the cached grids emptied.  delora_odometry_streams_adapt_reset: forget the previous frame of
+ * every stream with mask[s] != 0 (device int32 [S]); only launches.
+ *
+ * delora_odometry_streams_push_adapt, one tick: points [S, 3, n_stride], n_points [S], active [S] or NULL (all active),
+ * T [S, 16] and valid [S] as for delora_odometry_streams_push; losses [S, DELORA_LOSS_ROW] as for _streams_push_pre.
+ *   1. The training step's stages 1-3 at B = S: scan_1 of pair s is stream s's cached frame, scan_2 this tick's frame.
+ *      Only this tick's frames are projected (with normals; at w_pre > 0 at H x w_pre, then both frames of every pair
+ *      re-projected at H x W, divided by the pair factor with DELORA_TRAIN_NORMALIZATION_SCALING).
+ *   2. The quaternion of each row is divided by its own row's norm, not by that of the [S, 4] block, so a stream's T
+ *      does not depend on the other streams (the reference's training at batch_size 1 does the same).  The sum has the
+ *      block norm's fmaf order, so at S = 1 the bits are those of _train_step at B = 1 on (previous frame, this frame).
+ *   3. valid[s] = active[s] && stream s has a previous frame.  T (the weights before this tick's update; in metres for
+ *      normalised models) and the loss row are written for valid streams (losses[s][6] = the factor for normalised
+ *      models, as in the step); the T rows of the others are not written, their loss rows are zeros, and their ICP
+ *      sources are emptied, so they cost the ICP no search.
+ *   4. update = 1 only: the backward and one Adam update of the objective mean over the valid pairs of po2po +
+ *      lambda_po2pl * po2pl + pl2pl, i.e. the mean of the valid streams' B = 1 gradients.  1 / n_valid is read on the
+ *      device; invalid rows get dL/dT = 0 and add exact zeros to every sum.  With no valid pair the step count does not
+ *      advance and Adam does not run (the gradient section is still written).  The bf16 filters are re-prepped after
+ *      Adam, so the next tick serves the updated model.  update = 0 serves and scores only, so a host can adapt on its
+ *      own cadence (for instance when the residual rises).
+ *   5. Every active stream's stage-1 output of this tick becomes its cached frame; inactive streams keep theirs.
+ * Only launches, with a sequence that depends on neither `active`, the stream state nor n_valid: one captured graph per
+ * value of `update` serves every tick.  Refused before any launch, naming the field or pointer: everything _train_step
+ * refuses at B = S, update not 0 or 1, a null points / n_points / workspace / T / valid / losses,
+ * DELORA_LOSS_IDENTITY_FIT (a pre-training phase, not adaptation) and DELORA_TRAIN_DROPOUT (the served T is
+ * dropout-free, and one forward cannot be both).  Out of scope: dropout while adapting, mixed geometries in one tick,
+ * several GPUs, and any policy for when to adapt.
+ * Cost, measured on one H100 80GB HBM3 at a 700 W power limit (max SM clock 1980 MHz), graph-replayed ticks, all
+ * streams active, near-identity heads, lr 0, medians of alternating samples, ms per tick at S = 1 / 4 / 16,
+ * update = 0 | update = 1 | _train_step at B = S alone | the two-workspace composition a host needs without this call
+ * (a _streams_push_residual tick, or _streams_push_pre at w_pre > 0, + _train_step at B = S + _train_weights +
+ * _streams_load_weights):
+ *   64 x 720, w_pre 0:    1.20 / 1.41 / 5.12 | 3.51 / 4.43 / 14.20 | 3.50 / 4.42 / 14.23 | 4.82 / 5.95 / 19.54;
+ *   64 x 720, w_pre 2250: 1.23 / 1.47 / 5.45 | 3.58 / 4.50 / 14.46 | 3.56 / 4.51 / 14.52 | 4.92 / 6.11 / 20.12;
+ *   64 x 2048, w_pre 0:   1.31 / 2.33 / 8.78 | 3.79 / 6.67 / 22.89 | 3.76 / 6.66 / 22.91 | 5.20 / 9.13 / 31.83
+ * (scripts/gpu_odometry_streams_adapt.py, profiles/odometry_streams_adapt_h100_700w.json).  An update = 1 tick costs
+ * one _train_step at B = S (within 0.06 ms) and saves the streams tick and the weight hand-off: 1.3-1.6 ms at S = 1,
+ * 5.3-8.9 ms at S = 16.  An update = 0 tick costs what _streams_push_residual / _streams_push_pre cost. */
+int64_t delora_odometry_streams_adapt_workspace_bytes(const delora_odometry_desc* d);   /* host only, -1 if invalid */
+int delora_odometry_streams_adapt_init(const delora_odometry_desc* d, const float* weights, void* workspace,
+                                       void* stream);
+int delora_odometry_streams_push_adapt(const delora_odometry_desc* d, const delora_odometry_train_params* hp, int update,
+                                       const float* points, const int32_t* n_points, const int32_t* active,
+                                       void* workspace, float* T, int32_t* valid, float* losses, void* stream);
+int delora_odometry_streams_adapt_reset(const delora_odometry_desc* d, const int32_t* mask, void* workspace,
+                                        void* stream);
+
 /* ---- Dropout masks of the training step (DELORA_TRAIN_DROPOUT), exactly enough to re-implement them elsewhere:
  * Philox4x32-10 (multipliers 0xD2511F53, 0xCD9E8D57; Weyl constants 0x9E3779B9, 0xBB67AE85; curand's philox4x32_10),
  *   key = (low 32 bits of seed, high 32 bits of seed).  Element i of tensor t at step s: counter = (low 32 bits of
