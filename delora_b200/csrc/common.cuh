@@ -247,6 +247,14 @@ int grad_allreduce_launch(const uint64_t* peer_bufs, const uint64_t* peer_flags,
                           int world, long long offset, long long count, float scale, unsigned seq,
                           const long long* seq_step, unsigned seq_stride, int n_ctas, int n_threads, int32_t* status,
                           cudaStream_t st);
+// The valid-count exchange of the adapting streams' group tick: *tick += 1, then *n_out = the sum over the ranks of
+// their *n_local, through int32 [2][kArMaxWorld] slots at peer_slots[q] and flag word (phase 0, CTA 0) with
+// seq = *tick * seq_stride.
+int count_allreduce_launch(const uint64_t* peer_slots, const uint64_t* peer_flags, int rank, int world,
+                           unsigned seq_stride, long long* tick, const int32_t* n_local, int32_t* n_out, int32_t* status,
+                           cudaStream_t st);
+// Loads count_allreduce_kernel and the device-seq all-reduce kernels on the current device (see grad_allreduce.cu)
+int collective_kernels_preload(const char* who);
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

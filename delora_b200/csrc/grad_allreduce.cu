@@ -154,6 +154,69 @@ grad_allreduce_kernel(ArParams p) {
     ar_meet(p, seq, 1, cta);                                        // every rank's slice has landed everywhere
 }
 
+__device__ __forceinline__ void st_relaxed_sys(int* p, int v) {
+    asm volatile("st.relaxed.sys.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ int ld_relaxed_sys(const int* p) {
+    int v;
+    asm volatile("ld.relaxed.sys.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+
+// The adapting streams' valid-count exchange (delora_odometry_streams_push_adapt_group), one CTA.  p.peer_buf[q] is
+// rank q's exchange slots, int32 [2][kArMaxWorld].  The tick counter advances to t; thread q stores this rank's count in
+// slot [t & 1][rank] of rank q, before its flag store in ar_meet (CTA 0, phase 0, seq = t * seq_stride), whose release
+// orders it; after the meet, thread q's acquire of rank q's flag makes rank q's count of tick t visible in this rank's
+// slot [t & 1][q].  The counts are summed in rank order into *n_out.  The parity of t double-buffers the slots: a rank
+// writes the slots of tick t + 2 only after passing the meet of tick t + 1, i.e. after every peer has finished the
+// kernel of tick t, which read them.  A meet that times out sets *status and carries on with the slot as it is.
+__global__ void __launch_bounds__(kArMaxThreads)
+count_allreduce_kernel(ArParams p, long long* __restrict__ tick, const int32_t* __restrict__ n_local,
+                       int32_t* __restrict__ n_out) {
+    __shared__ int s_n[kArMaxWorld];
+    const long long t = *tick + 1;
+    const int par = (int)(t & 1);
+    const int q = threadIdx.x;
+    if (q < p.world) st_relaxed_sys(reinterpret_cast<int*>(p.peer_buf[q]) + par * kArMaxWorld + p.rank, *n_local);
+    ar_meet(p, (unsigned)t * p.seq_stride, 0, 0);
+    if (q < p.world) s_n[q] = ld_relaxed_sys(reinterpret_cast<const int*>(p.peer_buf[p.rank]) + par * kArMaxWorld + q);
+    __syncthreads();
+    if (q == 0) {
+        int n = 0;
+        for (int r = 0; r < p.world; ++r) n += s_n[r];
+        *n_out = n;
+        *tick = t;
+    }
+}
+
+int count_allreduce_launch(const uint64_t* peer_slots, const uint64_t* peer_flags, int rank, int world,
+                           unsigned seq_stride, long long* tick, const int32_t* n_local, int32_t* n_out, int32_t* status,
+                           cudaStream_t st) {
+    ArParams p;
+    memset(&p, 0, sizeof(p));
+    for (int q = 0; q < world; ++q) {
+        p.peer_buf[q] = peer_slots[q];
+        p.peer_flag[q] = peer_flags[q];
+    }
+    p.rank = rank; p.world = world; p.seq_stride = seq_stride; p.status = status;
+    count_allreduce_kernel<<<1, kArMaxThreads, 0, st>>>(p, tick, n_local, n_out);
+    DELORA_CHECK_LAUNCH("count_allreduce_kernel");
+    return 0;
+}
+
+// Loads the collective kernels of a group tick on the current device now.  Under lazy module loading (CUDA's default)
+// a kernel is loaded at its first launch, and the load waits for the kernels running on the device.  If that device
+// runs a rank that spins in a meet while the peer it waits for is still to be enqueued by the same host thread, the
+// load would hold both until the meet's timeout.
+int collective_kernels_preload(const char* who) {
+    cudaFuncAttributes a;
+    cudaError_t e = cudaFuncGetAttributes(&a, count_allreduce_kernel);
+    if (e == cudaSuccess) e = cudaFuncGetAttributes(&a, grad_allreduce_kernel<true, true>);
+    if (e == cudaSuccess) e = cudaFuncGetAttributes(&a, grad_allreduce_kernel<false, true>);
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+    return 0;
+}
+
 // Both entry points validate their arguments before they get here; count > 0.
 int grad_allreduce_launch(const uint64_t* peer_bufs, const uint64_t* peer_flags, uint64_t multicast_ptr, int rank,
                           int world, long long offset, long long count, float scale, unsigned seq,

@@ -2100,6 +2100,30 @@ static int adam_update(const TrainPlan& tp, char* ws, const delora_odometry_trai
     return delora_conv_weight_prep_multi(ws + tp.w.table, tp.m.t.n_conv, st);
 }
 
+// Bucket k of plan_buckets' schedule is complete on `st`: g->side_stream waits for it through fork_events[k] and
+// all-reduces it in place in every rank's gradient section, times `scale`, seq = *seq_step * seq_stride + seq_add.
+static int bucket_all_reduce(const TrainPlan& tp, const delora_odometry_train_group* g, const long long* b_off,
+                             const long long* b_cnt, int k, float scale, const long long* seq_step, unsigned seq_stride,
+                             unsigned seq_add, cudaStream_t st, const char* who) {
+    uint64_t peer_grad[kArMaxWorld];
+    for (int q = 0; q < g->world; ++q) peer_grad[q] = g->peer_ws[q] + tp.grad;
+    cudaStream_t side = (cudaStream_t)g->side_stream;
+    cudaError_t e = cudaEventRecord((cudaEvent_t)g->fork_events[k], st);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(side, (cudaEvent_t)g->fork_events[k], 0);
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: fork_events[%d]: %s", who, k, cudaGetErrorString(e));
+    return grad_allreduce_launch(peer_grad, g->peer_flags, g->multicast ? g->multicast + tp.grad : 0ull, g->rank,
+                                 g->world, b_off[k], b_cnt[k], scale, seq_add, seq_step, seq_stride, g->n_ctas,
+                                 g->n_threads, g->status, side);
+}
+
+// `st` waits for every bucket all-reduced on g->side_stream
+static int group_join(const delora_odometry_train_group* g, cudaStream_t st, const char* who) {
+    cudaError_t e = cudaEventRecord((cudaEvent_t)g->join_event, (cudaStream_t)g->side_stream);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(st, (cudaEvent_t)g->join_event, 0);
+    DELORA_CHECK_ARG(e == cudaSuccess, "%s: join_event: %s", who, cudaGetErrorString(e));
+    return 0;
+}
+
 // delora_odometry_train_step, and with g (world > 1) its group form: bucket k is all-reduced on g->side_stream once
 // the backward has produced it, and `stream` joins g->side_stream before the gradient is read.
 static int train_step(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
@@ -2119,21 +2143,12 @@ static int train_step(const delora_odometry_desc* d, const delora_odometry_train
     // the masks of this step, regenerated after odometry_out_bwd_kernel has advanced the step count
     const DropoutCtr drop_bwd{dropout ? ctr : nullptr, 1};
     long long b_off[kGroupBuckets], b_cnt[kGroupBuckets];
-    uint64_t peer_grad[kArMaxWorld];
-    if (g) {
-        plan_buckets(m, b_off, b_cnt);
-        for (int q = 0; q < g->world; ++q) peer_grad[q] = g->peer_ws[q] + tp.grad;
-    }
-    cudaStream_t side = g ? (cudaStream_t)g->side_stream : nullptr;
+    if (g) plan_buckets(m, b_off, b_cnt);
     // bucket k is complete on `st`: all-reduce it on the side stream; seq = the step count (advanced by
     // odometry_out_bwd_kernel before bucket 0) * kGroupBuckets + k
     auto all_reduce = [&](int k) -> int {
-        cudaError_t e = cudaEventRecord((cudaEvent_t)g->fork_events[k], st);
-        if (e == cudaSuccess) e = cudaStreamWaitEvent(side, (cudaEvent_t)g->fork_events[k], 0);
-        DELORA_CHECK_ARG(e == cudaSuccess, "%s: fork_events[%d]: %s", who, k, cudaGetErrorString(e));
-        return grad_allreduce_launch(peer_grad, g->peer_flags, g->multicast ? g->multicast + tp.grad : 0ull, g->rank,
-                                     g->world, b_off[k], b_cnt[k], 1.0f / (float)g->world, (unsigned)k, ctr,
-                                     (unsigned)kGroupBuckets, g->n_ctas, g->n_threads, g->status, side);
+        return bucket_all_reduce(tp, g, b_off, b_cnt, k, 1.0f / (float)g->world, ctr, (unsigned)kGroupBuckets,
+                                 (unsigned)k, st, who);
     };
     int rc;
     // 1-3. projection + normals, forward, ICP losses and dL/dT
@@ -2147,11 +2162,7 @@ static int train_step(const delora_odometry_desc* d, const delora_odometry_train
         if ((rc = trunk_backward(m.t, tp.t, ws, tp.w, ws, d->act, B, f(tp.g_pooled), conv_dw, s, st, drop_bwd))) return rc;
         if (g && (rc = all_reduce(4 - s))) return rc;
     }
-    if (g) {
-        cudaError_t e = cudaEventRecord((cudaEvent_t)g->join_event, side);
-        if (e == cudaSuccess) e = cudaStreamWaitEvent(st, (cudaEvent_t)g->join_event, 0);
-        DELORA_CHECK_ARG(e == cudaSuccess, "%s: join_event: %s", who, cudaGetErrorString(e));
-    }
+    if (g && (rc = group_join(g, st, who))) return rc;
     // outputs (T: the weights before the update)
     if ((rc = train_outputs(tp, ws, B, normalized, losses, T, pooled, st, who))) return rc;
     if (grads) {
@@ -2312,26 +2323,33 @@ static void make_adapt_plan(const delora_odometry_desc* d, TrainPlan* tp, AdaptP
     ap->total = off;
 }
 
-}  // namespace delora
+// The group section of delora_odometry_streams_push_adapt_group, one 256-byte block after the adapting-streams layout:
+// the tick counter (int64: group ticks with update = 1 so far), the fleet-wide count of valid pairs of the last such
+// tick (int32) and the count exchange's slots (int32 [2][kArMaxWorld], see count_allreduce_kernel).
+struct AdaptGroupPlan {
+    size_t tick, n_fleet, slots;
+    size_t total;
+};
 
-extern "C" int64_t delora_odometry_streams_adapt_workspace_bytes(const delora_odometry_desc* d) {
-    if (check_train_desc(d, "delora_odometry_streams_adapt_workspace_bytes")) return -1;
-    TrainPlan tp;
-    AdaptPlan ap;
-    make_adapt_plan(d, &tp, &ap);
-    return (int64_t)ap.total;
+static void make_adapt_group_plan(const delora_odometry_desc* d, TrainPlan* tp, AdaptPlan* ap, AdaptGroupPlan* gp) {
+    make_adapt_plan(d, tp, ap);
+    size_t off = ap->total;
+    const size_t base = take(off, 8 + 8 + 2 * kArMaxWorld * 4);
+    gp->tick = base;
+    gp->n_fleet = base + 8;
+    gp->slots = base + 16;
+    gp->total = off;
 }
 
-extern "C" int delora_odometry_streams_adapt_init(const delora_odometry_desc* d, const float* weights, void* workspace,
-                                                  void* stream) {
-    const char* who = "delora_odometry_streams_adapt_init";
-    if (check_train_desc(d, who)) return 1;
+// _streams_adapt_init on a workspace of `total` bytes (>= d's adapting-streams size); everything past the stream
+// section is zeroed too
+static int adapt_init(const delora_odometry_desc* d, size_t total, const float* weights, void* workspace,
+                      cudaStream_t st, const char* who) {
     TrainPlan tp;
     AdaptPlan ap;
     make_adapt_plan(d, &tp, &ap);
-    cudaStream_t st = (cudaStream_t)stream;
     // _train_init over the whole workspace zeroes the stream section too; the cached grids then start empty
-    const int rc = train_init(d, ap.total, weights, workspace, st, who);
+    const int rc = train_init(d, total, weights, workspace, st, who);
     if (rc) return rc;
     const size_t n = (size_t)d->max_batch * ap.cache_cells;
     odometry_streams_grid_clear_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
@@ -2341,11 +2359,10 @@ extern "C" int delora_odometry_streams_adapt_init(const delora_odometry_desc* d,
     return 0;
 }
 
-extern "C" int delora_odometry_streams_push_adapt(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
-                                                  int update, const float* points, const int32_t* n_points,
-                                                  const int32_t* active, void* workspace, float* T, int32_t* valid,
-                                                  float* losses, void* stream) {
-    const char* who = "delora_odometry_streams_push_adapt";
+// What _push_adapt and _push_adapt_group refuse alike
+static int check_push_adapt(const delora_odometry_desc* d, const delora_odometry_train_params* hp, int update,
+                            const float* points, const int32_t* n_points, void* workspace, float* T, int32_t* valid,
+                            float* losses, const char* who) {
     if (check_train_desc(d, who)) return 1;
     if (check_train_params(hp, who)) return 1;
     DELORA_CHECK_ARG(update == 0 || update == 1, "%s: update=%d must be 0 or 1", who, update);
@@ -2361,11 +2378,23 @@ extern "C" int delora_odometry_streams_push_adapt(const delora_odometry_desc* d,
     DELORA_CHECK_ARG(T, "%s: null T", who);
     DELORA_CHECK_ARG(valid, "%s: null valid", who);
     DELORA_CHECK_ARG(losses, "%s: null losses", who);
+    return check_train_call(d, hp, points, n_points, d->max_batch, workspace, who);
+}
+
+// One tick of _push_adapt, and with g (world > 1, update = 1) of its group form: the count of valid pairs is
+// exchanged (collective k = 0) before the backward, which then divides by the fleet-wide count; the gradient buckets
+// are summed over the ranks on g->side_stream (collectives k = 1 .. kGroupBuckets); Adam runs where that count is > 0.
+// The group's sequence numbers come from its tick counter, seq = tick * (kGroupBuckets + 1) + k, which advances on
+// every group tick with update = 1, so a tick without a valid pair still takes new numbers.
+static int push_adapt(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
+                      const delora_odometry_train_group* g, int update, const float* points, const int32_t* n_points,
+                      const int32_t* active, void* workspace, float* T, int32_t* valid, float* losses, void* stream,
+                      const char* who) {
     const int S = d->max_batch;
-    if (check_train_call(d, hp, points, n_points, S, workspace, who)) return 1;
     TrainPlan tp;
     AdaptPlan ap;
-    make_adapt_plan(d, &tp, &ap);
+    AdaptGroupPlan gp;
+    make_adapt_group_plan(d, &tp, &ap, &gp);
     cudaStream_t st = (cudaStream_t)stream;
     char* ws = (char*)workspace;
     auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
@@ -2389,13 +2418,97 @@ extern "C" int delora_odometry_streams_push_adapt(const delora_odometry_desc* d,
         DELORA_CHECK_LAUNCH("odometry_icp_batch_kernel");
         return 0;
     }
+    const int32_t* n_valid = at.n_valid;
+    long long* tick = reinterpret_cast<long long*>(ws + gp.tick);
+    constexpr unsigned kSeqStride = kGroupBuckets + 1;
+    long long b_off[kGroupBuckets], b_cnt[kGroupBuckets];
+    if (g) {                // the fleet-wide count of valid pairs, on every rank before its backward
+        uint64_t peer_slots[kArMaxWorld];
+        for (int q = 0; q < g->world; ++q) peer_slots[q] = g->peer_ws[q] + gp.slots;
+        int32_t* n_fleet = reinterpret_cast<int32_t*>(ws + gp.n_fleet);
+        if ((rc = count_allreduce_launch(peer_slots, g->peer_flags, g->rank, g->world, kSeqStride, tick, at.n_valid,
+                                         n_fleet, g->status, st))) return rc;
+        n_valid = n_fleet;
+        plan_buckets(tp.m, b_off, b_cnt);
+    }
+    // each rank divides by the fleet-wide count, so the buckets are summed (scale 1)
+    auto all_reduce = [&](int k) -> int {
+        return bucket_all_reduce(tp, g, b_off, b_cnt, k, 1.0f, tick, kSeqStride, (unsigned)k + 1u, st, who);
+    };
     // 4. the backward of the mean over the valid pairs (invalid rows: dL/dT = 0), then Adam where n_valid > 0
-    if ((rc = train_tail_backward(tp, ws, d->act, S, false, st, DropoutCtr{nullptr, 0}, valid, at.n_valid))) return rc;
+    if ((rc = train_tail_backward(tp, ws, d->act, S, false, st, DropoutCtr{nullptr, 0}, valid, n_valid))) return rc;
+    if (g && (rc = all_reduce(0))) return rc;
     float* conv_dw[kMaxConv];
     for (int i = 0; i < tp.m.t.n_conv; ++i) conv_dw[i] = f(tp.grad) + tp.m.t.conv[i].blob;
-    for (int s = 3; s >= 0; --s)
+    for (int s = 3; s >= 0; --s) {
         if ((rc = trunk_backward(tp.m.t, tp.t, ws, tp.w, ws, d->act, S, f(tp.g_pooled), conv_dw, s, st))) return rc;
-    return adam_update(tp, ws, hp, at.n_valid, st);
+        if (g && (rc = all_reduce(4 - s))) return rc;
+    }
+    if (g && (rc = group_join(g, st, who))) return rc;
+    return adam_update(tp, ws, hp, n_valid, st);
+}
+
+}  // namespace delora
+
+extern "C" int64_t delora_odometry_streams_adapt_workspace_bytes(const delora_odometry_desc* d) {
+    if (check_train_desc(d, "delora_odometry_streams_adapt_workspace_bytes")) return -1;
+    TrainPlan tp;
+    AdaptPlan ap;
+    make_adapt_plan(d, &tp, &ap);
+    return (int64_t)ap.total;
+}
+
+extern "C" int delora_odometry_streams_adapt_init(const delora_odometry_desc* d, const float* weights, void* workspace,
+                                                  void* stream) {
+    const char* who = "delora_odometry_streams_adapt_init";
+    if (check_train_desc(d, who)) return 1;
+    TrainPlan tp;
+    AdaptPlan ap;
+    make_adapt_plan(d, &tp, &ap);
+    return adapt_init(d, ap.total, weights, workspace, (cudaStream_t)stream, who);
+}
+
+extern "C" int delora_odometry_streams_push_adapt(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
+                                                  int update, const float* points, const int32_t* n_points,
+                                                  const int32_t* active, void* workspace, float* T, int32_t* valid,
+                                                  float* losses, void* stream) {
+    const char* who = "delora_odometry_streams_push_adapt";
+    if (check_push_adapt(d, hp, update, points, n_points, workspace, T, valid, losses, who)) return 1;
+    return push_adapt(d, hp, nullptr, update, points, n_points, active, workspace, T, valid, losses, stream, who);
+}
+
+extern "C" int64_t delora_odometry_streams_adapt_group_workspace_bytes(const delora_odometry_desc* d) {
+    if (check_train_desc(d, "delora_odometry_streams_adapt_group_workspace_bytes")) return -1;
+    TrainPlan tp;
+    AdaptPlan ap;
+    AdaptGroupPlan gp;
+    make_adapt_group_plan(d, &tp, &ap, &gp);
+    return (int64_t)gp.total;
+}
+
+extern "C" int delora_odometry_streams_adapt_group_init(const delora_odometry_desc* d, const float* weights,
+                                                        void* workspace, void* stream) {
+    const char* who = "delora_odometry_streams_adapt_group_init";
+    if (check_train_desc(d, who)) return 1;
+    TrainPlan tp;
+    AdaptPlan ap;
+    AdaptGroupPlan gp;
+    make_adapt_group_plan(d, &tp, &ap, &gp);
+    if (adapt_init(d, gp.total, weights, workspace, (cudaStream_t)stream, who)) return 1;
+    return collective_kernels_preload(who);
+}
+
+extern "C" int delora_odometry_streams_push_adapt_group(const delora_odometry_desc* d,
+                                                        const delora_odometry_train_params* hp,
+                                                        const delora_odometry_train_group* g, int update,
+                                                        const float* points, const int32_t* n_points,
+                                                        const int32_t* active, void* workspace, float* T,
+                                                        int32_t* valid, float* losses, void* stream) {
+    const char* who = "delora_odometry_streams_push_adapt_group";
+    if (check_push_adapt(d, hp, update, points, n_points, workspace, T, valid, losses, who)) return 1;
+    if (check_group(g, workspace, who)) return 1;
+    return push_adapt(d, hp, g->world > 1 && update ? g : nullptr, update, points, n_points, active, workspace, T,
+                      valid, losses, stream, who);
 }
 
 extern "C" int delora_odometry_streams_adapt_reset(const delora_odometry_desc* d, const int32_t* mask, void* workspace,

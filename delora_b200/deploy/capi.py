@@ -5,7 +5,8 @@
 `delora_odometry_streams_pre_*` / `_push_pre`) and training (`delora_odometry_train_*`, and
 `delora_odometry_train_step_group` for several workspaces stepped as one data-parallel group,
 `delora_odometry_train_geometries_*` / `_use_geometry` for one workspace shared by several sensor geometries), and
-streams that adapt the model while serving it (`delora_odometry_streams_adapt_*` / `_push_adapt`).
+streams that adapt the model while serving it (`delora_odometry_streams_adapt_*` / `_push_adapt`, and
+`delora_odometry_streams_push_adapt_group` for one model adapted from the streams of several workspaces).
 
 Each class holds one descriptor and one workspace, a torch uint8 tensor on the current device.  Every call runs on
 torch's current stream at call time, checks its status with `_lib.check` and does not synchronise (except
@@ -373,3 +374,36 @@ class TrainingGroup:
         """Zero every rank's flag words (after a set_state that moved the step count; no step in flight)."""
         for f in self.flags:
             f.zero_()
+
+
+class AdaptiveStreamsGroupWorkspace(AdaptiveStreamsWorkspace):
+    """delora_odometry_streams_adapt_group_*: the adapting-streams layout with the group section appended; every
+    AdaptiveStreamsWorkspace call works on it.  `push_group` takes one group tick with a _lib.OdometryTrainGroup."""
+    SIZE_QUERY = "delora_odometry_streams_adapt_group_workspace_bytes"
+
+    def _init(self, weights):
+        self._call("delora_odometry_streams_adapt_group_init", weights.data_ptr(), self.workspace.data_ptr())
+
+    def push_group(self, group, points, counts, active, T, valid, losses, update=True):
+        """AdaptiveStreamsWorkspace.push as rank `group.rank`: with update, the step on the mean over the valid pairs
+        of every rank."""
+        self._call("delora_odometry_streams_push_adapt_group", self._params, ctypes.byref(group), 1 if update else 0,
+                   points.data_ptr(), counts.data_ptr(), _ptr(active), self.workspace.data_ptr(), T.data_ptr(),
+                   valid.data_ptr(), losses.data_ptr())
+
+
+class AdaptingStreamsGroup(TrainingGroup):
+    """TrainingGroup over N AdaptiveStreamsGroupWorkspaces (same descriptor and state, N devices with peer access or
+    one device): one model adapted from the streams of every rank.  `push(r, ...)` runs rank r's tick on the current
+    stream of its device; every rank makes the same number of update = True calls."""
+
+    def push(self, rank, points, counts, active, update=True, out=None):
+        """points [S, 3, n_stride], counts [S], active [S] int32 or None -> (T [S, 16], valid [S], losses [S, LOSS_ROW]),
+        into `out` when given."""
+        w = self.workspaces[rank]
+        if out is None:
+            S, dev = w.desc.max_batch, w.workspace.device
+            out = (torch.empty((S, 16), dtype=torch.float32, device=dev), torch.empty((S,), dtype=torch.int32, device=dev),
+                   torch.empty((S, ops.LOSS_ROW), dtype=torch.float32, device=dev))
+        w.push_group(self.groups[rank], points, counts, active, *out, update=update)
+        return out

@@ -3,7 +3,7 @@
  * cudart only.
  *
  *   odometry_streams [--residual | --preprocessing] model.dlw stream0_dir stream1_dir ...
- *   odometry_streams --adapt LR --adapt-out adapted.dlw model.dlw stream0_dir stream1_dir ...
+ *   odometry_streams --adapt LR --adapt-out adapted.dlw [--gpus N] model.dlw stream0_dir stream1_dir ...
  *
  * model.dlw is written by bin/export_odometry_weights.py (layout: include/delora_b200.h); every directory holds one
  * stream's KITTI velodyne .bin files ([N, 4] float32 rows: x, y, z, reflectance), taken in name order.  All streams
@@ -32,11 +32,19 @@
  * adapted weights are written to FILE.dlw with the input file's header.  A tick costs one training step at B = S
  * (64 x 720: 3.51 ms for 1 stream, 14.20 ms for 16, on one H100 80GB HBM3 at 700 W; scripts/
  * gpu_odometry_streams_adapt.py, profiles/odometry_streams_adapt_h100_700w.json).
+ * --adapt ... --gpus N adapts ONE model from streams served on GPUs 0 .. N-1 of this process, one host thread per GPU,
+ * peer access between every pair, through delora_odometry_streams_push_adapt_group: each GPU serves S = ceil(streams /
+ * N) streams, stream s on GPU s / S (the streams past the last directory stay inactive), and every tick's update is
+ * the mean over the valid pairs of all GPUs, so all GPUs keep the same weights.  GPU 0 writes FILE.dlw.  The output
+ * lines are the same as on one GPU; --gpus 1 writes the file a run without the option writes.  --gpus is refused
+ * without --adapt.
  *
  * Build:  cc odometry_streams.c -I include -I $CUDA_HOME/include -L delora_b200 -ldelora_b200 \
- *            -L $CUDA_HOME/lib64 -lcudart -Wl,-rpath,$PWD/delora_b200 -o odometry_streams
+ *            -L $CUDA_HOME/lib64 -lcudart -lpthread -Wl,-rpath,$PWD/delora_b200 -o odometry_streams
  */
 #include <dirent.h>
+#include <pthread.h>
+#include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -115,6 +123,188 @@ static int32_t read_scan(const char* path, float* dst, int n_stride) {
     return n;
 }
 
+/* --adapt --gpus N: one GPU of the group, serving streams rank * S .. rank * S + S - 1 (those past the last directory
+ * stay inactive), and the tick its thread runs */
+typedef struct {
+    int rank, S, k;
+    const delora_odometry_desc* d;
+    const delora_odometry_train_params* hp;
+    const scan_list* lists;
+    int n_lists;
+    cudaStream_t stream, side;
+    cudaEvent_t events[DELORA_TRAIN_GROUP_BUCKETS + 1];
+    delora_odometry_train_group g;
+    void* workspace;
+    void* flags;
+    int32_t* status;
+    float *weights, *points, *T, *losses;
+    int32_t *count, *active, *valid;
+    float *h_points, *h_T, *h_losses;
+    int32_t *h_count, *h_active, *h_valid, h_status;
+    int rc;
+} rank_state;
+
+/* tick k of one rank: its scans up, one group tick with update = 1, T / valid / losses down */
+static int rank_tick(rank_state* r) {
+    const delora_odometry_desc* d = r->d;
+    const int S = r->S;
+    const size_t pts_floats = (size_t)S * 3 * d->n_stride;
+    CUDA_OK(cudaSetDevice(r->rank));
+    for (int s = 0; s < S; ++s) {
+        const int gs = r->rank * S + s;
+        r->h_active[s] = gs < r->n_lists && r->k < r->lists[gs].n;
+        r->h_count[s] = 0;
+        if (!r->h_active[s]) continue;
+        r->h_count[s] = read_scan(r->lists[gs].paths[r->k], r->h_points + (size_t)s * 3 * d->n_stride, d->n_stride);
+        if (r->h_count[s] < 0) return fail("cannot read a scan (missing, truncated or more points than n_stride)");
+    }
+    CUDA_OK(cudaMemcpyAsync(r->points, r->h_points, pts_floats * sizeof(float), cudaMemcpyHostToDevice, r->stream));
+    CUDA_OK(cudaMemcpyAsync(r->count, r->h_count, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, r->stream));
+    CUDA_OK(cudaMemcpyAsync(r->active, r->h_active, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, r->stream));
+    DELORA_OK(delora_odometry_streams_push_adapt_group(d, r->hp, &r->g, 1, r->points, r->count, r->active, r->workspace,
+                                                       r->T, r->valid, r->losses, r->stream));
+    CUDA_OK(cudaMemcpyAsync(r->h_losses, r->losses, (size_t)S * DELORA_LOSS_ROW * sizeof(float), cudaMemcpyDeviceToHost,
+                            r->stream));
+    CUDA_OK(cudaMemcpyAsync(r->h_T, r->T, (size_t)S * 16 * sizeof(float), cudaMemcpyDeviceToHost, r->stream));
+    CUDA_OK(cudaMemcpyAsync(r->h_valid, r->valid, (size_t)S * sizeof(int32_t), cudaMemcpyDeviceToHost, r->stream));
+    CUDA_OK(cudaMemcpyAsync(&r->h_status, r->status, sizeof(int32_t), cudaMemcpyDeviceToHost, r->stream));
+    CUDA_OK(cudaStreamSynchronize(r->stream));
+    if (r->h_status != 0) return fail("--gpus: a peer did not reach the collective within 20 s");
+    return 0;
+}
+
+static void* rank_thread(void* arg) {
+    rank_state* r = (rank_state*)arg;
+    r->rc = rank_tick(r);
+    return NULL;
+}
+
+/* one GPU's workspace (initialised from the host blob), buffers, streams, events and zeroed flag words */
+static int rank_setup(rank_state* r, int world, const float* h_blob, int64_t n_weights) {
+    const delora_odometry_desc* d = r->d;
+    const int S = r->S;
+    CUDA_OK(cudaSetDevice(r->rank));
+    for (int q = 0; q < world; ++q) {
+        if (q == r->rank) continue;
+        int can = 0;
+        CUDA_OK(cudaDeviceCanAccessPeer(&can, r->rank, q));
+        if (!can) return fail("--gpus: a pair of GPUs has no peer access");
+        const cudaError_t e = cudaDeviceEnablePeerAccess(q, 0);
+        if (e == cudaErrorPeerAccessAlreadyEnabled) cudaGetLastError();
+        else CUDA_OK(e);
+    }
+    const int64_t ws_bytes = delora_odometry_streams_adapt_group_workspace_bytes(d);
+    if (ws_bytes < 0) return fail(delora_last_error());
+    const size_t pts_floats = (size_t)S * 3 * d->n_stride;
+    CUDA_OK(cudaStreamCreate(&r->stream));
+    CUDA_OK(cudaStreamCreate(&r->side));
+    for (int k = 0; k <= DELORA_TRAIN_GROUP_BUCKETS; ++k)
+        CUDA_OK(cudaEventCreateWithFlags(&r->events[k], cudaEventDisableTiming));
+    CUDA_OK(cudaMalloc(&r->workspace, (size_t)ws_bytes));
+    CUDA_OK(cudaMalloc(&r->flags, (size_t)delora_grad_allreduce_flag_words() * sizeof(uint32_t)));
+    CUDA_OK(cudaMalloc((void**)&r->status, sizeof(int32_t)));
+    CUDA_OK(cudaMalloc((void**)&r->weights, (size_t)n_weights * sizeof(float)));
+    CUDA_OK(cudaMalloc((void**)&r->points, pts_floats * sizeof(float)));
+    CUDA_OK(cudaMalloc((void**)&r->count, (size_t)S * sizeof(int32_t)));
+    CUDA_OK(cudaMalloc((void**)&r->active, (size_t)S * sizeof(int32_t)));
+    CUDA_OK(cudaMalloc((void**)&r->valid, (size_t)S * sizeof(int32_t)));
+    CUDA_OK(cudaMalloc((void**)&r->T, (size_t)S * 16 * sizeof(float)));
+    CUDA_OK(cudaMalloc((void**)&r->losses, (size_t)S * DELORA_LOSS_ROW * sizeof(float)));
+    CUDA_OK(cudaMemset(r->flags, 0, (size_t)delora_grad_allreduce_flag_words() * sizeof(uint32_t)));
+    CUDA_OK(cudaMemset(r->status, 0, sizeof(int32_t)));
+    CUDA_OK(cudaMemcpy(r->weights, h_blob, (size_t)n_weights * sizeof(float), cudaMemcpyHostToDevice));
+    DELORA_OK(delora_odometry_streams_adapt_group_init(d, r->weights, r->workspace, r->stream));
+    CUDA_OK(cudaStreamSynchronize(r->stream));
+    r->h_points = (float*)malloc(pts_floats * sizeof(float));
+    r->h_count = (int32_t*)malloc((size_t)S * sizeof(int32_t));
+    r->h_active = (int32_t*)malloc((size_t)S * sizeof(int32_t));
+    r->h_valid = (int32_t*)malloc((size_t)S * sizeof(int32_t));
+    r->h_T = (float*)malloc((size_t)S * 16 * sizeof(float));
+    r->h_losses = (float*)calloc((size_t)S * DELORA_LOSS_ROW, sizeof(float));
+    if (!r->h_points || !r->h_count || !r->h_active || !r->h_valid || !r->h_T || !r->h_losses)
+        return fail("out of host memory");
+    return 0;
+}
+
+static void rank_release(rank_state* r) {
+    cudaSetDevice(r->rank);
+    free(r->h_losses); free(r->h_T); free(r->h_valid); free(r->h_active); free(r->h_count); free(r->h_points);
+    cudaFree(r->losses); cudaFree(r->T); cudaFree(r->valid); cudaFree(r->active); cudaFree(r->count);
+    cudaFree(r->points); cudaFree(r->weights); cudaFree(r->status); cudaFree(r->flags); cudaFree(r->workspace);
+    for (int k = 0; k <= DELORA_TRAIN_GROUP_BUCKETS; ++k) cudaEventDestroy(r->events[k]);
+    cudaStreamDestroy(r->side);
+    cudaStreamDestroy(r->stream);
+}
+
+/* --adapt --gpus N: n_streams streams over GPUs 0 .. N-1, one model adapted from all of them; GPU 0 writes `out` */
+static int adapt_group(int gpus, delora_odometry_desc desc, const delora_odometry_file_header* hdr, float* h_blob,
+                       int64_t n_weights, const scan_list* lists, int n_streams, int ticks,
+                       const delora_odometry_train_params* hp, const char* out) {
+    int n_dev = 0;
+    CUDA_OK(cudaGetDeviceCount(&n_dev));
+    if (gpus > n_dev) return fail("--gpus: more GPUs than the machine has");
+    const int S = (n_streams + gpus - 1) / gpus;
+    desc.max_batch = S;
+    rank_state* ranks = (rank_state*)calloc((size_t)gpus, sizeof *ranks);
+    pthread_t* threads = (pthread_t*)calloc((size_t)gpus, sizeof *threads);
+    if (!ranks || !threads) return fail("out of host memory");
+    for (int r = 0; r < gpus; ++r) {
+        rank_state* R = &ranks[r];
+        R->rank = r; R->S = S; R->d = &desc; R->hp = hp; R->lists = lists; R->n_lists = n_streams;
+        if (rank_setup(R, gpus, h_blob, n_weights)) return 1;
+    }
+    for (int r = 0; r < gpus; ++r) {
+        delora_odometry_train_group* g = &ranks[r].g;
+        memset(g, 0, sizeof *g);
+        g->rank = r; g->world = gpus;
+        for (int q = 0; q < gpus; ++q) {
+            g->peer_ws[q] = (uint64_t)(uintptr_t)ranks[q].workspace;
+            g->peer_flags[q] = (uint64_t)(uintptr_t)ranks[q].flags;
+        }
+        g->multicast = 0;
+        g->n_ctas = 8; g->n_threads = 128;
+        g->status = ranks[r].status;
+        g->side_stream = ranks[r].side;
+        for (int k = 0; k < DELORA_TRAIN_GROUP_BUCKETS; ++k) g->fork_events[k] = ranks[r].events[k];
+        g->join_event = ranks[r].events[DELORA_TRAIN_GROUP_BUCKETS];
+    }
+    for (int k = 0; k < ticks; ++k) {
+        for (int r = 0; r < gpus; ++r) {
+            ranks[r].k = k;
+            if (pthread_create(&threads[r], NULL, rank_thread, &ranks[r]) != 0) return fail("cannot start a thread");
+        }
+        int failed = 0;
+        for (int r = 0; r < gpus; ++r) {
+            pthread_join(threads[r], NULL);
+            failed |= ranks[r].rc;
+        }
+        if (failed) return 1;
+        for (int gs = 0; gs < n_streams; ++gs) {
+            const rank_state* R = &ranks[gs / S];
+            const int s = gs % S;
+            if (!R->h_valid[s]) continue;
+            printf("%d %d", gs, k);
+            for (int i = 0; i < 12; ++i) printf(" %.9g", R->h_T[(size_t)s * 16 + i]);
+            const float* l = R->h_losses + (size_t)s * DELORA_LOSS_ROW;
+            printf(" %.9g %.9g %.0f\n", l[1], l[2], l[3]);
+        }
+    }
+    rank_state* R0 = &ranks[0];             /* every rank holds the same weights: GPU 0 writes them */
+    CUDA_OK(cudaSetDevice(0));
+    DELORA_OK(delora_odometry_train_weights(&desc, R0->workspace, R0->weights, R0->stream));
+    CUDA_OK(cudaMemcpyAsync(h_blob, R0->weights, (size_t)n_weights * sizeof(float), cudaMemcpyDeviceToHost, R0->stream));
+    CUDA_OK(cudaStreamSynchronize(R0->stream));
+    FILE* o = fopen(out, "wb");
+    if (!o) return fail("cannot open the --adapt-out file");
+    const int ok = fwrite(hdr, sizeof *hdr, 1, o) == 1 &&
+                   fwrite(h_blob, sizeof(float), (size_t)n_weights, o) == (size_t)n_weights;
+    if (fclose(o) != 0 || !ok) return fail("cannot write the --adapt-out file");
+    for (int r = 0; r < gpus; ++r) rank_release(&ranks[r]);
+    free(threads);
+    free(ranks);
+    return 0;
+}
+
 /* the learning rate of --adapt: a finite number >= 0, the whole argument */
 static int parse_lr(const char* arg, float* lr) {
     char* end;
@@ -127,9 +317,12 @@ static int parse_lr(const char* arg, float* lr) {
 int main(int argc, char** argv) {
     const char* adapt_lr = NULL;
     const char* adapt_out = NULL;
-    while (argc > 2 && (strcmp(argv[1], "--adapt") == 0 || strcmp(argv[1], "--adapt-out") == 0)) {
+    const char* gpus_arg = NULL;
+    while (argc > 2 && (strcmp(argv[1], "--adapt") == 0 || strcmp(argv[1], "--adapt-out") == 0 ||
+                        strcmp(argv[1], "--gpus") == 0)) {
         if (strcmp(argv[1], "--adapt") == 0) adapt_lr = argv[2];
-        else adapt_out = argv[2];
+        else if (strcmp(argv[1], "--adapt-out") == 0) adapt_out = argv[2];
+        else gpus_arg = argv[2];
         argc -= 2;
         argv += 2;
     }
@@ -142,6 +335,15 @@ int main(int argc, char** argv) {
             snprintf(msg, sizeof msg, "--adapt: LR must be a finite number >= 0, got '%s'", adapt_lr);
             return fail(msg);
         }
+    }
+    int gpus = 0;
+    if (gpus_arg) {
+        if (!adapt) return fail("--gpus adapts one model on several GPUs: it needs --adapt LR --adapt-out FILE.dlw");
+        char* end;
+        const long v = strtol(gpus_arg, &end, 10);
+        if (end == gpus_arg || *end != '\0' || v < 1 || v > DELORA_GRAD_ALLREDUCE_MAX_WORLD)
+            return fail("--gpus must be in [1, 16]");
+        gpus = (int)v;
     }
     const int residual = argc > 1 && strcmp(argv[1], "--residual") == 0;
     const int pre = argc > 1 && strcmp(argv[1], "--preprocessing") == 0;
@@ -185,6 +387,24 @@ int main(int argc, char** argv) {
         if (lists[s].n > ticks) ticks = lists[s].n;
     }
 
+    delora_odometry_train_params hp;                       /* --adapt: Adam, and the residual's losses and neighbourhood */
+    hp.lr = lr; hp.beta1 = 0.9f; hp.beta2 = 0.999f; hp.eps = 1e-8f;
+    hp.lambda_po2pl = 1.0f;
+    hp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | (normalized ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u);
+    hp.nb_h = 7; hp.nb_w = 11;
+    hp.epsilon_range = 0.5f;
+    hp.min_neighbors = 10;
+    if (gpus) {
+        const int rc = adapt_group(gpus, desc, &hdr, h_blob, n_weights, lists, S, ticks, &hp, adapt_out);
+        for (int s = 0; s < S; ++s) {
+            for (int i = 0; i < lists[s].n; ++i) free(lists[s].paths[i]);
+            free(lists[s].paths);
+        }
+        free(lists);
+        free(h_blob);
+        return rc;
+    }
+
     cudaStream_t stream;
     CUDA_OK(cudaStreamCreate(&stream));
     const size_t pts_floats = (size_t)S * 3 * d->n_stride;
@@ -196,13 +416,6 @@ int main(int argc, char** argv) {
     rp.nb_h = 7; rp.nb_w = 11;
     rp.epsilon_range = 0.5f;
     rp.min_neighbors = 10;
-    delora_odometry_train_params hp;                       /* --adapt: Adam, and rp's losses and neighbourhood */
-    hp.lr = lr; hp.beta1 = 0.9f; hp.beta2 = 0.999f; hp.eps = 1e-8f;
-    hp.lambda_po2pl = rp.lambda_po2pl;
-    hp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | (normalized ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u);
-    hp.nb_h = rp.nb_h; hp.nb_w = rp.nb_w;
-    hp.epsilon_range = rp.epsilon_range;
-    hp.min_neighbors = rp.min_neighbors;
     int32_t *count, *active, *valid;
     void* workspace;
     const int64_t ws_bytes = adapt        ? delora_odometry_streams_adapt_workspace_bytes(d)

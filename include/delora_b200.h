@@ -912,7 +912,7 @@ int delora_odometry_train_set_state(const delora_odometry_desc* d, const float* 
  * refuses at B = S, update not 0 or 1, a null points / n_points / workspace / T / valid / losses,
  * DELORA_LOSS_IDENTITY_FIT (a pre-training phase, not adaptation) and DELORA_TRAIN_DROPOUT (the served T is
  * dropout-free, and one forward cannot be both).  Out of scope: dropout while adapting, mixed geometries in one tick,
- * several GPUs, and any policy for when to adapt.
+ * and any policy for when to adapt; several GPUs adapting one model: delora_odometry_streams_push_adapt_group below.
  * Cost, measured on one H100 80GB HBM3 at a 700 W power limit (max SM clock 1980 MHz), graph-replayed ticks, all
  * streams active, near-identity heads, lr 0, medians of alternating samples, ms per tick at S = 1 / 4 / 16,
  * update = 0 | update = 1 | _train_step at B = S alone | the two-workspace composition a host needs without this call
@@ -1069,6 +1069,55 @@ int64_t delora_odometry_train_grad_offset(const delora_odometry_desc* d);
  * bucket k covers gradient floats [offsets[k], offsets[k] + counts[k]) (multiples of 4).  Non-zero for an invalid
  * descriptor or a null output. */
 int delora_odometry_train_group_buckets(const delora_odometry_desc* d, int64_t* offsets, int64_t* counts);
+
+/* ---- Adapting streams on several GPUs: one model adapted from the streams every rank serves.  Each rank owns one
+ * adapting-streams group workspace (same descriptor, so the same S; a rank with fewer sensors marks the rest inactive;
+ * same weights and Adam state) and calls delora_odometry_streams_push_adapt_group once per tick on its own S streams.
+ * The update of a tick with update = 1 is one Adam step on the mean over the valid pairs of the WHOLE group, whatever
+ * their number on each rank, and every rank ends it with bit-identical weights, m, v and step count.
+ *
+ * Workspace: the adapting-streams layout of d (delora_odometry_streams_adapt_workspace_bytes(d) bytes, unchanged)
+ * followed by a 256-byte group section: a tick counter (int64, the group's update = 1 ticks so far), the fleet-wide
+ * count of valid pairs of the last such tick (int32) and the count exchange's slots.  So _streams_adapt_reset,
+ * _train_weights, _train_get_state / _set_state and _train_eval work on it unchanged.
+ * delora_odometry_streams_adapt_group_init: _streams_adapt_init over the group size; the group section starts at zero.
+ * It also loads the collective kernels on the current device: under lazy module loading a kernel's first launch waits
+ * for the device's running kernels.  Ranks that share one device and one host thread should also take one
+ * _push_adapt tick with update = 1 at the same descriptor first (or run with CUDA_MODULE_LOADING=EAGER), so that no
+ * first launch waits behind a rank that spins in the count exchange for a peer not yet enqueued.
+ *
+ * One tick, update = 1, world > 1 (`g` as for delora_odometry_train_step_group, peer_ws[q] = rank q's group workspace):
+ *   1. _push_adapt's stages 1-3: T, valid, the loss rows and the cache write, the same bits.
+ *   2. The valid-count exchange on `stream` (collective k = 0): one CTA meets the peers through the flag words and
+ *      sums every rank's count in rank order into the fleet-wide count N; the tick counter advances.  On every such
+ *      tick, N = 0 included.
+ *   3. The tail backward divides by N (so a rank without a valid pair contributes exact zeros), then the trunk
+ *      backward, with the DELORA_TRAIN_GROUP_BUCKETS buckets SUMMED over the ranks (scale 1: every rank has already
+ *      divided by N) on side_stream as in _train_step_group.
+ *   4. `stream` joins side_stream; Adam runs on every rank iff N > 0, and the step count advances iff N > 0.
+ * Sequence numbers come from the tick counter: seq = tick * (DELORA_TRAIN_GROUP_BUCKETS + 1) + k, the count exchange
+ * k = 0 and the buckets k = 1 .. DELORA_TRAIN_GROUP_BUCKETS, read on the device, so a captured tick replays correctly
+ * and a tick without a valid pair still takes new numbers.
+ * update = 0 is exactly _push_adapt(update = 0): no collective, the counter stays, so ranks may take different numbers
+ * of serve-only ticks between updates.  world = 1 launches exactly what _push_adapt launches: the same bits.
+ * Contract: every rank makes the same number of update = 1 calls; the flag words are zeroed on every rank before the
+ * first group tick and again after every _adapt_group_init; they serve no other collective (in particular not
+ * _train_step_group on the same workspaces).  status: as for _train_step_group (20 s per meet, then carries on).
+ * Refused before any launch, naming the field: everything _push_adapt refuses and everything _train_step_group
+ * refuses about g.  Out of scope: unequal S per rank, mixed geometries in one tick, dropout or the identity fit while
+ * adapting, more than one node, any policy for when to adapt.
+ * Measured on one H100 80GB HBM3 at a 700 W power limit (max SM clock 1980 MHz), 64 x 720, w_pre 0, graph-replayed
+ * update = 1 ticks, lr 0, medians of paired differences, world = 1 group tick - _push_adapt: -0.002 / -0.003 /
+ * -0.021 ms on 3.54 / 4.40 / 14.21 ms ticks at S = 1 / 4 / 16, i.e. within the noise
+ * (scripts/gpu_odometry_streams_adapt_group.py, profiles/odometry_streams_adapt_group_h100_700w.json).  The count
+ * exchange's cost on a multi-GPU node is not measured yet (the script's --gpus N measures it). */
+int64_t delora_odometry_streams_adapt_group_workspace_bytes(const delora_odometry_desc* d);   /* host only */
+int delora_odometry_streams_adapt_group_init(const delora_odometry_desc* d, const float* weights, void* workspace,
+                                             void* stream);
+int delora_odometry_streams_push_adapt_group(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
+                                             const delora_odometry_train_group* g, int update,
+                                             const float* points, const int32_t* n_points, const int32_t* active,
+                                             void* workspace, float* T, int32_t* valid, float* losses, void* stream);
 
 /* ---- Training on several sensor geometries from one workspace (the reference's `datasets` list,
  * config/deployment_options.yaml:3: its Trainer shuffles over the concatenated datasets, src/deploy/trainer.py:95-101,
