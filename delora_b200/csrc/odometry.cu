@@ -281,16 +281,14 @@ struct InferPlan {
     size_t total;
 };
 
-// streams: S = max_batch streams, this tick's S frames, each stream's previous frame and whether it has one; the
-// trunk and tail then run at B = S.  Otherwise (pairs / push): 2 * max_batch scans and the one cached image of _push.
-// residual (streams only): the sections of the per-frame ICP residual are appended; no other offset moves.
-static void make_infer_plan(const delora_odometry_desc* d, bool streams, bool residual, InferPlan* p) {
+// The frame section (see plan_frames), then the trunk and tail sections that run at up to B = max_batch
+static void plan_inference(const delora_odometry_desc* d, int n_scans, int n_cached, bool has_prev, InferPlan* p) {
     memset(p, 0, sizeof(InferPlan));
     plan_model(d, &p->m);
     const Model& m = p->m;
     const int MB = d->max_batch, nout = d->resnet_outputs;
     size_t off = 0;
-    p->f = streams ? plan_frames(d, MB, MB, true, d->W, off) : plan_frames(d, 2 * MB, 1, false, d->W, off);
+    p->f = plan_frames(d, n_scans, n_cached, has_prev, d->W, off);
     p->t = plan_trunk_acts(m.t, MB, false, off);
     p->pooled = take(off, (size_t)MB * 512 * 4);
     p->fc_out = take(off, (size_t)MB * nout * 4);
@@ -303,47 +301,55 @@ static void make_infer_plan(const delora_odometry_desc* d, bool streams, bool re
         p->lin_w[i] = take(off, (size_t)m.lin[i].K * m.lin[i].N * 4);
         p->lin_b[i] = take(off, (size_t)m.lin[i].N * 4);
     }
-    if (residual) {
-        const size_t HW = (size_t)d->H * d->W;
-        p->pts_grid = take(off, (size_t)MB * HW * 16);
-        p->nrm_grid = take(off, (size_t)MB * HW * 16);
-        p->prev_pts_grid = take(off, (size_t)MB * HW * 16);
-        p->prev_nrm_grid = take(off, (size_t)MB * HW * 16);
-        p->T12 = take(off, (size_t)MB * 12 * 4);
-        p->losses = take(off, (size_t)MB * DELORA_LOSS_ROW * 4);
-        p->grad_T = take(off, (size_t)MB * 12 * 4);
+    p->total = off;
+}
+
+// pairs / push: 2 * max_batch scans and the one cached image of _push
+static void make_infer_plan(const delora_odometry_desc* d, InferPlan* p) {
+    plan_inference(d, 2 * d->max_batch, 1, false, p);
+}
+
+// The streams workspace kinds.  Each one is the layout of the kind it extends with its own sections appended, so no
+// offset of that layout moves and _streams_load_weights and _streams_reset work on every kind.
+//   plain (delora_odometry_streams_push): S = max_batch streams, this tick's S frames, each stream's previous frame and
+//     whether it has one; the trunk and tail then run at B = S.
+//   residual (_push_residual): plain, then the sections of the per-frame ICP residual.
+//   normalized (_push_normalized): plain, then the staged point rows and the pair factors.  Its prev_image section
+//     holds this tick's projection of each previous frame; nothing reads it across ticks.
+//   pre (_push_pre): residual (its H x W grids and ICP sections serve the recipe's ICP), then the H x w_pre sections.
+//     The plain layout's key buffers serve both H x W projections of a tick, its images hold this tick's projection
+//     of both frames of each pair.
+enum class Streams { plain, residual, normalized, pre };
+
+static void make_streams_plan(const delora_odometry_desc* d, Streams kind, InferPlan* p) {
+    const int MB = d->max_batch;
+    plan_inference(d, MB, MB, true, p);
+    const size_t S = (size_t)MB, HW = (size_t)d->H * d->W, HWp = (size_t)d->H * d->w_pre;
+    size_t off = p->total;
+    if (kind == Streams::residual || kind == Streams::pre) {
+        p->pts_grid = take(off, S * HW * 16);
+        p->nrm_grid = take(off, S * HW * 16);
+        p->prev_pts_grid = take(off, S * HW * 16);
+        p->prev_nrm_grid = take(off, S * HW * 16);
+        p->T12 = take(off, S * 12 * 4);
+        p->losses = take(off, S * DELORA_LOSS_ROW * 4);
+        p->grad_T = take(off, S * 12 * 4);
         p->icp = take(off, (size_t)delora_icp_scratch_floats(MB, (int)HW) * 4);
     }
-    p->total = off;
-}
-
-// The normalised streams workspace: the streams layout unchanged (so _streams_load_weights and _streams_reset work on
-// it), then the sections of delora_odometry_streams_push_normalized.  Its prev_image section holds this tick's
-// projection of each previous frame; nothing reads it across ticks.
-static void make_normalized_streams_plan(const delora_odometry_desc* d, InferPlan* p) {
-    make_infer_plan(d, true, false, p);
-    const size_t S = (size_t)d->max_batch;
-    size_t off = p->total;
-    p->stage = take(off, 2 * S * 3 * (size_t)d->n_stride * 4);
-    p->stage_counts = take(off, 3 * S * 4);
-    p->factor = take(off, S * 4);
-    p->total = off;
-}
-
-// The recipe streams workspace: the residual layout unchanged (so _streams_load_weights and _streams_reset work on it;
-// its H x W grids and ICP sections serve the recipe's ICP), then the H x w_pre sections.  The streams layout's key
-// buffers serve both H x W projections of a tick, its images hold this tick's projection of both frames of each pair.
-static void make_pre_streams_plan(const delora_odometry_desc* d, InferPlan* p) {
-    make_infer_plan(d, true, true, p);
-    const size_t S = (size_t)d->max_batch, HWp = (size_t)d->H * d->w_pre;
-    size_t off = p->total;
-    p->pre_keys = take(off, S * HWp * 8);
-    p->pre_image = take(off, S * 4 * HWp * 4);
-    p->pre_index_map = take(off, S * HWp * 4);
-    p->pre_pts = take(off, 2 * S * HWp * 16);
-    p->pre_nrm = take(off, 2 * S * HWp * 16);
-    p->T16 = take(off, S * 16 * 4);
-    p->factor = take(off, S * 4);
+    if (kind == Streams::normalized) {
+        p->stage = take(off, 2 * S * 3 * (size_t)d->n_stride * 4);
+        p->stage_counts = take(off, 3 * S * 4);
+        p->factor = take(off, S * 4);
+    }
+    if (kind == Streams::pre) {
+        p->pre_keys = take(off, S * HWp * 8);
+        p->pre_image = take(off, S * 4 * HWp * 4);
+        p->pre_index_map = take(off, S * HWp * 4);
+        p->pre_pts = take(off, 2 * S * HWp * 16);
+        p->pre_nrm = take(off, 2 * S * HWp * 16);
+        p->T16 = take(off, S * 16 * 4);
+        p->factor = take(off, S * 4);
+    }
     p->total = off;
 }
 
@@ -555,7 +561,7 @@ extern "C" int64_t delora_odometry_weight_floats(const delora_odometry_desc* d) 
 extern "C" int64_t delora_odometry_workspace_bytes(const delora_odometry_desc* d) {
     if (check_desc(d, "delora_odometry_workspace_bytes")) return -1;
     InferPlan p;
-    make_infer_plan(d, false, false, &p);
+    make_infer_plan(d, &p);
     return (int64_t)p.total;
 }
 
@@ -563,7 +569,7 @@ extern "C" int delora_odometry_init(const delora_odometry_desc* d, void* workspa
     if (check_desc(d, "delora_odometry_init")) return 1;
     DELORA_CHECK_ARG(workspace, "delora_odometry_init: null workspace");
     InferPlan p;
-    make_infer_plan(d, false, false, &p);
+    make_infer_plan(d, &p);
     return init_workspace(p.f, p.total, workspace, (cudaStream_t)stream, "delora_odometry_init");
 }
 
@@ -572,7 +578,7 @@ extern "C" int delora_odometry_load_weights(const delora_odometry_desc* d, const
     if (check_desc(d, "delora_odometry_load_weights")) return 1;
     DELORA_CHECK_ARG(weights && workspace, "delora_odometry_load_weights: null pointer");
     InferPlan p;
-    make_infer_plan(d, false, false, &p);
+    make_infer_plan(d, &p);
     return load_weights(p, weights, workspace, (cudaStream_t)stream, "delora_odometry_load_weights");
 }
 
@@ -580,7 +586,7 @@ extern "C" int delora_odometry_load_weights(const delora_odometry_desc* d, const
 static int run_pairs(const delora_odometry_desc* d, const float* points, const int32_t* n_points, int B, void* workspace,
                      float* T, float* pooled, float* factor, cudaStream_t st, const char* who) {
     InferPlan p;
-    make_infer_plan(d, false, false, &p);
+    make_infer_plan(d, &p);
     char* ws = (char*)workspace;
     float* images = reinterpret_cast<float*>(ws + p.f.images);
     const size_t img = (size_t)4 * d->H * d->W;
@@ -627,7 +633,7 @@ extern "C" int delora_odometry_push(const delora_odometry_desc* d, const float* 
     if (check_desc(d, "delora_odometry_push")) return 1;
     DELORA_CHECK_ARG(points && n_points && workspace, "delora_odometry_push: null pointer");
     InferPlan p;
-    make_infer_plan(d, false, false, &p);
+    make_infer_plan(d, &p);
     cudaStream_t st = (cudaStream_t)stream;
     char* ws = (char*)workspace;
     float* image = reinterpret_cast<float*>(ws + p.f.images);
@@ -905,22 +911,131 @@ __global__ void odometry_streams_losses_kernel(const int32_t* __restrict__ valid
     if (i < S * DELORA_LOSS_ROW) losses[i] = valid[i / DELORA_LOSS_ROW] != 0 ? icp_losses[i] : 0.0f;
 }
 
-}  // namespace delora
+// check_desc plus the preprocessing width the recipe streams read (the training rule, but w_pre = 0 is refused)
+static int check_pre_desc(const delora_odometry_desc* d, const char* who) {
+    if (check_desc(d, who)) return 1;
+    DELORA_CHECK_ARG(d->w_pre >= 2 && (long long)d->H * d->w_pre < (1ll << 27),
+                     "%s: w_pre=%d must be >= 2 with H * w_pre < 2^27 (H=%d): the recipe streams estimate the normals "
+                     "at H x w_pre", who, d->w_pre, d->H);
+    return 0;
+}
 
-extern "C" int64_t delora_odometry_streams_workspace_bytes(const delora_odometry_desc* d) {
-    if (check_desc(d, "delora_odometry_streams_workspace_bytes")) return -1;
+static int check_streams_desc(const delora_odometry_desc* d, Streams kind, const char* who) {
+    return kind == Streams::pre ? check_pre_desc(d, who) : check_desc(d, who);
+}
+
+static int64_t streams_workspace_bytes(const delora_odometry_desc* d, Streams kind, const char* who) {
+    if (check_streams_desc(d, kind, who)) return -1;
     InferPlan p;
-    make_infer_plan(d, true, false, &p);
+    make_streams_plan(d, kind, &p);
     return (int64_t)p.total;
 }
 
-extern "C" int delora_odometry_streams_init(const delora_odometry_desc* d, void* workspace, void* stream) {
-    const char* who = "delora_odometry_streams_init";
-    if (check_desc(d, who)) return 1;
+// The n cells of the cached grids at offsets pts / nrm start empty: the target of a stream that has not had a frame yet
+static int clear_grids(char* ws, size_t pts, size_t nrm, size_t n, cudaStream_t st) {
+    odometry_streams_grid_clear_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
+        reinterpret_cast<float4*>(ws + pts), reinterpret_cast<float4*>(ws + nrm), n);
+    DELORA_CHECK_LAUNCH("odometry_streams_grid_clear_kernel");
+    return 0;
+}
+
+// The residual and recipe kinds' ICP scratch is zeroed here, once, and their cached grids start empty
+static int streams_init(const delora_odometry_desc* d, Streams kind, void* workspace, cudaStream_t st, const char* who) {
+    if (check_streams_desc(d, kind, who)) return 1;
     DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
     InferPlan p;
-    make_infer_plan(d, true, false, &p);
-    return init_workspace(p.f, p.total, workspace, (cudaStream_t)stream, who);
+    make_streams_plan(d, kind, &p);
+    char* ws = (char*)workspace;
+    const int rc = init_workspace(p.f, p.total, workspace, st, who);
+    if (rc) return rc;
+    const size_t S = (size_t)d->max_batch;
+    if (kind == Streams::residual) return clear_grids(ws, p.prev_pts_grid, p.prev_nrm_grid, S * d->H * d->W, st);
+    if (kind == Streams::pre) {
+        const size_t n = S * d->H * d->w_pre;
+        const cudaError_t e = cudaMemsetAsync(ws + p.pre_keys, 0xFF, n * 8, st);
+        DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+        return clear_grids(ws, p.pre_pts, p.pre_nrm, n, st);
+    }
+    return 0;
+}
+
+// The caller's buffers of a streams tick, refused in this order; extra is the kind's own output named extra_name
+// (losses or factor), or nothing with extra_name NULL
+static int check_tick(const float* points, const int32_t* n_points, const void* workspace, const float* T,
+                      const int32_t* valid, const float* extra, const char* extra_name, const char* who) {
+    DELORA_CHECK_ARG(points, "%s: null points", who);
+    DELORA_CHECK_ARG(n_points, "%s: null n_points", who);
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    DELORA_CHECK_ARG(T, "%s: null T", who);
+    DELORA_CHECK_ARG(valid, "%s: null valid", who);
+    DELORA_CHECK_ARG(!extra_name || extra, "%s: null %s", who, extra_name);
+    return 0;
+}
+
+// The residual's settings: loss_flags may have the ICP losses and DELORA_NORMAL_LINEAR and, with scaling (the recipe
+// streams), DELORA_TRAIN_NORMALIZATION_SCALING
+static int check_residual_params(const delora_odometry_residual_params* rp, bool scaling, const char* who) {
+    DELORA_CHECK_ARG(rp, "%s: null residual_params", who);
+    if (check_icp_params(rp->lambda_po2pl, rp->loss_flags, rp->nb_h, rp->nb_w, rp->epsilon_range, rp->min_neighbors, who))
+        return 1;
+    const uint32_t bits = DELORA_LOSS_PO2PO | DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | DELORA_NORMAL_LINEAR |
+                          (scaling ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u);
+    DELORA_CHECK_ARG((rp->loss_flags & ~bits) == 0u, "%s: loss_flags=0x%x has a bit other than %s", who, rp->loss_flags,
+                     scaling ? "the ICP losses, DELORA_NORMAL_LINEAR and DELORA_TRAIN_NORMALIZATION_SCALING"
+                             : "the ICP losses and DELORA_NORMAL_LINEAR");
+    return 0;
+}
+
+// The model at B = S on the trunk input of t: the trunk into pooled, the tail's hidden layers and
+// odometry_streams_out_kernel<kRescale>, which reads io.raw (see the kernel for its other arguments)
+template <bool kRescale>
+static int streams_forward(const Model& m, const TailIO& io, const TrunkActs& t, const TrunkWeights& w, char* ws,
+                           int act, float* pooled, int S, const int32_t* active, int32_t* has_prev, float* T,
+                           int32_t* valid, const float* factor, float* factor_out, int32_t* counts, int32_t* n_valid,
+                           cudaStream_t st) {
+    int rc;
+    if ((rc = trunk_forward(m.t, t, ws, w, ws, act, S, pooled, nullptr, st))) return rc;
+    TailLinear rot, trans;
+    if ((rc = run_tail_hidden(m, io, act, pooled, S, &rot, &trans, st))) return rc;
+    odometry_streams_out_kernel<kRescale><<<1, kTailWarps * 32, (size_t)S * 7 * sizeof(float), st>>>(
+        rot, trans, S, tail_vec(rot) && tail_vec(trans), active, has_prev, T, valid, factor, factor_out, counts, io.raw,
+        n_valid);
+    DELORA_CHECK_LAUNCH(kRescale ? "odometry_streams_out_kernel<true>" : "odometry_streams_out_kernel");
+    return 0;
+}
+
+// The ICP at B = S on a residual or recipe plan's H x W grids: source pts_grid moved by T12, target prev_pts_grid,
+// into its losses and grad_T.  The recipe's DELORA_TRAIN_NORMALIZATION_SCALING is not an ICP bit.
+static int streams_icp(const delora_odometry_desc* d, const delora_odometry_residual_params* rp, const InferPlan& p,
+                       char* ws, cudaStream_t st) {
+    auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
+    auto f4 = [&](size_t o) { return reinterpret_cast<delora_f4*>(ws + o); };
+    return delora_icp_dense_fwd_bwd(f4(p.pts_grid), f4(p.nrm_grid), f(p.T12), f4(p.prev_pts_grid), f4(p.prev_nrm_grid),
+                                    d->max_batch, d->H, d->W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, rp->lambda_po2pl,
+                                    rp->loss_flags & ~DELORA_TRAIN_NORMALIZATION_SCALING, f(p.losses), f(p.grad_T),
+                                    f(p.icp), st);
+}
+
+// delora_odometry_streams_reset and _streams_adapt_reset, on the has_prev flags at that offset
+static int reset_streams(const delora_odometry_desc* d, const int32_t* mask, void* workspace, size_t has_prev,
+                         void* stream, const char* who) {
+    DELORA_CHECK_ARG(mask, "%s: null mask", who);
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    const int S = d->max_batch;
+    odometry_streams_reset_kernel<<<(S + 255) / 256, 256, 0, (cudaStream_t)stream>>>(
+        mask, S, reinterpret_cast<int32_t*>((char*)workspace + has_prev));
+    DELORA_CHECK_LAUNCH("odometry_streams_reset_kernel");
+    return 0;
+}
+
+}  // namespace delora
+
+extern "C" int64_t delora_odometry_streams_workspace_bytes(const delora_odometry_desc* d) {
+    return streams_workspace_bytes(d, Streams::plain, "delora_odometry_streams_workspace_bytes");
+}
+
+extern "C" int delora_odometry_streams_init(const delora_odometry_desc* d, void* workspace, void* stream) {
+    return streams_init(d, Streams::plain, workspace, (cudaStream_t)stream, "delora_odometry_streams_init");
 }
 
 extern "C" int delora_odometry_streams_load_weights(const delora_odometry_desc* d, const float* weights, void* workspace,
@@ -930,7 +1045,7 @@ extern "C" int delora_odometry_streams_load_weights(const delora_odometry_desc* 
     DELORA_CHECK_ARG(weights, "%s: null weights", who);
     DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
     InferPlan p;
-    make_infer_plan(d, true, false, &p);
+    make_streams_plan(d, Streams::plain, &p);
     return load_weights(p, weights, workspace, (cudaStream_t)stream, who);
 }
 
@@ -939,7 +1054,7 @@ static int run_streams_push(const delora_odometry_desc* d, const delora_odometry
                             const int32_t* n_points, const int32_t* active, void* workspace, float* T, int32_t* valid,
                             float* losses, cudaStream_t st) {
     InferPlan p;
-    make_infer_plan(d, true, rp != nullptr, &p);
+    make_streams_plan(d, rp ? Streams::residual : Streams::plain, &p);
     char* ws = (char*)workspace;
     const int S = d->max_batch, H = d->H, W = d->W;
     float* cur = reinterpret_cast<float*>(ws + p.f.images);
@@ -970,14 +1085,9 @@ static int run_streams_push(const delora_odometry_desc* d, const delora_odometry
         odometry_streams_input_kernel<64><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(cur, prev, active, S, H, W, x_in);
     }
     DELORA_CHECK_LAUNCH("odometry_streams_input_kernel");
-    float* pooled = reinterpret_cast<float*>(ws + p.pooled);
-    if ((rc = trunk_forward(p.m.t, p.t, ws, p.w, ws, d->act, S, pooled, nullptr, st))) return rc;
-    TailLinear rot, trans;
-    if ((rc = run_tail_hidden(p.m, inference_tail_io(p, ws), d->act, pooled, S, &rot, &trans, st))) return rc;
-    const int vec = tail_vec(rot) && tail_vec(trans);
-    odometry_streams_out_kernel<false><<<1, kTailWarps * 32, (size_t)S * 7 * sizeof(float), st>>>(
-        rot, trans, S, vec, active, has_prev, T, valid, nullptr, nullptr, nullptr);
-    DELORA_CHECK_LAUNCH("odometry_streams_out_kernel");
+    if ((rc = streams_forward<false>(p.m, inference_tail_io(p, ws), p.t, p.w, ws, d->act,
+                                     reinterpret_cast<float*>(ws + p.pooled), S, active, has_prev, T, valid, nullptr,
+                                     nullptr, nullptr, nullptr, st))) return rc;
     if (!rp) return 0;
     // the residual: this frame moved by T against the stream's previous frame (the training step's orientation,
     // scan_2 -> scan_1), for all S streams in one ICP call whose sources are empty where there is no T
@@ -991,11 +1101,7 @@ static int run_streams_push(const delora_odometry_desc* d, const delora_odometry
     odometry_streams_grids_kernel<0><<<blocks, 256, 0, st>>>(pts_grid, nrm_grid, prev_pts, prev_nrm, active, valid, S, HW,
                                                              T, T12, icp_losses, losses);
     DELORA_CHECK_LAUNCH("odometry_streams_grids_kernel<0>");
-    if ((rc = delora_icp_dense_fwd_bwd(reinterpret_cast<delora_f4*>(pts_grid), reinterpret_cast<delora_f4*>(nrm_grid), T12,
-                                       reinterpret_cast<delora_f4*>(prev_pts), reinterpret_cast<delora_f4*>(prev_nrm), S,
-                                       H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, rp->lambda_po2pl, rp->loss_flags,
-                                       icp_losses, reinterpret_cast<float*>(ws + p.grad_T),
-                                       reinterpret_cast<float*>(ws + p.icp), st))) return rc;
+    if ((rc = streams_icp(d, rp, p, ws, st))) return rc;
     odometry_streams_grids_kernel<1><<<blocks, 256, 0, st>>>(pts_grid, nrm_grid, prev_pts, prev_nrm, active, valid, S, HW,
                                                              T, T12, icp_losses, losses);
     DELORA_CHECK_LAUNCH("odometry_streams_grids_kernel<1>");
@@ -1007,36 +1113,16 @@ extern "C" int delora_odometry_streams_push(const delora_odometry_desc* d, const
                                             void* stream) {
     const char* who = "delora_odometry_streams_push";
     if (check_desc(d, who)) return 1;
-    DELORA_CHECK_ARG(points, "%s: null points", who);
-    DELORA_CHECK_ARG(n_points, "%s: null n_points", who);
-    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
-    DELORA_CHECK_ARG(T, "%s: null T", who);
-    DELORA_CHECK_ARG(valid, "%s: null valid", who);
+    if (check_tick(points, n_points, workspace, T, valid, nullptr, nullptr, who)) return 1;
     return run_streams_push(d, nullptr, points, n_points, active, workspace, T, valid, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int64_t delora_odometry_streams_residual_workspace_bytes(const delora_odometry_desc* d) {
-    if (check_desc(d, "delora_odometry_streams_residual_workspace_bytes")) return -1;
-    InferPlan p;
-    make_infer_plan(d, true, true, &p);
-    return (int64_t)p.total;
+    return streams_workspace_bytes(d, Streams::residual, "delora_odometry_streams_residual_workspace_bytes");
 }
 
 extern "C" int delora_odometry_streams_residual_init(const delora_odometry_desc* d, void* workspace, void* stream) {
-    const char* who = "delora_odometry_streams_residual_init";
-    if (check_desc(d, who)) return 1;
-    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
-    InferPlan p;
-    make_infer_plan(d, true, true, &p);
-    cudaStream_t st = (cudaStream_t)stream;
-    const int rc = init_workspace(p.f, p.total, workspace, st, who);    // the ICP scratch is zeroed here, once
-    if (rc) return rc;
-    const size_t n = (size_t)d->max_batch * d->H * d->W;
-    odometry_streams_grid_clear_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
-        reinterpret_cast<float4*>((char*)workspace + p.prev_pts_grid),
-        reinterpret_cast<float4*>((char*)workspace + p.prev_nrm_grid), n);
-    DELORA_CHECK_LAUNCH("odometry_streams_grid_clear_kernel");
-    return 0;
+    return streams_init(d, Streams::residual, workspace, (cudaStream_t)stream, "delora_odometry_streams_residual_init");
 }
 
 extern "C" int delora_odometry_streams_push_residual(const delora_odometry_desc* d,
@@ -1045,36 +1131,18 @@ extern "C" int delora_odometry_streams_push_residual(const delora_odometry_desc*
                                                      float* T, int32_t* valid, float* losses, void* stream) {
     const char* who = "delora_odometry_streams_push_residual";
     if (check_desc(d, who)) return 1;
-    DELORA_CHECK_ARG(rp, "%s: null residual_params", who);
-    if (check_icp_params(rp->lambda_po2pl, rp->loss_flags, rp->nb_h, rp->nb_w, rp->epsilon_range, rp->min_neighbors, who))
-        return 1;
-    const uint32_t icp_bits = DELORA_LOSS_PO2PO | DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | DELORA_NORMAL_LINEAR;
-    DELORA_CHECK_ARG((rp->loss_flags & ~icp_bits) == 0u,
-                     "%s: loss_flags=0x%x has a bit other than the ICP losses and DELORA_NORMAL_LINEAR", who,
-                     rp->loss_flags);
-    DELORA_CHECK_ARG(points, "%s: null points", who);
-    DELORA_CHECK_ARG(n_points, "%s: null n_points", who);
-    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
-    DELORA_CHECK_ARG(T, "%s: null T", who);
-    DELORA_CHECK_ARG(valid, "%s: null valid", who);
-    DELORA_CHECK_ARG(losses, "%s: null losses", who);
+    if (check_residual_params(rp, false, who)) return 1;
+    if (check_tick(points, n_points, workspace, T, valid, losses, "losses", who)) return 1;
     return run_streams_push(d, rp, points, n_points, active, workspace, T, valid, losses, (cudaStream_t)stream);
 }
 
 extern "C" int64_t delora_odometry_streams_normalized_workspace_bytes(const delora_odometry_desc* d) {
-    if (check_desc(d, "delora_odometry_streams_normalized_workspace_bytes")) return -1;
-    InferPlan p;
-    make_normalized_streams_plan(d, &p);
-    return (int64_t)p.total;
+    return streams_workspace_bytes(d, Streams::normalized, "delora_odometry_streams_normalized_workspace_bytes");
 }
 
 extern "C" int delora_odometry_streams_normalized_init(const delora_odometry_desc* d, void* workspace, void* stream) {
-    const char* who = "delora_odometry_streams_normalized_init";
-    if (check_desc(d, who)) return 1;
-    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
-    InferPlan p;
-    make_normalized_streams_plan(d, &p);
-    return init_workspace(p.f, p.total, workspace, (cudaStream_t)stream, who);
+    return streams_init(d, Streams::normalized, workspace, (cudaStream_t)stream,
+                        "delora_odometry_streams_normalized_init");
 }
 
 // One tick of a normalised model: the staging of the point rows, the factor of the S pairs (side 0 = rows 0..S-1, the
@@ -1082,11 +1150,15 @@ extern "C" int delora_odometry_streams_normalized_init(const delora_odometry_des
 // prev_image, this tick's into images; each resolve re-arms the shared keys), the pairs' trunk-input conversion, the
 // trunk and the tail at B = S, and the rescaling output kernel.  A stream without a pair this tick has a row-s count of
 // 0, so its factor is 0 / 0 = NaN and its scaled coordinates project to no pixel; its outputs are not written.
-static int run_streams_push_normalized(const delora_odometry_desc* d, const float* points, const int32_t* n_points,
-                                       const int32_t* active, void* workspace, float* T, int32_t* valid,
-                                       float* factor_out, cudaStream_t st) {
+extern "C" int delora_odometry_streams_push_normalized(const delora_odometry_desc* d, const float* points,
+                                                       const int32_t* n_points, const int32_t* active, void* workspace,
+                                                       float* T, int32_t* valid, float* factor_out, void* stream) {
+    const char* who = "delora_odometry_streams_push_normalized";
+    if (check_desc(d, who)) return 1;
+    if (check_tick(points, n_points, workspace, T, valid, factor_out, "factor", who)) return 1;
+    cudaStream_t st = (cudaStream_t)stream;
     InferPlan p;
-    make_normalized_streams_plan(d, &p);
+    make_streams_plan(d, Streams::normalized, &p);
     char* ws = (char*)workspace;
     const int S = d->max_batch, ns = d->n_stride;
     float* stage = reinterpret_cast<float*>(ws + p.stage);
@@ -1107,64 +1179,17 @@ static int run_streams_push_normalized(const delora_odometry_desc* d, const floa
     if ((rc = project_fwd(stage + (size_t)S * 3 * ns, counts + S, S, 3, ns, g, keys, cur, index_map, factor, S, st)))
         return rc;
     if ((rc = trunk_input(p.m.t, p.t, ws, prev, cur, S, st))) return rc;
-    float* pooled = reinterpret_cast<float*>(ws + p.pooled);
-    if ((rc = trunk_forward(p.m.t, p.t, ws, p.w, ws, d->act, S, pooled, nullptr, st))) return rc;
-    TailLinear rot, trans;
-    if ((rc = run_tail_hidden(p.m, inference_tail_io(p, ws), d->act, pooled, S, &rot, &trans, st))) return rc;
-    const int vec = tail_vec(rot) && tail_vec(trans);
-    odometry_streams_out_kernel<true><<<1, kTailWarps * 32, (size_t)S * 7 * sizeof(float), st>>>(
-        rot, trans, S, vec, active, has_prev, T, valid, factor, factor_out, counts);
-    DELORA_CHECK_LAUNCH("odometry_streams_out_kernel<true>");
-    return 0;
-}
-
-extern "C" int delora_odometry_streams_push_normalized(const delora_odometry_desc* d, const float* points,
-                                                       const int32_t* n_points, const int32_t* active, void* workspace,
-                                                       float* T, int32_t* valid, float* factor, void* stream) {
-    const char* who = "delora_odometry_streams_push_normalized";
-    if (check_desc(d, who)) return 1;
-    DELORA_CHECK_ARG(points, "%s: null points", who);
-    DELORA_CHECK_ARG(n_points, "%s: null n_points", who);
-    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
-    DELORA_CHECK_ARG(T, "%s: null T", who);
-    DELORA_CHECK_ARG(valid, "%s: null valid", who);
-    DELORA_CHECK_ARG(factor, "%s: null factor", who);
-    return run_streams_push_normalized(d, points, n_points, active, workspace, T, valid, factor, (cudaStream_t)stream);
-}
-
-// check_desc plus the preprocessing width the recipe streams read (the training rule, but w_pre = 0 is refused)
-static int check_pre_desc(const delora_odometry_desc* d, const char* who) {
-    if (check_desc(d, who)) return 1;
-    DELORA_CHECK_ARG(d->w_pre >= 2 && (long long)d->H * d->w_pre < (1ll << 27),
-                     "%s: w_pre=%d must be >= 2 with H * w_pre < 2^27 (H=%d): the recipe streams estimate the normals "
-                     "at H x w_pre", who, d->w_pre, d->H);
-    return 0;
+    return streams_forward<true>(p.m, inference_tail_io(p, ws), p.t, p.w, ws, d->act,
+                                 reinterpret_cast<float*>(ws + p.pooled), S, active, has_prev, T, valid, factor,
+                                 factor_out, counts, nullptr, st);
 }
 
 extern "C" int64_t delora_odometry_streams_pre_workspace_bytes(const delora_odometry_desc* d) {
-    if (check_pre_desc(d, "delora_odometry_streams_pre_workspace_bytes")) return -1;
-    InferPlan p;
-    make_pre_streams_plan(d, &p);
-    return (int64_t)p.total;
+    return streams_workspace_bytes(d, Streams::pre, "delora_odometry_streams_pre_workspace_bytes");
 }
 
 extern "C" int delora_odometry_streams_pre_init(const delora_odometry_desc* d, void* workspace, void* stream) {
-    const char* who = "delora_odometry_streams_pre_init";
-    if (check_pre_desc(d, who)) return 1;
-    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
-    InferPlan p;
-    make_pre_streams_plan(d, &p);
-    cudaStream_t st = (cudaStream_t)stream;
-    char* ws = (char*)workspace;
-    const int rc = init_workspace(p.f, p.total, workspace, st, who);     // the ICP scratch is zeroed here, once
-    if (rc) return rc;
-    const size_t n = (size_t)d->max_batch * d->H * d->w_pre;
-    const cudaError_t e = cudaMemsetAsync(ws + p.pre_keys, 0xFF, n * 8, st);
-    DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
-    odometry_streams_grid_clear_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
-        reinterpret_cast<float4*>(ws + p.pre_pts), reinterpret_cast<float4*>(ws + p.pre_nrm), n);
-    DELORA_CHECK_LAUNCH("odometry_streams_grid_clear_kernel");
-    return 0;
+    return streams_init(d, Streams::pre, workspace, (cudaStream_t)stream, "delora_odometry_streams_pre_init");
 }
 
 // One tick of the recipe (the training step's stages 1-3 at B = S, each pair's first frame from the cache): the masked
@@ -1172,11 +1197,22 @@ extern "C" int delora_odometry_streams_pre_init(const delora_odometry_desc* d, v
 // (flagged models; cached frames are side 0, new ones side 1), both frames of every pair projected to H x W (scaled by
 // the pair's factor when flagged), the trunk input, trunk and tail at B = S, the output kernel into T16, the
 // bookkeeping kernel (T, T12, factor, emptied sources, cache write), the ICP at B = S and the masked loss rows.
-static int run_streams_push_pre(const delora_odometry_desc* d, const delora_odometry_residual_params* rp,
-                                const float* points, const int32_t* n_points, const int32_t* active, void* workspace,
-                                float* T, int32_t* valid, float* losses, float* factor_out, cudaStream_t st) {
+extern "C" int delora_odometry_streams_push_pre(const delora_odometry_desc* d, const delora_odometry_residual_params* rp,
+                                                const float* points, const int32_t* n_points, const int32_t* active,
+                                                void* workspace, float* T, int32_t* valid, float* losses,
+                                                float* factor_out, void* stream) {
+    const char* who = "delora_odometry_streams_push_pre";
+    if (check_pre_desc(d, who)) return 1;
+    if (check_residual_params(rp, true, who)) return 1;
+    if (check_tick(points, n_points, workspace, T, valid, losses, "losses", who)) return 1;
+    const bool normalized = (rp->loss_flags & DELORA_TRAIN_NORMALIZATION_SCALING) != 0u;
+    DELORA_CHECK_ARG(!normalized || factor_out, "%s: null factor with DELORA_TRAIN_NORMALIZATION_SCALING in loss_flags",
+                     who);
+    DELORA_CHECK_ARG(normalized || !factor_out, "%s: factor must be NULL without DELORA_TRAIN_NORMALIZATION_SCALING in "
+                     "loss_flags", who);
+    cudaStream_t st = (cudaStream_t)stream;
     InferPlan p;
-    make_pre_streams_plan(d, &p);
+    make_streams_plan(d, Streams::pre, &p);
     char* ws = (char*)workspace;
     const int S = d->max_batch, H = d->H, W = d->W, Wp = d->w_pre, HW = H * W, HWp = H * Wp;
     auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
@@ -1204,15 +1240,9 @@ static int run_streams_push_pre(const delora_odometry_desc* d, const delora_odom
     if ((rc = project_grids_fwd(pre_cur_pts, pre_cur_nrm, S, Wp, g, keys, cur, nullptr, f4(p.pts_grid), f4(p.nrm_grid),
                                 factor, S, st))) return rc;
     if ((rc = trunk_input(p.m.t, p.t, ws, prev, cur, S, st))) return rc;
-    float* pooled = f(p.pooled);
-    if ((rc = trunk_forward(p.m.t, p.t, ws, p.w, ws, d->act, S, pooled, nullptr, st))) return rc;
-    TailLinear rot, trans;
-    if ((rc = run_tail_hidden(p.m, inference_tail_io(p, ws), d->act, pooled, S, &rot, &trans, st))) return rc;
-    const int vec = tail_vec(rot) && tail_vec(trans);
     int32_t* has_prev = reinterpret_cast<int32_t*>(ws + p.f.has_prev);
-    odometry_streams_out_kernel<false><<<1, kTailWarps * 32, (size_t)S * 7 * sizeof(float), st>>>(
-        rot, trans, S, vec, active, has_prev, f(p.T16), valid, nullptr, nullptr, nullptr);
-    DELORA_CHECK_LAUNCH("odometry_streams_out_kernel");
+    if ((rc = streams_forward<false>(p.m, inference_tail_io(p, ws), p.t, p.w, ws, d->act, f(p.pooled), S, active,
+                                     has_prev, f(p.T16), valid, nullptr, nullptr, nullptr, nullptr, st))) return rc;
     int per_stream = HWp > HW ? HWp : HW;
     if (per_stream < 16) per_stream = 16;
     const size_t cells = (size_t)S * per_stream;
@@ -1222,56 +1252,19 @@ static int run_streams_push_pre(const delora_odometry_desc* d, const delora_odom
         reinterpret_cast<const float4*>(pre_cur_nrm), reinterpret_cast<float4*>(pre_prev_pts),
         reinterpret_cast<float4*>(pre_prev_nrm));
     DELORA_CHECK_LAUNCH("odometry_streams_pre_kernel");
-    if ((rc = delora_icp_dense_fwd_bwd(f4(p.pts_grid), f4(p.nrm_grid), f(p.T12), f4(p.prev_pts_grid), f4(p.prev_nrm_grid),
-                                       S, H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, rp->lambda_po2pl,
-                                       rp->loss_flags & ~DELORA_TRAIN_NORMALIZATION_SCALING, f(p.losses), f(p.grad_T),
-                                       f(p.icp), st))) return rc;
+    if ((rc = streams_icp(d, rp, p, ws, st))) return rc;
     odometry_streams_losses_kernel<<<(S * DELORA_LOSS_ROW + 255) / 256, 256, 0, st>>>(valid, S, f(p.losses), losses);
     DELORA_CHECK_LAUNCH("odometry_streams_losses_kernel");
     return 0;
-}
-
-extern "C" int delora_odometry_streams_push_pre(const delora_odometry_desc* d, const delora_odometry_residual_params* rp,
-                                                const float* points, const int32_t* n_points, const int32_t* active,
-                                                void* workspace, float* T, int32_t* valid, float* losses, float* factor,
-                                                void* stream) {
-    const char* who = "delora_odometry_streams_push_pre";
-    if (check_pre_desc(d, who)) return 1;
-    DELORA_CHECK_ARG(rp, "%s: null residual_params", who);
-    if (check_icp_params(rp->lambda_po2pl, rp->loss_flags, rp->nb_h, rp->nb_w, rp->epsilon_range, rp->min_neighbors, who))
-        return 1;
-    const uint32_t bits = DELORA_LOSS_PO2PO | DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | DELORA_NORMAL_LINEAR |
-                          DELORA_TRAIN_NORMALIZATION_SCALING;
-    DELORA_CHECK_ARG((rp->loss_flags & ~bits) == 0u,
-                     "%s: loss_flags=0x%x has a bit other than the ICP losses, DELORA_NORMAL_LINEAR and "
-                     "DELORA_TRAIN_NORMALIZATION_SCALING", who, rp->loss_flags);
-    DELORA_CHECK_ARG(points, "%s: null points", who);
-    DELORA_CHECK_ARG(n_points, "%s: null n_points", who);
-    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
-    DELORA_CHECK_ARG(T, "%s: null T", who);
-    DELORA_CHECK_ARG(valid, "%s: null valid", who);
-    DELORA_CHECK_ARG(losses, "%s: null losses", who);
-    const bool normalized = (rp->loss_flags & DELORA_TRAIN_NORMALIZATION_SCALING) != 0u;
-    DELORA_CHECK_ARG(!normalized || factor, "%s: null factor with DELORA_TRAIN_NORMALIZATION_SCALING in loss_flags", who);
-    DELORA_CHECK_ARG(normalized || !factor, "%s: factor must be NULL without DELORA_TRAIN_NORMALIZATION_SCALING in "
-                     "loss_flags", who);
-    return run_streams_push_pre(d, rp, points, n_points, active, workspace, T, valid, losses, factor,
-                                (cudaStream_t)stream);
 }
 
 extern "C" int delora_odometry_streams_reset(const delora_odometry_desc* d, const int32_t* mask, void* workspace,
                                              void* stream) {
     const char* who = "delora_odometry_streams_reset";
     if (check_desc(d, who)) return 1;
-    DELORA_CHECK_ARG(mask, "%s: null mask", who);
-    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
     InferPlan p;
-    make_infer_plan(d, true, false, &p);
-    const int S = d->max_batch;
-    odometry_streams_reset_kernel<<<(S + 255) / 256, 256, 0, (cudaStream_t)stream>>>(
-        mask, S, reinterpret_cast<int32_t*>((char*)workspace + p.f.has_prev));
-    DELORA_CHECK_LAUNCH("odometry_streams_reset_kernel");
-    return 0;
+    make_streams_plan(d, Streams::plain, &p);
+    return reset_streams(d, mask, workspace, p.f.has_prev, stream, who);
 }
 
 // ================================================================================================ training
@@ -1954,15 +1947,10 @@ static int train_forward_losses(const delora_odometry_desc* d, const delora_odom
     }
     // 2. forward, keeping the activations
     if ((rc = trunk_input(m.t, tp.t, ws, images, images + (size_t)B * 4 * HW, B, st, drop_fwd))) return rc;
-    if ((rc = trunk_forward(m.t, tp.t, ws, tp.w, ws, d->act, B, f(tp.pooled), nullptr, st, drop_fwd))) return rc;
-    if (at) {
-        const TailIO io = train_tail_io(tp, ws);
-        TailLinear rot, trans;
-        if ((rc = run_tail_hidden(m, io, d->act, f(tp.pooled), B, &rot, &trans, st))) return rc;
-        odometry_streams_out_kernel<false><<<1, kTailWarps * 32, (size_t)B * 7 * sizeof(float), st>>>(
-            rot, trans, B, tail_vec(rot) && tail_vec(trans), at->active, at->has_prev, f(tp.T16), at->valid, nullptr,
-            nullptr, nullptr, io.raw, at->n_valid);
-        DELORA_CHECK_LAUNCH("odometry_streams_out_kernel");
+    if (at) {               // dropout is off: the served T is dropout-free
+        if ((rc = streams_forward<false>(m, train_tail_io(tp, ws), tp.t, tp.w, ws, d->act, f(tp.pooled), B, at->active,
+                                         at->has_prev, f(tp.T16), at->valid, nullptr, nullptr, nullptr, at->n_valid,
+                                         st))) return rc;
         // T (normalised: the factor of the H x w_pre grids, kept in pre_image as below), T12, the cache, the sources
         size_t cells = HWc > (size_t)HW ? HWc : (size_t)HW;
         if (cells < 16) cells = 16;
@@ -1980,6 +1968,7 @@ static int train_forward_losses(const delora_odometry_desc* d, const delora_odom
             reinterpret_cast<float4*>(at->cache_image));
         DELORA_CHECK_LAUNCH("odometry_streams_pre_kernel");
     } else {
+        if ((rc = trunk_forward(m.t, tp.t, ws, tp.w, ws, d->act, B, f(tp.pooled), nullptr, st, drop_fwd))) return rc;
         if ((rc = run_tail(m, train_tail_io(tp, ws), d->act, f(tp.pooled), B, f(tp.T16), st, nullptr, drop_fwd)))
             return rc;
         const cudaError_t e = cudaMemcpy2DAsync(f(tp.T12), 12 * sizeof(float), f(tp.T16), 16 * sizeof(float),
@@ -2100,25 +2089,52 @@ static int adam_update(const TrainPlan& tp, char* ws, const delora_odometry_trai
     return delora_conv_weight_prep_multi(ws + tp.w.table, tp.m.t.n_conv, st);
 }
 
-// Bucket k of plan_buckets' schedule is complete on `st`: g->side_stream waits for it through fork_events[k] and
-// all-reduces it in place in every rank's gradient section, times `scale`, seq = *seq_step * seq_stride + seq_add.
-static int bucket_all_reduce(const TrainPlan& tp, const delora_odometry_train_group* g, const long long* b_off,
-                             const long long* b_cnt, int k, float scale, const long long* seq_step, unsigned seq_stride,
-                             unsigned seq_add, cudaStream_t st, const char* who) {
-    uint64_t peer_grad[kArMaxWorld];
-    for (int q = 0; q < g->world; ++q) peer_grad[q] = g->peer_ws[q] + tp.grad;
-    cudaStream_t side = (cudaStream_t)g->side_stream;
-    cudaError_t e = cudaEventRecord((cudaEvent_t)g->fork_events[k], st);
-    if (e == cudaSuccess) e = cudaStreamWaitEvent(side, (cudaEvent_t)g->fork_events[k], 0);
-    DELORA_CHECK_ARG(e == cudaSuccess, "%s: fork_events[%d]: %s", who, k, cudaGetErrorString(e));
-    return grad_allreduce_launch(peer_grad, g->peer_flags, g->multicast ? g->multicast + tp.grad : 0ull, g->rank,
-                                 g->world, b_off[k], b_cnt[k], scale, seq_add, seq_step, seq_stride, g->n_ctas,
-                                 g->n_threads, g->status, side);
-}
+// How the group form of a step all-reduces its gradient: bucket k times scale, seq = *seq_step * seq_stride +
+// seq_first + k
+struct GroupReduce {
+    const delora_odometry_train_group* g;
+    float scale;
+    const long long* seq_step;
+    unsigned seq_stride, seq_first;
+};
 
-// `st` waits for every bucket all-reduced on g->side_stream
-static int group_join(const delora_odometry_train_group* g, cudaStream_t st, const char* who) {
-    cudaError_t e = cudaEventRecord((cudaEvent_t)g->join_event, (cudaStream_t)g->side_stream);
+// Stage 4 of the step at B pairs: the tail backward (see train_tail_backward for identity, drop, valid and n_valid),
+// then the trunk backward of stage 3 down to 0.  With gr, bucket k of plan_buckets' schedule is all-reduced in place in
+// every rank's gradient section as soon as the backward has produced it on `st` (bucket 0 after the tail, bucket 4 - s
+// after stage s): g->side_stream waits for it through fork_events[k] and runs the all-reduce, and `st` then waits for
+// every bucket through join_event.
+static int step_backward(const TrainPlan& tp, char* ws, int act, int B, bool identity, DropoutCtr drop,
+                         const int32_t* valid, const int32_t* n_valid, const GroupReduce* gr, cudaStream_t st,
+                         const char* who) {
+    const delora_odometry_train_group* g = gr ? gr->g : nullptr;
+    cudaStream_t side = g ? (cudaStream_t)g->side_stream : nullptr;
+    long long b_off[kGroupBuckets], b_cnt[kGroupBuckets];
+    uint64_t peer_grad[kArMaxWorld];
+    if (g) {
+        plan_buckets(tp.m, b_off, b_cnt);
+        for (int q = 0; q < g->world; ++q) peer_grad[q] = g->peer_ws[q] + tp.grad;
+    }
+    auto all_reduce = [&](int k) -> int {
+        if (!g) return 0;
+        cudaError_t e = cudaEventRecord((cudaEvent_t)g->fork_events[k], st);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(side, (cudaEvent_t)g->fork_events[k], 0);
+        DELORA_CHECK_ARG(e == cudaSuccess, "%s: fork_events[%d]: %s", who, k, cudaGetErrorString(e));
+        return grad_allreduce_launch(peer_grad, g->peer_flags, g->multicast ? g->multicast + tp.grad : 0ull, g->rank,
+                                     g->world, b_off[k], b_cnt[k], gr->scale, gr->seq_first + (unsigned)k, gr->seq_step,
+                                     gr->seq_stride, g->n_ctas, g->n_threads, g->status, side);
+    };
+    int rc;
+    if ((rc = train_tail_backward(tp, ws, act, B, identity, st, drop, valid, n_valid))) return rc;
+    if ((rc = all_reduce(0))) return rc;
+    float* conv_dw[kMaxConv];
+    for (int i = 0; i < tp.m.t.n_conv; ++i) conv_dw[i] = reinterpret_cast<float*>(ws + tp.grad) + tp.m.t.conv[i].blob;
+    const float* g_pooled = reinterpret_cast<const float*>(ws + tp.g_pooled);
+    for (int s = 3; s >= 0; --s) {
+        if ((rc = trunk_backward(tp.m.t, tp.t, ws, tp.w, ws, act, B, g_pooled, conv_dw, s, st, drop))) return rc;
+        if ((rc = all_reduce(4 - s))) return rc;
+    }
+    if (!g) return 0;
+    cudaError_t e = cudaEventRecord((cudaEvent_t)g->join_event, side);
     if (e == cudaSuccess) e = cudaStreamWaitEvent(st, (cudaEvent_t)g->join_event, 0);
     DELORA_CHECK_ARG(e == cudaSuccess, "%s: join_event: %s", who, cudaGetErrorString(e));
     return 0;
@@ -2135,38 +2151,24 @@ static int train_step(const delora_odometry_desc* d, const delora_odometry_train
     const bool identity = (hp->loss_flags & DELORA_LOSS_IDENTITY_FIT) != 0u;
     TrainPlan tp;
     make_train_plan(d, &tp);
-    const Model& m = tp.m;
     cudaStream_t st = (cudaStream_t)stream;
     char* ws = (char*)workspace;
-    auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
     long long* ctr = reinterpret_cast<long long*>(ws + tp.ctr);
     // the masks of this step, regenerated after odometry_out_bwd_kernel has advanced the step count
     const DropoutCtr drop_bwd{dropout ? ctr : nullptr, 1};
-    long long b_off[kGroupBuckets], b_cnt[kGroupBuckets];
-    if (g) plan_buckets(m, b_off, b_cnt);
-    // bucket k is complete on `st`: all-reduce it on the side stream; seq = the step count (advanced by
-    // odometry_out_bwd_kernel before bucket 0) * kGroupBuckets + k
-    auto all_reduce = [&](int k) -> int {
-        return bucket_all_reduce(tp, g, b_off, b_cnt, k, 1.0f / (float)g->world, ctr, (unsigned)kGroupBuckets,
-                                 (unsigned)k, st, who);
-    };
+    // the buckets are averaged; seq = the step count (advanced by odometry_out_bwd_kernel before bucket 0) *
+    // kGroupBuckets + k
+    const GroupReduce gr{g, g ? 1.0f / (float)g->world : 1.0f, ctr, (unsigned)kGroupBuckets, 0u};
     int rc;
     // 1-3. projection + normals, forward, ICP losses and dL/dT
     if ((rc = train_forward_losses(d, hp, tp, ws, points, n_points, B, dropout, T, st, who))) return rc;
     // 4. backward: tail (dL/dT of the ICP mean or of the identity fit), average pool, trunk
-    if ((rc = train_tail_backward(tp, ws, d->act, B, identity, st, drop_bwd))) return rc;
-    if (g && (rc = all_reduce(0))) return rc;
-    float* conv_dw[kMaxConv];
-    for (int i = 0; i < m.t.n_conv; ++i) conv_dw[i] = f(tp.grad) + m.t.conv[i].blob;
-    for (int s = 3; s >= 0; --s) {
-        if ((rc = trunk_backward(m.t, tp.t, ws, tp.w, ws, d->act, B, f(tp.g_pooled), conv_dw, s, st, drop_bwd))) return rc;
-        if (g && (rc = all_reduce(4 - s))) return rc;
-    }
-    if (g && (rc = group_join(g, st, who))) return rc;
+    if ((rc = step_backward(tp, ws, d->act, B, identity, drop_bwd, nullptr, nullptr, g ? &gr : nullptr, st, who)))
+        return rc;
     // outputs (T: the weights before the update)
     if ((rc = train_outputs(tp, ws, B, normalized, losses, T, pooled, st, who))) return rc;
     if (grads) {
-        const cudaError_t e = cudaMemcpyAsync(grads, ws + tp.grad, (size_t)m.blob_floats * sizeof(float),
+        const cudaError_t e = cudaMemcpyAsync(grads, ws + tp.grad, (size_t)tp.m.blob_floats * sizeof(float),
                                               cudaMemcpyDeviceToDevice, st);
         DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
     }
@@ -2307,6 +2309,11 @@ struct AdaptPlan {
     size_t has_prev, n_valid;          // [S], [1]
     size_t cache_cells;                // cells of one stream's cached grid
     size_t total;
+    // The group section of delora_odometry_streams_push_adapt_group, one 256-byte block after the adapting-streams
+    // layout: the tick counter (int64: group ticks with update = 1 so far), the fleet-wide count of valid pairs of the
+    // last such tick (int32) and the count exchange's slots (int32 [2][kArMaxWorld], see count_allreduce_kernel).
+    size_t tick, n_fleet, slots;
+    size_t group_total;
 };
 
 static void make_adapt_plan(const delora_odometry_desc* d, TrainPlan* tp, AdaptPlan* ap) {
@@ -2321,42 +2328,35 @@ static void make_adapt_plan(const delora_odometry_desc* d, TrainPlan* tp, AdaptP
     ap->has_prev = take(off, S * 4);
     ap->n_valid = take(off, 4);
     ap->total = off;
-}
-
-// The group section of delora_odometry_streams_push_adapt_group, one 256-byte block after the adapting-streams layout:
-// the tick counter (int64: group ticks with update = 1 so far), the fleet-wide count of valid pairs of the last such
-// tick (int32) and the count exchange's slots (int32 [2][kArMaxWorld], see count_allreduce_kernel).
-struct AdaptGroupPlan {
-    size_t tick, n_fleet, slots;
-    size_t total;
-};
-
-static void make_adapt_group_plan(const delora_odometry_desc* d, TrainPlan* tp, AdaptPlan* ap, AdaptGroupPlan* gp) {
-    make_adapt_plan(d, tp, ap);
-    size_t off = ap->total;
     const size_t base = take(off, 8 + 8 + 2 * kArMaxWorld * 4);
-    gp->tick = base;
-    gp->n_fleet = base + 8;
-    gp->slots = base + 16;
-    gp->total = off;
+    ap->tick = base;
+    ap->n_fleet = base + 8;
+    ap->slots = base + 16;
+    ap->group_total = off;
 }
 
-// _streams_adapt_init on a workspace of `total` bytes (>= d's adapting-streams size); everything past the stream
-// section is zeroed too
-static int adapt_init(const delora_odometry_desc* d, size_t total, const float* weights, void* workspace,
-                      cudaStream_t st, const char* who) {
+// The adapting-streams workspace's size and, with group, its group form's
+static int64_t adapt_workspace_bytes(const delora_odometry_desc* d, bool group, const char* who) {
+    if (check_train_desc(d, who)) return -1;
+    TrainPlan tp;
+    AdaptPlan ap;
+    make_adapt_plan(d, &tp, &ap);
+    return (int64_t)(group ? ap.group_total : ap.total);
+}
+
+// _streams_adapt_init and, with group, _streams_adapt_group_init; the group section is zeroed too
+static int adapt_init(const delora_odometry_desc* d, bool group, const float* weights, void* workspace, cudaStream_t st,
+                      const char* who) {
+    if (check_train_desc(d, who)) return 1;
     TrainPlan tp;
     AdaptPlan ap;
     make_adapt_plan(d, &tp, &ap);
     // _train_init over the whole workspace zeroes the stream section too; the cached grids then start empty
-    const int rc = train_init(d, total, weights, workspace, st, who);
+    int rc = train_init(d, group ? ap.group_total : ap.total, weights, workspace, st, who);
     if (rc) return rc;
-    const size_t n = (size_t)d->max_batch * ap.cache_cells;
-    odometry_streams_grid_clear_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
-        reinterpret_cast<float4*>((char*)workspace + ap.cache_pts), reinterpret_cast<float4*>((char*)workspace + ap.cache_nrm),
-        n);
-    DELORA_CHECK_LAUNCH("odometry_streams_grid_clear_kernel");
-    return 0;
+    if ((rc = clear_grids((char*)workspace, ap.cache_pts, ap.cache_nrm, (size_t)d->max_batch * ap.cache_cells, st)))
+        return rc;
+    return group ? collective_kernels_preload(who) : 0;
 }
 
 // What _push_adapt and _push_adapt_group refuse alike
@@ -2372,12 +2372,7 @@ static int check_push_adapt(const delora_odometry_desc* d, const delora_odometry
     DELORA_CHECK_ARG((hp->loss_flags & DELORA_TRAIN_DROPOUT) == 0u,
                      "%s: loss_flags=0x%x has DELORA_TRAIN_DROPOUT: the served T is dropout-free, and one forward "
                      "cannot be both", who, hp->loss_flags);
-    DELORA_CHECK_ARG(points, "%s: null points", who);
-    DELORA_CHECK_ARG(n_points, "%s: null n_points", who);
-    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
-    DELORA_CHECK_ARG(T, "%s: null T", who);
-    DELORA_CHECK_ARG(valid, "%s: null valid", who);
-    DELORA_CHECK_ARG(losses, "%s: null losses", who);
+    if (check_tick(points, n_points, workspace, T, valid, losses, "losses", who)) return 1;
     return check_train_call(d, hp, points, n_points, d->max_batch, workspace, who);
 }
 
@@ -2393,8 +2388,7 @@ static int push_adapt(const delora_odometry_desc* d, const delora_odometry_train
     const int S = d->max_batch;
     TrainPlan tp;
     AdaptPlan ap;
-    AdaptGroupPlan gp;
-    make_adapt_group_plan(d, &tp, &ap, &gp);
+    make_adapt_plan(d, &tp, &ap);
     cudaStream_t st = (cudaStream_t)stream;
     char* ws = (char*)workspace;
     auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
@@ -2419,53 +2413,33 @@ static int push_adapt(const delora_odometry_desc* d, const delora_odometry_train
         return 0;
     }
     const int32_t* n_valid = at.n_valid;
-    long long* tick = reinterpret_cast<long long*>(ws + gp.tick);
+    long long* tick = reinterpret_cast<long long*>(ws + ap.tick);
     constexpr unsigned kSeqStride = kGroupBuckets + 1;
-    long long b_off[kGroupBuckets], b_cnt[kGroupBuckets];
     if (g) {                // the fleet-wide count of valid pairs, on every rank before its backward
         uint64_t peer_slots[kArMaxWorld];
-        for (int q = 0; q < g->world; ++q) peer_slots[q] = g->peer_ws[q] + gp.slots;
-        int32_t* n_fleet = reinterpret_cast<int32_t*>(ws + gp.n_fleet);
+        for (int q = 0; q < g->world; ++q) peer_slots[q] = g->peer_ws[q] + ap.slots;
+        int32_t* n_fleet = reinterpret_cast<int32_t*>(ws + ap.n_fleet);
         if ((rc = count_allreduce_launch(peer_slots, g->peer_flags, g->rank, g->world, kSeqStride, tick, at.n_valid,
                                          n_fleet, g->status, st))) return rc;
         n_valid = n_fleet;
-        plan_buckets(tp.m, b_off, b_cnt);
     }
     // each rank divides by the fleet-wide count, so the buckets are summed (scale 1)
-    auto all_reduce = [&](int k) -> int {
-        return bucket_all_reduce(tp, g, b_off, b_cnt, k, 1.0f, tick, kSeqStride, (unsigned)k + 1u, st, who);
-    };
+    const GroupReduce gr{g, 1.0f, tick, kSeqStride, 1u};
     // 4. the backward of the mean over the valid pairs (invalid rows: dL/dT = 0), then Adam where n_valid > 0
-    if ((rc = train_tail_backward(tp, ws, d->act, S, false, st, DropoutCtr{nullptr, 0}, valid, n_valid))) return rc;
-    if (g && (rc = all_reduce(0))) return rc;
-    float* conv_dw[kMaxConv];
-    for (int i = 0; i < tp.m.t.n_conv; ++i) conv_dw[i] = f(tp.grad) + tp.m.t.conv[i].blob;
-    for (int s = 3; s >= 0; --s) {
-        if ((rc = trunk_backward(tp.m.t, tp.t, ws, tp.w, ws, d->act, S, f(tp.g_pooled), conv_dw, s, st))) return rc;
-        if (g && (rc = all_reduce(4 - s))) return rc;
-    }
-    if (g && (rc = group_join(g, st, who))) return rc;
+    if ((rc = step_backward(tp, ws, d->act, S, false, DropoutCtr{nullptr, 0}, valid, n_valid, g ? &gr : nullptr, st,
+                            who))) return rc;
     return adam_update(tp, ws, hp, n_valid, st);
 }
 
 }  // namespace delora
 
 extern "C" int64_t delora_odometry_streams_adapt_workspace_bytes(const delora_odometry_desc* d) {
-    if (check_train_desc(d, "delora_odometry_streams_adapt_workspace_bytes")) return -1;
-    TrainPlan tp;
-    AdaptPlan ap;
-    make_adapt_plan(d, &tp, &ap);
-    return (int64_t)ap.total;
+    return adapt_workspace_bytes(d, false, "delora_odometry_streams_adapt_workspace_bytes");
 }
 
 extern "C" int delora_odometry_streams_adapt_init(const delora_odometry_desc* d, const float* weights, void* workspace,
                                                   void* stream) {
-    const char* who = "delora_odometry_streams_adapt_init";
-    if (check_train_desc(d, who)) return 1;
-    TrainPlan tp;
-    AdaptPlan ap;
-    make_adapt_plan(d, &tp, &ap);
-    return adapt_init(d, ap.total, weights, workspace, (cudaStream_t)stream, who);
+    return adapt_init(d, false, weights, workspace, (cudaStream_t)stream, "delora_odometry_streams_adapt_init");
 }
 
 extern "C" int delora_odometry_streams_push_adapt(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
@@ -2478,24 +2452,12 @@ extern "C" int delora_odometry_streams_push_adapt(const delora_odometry_desc* d,
 }
 
 extern "C" int64_t delora_odometry_streams_adapt_group_workspace_bytes(const delora_odometry_desc* d) {
-    if (check_train_desc(d, "delora_odometry_streams_adapt_group_workspace_bytes")) return -1;
-    TrainPlan tp;
-    AdaptPlan ap;
-    AdaptGroupPlan gp;
-    make_adapt_group_plan(d, &tp, &ap, &gp);
-    return (int64_t)gp.total;
+    return adapt_workspace_bytes(d, true, "delora_odometry_streams_adapt_group_workspace_bytes");
 }
 
 extern "C" int delora_odometry_streams_adapt_group_init(const delora_odometry_desc* d, const float* weights,
                                                         void* workspace, void* stream) {
-    const char* who = "delora_odometry_streams_adapt_group_init";
-    if (check_train_desc(d, who)) return 1;
-    TrainPlan tp;
-    AdaptPlan ap;
-    AdaptGroupPlan gp;
-    make_adapt_group_plan(d, &tp, &ap, &gp);
-    if (adapt_init(d, gp.total, weights, workspace, (cudaStream_t)stream, who)) return 1;
-    return collective_kernels_preload(who);
+    return adapt_init(d, true, weights, workspace, (cudaStream_t)stream, "delora_odometry_streams_adapt_group_init");
 }
 
 extern "C" int delora_odometry_streams_push_adapt_group(const delora_odometry_desc* d,
@@ -2515,16 +2477,10 @@ extern "C" int delora_odometry_streams_adapt_reset(const delora_odometry_desc* d
                                                    void* stream) {
     const char* who = "delora_odometry_streams_adapt_reset";
     if (check_train_desc(d, who)) return 1;
-    DELORA_CHECK_ARG(mask, "%s: null mask", who);
-    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
     TrainPlan tp;
     AdaptPlan ap;
     make_adapt_plan(d, &tp, &ap);
-    const int S = d->max_batch;
-    odometry_streams_reset_kernel<<<(S + 255) / 256, 256, 0, (cudaStream_t)stream>>>(
-        mask, S, reinterpret_cast<int32_t*>((char*)workspace + ap.has_prev));
-    DELORA_CHECK_LAUNCH("odometry_streams_reset_kernel");
-    return 0;
+    return reset_streams(d, mask, workspace, ap.has_prev, stream, who);
 }
 
 // ================================================================================================ dropout

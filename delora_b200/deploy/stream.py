@@ -176,7 +176,70 @@ class OdometryStream:
         self.relative = []
 
 
-class OdometryStreams:
+def _staging(fields, device):
+    """One pinned host buffer and one device buffer holding the 4-byte fields [(name, shape, dtype), ...] back to back.
+    Returns both buffers, the host views by name and the device slices in field order."""
+    sizes = [4 * int(np.prod(shape)) for _, shape, _ in fields]
+    host = torch.zeros((sum(sizes),), dtype=torch.uint8).pin_memory()
+    dev = torch.zeros((sum(sizes),), dtype=torch.uint8, device=device)
+    raw, views, slices, off = host.numpy(), {}, [], 0
+    for (name, shape, dtype), size in zip(fields, sizes):
+        views[name] = raw[off:off + size].view(dtype).reshape(shape)
+        slices.append(dev[off:off + size])
+        off += size
+    return host, dev, views, slices
+
+
+class _Streams:
+    """What the streams front-ends share: the host fill of a tick's scans, the per-stream results, poses and reset.
+    A subclass sets n_streams, n_max, device, workspace, relative (one list per stream) and _mask (device int32 [S])."""
+
+    def _fill(self, scans, points, counts, active):
+        """scans (see push) into the host arrays points [S, 3, n_max], counts [S] and active [S]."""
+        if len(scans) != self.n_streams:
+            raise ValueError(f"push takes {self.n_streams} entries (one per stream, None = inactive), got {len(scans)}")
+        for s, scan in enumerate(scans):
+            if scan is None:
+                active[s] = 0
+                counts[s] = 0
+                continue
+            scan = scan[0] if scan.dim() == 3 else scan
+            n = int(scan.shape[1])
+            if n > self.n_max:
+                raise ValueError(f"stream {s}: scan has more points than the streams were sized for")
+            np.copyto(points[s, :, :n], scan[:3].numpy())
+            counts[s] = n
+            active[s] = 1
+
+    def _results(self, T, valid, extras):
+        """Per stream: None without a transform; else T [1, 4, 4] (kept for poses), or with extras (arrays with a row
+        per stream) the tuple (T, row of each extra), a 1-D extra's row as a float."""
+        out = []
+        for s in range(self.n_streams):
+            if not valid[s]:
+                out.append(None)
+                continue
+            t = T[s].reshape(1, 4, 4).copy()
+            self.relative[s].append(t)
+            rows = tuple(e[s].copy() if e.ndim > 1 else float(e[s]) for e in extras)
+            out.append((t,) + rows if extras else t)
+        return out
+
+    def poses(self, s):
+        """World-frame KITTI poses of stream s so far (src/utility/poses.py:11-58)."""
+        return poses_module.compute_poses(self.relative[s])
+
+    def reset(self, s):
+        """Forget stream s's previous frame and its transforms: its next frame starts it again."""
+        with torch.cuda.device(self.device):
+            self._mask.zero_()
+            self._mask[s] = 1
+            self.workspace.reset(self._mask)
+            torch.cuda.current_stream().synchronize()
+        self.relative[s] = []
+
+
+class OdometryStreams(_Streams):
     """Several LiDAR streams (sensors of one robot, or vehicles served by one process) through one streams workspace of
     the C ABI (`delora_odometry_streams_*`): all streams share the image geometry and the model, and one tick runs the
     model once at batch `n_streams`.  Each stream's transforms are bit-identical to a `delora_odometry_push` workspace
@@ -210,10 +273,17 @@ class OdometryStreams:
         self.n_streams, self.n_max = int(n_streams), int(n_max)
         self.desc = export.desc_from_config(config, dataset, self.n_max, self.n_streams, preprocessing_normals=pre)
         S, n = self.n_streams, self.n_max
+        self.residual = bool(residual) or pre
+        self.normalized = bool(normalized)
+        # the tick's outputs in the order the workspace's push takes them: T and valid, the residual's losses, the
+        # normalised kinds' factor
+        outputs = [("T", (S, 4, 4), np.float32), ("valid", (S,), np.int32)]
+        if self.residual:
+            outputs.append(("losses", (S, ops.LOSS_ROW), np.float32))
+        if normalized:
+            outputs.append(("factor", (S,), np.float32))
         with torch.cuda.device(self.device):
             self.blob = torch.from_numpy(export.pack_state_dict(model.state_dict(), config)).to(self.device)
-            self.residual = bool(residual) or pre
-            self.normalized = bool(normalized)
             if pre:
                 flags = residual_flags | (ops.TRAIN_NORMALIZATION_SCALING if normalized else 0)
                 self.workspace = capi.PreStreamsWorkspace(self.desc, self.blob, capi.residual_params(config, flags))
@@ -224,34 +294,18 @@ class OdometryStreams:
                 self.workspace = capi.NormalizedStreamsWorkspace(self.desc, self.blob)
             else:
                 self.workspace = capi.StreamsWorkspace(self.desc, self.blob)
-            # staging: points [S, 3, n_max] fp32, then counts [S] and active [S] int32, one buffer each way
-            in_bytes = S * 3 * n * 4 + 2 * S * 4
-            self.host_in = torch.zeros((in_bytes,), dtype=torch.uint8).pin_memory()
-            self.dev_in = torch.zeros((in_bytes,), dtype=torch.uint8, device=self.device)
-            # T [S, 16] fp32, valid [S] int32, then with residual losses [S, LOSS_ROW] fp32, normalised factor [S] fp32
-            out_bytes = (S * 16 * 4 + S * 4 + (S * ops.LOSS_ROW * 4 if self.residual else 0)
-                         + (S * 4 if normalized else 0))
-            self.host_out = torch.zeros((out_bytes,), dtype=torch.uint8).pin_memory()
-            self.dev_out = torch.zeros((out_bytes,), dtype=torch.uint8, device=self.device)
-            self.dev_mask = torch.zeros((S,), dtype=torch.int32, device=self.device)
-        raw = self.host_in.numpy()
-        self._host_points = raw[:S * 3 * n * 4].view(np.float32).reshape(S, 3, n)
-        self._host_counts = raw[S * 3 * n * 4:S * 3 * n * 4 + S * 4].view(np.int32)
-        self._host_active = raw[S * 3 * n * 4 + S * 4:].view(np.int32)
-        out = self.host_out.numpy()
-        self._host_T = out[:S * 64].view(np.float32).reshape(S, 4, 4)
-        self._host_valid = out[S * 64:S * 68].view(np.int32)
-        self._host_losses = out[S * 68:S * 68 + S * ops.LOSS_ROW * 4 if pre else None].view(np.float32).reshape(S, -1)
-        self._host_factor = out[S * 68 + S * ops.LOSS_ROW * 4:].view(np.float32) if pre and normalized else None
-        # the push arguments of a tick: points, counts, active, T, valid in the device staging buffers
-        self._dev_active = self.dev_in[S * 3 * n * 4 + S * 4:]
-        self._tick = (self.dev_in[:S * 3 * n * 4], self.dev_in[S * 3 * n * 4:S * 3 * n * 4 + S * 4], self._dev_active,
-                      self.dev_out[:S * 64], self.dev_out[S * 64:S * 68])
-        if pre:
-            self._tick += (self.dev_out[S * 68:S * 68 + S * ops.LOSS_ROW * 4],
-                           self.dev_out[S * 68 + S * ops.LOSS_ROW * 4:] if normalized else None)
-        elif self.residual or normalized:
-            self._tick += (self.dev_out[S * 68:],)
+            self.host_in, self.dev_in, self._in, dev_in = _staging(
+                [("points", (S, 3, n), np.float32), ("counts", (S,), np.int32), ("active", (S,), np.int32)],
+                self.device)
+            self.host_out, self.dev_out, self._out, dev_out = _staging(outputs, self.device)
+            self._mask = torch.zeros((S,), dtype=torch.int32, device=self.device)
+        # the push arguments of a tick, all in the device staging buffers
+        self._dev_active = dev_in[2]
+        self._tick = tuple(dev_in) + tuple(dev_out)
+        # what push returns beside T: the residual's losses and the recipe's factor (the normalised raw-scan streams
+        # return T alone)
+        self._extras = (([self._out["losses"]] if self.residual else []) +
+                        ([self._out["factor"]] if pre and normalized else []))
         self.relative = [[] for _ in range(S)]
         self.use_cuda_graph = bool(use_cuda_graph)
         self.graph = None
@@ -272,23 +326,10 @@ class OdometryStreams:
         None for a stream without a frame this tick.  Returns a list of n_streams entries: the relative transform
         T_{k-1,k} of the stream as a [1, 4, 4] numpy array, or None (no frame, or the stream's first frame).  With
         residual=True an entry with a transform is the tuple (T, losses [LOSS_ROW] numpy array)."""
-        if len(scans) != self.n_streams:
-            raise ValueError(f"push takes {self.n_streams} entries (one per stream, None = inactive), got {len(scans)}")
+        self._fill(scans, self._in["points"], self._in["counts"], self._in["active"])
         with torch.cuda.device(self.device):
             if self.use_cuda_graph and self.graph is None:
                 self._capture()
-            for s, scan in enumerate(scans):
-                if scan is None:
-                    self._host_active[s] = 0
-                    self._host_counts[s] = 0
-                    continue
-                scan = scan[0] if scan.dim() == 3 else scan
-                n = int(scan.shape[1])
-                if n > self.n_max:
-                    raise Exception(f"stream {s}: scan has more points than the streams were sized for")
-                np.copyto(self._host_points[s, :, :n], scan[:3].numpy())
-                self._host_counts[s] = n
-                self._host_active[s] = 1
             self.dev_in.copy_(self.host_in, non_blocking=True)
             if self.graph is not None:
                 self.graph.replay()
@@ -296,31 +337,7 @@ class OdometryStreams:
                 self.workspace.push(*self._tick)
             self.host_out.copy_(self.dev_out, non_blocking=True)
             torch.cuda.current_stream().synchronize()
-        out = []
-        for s in range(self.n_streams):
-            if self._host_valid[s]:
-                t = self._host_T[s][None].copy()
-                self.relative[s].append(t)
-                if self._host_factor is not None:
-                    out.append((t, self._host_losses[s].copy(), float(self._host_factor[s])))
-                else:
-                    out.append((t, self._host_losses[s].copy()) if self.residual else t)
-            else:
-                out.append(None)
-        return out
-
-    def poses(self, s):
-        """World-frame KITTI poses of stream s so far (src/utility/poses.py:11-58)."""
-        return poses_module.compute_poses(self.relative[s])
-
-    def reset(self, s):
-        """Forget stream s's previous frame and its transforms: its next frame starts it again."""
-        with torch.cuda.device(self.device):
-            self.dev_mask.zero_()
-            self.dev_mask[s] = 1
-            self.workspace.reset(self.dev_mask)
-            torch.cuda.current_stream().synchronize()
-        self.relative[s] = []
+        return self._results(self._out["T"], self._out["valid"], self._extras)
 
 
 class NormalizedOdometryStreams(OdometryStreams):
@@ -356,7 +373,7 @@ class PreprocessedOdometryStreams(OdometryStreams):
                     bool(config.get("normalization_scaling", False)), pre=True)
 
 
-class AdaptiveOdometryStreams:
+class AdaptiveOdometryStreams(_Streams):
     """Several streams served while the model adapts to them (`delora_odometry_streams_push_adapt`): one tick runs the
     training step's forward at batch `n_streams`, each pair's first frame taken from the workspace, returns each
     stream's T and ICP loss row, and with update=True takes one Adam step (learning rate `lr`, torch's default betas)
@@ -392,55 +409,23 @@ class AdaptiveOdometryStreams:
             self.T = torch.zeros((S, 16), dtype=torch.float32, device=self.device)
             self.valid = torch.zeros((S,), dtype=torch.int32, device=self.device)
             self.losses = torch.zeros((S, ops.LOSS_ROW), dtype=torch.float32, device=self.device)
-            self.mask = torch.zeros((S,), dtype=torch.int32, device=self.device)
+            self._mask = torch.zeros((S,), dtype=torch.int32, device=self.device)
         self.relative = [[] for _ in range(S)]
 
     def push(self, scans, update=True):
         """scans: n_streams entries, each a [3, N] (or [1, 3, N]) float32 host tensor with N <= n_max, or None.  Returns
         n_streams entries: (T [1, 4, 4], losses [LOSS_ROW]) numpy arrays for a stream with a pair this tick, else None."""
-        if len(scans) != self.n_streams:
-            raise ValueError(f"push takes {self.n_streams} entries (one per stream, None = inactive), got {len(scans)}")
         pts = torch.zeros((self.n_streams, 3, self.n_max), dtype=torch.float32)
         counts = torch.zeros((self.n_streams,), dtype=torch.int32)
         active = torch.zeros((self.n_streams,), dtype=torch.int32)
-        for s, scan in enumerate(scans):
-            if scan is None:
-                continue
-            scan = scan[0] if scan.dim() == 3 else scan
-            n = int(scan.shape[1])
-            if n > self.n_max:
-                raise ValueError(f"stream {s}: scan has more points than the streams were sized for")
-            pts[s, :, :n] = scan[:3]
-            counts[s] = n
-            active[s] = 1
+        self._fill(scans, pts.numpy(), counts.numpy(), active.numpy())
         with torch.cuda.device(self.device):
             self.points.copy_(pts)
             self.counts.copy_(counts)
             self.active.copy_(active)
             self.workspace.push(self.points, self.counts, self.active, self.T, self.valid, self.losses, update)
             T, valid, losses = self.T.cpu().numpy(), self.valid.cpu().numpy(), self.losses.cpu().numpy()
-        out = []
-        for s in range(self.n_streams):
-            if valid[s]:
-                t = T[s].reshape(1, 4, 4).copy()
-                self.relative[s].append(t)
-                out.append((t, losses[s].copy()))
-            else:
-                out.append(None)
-        return out
-
-    def poses(self, s):
-        """World-frame KITTI poses of stream s so far (src/utility/poses.py:11-58)."""
-        return poses_module.compute_poses(self.relative[s])
-
-    def reset(self, s):
-        """Forget stream s's previous frame and its transforms: its next frame starts it again."""
-        with torch.cuda.device(self.device):
-            self.mask.zero_()
-            self.mask[s] = 1
-            self.workspace.reset(self.mask)
-            torch.cuda.current_stream().synchronize()
-        self.relative[s] = []
+        return self._results(T, valid, [losses])
 
     def state_dict(self):
         """The adapted weights as an OdometryModel state dict (fp32 CPU tensors)."""

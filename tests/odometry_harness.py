@@ -212,3 +212,39 @@ def build_example(name, out_dir, link):
     r = subprocess.run(cmd + ["-o", out], capture_output=True, text=True)
     assert r.returncode == 0, r.stdout + r.stderr
     return out
+
+
+def bits(t):
+    """A float32 tensor's bits as int32: bit-for-bit comparisons."""
+    return t.contiguous().view(torch.int32)
+
+
+def same(a, b):
+    return torch.equal(bits(a), bits(b))
+
+
+def align(n):
+    """n bytes rounded up to a workspace section's 256-byte alignment."""
+    return (n + 255) // 256 * 256
+
+
+def state(ws):
+    """A training workspace's (weights, exp_avg, exp_avg_sq, step), copied to the host."""
+    st = ws.get_state()
+    torch.cuda.synchronize()
+    return tuple(t.cpu().clone() for t in st)
+
+
+def same_state(a, b):
+    return all(same(x, y) if x.dtype == torch.float32 else torch.equal(x, y) for x, y in zip(a, b))
+
+
+def streams_desc(h=64, w=720, S=2, w_pre=0, n_stride=1000):
+    """The descriptor of an S-stream workspace, for the host-only queries."""
+    return desc(config(h, w, device="cpu"), n_stride, S, w_pre)
+
+
+def train_params(flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL, lr=1e-5):
+    from delora_b200 import _lib
+    return _lib.OdometryTrainParams(lr=lr, beta1=0.9, beta2=0.999, eps=1e-8, lambda_po2pl=1.0, loss_flags=flags,
+                                    nb_h=7, nb_w=11, epsilon_range=0.5, min_neighbors=10)

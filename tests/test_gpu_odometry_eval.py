@@ -32,14 +32,6 @@ ICP = ops.LOSS_PO2PL | ops.LOSS_PL2PL
 ALL_ICP = ops.LOSS_PO2PO | ops.LOSS_PO2PL | ops.LOSS_PL2PL
 
 
-def _bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-def _same(a, b):
-    return torch.equal(_bits(a), _bits(b))
-
-
 def _batch(pairs, s, b, n_stride):
     return H.stack_pairs([pairs[(s + j) % len(pairs)] for j in range(b)], n_stride)
 
@@ -94,7 +86,7 @@ def test_eval_returns_the_steps_bits_and_updates_nothing(cuda_lib, flags):
     cfg, blob, pairs, n_stride = _setup()
     ev, st = _eval_then_step(H.trainer(cfg, n_stride, 3, blob, 1e-4, flags=flags), pairs, n_stride, 2)
     for x, y, name in zip(ev, st, ("losses", "T", "pooled")):
-        assert _same(x, y), f"{name}: the eval differs from the step"
+        assert H.same(x, y), f"{name}: the eval differs from the step"
     assert float(ev[0][:, 3].min()) > 0, "no matched pairs: the comparison is empty"
 
 
@@ -104,7 +96,7 @@ def test_eval_at_the_preprocessing_width(cuda_lib, normalized):
     flags = ICP | (ops.TRAIN_NORMALIZATION_SCALING if normalized else 0)
     ev, st = _eval_then_step(H.trainer(cfg, n_stride, 3, blob, 1e-4, w_pre=360, flags=flags), pairs, n_stride, 2)
     for x, y, name in zip(ev, st, ("losses", "T", "pooled")):
-        assert _same(x, y), f"{name}: the eval differs from the step"
+        assert H.same(x, y), f"{name}: the eval differs from the step"
     assert bool((ev[0][:, 6] > 0).all()) == normalized          # the factor column
 
 
@@ -112,7 +104,7 @@ def test_eval_at_64x720(cuda_lib):
     cfg, blob, pairs, n_stride = _setup(64, 720, 1024, 3, seed=21)
     ev, st = _eval_then_step(H.trainer(cfg, n_stride, 2, blob, 1e-4), pairs, n_stride, 2)
     for x, y, name in zip(ev, st, ("losses", "T", "pooled")):
-        assert _same(x, y), f"{name}: the eval differs from the step"
+        assert H.same(x, y), f"{name}: the eval differs from the step"
 
 
 def test_steps_interleaved_with_evals_end_in_the_same_state(cuda_lib):
@@ -130,7 +122,7 @@ def test_steps_interleaved_with_evals_end_in_the_same_state(cuda_lib):
     torch.cuda.synchronize()
     for s, (x, y) in enumerate(zip(outs_p, outs_m)):
         for xx, yy, name in zip(x, y, ("losses", "T", "pooled", "grads")):
-            assert _same(xx, yy), f"step {s + 1}: {name} differ with evals in between"
+            assert H.same(xx, yy), f"step {s + 1}: {name} differ with evals in between"
     for x, y, name in zip(plain.get_state(), mixed.get_state(), ("weights", "exp_avg", "exp_avg_sq", "step")):
         assert torch.equal(x, y), f"{name} differ with evals in between"
 
@@ -144,10 +136,10 @@ def test_eval_ignores_the_dropout_and_identity_bits(cuda_lib):
     flagged = tr.eval(pts, counts)
     torch.cuda.synchronize()
     for x, y, name in zip(plain, flagged, ("losses", "T", "pooled")):
-        assert _same(x, y), f"{name}: the dropout / identity bits changed the eval"
+        assert H.same(x, y), f"{name}: the dropout / identity bits changed the eval"
     assert float(flagged[0][:, 5].abs().max()) == 0.0
     # the step they train with does apply the masks
-    assert not _same(tr.step(pts, counts)[2], plain[2])
+    assert not H.same(tr.step(pts, counts)[2], plain[2])
 
 
 def test_eval_replays_from_a_graph(cuda_lib):
@@ -167,7 +159,7 @@ def test_eval_replays_from_a_graph(cuda_lib):
         torch.cuda.synchronize()
         got = [t.clone() for t in out]
         for x, y, name in zip(got, tr.eval(p, c), ("losses", "T", "pooled")):
-            assert _same(x, y), f"replay on batch {s}: {name} differ from the eager eval"
+            assert H.same(x, y), f"replay on batch {s}: {name} differ from the eager eval"
 
 
 # ================================================================================================ _push_residual
@@ -307,7 +299,7 @@ def _check_rows(out, rows, S):
     for k, (_, valid, losses) in enumerate(out):
         for s in range(S):
             if (k, s) in rows:
-                assert _same(losses[s], rows[(k, s)]), \
+                assert H.same(losses[s], rows[(k, s)]), \
                     f"tick {k} stream {s}: {losses[s].tolist()} != the operator alone {rows[(k, s)].tolist()}"
                 matched += int(losses[s][3] > 0)
             else:
@@ -329,7 +321,7 @@ def test_residual_rows_and_transforms(cuda_lib, S, flags):
         "a write outside delora_odometry_streams_residual_workspace_bytes"
     for k, ((tp, vp), (tr, vr, _)) in enumerate(zip(plain, out)):
         assert torch.equal(vp, vr), f"tick {k}: valid differs from _streams_push"
-        assert _same(tp, tr), f"tick {k}: T differs from _streams_push"
+        assert H.same(tp, tr), f"tick {k}: T differs from _streams_push"
     # the first frames, the all-inactive tick 3 and the tick after the reset leave the ICP armed: later rows still match
     _check_rows(out, _reference_rows(cfg, ticks, act, resets, out, flags), S)
 
@@ -342,7 +334,7 @@ def test_residual_graph_replay_matches_eager(cuda_lib):
     graphed = _run_residual(capi.ResidualStreamsWorkspace(d, blob, rp), ticks, resets, graph=True)
     for k, (e, g) in enumerate(zip(eager, graphed)):
         assert torch.equal(e[1], g[1]), f"tick {k}: valid differs"
-        assert _same(e[0], g[0]) and _same(e[2], g[2]), f"tick {k}: the replay differs from the eager call"
+        assert H.same(e[0], g[0]) and H.same(e[2], g[2]), f"tick {k}: the replay differs from the eager call"
 
 
 def test_residual_at_64x720(cuda_lib):
@@ -351,7 +343,7 @@ def test_residual_at_64x720(cuda_lib):
     plain = _run_plain(capi.StreamsWorkspace(d, blob), ticks, resets)
     out = _run_residual(capi.ResidualStreamsWorkspace(d, blob, capi.residual_params(cfg)), ticks, resets)
     for k, ((tp, vp), (tr, vr, _)) in enumerate(zip(plain, out)):
-        assert torch.equal(vp, vr) and _same(tp, tr), f"tick {k}: T / valid differ from _streams_push"
+        assert torch.equal(vp, vr) and H.same(tp, tr), f"tick {k}: T / valid differ from _streams_push"
     _check_rows(out, _reference_rows(cfg, ticks, act, resets, out, ICP), 2)
 
 

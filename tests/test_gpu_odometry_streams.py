@@ -120,10 +120,6 @@ def _run_streams(st, ticks, resets, graph=False):
     return out
 
 
-def _bits(t):
-    return t.contiguous().view(torch.int32)
-
-
 def _check_against_push(out, want, act, resets):
     S = act.shape[1]
     expect_T = torch.full((S, 16), SENTINEL, dtype=torch.float32)
@@ -140,7 +136,7 @@ def _check_against_push(out, want, act, resets):
                 n_valid += 1
             if act[k, s]:
                 has[s] = True
-        assert torch.equal(_bits(T), _bits(expect_T)), f"tick {k}: T differs from the per-stream pushes"
+        assert torch.equal(H.bits(T), H.bits(expect_T)), f"tick {k}: T differs from the per-stream pushes"
     return n_valid
 
 
@@ -190,7 +186,7 @@ def test_graph_replay_matches_eager(cuda_lib):
     graphed = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 4), blob), ticks, resets, graph=True)
     for k, ((te, ve), (tg, vg)) in enumerate(zip(eager, graphed)):
         assert torch.equal(ve, vg), f"tick {k}: valid differs"
-        assert torch.equal(_bits(te), _bits(tg)), f"tick {k}: graph replay differs from the eager call"
+        assert torch.equal(H.bits(te), H.bits(tg)), f"tick {k}: graph replay differs from the eager call"
 
 
 def test_deterministic(cuda_lib):
@@ -198,7 +194,7 @@ def test_deterministic(cuda_lib):
     a = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 3), blob), ticks, resets)
     b = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 3), blob), ticks, resets)
     for (ta, va), (tb, vb) in zip(a, b):
-        assert torch.equal(va, vb) and torch.equal(_bits(ta), _bits(tb))
+        assert torch.equal(va, vb) and torch.equal(H.bits(ta), H.bits(tb))
 
 
 def test_null_active_means_all_active(cuda_lib):
@@ -211,7 +207,7 @@ def test_null_active_means_all_active(cuda_lib):
     for k, (p, c, _) in enumerate(all_on):
         st.push(p.to(DEV), c.to(DEV), None, T, valid)
         torch.cuda.synchronize()
-        assert torch.equal(valid.cpu(), a[k][1]) and torch.equal(_bits(T.cpu()), _bits(a[k][0]))
+        assert torch.equal(valid.cpu(), a[k][1]) and torch.equal(H.bits(T.cpu()), H.bits(a[k][0]))
 
 
 def test_inactive_stream_keeps_its_cached_frame(cuda_lib):
@@ -226,8 +222,8 @@ def test_inactive_stream_keeps_its_cached_frame(cuda_lib):
     out = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 3), blob), ticks, {})
     assert [int(v[1]) for _, v in out] == [0, 0, 0, 0, 1]
     want = _push_reference(cfg, n_stride, blob, [ticks[0], ticks[4]], act[[0, 4]], {})
-    assert torch.equal(_bits(out[4][0][1]), _bits(want[(1, 1)]))
-    assert torch.equal(_bits(out[3][0][1]), _bits(torch.full((16,), SENTINEL)))     # untouched while inactive
+    assert torch.equal(H.bits(out[4][0][1]), H.bits(want[(1, 1)]))
+    assert torch.equal(H.bits(out[3][0][1]), H.bits(torch.full((16,), SENTINEL)))     # untouched while inactive
 
 
 @pytest.mark.parametrize("w", [720, 2047])

@@ -28,14 +28,6 @@ ICP = ops.LOSS_PO2PL | ops.LOSS_PL2PL
 LR = 1e-4
 
 
-def _bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-def _same(a, b):
-    return torch.equal(_bits(a), _bits(b))
-
-
 def _cfg(h, w, w_pre, normalized=False):
     cfg = H.config(h, w)
     cfg["kitti"]["horizontal_cells_preprocessing"] = w_pre
@@ -93,17 +85,6 @@ def _run(ws, ticks, updates, resets=None):
     return out
 
 
-def _state(ws):
-    st = ws.get_state()
-    torch.cuda.synchronize()
-    return tuple(t.cpu().clone() for t in st)
-
-
-def _same_state(a, b):
-    return all(torch.equal(x.view(torch.int32) if x.dtype == torch.float32 else x, y.view(torch.int32)
-                           if y.dtype == torch.float32 else y) for x, y in zip(a, b))
-
-
 def _single_ticks(frames, n_stride, empty=()):
     out = []
     for k, f in enumerate(frames):
@@ -138,12 +119,12 @@ def test_one_stream_is_the_training_step(cuda_lib, h, w, w_raw, w_pre, normalize
             pts, counts = H.stack([frames[k - 1], frames[k]], n_stride)
             l_ref, t_ref, _, _ = tr.step(pts, counts)
             torch.cuda.synchronize()
-            assert _same(T[0], t_ref.reshape(16).cpu()), f"tick {k}: T differs from _train_step at B = 1"
-            assert _same(losses[0], l_ref[0].cpu()), f"tick {k}: {losses[0].tolist()} != {l_ref[0].tolist()}"
+            assert H.same(T[0], t_ref.reshape(16).cpu()), f"tick {k}: T differs from _train_step at B = 1"
+            assert H.same(losses[0], l_ref[0].cpu()), f"tick {k}: {losses[0].tolist()} != {l_ref[0].tolist()}"
         else:
             assert float(losses[0].abs().max()) == 0.0
-        assert _same_state(_state(ws), _state(tr)), f"tick {k}: the training state differs from _train_step's"
-    assert int(_state(ws)[3][0]) == K - 1
+        assert H.same_state(H.state(ws), H.state(tr)), f"tick {k}: the training state differs from _train_step's"
+    assert int(H.state(ws)[3][0]) == K - 1
 
 
 def _pattern(S, ticks=7):
@@ -188,8 +169,8 @@ def test_rows_are_independent(cuda_lib, w_pre, normalized):
         one = _run(_adapt(cfg, blob, n_stride, 1, w_pre, normalized), single, updates, res)
         for k, (e, o) in enumerate(zip(out, one)):
             assert int(e[1][s]) == int(o[1][0]), f"tick {k} stream {s}: valid differs from S = 1"
-            assert _same(e[0][s], o[0][0]), f"tick {k} stream {s}: T differs from S = 1"
-            assert _same(e[2][s], o[2][0]), f"tick {k} stream {s}: losses differ from S = 1"
+            assert H.same(e[0][s], o[0][0]), f"tick {k} stream {s}: T differs from S = 1"
+            assert H.same(e[2][s], o[2][0]), f"tick {k} stream {s}: losses differ from S = 1"
             if not int(e[1][s]):
                 assert float(e[2][s].abs().max()) == 0.0
 
@@ -204,7 +185,7 @@ def _mean_tick(cfg, blob, frames, n_stride, third):
              (p1.cpu(), c1.cpu(), torch.tensor([1, 1, 1], dtype=torch.int32))]
     out = _run(ws, ticks, [True, True])
     assert out[1][1].tolist() == [1, 1, 0]
-    st = _state(ws)
+    st = H.state(ws)
     return st[1], int(st[3][0])
 
 
@@ -240,16 +221,16 @@ def test_no_pair_no_update(cuda_lib, w_pre):
     act = np.ones((3, S), dtype=bool)
     ticks = _ticks(pool, S, n_stride, act, set())
     ws = _adapt(cfg, blob, n_stride, S, w_pre)
-    before = _state(ws)
+    before = H.state(ws)
     out = _run(ws, ticks[:1], [True])
     assert int(out[0][1].sum()) == 0
-    assert _same_state(_state(ws), before), "an update without a valid pair changed the training state"
+    assert H.same_state(H.state(ws), before), "an update without a valid pair changed the training state"
     # the cache advanced, and the filters are the ones a workspace that never updated serves with
     ref = _run(_adapt(cfg, blob, n_stride, S, w_pre), ticks[:2], [False, False])
     nxt = _run(ws, ticks[1:2], [False])
     assert nxt[0][1].tolist() == [1] * S
     for a, b in zip(nxt[0], ref[1]):
-        assert _same(a, b)
+        assert H.same(a, b)
 
 
 def test_graphs_replay_the_eager_calls(cuda_lib):
@@ -289,9 +270,9 @@ def test_graphs_replay_the_eager_calls(cuda_lib):
         graphs[updates[k]].replay()
         got = gio.out()
         for i, (x, y) in enumerate(zip(eager[k], got)):
-            assert _same(x, y), f"tick {k}: output {i} of the replay differs from the eager call"
-    assert _same_state(_state(eager_ws), _state(g_ws))
-    assert int(_state(g_ws)[3][0]) == 2          # ticks 1 and 3 update; tick 4 has no stream, so no pair
+            assert H.same(x, y), f"tick {k}: output {i} of the replay differs from the eager call"
+    assert H.same_state(H.state(eager_ws), H.state(g_ws))
+    assert int(H.state(g_ws)[3][0]) == 2          # ticks 1 and 3 update; tick 4 has no stream, so no pair
 
 
 def test_state_round_trip_leaves_the_streams_and_resumes(cuda_lib):
@@ -305,10 +286,10 @@ def test_state_round_trip_leaves_the_streams_and_resumes(cuda_lib):
     _run(a, ticks[:3], [True] * 3)
     train_bytes = capi.TrainingWorkspace.workspace_bytes(a.desc)
     section = a.workspace[train_bytes:].cpu().clone()
-    st = _state(a)
+    st = H.state(a)
     a.set_state(st[0], st[1], st[2], int(st[3][0]))
     assert torch.equal(a.workspace[train_bytes:].cpu(), section), "_train_set_state wrote into the stream section"
-    assert _same_state(_state(a), st)
+    assert H.same_state(H.state(a), st)
     want = _run(a, ticks[3:], [True] * 3)
     b = _adapt(cfg, blob, n_stride, S, w_pre)
     b.set_state(st[0], st[1], st[2], int(st[3][0]))
@@ -316,8 +297,8 @@ def test_state_round_trip_leaves_the_streams_and_resumes(cuda_lib):
     got = _run(b, ticks[3:], [True] * 3)
     for k, (x, y) in enumerate(zip(want, got)):
         for i, (u, v) in enumerate(zip(x, y)):
-            assert _same(u, v), f"resumed tick {k}: output {i} differs"
-    assert _same_state(_state(a), _state(b))
+            assert H.same(u, v), f"resumed tick {k}: output {i} differs"
+    assert H.same_state(H.state(a), H.state(b))
 
 
 def test_python_class(cuda_lib):

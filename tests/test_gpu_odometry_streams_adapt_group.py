@@ -34,14 +34,6 @@ LR = 1e-4
 HH, WW, W_RAW = 16, 180, 512
 
 
-def _bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-def _same(a, b):
-    return torch.equal(_bits(a), _bits(b))
-
-
 def _params(cfg, lr=LR, beta1=0.9):
     return capi.train_params(cfg, lr, loss_flags=ICP, beta1=beta1)
 
@@ -105,16 +97,6 @@ def _single_tick(ws, pts, counts, active, update):
     return T.cpu(), valid.cpu(), losses.cpu()
 
 
-def _state(ws):
-    st = ws.get_state()
-    torch.cuda.synchronize()
-    return tuple(t.cpu().clone() for t in st)
-
-
-def _same_state(a, b):
-    return all(_same(x, y) if x.dtype == torch.float32 else torch.equal(x, y) for x, y in zip(a, b))
-
-
 def _status_ok(g):
     return all(int(s.item()) == 0 for s in g.status)
 
@@ -131,13 +113,13 @@ def test_single_rank_group_is_push_adapt(cuda_lib):
         (got,) = _group_tick(g, streams, [inp], [u])
         want = _single_tick(plain, *inp, u)
         valid = want[1]
-        assert _same(got[1], valid), f"tick {k}: valid"
+        assert H.same(got[1], valid), f"tick {k}: valid"
         for s in range(S):
             if int(valid[s]):
-                assert _same(got[0][s], want[0][s]), f"tick {k}, stream {s}: T"
-        assert _same(got[2], want[2]), f"tick {k}: losses"
-        assert _same_state(_state(g.workspaces[0]), _state(plain)), f"tick {k}: the training state"
-    assert int(_state(plain)[3][0]) >= 2
+                assert H.same(got[0][s], want[0][s]), f"tick {k}, stream {s}: T"
+        assert H.same(got[2], want[2]), f"tick {k}: losses"
+        assert H.same_state(H.state(g.workspaces[0]), H.state(plain)), f"tick {k}: the training state"
+    assert int(H.state(plain)[3][0]) >= 2
     assert _status_ok(g)
 
 
@@ -147,14 +129,14 @@ def _check_rows(k, outs, single, world, S):
             row = r * S + s
             assert int(outs[r][1][s]) == int(single[1][row]), f"tick {k}, rank {r}, stream {s}: valid"
             if int(single[1][row]):
-                assert _same(outs[r][0][s], single[0][row]), f"tick {k}, rank {r}, stream {s}: T"
-            assert _same(outs[r][2][s], single[2][row]), f"tick {k}, rank {r}, stream {s}: losses"
+                assert H.same(outs[r][0][s], single[0][row]), f"tick {k}, rank {r}, stream {s}: T"
+            assert H.same(outs[r][2][s], single[2][row]), f"tick {k}, rank {r}, stream {s}: losses"
 
 
 def _check_ranks_agree(k, g):
-    states = [_state(w) for w in g.workspaces]
+    states = [H.state(w) for w in g.workspaces]
     for r in range(1, len(states)):
-        assert _same_state(states[r], states[0]), f"tick {k}: rank {r}'s state differs from rank 0's"
+        assert H.same_state(states[r], states[0]), f"tick {k}: rank {r}'s state differs from rank 0's"
     return states[0]
 
 
@@ -187,9 +169,9 @@ def _run_against_single(cfg, blob, pool, n_stride, world, S, extra_serve=None):
         state = _check_ranks_agree(k, g)
         if update:
             assert int(state[3][0]) == k
-            _check_mean(k, cfg, state[1], _state(single)[1])
+            _check_mean(k, cfg, state[1], H.state(single)[1])
     assert _status_ok(g)
-    return [_state(w) for w in g.workspaces]
+    return [H.state(w) for w in g.workspaces]
 
 
 @pytest.mark.parametrize("world", [2, 4])
@@ -203,7 +185,7 @@ def test_uneven_serve_only_ticks_change_nothing(cuda_lib):
     want = _run_against_single(cfg, blob, pool, n_stride, 2, 2)
     got = _run_against_single(cfg, blob, pool, n_stride, 2, 2, extra_serve=[0, 3])
     for r, (a, b) in enumerate(zip(got, want)):
-        assert _same_state(a, b), f"rank {r}: serve-only ticks changed the update"
+        assert H.same_state(a, b), f"rank {r}: serve-only ticks changed the update"
 
 
 def test_the_mean_is_over_pairs_not_ranks(cuda_lib):
@@ -220,7 +202,7 @@ def test_the_mean_is_over_pairs_not_ranks(cuda_lib):
         assert outs[1][1].tolist() == [0, 0]
     state = _check_ranks_agree(1, g)
     assert int(state[3][0]) == 1                    # tick 0 had no pair anywhere
-    want = _state(single)[1]
+    want = H.state(single)[1]
     _check_mean(1, cfg, state[1], want)
     # the mean of the ranks' means would be half of it
     tail, trunk = H.grad_spread(H.grad_dict(state[1], cfg), H.grad_dict(want * 0.5, cfg))
@@ -233,12 +215,12 @@ def test_no_pair_on_any_rank_no_update(cuda_lib):
     S, world = 2, 2
     empty, e_streams = _group(cfg, blob, n_stride, world, S)      # takes the empty update tick
     plain, p_streams = _group(cfg, blob, n_stride, world, S)      # serves that tick only
-    before = [_state(w) for w in empty.workspaces]
+    before = [H.state(w) for w in empty.workspaces]
     inputs = [_tick_inputs(pool, S, n_stride, 0, [1, 1], r * S) for r in range(world)]
     outs = _group_tick(empty, e_streams, inputs, [True] * world)
     assert all(int(o[1].sum()) == 0 for o in outs)
     for r in range(world):
-        assert _same_state(_state(empty.workspaces[r]), before[r]), f"rank {r}: an update without a pair"
+        assert H.same_state(H.state(empty.workspaces[r]), before[r]), f"rank {r}: an update without a pair"
     _group_tick(plain, p_streams, inputs, [False] * world)
     for k in (1, 2):
         inputs = [_tick_inputs(pool, S, n_stride, k, [1, 1], r * S) for r in range(world)]
@@ -246,9 +228,9 @@ def test_no_pair_on_any_rank_no_update(cuda_lib):
         want = _group_tick(plain, p_streams, inputs, [True] * world)
         for r in range(world):
             for i, (x, y) in enumerate(zip(got[r], want[r])):
-                assert _same(x, y), f"tick {k}, rank {r}: output {i}"
-            assert _same_state(_state(empty.workspaces[r]), _state(plain.workspaces[r])), f"tick {k}, rank {r}"
-    assert int(_state(empty.workspaces[0])[3][0]) == 2
+                assert H.same(x, y), f"tick {k}, rank {r}: output {i}"
+            assert H.same_state(H.state(empty.workspaces[r]), H.state(plain.workspaces[r])), f"tick {k}, rank {r}"
+    assert int(H.state(empty.workspaces[0])[3][0]) == 2
     assert _status_ok(empty) and _status_ok(plain)
 
 
@@ -300,15 +282,15 @@ def test_graph_replay_of_the_group_tick_matches_eager(cuda_lib):
         torch.cuda.synchronize()
         for r in range(world):
             valid = bufs[r][4].cpu()
-            assert _same(valid, want[k][r][1]), f"tick {k}, rank {r}: valid"
+            assert H.same(valid, want[k][r][1]), f"tick {k}, rank {r}: valid"
             for s in range(S):
                 if int(valid[s]):
-                    assert _same(bufs[r][3][s].cpu(), want[k][r][0][s]), f"tick {k}, rank {r}: T"
-            assert _same(bufs[r][5].cpu(), want[k][r][2]), f"tick {k}, rank {r}: losses"
+                    assert H.same(bufs[r][3][s].cpu(), want[k][r][0][s]), f"tick {k}, rank {r}: T"
+            assert H.same(bufs[r][5].cpu(), want[k][r][2]), f"tick {k}, rank {r}: losses"
         assert _status_ok(graphed), f"tick {k}: a collective timed out"
     for r in range(world):
-        assert _same_state(_state(graphed.workspaces[r]), _state(eager.workspaces[r])), f"rank {r}: the state"
-    assert int(_state(graphed.workspaces[0])[3][0]) == ticks - 1         # tick 0 has first frames only
+        assert H.same_state(H.state(graphed.workspaces[r]), H.state(eager.workspaces[r])), f"rank {r}: the state"
+    assert int(H.state(graphed.workspaces[0])[3][0]) == ticks - 1         # tick 0 has first frames only
     assert _status_ok(eager)
 
 

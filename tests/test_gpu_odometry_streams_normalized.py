@@ -136,10 +136,6 @@ def _run_streams(st, ticks, resets, graph=False, loads=None):
     return out
 
 
-def _bits(t):
-    return t.contiguous().view(torch.int32)
-
-
 def _check(out, want, act, resets, skip=()):
     """valid, T and factor after every tick against the references; rows of (tick, stream) in skip are only checked
     for their valid flag.  -> the number of rows compared."""
@@ -161,8 +157,8 @@ def _check(out, want, act, resets, skip=()):
                 n += 1
             if act[k, s]:
                 has[s] = True
-        assert torch.equal(_bits(T), _bits(expect_T)), f"tick {k}: T differs from pairs_normalized at B = 1"
-        assert torch.equal(_bits(factor), _bits(expect_f)), f"tick {k}: factor differs from pairs_normalized at B = 1"
+        assert torch.equal(H.bits(T), H.bits(expect_T)), f"tick {k}: T differs from pairs_normalized at B = 1"
+        assert torch.equal(H.bits(factor), H.bits(expect_f)), f"tick {k}: factor differs from pairs_normalized at B = 1"
     return n
 
 
@@ -222,8 +218,8 @@ def test_graph_replay_matches_the_direct_calls(cuda_lib):
     graphed = _run_streams(NormalizedStreamsWorkspace(d, blob), ticks, resets, graph=True)
     for k, (e, g) in enumerate(zip(eager, graphed)):
         assert torch.equal(e[1], g[1]), f"tick {k}: valid differs"
-        assert torch.equal(_bits(e[0]), _bits(g[0])), f"tick {k}: T differs under graph replay"
-        assert torch.equal(_bits(e[2]), _bits(g[2])), f"tick {k}: factor differs under graph replay"
+        assert torch.equal(H.bits(e[0]), H.bits(g[0])), f"tick {k}: T differs under graph replay"
+        assert torch.equal(H.bits(e[2]), H.bits(g[2])), f"tick {k}: factor differs under graph replay"
 
 
 def test_load_weights_and_reset_act_as_on_the_streams_workspace(cuda_lib):

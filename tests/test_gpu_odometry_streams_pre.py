@@ -30,14 +30,6 @@ ICP = ops.LOSS_PO2PL | ops.LOSS_PL2PL
 SIZES = [(16, 180, 512, 360), (64, 720, 2048, 2250)]                   # H, W, w_raw, w_pre
 
 
-def _bits(t):
-    return t.contiguous().view(torch.int32)
-
-
-def _same(a, b):
-    return torch.equal(_bits(a), _bits(b))
-
-
 def _cfg(h, w, w_pre, normalized):
     cfg = H.config(h, w)
     cfg["kitti"]["horizontal_cells_preprocessing"] = w_pre
@@ -169,7 +161,7 @@ def _check_against_references(cfg, blob, out, pairs, normalized, flags=ICP):
             t_ref = t_model.clone()
             if normalized:
                 t_ref[:, :3, 3] *= ft
-            assert _same(T[s], t_ref.reshape(16).cpu()), \
+            assert H.same(T[s], t_ref.reshape(16).cpu()), \
                 f"tick {k} stream {s}: T differs from delora_odometry_pairs on the preprocessed lists"
             grids = []
             for pp, cc in ((p1, c1), (p2, c2)):
@@ -182,7 +174,7 @@ def _check_against_references(cfg, blob, out, pairs, normalized, flags=ICP):
                 grids.append((g_pts, g_nrm))
             row = ops.icp_dense_fwd_bwd(grids[1][0], grids[1][1], t_model.reshape(1, 16)[:, :12].contiguous(),
                                         grids[0][0], grids[0][1], h, w, hf, vf, float(cfg["lambda_po2pl"]), flags)[0][0]
-            assert _same(losses[s], row.cpu()), \
+            assert H.same(losses[s], row.cpu()), \
                 f"tick {k} stream {s}: {losses[s].tolist()} != the operator alone {row.tolist()}"
 
 
@@ -205,7 +197,7 @@ def test_rows_are_the_testers_input_and_the_operators_residual(cuda_lib, h, w, w
     for k in range(1, len(out)):
         for s in range(S):
             if not int(out[k][1][s]):
-                assert _same(out[k][0][s], out[k - 1][0][s]), f"tick {k} stream {s}: an invalid T row was written"
+                assert H.same(out[k][0][s], out[k - 1][0][s]), f"tick {k} stream {s}: an invalid T row was written"
 
 
 @pytest.mark.parametrize("normalized", [False, True], ids=["plain", "normalized"])
@@ -219,7 +211,7 @@ def test_streams_are_independent_and_the_graph_replays(cuda_lib, normalized):
                    graph=True)
     for k, (e, g) in enumerate(zip(eager, graphed)):
         for i, (a, b) in enumerate(zip(e, g)):
-            assert a is None or _same(a, b), f"tick {k}: output {i} of the replay differs from the eager call"
+            assert a is None or H.same(a, b), f"tick {k}: output {i} of the replay differs from the eager call"
     for s in range(S):
         single = [(p[s:s + 1], c[s:s + 1], a[s:s + 1]) for p, c, a in ticks]
         res = {k: [0] for k, streams in resets.items() if s in streams}
@@ -227,10 +219,10 @@ def test_streams_are_independent_and_the_graph_replays(cuda_lib, normalized):
         for k, (e, o) in enumerate(zip(eager, one)):
             assert int(e[1][s]) == int(o[1][0]), f"tick {k} stream {s}: valid differs from S = 1"
             if int(o[1][0]):
-                assert _same(e[0][s], o[0][0]), f"tick {k} stream {s}: T differs from S = 1"
-            assert _same(e[2][s], o[2][0]), f"tick {k} stream {s}: losses differ from S = 1"
+                assert H.same(e[0][s], o[0][0]), f"tick {k} stream {s}: T differs from S = 1"
+            assert H.same(e[2][s], o[2][0]), f"tick {k} stream {s}: losses differ from S = 1"
             if normalized:
-                assert _same(e[3][s], o[3][0]), f"tick {k} stream {s}: factor differs from S = 1"
+                assert H.same(e[3][s], o[3][0]), f"tick {k} stream {s}: factor differs from S = 1"
 
 
 @pytest.mark.parametrize("normalized", [False, True], ids=["plain", "normalized"])
@@ -259,7 +251,7 @@ def test_agrees_with_the_training_eval(cuda_lib, normalized):
               f"{l_err:.2e}  pairs {m_err:.2e}")
         assert t_err <= 2e-3 and l_err <= 2e-2 and m_err <= 2e-2, (t_err, l_err, m_err)
         if normalized:
-            assert _same(out[k][3][0:1], losses[0, 6:7].cpu())
+            assert H.same(out[k][3][0:1], losses[0, 6:7].cpu())
         checked += 1
     assert checked >= 2
 

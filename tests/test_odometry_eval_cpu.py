@@ -29,10 +29,6 @@ def test_symbols_exported_and_the_abi_version_stays():
     assert L.delora_abi_version() == 3
 
 
-def _align(n):
-    return (n + 255) // 256 * 256
-
-
 @pytest.mark.parametrize("h,w", [(64, 2048), (64, 720), (16, 180)])
 @pytest.mark.parametrize("S", [1, 4, 16])
 def test_residual_workspace_is_the_streams_layout_plus_the_appended_sections(h, w, S):
@@ -43,8 +39,8 @@ def test_residual_workspace_is_the_streams_layout_plus_the_appended_sections(h, 
     dp = ctypes.byref(H.desc(H.config(h, w, device="cpu"), 131072, S))
     streams = L.delora_odometry_streams_workspace_bytes(dp)
     residual = L.delora_odometry_streams_residual_workspace_bytes(dp)
-    appended = (4 * _align(S * h * w * 16) + _align(S * 12 * 4) + _align(S * 8 * 4) + _align(S * 12 * 4) +
-                _align(L.delora_icp_scratch_floats(S, h * w) * 4))
+    appended = (4 * H.align(S * h * w * 16) + H.align(S * 12 * 4) + H.align(S * 8 * 4) + H.align(S * 12 * 4) +
+                H.align(L.delora_icp_scratch_floats(S, h * w) * 4))
     assert streams > 0 and residual == streams + appended
 
 

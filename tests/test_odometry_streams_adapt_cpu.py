@@ -18,20 +18,6 @@ SYMBOLS = ("delora_odometry_streams_adapt_workspace_bytes", "delora_odometry_str
            "delora_odometry_streams_push_adapt", "delora_odometry_streams_adapt_reset")
 
 
-def _align(n):
-    return (n + 255) // 256 * 256
-
-
-def _desc(h=64, w=720, S=2, w_pre=0, n_stride=1000):
-    return H.desc(H.config(h, w, device="cpu"), n_stride, S, w_pre)
-
-
-def _hp(flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL, lr=1e-5):
-    from delora_b200 import _lib
-    return _lib.OdometryTrainParams(lr=lr, beta1=0.9, beta2=0.999, eps=1e-8, lambda_po2pl=1.0, loss_flags=flags,
-                                    nb_h=7, nb_w=11, epsilon_range=0.5, min_neighbors=10)
-
-
 def test_symbols_are_exported():
     from delora_b200 import build
     lib = ctypes.CDLL(build.LIB)
@@ -73,7 +59,7 @@ HEADER_TABLE = {(64, 720, 0, 1): (325.2, 327.3), (64, 720, 0, 4): (521.3, 529.8)
 def test_sizes_are_the_ones_the_header_documents(h, w, w_pre, S):
     from delora_b200 import _lib
     L = _lib.lib()
-    dp = ctypes.byref(_desc(h, w, S, w_pre, 131072))
+    dp = ctypes.byref(H.streams_desc(h, w, S, w_pre, 131072))
     got = (L.delora_odometry_train_workspace_bytes(dp), L.delora_odometry_streams_adapt_workspace_bytes(dp))
     mib = HEADER_TABLE[(h, w, w_pre, S)]
     assert tuple(round(b / 2 ** 20, 1) for b in got) == mib
@@ -89,14 +75,14 @@ def test_workspace_is_the_training_layout_plus_the_stream_section(h, w, w_pre, S
     count of valid pairs, each 256-byte aligned, after the training workspace (whose offsets do not move)."""
     from delora_b200 import _lib
     L = _lib.lib()
-    dp = ctypes.byref(_desc(h, w, S, w_pre))
+    dp = ctypes.byref(H.streams_desc(h, w, S, w_pre))
     train = L.delora_odometry_train_workspace_bytes(dp)
     got = L.delora_odometry_streams_adapt_workspace_bytes(dp)
     if w_pre == 0:
         cache = [S * 4 * h * w * 4, S * h * w * 16, S * h * w * 16]
     else:
         cache = [S * h * w_pre * 16, S * h * w_pre * 16]
-    want = train + sum(_align(n) for n in cache + [S * 4, 4])
+    want = train + sum(H.align(n) for n in cache + [S * 4, 4])
     assert train > 0 and got == want
     assert L.delora_odometry_train_grad_offset(dp) > 0          # the training layout is the prefix
 
@@ -104,7 +90,7 @@ def test_workspace_is_the_training_layout_plus_the_stream_section(h, w, w_pre, S
 def test_invalid_descriptors_are_refused_by_name():
     from delora_b200 import _lib
     L = _lib.lib()
-    d = _desc()
+    d = H.streams_desc()
     d.act = 0
     dp = ctypes.byref(d)
     assert L.delora_odometry_streams_adapt_workspace_bytes(dp) == -1
@@ -115,7 +101,7 @@ def test_invalid_descriptors_are_refused_by_name():
     assert b"delora_odometry_streams_adapt_reset: act=0" in L.delora_last_error()
     rc, err = _push(desc=d)
     assert rc != 0 and f"{NAME}: act=0".encode() in err, err
-    d = _desc(w_pre=1)
+    d = H.streams_desc(w_pre=1)
     assert L.delora_odometry_streams_adapt_workspace_bytes(ctypes.byref(d)) == -1
     assert b"w_pre=1" in L.delora_last_error()
     assert L.delora_odometry_streams_adapt_workspace_bytes(None) == -1
@@ -125,7 +111,7 @@ def test_invalid_descriptors_are_refused_by_name():
 def test_reset_refuses_null_pointers_by_name():
     from delora_b200 import _lib
     L = _lib.lib()
-    dp = ctypes.byref(_desc())
+    dp = ctypes.byref(H.streams_desc())
     assert L.delora_odometry_streams_adapt_reset(dp, None, 32, None) != 0
     assert b"delora_odometry_streams_adapt_reset: null mask" in L.delora_last_error()
     assert L.delora_odometry_streams_adapt_reset(dp, 16, None, None) != 0
@@ -139,8 +125,8 @@ def _push(hp=None, update=1, desc=None, **null):
     L = _lib.lib()
     args = {"points": 16, "n_points": 32, "workspace": 48, "T": 64, "valid": 80, "losses": 96}
     args.update(null)
-    rc = L.delora_odometry_streams_push_adapt(ctypes.byref(desc or _desc()),
-                                              None if hp is False else ctypes.byref(hp or _hp()), update,
+    rc = L.delora_odometry_streams_push_adapt(ctypes.byref(desc or H.streams_desc()),
+                                              None if hp is False else ctypes.byref(hp or H.train_params()), update,
                                               args["points"], args["n_points"], None, args["workspace"], args["T"],
                                               args["valid"], args["losses"], None)
     return rc, L.delora_last_error()
@@ -161,7 +147,7 @@ def test_push_refuses_update_by_name(update):
 @pytest.mark.parametrize("flag,what", [(ops.LOSS_IDENTITY_FIT, b"DELORA_LOSS_IDENTITY_FIT"),
                                        (ops.TRAIN_DROPOUT, b"DELORA_TRAIN_DROPOUT")])
 def test_push_refuses_identity_fit_and_dropout_by_name(flag, what):
-    rc, err = _push(hp=_hp(ops.LOSS_PO2PL | flag))
+    rc, err = _push(hp=H.train_params(ops.LOSS_PO2PL | flag))
     assert rc != 0 and NAME.encode() in err and what in err and b"loss_flags=" in err, err
 
 
@@ -170,14 +156,14 @@ def test_push_refuses_what_the_training_step_refuses():
     assert rc != 0 and f"{NAME}: null hyperparameters".encode() in err, err
     for field, value in (("lr", -1.0), ("beta1", 1.0), ("eps", 0.0), ("nb_h", 6), ("min_neighbors", -1),
                          ("lambda_po2pl", float("nan"))):
-        hp = _hp()
+        hp = H.train_params()
         setattr(hp, field, value)
         rc, err = _push(hp=hp)
         assert rc != 0 and f"{NAME}: {field}=".encode() in err, (field, err)
-    rc, err = _push(hp=_hp(ops.NORMAL_LINEAR))
+    rc, err = _push(hp=H.train_params(ops.NORMAL_LINEAR))
     assert rc != 0 and b"sets no loss bit" in err, err
     # normalization_scaling needs the recipe's w_pre
-    rc, err = _push(hp=_hp(ops.LOSS_PO2PL | ops.TRAIN_NORMALIZATION_SCALING))
+    rc, err = _push(hp=H.train_params(ops.LOSS_PO2PL | ops.TRAIN_NORMALIZATION_SCALING))
     assert rc != 0 and f"{NAME}: DELORA_TRAIN_NORMALIZATION_SCALING needs w_pre > 0".encode() in err, err
 
 

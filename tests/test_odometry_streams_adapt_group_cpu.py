@@ -26,16 +26,6 @@ def _lib():
     return _lib, _lib.lib()
 
 
-def _desc(h=64, w=720, S=2, w_pre=0, n_stride=1000):
-    return H.desc(H.config(h, w, device="cpu"), n_stride, S, w_pre)
-
-
-def _hp(flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL, lr=1e-5):
-    _l, _ = _lib()
-    return _l.OdometryTrainParams(lr=lr, beta1=0.9, beta2=0.999, eps=1e-8, lambda_po2pl=1.0, loss_flags=flags,
-                                  nb_h=7, nb_w=11, epsilon_range=0.5, min_neighbors=10)
-
-
 def _group(world=2, rank=0, ws=48):
     _l, _ = _lib()
     g = _l.OdometryTrainGroup(rank=rank, world=world, multicast=0, n_ctas=8, n_threads=128, status=DUMMY,
@@ -64,8 +54,8 @@ def _push(g=None, hp=None, update=1, desc=None, **null):
     args = {"points": 16, "n_points": 32, "workspace": 48, "T": 64, "valid": 80, "losses": 96}
     args.update(null)
     g = _group() if g is None else g
-    rc = L.delora_odometry_streams_push_adapt_group(ctypes.byref(desc or _desc()),
-                                                    None if hp is False else ctypes.byref(hp or _hp()),
+    rc = L.delora_odometry_streams_push_adapt_group(ctypes.byref(desc or H.streams_desc()),
+                                                    None if hp is False else ctypes.byref(hp or H.train_params()),
                                                     None if g is False else ctypes.byref(g), update, args["points"],
                                                     args["n_points"], None, args["workspace"], args["T"],
                                                     args["valid"], args["losses"], None)
@@ -102,7 +92,7 @@ def test_header_compiles_as_c(tmp_path):
 @pytest.mark.parametrize("h,w,w_pre", [(64, 720, 0), (64, 720, 2250), (16, 180, 360), (16, 259, 100), (16, 180, 0)])
 def test_group_workspace_is_the_adapting_layout_plus_the_group_section(h, w, w_pre, S):
     _, L = _lib()
-    dp = ctypes.byref(_desc(h, w, S, w_pre))
+    dp = ctypes.byref(H.streams_desc(h, w, S, w_pre))
     adapt = L.delora_odometry_streams_adapt_workspace_bytes(dp)
     train = L.delora_odometry_train_workspace_bytes(dp)
     assert adapt > train > 0
@@ -113,13 +103,13 @@ def test_group_workspace_is_the_adapting_layout_plus_the_group_section(h, w, w_p
                                              (64, 2048, 0, 16, 3006.6)])
 def test_the_adapting_size_is_unchanged(h, w, w_pre, S, mib):
     _, L = _lib()
-    dp = ctypes.byref(_desc(h, w, S, w_pre, 131072))
+    dp = ctypes.byref(H.streams_desc(h, w, S, w_pre, 131072))
     assert round(L.delora_odometry_streams_adapt_workspace_bytes(dp) / 2 ** 20, 1) == mib
 
 
 def test_invalid_descriptors_are_refused_by_name():
     _, L = _lib()
-    d = _desc()
+    d = H.streams_desc()
     d.act = 0
     dp = ctypes.byref(d)
     assert L.delora_odometry_streams_adapt_group_workspace_bytes(dp) == -1
@@ -134,7 +124,7 @@ def test_invalid_descriptors_are_refused_by_name():
 
 def test_init_refuses_null_pointers():
     _, L = _lib()
-    assert L.delora_odometry_streams_adapt_group_init(ctypes.byref(_desc()), None, 32, None) != 0
+    assert L.delora_odometry_streams_adapt_group_init(ctypes.byref(H.streams_desc()), None, 32, None) != 0
     assert b"delora_odometry_streams_adapt_group_init: null pointer" in L.delora_last_error()
 
 
@@ -153,18 +143,18 @@ def test_push_refuses_update_by_name(update):
 @pytest.mark.parametrize("flag,what", [(ops.LOSS_IDENTITY_FIT, b"DELORA_LOSS_IDENTITY_FIT"),
                                        (ops.TRAIN_DROPOUT, b"DELORA_TRAIN_DROPOUT")])
 def test_push_refuses_identity_fit_and_dropout_by_name(flag, what):
-    rc, err = _push(hp=_hp(ops.LOSS_PO2PL | flag))
+    rc, err = _push(hp=H.train_params(ops.LOSS_PO2PL | flag))
     assert rc != 0 and NAME.encode() in err and what in err and b"loss_flags=" in err, err
 
 
 def test_push_refuses_what_the_training_step_refuses():
     rc, err = _push(hp=False)
     assert rc != 0 and f"{NAME}: null hyperparameters".encode() in err, err
-    hp = _hp()
+    hp = H.train_params()
     hp.eps = 0.0
     rc, err = _push(hp=hp)
     assert rc != 0 and f"{NAME}: eps=".encode() in err, err
-    rc, err = _push(hp=_hp(ops.LOSS_PO2PL | ops.TRAIN_NORMALIZATION_SCALING))
+    rc, err = _push(hp=H.train_params(ops.LOSS_PO2PL | ops.TRAIN_NORMALIZATION_SCALING))
     assert rc != 0 and f"{NAME}: DELORA_TRAIN_NORMALIZATION_SCALING needs w_pre > 0".encode() in err, err
 
 

@@ -14,10 +14,6 @@ SYMBOLS = ("delora_odometry_streams_normalized_workspace_bytes", "delora_odometr
            "delora_odometry_streams_push_normalized")
 
 
-def _align(n):
-    return (n + 255) // 256 * 256
-
-
 def _cfg(h=64, w=720, normalized=True):
     cfg = H.config(h, w, device="cpu")
     cfg["normalization_scaling"] = normalized
@@ -64,7 +60,7 @@ def test_workspace_is_the_streams_layout_plus_the_appended_sections(h, w, S):
         streams = L.delora_odometry_streams_workspace_bytes(dp)
         got = L.delora_odometry_streams_normalized_workspace_bytes(dp)
         assert streams > 0
-        assert got == streams + _align(2 * S * 3 * n_stride * 4) + _align(3 * S * 4) + _align(S * 4), (n_stride, got)
+        assert got == streams + H.align(2 * S * 3 * n_stride * 4) + H.align(3 * S * 4) + H.align(S * 4), (n_stride, got)
 
 
 def test_invalid_descriptors_are_refused():

@@ -15,10 +15,6 @@ from helpers import ROOT
 NAME = "delora_odometry_streams_push_pre"
 
 
-def _align(n):
-    return (n + 255) // 256 * 256
-
-
 def _desc(h=64, w=720, S=2, w_pre=2250, n_stride=1000):
     return H.desc(H.config(h, w, device="cpu"), n_stride, S, w_pre)
 
@@ -79,7 +75,7 @@ def test_workspace_is_the_residual_layout_plus_the_appended_sections(h, w, w_pre
     residual = L.delora_odometry_streams_residual_workspace_bytes(dp)
     got = L.delora_odometry_streams_pre_workspace_bytes(dp)
     hwp = h * w_pre
-    want = residual + sum(_align(n) for n in (S * hwp * 8, S * 4 * hwp * 4, S * hwp * 4, 2 * S * hwp * 16,
+    want = residual + sum(H.align(n) for n in (S * hwp * 8, S * 4 * hwp * 4, S * hwp * 4, 2 * S * hwp * 16,
                                                2 * S * hwp * 16, S * 16 * 4, S * 4))
     assert residual > 0 and got == want
 
