@@ -4,8 +4,8 @@
 // and returns (u, v) and the surviving point indices in that order (:105-106).  The projection
 // itself does not need the order (see projection.cu); this sort exists so that the drop-in
 // ImageProjectionLayer can hand back the reference-shaped, range-ordered outputs.  Stable LSD
-// passes over the 32 float bits leave equal ranges in index order, i.e. the deterministic
-// version of the reference's unstable argsort.
+// passes over the 32 bits of sort_key_bits leave equal ranges in index order, i.e. the deterministic
+// version of the reference's unstable argsort: torch.argsort(range, stable=True), on any fp32 keys.
 //
 // Per 8-bit pass: tile histograms -> per-digit exclusive scan over tiles -> stable scatter
 // (warp `match_any` ranking).  Integer work, bound by L2/HBM bandwidth: 16 B moved per key and pass.
@@ -18,8 +18,14 @@ constexpr int kSortWarps = kSortThreads / 32;
 constexpr int kSortItersPerWarp = 8;
 constexpr int kSortTile = kSortThreads * kSortItersPerWarp;   // 2048 keys per block
 
+// The radix key of a range, in torch.argsort's order: -0 is +0, every NaN (either sign, any payload) is one key above
+// +inf, and the sign flip (negative: all bits inverted; otherwise: the sign bit set) makes the unsigned order the
+// order of the values.  Both first passes read keys through here only.
 __device__ __forceinline__ unsigned sort_key_bits(const float* __restrict__ rng, int i) {
-    return __float_as_uint(__ldg(rng + i));
+    unsigned b = __float_as_uint(__ldg(rng + i));
+    if ((b & 0x7fffffffu) > 0x7f800000u) return 0xffffffffu;
+    if (b == 0x80000000u) b = 0u;
+    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
 
 template <bool FIRST>

@@ -86,7 +86,8 @@ int delora_project_uv(const float* points, const int32_t* n_points, int B, int C
 /* Stable ascending sort of each scan's points by fp32 range (ties: lower index first):
  * the order `torch.argsort(range)` imposes in src/utility/projection.py:63-67, made
  * deterministic.  LSD radix sort, 4 passes of 8 bits, one launch set for the batch.
- * range      [B, n_stride] fp32 (non-negative; NaN sorts last)
+ * range      [B, n_stride] fp32, any values: ordered as torch.argsort(stable=True) orders them
+ *            (-0 equals +0, every NaN sorts last in index order)
  * order      [B, n_stride] int32 out: point indices in ascending (range, index) order
  * scratch    bytes >= delora_sort_scratch_bytes(B, n_stride)
  */
