@@ -15,6 +15,8 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <memory>
+
 #include "common.cuh"
 #include "dropout.cuh"
 #include "projection.cuh"
@@ -1530,12 +1532,45 @@ odometry_out_bwd_kernel(OutBwd a, int B, float inv_B, int act) {
     }
 }
 
+// The gradient slices of geometries 1 .. n of delora_odometry_streams_push_adapt_geometries (blob layout each)
+constexpr int kMaxGeometries = 16;
+struct GradSlices {
+    const float* g[kMaxGeometries - 1];
+    int n;
+};
+
+// The gradient Adam reads at float4 i (or float i): g's, or with kSum g + more.g[0] + ... + more.g[n-1] in that order,
+// which is written back to g
+template <bool kSum>
+__device__ __forceinline__ float4 adam_grad4(float* __restrict__ g, const GradSlices& more, long long i) {
+    if (!kSum) return __ldg(reinterpret_cast<const float4*>(g) + i);
+    float4 a = reinterpret_cast<const float4*>(g)[i];
+    for (int k = 0; k < more.n; ++k) {
+        const float4 b = __ldg(reinterpret_cast<const float4*>(more.g[k]) + i);
+        a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
+    }
+    reinterpret_cast<float4*>(g)[i] = a;
+    return a;
+}
+
+template <bool kSum>
+__device__ __forceinline__ float adam_grad1(float* __restrict__ g, const GradSlices& more, long long i) {
+    if (!kSum) return g[i];
+    float a = g[i];
+    for (int k = 0; k < more.n; ++k) a += more.g[k][i];
+    g[i] = a;
+    return a;
+}
+
 // torch.optim.Adam (the fused implementation's formula; no weight decay, no amsgrad) on n floats.  run (device, or
 // NULL for always): the update runs only where *run != 0 (the adapting streams' count of valid pairs).
+// kSum (delora_odometry_streams_push_adapt_geometries): the gradient is g plus the slices of `more`, summed per float
+// in geometry order and written back to g before the update.
+template <bool kSum>
 __global__ void __launch_bounds__(256)
-odometry_adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
+odometry_adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
                      long long n, const long long* __restrict__ ctr, float lr, float beta1, float beta2, float eps,
-                     const int32_t* __restrict__ run) {
+                     const int32_t* __restrict__ run, const __grid_constant__ GradSlices more) {
     if (run && *run == 0) return;                           // run non-NULL: update only when *run != 0
     const float t = (float)ctr[0];
     const float bc1 = 1.0f - powf(beta1, t);
@@ -1551,7 +1586,7 @@ odometry_adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* 
     const long long stride = (long long)gridDim.x * blockDim.x;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += stride) {
         float4 pp = reinterpret_cast<float4*>(p)[i];
-        const float4 gg = __ldg(reinterpret_cast<const float4*>(g) + i);
+        const float4 gg = adam_grad4<kSum>(g, more, i);
         float4 mm = reinterpret_cast<float4*>(m)[i];
         float4 vv = reinterpret_cast<float4*>(v)[i];
         upd(pp.x, gg.x, mm.x, vv.x); upd(pp.y, gg.y, mm.y, vv.y);
@@ -1562,7 +1597,7 @@ odometry_adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* 
     }
     if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
         const long long i = n4 * 4 + threadIdx.x;
-        upd(p[i], g[i], m[i], v[i]);
+        upd(p[i], adam_grad1<kSum>(g, more, i), m[i], v[i]);
     }
 }
 
@@ -1605,7 +1640,9 @@ struct TrainPlan {
 // first and depends only on act, layers, resnet_outputs, single_mlp and the parity of W (the stem's filter layout).
 // The geometry section (frames, grids, ICP scratch, activations, tail buffers, the w_pre buffers) starts at f.keys.
 // delora_odometry_train_geometries_* rely on this split: one model section serves several geometry sections.
-static void make_train_plan(const delora_odometry_desc* d, TrainPlan* tp) {
+// geometry_at > 0: the geometry section starts at that byte offset instead (delora_odometry_streams_*_geometries: one
+// model section and one geometry section per descriptor, each further one after the previous geometry's sections).
+static void make_train_plan(const delora_odometry_desc* d, TrainPlan* tp, size_t geometry_at = 0) {
     memset(tp, 0, sizeof(TrainPlan));
     plan_model(d, &tp->m);
     const Model& m = tp->m;
@@ -1616,6 +1653,7 @@ static void make_train_plan(const delora_odometry_desc* d, TrainPlan* tp) {
     // [0] Adam's step count, [1] the ICP scratch's batch size, [2] the dropout seed (the slot has 256 bytes)
     tp->ctr = take(off, 3 * sizeof(long long));
     tp->w = plan_trunk_weights(m.t, true, off);
+    if (geometry_at) off = geometry_at;
     // one key buffer serves both projections of a step, one after the other
     tp->f = plan_frames(d, 2 * MB, 0, false, d->w_pre > W ? d->w_pre : W, off);
     tp->pts_grid = take(off, (size_t)2 * MB * HW * 16);
@@ -2075,16 +2113,20 @@ static int check_group(const delora_odometry_train_group* g, const void* workspa
 }
 
 // Stage 5 of the step: Adam on the master blob (only where *run != 0, run non-NULL), then the bf16 filters from the
-// master weights
+// master weights.  more (n > 0): Adam reads tp.grad plus those gradient slices and leaves their sum in tp.grad.
 static int adam_update(const TrainPlan& tp, char* ws, const delora_odometry_train_params* hp, const int32_t* run,
-                       cudaStream_t st) {
+                       cudaStream_t st, const GradSlices* more = nullptr) {
     auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
     const long long n = tp.m.blob_floats;
     const long long blocks = (n / 4 + 255) / 256;
     const int grid = (int)(blocks < 8ll * num_sms() ? (blocks > 0 ? blocks : 1) : 8ll * num_sms());
-    odometry_adam_kernel<<<grid, 256, 0, st>>>(f(tp.master), f(tp.grad), f(tp.adam_m), f(tp.adam_v), n,
-                                               reinterpret_cast<const long long*>(ws + tp.ctr), hp->lr, hp->beta1,
-                                               hp->beta2, hp->eps, run);
+    const long long* ctr = reinterpret_cast<const long long*>(ws + tp.ctr);
+    if (more && more->n > 0)
+        odometry_adam_kernel<true><<<grid, 256, 0, st>>>(f(tp.master), f(tp.grad), f(tp.adam_m), f(tp.adam_v), n, ctr,
+                                                         hp->lr, hp->beta1, hp->beta2, hp->eps, run, *more);
+    else
+        odometry_adam_kernel<false><<<grid, 256, 0, st>>>(f(tp.master), f(tp.grad), f(tp.adam_m), f(tp.adam_v), n, ctr,
+                                                          hp->lr, hp->beta1, hp->beta2, hp->eps, run, GradSlices{});
     DELORA_CHECK_LAUNCH("odometry_adam_kernel");
     return delora_conv_weight_prep_multi(ws + tp.w.table, tp.m.t.n_conv, st);
 }
@@ -2316,8 +2358,9 @@ struct AdaptPlan {
     size_t group_total;
 };
 
-static void make_adapt_plan(const delora_odometry_desc* d, TrainPlan* tp, AdaptPlan* ap) {
-    make_train_plan(d, tp);
+// geometry_at: see make_train_plan; the stream section follows the geometry section wherever that starts
+static void make_adapt_plan(const delora_odometry_desc* d, TrainPlan* tp, AdaptPlan* ap, size_t geometry_at = 0) {
+    make_train_plan(d, tp, geometry_at);
     memset(ap, 0, sizeof(AdaptPlan));
     const size_t S = (size_t)d->max_batch, HW = (size_t)d->H * d->W;
     size_t off = tp->total;
@@ -2359,11 +2402,8 @@ static int adapt_init(const delora_odometry_desc* d, bool group, const float* we
     return group ? collective_kernels_preload(who) : 0;
 }
 
-// What _push_adapt and _push_adapt_group refuse alike
-static int check_push_adapt(const delora_odometry_desc* d, const delora_odometry_train_params* hp, int update,
-                            const float* points, const int32_t* n_points, void* workspace, float* T, int32_t* valid,
-                            float* losses, const char* who) {
-    if (check_train_desc(d, who)) return 1;
+// The hyperparameters and update value every adapting tick refuses alike
+static int check_adapt_params(const delora_odometry_train_params* hp, int update, const char* who) {
     if (check_train_params(hp, who)) return 1;
     DELORA_CHECK_ARG(update == 0 || update == 1, "%s: update=%d must be 0 or 1", who, update);
     DELORA_CHECK_ARG((hp->loss_flags & DELORA_LOSS_IDENTITY_FIT) == 0u,
@@ -2372,8 +2412,46 @@ static int check_push_adapt(const delora_odometry_desc* d, const delora_odometry
     DELORA_CHECK_ARG((hp->loss_flags & DELORA_TRAIN_DROPOUT) == 0u,
                      "%s: loss_flags=0x%x has DELORA_TRAIN_DROPOUT: the served T is dropout-free, and one forward "
                      "cannot be both", who, hp->loss_flags);
+    return 0;
+}
+
+// What _push_adapt and _push_adapt_group refuse alike
+static int check_push_adapt(const delora_odometry_desc* d, const delora_odometry_train_params* hp, int update,
+                            const float* points, const int32_t* n_points, void* workspace, float* T, int32_t* valid,
+                            float* losses, const char* who) {
+    if (check_train_desc(d, who)) return 1;
+    if (check_adapt_params(hp, update, who)) return 1;
     if (check_tick(points, n_points, workspace, T, valid, losses, "losses", who)) return 1;
     return check_train_call(d, hp, points, n_points, d->max_batch, workspace, who);
+}
+
+// Stages 1-3 of one adapting tick of the S = d->max_batch streams of (tp, ap): T, valid, the loss rows and the cache
+// write; update = 0 then records the ICP scratch's batch marker
+static int serve_adapt(const delora_odometry_desc* d, const delora_odometry_train_params* hp, const TrainPlan& tp,
+                       const AdaptPlan& ap, int update, const float* points, const int32_t* n_points,
+                       const int32_t* active, char* ws, float* T, int32_t* valid, float* losses, cudaStream_t st,
+                       const char* who) {
+    const int S = d->max_batch;
+    auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
+    AdaptTick at;
+    at.active = active;
+    at.T = T;
+    at.valid = valid;
+    at.has_prev = reinterpret_cast<int32_t*>(ws + ap.has_prev);
+    at.n_valid = reinterpret_cast<int32_t*>(ws + ap.n_valid);
+    at.cache_image = d->w_pre == 0 ? f(ap.cache_image) : nullptr;
+    at.cache_pts = reinterpret_cast<delora_f4*>(ws + ap.cache_pts);
+    at.cache_nrm = reinterpret_cast<delora_f4*>(ws + ap.cache_nrm);
+    int rc;
+    // 1-3 at B = S, the first frame of every pair from the cache; T, valid, the cache and the emptied sources
+    if ((rc = train_forward_losses(d, hp, tp, ws, points, n_points, S, false, nullptr, st, who, &at))) return rc;
+    odometry_streams_losses_kernel<<<(S * DELORA_LOSS_ROW + 255) / 256, 256, 0, st>>>(valid, S, f(tp.losses), losses);
+    DELORA_CHECK_LAUNCH("odometry_streams_losses_kernel");
+    if (!update) {          // the ICP scratch now has the layout of S pairs, as after _train_eval
+        odometry_icp_batch_kernel<<<1, 1, 0, st>>>(reinterpret_cast<long long*>(ws + tp.ctr), S);
+        DELORA_CHECK_LAUNCH("odometry_icp_batch_kernel");
+    }
+    return 0;
 }
 
 // One tick of _push_adapt, and with g (world > 1, update = 1) of its group form: the count of valid pairs is
@@ -2391,35 +2469,17 @@ static int push_adapt(const delora_odometry_desc* d, const delora_odometry_train
     make_adapt_plan(d, &tp, &ap);
     cudaStream_t st = (cudaStream_t)stream;
     char* ws = (char*)workspace;
-    auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
-    AdaptTick at;
-    at.active = active;
-    at.T = T;
-    at.valid = valid;
-    at.has_prev = reinterpret_cast<int32_t*>(ws + ap.has_prev);
-    at.n_valid = reinterpret_cast<int32_t*>(ws + ap.n_valid);
-    at.cache_image = d->w_pre == 0 ? f(ap.cache_image) : nullptr;
-    at.cache_pts = reinterpret_cast<delora_f4*>(ws + ap.cache_pts);
-    at.cache_nrm = reinterpret_cast<delora_f4*>(ws + ap.cache_nrm);
     int rc;
-    // 1-3 at B = S, the first frame of every pair from the cache; T, valid, the cache and the emptied sources
-    if ((rc = train_forward_losses(d, hp, tp, ws, points, n_points, S, false, nullptr, st, who, &at))) return rc;
-    odometry_streams_losses_kernel<<<(S * DELORA_LOSS_ROW + 255) / 256, 256, 0, st>>>(valid, S, f(tp.losses), losses);
-    DELORA_CHECK_LAUNCH("odometry_streams_losses_kernel");
-    long long* ctr = reinterpret_cast<long long*>(ws + tp.ctr);
-    if (!update) {          // the ICP scratch now has the layout of S pairs, as after _train_eval
-        odometry_icp_batch_kernel<<<1, 1, 0, st>>>(ctr, S);
-        DELORA_CHECK_LAUNCH("odometry_icp_batch_kernel");
-        return 0;
-    }
-    const int32_t* n_valid = at.n_valid;
+    if ((rc = serve_adapt(d, hp, tp, ap, update, points, n_points, active, ws, T, valid, losses, st, who))) return rc;
+    if (!update) return 0;
+    const int32_t* n_valid = reinterpret_cast<const int32_t*>(ws + ap.n_valid);
     long long* tick = reinterpret_cast<long long*>(ws + ap.tick);
     constexpr unsigned kSeqStride = kGroupBuckets + 1;
     if (g) {                // the fleet-wide count of valid pairs, on every rank before its backward
         uint64_t peer_slots[kArMaxWorld];
         for (int q = 0; q < g->world; ++q) peer_slots[q] = g->peer_ws[q] + ap.slots;
         int32_t* n_fleet = reinterpret_cast<int32_t*>(ws + ap.n_fleet);
-        if ((rc = count_allreduce_launch(peer_slots, g->peer_flags, g->rank, g->world, kSeqStride, tick, at.n_valid,
+        if ((rc = count_allreduce_launch(peer_slots, g->peer_flags, g->rank, g->world, kSeqStride, tick, n_valid,
                                          n_fleet, g->status, st))) return rc;
         n_valid = n_fleet;
     }
@@ -2481,6 +2541,167 @@ extern "C" int delora_odometry_streams_adapt_reset(const delora_odometry_desc* d
     AdaptPlan ap;
     make_adapt_plan(d, &tp, &ap);
     return reset_streams(d, mask, workspace, ap.has_prev, stream, who);
+}
+
+// ================================================================================================ adapting streams of
+// several sensor geometries
+// delora_odometry_streams_push_adapt_geometries: one model adapted from the streams of n geometries in one workspace.
+// Layout: the adapting-streams workspace of d[0], unchanged; then for g = 1 .. n-1 d[g]'s geometry section (its
+// training plan with the geometry section at the running offset), its stream section and one gradient slice in blob
+// layout; then, for n > 1, the fleet section: the count of valid pairs over every geometry (int32 at +0) and geometry
+// g's counters at +8 + 24 (g - 1), in the layout of the model section's (int64 [3]: a backward count nothing reads,
+// the batch marker of g's ICP scratch, unused).  Geometry g's plan keeps d[0]'s model-section offsets (check_geometries
+// makes them equal) with grad and ctr moved to its slice and counters, so train_forward_losses and step_backward run
+// on it unchanged, and geometry 0's plan is _push_adapt's.
+namespace delora {
+
+struct GeometriesPlan {
+    TrainPlan tp[kMaxGeometries];
+    AdaptPlan ap[kMaxGeometries];
+    int row[kMaxGeometries];           // the first stream of geometry g in the caller's arrays
+    size_t fleet;                      // n > 1 only
+    size_t total;
+};
+
+// TrainPlan is large (the trunk plan's tables): the plans of up to kMaxGeometries geometries go on the heap
+static std::unique_ptr<GeometriesPlan> make_geometries_plan(const delora_odometry_desc* d, int n) {
+    std::unique_ptr<GeometriesPlan> p(new GeometriesPlan);
+    make_adapt_plan(&d[0], &p->tp[0], &p->ap[0]);
+    size_t off = p->ap[0].total;
+    p->row[0] = 0;
+    for (int g = 1; g < n; ++g) {
+        make_adapt_plan(&d[g], &p->tp[g], &p->ap[g], off);
+        off = p->ap[g].total;
+        p->tp[g].grad = take(off, (size_t)p->tp[g].m.blob_floats * 4);
+        p->row[g] = p->row[g - 1] + d[g - 1].max_batch;
+    }
+    p->fleet = 0;
+    if (n > 1) {
+        p->fleet = take(off, 8 + 24 * (size_t)(n - 1));
+        for (int g = 1; g < n; ++g) p->tp[g].ctr = p->fleet + 8 + 24 * (size_t)(g - 1);
+    }
+    p->total = off;
+    return p;
+}
+
+static int check_adapt_geometries(const delora_odometry_desc* d, int n, const char* who) {
+    DELORA_CHECK_ARG(n <= kMaxGeometries, "%s: n=%d must be <= %d", who, n, kMaxGeometries);
+    return check_geometries(d, n, who);
+}
+
+struct FleetCounts {
+    const int32_t* n_valid[kMaxGeometries];
+    int n;
+};
+
+// *fleet = the sum of every geometry's count of valid pairs, in geometry order
+__global__ void odometry_fleet_count_kernel(FleetCounts c, int32_t* __restrict__ fleet) {
+    int s = 0;
+    for (int g = 0; g < c.n; ++g) s += *c.n_valid[g];
+    *fleet = s;
+}
+
+static int push_adapt_geometries(const delora_odometry_desc* d, int n, const delora_odometry_train_params* hp,
+                                 int update, const float* const* points, const int32_t* const* n_points,
+                                 const int32_t* active, void* workspace, float* T, int32_t* valid, float* losses,
+                                 void* stream, const char* who) {
+    const std::unique_ptr<GeometriesPlan> p = make_geometries_plan(d, n);
+    cudaStream_t st = (cudaStream_t)stream;
+    char* ws = (char*)workspace;
+    int rc;
+    // 1-3 per geometry at B = S_g into its rows of the caller's arrays
+    for (int g = 0; g < n; ++g) {
+        const int r = p->row[g];
+        if ((rc = serve_adapt(&d[g], hp, p->tp[g], p->ap[g], update, points[g], n_points[g], active ? active + r : nullptr,
+                              ws, T + (size_t)r * 16, valid + r, losses + (size_t)r * DELORA_LOSS_ROW, st, who)))
+            return rc;
+    }
+    if (!update) return 0;
+    // 4. every geometry's backward divides by the fleet's count of valid pairs, geometry g >= 1 into its slice; Adam
+    // sums the slices into the model's gradient section
+    const int32_t* fleet = reinterpret_cast<const int32_t*>(ws + p->ap[0].n_valid);
+    GradSlices more;
+    memset(&more, 0, sizeof(more));
+    if (n > 1) {
+        FleetCounts c;
+        memset(&c, 0, sizeof(c));
+        c.n = n;
+        for (int g = 0; g < n; ++g) c.n_valid[g] = reinterpret_cast<const int32_t*>(ws + p->ap[g].n_valid);
+        odometry_fleet_count_kernel<<<1, 1, 0, st>>>(c, reinterpret_cast<int32_t*>(ws + p->fleet));
+        DELORA_CHECK_LAUNCH("odometry_fleet_count_kernel");
+        fleet = reinterpret_cast<const int32_t*>(ws + p->fleet);
+        more.n = n - 1;
+        for (int g = 1; g < n; ++g) more.g[g - 1] = reinterpret_cast<const float*>(ws + p->tp[g].grad);
+    }
+    for (int g = 0; g < n; ++g)
+        if ((rc = step_backward(p->tp[g], ws, d[g].act, d[g].max_batch, false, DropoutCtr{nullptr, 0}, valid + p->row[g],
+                                fleet, nullptr, st, who))) return rc;
+    return adam_update(p->tp[0], ws, hp, fleet, st, &more);
+}
+
+}  // namespace delora
+
+extern "C" int64_t delora_odometry_streams_adapt_geometries_workspace_bytes(const delora_odometry_desc* d, int n) {
+    if (check_adapt_geometries(d, n, "delora_odometry_streams_adapt_geometries_workspace_bytes")) return -1;
+    return (int64_t)make_geometries_plan(d, n)->total;
+}
+
+extern "C" int delora_odometry_streams_adapt_geometries_init(const delora_odometry_desc* d, int n, const float* weights,
+                                                             void* workspace, void* stream) {
+    const char* who = "delora_odometry_streams_adapt_geometries_init";
+    if (check_adapt_geometries(d, n, who)) return 1;
+    const std::unique_ptr<GeometriesPlan> p = make_geometries_plan(d, n);
+    cudaStream_t st = (cudaStream_t)stream;
+    char* ws = (char*)workspace;
+    // _train_init over the whole workspace arms geometry 0 and zeroes every other section
+    int rc = train_init(&d[0], p->total, weights, workspace, st, who);
+    if (rc) return rc;
+    for (int g = 0; g < n; ++g) {
+        const AdaptPlan& ap = p->ap[g];
+        if ((rc = clear_grids(ws, ap.cache_pts, ap.cache_nrm, (size_t)d[g].max_batch * ap.cache_cells, st))) return rc;
+        if (g == 0) continue;
+        const cudaError_t e = cudaMemsetAsync(ws + p->tp[g].f.keys, 0xFF, p->tp[g].f.keys_bytes, st);
+        DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
+    }
+    return 0;
+}
+
+extern "C" int delora_odometry_streams_push_adapt_geometries(const delora_odometry_desc* d, int n,
+                                                             const delora_odometry_train_params* hp, int update,
+                                                             const float* const* points,
+                                                             const int32_t* const* n_points, const int32_t* active,
+                                                             void* workspace, float* T, int32_t* valid, float* losses,
+                                                             void* stream) {
+    const char* who = "delora_odometry_streams_push_adapt_geometries";
+    if (check_adapt_geometries(d, n, who)) return 1;
+    if (check_adapt_params(hp, update, who)) return 1;
+    DELORA_CHECK_ARG(points, "%s: null points", who);
+    DELORA_CHECK_ARG(n_points, "%s: null n_points", who);
+    DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
+    DELORA_CHECK_ARG(T, "%s: null T", who);
+    DELORA_CHECK_ARG(valid, "%s: null valid", who);
+    DELORA_CHECK_ARG(losses, "%s: null losses", who);
+    for (int g = 0; g < n; ++g) {
+        DELORA_CHECK_ARG(points[g], "%s: points[%d] is null", who, g);
+        DELORA_CHECK_ARG(n_points[g], "%s: n_points[%d] is null", who, g);
+        char w[192];
+        snprintf(w, sizeof w, "%s: d[%d]", who, g);
+        if (check_train_call(&d[g], hp, points[g], n_points[g], d[g].max_batch, workspace, w)) return 1;
+    }
+    return push_adapt_geometries(d, n, hp, update, points, n_points, active, workspace, T, valid, losses, stream, who);
+}
+
+extern "C" int delora_odometry_streams_adapt_geometries_reset(const delora_odometry_desc* d, int n, const int32_t* mask,
+                                                              void* workspace, void* stream) {
+    const char* who = "delora_odometry_streams_adapt_geometries_reset";
+    if (check_adapt_geometries(d, n, who)) return 1;
+    DELORA_CHECK_ARG(mask, "%s: null mask", who);
+    const std::unique_ptr<GeometriesPlan> p = make_geometries_plan(d, n);
+    for (int g = 0; g < n; ++g) {
+        const int rc = reset_streams(&d[g], mask + p->row[g], workspace, p->ap[g].has_prev, stream, who);
+        if (rc) return rc;
+    }
+    return 0;
 }
 
 // ================================================================================================ dropout

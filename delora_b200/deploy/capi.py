@@ -332,6 +332,59 @@ class GeometriesTrainingWorkspace(TrainingWorkspace):
         self._dp = ctypes.byref(self.desc)
 
 
+class GeometriesAdaptingStreamsWorkspace(TrainingWorkspace):
+    """delora_odometry_streams_adapt_geometries_*: one model adapted from the streams of several sensor geometries in
+    one workspace.  Geometry g serves descs[g].max_batch streams; streams are numbered in geometry order
+    (`n_streams` in all).  Every TrainingWorkspace call runs with descs[0] (weights, get_state / set_state) and leaves
+    the stream sections alone; `params` from train_params (without use_dropout)."""
+
+    @staticmethod
+    def shared_bytes(descs):
+        """delora_odometry_streams_adapt_geometries_workspace_bytes; ValueError with the C side's message when it
+        refuses."""
+        L = _lib.lib()
+        arr = (_lib.OdometryDesc * len(descs))(*descs)
+        nbytes = int(L.delora_odometry_streams_adapt_geometries_workspace_bytes(arr, len(arr)))
+        if nbytes < 0:
+            raise ValueError(L.delora_last_error().decode())
+        return nbytes
+
+    def __init__(self, descs, weights, params, workspace=None):
+        self.descs = (_lib.OdometryDesc * len(descs))(*descs)
+        nbytes = self.shared_bytes(self.descs)
+        if workspace is None:
+            workspace = torch.empty((nbytes,), dtype=torch.uint8, device="cuda")
+        elif workspace.numel() < nbytes:
+            raise ValueError(f"the workspace has {workspace.numel()} bytes, the geometries need {nbytes}")
+        self.streams = [int(d.max_batch) for d in self.descs]
+        self.n_streams = sum(self.streams)
+        super().__init__(self.descs[0], weights, params, workspace)
+
+    def _geometries_call(self, name, *args):
+        _lib.check(getattr(self._L, name)(self.descs, len(self.descs), *args, _stream()), name)
+
+    def _init(self, weights):
+        self._geometries_call("delora_odometry_streams_adapt_geometries_init", weights.data_ptr(),
+                              self.workspace.data_ptr())
+
+    def push(self, points, counts, active, T, valid, losses, update=True):
+        """points / counts: one device tensor per geometry, [S_g, 3, descs[g].n_stride] and [S_g]; active [n_streams]
+        int32 or None (all active); T [n_streams, 16], valid [n_streams] and losses [n_streams, LOSS_ROW] out, as for
+        AdaptiveStreamsWorkspace.push.  update: then one Adam step on the mean objective of every geometry's valid
+        pairs."""
+        n = len(self.descs)
+        pts = (ctypes.c_void_p * n)(*(p.data_ptr() for p in points))
+        cnt = (ctypes.c_void_p * n)(*(c.data_ptr() for c in counts))
+        self._geometries_call("delora_odometry_streams_push_adapt_geometries", self._params,
+                              1 if update else 0, pts, cnt, _ptr(active), self.workspace.data_ptr(), T.data_ptr(),
+                              valid.data_ptr(), losses.data_ptr())
+
+    def reset(self, mask):
+        """Forget the previous frame of every stream with mask[s] != 0 (device int32 [n_streams])."""
+        self._geometries_call("delora_odometry_streams_adapt_geometries_reset", mask.data_ptr(),
+                              self.workspace.data_ptr())
+
+
 class TrainingGroup:
     """The delora_odometry_train_group of each of N TrainingWorkspaces (same descriptor and state), on N devices with
     peer access enabled between them or all on one device: the flag words and status word of every rank (on its

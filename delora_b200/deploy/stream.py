@@ -398,11 +398,15 @@ class AdaptiveOdometryStreams(_Streams):
         self.n_streams, self.n_max = int(n_streams), int(n_max)
         self.desc = export.desc_from_config(config, dataset, self.n_max, self.n_streams,
                                             preprocessing_normals=preprocessing_normals)
-        S, n = self.n_streams, self.n_max
         with torch.cuda.device(self.device):
             blob = torch.from_numpy(export.pack_state_dict(model.state_dict(), config)).to(self.device)
             self.workspace = capi.AdaptiveStreamsWorkspace(self.desc, blob,
                                                            capi.train_params(config, lr, loss_flags=loss_flags))
+        self._buffers()
+
+    def _buffers(self):
+        S, n = self.n_streams, self.n_max
+        with torch.cuda.device(self.device):
             self.points = torch.zeros((S, 3, n), dtype=torch.float32, device=self.device)
             self.counts = torch.zeros((S,), dtype=torch.int32, device=self.device)
             self.active = torch.zeros((S,), dtype=torch.int32, device=self.device)
@@ -423,9 +427,12 @@ class AdaptiveOdometryStreams(_Streams):
             self.points.copy_(pts)
             self.counts.copy_(counts)
             self.active.copy_(active)
-            self.workspace.push(self.points, self.counts, self.active, self.T, self.valid, self.losses, update)
+            self._push_device(update)
             T, valid, losses = self.T.cpu().numpy(), self.valid.cpu().numpy(), self.losses.cpu().numpy()
         return self._results(T, valid, [losses])
+
+    def _push_device(self, update):
+        self.workspace.push(self.points, self.counts, self.active, self.T, self.valid, self.losses, update)
 
     def state_dict(self):
         """The adapted weights as an OdometryModel state dict (fp32 CPU tensors)."""
@@ -433,3 +440,42 @@ class AdaptiveOdometryStreams(_Streams):
         with torch.cuda.device(self.device):
             w = self.workspace.weights().cpu().numpy()
         return export.unpack_blob(w, self.config)
+
+
+class GeometriesAdaptiveOdometryStreams(AdaptiveOdometryStreams):
+    """AdaptiveOdometryStreams over streams of several sensor geometries in one workspace
+    (`delora_odometry_streams_push_adapt_geometries`): `geometries` lists (dataset, n_streams) pairs, each dataset a
+    section of `config` with its own image size, vertical field of view and preprocessing width; streams are numbered
+    in that order.  One tick serves every geometry's streams, and with update=True takes one Adam step on the mean
+    objective over the pairs of all of them, so one model adapts to the whole fleet.  The datasets must share the
+    parity of their horizontal_cells.  `push`, `poses`, `reset` and `state_dict` are AdaptiveOdometryStreams'."""
+
+    def __init__(self, model, config, geometries, n_max, lr, preprocessing_normals=False,
+                 loss_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL):
+        from . import capi, export
+        if config.get("use_dropout", False):
+            raise ValueError("use_dropout: True is not supported by GeometriesAdaptiveOdometryStreams: the served "
+                             "transforms are dropout-free, and one forward cannot be both")
+        if config.get("normalization_scaling", False) and not preprocessing_normals:
+            raise ValueError("normalization_scaling: True needs preprocessing_normals=True (the reference's recipe: "
+                             "normals from the unscaled points at horizontal_cells_preprocessing)")
+        self.config = config
+        self.device = torch.device(config["device"])
+        if self.device.type != "cuda":
+            raise RuntimeError("GeometriesAdaptiveOdometryStreams runs on CUDA devices only (no CPU fallback)")
+        self.n_max = int(n_max)
+        self.descs = [export.desc_from_config(config, ds, self.n_max, int(s), preprocessing_normals=preprocessing_normals)
+                      for ds, s in geometries]
+        self.rows = np.cumsum([0] + [int(s) for _, s in geometries]).tolist()
+        self.n_streams = self.rows[-1]
+        with torch.cuda.device(self.device):
+            blob = torch.from_numpy(export.pack_state_dict(model.state_dict(), config)).to(self.device)
+            self.workspace = capi.GeometriesAdaptingStreamsWorkspace(
+                self.descs, blob, capi.train_params(config, lr, loss_flags=loss_flags))
+        self._buffers()
+
+    def _push_device(self, update):
+        r = self.rows
+        pts = [self.points[r[g]:r[g + 1]] for g in range(len(self.descs))]
+        counts = [self.counts[r[g]:r[g + 1]] for g in range(len(self.descs))]
+        self.workspace.push(pts, counts, self.active, self.T, self.valid, self.losses, update)

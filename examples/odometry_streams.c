@@ -4,6 +4,8 @@
  *
  *   odometry_streams [--residual | --preprocessing] model.dlw stream0_dir stream1_dir ...
  *   odometry_streams --adapt LR --adapt-out adapted.dlw [--gpus N] model.dlw stream0_dir stream1_dir ...
+ *   odometry_streams --adapt LR --adapt-out adapted.dlw [--geometry DIR,H,W,VFOV0,VFOV1[,W_PRE]]... model.dlw
+ *                    stream0_dir ...
  *
  * model.dlw is written by bin/export_odometry_weights.py (layout: include/delora_b200.h); every directory holds one
  * stream's KITTI velodyne .bin files ([N, 4] float32 rows: x, y, z, reflectance), taken in name order.  All streams
@@ -38,6 +40,13 @@
  * the mean over the valid pairs of all GPUs, so all GPUs keep the same weights.  GPU 0 writes FILE.dlw.  The output
  * lines are the same as on one GPU; --gpus 1 writes the file a run without the option writes.  --gpus is refused
  * without --adapt.
+ * --adapt ... --geometry DIR,H,W,VFOV0,VFOV1[,W_PRE] (repeatable, one GPU; the syntax of odometry_train.c): one more
+ * stream, recorded by another sensor: the .bin files of DIR, served at the header's descriptor with H, W, the vertical
+ * field of view (degrees) and w_pre (default 0) replaced.  The streams of every sensor adapt ONE model in one
+ * workspace through delora_odometry_streams_push_adapt_geometries: the directories after model.dlw are geometry 0
+ * (the header's), each --geometry is a geometry of one stream, numbered after them; every tick's update is the mean
+ * over the valid pairs of all sensors.  The output lines are as above.  --geometry is refused without --adapt and
+ * with --gpus; W must have the parity of the header's W, and a normalization_scaling file needs W_PRE > 0.
  *
  * Build:  cc odometry_streams.c -I include -I $CUDA_HOME/include -L delora_b200 -ldelora_b200 \
  *            -L $CUDA_HOME/lib64 -lcudart -lpthread -Wl,-rpath,$PWD/delora_b200 -o odometry_streams
@@ -52,6 +61,9 @@
 #include <cuda_runtime.h>
 
 #include "delora_b200.h"
+
+#define MAX_GEOMETRIES 16
+#define DEG_TO_RAD (3.14159265358979323846 / 180.0)
 
 static int fail(const char* what) {
     fprintf(stderr, "odometry_streams: %s\n", what);
@@ -121,6 +133,51 @@ static int32_t read_scan(const char* path, float* dst, int n_stride) {
         for (int c = 0; c < 3; ++c) dst[(size_t)c * n_stride + i] = rows[(size_t)i * 4 + c];
     free(rows);
     return n;
+}
+
+/* one ",value" field at *p: an integer in [0, 1e9] (integral) or a finite number; advances *p; 0 on success */
+static int next_field(const char** p, int integral, double* out) {
+    if (**p != ',') return 1;
+    const char* s = *p + 1;
+    char* end;
+    if (integral) {
+        const long v = strtol(s, &end, 10);
+        if (end == s || v < 0 || v > 1000000000L) return 1;
+        *out = (double)v;
+    } else {
+        const double v = strtod(s, &end);
+        if (end == s || !(v >= -1e300 && v <= 1e300)) return 1;     /* also refuses nan and inf */
+        *out = v;
+    }
+    if (*end != ',' && *end != '\0') return 1;
+    *p = end;
+    return 0;
+}
+
+/* "DIR,H,W,VFOV0,VFOV1[,W_PRE]" (fields of view in degrees) -> *dir (a copy) and *g: base with H, W, vfov and w_pre
+ * replaced; 0 on success.  The library validates the descriptor itself. */
+static int parse_geometry(const char* arg, const delora_odometry_desc* base, char** dir, delora_odometry_desc* g) {
+    const char* comma = strchr(arg, ',');
+    if (!comma || comma == arg) return 1;
+    double v[5] = {0, 0, 0, 0, 0};
+    const int integral[5] = {1, 1, 0, 0, 1};
+    const char* p = comma;
+    for (int i = 0; i < 5; ++i) {
+        if (i == 4 && *p == '\0') break;                              /* W_PRE is optional */
+        if (next_field(&p, integral[i], &v[i])) return 1;
+    }
+    if (*p != '\0' || v[0] < 1 || v[1] < 2 || !(v[3] > v[2])) return 1;
+    *g = *base;
+    g->H = (int)v[0];
+    g->W = (int)v[1];
+    g->vfov0 = v[2] * DEG_TO_RAD;
+    g->vfov1 = v[3] * DEG_TO_RAD;
+    g->w_pre = (int)v[4];
+    *dir = (char*)malloc((size_t)(comma - arg) + 1);
+    if (!*dir) return 1;
+    memcpy(*dir, arg, (size_t)(comma - arg));
+    (*dir)[comma - arg] = '\0';
+    return 0;
 }
 
 /* --adapt --gpus N: one GPU of the group, serving streams rank * S .. rank * S + S - 1 (those past the last directory
@@ -318,11 +375,17 @@ int main(int argc, char** argv) {
     const char* adapt_lr = NULL;
     const char* adapt_out = NULL;
     const char* gpus_arg = NULL;
+    int n_geom = 0;                           /* --geometry streams, after the directories of the header's geometry */
+    const char* geom_args[MAX_GEOMETRIES];
     while (argc > 2 && (strcmp(argv[1], "--adapt") == 0 || strcmp(argv[1], "--adapt-out") == 0 ||
-                        strcmp(argv[1], "--gpus") == 0)) {
+                        strcmp(argv[1], "--gpus") == 0 || strcmp(argv[1], "--geometry") == 0)) {
         if (strcmp(argv[1], "--adapt") == 0) adapt_lr = argv[2];
         else if (strcmp(argv[1], "--adapt-out") == 0) adapt_out = argv[2];
-        else gpus_arg = argv[2];
+        else if (strcmp(argv[1], "--gpus") == 0) gpus_arg = argv[2];
+        else {
+            if (n_geom == MAX_GEOMETRIES - 1) return fail("too many --geometry options");
+            geom_args[n_geom++] = argv[2];
+        }
         argc -= 2;
         argv += 2;
     }
@@ -345,13 +408,28 @@ int main(int argc, char** argv) {
             return fail("--gpus must be in [1, 16]");
         gpus = (int)v;
     }
+    if (n_geom > 0) {
+        if (!adapt) return fail("--geometry adapts one model from several sensors: it needs --adapt LR --adapt-out "
+                                "FILE.dlw");
+        if (gpus) return fail("--geometry serves every sensor on one GPU: it does not combine with --gpus");
+        for (int g = 0; g < n_geom; ++g) {         /* checked before anything is read, against a dummy descriptor */
+            delora_odometry_desc probe;
+            char* dir;
+            memset(&probe, 0, sizeof probe);
+            if (parse_geometry(geom_args[g], &probe, &dir, &probe))
+                return fail("--geometry wants DIR,H,W,VFOV0,VFOV1[,W_PRE]: a directory, integers H >= 1, W >= 2 and "
+                            "W_PRE >= 0, and the vertical field of view in degrees with VFOV0 < VFOV1");
+            free(dir);
+        }
+    }
     const int residual = argc > 1 && strcmp(argv[1], "--residual") == 0;
     const int pre = argc > 1 && strcmp(argv[1], "--preprocessing") == 0;
     if (residual || pre) { --argc; ++argv; }
     if (adapt && (residual || pre)) return fail("--adapt serves its own residual: drop --residual / --preprocessing");
     if (argc < 3)
         return fail("usage: odometry_streams [--residual | --preprocessing] model.dlw stream_dir [stream_dir ...]");
-    const int S = argc - 2;
+    const int S_dirs = argc - 2;              /* the streams of the header's geometry */
+    const int S = S_dirs + n_geom;            /* every stream, the --geometry ones last */
 
     /* weight file: fixed header, then the fp32 blob; the workspace serves S streams (max_batch = S) */
     FILE* f = fopen(argv[1], "rb");
@@ -370,8 +448,17 @@ int main(int argc, char** argv) {
         return fail("--preprocessing needs a file with w_pre > 0: export it with bin/export_odometry_weights.py "
                     "--preprocessing-normals");
     delora_odometry_desc desc = hdr.desc;
-    desc.max_batch = S;
+    desc.max_batch = S_dirs;
     const delora_odometry_desc* d = &desc;
+    /* --geometry: geometry 0 is the header's, geometry g >= 1 serves stream S_dirs + g - 1 */
+    const int n_sets = 1 + n_geom;
+    delora_odometry_desc descs[MAX_GEOMETRIES];
+    char* geom_dirs[MAX_GEOMETRIES];
+    descs[0] = desc;
+    for (int g = 1; g < n_sets; ++g) {
+        if (parse_geometry(geom_args[g - 1], &desc, &geom_dirs[g - 1], &descs[g])) return fail("bad --geometry");
+        descs[g].max_batch = 1;
+    }
     const int64_t n_weights = delora_odometry_weight_floats(d);
     if (n_weights < 0) return fail(delora_last_error());
     if (n_weights != hdr.blob_floats) return fail("blob length does not match the descriptor");
@@ -383,7 +470,8 @@ int main(int argc, char** argv) {
     if (!lists) return fail("out of host memory");
     int ticks = 0;
     for (int s = 0; s < S; ++s) {
-        if (list_scans(argv[2 + s], &lists[s])) return fail("cannot list a stream directory");
+        if (list_scans(s < S_dirs ? argv[2 + s] : geom_dirs[s - S_dirs], &lists[s]))
+            return fail("cannot list a stream directory");
         if (lists[s].n > ticks) ticks = lists[s].n;
     }
 
@@ -418,7 +506,8 @@ int main(int argc, char** argv) {
     rp.min_neighbors = 10;
     int32_t *count, *active, *valid;
     void* workspace;
-    const int64_t ws_bytes = adapt        ? delora_odometry_streams_adapt_workspace_bytes(d)
+    const int64_t ws_bytes = n_geom       ? delora_odometry_streams_adapt_geometries_workspace_bytes(descs, n_sets)
+                             : adapt      ? delora_odometry_streams_adapt_workspace_bytes(d)
                              : pre        ? delora_odometry_streams_pre_workspace_bytes(d)
                              : residual   ? delora_odometry_streams_residual_workspace_bytes(d)
                              : normalized ? delora_odometry_streams_normalized_workspace_bytes(d)
@@ -434,7 +523,17 @@ int main(int argc, char** argv) {
     CUDA_OK(cudaMalloc((void**)&losses, (size_t)S * DELORA_LOSS_ROW * sizeof(float)));
     CUDA_OK(cudaMalloc((void**)&factor, (size_t)S * sizeof(float)));
     CUDA_OK(cudaMemcpy(weights, h_blob, (size_t)n_weights * sizeof(float), cudaMemcpyHostToDevice));
-    if (adapt) {
+    /* --geometry: geometry g's scans and counts start at its first stream's row */
+    const float* g_points[MAX_GEOMETRIES];
+    const int32_t* g_count[MAX_GEOMETRIES];
+    for (int g = 0; g < n_sets; ++g) {
+        const int row = g == 0 ? 0 : S_dirs + g - 1;
+        g_points[g] = points + (size_t)row * 3 * d->n_stride;
+        g_count[g] = count + row;
+    }
+    if (n_geom) {
+        DELORA_OK(delora_odometry_streams_adapt_geometries_init(descs, n_sets, weights, workspace, stream));
+    } else if (adapt) {
         DELORA_OK(delora_odometry_streams_adapt_init(d, weights, workspace, stream));
     } else {
         if (pre) DELORA_OK(delora_odometry_streams_pre_init(d, workspace, stream));
@@ -463,7 +562,10 @@ int main(int argc, char** argv) {
         CUDA_OK(cudaMemcpyAsync(count, h_count, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
         CUDA_OK(cudaMemcpyAsync(active, h_active, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
         if (adapt || pre || residual) {
-            if (adapt)
+            if (n_geom)
+                DELORA_OK(delora_odometry_streams_push_adapt_geometries(descs, n_sets, &hp, 1, g_points, g_count, active,
+                                                                        workspace, T, valid, losses, stream));
+            else if (adapt)
                 DELORA_OK(delora_odometry_streams_push_adapt(d, &hp, 1, points, count, active, workspace, T, valid,
                                                              losses, stream));
             else if (pre)
@@ -509,6 +611,7 @@ int main(int argc, char** argv) {
         free(lists[s].paths);
     }
     free(lists);
+    for (int g = 0; g < n_geom; ++g) free(geom_dirs[g]);
     free(h_losses);
     free(h_T);
     free(h_valid);

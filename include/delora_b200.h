@@ -912,8 +912,9 @@ int delora_odometry_train_set_state(const delora_odometry_desc* d, const float* 
  * value of `update` serves every tick.  Refused before any launch, naming the field or pointer: everything _train_step
  * refuses at B = S, update not 0 or 1, a null points / n_points / workspace / T / valid / losses,
  * DELORA_LOSS_IDENTITY_FIT (a pre-training phase, not adaptation) and DELORA_TRAIN_DROPOUT (the served T is
- * dropout-free, and one forward cannot be both).  Out of scope: dropout while adapting, mixed geometries in one tick,
- * and any policy for when to adapt; several GPUs adapting one model: delora_odometry_streams_push_adapt_group below.
+ * dropout-free, and one forward cannot be both).  Out of scope: dropout while adapting and any policy for when to
+ * adapt; several GPUs adapting one model: delora_odometry_streams_push_adapt_group below; streams of several sensor
+ * geometries adapting one model: delora_odometry_streams_push_adapt_geometries below.
  * Cost, measured on one H100 80GB HBM3 at a 700 W power limit (max SM clock 1980 MHz), graph-replayed ticks, all
  * streams active, near-identity heads, lr 0, medians of alternating samples, ms per tick at S = 1 / 4 / 16,
  * update = 0 | update = 1 | _train_step at B = S alone | the two-workspace composition a host needs without this call
@@ -1147,7 +1148,8 @@ int delora_odometry_streams_push_adapt_group(const delora_odometry_desc* d, cons
  * d[0]'s (a different model-section layout); _use_geometry also refuses g outside [0, n) and a null workspace.
  * Not covered: one step that mixes geometries (the reference cannot either, config/hyperparameters.yaml:3); mixing W
  * parities; inference and streams.  A model trained this way is served per sensor by the inference and streams
- * workspaces from the same .dlw blob, one descriptor per sensor.
+ * workspaces from the same .dlw blob, one descriptor per sensor, and adapted from a mixed fleet by
+ * delora_odometry_streams_push_adapt_geometries below.
  * Memory, n_stride 131072, max_batch 16: 64 x 2048 with 64 x 720 (w_pre 2250) share 2911 MiB where two
  * single-geometry workspaces take 2911 + 1558 MiB.
  * Cost: the re-arm zeroes d[g]'s whole geometry section, which max_batch sizes, whatever B the next step takes.  So
@@ -1161,6 +1163,74 @@ int64_t delora_odometry_train_geometries_workspace_bytes(const delora_odometry_d
 int delora_odometry_train_geometries_init(const delora_odometry_desc* d, int n, const float* weights, void* workspace,
                                           void* stream);
 int delora_odometry_train_use_geometry(const delora_odometry_desc* d, int n, int g, void* workspace, void* stream);
+
+/* ---- Adapting streams of several sensor geometries in one workspace: one model, one call per tick, one Adam step on
+ * the mean over every geometry's valid pairs (a fleet that carries, say, a 64 x 720 and a 64 x 512 sensor adapting
+ * the model both were trained on through delora_odometry_train_geometries_*).
+ *
+ * d[0 .. n-1], 1 <= n <= 16: the set delora_odometry_train_geometries_* accepts (the same act, layers,
+ * resnet_outputs, single_mlp and W parity), each one a descriptor _push_adapt accepts.  Geometry g serves
+ * S_g = d[g].max_batch streams; streams are numbered in geometry order, S_total = S_0 + ... + S_{n-1}, and T
+ * [S_total, 16], valid [S_total], losses [S_total, DELORA_LOSS_ROW], active [S_total] (or NULL: all active) and the
+ * reset mask [S_total] use that order.  points and n_points are HOST arrays of n device pointers: points[g]
+ * [S_g, 3, d[g].n_stride], n_points[g] [S_g].
+ *
+ * Workspace, each buffer 256-byte aligned:
+ *   1. the adapting-streams workspace of d[0], unchanged: the model section, d[0]'s geometry section, its stream
+ *      section;
+ *   2. for g = 1 .. n-1 in order: d[g]'s training geometry section (at max_batch S_g), its stream section (as
+ *      _push_adapt's: the cache, has_prev, the count of valid pairs) and one gradient slice (fp32[weight_floats], blob
+ *      order);
+ *   3. n > 1 only: a fleet section of 8 + 24 (n - 1) bytes, the count of valid pairs over every geometry (int32) and
+ *      each geometry g >= 1's counters (the batch marker of its ICP scratch).
+ * So with n = 1 the workspace IS _push_adapt's, and every delora_odometry_train_* call with &d[0] works on it
+ * unchanged (_train_weights, _train_get_state / _set_state and the .dlt round trip, _train_grad_offset), as does
+ * _push_adapt(&d[0]), which drives geometry 0 alone.  A geometry section cannot be shared: the zero halo rows of the
+ * activations sit at other places for another H x W.  Sizes from the host-only query (layers {2,2,2,2},
+ * resnet_outputs 1000, two heads, n_stride 131072), 64 x 720 (w_pre 2250) + 64 x 512 (w_pre 512) at S_g = 1 / 4 / 16
+ * each: 475.6 / 879.2 / 2493.3 MiB, where two _push_adapt workspaces take 345.4 + 308.8 / 602.0 + 455.6 /
+ * 1628.7 + 1043.2 MiB (the second workspace's weights, Adam's m and v and bf16 filters are not repeated; of its
+ * 4 x 45.3 MiB fp32 blobs only the gradient slice remains).
+ *
+ * delora_odometry_streams_adapt_geometries_init: _train_init of d[0] on the whole workspace (every other section
+ * zeroed), every geometry's depth keys armed and cached grids emptied.  delora_odometry_streams_adapt_geometries_reset:
+ * forget the previous frame of every stream with mask[s] != 0; only launches.
+ *
+ * delora_odometry_streams_push_adapt_geometries, one tick:
+ *   1. For each g: _push_adapt's stages 1-3 of d[g] at B = S_g on its own geometry and stream sections, into rows
+ *      S_0 + ... + S_{g-1} onwards: T, valid, the loss rows (the factor in losses[s][6] with
+ *      DELORA_TRAIN_NORMALIZATION_SCALING) and the cache write, the bits a _push_adapt workspace of d[g] holding the
+ *      same weights writes.  update = 0 stops there (each geometry's ICP batch marker recorded as _push_adapt does).
+ *   2. update = 1: one kernel sums the geometries' counts of valid pairs in geometry order into the fleet count N.
+ *      Each geometry's backward divides by N (invalid rows add exact zeros); geometry 0 writes the model's gradient
+ *      section, geometry g >= 1 its slice.  Adam reads the n gradients, sums them per float in geometry order, writes
+ *      the sum to the gradient section (so _train_grad_offset holds the fleet's mean gradient after the tick) and
+ *      updates iff N > 0; with N = 0 the step count stays and the weights are not touched.  Then one bf16 re-prep.
+ * With n = 1 the tick launches exactly what _push_adapt launches: the same bits.  Only launches, with a sequence that
+ * depends on neither `active`, the stream state nor the counts: one captured graph per value of `update` serves every
+ * tick.  Refused before any launch, naming the index and the field: n outside [1, 16], every refusal of
+ * delora_odometry_train_geometries_*, everything _push_adapt refuses for any d[g] (DELORA_LOSS_IDENTITY_FIT and
+ * DELORA_TRAIN_DROPOUT included), a null points / n_points array, a null points[g] or n_points[g], and
+ * DELORA_TRAIN_NORMALIZATION_SCALING with any d[g].w_pre = 0.  Out of scope: mixed geometries across GPUs, mixed W
+ * parities, dropout or the identity fit while adapting, one trunk launch over unlike image sizes (each geometry's
+ * trunk runs at its own B).
+ * Cost, measured on one H100 80GB HBM3 at a 700 W power limit (max SM clock 1980 MHz), graph-replayed ticks, all
+ * streams active, near-identity heads, lr 0, medians of alternating samples, 64 x 720 (w_pre 2250) + 64 x 512
+ * (w_pre 512), ms per tick at S_g = 1 / 4, this call | a _push_adapt tick of each geometry's own workspace:
+ *   update = 0: 2.38 / 2.73 | 2.39 / 2.73 (paired difference -0.002 ms);
+ *   update = 1: 6.71 / 8.23 | 6.86 / 8.40 (paired difference -0.16 ms: one Adam step and one bf16 re-prep instead of
+ *               two, against one extra read of the gradient slice)
+ * (scripts/gpu_odometry_streams_adapt_geometries.py, profiles/odometry_streams_adapt_geometries_h100_700w.json). */
+int64_t delora_odometry_streams_adapt_geometries_workspace_bytes(const delora_odometry_desc* d, int n);   /* host only */
+int delora_odometry_streams_adapt_geometries_init(const delora_odometry_desc* d, int n, const float* weights,
+                                                  void* workspace, void* stream);
+int delora_odometry_streams_push_adapt_geometries(const delora_odometry_desc* d, int n,
+                                                  const delora_odometry_train_params* hp, int update,
+                                                  const float* const* points, const int32_t* const* n_points,
+                                                  const int32_t* active, void* workspace, float* T, int32_t* valid,
+                                                  float* losses, void* stream);
+int delora_odometry_streams_adapt_geometries_reset(const delora_odometry_desc* d, int n, const int32_t* mask,
+                                                   void* workspace, void* stream);
 
 #ifdef __cplusplus
 }
