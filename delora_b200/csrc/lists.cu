@@ -123,13 +123,24 @@ image_emit_kernel(const float* __restrict__ image, const float* __restrict__ nor
 }
 
 // ---- generic lists: counting sort by cell -----------------------------------------------
+// Points outside the field of view live in the border cells.  Rows clamp.  An azimuth in the horizontal gap (G =
+// circ_px - wm1 pixels from the centre of column W-1 round to the centre of column 0) goes to the border column it is
+// nearer to around the circle, not to the one on its side of atan2's +-pi wrap.  nn_search's column bounds take a
+// target in column W-1 to lie at least 0.5 - seam_px pixels before column 0's centre (seam_px = max(0, 1 - G)), and
+// one in column 0 as far past column W-1's centre.  Split at the gap's middle, the border columns keep their targets
+// at least G/2 away from each other's centre, and G/2 >= 0.5 - max(0, 1 - G) for every G.  The plain clamp put an
+// azimuth just short of column 0's centre into column W-1 (or the mirror image), which breaks the bound for G > 1/2.
 __device__ __forceinline__ int cell_of(const GridParams& g, float x, float y, float z) {
     float u, v;
     pixel_coords(g, x, y, z, u, v);
-    // clamp into the grid (NaN -> 0): points outside the FOV live in the border cells
-    const float ru = fminf(fmaxf(rintf(u), 0.0f), g.wm1);
+    float ru = rintf(u);
+    if (ru < 0.0f || ru > g.wm1) {                      // NaN fails both tests and is clamped to 0 below
+        const float past = u > g.wm1 ? u - g.wm1 : (u + g.circ_px) - g.wm1;    // pixels past column W-1's centre
+        ru = past <= 0.5f * (g.circ_px - g.wm1) ? g.wm1 : 0.0f;
+    }
+    const float cu = fminf(fmaxf(ru, 0.0f), g.wm1);
     const float rv = fminf(fmaxf(rintf(v), 0.0f), g.hm1);
-    return (int)rv * g.W + (int)ru;
+    return (int)rv * g.W + (int)cu;
 }
 
 __global__ void __launch_bounds__(256)

@@ -151,7 +151,8 @@ int delora_lists_from_images(const float* image, const float* normals, int B, in
 /* Bin arbitrary point lists (the reference's [1,3,N] tensors) into the spherical cell grid:
  * counting sort by cell.  Needed by losses.icp_losses.ICPLosses.forward for lists that did
  * not come from delora_lists_from_images (src/losses/icp_losses.py:34 builds a cKDTree here).
- * Points outside the field of view are clamped into the border cells (the search stays exact).
+ * Points outside the field of view go to the border cells (the search stays exact): rows clamp, and an azimuth in
+ * the horizontal gap goes to the border column (0 or W-1) it is nearer to around the circle.
  *
  * pts, nrm   [B, 3, n_stride] fp32 channels-first;  n [B] int32
  * pts4/nrm4  [B, n_stride] out, sorted by cell; pts4.w = bits(original list index)
