@@ -81,6 +81,10 @@ SIGNATURES = {
     "delora_icp_dense_fwd_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                          c_double, c_double, c_double, c_double, c_float, c_u32, c_void_p,
                                          c_void_p, c_void_p, c_void_p]),
+    "delora_icp_information_scratch_floats": (c_i64, [c_int, c_int, c_int]),
+    "delora_icp_dense_information": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                             c_double, c_double, c_double, c_double, c_float, c_u32, c_void_p,
+                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "delora_icp_fwd_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                    c_int, c_int, c_int, c_int, c_double, c_double, c_double, c_double, c_float,
                                    c_u32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
@@ -143,6 +147,10 @@ SIGNATURES = {
     "delora_odometry_streams_residual_init": (c_int, [c_desc_p, c_void_p, c_void_p]),
     "delora_odometry_streams_push_residual": (c_int, [c_desc_p, c_residual_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                                       c_void_p, c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_streams_info_workspace_bytes": (c_i64, [c_desc_p]),
+    "delora_odometry_streams_info_init": (c_int, [c_desc_p, c_void_p, c_void_p]),
+    "delora_odometry_streams_push_info": (c_int, [c_desc_p, c_residual_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_streams_normalized_workspace_bytes": (c_i64, [c_desc_p]),
     "delora_odometry_streams_normalized_init": (c_int, [c_desc_p, c_void_p, c_void_p]),
     "delora_odometry_streams_push_normalized": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,

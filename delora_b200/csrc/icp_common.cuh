@@ -143,6 +143,16 @@ __device__ __forceinline__ void accumulate_pair(uint32_t flags, const float4 p, 
     }
 }
 
+// The target id of a pair accumulate_pair keeps (a normal on both sides, or with po2po on neither), -1 otherwise.
+// (nsx..): the rotated source normal; j: the NN of a paired lane in the target normals tn.
+__device__ __forceinline__ int kept_nn(bool paired, bool po2po, float nsx, float nsy, float nsz,
+                                       const float4* __restrict__ tn, int j) {
+    if (!paired) return -1;
+    const bool src_has = (nsx != 0.0f) | (nsy != 0.0f) | (nsz != 0.0f);
+    const bool tgt_has = __ldg(tn + j).w != 0.0f;
+    return (src_has == tgt_has && (src_has || po2po)) ? j : -1;
+}
+
 // Sum of `acc[k]` over the 32 lanes for every k < N, lane k keeping column k (keep0) and column 32 + k (keep1).
 // Columns 0..31 go through a recursive-halving exchange: in the round with offset o the lanes whose bit o is clear
 // keep the lower half of the live columns and receive the partner's contribution to them (31 shuffles for 32
@@ -310,6 +320,29 @@ inline IcpScratch icp_scratch(float* base, const IcpLayout& L) {
     s.pend.result = reinterpret_cast<int*>(base + L.result);
     return s;
 }
+
+// The caller buffer of delora_icp_dense_information (delora_icp_information_scratch_floats floats), as element offsets:
+// the NN id of every source pixel (int32 [B, HW], first: the header documents it), then the per-warp partial rows of
+// the information pass (fp32 [B, rows, kInfoPartial]).  Every section is written before it is read, on every call.
+constexpr int kInfoSums = 21;                       // upper triangle of a symmetric 6 x 6, row by row
+constexpr int kInfoPartial = 64;                    // po2pl, pl2pl, po2po sums (3 x 21), one column of padding
+struct IcpInfoLayout {
+    int rows;
+    int64_t ids, partials, total;
+};
+
+inline IcpInfoLayout icp_info_layout(int B, int HW) {
+    IcpInfoLayout L;
+    L.rows = (HW + 31) / 32;
+    L.ids = 0;
+    L.partials = (int64_t)B * HW;
+    L.total = L.partials + (int64_t)B * L.rows * kInfoPartial;
+    return L;
+}
+
+// icp_info.cu: the information pass after the dense search (which wrote the NN ids) and the finalize (losses)
+int launch_icp_information(const float4* src_grid, const float4* src_ngrid, const float* T, const float4* tgt_ngrid, int B, int HW, float lambda_po2pl, uint32_t flags,
+                           const float* losses, float* info_scratch, float* info, cudaStream_t st);
 
 int launch_icp_finalize(const IcpScratch& sc, int B, int rows, float lambda_po2pl, float* losses, float* grad_T,
                         cudaStream_t st);

@@ -334,12 +334,15 @@ __device__ __forceinline__ void window_col_bounds(int e_lf, int e_rt, int cc, in
 // scan (NN distance ~ half the ring spacing, metres) and depth discontinuities; ~2-5 % of the warps,
 // but each needs thousands of cells or a serial per-lane block search, and as stragglers inside this
 // kernel they would set its duration.
-template <bool PO2PO, bool STATS>
+// IDS (delora_icp_dense_information): every source pixel also writes its kept NN to nn_ids [B, H*W] (kept_nn); the
+// lanes handed to kernel 2 write -1 here and their NN there.  Without IDS, nn_ids is not read.
+template <bool PO2PO, bool STATS, bool IDS = false>
 __global__ void __launch_bounds__(kDenseThreads, 8)
 icp_dense_kernel(const float4* __restrict__ src_grid, const float4* __restrict__ src_ngrid,
                  const float* __restrict__ T, const float4* __restrict__ tgt_grid,
                  const float4* __restrict__ tgt_ngrid, int max_strips, GridParams g, uint32_t flags,
-                 float* __restrict__ partial_rows, int rows_per_pair, PendingList pend, TargetExtents ext) {
+                 float* __restrict__ partial_rows, int rows_per_pair, PendingList pend, TargetExtents ext,
+                 int* __restrict__ nn_ids) {
     const int b = blockIdx.y;
     const int H = g.H, W = g.W, HW = H * W;
     const float4* __restrict__ tg = tgt_grid + (size_t)b * HW;
@@ -488,6 +491,8 @@ icp_dense_kernel(const float4* __restrict__ src_grid, const float4* __restrict__
             best_j = nn_exact_rescan(tg, H, W, rc, cc, e_dn, e_up, e_lf, e_rt, sx, sy, sz, nn.m1 * (1.0f + kNNBand));
         }
     }
+    if (IDS && i < HW)
+        nn_ids[(size_t)b * HW + i] = kept_nn(active && best_j >= 0, PO2PO, s.nsx, s.nsy, s.nsz, tn, best_j);
     accumulate_warp_row<(PO2PO ? kIcpAcc : kColPo2po), false>(active && best_j >= 0, flags, s.p, s.m, sx, sy, sz, s.nsx,
                                                               s.nsy, s.nsz, tg, tn, best_j, nullptr, nullptr,
                                                               partial_rows, b, rows_per_pair, warp_in_pair);
@@ -597,13 +602,13 @@ __device__ __noinline__ int exact_rerank_warp(const float4* __restrict__ tg, con
 // Persistent grid-stride over the entries; the last CTA re-arms the work list.
 constexpr int kPendThreads = 256;
 
-template <bool PO2PO, bool STATS>
+template <bool PO2PO, bool STATS, bool IDS = false>
 __global__ void __launch_bounds__(kPendThreads, 4)
 icp_dense_pending_kernel(const float4* __restrict__ src_grid, const float4* __restrict__ src_ngrid,
                          const float* __restrict__ T, const float4* __restrict__ tgt_grid,
                          const float4* __restrict__ tgt_ngrid, TargetExtents ext, int nbh, int nbw,
                          GridParams g, uint32_t flags, float* __restrict__ partial_rows, int rows_per_pair,
-                         PendingList pend) {
+                         PendingList pend, int* __restrict__ nn_ids) {
     const int H = g.H, W = g.W, HW = H * W;
     const int lane = threadIdx.x & 31;
     const int warps_per_cta = (int)blockDim.x >> 5;
@@ -696,6 +701,9 @@ icp_dense_pending_kernel(const float4* __restrict__ src_grid, const float4* __re
             const SrcLane s = load_src_lane(src_grid, src_ngrid, T, b, warp_in_pair * 32 + lane, HW, g);
             const bool mine = ((pending >> lane) & 1u) != 0u && s.active;
             const int best_j = mine ? __ldcg(pend.result + it.w + __popc(pending & ((1u << lane) - 1u))) : -1;
+            if (IDS && ((pending >> lane) & 1u))
+                nn_ids[(size_t)b * HW + warp_in_pair * 32 + lane] =
+                    kept_nn(mine && best_j >= 0, PO2PO, s.nsx, s.nsy, s.nsz, tn, best_j);
             accumulate_warp_row<(PO2PO ? kIcpAcc : kColPo2po), true>(mine && best_j >= 0, flags, s.p, s.m, s.sx, s.sy,
                                                                      s.sz, s.nsx, s.nsy, s.nsz, tg, tn, best_j, nullptr,
                                                                      nullptr, partial_rows, b, rows_per_pair,
@@ -716,21 +724,22 @@ icp_dense_pending_kernel(const float4* __restrict__ src_grid, const float4* __re
     }
 }
 
-// The window search of one (PO2PO, STATS) instantiation, as the programmatic dependent of target_extents_kernel (see
-// griddepcontrol.wait in the kernel: its CTAs load their source lanes and start windows while the pre-pass is still
+// The window search of one (PO2PO, STATS, IDS) instantiation, as the programmatic dependent of target_extents_kernel
+// (see griddepcontrol.wait in the kernel: its CTAs load their source lanes and start windows while the pre-pass is still
 // running), then the block search of the lanes it hands over.
-template <bool PO2PO, bool STATS>
+template <bool PO2PO, bool STATS, bool IDS = false>
 int launch_dense_search(const float4* src_grid, const float4* src_ngrid, const float* T, const float4* tgt_grid,
                         const float4* tgt_ngrid, int B, int rows, int nbh, int nbw, int max_strips, const GridParams& g,
-                        uint32_t flags, const IcpScratch& sc, cudaStream_t st) {
+                        uint32_t flags, const IcpScratch& sc, int* nn_ids, cudaStream_t st) {
     const dim3 grid((g.H * g.W + kDenseThreads - 1) / kDenseThreads, B);
-    const cudaError_t e = launch_pdl(icp_dense_kernel<PO2PO, STATS>, grid, dim3(kDenseThreads), st, src_grid, src_ngrid,
-                                     T, tgt_grid, tgt_ngrid, max_strips, g, flags, sc.rows, rows, sc.pend, sc.ext);
+    const cudaError_t e = launch_pdl(icp_dense_kernel<PO2PO, STATS, IDS>, grid, dim3(kDenseThreads), st, src_grid,
+                                     src_ngrid, T, tgt_grid, tgt_ngrid, max_strips, g, flags, sc.rows, rows, sc.pend,
+                                     sc.ext, nn_ids);
     DELORA_CHECK_LAUNCH_RESULT(e, "icp_dense_kernel");
     // persistent block search: enough CTAs for one wave (up to 4 per SM), never more than there can be items
     const int pend_grid = (int)std::min<long long>(((long long)B * rows * 32 + 7) / 8, 4ll * num_sms());
-    icp_dense_pending_kernel<PO2PO, STATS><<<pend_grid, kPendThreads, 0, st>>>(
-        src_grid, src_ngrid, T, tgt_grid, tgt_ngrid, sc.ext, nbh, nbw, g, flags, sc.rows, rows, sc.pend);
+    icp_dense_pending_kernel<PO2PO, STATS, IDS><<<pend_grid, kPendThreads, 0, st>>>(
+        src_grid, src_ngrid, T, tgt_grid, tgt_ngrid, sc.ext, nbh, nbw, g, flags, sc.rows, rows, sc.pend, nn_ids);
     DELORA_CHECK_LAUNCH("icp_dense_pending_kernel");
     return 0;
 }
@@ -752,32 +761,64 @@ extern "C" int delora_icp_stats(uint32_t* out32, int reset) {
     return 0;
 }
 
-extern "C" int delora_icp_dense_fwd_bwd(const delora_f4* src_grid, const delora_f4* src_ngrid, const float* T,
-                                        const delora_f4* tgt_grid, const delora_f4* tgt_ngrid, int B, int H, int W,
-                                        double hfov0, double hfov1, double vfov0, double vfov1, float lambda_po2pl,
-                                        uint32_t flags, float* losses, float* grad_T, float* scratch, void* stream) {
+// delora_icp_dense_fwd_bwd (nn_ids NULL) and the search + finalize of delora_icp_dense_information (nn_ids [B, H*W]:
+// the IDS instantiations, which the DELORA_ICP_STATS ones never are)
+static int dense_icp(const delora_f4* src_grid, const delora_f4* src_ngrid, const float* T, const delora_f4* tgt_grid,
+                     const delora_f4* tgt_ngrid, int B, int H, int W, double hfov0, double hfov1, double vfov0,
+                     double vfov1, float lambda_po2pl, uint32_t flags, float* losses, float* grad_T, float* scratch,
+                     int* nn_ids, cudaStream_t st, const char* who) {
     DELORA_CHECK_ARG(src_grid && src_ngrid && T && tgt_grid && tgt_ngrid && losses && grad_T && scratch,
-                     "delora_icp_dense_fwd_bwd: null pointer");
-    DELORA_CHECK_ARG(B > 0 && B <= 65535 && H > 0 && W > 0 && (long long)H * W < (1ll << 31),
-                     "delora_icp_dense_fwd_bwd: bad shape");
+                     "%s: null pointer", who);
+    DELORA_CHECK_ARG(B > 0 && B <= 65535 && H > 0 && W > 0 && (long long)H * W < (1ll << 31), "%s: bad shape", who);
     const IcpLayout L = icp_layout(B, H * W);
     const int nbh = (H + kBlkH - 1) / kBlkH, nbw = (W + kBlkW - 1) / kBlkW;
     DELORA_CHECK_ARG((int64_t)nbh * nbw <= L.blk_per_pair,
-                     "delora_icp_dense_fwd_bwd: H=%d W=%d needs %lld range-pyramid blocks per pair, the scratch holds %lld",
-                     H, W, (long long)nbh * nbw, (long long)L.blk_per_pair);
+                     "%s: H=%d W=%d needs %lld range-pyramid blocks per pair, the scratch holds %lld",
+                     who, H, W, (long long)nbh * nbw, (long long)L.blk_per_pair);
     const GridParams g = make_grid(H, W, hfov0, hfov1, vfov0, vfov1, 1);
     const IcpScratch sc = icp_scratch(scratch, L);
-    cudaStream_t st = (cudaStream_t)stream;
     int max_strips = kDefaultMaxStrips;
     if (const char* e = getenv("DELORA_ICP_MAX_STRIPS")) max_strips = atoi(e);      // tuning knob (tests / profiling)
     target_extents_kernel<<<dim3(nbh, B), kExtThreads, 0, st>>>((const float4*)tgt_grid, H, W, nbh, nbw, sc.ext);
     DELORA_CHECK_LAUNCH("target_extents_kernel");
     using DenseSearch = decltype(&launch_dense_search<false, false>);
-    constexpr DenseSearch kSearch[2][2] = {{launch_dense_search<false, false>, launch_dense_search<false, true>},
-                                           {launch_dense_search<true, false>, launch_dense_search<true, true>}};
-    const int rc = kSearch[(flags & DELORA_LOSS_PO2PO) != 0u][(flags & DELORA_ICP_STATS) != 0u](
+    constexpr DenseSearch kSearch[2][3] = {
+        {launch_dense_search<false, false>, launch_dense_search<false, true>, launch_dense_search<false, false, true>},
+        {launch_dense_search<true, false>, launch_dense_search<true, true>, launch_dense_search<true, false, true>}};
+    const int variant = nn_ids ? 2 : (flags & DELORA_ICP_STATS) != 0u ? 1 : 0;
+    const int rc = kSearch[(flags & DELORA_LOSS_PO2PO) != 0u][variant](
         (const float4*)src_grid, (const float4*)src_ngrid, T, (const float4*)tgt_grid, (const float4*)tgt_ngrid, B,
-        L.rows, nbh, nbw, max_strips, g, flags, sc, st);
+        L.rows, nbh, nbw, max_strips, g, flags, sc, nn_ids, st);
     if (rc != 0) return rc;
     return launch_icp_finalize(sc, B, L.rows, lambda_po2pl, losses, grad_T, st);
+}
+
+extern "C" int delora_icp_dense_fwd_bwd(const delora_f4* src_grid, const delora_f4* src_ngrid, const float* T,
+                                        const delora_f4* tgt_grid, const delora_f4* tgt_ngrid, int B, int H, int W,
+                                        double hfov0, double hfov1, double vfov0, double vfov1, float lambda_po2pl,
+                                        uint32_t flags, float* losses, float* grad_T, float* scratch, void* stream) {
+    return dense_icp(src_grid, src_ngrid, T, tgt_grid, tgt_ngrid, B, H, W, hfov0, hfov1, vfov0, vfov1, lambda_po2pl,
+                     flags, losses, grad_T, scratch, nullptr, (cudaStream_t)stream, "delora_icp_dense_fwd_bwd");
+}
+
+extern "C" int64_t delora_icp_information_scratch_floats(int B, int H, int W) {
+    if (B <= 0 || H <= 0 || W <= 0 || (long long)H * W >= (1ll << 31)) return -1;
+    return icp_info_layout(B, H * W).total;
+}
+
+extern "C" int delora_icp_dense_information(const delora_f4* src_grid, const delora_f4* src_ngrid, const float* T,
+                                            const delora_f4* tgt_grid, const delora_f4* tgt_ngrid, int B, int H, int W,
+                                            double hfov0, double hfov1, double vfov0, double vfov1, float lambda_po2pl,
+                                            uint32_t flags, float* losses, float* grad_T, float* scratch, float* info,
+                                            float* info_scratch, void* stream) {
+    const char* who = "delora_icp_dense_information";
+    DELORA_CHECK_ARG(info && info_scratch, "%s: null pointer", who);
+    DELORA_CHECK_ARG((flags & DELORA_ICP_STATS) == 0u, "%s: DELORA_ICP_STATS is not counted here", who);
+    cudaStream_t st = (cudaStream_t)stream;
+    int* nn_ids = reinterpret_cast<int*>(info_scratch);
+    const int rc = dense_icp(src_grid, src_ngrid, T, tgt_grid, tgt_ngrid, B, H, W, hfov0, hfov1, vfov0, vfov1,
+                             lambda_po2pl, flags, losses, grad_T, scratch, nn_ids, st, who);
+    if (rc != 0) return rc;
+    return launch_icp_information((const float4*)src_grid, (const float4*)src_ngrid, T, (const float4*)tgt_ngrid, B, H * W, lambda_po2pl, flags, losses, info_scratch, info,
+                                  st);
 }

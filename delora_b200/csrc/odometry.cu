@@ -272,6 +272,9 @@ struct InferPlan {
     // residual only (delora_odometry_streams_push_residual), after every other section: the dense grids of the S new
     // frames and of each stream's previous frame, the 3x4 transforms the ICP reads, its outputs and its scratch
     size_t pts_grid, nrm_grid, prev_pts_grid, prev_nrm_grid, T12, losses, grad_T, icp;
+    // information streams only (delora_odometry_streams_push_info), after every residual section: the information rows
+    // of the S pairs and the operator's info_scratch
+    size_t info, info_scratch;
     // normalised streams only (delora_odometry_streams_push_normalized), after every streams section: the point rows
     // [2S, 3, n_stride] (each stream's previous frame, then its last frame), their counts [2S] followed by the count
     // of each stream's last frame [S], and the factor of each pair [S]
@@ -316,19 +319,20 @@ static void make_infer_plan(const delora_odometry_desc* d, InferPlan* p) {
 //   plain (delora_odometry_streams_push): S = max_batch streams, this tick's S frames, each stream's previous frame and
 //     whether it has one; the trunk and tail then run at B = S.
 //   residual (_push_residual): plain, then the sections of the per-frame ICP residual.
+//   info (_push_info): residual, then the information rows and the information operator's scratch.
 //   normalized (_push_normalized): plain, then the staged point rows and the pair factors.  Its prev_image section
 //     holds this tick's projection of each previous frame; nothing reads it across ticks.
 //   pre (_push_pre): residual (its H x W grids and ICP sections serve the recipe's ICP), then the H x w_pre sections.
 //     The plain layout's key buffers serve both H x W projections of a tick, its images hold this tick's projection
 //     of both frames of each pair.
-enum class Streams { plain, residual, normalized, pre };
+enum class Streams { plain, residual, normalized, pre, info };
 
 static void make_streams_plan(const delora_odometry_desc* d, Streams kind, InferPlan* p) {
     const int MB = d->max_batch;
     plan_inference(d, MB, MB, true, p);
     const size_t S = (size_t)MB, HW = (size_t)d->H * d->W, HWp = (size_t)d->H * d->w_pre;
     size_t off = p->total;
-    if (kind == Streams::residual || kind == Streams::pre) {
+    if (kind == Streams::residual || kind == Streams::pre || kind == Streams::info) {
         p->pts_grid = take(off, S * HW * 16);
         p->nrm_grid = take(off, S * HW * 16);
         p->prev_pts_grid = take(off, S * HW * 16);
@@ -337,6 +341,10 @@ static void make_streams_plan(const delora_odometry_desc* d, Streams kind, Infer
         p->losses = take(off, S * DELORA_LOSS_ROW * 4);
         p->grad_T = take(off, S * 12 * 4);
         p->icp = take(off, (size_t)delora_icp_scratch_floats(MB, (int)HW) * 4);
+    }
+    if (kind == Streams::info) {
+        p->info = take(off, S * DELORA_INFO_ROW * 4);
+        p->info_scratch = take(off, (size_t)delora_icp_information_scratch_floats(MB, d->H, d->W) * 4);
     }
     if (kind == Streams::normalized) {
         p->stage = take(off, 2 * S * 3 * (size_t)d->n_stride * 4);
@@ -913,6 +921,13 @@ __global__ void odometry_streams_losses_kernel(const int32_t* __restrict__ valid
     if (i < S * DELORA_LOSS_ROW) losses[i] = valid[i / DELORA_LOSS_ROW] != 0 ? icp_losses[i] : 0.0f;
 }
 
+// After the information operator: info [S, DELORA_INFO_ROW] = its row for the valid streams, zeros for the others
+__global__ void odometry_streams_info_kernel(const int32_t* __restrict__ valid, int S, const float* __restrict__ icp_info,
+                                             float* __restrict__ info) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < S * DELORA_INFO_ROW) info[i] = valid[i / DELORA_INFO_ROW] != 0 ? icp_info[i] : 0.0f;
+}
+
 // check_desc plus the preprocessing width the recipe streams read (the training rule, but w_pre = 0 is refused)
 static int check_pre_desc(const delora_odometry_desc* d, const char* who) {
     if (check_desc(d, who)) return 1;
@@ -941,7 +956,7 @@ static int clear_grids(char* ws, size_t pts, size_t nrm, size_t n, cudaStream_t 
     return 0;
 }
 
-// The residual and recipe kinds' ICP scratch is zeroed here, once, and their cached grids start empty
+// The residual, information and recipe kinds' ICP scratch is zeroed here, once, and their cached grids start empty
 static int streams_init(const delora_odometry_desc* d, Streams kind, void* workspace, cudaStream_t st, const char* who) {
     if (check_streams_desc(d, kind, who)) return 1;
     DELORA_CHECK_ARG(workspace, "%s: null workspace", who);
@@ -951,7 +966,7 @@ static int streams_init(const delora_odometry_desc* d, Streams kind, void* works
     const int rc = init_workspace(p.f, p.total, workspace, st, who);
     if (rc) return rc;
     const size_t S = (size_t)d->max_batch;
-    if (kind == Streams::residual) return clear_grids(ws, p.prev_pts_grid, p.prev_nrm_grid, S * d->H * d->W, st);
+    if (kind == Streams::residual || kind == Streams::info) return clear_grids(ws, p.prev_pts_grid, p.prev_nrm_grid, S * d->H * d->W, st);
     if (kind == Streams::pre) {
         const size_t n = S * d->H * d->w_pre;
         const cudaError_t e = cudaMemsetAsync(ws + p.pre_keys, 0xFF, n * 8, st);
@@ -1007,11 +1022,17 @@ static int streams_forward(const Model& m, const TailIO& io, const TrunkActs& t,
 }
 
 // The ICP at B = S on a residual or recipe plan's H x W grids: source pts_grid moved by T12, target prev_pts_grid,
-// into its losses and grad_T.  The recipe's DELORA_TRAIN_NORMALIZATION_SCALING is not an ICP bit.
+// into its losses and grad_T; on an information plan (p.info set) also into its information rows.  The recipe's
+// DELORA_TRAIN_NORMALIZATION_SCALING is not an ICP bit.
 static int streams_icp(const delora_odometry_desc* d, const delora_odometry_residual_params* rp, const InferPlan& p,
                        char* ws, cudaStream_t st) {
     auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
     auto f4 = [&](size_t o) { return reinterpret_cast<delora_f4*>(ws + o); };
+    if (p.info)
+        return delora_icp_dense_information(f4(p.pts_grid), f4(p.nrm_grid), f(p.T12), f4(p.prev_pts_grid),
+                                            f4(p.prev_nrm_grid), d->max_batch, d->H, d->W, d->hfov0, d->hfov1,
+                                            d->vfov0, d->vfov1, rp->lambda_po2pl, rp->loss_flags, f(p.losses),
+                                            f(p.grad_T), f(p.icp), f(p.info), f(p.info_scratch), st);
     return delora_icp_dense_fwd_bwd(f4(p.pts_grid), f4(p.nrm_grid), f(p.T12), f4(p.prev_pts_grid), f4(p.prev_nrm_grid),
                                     d->max_batch, d->H, d->W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, rp->lambda_po2pl,
                                     rp->loss_flags & ~DELORA_TRAIN_NORMALIZATION_SCALING, f(p.losses), f(p.grad_T),
@@ -1051,12 +1072,13 @@ extern "C" int delora_odometry_streams_load_weights(const delora_odometry_desc* 
     return load_weights(p, weights, workspace, (cudaStream_t)stream, who);
 }
 
-// delora_odometry_streams_push (rp NULL) and delora_odometry_streams_push_residual (arguments checked by the callers)
+// delora_odometry_streams_push (rp NULL), delora_odometry_streams_push_residual and, with info, _streams_push_info
+// (arguments checked by the callers)
 static int run_streams_push(const delora_odometry_desc* d, const delora_odometry_residual_params* rp, const float* points,
                             const int32_t* n_points, const int32_t* active, void* workspace, float* T, int32_t* valid,
-                            float* losses, cudaStream_t st) {
+                            float* losses, float* info, cudaStream_t st) {
     InferPlan p;
-    make_streams_plan(d, rp ? Streams::residual : Streams::plain, &p);
+    make_streams_plan(d, info ? Streams::info : rp ? Streams::residual : Streams::plain, &p);
     char* ws = (char*)workspace;
     const int S = d->max_batch, H = d->H, W = d->W;
     float* cur = reinterpret_cast<float*>(ws + p.f.images);
@@ -1107,6 +1129,10 @@ static int run_streams_push(const delora_odometry_desc* d, const delora_odometry
     odometry_streams_grids_kernel<1><<<blocks, 256, 0, st>>>(pts_grid, nrm_grid, prev_pts, prev_nrm, active, valid, S, HW,
                                                              T, T12, icp_losses, losses);
     DELORA_CHECK_LAUNCH("odometry_streams_grids_kernel<1>");
+    if (!info) return 0;
+    const int n = S * DELORA_INFO_ROW;
+    odometry_streams_info_kernel<<<(n + 255) / 256, 256, 0, st>>>(valid, S, reinterpret_cast<float*>(ws + p.info), info);
+    DELORA_CHECK_LAUNCH("odometry_streams_info_kernel");
     return 0;
 }
 
@@ -1116,7 +1142,8 @@ extern "C" int delora_odometry_streams_push(const delora_odometry_desc* d, const
     const char* who = "delora_odometry_streams_push";
     if (check_desc(d, who)) return 1;
     if (check_tick(points, n_points, workspace, T, valid, nullptr, nullptr, who)) return 1;
-    return run_streams_push(d, nullptr, points, n_points, active, workspace, T, valid, nullptr, (cudaStream_t)stream);
+    return run_streams_push(d, nullptr, points, n_points, active, workspace, T, valid, nullptr, nullptr,
+                            (cudaStream_t)stream);
 }
 
 extern "C" int64_t delora_odometry_streams_residual_workspace_bytes(const delora_odometry_desc* d) {
@@ -1135,7 +1162,27 @@ extern "C" int delora_odometry_streams_push_residual(const delora_odometry_desc*
     if (check_desc(d, who)) return 1;
     if (check_residual_params(rp, false, who)) return 1;
     if (check_tick(points, n_points, workspace, T, valid, losses, "losses", who)) return 1;
-    return run_streams_push(d, rp, points, n_points, active, workspace, T, valid, losses, (cudaStream_t)stream);
+    return run_streams_push(d, rp, points, n_points, active, workspace, T, valid, losses, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int64_t delora_odometry_streams_info_workspace_bytes(const delora_odometry_desc* d) {
+    return streams_workspace_bytes(d, Streams::info, "delora_odometry_streams_info_workspace_bytes");
+}
+
+extern "C" int delora_odometry_streams_info_init(const delora_odometry_desc* d, void* workspace, void* stream) {
+    return streams_init(d, Streams::info, workspace, (cudaStream_t)stream, "delora_odometry_streams_info_init");
+}
+
+extern "C" int delora_odometry_streams_push_info(const delora_odometry_desc* d, const delora_odometry_residual_params* rp,
+                                                 const float* points, const int32_t* n_points, const int32_t* active,
+                                                 void* workspace, float* T, int32_t* valid, float* losses, float* info,
+                                                 void* stream) {
+    const char* who = "delora_odometry_streams_push_info";
+    if (check_desc(d, who)) return 1;
+    if (check_residual_params(rp, false, who)) return 1;
+    if (check_tick(points, n_points, workspace, T, valid, losses, "losses", who)) return 1;
+    DELORA_CHECK_ARG(info, "%s: null info", who);
+    return run_streams_push(d, rp, points, n_points, active, workspace, T, valid, losses, info, (cudaStream_t)stream);
 }
 
 extern "C" int64_t delora_odometry_streams_normalized_workspace_bytes(const delora_odometry_desc* d) {

@@ -157,6 +157,21 @@ class ResidualStreamsWorkspace(StreamsWorkspace):
                    _ptr(active), self.workspace.data_ptr(), T.data_ptr(), valid.data_ptr(), losses.data_ptr())
 
 
+class InformationStreamsWorkspace(ResidualStreamsWorkspace):
+    """delora_odometry_streams_info_* on the residual layout with the information section appended: `push` also writes
+    each stream's information row (the Gauss-Newton information of the residual's objective at T).  load_weights /
+    reset are the streams calls."""
+    SIZE_QUERY = "delora_odometry_streams_info_workspace_bytes"
+    INIT = "delora_odometry_streams_info_init"
+
+    def push(self, points, counts, active, T, valid, losses, info):
+        """ResidualStreamsWorkspace.push plus info [S, INFO_ROW] out: the information row of every valid stream, zeros
+        elsewhere."""
+        self._call("delora_odometry_streams_push_info", self._params, points.data_ptr(), counts.data_ptr(),
+                   _ptr(active), self.workspace.data_ptr(), T.data_ptr(), valid.data_ptr(), losses.data_ptr(),
+                   info.data_ptr())
+
+
 class NormalizedStreamsWorkspace(StreamsWorkspace):
     """delora_odometry_streams_normalized_* for a model trained with normalization_scaling, on the streams layout with
     the normalised sections appended: `push` also writes each pair's factor.  load_weights / reset are the streams

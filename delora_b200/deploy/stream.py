@@ -263,7 +263,7 @@ class OdometryStreams(_Streams):
         self._setup(model, config, dataset, n_streams, n_max, use_cuda_graph, residual, residual_flags, False)
 
     def _setup(self, model, config, dataset, n_streams, n_max, use_cuda_graph, residual, residual_flags, normalized,
-               pre=False):
+               pre=False, info=False):
         from . import capi, export
         self.config = config
         self.dataset = dataset
@@ -276,10 +276,12 @@ class OdometryStreams(_Streams):
         self.residual = bool(residual) or pre
         self.normalized = bool(normalized)
         # the tick's outputs in the order the workspace's push takes them: T and valid, the residual's losses, the
-        # normalised kinds' factor
+        # information rows, the normalised kinds' factor
         outputs = [("T", (S, 4, 4), np.float32), ("valid", (S,), np.int32)]
         if self.residual:
             outputs.append(("losses", (S, ops.LOSS_ROW), np.float32))
+        if info:
+            outputs.append(("info", (S, ops.INFO_ROW), np.float32))
         if normalized:
             outputs.append(("factor", (S,), np.float32))
         with torch.cuda.device(self.device):
@@ -287,6 +289,9 @@ class OdometryStreams(_Streams):
             if pre:
                 flags = residual_flags | (ops.TRAIN_NORMALIZATION_SCALING if normalized else 0)
                 self.workspace = capi.PreStreamsWorkspace(self.desc, self.blob, capi.residual_params(config, flags))
+            elif info:
+                self.workspace = capi.InformationStreamsWorkspace(self.desc, self.blob,
+                                                                  capi.residual_params(config, residual_flags))
             elif self.residual:
                 self.workspace = capi.ResidualStreamsWorkspace(self.desc, self.blob,
                                                                capi.residual_params(config, residual_flags))
@@ -304,7 +309,7 @@ class OdometryStreams(_Streams):
         self._tick = tuple(dev_in) + tuple(dev_out)
         # what push returns beside T: the residual's losses and the recipe's factor (the normalised raw-scan streams
         # return T alone)
-        self._extras = (([self._out["losses"]] if self.residual else []) +
+        self._extras = (([self._out["losses"]] if self.residual else []) + ([self._out["info"]] if info else []) +
                         ([self._out["factor"]] if pre and normalized else []))
         self.relative = [[] for _ in range(S)]
         self.use_cuda_graph = bool(use_cuda_graph)
@@ -338,6 +343,23 @@ class OdometryStreams(_Streams):
             self.host_out.copy_(self.dev_out, non_blocking=True)
             torch.cuda.current_stream().synchronize()
         return self._results(self._out["T"], self._out["valid"], self._extras)
+
+
+class InformationOdometryStreams(OdometryStreams):
+    """OdometryStreams served from the information workspace (`delora_odometry_streams_push_info`): `push` returns, per
+    stream with a transform, (T [1, 4, 4], losses [LOSS_ROW], info [INFO_ROW]).  losses is residual=True's row; info
+    is the Gauss-Newton information of that residual's objective at T (include/delora_b200.h, DELORA_INFO_ROW): H
+    [0:36] (6 x 6, xi = (x, y, z, rot x, rot y, rot z) perturbing T on the right), its eigenvalues ascending [36:42]
+    and their unit eigenvectors [42:78], M and M' [78:80].  A small eigenvalue is a direction of the pose the frame
+    does not determine (a corridor, an open field, a flat wall).  The transforms and losses are the same bits as
+    residual=True's; `residual_flags` selects the losses; `poses` and `reset` are OdometryStreams'."""
+
+    def __init__(self, model, config, dataset, n_streams, n_max, use_cuda_graph=True,
+                 residual_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL):
+        if config.get("normalization_scaling", False):
+            raise ValueError("normalization_scaling: True is not supported by InformationOdometryStreams (the "
+                             "information is that of the residual workspace, which serves plain models)")
+        self._setup(model, config, dataset, n_streams, n_max, use_cuda_graph, True, residual_flags, False, info=True)
 
 
 class NormalizedOdometryStreams(OdometryStreams):

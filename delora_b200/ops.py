@@ -41,6 +41,7 @@ TRAIN_DROPOUT = 2048    # delora_odometry_train_step: the model uses use_dropout
 # tensor ids of the training step's dropout masks (delora_dropout_keep_mask)
 DROPOUT_INPUT, DROPOUT_STAGE3, DROPOUT_FC = 0, 1, 2
 LOSS_ROW, ICP_PARTIAL = 8, 40
+INFO_ROW = 80      # DELORA_INFO_ROW: H [0:36], eigenvalues [36:42], eigenvectors [42:78], M, M' [78:80]
 
 _keys_cache = {}
 
@@ -324,6 +325,32 @@ def icp_dense_fwd_bwd(src_grid, src_ngrid, transform, tgt_grid, tgt_ngrid, h, w,
         float(vfov[1]), float(lambda_po2pl), int(flags), losses.data_ptr(), grad_t.data_ptr(),
         scratch.data_ptr(), _stream()), "delora_icp_dense_fwd_bwd")
     return losses, grad_t
+
+
+def icp_dense_information(src_grid, src_ngrid, transform, tgt_grid, tgt_ngrid, h, w, hfov, vfov, lambda_po2pl=1.0,
+                          flags=LOSS_PO2PL | LOSS_PL2PL, scratch=None, info_scratch=None):
+    """icp_dense_fwd_bwd plus the Gauss-Newton information of the ICP objective at T (delora_icp_dense_information):
+    -> losses [B, LOSS_ROW], grad_T [B, 12] (the same bits as icp_dense_fwd_bwd), info [B, INFO_ROW] and nn [B, H*W]
+    int32, every source pixel's kept nearest neighbour (-1 where the losses keep no pair)."""
+    b = src_grid.shape[0]
+    dev = src_grid.device
+    losses = torch.empty((b, LOSS_ROW), dtype=torch.float32, device=dev)
+    grad_t = torch.empty((b, 12), dtype=torch.float32, device=dev)
+    info = torch.empty((b, INFO_ROW), dtype=torch.float32, device=dev)
+    if scratch is None:
+        scratch = icp_scratch(b, h * w, dev)
+    L = _lib.lib()
+    if info_scratch is None:
+        info_scratch = torch.empty((int(L.delora_icp_information_scratch_floats(b, h, w)),), dtype=torch.float32,
+                                   device=dev)
+    _lib.check(L.delora_icp_dense_information(
+        _req(src_grid, torch.float32, "src_grid"), _req(src_ngrid, torch.float32, "src_ngrid"),
+        _req(transform, torch.float32, "transform"), _req(tgt_grid, torch.float32, "tgt_grid"),
+        _req(tgt_ngrid, torch.float32, "tgt_ngrid"), b, h, w, float(hfov[0]), float(hfov[1]), float(vfov[0]),
+        float(vfov[1]), float(lambda_po2pl), int(flags), losses.data_ptr(), grad_t.data_ptr(),
+        scratch.data_ptr(), info.data_ptr(), info_scratch.data_ptr(), _stream()), "delora_icp_dense_information")
+    nn = info_scratch[:b * h * w].view(torch.int32).view(b, h * w)
+    return losses, grad_t, info, nn
 
 
 def icp_stats(reset=True):

@@ -2,7 +2,7 @@
  * Several LiDAR streams from a C host, batched in one workspace: no Python, no torch.  Links libdelora_b200.so and
  * cudart only.
  *
- *   odometry_streams [--residual | --preprocessing] model.dlw stream0_dir stream1_dir ...
+ *   odometry_streams [--residual | --information | --preprocessing] model.dlw stream0_dir stream1_dir ...
  *   odometry_streams --adapt LR --adapt-out adapted.dlw [--gpus N] model.dlw stream0_dir stream1_dir ...
  *   odometry_streams --adapt LR --adapt-out adapted.dlw [--geometry DIR,H,W,VFOV0,VFOV1[,W_PRE]]... model.dlw
  *                    stream0_dir ...
@@ -15,6 +15,10 @@
  * --residual serves the streams through delora_odometry_streams_push_residual and appends to each line the frame's ICP
  * residual against the stream's previous frame: the point-to-plane loss, the plane-to-plane loss and the matched pairs
  * (normals on the model's image, 7 x 11 neighbourhood, the reference's defaults).  The transforms are the same bits.
+ * --information serves the streams through delora_odometry_streams_push_info: the --residual columns, then how well the
+ * frame determines its transform (the Gauss-Newton information H of the residual's objective at T): H's smallest
+ * eigenvalue, its unit eigenvector (x, y, z, rot x, rot y, rot z: the direction the frame constrains least) and the
+ * ratio of the largest eigenvalue to the smallest (large in a corridor, an open field or at a flat wall).
  * A model trained with normalization_scaling (model_flags has DELORA_MODEL_NORMALIZATION_SCALING) is served through
  * delora_odometry_streams_push_normalized, with the same output; --residual is refused for such a model.
  * --preprocessing serves the streams on the reference's two-resolution recipe through delora_odometry_streams_push_pre:
@@ -52,6 +56,7 @@
  *            -L $CUDA_HOME/lib64 -lcudart -lpthread -Wl,-rpath,$PWD/delora_b200 -o odometry_streams
  */
 #include <dirent.h>
+#include <math.h>
 #include <pthread.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -422,12 +427,14 @@ int main(int argc, char** argv) {
             free(dir);
         }
     }
-    const int residual = argc > 1 && strcmp(argv[1], "--residual") == 0;
+    const int information = argc > 1 && strcmp(argv[1], "--information") == 0;
+    const int residual = information || (argc > 1 && strcmp(argv[1], "--residual") == 0);
     const int pre = argc > 1 && strcmp(argv[1], "--preprocessing") == 0;
     if (residual || pre) { --argc; ++argv; }
-    if (adapt && (residual || pre)) return fail("--adapt serves its own residual: drop --residual / --preprocessing");
+    if (adapt && (residual || pre)) return fail("--adapt serves its own residual: drop --residual / --information / --preprocessing");
     if (argc < 3)
-        return fail("usage: odometry_streams [--residual | --preprocessing] model.dlw stream_dir [stream_dir ...]");
+        return fail("usage: odometry_streams [--residual | --information | --preprocessing] model.dlw stream_dir "
+                    "[stream_dir ...]");
     const int S_dirs = argc - 2;              /* the streams of the header's geometry */
     const int S = S_dirs + n_geom;            /* every stream, the --geometry ones last */
 
@@ -496,7 +503,7 @@ int main(int argc, char** argv) {
     cudaStream_t stream;
     CUDA_OK(cudaStreamCreate(&stream));
     const size_t pts_floats = (size_t)S * 3 * d->n_stride;
-    float *weights, *points, *T, *losses, *factor;
+    float *weights, *points, *T, *losses, *factor, *info;
     delora_odometry_residual_params rp;
     rp.lambda_po2pl = 1.0f;
     rp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL;
@@ -509,6 +516,7 @@ int main(int argc, char** argv) {
     const int64_t ws_bytes = n_geom       ? delora_odometry_streams_adapt_geometries_workspace_bytes(descs, n_sets)
                              : adapt      ? delora_odometry_streams_adapt_workspace_bytes(d)
                              : pre        ? delora_odometry_streams_pre_workspace_bytes(d)
+                             : information ? delora_odometry_streams_info_workspace_bytes(d)
                              : residual   ? delora_odometry_streams_residual_workspace_bytes(d)
                              : normalized ? delora_odometry_streams_normalized_workspace_bytes(d)
                                           : delora_odometry_streams_workspace_bytes(d);
@@ -522,6 +530,7 @@ int main(int argc, char** argv) {
     CUDA_OK(cudaMalloc((void**)&T, (size_t)S * 16 * sizeof(float)));
     CUDA_OK(cudaMalloc((void**)&losses, (size_t)S * DELORA_LOSS_ROW * sizeof(float)));
     CUDA_OK(cudaMalloc((void**)&factor, (size_t)S * sizeof(float)));
+    CUDA_OK(cudaMalloc((void**)&info, (size_t)S * DELORA_INFO_ROW * sizeof(float)));
     CUDA_OK(cudaMemcpy(weights, h_blob, (size_t)n_weights * sizeof(float), cudaMemcpyHostToDevice));
     /* --geometry: geometry g's scans and counts start at its first stream's row */
     const float* g_points[MAX_GEOMETRIES];
@@ -537,6 +546,7 @@ int main(int argc, char** argv) {
         DELORA_OK(delora_odometry_streams_adapt_init(d, weights, workspace, stream));
     } else {
         if (pre) DELORA_OK(delora_odometry_streams_pre_init(d, workspace, stream));
+        else if (information) DELORA_OK(delora_odometry_streams_info_init(d, workspace, stream));
         else if (residual) DELORA_OK(delora_odometry_streams_residual_init(d, workspace, stream));
         else if (normalized) DELORA_OK(delora_odometry_streams_normalized_init(d, workspace, stream));
         else DELORA_OK(delora_odometry_streams_init(d, workspace, stream));
@@ -549,7 +559,9 @@ int main(int argc, char** argv) {
     int32_t* h_valid = (int32_t*)malloc((size_t)S * sizeof(int32_t));
     float* h_T = (float*)malloc((size_t)S * 16 * sizeof(float));
     float* h_losses = (float*)calloc((size_t)S * DELORA_LOSS_ROW, sizeof(float));
-    if (!h_points || !h_count || !h_active || !h_valid || !h_T || !h_losses) return fail("out of host memory");
+    float* h_info = (float*)calloc((size_t)S * DELORA_INFO_ROW, sizeof(float));
+    if (!h_points || !h_count || !h_active || !h_valid || !h_T || !h_losses || !h_info)
+        return fail("out of host memory");
     for (int k = 0; k < ticks; ++k) {
         for (int s = 0; s < S; ++s) {
             h_active[s] = k < lists[s].n;
@@ -571,9 +583,15 @@ int main(int argc, char** argv) {
             else if (pre)
                 DELORA_OK(delora_odometry_streams_push_pre(d, &rp, points, count, active, workspace, T, valid, losses,
                                                            normalized ? factor : NULL, stream));
+            else if (information)
+                DELORA_OK(delora_odometry_streams_push_info(d, &rp, points, count, active, workspace, T, valid, losses,
+                                                            info, stream));
             else
                 DELORA_OK(delora_odometry_streams_push_residual(d, &rp, points, count, active, workspace, T, valid,
                                                                 losses, stream));
+            if (information)
+                CUDA_OK(cudaMemcpyAsync(h_info, info, (size_t)S * DELORA_INFO_ROW * sizeof(float),
+                                        cudaMemcpyDeviceToHost, stream));
             CUDA_OK(cudaMemcpyAsync(h_losses, losses, (size_t)S * DELORA_LOSS_ROW * sizeof(float), cudaMemcpyDeviceToHost,
                                     stream));
         } else if (normalized) {
@@ -592,6 +610,12 @@ int main(int argc, char** argv) {
             if (adapt || pre || residual) {
                 const float* l = h_losses + (size_t)s * DELORA_LOSS_ROW;
                 printf(" %.9g %.9g %.0f", l[1], l[2], l[3]);
+            }
+            if (information) {      /* [36, 42): eigenvalues ascending; [42, 48): the smallest one's eigenvector */
+                const float* r = h_info + (size_t)s * DELORA_INFO_ROW;
+                printf(" %.9g", r[36]);
+                for (int i = 0; i < 6; ++i) printf(" %.6f", r[42 + i]);
+                printf(" %.9g", r[36] > 0.0f ? r[41] / r[36] : INFINITY);
             }
             printf("\n");
         }
@@ -612,6 +636,7 @@ int main(int argc, char** argv) {
     }
     free(lists);
     for (int g = 0; g < n_geom; ++g) free(geom_dirs[g]);
+    free(h_info);
     free(h_losses);
     free(h_T);
     free(h_valid);
@@ -619,6 +644,7 @@ int main(int argc, char** argv) {
     free(h_count);
     free(h_points);
     free(h_blob);
+    cudaFree(info);
     cudaFree(factor);
     cudaFree(losses);
     cudaFree(T);

@@ -51,6 +51,10 @@ typedef struct { float x, y, z, w; } delora_f4;
 #define DELORA_LOSS_ROW 8   /* [po2po, po2pl, pl2pl, M_pairs, M_po2po, 0, 0, 0] */
 /* number of floats per block-partial row in the icp workspace */
 #define DELORA_ICP_PARTIAL 40
+/* number of floats in one row of the `info` output of delora_icp_dense_information:
+ * [0, 36) H row-major, [36, 42) its eigenvalues ascending, [42, 78) the unit eigenvector of eigenvalue k at 42 + 6 k,
+ * 78 M_pairs, 79 M_po2po */
+#define DELORA_INFO_ROW 80
 
 int         delora_abi_version(void);
 const char* delora_last_error(void);
@@ -256,6 +260,47 @@ int delora_icp_dense_fwd_bwd(const delora_f4* src_grid, const delora_f4* src_ngr
                              double hfov0, double hfov1, double vfov0, double vfov1,
                              float lambda_po2pl, uint32_t flags, float* losses, float* grad_T,
                              float* scratch, void* stream);
+
+/* How well each pair constrains its transform: the Gauss-Newton information of the ICP objective at T, beside the
+ * losses.  LiDAR odometry fails in degenerate scenes (a corridor or tunnel, a flat field, a single wall) where the
+ * residual is low and yet some direction of the pose is unobservable; H says which.  It needs no ground truth, uses
+ * the exact correspondences of the losses and leaves T unchanged.
+ *
+ * Per pair: source point p and normal m (before the transform), T = (R | t), s = R p + t; q, n_t: the matched target
+ * point and normal (the exact NN, with the masks of the losses).  T is perturbed on the right, in the source frame:
+ * T(xi) = T Exp(xi), xi = (rho, phi) = (x, y, z, rot x, rot y, rot z), ROS's covariance order; to first order
+ * s(xi) = s + R rho - R [p]x phi.  With u = R^T n_t and R_k the rows of R, the Jacobians per kept pair are
+ *   po2pl (a normal on both sides, DELORA_LOSS_PO2PL)   r = n_t.(s - q)          J = [u, p x u]            (1 x 6)
+ *   pl2pl squared (both sides, DELORA_LOSS_PL2PL)       e = R m - n_t            J = [0, -R [m]x]          (3 x 6)
+ *   pl2pl linear (with DELORA_NORMAL_LINEAR)            o = 1 - n_t.(R m)        J = [0, u x m]            (1 x 6)
+ *   po2po (a normal on neither side, DELORA_LOSS_PO2PO) d = s - q                J = [R, -R [p]x]          (3 x 6)
+ * and, over the enabled terms only,
+ *   H = 2 (lambda_po2pl / M  sum_po2pl J^T J  +  1 / M  sum_pl2pl J^T J  +  1 / (3 M')  sum_po2po J^T J),
+ * the Gauss-Newton approximation of the Hessian in xi of po2po + lambda_po2pl po2pl + pl2pl with the losses' own means
+ * (po2pl and pl2pl over the M pairs with a normal on both sides, po2po over the 3 M' coordinates of the M' pairs
+ * with a normal on neither); a term whose count is 0 contributes nothing.  Its eigenvalues say how well the pair
+ * constrains the pose, its eigenvectors in which directions: a near-zero eigenvalue is a direction the frame does not
+ * determine.  No covariance is returned, because any covariance needs a noise model and that is the host's choice;
+ * sigma^2 H^-1 (sigma^2 the variance of one residual, over the directions whose eigenvalue is not near zero) is one way
+ * to build one, e.g. for the 6 x 6 covariance of a ROS nav_msgs/Odometry.
+ *
+ * info [B, DELORA_INFO_ROW] out (layout above): H from fp32 per-pair J^T J and fp32 sums over each warp of 32 source
+ * pixels, then float64 sums over the warps in a fixed order, the weights in float64, stored as fp32; the eigenvalues
+ * and eigenvectors by a float64 cyclic Jacobi solve of that float64 H; each eigenvector's largest-magnitude component
+ * (the first of equals) is positive.  Bit-identical from run to run; a pair's row does not depend on B or on the other
+ * pairs.  losses and grad_T: bit-identical to delora_icp_dense_fwd_bwd on the same inputs (the same search kernels,
+ * instantiated to also write the NN ids; the scratch layout is the same).
+ * info_scratch: fp32 [delora_icp_information_scratch_floats(B, H, W)], no initialisation needed; after the call its
+ * first B * H * W int32 are the id of every source pixel's kept nearest neighbour (-1 where the losses keep no pair).
+ * Refused: what delora_icp_dense_fwd_bwd refuses, null info / info_scratch, DELORA_ICP_STATS in flags.
+ * Cost beside delora_icp_dense_fwd_bwd: two launches, icp_info_rows_kernel and icp_info_finalize_kernel (measured
+ * below, with delora_odometry_streams_push_info). */
+int64_t delora_icp_information_scratch_floats(int B, int H, int W);     /* host only, -1 for a bad shape */
+int delora_icp_dense_information(const delora_f4* src_grid, const delora_f4* src_ngrid, const float* T,
+                                 const delora_f4* tgt_grid, const delora_f4* tgt_ngrid, int B, int H, int W,
+                                 double hfov0, double hfov1, double vfov0, double vfov1,
+                                 float lambda_po2pl, uint32_t flags, float* losses, float* grad_T,
+                                 float* scratch, float* info, float* info_scratch, void* stream);
 
 /* Diagnostic for delora_icp_dense_fwd_bwd calls made with DELORA_ICP_STATS in `flags`: copies the 32 device
  * counters to the HOST array out32 (may be NULL) and optionally zeroes them.  [0] warps, [1] window-growing steps,
@@ -625,6 +670,41 @@ int delora_odometry_streams_residual_init(const delora_odometry_desc* d, void* w
 int delora_odometry_streams_push_residual(const delora_odometry_desc* d, const delora_odometry_residual_params* rp,
                                           const float* points, const int32_t* n_points, const int32_t* active,
                                           void* workspace, float* T, int32_t* valid, float* losses, void* stream);
+
+/* How well each streamed frame determines its transform, beside the residual: the Gauss-Newton information of the
+ * residual's ICP objective at the served T (delora_icp_dense_information), so that a host can tell a frame of a
+ * degenerate scene (corridor, open field, flat wall: low residual, an unobservable direction) from a good one, give a
+ * fusion filter a covariance or flag the frame.  A diagnostic: T is what _streams_push_residual serves.
+ *
+ * The information workspace is the residual workspace with one section appended: no offset of the residual layout
+ * moves, so delora_odometry_streams_load_weights and delora_odometry_streams_reset work on it unchanged (_info_init
+ * replaces _residual_init).  Appended (256-byte aligned): the information rows of the S pairs and the operator's
+ * info_scratch at B = S (delora_icp_information_scratch_floats(S, H, W): 4 bytes per cell and stream for the NN ids,
+ * 8 bytes per cell and stream for the partial rows, a 64-float row per 32 cells), 12 bytes per cell and stream in all: at 64 x 2048,
+ * 1.5 MiB per stream; at 64 x 720, 0.53 MiB per stream.
+ *
+ * delora_odometry_streams_push_info: the arguments of delora_odometry_streams_push_residual plus info
+ * [S, DELORA_INFO_ROW] (device, required).  T, valid and losses are what _streams_push_residual writes for the same
+ * history, byte for byte; info[s] is the row delora_icp_dense_information writes for that pair, bit-identical to the
+ * operator run alone at B = 1 on the two frames, for every stream with valid[s] = 1; rows with valid[s] = 0 are zeros.
+ * Graph-capturable like _streams_push_residual (the launch sequence depends on neither `active` nor the stream state).
+ * Refused before any launch: everything _streams_push_residual refuses, and a null info.
+ * Measured on one H100 80GB HBM3 at a 700 W power limit (max SM clock 1980 MHz), graph-replayed ticks, all streams
+ * active, near-identity heads on consecutive synthetic frames, medians of alternating samples,
+ * _streams_push_residual -> _streams_push_info per tick: 64 x 2048: S = 1 1.28 -> 1.34 ms, S = 4 2.31 -> 2.42 ms, S
+ * = 16 8.71 -> 8.96 ms; 64 x 720: S = 1 1.18 -> 1.22 ms, S = 4 1.39 -> 1.43 ms, S = 16 5.12 -> 5.19 ms. Of that, per
+ * tick (torch.profiler): icp_info_rows_kernel 4.3 / 16.4 / 60.0 us at 64 x 2048 (S = 1 / 4 / 16), 2.4 / 5.3 / 23.9
+ * us at 64 x 720; icp_info_finalize_kernel 57 / 63 / 90 us and 32 / 33 / 41 us, almost all of it the float64 Jacobi
+ * solve, which runs on one thread per pair (scripts/gpu_odometry_streams_info.py,
+ * profiles/odometry_streams_info_h100_700w.json). */
+int64_t delora_odometry_streams_info_workspace_bytes(const delora_odometry_desc* d);   /* host only, -1 if invalid */
+/* Zero the workspace, arm the projection keys and empty the cached grids.  Once after allocation, instead of
+ * delora_odometry_streams_residual_init. */
+int delora_odometry_streams_info_init(const delora_odometry_desc* d, void* workspace, void* stream);
+int delora_odometry_streams_push_info(const delora_odometry_desc* d, const delora_odometry_residual_params* rp,
+                                      const float* points, const int32_t* n_points, const int32_t* active,
+                                      void* workspace, float* T, int32_t* valid, float* losses, float* info,
+                                      void* stream);
 
 /* Several streams of a model flagged DELORA_MODEL_NORMALIZATION_SCALING in one workspace.  Such a model sees each pair
  * divided by the factor of that pair, so a stream's previous frame is projected anew every tick: the workspace keeps
