@@ -85,6 +85,10 @@ SIGNATURES = {
     "delora_icp_dense_information": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                              c_double, c_double, c_double, c_double, c_float, c_u32, c_void_p,
                                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "delora_icp_dense_information_scaled": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                                    c_int, c_double, c_double, c_double, c_double, c_float, c_u32,
+                                                    c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                    c_void_p]),
     "delora_icp_fwd_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                    c_int, c_int, c_int, c_int, c_double, c_double, c_double, c_double, c_float,
                                    c_u32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
@@ -159,6 +163,10 @@ SIGNATURES = {
     "delora_odometry_streams_pre_init": (c_int, [c_desc_p, c_void_p, c_void_p]),
     "delora_odometry_streams_push_pre": (c_int, [c_desc_p, c_residual_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_streams_pre_info_workspace_bytes": (c_i64, [c_desc_p]),
+    "delora_odometry_streams_pre_info_init": (c_int, [c_desc_p, c_void_p, c_void_p]),
+    "delora_odometry_streams_push_pre_info": (c_int, [c_desc_p, c_residual_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_train_workspace_bytes": (c_i64, [c_desc_p]),
     "delora_odometry_train_init": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_train_step": (c_int, [c_desc_p, c_train_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
@@ -184,6 +192,13 @@ SIGNATURES = {
     "delora_odometry_streams_adapt_group_init": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_streams_push_adapt_group": (c_int, [c_desc_p, c_train_p, c_group_p, c_int, c_void_p, c_void_p,
                                                          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_streams_adapt_info_workspace_bytes": (c_i64, [c_desc_p]),
+    "delora_odometry_streams_adapt_info_init": (c_int, [c_desc_p, c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_streams_push_adapt_info": (c_int, [c_desc_p, c_train_p, c_int, c_void_p, c_void_p, c_void_p,
+                                                        c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_streams_push_adapt_group_info": (c_int, [c_desc_p, c_train_p, c_group_p, c_int, c_void_p,
+                                                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                              c_void_p, c_void_p, c_void_p]),
     "delora_odometry_streams_adapt_geometries_workspace_bytes": (c_i64, [c_desc_p, c_int]),
     "delora_odometry_streams_adapt_geometries_init": (c_int, [c_desc_p, c_int, c_void_p, c_void_p, c_void_p]),
     "delora_odometry_streams_push_adapt_geometries": (c_int, [c_desc_p, c_int, c_train_p, c_int, c_void_p, c_void_p,

@@ -340,9 +340,10 @@ inline IcpInfoLayout icp_info_layout(int B, int HW) {
     return L;
 }
 
-// icp_info.cu: the information pass after the dense search (which wrote the NN ids) and the finalize (losses)
+// icp_info.cu: the information pass after the dense search (which wrote the NN ids) and the finalize (losses); factor
+// [B] or NULL: H in metres for pairs whose clouds were divided by factor[b] (delora_icp_dense_information_scaled)
 int launch_icp_information(const float4* src_grid, const float4* src_ngrid, const float* T, const float4* tgt_ngrid, int B, int HW, float lambda_po2pl, uint32_t flags,
-                           const float* losses, float* info_scratch, float* info, cudaStream_t st);
+                           const float* losses, float* info_scratch, float* info, const float* factor, cudaStream_t st);
 
 int launch_icp_finalize(const IcpScratch& sc, int B, int rows, float lambda_po2pl, float* losses, float* grad_T,
                         cudaStream_t st);

@@ -806,19 +806,42 @@ extern "C" int64_t delora_icp_information_scratch_floats(int B, int H, int W) {
     return icp_info_layout(B, H * W).total;
 }
 
-extern "C" int delora_icp_dense_information(const delora_f4* src_grid, const delora_f4* src_ngrid, const float* T,
-                                            const delora_f4* tgt_grid, const delora_f4* tgt_ngrid, int B, int H, int W,
-                                            double hfov0, double hfov1, double vfov0, double vfov1, float lambda_po2pl,
-                                            uint32_t flags, float* losses, float* grad_T, float* scratch, float* info,
-                                            float* info_scratch, void* stream) {
-    const char* who = "delora_icp_dense_information";
+// delora_icp_dense_information (factor NULL) and delora_icp_dense_information_scaled
+static int dense_information(const delora_f4* src_grid, const delora_f4* src_ngrid, const float* T,
+                             const delora_f4* tgt_grid, const delora_f4* tgt_ngrid, int B, int H, int W, double hfov0,
+                             double hfov1, double vfov0, double vfov1, float lambda_po2pl, uint32_t flags, float* losses,
+                             float* grad_T, float* scratch, float* info, float* info_scratch, const float* factor,
+                             cudaStream_t st, const char* who) {
     DELORA_CHECK_ARG(info && info_scratch, "%s: null pointer", who);
     DELORA_CHECK_ARG((flags & DELORA_ICP_STATS) == 0u, "%s: DELORA_ICP_STATS is not counted here", who);
-    cudaStream_t st = (cudaStream_t)stream;
     int* nn_ids = reinterpret_cast<int*>(info_scratch);
     const int rc = dense_icp(src_grid, src_ngrid, T, tgt_grid, tgt_ngrid, B, H, W, hfov0, hfov1, vfov0, vfov1,
                              lambda_po2pl, flags, losses, grad_T, scratch, nn_ids, st, who);
     if (rc != 0) return rc;
     return launch_icp_information((const float4*)src_grid, (const float4*)src_ngrid, T, (const float4*)tgt_ngrid, B, H * W, lambda_po2pl, flags, losses, info_scratch, info,
-                                  st);
+                                  factor, st);
+}
+
+extern "C" int delora_icp_dense_information(const delora_f4* src_grid, const delora_f4* src_ngrid, const float* T,
+                                            const delora_f4* tgt_grid, const delora_f4* tgt_ngrid, int B, int H, int W,
+                                            double hfov0, double hfov1, double vfov0, double vfov1, float lambda_po2pl,
+                                            uint32_t flags, float* losses, float* grad_T, float* scratch, float* info,
+                                            float* info_scratch, void* stream) {
+    return dense_information(src_grid, src_ngrid, T, tgt_grid, tgt_ngrid, B, H, W, hfov0, hfov1, vfov0, vfov1,
+                             lambda_po2pl, flags, losses, grad_T, scratch, info, info_scratch, nullptr,
+                             (cudaStream_t)stream, "delora_icp_dense_information");
+}
+
+extern "C" int delora_icp_dense_information_scaled(const delora_f4* src_grid, const delora_f4* src_ngrid,
+                                                   const float* T, const delora_f4* tgt_grid,
+                                                   const delora_f4* tgt_ngrid, int B, int H, int W, double hfov0,
+                                                   double hfov1, double vfov0, double vfov1, float lambda_po2pl,
+                                                   uint32_t flags, float* losses, float* grad_T, float* scratch,
+                                                   float* info, float* info_scratch, const float* factor,
+                                                   void* stream) {
+    const char* who = "delora_icp_dense_information_scaled";
+    DELORA_CHECK_ARG(factor, "%s: null factor", who);
+    return dense_information(src_grid, src_ngrid, T, tgt_grid, tgt_ngrid, B, H, W, hfov0, hfov1, vfov0, vfov1,
+                             lambda_po2pl, flags, losses, grad_T, scratch, info, info_scratch, factor,
+                             (cudaStream_t)stream, who);
 }

@@ -171,9 +171,13 @@ __device__ void jacobi6(double (&a)[6][6], double (&v)[6][6]) {
 
 // One CTA per pair.  Thread (column c = tid % 64, group g = tid / 64) sums rows g, g + 4, ... of column c in float64,
 // the groups are added in order; thread 0 then weights the three terms into H (float64), solves it and writes the row.
+// kScaled (delora_icp_dense_information_scaled): the pair's clouds were divided by factor[b], so H is taken in xi =
+// (rho / f, phi); H_m = D H D, D = diag(1/f, 1/f, 1/f, 1, 1, 1), is H in metres and radians.  D is applied to the
+// float64 H before it is stored and solved, so the eigen-pairs are H_m's; with f = 1 every product is by 1.0, exact.
+template <bool kScaled>
 __global__ void __launch_bounds__(kInfoFinThreads)
 icp_info_finalize_kernel(const float* __restrict__ partials, int rows, float lambda_po2pl, uint32_t flags,
-                         const float* __restrict__ losses, float* __restrict__ info) {
+                         const float* __restrict__ losses, float* __restrict__ info, const float* __restrict__ factor) {
     __shared__ double red[kInfoGroups][kInfoPartial];
     __shared__ double sum[kInfoPartial];
     __shared__ double evec[6][6], eval[6];
@@ -199,13 +203,18 @@ icp_info_finalize_kernel(const float* __restrict__ partials, int rows, float lam
     const double w_pl = (M > 0.0f && (flags & DELORA_LOSS_PO2PL)) ? 2.0 * (double)lambda_po2pl / (double)M : 0.0;
     const double w_nn = (M > 0.0f && (flags & DELORA_LOSS_PL2PL)) ? 2.0 / (double)M : 0.0;
     const double w_pp = (Mp > 0.0f && (flags & DELORA_LOSS_PO2PO)) ? 2.0 / (3.0 * (double)Mp) : 0.0;
+    const double inv_f = kScaled ? 1.0 / (double)factor[b] : 1.0;
     double a[6][6], v[6][6];
     int k = 0;
 #pragma unroll
     for (int i = 0; i < 6; ++i) {
 #pragma unroll
         for (int j = i; j < 6; ++j, ++k) {
-            const double h = w_pl * sum[k] + w_nn * sum[kInfoSums + k] + w_pp * sum[2 * kInfoSums + k];
+            double h = w_pl * sum[k] + w_nn * sum[kInfoSums + k] + w_pp * sum[2 * kInfoSums + k];
+            if constexpr (kScaled) {
+                if (i < 3) h *= inv_f;
+                if (j < 3) h *= inv_f;
+            }
             a[i][j] = h;
             a[j][i] = h;
         }
@@ -246,15 +255,22 @@ icp_info_finalize_kernel(const float* __restrict__ partials, int rows, float lam
 }
 
 int launch_icp_information(const float4* src_grid, const float4* src_ngrid, const float* T, const float4* tgt_ngrid, int B, int HW, float lambda_po2pl, uint32_t flags,
-                           const float* losses, float* info_scratch, float* info, cudaStream_t st) {
+                           const float* losses, float* info_scratch, float* info, const float* factor, cudaStream_t st) {
     const IcpInfoLayout L = icp_info_layout(B, HW);
     const int* nn_ids = reinterpret_cast<const int*>(info_scratch + L.ids);
     float* partials = info_scratch + L.partials;
     icp_info_rows_kernel<<<dim3((HW + kInfoThreads - 1) / kInfoThreads, B), kInfoThreads, 0, st>>>(
         src_grid, src_ngrid, T, tgt_ngrid, HW, L.rows, flags, nn_ids, partials);
     DELORA_CHECK_LAUNCH("icp_info_rows_kernel");
-    icp_info_finalize_kernel<<<B, kInfoFinThreads, 0, st>>>(partials, L.rows, lambda_po2pl, flags, losses, info);
-    DELORA_CHECK_LAUNCH("icp_info_finalize_kernel");
+    if (factor) {
+        icp_info_finalize_kernel<true><<<B, kInfoFinThreads, 0, st>>>(partials, L.rows, lambda_po2pl, flags, losses, info,
+                                                                      factor);
+        DELORA_CHECK_LAUNCH("icp_info_finalize_kernel<true>");
+    } else {
+        icp_info_finalize_kernel<false><<<B, kInfoFinThreads, 0, st>>>(partials, L.rows, lambda_po2pl, flags, losses, info,
+                                                                       nullptr);
+        DELORA_CHECK_LAUNCH("icp_info_finalize_kernel<false>");
+    }
     return 0;
 }
 

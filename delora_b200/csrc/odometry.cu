@@ -325,14 +325,16 @@ static void make_infer_plan(const delora_odometry_desc* d, InferPlan* p) {
 //   pre (_push_pre): residual (its H x W grids and ICP sections serve the recipe's ICP), then the H x w_pre sections.
 //     The plain layout's key buffers serve both H x W projections of a tick, its images hold this tick's projection
 //     of both frames of each pair.
-enum class Streams { plain, residual, normalized, pre, info };
+//   pre_info (_push_pre_info): pre, then info's information rows and scratch.
+enum class Streams { plain, residual, normalized, pre, info, pre_info };
 
 static void make_streams_plan(const delora_odometry_desc* d, Streams kind, InferPlan* p) {
     const int MB = d->max_batch;
     plan_inference(d, MB, MB, true, p);
     const size_t S = (size_t)MB, HW = (size_t)d->H * d->W, HWp = (size_t)d->H * d->w_pre;
     size_t off = p->total;
-    if (kind == Streams::residual || kind == Streams::pre || kind == Streams::info) {
+    const bool pre = kind == Streams::pre || kind == Streams::pre_info;
+    if (kind == Streams::residual || pre || kind == Streams::info) {
         p->pts_grid = take(off, S * HW * 16);
         p->nrm_grid = take(off, S * HW * 16);
         p->prev_pts_grid = take(off, S * HW * 16);
@@ -342,16 +344,12 @@ static void make_streams_plan(const delora_odometry_desc* d, Streams kind, Infer
         p->grad_T = take(off, S * 12 * 4);
         p->icp = take(off, (size_t)delora_icp_scratch_floats(MB, (int)HW) * 4);
     }
-    if (kind == Streams::info) {
-        p->info = take(off, S * DELORA_INFO_ROW * 4);
-        p->info_scratch = take(off, (size_t)delora_icp_information_scratch_floats(MB, d->H, d->W) * 4);
-    }
     if (kind == Streams::normalized) {
         p->stage = take(off, 2 * S * 3 * (size_t)d->n_stride * 4);
         p->stage_counts = take(off, 3 * S * 4);
         p->factor = take(off, S * 4);
     }
-    if (kind == Streams::pre) {
+    if (pre) {
         p->pre_keys = take(off, S * HWp * 8);
         p->pre_image = take(off, S * 4 * HWp * 4);
         p->pre_index_map = take(off, S * HWp * 4);
@@ -359,6 +357,10 @@ static void make_streams_plan(const delora_odometry_desc* d, Streams kind, Infer
         p->pre_nrm = take(off, 2 * S * HWp * 16);
         p->T16 = take(off, S * 16 * 4);
         p->factor = take(off, S * 4);
+    }
+    if (kind == Streams::info || kind == Streams::pre_info) {
+        p->info = take(off, S * DELORA_INFO_ROW * 4);
+        p->info_scratch = take(off, (size_t)delora_icp_information_scratch_floats(MB, d->H, d->W) * 4);
     }
     p->total = off;
 }
@@ -938,7 +940,7 @@ static int check_pre_desc(const delora_odometry_desc* d, const char* who) {
 }
 
 static int check_streams_desc(const delora_odometry_desc* d, Streams kind, const char* who) {
-    return kind == Streams::pre ? check_pre_desc(d, who) : check_desc(d, who);
+    return kind == Streams::pre || kind == Streams::pre_info ? check_pre_desc(d, who) : check_desc(d, who);
 }
 
 static int64_t streams_workspace_bytes(const delora_odometry_desc* d, Streams kind, const char* who) {
@@ -967,7 +969,7 @@ static int streams_init(const delora_odometry_desc* d, Streams kind, void* works
     if (rc) return rc;
     const size_t S = (size_t)d->max_batch;
     if (kind == Streams::residual || kind == Streams::info) return clear_grids(ws, p.prev_pts_grid, p.prev_nrm_grid, S * d->H * d->W, st);
-    if (kind == Streams::pre) {
+    if (kind == Streams::pre || kind == Streams::pre_info) {
         const size_t n = S * d->H * d->w_pre;
         const cudaError_t e = cudaMemsetAsync(ws + p.pre_keys, 0xFF, n * 8, st);
         DELORA_CHECK_ARG(e == cudaSuccess, "%s: %s", who, cudaGetErrorString(e));
@@ -1022,21 +1024,35 @@ static int streams_forward(const Model& m, const TailIO& io, const TrunkActs& t,
 }
 
 // The ICP at B = S on a residual or recipe plan's H x W grids: source pts_grid moved by T12, target prev_pts_grid,
-// into its losses and grad_T; on an information plan (p.info set) also into its information rows.  The recipe's
-// DELORA_TRAIN_NORMALIZATION_SCALING is not an ICP bit.
+// into its losses and grad_T; on an information plan (p.info set) also into its information rows, in metres with the
+// pair factors of a normalised recipe (factor non-NULL).  The recipe's DELORA_TRAIN_NORMALIZATION_SCALING is not an
+// ICP bit.
 static int streams_icp(const delora_odometry_desc* d, const delora_odometry_residual_params* rp, const InferPlan& p,
-                       char* ws, cudaStream_t st) {
+                       char* ws, const float* factor, cudaStream_t st) {
     auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
     auto f4 = [&](size_t o) { return reinterpret_cast<delora_f4*>(ws + o); };
+    const uint32_t flags = rp->loss_flags & ~DELORA_TRAIN_NORMALIZATION_SCALING;
+    if (p.info && factor)
+        return delora_icp_dense_information_scaled(f4(p.pts_grid), f4(p.nrm_grid), f(p.T12), f4(p.prev_pts_grid),
+                                                   f4(p.prev_nrm_grid), d->max_batch, d->H, d->W, d->hfov0, d->hfov1,
+                                                   d->vfov0, d->vfov1, rp->lambda_po2pl, flags, f(p.losses),
+                                                   f(p.grad_T), f(p.icp), f(p.info), f(p.info_scratch), factor, st);
     if (p.info)
         return delora_icp_dense_information(f4(p.pts_grid), f4(p.nrm_grid), f(p.T12), f4(p.prev_pts_grid),
                                             f4(p.prev_nrm_grid), d->max_batch, d->H, d->W, d->hfov0, d->hfov1,
-                                            d->vfov0, d->vfov1, rp->lambda_po2pl, rp->loss_flags, f(p.losses),
+                                            d->vfov0, d->vfov1, rp->lambda_po2pl, flags, f(p.losses),
                                             f(p.grad_T), f(p.icp), f(p.info), f(p.info_scratch), st);
     return delora_icp_dense_fwd_bwd(f4(p.pts_grid), f4(p.nrm_grid), f(p.T12), f4(p.prev_pts_grid), f4(p.prev_nrm_grid),
                                     d->max_batch, d->H, d->W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, rp->lambda_po2pl,
-                                    rp->loss_flags & ~DELORA_TRAIN_NORMALIZATION_SCALING, f(p.losses), f(p.grad_T),
-                                    f(p.icp), st);
+                                    flags, f(p.losses), f(p.grad_T), f(p.icp), st);
+}
+
+// info [S, DELORA_INFO_ROW] = the information rows at `rows` of the valid streams, zeros for the others
+static int streams_info_out(const int32_t* valid, int S, const float* rows, float* info, cudaStream_t st) {
+    const int n = S * DELORA_INFO_ROW;
+    odometry_streams_info_kernel<<<(n + 255) / 256, 256, 0, st>>>(valid, S, rows, info);
+    DELORA_CHECK_LAUNCH("odometry_streams_info_kernel");
+    return 0;
 }
 
 // delora_odometry_streams_reset and _streams_adapt_reset, on the has_prev flags at that offset
@@ -1125,15 +1141,11 @@ static int run_streams_push(const delora_odometry_desc* d, const delora_odometry
     odometry_streams_grids_kernel<0><<<blocks, 256, 0, st>>>(pts_grid, nrm_grid, prev_pts, prev_nrm, active, valid, S, HW,
                                                              T, T12, icp_losses, losses);
     DELORA_CHECK_LAUNCH("odometry_streams_grids_kernel<0>");
-    if ((rc = streams_icp(d, rp, p, ws, st))) return rc;
+    if ((rc = streams_icp(d, rp, p, ws, nullptr, st))) return rc;
     odometry_streams_grids_kernel<1><<<blocks, 256, 0, st>>>(pts_grid, nrm_grid, prev_pts, prev_nrm, active, valid, S, HW,
                                                              T, T12, icp_losses, losses);
     DELORA_CHECK_LAUNCH("odometry_streams_grids_kernel<1>");
-    if (!info) return 0;
-    const int n = S * DELORA_INFO_ROW;
-    odometry_streams_info_kernel<<<(n + 255) / 256, 256, 0, st>>>(valid, S, reinterpret_cast<float*>(ws + p.info), info);
-    DELORA_CHECK_LAUNCH("odometry_streams_info_kernel");
-    return 0;
+    return info ? streams_info_out(valid, S, reinterpret_cast<float*>(ws + p.info), info, st) : 0;
 }
 
 extern "C" int delora_odometry_streams_push(const delora_odometry_desc* d, const float* points, const int32_t* n_points,
@@ -1245,12 +1257,11 @@ extern "C" int delora_odometry_streams_pre_init(const delora_odometry_desc* d, v
 // count clamp, projection + normals of the S new frames at H x w_pre, the pair factors over the valid H x w_pre cells
 // (flagged models; cached frames are side 0, new ones side 1), both frames of every pair projected to H x W (scaled by
 // the pair's factor when flagged), the trunk input, trunk and tail at B = S, the output kernel into T16, the
-// bookkeeping kernel (T, T12, factor, emptied sources, cache write), the ICP at B = S and the masked loss rows.
-extern "C" int delora_odometry_streams_push_pre(const delora_odometry_desc* d, const delora_odometry_residual_params* rp,
-                                                const float* points, const int32_t* n_points, const int32_t* active,
-                                                void* workspace, float* T, int32_t* valid, float* losses,
-                                                float* factor_out, void* stream) {
-    const char* who = "delora_odometry_streams_push_pre";
+// bookkeeping kernel (T, T12, factor, emptied sources, cache write), the ICP at B = S and the masked loss rows; with
+// info (delora_odometry_streams_push_pre_info) the ICP is the information operator and the masked rows follow.
+static int check_push_pre(const delora_odometry_desc* d, const delora_odometry_residual_params* rp, const float* points,
+                          const int32_t* n_points, void* workspace, float* T, int32_t* valid, float* losses,
+                          float* factor_out, const char* who) {
     if (check_pre_desc(d, who)) return 1;
     if (check_residual_params(rp, true, who)) return 1;
     if (check_tick(points, n_points, workspace, T, valid, losses, "losses", who)) return 1;
@@ -1259,9 +1270,14 @@ extern "C" int delora_odometry_streams_push_pre(const delora_odometry_desc* d, c
                      who);
     DELORA_CHECK_ARG(normalized || !factor_out, "%s: factor must be NULL without DELORA_TRAIN_NORMALIZATION_SCALING in "
                      "loss_flags", who);
-    cudaStream_t st = (cudaStream_t)stream;
+    return 0;
+}
+
+static int run_push_pre(const delora_odometry_desc* d, const delora_odometry_residual_params* rp, const float* points,
+                        const int32_t* n_points, const int32_t* active, void* workspace, float* T, int32_t* valid,
+                        float* losses, float* factor_out, float* info, cudaStream_t st) {
     InferPlan p;
-    make_streams_plan(d, Streams::pre, &p);
+    make_streams_plan(d, info ? Streams::pre_info : Streams::pre, &p);
     char* ws = (char*)workspace;
     const int S = d->max_batch, H = d->H, W = d->W, Wp = d->w_pre, HW = H * W, HWp = H * Wp;
     auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
@@ -1301,11 +1317,43 @@ extern "C" int delora_odometry_streams_push_pre(const delora_odometry_desc* d, c
         reinterpret_cast<const float4*>(pre_cur_nrm), reinterpret_cast<float4*>(pre_prev_pts),
         reinterpret_cast<float4*>(pre_prev_nrm));
     DELORA_CHECK_LAUNCH("odometry_streams_pre_kernel");
-    if ((rc = streams_icp(d, rp, p, ws, st))) return rc;
+    if ((rc = streams_icp(d, rp, p, ws, factor, st))) return rc;
     odometry_streams_losses_kernel<<<(S * DELORA_LOSS_ROW + 255) / 256, 256, 0, st>>>(valid, S, f(p.losses), losses);
     DELORA_CHECK_LAUNCH("odometry_streams_losses_kernel");
-    return 0;
+    return info ? streams_info_out(valid, S, f(p.info), info, st) : 0;
 }
+
+extern "C" int delora_odometry_streams_push_pre(const delora_odometry_desc* d, const delora_odometry_residual_params* rp,
+                                                const float* points, const int32_t* n_points, const int32_t* active,
+                                                void* workspace, float* T, int32_t* valid, float* losses,
+                                                float* factor_out, void* stream) {
+    const char* who = "delora_odometry_streams_push_pre";
+    if (check_push_pre(d, rp, points, n_points, workspace, T, valid, losses, factor_out, who)) return 1;
+    return run_push_pre(d, rp, points, n_points, active, workspace, T, valid, losses, factor_out, nullptr,
+                        (cudaStream_t)stream);
+}
+
+extern "C" int64_t delora_odometry_streams_pre_info_workspace_bytes(const delora_odometry_desc* d) {
+    return streams_workspace_bytes(d, Streams::pre_info, "delora_odometry_streams_pre_info_workspace_bytes");
+}
+
+extern "C" int delora_odometry_streams_pre_info_init(const delora_odometry_desc* d, void* workspace, void* stream) {
+    return streams_init(d, Streams::pre_info, workspace, (cudaStream_t)stream, "delora_odometry_streams_pre_info_init");
+}
+
+extern "C" int delora_odometry_streams_push_pre_info(const delora_odometry_desc* d,
+                                                     const delora_odometry_residual_params* rp, const float* points,
+                                                     const int32_t* n_points, const int32_t* active, void* workspace,
+                                                     float* T, int32_t* valid, float* losses, float* factor_out,
+                                                     float* info, void* stream) {
+    const char* who = "delora_odometry_streams_push_pre_info";
+    if (check_push_pre(d, rp, points, n_points, workspace, T, valid, losses, factor_out, who)) return 1;
+    DELORA_CHECK_ARG(info, "%s: null info", who);
+    return run_push_pre(d, rp, points, n_points, active, workspace, T, valid, losses, factor_out, info,
+                        (cudaStream_t)stream);
+}
+
+
 
 extern "C" int delora_odometry_streams_reset(const delora_odometry_desc* d, const int32_t* mask, void* workspace,
                                              void* stream) {
@@ -1961,6 +2009,8 @@ struct AdaptTick {
     float* cache_image;                // [S, 4, H, W] w_pre = 0 only: each stream's previous image
     delora_f4* cache_pts;              // [S, H, W] (w_pre = 0) or [S, H, w_pre]: its previous stage-1 grids
     delora_f4* cache_nrm;
+    float* info;                       // [S, DELORA_INFO_ROW] or NULL (_push_adapt_info): the information rows
+    float* info_scratch;               // the information operator's info_scratch at B = S, with info
 };
 
 // Stages 1-3 of delora_odometry_train_step and all of delora_odometry_train_eval: the projection + normals of the 2B
@@ -1970,6 +2020,8 @@ struct AdaptTick {
 // inactive streams' counts masked to 0) and takes its first half, scan_1's, from the cache; the output kernel divides
 // each quaternion by its own row's norm, writes raw for the valid rows only, valid, has_prev and n_valid; then the
 // bookkeeping kernel writes at->T, T12, the masked cache write and empties the sources of the rows without a pair.
+// With at->info the ICP is the information operator (losses and dL/dT are the same bits), in metres for normalised
+// models: their grids were divided by the pair factors, kept in pre_image.
 static int train_forward_losses(const delora_odometry_desc* d, const delora_odometry_train_params* hp, const TrainPlan& tp,
                                 char* ws, const float* points, const int32_t* n_points, int B, bool dropout, float* T_out,
                                 cudaStream_t st, const char* who, const AdaptTick* at = nullptr) {
@@ -2065,11 +2117,24 @@ static int train_forward_losses(const delora_odometry_desc* d, const delora_odom
     const long long icp_n4 = (delora_icp_scratch_floats(B, HW) + 3) / 4;
     odometry_icp_rearm_kernel<<<2 * num_sms(), 256, 0, st>>>(reinterpret_cast<float4*>(ws + tp.icp), icp_n4, B, ctr);
     DELORA_CHECK_LAUNCH("odometry_icp_rearm_kernel");
-    if ((rc = delora_icp_dense_fwd_bwd(pts_grid + (size_t)B * HW, nrm_grid + (size_t)B * HW, f(tp.T12), pts_grid, nrm_grid,
-                                       B, H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, hp->lambda_po2pl,
-                                       hp->loss_flags & ~(DELORA_LOSS_IDENTITY_FIT | DELORA_TRAIN_NORMALIZATION_SCALING |
-                                                          DELORA_TRAIN_DROPOUT),
-                                       f(tp.losses), f(tp.grad_T), f(tp.icp), st))) return rc;
+    const uint32_t icp_flags =
+        hp->loss_flags & ~(DELORA_LOSS_IDENTITY_FIT | DELORA_TRAIN_NORMALIZATION_SCALING | DELORA_TRAIN_DROPOUT);
+    if (at && at->info && normalized) {
+        rc = delora_icp_dense_information_scaled(pts_grid + (size_t)B * HW, nrm_grid + (size_t)B * HW, f(tp.T12),
+                                                 pts_grid, nrm_grid, B, H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1,
+                                                 hp->lambda_po2pl, icp_flags, f(tp.losses), f(tp.grad_T), f(tp.icp),
+                                                 at->info, at->info_scratch, f(tp.pre_image), st);
+    } else if (at && at->info) {
+        rc = delora_icp_dense_information(pts_grid + (size_t)B * HW, nrm_grid + (size_t)B * HW, f(tp.T12), pts_grid,
+                                          nrm_grid, B, H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, hp->lambda_po2pl,
+                                          icp_flags, f(tp.losses), f(tp.grad_T), f(tp.icp), at->info,
+                                          at->info_scratch, st);
+    } else {
+        rc = delora_icp_dense_fwd_bwd(pts_grid + (size_t)B * HW, nrm_grid + (size_t)B * HW, f(tp.T12), pts_grid, nrm_grid,
+                                      B, H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, hp->lambda_po2pl, icp_flags,
+                                      f(tp.losses), f(tp.grad_T), f(tp.icp), st);
+    }
+    if (rc) return rc;
     if (normalized) {               // T in metres for the caller, the factor in losses[b][6]
         odometry_train_normalized_out_kernel<<<(B * 16 + 255) / 256, 256, 0, st>>>(f(tp.T16), f(tp.pre_image), B, T_out,
                                                                                       f(tp.losses));
@@ -2403,6 +2468,10 @@ struct AdaptPlan {
     // last such tick (int32) and the count exchange's slots (int32 [2][kArMaxWorld], see count_allreduce_kernel).
     size_t tick, n_fleet, slots;
     size_t group_total;
+    // The information section of delora_odometry_streams_push_adapt_info / _group_info, after the group section: the
+    // information rows of the S pairs and the operator's info_scratch at B = S
+    size_t info, info_scratch;
+    size_t info_total;
 };
 
 // geometry_at: see make_train_plan; the stream section follows the geometry section wherever that starts
@@ -2423,30 +2492,41 @@ static void make_adapt_plan(const delora_odometry_desc* d, TrainPlan* tp, AdaptP
     ap->n_fleet = base + 8;
     ap->slots = base + 16;
     ap->group_total = off;
+    ap->info = take(off, S * DELORA_INFO_ROW * 4);
+    ap->info_scratch = take(off, (size_t)delora_icp_information_scratch_floats(d->max_batch, d->H, d->W) * 4);
+    ap->info_total = off;
 }
 
-// The adapting-streams workspace's size and, with group, its group form's
-static int64_t adapt_workspace_bytes(const delora_odometry_desc* d, bool group, const char* who) {
+// The adapting-streams workspace forms: _adapt (total), _adapt_group (group_total), _adapt_info (info_total)
+enum class Adapt { plain, group, info };
+
+static size_t adapt_bytes(const AdaptPlan& ap, Adapt form) {
+    return form == Adapt::info ? ap.info_total : form == Adapt::group ? ap.group_total : ap.total;
+}
+
+// The adapting-streams workspace's size in one of its forms
+static int64_t adapt_workspace_bytes(const delora_odometry_desc* d, Adapt form, const char* who) {
     if (check_train_desc(d, who)) return -1;
     TrainPlan tp;
     AdaptPlan ap;
     make_adapt_plan(d, &tp, &ap);
-    return (int64_t)(group ? ap.group_total : ap.total);
+    return (int64_t)adapt_bytes(ap, form);
 }
 
-// _streams_adapt_init and, with group, _streams_adapt_group_init; the group section is zeroed too
-static int adapt_init(const delora_odometry_desc* d, bool group, const float* weights, void* workspace, cudaStream_t st,
+// _streams_adapt_init, _streams_adapt_group_init and _streams_adapt_info_init; the group and information sections are
+// zeroed too, and the forms with a group section preload the collective kernels
+static int adapt_init(const delora_odometry_desc* d, Adapt form, const float* weights, void* workspace, cudaStream_t st,
                       const char* who) {
     if (check_train_desc(d, who)) return 1;
     TrainPlan tp;
     AdaptPlan ap;
     make_adapt_plan(d, &tp, &ap);
     // _train_init over the whole workspace zeroes the stream section too; the cached grids then start empty
-    int rc = train_init(d, group ? ap.group_total : ap.total, weights, workspace, st, who);
+    int rc = train_init(d, adapt_bytes(ap, form), weights, workspace, st, who);
     if (rc) return rc;
     if ((rc = clear_grids((char*)workspace, ap.cache_pts, ap.cache_nrm, (size_t)d->max_batch * ap.cache_cells, st)))
         return rc;
-    return group ? collective_kernels_preload(who) : 0;
+    return form != Adapt::plain ? collective_kernels_preload(who) : 0;
 }
 
 // The hyperparameters and update value every adapting tick refuses alike
@@ -2473,11 +2553,12 @@ static int check_push_adapt(const delora_odometry_desc* d, const delora_odometry
 }
 
 // Stages 1-3 of one adapting tick of the S = d->max_batch streams of (tp, ap): T, valid, the loss rows and the cache
-// write; update = 0 then records the ICP scratch's batch marker
+// write, with info (an information workspace) the information rows at the served T; update = 0 then records the ICP
+// scratch's batch marker
 static int serve_adapt(const delora_odometry_desc* d, const delora_odometry_train_params* hp, const TrainPlan& tp,
                        const AdaptPlan& ap, int update, const float* points, const int32_t* n_points,
-                       const int32_t* active, char* ws, float* T, int32_t* valid, float* losses, cudaStream_t st,
-                       const char* who) {
+                       const int32_t* active, char* ws, float* T, int32_t* valid, float* losses, float* info,
+                       cudaStream_t st, const char* who) {
     const int S = d->max_batch;
     auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
     AdaptTick at;
@@ -2489,11 +2570,14 @@ static int serve_adapt(const delora_odometry_desc* d, const delora_odometry_trai
     at.cache_image = d->w_pre == 0 ? f(ap.cache_image) : nullptr;
     at.cache_pts = reinterpret_cast<delora_f4*>(ws + ap.cache_pts);
     at.cache_nrm = reinterpret_cast<delora_f4*>(ws + ap.cache_nrm);
+    at.info = info ? f(ap.info) : nullptr;
+    at.info_scratch = info ? f(ap.info_scratch) : nullptr;
     int rc;
     // 1-3 at B = S, the first frame of every pair from the cache; T, valid, the cache and the emptied sources
     if ((rc = train_forward_losses(d, hp, tp, ws, points, n_points, S, false, nullptr, st, who, &at))) return rc;
     odometry_streams_losses_kernel<<<(S * DELORA_LOSS_ROW + 255) / 256, 256, 0, st>>>(valid, S, f(tp.losses), losses);
     DELORA_CHECK_LAUNCH("odometry_streams_losses_kernel");
+    if (info && (rc = streams_info_out(valid, S, f(ap.info), info, st))) return rc;
     if (!update) {          // the ICP scratch now has the layout of S pairs, as after _train_eval
         odometry_icp_batch_kernel<<<1, 1, 0, st>>>(reinterpret_cast<long long*>(ws + tp.ctr), S);
         DELORA_CHECK_LAUNCH("odometry_icp_batch_kernel");
@@ -2506,10 +2590,11 @@ static int serve_adapt(const delora_odometry_desc* d, const delora_odometry_trai
 // are summed over the ranks on g->side_stream (collectives k = 1 .. kGroupBuckets); Adam runs where that count is > 0.
 // The group's sequence numbers come from its tick counter, seq = tick * (kGroupBuckets + 1) + k, which advances on
 // every group tick with update = 1, so a tick without a valid pair still takes new numbers.
+// info non-NULL: an information workspace (_push_adapt_info / _push_adapt_group_info).
 static int push_adapt(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
                       const delora_odometry_train_group* g, int update, const float* points, const int32_t* n_points,
-                      const int32_t* active, void* workspace, float* T, int32_t* valid, float* losses, void* stream,
-                      const char* who) {
+                      const int32_t* active, void* workspace, float* T, int32_t* valid, float* losses, float* info,
+                      void* stream, const char* who) {
     const int S = d->max_batch;
     TrainPlan tp;
     AdaptPlan ap;
@@ -2517,7 +2602,8 @@ static int push_adapt(const delora_odometry_desc* d, const delora_odometry_train
     cudaStream_t st = (cudaStream_t)stream;
     char* ws = (char*)workspace;
     int rc;
-    if ((rc = serve_adapt(d, hp, tp, ap, update, points, n_points, active, ws, T, valid, losses, st, who))) return rc;
+    if ((rc = serve_adapt(d, hp, tp, ap, update, points, n_points, active, ws, T, valid, losses, info, st, who)))
+        return rc;
     if (!update) return 0;
     const int32_t* n_valid = reinterpret_cast<const int32_t*>(ws + ap.n_valid);
     long long* tick = reinterpret_cast<long long*>(ws + ap.tick);
@@ -2541,12 +2627,12 @@ static int push_adapt(const delora_odometry_desc* d, const delora_odometry_train
 }  // namespace delora
 
 extern "C" int64_t delora_odometry_streams_adapt_workspace_bytes(const delora_odometry_desc* d) {
-    return adapt_workspace_bytes(d, false, "delora_odometry_streams_adapt_workspace_bytes");
+    return adapt_workspace_bytes(d, Adapt::plain, "delora_odometry_streams_adapt_workspace_bytes");
 }
 
 extern "C" int delora_odometry_streams_adapt_init(const delora_odometry_desc* d, const float* weights, void* workspace,
                                                   void* stream) {
-    return adapt_init(d, false, weights, workspace, (cudaStream_t)stream, "delora_odometry_streams_adapt_init");
+    return adapt_init(d, Adapt::plain, weights, workspace, (cudaStream_t)stream, "delora_odometry_streams_adapt_init");
 }
 
 extern "C" int delora_odometry_streams_push_adapt(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
@@ -2555,16 +2641,17 @@ extern "C" int delora_odometry_streams_push_adapt(const delora_odometry_desc* d,
                                                   float* losses, void* stream) {
     const char* who = "delora_odometry_streams_push_adapt";
     if (check_push_adapt(d, hp, update, points, n_points, workspace, T, valid, losses, who)) return 1;
-    return push_adapt(d, hp, nullptr, update, points, n_points, active, workspace, T, valid, losses, stream, who);
+    return push_adapt(d, hp, nullptr, update, points, n_points, active, workspace, T, valid, losses, nullptr, stream,
+                      who);
 }
 
 extern "C" int64_t delora_odometry_streams_adapt_group_workspace_bytes(const delora_odometry_desc* d) {
-    return adapt_workspace_bytes(d, true, "delora_odometry_streams_adapt_group_workspace_bytes");
+    return adapt_workspace_bytes(d, Adapt::group, "delora_odometry_streams_adapt_group_workspace_bytes");
 }
 
 extern "C" int delora_odometry_streams_adapt_group_init(const delora_odometry_desc* d, const float* weights,
                                                         void* workspace, void* stream) {
-    return adapt_init(d, true, weights, workspace, (cudaStream_t)stream, "delora_odometry_streams_adapt_group_init");
+    return adapt_init(d, Adapt::group, weights, workspace, (cudaStream_t)stream, "delora_odometry_streams_adapt_group_init");
 }
 
 extern "C" int delora_odometry_streams_push_adapt_group(const delora_odometry_desc* d,
@@ -2577,7 +2664,44 @@ extern "C" int delora_odometry_streams_push_adapt_group(const delora_odometry_de
     if (check_push_adapt(d, hp, update, points, n_points, workspace, T, valid, losses, who)) return 1;
     if (check_group(g, workspace, who)) return 1;
     return push_adapt(d, hp, g->world > 1 && update ? g : nullptr, update, points, n_points, active, workspace, T,
-                      valid, losses, stream, who);
+                      valid, losses, nullptr, stream, who);
+}
+
+extern "C" int64_t delora_odometry_streams_adapt_info_workspace_bytes(const delora_odometry_desc* d) {
+    return adapt_workspace_bytes(d, Adapt::info, "delora_odometry_streams_adapt_info_workspace_bytes");
+}
+
+extern "C" int delora_odometry_streams_adapt_info_init(const delora_odometry_desc* d, const float* weights,
+                                                       void* workspace, void* stream) {
+    return adapt_init(d, Adapt::info, weights, workspace, (cudaStream_t)stream,
+                      "delora_odometry_streams_adapt_info_init");
+}
+
+extern "C" int delora_odometry_streams_push_adapt_info(const delora_odometry_desc* d,
+                                                       const delora_odometry_train_params* hp, int update,
+                                                       const float* points, const int32_t* n_points,
+                                                       const int32_t* active, void* workspace, float* T,
+                                                       int32_t* valid, float* losses, float* info, void* stream) {
+    const char* who = "delora_odometry_streams_push_adapt_info";
+    if (check_push_adapt(d, hp, update, points, n_points, workspace, T, valid, losses, who)) return 1;
+    DELORA_CHECK_ARG(info, "%s: null info", who);
+    return push_adapt(d, hp, nullptr, update, points, n_points, active, workspace, T, valid, losses, info, stream,
+                      who);
+}
+
+extern "C" int delora_odometry_streams_push_adapt_group_info(const delora_odometry_desc* d,
+                                                             const delora_odometry_train_params* hp,
+                                                             const delora_odometry_train_group* g, int update,
+                                                             const float* points, const int32_t* n_points,
+                                                             const int32_t* active, void* workspace, float* T,
+                                                             int32_t* valid, float* losses, float* info,
+                                                             void* stream) {
+    const char* who = "delora_odometry_streams_push_adapt_group_info";
+    if (check_push_adapt(d, hp, update, points, n_points, workspace, T, valid, losses, who)) return 1;
+    DELORA_CHECK_ARG(info, "%s: null info", who);
+    if (check_group(g, workspace, who)) return 1;
+    return push_adapt(d, hp, g->world > 1 && update ? g : nullptr, update, points, n_points, active, workspace, T,
+                      valid, losses, info, stream, who);
 }
 
 extern "C" int delora_odometry_streams_adapt_reset(const delora_odometry_desc* d, const int32_t* mask, void* workspace,
@@ -2660,7 +2784,8 @@ static int push_adapt_geometries(const delora_odometry_desc* d, int n, const del
     for (int g = 0; g < n; ++g) {
         const int r = p->row[g];
         if ((rc = serve_adapt(&d[g], hp, p->tp[g], p->ap[g], update, points[g], n_points[g], active ? active + r : nullptr,
-                              ws, T + (size_t)r * 16, valid + r, losses + (size_t)r * DELORA_LOSS_ROW, st, who)))
+                              ws, T + (size_t)r * 16, valid + r, losses + (size_t)r * DELORA_LOSS_ROW, nullptr, st,
+                              who)))
             return rc;
     }
     if (!update) return 0;

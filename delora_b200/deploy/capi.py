@@ -204,6 +204,21 @@ class PreStreamsWorkspace(StreamsWorkspace):
                    self.workspace.data_ptr(), T.data_ptr(), valid.data_ptr(), losses.data_ptr(), _ptr(factor))
 
 
+class PreInformationStreamsWorkspace(PreStreamsWorkspace):
+    """delora_odometry_streams_pre_info_* on the recipe layout with the information section appended: `push` also writes
+    each stream's information row at T, in the metres and radians of T for normalised models too.  load_weights / reset
+    are the streams calls."""
+    SIZE_QUERY = "delora_odometry_streams_pre_info_workspace_bytes"
+    INIT = "delora_odometry_streams_pre_info_init"
+
+    def push(self, points, counts, active, T, valid, losses, info, factor=None):
+        """PreStreamsWorkspace.push plus info [S, INFO_ROW] out: the information row of every valid stream, zeros
+        elsewhere."""
+        self._call("delora_odometry_streams_push_pre_info", self._params, points.data_ptr(), counts.data_ptr(),
+                   _ptr(active), self.workspace.data_ptr(), T.data_ptr(), valid.data_ptr(), losses.data_ptr(),
+                   _ptr(factor), info.data_ptr())
+
+
 class TrainingWorkspace(_Workspace):
     """delora_odometry_train_*: fp32 master weights, Adam's state and the step's buffers; `params` from train_params."""
     SIZE_QUERY = "delora_odometry_train_workspace_bytes"
@@ -463,15 +478,39 @@ class AdaptiveStreamsGroupWorkspace(AdaptiveStreamsWorkspace):
 class AdaptingStreamsGroup(TrainingGroup):
     """TrainingGroup over N AdaptiveStreamsGroupWorkspaces (same descriptor and state, N devices with peer access or
     one device): one model adapted from the streams of every rank.  `push(r, ...)` runs rank r's tick on the current
-    stream of its device; every rank makes the same number of update = True calls."""
+    stream of its device; every rank makes the same number of update = True calls.  Over
+    AdaptiveInformationStreamsWorkspaces each tick also returns the information rows."""
 
     def push(self, rank, points, counts, active, update=True, out=None):
-        """points [S, 3, n_stride], counts [S], active [S] int32 or None -> (T [S, 16], valid [S], losses [S, LOSS_ROW]),
-        into `out` when given."""
+        """points [S, 3, n_stride], counts [S], active [S] int32 or None -> (T [S, 16], valid [S], losses [S, LOSS_ROW])
+        and, over information workspaces, info [S, INFO_ROW]; into `out` when given."""
         w = self.workspaces[rank]
         if out is None:
             S, dev = w.desc.max_batch, w.workspace.device
             out = (torch.empty((S, 16), dtype=torch.float32, device=dev), torch.empty((S,), dtype=torch.int32, device=dev),
                    torch.empty((S, ops.LOSS_ROW), dtype=torch.float32, device=dev))
+            if isinstance(w, AdaptiveInformationStreamsWorkspace):
+                out += (torch.empty((S, ops.INFO_ROW), dtype=torch.float32, device=dev),)
         w.push_group(self.groups[rank], points, counts, active, *out, update=update)
         return out
+
+
+class AdaptiveInformationStreamsWorkspace(AdaptiveStreamsGroupWorkspace):
+    """delora_odometry_streams_adapt_info_*: the group layout of the adapting streams with the information section
+    appended; every AdaptiveStreamsWorkspace call works on it.  `push` and `push_group` take info [S, INFO_ROW] out
+    after losses: the information row at the served T (before the tick's update) of every valid stream, in the metres
+    and radians of T for normalised models too; zeros elsewhere."""
+    SIZE_QUERY = "delora_odometry_streams_adapt_info_workspace_bytes"
+
+    def _init(self, weights):
+        self._call("delora_odometry_streams_adapt_info_init", weights.data_ptr(), self.workspace.data_ptr())
+
+    def push(self, points, counts, active, T, valid, losses, info, update=True):
+        self._call("delora_odometry_streams_push_adapt_info", self._params, 1 if update else 0, points.data_ptr(),
+                   counts.data_ptr(), _ptr(active), self.workspace.data_ptr(), T.data_ptr(), valid.data_ptr(),
+                   losses.data_ptr(), info.data_ptr())
+
+    def push_group(self, group, points, counts, active, T, valid, losses, info, update=True):
+        self._call("delora_odometry_streams_push_adapt_group_info", self._params, ctypes.byref(group),
+                   1 if update else 0, points.data_ptr(), counts.data_ptr(), _ptr(active), self.workspace.data_ptr(),
+                   T.data_ptr(), valid.data_ptr(), losses.data_ptr(), info.data_ptr())

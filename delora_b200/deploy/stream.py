@@ -288,7 +288,8 @@ class OdometryStreams(_Streams):
             self.blob = torch.from_numpy(export.pack_state_dict(model.state_dict(), config)).to(self.device)
             if pre:
                 flags = residual_flags | (ops.TRAIN_NORMALIZATION_SCALING if normalized else 0)
-                self.workspace = capi.PreStreamsWorkspace(self.desc, self.blob, capi.residual_params(config, flags))
+                kind = capi.PreInformationStreamsWorkspace if info else capi.PreStreamsWorkspace
+                self.workspace = kind(self.desc, self.blob, capi.residual_params(config, flags))
             elif info:
                 self.workspace = capi.InformationStreamsWorkspace(self.desc, self.blob,
                                                                   capi.residual_params(config, residual_flags))
@@ -307,8 +308,8 @@ class OdometryStreams(_Streams):
         # the push arguments of a tick, all in the device staging buffers
         self._dev_active = dev_in[2]
         self._tick = tuple(dev_in) + tuple(dev_out)
-        # what push returns beside T: the residual's losses and the recipe's factor (the normalised raw-scan streams
-        # return T alone)
+        # what push returns beside T: the residual's losses, the information rows and the recipe's factor (the
+        # normalised raw-scan streams return T alone)
         self._extras = (([self._out["losses"]] if self.residual else []) + ([self._out["info"]] if info else []) +
                         ([self._out["factor"]] if pre and normalized else []))
         self.relative = [[] for _ in range(S)]
@@ -384,15 +385,20 @@ class PreprocessedOdometryStreams(OdometryStreams):
     `--preprocessing-normals` saw in training and the reference's Tester feeds it.  Serves plain and
     normalization_scaling configs alike.  `push` returns, per stream with a transform, (T [1, 4, 4], losses [LOSS_ROW])
     -- the training step's ICP residual of the pair, in the model's units -- plus the pair's factor for a normalised
-    config: (T, losses, factor).  `residual_flags` selects the losses; `poses` and `reset` are OdometryStreams'."""
+    config: (T, losses, factor).  `residual_flags` selects the losses; `poses` and `reset` are OdometryStreams'.
+
+    information=True serves them from the recipe information workspace (`delora_odometry_streams_push_pre_info`):
+    each entry is then (T, losses, info [INFO_ROW][, factor]), info being the Gauss-Newton information of the residual's
+    objective at T (see InformationOdometryStreams), in the metres and radians of T for normalised configs too.  T,
+    losses and factor are the same bits either way."""
 
     def __init__(self, model, config, dataset, n_streams, n_max, use_cuda_graph=True,
-                 residual_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL):
+                 residual_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL, information=False):
         if "horizontal_cells_preprocessing" not in config[dataset]:
             raise ValueError(f"{dataset}: horizontal_cells_preprocessing is missing; PreprocessedOdometryStreams "
                              "serves the recipe's normals at that width (serve raw scans with OdometryStreams)")
         self._setup(model, config, dataset, n_streams, n_max, use_cuda_graph, True, residual_flags,
-                    bool(config.get("normalization_scaling", False)), pre=True)
+                    bool(config.get("normalization_scaling", False)), pre=True, info=bool(information))
 
 
 class AdaptiveOdometryStreams(_Streams):
@@ -402,10 +408,17 @@ class AdaptiveOdometryStreams(_Streams):
     on the mean objective of the pairs it served.  T is always that of the weights before the tick's update; the next
     tick serves the updated model.  Normals at the model's width, or with preprocessing_normals=True at
     `horizontal_cells_preprocessing` (the reference's recipe, which normalization_scaling needs).  `state_dict()` is the
-    adapted model.  Dropout configs are refused: the served T must be dropout-free."""
+    adapted model.  Dropout configs are refused: the served T must be dropout-free.
+
+    information=True serves them from the adapting information workspace (`delora_odometry_streams_push_adapt_info`):
+    each entry is then (T, losses, info [INFO_ROW]), info being the Gauss-Newton information of the tick's ICP objective
+    at the served T (see InformationOdometryStreams), in the metres and radians of T for normalised configs too.  T,
+    losses and the adapted model are the same bits either way."""
+
+    information = False
 
     def __init__(self, model, config, dataset, n_streams, n_max, lr, preprocessing_normals=False,
-                 loss_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL):
+                 loss_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL, information=False):
         from . import capi, export
         if config.get("use_dropout", False):
             raise ValueError("use_dropout: True is not supported by AdaptiveOdometryStreams: the served transforms "
@@ -420,10 +433,11 @@ class AdaptiveOdometryStreams(_Streams):
         self.n_streams, self.n_max = int(n_streams), int(n_max)
         self.desc = export.desc_from_config(config, dataset, self.n_max, self.n_streams,
                                             preprocessing_normals=preprocessing_normals)
+        self.information = bool(information)
         with torch.cuda.device(self.device):
             blob = torch.from_numpy(export.pack_state_dict(model.state_dict(), config)).to(self.device)
-            self.workspace = capi.AdaptiveStreamsWorkspace(self.desc, blob,
-                                                           capi.train_params(config, lr, loss_flags=loss_flags))
+            kind = capi.AdaptiveInformationStreamsWorkspace if self.information else capi.AdaptiveStreamsWorkspace
+            self.workspace = kind(self.desc, blob, capi.train_params(config, lr, loss_flags=loss_flags))
         self._buffers()
 
     def _buffers(self):
@@ -435,12 +449,14 @@ class AdaptiveOdometryStreams(_Streams):
             self.T = torch.zeros((S, 16), dtype=torch.float32, device=self.device)
             self.valid = torch.zeros((S,), dtype=torch.int32, device=self.device)
             self.losses = torch.zeros((S, ops.LOSS_ROW), dtype=torch.float32, device=self.device)
+            self.info = torch.zeros((S, ops.INFO_ROW), dtype=torch.float32, device=self.device)
             self._mask = torch.zeros((S,), dtype=torch.int32, device=self.device)
         self.relative = [[] for _ in range(S)]
 
     def push(self, scans, update=True):
         """scans: n_streams entries, each a [3, N] (or [1, 3, N]) float32 host tensor with N <= n_max, or None.  Returns
-        n_streams entries: (T [1, 4, 4], losses [LOSS_ROW]) numpy arrays for a stream with a pair this tick, else None."""
+        n_streams entries: (T [1, 4, 4], losses [LOSS_ROW]) numpy arrays for a stream with a pair this tick, else None;
+        with information=True, (T, losses, info [INFO_ROW])."""
         pts = torch.zeros((self.n_streams, 3, self.n_max), dtype=torch.float32)
         counts = torch.zeros((self.n_streams,), dtype=torch.int32)
         active = torch.zeros((self.n_streams,), dtype=torch.int32)
@@ -451,10 +467,14 @@ class AdaptiveOdometryStreams(_Streams):
             self.active.copy_(active)
             self._push_device(update)
             T, valid, losses = self.T.cpu().numpy(), self.valid.cpu().numpy(), self.losses.cpu().numpy()
-        return self._results(T, valid, [losses])
+            extras = [losses, self.info.cpu().numpy()] if self.information else [losses]
+        return self._results(T, valid, extras)
 
     def _push_device(self, update):
-        self.workspace.push(self.points, self.counts, self.active, self.T, self.valid, self.losses, update)
+        if self.information:
+            self.workspace.push(self.points, self.counts, self.active, self.T, self.valid, self.losses, self.info, update)
+        else:
+            self.workspace.push(self.points, self.counts, self.active, self.T, self.valid, self.losses, update)
 
     def state_dict(self):
         """The adapted weights as an OdometryModel state dict (fp32 CPU tensors)."""

@@ -353,6 +353,33 @@ def icp_dense_information(src_grid, src_ngrid, transform, tgt_grid, tgt_ngrid, h
     return losses, grad_t, info, nn
 
 
+def icp_dense_information_scaled(src_grid, src_ngrid, transform, tgt_grid, tgt_ngrid, h, w, hfov, vfov, factor,
+                                 lambda_po2pl=1.0, flags=LOSS_PO2PL | LOSS_PL2PL, scratch=None, info_scratch=None):
+    """icp_dense_information for grids divided by each pair's factor [B] (device fp32, > 0)
+    (delora_icp_dense_information_scaled): info's H, eigenvalues and eigenvectors are in metres and radians,
+    H_m = D H D with D = diag(1/f, 1/f, 1/f, 1, 1, 1); losses, grad_T and nn are icp_dense_information's bits."""
+    b = src_grid.shape[0]
+    dev = src_grid.device
+    losses = torch.empty((b, LOSS_ROW), dtype=torch.float32, device=dev)
+    grad_t = torch.empty((b, 12), dtype=torch.float32, device=dev)
+    info = torch.empty((b, INFO_ROW), dtype=torch.float32, device=dev)
+    if scratch is None:
+        scratch = icp_scratch(b, h * w, dev)
+    L = _lib.lib()
+    if info_scratch is None:
+        info_scratch = torch.empty((int(L.delora_icp_information_scratch_floats(b, h, w)),), dtype=torch.float32,
+                                   device=dev)
+    _lib.check(L.delora_icp_dense_information_scaled(
+        _req(src_grid, torch.float32, "src_grid"), _req(src_ngrid, torch.float32, "src_ngrid"),
+        _req(transform, torch.float32, "transform"), _req(tgt_grid, torch.float32, "tgt_grid"),
+        _req(tgt_ngrid, torch.float32, "tgt_ngrid"), b, h, w, float(hfov[0]), float(hfov[1]), float(vfov[0]),
+        float(vfov[1]), float(lambda_po2pl), int(flags), losses.data_ptr(), grad_t.data_ptr(),
+        scratch.data_ptr(), info.data_ptr(), info_scratch.data_ptr(), _req(factor, torch.float32, "factor"),
+        _stream()), "delora_icp_dense_information_scaled")
+    nn = info_scratch[:b * h * w].view(torch.int32).view(b, h * w)
+    return losses, grad_t, info, nn
+
+
 def icp_stats(reset=True):
     """Search statistics of dense ICP calls made with `flags | ICP_STATS` (include/delora_b200.h)."""
     import ctypes

@@ -2,8 +2,8 @@
  * Several LiDAR streams from a C host, batched in one workspace: no Python, no torch.  Links libdelora_b200.so and
  * cudart only.
  *
- *   odometry_streams [--residual | --information | --preprocessing] model.dlw stream0_dir stream1_dir ...
- *   odometry_streams --adapt LR --adapt-out adapted.dlw [--gpus N] model.dlw stream0_dir stream1_dir ...
+ *   odometry_streams [--residual | --information | --preprocessing [--information]] model.dlw stream0_dir ...
+ *   odometry_streams --adapt LR --adapt-out adapted.dlw [--gpus N] [--information] model.dlw stream0_dir ...
  *   odometry_streams --adapt LR --adapt-out adapted.dlw [--geometry DIR,H,W,VFOV0,VFOV1[,W_PRE]]... model.dlw
  *                    stream0_dir ...
  *
@@ -19,6 +19,11 @@
  * frame determines its transform (the Gauss-Newton information H of the residual's objective at T): H's smallest
  * eigenvalue, its unit eigenvector (x, y, z, rot x, rot y, rot z: the direction the frame constrains least) and the
  * ratio of the largest eigenvalue to the smallest (large in a corridor, an open field or at a flat wall).
+ * --information with --preprocessing (delora_odometry_streams_push_pre_info) or with --adapt, --gpus included
+ * (delora_odometry_streams_push_adapt_info / _push_adapt_group_info) appends the same three columns to those modes'
+ * lines, for plain and normalization_scaling files alike: the information is always in the metres and radians of the
+ * printed T.  The transforms, residual columns and adapted weights are the same bits as without it.  Options may come
+ * in any order before model.dlw; --information does not combine with --geometry.
  * A model trained with normalization_scaling (model_flags has DELORA_MODEL_NORMALIZATION_SCALING) is served through
  * delora_odometry_streams_push_normalized, with the same output; --residual is refused for such a model.
  * --preprocessing serves the streams on the reference's two-resolution recipe through delora_odometry_streams_push_pre:
@@ -203,8 +208,16 @@ typedef struct {
     int32_t *count, *active, *valid;
     float *h_points, *h_T, *h_losses;
     int32_t *h_count, *h_active, *h_valid, h_status;
+    float *info, *h_info;                     /* --information: the information rows, else NULL */
     int rc;
 } rank_state;
+
+/* --information's columns: the smallest eigenvalue of H, its unit eigenvector and the ratio of the largest to it */
+static void print_info(const float* r) {    /* [36, 42): eigenvalues ascending; [42, 48): the smallest one's eigenvector */
+    printf(" %.9g", r[36]);
+    for (int i = 0; i < 6; ++i) printf(" %.6f", r[42 + i]);
+    printf(" %.9g", r[36] > 0.0f ? r[41] / r[36] : INFINITY);
+}
 
 /* tick k of one rank: its scans up, one group tick with update = 1, T / valid / losses down */
 static int rank_tick(rank_state* r) {
@@ -223,8 +236,16 @@ static int rank_tick(rank_state* r) {
     CUDA_OK(cudaMemcpyAsync(r->points, r->h_points, pts_floats * sizeof(float), cudaMemcpyHostToDevice, r->stream));
     CUDA_OK(cudaMemcpyAsync(r->count, r->h_count, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, r->stream));
     CUDA_OK(cudaMemcpyAsync(r->active, r->h_active, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, r->stream));
-    DELORA_OK(delora_odometry_streams_push_adapt_group(d, r->hp, &r->g, 1, r->points, r->count, r->active, r->workspace,
-                                                       r->T, r->valid, r->losses, r->stream));
+    if (r->info) {
+        DELORA_OK(delora_odometry_streams_push_adapt_group_info(d, r->hp, &r->g, 1, r->points, r->count, r->active,
+                                                                r->workspace, r->T, r->valid, r->losses, r->info,
+                                                                r->stream));
+        CUDA_OK(cudaMemcpyAsync(r->h_info, r->info, (size_t)S * DELORA_INFO_ROW * sizeof(float), cudaMemcpyDeviceToHost,
+                                r->stream));
+    } else {
+        DELORA_OK(delora_odometry_streams_push_adapt_group(d, r->hp, &r->g, 1, r->points, r->count, r->active,
+                                                           r->workspace, r->T, r->valid, r->losses, r->stream));
+    }
     CUDA_OK(cudaMemcpyAsync(r->h_losses, r->losses, (size_t)S * DELORA_LOSS_ROW * sizeof(float), cudaMemcpyDeviceToHost,
                             r->stream));
     CUDA_OK(cudaMemcpyAsync(r->h_T, r->T, (size_t)S * 16 * sizeof(float), cudaMemcpyDeviceToHost, r->stream));
@@ -242,7 +263,7 @@ static void* rank_thread(void* arg) {
 }
 
 /* one GPU's workspace (initialised from the host blob), buffers, streams, events and zeroed flag words */
-static int rank_setup(rank_state* r, int world, const float* h_blob, int64_t n_weights) {
+static int rank_setup(rank_state* r, int world, const float* h_blob, int64_t n_weights, int information) {
     const delora_odometry_desc* d = r->d;
     const int S = r->S;
     CUDA_OK(cudaSetDevice(r->rank));
@@ -255,7 +276,8 @@ static int rank_setup(rank_state* r, int world, const float* h_blob, int64_t n_w
         if (e == cudaErrorPeerAccessAlreadyEnabled) cudaGetLastError();
         else CUDA_OK(e);
     }
-    const int64_t ws_bytes = delora_odometry_streams_adapt_group_workspace_bytes(d);
+    const int64_t ws_bytes = information ? delora_odometry_streams_adapt_info_workspace_bytes(d)
+                                         : delora_odometry_streams_adapt_group_workspace_bytes(d);
     if (ws_bytes < 0) return fail(delora_last_error());
     const size_t pts_floats = (size_t)S * 3 * d->n_stride;
     CUDA_OK(cudaStreamCreate(&r->stream));
@@ -272,10 +294,12 @@ static int rank_setup(rank_state* r, int world, const float* h_blob, int64_t n_w
     CUDA_OK(cudaMalloc((void**)&r->valid, (size_t)S * sizeof(int32_t)));
     CUDA_OK(cudaMalloc((void**)&r->T, (size_t)S * 16 * sizeof(float)));
     CUDA_OK(cudaMalloc((void**)&r->losses, (size_t)S * DELORA_LOSS_ROW * sizeof(float)));
+    if (information) CUDA_OK(cudaMalloc((void**)&r->info, (size_t)S * DELORA_INFO_ROW * sizeof(float)));
     CUDA_OK(cudaMemset(r->flags, 0, (size_t)delora_grad_allreduce_flag_words() * sizeof(uint32_t)));
     CUDA_OK(cudaMemset(r->status, 0, sizeof(int32_t)));
     CUDA_OK(cudaMemcpy(r->weights, h_blob, (size_t)n_weights * sizeof(float), cudaMemcpyHostToDevice));
-    DELORA_OK(delora_odometry_streams_adapt_group_init(d, r->weights, r->workspace, r->stream));
+    if (information) DELORA_OK(delora_odometry_streams_adapt_info_init(d, r->weights, r->workspace, r->stream));
+    else DELORA_OK(delora_odometry_streams_adapt_group_init(d, r->weights, r->workspace, r->stream));
     CUDA_OK(cudaStreamSynchronize(r->stream));
     r->h_points = (float*)malloc(pts_floats * sizeof(float));
     r->h_count = (int32_t*)malloc((size_t)S * sizeof(int32_t));
@@ -283,15 +307,16 @@ static int rank_setup(rank_state* r, int world, const float* h_blob, int64_t n_w
     r->h_valid = (int32_t*)malloc((size_t)S * sizeof(int32_t));
     r->h_T = (float*)malloc((size_t)S * 16 * sizeof(float));
     r->h_losses = (float*)calloc((size_t)S * DELORA_LOSS_ROW, sizeof(float));
-    if (!r->h_points || !r->h_count || !r->h_active || !r->h_valid || !r->h_T || !r->h_losses)
+    r->h_info = (float*)calloc((size_t)S * DELORA_INFO_ROW, sizeof(float));
+    if (!r->h_points || !r->h_count || !r->h_active || !r->h_valid || !r->h_T || !r->h_losses || !r->h_info)
         return fail("out of host memory");
     return 0;
 }
 
 static void rank_release(rank_state* r) {
     cudaSetDevice(r->rank);
-    free(r->h_losses); free(r->h_T); free(r->h_valid); free(r->h_active); free(r->h_count); free(r->h_points);
-    cudaFree(r->losses); cudaFree(r->T); cudaFree(r->valid); cudaFree(r->active); cudaFree(r->count);
+    free(r->h_info); free(r->h_losses); free(r->h_T); free(r->h_valid); free(r->h_active); free(r->h_count); free(r->h_points);
+    cudaFree(r->info); cudaFree(r->losses); cudaFree(r->T); cudaFree(r->valid); cudaFree(r->active); cudaFree(r->count);
     cudaFree(r->points); cudaFree(r->weights); cudaFree(r->status); cudaFree(r->flags); cudaFree(r->workspace);
     for (int k = 0; k <= DELORA_TRAIN_GROUP_BUCKETS; ++k) cudaEventDestroy(r->events[k]);
     cudaStreamDestroy(r->side);
@@ -301,7 +326,7 @@ static void rank_release(rank_state* r) {
 /* --adapt --gpus N: n_streams streams over GPUs 0 .. N-1, one model adapted from all of them; GPU 0 writes `out` */
 static int adapt_group(int gpus, delora_odometry_desc desc, const delora_odometry_file_header* hdr, float* h_blob,
                        int64_t n_weights, const scan_list* lists, int n_streams, int ticks,
-                       const delora_odometry_train_params* hp, const char* out) {
+                       const delora_odometry_train_params* hp, const char* out, int information) {
     int n_dev = 0;
     CUDA_OK(cudaGetDeviceCount(&n_dev));
     if (gpus > n_dev) return fail("--gpus: more GPUs than the machine has");
@@ -313,7 +338,7 @@ static int adapt_group(int gpus, delora_odometry_desc desc, const delora_odometr
     for (int r = 0; r < gpus; ++r) {
         rank_state* R = &ranks[r];
         R->rank = r; R->S = S; R->d = &desc; R->hp = hp; R->lists = lists; R->n_lists = n_streams;
-        if (rank_setup(R, gpus, h_blob, n_weights)) return 1;
+        if (rank_setup(R, gpus, h_blob, n_weights, information)) return 1;
     }
     for (int r = 0; r < gpus; ++r) {
         delora_odometry_train_group* g = &ranks[r].g;
@@ -348,7 +373,9 @@ static int adapt_group(int gpus, delora_odometry_desc desc, const delora_odometr
             printf("%d %d", gs, k);
             for (int i = 0; i < 12; ++i) printf(" %.9g", R->h_T[(size_t)s * 16 + i]);
             const float* l = R->h_losses + (size_t)s * DELORA_LOSS_ROW;
-            printf(" %.9g %.9g %.0f\n", l[1], l[2], l[3]);
+            printf(" %.9g %.9g %.0f", l[1], l[2], l[3]);
+            if (information) print_info(R->h_info + (size_t)s * DELORA_INFO_ROW);
+            printf("\n");
         }
     }
     rank_state* R0 = &ranks[0];             /* every rank holds the same weights: GPU 0 writes them */
@@ -382,8 +409,20 @@ int main(int argc, char** argv) {
     const char* gpus_arg = NULL;
     int n_geom = 0;                           /* --geometry streams, after the directories of the header's geometry */
     const char* geom_args[MAX_GEOMETRIES];
-    while (argc > 2 && (strcmp(argv[1], "--adapt") == 0 || strcmp(argv[1], "--adapt-out") == 0 ||
-                        strcmp(argv[1], "--gpus") == 0 || strcmp(argv[1], "--geometry") == 0)) {
+    int information = 0, residual_opt = 0, pre = 0;
+    for (;;) {
+        if (argc > 1 && (strcmp(argv[1], "--information") == 0 || strcmp(argv[1], "--residual") == 0 ||
+                         strcmp(argv[1], "--preprocessing") == 0)) {
+            if (strcmp(argv[1], "--information") == 0) information = 1;
+            else if (strcmp(argv[1], "--residual") == 0) residual_opt = 1;
+            else pre = 1;
+            --argc;
+            ++argv;
+            continue;
+        }
+        if (!(argc > 2 && (strcmp(argv[1], "--adapt") == 0 || strcmp(argv[1], "--adapt-out") == 0 ||
+                           strcmp(argv[1], "--gpus") == 0 || strcmp(argv[1], "--geometry") == 0)))
+            break;
         if (strcmp(argv[1], "--adapt") == 0) adapt_lr = argv[2];
         else if (strcmp(argv[1], "--adapt-out") == 0) adapt_out = argv[2];
         else if (strcmp(argv[1], "--gpus") == 0) gpus_arg = argv[2];
@@ -427,14 +466,14 @@ int main(int argc, char** argv) {
             free(dir);
         }
     }
-    const int information = argc > 1 && strcmp(argv[1], "--information") == 0;
-    const int residual = information || (argc > 1 && strcmp(argv[1], "--residual") == 0);
-    const int pre = argc > 1 && strcmp(argv[1], "--preprocessing") == 0;
-    if (residual || pre) { --argc; ++argv; }
-    if (adapt && (residual || pre)) return fail("--adapt serves its own residual: drop --residual / --information / --preprocessing");
+    if (adapt && (residual_opt || pre)) return fail("--adapt serves its own residual: drop --residual / --preprocessing");
+    if (residual_opt && pre) return fail("--preprocessing serves its own residual: drop --residual");
+    if (information && n_geom) return fail("--information does not combine with --geometry");
+    /* the raw-scan residual streams: --residual, or --information on its own */
+    const int residual = residual_opt || (information && !pre && !adapt);
     if (argc < 3)
-        return fail("usage: odometry_streams [--residual | --information | --preprocessing] model.dlw stream_dir "
-                    "[stream_dir ...]");
+        return fail("usage: odometry_streams [--residual | --information | --preprocessing [--information]] model.dlw "
+                    "stream_dir [stream_dir ...]");
     const int S_dirs = argc - 2;              /* the streams of the header's geometry */
     const int S = S_dirs + n_geom;            /* every stream, the --geometry ones last */
 
@@ -490,7 +529,7 @@ int main(int argc, char** argv) {
     hp.epsilon_range = 0.5f;
     hp.min_neighbors = 10;
     if (gpus) {
-        const int rc = adapt_group(gpus, desc, &hdr, h_blob, n_weights, lists, S, ticks, &hp, adapt_out);
+        const int rc = adapt_group(gpus, desc, &hdr, h_blob, n_weights, lists, S, ticks, &hp, adapt_out, information);
         for (int s = 0; s < S; ++s) {
             for (int i = 0; i < lists[s].n; ++i) free(lists[s].paths[i]);
             free(lists[s].paths);
@@ -514,7 +553,9 @@ int main(int argc, char** argv) {
     int32_t *count, *active, *valid;
     void* workspace;
     const int64_t ws_bytes = n_geom       ? delora_odometry_streams_adapt_geometries_workspace_bytes(descs, n_sets)
+                             : adapt && information ? delora_odometry_streams_adapt_info_workspace_bytes(d)
                              : adapt      ? delora_odometry_streams_adapt_workspace_bytes(d)
+                             : pre && information ? delora_odometry_streams_pre_info_workspace_bytes(d)
                              : pre        ? delora_odometry_streams_pre_workspace_bytes(d)
                              : information ? delora_odometry_streams_info_workspace_bytes(d)
                              : residual   ? delora_odometry_streams_residual_workspace_bytes(d)
@@ -542,10 +583,13 @@ int main(int argc, char** argv) {
     }
     if (n_geom) {
         DELORA_OK(delora_odometry_streams_adapt_geometries_init(descs, n_sets, weights, workspace, stream));
+    } else if (adapt && information) {
+        DELORA_OK(delora_odometry_streams_adapt_info_init(d, weights, workspace, stream));
     } else if (adapt) {
         DELORA_OK(delora_odometry_streams_adapt_init(d, weights, workspace, stream));
     } else {
-        if (pre) DELORA_OK(delora_odometry_streams_pre_init(d, workspace, stream));
+        if (pre && information) DELORA_OK(delora_odometry_streams_pre_info_init(d, workspace, stream));
+        else if (pre) DELORA_OK(delora_odometry_streams_pre_init(d, workspace, stream));
         else if (information) DELORA_OK(delora_odometry_streams_info_init(d, workspace, stream));
         else if (residual) DELORA_OK(delora_odometry_streams_residual_init(d, workspace, stream));
         else if (normalized) DELORA_OK(delora_odometry_streams_normalized_init(d, workspace, stream));
@@ -577,9 +621,15 @@ int main(int argc, char** argv) {
             if (n_geom)
                 DELORA_OK(delora_odometry_streams_push_adapt_geometries(descs, n_sets, &hp, 1, g_points, g_count, active,
                                                                         workspace, T, valid, losses, stream));
+            else if (adapt && information)
+                DELORA_OK(delora_odometry_streams_push_adapt_info(d, &hp, 1, points, count, active, workspace, T, valid,
+                                                                  losses, info, stream));
             else if (adapt)
                 DELORA_OK(delora_odometry_streams_push_adapt(d, &hp, 1, points, count, active, workspace, T, valid,
                                                              losses, stream));
+            else if (pre && information)
+                DELORA_OK(delora_odometry_streams_push_pre_info(d, &rp, points, count, active, workspace, T, valid,
+                                                                losses, normalized ? factor : NULL, info, stream));
             else if (pre)
                 DELORA_OK(delora_odometry_streams_push_pre(d, &rp, points, count, active, workspace, T, valid, losses,
                                                            normalized ? factor : NULL, stream));
@@ -611,12 +661,7 @@ int main(int argc, char** argv) {
                 const float* l = h_losses + (size_t)s * DELORA_LOSS_ROW;
                 printf(" %.9g %.9g %.0f", l[1], l[2], l[3]);
             }
-            if (information) {      /* [36, 42): eigenvalues ascending; [42, 48): the smallest one's eigenvector */
-                const float* r = h_info + (size_t)s * DELORA_INFO_ROW;
-                printf(" %.9g", r[36]);
-                for (int i = 0; i < 6; ++i) printf(" %.6f", r[42 + i]);
-                printf(" %.9g", r[36] > 0.0f ? r[41] / r[36] : INFINITY);
-            }
+            if (information) print_info(h_info + (size_t)s * DELORA_INFO_ROW);
             printf("\n");
         }
     }

@@ -301,6 +301,22 @@ int delora_icp_dense_information(const delora_f4* src_grid, const delora_f4* src
                                  double hfov0, double hfov1, double vfov0, double vfov1,
                                  float lambda_po2pl, uint32_t flags, float* losses, float* grad_T,
                                  float* scratch, float* info, float* info_scratch, void* stream);
+/* The information in metres for pairs whose clouds were divided by a factor (a model trained with
+ * normalization_scaling runs its ICP on the pair divided by the pair's factor f).  The arguments of
+ * delora_icp_dense_information plus factor [B] fp32 (device, every factor > 0; not checked on the host), the factor
+ * each pair's grids were divided by.  The operator's H is then taken in xi = (rho / f, phi) with rho in metres; since
+ * T(xi) = T Exp(xi) and a normalised translation of rho / f is rho metres, the information in the metres and radians
+ * of the T the model serves is H_m = D H D, D = diag(1/f, 1/f, 1/f, 1, 1, 1).  D is applied in float64 to the float64
+ * H before it is stored and solved, so the eigenvalues and eigenvectors are those of H_m.  The losses row stays in the
+ * model's units (the objective has no single rescale: pl2pl is unit-free), and losses, grad_T and the NN ids are
+ * delora_icp_dense_information's bits.  With every factor = 1 the output is delora_icp_dense_information's, bit for bit
+ * (each float64 product is by 1.0).  Refused: what delora_icp_dense_information refuses, a null factor. */
+int delora_icp_dense_information_scaled(const delora_f4* src_grid, const delora_f4* src_ngrid, const float* T,
+                                        const delora_f4* tgt_grid, const delora_f4* tgt_ngrid, int B, int H, int W,
+                                        double hfov0, double hfov1, double vfov0, double vfov1,
+                                        float lambda_po2pl, uint32_t flags, float* losses, float* grad_T,
+                                        float* scratch, float* info, float* info_scratch, const float* factor,
+                                        void* stream);
 
 /* Diagnostic for delora_icp_dense_fwd_bwd calls made with DELORA_ICP_STATS in `flags`: copies the 32 device
  * counters to the HOST array out32 (may be NULL) and optionally zeroes them.  [0] warps, [1] window-growing steps,
@@ -816,6 +832,34 @@ int delora_odometry_streams_push_pre(const delora_odometry_desc* d, const delora
                                      void* workspace, float* T, int32_t* valid, float* losses, float* factor,
                                      void* stream);
 
+/* The recipe streams with the information of each frame's residual beside it (see delora_icp_dense_information and
+ * _streams_push_info): the Gauss-Newton information of the recipe's ICP objective at the served T, so that a host
+ * serving a model on the images it trained on, plain or normalization_scaling, can tell a frame of a degenerate scene
+ * from a good one.  The recipe streams workspace with the information section of _streams_info appended (the rows of
+ * the S pairs and delora_icp_information_scratch_floats(S, H, W) floats, each 256-byte aligned): no offset of the
+ * recipe layout moves, so delora_odometry_streams_load_weights and delora_odometry_streams_reset work on it unchanged
+ * (_pre_info_init replaces _pre_init).
+ * delora_odometry_streams_push_pre_info: the arguments of delora_odometry_streams_push_pre plus info
+ * [S, DELORA_INFO_ROW] (device, required).  T, valid, losses and factor are what _streams_push_pre writes for the same
+ * history, byte for byte.  Where valid[s] = 1, info[s] is, bit for bit, the row of the operator run alone at B = 1 on
+ * the pair's H x W grids and T's 3x4 in the model's units: delora_icp_dense_information for a plain model;
+ * delora_icp_dense_information_scaled with the pair's factor for a flagged one, whose grids are divided by that
+ * factor.  So H, its eigenvalues and eigenvectors are always in the metres and radians of the served T, xi = (x, y, z,
+ * rot x, rot y, rot z) perturbing T on the right; the losses row and M, M' stay the model's.  Rows with valid[s] = 0
+ * are zeros.  Graph-capturable like _streams_push_pre.  Refused before any launch: everything _streams_push_pre
+ * refuses, and a null info.
+ * Measured on one H100 80GB HBM3 at a 700 W power limit (max SM clock 1980 MHz), graph-replayed ticks, all streams
+ * active, near-identity heads on consecutive synthetic frames, w_pre 2250, medians of alternating samples,
+ * _streams_push_pre -> _streams_push_pre_info per tick: 64 x 2048: S = 1 1.30 -> 1.36 ms, S = 4 2.34 -> 2.46 ms,
+ * S = 16 8.98 -> 9.21 ms; 64 x 720: S = 1 1.20 -> 1.23 ms, S = 4 1.46 -> 1.50 ms, S = 16 5.41 -> 5.52 ms
+ * (scripts/gpu_odometry_streams_pre_adapt_info.py, profiles/odometry_streams_pre_adapt_info_h100_700w.json). */
+int64_t delora_odometry_streams_pre_info_workspace_bytes(const delora_odometry_desc* d);   /* host only, -1 if invalid */
+int delora_odometry_streams_pre_info_init(const delora_odometry_desc* d, void* workspace, void* stream);
+int delora_odometry_streams_push_pre_info(const delora_odometry_desc* d, const delora_odometry_residual_params* rp,
+                                          const float* points, const int32_t* n_points, const int32_t* active,
+                                          void* workspace, float* T, int32_t* valid, float* losses, float* factor,
+                                          float* info, void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * Odometry training: raw scan pairs -> updated weights, one call per step.
  * Replaces, for the self-supervised step, deploy.deployer.Deployer.step + Trainer's Adam
@@ -1201,6 +1245,42 @@ int delora_odometry_streams_push_adapt_group(const delora_odometry_desc* d, cons
                                              const delora_odometry_train_group* g, int update,
                                              const float* points, const int32_t* n_points, const int32_t* active,
                                              void* workspace, float* T, int32_t* valid, float* losses, void* stream);
+
+/* ---- Adapting streams with the information of each frame's residual: the Gauss-Newton information of the tick's ICP
+ * objective at the served T (before the tick's update), beside the losses, so that a fleet adapting its model while it
+ * drives can tell when a frame comes from a degenerate scene (see delora_icp_dense_information).
+ * Workspace: the group layout of the adapting streams (delora_odometry_streams_adapt_group_workspace_bytes(d) bytes,
+ * unchanged) followed by the information section: the rows of the S pairs and delora_icp_information_scratch_floats(S,
+ * H, W) floats, each 256-byte aligned.  One workspace serves both pushes below; _streams_adapt_reset, _train_weights,
+ * _train_get_state / _set_state and _train_eval work on it unchanged.  delora_odometry_streams_adapt_info_init:
+ * _streams_adapt_group_init over this size (the collective kernels preloaded too).
+ * delora_odometry_streams_push_adapt_info: the arguments of _push_adapt plus info [S, DELORA_INFO_ROW] (device,
+ * required); delora_odometry_streams_push_adapt_group_info: those of _push_adapt_group plus info.  The tick's ICP is
+ * the information operator in place of delora_icp_dense_fwd_bwd; its losses and dL/dT are that operator's bits, so T,
+ * valid, the loss rows and the updated model (weights, Adam state) are _push_adapt's (_push_adapt_group's) bytes over
+ * the same ticks.  Where valid[s] = 1, info[s] is bit for bit the row of the operator run alone at B = 1 on the tick's
+ * H x W grids and T's 3x4 in the model's units: delora_icp_dense_information for a plain model,
+ * delora_icp_dense_information_scaled with the pair's factor for a DELORA_TRAIN_NORMALIZATION_SCALING one, so H is in
+ * the metres and radians of the served T.  Rows with valid[s] = 0 are zeros.  Refused before any launch: what
+ * _push_adapt (_push_adapt_group) refuses, and a null info.  Out of scope: _push_adapt_geometries.
+ * Measured on one H100 80GB HBM3 at a 700 W power limit (max SM clock 1980 MHz), graph-replayed update = 1 ticks,
+ * lr 0, w_pre 0, all streams active, medians of alternating samples, _push_adapt -> _push_adapt_info per tick:
+ * 64 x 2048: S = 1 3.73 -> 3.79 ms, S = 4 6.69 -> 6.77 ms, S = 16 23.05 -> 23.19 ms; 64 x 720: S = 1 3.54 -> 3.57 ms,
+ * S = 4 4.44 -> 4.48 ms, S = 16 14.23 -> 14.30 ms (scripts/gpu_odometry_streams_pre_adapt_info.py,
+ * profiles/odometry_streams_pre_adapt_info_h100_700w.json).  The group push's cost across several GPUs is not
+ * measured. */
+int64_t delora_odometry_streams_adapt_info_workspace_bytes(const delora_odometry_desc* d);   /* host only */
+int delora_odometry_streams_adapt_info_init(const delora_odometry_desc* d, const float* weights, void* workspace,
+                                            void* stream);
+int delora_odometry_streams_push_adapt_info(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
+                                            int update, const float* points, const int32_t* n_points,
+                                            const int32_t* active, void* workspace, float* T, int32_t* valid,
+                                            float* losses, float* info, void* stream);
+int delora_odometry_streams_push_adapt_group_info(const delora_odometry_desc* d, const delora_odometry_train_params* hp,
+                                                  const delora_odometry_train_group* g, int update,
+                                                  const float* points, const int32_t* n_points, const int32_t* active,
+                                                  void* workspace, float* T, int32_t* valid, float* losses, float* info,
+                                                  void* stream);
 
 /* ---- Training on several sensor geometries from one workspace (the reference's `datasets` list,
  * config/deployment_options.yaml:3: its Trainer shuffles over the concatenated datasets, src/deploy/trainer.py:95-101,
