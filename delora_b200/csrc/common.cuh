@@ -256,6 +256,14 @@ int count_allreduce_launch(const uint64_t* peer_slots, const uint64_t* peer_flag
 // Loads count_allreduce_kernel and the device-seq all-reduce kernels on the current device (see grad_allreduce.cu)
 int collective_kernels_preload(const char* who);
 
+// The dense ICP operator (icp_dense.cu) behind delora_icp_dense_fwd_bwd (info NULL) and
+// delora_icp_dense_information[_scaled] (info and info_scratch non-NULL; factor NULL: H unscaled), its refusals
+// naming `who`.  The callers check info, info_scratch and factor.
+int icp_dense_launch(const delora_f4* src_grid, const delora_f4* src_ngrid, const float* T, const delora_f4* tgt_grid,
+                     const delora_f4* tgt_ngrid, int B, int H, int W, double hfov0, double hfov1, double vfov0,
+                     double vfov1, float lambda_po2pl, uint32_t flags, float* losses, float* grad_T, float* scratch,
+                     float* info, float* info_scratch, const float* factor, cudaStream_t st, const char* who);
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -761,12 +761,13 @@ extern "C" int delora_icp_stats(uint32_t* out32, int reset) {
     return 0;
 }
 
-// delora_icp_dense_fwd_bwd (nn_ids NULL) and the search + finalize of delora_icp_dense_information (nn_ids [B, H*W]:
-// the IDS instantiations, which the DELORA_ICP_STATS ones never are)
-static int dense_icp(const delora_f4* src_grid, const delora_f4* src_ngrid, const float* T, const delora_f4* tgt_grid,
+namespace delora {
+
+int icp_dense_launch(const delora_f4* src_grid, const delora_f4* src_ngrid, const float* T, const delora_f4* tgt_grid,
                      const delora_f4* tgt_ngrid, int B, int H, int W, double hfov0, double hfov1, double vfov0,
                      double vfov1, float lambda_po2pl, uint32_t flags, float* losses, float* grad_T, float* scratch,
-                     int* nn_ids, cudaStream_t st, const char* who) {
+                     float* info, float* info_scratch, const float* factor, cudaStream_t st, const char* who) {
+    DELORA_CHECK_ARG(!info || (flags & DELORA_ICP_STATS) == 0u, "%s: DELORA_ICP_STATS is not counted here", who);
     DELORA_CHECK_ARG(src_grid && src_ngrid && T && tgt_grid && tgt_ngrid && losses && grad_T && scratch,
                      "%s: null pointer", who);
     DELORA_CHECK_ARG(B > 0 && B <= 65535 && H > 0 && W > 0 && (long long)H * W < (1ll << 31), "%s: bad shape", who);
@@ -781,24 +782,31 @@ static int dense_icp(const delora_f4* src_grid, const delora_f4* src_ngrid, cons
     if (const char* e = getenv("DELORA_ICP_MAX_STRIPS")) max_strips = atoi(e);      // tuning knob (tests / profiling)
     target_extents_kernel<<<dim3(nbh, B), kExtThreads, 0, st>>>((const float4*)tgt_grid, H, W, nbh, nbw, sc.ext);
     DELORA_CHECK_LAUNCH("target_extents_kernel");
+    // the information reads each pixel's kept NN from info_scratch (the IDS instantiations, never the STATS ones)
+    int* nn_ids = info ? reinterpret_cast<int*>(info_scratch) : nullptr;
     using DenseSearch = decltype(&launch_dense_search<false, false>);
     constexpr DenseSearch kSearch[2][3] = {
         {launch_dense_search<false, false>, launch_dense_search<false, true>, launch_dense_search<false, false, true>},
         {launch_dense_search<true, false>, launch_dense_search<true, true>, launch_dense_search<true, false, true>}};
     const int variant = nn_ids ? 2 : (flags & DELORA_ICP_STATS) != 0u ? 1 : 0;
-    const int rc = kSearch[(flags & DELORA_LOSS_PO2PO) != 0u][variant](
+    int rc = kSearch[(flags & DELORA_LOSS_PO2PO) != 0u][variant](
         (const float4*)src_grid, (const float4*)src_ngrid, T, (const float4*)tgt_grid, (const float4*)tgt_ngrid, B,
         L.rows, nbh, nbw, max_strips, g, flags, sc, nn_ids, st);
-    if (rc != 0) return rc;
-    return launch_icp_finalize(sc, B, L.rows, lambda_po2pl, losses, grad_T, st);
+    if (rc == 0) rc = launch_icp_finalize(sc, B, L.rows, lambda_po2pl, losses, grad_T, st);
+    if (rc != 0 || !info) return rc;
+    return launch_icp_information((const float4*)src_grid, (const float4*)src_ngrid, T, (const float4*)tgt_ngrid, B,
+                                  H * W, lambda_po2pl, flags, losses, info_scratch, info, factor, st);
 }
+
+}  // namespace delora
 
 extern "C" int delora_icp_dense_fwd_bwd(const delora_f4* src_grid, const delora_f4* src_ngrid, const float* T,
                                         const delora_f4* tgt_grid, const delora_f4* tgt_ngrid, int B, int H, int W,
                                         double hfov0, double hfov1, double vfov0, double vfov1, float lambda_po2pl,
                                         uint32_t flags, float* losses, float* grad_T, float* scratch, void* stream) {
-    return dense_icp(src_grid, src_ngrid, T, tgt_grid, tgt_ngrid, B, H, W, hfov0, hfov1, vfov0, vfov1, lambda_po2pl,
-                     flags, losses, grad_T, scratch, nullptr, (cudaStream_t)stream, "delora_icp_dense_fwd_bwd");
+    return icp_dense_launch(src_grid, src_ngrid, T, tgt_grid, tgt_ngrid, B, H, W, hfov0, hfov1, vfov0, vfov1,
+                            lambda_po2pl, flags, losses, grad_T, scratch, nullptr, nullptr, nullptr,
+                            (cudaStream_t)stream, "delora_icp_dense_fwd_bwd");
 }
 
 extern "C" int64_t delora_icp_information_scratch_floats(int B, int H, int W) {
@@ -806,30 +814,16 @@ extern "C" int64_t delora_icp_information_scratch_floats(int B, int H, int W) {
     return icp_info_layout(B, H * W).total;
 }
 
-// delora_icp_dense_information (factor NULL) and delora_icp_dense_information_scaled
-static int dense_information(const delora_f4* src_grid, const delora_f4* src_ngrid, const float* T,
-                             const delora_f4* tgt_grid, const delora_f4* tgt_ngrid, int B, int H, int W, double hfov0,
-                             double hfov1, double vfov0, double vfov1, float lambda_po2pl, uint32_t flags, float* losses,
-                             float* grad_T, float* scratch, float* info, float* info_scratch, const float* factor,
-                             cudaStream_t st, const char* who) {
-    DELORA_CHECK_ARG(info && info_scratch, "%s: null pointer", who);
-    DELORA_CHECK_ARG((flags & DELORA_ICP_STATS) == 0u, "%s: DELORA_ICP_STATS is not counted here", who);
-    int* nn_ids = reinterpret_cast<int*>(info_scratch);
-    const int rc = dense_icp(src_grid, src_ngrid, T, tgt_grid, tgt_ngrid, B, H, W, hfov0, hfov1, vfov0, vfov1,
-                             lambda_po2pl, flags, losses, grad_T, scratch, nn_ids, st, who);
-    if (rc != 0) return rc;
-    return launch_icp_information((const float4*)src_grid, (const float4*)src_ngrid, T, (const float4*)tgt_ngrid, B, H * W, lambda_po2pl, flags, losses, info_scratch, info,
-                                  factor, st);
-}
-
 extern "C" int delora_icp_dense_information(const delora_f4* src_grid, const delora_f4* src_ngrid, const float* T,
                                             const delora_f4* tgt_grid, const delora_f4* tgt_ngrid, int B, int H, int W,
                                             double hfov0, double hfov1, double vfov0, double vfov1, float lambda_po2pl,
                                             uint32_t flags, float* losses, float* grad_T, float* scratch, float* info,
                                             float* info_scratch, void* stream) {
-    return dense_information(src_grid, src_ngrid, T, tgt_grid, tgt_ngrid, B, H, W, hfov0, hfov1, vfov0, vfov1,
-                             lambda_po2pl, flags, losses, grad_T, scratch, info, info_scratch, nullptr,
-                             (cudaStream_t)stream, "delora_icp_dense_information");
+    const char* who = "delora_icp_dense_information";
+    DELORA_CHECK_ARG(info && info_scratch, "%s: null pointer", who);
+    return icp_dense_launch(src_grid, src_ngrid, T, tgt_grid, tgt_ngrid, B, H, W, hfov0, hfov1, vfov0, vfov1,
+                            lambda_po2pl, flags, losses, grad_T, scratch, info, info_scratch, nullptr,
+                            (cudaStream_t)stream, who);
 }
 
 extern "C" int delora_icp_dense_information_scaled(const delora_f4* src_grid, const delora_f4* src_ngrid,
@@ -841,7 +835,8 @@ extern "C" int delora_icp_dense_information_scaled(const delora_f4* src_grid, co
                                                    void* stream) {
     const char* who = "delora_icp_dense_information_scaled";
     DELORA_CHECK_ARG(factor, "%s: null factor", who);
-    return dense_information(src_grid, src_ngrid, T, tgt_grid, tgt_ngrid, B, H, W, hfov0, hfov1, vfov0, vfov1,
-                             lambda_po2pl, flags, losses, grad_T, scratch, info, info_scratch, factor,
-                             (cudaStream_t)stream, who);
+    DELORA_CHECK_ARG(info && info_scratch, "%s: null pointer", who);
+    return icp_dense_launch(src_grid, src_ngrid, T, tgt_grid, tgt_ngrid, B, H, W, hfov0, hfov1, vfov0, vfov1,
+                            lambda_po2pl, flags, losses, grad_T, scratch, info, info_scratch, factor,
+                            (cudaStream_t)stream, who);
 }

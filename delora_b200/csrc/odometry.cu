@@ -916,18 +916,13 @@ odometry_streams_pre_kernel(const float* __restrict__ T16, const float* __restri
     }
 }
 
-// After the ICP: losses [S, DELORA_LOSS_ROW] = the ICP's row of the valid streams, zeros for the others
-__global__ void odometry_streams_losses_kernel(const int32_t* __restrict__ valid, int S,
-                                               const float* __restrict__ icp_losses, float* __restrict__ losses) {
+// out [S, kRow] = the rows [S, kRow] of the valid streams, zeros for the others: the ICP's loss rows
+// (DELORA_LOSS_ROW) or the information operator's rows (DELORA_INFO_ROW)
+template <int kRow>
+__global__ void odometry_streams_rows_kernel(const int32_t* __restrict__ valid, int S, const float* __restrict__ rows,
+                                             float* __restrict__ out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < S * DELORA_LOSS_ROW) losses[i] = valid[i / DELORA_LOSS_ROW] != 0 ? icp_losses[i] : 0.0f;
-}
-
-// After the information operator: info [S, DELORA_INFO_ROW] = its row for the valid streams, zeros for the others
-__global__ void odometry_streams_info_kernel(const int32_t* __restrict__ valid, int S, const float* __restrict__ icp_info,
-                                             float* __restrict__ info) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < S * DELORA_INFO_ROW) info[i] = valid[i / DELORA_INFO_ROW] != 0 ? icp_info[i] : 0.0f;
+    if (i < S * kRow) out[i] = valid[i / kRow] != 0 ? rows[i] : 0.0f;
 }
 
 // check_desc plus the preprocessing width the recipe streams read (the training rule, but w_pre = 0 is refused)
@@ -1023,6 +1018,12 @@ static int streams_forward(const Model& m, const TailIO& io, const TrunkActs& t,
     return 0;
 }
 
+// The ICP entry point whose work icp_dense_launch does with these info and factor pointers: the name its refusals give
+static const char* icp_entry(const float* info, const float* factor) {
+    return !info ? "delora_icp_dense_fwd_bwd" : factor ? "delora_icp_dense_information_scaled"
+                                                       : "delora_icp_dense_information";
+}
+
 // The ICP at B = S on a residual or recipe plan's H x W grids: source pts_grid moved by T12, target prev_pts_grid,
 // into its losses and grad_T; on an information plan (p.info set) also into its information rows, in metres with the
 // pair factors of a normalised recipe (factor non-NULL).  The recipe's DELORA_TRAIN_NORMALIZATION_SCALING is not an
@@ -1032,26 +1033,20 @@ static int streams_icp(const delora_odometry_desc* d, const delora_odometry_resi
     auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
     auto f4 = [&](size_t o) { return reinterpret_cast<delora_f4*>(ws + o); };
     const uint32_t flags = rp->loss_flags & ~DELORA_TRAIN_NORMALIZATION_SCALING;
-    if (p.info && factor)
-        return delora_icp_dense_information_scaled(f4(p.pts_grid), f4(p.nrm_grid), f(p.T12), f4(p.prev_pts_grid),
-                                                   f4(p.prev_nrm_grid), d->max_batch, d->H, d->W, d->hfov0, d->hfov1,
-                                                   d->vfov0, d->vfov1, rp->lambda_po2pl, flags, f(p.losses),
-                                                   f(p.grad_T), f(p.icp), f(p.info), f(p.info_scratch), factor, st);
-    if (p.info)
-        return delora_icp_dense_information(f4(p.pts_grid), f4(p.nrm_grid), f(p.T12), f4(p.prev_pts_grid),
-                                            f4(p.prev_nrm_grid), d->max_batch, d->H, d->W, d->hfov0, d->hfov1,
-                                            d->vfov0, d->vfov1, rp->lambda_po2pl, flags, f(p.losses),
-                                            f(p.grad_T), f(p.icp), f(p.info), f(p.info_scratch), st);
-    return delora_icp_dense_fwd_bwd(f4(p.pts_grid), f4(p.nrm_grid), f(p.T12), f4(p.prev_pts_grid), f4(p.prev_nrm_grid),
-                                    d->max_batch, d->H, d->W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, rp->lambda_po2pl,
-                                    flags, f(p.losses), f(p.grad_T), f(p.icp), st);
+    float* info = p.info ? f(p.info) : nullptr;
+    if (!info) factor = nullptr;
+    return icp_dense_launch(f4(p.pts_grid), f4(p.nrm_grid), f(p.T12), f4(p.prev_pts_grid), f4(p.prev_nrm_grid),
+                            d->max_batch, d->H, d->W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, rp->lambda_po2pl, flags,
+                            f(p.losses), f(p.grad_T), f(p.icp), info, info ? f(p.info_scratch) : nullptr, factor, st,
+                            icp_entry(info, factor));
 }
 
-// info [S, DELORA_INFO_ROW] = the information rows at `rows` of the valid streams, zeros for the others
-static int streams_info_out(const int32_t* valid, int S, const float* rows, float* info, cudaStream_t st) {
-    const int n = S * DELORA_INFO_ROW;
-    odometry_streams_info_kernel<<<(n + 255) / 256, 256, 0, st>>>(valid, S, rows, info);
-    DELORA_CHECK_LAUNCH("odometry_streams_info_kernel");
+// out [S, kRow] = the rows [S, kRow] at `rows` of the valid streams, zeros for the others
+template <int kRow>
+static int streams_rows_out(const int32_t* valid, int S, const float* rows, float* out, cudaStream_t st) {
+    odometry_streams_rows_kernel<kRow><<<(S * kRow + 255) / 256, 256, 0, st>>>(valid, S, rows, out);
+    DELORA_CHECK_LAUNCH(kRow == DELORA_INFO_ROW ? "odometry_streams_rows_kernel<DELORA_INFO_ROW>"
+                                                : "odometry_streams_rows_kernel<DELORA_LOSS_ROW>");
     return 0;
 }
 
@@ -1145,7 +1140,7 @@ static int run_streams_push(const delora_odometry_desc* d, const delora_odometry
     odometry_streams_grids_kernel<1><<<blocks, 256, 0, st>>>(pts_grid, nrm_grid, prev_pts, prev_nrm, active, valid, S, HW,
                                                              T, T12, icp_losses, losses);
     DELORA_CHECK_LAUNCH("odometry_streams_grids_kernel<1>");
-    return info ? streams_info_out(valid, S, reinterpret_cast<float*>(ws + p.info), info, st) : 0;
+    return info ? streams_rows_out<DELORA_INFO_ROW>(valid, S, reinterpret_cast<float*>(ws + p.info), info, st) : 0;
 }
 
 extern "C" int delora_odometry_streams_push(const delora_odometry_desc* d, const float* points, const int32_t* n_points,
@@ -1318,9 +1313,8 @@ static int run_push_pre(const delora_odometry_desc* d, const delora_odometry_res
         reinterpret_cast<float4*>(pre_prev_nrm));
     DELORA_CHECK_LAUNCH("odometry_streams_pre_kernel");
     if ((rc = streams_icp(d, rp, p, ws, factor, st))) return rc;
-    odometry_streams_losses_kernel<<<(S * DELORA_LOSS_ROW + 255) / 256, 256, 0, st>>>(valid, S, f(p.losses), losses);
-    DELORA_CHECK_LAUNCH("odometry_streams_losses_kernel");
-    return info ? streams_info_out(valid, S, f(p.info), info, st) : 0;
+    if ((rc = streams_rows_out<DELORA_LOSS_ROW>(valid, S, f(p.losses), losses, st))) return rc;
+    return info ? streams_rows_out<DELORA_INFO_ROW>(valid, S, f(p.info), info, st) : 0;
 }
 
 extern "C" int delora_odometry_streams_push_pre(const delora_odometry_desc* d, const delora_odometry_residual_params* rp,
@@ -2119,22 +2113,12 @@ static int train_forward_losses(const delora_odometry_desc* d, const delora_odom
     DELORA_CHECK_LAUNCH("odometry_icp_rearm_kernel");
     const uint32_t icp_flags =
         hp->loss_flags & ~(DELORA_LOSS_IDENTITY_FIT | DELORA_TRAIN_NORMALIZATION_SCALING | DELORA_TRAIN_DROPOUT);
-    if (at && at->info && normalized) {
-        rc = delora_icp_dense_information_scaled(pts_grid + (size_t)B * HW, nrm_grid + (size_t)B * HW, f(tp.T12),
-                                                 pts_grid, nrm_grid, B, H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1,
-                                                 hp->lambda_po2pl, icp_flags, f(tp.losses), f(tp.grad_T), f(tp.icp),
-                                                 at->info, at->info_scratch, f(tp.pre_image), st);
-    } else if (at && at->info) {
-        rc = delora_icp_dense_information(pts_grid + (size_t)B * HW, nrm_grid + (size_t)B * HW, f(tp.T12), pts_grid,
-                                          nrm_grid, B, H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, hp->lambda_po2pl,
-                                          icp_flags, f(tp.losses), f(tp.grad_T), f(tp.icp), at->info,
-                                          at->info_scratch, st);
-    } else {
-        rc = delora_icp_dense_fwd_bwd(pts_grid + (size_t)B * HW, nrm_grid + (size_t)B * HW, f(tp.T12), pts_grid, nrm_grid,
-                                      B, H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, hp->lambda_po2pl, icp_flags,
-                                      f(tp.losses), f(tp.grad_T), f(tp.icp), st);
-    }
-    if (rc) return rc;
+    float* info = at ? at->info : nullptr;
+    const float* factor = info && normalized ? f(tp.pre_image) : nullptr;
+    if ((rc = icp_dense_launch(pts_grid + (size_t)B * HW, nrm_grid + (size_t)B * HW, f(tp.T12), pts_grid, nrm_grid, B,
+                               H, W, d->hfov0, d->hfov1, d->vfov0, d->vfov1, hp->lambda_po2pl, icp_flags,
+                               f(tp.losses), f(tp.grad_T), f(tp.icp), info, at ? at->info_scratch : nullptr, factor,
+                               st, icp_entry(info, factor)))) return rc;
     if (normalized) {               // T in metres for the caller, the factor in losses[b][6]
         odometry_train_normalized_out_kernel<<<(B * 16 + 255) / 256, 256, 0, st>>>(f(tp.T16), f(tp.pre_image), B, T_out,
                                                                                       f(tp.losses));
@@ -2575,9 +2559,8 @@ static int serve_adapt(const delora_odometry_desc* d, const delora_odometry_trai
     int rc;
     // 1-3 at B = S, the first frame of every pair from the cache; T, valid, the cache and the emptied sources
     if ((rc = train_forward_losses(d, hp, tp, ws, points, n_points, S, false, nullptr, st, who, &at))) return rc;
-    odometry_streams_losses_kernel<<<(S * DELORA_LOSS_ROW + 255) / 256, 256, 0, st>>>(valid, S, f(tp.losses), losses);
-    DELORA_CHECK_LAUNCH("odometry_streams_losses_kernel");
-    if (info && (rc = streams_info_out(valid, S, f(ap.info), info, st))) return rc;
+    if ((rc = streams_rows_out<DELORA_LOSS_ROW>(valid, S, f(tp.losses), losses, st))) return rc;
+    if (info && (rc = streams_rows_out<DELORA_INFO_ROW>(valid, S, f(ap.info), info, st))) return rc;
     if (!update) {          // the ICP scratch now has the layout of S pairs, as after _train_eval
         odometry_icp_batch_kernel<<<1, 1, 0, st>>>(reinterpret_cast<long long*>(ws + tp.ctr), S);
         DELORA_CHECK_LAUNCH("odometry_icp_batch_kernel");

@@ -8,6 +8,7 @@ import functools
 import os
 import subprocess
 
+import numpy as np
 import torch
 
 from delora_b200 import ops
@@ -248,3 +249,180 @@ def train_params(flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL, lr=1e-5):
     from delora_b200 import _lib
     return _lib.OdometryTrainParams(lr=lr, beta1=0.9, beta2=0.999, eps=1e-8, lambda_po2pl=1.0, loss_flags=flags,
                                     nb_h=7, nb_w=11, epsilon_range=0.5, min_neighbors=10)
+
+
+# ------------------------------------------------------------------------------------------- streams workspaces
+SENTINEL = 1234.5          # what the float outputs hold before a streams call writes them; valid holds 7
+GUARD = 4096               # guard bytes on each side of a guarded workspace
+
+
+def stage_ticks(act, n_stride, frame, count=None):
+    """Host staging of every tick of S = act.shape[1] streams: frame(k, s) -> the points [3, n] stream s is given at
+    tick k (an inactive stream too: only `active` keeps it out), count(k, s, n) -> its count (default n)
+    -> [(points [S, 3, n_stride], counts [S], active [S])]."""
+    out = []
+    for k in range(act.shape[0]):
+        pts = torch.zeros((act.shape[1], 3, n_stride), dtype=torch.float32)
+        counts = torch.zeros((act.shape[1],), dtype=torch.int32)
+        for s in range(act.shape[1]):
+            f = frame(k, s)
+            pts[s, :, :f.shape[1]] = f
+            counts[s] = f.shape[1] if count is None else count(k, s, f.shape[1])
+        out.append((pts, counts, torch.from_numpy(act[k].astype(np.int32))))
+    return out
+
+
+def recipe_pattern(S, ticks=7):
+    """The adapting and recipe streams' activity: active [ticks, S] with an inactive stream at tick 1, an idle tick 4
+    and stream 0 out at tick 6, the (tick, stream) with an empty frame and the resets {tick: [streams]}."""
+    act = np.ones((ticks, S), dtype=bool)
+    act[1, S - 1] = False
+    act[4, :] = False
+    if ticks > 6:
+        act[6, 0] = False
+    return act, {(2, 1 % S)}, {3: [0]}
+
+
+def recipe_ticks(pool, S, n_stride, act, empty):
+    """stage_ticks of stream s on pool[(3 s + k) % len(pool)] at tick k, an inactive one on another pool frame with its
+    real count (only the mask keeps it out), the frames in `empty` with count 0."""
+    return stage_ticks(act, n_stride, lambda k, s: pool[(3 * s + k + (0 if act[k, s] else 5)) % len(pool)],
+                       lambda k, s, n: 0 if (k, s) in empty else n)
+
+
+def pool_tick(pool, S, n_stride, k, active, offset=0):
+    """Tick k of S streams on the device: stream s serves pool[(3 * (s + offset) + k) % len(pool)] where active[s]."""
+    pts = torch.zeros((S, 3, n_stride), dtype=torch.float32)
+    counts = torch.zeros((S,), dtype=torch.int32)
+    for s in range(S):
+        f = pool[(3 * (s + offset) + k) % len(pool)]
+        pts[s, :, :f.shape[1]] = f
+        counts[s] = f.shape[1]
+    return pts.to(DEV), counts.to(DEV), torch.tensor(active, dtype=torch.int32, device=DEV)
+
+
+def group_tick(g, streams, inputs, updates):
+    """Every rank's tick of an AdaptingStreamsGroup on its own stream, all enqueued before one synchronisation -> its
+    outputs per rank on the host."""
+    torch.cuda.synchronize()
+    outs = []
+    for r, (pts, counts, active) in enumerate(inputs):
+        with torch.cuda.stream(streams[r]):
+            outs.append(g.push(r, pts, counts, active, update=updates[r]))
+    torch.cuda.synchronize()
+    return [tuple(t.cpu() for t in o) for o in outs]
+
+
+def group_status_ok(g):
+    return all(int(s.item()) == 0 for s in g.status)
+
+
+def history(ticks, act, resets):
+    """{(k, s): (previous frame, this frame)} of every pair the streams should serve: (points [3, n], count)."""
+    pairs, prev = {}, [None] * act.shape[1]
+    for k, (p, c, _) in enumerate(ticks):
+        for s in resets.get(k, []):
+            prev[s] = None
+        for s in range(act.shape[1]):
+            if not act[k, s]:
+                continue
+            if prev[s] is not None:
+                pairs[(k, s)] = (prev[s], (p[s], c[s]))
+            prev[s] = (p[s], c[s])
+    return pairs
+
+
+def guarded_workspace(nbytes):
+    """A device workspace of exactly nbytes between GUARD guard bytes on each side, its own bytes all 0xFF (NaN floats)
+    -> (workspace, intact), intact() True while no call has written outside it."""
+    buf = torch.full((nbytes + 2 * GUARD,), 0xFF, dtype=torch.uint8, device=DEV)
+    pattern = torch.arange(GUARD, device=DEV).to(torch.uint8) ^ 0xA5
+    buf[:GUARD] = pattern
+    buf[GUARD + nbytes:] = pattern
+
+    def intact():
+        torch.cuda.synchronize()
+        return torch.equal(buf[:GUARD], pattern) and torch.equal(buf[GUARD + nbytes:], pattern)
+    return buf[GUARD:GUARD + nbytes], intact
+
+
+ROW_WIDTH = {"losses": ops.LOSS_ROW, "info": ops.INFO_ROW, "factor": None}
+
+
+class Outputs:
+    """The outputs of a streams push in its argument order: T [S, 16], valid [S], then the rows named in `rows` (any of
+    "losses" [S, LOSS_ROW], "info" [S, INFO_ROW], "factor" [S], in that order), each between a guard row on either
+    side.  Every float holds SENTINEL and valid holds 7 until a call writes them."""
+
+    def __init__(self, S, rows=()):
+        assert list(rows) == [r for r in ROW_WIDTH if r in rows], rows
+        self.T = torch.empty((S, 16), dtype=torch.float32, device=DEV)
+        self.valid = torch.empty((S,), dtype=torch.int32, device=DEV)
+        self.guarded = [torch.empty((S + 2,) + ((ROW_WIDTH[r],) if ROW_WIDTH[r] else ()), dtype=torch.float32,
+                                    device=DEV) for r in rows]
+        self.tensors = (self.T, self.valid) + tuple(g[1:S + 1] for g in self.guarded)
+        self.fill()
+
+    def fill(self):
+        self.valid.fill_(7)
+        for t in (self.T, *self.guarded):
+            t.fill_(SENTINEL)
+
+    def snapshot(self, k=None):
+        """Synchronises, asserts every guard row still holds SENTINEL -> the outputs copied to the host."""
+        torch.cuda.synchronize()
+        for g in self.guarded:
+            assert bool((g[0] == SENTINEL).all()) and bool((g[-1] == SENTINEL).all()), \
+                f"tick {k}: a write outside an output row"
+        return tuple(t.cpu().clone() for t in self.tensors)
+
+
+def run_streams(ws, ticks, rows=(), resets=None, updates=None, loads=None, graph=False, hook=None):
+    """Every tick (points [S, 3, n], counts [S], active [S]) through one streams workspace -> per tick the outputs of
+    Outputs(S, rows) on the host, plus hook(ws) when given.
+
+    Before tick k: the streams in resets[k] are reset through a mask, then loads[k] is loaded (load_weights).  updates:
+    the adapting workspaces' update flag of each tick.  graph: every stream inactive, one push per update value (which
+    changes no stream's state), the sentinels restored, then one captured push per update value replays each tick."""
+    S = ws.desc.max_batch
+    pts = torch.zeros((S, 3, ticks[0][0].shape[2]), dtype=torch.float32, device=DEV)
+    counts = torch.zeros((S,), dtype=torch.int32, device=DEV)
+    active = torch.zeros((S,), dtype=torch.int32, device=DEV)
+    mask = torch.zeros((S,), dtype=torch.int32, device=DEV)
+    out = Outputs(S, rows)
+    args = (pts, counts, active) + out.tensors
+    modes = sorted(set(updates)) if updates is not None else [None]
+
+    def push(u):
+        if u is None:
+            ws.push(*args)
+        else:
+            ws.push(*args, update=u)
+    graphs = {}
+    if graph:
+        for u in modes:
+            push(u)
+        torch.cuda.synchronize()
+        out.fill()
+        for u in modes:
+            graphs[u] = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graphs[u]):
+                push(u)
+    got = []
+    for k, (p, c, a) in enumerate(ticks):
+        if resets and k in resets:
+            mask.zero_()
+            mask[list(resets[k])] = 1
+            ws.reset(mask)
+        if loads and k in loads:
+            ws.load_weights(loads[k])
+        pts.copy_(p)
+        counts.copy_(c)
+        active.copy_(a)
+        u = None if updates is None else updates[k]
+        if graph:
+            graphs[u].replay()
+        else:
+            push(u)
+        got.append(out.snapshot(k) + ((hook(ws),) if hook else ()))
+    return got

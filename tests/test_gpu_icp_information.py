@@ -210,40 +210,7 @@ def test_box_room_constrains_every_direction(cuda_lib):
 
 
 # ============================================================================================ _push_info
-from test_gpu_odometry_eval import SENTINEL, _reset, _run_residual, _streams_setup  # noqa: E402
-
-
-def _run_info(st, ticks, resets, graph=False):
-    S = st.desc.max_batch
-    pts, counts, active = (torch.zeros_like(t) for t in ticks[0])
-    T = torch.full((S, 16), SENTINEL, dtype=torch.float32, device=DEV)
-    valid = torch.full((S,), 7, dtype=torch.int32, device=DEV)
-    losses = torch.full((S, ops.LOSS_ROW), SENTINEL, dtype=torch.float32, device=DEV)
-    guarded = torch.full((S + 2, ops.INFO_ROW), SENTINEL, dtype=torch.float32, device=DEV)
-    info = guarded[1:S + 1]
-    g = None
-    if graph:
-        st.push(pts, counts, active, T, valid, losses, info)
-        valid.fill_(7)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            st.push(pts, counts, active, T, valid, losses, info)
-    out = []
-    for k, (p, c, a) in enumerate(ticks):
-        if k in resets:
-            _reset(st, S, resets[k])
-        pts.copy_(p)
-        counts.copy_(c)
-        active.copy_(a)
-        if g is not None:
-            g.replay()
-        else:
-            st.push(pts, counts, active, T, valid, losses, info)
-        out.append((T.clone(), valid.clone(), losses.clone(), info.clone()))
-        assert bool((guarded[0] == SENTINEL).all()) and bool((guarded[S + 1] == SENTINEL).all()), \
-            f"tick {k}: a write outside info [S, INFO_ROW]"
-    return out
+from test_gpu_odometry_eval import _streams_setup  # noqa: E402
 
 
 def _info_rows(cfg, ticks, act, resets, out, flags):
@@ -259,12 +226,13 @@ def _info_rows(cfg, ticks, act, resets, out, flags):
         for s in range(S):
             if not act[k, s]:
                 continue
-            _, _, pg, ng = ops.project_normals(p[s:s + 1], c[s:s + 1], h, w, hf, vf, ds["neighborhood_side_length"],
-                                               cfg["epsilon_range"],
+            _, _, pg, ng = ops.project_normals(p[s:s + 1].to(DEV), c[s:s + 1].to(DEV), h, w, hf, vf,
+                                               ds["neighborhood_side_length"], cfg["epsilon_range"],
                                                cfg["min_num_points_in_neighborhood_to_determine_point_class"])
             if prev[s] is not None:
-                rows[(k, s)] = ops.icp_dense_information(pg, ng, T[s:s + 1, :12].contiguous(), prev[s][0], prev[s][1],
-                                                         h, w, hf, vf, float(cfg["lambda_po2pl"]), flags)[2][0]
+                rows[(k, s)] = ops.icp_dense_information(pg, ng, T[s:s + 1, :12].contiguous().to(DEV), prev[s][0],
+                                                         prev[s][1], h, w, hf, vf, float(cfg["lambda_po2pl"]),
+                                                         flags)[2][0].cpu()
             prev[s] = (pg, ng)
     return rows
 
@@ -275,8 +243,10 @@ def _info_rows(cfg, ticks, act, resets, out, flags):
 def test_streams_info_rows_beside_the_residuals_bytes(S, flags, cuda_lib):
     cfg, blob, n_stride, ticks, act, resets = _streams_setup(S)
     d = OH.desc(cfg, n_stride, S)
-    res = _run_residual(capi.ResidualStreamsWorkspace(d, blob, capi.residual_params(cfg, flags)), ticks, resets)
-    out = _run_info(capi.InformationStreamsWorkspace(d, blob, capi.residual_params(cfg, flags)), ticks, resets)
+    res = OH.run_streams(capi.ResidualStreamsWorkspace(d, blob, capi.residual_params(cfg, flags)), ticks, ("losses",),
+                         resets=resets)
+    out = OH.run_streams(capi.InformationStreamsWorkspace(d, blob, capi.residual_params(cfg, flags)), ticks,
+                         ("losses", "info"), resets=resets)
     for k, (r, o) in enumerate(zip(res, out)):
         assert torch.equal(r[1], o[1]), f"tick {k}: valid differs from _push_residual"
         for a, b, what in ((r[0], o[0], "T"), (r[2], o[2], "losses")):
@@ -298,8 +268,9 @@ def test_streams_info_graph_replay_matches_eager(cuda_lib):
     cfg, blob, n_stride, ticks, act, resets = _streams_setup(4)
     d = OH.desc(cfg, n_stride, 4)
     rp = capi.residual_params(cfg)
-    eager = _run_info(capi.InformationStreamsWorkspace(d, blob, rp), ticks, resets)
-    graphed = _run_info(capi.InformationStreamsWorkspace(d, blob, rp), ticks, resets, graph=True)
+    eager = OH.run_streams(capi.InformationStreamsWorkspace(d, blob, rp), ticks, ("losses", "info"), resets=resets)
+    graphed = OH.run_streams(capi.InformationStreamsWorkspace(d, blob, rp), ticks, ("losses", "info"), resets=resets,
+                             graph=True)
     for k, (e, g) in enumerate(zip(eager, graphed)):
         for a, b in zip(e, g):
             assert torch.equal(a.view(torch.int32), b.view(torch.int32)), f"tick {k}: the replay differs"

@@ -31,7 +31,6 @@ from delora_b200.deploy import capi
 pytestmark = pytest.mark.gpu
 DEV = H.DEV
 U = 2.0 ** -24
-SENTINEL = 1234.5
 ICP = ops.LOSS_PO2PL | ops.LOSS_PL2PL
 LR = 1e-4
 
@@ -151,56 +150,25 @@ def test_scaled_operator_is_D_H_D_in_metres(cuda_lib, name):
 
 
 # ============================================================================================ recipe streams
-from test_gpu_odometry_streams_pre import _history, _setup as _pre_setup  # noqa: E402
-
 W_PRE_CASE = (16, 180, 512, 360)             # H, W, w_raw, w_pre
 
 
-def _run_pre(st, ticks, resets, normalized, info, graph=False):
-    """Every tick through one recipe workspace (with info: the information one) -> [(T, valid, losses, factor, info)]."""
-    S = st.desc.max_batch
-    n_stride = ticks[0][0].shape[2]
-    pts = torch.zeros((S, 3, n_stride), dtype=torch.float32, device=DEV)
-    counts = torch.zeros((S,), dtype=torch.int32, device=DEV)
-    active = torch.zeros((S,), dtype=torch.int32, device=DEV)
-    T = torch.full((S, 16), SENTINEL, dtype=torch.float32, device=DEV)
-    valid = torch.full((S,), 7, dtype=torch.int32, device=DEV)
-    losses = torch.full((S, ops.LOSS_ROW), SENTINEL, dtype=torch.float32, device=DEV)
-    factor = torch.full((S,), SENTINEL, dtype=torch.float32, device=DEV) if normalized else None
-    guarded = torch.full((S + 2, ops.INFO_ROW), SENTINEL, dtype=torch.float32, device=DEV)
-    rows = guarded[1:S + 1]
-    mask = torch.zeros((S,), dtype=torch.int32, device=DEV)
+def _pre_setup(h, w, w_raw, w_pre, normalized, S, seed=3):
+    """The recipe streams' history of test_gpu_odometry_streams_pre.py: a tick of first frames, an inactive stream, an
+    empty active frame (tick 2), a reset (before tick 3) and an idle tick."""
+    cfg = _adapt_cfg(h, w, w_pre, normalized)
+    pool = H.frames(h, w_raw, 8)
+    n_stride = max(f.shape[1] for f in pool)
+    act, empty, resets = H.recipe_pattern(S)
+    blob = H.blob(H.model(cfg, seed, near_identity=True), cfg)
+    return cfg, blob, n_stride, H.recipe_ticks(pool, S, n_stride, act, empty), act, resets
 
-    def push():
-        if info:
-            st.push(pts, counts, active, T, valid, losses, rows, factor)
-        else:
-            st.push(pts, counts, active, T, valid, losses, factor)
-    g = None
-    if graph:
-        push()
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            push()
-    out = []
-    for k, (p, c, a) in enumerate(ticks):
-        if k in resets:
-            mask.zero_()
-            mask[resets[k]] = 1
-            st.reset(mask)
-        pts.copy_(p)
-        counts.copy_(c)
-        active.copy_(a)
-        if g is not None:
-            g.replay()
-        else:
-            push()
-        torch.cuda.synchronize()
-        out.append((T.cpu().clone(), valid.cpu().clone(), losses.cpu().clone(),
-                    None if factor is None else factor.cpu().clone(), rows.cpu().clone() if info else None))
-        assert bool((guarded[0] == SENTINEL).all()) and bool((guarded[S + 1] == SENTINEL).all())
-    return out
+
+def _run_pre(st, ticks, resets, normalized, info, graph=False):
+    """Every tick through one recipe workspace (with info: the information one) -> [(T, valid, losses[, info][,
+    factor])]."""
+    rows = ("losses",) + (("info",) if info else ()) + (("factor",) if normalized else ())
+    return H.run_streams(st, ticks, rows, resets=resets, graph=graph)
 
 
 def _pre_grids(cfg, frame, count, ft=None):
@@ -265,11 +233,13 @@ def test_pre_info_streams_are_push_pre_bytes_and_the_operators_rows(cuda_lib, no
     ref = _run_pre(capi.PreStreamsWorkspace(d, blob, rp), ticks, resets, normalized, False)
     out = _run_pre(capi.PreInformationStreamsWorkspace(d, blob, rp), ticks, resets, normalized, True)
     for k, (r, o) in enumerate(zip(ref, out)):
-        for i, what in enumerate(("T", "valid", "losses", "factor")):
-            assert r[i] is None or _bits_equal(r[i], o[i]), f"tick {k}: {what} differs from _push_pre"
-    pairs = _history(ticks, act, resets)
+        for i, what in enumerate(("T", "valid", "losses")):
+            assert _bits_equal(r[i], o[i]), f"tick {k}: {what} differs from _push_pre"
+        assert not normalized or _bits_equal(r[3], o[4]), f"tick {k}: factor differs from _push_pre"
+    pairs = H.history(ticks, act, resets)
     checked = 0
-    for k, (T, valid, losses, factor, rows) in enumerate(out):
+    for k, (T, valid, losses, rows, *factor) in enumerate(out):
+        factor = factor[0] if normalized else None
         for s in range(S):
             if not int(valid[s]):
                 assert float(rows[s].abs().max()) == 0.0, f"tick {k} stream {s}: an invalid row is not zero"
@@ -313,13 +283,9 @@ def test_corridor_served_to_a_normalised_model_leaves_translation_along_it_free(
     blob = H.blob(H.model(base, 3, near_identity=True), base)
     st = capi.PreInformationStreamsWorkspace(H.desc(base, n_stride, 1, 2 * WW), blob,
                                              capi.residual_params(base, ops.LOSS_PO2PL | ops.TRAIN_NORMALIZATION_SCALING))
-    ticks = []
-    for f in frames:
-        p = torch.zeros((1, 3, n_stride), dtype=torch.float32)
-        p[0, :, :f.shape[1]] = f
-        ticks.append((p, torch.tensor([f.shape[1]], dtype=torch.int32), torch.ones((1,), dtype=torch.int32)))
+    ticks = H.stage_ticks(np.ones((2, 1), dtype=bool), n_stride, lambda k, s: frames[k])
     out = _run_pre(st, ticks, {}, True, True)
-    T, valid, losses, factor, rows = out[1]
+    T, valid, losses, rows, factor = out[1]
     assert int(valid[0]) == 1 and float(factor[0]) > 0
     row = rows[0].numpy().astype(np.float64)
     ev, V = row[36:42], row[42:78].reshape(6, 6)
@@ -331,9 +297,6 @@ def test_corridor_served_to_a_normalised_model_leaves_translation_along_it_free(
 
 
 # ============================================================================================ adapting streams
-from test_gpu_odometry_streams_adapt import _Io, _pattern, _ticks  # noqa: E402
-
-
 def _adapt_cfg(h, w, w_pre, normalized):
     cfg = H.config(h, w)
     cfg["kitti"]["horizontal_cells_preprocessing"] = w_pre
@@ -346,23 +309,9 @@ def _train_params(cfg, normalized):
 
 
 def _run_adapt(ws, ticks, updates, resets, info):
-    S = ws.desc.max_batch
-    io = _Io(S, ticks[0][0].shape[2])
-    rows = torch.full((S, ops.INFO_ROW), SENTINEL, dtype=torch.float32, device=DEV)
-    out = []
-    for k, (p, c, a) in enumerate(ticks):
-        if k in resets:
-            io.mask.zero_()
-            io.mask[resets[k]] = 1
-            ws.reset(io.mask)
-        io.load(p, c, a)
-        if info:
-            ws.push(*io.args(), rows, update=updates[k])
-        else:
-            ws.push(*io.args(), update=updates[k])
-        T, valid, losses = io.out()
-        out.append((T, valid, losses, rows.cpu().clone() if info else None, H.state(ws)))
-    return out
+    """-> per tick (T, valid, losses[, info], the training state)."""
+    rows = ("losses", "info") if info else ("losses",)
+    return H.run_streams(ws, ticks, rows, resets=resets, updates=updates, hook=H.state)
 
 
 @pytest.mark.parametrize("w_pre,normalized", [(0, False), (360, False), (360, True)],
@@ -372,8 +321,8 @@ def test_adapt_info_is_push_adapt_bytes_and_the_operators_rows(cuda_lib, w_pre, 
     cfg = _adapt_cfg(h, w, w_pre, normalized)
     pool = H.frames(h, w_raw, 8)
     n_stride = max(f.shape[1] for f in pool)
-    act, empty, resets = _pattern(S)
-    ticks = _ticks(pool, S, n_stride, act, empty)
+    act, empty, resets = H.recipe_pattern(S)
+    ticks = H.recipe_ticks(pool, S, n_stride, act, empty)
     blob = H.blob(H.model(cfg, 5, near_identity=True), cfg)
     d = H.desc(cfg, n_stride, S, w_pre)
     updates = [True, True, False, True, True, False, True]
@@ -387,12 +336,12 @@ def test_adapt_info_is_push_adapt_bytes_and_the_operators_rows(cuda_lib, w_pre, 
         for s in range(S):
             if int(r[1][s]):
                 assert _bits_equal(r[0][s], o[0][s]), f"tick {k} stream {s}: T differs from _push_adapt"
-        assert H.same_state(r[4], o[4]), f"tick {k}: the training state differs from _push_adapt's"
+        assert H.same_state(r[-1], o[-1]), f"tick {k}: the training state differs from _push_adapt's"
     assert int(out[-1][4][3][0]) >= 3
     # each valid row: the B = 1 operator on the tick's grids at the served T (the weights before the tick's update)
     ds = cfg["kitti"]
     hf, vf = tuple(cfg["horizontal_field_of_view"]), tuple(ds["vertical_field_of_view"])
-    pairs = _history(ticks, act, resets)
+    pairs = H.history(ticks, act, resets)
     checked = 0
     for k, (T, valid, losses, rows, _) in enumerate(out):
         for s in range(S):
@@ -419,8 +368,12 @@ def test_adapt_info_is_push_adapt_bytes_and_the_operators_rows(cuda_lib, w_pre, 
     assert checked >= 6
 
 
-from test_gpu_odometry_streams_adapt_group import (_group_tick, _setup as _group_setup, _single,  # noqa: E402
-                                                   _single_tick, _status_ok, _tick_inputs)
+def _group_setup():
+    """The adapting group's scans and model of test_gpu_odometry_streams_adapt_group.py."""
+    cfg = H.config(16, 180)
+    pool = H.frames(16, 512, 10)
+    n_stride = max(f.shape[1] for f in pool)
+    return cfg, H.blob(H.model(cfg, 3, near_identity=True), cfg), pool, n_stride
 
 
 def _info_group(cfg, blob, n_stride, world, S=2):
@@ -440,13 +393,10 @@ def _warm(cfg, blob, pool, n_stride, S):
     but the collectives (which _adapt_info_init loads): the ranks here share one device and one host thread, and under
     lazy module loading a kernel's first launch waits for the device's running kernels, a rank spinning in the count
     exchange among them."""
-    inp = _tick_inputs(pool, S, n_stride, 0, [1] * S)
-    _single_tick(_single(cfg, blob, n_stride, S), *inp, True)
-    ws = capi.AdaptiveInformationStreamsWorkspace(H.desc(cfg, n_stride, S), blob, capi.train_params(cfg, LR))
-    io = _Io(S, n_stride)
-    io.load(*inp)
-    ws.push(*io.args(), torch.empty((S, ops.INFO_ROW), dtype=torch.float32, device=DEV), update=True)
-    torch.cuda.synchronize()
+    inp = [H.pool_tick(pool, S, n_stride, 0, [1] * S)]
+    for cls, rows in ((capi.AdaptiveStreamsWorkspace, ("losses",)),
+                      (capi.AdaptiveInformationStreamsWorkspace, ("losses", "info"))):
+        H.run_streams(cls(H.desc(cfg, n_stride, S), blob, capi.train_params(cfg, LR)), inp, rows, updates=[True])
 
 
 def test_adapt_group_info_at_world_1_is_push_adapt_info(cuda_lib):
@@ -455,23 +405,19 @@ def test_adapt_group_info_at_world_1_is_push_adapt_info(cuda_lib):
     _warm(cfg, blob, pool, n_stride, S)
     g, streams = _info_group(cfg, blob, n_stride, 1, S)
     one = capi.AdaptiveInformationStreamsWorkspace(H.desc(cfg, n_stride, S), blob, capi.train_params(cfg, LR))
-    io = _Io(S, n_stride)
-    rows = torch.empty((S, ops.INFO_ROW), dtype=torch.float32, device=DEV)
     updates = [True, False, True, True, False, True]
     acts = [[1, 1, 0], [1, 1, 1], [1, 0, 1], [0, 0, 0], [1, 1, 1], [1, 1, 1]]
-    for k, (u, a) in enumerate(zip(updates, acts)):
-        inp = _tick_inputs(pool, S, n_stride, k, a)
-        (got,) = _group_tick(g, streams, [inp], [u])
-        io.load(*inp)
-        one.push(*io.args(), rows, update=u)
-        want = io.out() + (rows.cpu(),)
+    inputs = [H.pool_tick(pool, S, n_stride, k, a) for k, a in enumerate(acts)]
+    wants = _run_adapt(one, inputs, updates, None, True)
+    for k, (u, inp, want) in enumerate(zip(updates, inputs, wants)):
+        (got,) = H.group_tick(g, streams, [inp], [u])
         assert _bits_equal(got[1], want[1]), f"tick {k}: valid"
         for s in range(S):
             if int(want[1][s]):
                 assert _bits_equal(got[0][s], want[0][s]), f"tick {k}, stream {s}: T"
         assert _bits_equal(got[2], want[2]) and _bits_equal(got[3], want[3]), f"tick {k}: losses or info"
-        assert H.same_state(H.state(g.workspaces[0]), H.state(one)), f"tick {k}: the training state"
-    assert _status_ok(g)
+        assert H.same_state(H.state(g.workspaces[0]), want[4]), f"tick {k}: the training state"
+    assert H.group_status_ok(g)
 
 
 @pytest.mark.parametrize("world", [2, 4])
@@ -484,9 +430,9 @@ def test_adapt_group_info_ranks_are_push_adapt_group_bytes(cuda_lib, world):
     rng = np.random.default_rng(world)
     for k in range(5):
         acts = [[int(x) for x in rng.integers(0, 2, S)] if k else [1] * S for _ in range(world)]
-        inputs = [_tick_inputs(pool, S, n_stride, k, acts[r], offset=r * S) for r in range(world)]
-        got = _group_tick(gi, si, inputs, [True] * world)
-        want = _group_tick(gp, sp, inputs, [True] * world)
+        inputs = [H.pool_tick(pool, S, n_stride, k, acts[r], offset=r * S) for r in range(world)]
+        got = H.group_tick(gi, si, inputs, [True] * world)
+        want = H.group_tick(gp, sp, inputs, [True] * world)
         for r in range(world):
             assert _bits_equal(got[r][1], want[r][1]), f"tick {k} rank {r}: valid"
             for s in range(S):
@@ -496,7 +442,7 @@ def test_adapt_group_info_ranks_are_push_adapt_group_bytes(cuda_lib, world):
                     assert float(got[r][3][s].abs().max()) == 0.0
             assert _bits_equal(got[r][2], want[r][2]), f"tick {k} rank {r}: losses"
             assert H.same_state(H.state(gi.workspaces[r]), H.state(gp.workspaces[r])), f"tick {k} rank {r}: state"
-    assert _status_ok(gi) and _status_ok(gp)
+    assert H.group_status_ok(gi) and H.group_status_ok(gp)
 
 
 # ============================================================================================ Python and the example

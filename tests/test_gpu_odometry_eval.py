@@ -164,7 +164,6 @@ def test_eval_replays_from_a_graph(cuda_lib):
 
 # ================================================================================================ _push_residual
 TICKS = 8
-SENTINEL = 1234.5
 
 
 def _frame(pool, s, k):
@@ -187,12 +186,8 @@ def _pattern(S, seed):
 
 
 def _ticks(pool, S, n_stride, act):
-    out = []
-    for k in range(act.shape[0]):
-        frames = [_frame(pool, s, k) if act[k, s] else _frame(pool, s + 3, k + 2) for s in range(S)]
-        pts, counts = H.stack(frames, n_stride)         # inactive streams are staged with points: `active` masks them
-        out.append((pts, counts, torch.from_numpy(act[k].astype(np.int32)).to(DEV)))
-    return out
+    # inactive streams are staged with points: `active` masks them
+    return H.stage_ticks(act, n_stride, lambda k, s: _frame(pool, s, k) if act[k, s] else _frame(pool, s + 3, k + 2))
 
 
 def _streams_setup(S, h=16, w=180, w_raw=256, seed=30):
@@ -202,67 +197,6 @@ def _streams_setup(S, h=16, w=180, w_raw=256, seed=30):
     n_stride = max(s.shape[1] for s in pool) + 32
     act, resets = _pattern(S, seed + S)
     return cfg, blob, n_stride, _ticks(pool, S, n_stride, act), act, resets
-
-
-def _reset(st, S, streams):
-    mask = torch.zeros((S,), dtype=torch.int32, device=DEV)
-    mask[list(streams)] = 1
-    st.reset(mask)
-
-
-def _run_plain(st, ticks, resets):
-    S = st.desc.max_batch
-    T = torch.full((S, 16), SENTINEL, dtype=torch.float32, device=DEV)
-    valid = torch.full((S,), 7, dtype=torch.int32, device=DEV)
-    out = []
-    for k, (p, c, a) in enumerate(ticks):
-        if k in resets:
-            _reset(st, S, resets[k])
-        st.push(p, c, a, T, valid)
-        out.append((T.clone(), valid.clone()))
-    return out
-
-
-def _run_residual(st, ticks, resets, graph=False):
-    """-> per tick (T, valid, losses), with guard rows around `losses` checked after every tick."""
-    S = st.desc.max_batch
-    pts, counts, active = (torch.zeros_like(t) for t in ticks[0])
-    T = torch.full((S, 16), SENTINEL, dtype=torch.float32, device=DEV)
-    valid = torch.full((S,), 7, dtype=torch.int32, device=DEV)
-    guarded = torch.full((S + 2, ops.LOSS_ROW), SENTINEL, dtype=torch.float32, device=DEV)
-    losses = guarded[1:S + 1]
-    g = None
-    if graph:
-        st.push(pts, counts, active, T, valid, losses)       # all inactive: changes no stream state
-        valid.fill_(7)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            st.push(pts, counts, active, T, valid, losses)
-    out = []
-    for k, (p, c, a) in enumerate(ticks):
-        if k in resets:
-            _reset(st, S, resets[k])
-        pts.copy_(p)
-        counts.copy_(c)
-        active.copy_(a)
-        if g is not None:
-            g.replay()
-        else:
-            st.push(pts, counts, active, T, valid, losses)
-        out.append((T.clone(), valid.clone(), losses.clone()))
-        assert bool((guarded[0] == SENTINEL).all()) and bool((guarded[S + 1] == SENTINEL).all()), \
-            f"tick {k}: a write outside losses [S, LOSS_ROW]"
-    return out
-
-
-def _guarded_workspace(d):
-    nbytes, guard = capi.ResidualStreamsWorkspace.workspace_bytes(d), 4096
-    buf = torch.empty((nbytes + 2 * guard,), dtype=torch.uint8, device=DEV)
-    pattern = torch.arange(guard, device=DEV).to(torch.uint8) ^ 0xA5
-    buf[:guard] = pattern
-    buf[guard + nbytes:] = pattern
-    return buf, buf[guard:guard + nbytes], pattern
 
 
 def _reference_rows(cfg, ticks, act, resets, out, flags):
@@ -283,12 +217,14 @@ def _reference_rows(cfg, ticks, act, resets, out, flags):
             assert int(valid[s]) == int(ok), f"tick {k} stream {s}: valid={int(valid[s])}, expected {int(ok)}"
             if not act[k, s]:
                 continue
-            _, _, pg, ng = ops.project_normals(p[s:s + 1], c[s:s + 1], h, w, hf, vf, ds["neighborhood_side_length"],
+            _, _, pg, ng = ops.project_normals(p[s:s + 1].to(DEV), c[s:s + 1].to(DEV), h, w, hf, vf,
+                                               ds["neighborhood_side_length"],
                                                cfg["epsilon_range"],
                                                cfg["min_num_points_in_neighborhood_to_determine_point_class"])
             if ok:
-                rows[(k, s)] = ops.icp_dense_fwd_bwd(pg, ng, T[s:s + 1, :12].contiguous(), prev[s][0], prev[s][1], h, w,
-                                                     hf, vf, float(cfg["lambda_po2pl"]), flags)[0][0]
+                rows[(k, s)] = ops.icp_dense_fwd_bwd(pg, ng, T[s:s + 1, :12].contiguous().to(DEV), prev[s][0],
+                                                     prev[s][1], h, w, hf, vf, float(cfg["lambda_po2pl"]),
+                                                     flags)[0][0].cpu()
             prev[s] = (pg, ng)
     return rows
 
@@ -312,13 +248,11 @@ def _check_rows(out, rows, S):
 def test_residual_rows_and_transforms(cuda_lib, S, flags):
     cfg, blob, n_stride, ticks, act, resets = _streams_setup(S)
     d = H.desc(cfg, n_stride, S)
-    plain = _run_plain(capi.StreamsWorkspace(d, blob), ticks, resets)
-    buf, ws, pattern = _guarded_workspace(d)
+    plain = H.run_streams(capi.StreamsWorkspace(d, blob), ticks, resets=resets)
+    ws, intact = H.guarded_workspace(capi.ResidualStreamsWorkspace.workspace_bytes(d))
     st = capi.ResidualStreamsWorkspace(d, blob, capi.residual_params(cfg, flags), workspace=ws)
-    out = _run_residual(st, ticks, resets)
-    torch.cuda.synchronize()
-    assert torch.equal(buf[:4096], pattern) and torch.equal(buf[4096 + ws.numel():], pattern), \
-        "a write outside delora_odometry_streams_residual_workspace_bytes"
+    out = H.run_streams(st, ticks, ("losses",), resets=resets)
+    assert intact(), "a write outside delora_odometry_streams_residual_workspace_bytes"
     for k, ((tp, vp), (tr, vr, _)) in enumerate(zip(plain, out)):
         assert torch.equal(vp, vr), f"tick {k}: valid differs from _streams_push"
         assert H.same(tp, tr), f"tick {k}: T differs from _streams_push"
@@ -330,8 +264,8 @@ def test_residual_graph_replay_matches_eager(cuda_lib):
     cfg, blob, n_stride, ticks, act, resets = _streams_setup(4)
     d = H.desc(cfg, n_stride, 4)
     rp = capi.residual_params(cfg)
-    eager = _run_residual(capi.ResidualStreamsWorkspace(d, blob, rp), ticks, resets)
-    graphed = _run_residual(capi.ResidualStreamsWorkspace(d, blob, rp), ticks, resets, graph=True)
+    eager = H.run_streams(capi.ResidualStreamsWorkspace(d, blob, rp), ticks, ("losses",), resets=resets)
+    graphed = H.run_streams(capi.ResidualStreamsWorkspace(d, blob, rp), ticks, ("losses",), resets=resets, graph=True)
     for k, (e, g) in enumerate(zip(eager, graphed)):
         assert torch.equal(e[1], g[1]), f"tick {k}: valid differs"
         assert H.same(e[0], g[0]) and H.same(e[2], g[2]), f"tick {k}: the replay differs from the eager call"
@@ -340,8 +274,9 @@ def test_residual_graph_replay_matches_eager(cuda_lib):
 def test_residual_at_64x720(cuda_lib):
     cfg, blob, n_stride, ticks, act, resets = _streams_setup(2, 64, 720, 1024, seed=31)
     d = H.desc(cfg, n_stride, 2)
-    plain = _run_plain(capi.StreamsWorkspace(d, blob), ticks, resets)
-    out = _run_residual(capi.ResidualStreamsWorkspace(d, blob, capi.residual_params(cfg)), ticks, resets)
+    plain = H.run_streams(capi.StreamsWorkspace(d, blob), ticks, resets=resets)
+    out = H.run_streams(capi.ResidualStreamsWorkspace(d, blob, capi.residual_params(cfg)), ticks, ("losses",),
+                        resets=resets)
     for k, ((tp, vp), (tr, vr, _)) in enumerate(zip(plain, out)):
         assert torch.equal(vp, vr) and H.same(tp, tr), f"tick {k}: T / valid differ from _streams_push"
     _check_rows(out, _reference_rows(cfg, ticks, act, resets, out, ICP), 2)

@@ -44,19 +44,12 @@ def _pattern(S, seed):
 
 
 def _ticks(pool, S, n_stride, act, override):
-    """Host staging of every tick: points [S, 3, n_stride], counts [S], active [S]."""
-    out = []
-    for k in range(act.shape[0]):
-        pts = torch.zeros((S, 3, n_stride), dtype=torch.float32)
-        counts = torch.zeros((S,), dtype=torch.int32)
-        for s in range(S):
-            # inactive streams get another stream's scan and a real count: only `active` keeps them out
-            f = _frame(pool, s, k) if act[k, s] else _frame(pool, s + 11, k + 5)
-            pts[s, :, :f.shape[1]] = f
-            kind = override.get((k, s))
-            counts[s] = 0 if kind == "empty" else (n_stride + 1000 if kind == "over" else f.shape[1])
-        out.append((pts, counts, torch.from_numpy(act[k].astype(np.int32))))
-    return out
+    """Host staging of every tick; inactive streams get another stream's scan and a real count."""
+    def count(k, s, n):
+        kind = override.get((k, s))
+        return 0 if kind == "empty" else (n_stride + 1000 if kind == "over" else n)
+    return H.stage_ticks(act, n_stride, lambda k, s: _frame(pool, s, k) if act[k, s] else _frame(pool, s + 11, k + 5),
+                         count)
 
 
 def _push_reference(cfg, n_stride, blob, ticks, act, resets):
@@ -82,42 +75,7 @@ def _push_reference(cfg, n_stride, blob, ticks, act, resets):
     return {key: v.cpu() for key, v in want.items()}
 
 
-SENTINEL = 1234.5
-
-
-def _run_streams(st, ticks, resets, graph=False):
-    """All ticks through one streams workspace -> list of (T [S, 16] cpu, valid [S] cpu) after each tick."""
-    S = st.desc.max_batch
-    n_stride = ticks[0][0].shape[2]
-    pts = torch.zeros((S, 3, n_stride), dtype=torch.float32, device=DEV)
-    counts = torch.zeros((S,), dtype=torch.int32, device=DEV)
-    active = torch.zeros((S,), dtype=torch.int32, device=DEV)
-    T = torch.full((S, 16), SENTINEL, dtype=torch.float32, device=DEV)
-    valid = torch.full((S,), 7, dtype=torch.int32, device=DEV)
-    g = None
-    if graph:
-        st.push(pts, counts, active, T, valid)       # all inactive: changes no stream state
-        valid.fill_(7)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            st.push(pts, counts, active, T, valid)
-    out = []
-    for k, (p, c, a) in enumerate(ticks):
-        if k in resets:
-            mask = torch.zeros((S,), dtype=torch.int32, device=DEV)
-            mask[list(resets[k])] = 1
-            st.reset(mask)
-        pts.copy_(p)
-        counts.copy_(c)
-        active.copy_(a)
-        if g is not None:
-            g.replay()
-        else:
-            st.push(pts, counts, active, T, valid)
-        torch.cuda.synchronize()
-        out.append((T.cpu().clone(), valid.cpu().clone()))
-    return out
+SENTINEL = H.SENTINEL
 
 
 def _check_against_push(out, want, act, resets):
@@ -154,7 +112,7 @@ def test_rows_are_bit_identical_to_push(cuda_lib, h, w, w_raw, act_fn, S):
     act, override, resets = _pattern(S, seed=S * 31 + w)
     ticks = _ticks(pool, S, n_stride, act, override)
     want = _push_reference(cfg, n_stride, blob, ticks, act, resets)
-    out = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, S), blob), ticks, resets)
+    out = H.run_streams(StreamsWorkspace(H.desc(cfg, n_stride, S), blob), ticks, resets=resets)
     assert _check_against_push(out, want, act, resets) == len(want) > 0
 
 
@@ -167,7 +125,7 @@ def test_single_mlp_head_rows_are_bit_identical_to_push(cuda_lib, act_fn):
     act, override, resets = _pattern(3, seed=5)
     ticks = _ticks(pool, 3, n_stride, act, override)
     want = _push_reference(cfg, n_stride, blob, ticks, act, resets)
-    out = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 3), blob), ticks, resets)
+    out = H.run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 3), blob), ticks, resets=resets)
     assert _check_against_push(out, want, act, resets) == len(want) > 0
 
 
@@ -182,8 +140,8 @@ def _small_setup(S=4, w=720, seed=9):
 
 def test_graph_replay_matches_eager(cuda_lib):
     cfg, blob, n_stride, ticks, act, resets = _small_setup()
-    eager = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 4), blob), ticks, resets)
-    graphed = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 4), blob), ticks, resets, graph=True)
+    eager = H.run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 4), blob), ticks, resets=resets)
+    graphed = H.run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 4), blob), ticks, resets=resets, graph=True)
     for k, ((te, ve), (tg, vg)) in enumerate(zip(eager, graphed)):
         assert torch.equal(ve, vg), f"tick {k}: valid differs"
         assert torch.equal(H.bits(te), H.bits(tg)), f"tick {k}: graph replay differs from the eager call"
@@ -191,8 +149,8 @@ def test_graph_replay_matches_eager(cuda_lib):
 
 def test_deterministic(cuda_lib):
     cfg, blob, n_stride, ticks, act, resets = _small_setup(S=3, seed=4)
-    a = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 3), blob), ticks, resets)
-    b = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 3), blob), ticks, resets)
+    a = H.run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 3), blob), ticks, resets=resets)
+    b = H.run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 3), blob), ticks, resets=resets)
     for (ta, va), (tb, vb) in zip(a, b):
         assert torch.equal(va, vb) and torch.equal(H.bits(ta), H.bits(tb))
 
@@ -200,7 +158,7 @@ def test_deterministic(cuda_lib):
 def test_null_active_means_all_active(cuda_lib):
     cfg, blob, n_stride, ticks, _, _ = _small_setup(S=3, seed=6)
     all_on = [(p, c, torch.ones_like(a)) for p, c, a in ticks[:3]]
-    a = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 3), blob), all_on, {})
+    a = H.run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 3), blob), all_on)
     st = StreamsWorkspace(H.desc(cfg, n_stride, 3), blob)
     T = torch.full((3, 16), SENTINEL, device=DEV)
     valid = torch.zeros((3,), dtype=torch.int32, device=DEV)
@@ -219,7 +177,7 @@ def test_inactive_stream_keeps_its_cached_frame(cuda_lib):
     act = np.ones((5, 3), dtype=bool)
     act[1:4, 1] = False
     ticks = _ticks(pool, 3, n_stride, act, {})
-    out = _run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 3), blob), ticks, {})
+    out = H.run_streams(StreamsWorkspace(H.desc(cfg, n_stride, 3), blob), ticks)
     assert [int(v[1]) for _, v in out] == [0, 0, 0, 0, 1]
     want = _push_reference(cfg, n_stride, blob, [ticks[0], ticks[4]], act[[0, 4]], {})
     assert torch.equal(H.bits(out[4][0][1]), H.bits(want[(1, 1)]))
@@ -230,14 +188,9 @@ def test_inactive_stream_keeps_its_cached_frame(cuda_lib):
 def test_workspace_bounds(cuda_lib, w):
     cfg, blob, n_stride, ticks, act, resets = _small_setup(S=3, w=w, seed=8)
     d = H.desc(cfg, n_stride, 3)
-    nbytes, extra = StreamsWorkspace.workspace_bytes(d), 4096
-    ws = torch.empty((nbytes + extra,), dtype=torch.uint8, device=DEV)
-    ws[nbytes:] = torch.arange(extra, device=DEV).to(torch.uint8) ^ 0xA5
-    st = StreamsWorkspace(d, blob, workspace=ws)
-    canary = ws[nbytes:].clone()
-    _run_streams(st, ticks, resets)
-    torch.cuda.synchronize()
-    assert torch.equal(ws[nbytes:], canary), "a streams call wrote past delora_odometry_streams_workspace_bytes"
+    ws, intact = H.guarded_workspace(StreamsWorkspace.workspace_bytes(d))
+    H.run_streams(StreamsWorkspace(d, blob, workspace=ws), ticks, resets=resets)
+    assert intact(), "a streams call wrote outside delora_odometry_streams_workspace_bytes"
 
 
 @pytest.mark.parametrize("use_graph", [True, False])

@@ -23,7 +23,6 @@ from delora_b200.deploy import capi
 
 pytestmark = pytest.mark.gpu
 DEV = H.DEV
-SENTINEL = 1234.5
 ICP = ops.LOSS_PO2PL | ops.LOSS_PL2PL
 LR = 1e-4
 
@@ -44,55 +43,13 @@ def _adapt(cfg, blob, n_stride, S, w_pre, normalized=False, lr=LR, beta1=0.9):
     return capi.AdaptiveStreamsWorkspace(H.desc(cfg, n_stride, S, w_pre), blob, _params(cfg, normalized, lr, beta1))
 
 
-class _Io:
-    """The device arguments of one workspace's ticks."""
-
-    def __init__(self, S, n_stride):
-        self.pts = torch.zeros((S, 3, n_stride), dtype=torch.float32, device=DEV)
-        self.counts = torch.zeros((S,), dtype=torch.int32, device=DEV)
-        self.active = torch.zeros((S,), dtype=torch.int32, device=DEV)
-        self.T = torch.full((S, 16), SENTINEL, dtype=torch.float32, device=DEV)
-        self.valid = torch.full((S,), 7, dtype=torch.int32, device=DEV)
-        self.losses = torch.full((S, ops.LOSS_ROW), SENTINEL, dtype=torch.float32, device=DEV)
-        self.mask = torch.zeros((S,), dtype=torch.int32, device=DEV)
-
-    def load(self, p, c, a):
-        self.pts.copy_(p)
-        self.counts.copy_(c)
-        self.active.copy_(a)
-
-    def args(self):
-        return self.pts, self.counts, self.active, self.T, self.valid, self.losses
-
-    def out(self):
-        torch.cuda.synchronize()
-        return self.T.cpu().clone(), self.valid.cpu().clone(), self.losses.cpu().clone()
-
-
-def _run(ws, ticks, updates, resets=None):
+def _run(ws, ticks, updates, resets=None, hook=None):
     """Every tick (points [S, 3, n], counts [S], active [S]) through one workspace, eagerly -> [(T, valid, losses)]."""
-    S = ws.desc.max_batch
-    io = _Io(S, ticks[0][0].shape[2])
-    out = []
-    for k, (p, c, a) in enumerate(ticks):
-        if resets and k in resets:
-            io.mask.zero_()
-            io.mask[resets[k]] = 1
-            ws.reset(io.mask)
-        io.load(p, c, a)
-        ws.push(*io.args(), update=updates[k])
-        out.append(io.out())
-    return out
+    return H.run_streams(ws, ticks, ("losses",), resets=resets, updates=updates, hook=hook)
 
 
-def _single_ticks(frames, n_stride, empty=()):
-    out = []
-    for k, f in enumerate(frames):
-        p = torch.zeros((1, 3, n_stride), dtype=torch.float32)
-        p[0, :, :f.shape[1]] = f
-        out.append((p, torch.tensor([0 if k in empty else f.shape[1]], dtype=torch.int32),
-                    torch.ones((1,), dtype=torch.int32)))
-    return out
+def _single_ticks(frames, n_stride):
+    return H.stage_ticks(np.ones((len(frames), 1), dtype=bool), n_stride, lambda k, s: frames[k])
 
 
 CASES = [(16, 180, 512, 0, False), (16, 180, 512, 360, False), (16, 180, 512, 360, True),
@@ -109,11 +66,8 @@ def test_one_stream_is_the_training_step(cuda_lib, h, w, w_raw, w_pre, normalize
     blob = H.blob(H.model(cfg, 11, near_identity=True), cfg)
     ws = _adapt(cfg, blob, n_stride, 1, w_pre, normalized)
     tr = capi.TrainingWorkspace(H.desc(cfg, n_stride, 1, w_pre), blob, _params(cfg, normalized))
-    io = _Io(1, n_stride)
-    for k, (p, c, a) in enumerate(_single_ticks(frames, n_stride)):
-        io.load(p, c, a)
-        ws.push(*io.args(), update=True)
-        T, valid, losses = io.out()
+    out = _run(ws, _single_ticks(frames, n_stride), [True] * K, hook=H.state)
+    for k, (T, valid, losses, state) in enumerate(out):
         assert int(valid[0]) == (1 if k else 0), (k, int(valid[0]))
         if k:
             pts, counts = H.stack([frames[k - 1], frames[k]], n_stride)
@@ -123,31 +77,8 @@ def test_one_stream_is_the_training_step(cuda_lib, h, w, w_raw, w_pre, normalize
             assert H.same(losses[0], l_ref[0].cpu()), f"tick {k}: {losses[0].tolist()} != {l_ref[0].tolist()}"
         else:
             assert float(losses[0].abs().max()) == 0.0
-        assert H.same_state(H.state(ws), H.state(tr)), f"tick {k}: the training state differs from _train_step's"
+        assert H.same_state(state, H.state(tr)), f"tick {k}: the training state differs from _train_step's"
     assert int(H.state(ws)[3][0]) == K - 1
-
-
-def _pattern(S, ticks=7):
-    act = np.ones((ticks, S), dtype=bool)
-    act[1, S - 1] = False                   # an inactive stream
-    act[4, :] = False                       # an idle tick
-    if ticks > 6:
-        act[6, 0] = False
-    return act, {(2, 1 % S)}, {3: [0]}
-
-
-def _ticks(pool, S, n_stride, act, empty):
-    out = []
-    for k in range(act.shape[0]):
-        pts = torch.zeros((S, 3, n_stride), dtype=torch.float32)
-        counts = torch.zeros((S,), dtype=torch.int32)
-        for s in range(S):
-            # an inactive stream is staged with real points and count: only the mask keeps it out
-            f = pool[(3 * s + k) % len(pool)] if act[k, s] else pool[(3 * s + k + 5) % len(pool)]
-            pts[s, :, :f.shape[1]] = f
-            counts[s] = 0 if (k, s) in empty else f.shape[1]
-        out.append((pts, counts, torch.from_numpy(act[k].astype(np.int32))))
-    return out
 
 
 @pytest.mark.parametrize("w_pre,normalized", [(0, False), (360, False), (360, True)],
@@ -157,8 +88,8 @@ def test_rows_are_independent(cuda_lib, w_pre, normalized):
     cfg = _cfg(h, w, w_pre, normalized)
     pool = H.frames(h, w_raw, 8)
     n_stride = max(f.shape[1] for f in pool)
-    act, empty, resets = _pattern(S)
-    ticks = _ticks(pool, S, n_stride, act, empty)
+    act, empty, resets = H.recipe_pattern(S)
+    ticks = H.recipe_ticks(pool, S, n_stride, act, empty)
     blob = H.blob(H.model(cfg, 5, near_identity=True), cfg)
     updates = [False] * len(ticks)
     out = _run(_adapt(cfg, blob, n_stride, S, w_pre, normalized), ticks, updates, resets)
@@ -219,7 +150,7 @@ def test_no_pair_no_update(cuda_lib, w_pre):
     n_stride = max(f.shape[1] for f in pool)
     blob = H.blob(H.model(cfg, 3, near_identity=True), cfg)
     act = np.ones((3, S), dtype=bool)
-    ticks = _ticks(pool, S, n_stride, act, set())
+    ticks = H.recipe_ticks(pool, S, n_stride, act, set())
     ws = _adapt(cfg, blob, n_stride, S, w_pre)
     before = H.state(ws)
     out = _run(ws, ticks[:1], [True])
@@ -238,38 +169,15 @@ def test_graphs_replay_the_eager_calls(cuda_lib):
     cfg = _cfg(h, w, w_pre)
     pool = H.frames(h, w_raw, 8)
     n_stride = max(f.shape[1] for f in pool)
-    act, empty, _ = _pattern(S, 6)
-    ticks = _ticks(pool, S, n_stride, act, empty)
+    act, empty, _ = H.recipe_pattern(S, 6)
+    ticks = H.recipe_ticks(pool, S, n_stride, act, empty)
     updates = [False, True, False, True, True, False]
     blob = H.blob(H.model(cfg, 8, near_identity=True), cfg)
-
-    def warm(ws, io):
-        io.active.zero_()                    # all inactive: no stream state or weight changes
-        for u in (False, True):
-            ws.push(*io.args(), update=u)
-        torch.cuda.synchronize()
-
-    eager_ws = _adapt(cfg, blob, n_stride, S, w_pre)
-    io = _Io(S, n_stride)
-    warm(eager_ws, io)
-    eager = []
-    for k, (p, c, a) in enumerate(ticks):
-        io.load(p, c, a)
-        eager_ws.push(*io.args(), update=updates[k])
-        eager.append(io.out())
-    g_ws = _adapt(cfg, blob, n_stride, S, w_pre)
-    gio = _Io(S, n_stride)
-    warm(g_ws, gio)
-    graphs = {}
-    for u in (False, True):
-        graphs[u] = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graphs[u]):
-            g_ws.push(*gio.args(), update=u)
-    for k, (p, c, a) in enumerate(ticks):
-        gio.load(p, c, a)
-        graphs[updates[k]].replay()
-        got = gio.out()
-        for i, (x, y) in enumerate(zip(eager[k], got)):
+    eager_ws, g_ws = _adapt(cfg, blob, n_stride, S, w_pre), _adapt(cfg, blob, n_stride, S, w_pre)
+    eager = _run(eager_ws, ticks, updates)
+    graphed = H.run_streams(g_ws, ticks, ("losses",), updates=updates, graph=True)
+    for k, (e, g) in enumerate(zip(eager, graphed)):
+        for i, (x, y) in enumerate(zip(e, g)):
             assert H.same(x, y), f"tick {k}: output {i} of the replay differs from the eager call"
     assert H.same_state(H.state(eager_ws), H.state(g_ws))
     assert int(H.state(g_ws)[3][0]) == 2          # ticks 1 and 3 update; tick 4 has no stream, so no pair
@@ -280,7 +188,7 @@ def test_state_round_trip_leaves_the_streams_and_resumes(cuda_lib):
     cfg = _cfg(h, w, w_pre)
     pool = H.frames(h, w_raw, 8)
     n_stride = max(f.shape[1] for f in pool)
-    ticks = _ticks(pool, S, n_stride, np.ones((6, S), dtype=bool), set())
+    ticks = H.recipe_ticks(pool, S, n_stride, np.ones((6, S), dtype=bool), set())
     blob = H.blob(H.model(cfg, 4, near_identity=True), cfg)
     a = _adapt(cfg, blob, n_stride, S, w_pre)
     _run(a, ticks[:3], [True] * 3)
@@ -309,9 +217,9 @@ def test_python_class(cuda_lib):
     cfg = _cfg(h, w, w_pre)
     pool = H.frames(h, w_raw, 8)
     n_stride = max(f.shape[1] for f in pool)
-    act, _, _ = _pattern(S, 5)
+    act, _, _ = H.recipe_pattern(S, 5)
     act[4, :] = True
-    ticks = _ticks(pool, S, n_stride, act, set())
+    ticks = H.recipe_ticks(pool, S, n_stride, act, set())
     model = H.model(cfg, 9, near_identity=True)
     cls = AdaptiveOdometryStreams(model, cfg, "kitti", S, n_stride, LR, preprocessing_normals=True)
     ws = _adapt(cfg, H.blob(model, cfg), n_stride, S, w_pre)

@@ -89,28 +89,16 @@ def _tick(pool, n_stride, k, active, geoms=GEOMS):
     return pts, counts, torch.tensor(active, dtype=torch.int32, device=DEV)
 
 
-def _outs(S):
-    return (torch.full((S, 16), 1234.5, dtype=torch.float32, device=DEV),
-            torch.full((S,), 7, dtype=torch.int32, device=DEV),
-            torch.full((S, ops.LOSS_ROW), 1234.5, dtype=torch.float32, device=DEV))
-
-
 def _push_multi(ws, tick, update):
-    pts, counts, active = tick
-    out = _outs(ws.n_streams)
-    ws.push(pts, counts, active, *out, update=update)
-    torch.cuda.synchronize()
-    return tuple(t.cpu() for t in out)
+    out = H.Outputs(ws.n_streams, ("losses",))
+    ws.push(*tick, *out.tensors, update=update)
+    return out.snapshot()
 
 
 def _push_single(ws, tick, g, update, geoms=GEOMS):
     pts, counts, active = tick
     r = sum(S for *_, S in geoms[:g])
-    S = geoms[g][3]
-    out = _outs(S)
-    ws.push(pts[g], counts[g], active[r:r + S].contiguous(), *out, update=update)
-    torch.cuda.synchronize()
-    return tuple(t.cpu() for t in out)
+    return H.run_streams(ws, [(pts[g], counts[g], active[r:r + geoms[g][3]])], ("losses",), updates=[update])[0]
 
 
 def _same_rows(k, got, want, r0, geoms=GEOMS):
@@ -261,7 +249,7 @@ def test_determinism_and_graphs(setup):
     def bufs():
         return ([torch.zeros((g[3], 3, n_stride), dtype=torch.float32, device=DEV) for g in GEOMS],
                 [torch.zeros((g[3],), dtype=torch.int32, device=DEV) for g in GEOMS],
-                torch.zeros((S,), dtype=torch.int32, device=DEV)) + _outs(S)
+                torch.zeros((S,), dtype=torch.int32, device=DEV)) + H.Outputs(S, ("losses",)).tensors
 
     def load(b, k):
         pts, counts, active = _tick(pool, n_stride, k, acts[k])

@@ -52,7 +52,7 @@ def _kernels_loaded(cuda_lib):
     kernel's first launch waits for the device's running kernels: a first load behind a rank that spins in the count
     exchange would hold its peers until the meet's timeout."""
     cfg, blob, pool, n_stride = _setup()
-    _single_tick(_single(cfg, blob, n_stride, 2), *_tick_inputs(pool, 2, n_stride, 0, [1, 1]), True)
+    _single_tick(_single(cfg, blob, n_stride, 2), *H.pool_tick(pool, 2, n_stride, 0, [1, 1]), True)
 
 
 def _group(cfg, blob, n_stride, world, S=2, lr=LR, beta1=0.9):
@@ -65,40 +65,8 @@ def _single(cfg, blob, n_stride, S, lr=LR, beta1=0.9):
     return capi.AdaptiveStreamsWorkspace(H.desc(cfg, n_stride, S), blob, _params(cfg, lr, beta1))
 
 
-def _tick_inputs(pool, S, n_stride, k, active, offset=0):
-    """Tick k of S streams: stream s serves pool[(3 * (s + offset) + k) % len(pool)] where active[s]."""
-    pts = torch.zeros((S, 3, n_stride), dtype=torch.float32)
-    counts = torch.zeros((S,), dtype=torch.int32)
-    for s in range(S):
-        f = pool[(3 * (s + offset) + k) % len(pool)]
-        pts[s, :, :f.shape[1]] = f
-        counts[s] = f.shape[1]
-    return pts.to(DEV), counts.to(DEV), torch.tensor(active, dtype=torch.int32, device=DEV)
-
-
-def _group_tick(g, streams, inputs, updates):
-    """Every rank's tick on its own stream, all enqueued before one synchronisation -> [(T, valid, losses)] per rank."""
-    torch.cuda.synchronize()
-    outs = []
-    for r, (pts, counts, active) in enumerate(inputs):
-        with torch.cuda.stream(streams[r]):
-            outs.append(g.push(r, pts, counts, active, update=updates[r]))
-    torch.cuda.synchronize()
-    return [tuple(t.cpu() for t in o) for o in outs]
-
-
 def _single_tick(ws, pts, counts, active, update):
-    S = ws.desc.max_batch
-    T = torch.empty((S, 16), dtype=torch.float32, device=DEV)
-    valid = torch.empty((S,), dtype=torch.int32, device=DEV)
-    losses = torch.empty((S, ops.LOSS_ROW), dtype=torch.float32, device=DEV)
-    ws.push(pts, counts, active, T, valid, losses, update=update)
-    torch.cuda.synchronize()
-    return T.cpu(), valid.cpu(), losses.cpu()
-
-
-def _status_ok(g):
-    return all(int(s.item()) == 0 for s in g.status)
+    return H.run_streams(ws, [(pts, counts, active)], ("losses",), updates=[update])[0]
 
 
 def test_single_rank_group_is_push_adapt(cuda_lib):
@@ -109,8 +77,8 @@ def test_single_rank_group_is_push_adapt(cuda_lib):
     updates = [True, False, True, True, False, True]
     acts = [[1, 1, 0], [1, 1, 1], [1, 0, 1], [0, 0, 0], [1, 1, 1], [1, 1, 1]]
     for k, (u, a) in enumerate(zip(updates, acts)):
-        inp = _tick_inputs(pool, S, n_stride, k, a)
-        (got,) = _group_tick(g, streams, [inp], [u])
+        inp = H.pool_tick(pool, S, n_stride, k, a)
+        (got,) = H.group_tick(g, streams, [inp], [u])
         want = _single_tick(plain, *inp, u)
         valid = want[1]
         assert H.same(got[1], valid), f"tick {k}: valid"
@@ -120,7 +88,7 @@ def test_single_rank_group_is_push_adapt(cuda_lib):
         assert H.same(got[2], want[2]), f"tick {k}: losses"
         assert H.same_state(H.state(g.workspaces[0]), H.state(plain)), f"tick {k}: the training state"
     assert int(H.state(plain)[3][0]) >= 2
-    assert _status_ok(g)
+    assert H.group_status_ok(g)
 
 
 def _check_rows(k, outs, single, world, S):
@@ -155,22 +123,22 @@ def _run_against_single(cfg, blob, pool, n_stride, world, S, extra_serve=None):
     for k in range(4):
         if k == 2 and extra_serve:                  # serve-only ticks run no collective: rank by rank
             for r in range(world):
-                inp = _tick_inputs(pool, S, n_stride, 1, [1] * S, r * S)
+                inp = H.pool_tick(pool, S, n_stride, 1, [1] * S, r * S)
                 torch.cuda.synchronize()
                 for _ in range(extra_serve[r]):
                     with torch.cuda.stream(streams[r]):
                         g.push(r, *inp, update=False)
             torch.cuda.synchronize()
-        inputs = [_tick_inputs(pool, S, n_stride, k, acts[k], r * S) for r in range(world)]
+        inputs = [H.pool_tick(pool, S, n_stride, k, acts[k], r * S) for r in range(world)]
         update = k > 0
-        outs = _group_tick(g, streams, inputs, [update] * world)
-        ref = _single_tick(single, *_tick_inputs(pool, S * world, n_stride, k, acts[k] * world), update)
+        outs = H.group_tick(g, streams, inputs, [update] * world)
+        ref = _single_tick(single, *H.pool_tick(pool, S * world, n_stride, k, acts[k] * world), update)
         _check_rows(k, outs, ref, world, S)
         state = _check_ranks_agree(k, g)
         if update:
             assert int(state[3][0]) == k
             _check_mean(k, cfg, state[1], H.state(single)[1])
-    assert _status_ok(g)
+    assert H.group_status_ok(g)
     return [H.state(w) for w in g.workspaces]
 
 
@@ -195,8 +163,8 @@ def test_the_mean_is_over_pairs_not_ranks(cuda_lib):
     single = _single(cfg, blob, n_stride, S, lr=0.0, beta1=0.0)
     # tick 0: rank 0's first frames, rank 1 idle; tick 1: rank 0's two pairs, rank 1 on first frames only
     for k, (a0, a1) in enumerate(([[1, 1], [0, 0]], [[1, 1], [1, 1]])):
-        inputs = [_tick_inputs(pool, S, n_stride, k, a0), _tick_inputs(pool, S, n_stride, k, a1, S)]
-        outs = _group_tick(g, streams, inputs, [True, True])
+        inputs = [H.pool_tick(pool, S, n_stride, k, a0), H.pool_tick(pool, S, n_stride, k, a1, S)]
+        outs = H.group_tick(g, streams, inputs, [True, True])
         ref = _single_tick(single, *inputs[0], True)
         assert outs[0][1].tolist() == ref[1].tolist() == ([0, 0] if k == 0 else [1, 1])
         assert outs[1][1].tolist() == [0, 0]
@@ -207,7 +175,7 @@ def test_the_mean_is_over_pairs_not_ranks(cuda_lib):
     # the mean of the ranks' means would be half of it
     tail, trunk = H.grad_spread(H.grad_dict(state[1], cfg), H.grad_dict(want * 0.5, cfg))
     assert tail > 0.5 and trunk > 0.5, (tail, trunk)
-    assert _status_ok(g)
+    assert H.group_status_ok(g)
 
 
 def test_no_pair_on_any_rank_no_update(cuda_lib):
@@ -216,22 +184,22 @@ def test_no_pair_on_any_rank_no_update(cuda_lib):
     empty, e_streams = _group(cfg, blob, n_stride, world, S)      # takes the empty update tick
     plain, p_streams = _group(cfg, blob, n_stride, world, S)      # serves that tick only
     before = [H.state(w) for w in empty.workspaces]
-    inputs = [_tick_inputs(pool, S, n_stride, 0, [1, 1], r * S) for r in range(world)]
-    outs = _group_tick(empty, e_streams, inputs, [True] * world)
+    inputs = [H.pool_tick(pool, S, n_stride, 0, [1, 1], r * S) for r in range(world)]
+    outs = H.group_tick(empty, e_streams, inputs, [True] * world)
     assert all(int(o[1].sum()) == 0 for o in outs)
     for r in range(world):
         assert H.same_state(H.state(empty.workspaces[r]), before[r]), f"rank {r}: an update without a pair"
-    _group_tick(plain, p_streams, inputs, [False] * world)
+    H.group_tick(plain, p_streams, inputs, [False] * world)
     for k in (1, 2):
-        inputs = [_tick_inputs(pool, S, n_stride, k, [1, 1], r * S) for r in range(world)]
-        got = _group_tick(empty, e_streams, inputs, [True] * world)
-        want = _group_tick(plain, p_streams, inputs, [True] * world)
+        inputs = [H.pool_tick(pool, S, n_stride, k, [1, 1], r * S) for r in range(world)]
+        got = H.group_tick(empty, e_streams, inputs, [True] * world)
+        want = H.group_tick(plain, p_streams, inputs, [True] * world)
         for r in range(world):
             for i, (x, y) in enumerate(zip(got[r], want[r])):
                 assert H.same(x, y), f"tick {k}, rank {r}: output {i}"
             assert H.same_state(H.state(empty.workspaces[r]), H.state(plain.workspaces[r])), f"tick {k}, rank {r}"
     assert int(H.state(empty.workspaces[0])[3][0]) == 2
-    assert _status_ok(empty) and _status_ok(plain)
+    assert H.group_status_ok(empty) and H.group_status_ok(plain)
 
 
 def test_graph_replay_of_the_group_tick_matches_eager(cuda_lib):
@@ -242,7 +210,7 @@ def test_graph_replay_of_the_group_tick_matches_eager(cuda_lib):
     def warm(g, streams, bufs):
         for b in bufs:                              # all inactive: no stream state or weight changes
             b[2].zero_()
-        _group_tick(g, streams, [b[:3] for b in bufs], [True] * world)
+        H.group_tick(g, streams, [b[:3] for b in bufs], [True] * world)
 
     def buffers():
         return [[torch.zeros((S, 3, n_stride), dtype=torch.float32, device=DEV),
@@ -253,7 +221,7 @@ def test_graph_replay_of_the_group_tick_matches_eager(cuda_lib):
 
     def load(bufs, k):
         for r in range(world):
-            for dst, src in zip(bufs[r][:3], _tick_inputs(pool, S, n_stride, k, acts[k], r * S)):
+            for dst, src in zip(bufs[r][:3], H.pool_tick(pool, S, n_stride, k, acts[k], r * S)):
                 dst.copy_(src)
 
     eager, e_streams = _group(cfg, blob, n_stride, world, S)
@@ -262,7 +230,7 @@ def test_graph_replay_of_the_group_tick_matches_eager(cuda_lib):
     want = []
     for k in range(ticks):
         load(ebufs, k)
-        want.append(_group_tick(eager, e_streams, [b[:3] for b in ebufs], [True] * world))
+        want.append(H.group_tick(eager, e_streams, [b[:3] for b in ebufs], [True] * world))
     graphed, streams = _group(cfg, blob, n_stride, world, S)
     bufs = buffers()
     warm(graphed, streams, bufs)
@@ -287,11 +255,11 @@ def test_graph_replay_of_the_group_tick_matches_eager(cuda_lib):
                 if int(valid[s]):
                     assert H.same(bufs[r][3][s].cpu(), want[k][r][0][s]), f"tick {k}, rank {r}: T"
             assert H.same(bufs[r][5].cpu(), want[k][r][2]), f"tick {k}, rank {r}: losses"
-        assert _status_ok(graphed), f"tick {k}: a collective timed out"
+        assert H.group_status_ok(graphed), f"tick {k}: a collective timed out"
     for r in range(world):
         assert H.same_state(H.state(graphed.workspaces[r]), H.state(eager.workspaces[r])), f"rank {r}: the state"
     assert int(H.state(graphed.workspaces[0])[3][0]) == ticks - 1         # tick 0 has first frames only
-    assert _status_ok(eager)
+    assert H.group_status_ok(eager)
 
 
 def test_example_with_one_gpu_writes_the_same_file(cuda_lib, tmp_path):

@@ -20,7 +20,7 @@ from helpers import ROOT
 pytestmark = pytest.mark.gpu
 DEV = H.DEV
 TICKS = 9
-SENTINEL = 1234.5
+SENTINEL = H.SENTINEL
 
 
 def _cfg(h, w, act="tanh", single=False, **kw):
@@ -59,19 +59,12 @@ def _pattern(S, seed, empty=False):
 
 
 def _ticks(pool, S, n_stride, act, override):
-    """Host staging of every tick: points [S, 3, n_stride], counts [S], active [S]."""
-    out = []
-    for k in range(act.shape[0]):
-        pts = torch.zeros((S, 3, n_stride), dtype=torch.float32)
-        counts = torch.zeros((S,), dtype=torch.int32)
-        for s in range(S):
-            # inactive streams get another stream's scan and a real count: only `active` keeps them out
-            f = _frame(pool, s, k) if act[k, s] else _frame(pool, s + 11, k + 5)
-            pts[s, :, :f.shape[1]] = f
-            kind = override.get((k, s))
-            counts[s] = 0 if kind == "empty" else (n_stride + 1000 if kind == "over" else f.shape[1])
-        out.append((pts, counts, torch.from_numpy(act[k].astype(np.int32))))
-    return out
+    """Host staging of every tick; inactive streams get another stream's scan and a real count."""
+    def count(k, s, n):
+        kind = override.get((k, s))
+        return 0 if kind == "empty" else (n_stride + 1000 if kind == "over" else n)
+    return H.stage_ticks(act, n_stride, lambda k, s: _frame(pool, s, k) if act[k, s] else _frame(pool, s + 11, k + 5),
+                         count)
 
 
 def _pairs_reference(cfg, n_stride, blobs, ticks, act, resets):
@@ -94,46 +87,6 @@ def _pairs_reference(cfg, n_stride, blobs, ticks, act, resets):
             prev = (pts[s], counts[s])
     torch.cuda.synchronize()
     return {key: (t.cpu(), f.cpu()) for key, (t, f) in want.items()}
-
-
-def _run_streams(st, ticks, resets, graph=False, loads=None):
-    """All ticks through one normalised streams workspace -> list of (T [S, 16], valid [S], factor [S]) on the host
-    after each tick.  loads: {tick: blob} loaded with delora_odometry_streams_load_weights before that tick."""
-    S = st.desc.max_batch
-    n_stride = ticks[0][0].shape[2]
-    pts = torch.zeros((S, 3, n_stride), dtype=torch.float32, device=DEV)
-    counts = torch.zeros((S,), dtype=torch.int32, device=DEV)
-    active = torch.zeros((S,), dtype=torch.int32, device=DEV)
-    T = torch.full((S, 16), SENTINEL, dtype=torch.float32, device=DEV)
-    valid = torch.full((S,), 7, dtype=torch.int32, device=DEV)
-    factor = torch.full((S,), SENTINEL, dtype=torch.float32, device=DEV)
-    g = None
-    if graph:
-        st.push(pts, counts, active, T, valid, factor)     # all inactive: changes no stream state
-        valid.fill_(7)
-        factor.fill_(SENTINEL)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            st.push(pts, counts, active, T, valid, factor)
-    out = []
-    for k, (p, c, a) in enumerate(ticks):
-        if loads and k in loads:
-            st.load_weights(loads[k])
-        if k in resets:
-            mask = torch.zeros((S,), dtype=torch.int32, device=DEV)
-            mask[list(resets[k])] = 1
-            st.reset(mask)
-        pts.copy_(p)
-        counts.copy_(c)
-        active.copy_(a)
-        if g is not None:
-            g.replay()
-        else:
-            st.push(pts, counts, active, T, valid, factor)
-        torch.cuda.synchronize()
-        out.append((T.cpu().clone(), valid.cpu().clone(), factor.cpu().clone()))
-    return out
 
 
 def _check(out, want, act, resets, skip=()):
@@ -179,7 +132,7 @@ CASES = [(16, 180, 1024, "tanh", False), (16, 259, 1024, "relu", True)]    # W e
 def test_rows_are_bit_identical_to_pairs_normalized(cuda_lib, h, w, w_raw, act_fn, single, S):
     cfg, blob, n_stride, ticks, act, resets = _setup(h, w, w_raw, S, act_fn, single, seed=S * 31 + w)
     want = _pairs_reference(cfg, n_stride, {0: blob}, ticks, act, resets)
-    out = _run_streams(NormalizedStreamsWorkspace(H.desc(cfg, n_stride, S), blob), ticks, resets)
+    out = H.run_streams(NormalizedStreamsWorkspace(H.desc(cfg, n_stride, S), blob), ticks, ("factor",), resets=resets)
     assert _check(out, want, act, resets) == len(want) > 0
     # the factors differ between streams and ticks: a row with another pair's factor could not have matched
     fs = [float(f[0]) for _, f in want.values()]
@@ -189,7 +142,7 @@ def test_rows_are_bit_identical_to_pairs_normalized(cuda_lib, h, w, w_raw, act_f
 def test_rows_are_bit_identical_at_64x720(cuda_lib):
     cfg, blob, n_stride, ticks, act, resets = _setup(64, 720, 1024, 4, seed=3)
     want = _pairs_reference(cfg, n_stride, {0: blob}, ticks, act, resets)
-    out = _run_streams(NormalizedStreamsWorkspace(H.desc(cfg, n_stride, 4), blob), ticks, resets)
+    out = H.run_streams(NormalizedStreamsWorkspace(H.desc(cfg, n_stride, 4), blob), ticks, ("factor",), resets=resets)
     assert _check(out, want, act, resets) == len(want) > 0
 
 
@@ -199,7 +152,7 @@ def test_an_empty_frame_touches_only_its_own_pairs(cuda_lib):
     S = 3
     cfg, blob, n_stride, ticks, act, resets = _setup(16, 180, 1024, S, seed=12, empty=True)
     want = _pairs_reference(cfg, n_stride, {0: blob}, ticks, act, resets)
-    out = _run_streams(NormalizedStreamsWorkspace(H.desc(cfg, n_stride, S), blob), ticks, resets)
+    out = H.run_streams(NormalizedStreamsWorkspace(H.desc(cfg, n_stride, S), blob), ticks, ("factor",), resets=resets)
     # the pairs that hold the empty frame: tick 3 (this frame) and stream 1's next active tick (previous frame)
     nxt = next(k for k in range(4, TICKS) if act[k, 1])
     bad = {(k, 1) for k in (3, nxt) if (k, 1) in want}
@@ -214,8 +167,8 @@ def test_an_empty_frame_touches_only_its_own_pairs(cuda_lib):
 def test_graph_replay_matches_the_direct_calls(cuda_lib):
     cfg, blob, n_stride, ticks, act, resets = _setup(16, 259, 1024, 4, seed=9)
     d = H.desc(cfg, n_stride, 4)
-    eager = _run_streams(NormalizedStreamsWorkspace(d, blob), ticks, resets)
-    graphed = _run_streams(NormalizedStreamsWorkspace(d, blob), ticks, resets, graph=True)
+    eager = H.run_streams(NormalizedStreamsWorkspace(d, blob), ticks, ("factor",), resets=resets)
+    graphed = H.run_streams(NormalizedStreamsWorkspace(d, blob), ticks, ("factor",), resets=resets, graph=True)
     for k, (e, g) in enumerate(zip(eager, graphed)):
         assert torch.equal(e[1], g[1]), f"tick {k}: valid differs"
         assert torch.equal(H.bits(e[0]), H.bits(g[0])), f"tick {k}: T differs under graph replay"
@@ -229,7 +182,8 @@ def test_load_weights_and_reset_act_as_on_the_streams_workspace(cuda_lib):
     cfg, blob, n_stride, ticks, act, resets = _setup(16, 180, 1024, S, seed=21)
     blob2 = H.blob(H.model(cfg, 7).eval(), cfg)
     want = _pairs_reference(cfg, n_stride, {0: blob, 5: blob2}, ticks, act, resets)
-    out = _run_streams(NormalizedStreamsWorkspace(H.desc(cfg, n_stride, S), blob), ticks, resets, loads={5: blob2})
+    out = H.run_streams(NormalizedStreamsWorkspace(H.desc(cfg, n_stride, S), blob), ticks, ("factor",), resets=resets,
+                          loads={5: blob2})
     assert _check(out, want, act, resets) == len(want) > 0
     assert any(k >= 5 for k, _ in want), "no tick ran on the second blob"
 
@@ -237,14 +191,9 @@ def test_load_weights_and_reset_act_as_on_the_streams_workspace(cuda_lib):
 def test_workspace_bounds(cuda_lib):
     cfg, blob, n_stride, ticks, act, resets = _setup(16, 259, 1024, 3, seed=8)
     d = H.desc(cfg, n_stride, 3)
-    nbytes, extra = NormalizedStreamsWorkspace.workspace_bytes(d), 4096
-    ws = torch.empty((nbytes + extra,), dtype=torch.uint8, device=DEV)
-    ws[nbytes:] = torch.arange(extra, device=DEV).to(torch.uint8) ^ 0xA5
-    st = NormalizedStreamsWorkspace(d, blob, workspace=ws)
-    canary = ws[nbytes:].clone()
-    _run_streams(st, ticks, resets)
-    torch.cuda.synchronize()
-    assert torch.equal(ws[nbytes:], canary), "a call wrote past delora_odometry_streams_normalized_workspace_bytes"
+    ws, intact = H.guarded_workspace(NormalizedStreamsWorkspace.workspace_bytes(d))
+    H.run_streams(NormalizedStreamsWorkspace(d, blob, workspace=ws), ticks, ("factor",), resets=resets)
+    assert intact(), "a call wrote outside delora_odometry_streams_normalized_workspace_bytes"
 
 
 @pytest.mark.parametrize("use_graph", [True, False])

@@ -24,8 +24,6 @@ from delora_b200.deploy import capi
 
 pytestmark = pytest.mark.gpu
 DEV = H.DEV
-SENTINEL = 1234.5
-GUARD = 4096
 ICP = ops.LOSS_PO2PL | ops.LOSS_PL2PL
 SIZES = [(16, 180, 512, 360), (64, 720, 2048, 2250)]                   # H, W, w_raw, w_pre
 
@@ -41,94 +39,18 @@ def _flags(normalized, flags=ICP):
     return flags | (ops.TRAIN_NORMALIZATION_SCALING if normalized else 0)
 
 
-def _pattern(S):
-    """active [ticks, S], the (tick, stream) with an empty frame, resets {tick: [streams]} applied before the tick."""
-    act = np.ones((7, S), dtype=bool)
-    act[1, S - 1] = False                   # an inactive stream
-    act[4, :] = False                       # an idle tick
-    act[6, 0] = False
-    return act, {(2, 1 % S)}, {3: [0]}
-
-
-def _ticks(pool, S, n_stride, act, empty):
-    out = []
-    for k in range(act.shape[0]):
-        pts = torch.zeros((S, 3, n_stride), dtype=torch.float32)
-        counts = torch.zeros((S,), dtype=torch.int32)
-        for s in range(S):
-            f = pool[(3 * s + k) % len(pool)] if act[k, s] else pool[(3 * s + k + 5) % len(pool)]
-            pts[s, :, :f.shape[1]] = f
-            counts[s] = 0 if (k, s) in empty else f.shape[1]
-        out.append((pts, counts, torch.from_numpy(act[k].astype(np.int32))))
-    return out
-
-
 def _setup(h, w, w_raw, w_pre, normalized, S, seed=3):
     cfg = _cfg(h, w, w_pre, normalized)
     pool = H.frames(h, w_raw, 8)
     n_stride = max(f.shape[1] for f in pool)
-    act, empty, resets = _pattern(S)
+    act, empty, resets = H.recipe_pattern(S)
     blob = H.blob(H.model(cfg, seed, near_identity=True), cfg)
-    return cfg, blob, n_stride, _ticks(pool, S, n_stride, act, empty), act, resets
-
-
-def _guarded(d):
-    nbytes = capi.PreStreamsWorkspace.workspace_bytes(d)
-    buf = torch.full((nbytes + 2 * GUARD,), 0xFF, dtype=torch.uint8, device=DEV)      # NaN-filled floats
-    return buf, buf[GUARD:GUARD + nbytes]
+    return cfg, blob, n_stride, H.recipe_ticks(pool, S, n_stride, act, empty), act, resets
 
 
 def _run(st, ticks, resets, normalized, graph=False):
-    """Every tick through one recipe streams workspace -> [(T [S,16], valid [S], losses [S,8], factor [S] or None)]."""
-    S = st.desc.max_batch
-    n_stride = ticks[0][0].shape[2]
-    pts = torch.zeros((S, 3, n_stride), dtype=torch.float32, device=DEV)
-    counts = torch.zeros((S,), dtype=torch.int32, device=DEV)
-    active = torch.zeros((S,), dtype=torch.int32, device=DEV)
-    T = torch.full((S, 16), SENTINEL, dtype=torch.float32, device=DEV)
-    valid = torch.full((S,), 7, dtype=torch.int32, device=DEV)
-    losses = torch.full((S, ops.LOSS_ROW), SENTINEL, dtype=torch.float32, device=DEV)
-    factor = torch.full((S,), SENTINEL, dtype=torch.float32, device=DEV) if normalized else None
-    mask = torch.zeros((S,), dtype=torch.int32, device=DEV)
-    g = None
-    if graph:
-        st.push(pts, counts, active, T, valid, losses, factor)        # all inactive: changes no stream's state
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            st.push(pts, counts, active, T, valid, losses, factor)
-    out = []
-    for k, (p, c, a) in enumerate(ticks):
-        if k in resets:
-            mask.zero_()
-            mask[resets[k]] = 1
-            st.reset(mask)
-        pts.copy_(p)
-        counts.copy_(c)
-        active.copy_(a)
-        if g is not None:
-            g.replay()
-        else:
-            st.push(pts, counts, active, T, valid, losses, factor)
-        torch.cuda.synchronize()
-        out.append((T.cpu().clone(), valid.cpu().clone(), losses.cpu().clone(),
-                    None if factor is None else factor.cpu().clone()))
-    return out
-
-
-def _history(ticks, act, resets):
-    """{(k, s): (previous frame, this frame)} of every pair the streams should serve: (points [3, n], count)."""
-    pairs, prev = {}, [None] * act.shape[1]
-    for k, (p, c, _) in enumerate(ticks):
-        for s in resets.get(k, []):
-            prev[s] = None
-        for s in range(act.shape[1]):
-            if not act[k, s]:
-                continue
-            if prev[s] is not None:
-                pairs[(k, s)] = (prev[s], (p[s], c[s]))
-            prev[s] = (p[s], c[s])
-    return pairs
+    """Every tick through one recipe streams workspace -> [(T [S,16], valid [S], losses [S,8][, factor [S]])]."""
+    return H.run_streams(st, ticks, ("losses", "factor") if normalized else ("losses",), resets=resets, graph=graph)
 
 
 def _check_against_references(cfg, blob, out, pairs, normalized, flags=ICP):
@@ -137,7 +59,8 @@ def _check_against_references(cfg, blob, out, pairs, normalized, flags=ICP):
     hf, vf = tuple(cfg["horizontal_field_of_view"]), tuple(ds["vertical_field_of_view"])
     inf = capi.InferenceWorkspace(H.desc(cfg, h * w_pre, 1), blob)
     S = out[0][0].shape[0]
-    for k, (T, valid, losses, factor) in enumerate(out):
+    for k, (T, valid, losses, *factor) in enumerate(out):
+        factor = factor[0] if normalized else None
         for s in range(S):
             want = (k, s) in pairs
             assert int(valid[s]) == int(want), f"tick {k} stream {s}: valid={int(valid[s])}, expected {int(want)}"
@@ -184,13 +107,11 @@ def test_rows_are_the_testers_input_and_the_operators_residual(cuda_lib, h, w, w
     S = 3
     cfg, blob, n_stride, ticks, act, resets = _setup(h, w, w_raw, w_pre, normalized, S)
     d = H.desc(cfg, n_stride, S, w_pre)
-    buf, ws = _guarded(d)
+    ws, intact = H.guarded_workspace(capi.PreStreamsWorkspace.workspace_bytes(d))
     st = capi.PreStreamsWorkspace(d, blob, capi.residual_params(cfg, _flags(normalized)), workspace=ws)
     out = _run(st, ticks, resets, normalized)
-    torch.cuda.synchronize()
-    assert bool((buf[:GUARD] == 0xFF).all()) and bool((buf[GUARD + ws.numel():] == 0xFF).all()), \
-        "a write outside delora_odometry_streams_pre_workspace_bytes"
-    pairs = _history(ticks, act, resets)
+    assert intact(), "a write outside delora_odometry_streams_pre_workspace_bytes"
+    pairs = H.history(ticks, act, resets)
     assert len(pairs) >= 8 and int(out[0][1].sum()) == 0
     _check_against_references(cfg, blob, out, pairs, normalized)
     # rows without a transform this tick keep the T row of the tick before
@@ -211,7 +132,7 @@ def test_streams_are_independent_and_the_graph_replays(cuda_lib, normalized):
                    graph=True)
     for k, (e, g) in enumerate(zip(eager, graphed)):
         for i, (a, b) in enumerate(zip(e, g)):
-            assert a is None or H.same(a, b), f"tick {k}: output {i} of the replay differs from the eager call"
+            assert H.same(a, b), f"tick {k}: output {i} of the replay differs from the eager call"
     for s in range(S):
         single = [(p[s:s + 1], c[s:s + 1], a[s:s + 1]) for p, c, a in ticks]
         res = {k: [0] for k, streams in resets.items() if s in streams}
@@ -232,7 +153,7 @@ def test_agrees_with_the_training_eval(cuda_lib, normalized):
     and matched pairs; the factor is the same bits (the same grid factor kernel on the same H x w_pre grids)."""
     h, w, w_raw, w_pre = SIZES[1]
     cfg, blob, n_stride, _, _, _ = _setup(h, w, w_raw, w_pre, normalized, 1, seed=7)
-    ticks = _ticks(H.frames(h, w_raw, 8), 1, n_stride, np.ones((4, 1), dtype=bool), set())
+    ticks = H.recipe_ticks(H.frames(h, w_raw, 8), 1, n_stride, np.ones((4, 1), dtype=bool), set())
     flags = _flags(normalized)
     st = capi.PreStreamsWorkspace(H.desc(cfg, n_stride, 1, w_pre), blob, capi.residual_params(cfg, flags))
     out = _run(st, ticks, {}, normalized)
