@@ -232,14 +232,18 @@ icp_info_finalize_kernel(const float* __restrict__ partials, int rows, float lam
 #pragma unroll
         for (int j = 0; j < 6; ++j) evec[i][j] = v[i][j];
     }
-    // ascending eigenvalues (stable selection: the lower column first on equal values); each eigenvector's
+    // ascending eigenvalues, the lower column first on equal values: a selection sort on the pair (eigenvalue, column),
+    // whose keys are all distinct (a swap-based selection on the eigenvalue alone is not stable); each eigenvector's
     // largest-magnitude component (the first of equals) is positive
     int order[6] = {0, 1, 2, 3, 4, 5};
 #pragma unroll
     for (int x = 0; x < 6; ++x) {
 #pragma unroll
         for (int y = x + 1; y < 6; ++y) {
-            if (eval[order[y]] < eval[order[x]]) { const int t = order[x]; order[x] = order[y]; order[y] = t; }
+            const double ey = eval[order[y]], ex = eval[order[x]];
+            if (ey < ex || (ey == ex && order[y] < order[x])) {
+                const int t = order[x]; order[x] = order[y]; order[y] = t;
+            }
         }
     }
     for (int x = 0; x < 6; ++x) {

@@ -53,7 +53,8 @@ typedef struct { float x, y, z, w; } delora_f4;
 #define DELORA_ICP_PARTIAL 40
 /* number of floats in one row of the `info` output of delora_icp_dense_information:
  * [0, 36) H row-major, [36, 42) its eigenvalues ascending, [42, 78) the unit eigenvector of eigenvalue k at 42 + 6 k,
- * 78 M_pairs, 79 M_po2po */
+ * 78 M_pairs, 79 M_po2po.  Equal eigenvalues keep the order of the eigen-solve's columns (the lower column first): on a
+ * diagonal H the eigenvectors of a repeated eigenvalue are the unit axes in increasing index. */
 #define DELORA_INFO_ROW 80
 
 int         delora_abi_version(void);

@@ -10,6 +10,7 @@ import pytest
 import icp_reference as R
 import info_reference as IR
 import odometry_harness as H
+import projection_reference as PR
 
 NEW_SYMBOLS = ("delora_icp_information_scratch_floats", "delora_icp_dense_information",
                "delora_odometry_streams_info_workspace_bytes", "delora_odometry_streams_info_init",
@@ -187,3 +188,138 @@ def test_operator_refuses_null_outputs_and_stats():
     args[5] = 0
     assert L.delora_icp_dense_information(*args, 16, 16, None) != 0
     assert b"delora_icp_dense_information: bad shape" in L.delora_last_error()
+
+
+def test_vectorised_restatement_is_the_sum_over_pairs():
+    """information and term_sums (every pair's Jacobians at once) equal the weighted sum of each pair's `jacobians`,
+    with unpaired sources, sources and targets without normals, and every flag set."""
+    g = np.random.default_rng(1)
+    n = 200
+    T = IR.exp_se3(g.normal(size=6) * 0.3)[:3].astype(np.float32)
+    p = g.uniform(-8, 8, (n, 3)).astype(np.float32)
+    m = g.normal(size=(n, 3)).astype(np.float32)
+    m[:50] = 0.0
+    tn = g.normal(size=(n, 3)).astype(np.float32)
+    has = np.ones(n, bool)
+    has[40:90] = False
+    tn[~has] = 0.0
+    nn = g.permutation(n)
+    nn[:10] = -1
+    for flags in R.flag_matrix():
+        Hm, _, M, Mp = IR.information(T, p, m, tn, has, nn, flags, 0.7)
+        S, M2, Mp2 = IR.term_sums(T, p, m, tn, has, nn, flags)
+        kind = IR.pair_masks(T, p, m, tn, has, nn, flags)
+        w = dict(zip(("po2pl", "pl2pl", "po2po"), IR.weights(M, Mp, flags, 0.7)))
+        H2, S2 = np.zeros((6, 6)), {k: np.zeros((6, 6)) for k in w}
+        for i in np.nonzero(kind)[0]:
+            for term, J in IR.jacobians(T, p[i], m[i], tn[nn[i]], kind[i], flags):
+                H2 += w[term] * J.T @ J
+                S2[term] += J.T @ J
+        assert (M, Mp) == (M2, Mp2) == (int((kind == 1).sum()), int((kind == 2).sum()))
+        assert np.allclose(Hm, H2, rtol=1e-12, atol=1e-12 * np.abs(H2).max()), R.flag_name(flags)
+        for k in w:
+            assert np.allclose(S[k], S2[k], rtol=1e-12, atol=1e-9), (R.flag_name(flags), k)
+
+
+def _nearest_is_fma(h, a, b, c):
+    from fractions import Fraction
+    exact = Fraction(a) * Fraction(b) + Fraction(c)
+    err = abs(Fraction(h) - exact)
+    return all(err <= abs(Fraction(float(x)) - exact) for x in (np.nextafter(h, np.inf), np.nextafter(h, -np.inf)))
+
+
+def test_kernel_order_evaluator():
+    """kernel_order: h = fma(w_pp, S3, fma(w_nn, S2, w_pl S1)), each fma rounded once to the nearest float64, with the
+    weights of the finalize (lam rounded to fp32 first, 2 lam / M, 2 / M, 2 / (3 M')); a term the flags leave out or
+    whose count is 0 weighs 0; the scaled operator multiplies by 1 / f once per translation index."""
+    g = np.random.default_rng(5)
+    S = {k: np.zeros((6, 6)) for k in ("po2pl", "pl2pl", "po2po")}
+    for k in S:
+        X = g.integers(-40, 40, (6, 6)).astype(np.float64)
+        S[k] = X + X.T
+    every = R.LOSS_PO2PO | R.LOSS_PO2PL | R.LOSS_PL2PL
+    M, Mp, lam = 37, 11, 0.3
+    H, H32 = IR.kernel_order(S, M, Mp, every, lam)
+    w_pl, w_nn, w_pp = 2.0 * float(np.float32(lam)) / M, 2.0 / M, 2.0 / (3.0 * Mp)
+    assert IR.weights(M, Mp, every, lam) == (w_pl, w_nn, w_pp)
+    fused = 0
+    for i in range(6):
+        for j in range(6):
+            inner = IR._fma(w_nn, S["pl2pl"][i, j], w_pl * S["po2pl"][i, j])
+            assert _nearest_is_fma(inner, w_nn, S["pl2pl"][i, j], w_pl * S["po2pl"][i, j])
+            assert _nearest_is_fma(H[i, j], w_pp, S["po2po"][i, j], inner)
+            fused += H[i, j] != (w_pl * S["po2pl"][i, j] + w_nn * S["pl2pl"][i, j]) + w_pp * S["po2po"][i, j]
+    assert fused > 0, "no entry where the contraction changes the result: the evaluator is not tested"
+    assert np.array_equal(H32, H.astype(np.float32)) and np.array_equal(H, H.T)
+    assert IR.weights(M, Mp, R.LOSS_PO2PL, lam) == (w_pl, 0.0, 0.0)
+    assert IR.weights(0, Mp, every, lam) == (0.0, 0.0, w_pp) and IR.weights(M, 0, every, lam) == (w_pl, w_nn, 0.0)
+    only_pl, _ = IR.kernel_order(S, M, Mp, R.LOSS_PO2PL, lam)
+    assert np.array_equal(only_pl, w_pl * S["po2pl"])
+    for f in (0.25, 4.0, 0.3):
+        Hs, _ = IR.kernel_order(S, M, Mp, every, lam, factor=f)
+        inv = 1.0 / float(np.float32(f))
+        D = np.array([inv] * 3 + [1.0] * 3)
+        want = H.copy()
+        for i in range(6):
+            for j in range(6):
+                want[i, j] = want[i, j] * D[min(i, j)] * D[max(i, j)] if min(i, j) < 3 else want[i, j]
+        assert np.array_equal(Hs, want), f
+        if f != 0.3:                                        # powers of two: D H D exactly
+            assert np.array_equal(Hs, D[:, None] * H * D[None, :])
+
+
+EXACT_DESIGNS = ("tie", "triple", "zeros", "near", "mixed")
+
+
+@pytest.mark.parametrize("name", EXACT_DESIGNS)
+def test_exact_designs(name):
+    """Every source and every target owns its pixel; every Jacobian entry and every sum the kernels form in fp32 is an
+    integer below 2^24 (so the fp32 sums are exact: the float64 sums equal their fp32 rounding); the spectrum is the
+    intended one."""
+    d = IR.exact_design(name)
+    h, w, hf, vf = IR.DESIGN_GRID
+    for pts in (d.p, d.tgt_p):
+        pr = PR.project(pts.T, h, w, hf, vf)
+        assert (pr["pixel"] >= 0).all() and len(np.unique(pr["pixel"])) == len(pts)
+    assert np.array_equal(d.p, np.round(d.p)) and np.array_equal(d.tgt_p, np.round(d.tgt_p))
+    assert np.array_equal(d.tgt_p.astype(np.float64), d.p.astype(np.float64) @ d.T[:, :3].T.astype(np.float64) + d.T[:, 3])
+    for flags in (R.flag_matrix() if name == "mixed" else [d.flags]):
+        kind = IR.pair_masks(d.T, d.p, d.m, d.tgt_n, d.tgt_has, np.arange(len(d.p)), flags)
+        bound = np.zeros((6, 6))
+        for J in IR.term_jacobians(d.T, d.p, d.m, d.tgt_n, kind, flags).values():
+            assert np.array_equal(J, np.round(J))
+            bound += np.einsum("nka,nkb->ab", np.abs(J), np.abs(J))
+        assert bound.max() < 2 ** 24
+        S, M, Mp = IR.design_sums(d, flags)
+        for v in S.values():
+            assert np.array_equal(v, v.astype(np.float32).astype(np.float64))
+    S, M, Mp = IR.design_sums(d)
+    H, H32 = IR.kernel_order(S, M, Mp, d.flags, d.lam)
+    ev = np.linalg.eigvalsh(H)
+    off = H - np.diag(np.diag(H))
+    if name == "tie":
+        b, a = H[0, 0], H[2, 2]
+        assert not off.any() and H[1, 1] == b and a < b < np.diag(H)[3:].min()
+    elif name == "triple":
+        assert not off.any() and len(set(np.diag(H)[:3])) == 1 and len(set(np.diag(H)[3:])) == 1 and H[0, 0] < H[3, 3]
+    elif name == "zeros":
+        assert not H[:3].any() and not H[:, :3].any() and not off.any() and np.diag(H)[3:].min() > 0
+        assert np.array_equal(ev[:3], np.zeros(3))
+    elif name == "near":
+        assert not H[:3, 3:].any() and H[3, 4] != 0 and S["pl2pl"][3, 3] == S["pl2pl"][4, 4] != S["pl2pl"][5, 5]
+    else:
+        assert M > 0 and Mp > 0 and all(np.abs(v).max() > 0 for v in S.values()) and np.abs(off).max() > 0
+
+
+@pytest.mark.parametrize("ratio", (1e-3, 1e-6, 1e-9, 1e-12))
+def test_near_tie_design_gaps(ratio):
+    """near_tie_lambda gives the near design a pair of rotation eigenvalues whose gap is ratio (within 3x) of the
+    largest, and a gap to the rest of the spectrum above 0.1 of it."""
+    d = IR.exact_design("near")
+    lam = IR.near_tie_lambda(d, ratio)
+    S, M, Mp = IR.design_sums(d)
+    H, _ = IR.kernel_order(S, M, Mp, d.flags, lam)
+    ev = np.linalg.eigvalsh(H)
+    gap = ev[5] - ev[4]
+    assert ratio / 3 <= gap / ev[5] <= 3 * ratio, (gap / ev[5], ratio)
+    assert ev[4] - ev[3] > 0.1 * ev[5]
