@@ -132,6 +132,10 @@ SIGNATURES = {
                                      c_void_p, c_void_p, c_void_p]),
     "delora_trunk_backward": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                       c_int, c_void_p]),
+    "delora_trunk_forward_dropout": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "delora_trunk_backward_dropout": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                              c_void_p, c_int, c_void_p, c_void_p]),
     "delora_odometry_weight_floats": (c_i64, [c_desc_p]),
     "delora_odometry_workspace_bytes": (c_i64, [c_desc_p]),
     "delora_odometry_init": (c_int, [c_desc_p, c_void_p, c_void_p]),

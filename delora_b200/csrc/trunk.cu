@@ -364,10 +364,18 @@ extern "C" int64_t delora_trunk_activation_bytes(const int* layers, int B, int H
     return (int64_t)off;
 }
 
-extern "C" int delora_trunk_forward(const int* layers, int B, int H, int W, int act, int saving, const float* img1,
-                                    const float* img2, const void* weights, void* acts, float* pooled, void** stage_out,
-                                    void* stream) {
-    const char* who = "delora_trunk_forward";
+// dropout_ctr (device int64[3], the training workspace's counter-slot layout: [0] the step, [2] the seed) non-NULL: the
+// input and stage-3 dropouts of a training step at that step, read as DropoutCtr{ctr, 0} by the forward and by every
+// backward call; NULL: no dropout.
+static DropoutCtr trunk_dropout(const int64_t* dropout_ctr) {
+    return DropoutCtr{reinterpret_cast<const long long*>(dropout_ctr), 0};
+}
+
+extern "C" int delora_trunk_forward_dropout(const int* layers, int B, int H, int W, int act, int saving,
+                                            const float* img1, const float* img2, const void* weights, void* acts,
+                                            float* pooled, void** stage_out, const int64_t* dropout_ctr,
+                                            void* stream) {
+    const char* who = dropout_ctr ? "delora_trunk_forward_dropout" : "delora_trunk_forward";
     if (check_trunk(layers, H, W, who) || check_batch(B, saving, who)) return 1;
     DELORA_CHECK_ARG(act == 1 || act == 2, "%s: act=%d must be 1 (relu) or 2 (tanh)", who, act);
     DELORA_CHECK_ARG(img1, "%s: null img1", who);
@@ -375,20 +383,31 @@ extern "C" int delora_trunk_forward(const int* layers, int B, int H, int W, int 
     DELORA_CHECK_ARG(weights, "%s: null weights", who);
     DELORA_CHECK_ARG(acts, "%s: null acts", who);
     DELORA_CHECK_ARG(pooled, "%s: null pooled", who);
+    // x3d lives in a backward buffer of the saving layout
+    DELORA_CHECK_ARG(!dropout_ctr || saving == 1, "%s: dropout_ctr needs saving=1 (saving=%d)", who, saving);
     TrunkPlan m;
     plan_trunk(layers, H, W, &m);
     size_t woff = 0, aoff = 0;
     const TrunkWeights w = plan_trunk_weights(m, true, woff);
     const TrunkActs a = plan_trunk_acts(m, B, saving != 0, aoff);
     cudaStream_t st = (cudaStream_t)stream;
-    const int rc = trunk_input(m, a, (char*)acts, img1, img2, B, st);
+    const DropoutCtr drop = trunk_dropout(dropout_ctr);
+    const int rc = trunk_input(m, a, (char*)acts, img1, img2, B, st, drop);
     if (rc) return rc;
-    return trunk_forward(m, a, (char*)acts, w, (const char*)weights, act, B, pooled, stage_out, st);
+    return trunk_forward(m, a, (char*)acts, w, (const char*)weights, act, B, pooled, stage_out, st, drop);
 }
 
-extern "C" int delora_trunk_backward(const int* layers, int B, int H, int W, int act, const void* weights, void* acts,
-                                     const float* g_pooled, float* const* conv_dw, int stage, void* stream) {
-    const char* who = "delora_trunk_backward";
+extern "C" int delora_trunk_forward(const int* layers, int B, int H, int W, int act, int saving, const float* img1,
+                                    const float* img2, const void* weights, void* acts, float* pooled, void** stage_out,
+                                    void* stream) {
+    return delora_trunk_forward_dropout(layers, B, H, W, act, saving, img1, img2, weights, acts, pooled, stage_out,
+                                        nullptr, stream);
+}
+
+extern "C" int delora_trunk_backward_dropout(const int* layers, int B, int H, int W, int act, const void* weights,
+                                             void* acts, const float* g_pooled, float* const* conv_dw, int stage,
+                                             const int64_t* dropout_ctr, void* stream) {
+    const char* who = dropout_ctr ? "delora_trunk_backward_dropout" : "delora_trunk_backward";
     if (check_trunk(layers, H, W, who) || check_batch(B, 1, who)) return 1;
     DELORA_CHECK_ARG(act == 1 || act == 2, "%s: act=%d must be 1 (relu) or 2 (tanh)", who, act);
     DELORA_CHECK_ARG(stage >= 0 && stage <= 3, "%s: stage=%d must be in [0, 3]", who, stage);
@@ -409,5 +428,11 @@ extern "C" int delora_trunk_backward(const int* layers, int B, int H, int W, int
     const TrunkWeights w = plan_trunk_weights(m, true, woff);
     const TrunkActs a = plan_trunk_acts(m, B, true, aoff);
     return trunk_backward(m, a, (char*)acts, w, (const char*)weights, act, B, g_pooled, conv_dw, stage,
-                          (cudaStream_t)stream);
+                          (cudaStream_t)stream, trunk_dropout(dropout_ctr));
+}
+
+extern "C" int delora_trunk_backward(const int* layers, int B, int H, int W, int act, const void* weights, void* acts,
+                                     const float* g_pooled, float* const* conv_dw, int stage, void* stream) {
+    return delora_trunk_backward_dropout(layers, B, H, W, act, weights, acts, g_pooled, conv_dw, stage, nullptr,
+                                         stream);
 }

@@ -471,7 +471,15 @@ int delora_quat_to_T_bwd(const float* quaternion, const float* grad_T, int B,
  * order.  Stage 3 starts from g_pooled [B, 512] fp32 (read by stage 3 only); stage 0 ends with the max-pool and the
  * stem.  Each call writes the weight gradient of every convolution of its stage (stage 0: and the stem) to
  * conv_dw[c] (fp32 [Cout, Cin, k, k], c in the order of `filters`; a HOST array of device pointers), so that the
- * gradients of a stage can be used once its call is enqueued. */
+ * gradients of a stage can be used once its call is enqueued.
+ * _dropout variants: the input and stage-3 dropouts of a DELORA_TRAIN_DROPOUT training step (see _train_step), with
+ * their masks at the step and seed of dropout_ctr, a device int64[3] in the training workspace's counter-slot layout:
+ * [0] the step, [2] the seed ([1] is not read).  Pass the same counter to the forward and to the four backward calls;
+ * the backward overwrites x3d, so each backward with a counter follows its own forward.
+ * x1 .. x4 (stage_out) are the stage outputs before the stage-3 dropout, as the step keeps them; `pooled` and the weight
+ * gradients are the step's.  dropout_ctr NULL: exactly delora_trunk_forward / delora_trunk_backward.  A counter needs
+ * saving = 1 (x3d lives in a backward buffer); refused before any launch otherwise.  The fc dropout is not the trunk's.
+ */
 int64_t delora_trunk_weight_bytes(const int* layers, int W);
 int delora_trunk_prep_weights(const int* layers, int W, const float* const* filters, void* weights, void* stream);
 int64_t delora_trunk_activation_bytes(const int* layers, int B, int H, int W, int saving);
@@ -480,6 +488,12 @@ int delora_trunk_forward(const int* layers, int B, int H, int W, int act, int sa
                          void* stream);
 int delora_trunk_backward(const int* layers, int B, int H, int W, int act, const void* weights, void* acts,
                           const float* g_pooled, float* const* conv_dw, int stage, void* stream);
+int delora_trunk_forward_dropout(const int* layers, int B, int H, int W, int act, int saving, const float* img1,
+                                 const float* img2, const void* weights, void* acts, float* pooled, void** stage_out,
+                                 const int64_t* dropout_ctr, void* stream);
+int delora_trunk_backward_dropout(const int* layers, int B, int H, int W, int act, const void* weights, void* acts,
+                                  const float* g_pooled, float* const* conv_dw, int stage, const int64_t* dropout_ctr,
+                                  void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Odometry inference: raw scans -> relative transforms, the whole model behind one call.

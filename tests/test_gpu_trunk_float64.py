@@ -24,6 +24,16 @@ slice: x relu 6.4e-3, tanh 1.1e-2; pooled relu 5.9e-3, tanh 1.4e-2; dW relu 1.4e
 the loosest: with relu, an element of a sparse output-channel gradient whose act' flips between 0 and 1 (an activation
 within a rounding of zero) changes that slice by the element's whole share.  TAU leaves a margin of 2.1 .. 2.4x.
 
+Dropout (the training step's input and stage-3 dropouts through delora_trunk_forward_dropout / _backward_dropout, at a
+counter whose step and seed both have a nonzero high word; the reference with the numpy generator's masks): the exact
+tier at saving 1 on designs with images in 16 x [-2, 2], so that 1.25 x and 1.25 x3 are integers (x3 is compared
+before the dropout, as stage_out gives it), on both stem routes (the channel-padded conversion of an odd W, the
+16-channel one of an even W) times both data-gradient routes of layer4's first block (phase at W = 23 and 180, the
+zero-upsample fallback at 259, 720 and 4), each of which applies the gradient mask of x3 in its own branch; and the
+Gaussian tier at the same TAU on {2,2,2,2} and {1,3,1,2} x 5x23, 16x180, 64x720, 16x259.  Measured on an H100 80GB
+HBM3 (700 W power limit) over the 16 dropout cases, worst slice: x relu 7.0e-3, tanh 1.1e-2; pooled relu 7.0e-3, tanh
+1.9e-2; dW relu 2.3e-1 (1x3x1x2 16x180, a relu' flip as above), tanh 1.1e-1: margins of 1.3 .. 2.4x under the same TAU.
+
 The odometry ABI on the plans {3,4,6,3} and {1,3,1,2}, at an even and an odd W: delora_odometry_pairs' pooled equals
 delora_trunk_forward's bit for bit, and one relu training step stays within odometry_harness's TAIL_TOL / TRUNK_TOL of
 the Python step (measured on the H100: the trunk gradients bit-identical, the tail within 6.1e-7).  With tanh the
@@ -58,9 +68,20 @@ EXACT_PLANS = [
     ((64, 1, 1, 1), [(2, 7)]),
     ((1, 1, 1, 64), [(1, 4)]),
 ]
-EXACT_CASES = [(layers, h, w, b) for layers, sizes in EXACT_PLANS for h, w in sizes for b in (1, 3)]
-GAUSS_CASES = [(layers, h, w, act) for layers in ((1, 1, 1, 1), (2, 2, 2, 2), (1, 3, 1, 2))
-               for h, w in ((5, 23), (16, 180), (64, 720)) for act in ("relu", "tanh")]
+# The dropout cases: every stem route (W odd: channel-padded, W even: 16-channel) with every data-gradient route of
+# layer4's first block (phase when the stage-3 width is even: W = 23, 180; fallback: W = 259, 720, 4).
+DROPOUT_CTR = (2 ** 32 + 7, 2 ** 40 + 0x5EED)          # (step, seed): both with a nonzero high word
+DROPOUT_PLANS = [
+    ((1, 1, 1, 1), [(5, 23), (16, 259), (16, 180), (16, 720), (1, 4)]),
+    ((2, 2, 2, 2), [(5, 23), (16, 259), (16, 180), (64, 720)]),
+    ((1, 1, 1, 64), [(5, 23), (1, 4)]),
+]
+EXACT_CASES = [(layers, h, w, b, None) for layers, sizes in EXACT_PLANS for h, w in sizes for b in (1, 3)] + \
+    [(layers, h, w, b, DROPOUT_CTR) for layers, sizes in DROPOUT_PLANS for h, w in sizes for b in (1, 3)]
+GAUSS_CASES = [(layers, h, w, act, None) for layers in ((1, 1, 1, 1), (2, 2, 2, 2), (1, 3, 1, 2))
+               for h, w in ((5, 23), (16, 180), (64, 720)) for act in ("relu", "tanh")] + \
+    [(layers, h, w, act, DROPOUT_CTR) for layers in ((2, 2, 2, 2), (1, 3, 1, 2))
+     for h, w in ((5, 23), (16, 180), (64, 720), (16, 259)) for act in ("relu", "tanh")]
 
 
 def _lib():
@@ -70,6 +91,16 @@ def _lib():
 
 def _id(layers):
     return "x".join(map(str, layers))
+
+
+def case_id(layers, h, w, last, counter):
+    return f"{_id(layers)}-{h}x{w}-{last}" + ("" if counter is None else "-dropout")
+
+
+def counter_tensor(counter):
+    """(step, seed) -> the device int64[3] counter of the _dropout entry points: [0] the step, [2] the seed."""
+    step, seed = counter
+    return torch.tensor([(v + 2 ** 63) % 2 ** 64 - 2 ** 63 for v in (step, 0, seed)], dtype=torch.int64, device=DEV)
 
 
 class TrunkRun:
@@ -100,16 +131,19 @@ class TrunkRun:
             self.acts[saving] = (buf, n)
         return self.acts[saving][0]
 
-    def forward(self, img1, img2, saving):
-        """-> ([x1 .. x4] padded NHWC bf16 copies, pooled [B, 512] fp32)."""
+    def forward(self, img1, img2, saving, ctr=None):
+        """-> ([x1 .. x4] padded NHWC bf16 copies, pooled [B, 512] fp32).  ctr (counter_tensor): the dropout forward."""
         ops = self.ops
         acts = self._acts(saving)
         pooled = torch.full((self.b, 512), float("nan"), dtype=torch.float32, device=DEV)
         so = (ctypes.c_void_p * 4)()
-        _lib().check(self.L.delora_trunk_forward(
-            self.lay, self.b, self.h, self.w, self.act, saving, ops._req(img1, torch.float32, "img1"),
-            ops._req(img2, torch.float32, "img2"), self.weights.data_ptr(), acts.data_ptr(), pooled.data_ptr(), so,
-            ops._stream()), "delora_trunk_forward")
+        args = (self.lay, self.b, self.h, self.w, self.act, saving, ops._req(img1, torch.float32, "img1"),
+                ops._req(img2, torch.float32, "img2"), self.weights.data_ptr(), acts.data_ptr(), pooled.data_ptr(), so)
+        if ctr is None:
+            _lib().check(self.L.delora_trunk_forward(*args, ops._stream()), "delora_trunk_forward")
+        else:
+            _lib().check(self.L.delora_trunk_forward_dropout(*args, ctr.data_ptr(), ops._stream()),
+                         "delora_trunk_forward_dropout")
         xs = []
         for s, ((hs, ws), c) in enumerate(zip(R.stage_sizes(self.h, self.w), R.WIDTHS)):
             off = so[s] - acts.data_ptr()
@@ -118,8 +152,9 @@ class TrunkRun:
             xs.append(acts[off:off + n].view(torch.bfloat16).view(self.b, hs + 2, ws + 2, c).clone())
         return xs, pooled
 
-    def backward(self, g_pooled):
-        """The four stage calls after a saving forward -> every conv_dw[c], each a slice of one NaN-filled buffer."""
+    def backward(self, g_pooled, ctr=None):
+        """The four stage calls after a saving forward -> every conv_dw[c], each a slice of one NaN-filled buffer.
+        ctr: the dropout backward, with the forward's counter."""
         ops = self.ops
         numels = [f.numel() for f in self.filters]
         flat = torch.full((sum(numels),), float("nan"), dtype=torch.float32, device=DEV)
@@ -130,10 +165,13 @@ class TrunkRun:
         ptrs = (ctypes.c_void_p * self.n_conv)(*[d.data_ptr() for d in dws])
         g = g_pooled.float().contiguous()
         for stage in (3, 2, 1, 0):
-            _lib().check(self.L.delora_trunk_backward(self.lay, self.b, self.h, self.w, self.act,
-                                                      self.weights.data_ptr(), self._acts(1).data_ptr(),
-                                                      ops._req(g, torch.float32, "g_pooled"), ptrs, stage,
-                                                      ops._stream()), "delora_trunk_backward")
+            args = (self.lay, self.b, self.h, self.w, self.act, self.weights.data_ptr(), self._acts(1).data_ptr(),
+                    ops._req(g, torch.float32, "g_pooled"), ptrs, stage)
+            if ctr is None:
+                _lib().check(self.L.delora_trunk_backward(*args, ops._stream()), "delora_trunk_backward")
+            else:
+                _lib().check(self.L.delora_trunk_backward_dropout(*args, ctr.data_ptr(), ops._stream()),
+                             "delora_trunk_backward_dropout")
         bad = ~torch.isfinite(flat)
         assert not bool(bad.any()), f"{int(bad.sum())} conv_dw entries not written"
         return dws
@@ -158,46 +196,68 @@ def nchw(x):
 
 
 # ------------------------------------------------------------------------------------------------ exact tier
-def test_exact_matrix_runs_both_dgrad_routes():
+def _eligible(ci, co, wi, st):
     from delora_b200 import ops
-    routes = {r for layers, h, w, _ in EXACT_CASES
-              for _, r in R.dgrad_routes(layers, h, w, lambda ci, co, wi, st: ops.conv2d_dgrad_eligible(ci, co, wi, st))}
+    return ops.conv2d_dgrad_eligible(ci, co, wi, st)
+
+
+def test_exact_matrix_runs_both_dgrad_routes():
+    routes = {r for layers, h, w, _, _ in EXACT_CASES for _, r in R.dgrad_routes(layers, h, w, _eligible)}
     assert routes == {"phase", "fallback"}, routes
 
 
-@pytest.mark.parametrize("layers,h,w,b", EXACT_CASES, ids=[f"{_id(c[0])}-{c[1]}x{c[2]}-b{c[3]}" for c in EXACT_CASES])
-def test_exact_integer_design(layers, h, w, b, cuda_lib):
-    from delora_b200 import ops
-    label = f"exact {_id(layers)} {h}x{w} B={b}"
-    d = R.exact_design(layers, b, h, w, device=DEV)
-    routes = R.dgrad_routes(layers, h, w, lambda ci, co, wi, st: ops.conv2d_dgrad_eligible(ci, co, wi, st))
+def layer4_route(layers, h, w):
+    """The data-gradient route of layer4's first block, the block that reads x3d in a dropout step."""
+    first4 = sum(layers[:3])
+    return dict(R.dgrad_routes(layers, h, w, _eligible))[first4]
+
+
+def test_dropout_matrix_runs_every_stem_and_layer4_route():
+    """The masked input conversion of both stem layouts, and the stage-3 gradient mask after both data-gradient routes
+    of layer4's first block (trunk.cu applies it in each route's branch)."""
+    combos = {("16-channel" if w % 2 == 0 else "channel-padded", layer4_route(layers, h, w))
+              for layers, h, w, _, ctr in EXACT_CASES if ctr is not None}
+    print(f"\n[dropout routes] {sorted(combos)}", flush=True)
+    assert combos == {(stem, r) for stem in ("16-channel", "channel-padded") for r in ("phase", "fallback")}, combos
+
+
+@pytest.mark.parametrize("layers,h,w,b,counter", EXACT_CASES, ids=[case_id(*c[:3], f"b{c[3]}", c[4]) for c in EXACT_CASES])
+def test_exact_integer_design(layers, h, w, b, counter, cuda_lib):
+    """With a counter: saving 1 only (the dropout forward needs it); x3 is stage_out's, before the stage-3 dropout.
+    The backward overwrites x3d, so the second backward follows a second forward."""
+    label = f"exact {_id(layers)} {h}x{w} B={b}" + ("" if counter is None else f" dropout {counter}")
+    d = R.exact_design(layers, b, h, w, device=DEV, counter=counter)
+    routes = R.dgrad_routes(layers, h, w, _eligible)
+    ctr = None if counter is None else counter_tensor(counter)
     tr = TrunkRun(layers, b, h, w, "relu", d.filters)
     img1, img2 = d.img1.contiguous(), d.img2.contiguous()
     h4, w4 = R.stage_sizes(h, w)[3]
     total = d.x[3].sum(dim=(2, 3))
     assert bool((total.abs() < R.SUM_MAX).all())
     want_pooled = total.float() / torch.tensor(float(h4 * w4), dtype=torch.float32, device=DEV)
-    for saving in (0, 1):
-        xs, pooled = tr.forward(img1, img2, saving)
+    for saving in ((0, 1) if ctr is None else (1,)):
+        xs, pooled = tr.forward(img1, img2, saving, ctr)
         for s in range(4):
             check_halo(xs[s], f"{label} saving={saving} x{s + 1}")
             check_exact(nchw(xs[s]), d.x[s], f"{label} saving={saving} x{s + 1}")
         assert torch.equal(pooled, want_pooled), f"{label} saving={saving}: pooled differs from the fp32 exact mean"
-        xs2, pooled2 = tr.forward(img1, img2, saving)
+        xs2, pooled2 = tr.forward(img1, img2, saving, ctr)
         assert torch.equal(pooled2.view(torch.int32), pooled.view(torch.int32)), f"{label}: second forward differs"
         for a, c in zip(xs, xs2):
             assert torch.equal(a.view(torch.int16), c.view(torch.int16)), f"{label}: second forward differs"
-    dws = tr.backward(d.g_pooled)
+    dws = tr.backward(d.g_pooled, ctr)
     for c, (got, ref) in enumerate(zip(dws, d.dw)):
         check_exact(got.double(), ref, f"{label} conv_dw[{c}]")
-    again = tr.backward(d.g_pooled)
+    if ctr is not None:
+        tr.forward(img1, img2, 1, ctr)
+    again = tr.backward(d.g_pooled, ctr)
     for c, (x, y) in enumerate(zip(dws, again)):
         assert torch.equal(x.view(torch.int32), y.view(torch.int32)), f"{label}: second backward differs at conv {c}"
     torch.cuda.synchronize()
     tr.check_guards(label)
     fr = d.stats["relu"]
-    print(f"\n[{label}] exact: x1..x4, pooled (saving 0 / 1) and {len(dws)} conv_dw bit-identical; "
-          f"{len(d.stats['nonzero_dw'])} nonzero dW; dgrad routes {routes or 'none'}; relu'=1 fraction "
+    print(f"\n[{label}] exact: x1..x4, pooled (saving {'0 / 1' if ctr is None else '1'}) and {len(dws)} conv_dw "
+          f"bit-identical; {len(d.stats['nonzero_dw'])} nonzero dW; dgrad routes {routes or 'none'}; relu'=1 fraction "
           f"min {min(f for _, f in fr):.3f} max {max(f for _, f in fr):.3f} over {len(fr)} activations", flush=True)
 
 
@@ -213,29 +273,32 @@ def gaussian_problem(layers, h, w, act, b=2, seed=0):
     return filters, img1, img2, g_pooled
 
 
-def gaussian_worst(layers, h, w, act):
-    """-> {kind: (worst slice ratio, where)} of the kernels against the teacher-forced, bf16-faithful reference."""
+def gaussian_worst(layers, h, w, act, counter=None):
+    """-> {kind: (worst slice ratio, where)} of the kernels against the teacher-forced, bf16-faithful reference.
+    counter: the dropout entry points (saving 1) against the reference with the numpy generator's masks."""
     filters, img1, img2, g_pooled = gaussian_problem(layers, h, w, act)
     b = img1.shape[0]
     tr = TrunkRun(layers, b, h, w, act, filters)
+    ctr = None if counter is None else counter_tensor(counter)
+    masks = None if counter is None else R.dropout_masks(counter[1], counter[0], b, h, w, DEV)
     worst = {"x": (0.0, ""), "pooled": (0.0, ""), "dw": (0.0, "")}
 
     def note(kind, got, ref, axes, where):
         r, at = R.worst_slice(got, ref, axes)
         if r >= worst[kind][0]:
             worst[kind] = (r, f"{where} {at}")
-    for saving in (0, 1):
-        xs, pooled = tr.forward(img1, img2, saving)
+    for saving in ((0, 1) if ctr is None else (1,)):
+        xs, pooled = tr.forward(img1, img2, saving, ctr)
         fs = [f.double().requires_grad_(True) for f in filters]
         with torch.backends.cudnn.flags(enabled=False):
             ref = R.trunk(img1, img2, fs, layers, act, hooks=True, saving=bool(saving), bwd_round=True,
-                          teacher=[nchw(x) for x in xs[:3]])
+                          teacher=[nchw(x) for x in xs[:3]], masks=masks)
             for s in range(4):
                 check_halo(xs[s], f"saving={saving} x{s + 1}")
                 note("x", nchw(xs[s]), ref["x"][s].detach(), R.X_AXES, f"saving={saving} x{s + 1}")
             note("pooled", pooled, ref["pooled"].detach(), R.POOLED_AXES, f"saving={saving} pooled")
             if saving:
-                dws = tr.backward(g_pooled)
+                dws = tr.backward(g_pooled, ctr)
                 for c, (got, want) in enumerate(zip(dws, R.weight_grads(ref, fs, g_pooled.double()))):
                     note("dw", got, want, R.DW_AXES, f"conv_dw[{c}]")
     torch.cuda.synchronize()
@@ -243,12 +306,11 @@ def gaussian_worst(layers, h, w, act):
     return worst
 
 
-@pytest.mark.parametrize("layers,h,w,act", GAUSS_CASES,
-                         ids=[f"{_id(c[0])}-{c[1]}x{c[2]}-{c[3]}" for c in GAUSS_CASES])
-def test_gaussian_slices(layers, h, w, act, cuda_lib):
-    worst = gaussian_worst(layers, h, w, act)
+@pytest.mark.parametrize("layers,h,w,act,counter", GAUSS_CASES, ids=[case_id(*c) for c in GAUSS_CASES])
+def test_gaussian_slices(layers, h, w, act, counter, cuda_lib):
+    worst = gaussian_worst(layers, h, w, act, counter)
     line = "  ".join(f"{k} {v[0]:.2e} ({v[1]}) / tau {TAU[(k, act)]:.1e}" for k, v in worst.items())
-    print(f"\n[gauss {_id(layers)} {h}x{w} {act}] {line}", flush=True)
+    print(f"\n[gauss {case_id(layers, h, w, act, counter)}] {line}", flush=True)
     for k, (r, at) in worst.items():
         assert r <= TAU[(k, act)], f"{k}: slice {at} off by {r:.3e} of its norm (tau {TAU[(k, act)]:.1e})"
 

@@ -116,6 +116,23 @@ def test_launches_refuse_bad_arguments_by_name():
         (lambda: L.delora_trunk_backward(ok, 1, 64, 2048, 1, p, p, p, dw_hole, 0, None), b"conv_dw[0]"),
         (lambda: L.delora_trunk_backward(ok, 1, 64, 2048, 1, None, p, p, dw, 3, None), b"null weights"),
         (lambda: L.delora_trunk_backward(ok, 0, 64, 2048, 1, p, p, p, dw, 3, None), b"B=0"),
+        # the dropout variants: the same checks under their own name, and a counter only with saving = 1
+        (lambda: L.delora_trunk_forward_dropout(ok, 1, 64, 2048, 1, 0, p, p, p, p, p, None, p, None),
+         b"delora_trunk_forward_dropout: dropout_ctr needs saving=1"),
+        (lambda: L.delora_trunk_forward_dropout(ok, 1, 64, 2047, 1, 0, p, p, p, p, p, None, p, None),
+         b"delora_trunk_forward_dropout: dropout_ctr needs saving=1"),
+        (lambda: L.delora_trunk_forward_dropout(ok, 1, 64, 2048, 3, 1, p, p, p, p, p, None, p, None),
+         b"delora_trunk_forward_dropout: act=3"),
+        (lambda: L.delora_trunk_forward_dropout(ok, 1, 64, 2048, 1, 1, p, None, p, p, p, None, p, None),
+         b"delora_trunk_forward_dropout: null img2"),
+        (lambda: L.delora_trunk_forward_dropout(ok, 1, 64, 2048, 1, 0, p, p, p, p, None, None, None, None),
+         b"delora_trunk_forward: null pooled"),                    # no counter: the plain call
+        (lambda: L.delora_trunk_backward_dropout(ok, 1, 64, 2048, 1, p, p, p, dw, -1, p, None),
+         b"delora_trunk_backward_dropout: stage=-1"),
+        (lambda: L.delora_trunk_backward_dropout(ok, 1, 64, 2048, 1, p, p, None, dw, 3, p, None),
+         b"delora_trunk_backward_dropout: null g_pooled"),
+        (lambda: L.delora_trunk_backward_dropout(ok, 1, 64, 2048, 1, p, p, p, dw_hole, 0, p, None),
+         b"delora_trunk_backward_dropout: null conv_dw[0]"),
     ]
     for call, msg in cases:
         assert call() != 0

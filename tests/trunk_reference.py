@@ -9,6 +9,12 @@ Definition (src/models/resnet_modified.py):
 - every 3x3 convolution pads circularly in W and with zeros in H; relu or tanh; global average pool.
 Filters come in state_dict order (`plan`), the order delora_trunk_prep_weights documents.
 
+Dropout (`masks`, a DELORA_TRAIN_DROPOUT training step; the contract of include/delora_b200.h, the Dropout paragraph
+of delora_odometry_train_step): every element of cat(image_1, image_2) becomes fp32(x * 1.25f) * keep before the bf16
+split; layer4's first block (its conv1, its downsample and their weight gradients) reads x3d = bf16(fp32(x3 * 1.25f))
+* keep [pair, channel] while x3 (layer3's output, in "x") stays for act'; the backward takes act'(x3) first, rounds
+(bwd_round), then multiplies by keep * 1.25 and rounds again (the dz2 store of layer3's last block).
+
 Rounding hooks (`hooks=True`) round to the type the trunk stores, where it stores it: the filters and the input (bf16;
 an even W keeps the rounding residual as a second bf16 term, the 16-channel layout), the stem output (fp16 on the
 16-channel route in saving mode with the activation deferred to the pool, bf16 pre-activation on the other route in
@@ -30,7 +36,8 @@ WIDTHS = (64, 128, 256, 512)
 STRIDES = ((1, 1), (1, 2), (1, 2), (2, 2))
 
 Block = collections.namedtuple("Block", "stage index cin cout stride c1 c2 ds")
-DEFECTS = ("zero_pad", "residual_from_input", "swap_blocks", "shift_pair", "argmax_last")
+DEFECTS = ("zero_pad", "residual_from_input", "swap_blocks", "shift_pair", "argmax_last", "drop_grad_unmasked",
+           "drop_stage3_shift", "drop_input_swap", "drop_act_from_x3d")
 
 
 def out_size(n, s):
@@ -116,23 +123,56 @@ class _GradStore(torch.autograd.Function):
         return (bf16(g) if ctx.opt.bwd_round else g), None, None
 
 
+def x3d(x3, keep, hooks):
+    """The stage-3 channel dropout as the trunk stores it: bf16(fp32(x3 * 1.25f)) * keep [B, C] (the fp32 product of a
+    bf16 and 1.25 is exact); x3 * 1.25 * keep without the hooks."""
+    y = x3 * 1.25
+    return (bf16(y) if hooks else y) * keep[:, :, None, None].to(x3)
+
+
 class _Act(torch.autograd.Function):
-    """y = act(x), stored (bf16 with the hooks); act' from the stored y: relu' = y > 0, tanh' = 1 - y^2."""
+    """y = act(x), stored (bf16 with the hooks); act' from the stored y: relu' = y > 0, tanh' = 1 - y^2.
+    drop (layer3's output x3 in a dropout step): (keep3 [B, C], opt, defect name) -- the backward multiplies by
+    keep * 1.25 after act', as the trunk does: bf16(act'(x3) g) with bwd_round, then keep * 1.25 (the dz2 store that
+    follows rounds once more).  The forward's x3d is _Drop3's."""
 
     @staticmethod
-    def forward(ctx, x, act, rnd):
+    def forward(ctx, x, act, rnd, drop=None):
         y = torch.relu(x) if act == "relu" else torch.tanh(x)
         if rnd:
             y = bf16(y)
-        ctx.act = act
+        ctx.act, ctx.drop = act, drop
         ctx.save_for_backward(y)
         return y
 
     @staticmethod
     def backward(ctx, g):
         y, = ctx.saved_tensors
-        d = (y > 0).to(y.dtype) if ctx.act == "relu" else 1.0 - y * y
-        return g * d, None, None
+        if ctx.drop is None:
+            d = (y > 0).to(y.dtype) if ctx.act == "relu" else 1.0 - y * y
+            return g * d, None, None, None
+        keep, opt, defect = ctx.drop
+        a = x3d(y, keep, opt.hooks) if defect == "drop_act_from_x3d" else y
+        g = g * ((a > 0).to(a.dtype) if ctx.act == "relu" else 1.0 - a * a)
+        if opt.trace is not None:
+            opt.trace["bwd"].append(("g_x3", g.detach()))
+        if opt.bwd_round:
+            g = bf16(g)
+        if defect != "drop_grad_unmasked":
+            g = g * keep[:, :, None, None].to(g) * 1.25
+        return g, None, None, None
+
+
+class _Drop3(torch.autograd.Function):
+    """Forward: x3d of x3; backward: the gradient passes unchanged (_Act applies keep * 1.25 after act')."""
+
+    @staticmethod
+    def forward(ctx, x, keep, hooks):
+        return x3d(x, keep, hooks)
+
+    @staticmethod
+    def backward(ctx, g):
+        return g, None, None
 
 
 class _Opt:
@@ -147,8 +187,8 @@ class _Opt:
             self.trace["fwd"].append((name, x.detach()))
         return x
 
-    def activation(self, x, name):
-        y = _Act.apply(x, self.act, self.hooks)
+    def activation(self, x, name, drop=None):
+        y = _Act.apply(x, self.act, self.hooks, drop)
         if self.trace is not None:
             self.trace["fwd"].append((name, y.detach()))
             if self.act == "relu":
@@ -181,12 +221,15 @@ def maxpool(z, rule="first"):
     return torch.gather(wins, 0, arg[None])[0]
 
 
-def trunk_input(img1, img2, hooks):
-    """cat(image_1, image_2) as the trunk reads it: bf16, plus the bf16 rounding residual for an even W."""
+def trunk_input(img1, img2, hooks, keep=None):
+    """cat(image_1, image_2) as the trunk reads it: bf16, plus the bf16 rounding residual for an even W.  keep
+    [B, 8, H, W] (the input dropout): fp32(x * 1.25f) * keep before the split."""
     x = torch.cat((img1, img2), dim=1).double()
     if not hooks:
-        return x
+        return x if keep is None else x * 1.25 * keep.to(x)
     x32 = x.float()
+    if keep is not None:
+        x32 = (x32 * 1.25) * keep.float()          # a float32 product, rounded as the kernels round it
     hi = x32.bfloat16().float()
     if x.shape[-1] % 2:
         return hi.double()
@@ -194,13 +237,17 @@ def trunk_input(img1, img2, hooks):
 
 
 def trunk(img1, img2, filters, layers, act, hooks=True, saving=True, bwd_round=False, teacher=None, defect=None,
-          trace=None):
+          trace=None, masks=None):
     """-> {"x": [x1 .. x4] NCHW, "pooled": [B, 512]} in float64, differentiable w.r.t. `filters`.
 
     defect (a negative control): (name, arg) with name in DEFECTS -- zero_pad: conv `arg` pads W with zeros;
     residual_from_input: the first downsampling block of stage `arg` adds its (strided, zero-channel-padded) input
     instead of the downsample; swap_blocks: conv2 of blocks 0 and 1 of stage `arg` trade filters; shift_pair: pair
-    `arg` of x1 moves down one row (zero row on top); argmax_last: the pool's winner is the last maximum.
+    `arg` of x1 moves down one row (zero row on top); argmax_last: the pool's winner is the last maximum.  With masks:
+    drop_grad_unmasked: the gradient of x3 is not multiplied by keep * 1.25; drop_stage3_shift: the stage-3 mask of
+    the next pair (arg "pair") or channel (arg "channel"), cyclically; drop_input_swap: image_1 and image_2 trade
+    input masks; drop_act_from_x3d: act' of x3's gradient is taken from x3d (relu cannot see it).
+    masks: (keep_input [B, 8, H, W], keep_stage3 [B, 256]) 0 / 1 (dropout_masks), or None for no dropout.
     trace: a dict the design checks fill -- "fwd" / "bwd": (name, tensor) of every store, "relu": (name, fraction of
     relu' = 1), "conv": {conv index: (input, output, stride)}."""
     blocks, _ = plan(layers)
@@ -221,7 +268,15 @@ def trunk(img1, img2, filters, layers, act, hooks=True, saving=True, bwd_round=F
             y.retain_grad()
         return y
 
-    x = opt.store(trunk_input(img1, img2, hooks), "input", lambda v: v)
+    keep_in = keep3 = None
+    if masks is not None:
+        keep_in, keep3 = masks
+        if name == "drop_input_swap":
+            keep_in = torch.cat((keep_in[:, 4:], keep_in[:, :4]), dim=1)
+        if name == "drop_stage3_shift":
+            keep3 = torch.roll(keep3, -1, dims=0 if arg == "pair" else 1)
+    x3_block = max(i for i, b in enumerate(blocks) if b.stage == 2)
+    x = opt.store(trunk_input(img1, img2, hooks, keep_in), "input", lambda v: v)
     z = run_conv(x, 0, (1, 2))
     if saving:
         z = opt.store(z, "stem", fp16 if img1.shape[-1] % 2 == 0 else bf16)
@@ -236,6 +291,8 @@ def trunk(img1, img2, filters, layers, act, hooks=True, saving=True, bwd_round=F
     for i, b in enumerate(blocks):
         if b.index == 0 and b.stage > 0 and teacher is not None:
             cur = cur + (teacher[b.stage - 1].to(cur) - cur).detach()
+        if keep3 is not None and i == x3_block + 1:
+            cur = opt.store(_Drop3.apply(cur, keep3, hooks), "x3d", lambda v: v)
         t1 = opt.activation(_GradStore.apply(run_conv(cur, b.c1, b.stride), f"dz1[{i}]", opt), f"t1[{i}]")
         ident = cur
         if b.ds >= 0:
@@ -244,7 +301,8 @@ def trunk(img1, img2, filters, layers, act, hooks=True, saving=True, bwd_round=F
             else:
                 ident = opt.store(run_conv(_GradStore.apply(cur, f"gds[{i}]", opt), b.ds, b.stride), f"ds[{i}]")
         pre = run_conv(t1, b.c2, (1, 1)) + ident
-        cur = opt.activation(_GradStore.apply(pre, f"dz2[{i}]", opt), f"out[{i}]")
+        drop = (keep3, opt, name) if keep3 is not None and i == x3_block else None
+        cur = opt.activation(_GradStore.apply(pre, f"dz2[{i}]", opt), f"out[{i}]", drop)
         if i + 1 == len(blocks) or blocks[i + 1].stage != b.stage:
             if name == "shift_pair" and b.stage == 0:
                 cur = torch.cat((cur[:arg], F.pad(cur[arg:arg + 1, :, :-1], (0, 0, 1, 0)), cur[arg + 1:]))
@@ -297,10 +355,18 @@ DW_AXES = ("out", "in")
 
 
 # ------------------------------------------------------------------------------------------------ exact-tier designs
-Design = collections.namedtuple("Design", "layers B H W img1 img2 filters g_pooled x pooled dw stats")
-BF16_INT_MAX = 256            # every integer of magnitude <= 256 is a bf16
-FP16_INT_MAX = 2048
+Design = collections.namedtuple("Design", "layers B H W img1 img2 filters g_pooled x pooled dw stats counter masks")
 SUM_MAX = 2 ** 24             # fp32 adds integers below this exactly, in any order
+
+
+def dropout_masks(seed, step, B, H, W, device="cpu"):
+    """The training step's input and stage-3 keep masks at (seed, step) from the numpy generator -> (keep_input
+    [B, 8, H, W], keep_stage3 [B, 256]) float64 0 / 1."""
+    import numpy as np
+    from dropout_reference import INPUT, STAGE3, keep_mask
+    k_in = keep_mask(seed, step, INPUT, B * 8 * H * W).reshape(B, 8, H, W)
+    k3 = keep_mask(seed, step, STAGE3, B * WIDTHS[2]).reshape(B, WIDTHS[2])
+    return tuple(torch.from_numpy(k.astype(np.float64)).to(device) for k in (k_in, k3))
 
 
 def _taps(g, cout, cin, k, per_out, sign, keep=1.0):
@@ -317,11 +383,12 @@ def _taps(g, cout, cin, k, per_out, sign, keep=1.0):
     return w.view(cout, cin, k, k)
 
 
-def _is_int(t, bound):
-    return bool((t == t.round()).all()) and t.abs().max().item() <= bound
+def _exact_in(t, fn):
+    """Every element an integer that the storage type (fn: bf16 or fp16) represents exactly."""
+    return bool((t == t.round()).all()) and torch.equal(fn(t), t)
 
 
-def exact_design(layers, B, H, W, device="cpu", seed=0):
+def exact_design(layers, B, H, W, device="cpu", seed=0, counter=None):
     """An integer design for the exact tier and its float64 reference, with its premises asserted:
     - images of integers in [-2, 2] (the even-W layout's residual channels are exactly 0);
     - the stem and conv1 with +-1 taps of mixed sign, conv2 with -1 taps only and the downsample one +1 tap per output
@@ -329,13 +396,20 @@ def exact_design(layers, B, H, W, device="cpu", seed=0):
       stays a small integer; conv2 is zero from the third block of a stage on (an identity block), so the data
       gradients of deep plans stay within bf16's integers too;
     - g_pooled = k h4 w4 with k in [-2, 2]: the average pool's backward (fp32 g * (1 / (h4 w4)), bf16) gives exactly k.
-    Asserted: every bf16 store an integer of magnitude <= 256, every fp16 stem value <= 2048, every partial sum of the
-    forward, data-gradient and weight-gradient convolutions below 2^24, each relu' both 0 and 1 on >= 1 % of its
-    elements, every stage output nonzero.  stats: the relu' fractions and the filters with a nonzero gradient."""
+    counter (step, seed): the input and stage-3 dropouts of a training step at that counter (dropout_masks).  Then the
+    images are 16 x [-2, 2] and k is 4 x [-2, 2]: the trunk has no biases and relu is homogeneous, so every value before
+    x3d is a multiple of 20 (the masked input is 20 x [-2, 2]) and 1.25 x3 an integer, and every data gradient at x3d
+    is a multiple of 4, so that keep * 1.25 times it is one too.
+    Asserted: every bf16 store (and x3d, and the gradient of x3 before its mask) an integer that bf16 represents exactly,
+    every stem value one that fp16 does on the 16-channel route, every partial sum of the forward, data-gradient and
+    weight-gradient convolutions below 2^24, each relu' both 0 and 1 on >= 1 % of its elements, every stage output
+    nonzero.  stats: the relu' fractions and the filters with a nonzero gradient."""
     import zlib
-    g = torch.Generator().manual_seed(zlib.crc32(repr((tuple(layers), B, H, W, seed)).encode()))
+    key = (tuple(layers), B, H, W, seed) if counter is None else (tuple(layers), B, H, W, seed, tuple(counter))
+    g = torch.Generator().manual_seed(zlib.crc32(repr(key).encode()))
     blocks, convs = plan(layers)
-    img = torch.randint(-2, 3, (2, B, 4, H, W), generator=g).float()
+    scale, gscale = (1, 1) if counter is None else (16, 4)
+    img = torch.randint(-2, 3, (2, B, 4, H, W), generator=g).float() * scale
     filters = [None] * len(convs)
     filters[0] = _taps(g, 64, 8, 3, 3, 0)
     for b in blocks:
@@ -344,25 +418,27 @@ def exact_design(layers, B, H, W, device="cpu", seed=0):
         if b.ds >= 0:
             filters[b.ds] = _taps(g, b.cout, b.cin, 1, 1, 1)
     h4, w4 = stage_sizes(H, W)[3]
-    k = torch.randint(-2, 3, (B, 512), generator=g).double()
+    k = torch.randint(-2, 3, (B, 512), generator=g).double() * gscale
     g_pooled = (k * (h4 * w4)).float()
     # the average pool's backward: bf16(g * fp32(1 / (h4 w4))) must be k itself
     inv = torch.tensor(1.0, dtype=torch.float32) / torch.tensor(float(h4 * w4), dtype=torch.float32)
     assert torch.equal(bf16(g_pooled * inv).double(), k), "avgpool backward does not give back k"
 
     img1, img2 = img[0].to(device), img[1].to(device)
+    masks = None if counter is None else dropout_masks(counter[1], counter[0], B, H, W, device)
     fs = [w.to(device).requires_grad_(True) for w in filters]
     trace = {}
     with torch.backends.cudnn.flags(enabled=False):
-        out = trunk(img1, img2, fs, layers, "relu", hooks=True, saving=True, bwd_round=True, trace=trace)
+        out = trunk(img1, img2, fs, layers, "relu", hooks=True, saving=True, bwd_round=True, trace=trace, masks=masks)
         out["pooled"].backward(g_pooled.to(device).double())
-    label = f"design {tuple(layers)} B={B} {H}x{W}"
+    label = f"design {tuple(layers)} B={B} {H}x{W}" + ("" if counter is None else f" counter {counter}")
     for name, t in trace["fwd"]:
-        bound = FP16_INT_MAX if name == "stem" and W % 2 == 0 else BF16_INT_MAX
-        assert _is_int(t, bound), f"{label}: forward store {name} is not an integer within {bound}"
+        fn = fp16 if name == "stem" and W % 2 == 0 else bf16
+        assert _exact_in(t, fn), f"{label}: forward store {name} max {t.abs().max().item()} is not an integer " \
+                                 f"exact in {fn.__name__}"
     for name, t in trace["bwd"]:
-        assert _is_int(t, BF16_INT_MAX), f"{label}: backward store {name} max {t.abs().max().item()} is not an " \
-                                         f"integer within {BF16_INT_MAX}"
+        assert _exact_in(t, bf16), f"{label}: backward store {name} max {t.abs().max().item()} is not an integer " \
+                                   f"exact in bf16"
     for c, (x, y, stride) in trace["conv"].items():
         w = fs[c].detach()
         taps = (w != 0).flatten(1).sum(1).max().item()
@@ -387,8 +463,13 @@ def exact_design(layers, B, H, W, device="cpu", seed=0):
         assert xs.abs().max().item() > 0, f"{label}: x{s + 1} is zero"
     dw = [w.grad.detach() for w in fs]
     stats = {"relu": fractions, "nonzero_dw": [c for c, d in enumerate(dw) if d.abs().max().item() > 0]}
+    # the trace's graph tensors and the autograd contexts that hold the trace form reference cycles: release them now,
+    # or a matrix of designs in one process keeps every design's graph until a full garbage collection
+    trace.clear()
+    total = out["x"][3].detach().sum(dim=(2, 3))
+    assert bool((total.abs() < SUM_MAX).all()), f"{label}: the average pool's sums reach 2^24"
     return Design(tuple(layers), B, H, W, img1, img2, [w.detach() for w in fs], g_pooled.to(device),
-                  [t.detach() for t in out["x"]], out["pooled"].detach(), dw, stats)
+                  [t.detach() for t in out["x"]], out["pooled"].detach(), dw, stats, counter, masks)
 
 
 def dw_coverage(layers, nonzero):
