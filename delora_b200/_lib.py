@@ -209,6 +209,10 @@ SIGNATURES = {
                                                               c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                                               c_void_p]),
     "delora_odometry_streams_adapt_geometries_reset": (c_int, [c_desc_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_streams_adapt_geometries_info_workspace_bytes": (c_i64, [c_desc_p, c_int]),
+    "delora_odometry_streams_push_adapt_geometries_info": (c_int, [c_desc_p, c_int, c_train_p, c_int, c_void_p,
+                                                                   c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                                   c_void_p, c_void_p, c_void_p]),
     "delora_odometry_train_set_dropout_seed":(c_int, [c_desc_p, ctypes.c_uint64, c_void_p, c_void_p]),
     "delora_dropout_keep_mask": (c_int, [ctypes.c_uint64, c_i64, c_int, c_i64, c_void_p, c_void_p]),
 }

@@ -2706,7 +2706,8 @@ extern "C" int delora_odometry_streams_adapt_reset(const delora_odometry_desc* d
 // g's counters at +8 + 24 (g - 1), in the layout of the model section's (int64 [3]: a backward count nothing reads,
 // the batch marker of g's ICP scratch, unused).  Geometry g's plan keeps d[0]'s model-section offsets (check_geometries
 // makes them equal) with grad and ctr moved to its slice and counters, so train_forward_losses and step_backward run
-// on it unchanged, and geometry 0's plan is _push_adapt's.
+// on it unchanged, and geometry 0's plan is _push_adapt's.  The _adapt_geometries_info form appends the information
+// section after all of that (see make_geometries_plan), so no other offset moves.
 namespace delora {
 
 struct GeometriesPlan {
@@ -2715,6 +2716,7 @@ struct GeometriesPlan {
     int row[kMaxGeometries];           // the first stream of geometry g in the caller's arrays
     size_t fleet;                      // n > 1 only
     size_t total;
+    size_t info_total;                 // with the information section of _push_adapt_geometries_info
 };
 
 // TrainPlan is large (the trunk plan's tables): the plans of up to kMaxGeometries geometries go on the heap
@@ -2735,6 +2737,22 @@ static std::unique_ptr<GeometriesPlan> make_geometries_plan(const delora_odometr
         for (int g = 1; g < n; ++g) p->tp[g].ctr = p->fleet + 8 + 24 * (size_t)(g - 1);
     }
     p->total = off;
+    // the information section of _push_adapt_geometries_info: the rows of all S_total pairs, then one info_scratch
+    // sized for the largest geometry (their ICPs run one after another on one stream, and the scratch needs no
+    // initialisation).  make_adapt_plan put ap.info / ap.info_scratch after a single-geometry group section, which here
+    // lies in the next geometry's sections: every geometry's, g = 0 included, are moved into this section
+    const size_t rows = take(off, (size_t)(p->row[n - 1] + d[n - 1].max_batch) * DELORA_INFO_ROW * 4);
+    int64_t scratch = 0;
+    for (int g = 0; g < n; ++g) {
+        const int64_t floats = delora_icp_information_scratch_floats(d[g].max_batch, d[g].H, d[g].W);
+        if (floats > scratch) scratch = floats;
+    }
+    const size_t info_scratch = take(off, (size_t)scratch * 4);
+    for (int g = 0; g < n; ++g) {
+        p->ap[g].info = rows + (size_t)p->row[g] * DELORA_INFO_ROW * 4;
+        p->ap[g].info_scratch = info_scratch;
+    }
+    p->info_total = off;
     return p;
 }
 
@@ -2755,10 +2773,12 @@ __global__ void odometry_fleet_count_kernel(FleetCounts c, int32_t* __restrict__
     *fleet = s;
 }
 
+// One tick of _push_adapt_geometries; info non-NULL: of _push_adapt_geometries_info, each geometry's information rows
+// into its rows of info
 static int push_adapt_geometries(const delora_odometry_desc* d, int n, const delora_odometry_train_params* hp,
                                  int update, const float* const* points, const int32_t* const* n_points,
                                  const int32_t* active, void* workspace, float* T, int32_t* valid, float* losses,
-                                 void* stream, const char* who) {
+                                 float* info, void* stream, const char* who) {
     const std::unique_ptr<GeometriesPlan> p = make_geometries_plan(d, n);
     cudaStream_t st = (cudaStream_t)stream;
     char* ws = (char*)workspace;
@@ -2767,8 +2787,8 @@ static int push_adapt_geometries(const delora_odometry_desc* d, int n, const del
     for (int g = 0; g < n; ++g) {
         const int r = p->row[g];
         if ((rc = serve_adapt(&d[g], hp, p->tp[g], p->ap[g], update, points[g], n_points[g], active ? active + r : nullptr,
-                              ws, T + (size_t)r * 16, valid + r, losses + (size_t)r * DELORA_LOSS_ROW, nullptr, st,
-                              who)))
+                              ws, T + (size_t)r * 16, valid + r, losses + (size_t)r * DELORA_LOSS_ROW,
+                              info ? info + (size_t)r * DELORA_INFO_ROW : nullptr, st, who)))
             return rc;
     }
     if (!update) return 0;
@@ -2821,13 +2841,12 @@ extern "C" int delora_odometry_streams_adapt_geometries_init(const delora_odomet
     return 0;
 }
 
-extern "C" int delora_odometry_streams_push_adapt_geometries(const delora_odometry_desc* d, int n,
-                                                             const delora_odometry_train_params* hp, int update,
-                                                             const float* const* points,
-                                                             const int32_t* const* n_points, const int32_t* active,
-                                                             void* workspace, float* T, int32_t* valid, float* losses,
-                                                             void* stream) {
-    const char* who = "delora_odometry_streams_push_adapt_geometries";
+namespace delora {
+
+// What _push_adapt_geometries and _push_adapt_geometries_info refuse alike
+static int check_push_adapt_geometries(const delora_odometry_desc* d, int n, const delora_odometry_train_params* hp,
+                                       int update, const float* const* points, const int32_t* const* n_points,
+                                       void* workspace, float* T, int32_t* valid, float* losses, const char* who) {
     if (check_adapt_geometries(d, n, who)) return 1;
     if (check_adapt_params(hp, update, who)) return 1;
     DELORA_CHECK_ARG(points, "%s: null points", who);
@@ -2843,7 +2862,40 @@ extern "C" int delora_odometry_streams_push_adapt_geometries(const delora_odomet
         snprintf(w, sizeof w, "%s: d[%d]", who, g);
         if (check_train_call(&d[g], hp, points[g], n_points[g], d[g].max_batch, workspace, w)) return 1;
     }
-    return push_adapt_geometries(d, n, hp, update, points, n_points, active, workspace, T, valid, losses, stream, who);
+    return 0;
+}
+
+}  // namespace delora
+
+extern "C" int delora_odometry_streams_push_adapt_geometries(const delora_odometry_desc* d, int n,
+                                                             const delora_odometry_train_params* hp, int update,
+                                                             const float* const* points,
+                                                             const int32_t* const* n_points, const int32_t* active,
+                                                             void* workspace, float* T, int32_t* valid, float* losses,
+                                                             void* stream) {
+    const char* who = "delora_odometry_streams_push_adapt_geometries";
+    if (check_push_adapt_geometries(d, n, hp, update, points, n_points, workspace, T, valid, losses, who)) return 1;
+    return push_adapt_geometries(d, n, hp, update, points, n_points, active, workspace, T, valid, losses, nullptr,
+                                 stream, who);
+}
+
+extern "C" int64_t delora_odometry_streams_adapt_geometries_info_workspace_bytes(const delora_odometry_desc* d, int n) {
+    if (check_adapt_geometries(d, n, "delora_odometry_streams_adapt_geometries_info_workspace_bytes")) return -1;
+    return (int64_t)make_geometries_plan(d, n)->info_total;
+}
+
+extern "C" int delora_odometry_streams_push_adapt_geometries_info(const delora_odometry_desc* d, int n,
+                                                                  const delora_odometry_train_params* hp, int update,
+                                                                  const float* const* points,
+                                                                  const int32_t* const* n_points,
+                                                                  const int32_t* active, void* workspace, float* T,
+                                                                  int32_t* valid, float* losses, float* info,
+                                                                  void* stream) {
+    const char* who = "delora_odometry_streams_push_adapt_geometries_info";
+    if (check_push_adapt_geometries(d, n, hp, update, points, n_points, workspace, T, valid, losses, who)) return 1;
+    DELORA_CHECK_ARG(info, "%s: null info", who);
+    return push_adapt_geometries(d, n, hp, update, points, n_points, active, workspace, T, valid, losses, info, stream,
+                                 who);
 }
 
 extern "C" int delora_odometry_streams_adapt_geometries_reset(const delora_odometry_desc* d, int n, const int32_t* mask,

@@ -367,14 +367,14 @@ class GeometriesAdaptingStreamsWorkspace(TrainingWorkspace):
     one workspace.  Geometry g serves descs[g].max_batch streams; streams are numbered in geometry order
     (`n_streams` in all).  Every TrainingWorkspace call runs with descs[0] (weights, get_state / set_state) and leaves
     the stream sections alone; `params` from train_params (without use_dropout)."""
+    GEOMETRIES_SIZE_QUERY = "delora_odometry_streams_adapt_geometries_workspace_bytes"
 
-    @staticmethod
-    def shared_bytes(descs):
-        """delora_odometry_streams_adapt_geometries_workspace_bytes; ValueError with the C side's message when it
-        refuses."""
+    @classmethod
+    def shared_bytes(cls, descs):
+        """The kind's size query over descs; ValueError with the C side's message when it refuses."""
         L = _lib.lib()
         arr = (_lib.OdometryDesc * len(descs))(*descs)
-        nbytes = int(L.delora_odometry_streams_adapt_geometries_workspace_bytes(arr, len(arr)))
+        nbytes = int(getattr(L, cls.GEOMETRIES_SIZE_QUERY)(arr, len(arr)))
         if nbytes < 0:
             raise ValueError(L.delora_last_error().decode())
         return nbytes
@@ -413,6 +413,22 @@ class GeometriesAdaptingStreamsWorkspace(TrainingWorkspace):
         """Forget the previous frame of every stream with mask[s] != 0 (device int32 [n_streams])."""
         self._geometries_call("delora_odometry_streams_adapt_geometries_reset", mask.data_ptr(),
                               self.workspace.data_ptr())
+
+
+class GeometriesAdaptingInformationStreamsWorkspace(GeometriesAdaptingStreamsWorkspace):
+    """delora_odometry_streams_adapt_geometries_info_*: the geometries layout of the adapting streams with the
+    information section appended; every GeometriesAdaptingStreamsWorkspace call works on it.  `push` takes info
+    [n_streams, INFO_ROW] out after losses: the information row at the served T (before the tick's update) of every
+    valid stream, in the metres and radians of T for normalised models too; zeros elsewhere."""
+    GEOMETRIES_SIZE_QUERY = "delora_odometry_streams_adapt_geometries_info_workspace_bytes"
+
+    def push(self, points, counts, active, T, valid, losses, info, update=True):
+        n = len(self.descs)
+        pts = (ctypes.c_void_p * n)(*(p.data_ptr() for p in points))
+        cnt = (ctypes.c_void_p * n)(*(c.data_ptr() for c in counts))
+        self._geometries_call("delora_odometry_streams_push_adapt_geometries_info", self._params,
+                              1 if update else 0, pts, cnt, _ptr(active), self.workspace.data_ptr(), T.data_ptr(),
+                              valid.data_ptr(), losses.data_ptr(), info.data_ptr())
 
 
 class TrainingGroup:

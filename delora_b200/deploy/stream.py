@@ -490,10 +490,14 @@ class GeometriesAdaptiveOdometryStreams(AdaptiveOdometryStreams):
     section of `config` with its own image size, vertical field of view and preprocessing width; streams are numbered
     in that order.  One tick serves every geometry's streams, and with update=True takes one Adam step on the mean
     objective over the pairs of all of them, so one model adapts to the whole fleet.  The datasets must share the
-    parity of their horizontal_cells.  `push`, `poses`, `reset` and `state_dict` are AdaptiveOdometryStreams'."""
+    parity of their horizontal_cells.  `push`, `poses`, `reset` and `state_dict` are AdaptiveOdometryStreams'.
+
+    information=True serves them from the geometries information workspace
+    (`delora_odometry_streams_push_adapt_geometries_info`): each entry is then (T, losses, info [INFO_ROW]), as for
+    AdaptiveOdometryStreams(information=True).  T, losses and the adapted model are the same bits either way."""
 
     def __init__(self, model, config, geometries, n_max, lr, preprocessing_normals=False,
-                 loss_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL):
+                 loss_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL, information=False):
         from . import capi, export
         if config.get("use_dropout", False):
             raise ValueError("use_dropout: True is not supported by GeometriesAdaptiveOdometryStreams: the served "
@@ -510,14 +514,17 @@ class GeometriesAdaptiveOdometryStreams(AdaptiveOdometryStreams):
                       for ds, s in geometries]
         self.rows = np.cumsum([0] + [int(s) for _, s in geometries]).tolist()
         self.n_streams = self.rows[-1]
+        self.information = bool(information)
         with torch.cuda.device(self.device):
             blob = torch.from_numpy(export.pack_state_dict(model.state_dict(), config)).to(self.device)
-            self.workspace = capi.GeometriesAdaptingStreamsWorkspace(
-                self.descs, blob, capi.train_params(config, lr, loss_flags=loss_flags))
+            kind = (capi.GeometriesAdaptingInformationStreamsWorkspace if self.information
+                    else capi.GeometriesAdaptingStreamsWorkspace)
+            self.workspace = kind(self.descs, blob, capi.train_params(config, lr, loss_flags=loss_flags))
         self._buffers()
 
     def _push_device(self, update):
         r = self.rows
         pts = [self.points[r[g]:r[g + 1]] for g in range(len(self.descs))]
         counts = [self.counts[r[g]:r[g + 1]] for g in range(len(self.descs))]
-        self.workspace.push(pts, counts, self.active, self.T, self.valid, self.losses, update)
+        extras = (self.info,) if self.information else ()
+        self.workspace.push(pts, counts, self.active, self.T, self.valid, self.losses, *extras, update=update)

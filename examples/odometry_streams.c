@@ -4,8 +4,8 @@
  *
  *   odometry_streams [--residual | --information | --preprocessing [--information]] model.dlw stream0_dir ...
  *   odometry_streams --adapt LR --adapt-out adapted.dlw [--gpus N] [--information] model.dlw stream0_dir ...
- *   odometry_streams --adapt LR --adapt-out adapted.dlw [--geometry DIR,H,W,VFOV0,VFOV1[,W_PRE]]... model.dlw
- *                    stream0_dir ...
+ *   odometry_streams --adapt LR --adapt-out adapted.dlw [--geometry DIR,H,W,VFOV0,VFOV1[,W_PRE]]... [--information]
+ *                    model.dlw stream0_dir ...
  *
  * model.dlw is written by bin/export_odometry_weights.py (layout: include/delora_b200.h); every directory holds one
  * stream's KITTI velodyne .bin files ([N, 4] float32 rows: x, y, z, reflectance), taken in name order.  All streams
@@ -20,10 +20,11 @@
  * eigenvalue, its unit eigenvector (x, y, z, rot x, rot y, rot z: the direction the frame constrains least) and the
  * ratio of the largest eigenvalue to the smallest (large in a corridor, an open field or at a flat wall).
  * --information with --preprocessing (delora_odometry_streams_push_pre_info) or with --adapt, --gpus included
- * (delora_odometry_streams_push_adapt_info / _push_adapt_group_info) appends the same three columns to those modes'
- * lines, for plain and normalization_scaling files alike: the information is always in the metres and radians of the
- * printed T.  The transforms, residual columns and adapted weights are the same bits as without it.  Options may come
- * in any order before model.dlw; --information does not combine with --geometry.
+ * (delora_odometry_streams_push_adapt_info / _push_adapt_group_info) or with --adapt and --geometry
+ * (delora_odometry_streams_push_adapt_geometries_info, every stream of every sensor) appends the same three columns to
+ * those modes' lines, for plain and normalization_scaling files alike: the information is always in the metres and
+ * radians of the printed T.  The transforms, residual columns and adapted weights are the same bits as without it.
+ * Options may come in any order before model.dlw.
  * A model trained with normalization_scaling (model_flags has DELORA_MODEL_NORMALIZATION_SCALING) is served through
  * delora_odometry_streams_push_normalized, with the same output; --residual is refused for such a model.
  * --preprocessing serves the streams on the reference's two-resolution recipe through delora_odometry_streams_push_pre:
@@ -468,7 +469,6 @@ int main(int argc, char** argv) {
     }
     if (adapt && (residual_opt || pre)) return fail("--adapt serves its own residual: drop --residual / --preprocessing");
     if (residual_opt && pre) return fail("--preprocessing serves its own residual: drop --residual");
-    if (information && n_geom) return fail("--information does not combine with --geometry");
     /* the raw-scan residual streams: --residual, or --information on its own */
     const int residual = residual_opt || (information && !pre && !adapt);
     if (argc < 3)
@@ -552,7 +552,9 @@ int main(int argc, char** argv) {
     rp.min_neighbors = 10;
     int32_t *count, *active, *valid;
     void* workspace;
-    const int64_t ws_bytes = n_geom       ? delora_odometry_streams_adapt_geometries_workspace_bytes(descs, n_sets)
+    const int64_t ws_bytes = n_geom && information
+                                 ? delora_odometry_streams_adapt_geometries_info_workspace_bytes(descs, n_sets)
+                             : n_geom     ? delora_odometry_streams_adapt_geometries_workspace_bytes(descs, n_sets)
                              : adapt && information ? delora_odometry_streams_adapt_info_workspace_bytes(d)
                              : adapt      ? delora_odometry_streams_adapt_workspace_bytes(d)
                              : pre && information ? delora_odometry_streams_pre_info_workspace_bytes(d)
@@ -618,7 +620,11 @@ int main(int argc, char** argv) {
         CUDA_OK(cudaMemcpyAsync(count, h_count, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
         CUDA_OK(cudaMemcpyAsync(active, h_active, (size_t)S * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
         if (adapt || pre || residual) {
-            if (n_geom)
+            if (n_geom && information)
+                DELORA_OK(delora_odometry_streams_push_adapt_geometries_info(descs, n_sets, &hp, 1, g_points, g_count,
+                                                                             active, workspace, T, valid, losses, info,
+                                                                             stream));
+            else if (n_geom)
                 DELORA_OK(delora_odometry_streams_push_adapt_geometries(descs, n_sets, &hp, 1, g_points, g_count, active,
                                                                         workspace, T, valid, losses, stream));
             else if (adapt && information)

@@ -1277,7 +1277,8 @@ int delora_odometry_streams_push_adapt_group(const delora_odometry_desc* d, cons
  * H x W grids and T's 3x4 in the model's units: delora_icp_dense_information for a plain model,
  * delora_icp_dense_information_scaled with the pair's factor for a DELORA_TRAIN_NORMALIZATION_SCALING one, so H is in
  * the metres and radians of the served T.  Rows with valid[s] = 0 are zeros.  Refused before any launch: what
- * _push_adapt (_push_adapt_group) refuses, and a null info.  Out of scope: _push_adapt_geometries.
+ * _push_adapt (_push_adapt_group) refuses, and a null info.  The information of the adapting streams of several
+ * geometries: delora_odometry_streams_push_adapt_geometries_info below.
  * Measured on one H100 80GB HBM3 at a 700 W power limit (max SM clock 1980 MHz), graph-replayed update = 1 ticks,
  * lr 0, w_pre 0, all streams active, medians of alternating samples, _push_adapt -> _push_adapt_info per tick:
  * 64 x 2048: S = 1 3.73 -> 3.79 ms, S = 4 6.69 -> 6.77 ms, S = 16 23.05 -> 23.19 ms; 64 x 720: S = 1 3.54 -> 3.57 ms,
@@ -1407,6 +1408,45 @@ int delora_odometry_streams_push_adapt_geometries(const delora_odometry_desc* d,
                                                   float* losses, void* stream);
 int delora_odometry_streams_adapt_geometries_reset(const delora_odometry_desc* d, int n, const int32_t* mask,
                                                    void* workspace, void* stream);
+
+/* ---- The same adapting streams of several geometries with the information of each frame's residual: the
+ * Gauss-Newton information of the tick's ICP objective at the served T, as _push_adapt_info serves it for one geometry.
+ *
+ * Workspace: the _adapt_geometries workspace of (d, n), unchanged, followed by one information section: the rows of
+ * all S_total pairs in fleet stream order, then one info_scratch of max_g delora_icp_information_scratch_floats(S_g,
+ * H_g, W_g) floats, each 256-byte aligned.  The geometries' ICPs run one after another on one stream, so they share
+ * that scratch.  No other offset moves: delora_odometry_streams_adapt_geometries_init (which leaves the information
+ * section as it was: every row is written before it is read, and the scratch needs no initialisation) and _reset,
+ * _push_adapt_geometries itself and the delora_odometry_train_* calls listed above work on it unchanged.
+ * delora_odometry_streams_adapt_geometries_info_workspace_bytes: host only; -1 (and delora_last_error()) for every set
+ * _adapt_geometries_workspace_bytes refuses, with the same message.
+ *
+ * delora_odometry_streams_push_adapt_geometries_info: the arguments of _push_adapt_geometries plus info [S_total,
+ * DELORA_INFO_ROW] (device, required), in fleet stream order.  Each geometry's ICP is the information operator in place
+ * of delora_icp_dense_fwd_bwd (delora_icp_dense_information, or delora_icp_dense_information_scaled with the pair's
+ * factor for DELORA_TRAIN_NORMALIZATION_SCALING), whose losses and dL/dT are the same bits.  So:
+ *   - T, valid, the loss rows and the model after the tick (weights, Adam's m, v and step count, the gradient section)
+ *     are _push_adapt_geometries's bytes over the same ticks;
+ *   - where valid[s] = 1, info[s] is bit for bit the row a _push_adapt_info workspace of d[g] holding the same weights
+ *     writes: the operator's row at B = 1, in the metres and radians of the served T, before the tick's update;
+ *   - rows with valid[s] = 0 are zeros;
+ *   - with n = 1 every output is _push_adapt_info's bytes.
+ * Only launches, with a sequence that depends on neither `active`, the stream state nor the counts: one captured graph
+ * per value of `update` serves every tick.  Refused before any launch: everything _push_adapt_geometries refuses, and a
+ * null info.  Out of scope: geometries across several GPUs.
+ * Cost, measured on one H100 80GB HBM3 at a 700 W power limit (max SM clock 1980 MHz), graph-replayed ticks, all
+ * streams active, near-identity heads, lr 0, medians of 7 alternating samples, 64 x 720 (w_pre 2250) + 64 x 512
+ * (w_pre 512), _push_adapt_geometries -> _push_adapt_geometries_info per tick:
+ *   S_g = 1: update = 0 2.39 -> 2.46 ms (paired difference +0.066 ms), update = 1 6.75 -> 6.82 ms (+0.067 ms);
+ *   S_g = 4: update = 0 2.71 -> 2.79 ms (+0.073 ms), update = 1 8.14 -> 8.21 ms (+0.073 ms);
+ * the workspace grows by 0.5 / 2.1 MiB (scripts/gpu_odometry_streams_adapt_geometries_info.py,
+ * profiles/odometry_streams_adapt_geometries_info_h100_700w.json). */
+int64_t delora_odometry_streams_adapt_geometries_info_workspace_bytes(const delora_odometry_desc* d, int n);   /* host only */
+int delora_odometry_streams_push_adapt_geometries_info(const delora_odometry_desc* d, int n,
+                                                       const delora_odometry_train_params* hp, int update,
+                                                       const float* const* points, const int32_t* const* n_points,
+                                                       const int32_t* active, void* workspace, float* T, int32_t* valid,
+                                                       float* losses, float* info, void* stream);
 
 #ifdef __cplusplus
 }
