@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdelora_b200.so")
-SOURCES = ["api.cu", "projection.cu", "normals.cu", "lists.cu", "icp.cu", "icp_dense.cu", "icp_info.cu", "sort.cu", "conv_tc.cu", "conv_rows.cu", "conv_wgrad.cu", "conv_stem.cu", "grad_allreduce.cu", "trunk.cu", "odometry.cu"]
+SOURCES = ["api.cu", "projection.cu", "normals.cu", "lists.cu", "icp.cu", "icp_dense.cu", "icp_info.cu", "sort.cu", "conv_tc.cu", "conv_rows.cu", "conv_wgrad.cu", "conv_stem.cu", "grad_allreduce.cu", "trunk.cu", "odometry.cu", "odometry_tail.cu", "odometry_streams.cu", "odometry_train.cu", "odometry_adapt.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + [ "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xptxas=-v"]

@@ -1,6 +1,6 @@
 // The encoder trunk (ResNetModified up to its average pool), decided once: the conv/block plan, the bf16 weight section,
 // the activation buffers and the launch sequences of its forward and backward.  The odometry entry points
-// (odometry.cu) and the delora_trunk_* entry points that models/tc_encoder.py calls both run it.
+// (odometry*.cu) and the delora_trunk_* entry points that models/tc_encoder.py calls both run it.
 #pragma once
 #include <stddef.h>
 #include <stdint.h>

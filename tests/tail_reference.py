@@ -1,5 +1,5 @@
 """Float64 restatement of the odometry tail (resnet.fc, the heads, quaternion -> T, their backward) and of Adam, each
-with a per-element bound on the error of an fp32 implementation that follows odometry.cu's arithmetic (test
+with a per-element bound on the error of an fp32 implementation that follows odometry_tail.cu's arithmetic (test
 infrastructure, imported like helpers).
 
 The bounds are a running error analysis, with u = 2^-24 and gamma_d = d u / (1 - d u):

@@ -1,4 +1,4 @@
-"""The odometry tail's kernels (odometry.cu: resnet.fc and the heads, the block-normalised quaternion -> T, their
+"""The odometry tail's kernels (odometry_tail.cu: resnet.fc and the heads, the block-normalised quaternion -> T, their
 backward, Adam) against the float64 reference of tail_reference.py, element by element, on the H100.
 
 Teacher forcing: every comparison starts from bits the GPU returns, so that only the tail is under test.  pooled comes
