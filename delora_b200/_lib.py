@@ -45,6 +45,19 @@ class OdometryTrainGroup(ctypes.Structure):
                 ("side_stream", c_void_p), ("fork_events", c_void_p * TRAIN_GROUP_BUCKETS), ("join_event", c_void_p)]
 
 
+class WsSection(ctypes.Structure):
+    """delora_ws_section (include/delora_b200.h): one section of an odometry workspace's layout."""
+    _fields_ = [("offset", c_i64), ("bytes", c_i64), ("role", ctypes.c_int32), ("geometry", ctypes.c_int32),
+                ("flags", ctypes.c_int32), ("name", ctypes.c_char * 44)]
+
+
+# workspace kinds, section roles and flags of delora_odometry_workspace_sections (DELORA_WS_* in include/delora_b200.h)
+WS_KINDS = ("pairs", "streams", "streams_residual", "streams_info", "streams_normalized", "streams_pre",
+            "streams_pre_info", "train", "train_geometries", "adapt", "adapt_group", "adapt_info", "adapt_geometries",
+            "adapt_geometries_info")
+WS_ROLES = ("weights", "state", "scratch", "output")
+WS_SUBRANGE, WS_SHARED = 1, 2
+
 c_desc_p = ctypes.POINTER(OdometryDesc)
 c_train_p = ctypes.POINTER(OdometryTrainParams)
 c_residual_p = ctypes.POINTER(OdometryResidualParams)
@@ -213,6 +226,7 @@ SIGNATURES = {
     "delora_odometry_streams_push_adapt_geometries_info": (c_int, [c_desc_p, c_int, c_train_p, c_int, c_void_p,
                                                                    c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                                                    c_void_p, c_void_p, c_void_p]),
+    "delora_odometry_workspace_sections": (c_int, [c_int, c_desc_p, c_int, c_void_p, c_int]),
     "delora_odometry_train_set_dropout_seed":(c_int, [c_desc_p, ctypes.c_uint64, c_void_p, c_void_p]),
     "delora_dropout_keep_mask": (c_int, [ctypes.c_uint64, c_i64, c_int, c_i64, c_void_p, c_void_p]),
 }

@@ -6,7 +6,10 @@
 // and the projection; and the entry points of the pairs / push workspace (delora_odometry_pairs, _pairs_normalized,
 // _push).
 #include <math.h>
+#include <stdio.h>
 #include <string.h>
+
+#include <algorithm>
 
 #include "odometry.cuh"
 #include "projection.cuh"
@@ -201,9 +204,139 @@ int load_weights(const InferPlan& p, const float* weights, void* workspace, cuda
     return 0;
 }
 
+// ---------------------------------------------------------------- the section map
+void SectionMap::add(const char* name, size_t off, size_t bytes, int role, int add_flags) {
+    if (n < cap) {
+        delora_ws_section& r = out[n];
+        memset(&r, 0, sizeof(r));
+        r.offset = (int64_t)off;
+        r.bytes = (int64_t)bytes;
+        r.role = role;
+        r.geometry = geometry;
+        r.flags = flags | add_flags;
+        strncpy(r.name, name, sizeof(r.name) - 1);
+    }
+    ++n;
+}
+
+void SectionMap::field(const char* name, size_t off, int role) {
+    for (size_t i = log->off.size(); i-- > 0;)
+        if (log->off[i] == off) return add(name, off, log->bytes[i], role, 0);
+    if (!missing) missing = name;
+}
+
+void SectionMap::range(const char* name, size_t off, size_t bytes, int role) {
+    bool starts = false;
+    for (size_t o : log->off) starts = starts || o == off;
+    add(name, off, bytes, role, starts ? 0 : DELORA_WS_SUBRANGE);
+}
+
+// The buffers of a sub-plan whose fields alias one another (the inference trunk's activations): one record per take()
+// offset in [begin, end), sized by the last take() there
+void SectionMap::span(const char* prefix, size_t begin, size_t end, int role) {
+    std::vector<size_t> offs;
+    for (size_t o : log->off)
+        if (o >= begin && o < end) offs.push_back(o);
+    std::sort(offs.begin(), offs.end());
+    offs.erase(std::unique(offs.begin(), offs.end()), offs.end());
+    char name[64];
+    for (size_t k = 0; k < offs.size(); ++k) {
+        snprintf(name, sizeof name, "%s[%zu]", prefix, k);
+        field(name, offs[k], role);
+    }
+}
+
+// The projection's keys are all ones between calls (each resolve re-arms them): scratch
+void map_frames(SectionMap& s, const Frames& f, bool index_map, bool counts, int prev_role) {
+    s.field("keys", f.keys, DELORA_WS_SCRATCH);
+    if (index_map) s.field("index_map", f.index_map, DELORA_WS_SCRATCH);
+    if (counts) s.field("counts", f.counts, DELORA_WS_SCRATCH);
+    s.field("images", f.images, DELORA_WS_SCRATCH);
+    if (f.prev_image) s.field("prev_image", f.prev_image, prev_role);
+    if (f.has_prev) s.field("has_prev", f.has_prev, DELORA_WS_STATE);
+}
+
+void map_trunk_weights(SectionMap& s, const TrunkPlan& m, const TrunkWeights& w) {
+    char name[32];
+    s.field("trunk.table", w.table, DELORA_WS_WEIGHTS);
+    for (int i = 0; i < m.n_conv; ++i) {
+        snprintf(name, sizeof name, "trunk.fwd[%d]", i);
+        s.field(name, w.w_fwd[i], DELORA_WS_WEIGHTS);
+        if (!w.flip || i == 0) continue;
+        snprintf(name, sizeof name, "trunk.flip[%d]", i);
+        s.field(name, w.w_flip[i], DELORA_WS_WEIGHTS);
+    }
+}
+
+// The inference trunk's activation fields alias by design (each stage's blocks alternate over three buffers): one
+// record per buffer.  hid[0] and hid[1] are the tail's alternating hidden buffers.
+void map_inference(SectionMap& s, const InferPlan& p, int pooled_role) {
+    s.span("trunk.acts", p.t.x_in, p.pooled, DELORA_WS_SCRATCH);
+    s.field("pooled", p.pooled, pooled_role);
+    s.field("fc_out", p.fc_out, DELORA_WS_SCRATCH);
+    s.field("hid[0]", p.hid[0], DELORA_WS_SCRATCH);
+    s.field("hid[1]", p.hid[1], DELORA_WS_SCRATCH);
+    map_trunk_weights(s, p.m.t, p.w);
+    s.field("fc_w", p.fc_w, DELORA_WS_WEIGHTS);
+    s.field("fc_b", p.fc_b, DELORA_WS_WEIGHTS);
+    char name[32];
+    for (int i = 0; i < p.m.n_lin; ++i) {
+        snprintf(name, sizeof name, "lin_w[%d]", i);
+        s.field(name, p.lin_w[i], DELORA_WS_WEIGHTS);
+        snprintf(name, sizeof name, "lin_b[%d]", i);
+        s.field(name, p.lin_b[i], DELORA_WS_WEIGHTS);
+    }
+}
+
+// Arms take_log for one section-map call and disarms it on every return
+struct TakeLogArm {
+    TakeLog log;
+    TakeLogArm() { take_log = &log; }
+    ~TakeLogArm() { take_log = nullptr; }
+};
+
 }  // namespace delora
 
 using namespace delora;
+
+// delora_odometry_workspace_sections: 0 with the number of sections in *count, 1 for a refusal
+static int workspace_sections(int kind, const delora_odometry_desc* d, int n, delora_ws_section* out, int cap,
+                              int* count) {
+    const char* who = "delora_odometry_workspace_sections";
+    DELORA_CHECK_ARG(kind >= 0 && kind < DELORA_WS_KINDS, "%s: kind=%d outside [0, %d)", who, kind, DELORA_WS_KINDS);
+    DELORA_CHECK_ARG(cap >= 0 && (out || cap == 0), "%s: cap=%d with %s out", who, cap, out ? "an" : "a null");
+    const bool geometries = kind == DELORA_WS_TRAIN_GEOMETRIES || kind == DELORA_WS_ADAPT_GEOMETRIES ||
+                            kind == DELORA_WS_ADAPT_GEOMETRIES_INFO;
+    DELORA_CHECK_ARG(geometries || n == 1, "%s: n=%d must be 1 for kind %d", who, n, kind);
+    DELORA_CHECK_ARG(n >= 1 && n <= kMaxGeometries, "%s: n=%d outside [1, %d]", who, n, kMaxGeometries);
+    TakeLogArm arm;
+    SectionMap s{&arm.log, out, cap, 0, 0, 0, nullptr};
+    int rc = 0;
+    if (kind == DELORA_WS_PAIRS) {
+        if (check_desc(d, who)) return 1;
+        InferPlan p;
+        make_infer_plan(d, &p);
+        // _push's cached image carries over to its next call; pairs copies pooled to the caller
+        map_frames(s, p.f, true, true, DELORA_WS_STATE);
+        map_inference(s, p, DELORA_WS_OUTPUT);
+    } else if (kind <= DELORA_WS_STREAMS_PRE_INFO) {
+        rc = map_streams(s, d, kind, who);
+    } else if (kind <= DELORA_WS_TRAIN_GEOMETRIES) {
+        rc = map_train_kind(s, d, n, kind, who);
+    } else {
+        rc = map_adapt(s, d, n, kind, who);
+    }
+    if (rc) return 1;
+    DELORA_CHECK_ARG(!s.missing, "%s: kind %d: no take() at the offset of %s", who, kind, s.missing);
+    *count = s.n;
+    return 0;
+}
+
+extern "C" int delora_odometry_workspace_sections(int kind, const delora_odometry_desc* d, int n,
+                                                  delora_ws_section* out, int cap) {
+    int count = 0;
+    return workspace_sections(kind, d, n, out, cap, &count) ? -1 : count;
+}
 
 extern "C" int64_t delora_odometry_weight_floats(const delora_odometry_desc* d) {
     if (check_desc(d, "delora_odometry_weight_floats")) return -1;

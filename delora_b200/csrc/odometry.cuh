@@ -130,6 +130,21 @@ struct GroupReduce {
     unsigned seq_stride, seq_first;
 };
 
+// The records of delora_odometry_workspace_sections, from the take() log of the plan builds (take_log armed).
+// field: the section at off, sized by the last take() there (a plan that moves a field after its build takes again at
+// the new offset, later); range: a section the caller sizes, inside one take().  Each family's source lists the fields
+// its entry points dereference (map_* below).
+struct SectionMap {
+    const TakeLog* log;
+    delora_ws_section* out;
+    int cap, n, geometry, flags;       // geometry and flags of the records added next
+    const char* missing;               // a field with no take() at its offset: the plan and the map disagree
+    void add(const char* name, size_t off, size_t bytes, int role, int flags);
+    void field(const char* name, size_t off, int role);
+    void range(const char* name, size_t off, size_t bytes, int role);
+    void span(const char* prefix, size_t begin, size_t end, int role);      // every take() in [begin, end), in order
+};
+
 // ---------------------------------------------------------------- odometry.cu
 int check_desc(const delora_odometry_desc* d, const char* who);
 int check_icp_params(float lambda_po2pl, uint32_t loss_flags, int nb_h, int nb_w, float epsilon_range,
@@ -146,6 +161,11 @@ int init_workspace(const Frames& f, size_t total, void* workspace, cudaStream_t 
 int prep_blob_weights(const Model& m, const TrunkWeights& w, char* ws, const float* blob, cudaStream_t st,
                       const char* who);
 int load_weights(const InferPlan& p, const float* weights, void* workspace, cudaStream_t st, const char* who);
+// the section map of a frame section (index_map / counts: whether the kind reads them; prev_role: its cached images'),
+// of a weight section, and of everything plan_inference places after the frame section
+void map_frames(SectionMap& s, const Frames& f, bool index_map, bool counts, int prev_role);
+void map_trunk_weights(SectionMap& s, const TrunkPlan& m, const TrunkWeights& w);
+void map_inference(SectionMap& s, const InferPlan& p, int pooled_role);
 
 // ---------------------------------------------------------------- odometry_tail.cu
 int run_tail(const Model& m, const TailIO& io, int act, const float* pooled, int B, float* T, cudaStream_t st,
@@ -171,6 +191,7 @@ int streams_pre(const float* T16, const float* factor, const int32_t* active, co
                 const float4* pre_cur_pts, const float4* pre_cur_nrm, float4* pre_prev_pts, float4* pre_prev_nrm,
                 const float4* cur_image, float4* cache_image, cudaStream_t st);
 int streams_rows_out(int row, const int32_t* valid, int S, const float* rows, float* out, cudaStream_t st);
+int map_streams(SectionMap& s, const delora_odometry_desc* d, int kind, const char* who);   // DELORA_WS_STREAMS*
 
 // ---------------------------------------------------------------- odometry_train.cu
 void make_train_plan(const delora_odometry_desc* d, TrainPlan* tp, size_t geometry_at = 0);
@@ -188,5 +209,13 @@ int train_forward_losses(const delora_odometry_desc* d, const delora_odometry_tr
 int step_backward(const TrainPlan& tp, char* ws, int act, int B, bool identity, DropoutCtr drop, const int32_t* valid,
                   const int32_t* n_valid, const GroupReduce* gr, cudaStream_t st, const char* who);
 int record_icp_batch(const TrainPlan& tp, char* ws, int B, cudaStream_t st);
+// the sections of one training plan: the model section's (the weights under weights_flags; the gradient, with adam
+// Adam's moments, and the counters with ctr_role under model_flags), then the geometry section's
+void map_train(SectionMap& s, const delora_odometry_desc* d, const TrainPlan& tp, bool adam, int ctr_role,
+               int weights_flags, int model_flags);
+int map_train_kind(SectionMap& s, const delora_odometry_desc* d, int n, int kind, const char* who);
+
+// ---------------------------------------------------------------- odometry_adapt.cu
+int map_adapt(SectionMap& s, const delora_odometry_desc* d, int n, int kind, const char* who);   // DELORA_WS_ADAPT*
 
 }  // namespace delora

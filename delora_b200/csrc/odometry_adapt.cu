@@ -475,3 +475,63 @@ extern "C" int delora_odometry_streams_adapt_geometries_reset(const delora_odome
     }
     return 0;
 }
+
+namespace delora {
+
+// One adapting-streams plan's stream section
+static void map_adapt_streams(SectionMap& s, const delora_odometry_desc* d, const AdaptPlan& ap) {
+    if (d->w_pre == 0) s.field("cache_image", ap.cache_image, DELORA_WS_STATE);
+    s.field("cache_pts", ap.cache_pts, DELORA_WS_STATE);
+    s.field("cache_nrm", ap.cache_nrm, DELORA_WS_STATE);
+    s.field("has_prev", ap.has_prev, DELORA_WS_STATE);
+    s.field("n_valid", ap.n_valid, DELORA_WS_SCRATCH);
+}
+
+// DELORA_WS_ADAPT*.  Offsets a plan sets but its kind never reads, left out:
+//   - _adapt: ap.tick / n_fleet / slots lie past the end of the workspace.  push_adapt forms the tick pointer on every
+//     update tick but dereferences it, n_fleet and slots only with a group, which only _push_adapt_group and
+//     _push_adapt_group_info pass (and only with world > 1), on the _adapt_group / _adapt_info workspaces.
+//   - _adapt and _adapt_group: ap.info / info_scratch lie past the end.  serve_adapt reads them only with info
+//     non-NULL, which only _push_adapt_info and _push_adapt_group_info pass.
+//   - _adapt_geometries*, geometry g >= 1: ap[g].tick / n_fleet / slots lie inside g's gradient slice (which
+//     make_geometries_plan takes at the same offset); push_adapt_geometries passes no group to anything.  ap[g].info /
+//     info_scratch, moved into the information section, lie past the end of the _adapt_geometries form, where
+//     serve_adapt reads them only with info (only _push_adapt_geometries_info passes it).  tp[g].adam_m / adam_v are
+//     geometry 0's: adam_update runs on tp[0] alone.
+// Geometry g >= 1's counters are its fleet slot: [0] advances on every update tick and nothing reads it, [1] only
+// decides whether its next ICP re-arms the scratch, so they are scratch, not state.
+int map_adapt(SectionMap& s, const delora_odometry_desc* d, int n, int kind, const char* who) {
+    if (kind == DELORA_WS_ADAPT || kind == DELORA_WS_ADAPT_GROUP || kind == DELORA_WS_ADAPT_INFO) {
+        if (check_train_desc(d, who)) return 1;
+        TrainPlan tp;
+        AdaptPlan ap;
+        make_adapt_plan(d, &tp, &ap);
+        map_train(s, d, tp, true, DELORA_WS_STATE, 0, 0);
+        map_adapt_streams(s, d, ap);
+        if (kind == DELORA_WS_ADAPT) return 0;
+        s.range("tick", ap.tick, 8, DELORA_WS_STATE);
+        s.range("n_fleet", ap.n_fleet, 4, DELORA_WS_SCRATCH);
+        s.range("slots", ap.slots, 2 * kArMaxWorld * 4, DELORA_WS_STATE);
+        if (kind == DELORA_WS_ADAPT_INFO) {
+            s.field("info", ap.info, DELORA_WS_OUTPUT);
+            s.field("info_scratch", ap.info_scratch, DELORA_WS_SCRATCH);
+        }
+        return 0;
+    }
+    if (check_adapt_geometries(d, n, who)) return 1;
+    const std::unique_ptr<GeometriesPlan> p = make_geometries_plan(d, n);
+    for (int g = 0; g < n; ++g) {
+        s.geometry = g;
+        map_train(s, &d[g], p->tp[g], g == 0, g == 0 ? DELORA_WS_STATE : DELORA_WS_SCRATCH, DELORA_WS_SHARED, 0);
+        map_adapt_streams(s, &d[g], p->ap[g]);
+        if (g == 0 && n > 1) s.range("fleet", p->fleet, 4, DELORA_WS_SCRATCH);      // the fleet count of valid pairs
+        if (kind != DELORA_WS_ADAPT_GEOMETRIES_INFO) continue;
+        s.range("info", p->ap[g].info, (size_t)d[g].max_batch * DELORA_INFO_ROW * 4, DELORA_WS_OUTPUT);
+        s.flags = DELORA_WS_SHARED;
+        s.field("info_scratch", p->ap[g].info_scratch, DELORA_WS_SCRATCH);
+        s.flags = 0;
+    }
+    return 0;
+}
+
+}  // namespace delora

@@ -307,6 +307,53 @@ static int64_t streams_workspace_bytes(const delora_odometry_desc* d, Streams ki
     return (int64_t)p.total;
 }
 
+// The sections the streams entry points of one kind dereference.  Offsets of a section the kind does not have stay 0
+// in its plan (run_streams_push forms the grid pointers of a plain workspace at ws + 0, the keys, and reads them only
+// with rp, i.e. on the residual and information kinds); those are not listed.  Nor are the normalised kind's counts
+// (its count clamp writes stage_counts) and the recipe kinds' index map (their H x W projections pass none).
+int map_streams(SectionMap& s, const delora_odometry_desc* d, int kind, const char* who) {
+    static const Streams kinds[] = {Streams::plain, Streams::residual, Streams::info, Streams::normalized, Streams::pre,
+                                    Streams::pre_info};
+    const Streams k = kinds[kind - DELORA_WS_STREAMS];
+    if (check_streams_desc(d, k, who)) return 1;
+    StreamsPlan p;
+    make_streams_plan(d, k, &p);
+    const bool pre = k == Streams::pre || k == Streams::pre_info;
+    // the recipe and normalised kinds project both frames of every pair each tick: their prev_image holds no state
+    const bool cached = !pre && k != Streams::normalized;
+    map_frames(s, p.f, !pre, k != Streams::normalized, cached ? DELORA_WS_STATE : DELORA_WS_SCRATCH);
+    map_inference(s, p, DELORA_WS_SCRATCH);
+    if (p.pts_grid) {
+        s.field("pts_grid", p.pts_grid, DELORA_WS_SCRATCH);
+        s.field("nrm_grid", p.nrm_grid, DELORA_WS_SCRATCH);
+        // the residual kinds cache each stream's grids here; the recipe re-projects them from pre_pts every tick
+        s.field("prev_pts_grid", p.prev_pts_grid, pre ? DELORA_WS_SCRATCH : DELORA_WS_STATE);
+        s.field("prev_nrm_grid", p.prev_nrm_grid, pre ? DELORA_WS_SCRATCH : DELORA_WS_STATE);
+        s.field("T12", p.T12, DELORA_WS_SCRATCH);
+        s.field("losses", p.losses, DELORA_WS_OUTPUT);
+        s.field("grad_T", p.grad_T, DELORA_WS_SCRATCH);
+        s.field("icp", p.icp, DELORA_WS_SCRATCH);
+    }
+    if (p.stage) {
+        s.field("stage", p.stage, DELORA_WS_STATE);                  // row S + s: each stream's last frame
+        s.field("stage_counts", p.stage_counts, DELORA_WS_STATE);    // [2S + s]: its count
+    }
+    if (pre) {
+        s.field("pre_keys", p.pre_keys, DELORA_WS_SCRATCH);
+        s.field("pre_image", p.pre_image, DELORA_WS_SCRATCH);
+        s.field("pre_index_map", p.pre_index_map, DELORA_WS_SCRATCH);
+        s.field("pre_pts", p.pre_pts, DELORA_WS_STATE);               // [0, S): each stream's cached grids
+        s.field("pre_nrm", p.pre_nrm, DELORA_WS_STATE);
+        s.field("T16", p.T16, DELORA_WS_SCRATCH);
+    }
+    if (p.factor) s.field("factor", p.factor, DELORA_WS_SCRATCH);
+    if (p.info) {
+        s.field("info", p.info, DELORA_WS_OUTPUT);
+        s.field("info_scratch", p.info_scratch, DELORA_WS_SCRATCH);
+    }
+    return 0;
+}
+
 // The n cells of the cached grids at offsets pts / nrm start empty: the target of a stream that has not had a frame yet
 int clear_grids(char* ws, size_t pts, size_t nrm, size_t n, cudaStream_t st) {
     odometry_streams_grid_clear_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(

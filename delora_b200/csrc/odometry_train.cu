@@ -96,6 +96,72 @@ void make_train_plan(const delora_odometry_desc* d, TrainPlan* tp, size_t geomet
     tp->total = off;
 }
 
+// The training step's sections.  A training plan has no cached image (prev_image, has_prev stay 0, unread).
+void map_train(SectionMap& s, const delora_odometry_desc* d, const TrainPlan& tp, bool adam, int ctr_role,
+               int weights_flags, int model_flags) {
+    s.flags = weights_flags;
+    s.field("master", tp.master, DELORA_WS_WEIGHTS);
+    map_trunk_weights(s, tp.m.t, tp.w);
+    s.flags = model_flags;
+    // the group step's last bucket ends up to 3 floats past the blob (plan_buckets)
+    s.range("grad", tp.grad, (size_t)(tp.m.blob_floats + 3) / 4 * 16, DELORA_WS_OUTPUT);
+    if (adam) {
+        s.field("adam_m", tp.adam_m, DELORA_WS_STATE);
+        s.field("adam_v", tp.adam_v, DELORA_WS_STATE);
+    }
+    // [0] Adam's step count, [1] the ICP scratch's batch size, [2] the dropout seed; a slot of the fleet section for
+    // the adapting streams' geometries g >= 1
+    s.range("ctr", tp.ctr, 3 * sizeof(long long), ctr_role);
+    s.flags = 0;
+    map_frames(s, tp.f, true, true, DELORA_WS_SCRATCH);
+    s.field("pts_grid", tp.pts_grid, DELORA_WS_SCRATCH);
+    s.field("nrm_grid", tp.nrm_grid, DELORA_WS_SCRATCH);
+    // odometry_icp_rearm_kernel zeroes the scratch in whole float4s: up to 12 bytes past its last float
+    s.range("icp", tp.icp, (size_t)(delora_icp_scratch_floats(d->max_batch, d->H * d->W) + 3) / 4 * 16,
+            DELORA_WS_SCRATCH);
+    s.field("losses", tp.losses, DELORA_WS_OUTPUT);
+    s.field("grad_T", tp.grad_T, DELORA_WS_SCRATCH);
+    s.field("T16", tp.T16, DELORA_WS_OUTPUT);
+    s.field("T12", tp.T12, DELORA_WS_SCRATCH);
+    s.span("trunk.acts", tp.t.x_in, tp.pooled, DELORA_WS_SCRATCH);
+    s.field("pooled", tp.pooled, DELORA_WS_OUTPUT);
+    s.field("g_pooled", tp.g_pooled, DELORA_WS_SCRATCH);
+    s.field("fc_out", tp.fc_out, DELORA_WS_SCRATCH);
+    s.field("dz_fc", tp.dz_fc, DELORA_WS_SCRATCH);
+    s.field("raw", tp.raw, DELORA_WS_SCRATCH);
+    char name[32];
+    for (int i = 0; i < (tp.m.n_lin == 4 ? 1 : tp.m.n_lin - 1); ++i) {       // two heads: one [rot1 | trans1] buffer
+        snprintf(name, sizeof name, "hid[%d]", i);
+        s.field(name, tp.hid[i], DELORA_WS_SCRATCH);
+        snprintf(name, sizeof name, "dz_hid[%d]", i);
+        s.field(name, tp.dz_hid[i], DELORA_WS_SCRATCH);
+    }
+    if (d->w_pre > 0) {
+        // pre_image also holds the pair factors of a normalised step
+        s.field("pre_image", tp.pre_image, DELORA_WS_SCRATCH);
+        s.field("pre_index_map", tp.pre_index_map, DELORA_WS_SCRATCH);
+        s.field("pre_pts_grid", tp.pre_pts_grid, DELORA_WS_SCRATCH);
+        s.field("pre_nrm_grid", tp.pre_nrm_grid, DELORA_WS_SCRATCH);
+    }
+}
+
+// DELORA_WS_TRAIN and DELORA_WS_TRAIN_GEOMETRIES.  Each geometry of the latter trains the whole model section (shared)
+// on its own geometry section, which _train_use_geometry lays over the same bytes as every other geometry's.
+int map_train_kind(SectionMap& s, const delora_odometry_desc* d, int n, int kind, const char* who) {
+    if (kind == DELORA_WS_TRAIN ? check_train_desc(d, who) : check_geometries(d, n, who)) return 1;
+    const bool shared = kind == DELORA_WS_TRAIN_GEOMETRIES;
+    for (int g = 0; g < n; ++g) {
+        // the geometry sections start at one offset: each geometry's fields are sized from its own plan's log
+        take_log->off.clear();
+        take_log->bytes.clear();
+        TrainPlan tp;
+        make_train_plan(&d[g], &tp);
+        s.geometry = g;
+        map_train(s, &d[g], tp, true, DELORA_WS_STATE, shared ? DELORA_WS_SHARED : 0, shared ? DELORA_WS_SHARED : 0);
+    }
+    return 0;
+}
+
 // check_desc plus the field only training reads
 int check_train_desc(const delora_odometry_desc* d, const char* who) {
     if (check_desc(d, who)) return 1;

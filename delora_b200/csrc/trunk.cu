@@ -7,6 +7,8 @@
 
 namespace delora {
 
+thread_local TakeLog* take_log = nullptr;
+
 int check_trunk(const int* layers, int H, int W, const char* who) {
     DELORA_CHECK_ARG(layers != nullptr, "%s: null layers", who);
     DELORA_CHECK_ARG(H >= 1 && W >= 2, "%s: bad image size H=%d W=%d", who, H, W);

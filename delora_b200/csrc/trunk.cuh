@@ -5,6 +5,8 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <vector>
+
 #include "common.cuh"
 #include "dropout.cuh"
 
@@ -15,7 +17,20 @@ constexpr int kMaxBlocks = 4 * kMaxBlocksPerStage;
 constexpr int kMaxConv = 1 + 2 * kMaxBlocks + 3;   // stem, two 3x3 per block, the 1x1 downsamples of stages 1..3
 
 inline size_t align256(size_t n) { return (n + 255) & ~(size_t)255; }
-inline size_t take(size_t& off, size_t bytes) { const size_t o = off; off += align256(bytes); return o; }
+
+// Every take() of a plan build while take_log is armed (delora_odometry_workspace_sections): its offset and the bytes
+// asked for, in call order.  Unarmed (nullptr, every other caller) take() records nothing.
+struct TakeLog {
+    std::vector<size_t> off, bytes;
+};
+extern thread_local TakeLog* take_log;
+
+inline size_t take(size_t& off, size_t bytes) {
+    const size_t o = off;
+    off += align256(bytes);
+    if (take_log) { take_log->off.push_back(o); take_log->bytes.push_back(bytes); }
+    return o;
+}
 inline int out_size(int n, int s) { return (n - 1) / s + 1; }
 inline size_t nhwc_bytes(int b, int h, int w, int c) { return (size_t)b * (h + 2) * (w + 2) * c * 2; }
 

@@ -1448,6 +1448,80 @@ int delora_odometry_streams_push_adapt_geometries_info(const delora_odometry_des
                                                        const int32_t* active, void* workspace, float* T, int32_t* valid,
                                                        float* losses, float* info, void* stream);
 
+/* ---- The section map of an odometry workspace: where each buffer the entry points of a workspace kind read or write
+ * lies, for tests and tools that check a layout (disjoint sections, which calls write where).  Host only, launches
+ * nothing; the layout is the one the kind's entry points plan, built by the same plan functions.
+ *
+ * kind, and the entry points whose workspace it is:
+ *   DELORA_WS_PAIRS                     delora_odometry_init / _load_weights / _pairs / _pairs_normalized / _push
+ *   DELORA_WS_STREAMS                   delora_odometry_streams_init / _load_weights / _push / _reset
+ *   DELORA_WS_STREAMS_RESIDUAL          _streams_residual_init, _streams_push_residual
+ *   DELORA_WS_STREAMS_INFO              _streams_info_init, _streams_push_info
+ *   DELORA_WS_STREAMS_NORMALIZED        _streams_normalized_init, _streams_push_normalized
+ *   DELORA_WS_STREAMS_PRE               _streams_pre_init, _streams_push_pre (w_pre >= 2)
+ *   DELORA_WS_STREAMS_PRE_INFO          _streams_pre_info_init, _streams_push_pre_info (w_pre >= 2)
+ *   DELORA_WS_TRAIN                     delora_odometry_train_* of one geometry: _init, _step, _step_group, _eval, the
+ *                                       state calls and the dropout seed (w_pre > 0 adds the preprocessing sections)
+ *   DELORA_WS_TRAIN_GEOMETRIES          _train_geometries_init, _train_use_geometry and the calls above on geometry g
+ *   DELORA_WS_ADAPT                     _streams_adapt_init, _streams_push_adapt, _streams_adapt_reset
+ *   DELORA_WS_ADAPT_GROUP               _streams_adapt_group_init, _streams_push_adapt_group
+ *   DELORA_WS_ADAPT_INFO                _streams_adapt_info_init, _streams_push_adapt_info, _streams_push_adapt_group_info
+ *   DELORA_WS_ADAPT_GEOMETRIES          _streams_adapt_geometries_init / _push_adapt_geometries / _reset
+ *   DELORA_WS_ADAPT_GEOMETRIES_INFO     the same and _streams_push_adapt_geometries_info
+ * n: the number of descriptors in d; 1 for every kind but the three geometries kinds.
+ *
+ * Each record: the byte offset and size of one section (the bytes asked for, without the padding to the next 256-byte
+ * boundary), its role and name, the geometry whose entry points read it (0 for kinds of one geometry) and flags:
+ *   DELORA_WS_SUBRANGE  the section lies inside a larger 256-byte aligned allocation and need not itself be aligned;
+ *   DELORA_WS_SHARED    geometries kinds: the model section every geometry reads, listed once per geometry at the
+ *                       same offset (its weights, and the information scratch the geometries' ICPs share).
+ * Roles: DELORA_WS_WEIGHTS (written only by init, load_weights, set_state and Adam), DELORA_WS_STATE (carried from one
+ * call to the next: a stream's cached frame, Adam's moments and step count), DELORA_WS_SCRATCH (written and read
+ * within a call), DELORA_WS_OUTPUT (a result the call copies to the caller's arrays, or the gradient section
+ * delora_odometry_train_grad_offset names).  Every record but DELORA_WS_TRAIN_GEOMETRIES's lies inside the kind's
+ * *_workspace_bytes and no two overlap, the DELORA_WS_SHARED copies aside; DELORA_WS_TRAIN_GEOMETRIES's geometries each
+ * have their geometry section over the same bytes (one geometry trains at a time).  No section is empty.  The smaller
+ * kind's records appear unchanged in the larger one: STREAMS in RESIDUAL in INFO, TRAIN in ADAPT in ADAPT_GROUP in
+ * ADAPT_INFO, ADAPT_GEOMETRIES in ADAPT_GEOMETRIES_INFO.
+ *
+ * Returns the number of sections, and writes the first min(that, cap) of them to out (out may be NULL with cap = 0);
+ * -1 (and delora_last_error()) for a bad kind, n or cap and for every descriptor the kind's *_workspace_bytes
+ * refuses. */
+#define DELORA_WS_PAIRS                  0
+#define DELORA_WS_STREAMS                1
+#define DELORA_WS_STREAMS_RESIDUAL       2
+#define DELORA_WS_STREAMS_INFO           3
+#define DELORA_WS_STREAMS_NORMALIZED     4
+#define DELORA_WS_STREAMS_PRE            5
+#define DELORA_WS_STREAMS_PRE_INFO       6
+#define DELORA_WS_TRAIN                  7
+#define DELORA_WS_TRAIN_GEOMETRIES       8
+#define DELORA_WS_ADAPT                  9
+#define DELORA_WS_ADAPT_GROUP           10
+#define DELORA_WS_ADAPT_INFO            11
+#define DELORA_WS_ADAPT_GEOMETRIES      12
+#define DELORA_WS_ADAPT_GEOMETRIES_INFO 13
+#define DELORA_WS_KINDS                 14
+
+#define DELORA_WS_WEIGHTS 0
+#define DELORA_WS_STATE   1
+#define DELORA_WS_SCRATCH 2
+#define DELORA_WS_OUTPUT  3
+
+#define DELORA_WS_SUBRANGE 1
+#define DELORA_WS_SHARED   2
+
+typedef struct {
+    int64_t offset;
+    int64_t bytes;
+    int32_t role;
+    int32_t geometry;
+    int32_t flags;
+    char name[44];         /* NUL-terminated, e.g. "cache_pts", "trunk.fwd[3]", "trunk.acts[12]" */
+} delora_ws_section;
+int delora_odometry_workspace_sections(int kind, const delora_odometry_desc* d, int n, delora_ws_section* out,
+                                       int cap);   /* host only */
+
 #ifdef __cplusplus
 }
 #endif

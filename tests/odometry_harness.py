@@ -245,6 +245,24 @@ def streams_desc(h=64, w=720, S=2, w_pre=0, n_stride=1000):
     return desc(config(h, w, device="cpu"), n_stride, S, w_pre)
 
 
+Section = collections.namedtuple("Section", "name offset bytes role geometry flags")
+
+
+def sections(kind, descs):
+    """delora_odometry_workspace_sections of kind (a name of _lib.WS_KINDS) over the descriptors descs (one, or each
+    geometry's) -> [Section], or None where the library refuses them."""
+    from delora_b200 import _lib
+    L = _lib.lib()
+    k = _lib.WS_KINDS.index(kind)
+    arr = (_lib.OdometryDesc * len(descs))(*descs)
+    n = L.delora_odometry_workspace_sections(k, arr, len(descs), None, 0)
+    if n < 0:
+        return None
+    out = (_lib.WsSection * n)()
+    assert L.delora_odometry_workspace_sections(k, arr, len(descs), out, n) == n
+    return [Section(r.name.decode(), r.offset, r.bytes, _lib.WS_ROLES[r.role], r.geometry, r.flags) for r in out]
+
+
 def train_params(flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL, lr=1e-5):
     from delora_b200 import _lib
     return _lib.OdometryTrainParams(lr=lr, beta1=0.9, beta2=0.999, eps=1e-8, lambda_po2pl=1.0, loss_flags=flags,
