@@ -9,9 +9,7 @@ The card's name, power limit and SM clock are read in the same run.
     python scripts/gpu_odometry_capi.py [--frames 300] [--json out.json]
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
 import time
 
@@ -20,19 +18,13 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
-from delora_b200 import synthetic  # noqa: E402
 from delora_b200.deploy import export  # noqa: E402
 from delora_b200.deploy.capi import InferenceWorkspace  # noqa: E402
 from delora_b200.deploy.stream import OdometryStream  # noqa: E402
 from delora_b200.models.model import OdometryModel  # noqa: E402
+from measure import DEV, capture, emit, gpu_info, model_config, n_stride, pairs, staged  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12       # H100 SXM data sheet
-
-
-def gpu_info():
-    q = "name,power.limit,clocks.sm,clocks.max.sm,clocks_throttle_reasons.active"
-    r = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True)
-    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "unavailable"
 
 
 def pct(ts, p):
@@ -45,37 +37,27 @@ def main():
     ap.add_argument("--json", default="")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs a GPU"
-    dev = "cuda:0"
     h, w = 64, 2048
-    cfg = synthetic.fov_config(h=h, w=w, device=dev)
-    cfg.update({"activation_fct": "tanh", "use_single_mlp_at_output": False, "layers": [2, 2, 2, 2],
-                "resnet_outputs": 1000, "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1,
-                "use_dropout": False})
+    cfg = model_config(h, w)
     torch.manual_seed(0)
-    model = OdometryModel(cfg).to(dev).eval()
-    scans = []
-    for i in range(3):
-        s1, s2, _, _ = synthetic.make_pair(i, w_raw=2048, rings=64)
-        scans += [s1, s2]
-    n_stride = max(s.shape[1] for s in scans)
-    info_before = gpu_info()
+    model = OdometryModel(cfg).to(DEV).eval()
+    ps = pairs(64, 3)
+    scans = [s for p in ps for s in p]
+    stride = n_stride(ps)
 
-    res = {"gpu_before": info_before, "H": h, "W": w, "n_stride": n_stride}
+    res = {"gpu_before": gpu_info(), "H": h, "W": w, "n_stride": stride}
     for mb in (1, 16):
-        dd = export.desc_from_config(cfg, "kitti", n_stride, mb)
+        dd = export.desc_from_config(cfg, "kitti", stride, mb)
         res[f"workspace_bytes_max_batch_{mb}"] = InferenceWorkspace.workspace_bytes(dd)
     st = torch.cuda.current_stream()
-    blob = torch.from_numpy(export.pack_state_dict(model.state_dict(), cfg)).to(dev)
-    ws = InferenceWorkspace(export.desc_from_config(cfg, "kitti", n_stride, 1), blob)
+    blob = torch.from_numpy(export.pack_state_dict(model.state_dict(), cfg)).to(DEV)
+    ws = InferenceWorkspace(export.desc_from_config(cfg, "kitti", stride, 1), blob)
 
-    host_pts = torch.zeros((len(scans), 3, n_stride), dtype=torch.float32).pin_memory()
-    host_cnt = torch.zeros((len(scans),), dtype=torch.int32).pin_memory()
-    for i, s in enumerate(scans):
-        host_pts[i, :, :s.shape[1]] = s
-        host_cnt[i] = s.shape[1]
-    pts = torch.zeros((1, 3, n_stride), dtype=torch.float32, device=dev)
-    cnt = torch.zeros((1,), dtype=torch.int32, device=dev)
-    t_dev = torch.zeros((16,), dtype=torch.float32, device=dev)
+    # every frame is uploaded from pinned host memory, as a caller's would be
+    host_pts, host_cnt = (t.cpu().pin_memory() for t in staged(scans, stride))
+    pts = torch.zeros((1, 3, stride), dtype=torch.float32, device=DEV)
+    cnt = torch.zeros((1,), dtype=torch.int32, device=DEV)
+    t_dev = torch.zeros((16,), dtype=torch.float32, device=DEV)
     t_host = torch.zeros((16,), dtype=torch.float32).pin_memory()
 
     def upload(k):
@@ -86,7 +68,8 @@ def main():
         upload(k)
         ws.push(pts, cnt, None if first else t_dev)
 
-    def timed(step, n):
+    def latencies(step, n):
+        """Seconds from each frame's upload to its T on the host."""
         ts = []
         for k in range(n):
             t0 = time.perf_counter()
@@ -100,11 +83,9 @@ def main():
     for k in range(1, 20):
         push(k)
     st.synchronize()
-    eager = timed(lambda k: push(k + 1), args.frames)
+    eager = latencies(lambda k: push(k + 1), args.frames)
 
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        ws.push(pts, cnt, t_dev)
+    graph = capture(lambda: ws.push(pts, cnt, t_dev), warmup=0)
 
     def replay(k):
         upload(k)
@@ -112,9 +93,9 @@ def main():
     for k in range(20):
         replay(k)
     st.synchronize()
-    graphed = timed(replay, args.frames)
+    graphed = latencies(replay, args.frames)
 
-    stream = OdometryStream(model, cfg, "kitti", n_stride)
+    stream = OdometryStream(model, cfg, "kitti", stride)
     stream.push(scans[0])
     for k in range(1, 20):
         stream.push(scans[k % len(scans)])
@@ -125,7 +106,7 @@ def main():
         ts_stream.append(time.perf_counter() - t0)
 
     # one-frame parity against the stream (same model, same pair of frames)
-    stream2 = OdometryStream(model, cfg, "kitti", n_stride)
+    stream2 = OdometryStream(model, cfg, "kitti", stride)
     stream2.push(scans[0])
     t_ref = torch.from_numpy(stream2.push(scans[1])[0]).reshape(16)
     push(0, first=True)
@@ -154,12 +135,7 @@ def main():
     res["tail"] = {"kernel_us": tail_us, "weight_bytes": tail_floats * 4, "hbm_floor_us": floor_us,
                    "share_of_floor": floor_us / tail_us if tail_us > 0 else None}
     res["gpu_after"] = gpu_info()
-    line = json.dumps(res, indent=1)
-    print(line)
-    if args.json:
-        os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)
-        with open(args.json, "w") as f:
-            f.write(line)
+    emit(res, args.json)
 
 
 if __name__ == "__main__":

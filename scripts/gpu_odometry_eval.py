@@ -16,7 +16,6 @@ run.  Writes odometry_eval.json to --out.
     python scripts/gpu_odometry_eval.py [--seconds 0.5] [--samples 3] [--out DIR]
 """
 import argparse
-import json
 import os
 import statistics
 import sys
@@ -25,24 +24,12 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 import torch  # noqa: E402
 
-from delora_b200 import synthetic  # noqa: E402
 from delora_b200.deploy import capi, export  # noqa: E402
-from delora_b200.models.model import OdometryModel  # noqa: E402
-from gpu_odometry_streams import DEV, gpu_info, staged, time_replays  # noqa: E402
+from measure import (DEV, GPU_QUERY, alternate, capture, emit, events_ms, gpu_info, model_config,  # noqa: E402
+                     n_stride, near_identity_blob, pairs, staged)
 
 SIZES = ((64, 2048), (64, 720))
 BATCHES = (1, 4, 16)
-
-
-def near_identity_blob(cfg):
-    torch.manual_seed(0)
-    model = OdometryModel(cfg).to(DEV).eval()
-    with torch.no_grad():
-        for head, bias in ((model.fully_connected_rotation, [0.0, 0.0, 0.0, 1.0]),
-                           (model.fully_connected_translation, [0.0, 0.0, 0.0])):
-            head[3].weight.mul_(0.01)
-            head[3].bias.copy_(torch.tensor(bias))
-    return torch.from_numpy(export.pack_state_dict(model.state_dict(), cfg)).to(DEV)
 
 
 class Ticks:
@@ -58,11 +45,7 @@ class Ticks:
         self.T = torch.zeros((S, 16), dtype=torch.float32, device=DEV)
         self.valid = torch.zeros((S,), dtype=torch.int32, device=DEV)
         self.out = (self.T, self.valid) + ((torch.zeros((S, 8), dtype=torch.float32, device=DEV),) if residual else ())
-        self.two_ticks()                 # first frames cached; warms the launchers' host-side state
-        torch.cuda.synchronize()
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self.two_ticks()
+        self.graph = capture(self.two_ticks, warmup=1)      # the warm-up caches the first frames
 
     def two_ticks(self):
         for pts, counts in self.frames:
@@ -79,20 +62,10 @@ class Train:
         self.ws = capi.TrainingWorkspace(d, blob, capi.train_params(cfg, 0.0))
         self.pts, self.counts = staged([p[0] for p in pairs] + [p[1] for p in pairs], n_stride)
         self.call = self.ws.eval if evaluate else self.ws.step
-        self.call(self.pts, self.counts)
-        torch.cuda.synchronize()
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self.result = self.call(self.pts, self.counts)
+        self.graph = capture(self.run, warmup=1)
 
-
-def alternate(a, b, seconds, samples):
-    """-> (samples of a, samples of b) in ms per replay, taken a, b, a, b, ..."""
-    xs, ys = [], []
-    for _ in range(samples):
-        xs.append(time_replays(a.graph.replay, seconds)[0])
-        ys.append(time_replays(b.graph.replay, seconds)[0])
-    return xs, ys
+    def run(self):
+        self.result = self.call(self.pts, self.counts)
 
 
 def main():
@@ -102,21 +75,23 @@ def main():
     ap.add_argument("--out", default="")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs a GPU"
-    res = {"gpu_before": gpu_info(), "gpu_query": "name, power.limit, clocks.sm, clocks.max.sm",
+    res = {"gpu_before": gpu_info(), "gpu_query": GPU_QUERY,
            "seconds_per_sample": args.seconds, "sizes": {}}
+
+    def timer(fn):
+        return events_ms(fn, seconds=args.seconds)[0]
+
     for h, w in SIZES:
-        cfg = synthetic.fov_config(h=h, w=w, device=DEV)
-        cfg.update({"activation_fct": "tanh", "use_single_mlp_at_output": False, "layers": [2, 2, 2, 2],
-                    "resnet_outputs": 1000, "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1,
-                    "use_dropout": False})
+        cfg = model_config(h, w)
         blob = near_identity_blob(cfg)
-        pairs_all = [synthetic.make_pair(i, w_raw=2048, rings=h)[:2] for i in range(max(BATCHES))]
-        n_stride = max(max(a.shape[1], b.shape[1]) for a, b in pairs_all)
+        pairs_all = pairs(h, max(BATCHES))
+        stride = n_stride(pairs_all)
         streams, train = {}, {}
         for n in BATCHES:
-            pairs = pairs_all[:n]
-            plain, scored = Ticks(cfg, blob, pairs, n_stride, False), Ticks(cfg, blob, pairs, n_stride, True)
-            xs, ys = alternate(plain, scored, args.seconds, args.samples)
+            ps = pairs_all[:n]
+            plain, scored = Ticks(cfg, blob, ps, stride, False), Ticks(cfg, blob, ps, stride, True)
+            t = alternate({"plain": plain.graph.replay, "scored": scored.graph.replay}, args.samples, timer)
+            xs, ys = t["plain"], t["scored"]
             torch.cuda.synchronize()
             ms_p, ms_r = statistics.median(xs) / 2, statistics.median(ys) / 2       # two ticks per replay
             streams[n] = {"push_ms_per_tick": ms_p, "push_residual_ms_per_tick": ms_r, "added_ms_per_tick": ms_r - ms_p,
@@ -126,22 +101,18 @@ def main():
                           "workspace_MiB": [plain.ws.workspace.numel() / 2**20, scored.ws.workspace.numel() / 2**20]}
             del plain, scored
             torch.cuda.empty_cache()
-            step, ev = Train(cfg, blob, pairs, n_stride, False), Train(cfg, blob, pairs, n_stride, True)
-            xs, ys = alternate(step, ev, args.seconds, args.samples)
+            step, ev = Train(cfg, blob, ps, stride, False), Train(cfg, blob, ps, stride, True)
+            t = alternate({"step": step.graph.replay, "eval": ev.graph.replay}, args.samples, timer)
+            xs, ys = t["step"], t["eval"]
             torch.cuda.synchronize()
             train[n] = {"train_step_ms": statistics.median(xs), "train_eval_ms": statistics.median(ys),
                         "train_step_samples_ms": xs, "train_eval_samples_ms": ys,
                         "outputs_bit_identical": all(bool(torch.equal(a, b)) for a, b in zip(step.result[:3], ev.result))}
             del step, ev
             torch.cuda.empty_cache()
-        res["sizes"][f"{h}x{w}"] = {"n_stride": n_stride, "streams_S": streams, "train_B": train}
+        res["sizes"][f"{h}x{w}"] = {"n_stride": stride, "streams_S": streams, "train_B": train}
     res["gpu_after"] = gpu_info()
-    text = json.dumps(res, indent=1)
-    print(text)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "odometry_eval.json"), "w") as f:
-            f.write(text)
+    emit(res, args.out and os.path.join(args.out, "odometry_eval.json"))
 
 
 if __name__ == "__main__":

@@ -10,37 +10,24 @@ torch.profiler splits one eager tick (streams, and the S pushes) into kernels at
     python scripts/gpu_odometry_streams.py [--seconds 1.0] [--profile] [--out DIR]
 """
 import argparse
-import json
 import math
 import os
-import subprocess
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 import torch  # noqa: E402
 
-from delora_b200 import synthetic  # noqa: E402
 from delora_b200.deploy import export  # noqa: E402
 from delora_b200.deploy.capi import InferenceWorkspace, StreamsWorkspace  # noqa: E402
-from delora_b200.models.model import OdometryModel  # noqa: E402
+from measure import DEV, capture, emit, events_ms, gpu_info, model_config, pairs, staged, untrained_blob  # noqa: E402
 
-DEV = "cuda:0"
 STREAMS = (1, 2, 4, 8, 16)
 SIZES = ((64, 2048), (64, 720))
 
 
-def gpu_info():
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    r = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True)
-    return r.stdout.strip().splitlines()[0] if r.returncode == 0 and r.stdout.strip() else "unavailable"
-
-
 def frames(h, n):
-    pool = []
-    for i in range(3):
-        s1, s2, _, _ = synthetic.make_pair(i, w_raw=2048, rings=h)
-        pool += [s1, s2]
+    pool = [s for p in pairs(h, 3) for s in p]
     out = []
     for s in range(n):
         yaw = math.radians(7.0 * s)
@@ -48,35 +35,6 @@ def frames(h, n):
         rot = torch.tensor([[c, -si, 0.0], [si, c, 0.0], [0.0, 0.0, 1.0]], dtype=torch.float32)
         out.append((rot @ pool[s % len(pool)]).contiguous())
     return out
-
-
-def time_replays(fn, seconds):
-    """ms per call of fn (graph replays), from CUDA events, over >= `seconds` of work after a warm-up."""
-    for _ in range(10):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(10):
-        fn()
-    e1.record()
-    e1.synchronize()
-    est = e0.elapsed_time(e1) / 10
-    n = max(50, int(math.ceil(seconds * 1e3 / max(est, 1e-3))))
-    e0.record()
-    for _ in range(n):
-        fn()
-    e1.record()
-    e1.synchronize()
-    return e0.elapsed_time(e1) / n, n
-
-
-def staged(scans, n_stride):
-    pts = torch.zeros((len(scans), 3, n_stride), dtype=torch.float32)
-    for i, s in enumerate(scans):
-        pts[i, :, :s.shape[1]] = s
-    counts = torch.tensor([s.shape[1] for s in scans], dtype=torch.int32)
-    return pts.to(DEV), counts.to(DEV)
 
 
 class StreamsRun:
@@ -87,11 +45,7 @@ class StreamsRun:
         self.active = torch.ones((S,), dtype=torch.int32, device=DEV)
         self.T = torch.zeros((S, 16), dtype=torch.float32, device=DEV)
         self.valid = torch.zeros((S,), dtype=torch.int32, device=DEV)
-        self.push()                 # first frames: cached; also warms the launchers' host-side state
-        torch.cuda.synchronize()
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self.push()
+        self.graph = capture(self.push, warmup=1)      # the warm-up caches the first frames
 
     def push(self):
         self.ws.push(self.pts, self.counts, self.active, self.T, self.valid)
@@ -99,7 +53,7 @@ class StreamsRun:
 
 class PushRun:
     def __init__(self, cfg, blob, scans, n_stride):
-        self.ws, self.pts, self.counts, self.T, self.graphs = [], [], [], [], []
+        self.ws, self.pts, self.counts, self.T = [], [], [], []
         for s in scans:
             ws = InferenceWorkspace(export.desc_from_config(cfg, "kitti", n_stride, 1), blob)
             p, c = staged([s], n_stride)
@@ -108,12 +62,7 @@ class PushRun:
         for i in range(len(scans)):
             self.push(i, first=True)
             self.push(i)
-        torch.cuda.synchronize()
-        for i in range(len(scans)):
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self.push(i)
-            self.graphs.append(g)
+        self.graphs = [capture(lambda i=i: self.push(i), warmup=0) for i in range(len(scans))]
 
     def push(self, i, first=False):
         self.ws[i].push(self.pts[i], self.counts[i], None if first else self.T[i])
@@ -148,13 +97,8 @@ def main():
     assert torch.cuda.is_available(), "needs a GPU"
     res = {"gpu_before": gpu_info(), "seconds_per_point": args.seconds, "sizes": {}}
     for h, w in SIZES:
-        cfg = synthetic.fov_config(h=h, w=w, device=DEV)
-        cfg.update({"activation_fct": "tanh", "use_single_mlp_at_output": False, "layers": [2, 2, 2, 2],
-                    "resnet_outputs": 1000, "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1,
-                    "use_dropout": False})
-        torch.manual_seed(0)
-        model = OdometryModel(cfg).to(DEV).eval()
-        blob = torch.from_numpy(export.pack_state_dict(model.state_dict(), cfg)).to(DEV)
+        cfg = model_config(h, w)
+        blob = untrained_blob(cfg)
         scans_all = frames(h, max(STREAMS))
         n_stride = max(s.shape[1] for s in scans_all)
         key = f"{h}x{w}"
@@ -164,10 +108,10 @@ def main():
             st = StreamsRun(cfg, blob, scans, n_stride)
             pu = PushRun(cfg, blob, scans, n_stride)
             # alternate the two so drift of the card's clock hits both alike
-            ms_s1, n_s = time_replays(st.graph.replay, args.seconds / 2)
-            ms_p1, n_p = time_replays(pu.replay, args.seconds / 2)
-            ms_s2, _ = time_replays(st.graph.replay, args.seconds / 2)
-            ms_p2, _ = time_replays(pu.replay, args.seconds / 2)
+            ms_s1, n_s = events_ms(st.graph.replay, seconds=args.seconds / 2)
+            ms_p1, n_p = events_ms(pu.replay, seconds=args.seconds / 2)
+            ms_s2, _ = events_ms(st.graph.replay, seconds=args.seconds / 2)
+            ms_p2, _ = events_ms(pu.replay, seconds=args.seconds / 2)
             ms_s, ms_p = (ms_s1 + ms_s2) / 2, (ms_p1 + ms_p2) / 2
             torch.cuda.synchronize()
             same = all(torch.equal(st.T[i], pu.T[i]) for i in range(S)) and bool(st.valid.all())
@@ -184,12 +128,7 @@ def main():
             torch.cuda.empty_cache()
         res["sizes"][key] = {"n_stride": n_stride, "S": rows}
     res["gpu_after"] = gpu_info()
-    text = json.dumps(res, indent=1)
-    print(text)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "odometry_streams.json"), "w") as f:
-            f.write(text)
+    emit(res, args.out and os.path.join(args.out, "odometry_streams.json"))
 
 
 if __name__ == "__main__":

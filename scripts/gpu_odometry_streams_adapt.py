@@ -2,7 +2,7 @@
 needs without delora_odometry_streams_push_adapt.
 
 Per tick, ms at S in {1, 4, 16} for 64 x 720 (w_pre 0 and 2250) and 64 x 2048 (w_pre 0), all streams active, on the
-same near-identity weights (gpu_odometry_eval.near_identity_blob), lr 0 (Adam runs, the weights stay put, so every
+same near-identity weights (measure.near_identity_blob), lr 0 (Adam runs, the weights stay put, so every
 sample times the same work):
   adapt0     delora_odometry_streams_push_adapt, update = 0 (serve and score);
   adapt1     delora_odometry_streams_push_adapt, update = 1 (serve, score and one Adam step on the S pairs);
@@ -20,7 +20,6 @@ the same run.  Writes odometry_streams_adapt.json to --out.
     python scripts/gpu_odometry_streams_adapt.py [--seconds 0.3] [--samples 5] [--out DIR]
 """
 import argparse
-import json
 import os
 import statistics
 import sys
@@ -29,23 +28,13 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 import torch  # noqa: E402
 
-from delora_b200 import ops, synthetic  # noqa: E402
+from delora_b200 import ops  # noqa: E402
 from delora_b200.deploy import capi, export  # noqa: E402
-from gpu_odometry_eval import near_identity_blob  # noqa: E402
-from gpu_odometry_streams import DEV, gpu_info, staged, time_replays  # noqa: E402
+from measure import (DEV, GPU_QUERY, alternate, capture, emit, events_ms, gpu_info, model_config,  # noqa: E402
+                     n_stride, near_identity_blob, pairs, staged)
 
 SIZES = ((64, 720, 0), (64, 720, 2250), (64, 2048, 0))
 STREAMS = (1, 4, 16)
-SIDES = ("adapt0", "adapt1", "train", "compose")
-
-
-def _graph(fn):
-    fn()                                 # warms the launchers' host-side state
-    torch.cuda.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        fn()
-    return g
 
 
 class Sides:
@@ -68,12 +57,11 @@ class Sides:
         self.streams = (capi.PreStreamsWorkspace(d, blob, rp) if w_pre > 0 else
                         capi.ResidualStreamsWorkspace(d, blob, rp))
         self.weights = blob.clone()
-        self.graphs = {"adapt0": _graph(lambda: self.adapt_ticks(False)),
-                       "adapt1": _graph(lambda: self.adapt_ticks(True)),
-                       "train": _graph(self.train_steps)}
-        self.compose_graphs = [_graph(lambda i=i: self.compose_tick(i)) for i in (0, 1)]
-        self.fn = {k: g.replay for k, g in self.graphs.items()}
-        self.fn["compose"] = self.compose
+        self.fn = {"adapt0": capture(lambda: self.adapt_ticks(False), warmup=1).replay,
+                   "adapt1": capture(lambda: self.adapt_ticks(True), warmup=1).replay,
+                   "train": capture(self.train_steps, warmup=1).replay,
+                   "compose": self.compose}
+        self.compose_graphs = [capture(lambda i=i: self.compose_tick(i), warmup=1) for i in (0, 1)]
 
     def adapt_ticks(self, update):
         for pts, counts in self.frames:
@@ -101,25 +89,20 @@ def main():
     ap.add_argument("--out", default="")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs a GPU"
-    res = {"gpu_before": gpu_info(), "gpu_query": "name, power.limit, clocks.sm, clocks.max.sm",
+    res = {"gpu_before": gpu_info(), "gpu_query": GPU_QUERY,
            "seconds_per_sample": args.seconds, "lr": 0.0, "sizes": {}}
     for h, w, w_pre in SIZES:
-        cfg = synthetic.fov_config(h=h, w=w, device=DEV)
-        cfg.update({"activation_fct": "tanh", "use_single_mlp_at_output": False, "layers": [2, 2, 2, 2],
-                    "resnet_outputs": 1000, "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1,
-                    "use_dropout": False})
+        cfg = model_config(h, w)
         if w_pre:
             cfg["kitti"]["horizontal_cells_preprocessing"] = w_pre
         blob = near_identity_blob(cfg)
-        pairs_all = [synthetic.make_pair(i, w_raw=2048, rings=h)[:2] for i in range(max(STREAMS))]
-        n_stride = max(max(a.shape[1], b.shape[1]) for a, b in pairs_all)
+        pairs_all = pairs(h, max(STREAMS))
+        stride = n_stride(pairs_all)
         per_s = {}
         for S in STREAMS:
-            sides = Sides(cfg, blob, pairs_all[:S], n_stride, w_pre)
-            samples = {k: [] for k in SIDES}
-            for _ in range(args.samples):
-                for k in SIDES:
-                    samples[k].append(time_replays(sides.fn[k], args.seconds)[0] / 2)      # two ticks per call
+            sides = Sides(cfg, blob, pairs_all[:S], stride, w_pre)
+            samples = alternate(sides.fn, args.samples,
+                                lambda fn: events_ms(fn, seconds=args.seconds)[0] / 2)      # two ticks per call
             torch.cuda.synchronize()
             med = {k: statistics.median(v) for k, v in samples.items()}
             per_s[S] = {**{f"{k}_ms_per_tick": m for k, m in med.items()},
@@ -133,14 +116,9 @@ def main():
                                           "streams": sides.streams.workspace.numel() / 2**20}}
             del sides
             torch.cuda.empty_cache()
-        res["sizes"][f"{h}x{w}_wpre{w_pre}"] = {"n_stride": n_stride, "streams_S": per_s}
+        res["sizes"][f"{h}x{w}_wpre{w_pre}"] = {"n_stride": stride, "streams_S": per_s}
     res["gpu_after"] = gpu_info()
-    text = json.dumps(res, indent=1)
-    print(text)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "odometry_streams_adapt.json"), "w") as f:
-            f.write(text)
+    emit(res, args.out and os.path.join(args.out, "odometry_streams_adapt.json"))
 
 
 if __name__ == "__main__":

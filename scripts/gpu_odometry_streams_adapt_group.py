@@ -18,22 +18,18 @@ The card's name, power limit and SM clocks are read in the same run.  Writes odo
     python scripts/gpu_odometry_streams_adapt_group.py [--gpus N] [--seconds 0.5] [--samples 5] [--out DIR]
 """
 import argparse
-import json
 import os
 import statistics
 import sys
-import time
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 import torch  # noqa: E402
 
-from delora_b200 import ops, synthetic  # noqa: E402
+from delora_b200 import ops  # noqa: E402
 from delora_b200.deploy import capi, export  # noqa: E402
-from gpu_odometry_eval import near_identity_blob  # noqa: E402
-from gpu_odometry_streams import DEV, gpu_info, staged  # noqa: E402
-from gpu_train_group import enable_peer_access  # noqa: E402
+from measure import (GPU_QUERY, alternate, capture, emit, enable_peer_access, gpu_info, host_ms,  # noqa: E402
+                     model_config, n_stride, near_identity_blob, paired, pairs, staged)
 
 H, W = 64, 720
 STREAMS = (1, 4, 16)
@@ -65,11 +61,7 @@ class Ranks:
         self.graphs = []
         for r, dev in enumerate(self.devs):
             with torch.cuda.device(dev):
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g, stream=self.streams[r]):
-                    self.ticks(r)
-                self.graphs.append(g)
-        self.sync()
+                self.graphs.append(capture(lambda r=r: self.ticks(r), warmup=0, stream=self.streams[r]))
 
     def ticks(self, r):
         active, T, valid, losses = self.bufs[r]
@@ -92,21 +84,6 @@ class Ranks:
     def sync(self):
         for dev in self.devs:
             torch.cuda.synchronize(dev)
-
-    def time(self, seconds):
-        """ms per tick of every rank (host clock around synchronised replays of two ticks), over >= `seconds`."""
-        for _ in range(4):
-            self.replay()
-        self.sync()
-        n, t0 = 0, time.perf_counter()
-        while True:
-            self.replay()
-            n += 1
-            if n % 4 == 0:
-                self.sync()
-                el = time.perf_counter() - t0
-                if el >= seconds:
-                    return el * 1e3 / n / 2
 
     def exchange_us(self, replays=20):
         """Median device time of count_allreduce_kernel per rank over `replays` replays (torch.profiler)."""
@@ -140,25 +117,21 @@ def main():
     assert torch.cuda.device_count() >= args.gpus, f"--gpus {args.gpus}: {torch.cuda.device_count()} GPU(s) here"
     if args.gpus > 1:
         enable_peer_access(args.gpus)
-    res = {"gpu_before": gpu_info(), "gpu_query": "name, power.limit, clocks.sm, clocks.max.sm", "gpus": args.gpus,
+    res = {"gpu_before": gpu_info(), "gpu_query": GPU_QUERY, "gpus": args.gpus,
            "size": f"{H}x{W}_wpre0", "lr": 0.0, "seconds_per_sample": args.seconds, "streams_S": {}}
-    cfg = synthetic.fov_config(h=H, w=W, device=DEV)
-    cfg.update({"activation_fct": "tanh", "use_single_mlp_at_output": False, "layers": [2, 2, 2, 2],
-                "resnet_outputs": 1000, "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1,
-                "use_dropout": False})
+    cfg = model_config(H, W)
     blob = near_identity_blob(cfg)
-    pairs_all = [synthetic.make_pair(i, w_raw=2048, rings=H)[:2] for i in range(max(STREAMS))]
-    n_stride = max(max(a.shape[1], b.shape[1]) for a, b in pairs_all)
+    pairs_all = pairs(H, max(STREAMS))
+    stride = n_stride(pairs_all)
     for S in STREAMS:
-        plain = Ranks(cfg, blob, pairs_all[:S], n_stride, args.gpus, False)
-        group = Ranks(cfg, blob, pairs_all[:S], n_stride, args.gpus, True)
-        xs, ys = [], []
-        for _ in range(args.samples):
-            xs.append(plain.time(args.seconds))
-            ys.append(group.time(args.seconds))
-        diffs = [y - x for x, y in zip(xs, ys)]
+        plain = Ranks(cfg, blob, pairs_all[:S], stride, args.gpus, False)
+        group = Ranks(cfg, blob, pairs_all[:S], stride, args.gpus, True)
+        t = alternate({"plain": plain, "group": group}, args.samples,            # two ticks per replay
+                      lambda ranks: host_ms(ranks.replay, args.seconds, ranks.devs, every=4, warmup=4) / 2)
+        xs, ys = t["plain"], t["group"]
+        diffs, diff = paired(xs, ys)
         row = {"push_adapt_ms_per_tick": statistics.median(xs), "group_ms_per_tick": statistics.median(ys),
-               "paired_difference_ms": statistics.median(diffs), "push_adapt_samples_ms": xs,
+               "paired_difference_ms": diff, "push_adapt_samples_ms": xs,
                "group_samples_ms": ys, "paired_differences_ms": diffs, "status": group.status(),
                "group_step_counts": group.steps(), "plain_step_counts": plain.steps(),
                "all_valid": bool(all(bool(b[2].all()) for b in group.bufs))}
@@ -170,12 +143,7 @@ def main():
         del plain, group
         torch.cuda.empty_cache()
     res["gpu_after"] = gpu_info()
-    text = json.dumps(res, indent=1)
-    print(text)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "odometry_streams_adapt_group.json"), "w") as f:
-            f.write(text)
+    emit(res, args.out and os.path.join(args.out, "odometry_streams_adapt_group.json"))
 
 
 if __name__ == "__main__":

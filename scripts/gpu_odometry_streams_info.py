@@ -12,20 +12,18 @@ The card's name, power limit and SM clocks are read in the same run.  Writes odo
     python scripts/gpu_odometry_streams_info.py [--seconds 0.5] [--samples 3] [--out DIR]
 """
 import argparse
-import json
 import os
 import statistics
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 import torch  # noqa: E402
 
-from delora_b200 import ops, synthetic  # noqa: E402
+from delora_b200 import ops  # noqa: E402
 from delora_b200.deploy import capi, export  # noqa: E402
-from gpu_odometry_eval import near_identity_blob  # noqa: E402
-from gpu_odometry_streams import DEV, gpu_info, staged, time_replays  # noqa: E402
+from measure import (DEV, GPU_QUERY, alternate, capture, emit, events_ms, gpu_info, model_config,  # noqa: E402
+                     n_stride, near_identity_blob, pairs, staged)
 
 SIZES = ((64, 2048), (64, 720))
 BATCHES = (1, 4, 16)
@@ -49,11 +47,7 @@ class Ticks:
         if info:
             self.info = torch.zeros((S, ops.INFO_ROW), dtype=torch.float32, device=DEV)
             self.out += (self.info,)
-        self.two_ticks()
-        torch.cuda.synchronize()
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self.two_ticks()
+        self.graph = capture(self.two_ticks, warmup=1)      # the warm-up caches the first frames
 
     def two_ticks(self):
         for pts, counts in self.frames:
@@ -83,24 +77,20 @@ def main():
     ap.add_argument("--out", default="")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs a GPU"
-    res = {"gpu_before": gpu_info(), "gpu_query": "name, power.limit, clocks.sm, clocks.max.sm",
+    res = {"gpu_before": gpu_info(), "gpu_query": GPU_QUERY,
            "seconds_per_sample": args.seconds, "sizes": {}}
     for h, w in SIZES:
-        cfg = synthetic.fov_config(h=h, w=w, device=DEV)
-        cfg.update({"activation_fct": "tanh", "use_single_mlp_at_output": False, "layers": [2, 2, 2, 2],
-                    "resnet_outputs": 1000, "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1,
-                    "use_dropout": False})
+        cfg = model_config(h, w)
         blob = near_identity_blob(cfg)
-        pairs_all = [synthetic.make_pair(i, w_raw=2048, rings=h)[:2] for i in range(max(BATCHES))]
-        n_stride = max(max(a.shape[1], b.shape[1]) for a, b in pairs_all)
+        pairs_all = pairs(h, max(BATCHES))
+        stride = n_stride(pairs_all)
         streams = {}
         for n in BATCHES:
-            pairs = pairs_all[:n]
-            resid, info = Ticks(cfg, blob, pairs, n_stride, False), Ticks(cfg, blob, pairs, n_stride, True)
-            xs, ys = [], []
-            for _ in range(args.samples):
-                xs.append(time_replays(resid.graph.replay, args.seconds)[0] / 2)      # two ticks per replay
-                ys.append(time_replays(info.graph.replay, args.seconds)[0] / 2)
+            ps = pairs_all[:n]
+            resid, info = Ticks(cfg, blob, ps, stride, False), Ticks(cfg, blob, ps, stride, True)
+            t = alternate({"resid": resid.graph.replay, "info": info.graph.replay}, args.samples,
+                          lambda fn: events_ms(fn, seconds=args.seconds)[0] / 2)      # two ticks per replay
+            xs, ys = t["resid"], t["info"]
             torch.cuda.synchronize()
             ms_r, ms_i = statistics.median(xs), statistics.median(ys)
             ev = info.info[:, 36:42].cpu()
@@ -113,14 +103,9 @@ def main():
                           "workspace_MiB": [resid.ws.workspace.numel() / 2**20, info.ws.workspace.numel() / 2**20]}
             del resid, info
             torch.cuda.empty_cache()
-        res["sizes"][f"{h}x{w}"] = {"n_stride": n_stride, "streams_S": streams}
+        res["sizes"][f"{h}x{w}"] = {"n_stride": stride, "streams_S": streams}
     res["gpu_after"] = gpu_info()
-    text = json.dumps(res, indent=1)
-    print(text)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "odometry_streams_info.json"), "w") as f:
-            f.write(text)
+    emit(res, args.out and os.path.join(args.out, "odometry_streams_info.json"))
 
 
 if __name__ == "__main__":

@@ -2,7 +2,7 @@
 differs from the raw-scan one.
 
 Per tick, ms at S in {1, 4, 16} for 64 x 720 and 64 x 2048, both with w_pre 2250, all streams active,
-graph-replayed, on the same near-identity weights (gpu_odometry_eval.near_identity_blob):
+graph-replayed, on the same near-identity weights (measure.near_identity_blob):
   push           delora_odometry_streams_push (raw scans projected at H x W, the image cache);
   push_residual  delora_odometry_streams_push_residual (the same, plus normals at H x W and the ICP);
   push_pre       delora_odometry_streams_push_pre (projection + normals at H x w_pre, both frames of every pair
@@ -17,7 +17,6 @@ run.  Writes odometry_streams_pre.json to --out.
     python scripts/gpu_odometry_streams_pre.py [--seconds 0.5] [--samples 5] [--out DIR]
 """
 import argparse
-import json
 import os
 import statistics
 import sys
@@ -26,10 +25,10 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 import torch  # noqa: E402
 
-from delora_b200 import ops, synthetic  # noqa: E402
+from delora_b200 import ops  # noqa: E402
 from delora_b200.deploy import capi, export  # noqa: E402
-from gpu_odometry_eval import near_identity_blob  # noqa: E402
-from gpu_odometry_streams import DEV, gpu_info, staged, time_replays  # noqa: E402
+from measure import (DEV, GPU_QUERY, alternate, capture, emit, events_ms, gpu_info, model_config,  # noqa: E402
+                     n_stride, near_identity_blob, pairs, staged)
 
 SIZES = ((64, 720), (64, 2048))
 W_PRE = 2250
@@ -52,11 +51,7 @@ class StreamTicks:
                     torch.zeros((S,), dtype=torch.int32, device=DEV))
         if kind != "push":
             self.out += (torch.zeros((S, ops.LOSS_ROW), dtype=torch.float32, device=DEV),)
-        self.two_ticks()                 # first frames cached; warms the launchers' host-side state
-        torch.cuda.synchronize()
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self.two_ticks()
+        self.graph = capture(self.two_ticks, warmup=1)      # the warm-up caches the first frames
 
     def two_ticks(self):
         for pts, counts in self.frames:
@@ -84,26 +79,20 @@ def main():
     ap.add_argument("--out", default="")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs a GPU"
-    res = {"gpu_before": gpu_info(), "gpu_query": "name, power.limit, clocks.sm, clocks.max.sm",
+    res = {"gpu_before": gpu_info(), "gpu_query": GPU_QUERY,
            "seconds_per_sample": args.seconds, "w_pre": W_PRE, "sizes": {}}
     for h, w in SIZES:
-        cfg = synthetic.fov_config(h=h, w=w, device=DEV)
-        cfg.update({"activation_fct": "tanh", "use_single_mlp_at_output": False, "layers": [2, 2, 2, 2],
-                    "resnet_outputs": 1000, "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1,
-                    "use_dropout": False})
+        cfg = model_config(h, w)
         cfg["kitti"]["horizontal_cells_preprocessing"] = W_PRE
         blob = near_identity_blob(cfg)
-        pairs_all = [synthetic.make_pair(i, w_raw=2048, rings=h)[:2] for i in range(max(STREAMS))]
-        n_stride = max(max(a.shape[1], b.shape[1]) for a, b in pairs_all)
-        n_diff, n_pix = differing_pixels(cfg, [s for p in pairs_all for s in p], n_stride)
+        pairs_all = pairs(h, max(STREAMS))
+        stride = n_stride(pairs_all)
+        n_diff, n_pix = differing_pixels(cfg, [s for p in pairs_all for s in p], stride)
         per_s = {}
         for S in STREAMS:
-            pairs = pairs_all[:S]
-            sides = {k: StreamTicks(cfg, blob, pairs, n_stride, k) for k in ("push", "push_residual", "push_pre")}
-            samples = {k: [] for k in sides}
-            for _ in range(args.samples):
-                for k, side in sides.items():
-                    samples[k].append(time_replays(side.graph.replay, args.seconds)[0] / 2)     # two ticks per replay
+            sides = {k: StreamTicks(cfg, blob, pairs_all[:S], stride, k) for k in ("push", "push_residual", "push_pre")}
+            samples = alternate({k: side.graph.replay for k, side in sides.items()}, args.samples,
+                                lambda fn: events_ms(fn, seconds=args.seconds)[0] / 2)     # two ticks per replay
             torch.cuda.synchronize()
             med = {k: statistics.median(v) for k, v in samples.items()}
             per_s[S] = {**{f"{k}_ms_per_tick": m for k, m in med.items()},
@@ -114,17 +103,12 @@ def main():
                         "workspace_MiB": {k: s.ws.workspace.numel() / 2**20 for k, s in sides.items()}}
             del sides
             torch.cuda.empty_cache()
-        res["sizes"][f"{h}x{w}"] = {"n_stride": n_stride, "streams_S": per_s,
+        res["sizes"][f"{h}x{w}"] = {"n_stride": stride, "streams_S": per_s,
                                     "recipe_vs_raw_image": {"differing_pixels": n_diff, "pixels": n_pix,
                                                             "fraction": n_diff / n_pix,
                                                             "scans": 2 * max(STREAMS)}}
     res["gpu_after"] = gpu_info()
-    text = json.dumps(res, indent=1)
-    print(text)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "odometry_streams_pre.json"), "w") as f:
-            f.write(text)
+    emit(res, args.out and os.path.join(args.out, "odometry_streams_pre.json"))
 
 
 if __name__ == "__main__":

@@ -10,20 +10,18 @@ Writes odometry_streams_pre_adapt_info.json to --out.
     python scripts/gpu_odometry_streams_pre_adapt_info.py [--seconds 0.3] [--samples 3] [--out DIR]
 """
 import argparse
-import json
 import os
 import statistics
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 import torch  # noqa: E402
 
-from delora_b200 import ops, synthetic  # noqa: E402
+from delora_b200 import ops  # noqa: E402
 from delora_b200.deploy import capi, export  # noqa: E402
-from gpu_odometry_eval import near_identity_blob  # noqa: E402
-from gpu_odometry_streams import DEV, gpu_info, staged, time_replays  # noqa: E402
+from measure import (DEV, GPU_QUERY, alternate, capture, emit, events_ms, gpu_info, model_config,  # noqa: E402
+                     n_stride, near_identity_blob, pairs, staged)
 
 SIZES = ((64, 2048), (64, 720))
 BATCHES = (1, 4, 16)
@@ -52,11 +50,7 @@ class Ticks:
         self.valid = torch.zeros((S,), dtype=torch.int32, device=DEV)
         self.losses = torch.zeros((S, ops.LOSS_ROW), dtype=torch.float32, device=DEV)
         self.rows = torch.zeros((S, ops.INFO_ROW), dtype=torch.float32, device=DEV)
-        self.two_ticks()
-        torch.cuda.synchronize()
-        self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
-            self.two_ticks()
+        self.graph = capture(self.two_ticks, warmup=1)      # the warm-up caches the first frames
 
     def two_ticks(self):
         out = (self.T, self.valid, self.losses) + ((self.rows,) if self.info else ())
@@ -74,27 +68,22 @@ def main():
     ap.add_argument("--out", default="")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs a GPU"
-    res = {"gpu_before": gpu_info(), "gpu_query": "name, power.limit, clocks.sm, clocks.max.sm",
+    res = {"gpu_before": gpu_info(), "gpu_query": GPU_QUERY,
            "seconds_per_sample": args.seconds, "w_pre_of_pre": W_PRE, "sizes": {}}
     for h, w in SIZES:
-        cfg = synthetic.fov_config(h=h, w=w, device=DEV)
-        cfg.update({"activation_fct": "tanh", "use_single_mlp_at_output": False, "layers": [2, 2, 2, 2],
-                    "resnet_outputs": 1000, "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1,
-                    "use_dropout": False})
+        cfg = model_config(h, w)
         cfg["kitti"]["horizontal_cells_preprocessing"] = W_PRE
         blob = near_identity_blob(cfg)
-        pairs_all = [synthetic.make_pair(i, w_raw=2048, rings=h)[:2] for i in range(max(BATCHES))]
-        n_stride = max(max(a.shape[1], b.shape[1]) for a, b in pairs_all)
+        pairs_all = pairs(h, max(BATCHES))
+        stride = n_stride(pairs_all)
         per = {}
         for mode in ("pre", "adapt"):
             for n in BATCHES:
-                pairs = pairs_all[:n]
-                a = Ticks(cfg, blob, pairs, n_stride, mode, False)
-                b = Ticks(cfg, blob, pairs, n_stride, mode, True)
-                xs, ys = [], []
-                for _ in range(args.samples):
-                    xs.append(time_replays(a.graph.replay, args.seconds)[0] / 2)      # two ticks per replay
-                    ys.append(time_replays(b.graph.replay, args.seconds)[0] / 2)
+                a = Ticks(cfg, blob, pairs_all[:n], stride, mode, False)
+                b = Ticks(cfg, blob, pairs_all[:n], stride, mode, True)
+                t = alternate({"a": a.graph.replay, "b": b.graph.replay}, args.samples,
+                              lambda fn: events_ms(fn, seconds=args.seconds)[0] / 2)      # two ticks per replay
+                xs, ys = t["a"], t["b"]
                 torch.cuda.synchronize()
                 ms_a, ms_b = statistics.median(xs), statistics.median(ys)
                 per[f"{mode}_S{n}"] = {
@@ -107,15 +96,9 @@ def main():
                 print(f"{h}x{w} {mode} S={n}: {ms_a:.3f} -> {ms_b:.3f} ms per tick", flush=True)
                 del a, b
                 torch.cuda.empty_cache()
-        res["sizes"][f"{h}x{w}"] = {"n_stride": n_stride, "ticks": per}
+        res["sizes"][f"{h}x{w}"] = {"n_stride": stride, "ticks": per}
     res["gpu_after"] = gpu_info()
-    text = json.dumps(res, indent=1)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "odometry_streams_pre_adapt_info.json"), "w") as f:
-            f.write(text)
-    else:
-        print(text)
+    emit(res, args.out and os.path.join(args.out, "odometry_streams_pre_adapt_info.json"))
 
 
 if __name__ == "__main__":

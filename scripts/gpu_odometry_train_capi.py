@@ -11,25 +11,18 @@ kernels this path adds (the tail backward, Adam, the ICP scratch re-arm) against
 Prints the result as JSON; with --out it is also written to DIR/odometry_train_capi.json.
 """
 import argparse
-import json
 import os
-import statistics
-import subprocess
 import sys
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
+from measure import DEV, alternate, emit, events_ms, gpu_info, n_stride, staged, summary  # noqa: E402
+
 HBM_BYTES_PER_S = 3.35e12
 NEW_KERNELS = ("odometry_out_bwd_kernel", "odometry_linear_bwd_kernel", "odometry_adam_kernel",
                "odometry_icp_rearm_kernel")
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
 
 
 def main():
@@ -46,26 +39,17 @@ def main():
     from delora_b200 import _lib, synthetic
     from delora_b200.deploy import capi, export
     from delora_b200.train_step import SyntheticTrainStep
-    dev = torch.device("cuda:0")
     b = a.batch
-    scans = []
-    for i in range(b):
-        s1, s2, _, _ = synthetic.make_pair(i, w_raw=a.w, rings=a.h)
-        scans.append((s1, s2))
-    n_max = max(max(x.shape[1], y.shape[1]) for x, y in scans)
-    allsc = [s[0] for s in scans] + [s[1] for s in scans]
-    pts = torch.zeros((2 * b, 3, n_max), dtype=torch.float32)
-    for i, s in enumerate(allsc):
-        pts[i, :, :s.shape[1]] = s
-    counts = torch.tensor([s.shape[1] for s in allsc], dtype=torch.int32)
-    pts, counts = pts.to(dev), counts.to(dev)
+    scans = [synthetic.make_pair(i, w_raw=a.w, rings=a.h)[:2] for i in range(b)]
+    n_max = n_stride(scans)
+    pts, counts = staged([s[0] for s in scans] + [s[1] for s in scans], n_max)
 
-    cfg = synthetic.fov_config(h=a.h, w=a.w, device="cuda:0")
+    cfg = synthetic.fov_config(h=a.h, w=a.w, device=DEV)
     torch.manual_seed(0)
     py = SyntheticTrainStep(cfg, b, n_max)
     py.load(pts, counts)
     cfg = py.cfg
-    blob = torch.from_numpy(export.pack_state_dict(py.model.state_dict(), cfg)).to(dev)
+    blob = torch.from_numpy(export.pack_state_dict(py.model.state_dict(), cfg)).to(DEV)
     tr = capi.TrainingWorkspace(export.desc_from_config(cfg, "kitti", n_max, b), blob,
                                 capi.train_params(cfg, py.optimizer.param_groups[0]["lr"]))
     ws_bytes = tr.workspace.numel()
@@ -74,25 +58,13 @@ def main():
         # B = rows // 2: at bsz < b the step reads the buffer's first 2 * bsz rows (they serve the timing only)
         tr.step(pts[:2 * bsz], counts[:2 * bsz], outputs=False)
 
-    def timed(fn):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        fn()
-        e1.record()
-        e1.synchronize()
-        return e0.elapsed_time(e1)
-
     for _ in range(a.warmup):
         c_step()
         py.step()
     torch.cuda.synchronize()
-    t_c, t_py = [], []
-    for _ in range(a.rounds):
-        t_c.append(timed(c_step))
-        t_py.append(timed(py.step))
-    res = {"card": card(), "batch": b, "H": a.h, "W": a.w, "workspace_bytes": ws_bytes,
-           "c_step_ms": {"median": statistics.median(t_c), "min": min(t_c), "max": max(t_c)},
-           "synthetic_train_step_ms": {"median": statistics.median(t_py), "min": min(t_py), "max": max(t_py)}}
+    t = alternate({"c": c_step, "py": py.step}, a.rounds, lambda fn: events_ms(fn, calls=1)[0])
+    res = {"card": gpu_info(), "batch": b, "H": a.h, "W": a.w, "workspace_bytes": ws_bytes,
+           "c_step_ms": summary(t["c"]), "synthetic_train_step_ms": summary(t["py"])}
 
     # per-kernel times in a separate, profiled pass; the re-arm kernel once with an unchanged B (every CTA exits) and
     # once after a step with another B (it zeroes the ICP scratch)
@@ -124,11 +96,7 @@ def main():
             v["floor_us"] = floors[k] / HBM_BYTES_PER_S * 1e6
     res["kernels"] = kernels
     res["new_kernels_us_per_step"] = sum(v["us_per_call"] * v.get("calls_per_step", 0) for v in kernels.values())
-    if a.out:
-        os.makedirs(a.out, exist_ok=True)
-        with open(os.path.join(a.out, "odometry_train_capi.json"), "w") as f:
-            json.dump(res, f, indent=1)
-    print(json.dumps(res, indent=1))
+    emit(res, a.out and os.path.join(a.out, "odometry_train_capi.json"))
 
 
 if __name__ == "__main__":

@@ -17,20 +17,18 @@ queries.  The card's name, power limit and SM clocks are read in the same run.  
 """
 import argparse
 import ctypes
-import json
 import os
 import statistics
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 import torch  # noqa: E402
 
 from delora_b200 import _lib, synthetic  # noqa: E402
 from delora_b200.deploy import capi, export  # noqa: E402
-from gpu_odometry_eval import near_identity_blob  # noqa: E402
-from gpu_odometry_streams import DEV, gpu_info, staged  # noqa: E402
+from measure import (GPU_QUERY, alternate, capture, emit, events_ms, gpu_info, model_config,  # noqa: E402
+                     near_identity_blob, paired, staged)
 
 KITTI = (-24.5, 2.0)
 GEOMETRIES = {"64x2048": (64, 2048, KITTI, 0), "64x720_w2250": (64, 720, KITTI, 2250),
@@ -38,47 +36,21 @@ GEOMETRIES = {"64x2048": (64, 2048, KITTI, 0), "64x720_w2250": (64, 720, KITTI, 
 SETS = (("64x2048", "64x720_w2250"), ("64x720_w2250", "64x512_w512"))
 
 
-def model_config(h, w, vfov):
-    cfg = synthetic.fov_config(h=h, w=w, vfov_deg=vfov, device=DEV)
-    cfg.update({"activation_fct": "tanh", "use_single_mlp_at_output": False, "layers": [2, 2, 2, 2],
-                "resnet_outputs": 1000, "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1,
-                "use_dropout": False})
-    return cfg
-
-
 def geometry(name, B, max_batch):
     """-> (descriptor for max_batch pairs, points, counts) of B synthetic pairs at the geometry."""
     h, w, vfov, w_pre = GEOMETRIES[name]
     pairs = [synthetic.make_pair(i, w_raw=2048, rings=h, vfov_deg=vfov)[:2] for i in range(B)]
     n_stride = max(max(a.shape[1], b.shape[1]) for a, b in pairs)
-    d = export.desc_from_config(model_config(h, w, vfov), "kitti", n_stride, max_batch)
+    d = export.desc_from_config(model_config(h, w, vfov=vfov), "kitti", n_stride, max_batch)
     d.w_pre = w_pre
     pts, counts = staged([p[0] for p in pairs] + [p[1] for p in pairs], n_stride)
     return d, pts, counts
 
 
-def capture(fn):
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        fn()
-    torch.cuda.synchronize()
-    return g
-
-
-def time_graph(g, seconds):
-    """ms per replay, device events around at least `seconds` of replays (calibrated on a first short run)."""
-    start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-
-    def run(n):
-        start.record()
-        for _ in range(n):
-            g.replay()
-        end.record()
-        end.synchronize()
-        return start.elapsed_time(end) / n
-
-    n = max(3, int(seconds * 1e3 / max(run(3), 1e-3)))
-    return run(n)
+def replays_ms(fn, seconds):
+    """ms per call of fn, CUDA events around at least `seconds` of calls (the count from a first run of 3)."""
+    n = max(3, int(seconds * 1e3 / max(events_ms(fn, calls=3)[0], 1e-3)))
+    return events_ms(fn, calls=n)[0]
 
 
 def measure(names, max_batch, B, blob, seconds, samples):
@@ -99,8 +71,8 @@ def measure(names, max_batch, B, blob, seconds, samples):
         for k in range(10):
             ws.use(k % 2)
 
-    g_use = capture(alternate_uses)
-    out["use_samples_ms"] = [time_graph(g_use, seconds) / 10 for _ in range(samples)]
+    g_use = capture(alternate_uses, warmup=0)
+    out["use_samples_ms"] = [replays_ms(g_use.replay, seconds) / 10 for _ in range(samples)]
     out["use_ms"] = statistics.median(out["use_samples_ms"])
     for g, name in enumerate(names):
         def switched(g=g):
@@ -111,14 +83,13 @@ def measure(names, max_batch, B, blob, seconds, samples):
             ws.step(geo[g][1], geo[g][2], outputs=False)
 
         ws.use(g)
-        g_switch, g_steady = capture(switched), capture(steady)
-        xs, ys = [], []
-        for _ in range(samples):
-            xs.append(time_graph(g_steady, seconds))
-            ys.append(time_graph(g_switch, seconds))
-        diffs = [y - x for x, y in zip(xs, ys)]
+        g_switch, g_steady = capture(switched, warmup=0), capture(steady, warmup=0)
+        t = alternate({"steady": g_steady.replay, "switch": g_switch.replay}, samples,
+                      lambda fn: replays_ms(fn, seconds))
+        xs, ys = t["steady"], t["switch"]
+        diffs, diff = paired(xs, ys)
         out[name] = {"steady_step_ms": statistics.median(xs), "step_after_switch_ms": statistics.median(ys),
-                     "paired_difference_ms": statistics.median(diffs), "steady_samples_ms": xs,
+                     "paired_difference_ms": diff, "steady_samples_ms": xs,
                      "after_switch_samples_ms": ys, "paired_differences_ms": diffs}
         del g_switch, g_steady
     del g_use, ws
@@ -136,7 +107,7 @@ def main():
     assert torch.cuda.is_available(), "needs a GPU"
     torch.cuda.set_device(0)
     blob = near_identity_blob(model_config(64, 720, KITTI))
-    res = {"gpu_before": gpu_info(), "gpu_query": "name, power.limit, clocks.sm, clocks.max.sm",
+    res = {"gpu_before": gpu_info(), "gpu_query": GPU_QUERY,
            "seconds_per_sample": args.seconds, "geometries": {k: {"H": v[0], "W": v[1], "vfov_deg": v[2],
                                                                   "w_pre": v[3]} for k, v in GEOMETRIES.items()},
            "sets": {}}
@@ -145,12 +116,7 @@ def main():
         res["sets"][key] = [measure(names, int(mb), int(b), blob, args.seconds, args.samples)
                             for mb, b in (c.split(":") for c in args.configs.split(","))]
     res["gpu_after"] = gpu_info()
-    text = json.dumps(res, indent=1)
-    print(text)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "train_geometries.json"), "w") as f:
-            f.write(text)
+    emit(res, args.out and os.path.join(args.out, "train_geometries.json"))
 
 
 if __name__ == "__main__":

@@ -14,36 +14,19 @@ The card's name, power limit and SM clocks are read in the same run.  Writes tra
     python scripts/gpu_train_group.py [--gpus N] [--batch 16] [--seconds 0.5] [--samples 5] [--out DIR]
 """
 import argparse
-import ctypes
-import json
 import os
 import statistics
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 import torch  # noqa: E402
 
-from delora_b200 import synthetic  # noqa: E402
 from delora_b200.deploy import capi, export  # noqa: E402
-from gpu_odometry_eval import near_identity_blob  # noqa: E402
-from gpu_odometry_streams import DEV, gpu_info, staged  # noqa: E402
+from measure import (GPU_QUERY, alternate, capture, emit, enable_peer_access, gpu_info, host_ms,  # noqa: E402
+                     model_config, n_stride, near_identity_blob, paired, pairs, staged)
 
 SIZES = ((64, 720), (64, 2048))
-
-
-def enable_peer_access(n):
-    from delora_b200 import _lib
-    _lib.lib()
-    cudart = ctypes.CDLL("libcudart.so.12")        # the runtime libdelora_b200.so loaded
-    for i in range(n):
-        torch.cuda.set_device(i)
-        for j in range(n):
-            if i != j:
-                rc = cudart.cudaDeviceEnablePeerAccess(j, 0)
-                assert rc in (0, 704), f"cudaDeviceEnablePeerAccess({i} -> {j}) failed: {rc}"   # 704: already on
-    torch.cuda.set_device(0)
 
 
 class Ranks:
@@ -68,11 +51,7 @@ class Ranks:
         self.graphs = []
         for r, dev in enumerate(self.devs):
             with torch.cuda.device(dev):
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g, stream=self.streams[r]):
-                    self.step(r)
-                self.graphs.append(g)
-        self.sync()
+                self.graphs.append(capture(lambda r=r: self.step(r), warmup=0, stream=self.streams[r]))
 
     def step(self, r):
         if self.group:
@@ -94,20 +73,6 @@ class Ranks:
         for dev in self.devs:
             torch.cuda.synchronize(dev)
 
-    def time(self, seconds):
-        """ms per replay of every rank's step, over at least `seconds` of work (host clock around synchronised work)."""
-        import time
-        self.sync()
-        n, t0 = 0, time.perf_counter()
-        while True:
-            self.replay()
-            n += 1
-            if n % 8 == 0:
-                self.sync()
-                el = time.perf_counter() - t0
-                if el >= seconds:
-                    return el * 1e3 / n
-
     def status(self):
         return [int(s.item()) for s in self.group.status] if self.group else []
 
@@ -124,36 +89,27 @@ def main():
     assert torch.cuda.device_count() >= args.gpus, f"--gpus {args.gpus}: {torch.cuda.device_count()} GPU(s) here"
     if args.gpus > 1:
         enable_peer_access(args.gpus)
-    res = {"gpu_before": gpu_info(), "gpu_query": "name, power.limit, clocks.sm, clocks.max.sm", "gpus": args.gpus,
+    res = {"gpu_before": gpu_info(), "gpu_query": GPU_QUERY, "gpus": args.gpus,
            "batch_per_gpu": args.batch, "seconds_per_sample": args.seconds, "sizes": {}}
     for h, w in SIZES:
-        cfg = synthetic.fov_config(h=h, w=w, device=DEV)
-        cfg.update({"activation_fct": "tanh", "use_single_mlp_at_output": False, "layers": [2, 2, 2, 2],
-                    "resnet_outputs": 1000, "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1,
-                    "use_dropout": False})
+        cfg = model_config(h, w)
         blob = near_identity_blob(cfg)
-        pairs = [synthetic.make_pair(i, w_raw=2048, rings=h)[:2] for i in range(args.batch)]
-        n_stride = max(max(a.shape[1], b.shape[1]) for a, b in pairs)
-        plain = Ranks(cfg, blob, pairs, n_stride, args.gpus, False)
-        group = Ranks(cfg, blob, pairs, n_stride, args.gpus, True)
-        xs, ys = [], []
-        for _ in range(args.samples):
-            xs.append(plain.time(args.seconds))
-            ys.append(group.time(args.seconds))
-        diffs = [y - x for x, y in zip(xs, ys)]
+        ps = pairs(h, args.batch)
+        stride = n_stride(ps)
+        plain = Ranks(cfg, blob, ps, stride, args.gpus, False)
+        group = Ranks(cfg, blob, ps, stride, args.gpus, True)
+        t = alternate({"plain": plain, "group": group}, args.samples,
+                      lambda ranks: host_ms(ranks.replay, args.seconds, ranks.devs, every=8, warmup=0))
+        xs, ys = t["plain"], t["group"]
+        diffs, diff = paired(xs, ys)
         res["sizes"][f"{h}x{w}"] = {
-            "n_stride": n_stride, "train_step_ms": statistics.median(xs), "train_step_group_ms": statistics.median(ys),
-            "paired_difference_ms": statistics.median(diffs), "train_step_samples_ms": xs,
+            "n_stride": stride, "train_step_ms": statistics.median(xs), "train_step_group_ms": statistics.median(ys),
+            "paired_difference_ms": diff, "train_step_samples_ms": xs,
             "train_step_group_samples_ms": ys, "paired_differences_ms": diffs, "status": group.status()}
         del plain, group
         torch.cuda.empty_cache()
     res["gpu_after"] = gpu_info()
-    text = json.dumps(res, indent=1)
-    print(text)
-    if args.out:
-        os.makedirs(args.out, exist_ok=True)
-        with open(os.path.join(args.out, "train_group.json"), "w") as f:
-            f.write(text)
+    emit(res, args.out and os.path.join(args.out, "train_group.json"))
 
 
 if __name__ == "__main__":

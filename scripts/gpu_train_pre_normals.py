@@ -16,38 +16,19 @@ DIR/train_pre_normals.json).
 """
 import argparse
 import ctypes
-import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
+from measure import (DEV, alternate, capture, emit, events_ms, gpu_info, model_config, n_stride, paired,  # noqa: E402
+                     pairs, staged, summary, untrained_blob)
+
 HBM_BYTES_PER_S = 3.35e12
 H, W, W_PRE, W_RAW = 64, 720, 2250, 2048
-
-
-def card():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
-
-
-def timed(fn, reps=1):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    e1.synchronize()
-    return e0.elapsed_time(e1) / reps
-
-
-def summary(ts):
-    return {"median": statistics.median(ts), "min": min(ts), "max": max(ts)}
 
 
 def main():
@@ -61,60 +42,37 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("no CUDA device: this script measures the GPU")
-    from delora_b200 import _lib, ops, synthetic
+    from delora_b200 import _lib, ops
     from delora_b200.deploy import capi, export
-    from delora_b200.models.model import OdometryModel
-    dev = torch.device("cuda:0")
     L = _lib.lib()
     st = lambda: ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
     batches = [int(v) for v in a.batches.split(",")]
-    b_max = max(batches)
-    pairs = [synthetic.make_pair(i, w_raw=W_RAW, rings=H)[:2] for i in range(b_max)]
-    n_max = max(max(x.shape[1], y.shape[1]) for x, y in pairs)
+    ps = pairs(H, max(batches))
+    n_max = n_stride(ps)
 
-    cfg = synthetic.fov_config(h=H, w=W, device="cuda:0")
-    cfg.update({"activation_fct": "tanh", "use_single_mlp_at_output": False, "layers": [2, 2, 2, 2],
-                "resnet_outputs": 1000, "pre_feature_extraction": False, "factor_fewer_resnet_channels": 1,
-                "use_dropout": False, "lambda_po2pl": 1.0})
-    torch.manual_seed(0)
-    blob = torch.from_numpy(export.pack_state_dict(OdometryModel(cfg).state_dict(), cfg)).to(dev)
+    cfg = model_config(H, W)
+    blob = untrained_blob(cfg)
     hp = capi.train_params(cfg, 1e-6)
-    res = {"card": card(), "H": H, "W": W, "w_pre": W_PRE, "scan_columns": W_RAW, "steps": {}}
+    res = {"card": gpu_info(), "H": H, "W": W, "w_pre": W_PRE, "scan_columns": W_RAW, "steps": {}}
 
     for b in batches:
-        scans = [p[0] for p in pairs[:b]] + [p[1] for p in pairs[:b]]
-        pts = torch.zeros((2 * b, 3, n_max), dtype=torch.float32)
-        for i, s in enumerate(scans):
-            pts[i, :, :s.shape[1]] = s
-        counts = torch.tensor([s.shape[1] for s in scans], dtype=torch.int32)
-        pts, counts = pts.to(dev), counts.to(dev)
+        pts, counts = staged([p[0] for p in ps[:b]] + [p[1] for p in ps[:b]], n_max)
         runs = {}
         for w_pre in (0, W_PRE):
             d = export.desc_from_config(cfg, "kitti", n_max, b)
             d.w_pre = w_pre
             runs[w_pre] = capi.TrainingWorkspace(d, blob, hp)
 
-        def step(w_pre):
-            runs[w_pre].step(pts, counts, outputs=False)
-
-        for _ in range(a.warmup):
-            step(0)
-            step(W_PRE)
-        torch.cuda.synchronize()
         # one captured step per setting: a sample is the mean of `replays` back-to-back replays (no host gaps), the
         # settings alternate sample by sample, and the cost of the option is the paired difference of adjacent samples
         graphs = {}
         for w_pre in (0, W_PRE):
-            graphs[w_pre] = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graphs[w_pre]):
-                step(w_pre)
+            graphs[w_pre] = capture(lambda w_pre=w_pre: runs[w_pre].step(pts, counts, outputs=False), warmup=a.warmup)
             graphs[w_pre].replay()
         torch.cuda.synchronize()
-        t = {0: [], W_PRE: []}
-        for _ in range(a.rounds):
-            for w_pre in (0, W_PRE):
-                t[w_pre].append(timed(graphs[w_pre].replay, a.replays))
-        deltas = [y - x for x, y in zip(t[0], t[W_PRE])]
+        t = alternate({w_pre: g.replay for w_pre, g in graphs.items()}, a.rounds,
+                      lambda fn: events_ms(fn, calls=a.replays)[0])
+        deltas, _ = paired(t[0], t[W_PRE])
         res["steps"][b] = {"workspace_bytes": {str(k): int(v.workspace.numel()) for k, v in runs.items()},
                            "samples": a.rounds, "replays_per_sample": a.replays,
                            "step_ms_w_pre_0": summary(t[0]), f"step_ms_w_pre_{W_PRE}": summary(t[W_PRE]),
@@ -123,13 +81,13 @@ def main():
         torch.cuda.empty_cache()
 
     # the re-projection alone, 2 * b_max scans
-    scans = [p[0] for p in pairs] + [p[1] for p in pairs]
+    scans = [p[0] for p in ps] + [p[1] for p in ps]
     s = len(scans)
     pts = torch.full((s, 3, n_max), float("nan"))
     for i, c in enumerate(scans):
         pts[i, :, :c.shape[1]] = c
     counts = torch.tensor([c.shape[1] for c in scans], dtype=torch.int32)
-    pts, counts = pts.to(dev), counts.to(dev)
+    pts, counts = pts.to(DEV), counts.to(DEV)
     hf, vf = cfg["horizontal_field_of_view"], cfg["kitti"]["vertical_field_of_view"]
     image_pre, _, pg, ng = ops.project_normals(pts, counts, H, W_PRE, hf, vf)
     normals = ops.normals(image_pre)
@@ -153,18 +111,15 @@ def main():
     for _ in range(5):
         new()
         old()
-    tn, to = [], []
-    for _ in range(5):
-        tn.append(timed(new, a.reps))
-        to.append(timed(old, a.reps))
+    t = alternate({"new": new, "old": old}, 5, lambda fn: events_ms(fn, calls=a.reps)[0])
     # bytes the two kernels must move: the pre-resolution points grid once (scatter), per model pixel its key
     # read + re-arm, the image, and the two grids; per kept point its two pre-grid entries (gathers)
     kept = int((a_pg[:, :, 3].view(torch.int32) >= 0).sum())
     bytes_ = s * H * W_PRE * 16 + s * H * W * (16 + 16 + 32) + kept * 32
     # the public wrapper allocates its four outputs with torch each call; time the bare C call too
-    img = torch.empty((s, 4, H, W), device=dev)
-    opg, ong = torch.empty((s, H * W, 4), device=dev), torch.empty((s, H * W, 4), device=dev)
-    keys = ops._keys(dev, s, H * W)
+    img = torch.empty((s, 4, H, W), device=DEV)
+    opg, ong = torch.empty((s, H * W, 4), device=DEV), torch.empty((s, H * W, 4), device=DEV)
+    keys = ops._keys(torch.device(DEV), s, H * W)
 
     def bare():
         _lib.check(L.delora_project_grids_fwd(pg.data_ptr(), ng.data_ptr(), s, H, W_PRE, W, hf[0], hf[1], vf[0], vf[1], 0,
@@ -172,17 +127,13 @@ def main():
                                               st()), "project_grids")
 
     bare()
-    tb = [timed(bare, a.reps) for _ in range(5)]
+    tb = [events_ms(bare, calls=a.reps)[0] for _ in range(5)]
     res["reprojection"] = {
         "scans": s, "bit_identical": same, "kept_points": kept,
-        "project_grids_ms": summary(tb), "ops_project_grids_ms": summary(tn), "list_path_ms": summary(to),
+        "project_grids_ms": summary(tb), "ops_project_grids_ms": summary(t["new"]), "list_path_ms": summary(t["old"]),
         "bytes": bytes_, "floor_ms": bytes_ / HBM_BYTES_PER_S * 1e3,
         "bandwidth_TB_s": bytes_ / (statistics.median(tb) * 1e-3) / 1e12}
-    if a.out:
-        os.makedirs(a.out, exist_ok=True)
-        with open(os.path.join(a.out, "train_pre_normals.json"), "w") as f:
-            json.dump(res, f, indent=1)
-    print(json.dumps(res, indent=1))
+    emit(res, a.out and os.path.join(a.out, "train_pre_normals.json"))
 
 
 if __name__ == "__main__":
