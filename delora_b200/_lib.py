@@ -78,6 +78,9 @@ SIGNATURES = {
     "delora_project_normals_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_double, c_double,
                                            c_double, c_double, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                            c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "delora_project_points_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_double, c_double,
+                                          c_double, c_double, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                          c_void_p]),
     "delora_scan_blocks": (c_int, [c_int]),
     "delora_lists_from_images": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                          c_void_p, c_void_p, c_void_p, c_void_p]),
@@ -149,6 +152,7 @@ SIGNATURES = {
                                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "delora_trunk_backward_dropout": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                               c_void_p, c_int, c_void_p, c_void_p]),
+    "delora_odometry_file_objective": (c_int, [c_void_p, c_void_p, c_void_p]),
     "delora_odometry_weight_floats": (c_i64, [c_desc_p]),
     "delora_odometry_workspace_bytes": (c_i64, [c_desc_p]),
     "delora_odometry_init": (c_int, [c_desc_p, c_void_p, c_void_p]),
@@ -235,6 +239,8 @@ ABI_VERSION = 3
 # model_flags bits of the .dlw / .dlt header (DELORA_MODEL_* in include/delora_b200.h)
 MODEL_NORMALIZATION_SCALING = 1
 MODEL_DROPOUT = 2
+# the loss_flags bits a .dlw / .dlt header's objective_flags holds (DELORA_LOSS_* / DELORA_NORMAL_LINEAR)
+LOSS_PO2PO, LOSS_PO2PL, LOSS_PL2PL, NORMAL_LINEAR, LOSS_PO2PO_ALONE = 1, 2, 4, 8, 4096
 _lib = None
 
 

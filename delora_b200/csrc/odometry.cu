@@ -153,10 +153,25 @@ static int project_normalized(const Frames& f, const delora_odometry_desc* d, ch
                        st);
 }
 
+// DELORA_LOSS_PO2PO_ALONE's companions: PO2PO required, the normal-reading bits refused, each named
+static int check_po2po_alone(uint32_t loss_flags, const char* field, const char* who) {
+    if ((loss_flags & DELORA_LOSS_PO2PO_ALONE) == 0u) return 0;
+    DELORA_CHECK_ARG((loss_flags & DELORA_LOSS_PO2PO) != 0u,
+                     "%s: %s=0x%x has DELORA_LOSS_PO2PO_ALONE without DELORA_LOSS_PO2PO", who, field, loss_flags);
+    static const struct { uint32_t bit; const char* name; } refused[3] = {
+        {DELORA_LOSS_PO2PL, "DELORA_LOSS_PO2PL"}, {DELORA_LOSS_PL2PL, "DELORA_LOSS_PL2PL"},
+        {DELORA_NORMAL_LINEAR, "DELORA_NORMAL_LINEAR"}};
+    for (const auto& r : refused)
+        DELORA_CHECK_ARG((loss_flags & r.bit) == 0u, "%s: %s=0x%x has DELORA_LOSS_PO2PO_ALONE with %s (po2po_alone "
+                         "reads no normal)", who, field, loss_flags, r.name);
+    return 0;
+}
+
 // The loss and normals' settings of delora_odometry_train_params and delora_odometry_residual_params
 int check_icp_params(float lambda_po2pl, uint32_t loss_flags, int nb_h, int nb_w, float epsilon_range,
                      int min_neighbors, const char* who) {
     DELORA_CHECK_ARG(isfinite(lambda_po2pl), "%s: lambda_po2pl=%g must be finite", who, (double)lambda_po2pl);
+    if (check_po2po_alone(loss_flags, "loss_flags", who)) return 1;
     DELORA_CHECK_ARG((loss_flags & (DELORA_LOSS_PO2PO | DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL)) != 0,
                      "%s: loss_flags=0x%x sets no loss bit", who, loss_flags);
     DELORA_CHECK_ARG(nb_h >= 1 && nb_h % 2 == 1, "%s: nb_h=%d must be odd and positive", who, nb_h);
@@ -165,6 +180,21 @@ int check_icp_params(float lambda_po2pl, uint32_t loss_flags, int nb_h, int nb_w
                      (double)epsilon_range);
     DELORA_CHECK_ARG(min_neighbors >= 0, "%s: min_neighbors=%d must be >= 0", who, min_neighbors);
     return 0;
+}
+
+// The front end of the ICP objectives: n scans projected at H x w with their dense grids.  Under
+// DELORA_LOSS_PO2PO_ALONE no normal is estimated and the normal grid is zero; otherwise the normals of the nb_h x nb_w
+// neighbourhood.  Image, index map and point grid are the same bits either way.
+int project_scan_grids(const delora_odometry_desc* d, int w, uint32_t loss_flags, int nb_h, int nb_w,
+                       float epsilon_range, int min_neighbors, const float* points, const int32_t* counts, int n,
+                       uint64_t* keys, float* image, int32_t* index_map, delora_f4* pts_grid, delora_f4* nrm_grid,
+                       cudaStream_t st) {
+    if (loss_flags & DELORA_LOSS_PO2PO_ALONE)
+        return delora_project_points_fwd(points, counts, n, 3, d->n_stride, d->H, w, d->hfov0, d->hfov1, d->vfov0,
+                                         d->vfov1, 0, keys, image, index_map, pts_grid, nrm_grid, st);
+    return delora_project_normals_fwd(points, counts, n, 3, d->n_stride, d->H, w, d->hfov0, d->hfov1, d->vfov0,
+                                      d->vfov1, 0, keys, image, index_map, nb_h, nb_w, epsilon_range, min_neighbors,
+                                      pts_grid, nrm_grid, nullptr, st);
 }
 
 // Every workspace starts zeroed, with its depth keys at all ones (the projection's empty key).  from > 0: only bytes
@@ -336,6 +366,29 @@ extern "C" int delora_odometry_workspace_sections(int kind, const delora_odometr
                                                   delora_ws_section* out, int cap) {
     int count = 0;
     return workspace_sections(kind, d, n, out, cap, &count) ? -1 : count;
+}
+
+extern "C" int delora_odometry_file_objective(const delora_odometry_file_header* h, uint32_t* loss_flags,
+                                              float* lambda_po2pl) {
+    const char* who = "delora_odometry_file_objective";
+    DELORA_CHECK_ARG(h && loss_flags && lambda_po2pl, "%s: null pointer", who);
+    const uint32_t f = h->objective_flags;
+    if (f == 0u) {                  // written before the field: the shipped objective
+        *loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL;
+        *lambda_po2pl = 1.0f;
+        return 0;
+    }
+    const uint32_t bits = DELORA_LOSS_PO2PO | DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | DELORA_NORMAL_LINEAR |
+                          DELORA_LOSS_PO2PO_ALONE;
+    DELORA_CHECK_ARG((f & ~bits) == 0u, "%s: objective_flags=0x%x has a bit other than the ICP losses, "
+                     "DELORA_NORMAL_LINEAR and DELORA_LOSS_PO2PO_ALONE", who, f);
+    if (check_po2po_alone(f, "objective_flags", who)) return 1;
+    DELORA_CHECK_ARG((f & (DELORA_LOSS_PO2PO | DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL)) != 0u,
+                     "%s: objective_flags=0x%x sets no loss bit", who, f);
+    DELORA_CHECK_ARG(isfinite(h->lambda_po2pl), "%s: lambda_po2pl=%g must be finite", who, (double)h->lambda_po2pl);
+    *loss_flags = f;
+    *lambda_po2pl = h->lambda_po2pl;
+    return 0;
 }
 
 extern "C" int64_t delora_odometry_weight_floats(const delora_odometry_desc* d) {

@@ -157,6 +157,10 @@ int clamp_counts(const Frames& f, char* ws, const int32_t* n_points, const int32
                  cudaStream_t st);
 int project(const Frames& f, const delora_odometry_desc* d, char* ws, const float* points, const int32_t* n_points,
             const int32_t* active, int n_scans, cudaStream_t st);
+int project_scan_grids(const delora_odometry_desc* d, int w, uint32_t loss_flags, int nb_h, int nb_w,
+                       float epsilon_range, int min_neighbors, const float* points, const int32_t* counts, int n,
+                       uint64_t* keys, float* image, int32_t* index_map, delora_f4* pts_grid, delora_f4* nrm_grid,
+                       cudaStream_t st);
 int init_workspace(const Frames& f, size_t total, void* workspace, cudaStream_t st, const char* who, size_t from = 0);
 int prep_blob_weights(const Model& m, const TrunkWeights& w, char* ws, const float* blob, cudaStream_t st,
                       const char* who);

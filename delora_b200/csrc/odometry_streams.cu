@@ -395,17 +395,18 @@ int check_tick(const void* points, const void* n_points, const void* workspace, 
     return 0;
 }
 
-// The residual's settings: loss_flags may have the ICP losses and DELORA_NORMAL_LINEAR and, with scaling (the recipe
-// streams), DELORA_TRAIN_NORMALIZATION_SCALING
+// The residual's settings: loss_flags may have the ICP losses, DELORA_NORMAL_LINEAR, DELORA_LOSS_PO2PO_ALONE and, with
+// scaling (the recipe streams), DELORA_TRAIN_NORMALIZATION_SCALING
 static int check_residual_params(const delora_odometry_residual_params* rp, bool scaling, const char* who) {
     DELORA_CHECK_ARG(rp, "%s: null residual_params", who);
     if (check_icp_params(rp->lambda_po2pl, rp->loss_flags, rp->nb_h, rp->nb_w, rp->epsilon_range, rp->min_neighbors, who))
         return 1;
     const uint32_t bits = DELORA_LOSS_PO2PO | DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | DELORA_NORMAL_LINEAR |
-                          (scaling ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u);
+                          DELORA_LOSS_PO2PO_ALONE | (scaling ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u);
     DELORA_CHECK_ARG((rp->loss_flags & ~bits) == 0u, "%s: loss_flags=0x%x has a bit other than %s", who, rp->loss_flags,
-                     scaling ? "the ICP losses, DELORA_NORMAL_LINEAR and DELORA_TRAIN_NORMALIZATION_SCALING"
-                             : "the ICP losses and DELORA_NORMAL_LINEAR");
+                     scaling ? "the ICP losses, DELORA_NORMAL_LINEAR, DELORA_LOSS_PO2PO_ALONE and "
+                               "DELORA_TRAIN_NORMALIZATION_SCALING"
+                             : "the ICP losses, DELORA_NORMAL_LINEAR and DELORA_LOSS_PO2PO_ALONE");
     return 0;
 }
 
@@ -418,12 +419,12 @@ const char* icp_entry(const float* info, const float* factor) {
 // The ICP at B = S on a residual or recipe plan's H x W grids: source pts_grid moved by T12, target prev_pts_grid,
 // into its losses and grad_T; on an information plan (p.info set) also into its information rows, in metres with the
 // pair factors of a normalised recipe (factor non-NULL).  The recipe's DELORA_TRAIN_NORMALIZATION_SCALING is not an
-// ICP bit.
+// ICP bit; DELORA_LOSS_PO2PO_ALONE is DELORA_LOSS_PO2PO on the zero normal grids of the points-only front end.
 static int streams_icp(const delora_odometry_desc* d, const delora_odometry_residual_params* rp, const StreamsPlan& p,
                        char* ws, const float* factor, cudaStream_t st) {
     auto f = [&](size_t o) { return reinterpret_cast<float*>(ws + o); };
     auto f4 = [&](size_t o) { return reinterpret_cast<delora_f4*>(ws + o); };
-    const uint32_t flags = rp->loss_flags & ~DELORA_TRAIN_NORMALIZATION_SCALING;
+    const uint32_t flags = rp->loss_flags & ~(DELORA_TRAIN_NORMALIZATION_SCALING | DELORA_LOSS_PO2PO_ALONE);
     float* info = p.info ? f(p.info) : nullptr;
     if (!info) factor = nullptr;
     return icp_dense_launch(f4(p.pts_grid), f4(p.nrm_grid), f(p.T12), f4(p.prev_pts_grid), f4(p.prev_nrm_grid),
@@ -514,13 +515,12 @@ static int run_streams_push(const delora_odometry_desc* d, const delora_odometry
     if (rp) {
         // the image of delora_project_fwd, bit for bit, plus the grids of the S frames with their normals
         if ((rc = clamp_counts(p.f, ws, n_points, active, S, d->n_stride, st))) return rc;
-        if ((rc = delora_project_normals_fwd(points, reinterpret_cast<int32_t*>(ws + p.f.counts), S, 3, d->n_stride, H, W,
-                                             d->hfov0, d->hfov1, d->vfov0, d->vfov1, 0,
-                                             reinterpret_cast<uint64_t*>(ws + p.f.keys), cur,
-                                             reinterpret_cast<int32_t*>(ws + p.f.index_map), rp->nb_h, rp->nb_w,
-                                             rp->epsilon_range, rp->min_neighbors,
-                                             reinterpret_cast<delora_f4*>(pts_grid), reinterpret_cast<delora_f4*>(nrm_grid),
-                                             nullptr, st))) return rc;
+        if ((rc = project_scan_grids(d, W, rp->loss_flags, rp->nb_h, rp->nb_w, rp->epsilon_range, rp->min_neighbors,
+                                     points, reinterpret_cast<int32_t*>(ws + p.f.counts), S,
+                                     reinterpret_cast<uint64_t*>(ws + p.f.keys), cur,
+                                     reinterpret_cast<int32_t*>(ws + p.f.index_map),
+                                     reinterpret_cast<delora_f4*>(pts_grid), reinterpret_cast<delora_f4*>(nrm_grid), st)))
+            return rc;
     } else if ((rc = project(p.f, d, ws, points, n_points, active, S, st))) {
         return rc;
     }
@@ -699,11 +699,10 @@ static int run_push_pre(const delora_odometry_desc* d, const delora_odometry_res
     uint64_t* keys = reinterpret_cast<uint64_t*>(ws + p.f.keys);
     int rc;
     if ((rc = clamp_counts(p.f, ws, n_points, active, S, d->n_stride, st))) return rc;
-    if ((rc = delora_project_normals_fwd(points, reinterpret_cast<int32_t*>(ws + p.f.counts), S, 3, d->n_stride, H, Wp,
-                                         d->hfov0, d->hfov1, d->vfov0, d->vfov1, 0,
-                                         reinterpret_cast<uint64_t*>(ws + p.pre_keys), f(p.pre_image),
-                                         reinterpret_cast<int32_t*>(ws + p.pre_index_map), rp->nb_h, rp->nb_w,
-                                         rp->epsilon_range, rp->min_neighbors, pre_cur_pts, pre_cur_nrm, nullptr, st)))
+    if ((rc = project_scan_grids(d, Wp, rp->loss_flags, rp->nb_h, rp->nb_w, rp->epsilon_range, rp->min_neighbors,
+                                 points, reinterpret_cast<int32_t*>(ws + p.f.counts), S,
+                                 reinterpret_cast<uint64_t*>(ws + p.pre_keys), f(p.pre_image),
+                                 reinterpret_cast<int32_t*>(ws + p.pre_index_map), pre_cur_pts, pre_cur_nrm, st)))
         return rc;
     float* factor = factor_out ? f(p.factor) : nullptr;
     if (factor && (rc = launch_grid_normalization_factors(pre_prev_pts, S, HWp, factor, st))) return rc;

@@ -350,11 +350,10 @@ int train_forward_losses(const delora_odometry_desc* d, const delora_odometry_tr
     if (d->w_pre > 0) {
         delora_f4* pre_pts = reinterpret_cast<delora_f4*>(ws + tp.pre_pts_grid);
         delora_f4* pre_nrm = reinterpret_cast<delora_f4*>(ws + tp.pre_nrm_grid);
-        if ((rc = delora_project_normals_fwd(points, counts, n_proj, 3, d->n_stride, H, d->w_pre, d->hfov0, d->hfov1,
-                                             d->vfov0, d->vfov1, 0, keys, f(tp.pre_image) + first * 4 * HWc,
-                                             reinterpret_cast<int32_t*>(ws + tp.pre_index_map) + first * HWc, hp->nb_h,
-                                             hp->nb_w, hp->epsilon_range, hp->min_neighbors, pre_pts + first * HWc,
-                                             pre_nrm + first * HWc, nullptr, st)))
+        if ((rc = project_scan_grids(d, d->w_pre, hp->loss_flags, hp->nb_h, hp->nb_w, hp->epsilon_range,
+                                     hp->min_neighbors, points, counts, n_proj, keys, f(tp.pre_image) + first * 4 * HWc,
+                                     reinterpret_cast<int32_t*>(ws + tp.pre_index_map) + first * HWc,
+                                     pre_pts + first * HWc, pre_nrm + first * HWc, st)))
             return rc;
         if (at && ((rc = from_cache(pre_pts, at->cache_pts, (size_t)B * HWc * 16)) ||
                    (rc = from_cache(pre_nrm, at->cache_nrm, (size_t)B * HWc * 16)))) return rc;
@@ -368,11 +367,10 @@ int train_forward_losses(const delora_odometry_desc* d, const delora_odometry_tr
                                     reinterpret_cast<int32_t*>(ws + tp.f.index_map), pts_grid, nrm_grid, factor, B, st)))
             return rc;
     } else {
-        if ((rc = delora_project_normals_fwd(points, counts, n_proj, 3, d->n_stride, H, W, d->hfov0, d->hfov1, d->vfov0,
-                                             d->vfov1, 0, keys, images + first * 4 * HW,
-                                             reinterpret_cast<int32_t*>(ws + tp.f.index_map) + first * HW, hp->nb_h,
-                                             hp->nb_w, hp->epsilon_range, hp->min_neighbors, pts_grid + first * HW,
-                                             nrm_grid + first * HW, nullptr, st)))
+        if ((rc = project_scan_grids(d, W, hp->loss_flags, hp->nb_h, hp->nb_w, hp->epsilon_range, hp->min_neighbors,
+                                     points, counts, n_proj, keys, images + first * 4 * HW,
+                                     reinterpret_cast<int32_t*>(ws + tp.f.index_map) + first * HW,
+                                     pts_grid + first * HW, nrm_grid + first * HW, st)))
             return rc;
         if (at && ((rc = from_cache(images, at->cache_image, (size_t)B * 4 * HW * 4)) ||
                    (rc = from_cache(pts_grid, at->cache_pts, (size_t)B * HW * 16)) ||
@@ -408,8 +406,9 @@ int train_forward_losses(const delora_odometry_desc* d, const delora_odometry_tr
     const long long icp_n4 = (delora_icp_scratch_floats(B, HW) + 3) / 4;
     odometry_icp_rearm_kernel<<<2 * num_sms(), 256, 0, st>>>(reinterpret_cast<float4*>(ws + tp.icp), icp_n4, B, ctr);
     DELORA_CHECK_LAUNCH("odometry_icp_rearm_kernel");
-    const uint32_t icp_flags =
-        hp->loss_flags & ~(DELORA_LOSS_IDENTITY_FIT | DELORA_TRAIN_NORMALIZATION_SCALING | DELORA_TRAIN_DROPOUT);
+    // po2po_alone: DELORA_LOSS_PO2PO on the zero normal grids of stage 1
+    const uint32_t icp_flags = hp->loss_flags & ~(DELORA_LOSS_IDENTITY_FIT | DELORA_TRAIN_NORMALIZATION_SCALING |
+                                                  DELORA_TRAIN_DROPOUT | DELORA_LOSS_PO2PO_ALONE);
     float* info = at ? at->info : nullptr;
     const float* factor = info && normalized ? f(tp.pre_image) : nullptr;
     if ((rc = icp_dense_launch(pts_grid + (size_t)B * HW, nrm_grid + (size_t)B * HW, f(tp.T12), pts_grid, nrm_grid, B,

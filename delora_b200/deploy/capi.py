@@ -27,26 +27,39 @@ def _ptr(t):
     return None if t is None else t.data_ptr()
 
 
-def train_params(config, lr, loss_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL, beta1=0.9, beta2=0.999, eps=1e-8):
+def _objective(config, loss_flags):
+    """(loss_flags, lambda_po2pl): the caller's flags with the config's lambda_po2pl, or with loss_flags None the
+    objective the config names (export.objective_from_config, the objective a .dlw / .dlt records)."""
+    from . import export
+    if loss_flags is None:
+        return export.objective_from_config(config)
+    return loss_flags, config["lambda_po2pl"]
+
+
+def train_params(config, lr, loss_flags=None, beta1=0.9, beta2=0.999, eps=1e-8):
     """delora_odometry_train_params: Adam's settings and the loss and normals' settings of a reference-style config.
+    loss_flags: the ICP loss bits, or None for the objective the config names (po2po_alone included).
     normalization_scaling: True adds DELORA_TRAIN_NORMALIZATION_SCALING (the step then needs a descriptor with
     w_pre > 0, and refuses w_pre = 0); use_dropout: True adds DELORA_TRAIN_DROPOUT."""
     nb = config["kitti"]["neighborhood_side_length"]
+    loss_flags, lam = _objective(config, loss_flags)
     if config.get("normalization_scaling", False):
         loss_flags |= ops.TRAIN_NORMALIZATION_SCALING
     if config.get("use_dropout", False):
         loss_flags |= ops.TRAIN_DROPOUT
     return _lib.OdometryTrainParams(
-        lr=lr, beta1=beta1, beta2=beta2, eps=eps, lambda_po2pl=config["lambda_po2pl"], loss_flags=loss_flags,
+        lr=lr, beta1=beta1, beta2=beta2, eps=eps, lambda_po2pl=lam, loss_flags=loss_flags,
         nb_h=nb[0], nb_w=nb[1], epsilon_range=config["epsilon_range"],
         min_neighbors=config["min_num_points_in_neighborhood_to_determine_point_class"])
 
 
-def residual_params(config, loss_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL):
-    """delora_odometry_residual_params: the loss and normals' settings of a reference-style config."""
+def residual_params(config, loss_flags=None):
+    """delora_odometry_residual_params: the loss and normals' settings of a reference-style config; loss_flags as for
+    train_params."""
     nb = config["kitti"]["neighborhood_side_length"]
+    loss_flags, lam = _objective(config, loss_flags)
     return _lib.OdometryResidualParams(
-        lambda_po2pl=config["lambda_po2pl"], loss_flags=loss_flags, nb_h=nb[0], nb_w=nb[1],
+        lambda_po2pl=lam, loss_flags=loss_flags, nb_h=nb[0], nb_w=nb[1],
         epsilon_range=config["epsilon_range"],
         min_neighbors=config["min_num_points_in_neighborhood_to_determine_point_class"])
 

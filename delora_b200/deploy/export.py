@@ -9,7 +9,10 @@ alone and hands the blob to `delora_odometry_load_weights`.  The network configu
 `normalization_scaling: True` is recorded in the header's `model_flags` (DELORA_MODEL_NORMALIZATION_SCALING): such a
 model runs through `delora_odometry_pairs_normalized`, and reading the file back restores the key.  `use_dropout: True`
 is recorded as DELORA_MODEL_DROPOUT: training steps then apply the encoder's dropouts (DELORA_TRAIN_DROPOUT), inference
-ignores the bit, and reading the file back restores the key.
+ignores the bit, and reading the file back restores the key.  The ICP objective the model is configured with
+(`point_to_point_loss`, `point_to_plane_loss`, `plane_to_plane_loss`, `normal_loss`, `lambda_po2pl`, `po2po_alone`) is
+recorded as `objective_flags` and `lambda_po2pl` (header bytes 108 and 112), so C hosts train, score and adapt on it;
+files with zeros there stand for the shipped objective (point-to-plane and plane-to-plane, squared, lambda_po2pl 1).
 
 A .dlt file is a training checkpoint for `delora_odometry_train_set_state`: a 256-byte header (the .dlw header with
 its own magic, then Adam's step count, the epoch, the phase, Adam's hyperparameters, the last epoch loss and the
@@ -30,8 +33,11 @@ MAGIC = b"DELORAW\x00"
 HEADER_BYTES = 128
 # magic, abi_version, header_bytes | H, W, hfov0, hfov1, vfov0, vfov1 | n_stride, max_batch, act, layers[4],
 # resnet_outputs, single_mlp, w_pre (byte 92; files written before the field have zeros there) | blob_floats |
-# model_flags (byte 104; zeros in files written before the field: no flag) | 20 reserved bytes
-_HEADER = struct.Struct("<8sii" + "ii4d" + "iii4iiii" + "q" + "I20x")
+# model_flags (byte 104; zeros in files written before the field: no flag) | objective_flags, lambda_po2pl (bytes 108,
+# 112; zeros in files written before the fields: the shipped objective) | 12 reserved bytes
+_HEADER = struct.Struct("<8sii" + "ii4d" + "iii4iiii" + "q" + "IIf12x")
+# the shipped objective (config/hyperparameters.yaml), which objective_flags = 0 stands for
+SHIPPED_OBJECTIVE = (_lib.LOSS_PO2PL | _lib.LOSS_PL2PL, 1.0)
 assert _HEADER.size == HEADER_BYTES
 
 
@@ -67,6 +73,53 @@ def model_flags_from_config(config):
     DELORA_MODEL_DROPOUT for use_dropout."""
     flags = _lib.MODEL_NORMALIZATION_SCALING if config.get("normalization_scaling", False) else 0
     return flags | (_lib.MODEL_DROPOUT if config.get("use_dropout", False) else 0)
+
+
+def objective_from_config(config):
+    """-> (objective_flags, lambda_po2pl) of a configuration's ICP objective, as Deployer._flags derives the loss bits,
+    plus DELORA_LOSS_PO2PO_ALONE for po2po_alone.  Missing keys take config/hyperparameters.yaml's values (the shipped
+    objective).  Refused, naming the key: no loss enabled, a normal_loss other than "squared" and "linear"
+    (src/losses/icp_losses.py:240), and po2po_alone with point_to_plane_loss or plane_to_plane_loss (the reference
+    would read lists it never built, :135-146)."""
+    po2po = bool(config.get("point_to_point_loss", False))
+    po2pl = bool(config.get("point_to_plane_loss", True))
+    pl2pl = bool(config.get("plane_to_plane_loss", True))
+    alone = bool(config.get("po2po_alone", False))
+    normal_loss = config.get("normal_loss", "squared")
+    lam = float(config.get("lambda_po2pl", 1.0))
+    if normal_loss not in ("squared", "linear"):
+        raise ValueError(f"normal_loss: {normal_loss!r} must be 'squared' or 'linear'")
+    if alone and (po2pl or pl2pl):
+        raise ValueError("po2po_alone: True cannot be combined with point_to_plane_loss or plane_to_plane_loss (the "
+                         "point-only objective estimates no normals)")
+    if not (po2po or po2pl or pl2pl or alone):
+        raise ValueError("point_to_point_loss, point_to_plane_loss, plane_to_plane_loss: no loss is enabled")
+    if not np.isfinite(lam):
+        raise ValueError(f"lambda_po2pl: {lam} must be finite")
+    if alone:
+        return _lib.LOSS_PO2PO | _lib.LOSS_PO2PO_ALONE, lam
+    flags = (_lib.LOSS_PO2PO if po2po else 0) | (_lib.LOSS_PO2PL if po2pl else 0)
+    if pl2pl:
+        flags |= _lib.LOSS_PL2PL | (_lib.NORMAL_LINEAR if normal_loss == "linear" else 0)
+    return flags, lam
+
+
+def file_objective(header):
+    """(objective_flags, lambda_po2pl) of a read_dlw / read_dlt header dict, the shipped objective for a file written
+    before the fields (zeros there): the loss_flags ICP bits and lambda_po2pl its model trains on."""
+    if header["objective_flags"] == 0:
+        return SHIPPED_OBJECTIVE
+    return int(header["objective_flags"]), float(header["lambda_po2pl"])
+
+
+def config_objective(objective):
+    """The configuration keys of an (objective_flags, lambda_po2pl) pair: the inverse of objective_from_config."""
+    flags, lam = objective if objective[0] else SHIPPED_OBJECTIVE
+    alone = bool(flags & _lib.LOSS_PO2PO_ALONE)
+    return {"point_to_point_loss": bool(flags & _lib.LOSS_PO2PO), "point_to_plane_loss": bool(flags & _lib.LOSS_PO2PL),
+            "plane_to_plane_loss": bool(flags & _lib.LOSS_PL2PL),
+            "normal_loss": "linear" if flags & _lib.NORMAL_LINEAR else "squared", "lambda_po2pl": float(lam),
+            "po2po_alone": alone}
 
 
 def desc_from_config(config, dataset, n_stride, max_batch=1, preprocessing_normals=False):
@@ -140,10 +193,11 @@ def unpack_blob(blob, config):
     return state
 
 
-def _pack_header(magic, header_bytes, desc, blob_floats, model_flags):
+def _pack_header(magic, header_bytes, desc, blob_floats, model_flags, objective):
+    flags, lam = objective if objective is not None else (0, 0.0)
     return _HEADER.pack(magic, _lib.ABI_VERSION, header_bytes, desc.H, desc.W, desc.hfov0, desc.hfov1, desc.vfov0,
                         desc.vfov1, desc.n_stride, desc.max_batch, desc.act, *list(desc.layers), desc.resnet_outputs,
-                        desc.single_mlp, desc.w_pre, blob_floats, int(model_flags))
+                        desc.single_mlp, desc.w_pre, blob_floats, int(model_flags), int(flags), float(lam))
 
 
 def _unpack_header(raw, path, magic, what):
@@ -155,7 +209,7 @@ def _unpack_header(raw, path, magic, what):
         raise ValueError(f"{path}: not an odometry {what} file (magic {v[0]!r})")
     names = ("magic", "abi_version", "header_bytes", "H", "W", "hfov0", "hfov1", "vfov0", "vfov1", "n_stride",
              "max_batch", "act", "l0", "l1", "l2", "l3", "resnet_outputs", "single_mlp", "w_pre", "blob_floats",
-             "model_flags")
+             "model_flags", "objective_flags", "lambda_po2pl")
     h = dict(zip(names, v))
     h["layers"] = [h.pop("l0"), h.pop("l1"), h.pop("l2"), h.pop("l3")]
     d = _lib.OdometryDesc()
@@ -166,16 +220,18 @@ def _unpack_header(raw, path, magic, what):
     return h, d
 
 
-def write_dlw(path, desc, blob, model_flags=0):
-    """model_flags: DELORA_MODEL_* bits (model_flags_from_config)."""
+def write_dlw(path, desc, blob, model_flags=0, objective=None):
+    """model_flags: DELORA_MODEL_* bits (model_flags_from_config); objective: (objective_flags, lambda_po2pl)
+    (objective_from_config), or None for zeros (the shipped objective)."""
     blob = np.ascontiguousarray(blob, dtype=np.float32)
     with open(path, "wb") as f:
-        f.write(_pack_header(MAGIC, HEADER_BYTES, desc, blob.size, model_flags))
+        f.write(_pack_header(MAGIC, HEADER_BYTES, desc, blob.size, model_flags, objective))
         f.write(blob.tobytes())
 
 
 def read_dlw(path):
-    """-> (header dict, desc, blob float32 array); the header dict has `model_flags`."""
+    """-> (header dict, desc, blob float32 array); the header dict has `model_flags`, `objective_flags` and
+    `lambda_po2pl` as stored (file_objective resolves zeros to the shipped objective)."""
     with open(path, "rb") as f:
         h, d = _unpack_header(f.read(HEADER_BYTES), path, MAGIC, "weight")
         blob = np.fromfile(f, dtype=np.float32)
@@ -212,14 +268,15 @@ class TrainingState:
     dropout_seed: int = 0
 
 
-def write_dlt(path, desc, state, model_flags=0):
+def write_dlt(path, desc, state, model_flags=0, objective=None):
+    """model_flags and objective as for write_dlw."""
     arrays = [np.ascontiguousarray(a, dtype=np.float32).reshape(-1)
               for a in (state.weights, state.exp_avg, state.exp_avg_sq)]
     n = arrays[0].size
     if any(a.size != n for a in arrays):
         raise ValueError(f"weights, exp_avg and exp_avg_sq must have the same length ({[a.size for a in arrays]})")
     with open(path, "wb") as f:
-        f.write(_pack_header(TRAIN_MAGIC, TRAIN_HEADER_BYTES, desc, n, model_flags))
+        f.write(_pack_header(TRAIN_MAGIC, TRAIN_HEADER_BYTES, desc, n, model_flags, objective))
         f.write(_TRAIN_TAIL.pack(int(state.step), int(state.epoch), int(state.unsupervised), state.lr, state.beta1,
                                  state.beta2, state.eps, state.loss, int(state.dropout_seed) & 0xFFFFFFFFFFFFFFFF))
         for a in arrays:
@@ -227,7 +284,7 @@ def write_dlt(path, desc, state, model_flags=0):
 
 
 def read_dlt(path):
-    """-> (header dict, desc, TrainingState)."""
+    """-> (header dict, desc, TrainingState); the header dict as read_dlw's."""
     with open(path, "rb") as f:
         h, d = _unpack_header(f.read(HEADER_BYTES), path, TRAIN_MAGIC, "training")
         raw = f.read(_TRAIN_TAIL.size)
@@ -341,10 +398,12 @@ def initial_training_state(config, seed):
                          float(config.get("learning_rate", 1e-5)))
 
 
-def config_from_desc(desc, base=None, dataset="kitti", model_flags=None):
+def config_from_desc(desc, base=None, dataset="kitti", model_flags=None, objective=None):
     """`base` (e.g. the YAML configuration) with the network and range-image keys set from a .dlw / .dlt descriptor,
     so that the configuration describes the weights of the file.  model_flags (the header's, or None to keep `base`'s
-    values): sets normalization_scaling and use_dropout (a file without a bit means False)."""
+    values): sets normalization_scaling and use_dropout (a file without a bit means False).  objective (the header's
+    (objective_flags, lambda_po2pl), or None to keep `base`'s values): sets the ICP objective's keys (config_objective;
+    zeros: the shipped objective)."""
     cfg = dict(base or {})
     ds = dict(cfg.get(dataset, {}))
     ds.update({"vertical_cells": int(desc.H), "horizontal_cells": int(desc.W),
@@ -359,6 +418,8 @@ def config_from_desc(desc, base=None, dataset="kitti", model_flags=None):
     if model_flags is not None:
         cfg["normalization_scaling"] = bool(int(model_flags) & _lib.MODEL_NORMALIZATION_SCALING)
         cfg["use_dropout"] = bool(int(model_flags) & _lib.MODEL_DROPOUT)
+    if objective is not None:
+        cfg.update(config_objective(objective))
     cfg.setdefault("use_dropout", False)
     cfg.setdefault("datasets", [dataset])
     return cfg
@@ -380,8 +441,10 @@ def export(checkpoint_path, dataset, out_path, n_stride, max_batch=1, config_dir
         state = training_state_from_checkpoint(ckpt, config) if training_state else None
     desc = desc_from_config(config, dataset, n_stride, max_batch, preprocessing_normals)
     flags = model_flags_from_config(config)
+    objective = objective_from_config(config)
     if training_state:
-        write_dlt(out_path, desc, state, flags)
+        write_dlt(out_path, desc, state, flags, objective)
     else:
-        write_dlw(out_path, desc, state.weights if state else pack_state_dict(ckpt["model_state_dict"], config), flags)
+        write_dlw(out_path, desc, state.weights if state else pack_state_dict(ckpt["model_state_dict"], config), flags,
+                  objective)
     return desc

@@ -251,11 +251,11 @@ class OdometryStreams(_Streams):
     residual=True serves the streams from the residual workspace (`delora_odometry_streams_push_residual`): `push` then
     returns, beside each transform, the stream's ICP loss row [LOSS_ROW] (po2po, po2pl, pl2pl, matched pairs, matched
     po2po pairs, ...) of this frame moved by T against the previous frame, with the normals estimated on the model's
-    H x W image and the config's neighbourhood; `residual_flags` selects the losses.  The transforms are the same bits
-    either way."""
+    H x W image and the config's neighbourhood; `residual_flags` selects the losses (None: the objective the config
+    names, po2po_alone included, as a .dlw records it).  The transforms are the same bits either way."""
 
     def __init__(self, model, config, dataset, n_streams, n_max, use_cuda_graph=True, residual=False,
-                 residual_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL):
+                 residual_flags=None):
         if config.get("normalization_scaling", False):
             raise ValueError("normalization_scaling: True is not supported by OdometryStreams (its workspace caches "
                              "each stream's projected image, which a normalised model cannot reuse); serve such a "
@@ -287,6 +287,8 @@ class OdometryStreams(_Streams):
         with torch.cuda.device(self.device):
             self.blob = torch.from_numpy(export.pack_state_dict(model.state_dict(), config)).to(self.device)
             if pre:
+                if residual_flags is None:
+                    residual_flags = export.objective_from_config(config)[0]
                 flags = residual_flags | (ops.TRAIN_NORMALIZATION_SCALING if normalized else 0)
                 kind = capi.PreInformationStreamsWorkspace if info else capi.PreStreamsWorkspace
                 self.workspace = kind(self.desc, self.blob, capi.residual_params(config, flags))
@@ -356,7 +358,7 @@ class InformationOdometryStreams(OdometryStreams):
     residual=True's; `residual_flags` selects the losses; `poses` and `reset` are OdometryStreams'."""
 
     def __init__(self, model, config, dataset, n_streams, n_max, use_cuda_graph=True,
-                 residual_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL):
+                 residual_flags=None):
         if config.get("normalization_scaling", False):
             raise ValueError("normalization_scaling: True is not supported by InformationOdometryStreams (the "
                              "information is that of the residual workspace, which serves plain models)")
@@ -393,7 +395,7 @@ class PreprocessedOdometryStreams(OdometryStreams):
     losses and factor are the same bits either way."""
 
     def __init__(self, model, config, dataset, n_streams, n_max, use_cuda_graph=True,
-                 residual_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL, information=False):
+                 residual_flags=None, information=False):
         if "horizontal_cells_preprocessing" not in config[dataset]:
             raise ValueError(f"{dataset}: horizontal_cells_preprocessing is missing; PreprocessedOdometryStreams "
                              "serves the recipe's normals at that width (serve raw scans with OdometryStreams)")
@@ -405,8 +407,8 @@ class AdaptiveOdometryStreams(_Streams):
     """Several streams served while the model adapts to them (`delora_odometry_streams_push_adapt`): one tick runs the
     training step's forward at batch `n_streams`, each pair's first frame taken from the workspace, returns each
     stream's T and ICP loss row, and with update=True takes one Adam step (learning rate `lr`, torch's default betas)
-    on the mean objective of the pairs it served.  T is always that of the weights before the tick's update; the next
-    tick serves the updated model.  Normals at the model's width, or with preprocessing_normals=True at
+    on the mean objective of the pairs it served (`loss_flags`, or None for the objective the config names, po2po_alone
+    included).  T is always that of the weights before the tick's update; the next tick serves the updated model.  Normals at the model's width, or with preprocessing_normals=True at
     `horizontal_cells_preprocessing` (the reference's recipe, which normalization_scaling needs).  `state_dict()` is the
     adapted model.  Dropout configs are refused: the served T must be dropout-free.
 
@@ -418,7 +420,7 @@ class AdaptiveOdometryStreams(_Streams):
     information = False
 
     def __init__(self, model, config, dataset, n_streams, n_max, lr, preprocessing_normals=False,
-                 loss_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL, information=False):
+                 loss_flags=None, information=False):
         from . import capi, export
         if config.get("use_dropout", False):
             raise ValueError("use_dropout: True is not supported by AdaptiveOdometryStreams: the served transforms "
@@ -497,7 +499,7 @@ class GeometriesAdaptiveOdometryStreams(AdaptiveOdometryStreams):
     AdaptiveOdometryStreams(information=True).  T, losses and the adapted model are the same bits either way."""
 
     def __init__(self, model, config, geometries, n_max, lr, preprocessing_normals=False,
-                 loss_flags=ops.LOSS_PO2PL | ops.LOSS_PL2PL, information=False):
+                 loss_flags=None, information=False):
         from . import capi, export
         if config.get("use_dropout", False):
             raise ValueError("use_dropout: True is not supported by GeometriesAdaptiveOdometryStreams: the served "

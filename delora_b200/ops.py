@@ -38,6 +38,7 @@ ICP_STATS = 256      # DELORA_ICP_STATS flag bit
 LOSS_IDENTITY_FIT = 512      # delora_odometry_train_step's identity pre-training objective
 TRAIN_NORMALIZATION_SCALING = 1024   # delora_odometry_train_step: the model uses normalization_scaling (needs w_pre > 0)
 TRAIN_DROPOUT = 2048    # delora_odometry_train_step: the model uses use_dropout (the three dropouts, p = 0.2)
+LOSS_PO2PO_ALONE = 4096  # po2po_alone: with LOSS_PO2PO, every point against its nearest neighbour, no normals
 # tensor ids of the training step's dropout masks (delora_dropout_keep_mask)
 DROPOUT_INPUT, DROPOUT_STAGE3, DROPOUT_FC = 0, 1, 2
 LOSS_ROW, ICP_PARTIAL = 8, 40
@@ -137,6 +138,26 @@ def project_normals(points, n_points, h, w, hfov, vfov, neighborhood=(7, 11), ep
                                             int(neighborhood[0]), int(neighborhood[1]), float(epsilon_range),
                                             int(min_neighbors), pg.data_ptr(), ng.data_ptr(), None, _stream()),
                "delora_project_normals_fwd")
+    return image, index_map, pg, ng
+
+
+def project_points(points, n_points, h, w, hfov, vfov, div_mode=0):
+    """project_normals without the normals (the front end of LOSS_PO2PO_ALONE): the same image, index_map and
+    pts_grid bits, and nrm_grid all zeros."""
+    b, c, n = points.shape
+    dev = points.device
+    image = torch.empty((b, c + 1, h, w), dtype=torch.float32, device=dev)
+    index_map = torch.empty((b, h, w), dtype=torch.int32, device=dev)
+    pg = torch.empty((b, h * w, 4), dtype=torch.float32, device=dev)
+    ng = torch.empty((b, h * w, 4), dtype=torch.float32, device=dev)
+    keys = _keys(dev, b, h * w)
+    L = _lib.lib()
+    _lib.check(L.delora_project_points_fwd(_req(points, torch.float32, "points"),
+                                           _req(n_points, torch.int32, "n_points"), b, c, n, h, w, float(hfov[0]),
+                                           float(hfov[1]), float(vfov[0]), float(vfov[1]), int(div_mode),
+                                           keys.data_ptr(), image.data_ptr(), index_map.data_ptr(), pg.data_ptr(),
+                                           ng.data_ptr(), _stream()),
+               "delora_project_points_fwd")
     return image, index_map, pg, ng
 
 

@@ -8,8 +8,10 @@
  * consecutive pairs (scan k, scan k+1), min(max_batch, pairs) pairs per step, cycling through the list, and writes the
  * updated weights to out.dlw (same header).  Prints the objective (mean over the step's pairs of
  * po2po + lambda * po2pl + pl2pl, before that step's update) once per step.  No ground truth is needed.
- * The normals the losses use are estimated at the resolution the header's w_pre names (export with
- * --preprocessing-normals for the reference's recipe); the program says which on stderr.
+ * The objective is the one the header records (objective_flags and lambda_po2pl; zeros there: po2pl + pl2pl, lambda_po2pl
+ * 1), printed once on stderr.  The normals the losses use are estimated at the resolution the header's w_pre names
+ * (export with --preprocessing-normals for the reference's recipe; po2po_alone estimates none); the program says which
+ * on stderr.
  * A model configured with use_dropout (model_flags has DELORA_MODEL_DROPOUT) trains with its dropouts
  * (DELORA_TRAIN_DROPOUT); the seed of the masks is --dropout-seed, else the DELORA_DROPOUT_SEED environment variable,
  * else 0.
@@ -28,6 +30,16 @@
 static int fail(const char* what) {
     fprintf(stderr, "odometry_finetune: %s\n", what);
     return 1;
+}
+
+/* the ICP objective a host trains, scores or adapts on, as it prints it once at start */
+static void print_objective(const char* who, uint32_t f, float lambda_po2pl) {
+    fprintf(stderr, "%s: objective%s%s%s%s, lambda_po2pl %g\n", who,
+            (f & DELORA_LOSS_PO2PO_ALONE) ? " po2po_alone" : (f & DELORA_LOSS_PO2PO) ? " po2po" : "",
+            (f & DELORA_LOSS_PO2PL) ? " po2pl" : "", (f & DELORA_LOSS_PL2PL) ? " pl2pl" : "",
+            (f & DELORA_LOSS_PL2PL) ? ((f & DELORA_NORMAL_LINEAR) ? " (linear normal loss)" : " (squared normal loss)")
+                                    : "",
+            (double)lambda_po2pl);
 }
 
 #define CUDA_OK(call)                                                                  \
@@ -117,9 +129,11 @@ int main(int argc, char** argv) {
 
     delora_odometry_train_params hp;
     hp.lr = lr; hp.beta1 = 0.9f; hp.beta2 = 0.999f; hp.eps = 1e-8f;
-    hp.lambda_po2pl = 1.0f;
+    uint32_t objective;                       /* the file's ICP objective (zeros in the header: the shipped one) */
+    if (delora_odometry_file_objective(&hdr, &objective, &hp.lambda_po2pl)) return fail(delora_last_error());
+    print_objective("odometry_finetune", objective, hp.lambda_po2pl);
     const int dropout = (hdr.model_flags & DELORA_MODEL_DROPOUT) != 0;
-    hp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | (normalized ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u) |
+    hp.loss_flags = objective | (normalized ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u) |
                     (dropout ? DELORA_TRAIN_DROPOUT : 0u);
     hp.nb_h = 7; hp.nb_w = 11;
     hp.epsilon_range = 0.5f;

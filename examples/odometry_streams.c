@@ -81,6 +81,16 @@ static int fail(const char* what) {
     return 1;
 }
 
+/* the ICP objective a host trains, scores or adapts on, as it prints it once at start */
+static void print_objective(const char* who, uint32_t f, float lambda_po2pl) {
+    fprintf(stderr, "%s: objective%s%s%s%s, lambda_po2pl %g\n", who,
+            (f & DELORA_LOSS_PO2PO_ALONE) ? " po2po_alone" : (f & DELORA_LOSS_PO2PO) ? " po2po" : "",
+            (f & DELORA_LOSS_PO2PL) ? " po2pl" : "", (f & DELORA_LOSS_PL2PL) ? " pl2pl" : "",
+            (f & DELORA_LOSS_PL2PL) ? ((f & DELORA_NORMAL_LINEAR) ? " (linear normal loss)" : " (squared normal loss)")
+                                    : "",
+            (double)lambda_po2pl);
+}
+
 #define CUDA_OK(call)                                                                  \
     do {                                                                               \
         cudaError_t e_ = (call);                                                       \
@@ -523,8 +533,12 @@ int main(int argc, char** argv) {
 
     delora_odometry_train_params hp;                       /* --adapt: Adam, and the residual's losses and neighbourhood */
     hp.lr = lr; hp.beta1 = 0.9f; hp.beta2 = 0.999f; hp.eps = 1e-8f;
-    hp.lambda_po2pl = 1.0f;
-    hp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | (normalized ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u);
+    uint32_t objective;                       /* the file's ICP objective (zeros in the header: the shipped one) */
+    float lambda_po2pl;
+    if (delora_odometry_file_objective(&hdr, &objective, &lambda_po2pl)) return fail(delora_last_error());
+    if (adapt || residual || pre) print_objective("odometry_streams", objective, lambda_po2pl);
+    hp.lambda_po2pl = lambda_po2pl;
+    hp.loss_flags = objective | (normalized ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u);
     hp.nb_h = 7; hp.nb_w = 11;
     hp.epsilon_range = 0.5f;
     hp.min_neighbors = 10;
@@ -544,8 +558,8 @@ int main(int argc, char** argv) {
     const size_t pts_floats = (size_t)S * 3 * d->n_stride;
     float *weights, *points, *T, *losses, *factor, *info;
     delora_odometry_residual_params rp;
-    rp.lambda_po2pl = 1.0f;
-    rp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL;
+    rp.lambda_po2pl = lambda_po2pl;
+    rp.loss_flags = objective;
     if (pre && normalized) rp.loss_flags |= DELORA_TRAIN_NORMALIZATION_SCALING;
     rp.nb_h = 7; rp.nb_w = 11;
     rp.epsilon_range = 0.5f;

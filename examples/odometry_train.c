@@ -16,7 +16,8 @@
  * unsupervised.  A .dlw, or a .dlt made from a checkpoint, starts unsupervised, as the reference does with a
  * checkpoint.  After every epoch the state goes to out.dlt (written to out.dlt.tmp, then renamed), so a run that
  * stops can resume from it: N epochs in one run and N1 + N2 = N epochs in two give the same bytes.
- * Losses as odometry_finetune.c: po2pl + pl2pl, lambda_po2pl 1, normals at the resolution the header's w_pre names.
+ * Losses as odometry_finetune.c: the objective the header records (objective_flags, lambda_po2pl; zeros there: po2pl +
+ * pl2pl, lambda_po2pl 1), normals at the resolution the header's w_pre names (none under po2po_alone).
  * A model configured with use_dropout (model_flags has DELORA_MODEL_DROPOUT) trains with its dropouts
  * (DELORA_TRAIN_DROPOUT).  The seed of the masks is --dropout-seed, else the DELORA_DROPOUT_SEED environment variable,
  * else the .dlt's (0 for a .dlw); it is written into every out.dlt, so a resumed run draws the masks of an
@@ -59,6 +60,16 @@
 static int fail(const char* what) {
     fprintf(stderr, "odometry_train: %s\n", what);
     return 1;
+}
+
+/* the ICP objective a host trains, scores or adapts on, as it prints it once at start */
+static void print_objective(const char* who, uint32_t f, float lambda_po2pl) {
+    fprintf(stderr, "%s: objective%s%s%s%s, lambda_po2pl %g\n", who,
+            (f & DELORA_LOSS_PO2PO_ALONE) ? " po2po_alone" : (f & DELORA_LOSS_PO2PO) ? " po2po" : "",
+            (f & DELORA_LOSS_PO2PL) ? " po2pl" : "", (f & DELORA_LOSS_PL2PL) ? " pl2pl" : "",
+            (f & DELORA_LOSS_PL2PL) ? ((f & DELORA_NORMAL_LINEAR) ? " (linear normal loss)" : " (squared normal loss)")
+                                    : "",
+            (double)lambda_po2pl);
 }
 
 static int by_name(const void* a, const void* b) { return strcmp(*(char* const*)a, *(char* const*)b); }
@@ -446,6 +457,10 @@ int main(int argc, char** argv) {
     }
     const uint64_t dropout_seed = (uint64_t)hdr.dropout_seed[0] | ((uint64_t)hdr.dropout_seed[1] << 32);
     const int dropout = (hdr.base.model_flags & DELORA_MODEL_DROPOUT) != 0;
+    uint32_t objective;                       /* the file's ICP objective (zeros in the header: the shipped one) */
+    float lambda_po2pl;
+    if (delora_odometry_file_objective(&hdr.base, &objective, &lambda_po2pl)) return fail(delora_last_error());
+    print_objective("odometry_train", objective, lambda_po2pl);
 
     const int n_pairs = n_scans - 1;
     if (B_max < 1 || B_max > d->max_batch) return fail("B must be in [1, the header's max_batch]");
@@ -467,7 +482,7 @@ int main(int argc, char** argv) {
 
     delora_odometry_train_params hp;
     hp.lr = hdr.lr; hp.beta1 = hdr.beta1; hp.beta2 = hdr.beta2; hp.eps = hdr.eps;
-    hp.lambda_po2pl = 1.0f;
+    hp.lambda_po2pl = lambda_po2pl;
     hp.nb_h = 7; hp.nb_w = 11;
     hp.epsilon_range = 0.5f;
     hp.min_neighbors = 10;
@@ -518,7 +533,7 @@ int main(int argc, char** argv) {
                 (long long)hdr.step, hdr.unsupervised ? "unsupervised" : "identity pre-training", per * gpus, gpus);
         rank_state* R0 = &ranks[0];
         for (int e = 0; e < epochs; ++e) {
-            hp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | (hdr.unsupervised ? 0u : DELORA_LOSS_IDENTITY_FIT) |
+            hp.loss_flags = objective | (hdr.unsupervised ? 0u : DELORA_LOSS_IDENTITY_FIT) |
                             (normalized ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u) | (dropout ? DELORA_TRAIN_DROPOUT : 0u);
             for (int r = 0; r < gpus; ++r) {
                 ranks[r].hp = hp;
@@ -632,7 +647,7 @@ int main(int argc, char** argv) {
     int32_t* h_step_counts = (int32_t*)malloc((size_t)2 * B_max * sizeof(int32_t));
     if (!h_losses || !h_step_counts) return fail("out of host memory");
     for (int e = 0; e < epochs; ++e) {
-        hp.loss_flags = DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL | (hdr.unsupervised ? 0u : DELORA_LOSS_IDENTITY_FIT) |
+        hp.loss_flags = objective | (hdr.unsupervised ? 0u : DELORA_LOSS_IDENTITY_FIT) |
                         (normalized ? DELORA_TRAIN_NORMALIZATION_SCALING : 0u) | (dropout ? DELORA_TRAIN_DROPOUT : 0u);
         int nb = 0;
         for (int g = 0; g < n_sets; ++g)

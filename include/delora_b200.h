@@ -46,6 +46,12 @@ typedef struct { float x, y, z, w; } delora_f4;
                                                     normalization_scaling (see _train_step; needs w_pre > 0) */
 #define DELORA_TRAIN_DROPOUT 2048u /* delora_odometry_train_step only: the model is trained with use_dropout (the
                                       three dropouts of the reference's encoder; see _train_step) */
+#define DELORA_LOSS_PO2PO_ALONE 4096u /* po2po_alone (src/losses/icp_losses.py:36-46), read by the odometry training,
+                                         streams and adapting entry points: every surviving point of scan_2 is paired
+                                         with its nearest surviving point of scan_1 and no normal plays a part.  Needs
+                                         DELORA_LOSS_PO2PO; refuses DELORA_LOSS_PO2PL, _PL2PL and DELORA_NORMAL_LINEAR.
+                                         The outputs are the bits of the same call with DELORA_LOSS_PO2PO alone on
+                                         all-zero normal grids; no normal is estimated (delora_project_points_fwd). */
 
 /* number of floats in one row of the `losses` output of delora_icp_fwd_bwd */
 #define DELORA_LOSS_ROW 8   /* [po2po, po2pl, pl2pl, M_pairs, M_po2po, 0, 0, 0] */
@@ -136,6 +142,14 @@ int delora_project_normals_fwd(const float* points, const int32_t* n_points, int
                                int div_mode, uint64_t* keys, float* image, int32_t* index_map, int nb_h, int nb_w,
                                float epsilon_range, int min_neighbors, delora_f4* pts_grid, delora_f4* nrm_grid,
                                void* split_event, void* stream);
+
+/* The points-only front end of DELORA_LOSS_PO2PO_ALONE: delora_project_normals_fwd without the normals.  The same
+ * depth keys and resolve pass, so image, index_map and pts_grid are bit-identical to that call's (for any
+ * neighbourhood); nrm_grid [B, H*W] float4 is written all zeros.  No neighbourhood is staged, no tap accumulated and no
+ * eigen-solve run.  Keys all-ones on entry and on exit.  C must be 3 or 4. */
+int delora_project_points_fwd(const float* points, const int32_t* n_points, int B, int C, int n_stride, int H, int W,
+                              double hfov0, double hfov1, double vfov0, double vfov1, int div_mode, uint64_t* keys,
+                              float* image, int32_t* index_map, delora_f4* pts_grid, delora_f4* nrm_grid, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Image -> lists (row-major order of the valid pixels), the layout the reference stores and
@@ -537,8 +551,9 @@ typedef struct {
  *   bytes   0..127  delora_odometry_file_header below (explicit offsets: magic 0, abi_version 8, header_bytes 12,
  *                   desc 16: H 16, W 20, hfov0 24, hfov1 32, vfov0 40, vfov1 48, n_stride 56, max_batch 60, act 64,
  *                   layers 68..83, resnet_outputs 84, single_mlp 88, w_pre 92; blob_floats 96; model_flags 104;
- *                   zero 108..127; exporters before w_pre wrote zeros at 92, i.e. w_pre = 0, and exporters before
- *                   model_flags wrote zeros at 104, i.e. no flag)
+ *                   objective_flags 108; lambda_po2pl 112; zero 116..127; exporters before w_pre wrote zeros at 92,
+ *                   i.e. w_pre = 0, exporters before model_flags wrote zeros at 104, i.e. no flag, and exporters
+ *                   before the objective wrote zeros at 108..115, i.e. the shipped objective)
  *   bytes 128..     float32[blob_floats]: the tensors of OdometryModel.state_dict() concatenated in state_dict order,
  *                   each tensor row-major (the blob delora_odometry_load_weights takes). */
 #define DELORA_ODOMETRY_FILE_MAGIC "DELORAW"     /* 7 characters + NUL = the 8 magic bytes */
@@ -554,8 +569,20 @@ typedef struct {
     delora_odometry_desc desc;
     int64_t blob_floats;                 /* == delora_odometry_weight_floats(&desc) */
     uint32_t model_flags;                /* DELORA_MODEL_* bits (byte 104) */
-    uint8_t reserved[20];
+    uint32_t objective_flags;            /* byte 108: the ICP objective the model is configured with, the loss_flags
+                                            bits DELORA_LOSS_PO2PO / _PO2PL / _PL2PL, DELORA_NORMAL_LINEAR and
+                                            DELORA_LOSS_PO2PO_ALONE (at least one ICP loss bit); 0: written before
+                                            the field, the shipped objective (see delora_odometry_file_objective) */
+    float lambda_po2pl;                  /* byte 112: the objective's lambda_po2pl (ignored when objective_flags = 0) */
+    uint8_t reserved[12];
 } delora_odometry_file_header;
+
+/* Host only (no GPU needed): the objective a .dlw / .dlt header records, as the loss_flags ICP bits and lambda_po2pl
+ * of delora_odometry_train_params / delora_odometry_residual_params.  objective_flags = 0 gives the shipped objective,
+ * DELORA_LOSS_PO2PL | DELORA_LOSS_PL2PL with lambda_po2pl 1.  Refused (non-zero, delora_last_error() naming the field):
+ * a null pointer, objective_flags with a bit outside the five above or without an ICP loss bit, DELORA_LOSS_PO2PO_ALONE
+ * without DELORA_LOSS_PO2PO or with _PO2PL, _PL2PL or DELORA_NORMAL_LINEAR, and a lambda_po2pl that is not finite. */
+int delora_odometry_file_objective(const delora_odometry_file_header* h, uint32_t* loss_flags, float* lambda_po2pl);
 
 /* Host only (no GPU needed): validate the descriptor (non-zero + delora_last_error() if it is invalid; the size
  * functions then return -1) and size the weight blob / the workspace. */
